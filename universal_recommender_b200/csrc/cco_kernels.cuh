@@ -431,8 +431,8 @@ __global__ void k_col_terms(int32_t n_cols, const int32_t *__restrict__ marg, lo
 // ------------------------------------------------------------------------------------------------
 // The fused row kernel.  A GROUP of threads (one warp, or a whole CTA of 256 / 1024 threads) owns one
 // primary item a at a time and keeps everything for that row in shared memory:
-//   count  : for u in users(a): for b in B'[u]: table[b]++     32-user chunks per warp, products flattened
-//                                                               over lanes by a warp prefix-sum + shuffle search
+//   count  : for u in users(a): for b in B'[u]: table[b]++     products flattened over lanes by a prefix sum +
+//                                                               shuffle search; CTA-owned rows split them evenly over warps
 //   compact: occupied table words -> dense per-warp lists (in place)
 //   score  : LLR(k11, colA[a], colB[b], N) in fp64, in registers, 2 logs per cell (the other xLogX terms
 //            are per-row / per-column / small-integer tables holding bit-identical values)
@@ -604,8 +604,47 @@ __device__ __forceinline__ void accumulate(uint32_t *table, uint32_t tsize, uint
   }
 }
 
+// Count the products [p_lo, p_hi) of a window of up to 32 users held in registers: lane l holds user l's first product
+// index `off` (non-decreasing over the lanes, lane 0's <= p_lo; unused lanes hold 0xffffffff) and the start `s` of its
+// B' row.  Each lane finds the user of its product by a 5-step shuffle search, then gathers the column.
 template <int GROUP, bool DENSE>
-__global__ void __launch_bounds__(GROUP == 32 ? 256 : GROUP) k_rows(const RowArgs a) {
+__device__ __forceinline__ void count_window(const RowArgs &a, uint32_t *table, uint32_t tsize, int cbits, uint32_t n_pass,
+                                             uint32_t pass, uint32_t off, uint32_t s, uint32_t p_lo, uint32_t p_hi, int lane) {
+  for (uint32_t p0 = p_lo; p0 < p_hi; p0 += 64) {
+    // two products per lane per trip (two independent gathers in flight)
+    uint32_t bb[2];
+    bool act[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const uint32_t p = p0 + h * 32 + lane;
+      int j = 0;
+#pragma unroll
+      for (int st = 16; st > 0; st >>= 1) {
+        const int c = j + st;
+        const uint32_t v = __shfl_sync(0xffffffffu, off, c);
+        if (v <= p) j = c;
+      }
+      const uint32_t sj = __shfl_sync(0xffffffffu, s, j), oj = __shfl_sync(0xffffffffu, off, j);
+      act[h] = p < p_hi;
+      bb[h] = act[h] ? (uint32_t)a.b_col[sj + (p - oj)] : 0u;
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      if (act[h]) accumulate<GROUP, DENSE>(table, tsize, bb[h], cbits, n_pass, pass, a.err_flag);
+  }
+}
+
+// Minimum resident CTAs per SM that the register allocation must allow.  At top_k 50 make_cfg (cco_api.cu) fits 2 / 4 / 9
+// hashed 512 / 256 / 128-thread CTAs per SM in shared memory; 8 instead of 9 keeps 64 registers (9 forces 56 and measured
+// no faster).  Warp-owned rows run as 64-thread CTAs whose three bins fit 8 / 13 / 16 per SM: 12 is what their spill-free
+// 80 registers allow, and a 16-CTA bound (64 registers) measured no faster.  DESIGN.md 3.2 lists registers and spills.
+template <int GROUP>
+struct RowsMinBlocks {
+  static constexpr int value = GROUP == 512 ? 2 : GROUP == 256 ? 4 : GROUP == 128 ? 8 : GROUP == 32 ? 12 : 1;
+};
+
+template <int GROUP, bool DENSE>
+__global__ void __launch_bounds__(GROUP == 32 ? 64 : GROUP, RowsMinBlocks<GROUP>::value) k_rows(const RowArgs a) {
   const int GROUPS = GROUP == 32 ? (int)(blockDim.x >> 5) : 1;  // warp-owned rows: several independent warps per CTA
   constexpr int NW = GROUP / 32;
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -662,47 +701,78 @@ __global__ void __launch_bounds__(GROUP == 32 ? 256 : GROUP) k_rows(const RowArg
       // ---- clear --------------------------------------------------------------------------------------
       for (uint32_t i = gtid; i < tsize; i += GROUP) table[i] = DENSE ? 0u : kEmpty;
       group_sync<GROUP>();
-      // ---- count: each warp takes 32-user chunks; products of a chunk are flattened over the lanes -----
-      // users are dealt to the group's warps in equal chunks of <= 32 so short rows still use every warp
-      const uint32_t deg = u_end - u_begin;
-      const uint32_t per = NW == 1 ? 32u : min(32u, max(1u, (deg + NW - 1) / NW));
-      for (uint32_t c0 = u_begin + gw * per; c0 < u_end; c0 += NW * per) {
-        const uint32_t i = c0 + lane;
-        uint32_t s = 0, len = 0;
-        if (lane < per && i < u_end) {
-          const int32_t u = a.at_users[i];
-          s = a.b_ptr[u];
-          len = a.b_ptr[u + 1] - s;
-        }
-        uint32_t off = len;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-          const uint32_t v = __shfl_up_sync(0xffffffffu, off, d);
-          if (lane >= d) off += v;
-        }
-        const uint32_t total = __shfl_sync(0xffffffffu, off, 31);
-        off -= len;  // exclusive
-        for (uint32_t p0 = 0; p0 < total; p0 += 64) {
-          // two products per lane per trip (two independent gathers in flight)
-          uint32_t bb[2];
-          bool act[2];
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const uint32_t p = p0 + h * 32 + lane;
-            int j = 0;
-#pragma unroll
-            for (int st = 16; st > 0; st >>= 1) {
-              const int c = j + st;
-              const uint32_t v = __shfl_sync(0xffffffffu, off, c);
-              if (v <= p) j = c;
-            }
-            const uint32_t sj = __shfl_sync(0xffffffffu, s, j), oj = __shfl_sync(0xffffffffu, off, j);
-            act[h] = p < total;
-            bb[h] = act[h] ? (uint32_t)a.b_col[sj + (p - oj)] : 0u;
+      // ---- count -------------------------------------------------------------------------------------------
+      if (NW == 1) {
+        // warp-owned row: 32-user chunks, the products of a chunk flattened over the lanes by a warp prefix sum
+        for (uint32_t c0 = u_begin; c0 < u_end; c0 += 32) {
+          const uint32_t i = c0 + lane;
+          uint32_t s = 0, len = 0;
+          if (i < u_end) {
+            const int32_t u = a.at_users[i];
+            s = a.b_ptr[u];
+            len = a.b_ptr[u + 1] - s;
           }
+          uint32_t off = len;
 #pragma unroll
-          for (int h = 0; h < 2; ++h)
-            if (act[h]) accumulate<GROUP, DENSE>(table, tsize, bb[h], cbits, n_pass, pass, a.err_flag);
+          for (int d = 1; d < 32; d <<= 1) {
+            const uint32_t v = __shfl_up_sync(0xffffffffu, off, d);
+            if (lane >= d) off += v;
+          }
+          const uint32_t total = __shfl_sync(0xffffffffu, off, 31);
+          off = i < u_end ? off - len : 0xffffffffu;  // exclusive
+          count_window<GROUP, DENSE>(a, table, tsize, cbits, n_pass, pass, off, s, 0u, total, lane);
+        }
+      } else {
+        // CTA-owned row: the count barrier waits for the busiest warp, and B' degrees are Zipf-skewed, so the warps
+        // split the PRODUCTS of a window of GROUP users evenly (not the users).  Thread t loads user t of the window;
+        // a CTA scan of the degrees goes to `wofs` = (B' row start, first product) per user, which aliases the
+        // evaluation queues (dead until the score stage).  Warp g counts products [g T / NW, (g + 1) T / NW) of the
+        // window's T, 32 users at a time in registers.
+        uint2 *wofs = reinterpret_cast<uint2 *>(wqueue);   // GROUP entries = NW * 64 words
+        int *wsum = hist;                                  // NW warp totals (the select histogram is dead here)
+        for (uint32_t w0 = u_begin; w0 < u_end; w0 += GROUP) {
+          const uint32_t nwin = min((uint32_t)GROUP, u_end - w0);
+          uint32_t s = 0, len = 0;
+          if ((uint32_t)gtid < nwin) {
+            const int32_t u = a.at_users[w0 + gtid];
+            s = a.b_ptr[u];
+            len = a.b_ptr[u + 1] - s;
+          }
+          uint32_t incl = len;
+#pragma unroll
+          for (int d = 1; d < 32; d <<= 1) {
+            const uint32_t v = __shfl_up_sync(0xffffffffu, incl, d);
+            if (lane >= d) incl += v;
+          }
+          if (lane == 31) wsum[gw] = (int)incl;
+          __syncthreads();
+          uint32_t wpre = lane < NW ? (uint32_t)wsum[lane] : 0u;
+#pragma unroll
+          for (int d = 1; d < NW; d <<= 1) {
+            const uint32_t v = __shfl_up_sync(0xffffffffu, wpre, d);
+            if (lane >= d) wpre += v;
+          }
+          const uint32_t T = __shfl_sync(0xffffffffu, wpre, NW - 1);
+          const uint32_t before = gw == 0 ? 0u : __shfl_sync(0xffffffffu, wpre, gw - 1);
+          wofs[gtid] = make_uint2(s, before + incl - len);
+          __syncthreads();
+          const uint32_t p_lo = (uint32_t)((unsigned long long)T * gw / NW);
+          const uint32_t p_hi = (uint32_t)((unsigned long long)T * (gw + 1) / NW);
+          if (p_lo < p_hi) {
+            // first user of the warp's range: the last one whose first product is <= p_lo
+            uint32_t lo = 0, hi = nwin - 1;
+            while (lo < hi) {
+              const uint32_t mid = (lo + hi + 1) >> 1;
+              if (wofs[mid].y <= p_lo) lo = mid; else hi = mid - 1;
+            }
+            for (uint32_t j0 = lo, p = p_lo; p < p_hi; j0 += 32) {
+              const uint2 e = j0 + lane < nwin ? wofs[j0 + lane] : make_uint2(0u, 0xffffffffu);
+              const uint32_t wend = min(p_hi, j0 + 32 < nwin ? wofs[j0 + 32].y : T);
+              count_window<GROUP, DENSE>(a, table, tsize, cbits, n_pass, pass, e.y, e.x, p, wend, lane);
+              p = wend;
+            }
+          }
+          __syncthreads();   // wofs / wsum are rewritten by the next window
         }
       }
       group_sync<GROUP>();
