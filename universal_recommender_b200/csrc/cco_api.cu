@@ -735,11 +735,18 @@ static int enqueue_indicator(cco_ctx *c, Arena &ar, const uint32_t *at_ptr, cons
   unsigned long long *work64;
   long long *work_prefix;
   int32_t *ids, *rows_sorted, *d_pb = nullptr;
-  size_t sort_tb = 0;
+  size_t sort_tb = 0, order_tb = 0;
   if (n_items_a > 0)
     CK(cub::DeviceRadixSort::SortPairsDescending(nullptr, sort_tb, (const uint32_t *)nullptr, (uint32_t *)nullptr, (const int32_t *)nullptr,
                                                  (int32_t *)nullptr, n_items_a, 0, 32, s));
-  const bool beside = inputs_ready && ar.c && ((size_t)n_items_a + 1) * 8 <= Arena::kSlabMax && sort_tb <= Arena::kSlabMax;
+  int cb_bits = 1;   // colB <= max_marg_b: the column-order sort looks at these key bits only
+  while ((1LL << cb_bits) <= (long long)max_marg_b) ++cb_bits;
+  cub::DoubleBuffer<uint32_t> order_cb(nullptr, nullptr);
+  cub::DoubleBuffer<int32_t> order_id(nullptr, nullptr);
+  if (n_cols_b > 0) CK(cub::DeviceRadixSort::SortPairs(nullptr, order_tb, order_cb, order_id, n_cols_b, 0, cb_bits, s));
+  const bool beside = inputs_ready && ar.c && ((size_t)n_items_a + 1) * 8 <= Arena::kSlabMax && sort_tb <= Arena::kSlabMax &&
+                      (size_t)n_cols_b * 4 <= Arena::kSlabMax && order_tb <= Arena::kSlabMax &&
+                      ((size_t)max_marg_b + 2) * 4 <= Arena::kSlabMax;
   cudaStream_t ss = beside ? c->sched_stream : s;
   if (beside) CK(cudaStreamWaitEvent(ss, inputs_ready, 0));
   CKR(ar.alloc(&row_work, n_items_a + 1));
@@ -818,17 +825,44 @@ static int enqueue_indicator(cco_ctx *c, Arena &ar, const uint32_t *at_ptr, cons
   for (int b = 0; b < kBins; ++b) bt.t[b] = h_thr[b];
   k_bin_bounds<<<1, 32, 0, ss>>>(n_items_a, sorted_work, kBins, bt, d_bounds);
   c->launches++;
+  // column order of B' (DESIGN.md 3.1, step 3): key = rank under (colB ascending, column id ascending), from a stable
+  // sort of the final post-sample marginals (identical on every rank).  B' is relabelled to keys IN PLACE: every B' is
+  // this train's own sampled copy, and A' (the B' of the self indicator) has already been transposed.  Like the
+  // schedule, it runs beside the previous indicator's row kernels.
+  int32_t *key_of_col, *first_key_of_cb, *order_id0, *order_id1;
+  uint32_t *order_cb0, *order_cb1;
+  const int32_t n_order = std::max<int32_t>(n_cols_b, 1);
+  CKR(ar.alloc(&key_of_col, n_order));
+  CKR(ar.alloc(&first_key_of_cb, (size_t)max_marg_b + 2));
+  CKR(ar.alloc(&order_cb0, n_order));
+  CKR(ar.alloc(&order_cb1, n_order));
+  CKR(ar.alloc(&order_id0, n_order));
+  CKR(ar.alloc(&order_id1, n_order));
+  order_cb = cub::DoubleBuffer<uint32_t>(order_cb0, order_cb1);
+  order_id = cub::DoubleBuffer<int32_t>(order_id0, order_id1);
+  if (n_cols_b > 0) {
+    k_col_order_init<<<grid_for(n_cols_b, 256, c->sm_count, 4), 256, 0, ss>>>(n_cols_b, B.marg, order_cb0, order_id0);
+    void *tmp;
+    CKR(ar.alloc((char **)&tmp, order_tb));
+    CK(cub::DeviceRadixSort::SortPairs(tmp, order_tb, order_cb, order_id, n_cols_b, 0, cb_bits, ss));
+    ar.release(tmp);
+    k_col_order<<<grid_for(n_cols_b, 256, c->sm_count, 4), 256, 0, ss>>>(n_cols_b, max_marg_b, order_cb.Current(), order_id.Current(),
+                                                                        key_of_col, first_key_of_cb);
+    k_relabel_cols<<<c->sm_count * 8, 256, 0, ss>>>(B.rp + B.n_rows, key_of_col, B.col);
+    c->launches += 3;
+  }
+  const int32_t *marg_key = reinterpret_cast<const int32_t *>(order_cb.Current()), *col_of_key = order_id.Current();
   if (beside) {
     cudaEvent_t scheduled;
     CKR(pooled_event(c, false, &scheduled));
     CK(cudaEventRecord(scheduled, ss));
     CK(cudaStreamWaitEvent(s, scheduled, 0));
   }
-  // per-column constants of B' for the fused LLR
+  // per-column constants of B' for the fused LLR, in key order
   ColTerm *col_terms;
   CKR(ar.alloc(&col_terms, std::max<int32_t>(n_cols_b, 1)));
   if (n_cols_b > 0) {
-    k_col_terms<<<grid_for(n_cols_b, 256, c->sm_count, 4), 256, 0, s>>>(n_cols_b, B.marg, n_users, flags, col_terms);
+    k_col_terms<<<grid_for(n_cols_b, 256, c->sm_count, 4), 256, 0, s>>>(n_cols_b, marg_key, col_of_key, n_users, flags, col_terms);
     c->launches++;
   }
   // 3. outputs ----------------------------------------------------------------------------------------
@@ -855,7 +889,11 @@ static int enqueue_indicator(cco_ctx *c, Arena &ar, const uint32_t *at_ptr, cons
   a.b_ptr = B.rp;
   a.b_col = B.col;
   a.marg_a = marg_a;
-  a.marg_b = B.marg;
+  a.marg_b = marg_key;
+  a.key_of_col = key_of_col;
+  a.first_key_of_cb = first_key_of_cb;
+  a.key_shift = 0;
+  while (((long long)std::max(n_cols_b - 1, 0) >> a.key_shift) >= kCutBins) ++a.key_shift;
   a.max_marg_b = max_marg_b;
   a.col_terms = col_terms;
   a.rows_sorted = rows_sorted;
@@ -1507,7 +1545,11 @@ static int ctx_init_device(cco_ctx *c) {
   for (auto &ev : c->tev) CK(cudaEventCreate(&ev));
   for (auto &ev : c->copy_ev) CK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
   for (auto &st : c->bin_stream) CK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
-  CK(cudaStreamCreateWithFlags(&c->sched_stream, cudaStreamNonBlocking));
+  // The schedule and column order of indicator i+1 are short dependent kernels on the path to its row kernels; at the
+  // highest priority their CTAs are dispatched ahead of the queued CTAs of indicator i's row kernels.
+  int lo_pri = 0, hi_pri = 0;
+  CK(cudaDeviceGetStreamPriorityRange(&lo_pri, &hi_pri));
+  CK(cudaStreamCreateWithPriority(&c->sched_stream, cudaStreamNonBlocking, hi_pri));
   for (auto &ev : c->bin_ev) CK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
   CK(cudaHostAlloc((void **)&c->mail_h, kMailBytes, cudaHostAllocMapped | cudaHostAllocPortable));
   CK(cudaHostGetDevicePointer((void **)&c->mail_d, c->mail_h, 0));

@@ -7,7 +7,8 @@
 //   H3 numNonZeroElementsPerColumn -> k_col_histogram (raw, before the allreduce), k_downsample_count or
 //                                 k_col_histogram_u32 (post-sample)
 //   `drmA.t`                   -> k_transpose_scatter
-//   scheduling                 -> k_row_work, k_bin_bounds, k_partition_rows; per-column LLR constants k_col_terms
+//   scheduling                 -> k_row_work, k_bin_bounds, k_partition_rows; column order of B' k_col_order_init /
+//                                 k_col_order / k_relabel_cols; per-column LLR constants k_col_terms
 //   H4 A'^T B' counts, H5 LLR, H6 top-k -> k_rows<GROUP, DENSE> (one fused kernel, nothing materialised)
 //   result assembly            -> k_len_to_i64, k_compact_rows; small device->host results k_mail_bytes
 //
@@ -30,9 +31,12 @@ struct RowArgs {
   const int32_t *at_users;
   // B' (CSR over users)
   const uint32_t *b_ptr;
-  const int32_t *b_col;
+  const int32_t *b_col;   // column KEYS (k_col_order): B' relabelled by the order (colB ascending, column id ascending)
   const int32_t *marg_a;  // colA, downsampled, per primary item
-  const int32_t *marg_b;  // colB, downsampled, per column of B'
+  const int32_t *marg_b;  // colB, downsampled, per column key (ascending)
+  const int32_t *key_of_col;       // column id -> key (the diagonal of A'^T A')
+  const int32_t *first_key_of_cb;  // [c] = first key whose colB >= c, for c in [0, max_marg_b + 1]
+  int32_t key_shift;      // (n_cols_b - 1) >> key_shift < kCutBins: first level of the key cut
   const uint2 *ext;       // experiment (tools/experiments/cco_rows2.cuh): (start, len) of B'[u] per (item, user) pair; unused
   int32_t max_marg_b;     // largest colB (bounds every co-occurrence count together with rowA)
   // schedule: items sorted by estimated work, descending; bin b = rows_sorted[bin_bounds[b], bin_bounds[b+1])
@@ -56,7 +60,7 @@ struct RowArgs {
   int32_t keep_max;    // M: a prune keeps between top_k and max(M, top_k) candidates
   int32_t final_max;   // the final sort runs on at most this many candidates (next_pow2(top_k))
   int32_t group_smem_bytes;  // shared memory of one group (multiple of 16)
-  const struct ColTerm *col_terms;  // per column of B': {columnEntropy, xLogX(colB - 1), colB}
+  const struct ColTerm *col_terms;  // per column key: {columnEntropy, xLogX(colB - 1), colB, column id}
   // outputs, strided
   int32_t out_stride;
   int32_t *out_col;
@@ -412,20 +416,52 @@ struct __align__(16) ColTerm {
   double col_e;     // entropy(cb, N - cb)
   double x_cbm1;    // xLogX(cb - 1): the k21 term of every k11 == 1 cell of this column
   int32_t cb;
-  int32_t pad[3];
+  int32_t col;      // original column id (what the output rows hold)
+  int32_t pad[2];
 };
-__global__ void k_col_terms(int32_t n_cols, const int32_t *__restrict__ marg, long long n_users, uint32_t flags,
-                            ColTerm *__restrict__ out) {
+// terms in key order: marg_key[k] = colB and col_of_key[k] = column id of key k (k_col_order)
+__global__ void k_col_terms(int32_t n_cols, const int32_t *__restrict__ marg_key, const int32_t *__restrict__ col_of_key,
+                            long long n_users, uint32_t flags, ColTerm *__restrict__ out) {
   const bool varargs = (flags & CCO_FLAG_ENTROPY_VARARGS) != 0;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_cols; i += gridDim.x * blockDim.x) {
-    long long cb = marg[i];
+    long long cb = marg_key[i];
     ColTerm t;
     t.col_e = entropy2(cb, n_users - cb, varargs);
     t.x_cbm1 = cb >= 1 ? xlogx(cb - 1) : 0.0;
     t.cb = (int32_t)cb;
-    t.pad[0] = t.pad[1] = t.pad[2] = 0;
+    t.col = col_of_key[i];
+    t.pad[0] = t.pad[1] = 0;
     out[i] = t;
   }
+}
+
+// ---- column order of B' (DESIGN.md 3.1, step 3) -------------------------------------------------------------------
+// key = rank of a column under (colB ascending, column id ascending).  k_col_order_init writes the (colB, id) pairs a
+// stable radix sort by colB turns into marg_key / col_of_key; k_col_order inverts the permutation and tabulates the
+// first key of every colB value.
+__global__ void k_col_order_init(int32_t n_cols, const int32_t *__restrict__ marg, uint32_t *__restrict__ cb_out,
+                                 int32_t *__restrict__ id_out) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_cols; i += gridDim.x * blockDim.x) {
+    cb_out[i] = (uint32_t)marg[i];
+    id_out[i] = i;
+  }
+}
+__global__ void k_col_order(int32_t n_cols, int32_t max_cb, const uint32_t *__restrict__ marg_key, const int32_t *__restrict__ col_of_key,
+                            int32_t *__restrict__ key_of_col, int32_t *__restrict__ first_key_of_cb) {
+  for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < n_cols; k += gridDim.x * blockDim.x) {
+    key_of_col[col_of_key[k]] = k;
+    // key k is the first key of every colB value in (marg_key[k - 1], marg_key[k]]; the last key also closes the table
+    const int32_t cb = (int32_t)marg_key[k], lo = k == 0 ? 0 : (int32_t)marg_key[k - 1] + 1;
+    for (int32_t c = lo; c <= cb; ++c) first_key_of_cb[c] = k;
+    if (k == n_cols - 1)
+      for (int32_t c = cb + 1; c <= max_cb + 1; ++c) first_key_of_cb[c] = n_cols;
+  }
+}
+// B' column ids -> keys, in place; the entry count is read on the device (*end = row_ptr[U])
+__global__ void k_relabel_cols(const uint32_t *__restrict__ end, const int32_t *__restrict__ key_of_col, int32_t *__restrict__ col) {
+  const long long n = *end;
+  for (long long q = blockIdx.x * (long long)blockDim.x + threadIdx.x; q < n; q += (long long)gridDim.x * blockDim.x)
+    col[q] = key_of_col[col[q]];
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -580,6 +616,39 @@ constexpr int kCutBins = 512;   // level-1 integer cut: u16 colB bins; they alia
 constexpr int kDomLevels = 15;  // dominance filter keeps cfail[1..15] in ctrl[41..55]
 constexpr int kX12N = 31;  // x12tab[j] = xLogX(ra - j) for j < 31; x12tab[31] = xLogX(N - ra)
 
+// One warp: the smallest of the kCutBins u16 bins of h1 at which the running count reaches `need` -> ctrl[9]
+// (0x7fffffff if the bins hold fewer cells), and the cells in the bins below it -> ctrl[10].
+__device__ __forceinline__ void cut_find(const uint32_t *h1, uint32_t need, int lane, int *ctrl) {
+  // lane l owns bins [16 l, 16 l + 16): 8 words
+  uint32_t sum = 0;
+  for (int wi = 0; wi < 8; ++wi) { const uint32_t v = h1[lane * 8 + wi]; sum += (v & 0xffffu) + (v >> 16); }
+  uint32_t incl = sum;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const uint32_t v = __shfl_up_sync(0xffffffffu, incl, d);
+    if (lane >= d) incl += v;
+  }
+  const uint32_t excl = incl - sum;
+  int found = 0x7fffffff;
+  uint32_t below = 0;
+  if (excl < need && incl >= need) {
+    uint32_t run = excl;
+    for (int wi = 0; wi < 8; ++wi) {
+      const uint32_t v = h1[lane * 8 + wi];
+      if (run + (v & 0xffffu) >= need) { found = lane * 16 + 2 * wi; below = run; break; }
+      run += v & 0xffffu;
+      if (run + (v >> 16) >= need) { found = lane * 16 + 2 * wi + 1; below = run; break; }
+      run += v >> 16;
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {   // at most one lane found the bin
+    found = min(found, __shfl_xor_sync(0xffffffffu, found, o));
+    below = max(below, __shfl_xor_sync(0xffffffffu, below, o));
+  }
+  if (lane == 0) { ctrl[9] = found; ctrl[10] = (int)below; }
+}
+
 template <int GROUP, bool DENSE>
 __device__ __forceinline__ void accumulate(uint32_t *table, uint32_t tsize, uint32_t b, int cbits, uint32_t n_pass,
                                            uint32_t pass, int *err_flag) {
@@ -676,6 +745,11 @@ __global__ void __launch_bounds__(GROUP == 32 ? 64 : GROUP, RowsMinBlocks<GROUP>
     const int item = a.rows_sorted[ri];
     const uint32_t u_begin = a.at_ptr[item], u_end = a.at_ptr[item + 1];
     const long long ra = a.marg_a[item];
+    const int diag = a.self ? a.key_of_col[item] : -1;   // the key of the A'^T A' diagonal cell
+    // Key path: 2 rowA colB < N for every column of B' (every row at C3 / C4), so every cell is strongly positive and both
+    // the level-1 cut and the dominance filter are monotone in colB -- hence in the key.  They compare keys, and no cell
+    // gathers its colB.  Other rows read colB from marg_b[key].
+    const bool keyed = 2ull * (unsigned long long)ra * (unsigned long long)a.max_marg_b < (unsigned long long)N;
     // table sized to the row: load factor <= 1/2 of the distinct-cell bound D = min(w, n_cols_b)
     uint32_t n_pass = 1, tsize = (uint32_t)a.n_cols_b;
     if (!DENSE) {
@@ -801,7 +875,7 @@ __global__ void __launch_bounds__(GROUP == 32 ? 64 : GROUP, RowsMinBlocks<GROUP>
         for (uint32_t q = lane; q < n_mine; q += 32) {
           const uint32_t word = table[seg_lo + q];
           const size_t o = (size_t)item * a.out_stride + emitted + basepos + q;
-          a.out_col[o] = (int32_t)(word >> cbits);
+          a.out_col[o] = a.col_terms[word >> cbits].col;
           a.out_cnt[o] = (int32_t)(word & cmask);
         }
         group_sync<GROUP>();
@@ -815,51 +889,43 @@ __global__ void __launch_bounds__(GROUP == 32 ? 64 : GROUP, RowsMinBlocks<GROUP>
       // On the strongly positive side (2*rowA*colB < k11*N) the LLR of k11 == 1 cells is strictly decreasing in colB, so
       // the smallest colB c1 with >= top_k such cells at or below it bounds the row's k-th best from below: k11 == 1 cells
       // with colB > c1 can never be kept and are dropped by an integer compare in the filter stage.
+      // Key path: c1 is the k-th smallest KEY of those cells (MSB-first radix select, 9 key bits per level): ties in
+      // colB are ordered by column id, the output's tie order, so the cut is exact and drops ties beyond the k-th too.
       int cut1 = 0x7fffffff;
       if (a.row_work[item] < 65536u) {   // u16 bins cannot overflow
-        for (int i = gtid; i < kCutBins / 2; i += GROUP) h1[i] = 0u;
-        group_sync<GROUP>();
-        for (uint32_t q0 = 0; q0 < n_mine; q0 += 32) {
-          const uint32_t q = q0 + lane;
-          if (q < n_mine) {
-            const uint32_t word = table[seg_lo + q];
-            const uint32_t b = word >> cbits;
-            if ((word & cmask) == 1u && !(a.self && (int)b == item)) {
-              const uint32_t cb = (uint32_t)a.marg_b[b];
-              if (cb < (uint32_t)kCutBins && 2ull * (unsigned long long)ra * cb < (unsigned long long)N)
-                atomicAdd(&h1[cb >> 1], 1u << (16u * (cb & 1u)));
+        int sh = keyed ? a.key_shift : 0, hi_sh = 32;   // level: bins over key bits [sh, hi_sh) of keys matching `prefix` above
+        uint32_t prefix = 0, need = (uint32_t)a.top_k;
+        while (true) {
+          for (int i = gtid; i < kCutBins / 2; i += GROUP) h1[i] = 0u;
+          group_sync<GROUP>();
+          for (uint32_t q0 = 0; q0 < n_mine; q0 += 32) {
+            const uint32_t q = q0 + lane;
+            if (q < n_mine) {
+              const uint32_t word = table[seg_lo + q];
+              const uint32_t b = word >> cbits;
+              if ((word & cmask) == 1u && (int)b != diag) {
+                uint32_t bin = kCutBins;
+                if (keyed) {
+                  if (((unsigned long long)(b ^ prefix) >> hi_sh) == 0) bin = (b >> sh) & (kCutBins - 1);
+                } else {
+                  const uint32_t cb = (uint32_t)a.marg_b[b];
+                  if (cb < (uint32_t)kCutBins && 2ull * (unsigned long long)ra * cb < (unsigned long long)N) bin = cb;
+                }
+                if (bin < (uint32_t)kCutBins) atomicAdd(&h1[bin >> 1], 1u << (16u * (bin & 1u)));
+              }
             }
           }
+          group_sync<GROUP>();
+          if (gtid < 32) cut_find(h1, need, lane, ctrl);
+          group_sync<GROUP>();
+          const int found = vctrl[9];
+          if (!keyed || found == 0x7fffffff) { cut1 = found; break; }
+          prefix |= (uint32_t)found << sh;
+          need -= (uint32_t)vctrl[10];
+          if (sh == 0) { cut1 = (int)prefix; break; }
+          hi_sh = sh;
+          sh = sh > 9 ? sh - 9 : 0;
         }
-        group_sync<GROUP>();
-        if (gtid < 32) {
-          // lane l owns bins [16 l, 16 l + 16): 8 words
-          uint32_t sum = 0;
-          for (int wi = 0; wi < 8; ++wi) { const uint32_t v = h1[gtid * 8 + wi]; sum += (v & 0xffffu) + (v >> 16); }
-          uint32_t incl = sum;
-#pragma unroll
-          for (int d = 1; d < 32; d <<= 1) {
-            const uint32_t v = __shfl_up_sync(0xffffffffu, incl, d);
-            if (gtid >= d) incl += v;
-          }
-          const uint32_t excl = incl - sum;
-          int found = 0x7fffffff;
-          if (excl < (uint32_t)a.top_k && incl >= (uint32_t)a.top_k) {
-            uint32_t run = excl;
-            for (int wi = 0; wi < 8 && found == 0x7fffffff; ++wi) {
-              const uint32_t v = h1[gtid * 8 + wi];
-              run += v & 0xffffu;
-              if (run >= (uint32_t)a.top_k) { found = gtid * 16 + 2 * wi; break; }
-              run += v >> 16;
-              if (run >= (uint32_t)a.top_k) { found = gtid * 16 + 2 * wi + 1; break; }
-            }
-          }
-#pragma unroll
-          for (int o = 16; o > 0; o >>= 1) found = min(found, __shfl_xor_sync(0xffffffffu, found, o));
-          if (gtid == 0) ctrl[9] = found;
-        }
-        group_sync<GROUP>();
-        cut1 = vctrl[9];
       }
       // ---- score + select -----------------------------------------------------------------------------------
       const double x_ra = x12tab[0], x_nra = x12tab[kX12N];
@@ -880,15 +946,21 @@ __global__ void __launch_bounds__(GROUP == 32 ? 64 : GROUP, RowsMinBlocks<GROUP>
           if (q < n_mine) {
             word = table[seg_lo + q];
             const uint32_t b = word >> cbits, k11 = word & cmask;
-            if (!(a.self && (int)b == item)) {
+            if ((int)b != diag) {
               // Dominance filter (exact, DESIGN.md "dominance"): for fixed rowA and N, on the positively associated
               // side (rowA*cb < k11*N) the LLR grows with k11 and shrinks with cb, so every evaluated cell (k, c) that
               // fails strictly on LLR proves that all cells (k' <= k, c' >= c) fail too; cfail[k'] = smallest such c.
-              const long long cb = a.marg_b[b];
-              const bool pos_side = (unsigned long long)ra * (unsigned long long)cb < (unsigned long long)k11 * (unsigned long long)N;
-              surv = !(pos_side && k11 <= (uint32_t)kDomLevels && (int)cb >= vctrl[40 + k11]);
-              if (k11 == 1u && (int)cb > cut1 && 2ull * (unsigned long long)ra * (unsigned long long)cb < (unsigned long long)N)
-                surv = false;   // beyond the level-1 integer cut
+              // Key path: every cell is on that side, cfail holds first_key_of_cb[c], and key >= it iff colB >= c.
+              if (keyed) {
+                surv = !(k11 <= (uint32_t)kDomLevels && (int)b >= vctrl[40 + k11]);
+                if (k11 == 1u && (int)b > cut1) surv = false;   // beyond the level-1 key cut
+              } else {
+                const long long cb = a.marg_b[b];
+                const bool pos_side = (unsigned long long)ra * (unsigned long long)cb < (unsigned long long)k11 * (unsigned long long)N;
+                surv = !(pos_side && k11 <= (uint32_t)kDomLevels && (int)cb >= vctrl[40 + k11]);
+                if (k11 == 1u && (int)cb > cut1 && 2ull * (unsigned long long)ra * (unsigned long long)cb < (unsigned long long)N)
+                  surv = false;   // beyond the level-1 integer cut
+              }
             }
           }
           const unsigned m = __ballot_sync(0xffffffffu, surv);
@@ -924,14 +996,16 @@ __global__ void __launch_bounds__(GROUP == 32 ? 64 : GROUP, RowsMinBlocks<GROUP>
           // (cells whose LLR rounds to 0 are cancellation noise: they teach nothing)
           bool strict_fail = v > 0.0 && !min_ok;
           const unsigned long long key = (unsigned long long)__double_as_longlong(v);
-          e = make_uint4((uint32_t)key, (uint32_t)(key >> 32), b, k11);
+          e = make_uint4((uint32_t)key, (uint32_t)(key >> 32), (uint32_t)ct.col, k11);
           if (pass_ok && vctrl[1]) {
             const uint4 thr = make_uint4((uint32_t)vctrl[4], (uint32_t)vctrl[5], (uint32_t)vctrl[6], (uint32_t)vctrl[7]);
             pass_ok = !cand_better(thr, e);
             strict_fail = e.y < thr.y || (e.y == thr.y && e.x < thr.x);
           }
-          if (strict_fail && pos_side)
-            for (uint32_t kk = kf; kk >= 1 && (int)cb < vctrl[40 + kk]; --kk) atomicMin(&ctrl[40 + kk], (int)cb);
+          if (strict_fail && pos_side) {
+            const int f = keyed ? a.first_key_of_cb[cb] : (int)cb;
+            for (uint32_t kk = kf; kk >= 1 && f < vctrl[40 + kk]; --kk) atomicMin(&ctrl[40 + kk], f);
+          }
         }
         qn -= take;
         const unsigned m = __ballot_sync(0xffffffffu, pass_ok);
