@@ -6,6 +6,7 @@ relative (in practice the device log matches glibc bit-for-bit on these inputs).
 import numpy as np
 import pytest
 
+import rowref
 import synth
 import universal_recommender_b200 as ur
 from conftest import load_golden, prepared_from_fixture
@@ -205,6 +206,7 @@ def test_empty_and_degenerate_inputs(orc, ctx):
     full = (6, 2, np.arange(0, 13, 2, dtype=np.int64), np.tile(np.array([0, 1], dtype=np.int32), 6))
     got = ctx.train_csr([full], [(500, 50, None)], seed=1)
     assert got[0][3][-1] == 0
+    rowref.assert_matches(rowref.expected(ctx, [full], [(500, 50, None)], 1), got, "item everybody bought")
 
 
 def test_error_behaviour(ctx):

@@ -11,6 +11,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <cmath>
 #include <functional>
 #include <cub/cub.cuh>
 #include <nvtx3/nvToolsExt.h>
@@ -702,6 +703,40 @@ static BinCfg make_cfg(cco_ctx *c, int group, int want_slots, int top_k, int n_c
   return f;
 }
 
+// ---- exactness of the level-1 cut and the dominance filter under fp64 rounding (DESIGN.md 3.1) ---------------------------
+// eps bounds |computed - real| of one LLR as k_rows (and llr_cells) evaluates it, u = 2^-53, M = N ln N:
+//   * xlogx(x) = fl(x * log(x)) with the device log within 1 ulp: relative error <= 2u + u + 2u^2 < 3.01u.  The terms
+//     enter the LLR as xN (once, net: the three copies are the same computed value) and three groups whose arguments
+//     sum to N -- {ra, N - ra}, {cb, N - cb}, {k11, k12, k21, k22} -- and x ln x is superadditive, so each group sums
+//     to <= M: the terms contribute <= 4 * 3.01u M.
+//   * ten additions / subtractions, eight with |result| <= M and two (sre, sre - mat_e) with |result| <= 2M:
+//     <= 12u M.  (The same holds for the ENTROPY_VARARGS order: its partial sums are also <= M.)
+//   * the final * 2 is exact: eps <= 2 (12.04 + 12) u M + O(u^2 M) < 64u M = 2^-47 M.  A computed 0 (the clamp of
+//     s < mat_e) only happens when the real LLR is below eps too.
+static double llr_error_bound(long long n_users) {
+  const double n = (double)n_users;
+  return n > 1.0 ? std::ldexp(n * std::log(n), -47) : 0.0;
+}
+// The cut drops k11 == 1 cells of colB c + 1 (and above) because they rank below cells of colB c.  Real-valued, with
+// r = rowA <= R = max rowA and c + 1 <= C = max colB:
+//   -dLLR/dx = 2 [-ln(1 - 1/x) - ln((N - x) / (N - x - r + 1))] >= 2 [1/x - (r - 1) / (N - x - r + 1)]
+// (-ln(1 - t) >= t and ln(1 + t) <= t), which decreases in x and in r, so over x in [c, c + 1]
+//   LLR(c) - LLR(c + 1) >= G1 = 2 [1/C - (R - 1) / (N - C - R + 1)]      (when N - C - R + 1 > 0).
+// When R C comes close to N / 2, G1 vanishes; there the dropped cell's side of the cut (2 r (c + 1) < N, so
+// N - x - r + 1 >= r x) gives -dLLR/dx >= 2 / (r x), hence a gap >= 2 / (r (c + 1)) >= G2 = 2 / min(R C, N / 2).
+// If max(G1, G2) > 2 eps, the computed values are strictly decreasing in colB too, and the cut (colB or key) is exact
+// for them.  Otherwise the rows run without it (same output, more evaluations).  With the default m = 500 every
+// marginal is ~560 and G1 ~ 3.5e-3, above 2 eps for every N < 2^31 (2 eps = 6.6e-4 there; 2.3e-6 at C4).  The cut goes
+// off only when max colB nears 1 / eps: ~7.6e4 at N = 1e8, ~3000 at N = 2^31.
+static bool cut_exact(long long n_users, int32_t max_marg_a, int32_t max_marg_b) {
+  const double n = (double)n_users, r = (double)max_marg_a, c = (double)max_marg_b;
+  if (r <= 0.0 || c <= 0.0) return true;
+  double g = 2.0 / std::min(r * c, 0.5 * n);
+  const double d = n - c - r + 1.0;
+  if (d > 0.0) g = std::max(g, 2.0 * (1.0 / c - (r - 1.0) / d));
+  return g > 2.0 * llr_error_bound(n_users);
+}
+
 // ---- one indicator = rows [lo, hi) of A'^T B' on this rank ---------------------------------------------------------------
 // enqueue_indicator puts everything of one indicator on the stream without a single host round trip (the rank partition,
 // the bin bounds and the packed sizes stay on the device); finish_indicator waits for that indicator's mailbox record
@@ -905,6 +940,8 @@ static int enqueue_indicator(cco_ctx *c, Arena &ar, const uint32_t *at_ptr, cons
   a.top_k = k_eff;
   a.has_min_llr = prm.has_min_llr;
   a.min_llr = prm.min_llr;
+  a.cut_ok = cut_exact(n_users, max_marg_a, max_marg_b) ? 1 : 0;
+  a.llr_eps2 = 2.0 * llr_error_bound(n_users);
   a.flags = flags;
   a.count_bits = count_bits;
   a.out_stride = stride;

@@ -50,6 +50,8 @@ struct RowArgs {
   int32_t top_k;
   int32_t has_min_llr;
   double min_llr;
+  int32_t cut_ok;    // the level-1 cut is exact for the computed LLRs at this (N, max rowA, max colB): cut_exact (cco_api.cu)
+  double llr_eps2;   // 2 eps: eps bounds |computed - real| of one fp64 LLR at this N (llr_error_bound, cco_api.cu)
   uint32_t flags;
   int32_t count_bits;  // packed hash word = (key << count_bits) | count
   int32_t slots;       // hash/dense table words in shared memory
@@ -885,14 +887,16 @@ __global__ void __launch_bounds__(GROUP == 32 ? 64 : GROUP, RowsMinBlocks<GROUP>
         group_sync<GROUP>();
         continue;
       }
-      // ---- level-1 integer cut (exact; DESIGN.md 8.1) ---------------------------------------------------------------
-      // On the strongly positive side (2*rowA*colB < k11*N) the LLR of k11 == 1 cells is strictly decreasing in colB, so
+      // ---- level-1 integer cut (exact; DESIGN.md 3.1) ---------------------------------------------------------------
+      // On the strongly positive side (2*rowA*colB < N) the real LLR of k11 == 1 cells is strictly decreasing in colB, so
       // the smallest colB c1 with >= top_k such cells at or below it bounds the row's k-th best from below: k11 == 1 cells
       // with colB > c1 can never be kept and are dropped by an integer compare in the filter stage.
       // Key path: c1 is the k-th smallest KEY of those cells (MSB-first radix select, 9 key bits per level): ties in
       // colB are ordered by column id, the output's tie order, so the cut is exact and drops ties beyond the k-th too.
+      // Both hold for the COMPUTED fp64 values only when adjacent colB values are further apart than the evaluation
+      // error: the host checks that once per indicator (a.cut_ok) and otherwise the row runs without the cut.
       int cut1 = 0x7fffffff;
-      if (a.row_work[item] < 65536u) {   // u16 bins cannot overflow
+      if (a.cut_ok && a.row_work[item] < 65536u) {   // u16 bins cannot overflow
         int sh = keyed ? a.key_shift : 0, hi_sh = 32;   // level: bins over key bits [sh, hi_sh) of keys matching `prefix` above
         uint32_t prefix = 0, need = (uint32_t)a.top_k;
         while (true) {
@@ -948,8 +952,8 @@ __global__ void __launch_bounds__(GROUP == 32 ? 64 : GROUP, RowsMinBlocks<GROUP>
             const uint32_t b = word >> cbits, k11 = word & cmask;
             if ((int)b != diag) {
               // Dominance filter (exact, DESIGN.md "dominance"): for fixed rowA and N, on the positively associated
-              // side (rowA*cb < k11*N) the LLR grows with k11 and shrinks with cb, so every evaluated cell (k, c) that
-              // fails strictly on LLR proves that all cells (k' <= k, c' >= c) fail too; cfail[k'] = smallest such c.
+              // side (rowA*cb < k11*N) the real LLR grows with k11 and shrinks with cb, so every evaluated cell (k, c) that
+              // fails by more than 2 eps proves that all cells (k' <= k, c' >= c) fail too; cfail[k'] = smallest such c.
               // Key path: every cell is on that side, cfail holds first_key_of_cb[c], and key >= it iff colB >= c.
               if (keyed) {
                 surv = !(k11 <= (uint32_t)kDomLevels && (int)b >= vctrl[40 + k11]);
@@ -994,13 +998,16 @@ __global__ void __launch_bounds__(GROUP == 32 ? 64 : GROUP, RowsMinBlocks<GROUP>
           const bool min_ok = !a.has_min_llr || v >= a.min_llr;
           pass_ok = v > 0.0 && min_ok;
           // (cells whose LLR rounds to 0 are cancellation noise: they teach nothing)
-          bool strict_fail = v > 0.0 && !min_ok;
+          // A failing cell proves that the cells it dominates fail only if it misses the bar T (minLLR or the running
+          // threshold) by more than 2 eps: their computed LLR is at most v + 2 eps (DESIGN.md 3.1, "dominance").
+          const double vm = __dadd_rn(v, a.llr_eps2);
+          bool strict_fail = v > 0.0 && !min_ok && vm < a.min_llr;
           const unsigned long long key = (unsigned long long)__double_as_longlong(v);
           e = make_uint4((uint32_t)key, (uint32_t)(key >> 32), (uint32_t)ct.col, k11);
           if (pass_ok && vctrl[1]) {
             const uint4 thr = make_uint4((uint32_t)vctrl[4], (uint32_t)vctrl[5], (uint32_t)vctrl[6], (uint32_t)vctrl[7]);
             pass_ok = !cand_better(thr, e);
-            strict_fail = e.y < thr.y || (e.y == thr.y && e.x < thr.x);
+            strict_fail = vm < __hiloint2double((int)thr.y, (int)thr.x);
           }
           if (strict_fail && pos_side) {
             const int f = keyed ? a.first_key_of_cb[cb] : (int)cb;
