@@ -293,6 +293,33 @@ int cco_format_es_bulk(cco_ctx_t *ctx, const cco_result_t *res, int32_t n_names,
                        const cco_dictionary_t *row_ids, const cco_dictionary_t *col_ids, char **out_bytes, int64_t *out_len);
 
 /*
+ * SURVEY.md 8f-1 on string ids: Preparator.prepare (src/main/scala/Preparator.scala:44-87, 100-216) on (user id, item id)
+ * byte strings, dictionaries included.  Type 0 is the primary event.  Exactly what the host mirror preparator.prepare returns:
+ *  - user dictionary: users with >= max(min_events_per_user, 1) primary events (duplicates count, :129-132), ordered by
+ *    first appearance in the primary stream;
+ *  - events of type t survive iff their user is in the user dictionary (:175-178);
+ *  - item dictionary of type t: items with a surviving event of type t, ordered by first appearance among those events;
+ *  - matrix t: binary CSR over the user dictionary, duplicates collapsed, columns ascending.
+ * Ids are arbitrary byte strings compared bytewise (UTF-8 of a Python str; the empty string is an id), in the Arrow
+ * large_string layout: id e = bytes[offsets[e] .. offsets[e + 1]).  n_events < 2^31 per type.  Offsets below 0, decreasing
+ * offsets and offsets[0] > offsets[n] give CCO_E_INVALID_ARG before any kernel reads bytes through them.  The dataset is
+ * resident like one from cco_ingest (every rank of a multi-GPU job builds the whole matrices and works on its user block);
+ * per-GPU contexts only, as every resident dataset.
+ */
+typedef struct {
+  int64_t n_events;
+  const int64_t *user_offsets; /* [n_events + 1] */
+  const char *user_bytes;
+  const int64_t *item_offsets; /* [n_events + 1] */
+  const char *item_bytes;
+} cco_string_events_t;
+int cco_ingest_strings(cco_ctx_t *ctx, int32_t n_types, const cco_string_events_t *events, int32_t min_events_per_user,
+                       cco_dataset_t **out);
+/* which = -1: the user dictionary; which = t: the item dictionary of type t.  Pinned host memory owned by the dataset,
+ * valid until cco_dataset_free.  CCO_E_INVALID_ARG on datasets that were not built from strings. */
+int cco_dataset_dictionary(const cco_dataset_t *ds, int32_t which, cco_dictionary_t *out);
+
+/*
  * Next row (SURVEY.md 8f-3): the backfill ranks of PopModel (src/main/scala/PopModel.scala:113-182) as per-item event
  * histograms over 1 / 2 / 3 time buckets of [start_ms, end_ms) -- what URAlgorithm.getRanksRDD (URAlgorithm.scala:537-560)
  * joins into the model.  events: (item index, event time in epoch milliseconds), already restricted to the ranking's event
@@ -319,6 +346,10 @@ int cco_debug_downsample(cco_ctx_t *ctx, const cco_csr_t *m, int32_t max_interac
 /* Debug/parity entry (tests only): the device LLR of n cells. */
 int cco_debug_llr(cco_ctx_t *ctx, int64_t n, const int64_t *k11, const int64_t *k12, const int64_t *k21,
                   const int64_t *k22, uint32_t flags, double *out);
+/* Debug/parity entry (tests only): the string-dictionary stage of cco_ingest_strings on one column, with the hash
+ * truncated to hash_bits (0..64) bits so that distinct ids collide on purpose.  ids[e] = dictionary id of id e, the
+ * dictionary ordered by first appearance; the result is the same for every hash_bits. */
+int cco_debug_string_ids(cco_ctx_t *ctx, int64_t n, const int64_t *offsets, const char *bytes, int32_t hash_bits, int32_t *ids);
 void cco_free(void *p);
 
 #ifdef __cplusplus

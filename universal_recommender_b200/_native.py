@@ -61,6 +61,11 @@ class DictionaryT(C.Structure):
     _fields_ = [("n", C.c_int64), ("offsets", C.POINTER(C.c_int64)), ("bytes", C.c_char_p)]
 
 
+class StringEventsT(C.Structure):
+    _fields_ = [("n_events", C.c_int64), ("user_offsets", C.POINTER(C.c_int64)), ("user_bytes", C.c_void_p),
+                ("item_offsets", C.POINTER(C.c_int64)), ("item_bytes", C.c_void_p)]
+
+
 class StatsT(C.Structure):
     _fields_ = [("n_users", C.c_int64), ("nnz_in_total", C.c_int64),
                 ("nnz_downsampled", C.c_int64 * 16), ("products", C.c_int64 * 16),
@@ -76,9 +81,9 @@ EXPORTS = [
     "cco_create", "cco_create_group", "cco_destroy", "cco_host_alloc", "cco_host_free", "cco_train", "cco_cooccurrences_idss",
     "cco_dataset_upload", "cco_train_dataset", "cco_dataset_free", "cco_timer_start", "cco_timer_stop",
     "cco_partition_rows", "cco_ingest", "cco_synth_ingest", "cco_dataset_shape", "cco_dataset_download",
-    "cco_dataset_copy_to_host", "cco_format_es_bulk", "cco_pop_model",
+    "cco_dataset_copy_to_host", "cco_format_es_bulk", "cco_ingest_strings", "cco_dataset_dictionary", "cco_pop_model",
     "cco_result_num_matrices", "cco_result_row_range", "cco_result_matrix", "cco_result_stats", "cco_result_free",
-    "cco_debug_cooccurrence", "cco_debug_downsample", "cco_debug_llr", "cco_free",
+    "cco_debug_cooccurrence", "cco_debug_downsample", "cco_debug_llr", "cco_debug_string_ids", "cco_free",
 ]
 
 _lib = None
@@ -117,6 +122,8 @@ def lib():
     L.cco_dataset_copy_to_host.argtypes = [C.c_void_p, C.c_int32, p(C.c_int64), p(C.c_int32)]
     L.cco_format_es_bulk.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, p(C.c_char_p), p(DictionaryT), p(DictionaryT), p(C.c_void_p),
                                      p(C.c_int64)]
+    L.cco_ingest_strings.argtypes = [C.c_void_p, C.c_int32, p(StringEventsT), C.c_int32, p(C.c_void_p)]
+    L.cco_dataset_dictionary.argtypes = [C.c_void_p, C.c_int32, p(DictionaryT)]
     L.cco_pop_model.argtypes = [C.c_void_p, C.c_int32, C.c_int64, p(C.c_int32), p(C.c_int64), C.c_int32, C.c_int64, C.c_int64, p(C.c_double),
                                 p(C.c_ubyte)]
     L.cco_dataset_shape.argtypes = [C.c_void_p, C.c_int32, p(C.c_int64), p(C.c_int32), p(C.c_int64)]
@@ -134,6 +141,7 @@ def lib():
                                        p(p(C.c_int32)), p(C.c_int32), p(C.c_int32)]
     L.cco_debug_llr.argtypes = [C.c_void_p, C.c_int64, p(C.c_int64), p(C.c_int64), p(C.c_int64), p(C.c_int64), C.c_uint32,
                                 p(C.c_double)]
+    L.cco_debug_string_ids.argtypes = [C.c_void_p, C.c_int64, p(C.c_int64), C.c_void_p, C.c_int32, p(C.c_int32)]
     L.cco_free.argtypes = [C.c_void_p]
     L.cco_free.restype = None
     _lib = L

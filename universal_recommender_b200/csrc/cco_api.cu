@@ -25,6 +25,7 @@
 #include "cco_kernels.cuh"
 #include "cco_sampler.cuh"
 #include "cco_format.cuh"
+#include "cco_strings.cuh"
 
 namespace cco {
 
@@ -237,6 +238,8 @@ struct cco_dataset {
   bool validated = false;          // k_check_rows has run (and the rows are canonical)
   bool whole = false;              // rp_alloc / col_alloc hold the WHOLE matrices (device-built datasets, single-GPU uploads)
   float ms_h2d = 0;
+  // cco_ingest_strings: [0] the user dictionary, [1 + t] the item dictionary of type t, in pinned memory of the context
+  std::vector<cco_dictionary_t> dicts;
 };
 
 struct cco_result {
@@ -1134,6 +1137,10 @@ static void dataset_release(cco_dataset *d) {
     if (p) cudaFreeAsync(p, d->ctx->stream);
   for (auto e : d->ready)
     if (e) cudaEventDestroy(e);
+  for (auto &dc : d->dicts) {
+    if (dc.offsets) d->ctx->pinned_put((void *)dc.offsets);
+    if (dc.bytes) d->ctx->pinned_put((void *)dc.bytes);
+  }
   delete d;
 }
 
@@ -1821,15 +1828,8 @@ struct IngestSource {
   std::function<int(int, long long *, int32_t *)> fill;
 };
 
-static int ingest_core(cco_ctx *c, const IngestSource &src, int32_t min_events_per_user, int32_t *user_map,
-                       int32_t *const *item_maps, cco_dataset **out) {
-  const int n_types = src.n_types;
-  const long long n_users_raw = src.n_users_raw;
-  *out = nullptr;
-  CK(cudaSetDevice(c->device));
-  cudaStream_t s = c->stream;
-  mail_reset(c);
-  Arena ar(s);
+// an empty device-built dataset of n_types matrices: canonical by construction, every rank holds the whole matrices
+static cco_dataset *ingest_dataset_new(cco_ctx *c, int n_types) {
   cco_dataset *d = new cco_dataset();
   d->ctx = c;
   d->n_mats = n_types;
@@ -1845,6 +1845,95 @@ static int ingest_core(cco_ctx *c, const IngestSource &src, int32_t min_events_p
   d->ready.assign(n_types, nullptr);
   d->validated = true;   // built here: canonical by construction
   d->whole = true;
+  return d;
+}
+
+// binary CSR of matrix t (n_users rows) from the (user << 32 | item) keys of its ne events in k0 (dropped events carry ~0,
+// `kept` do not): radix sort, unique, row_ptr.  k1 is scratch of ne keys.
+static int ingest_csr(cco_ctx *c, Arena &ar, cco_dataset *d, int t, long long ne, uint32_t n_users, unsigned long long *k0,
+                      unsigned long long *k1, unsigned long long kept) {
+  cudaStream_t s = c->stream;
+  void *p = nullptr;
+  cudaError_t e = cudaMallocAsync(&p, sizeof(int64_t) * ((size_t)n_users + 1), s);
+  if (e != cudaSuccess) return set_error(CCO_E_OOM, "cudaMallocAsync row_ptr: %s", cudaGetErrorString(e));
+  d->rp[t] = (long long *)p;
+  d->rp_alloc[t] = p;
+  e = cudaMallocAsync(&p, sizeof(int32_t) * (size_t)std::max<unsigned long long>(kept, 4), s);
+  if (e != cudaSuccess) return set_error(CCO_E_OOM, "cudaMallocAsync col_idx: %s", cudaGetErrorString(e));
+  d->col[t] = (int32_t *)p;
+  d->col_alloc[t] = p;
+  CK(cudaEventCreateWithFlags(&d->ready[t], cudaEventDisableTiming));
+  long long n_unique = 0;
+  if (kept > 0) {
+    int row_bits = 1;
+    while ((1LL << row_bits) < (long long)n_users) ++row_bits;
+    cub::DoubleBuffer<unsigned long long> db(k0, k1);
+    size_t tb = 0;
+    // dropped events carry the key ~0 and sort to the end: all 64 bits take part
+    CK(cub::DeviceRadixSort::SortKeys(nullptr, tb, db, (long long)ne, 0, 64, s));
+    void *tmp;
+    CKR(ar.alloc((char **)&tmp, tb));
+    CK(cub::DeviceRadixSort::SortKeys(tmp, tb, db, (long long)ne, 0, 64, s));
+    ar.release(tmp);
+    unsigned long long *sorted = db.Current(), *other = db.Alternate();
+    uint32_t *flag, *pos;
+    CKR(ar.alloc(&flag, kept + 1));
+    CKR(ar.alloc(&pos, kept + 1));
+    CK(cudaMemsetAsync(flag + kept, 0, 4, s));
+    k_unique_flags<<<grid_for((long long)kept, 256, c->sm_count), 256, 0, s>>>((long long)kept, sorted, flag);
+    CKR(exclusive_sum_u32(c, ar, flag, pos, (long long)kept + 1));
+    uint32_t nuq = 0;
+    CKR(mail_fetch(c, &nuq, pos + kept, 4));
+    k_unique_scatter<<<grid_for((long long)kept, 256, c->sm_count), 256, 0, s>>>((long long)kept, sorted, flag, pos, other, d->col[t]);
+    CKR(mail_wait(c));
+    n_unique = nuq;
+    k_rowptr_from_keys<<<grid_for((long long)n_users + 1, 256, c->sm_count), 256, 0, s>>>((long long)n_users, n_unique, other, d->rp[t]);
+    c->launches += 3;
+    ar.release(flag);
+    ar.release(pos);
+  } else {
+    CK(cudaMemsetAsync(d->rp[t], 0, sizeof(int64_t) * ((size_t)n_users + 1), s));
+  }
+  d->nnz[t] = n_unique;
+  CK(cudaEventRecord(d->ready[t], s));
+  return CCO_OK;
+}
+
+// every rank of a multi-GPU job builds the whole matrices (the events are all here) and then works on its block of
+// users like an uploaded dataset does; the block sizes (padding of the column-block all-gather) come from row_ptr
+static int ingest_blocks(cco_ctx *c, cco_dataset *d, uint32_t n_users) {
+  const int n_types = d->n_mats;
+  long long u_lo, u_hi;
+  user_block(n_users, c->world, c->rank, &u_lo, &u_hi);
+  d->row_base = u_lo;
+  d->n_local = u_hi - u_lo;
+  std::vector<std::vector<long long>> edge(n_types, std::vector<long long>((size_t)c->world + 1, 0));
+  for (int t = 0; t < n_types; ++t)
+    for (int q = 0; q <= c->world; ++q) {
+      long long a0, a1;
+      user_block(n_users, c->world, std::min(q, c->world - 1), &a0, &a1);
+      CKR(mail_fetch(c, &edge[t][q], d->rp[t] + (q < c->world ? a0 : a1), 8));
+    }
+  CKR(mail_wait(c));
+  for (int t = 0; t < n_types; ++t) {
+    for (int q = 0; q < c->world; ++q) d->block_cap[t] = std::max(d->block_cap[t], edge[t][q + 1] - edge[t][q]);
+    d->q_lo[t] = edge[t][c->rank];
+    d->q_hi[t] = edge[t][c->rank + 1];
+    d->rp[t] += u_lo;   // views of the block; rp_alloc / col_alloc keep the whole matrices
+  }
+  return CCO_OK;
+}
+
+static int ingest_core(cco_ctx *c, const IngestSource &src, int32_t min_events_per_user, int32_t *user_map,
+                       int32_t *const *item_maps, cco_dataset **out) {
+  const int n_types = src.n_types;
+  const long long n_users_raw = src.n_users_raw;
+  *out = nullptr;
+  CK(cudaSetDevice(c->device));
+  cudaStream_t s = c->stream;
+  mail_reset(c);
+  Arena ar(s);
+  cco_dataset *d = ingest_dataset_new(c, n_types);
   struct G {
     cco_dataset *d;
     bool ok = false;
@@ -1917,75 +2006,14 @@ static int ingest_core(cco_ctx *c, const IngestSource &src, int32_t min_events_p
     ar.release(d_user);   // the raw events are dead once the keys exist
     ar.release(d_item);
     d->n_cols[t] = n_items;
-    void *p = nullptr;
-    cudaError_t e = cudaMallocAsync(&p, sizeof(int64_t) * ((size_t)n_users + 1), s);
-    if (e != cudaSuccess) return set_error(CCO_E_OOM, "cudaMallocAsync row_ptr: %s", cudaGetErrorString(e));
-    d->rp[t] = (long long *)p;
-    d->rp_alloc[t] = p;
-    e = cudaMallocAsync(&p, sizeof(int32_t) * (size_t)std::max<unsigned long long>(kept, 4), s);
-    if (e != cudaSuccess) return set_error(CCO_E_OOM, "cudaMallocAsync col_idx: %s", cudaGetErrorString(e));
-    d->col[t] = (int32_t *)p;
-    d->col_alloc[t] = p;
-    CK(cudaEventCreateWithFlags(&d->ready[t], cudaEventDisableTiming));
-    long long n_unique = 0;
-    if (kept > 0) {
-      int row_bits = 1;
-      while ((1LL << row_bits) < (long long)n_users) ++row_bits;
-      cub::DoubleBuffer<unsigned long long> db(k0, k1);
-      size_t tb = 0;
-      // dropped events carry the key ~0 and sort to the end: all 64 bits take part
-      CK(cub::DeviceRadixSort::SortKeys(nullptr, tb, db, (long long)ne, 0, 64, s));
-      void *tmp;
-      CKR(ar.alloc((char **)&tmp, tb));
-      CK(cub::DeviceRadixSort::SortKeys(tmp, tb, db, (long long)ne, 0, 64, s));
-      ar.release(tmp);
-      unsigned long long *sorted = db.Current(), *other = db.Alternate();
-      uint32_t *flag, *pos;
-      CKR(ar.alloc(&flag, kept + 1));
-      CKR(ar.alloc(&pos, kept + 1));
-      CK(cudaMemsetAsync(flag + kept, 0, 4, s));
-      k_unique_flags<<<grid_for((long long)kept, 256, c->sm_count), 256, 0, s>>>((long long)kept, sorted, flag);
-      CKR(exclusive_sum_u32(c, ar, flag, pos, (long long)kept + 1));
-      uint32_t nuq = 0;
-      CKR(mail_fetch(c, &nuq, pos + kept, 4));
-      k_unique_scatter<<<grid_for((long long)kept, 256, c->sm_count), 256, 0, s>>>((long long)kept, sorted, flag, pos, other, d->col[t]);
-      CKR(mail_wait(c));
-      n_unique = nuq;
-      k_rowptr_from_keys<<<grid_for((long long)n_users + 1, 256, c->sm_count), 256, 0, s>>>((long long)n_users, n_unique, other, d->rp[t]);
-      c->launches += 3;
-      ar.release(flag);
-      ar.release(pos);
-    } else {
-      CK(cudaMemsetAsync(d->rp[t], 0, sizeof(int64_t) * ((size_t)n_users + 1), s));
-    }
-    d->nnz[t] = n_unique;
-    CK(cudaEventRecord(d->ready[t], s));
+    CKR(ingest_csr(c, ar, d, t, ne, n_users, k0, k1, kept));
     ar.release(k0);
     ar.release(k1);
     ar.release(iflag);
     ar.release(ipos);
     ar.release(d_item_map);
   }
-  // every rank of a multi-GPU job builds the whole matrices (the events are all here) and then works on its block of
-  // users like an uploaded dataset does; the block sizes (padding of the column-block all-gather) come from row_ptr
-  long long u_lo, u_hi;
-  user_block(n_users, c->world, c->rank, &u_lo, &u_hi);
-  d->row_base = u_lo;
-  d->n_local = u_hi - u_lo;
-  std::vector<std::vector<long long>> edge(n_types, std::vector<long long>((size_t)c->world + 1, 0));
-  for (int t = 0; t < n_types; ++t)
-    for (int q = 0; q <= c->world; ++q) {
-      long long a0, a1;
-      user_block(n_users, c->world, std::min(q, c->world - 1), &a0, &a1);
-      CKR(mail_fetch(c, &edge[t][q], d->rp[t] + (q < c->world ? a0 : a1), 8));
-    }
-  CKR(mail_wait(c));
-  for (int t = 0; t < n_types; ++t) {
-    for (int q = 0; q < c->world; ++q) d->block_cap[t] = std::max(d->block_cap[t], edge[t][q + 1] - edge[t][q]);
-    d->q_lo[t] = edge[t][c->rank];
-    d->q_hi[t] = edge[t][c->rank + 1];
-    d->rp[t] += u_lo;   // views of the block; rp_alloc / col_alloc keep the whole matrices
-  }
+  CKR(ingest_blocks(c, d, n_users));
   CK(cudaStreamSynchronize(s));
   CK(cudaGetLastError());
   g.ok = true;
@@ -2073,6 +2101,321 @@ int cco_synth_ingest(cco_ctx_t *c, int32_t n_types, const cco_synth_type_t *type
   rc = ingest_core(c, src, min_events_per_user, nullptr, nullptr, out);
   drop();
   return rc;
+}
+
+// ---- SURVEY.md 8f-1 on string ids: cco_ingest_strings (kernels in cco_strings.cuh) ------------------------------------
+namespace cco {
+// one column of string ids in HBM
+struct DevStrCol {
+  long long n = 0, base = 0;   // base = the caller's offsets[0]: byte offsets index the uploaded buffer as off[i] - base
+  long long *off = nullptr;    // [n + 1], the caller's values
+  uint64_t *w = nullptr;       // bytes [off[0], off[n]) as 8-byte words, 16 bytes of padding
+  uint64_t *hash = nullptr;    // [n]
+};
+// the host-side checks of a column (the device checks that no offset decreases before any kernel reads bytes through them)
+static int str_check_host(long long n, const int64_t *off, const char *bytes, int t, const char *what) {
+  if (n < 0) return set_error(CCO_E_INVALID_ARG, "type %d: negative event count", t);
+  if (n >= 0x7fffffffLL) return set_error(CCO_E_UNSUPPORTED, "type %d: %lld events, string ingest takes < 2^31 per type", t, n);
+  if (n == 0) return CCO_OK;
+  if (!off) return set_error(CCO_E_INVALID_ARG, "type %d: null %s offsets", t, what);
+  if (off[0] < 0) return set_error(CCO_E_INVALID_ARG, "type %d: %s offsets[0] = %lld is negative", t, what, (long long)off[0]);
+  if (off[0] > off[n])
+    return set_error(CCO_E_INVALID_ARG, "type %d: %s offsets[0] = %lld > offsets[n] = %lld", t, what, (long long)off[0], (long long)off[n]);
+  if (off[n] > off[0] && !bytes) return set_error(CCO_E_INVALID_ARG, "type %d: null %s bytes", t, what);
+  return CCO_OK;
+}
+static int str_upload(cco_ctx *c, Arena &ar, long long n, const int64_t *off, const char *bytes, DevStrCol *col) {
+  cudaStream_t s = c->stream;
+  col->n = n;
+  col->base = n > 0 ? off[0] : 0;
+  const long long nb = n > 0 ? off[n] - off[0] : 0;
+  CKR(ar.alloc(&col->off, n + 1));
+  CKR(ar.alloc(&col->w, (nb + 16 + 7) / 8));
+  CKR(ar.alloc(&col->hash, std::max<long long>(n, 1)));
+  if (n > 0) {
+    CK(cudaMemcpyAsync(col->off, off, sizeof(int64_t) * ((size_t)n + 1), cudaMemcpyHostToDevice, s));
+    if (nb > 0) CK(cudaMemcpyAsync(col->w, bytes + off[0], (size_t)nb, cudaMemcpyHostToDevice, s));
+  }
+  return CCO_OK;
+}
+static void str_release(Arena &ar, DevStrCol &col) {
+  ar.release(col.off);
+  ar.release(col.w);
+  ar.release(col.hash);
+}
+// launch the decreasing-offset check of a column into *bad
+static void str_check_device(cco_ctx *c, const DevStrCol &col, int *bad) {
+  if (col.n == 0) return;
+  k_str_check<<<grid_for(col.n, 256, c->sm_count), 256, 0, c->stream>>>(col.n, col.off, bad);
+  c->launches++;
+}
+static void str_hash(cco_ctx *c, const DevStrCol &col, uint64_t mask) {
+  if (col.n == 0) return;
+  k_str_hash<<<grid_for(col.n, 256, c->sm_count), 256, 0, c->stream>>>(col.n, col.off, col.base, col.w, mask, col.hash);
+  c->launches++;
+}
+
+// the string table of one column and the dictionary it defines
+struct StrTable {
+  long long cap = 0;                // power of two, > 1.5 x the ids inserted
+  uint32_t *table = nullptr;        // [cap]: index of the id that claimed the slot, kStrEmpty
+  uint32_t *slot_of = nullptr;      // [n]: slot of each id, kStrEmpty for gated ids
+  uint32_t *first = nullptr;        // [cap]: first index of the slot's string
+  uint32_t *count = nullptr;        // [cap]: ids of the slot (primary user column only)
+  int32_t *rank_of_slot = nullptr;  // [cap]: dictionary id, -1
+  uint32_t *first_sorted = nullptr; // [n_groups]: first index of each dictionary entry, in dictionary order
+  long long n_groups = 0;
+};
+static void str_table_release(Arena &ar, StrTable &tb) {
+  for (void *p : {(void *)tb.table, (void *)tb.slot_of, (void *)tb.first, (void *)tb.count, (void *)tb.rank_of_slot, (void *)tb.first_sorted})
+    if (p) ar.release(p);
+  tb = StrTable();
+}
+// Group the ids of a column by string (exact: hash, then bytes), keep the groups with >= need ids (counting) or all of them,
+// number them by first appearance, and write each id's dictionary id (-1: gated or filtered out).  gate[i] < 0 keeps id i
+// out of the table, so `first` is the first appearance among the ids that pass the gate.
+static int str_group(cco_ctx *c, Arena &ar, const DevStrCol &col, const int32_t *gate, bool counting, uint32_t need, StrTable *tb,
+                     int32_t *id) {
+  cudaStream_t s = c->stream;
+  const long long n = col.n;
+  long long cap = 64;
+  while (cap < n + n / 2 + 1) cap <<= 1;
+  tb->cap = cap;
+  CKR(ar.alloc(&tb->table, cap));
+  CKR(ar.alloc(&tb->slot_of, std::max<long long>(n, 1)));
+  CKR(ar.alloc(&tb->first, cap));
+  CKR(ar.alloc(&tb->rank_of_slot, cap));
+  CK(cudaMemsetAsync(tb->table, 0xff, sizeof(uint32_t) * (size_t)cap, s));
+  CK(cudaMemsetAsync(tb->first, 0xff, sizeof(uint32_t) * (size_t)cap, s));
+  CK(cudaMemsetAsync(tb->rank_of_slot, 0xff, sizeof(int32_t) * (size_t)cap, s));
+  if (counting) {
+    CKR(ar.alloc(&tb->count, cap));
+    CK(cudaMemsetAsync(tb->count, 0, sizeof(uint32_t) * (size_t)cap, s));
+  }
+  if (n > 0) {
+    k_str_insert<<<grid_for(n, 256, c->sm_count), 256, 0, s>>>(n, col.off, col.base, col.w, col.hash, gate, (uint64_t)cap - 1, tb->table,
+                                                              tb->slot_of, tb->first, tb->count);
+    c->launches++;
+  }
+  uint32_t *flag, *pos;
+  CKR(ar.alloc(&flag, cap + 1));
+  CKR(ar.alloc(&pos, cap + 1));
+  CK(cudaMemsetAsync(flag + cap, 0, 4, s));
+  k_str_flags<<<grid_for(cap, 256, c->sm_count), 256, 0, s>>>(cap, tb->table, tb->count, need, flag);
+  CKR(exclusive_sum_u32(c, ar, flag, pos, cap + 1));
+  uint32_t ng = 0;
+  CKR(mail_fetch(c, &ng, pos + cap, 4));
+  CKR(mail_wait(c));
+  tb->n_groups = ng;
+  CKR(ar.alloc(&tb->first_sorted, std::max<long long>(ng, 1)));
+  if (ng > 0) {
+    uint32_t *k0, *v0, *v1;
+    CKR(ar.alloc(&k0, ng));
+    CKR(ar.alloc(&v0, ng));
+    CKR(ar.alloc(&v1, ng));
+    k_str_compact<<<grid_for(cap, 256, c->sm_count), 256, 0, s>>>(cap, flag, pos, tb->first, k0, v0);
+    // first indices are distinct: the sort by them is the dictionary order
+    int bits = 1;
+    while ((1LL << bits) < n) ++bits;
+    cub::DoubleBuffer<uint32_t> kb(k0, tb->first_sorted), vb(v0, v1);
+    size_t tbytes = 0;
+    CK(cub::DeviceRadixSort::SortPairs(nullptr, tbytes, kb, vb, (long long)ng, 0, bits, s));
+    void *tmp;
+    CKR(ar.alloc((char **)&tmp, tbytes));
+    CK(cub::DeviceRadixSort::SortPairs(tmp, tbytes, kb, vb, (long long)ng, 0, bits, s));
+    ar.release(tmp);
+    if (kb.Current() != tb->first_sorted)
+      CK(cudaMemcpyAsync(tb->first_sorted, kb.Current(), sizeof(uint32_t) * ng, cudaMemcpyDeviceToDevice, s));
+    k_str_rank<<<grid_for(ng, 256, c->sm_count), 256, 0, s>>>(ng, vb.Current(), tb->rank_of_slot);
+    c->launches += 3;
+    ar.release(k0);
+    ar.release(v0);
+    ar.release(v1);
+  }
+  if (n > 0) {
+    k_str_ids<<<grid_for(n, 256, c->sm_count), 256, 0, s>>>(n, tb->slot_of, tb->rank_of_slot, id);
+    c->launches++;
+  }
+  ar.release(flag);
+  ar.release(pos);
+  return CCO_OK;
+}
+// the dictionary of a grouped column as offsets + bytes in pinned host memory of the context (copies enqueued on the stream)
+static int str_dictionary(cco_ctx *c, Arena &ar, const DevStrCol &col, const StrTable &tb, cco_dictionary_t *out) {
+  cudaStream_t s = c->stream;
+  const long long ng = tb.n_groups;
+  long long *len, *off;
+  CKR(ar.alloc(&len, ng + 1));
+  CKR(ar.alloc(&off, ng + 1));
+  CK(cudaMemsetAsync(len + ng, 0, 8, s));
+  if (ng > 0) {
+    k_str_dict_len<<<grid_for(ng, 256, c->sm_count), 256, 0, s>>>(ng, tb.first_sorted, col.off, len);
+    c->launches++;
+  }
+  CKR(exclusive_sum_i64(c, ar, len, off, ng + 1));
+  long long total = 0;
+  CKR(mail_fetch(c, &total, off + ng, 8));
+  CKR(mail_wait(c));
+  unsigned char *bytes;
+  CKR(ar.alloc(&bytes, std::max<long long>(total, 1)));
+  if (ng > 0 && total > 0) {
+    k_str_dict_gather<<<grid_for(ng, 256, c->sm_count), 256, 0, s>>>(ng, tb.first_sorted, col.off, col.base,
+                                                                    (const unsigned char *)col.w, off, bytes);
+    c->launches++;
+  }
+  out->n = ng;
+  out->offsets = (const int64_t *)c->pinned_get(sizeof(int64_t) * ((size_t)ng + 1), /*for_result=*/false);
+  if (!out->offsets) return set_error(CCO_E_OOM, "pinned host allocation failed");
+  out->bytes = (const char *)c->pinned_get((size_t)std::max<long long>(total, 1), /*for_result=*/false);
+  if (!out->bytes) return set_error(CCO_E_OOM, "pinned host allocation failed");
+  CK(cudaMemcpyAsync((void *)out->offsets, off, sizeof(int64_t) * ((size_t)ng + 1), cudaMemcpyDeviceToHost, s));
+  if (total > 0) CK(cudaMemcpyAsync((void *)out->bytes, bytes, (size_t)total, cudaMemcpyDeviceToHost, s));
+  ar.release(len);
+  ar.release(off);
+  ar.release(bytes);   // stream-ordered: freed after the copy
+  return CCO_OK;
+}
+
+static int ingest_strings_core(cco_ctx *c, int32_t n_types, const cco_string_events_t *ev, int32_t min_events_per_user,
+                               cco_dataset **out) {
+  CK(cudaSetDevice(c->device));
+  cudaStream_t s = c->stream;
+  nvtx_push("cco:ingest_strings");
+  struct Pop { ~Pop() { nvtx_pop(); } } pop;
+  mail_reset(c);
+  Arena ar(s);
+  cco_dataset *d = ingest_dataset_new(c, n_types);
+  d->dicts.assign((size_t)n_types + 1, cco_dictionary_t{0, nullptr, nullptr});
+  struct G {
+    cco_dataset *d;
+    bool ok = false;
+    ~G() {
+      if (!ok) {
+        cudaStreamSynchronize(d->ctx->stream);   // no dictionary copy still writes the pinned buffers released here
+        dataset_release(d);
+      }
+    }
+  } g{d};
+  const uint32_t need = min_events_per_user > 1 ? (uint32_t)min_events_per_user : 1u;
+  DevStrCol pu;   // the primary user column and its table stay resident: later types look their users up there
+  StrTable ut;
+  uint32_t n_users = 0;
+  int *bad;
+  CKR(ar.alloc(&bad, 1));
+  for (int t = 0; t < n_types; ++t) {
+    const long long ne = ev[t].n_events;
+    DevStrCol uc, ic;
+    CKR(str_upload(c, ar, ne, ev[t].user_offsets, ev[t].user_bytes, &uc));
+    CKR(str_upload(c, ar, ne, ev[t].item_offsets, ev[t].item_bytes, &ic));
+    CK(cudaMemsetAsync(bad, 0, sizeof(int), s));
+    str_check_device(c, uc, bad);
+    str_check_device(c, ic, bad);
+    int h_bad = 0;
+    CKR(mail_fetch(c, &h_bad, bad, 4));
+    CKR(mail_wait(c));
+    if (h_bad) return set_error(CCO_E_INVALID_ARG, "type %d: offsets decrease", t);
+    str_hash(c, uc, ~0ULL);
+    str_hash(c, ic, ~0ULL);
+    int32_t *uid, *iid;
+    CKR(ar.alloc(&uid, std::max<long long>(ne, 1)));
+    CKR(ar.alloc(&iid, std::max<long long>(ne, 1)));
+    if (t == 0) {
+      // user dictionary: primary users with >= need events (duplicates count, Preparator.scala:129-132), first appearance order
+      CKR(str_group(c, ar, uc, nullptr, true, need, &ut, uid));
+      if (ut.n_groups >= 0x7fffffffLL) return set_error(CCO_E_UNSUPPORTED, "%lld users: the user space must stay < 2^31 - 1", ut.n_groups);
+      n_users = (uint32_t)ut.n_groups;
+      d->n_users = n_users;
+      CKR(str_dictionary(c, ar, uc, ut, &d->dicts[0]));
+      pu = uc;
+    } else if (ne > 0) {
+      // secondary events of users outside the dictionary are dropped (Preparator.scala:175-178)
+      k_str_lookup<<<grid_for(ne, 256, c->sm_count), 256, 0, s>>>(ne, uc.off, uc.base, uc.w, uc.hash, pu.off, pu.base, pu.w, pu.hash,
+                                                                   (uint64_t)ut.cap - 1, ut.table, ut.rank_of_slot, uid);
+      c->launches++;
+    }
+    // item dictionary of type t: items with a surviving event, ordered by first surviving appearance
+    StrTable it;
+    CKR(str_group(c, ar, ic, uid, false, 0, &it, iid));
+    if (it.n_groups >= 0x7ffffffeLL) return set_error(CCO_E_UNSUPPORTED, "type %d: %lld items, at most 2^31 - 2", t, it.n_groups);
+    d->n_cols[t] = it.n_groups;
+    CKR(str_dictionary(c, ar, ic, it, &d->dicts[1 + t]));
+    str_table_release(ar, it);
+    if (t > 0) str_release(ar, uc);
+    str_release(ar, ic);
+    unsigned long long *k0, *k1, *d_kept;
+    CKR(ar.alloc(&k0, std::max<long long>(ne, 1)));
+    CKR(ar.alloc(&k1, std::max<long long>(ne, 1)));
+    CKR(ar.alloc(&d_kept, 1));
+    CK(cudaMemsetAsync(d_kept, 0, 8, s));
+    if (ne > 0) {
+      k_str_keys<<<grid_for(ne, 256, c->sm_count), 256, 0, s>>>(ne, uid, iid, k0, d_kept);
+      c->launches++;
+    }
+    unsigned long long kept = 0;
+    CKR(mail_fetch(c, &kept, d_kept, 8));
+    CKR(mail_wait(c));
+    ar.release(uid);
+    ar.release(iid);
+    CKR(ingest_csr(c, ar, d, t, ne, n_users, k0, k1, kept));
+    ar.release(k0);
+    ar.release(k1);
+  }
+  CKR(ingest_blocks(c, d, n_users));
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  g.ok = true;
+  *out = d;
+  return CCO_OK;
+}
+}  // namespace cco
+
+int cco_ingest_strings(cco_ctx_t *c, int32_t n_types, const cco_string_events_t *ev, int32_t min_events_per_user, cco_dataset_t **out) {
+  if (!c || !ev || !out || n_types < 1) return set_error(CCO_E_INVALID_ARG, "bad argument");
+  *out = nullptr;
+  if (!c->members.empty()) return set_error(CCO_E_UNSUPPORTED, "resident datasets are per GPU: ingest on a per-GPU context");
+  for (int t = 0; t < n_types; ++t) {
+    CKR(str_check_host(ev[t].n_events, ev[t].user_offsets, ev[t].user_bytes, t, "user"));
+    CKR(str_check_host(ev[t].n_events, ev[t].item_offsets, ev[t].item_bytes, t, "item"));
+  }
+  return ingest_strings_core(c, n_types, ev, min_events_per_user, out);
+}
+
+int cco_dataset_dictionary(const cco_dataset_t *ds, int32_t which, cco_dictionary_t *out) {
+  if (!ds || !out) return set_error(CCO_E_INVALID_ARG, "null argument");
+  if (ds->dicts.empty()) return set_error(CCO_E_INVALID_ARG, "this dataset was not built from strings (cco_ingest_strings)");
+  if (which < -1 || which >= ds->n_mats) return set_error(CCO_E_INVALID_ARG, "dictionary %d not in [-1, %d)", which, ds->n_mats);
+  *out = ds->dicts[(size_t)which + 1];
+  return CCO_OK;
+}
+
+int cco_debug_string_ids(cco_ctx_t *c, int64_t n, const int64_t *offsets, const char *bytes, int32_t hash_bits, int32_t *ids) {
+  if (!c || (n > 0 && !ids)) return set_error(CCO_E_INVALID_ARG, "bad argument");
+  if (hash_bits < 0 || hash_bits > 64) return set_error(CCO_E_INVALID_ARG, "hash_bits %d not in [0, 64]", hash_bits);
+  if (!c->members.empty()) return set_error(CCO_E_UNSUPPORTED, "per-GPU contexts only");
+  CKR(str_check_host(n, offsets, bytes, 0, "id"));
+  CK(cudaSetDevice(c->device));
+  cudaStream_t s = c->stream;
+  mail_reset(c);
+  Arena ar(s);
+  DevStrCol col;
+  CKR(str_upload(c, ar, n, offsets, bytes, &col));
+  int *bad;
+  CKR(ar.alloc(&bad, 1));
+  CK(cudaMemsetAsync(bad, 0, sizeof(int), s));
+  str_check_device(c, col, bad);
+  int h_bad = 0;
+  CKR(mail_fetch(c, &h_bad, bad, 4));
+  CKR(mail_wait(c));
+  if (h_bad) return set_error(CCO_E_INVALID_ARG, "offsets decrease");
+  str_hash(c, col, hash_bits == 64 ? ~0ULL : (1ULL << hash_bits) - 1);
+  int32_t *d_ids;
+  CKR(ar.alloc(&d_ids, std::max<long long>(n, 1)));
+  StrTable tb;
+  CKR(str_group(c, ar, col, nullptr, false, 0, &tb, d_ids));
+  if (n > 0) CK(cudaMemcpyAsync(ids, d_ids, sizeof(int32_t) * (size_t)n, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  return CCO_OK;
 }
 
 // copy matrix i of a resident dataset into caller-provided host arrays (pinned ones from cco_host_alloc copy at PCIe speed)

@@ -2,8 +2,8 @@
 (src/main/scala/Preparator.scala:44-87, 100-216): event (user, item) string pairs
 per event name -> IndexedDatasets that share one user dictionary.
 
-This is the INPUT side of the hot-path boundary (SURVEY.md 8a-H1); it is host logic in numpy and
-is listed as the next row to move to the device (SURVEY.md 8f-1)."""
+This is the INPUT side of the hot-path boundary (SURVEY.md 8a-H1).  `prepare` is host logic and the definition the
+device path is held to; `prepare_on_device` returns the same value, built by cco_ingest_strings (SURVEY.md 8f-1)."""
 from __future__ import annotations
 
 from typing import Sequence
@@ -65,4 +65,30 @@ def prepare(actions: Sequence[tuple[str, Sequence[tuple[str, str]]]],
             ids = _build(pairs, user_dict, freeze_rows=True)          # :69 IndexedDatasetSpark(eventRDD, userDictionary)
         user_dict = ids.row_ids
         out.append((name, ids))
+    return out
+
+
+def prepare_on_device(actions: Sequence[tuple[str, Sequence[tuple[str, str]]]], min_events_per_user: int | None = None,
+                      ctx=None) -> list[tuple[str, IndexedDataset]]:
+    """`prepare` on the GPU: the same input and the same return value (host CSR + BiDictionaries, the secondary datasets
+    sharing the primary's row_ids object).  Dictionaries and matrices are built by cco_ingest_strings; the host only
+    encodes the ids (encode_ids) and decodes the dictionaries.  Callers that already hold id columns in the offsets +
+    bytes layout skip the encoding with CcoContext.ingest_strings."""
+    from .similarity_analysis import default_context, encode_ids
+    if not actions:
+        return []
+    ctx = ctx or default_context()
+    columns = []
+    for _, pairs in actions:
+        users, items = (list(x) for x in zip(*pairs)) if len(pairs) else ([], [])
+        columns.append((*encode_ids(users), *encode_ids(items)))
+    ds, user_ids, item_ids = ctx.ingest_strings(columns, min_events_per_user or 0)
+    try:
+        row_ids = BiDictionary(user_ids)
+        out = []
+        for t, (name, _) in enumerate(actions):
+            n_rows, n_cols, row_ptr, col_idx = ctx.dataset_matrix(ds, t)
+            out.append((name, IndexedDataset(row_ptr, col_idx, row_ids, BiDictionary(item_ids[t]), n_rows=n_rows, n_cols=n_cols)))
+    finally:
+        ctx.free_dataset(ds)
     return out

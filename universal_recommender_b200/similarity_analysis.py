@@ -238,11 +238,13 @@ class CcoContext:
         N.check(self._L.cco_dataset_upload(self._h, len(mats), cm, flags, C.byref(ds)))
         return (ds, len(mats))
 
-    def train_dataset(self, dataset, params, seed: int, flags: int = 0, copy_arrays: bool = True):
+    def train_dataset(self, dataset, params, seed: int, flags: int = 0, copy_arrays: bool = True, keep: bool = False):
+        """cco_train_dataset on a resident dataset -> as train_csr (keep=True: zero-copy views + a handle for free_result,
+        e.g. for format_es_bulk)."""
         ds, n = dataset
         res = C.c_void_p()
         N.check(self._L.cco_train_dataset(self._h, ds, self._params_array(params), C.c_int32(_to_i32(seed)), flags, C.byref(res)))
-        return self._collect(res, n, copy_arrays)
+        return self._collect(res, n, copy_arrays, keep)
 
     def ingest(self, events, n_users_raw: int, min_events_per_user: int = 0):
         """Preparator.prepare on the device (SURVEY.md 8f-1).  events = [(users int64[], items int32[], n_items_raw)], type 0
@@ -261,6 +263,51 @@ class CcoContext:
         N.check(self._L.cco_ingest(self._h, n, ev, n_users_raw, min_events_per_user, user_map.ctypes.data_as(C.POINTER(C.c_int32)),
                                    maps, C.byref(ds)))
         return (ds, n), user_map[:n_users_raw], [m[:ni] for m, (_, _, ni) in zip(item_maps, events)]
+
+    def ingest_strings(self, columns, min_events_per_user: int = 0):
+        """Preparator.prepare on the device from string ids (cco_ingest_strings).  columns = one (user_offsets int64[n + 1],
+        user_bytes uint8[], item_offsets int64[n + 1], item_bytes uint8[]) per event type, type 0 = primary, in the layout
+        encode_ids produces (and Arrow large_string columns have).  Pinned arrays (host_array) copy at full PCIe speed.
+        -> (dataset for train_dataset, user ids list[str], [item ids list[str] per type]), dictionaries in the order of
+        preparator.prepare."""
+        dataset = self.ingest_strings_dataset(columns, min_events_per_user)
+        try:
+            users = self.dataset_dictionary(dataset, -1)
+            items = [self.dataset_dictionary(dataset, t) for t in range(dataset[1])]
+        except BaseException:
+            self.free_dataset(dataset)
+            raise
+        return dataset, users, items
+
+    def ingest_strings_dataset(self, columns, min_events_per_user: int = 0):
+        """ingest_strings without decoding the dictionaries: -> the resident dataset (dictionaries via dataset_dictionary)"""
+        n = len(columns)
+        keep, ev = [], (N.StringEventsT * n)()
+        p64 = C.POINTER(C.c_int64)
+        as_u8 = lambda b: np.frombuffer(b, dtype=np.uint8) if isinstance(b, (bytes, bytearray)) else np.ascontiguousarray(b, dtype=np.uint8)
+        for t, (uo, ub, io, ib) in enumerate(columns):
+            uo = np.ascontiguousarray(uo, dtype=np.int64)
+            io = np.ascontiguousarray(io, dtype=np.int64)
+            ub, ib = as_u8(ub), as_u8(ib)
+            if len(uo) < 1 or len(uo) != len(io):
+                raise N.CcoInvalidArgument(N.E_INVALID_ARG, f"type {t}: user and item offsets need n_events + 1 entries each")
+            keep.append((uo, ub, io, ib))
+            ev[t] = N.StringEventsT(len(uo) - 1, uo.ctypes.data_as(p64), ub.ctypes.data if len(ub) else None,
+                                    io.ctypes.data_as(p64), ib.ctypes.data if len(ib) else None)
+        ds = C.c_void_p()
+        N.check(self._L.cco_ingest_strings(self._h, n, ev, int(min_events_per_user or 0), C.byref(ds)))
+        return (ds, n)
+
+    def dataset_dictionary(self, dataset, which: int) -> list[str]:
+        """the user dictionary (which = -1) or the item dictionary of type `which` of a string-ingested dataset"""
+        d = N.DictionaryT()
+        N.check(self._L.cco_dataset_dictionary(dataset[0], which, C.byref(d)))
+        off = np.ctypeslib.as_array(d.offsets, shape=(d.n + 1,)).copy()
+        nb = int(off[-1])
+        # the raw pointer: reading the c_char_p field would stop at the first NUL byte, and ids may contain NULs
+        addr = C.c_void_p.from_buffer(d, N.DictionaryT.bytes.offset).value
+        blob = C.string_at(addr, nb) if nb else b""
+        return decode_ids(off, blob)
 
     def synth_dataset(self, types, n_users_raw: int, user_cdf: np.ndarray, user_perm: np.ndarray, min_events_per_user: int = 0,
                       raw_item_space: bool = False):
@@ -329,6 +376,15 @@ class CcoContext:
                                       out.ctypes.data_as(C.POINTER(C.c_double))))
         return out
 
+    def debug_string_ids(self, offsets, data, hash_bits: int = 64) -> np.ndarray:
+        """cco_debug_string_ids: dictionary id (first-appearance order) of every id of one column, hash cut to hash_bits"""
+        off = np.ascontiguousarray(offsets, dtype=np.int64)
+        b = np.ascontiguousarray(data, dtype=np.uint8)
+        ids = np.zeros(max(len(off) - 1, 1), dtype=np.int32)
+        N.check(self._L.cco_debug_string_ids(self._h, len(off) - 1, off.ctypes.data_as(C.POINTER(C.c_int64)), b.ctypes.data if len(b) else None,
+                                             hash_bits, ids.ctypes.data_as(C.POINTER(C.c_int32))))
+        return ids[:len(off) - 1]
+
     def debug_downsample(self, n_rows, n_cols, row_ptr, col_idx, max_interactions: int, seed: int, flags: int = 0):
         rp = np.ascontiguousarray(row_ptr, dtype=np.int64)
         ci = np.ascontiguousarray(col_idx, dtype=np.int32)
@@ -364,6 +420,33 @@ class CcoContext:
         for p in (orp, oci, ocn):
             self._L.cco_free(p)
         return r, c, n
+
+
+def encode_ids(ids: Sequence[str]) -> tuple[np.ndarray, np.ndarray]:
+    """id strings -> (offsets int64[n + 1], bytes uint8[]): UTF-8, id i = bytes[offsets[i]:offsets[i + 1]] (the Arrow
+    large_string layout cco_ingest_strings takes)."""
+    ids = ids if isinstance(ids, list) else list(ids)
+    joined = "".join(ids)
+    if joined.isascii():   # one byte per character: lengths are str lengths, one encode for the whole column
+        lens = np.fromiter(map(len, ids), dtype=np.int64, count=len(ids))
+        blob = joined.encode("ascii")
+    else:
+        enc = [x.encode("utf-8") for x in ids]
+        lens = np.fromiter(map(len, enc), dtype=np.int64, count=len(enc))
+        blob = b"".join(enc)
+    off = np.zeros(len(ids) + 1, dtype=np.int64)
+    np.cumsum(lens, out=off[1:])
+    return off, np.frombuffer(blob, dtype=np.uint8)
+
+
+def decode_ids(offsets: np.ndarray, blob: bytes) -> list[str]:
+    """inverse of encode_ids (bytes that are not UTF-8 decode with surrogateescape, so they round-trip too)"""
+    off = np.asarray(offsets, dtype=np.int64)
+    base = int(off[0]) if len(off) else 0
+    if blob.isascii():
+        text = blob.decode("ascii")
+        return [text[a - base:b - base] for a, b in zip(off[:-1].tolist(), off[1:].tolist())]
+    return [blob[a - base:b - base].decode("utf-8", "surrogateescape") for a, b in zip(off[:-1].tolist(), off[1:].tolist())]
 
 
 def _to_i32(seed: int) -> int:
