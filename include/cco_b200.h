@@ -333,6 +333,52 @@ int cco_pop_model(cco_ctx_t *ctx, int32_t mode, int64_t n_events, const int32_t 
                   int64_t start_ms, int64_t end_ms, double *score, unsigned char *present);
 
 /*
+ * The complete model index (SURVEY.md 8f-2 + 8f-3): calcAll's propertiesRDD (URAlgorithm.scala:351-367) joined into the
+ * documents of cco_format_es_bulk the way URModel.save's groupAll + ("id" -> item) does (URModel.scala:57-102).
+ * Documents: every row of the result, then (only in the call whose result begins at row 0) every item without a row that
+ * has a property or a score in a ranking, in order of first appearance (property items first, then the ranking streams in
+ * order).  Items are matched by id string.  Fields: "id", the indicators in name order, the properties in field index order,
+ * the rankings in order:
+ *     {"index":{"_id":"<id>"}}\n{"id":"<id>"[,"<indicator>":[...]]*[,"<field>":<value>]*[,"<ranking>":<number>]*}\n
+ * Where names repeat, precedence per document (lowest to highest): indicators < properties < rankings (a later ranking beats
+ * an earlier one) < "id"; the lower field is not written.  Indicator names that repeat each other (or are "id") are written
+ * as cco_format_es_bulk writes them.  Property values are JSON text, spliced verbatim (never parsed); ids and names are
+ * JSON-escaped.  Rank numbers are Java's Double.toString of an integer: "-"?digits".0" below 10^7, else d.ddd"E"n with the
+ * trailing zeros of the digits dropped (1.0E7, 1.2345678E7).  Without properties and rankings the body is byte-identical
+ * to cco_format_es_bulk.
+ * Errors: CCO_E_INVALID_ARG for negative or decreasing offsets in any column, a field index outside [0, n_fields), an empty
+ * value, repeated field names, end_ms < start_ms or a bad mode (decided on the device before any kernel reads bytes through
+ * the offsets); CCO_E_UNSUPPORTED for more than CCO_MAX_RANKINGS rankings or rows + property triples + ranking events >= 2^31.
+ */
+typedef struct {
+  int64_t n;                      /* (item, field, value) triples; a repeated (item, field) pair: the last triple wins */
+  const int64_t *item_offsets;    /* [n + 1] item id t = item_bytes[item_offsets[t] .. item_offsets[t + 1]) */
+  const char *item_bytes;
+  const int32_t *field;           /* [n] index into field_names */
+  const int64_t *value_offsets;   /* [n + 1] JSON text of value t, not empty */
+  const char *value_bytes;
+  int32_t n_fields;
+  const char *const *field_names; /* [n_fields] distinct, NUL-terminated UTF-8 */
+} cco_item_properties_t;
+typedef struct {                  /* the events of one event name: target item ids and event times */
+  int64_t n_events;
+  const int64_t *item_offsets;    /* [n_events + 1] */
+  const char *item_bytes;
+  const int64_t *time_ms;         /* [n_events] epoch milliseconds */
+} cco_ranking_stream_t;
+typedef struct {                  /* one PopModel ranking over [start_ms, end_ms) of its streams, as cco_pop_model */
+  const char *name;               /* the document field */
+  int32_t mode;                   /* CCO_POP_* */
+  int32_t n_streams;              /* >= 1 */
+  int64_t start_ms, end_ms;
+  const cco_ranking_stream_t *streams;
+} cco_ranking_t;
+#define CCO_MAX_RANKINGS 8
+int cco_format_model(cco_ctx_t *ctx, const cco_result_t *res, int32_t n_names, const char *const *names,
+                     const cco_dictionary_t *row_ids, const cco_dictionary_t *col_ids, const cco_item_properties_t *props /* nullable */,
+                     int32_t n_rankings, const cco_ranking_t *rankings, char **out_bytes, int64_t *out_len);
+
+/*
  * Debug/parity entry (tests only): full integer co-occurrence matrix A^T B of two canonical
  * binary matrices computed by the same accumulation kernel as cco_train, no LLR, no top-k.
  * Output CSR over the columns of A with ascending column ids, malloc'ed; free with cco_free.

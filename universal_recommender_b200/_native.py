@@ -19,6 +19,8 @@ FLAG_RESULT_ON_DEVICE = 8
 FLAG_RESULT_NO_COUNT = 16
 FLAG_RESULT_NO_LLR = 32
 MAX_TOP_K = 2048
+MAX_RANKINGS = 8
+POP_MODES = {"popular": 0, "trending": 1, "hot": 2}
 
 
 class CcoError(RuntimeError):
@@ -66,6 +68,22 @@ class StringEventsT(C.Structure):
                 ("item_offsets", C.POINTER(C.c_int64)), ("item_bytes", C.c_void_p)]
 
 
+class ItemPropertiesT(C.Structure):
+    _fields_ = [("n", C.c_int64), ("item_offsets", C.POINTER(C.c_int64)), ("item_bytes", C.c_void_p), ("field", C.POINTER(C.c_int32)),
+                ("value_offsets", C.POINTER(C.c_int64)), ("value_bytes", C.c_void_p), ("n_fields", C.c_int32),
+                ("field_names", C.POINTER(C.c_char_p))]
+
+
+class RankingStreamT(C.Structure):
+    _fields_ = [("n_events", C.c_int64), ("item_offsets", C.POINTER(C.c_int64)), ("item_bytes", C.c_void_p),
+                ("time_ms", C.POINTER(C.c_int64))]
+
+
+class RankingT(C.Structure):
+    _fields_ = [("name", C.c_char_p), ("mode", C.c_int32), ("n_streams", C.c_int32), ("start_ms", C.c_int64), ("end_ms", C.c_int64),
+                ("streams", C.POINTER(RankingStreamT))]
+
+
 class StatsT(C.Structure):
     _fields_ = [("n_users", C.c_int64), ("nnz_in_total", C.c_int64),
                 ("nnz_downsampled", C.c_int64 * 16), ("products", C.c_int64 * 16),
@@ -82,6 +100,7 @@ EXPORTS = [
     "cco_dataset_upload", "cco_train_dataset", "cco_dataset_free", "cco_timer_start", "cco_timer_stop",
     "cco_partition_rows", "cco_ingest", "cco_synth_ingest", "cco_dataset_shape", "cco_dataset_download",
     "cco_dataset_copy_to_host", "cco_format_es_bulk", "cco_ingest_strings", "cco_dataset_dictionary", "cco_pop_model",
+    "cco_format_model",
     "cco_result_num_matrices", "cco_result_row_range", "cco_result_matrix", "cco_result_stats", "cco_result_free",
     "cco_debug_cooccurrence", "cco_debug_downsample", "cco_debug_llr", "cco_debug_string_ids", "cco_free",
 ]
@@ -126,6 +145,8 @@ def lib():
     L.cco_dataset_dictionary.argtypes = [C.c_void_p, C.c_int32, p(DictionaryT)]
     L.cco_pop_model.argtypes = [C.c_void_p, C.c_int32, C.c_int64, p(C.c_int32), p(C.c_int64), C.c_int32, C.c_int64, C.c_int64, p(C.c_double),
                                 p(C.c_ubyte)]
+    L.cco_format_model.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, p(C.c_char_p), p(DictionaryT), p(DictionaryT), p(ItemPropertiesT),
+                                   C.c_int32, p(RankingT), p(C.c_void_p), p(C.c_int64)]
     L.cco_dataset_shape.argtypes = [C.c_void_p, C.c_int32, p(C.c_int64), p(C.c_int32), p(C.c_int64)]
     L.cco_dataset_download.argtypes = [C.c_void_p, C.c_int32, p(p(C.c_int64)), p(p(C.c_int32))]
     L.cco_timer_start.argtypes = [C.c_void_p]

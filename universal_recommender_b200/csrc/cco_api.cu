@@ -2578,8 +2578,285 @@ static int escape_dict(cco_ctx *c, Arena &ar, const DevDict &raw, DevDict *esc) 
 }
 }  // namespace cco
 
-int cco_format_es_bulk(cco_ctx_t *ctx, const cco_result_t *res, int32_t n_names, const char *const *names,
-                       const cco_dictionary_t *row_ids, const cco_dictionary_t *col_ids, char **out_bytes, int64_t *out_len) {
+namespace cco {
+// PopModel's bucket edges for one ranking window (Joda integer millisecond arithmetic)
+static PopArgs pop_args(int mode, long long start_ms, long long end_ms, int32_t n_keys) {
+  PopArgs a;
+  memset(&a, 0, sizeof a);
+  a.n_items = n_keys;
+  const long long dur = end_ms - start_ms;
+  if (mode == CCO_POP_POPULAR) {
+    a.n_buckets = 1;
+    a.edge[0] = start_ms;
+    a.edge[1] = end_ms;
+  } else if (mode == CCO_POP_TRENDING) {   // PopModel.scala:134-138: halfInterval = durationMillis / 2
+    a.n_buckets = 2;
+    a.edge[0] = start_ms;
+    a.edge[1] = start_ms + dur / 2;
+    a.edge[2] = end_ms;
+  } else {                                  // PopModel.scala:159-164: older = dur / 3, middle = the same length, newer = the rest
+    a.n_buckets = 3;
+    a.edge[0] = start_ms;
+    a.edge[1] = start_ms + dur / 3;
+    a.edge[2] = a.edge[1] + dur / 3;
+    a.edge[3] = end_ms;
+  }
+  return a;
+}
+
+// one section of the combined key column: the row dictionary, the property items or one ranking stream
+struct KeySection {
+  long long n;
+  const int64_t *off;
+  const char *bytes;
+};
+
+// The model part of FormatArgs (cco_format_model): group the item ids of every source, score the rankings per group,
+// sort the properties, and list the documents of items without a row.  The caller's columns have passed str_check_host.
+static int model_fields(cco_ctx *c, Arena &ar, FormatArgs *fa, const cco_dictionary_t &row_ids, const cco_item_properties_t *props,
+                        int32_t n_rank, const cco_ranking_t *rk, bool extra_docs) {
+  cudaStream_t s = c->stream;
+  mail_reset(c);
+  const long long R = row_ids.n, P = props ? props->n : 0;
+  std::vector<KeySection> sec;
+  sec.push_back({R, row_ids.offsets, row_ids.bytes});
+  sec.push_back({P, P > 0 ? props->item_offsets : nullptr, P > 0 ? props->item_bytes : nullptr});
+  std::vector<long long> rank_begin(n_rank + 1);   // ranking k's events are key entries R + P + [rank_begin[k], rank_begin[k + 1])
+  long long E = 0;
+  for (int k = 0; k < n_rank; ++k) {
+    rank_begin[k] = E;
+    for (int q = 0; q < rk[k].n_streams; ++q) {
+      const cco_ranking_stream_t &st = rk[k].streams[q];
+      sec.push_back({st.n_events, st.item_offsets, st.item_bytes});
+      E += st.n_events;
+    }
+  }
+  rank_begin[n_rank] = E;
+  const long long N = R + P + E;
+  long long nb = 0;
+  for (const KeySection &k : sec) nb += k.n > 0 ? k.off[k.n] - k.off[0] : 0;
+  DevStrCol key;
+  key.n = N;
+  key.base = 0;
+  CKR(ar.alloc(&key.off, N + 1));
+  CKR(ar.alloc(&key.w, (nb + 16 + 7) / 8));
+  CKR(ar.alloc(&key.hash, std::max<long long>(N, 1)));
+  CK(cudaMemsetAsync(key.off, 0, 8, s));
+  int *bad;
+  CKR(ar.alloc(&bad, 1));
+  CK(cudaMemsetAsync(bad, 0, sizeof(int), s));
+  long long *tmp_off;
+  long long max_n = 0;
+  for (const KeySection &k : sec) max_n = std::max(max_n, k.n);
+  CKR(ar.alloc(&tmp_off, max_n + 1));
+  // every section: raw offsets -> decreasing check -> rebased into the key column; bytes appended to the word buffer
+  long long at = 0, byte_at = 0;
+  for (const KeySection &k : sec) {
+    if (k.n == 0) continue;
+    const long long kb = k.off[k.n] - k.off[0];
+    CK(cudaMemcpyAsync(tmp_off, k.off, sizeof(int64_t) * ((size_t)k.n + 1), cudaMemcpyHostToDevice, s));
+    k_str_check<<<grid_for(k.n, 256, c->sm_count), 256, 0, s>>>(k.n, tmp_off, bad);
+    k_rebase<<<grid_for(k.n + 1, 256, c->sm_count), 256, 0, s>>>(k.n + 1, tmp_off, byte_at - k.off[0], key.off + at);
+    c->launches += 2;
+    if (kb > 0) CK(cudaMemcpyAsync((char *)key.w + byte_at, k.bytes + k.off[0], (size_t)kb, cudaMemcpyHostToDevice, s));
+    at += k.n;
+    byte_at += kb;
+  }
+  // property fields and values
+  int32_t *d_field = nullptr;
+  if (P > 0) {
+    const long long vb = props->value_offsets[P] - props->value_offsets[0];
+    long long *d_voff;
+    unsigned char *d_vals;
+    CKR(ar.alloc(&d_field, P));
+    CKR(ar.alloc(&d_voff, P + 1));
+    CKR(ar.alloc(&d_vals, std::max<long long>(vb, 1)));
+    CK(cudaMemcpyAsync(d_field, props->field, sizeof(int32_t) * (size_t)P, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(d_voff, props->value_offsets, sizeof(int64_t) * ((size_t)P + 1), cudaMemcpyHostToDevice, s));
+    if (vb > 0) CK(cudaMemcpyAsync(d_vals, props->value_bytes + props->value_offsets[0], (size_t)vb, cudaMemcpyHostToDevice, s));
+    k_str_check<<<grid_for(P, 256, c->sm_count), 256, 0, s>>>(P, d_voff, bad);
+    k_prop_check<<<grid_for(P, 256, c->sm_count), 256, 0, s>>>(P, d_field, props->n_fields, d_voff, bad);
+    c->launches += 2;
+    fa->val_off = d_voff;
+    fa->val_base = props->value_offsets[0];
+    fa->vals = d_vals;
+  }
+  // event times, all rankings' streams in order
+  long long *d_t;
+  CKR(ar.alloc(&d_t, std::max<long long>(E, 1)));
+  for (int k = 0; k < n_rank; ++k) {
+    long long e = rank_begin[k];
+    for (int q = 0; q < rk[k].n_streams; ++q) {
+      const cco_ranking_stream_t &st = rk[k].streams[q];
+      if (st.n_events > 0) CK(cudaMemcpyAsync(d_t + e, st.time_ms, sizeof(int64_t) * (size_t)st.n_events, cudaMemcpyHostToDevice, s));
+      e += st.n_events;
+    }
+  }
+  // the device verdict comes before any kernel reads bytes through the offsets
+  int h_bad = 0;
+  CKR(mail_fetch(c, &h_bad, bad, 4));
+  CKR(mail_wait(c));
+  if (h_bad & 1) return set_error(CCO_E_INVALID_ARG, "offsets decrease");
+  if (h_bad & 2) return set_error(CCO_E_INVALID_ARG, "a property field index is outside [0, %d)", props->n_fields);
+  if (h_bad & 4) return set_error(CCO_E_INVALID_ARG, "an empty property value (values are JSON text)");
+  ar.release(tmp_off);
+
+  // 1. item key space: one exact grouping by string over every source, numbered by first appearance
+  str_hash(c, key, ~0ULL);
+  int32_t *gid;
+  CKR(ar.alloc(&gid, std::max<long long>(N, 1)));
+  StrTable tb;
+  CKR(str_group(c, ar, key, nullptr, false, 0, &tb, gid));
+  const long long G = tb.n_groups;
+  fa->n_groups = G;
+  fa->row_group = gid + fa->row_id_base;
+  // 2. rankings: PopModel histograms over the groups
+  fa->n_rank = n_rank;
+  if (n_rank > 0) {
+    long long *score;
+    unsigned char *pmask, *present;
+    int32_t *counts;
+    unsigned long long *tot;
+    CKR(ar.alloc(&score, (size_t)n_rank * G));
+    CKR(ar.alloc(&pmask, G));
+    CKR(ar.alloc(&present, G));
+    CKR(ar.alloc(&counts, (size_t)3 * G));
+    CKR(ar.alloc(&tot, 4));
+    CK(cudaMemsetAsync(pmask, 0, (size_t)G, s));
+    for (int k = 0; k < n_rank; ++k) {
+      const PopArgs pa = pop_args(rk[k].mode, rk[k].start_ms, rk[k].end_ms, (int32_t)G);
+      const long long ne = rank_begin[k + 1] - rank_begin[k];
+      CK(cudaMemsetAsync(counts, 0, sizeof(int32_t) * (size_t)pa.n_buckets * G, s));
+      CK(cudaMemsetAsync(tot, 0, 32, s));
+      if (ne > 0) {
+        k_pop_count<<<grid_for(ne, 256, c->sm_count), 256, 0, s>>>(ne, gid + R + P + rank_begin[k], d_t + rank_begin[k], pa, counts, tot);
+        c->launches++;
+      }
+      k_pop_score<long long><<<grid_for(G, 256, c->sm_count), 256, 0, s>>>(pa, rk[k].mode, counts, tot, score + (size_t)k * G, present);
+      k_rank_mask<<<grid_for(G, 256, c->sm_count), 256, 0, s>>>(G, present, k, pmask);
+      c->launches += 2;
+    }
+    ar.release(counts);
+    ar.release(present);
+    fa->score = score;
+    fa->pmask = pmask;
+  }
+  // 3. properties: sorted by (group, field), stable in the triple index, so the last triple of each run wins
+  if (P > 0) {
+    unsigned long long *k0, *k1;
+    int32_t *v0, *v1, *pbeg, *pend;
+    CKR(ar.alloc(&k0, P));
+    CKR(ar.alloc(&k1, P));
+    CKR(ar.alloc(&v0, P));
+    CKR(ar.alloc(&v1, P));
+    CKR(ar.alloc(&pbeg, G));
+    CKR(ar.alloc(&pend, G));
+    CK(cudaMemsetAsync(pbeg, 0, sizeof(int32_t) * (size_t)G, s));
+    CK(cudaMemsetAsync(pend, 0, sizeof(int32_t) * (size_t)G, s));
+    k_prop_keys<<<grid_for(P, 256, c->sm_count), 256, 0, s>>>(P, gid + R, d_field, k0, v0);
+    int gbits = 1;
+    while ((1LL << gbits) < G) ++gbits;
+    cub::DoubleBuffer<unsigned long long> kb(k0, k1);
+    cub::DoubleBuffer<int32_t> vb(v0, v1);
+    size_t tbytes = 0;
+    CK(cub::DeviceRadixSort::SortPairs(nullptr, tbytes, kb, vb, (long long)P, 0, 32 + gbits, s));
+    void *tmp;
+    CKR(ar.alloc((char **)&tmp, tbytes));
+    CK(cub::DeviceRadixSort::SortPairs(tmp, tbytes, kb, vb, (long long)P, 0, 32 + gbits, s));
+    ar.release(tmp);
+    k_prop_ranges<<<grid_for(P, 256, c->sm_count), 256, 0, s>>>(P, kb.Current(), pbeg, pend);
+    c->launches += 3;
+    fa->pkey = kb.Current();
+    fa->ptri = vb.Current();
+    fa->pbeg = pbeg;
+    fa->pend = pend;
+  }
+  // 4. documents of items without a row, in order of first appearance (only the result that begins at row 0 writes them)
+  fa->n_extra = 0;
+  if (extra_docs && G > 0) {
+    uint32_t *flag, *pos;
+    CKR(ar.alloc(&flag, G + 1));
+    CKR(ar.alloc(&pos, G + 1));
+    CK(cudaMemsetAsync(flag + G, 0, 4, s));
+    k_extra_flags<<<grid_for(G, 256, c->sm_count), 256, 0, s>>>(G, tb.first_sorted, R, fa->pbeg, fa->pend, fa->pmask, flag);
+    c->launches++;
+    CKR(exclusive_sum_u32(c, ar, flag, pos, G + 1));
+    uint32_t n_extra = 0;
+    CKR(mail_fetch(c, &n_extra, pos + G, 4));
+    CKR(mail_wait(c));
+    if (n_extra > 0) {
+      int32_t *extra_group;
+      uint32_t *extra_first;
+      long long *len, *off;
+      CKR(ar.alloc(&extra_group, n_extra));
+      CKR(ar.alloc(&extra_first, n_extra));
+      CKR(ar.alloc(&len, (long long)n_extra + 1));
+      CKR(ar.alloc(&off, (long long)n_extra + 1));
+      k_extra_compact<<<grid_for(G, 256, c->sm_count), 256, 0, s>>>(G, flag, pos, tb.first_sorted, extra_group, extra_first);
+      CK(cudaMemsetAsync(len + n_extra, 0, 8, s));
+      k_str_dict_len<<<grid_for(n_extra, 256, c->sm_count), 256, 0, s>>>(n_extra, extra_first, key.off, len);
+      CKR(exclusive_sum_i64(c, ar, len, off, (long long)n_extra + 1));
+      long long total = 0;
+      CKR(mail_fetch(c, &total, off + n_extra, 8));
+      CKR(mail_wait(c));
+      unsigned char *bytes;
+      CKR(ar.alloc(&bytes, std::max<long long>(total, 1)));
+      k_str_dict_gather<<<grid_for(n_extra, 256, c->sm_count), 256, 0, s>>>(n_extra, extra_first, key.off, 0, (const unsigned char *)key.w,
+                                                                           off, bytes);
+      c->launches += 3;
+      const DevDict raw = {off, bytes, (long long)n_extra};
+      CKR(escape_dict(c, ar, raw, &fa->extra_ids));
+      fa->extra_group = extra_group;
+      fa->n_extra = (int32_t)n_extra;
+    }
+  }
+  return CCO_OK;
+}
+
+// host checks of the model inputs (the device checks decreasing offsets, field indices and empty values)
+static int model_check_host(const cco_dictionary_t *row_ids, const cco_item_properties_t *props, int32_t n_rank, const cco_ranking_t *rk) {
+  if (n_rank < 0 || (n_rank > 0 && !rk)) return set_error(CCO_E_INVALID_ARG, "bad rankings");
+  if (n_rank > kMaxRankings) return set_error(CCO_E_UNSUPPORTED, "%d rankings, at most %d", n_rank, kMaxRankings);
+  long long total = row_ids->n;
+  CKR(str_check_host(row_ids->n, row_ids->offsets, row_ids->bytes, -1, "row id"));
+  if (props) {
+    if (props->n < 0 || props->n_fields < 0 || (props->n_fields > 0 && !props->field_names)) return set_error(CCO_E_INVALID_ARG, "bad properties");
+    for (int f = 0; f < props->n_fields; ++f) {
+      if (!props->field_names[f]) return set_error(CCO_E_INVALID_ARG, "null field name %d", f);
+      for (int h = 0; h < f; ++h)
+        if (!strcmp(props->field_names[h], props->field_names[f]))
+          return set_error(CCO_E_INVALID_ARG, "field names %d and %d are both \"%s\"", h, f, props->field_names[f]);
+    }
+    if (props->n > 0) {
+      if (!props->field) return set_error(CCO_E_INVALID_ARG, "null property field indices");
+      CKR(str_check_host(props->n, props->item_offsets, props->item_bytes, -1, "property item"));
+      CKR(str_check_host(props->n, props->value_offsets, props->value_bytes, -1, "property value"));
+    }
+    total += props->n;
+  }
+  for (int k = 0; k < n_rank; ++k) {
+    const cco_ranking_t &r = rk[k];
+    if (!r.name) return set_error(CCO_E_INVALID_ARG, "ranking %d: null name", k);
+    if (r.mode < CCO_POP_POPULAR || r.mode > CCO_POP_HOT) return set_error(CCO_E_INVALID_ARG, "ranking %d: mode must be CCO_POP_POPULAR, _TRENDING or _HOT", k);
+    if (r.end_ms < r.start_ms) return set_error(CCO_E_INVALID_ARG, "ranking %d: end before start (Joda Interval would throw)", k);
+    if (r.n_streams < 1 || !r.streams) return set_error(CCO_E_INVALID_ARG, "ranking %d: needs at least one stream", k);
+    for (int q = 0; q < r.n_streams; ++q) {
+      const cco_ranking_stream_t &st = r.streams[q];
+      CKR(str_check_host(st.n_events, st.item_offsets, st.item_bytes, k, "ranking item"));
+      if (st.n_events > 0 && !st.time_ms) return set_error(CCO_E_INVALID_ARG, "ranking %d: null event times", k);
+      total += st.n_events;
+      if (total >= 0x7fffffffLL) break;
+    }
+    if (total >= 0x7fffffffLL) break;
+  }
+  if (total >= 0x7fffffffLL) return set_error(CCO_E_UNSUPPORTED, "rows + property triples + ranking events must stay < 2^31 per call");
+  return CCO_OK;
+}
+
+// cco_format_es_bulk == format_model without properties and rankings: one set of document kernels
+static int format_model(cco_ctx_t *ctx, const cco_result_t *res, int32_t n_names, const char *const *names, const cco_dictionary_t *row_ids,
+                        const cco_dictionary_t *col_ids, const cco_item_properties_t *props, int32_t n_rank, const cco_ranking_t *rk,
+                        char **out_bytes, int64_t *out_len, const char *range) {
   if (!ctx || !res || !names || !row_ids || !col_ids || !out_bytes || !out_len) return set_error(CCO_E_INVALID_ARG, "null argument");
   const int n_ind = (int)res->mats.size();
   if (n_names != n_ind) return set_error(CCO_E_INVALID_ARG, "%d event names for %d indicators", n_names, n_ind);
@@ -2594,10 +2871,13 @@ int cco_format_es_bulk(cco_ctx_t *ctx, const cco_result_t *res, int32_t n_names,
     if (!names[i]) return set_error(CCO_E_INVALID_ARG, "null event name");
   }
   if (row_ids->n < row_hi) return set_error(CCO_E_INVALID_ARG, "row dictionary has %lld ids, rows go up to %lld", (long long)row_ids->n, (long long)row_hi);
+  const bool model = (props && props->n > 0) || n_rank > 0;
+  if (model) CKR(model_check_host(row_ids, props, n_rank, rk));
+  const int n_fields = props ? props->n_fields : 0;
   CK(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   Arena ar(s);
-  nvtx_push("cco:format_es_bulk");
+  nvtx_push(range);
   struct Pop { ~Pop() { nvtx_pop(); } } pop;
   FormatArgs fa;
   memset(&fa, 0, sizeof fa);
@@ -2607,24 +2887,63 @@ int cco_format_es_bulk(cco_ctx_t *ctx, const cco_result_t *res, int32_t n_names,
   DevDict raw;
   CKR(upload_dict(c, ar, *row_ids, &raw));
   CKR(escape_dict(c, ar, raw, &fa.row_ids));
-  // event names as one more tiny dictionary
+  // event names, field names and ranking names as one more tiny dictionary
+  std::vector<const char *> all_names(names, names + n_ind);
+  if (model) {
+    for (int f = 0; f < n_fields; ++f) all_names.push_back(props->field_names[f]);
+    for (int k = 0; k < n_rank; ++k) all_names.push_back(rk[k].name);
+  }
+  const int n_all = (int)all_names.size();
+  std::vector<long long> eoff(n_all + 1);
   {
-    std::vector<int64_t> noff(n_ind + 1, 0);
+    std::vector<int64_t> noff(n_all + 1, 0);
     std::string blob;
-    for (int i = 0; i < n_ind; ++i) {
-      blob += names[i];
+    for (int i = 0; i < n_all; ++i) {
+      blob += all_names[i];
       noff[i + 1] = (int64_t)blob.size();
     }
-    cco_dictionary_t nd = {n_ind, noff.data(), blob.data()};
+    cco_dictionary_t nd = {n_all, noff.data(), blob.data()};
     DevDict nraw, nesc;
     CKR(upload_dict(c, ar, nd, &nraw));
     CK(cudaStreamSynchronize(s));   // noff / blob are locals
     CKR(escape_dict(c, ar, nraw, &nesc));
-    std::vector<long long> eoff(n_ind + 1);
-    CK(cudaMemcpyAsync(eoff.data(), nesc.off, sizeof(long long) * ((size_t)n_ind + 1), cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(eoff.data(), nesc.off, sizeof(long long) * ((size_t)n_all + 1), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
     fa.names = nesc.bytes;
     for (int i = 0; i <= n_ind; ++i) fa.name_off[i] = (int32_t)eoff[i];
+    if (model) {
+      fa.field_off = nesc.off + n_ind;
+      for (int k = 0; k <= n_rank; ++k) fa.rank_name_off[k] = (int32_t)eoff[n_ind + n_fields + k];
+    }
+  }
+  if (model) {
+    // precedence, lowest to highest: indicators < properties < rankings (a later ranking beats an earlier one) < "id".
+    // The names are few, so the host resolves who beats whom and the device only checks presence per document.
+    auto same = [](const char *x, const char *y) { return strcmp(x, y) == 0; };
+    std::vector<uint16_t> fclash(std::max(n_fields, 1), 0);
+    for (int f = 0; f < n_fields; ++f) {
+      if (same(props->field_names[f], "id")) fclash[f] |= kClashId;
+      for (int k = 0; k < n_rank; ++k)
+        if (same(props->field_names[f], rk[k].name)) fclash[f] |= (uint16_t)(1u << k);
+    }
+    for (int i = 0; i < n_ind; ++i) {
+      fa.ind_field[i] = -1;
+      for (int f = 0; f < n_fields; ++f)
+        if (same(names[i], props->field_names[f])) fa.ind_field[i] = f;
+      for (int k = 0; k < n_rank; ++k)
+        if (same(names[i], rk[k].name)) fa.ind_rank[i] |= (uint8_t)(1u << k);
+    }
+    for (int k = 0; k < n_rank; ++k) {
+      if (same(rk[k].name, "id")) fa.rank_clash[k] |= kClashId;
+      for (int l = k + 1; l < n_rank; ++l)
+        if (same(rk[k].name, rk[l].name)) fa.rank_clash[k] |= (uint16_t)(1u << l);
+    }
+    uint16_t *d_fclash;
+    CKR(ar.alloc(&d_fclash, fclash.size()));
+    CK(cudaMemcpyAsync(d_fclash, fclash.data(), sizeof(uint16_t) * fclash.size(), cudaMemcpyHostToDevice, s));
+    fa.field_clash = d_fclash;
+    CKR(model_fields(c, ar, &fa, *row_ids, props, n_rank, rk, row_lo == 0));
+    CK(cudaStreamSynchronize(s));   // fclash is a local
   }
   for (int i = 0; i < n_ind; ++i) {
     const ResultMat &m = res->mats[i];
@@ -2644,22 +2963,23 @@ int cco_format_es_bulk(cco_ctx_t *ctx, const cco_result_t *res, int32_t n_names,
     fa.row_ptr[i] = d_rp;
     fa.col[i] = d_col;
   }
+  const int32_t n_docs = fa.n_rows + fa.n_extra;
   long long *doc_len, *doc_off;
-  CKR(ar.alloc(&doc_len, fa.n_rows + 1));
-  CKR(ar.alloc(&doc_off, fa.n_rows + 1));
-  CK(cudaMemsetAsync(doc_len + fa.n_rows, 0, 8, s));
-  if (fa.n_rows > 0) {
-    k_doc_len<<<grid_for(fa.n_rows, 256, c->sm_count), 256, 0, s>>>(fa, doc_len);
+  CKR(ar.alloc(&doc_len, (long long)n_docs + 1));
+  CKR(ar.alloc(&doc_off, (long long)n_docs + 1));
+  CK(cudaMemsetAsync(doc_len + n_docs, 0, 8, s));
+  if (n_docs > 0) {
+    k_doc_len<<<grid_for(n_docs, 256, c->sm_count), 256, 0, s>>>(fa, n_docs, doc_len);
     c->launches++;
   }
-  CKR(exclusive_sum_i64(c, ar, doc_len, doc_off, (long long)fa.n_rows + 1));
+  CKR(exclusive_sum_i64(c, ar, doc_len, doc_off, (long long)n_docs + 1));
   long long total = 0;
-  CK(cudaMemcpyAsync(&total, doc_off + fa.n_rows, 8, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(&total, doc_off + n_docs, 8, cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
   unsigned char *d_out;
   CKR(ar.alloc(&d_out, std::max<long long>(total, 1)));
-  if (fa.n_rows > 0 && total > 0) {
-    k_doc_write<<<grid_for((long long)fa.n_rows * 32, 256, c->sm_count), 256, 0, s>>>(fa, doc_off, d_out);
+  if (n_docs > 0 && total > 0) {
+    k_doc_write<<<grid_for((long long)n_docs * 32, 256, c->sm_count), 256, 0, s>>>(fa, n_docs, doc_off, d_out);
     c->launches++;
   }
   char *host = (char *)ctx->pinned_get((size_t)std::max<long long>(total, 1), /*for_result=*/false);
@@ -2670,6 +2990,18 @@ int cco_format_es_bulk(cco_ctx_t *ctx, const cco_result_t *res, int32_t n_names,
   *out_bytes = host;
   *out_len = total;
   return CCO_OK;
+}
+}  // namespace cco
+
+int cco_format_es_bulk(cco_ctx_t *ctx, const cco_result_t *res, int32_t n_names, const char *const *names,
+                       const cco_dictionary_t *row_ids, const cco_dictionary_t *col_ids, char **out_bytes, int64_t *out_len) {
+  return format_model(ctx, res, n_names, names, row_ids, col_ids, nullptr, 0, nullptr, out_bytes, out_len, "cco:format_es_bulk");
+}
+
+int cco_format_model(cco_ctx_t *ctx, const cco_result_t *res, int32_t n_names, const char *const *names, const cco_dictionary_t *row_ids,
+                     const cco_dictionary_t *col_ids, const cco_item_properties_t *props, int32_t n_rankings, const cco_ranking_t *rankings,
+                     char **out_bytes, int64_t *out_len) {
+  return format_model(ctx, res, n_names, names, row_ids, col_ids, props, n_rankings, rankings, out_bytes, out_len, "cco:format_model");
 }
 
 // ---- SURVEY.md 8f-3: PopModel rank histograms -------------------------------------------------------------------------
@@ -2686,26 +3018,7 @@ int cco_pop_model(cco_ctx_t *ctx, int32_t mode, int64_t n_events, const int32_t 
   Arena ar(s);
   nvtx_push("cco:pop_model");
   struct Pop { ~Pop() { nvtx_pop(); } } pop;
-  PopArgs a;
-  memset(&a, 0, sizeof a);
-  a.n_items = n_items;
-  const long long dur = end_ms - start_ms;
-  if (mode == CCO_POP_POPULAR) {
-    a.n_buckets = 1;
-    a.edge[0] = start_ms;
-    a.edge[1] = end_ms;
-  } else if (mode == CCO_POP_TRENDING) {   // PopModel.scala:134-138: halfInterval = durationMillis / 2
-    a.n_buckets = 2;
-    a.edge[0] = start_ms;
-    a.edge[1] = start_ms + dur / 2;
-    a.edge[2] = end_ms;
-  } else {                                  // PopModel.scala:159-164: older = dur / 3, middle = the same length, newer = the rest
-    a.n_buckets = 3;
-    a.edge[0] = start_ms;
-    a.edge[1] = start_ms + dur / 3;
-    a.edge[2] = a.edge[1] + dur / 3;
-    a.edge[3] = end_ms;
-  }
+  const PopArgs a = pop_args(mode, start_ms, end_ms, n_items);
   int32_t *d_item, *d_counts;
   long long *d_t;
   unsigned long long *d_tot;
@@ -2725,7 +3038,7 @@ int cco_pop_model(cco_ctx_t *ctx, int32_t mode, int64_t n_events, const int32_t 
     k_pop_count<<<grid_for(n_events, 256, c->sm_count), 256, 0, s>>>(n_events, d_item, d_t, a, d_counts, d_tot);
     c->launches++;
   }
-  k_pop_score<<<grid_for(n_items, 256, c->sm_count), 256, 0, s>>>(a, mode, d_counts, d_tot, d_score, d_present);
+  k_pop_score<double><<<grid_for(n_items, 256, c->sm_count), 256, 0, s>>>(a, mode, d_counts, d_tot, d_score, d_present);
   c->launches++;
   CK(cudaMemcpyAsync(score, d_score, sizeof(double) * (size_t)n_items, cudaMemcpyDeviceToHost, s));
   CK(cudaMemcpyAsync(present, d_present, (size_t)n_items, cudaMemcpyDeviceToHost, s));

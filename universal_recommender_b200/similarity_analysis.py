@@ -200,12 +200,8 @@ class CcoContext:
         buf = C.create_string_buffer(blob, max(len(blob), 1))
         return N.DictionaryT(len(enc), off.ctypes.data_as(C.POINTER(C.c_int64)), C.cast(buf, C.c_char_p)), (off, buf)
 
-    def format_es_bulk(self, handle, names, row_ids, col_ids) -> bytes:
-        """cco_format_es_bulk on a kept result (train_csr(..., keep=True)): one Elasticsearch bulk index action per row,
-        `{"index":{"_id":id}}\\n{"id":id,"<event>":[ordered correlator ids],...}\\n` -- what toStringMapRDD + URModel.save +
-        saveToEs produce for the reference (package.scala:82-110, URModel.scala:47-102, EsClient.scala:300-313)."""
+    def _format_args(self, names, row_ids, col_ids, keep):
         n = len(names)
-        keep = []
         rd, k = self._dictionary(row_ids)
         keep.append(k)
         cds = (N.DictionaryT * n)()
@@ -213,12 +209,63 @@ class CcoContext:
             cds[i], k = self._dictionary(ids)
             keep.append(k)
         nm = (C.c_char_p * n)(*[x.encode("utf-8") for x in names])
-        out, ln = C.c_void_p(), C.c_int64()
-        N.check(self._L.cco_format_es_bulk(self._h, handle, n, nm, C.byref(rd), cds, C.byref(out), C.byref(ln)))
+        return n, nm, rd, cds
+
+    def _take_body(self, out, ln) -> bytes:
         try:
             return C.string_at(out.value, ln.value)
         finally:
             self._L.cco_host_free(self._h, out)
+
+    def format_es_bulk(self, handle, names, row_ids, col_ids) -> bytes:
+        """cco_format_es_bulk on a kept result (train_csr(..., keep=True)): one Elasticsearch bulk index action per row,
+        `{"index":{"_id":id}}\\n{"id":id,"<event>":[ordered correlator ids],...}\\n` -- what toStringMapRDD + URModel.save +
+        saveToEs produce for the reference (package.scala:82-110, URModel.scala:47-102, EsClient.scala:300-313)."""
+        keep = []
+        n, nm, rd, cds = self._format_args(names, row_ids, col_ids, keep)
+        out, ln = C.c_void_p(), C.c_int64()
+        N.check(self._L.cco_format_es_bulk(self._h, handle, n, nm, C.byref(rd), cds, C.byref(out), C.byref(ln)))
+        return self._take_body(out, ln)
+
+    def format_model(self, handle, names, row_ids, col_ids, properties=None, rankings=None) -> bytes:
+        """cco_format_model: format_es_bulk plus the item properties and PopModel rankings joined in by item id, and a
+        document for every item without a row that has a property or a score (URAlgorithm.scala:351-367, URModel.scala:57-102).
+        properties = (field_names, item_offsets int64[n + 1], item_bytes uint8[], field int32[n], value_offsets int64[n + 1],
+        value_bytes uint8[]): n (item, field, JSON text) triples, the last of a repeated (item, field) wins.
+        rankings = [(field name, "popular" | "trending" | "hot", start_ms, end_ms, [(item_offsets, item_bytes, time_ms int64[])
+        per event name])].  Id columns in the layout of encode_ids."""
+        keep = []
+        n, nm, rd, cds = self._format_args(names, row_ids, col_ids, keep)
+        p64, p32 = C.POINTER(C.c_int64), C.POINTER(C.c_int32)
+        arr = lambda x, dt: np.ascontiguousarray(x, dtype=dt)
+        ptr = lambda b: b.ctypes.data if len(b) else None
+        props = None
+        if properties is not None:
+            fields, io, ib, fi, vo, vb = properties
+            io, ib, fi, vo, vb = arr(io, np.int64), arr(ib, np.uint8), arr(fi, np.int32), arr(vo, np.int64), arr(vb, np.uint8)
+            if len(io) < 1 or len(vo) != len(io) or len(fi) != len(io) - 1:
+                raise N.CcoInvalidArgument(N.E_INVALID_ARG, "properties need n + 1 item and value offsets and n field indices")
+            fn = (C.c_char_p * max(len(fields), 1))(*[f.encode("utf-8") for f in fields])
+            keep.append((io, ib, fi, vo, vb, fn))
+            props = N.ItemPropertiesT(len(io) - 1, io.ctypes.data_as(p64), ptr(ib), fi.ctypes.data_as(p32), vo.ctypes.data_as(p64), ptr(vb),
+                                      len(fields), fn)
+        rankings = list(rankings or [])
+        rk = (N.RankingT * max(len(rankings), 1))()
+        for k, (name, mode, start_ms, end_ms, streams) in enumerate(rankings):
+            st = (N.RankingStreamT * max(len(streams), 1))()
+            for q, (io, ib, tm) in enumerate(streams):
+                io, ib, tm = arr(io, np.int64), arr(ib, np.uint8), arr(tm, np.int64)
+                if len(io) < 1 or len(tm) != len(io) - 1:
+                    raise N.CcoInvalidArgument(N.E_INVALID_ARG, f"ranking {k}: a stream needs n + 1 offsets and n times")
+                keep.append((io, ib, tm))
+                st[q] = N.RankingStreamT(len(tm), io.ctypes.data_as(p64), ptr(ib), tm.ctypes.data_as(p64))
+            nb = name.encode("utf-8")
+            keep.append((st, nb))
+            rk[k] = N.RankingT(nb, N.POP_MODES.get(mode, -1), len(streams), int(start_ms), int(end_ms), st)
+        out, ln = C.c_void_p(), C.c_int64()
+        N.check(self._L.cco_format_model(self._h, handle, n, nm, C.byref(rd), cds, C.byref(props) if props is not None else None,
+                                         len(rankings), rk, C.byref(out), C.byref(ln)))
+        return self._take_body(out, ln)
 
     def train_csr(self, mats: Sequence[tuple[int, int, np.ndarray, np.ndarray]], params: Sequence[tuple[int, int, Optional[float]]],
                   seed: int, flags: int = 0, copy_arrays: bool = True, keep: bool = False):

@@ -1,6 +1,7 @@
 """Mirror of the train half of URAlgorithm that reaches the hot path
-(src/main/scala/URAlgorithm.scala:130-171 params, :310-349 calcAll).
-Everything else in URAlgorithm (popularity model, ES query building) is out of scope."""
+(src/main/scala/URAlgorithm.scala:130-171 params, :310-369 calcAll).
+calc_all_on_device runs the whole train half on the GPU, string events in and the Elasticsearch bulk body out.
+Everything else in URAlgorithm (calcPop, ES query building) is out of scope."""
 from __future__ import annotations
 
 import time
@@ -8,7 +9,8 @@ from dataclasses import dataclass, field
 from typing import Optional, Sequence
 
 from .indexed_dataset import IndexedDataset
-from .similarity_analysis import CcoContext, DownsamplableCrossOccurrenceDataset, SimilarityAnalysis
+from .similarity_analysis import CcoContext, DownsamplableCrossOccurrenceDataset, SimilarityAnalysis, default_context, encode_ids
+from .ur_model import RankingParams, aggregate_properties, extract_jvalue, property_json, rankings_for, rankings_params
 
 
 class DefaultURAlgoParams:
@@ -35,6 +37,7 @@ class URAlgorithmParams:
     indicators: Optional[Sequence[IndicatorParams]] = None
     seed: Optional[int] = None
     recsModel: str = "all"
+    rankings: Optional[Sequence[RankingParams]] = None
     # not an engine.json key of the reference: selects the literal Int/Int row sample rate recalled from Mahout 0.13.0's
     # sampleDownAndBinarize (SURVEY.md A.1; every interaction of a user above maxItemsPerUser is dropped) instead of the
     # real division min(m, d) / d this build defaults to (INTEGRATION.md "Deviation to know about")
@@ -50,7 +53,12 @@ class URAlgorithmParams:
             indicators=None if ind is None else [IndicatorParams(i["name"], i.get("maxItemsPerUser"),
                                                                  i.get("maxCorrelatorsPerItem"), i.get("minLLR")) for i in ind],
             seed=algo_params.get("seed"), recsModel=algo_params.get("recsModel", "all"),
+            rankings=None if algo_params.get("rankings") is None else [RankingParams.from_json(r) for r in algo_params["rankings"]],
             rowRateIntDiv=bool(algo_params.get("rowRateIntDiv", False)))
+
+    def model_event_names(self) -> list[str]:
+        """URAlgorithm.scala:230-235: the indicator names if given, else eventNames"""
+        return [i.name for i in self.indicators] if self.indicators else list(self.eventNames or [])
 
 
 def calc_all(actions: Sequence[tuple[str, IndexedDataset]], ap: URAlgorithmParams,
@@ -58,14 +66,10 @@ def calc_all(actions: Sequence[tuple[str, IndexedDataset]], ap: URAlgorithmParam
     """URAlgorithm.calcAll up to `cooccurrenceCorrelators` (URAlgorithm.scala:310-349): picks the global-
     params call or the per-indicator call, then zips the event names back on positionally (:349).
     `indicators(i)` is indexed by POSITION in `actions` exactly like the reference (:334-340)."""
-    if ap.recsModel not in ("all", "collabFiltering", "backfill"):
-        raise ValueError(f"Bad algorithm param recsModel=[{ap.recsModel}] in engine definition params, possibly a bad json "
-                         "value. Use one of the available parameter values (all, collabFiltering, backfill).")
+    _check_recs_model(ap)
     if ap.recsModel == "backfill":
         return []  # calcPop only: no CCO (URAlgorithm.scala:296)
-    seed = ap.seed if ap.seed is not None else int(time.time() * 1000)   # System.currentTimeMillis() (:325,345)
-    if ap.rowRateIntDiv:
-        flags |= 1   # CCO_FLAG_ROWRATE_INTDIV
+    seed, flags = _seed_and_flags(ap, flags)
     ids = [d for _, d in actions]
     if not ap.indicators:
         out = SimilarityAnalysis.cooccurrencesIDSs(
@@ -80,3 +84,67 @@ def calc_all(actions: Sequence[tuple[str, IndexedDataset]], ap: URAlgorithmParam
             for i, iD in enumerate(ids)]
         out = SimilarityAnalysis.crossOccurrenceDownsampled(datasets, seed, ctx=ctx, flags=flags)
     return [(name, o) for (name, _), o in zip(actions, out)]
+
+
+def _check_recs_model(ap: URAlgorithmParams):
+    if ap.recsModel not in ("all", "collabFiltering", "backfill"):
+        raise ValueError(f"Bad algorithm param recsModel=[{ap.recsModel}] in engine definition params, possibly a bad json "
+                         "value. Use one of the available parameter values (all, collabFiltering, backfill).")
+
+
+def _seed_and_flags(ap: URAlgorithmParams, flags: int):
+    seed = ap.seed if ap.seed is not None else int(time.time() * 1000)   # System.currentTimeMillis() (:325,345)
+    if ap.rowRateIntDiv:
+        flags |= 1   # CCO_FLAG_ROWRATE_INTDIV
+    return seed, flags
+
+
+def calc_all_on_device(events: Sequence[tuple[str, str, str, int]], set_events: Sequence[tuple[str, dict]], ap: URAlgorithmParams,
+                       min_events_per_user: Optional[int] = None, now_ms: Optional[int] = None, ctx: CcoContext | None = None,
+                       flags: int = 0) -> bytes:
+    """URAlgorithm.calcAll (URAlgorithm.scala:310-369) through URModel.save's documents, on the GPU: string events in, the
+    Elasticsearch bulk body out.  events = (user id, event name, item id, time ms); set_events = (item id, {field: value}) of
+    the items' `$set` events in event-time order.  Steps: cco_ingest_strings (Preparator) -> cco_train_dataset -> the
+    rankings' PopModel histograms and the property join -> cco_format_model.  "collabFiltering" writes the correlators only
+    (propertiesRDD is empty there); "backfill" (calcPop, which reads the live index) is not supported.
+    now_ms: the rankings' end when a ranking has no offsetDate (default: the wall clock)."""
+    _check_recs_model(ap)
+    if ap.recsModel == "backfill":
+        raise ValueError("recsModel=backfill runs calcPop against the live index; it has no train half to run here")
+    ctx = ctx or default_context()
+    seed, flags = _seed_and_flags(ap, flags)
+    names = ap.model_event_names()
+    by_name: dict = {}
+    for u, e, i, t in events:
+        by_name.setdefault(e, []).append((u, i, t))
+    actions = [(n, by_name[n]) for n in names if by_name.get(n)]   # DataSource.scala:79-89 drops empty event RDDs
+    if not actions:
+        raise ValueError("no events of the model's event names")
+    cols = [(*encode_ids([u for u, _, _ in ev]), *encode_ids([i for _, i, _ in ev])) for _, ev in actions]
+    if ap.indicators:
+        ind = {i.name: i for i in ap.indicators}
+        params = [(ind[n].maxItemsPerUser or DefaultURAlgoParams.MaxEventsPerEventType,
+                   ind[n].maxCorrelatorsPerItem or DefaultURAlgoParams.MaxCorrelatorsPerEventType, ind[n].minLLR) for n, _ in actions]
+    else:
+        params = [(ap.maxEventsPerEventType or DefaultURAlgoParams.MaxEventsPerEventType,
+                   ap.maxCorrelatorsPerEventType or DefaultURAlgoParams.MaxCorrelatorsPerEventType, None)] * len(actions)
+    props, rankings = None, None
+    if ap.recsModel == "all":
+        triples = [(i, f, extract_jvalue(f, v)) for i, f, v in aggregate_properties(set_events)]
+        fields = list(dict.fromkeys(f for _, f, _ in triples))
+        fidx = {f: k for k, f in enumerate(fields)}
+        props = (fields, *encode_ids([i for i, _, _ in triples]), [fidx[f] for _, f, _ in triples],
+                 *encode_ids([property_json(v) for _, _, v in triples]))
+        now = now_ms if now_ms is not None else int(time.time() * 1000)
+        ev_by_name = {n: [(i, t) for _, i, t in ev] for n, ev in by_name.items()}
+        rankings = [(r.field, r.mode, r.start_ms, r.end_ms, [(*encode_ids(items), times) for items, times in r.streams])
+                    for r in rankings_for(rankings_params(ap.rankings, names), ev_by_name, now, names)]
+    ds, _, items = ctx.ingest_strings(cols, min_events_per_user or 0)
+    try:
+        _, h = ctx.train_dataset(ds, params, seed, flags, keep=True)
+        try:
+            return ctx.format_model(h, [n for n, _ in actions], items[0], items, props, rankings)
+        finally:
+            ctx.free_result(h)
+    finally:
+        ctx.free_dataset(ds)

@@ -1,0 +1,274 @@
+"""Host mirror of what calcAll writes besides the correlators (SURVEY.md 8f-2, 8f-3): the item properties and PopModel ranks
+of `propertiesRDD` (URAlgorithm.scala:351-367), joined into one document per item by URModel.save's groupAll
+(URModel.scala:57-102).  This is the definition cco_format_model is held to; the device builds the same documents from id
+strings with CcoContext.format_model.
+
+Precedence inside a document, lowest to highest (Scala `++` and `+`: the later source wins):
+  correlator fields < properties (fieldsPropMap ++ rankPropMap) < ranks (a later ranking beats an earlier one of the same
+  name, getRanksRDD's foldLeft) < "id" (propsMap + ("id" -> itemId)).
+"""
+from __future__ import annotations
+
+import datetime
+import re
+from collections import Counter
+from dataclasses import dataclass
+from decimal import Decimal
+from typing import Iterable, Optional, Sequence
+
+
+class RankingFieldName:
+    """PopModel.scala:31-41"""
+    UserRank, UniqueRank, PopRank, TrendRank, HotRank, UnknownRank = "userRank", "uniqueRank", "popRank", "trendRank", "hotRank", "unknownRank"
+    ALL = (UserRank, UniqueRank, PopRank, TrendRank, HotRank)
+
+
+class RankingType:
+    """PopModel.scala:43-51"""
+    Popular, Trending, Hot, UserDefined, Random = "popular", "trending", "hot", "userDefined", "random"
+
+
+NAME_BY_TYPE = {RankingType.Popular: RankingFieldName.PopRank, RankingType.Trending: RankingFieldName.TrendRank,
+                RankingType.Hot: RankingFieldName.HotRank, RankingType.UserDefined: RankingFieldName.UserRank,
+                RankingType.Random: RankingFieldName.UniqueRank}   # PopModel.scala:205-210, default unknownRank
+
+BACKFILL_FIELD_NAME = RankingFieldName.PopRank   # URAlgorithm.scala:64-66
+BACKFILL_TYPE = RankingType.Popular
+BACKFILL_DURATION = "3650 days"
+
+
+@dataclass
+class RankingParams:
+    """URAlgorithm.scala:110-117 (one entry of the engine.json `rankings` list)"""
+    name: Optional[str] = None
+    type: Optional[str] = None
+    eventNames: Optional[Sequence[str]] = None
+    offsetDate: Optional[str] = None
+    endDate: Optional[str] = None
+    duration: Optional[str] = None
+
+    @staticmethod
+    def from_json(d: dict) -> "RankingParams":
+        return RankingParams(d.get("name"), d.get("type"), d.get("eventNames"), d.get("offsetDate"), d.get("endDate"), d.get("duration"))
+
+    def ranking_type(self) -> str:
+        return self.type or BACKFILL_TYPE
+
+    def field_name(self) -> str:
+        return self.name or NAME_BY_TYPE.get(self.ranking_type(), RankingFieldName.UnknownRank)
+
+
+def rankings_params(rankings: Optional[Sequence[RankingParams]], model_event_names: Sequence[str]) -> list[RankingParams]:
+    """URAlgorithm.scala:249-256: the configured rankings, or one `popRank` popular ranking over the first model event name
+    for "3650 days"; then one ranking per type, the first of each.  Scala's groupBy gives no order; this mirror keeps the
+    types in order of first appearance."""
+    rs = list(rankings) if rankings is not None else [
+        RankingParams(BACKFILL_FIELD_NAME, BACKFILL_TYPE, list(model_event_names[:1]), None, None, BACKFILL_DURATION)]
+    by_type: dict = {}
+    for r in rs:
+        by_type.setdefault(r.type, r)
+    return list(by_type.values())
+
+
+_UNITS = {"d": 86400, "day": 86400, "days": 86400, "h": 3600, "hour": 3600, "hours": 3600,
+          "min": 60, "mins": 60, "minute": 60, "minutes": 60, "m": 60,
+          "s": 1, "sec": 1, "secs": 1, "second": 1, "seconds": 1,
+          "ms": Decimal("0.001"), "milli": Decimal("0.001"), "millis": Decimal("0.001"), "millisecond": Decimal("0.001"),
+          "milliseconds": Decimal("0.001")}
+
+
+def duration_seconds(duration) -> int:
+    """`Duration(durationAsString).toSeconds.toInt` for "<n> <unit>" strings (units of scala.concurrent.duration, day to
+    millisecond).  A bare number, as examples/pop-engine.json writes it (259200), is read as seconds."""
+    if isinstance(duration, (int, float)) and not isinstance(duration, bool):
+        return int(duration)
+    m = re.fullmatch(r"\s*([0-9]+(?:\.[0-9]+)?)\s*([A-Za-z]*)\s*", str(duration))
+    if not m or (m.group(2) and m.group(2) not in _UNITS):
+        raise ValueError(f"bad duration {duration!r}")
+    return int(Decimal(m.group(1)) * (_UNITS[m.group(2)] if m.group(2) else 1))
+
+
+def ranking_window(rp: RankingParams, now_ms: int) -> tuple[int, int]:
+    """PopModel.calc (PopModel.scala:57-77): end = offsetDate (ISO 8601; 'now' if it does not parse, as the reference
+    warns and does), start = end - duration seconds.  Events count in [start, end)."""
+    end = now_ms
+    if rp.offsetDate is not None:
+        try:
+            dt = datetime.datetime.fromisoformat(rp.offsetDate.replace("Z", "+00:00"))
+            if dt.tzinfo is None:
+                dt = dt.replace(tzinfo=datetime.timezone.utc)
+            end = int(dt.timestamp() * 1000)
+        except ValueError:
+            end = now_ms
+    return end - duration_seconds(rp.duration if rp.duration is not None else BACKFILL_DURATION) * 1000, end
+
+
+def pop_scores(mode: str, items: Sequence[str], times_ms: Sequence[int], start_ms: int, end_ms: int) -> dict:
+    """PopModel.calcPopular / calcTrending / calcHot (PopModel.scala:113-182) per item id: {item: score} for the items the
+    reference's RDD holds.  Same rules as cco_pop_model, including the empty-bucket ones."""
+    def count(lo, hi):
+        return Counter(j for j, t in zip(items, times_ms) if lo <= t < hi)
+    dur = end_ms - start_ms
+    if mode == RankingType.Popular:
+        return {j: float(c) for j, c in count(start_ms, end_ms).items()}
+    if mode == RankingType.Trending:
+        half = dur // 2
+        older = count(start_ms, start_ms + half)
+        if not older:
+            return {}
+        newer = count(start_ms + half, end_ms)
+        return {j: float(newer[j] - older[j]) for j in newer if j in older}
+    if mode == RankingType.Hot:
+        third = dur // 3
+        older = count(start_ms, start_ms + third)
+        middle = count(start_ms + third, start_ms + 2 * third)
+        if not older or not middle:
+            return {}
+        newer = count(start_ms + 2 * third, end_ms)
+        return {j: float((newer[j] - middle[j]) - (middle[j] - older[j])) for j in newer if j in middle and j in older}
+    raise ValueError(mode)
+
+
+@dataclass
+class Ranking:
+    """One ranking ready for the model: its field, PopModel mode, window and per-event-name streams of (item, time)."""
+    field: str
+    mode: str
+    start_ms: int
+    end_ms: int
+    streams: list   # [(item ids list[str], times list[int])] one per event name
+
+    def scores(self) -> dict:
+        items = [i for s in self.streams for i in s[0]]
+        times = [t for s in self.streams for t in s[1]]
+        return pop_scores(self.mode, items, times, self.start_ms, self.end_ms)
+
+
+def rankings_for(params: Sequence[RankingParams], events_by_name: dict, now_ms: int, model_event_names: Sequence[str]) -> list[Ranking]:
+    """getRanksRDD (URAlgorithm.scala:537-560): one Ranking per histogram ranking.  A ranking reads the event store (every
+    user's events of its event names, {name: [(item, time ms)]}), not the Preparator output; without eventNames it reads the
+    first model event name.  userDefined rankings produce nothing (PopModel returns an
+    empty RDD; the field comes from the item's own properties); random (uniqueRank) is not reproducible and is refused."""
+    out = []
+    for rp in params:
+        t = rp.ranking_type()
+        if t == RankingType.Random:
+            raise ValueError("random rankings (uniqueRank) are not supported: pass such a rank as an item property")
+        if t not in (RankingType.Popular, RankingType.Trending, RankingType.Hot):
+            continue   # userDefined, or an unknown type the reference warns about and skips
+        start, end = ranking_window(rp, now_ms)
+        names = rp.eventNames if rp.eventNames is not None else list(model_event_names[:1])
+        streams = [([i for i, _ in events_by_name.get(n, [])], [tm for _, tm in events_by_name.get(n, [])]) for n in names]
+        out.append(Ranking(rp.field_name(), t, start, end, streams or [([], [])]))
+    return out
+
+
+def aggregate_properties(set_events: Iterable[tuple[str, dict]]) -> list[tuple[str, str, object]]:
+    """`$set` events in event-time order -> (item, field, value) triples, one per (item, field): later sets of a key win.
+    Items and fields keep the order of their first `$set`.  `$unset` / `$delete` stay with the event store."""
+    props: dict = {}
+    for item, fields in set_events:
+        d = props.setdefault(item, {})
+        for k, v in fields.items():
+            d[k] = v
+    return [(item, k, v) for item, d in props.items() for k, v in d.items()]
+
+
+def extract_jvalue(key: str, value):
+    """URModel.extractJvalue (URModel.scala:126-140) without the date conversion: a string under a RankingFieldName becomes a
+    double, lists convert elementwise, everything else stays."""
+    if isinstance(value, list):
+        return [extract_jvalue(key, v) for v in value]
+    if isinstance(value, str) and key in RankingFieldName.ALL:
+        return float(value)
+    return value
+
+
+def java_double(x: float) -> str:
+    """Java's Double.toString: plain decimal with at least one fraction digit for 1e-3 <= |x| < 1e7, else computerised
+    scientific notation (1.0E7, 1.5E-4), over the shortest digits that round-trip (Python's repr digits, as JDK 19+ prints
+    them).  Not checked against a JVM here."""
+    x = float(x)
+    if x != x or x in (float("inf"), float("-inf")):
+        raise ValueError(f"{x} has no JSON text")
+    sign = "-" if str(x).startswith("-") else ""
+    if x == 0:
+        return sign + "0.0"
+    _, digits, exp = Decimal(repr(abs(x))).normalize().as_tuple()
+    ds = "".join(map(str, digits))   # significant digits, no leading or trailing zeros
+    point = len(ds) + exp            # digits before the decimal point
+    if 1e-3 <= abs(x) < 1e7:
+        if point <= 0:
+            return sign + "0." + "0" * (-point) + ds
+        if point >= len(ds):
+            return sign + ds + "0" * (point - len(ds)) + ".0"
+        return sign + ds[:point] + "." + ds[point:]
+    return sign + ds[0] + "." + (ds[1:] or "0") + "E" + str(point - 1)
+
+
+def json_string(s: str) -> str:
+    """the repo's JSON string escaping (cco_format_es_bulk): '"' and '\\' get a backslash, code points below 0x20 become
+    \\u00xx, everything else passes through"""
+    out = []
+    for ch in s:
+        if ch in '"\\':
+            out.append("\\" + ch)
+        elif ord(ch) < 0x20:
+            out.append("\\u%04x" % ord(ch))
+        else:
+            out.append(ch)
+    return '"' + "".join(out) + '"'
+
+
+def property_json(value) -> str:
+    """a property value -> the JSON text the device splices verbatim (floats as Java's Double.toString)"""
+    if value is None:
+        return "null"
+    if isinstance(value, bool):
+        return "true" if value else "false"
+    if isinstance(value, int):
+        return str(value)
+    if isinstance(value, float):
+        return java_double(value)
+    if isinstance(value, str):
+        return json_string(value)
+    if isinstance(value, (list, tuple)):
+        return "[" + ",".join(property_json(v) for v in value) + "]"
+    if isinstance(value, dict):
+        return "{" + ",".join(json_string(str(k)) + ":" + property_json(v) for k, v in value.items()) + "}"
+    raise TypeError(f"no JSON text for {type(value).__name__}")
+
+
+def model_documents(row_ids: Sequence[str], indicators: Sequence[tuple[str, Sequence[Sequence[str]]]],
+                    properties: Sequence[tuple[str, str, object]], rankings: Sequence[Ranking]) -> list[dict]:
+    """URModel.save's groupAll / getRanksRDD's fullOuterJoin as one dict per item, in the documents' order: the rows first
+    (row order), then the items without a row that have a property or a score, by first appearance (property triples, then
+    the ranking streams in order).  indicators = [(event name, correlator ids per row)]; properties = (item, field, value)
+    triples, the last of a repeated (item, field) wins."""
+    props: dict = {}
+    for item, f, v in properties:
+        props.setdefault(item, {})[f] = v
+    scored = [(r.field, r.scores()) for r in rankings]
+    rows = set(row_ids)
+    order = list(row_ids)
+    seen = set()
+    candidates = [i for i, _, _ in properties] + [i for r in rankings for s in r.streams for i in s[0]]
+    for item in candidates:
+        if item in rows or item in seen:
+            continue
+        seen.add(item)
+        if item in props or any(item in sc for _, sc in scored):
+            order.append(item)
+    docs = []
+    for d, item in enumerate(order):
+        doc: dict = {}
+        if d < len(row_ids):
+            for name, lists in indicators:
+                doc[name] = list(lists[d])
+        doc.update(props.get(item, {}))
+        for name, sc in scored:
+            if item in sc:
+                doc[name] = sc[item]
+        doc["id"] = item
+        docs.append(doc)
+    return docs
