@@ -326,9 +326,10 @@ int cco_dataset_dictionary(const cco_dataset_t *ds, int32_t which, cco_dictionar
  * names.  score[j] is meaningful iff present[j] != 0: `popular` lists the items with an event in the interval, `trending`
  * the items seen in both halves (newer - older), `hot` the items seen in all three thirds ((newer - middle) - (middle -
  * older)); `trending` / `hot` are empty when the older (or middle) bucket has no event at all, as in the reference.
- * RankingType.Random / UserDefined are not histograms and stay with the caller.
+ * RankingType.UserDefined is not a histogram and stays with the caller.  CCO_POP_RANDOM is accepted by cco_format_model only
+ * (a random rank is keyed by id string; this entry works on item indices): see there.
  */
-enum { CCO_POP_POPULAR = 0, CCO_POP_TRENDING = 1, CCO_POP_HOT = 2 };
+enum { CCO_POP_POPULAR = 0, CCO_POP_TRENDING = 1, CCO_POP_HOT = 2, CCO_POP_RANDOM = 3 };
 int cco_pop_model(cco_ctx_t *ctx, int32_t mode, int64_t n_events, const int32_t *item, const int64_t *time_ms, int32_t n_items,
                   int64_t start_ms, int64_t end_ms, double *score, unsigned char *present);
 
@@ -346,6 +347,14 @@ int cco_pop_model(cco_ctx_t *ctx, int32_t mode, int64_t n_events, const int32_t 
  * JSON-escaped.  Rank numbers are Java's Double.toString of an integer: "-"?digits".0" below 10^7, else d.ddd"E"n with the
  * trailing zeros of the digits dropped (1.0E7, 1.2345678E7).  Without properties and rankings the body is byte-identical
  * to cco_format_es_bulk.
+ * CCO_POP_RANDOM (RankingType.Random, PopModel.calcRandom, PopModel.scala:98-110): the items are the targets of every event
+ * of the ranking's streams in [start_ms, end_ms) -- pass every event name's stream, as the reference ignores eventNames --
+ * plus every item with a property triple.  The value is n · 10^-15, uniform in [0, 1), a function of the id bytes and the
+ * window only: h = the id's 64-bit string hash (cco_strings.cuh k_str_hash), r = mix64(h ^ mix64((uint64)start_ms ^
+ * mix64((uint64)end_ms))), n = floor(r · 10^15 / 2^64).  So the values repeat for a repeated window and change with it (an
+ * ordinary train ends "now"), and every rank of a group writes the same value.  Text: Java's Double.toString of n / 10^15:
+ * "0.0" for n = 0, "0." and n's 15 digits with the trailing zeros dropped for n >= 10^12 (0.001, 0.5, 0.123456789012345),
+ * else d.ddd"E-"k (1.0E-15, 1.23E-13, 9.99999999999E-4).
  * Errors: CCO_E_INVALID_ARG for negative or decreasing offsets in any column, a field index outside [0, n_fields), an empty
  * value, repeated field names, end_ms < start_ms or a bad mode (decided on the device before any kernel reads bytes through
  * the offsets); CCO_E_UNSUPPORTED for more than CCO_MAX_RANKINGS rankings or rows + property triples + ranking events >= 2^31.
@@ -368,7 +377,7 @@ typedef struct {                  /* the events of one event name: target item i
 } cco_ranking_stream_t;
 typedef struct {                  /* one PopModel ranking over [start_ms, end_ms) of its streams, as cco_pop_model */
   const char *name;               /* the document field */
-  int32_t mode;                   /* CCO_POP_* */
+  int32_t mode;                   /* CCO_POP_*, CCO_POP_RANDOM included */
   int32_t n_streams;              /* >= 1 */
   int64_t start_ms, end_ms;
   const cco_ranking_stream_t *streams;

@@ -10,7 +10,9 @@ Prints one JSON line:
   - host_mirror: ur_model.model_documents on a sample (the first --sample events of each stream, all properties), its rate
   - parity_ok: json.loads of every document of format_model on that sample == model_documents
   - gpu name and power limit, read in the same run
-usage: python tools/model_format_bench.py --config C3 --steps 5 --warmup 1 --sample 200000
+  - with --random: model_random_ms_median / model_random_bytes, the same call with a third ranking, uniqueRank (random) over
+    every event stream, timed after the call without it; the parity sample then holds the random ranking too
+usage: python tools/model_format_bench.py --config C3 --steps 5 --warmup 1 --sample 200000 [--random]
 """
 from __future__ import annotations
 
@@ -46,6 +48,7 @@ def main():
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=1)
     ap.add_argument("--sample", type=int, default=200_000, help="events per stream for the host mirror and the parity check")
+    ap.add_argument("--random", action="store_true", help="also time format_model with a random (uniqueRank) ranking added")
     a = ap.parse_args()
     cfg = synth.CONFIGS[a.config]
     n_types, n_users, n_items = cfg["n_types"], cfg["n_users"], cfg["n_items"]
@@ -79,6 +82,7 @@ def main():
         del items
     rankings = [("popRank", "popular", END_MS - WINDOW_MS, END_MS, streams[:1]),
                 ("trendRank", "trending", END_MS - WINDOW_MS, END_MS, streams)]
+    random_ranking = ("uniqueRank", "random", END_MS - WINDOW_MS, END_MS, streams)
     model_h2d = int(sum(o.nbytes + (o[-1] - o[0]) + tm.nbytes for o, _, tm in streams) + sum(o.nbytes + (o[-1] - o[0]) for o, _, _ in streams[:1])
                     + props[1].nbytes + len(props[2]) + props[3].nbytes + props[4].nbytes + len(props[5]))
 
@@ -94,6 +98,12 @@ def main():
 
     es, es_ms = timed(lambda: ctx.format_es_bulk(h, names, ids, cols))
     body, model_ms = timed(lambda: ctx.format_model(h, names, ids, cols, props, rankings))
+    extra = {}
+    if a.random:
+        body_r, random_ms = timed(lambda: ctx.format_model(h, names, ids, cols, props, rankings + [random_ranking]))
+        extra = {"model_random_ms_median": round(float(np.median(random_ms)), 2), "model_random_ms_all": [round(x, 2) for x in random_ms],
+                 "model_random_bytes": len(body_r)}
+        del body_r
 
     # host mirror and parity on a sample of every stream
     S = min(a.sample, per_type)
@@ -102,6 +112,8 @@ def main():
         sample_streams.append((ur.decode_ids(off[:S + 1], bytes(data[:off[S]])), tm[:S].tolist()))
     sample_rankings = [um.Ranking("popRank", "popular", END_MS - WINDOW_MS, END_MS, sample_streams[:1]),
                        um.Ranking("trendRank", "trending", END_MS - WINDOW_MS, END_MS, sample_streams)]
+    if a.random:
+        sample_rankings.append(um.Ranking("uniqueRank", "random", END_MS - WINDOW_MS, END_MS, sample_streams))
     per_row = [(n, [[ids[c] for c in r[4][r[3][q]:r[3][q + 1]]] for q in range(len(r[3]) - 1)]) for n, r in zip(names, res)]
     triples = [(i, fields[k % 2], json.loads(v)) for k, (i, v) in enumerate(zip(triples_items, values))]
     t0 = time.perf_counter()
@@ -121,6 +133,7 @@ def main():
         "es_bulk_ms_median": round(float(np.median(es_ms)), 2), "es_bulk_ms_all": [round(x, 2) for x in es_ms],
         "model_ms_median": round(float(np.median(model_ms)), 2), "model_ms_all": [round(x, 2) for x in model_ms],
         "es_bulk_bytes": len(es), "model_bytes": len(body), "model_documents": body.count(b"\n") // 2, "model_h2d_bytes": model_h2d,
+        **extra,
         "host_mirror": {"ranking_events": S * (n_types + 1), "documents": len(want), "s": round(host_s, 3), "threads": 1},
         "parity_ok": bool(parity),
     }), flush=True)

@@ -20,7 +20,7 @@ FLAG_RESULT_NO_COUNT = 16
 FLAG_RESULT_NO_LLR = 32
 MAX_TOP_K = 2048
 MAX_RANKINGS = 8
-POP_MODES = {"popular": 0, "trending": 1, "hot": 2}
+POP_MODES = {"popular": 0, "trending": 1, "hot": 2, "random": 3}   # random: cco_format_model only
 
 
 class CcoError(RuntimeError):

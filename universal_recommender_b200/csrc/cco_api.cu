@@ -2710,38 +2710,7 @@ static int model_fields(cco_ctx *c, Arena &ar, FormatArgs *fa, const cco_diction
   const long long G = tb.n_groups;
   fa->n_groups = G;
   fa->row_group = gid + fa->row_id_base;
-  // 2. rankings: PopModel histograms over the groups
-  fa->n_rank = n_rank;
-  if (n_rank > 0) {
-    long long *score;
-    unsigned char *pmask, *present;
-    int32_t *counts;
-    unsigned long long *tot;
-    CKR(ar.alloc(&score, (size_t)n_rank * G));
-    CKR(ar.alloc(&pmask, G));
-    CKR(ar.alloc(&present, G));
-    CKR(ar.alloc(&counts, (size_t)3 * G));
-    CKR(ar.alloc(&tot, 4));
-    CK(cudaMemsetAsync(pmask, 0, (size_t)G, s));
-    for (int k = 0; k < n_rank; ++k) {
-      const PopArgs pa = pop_args(rk[k].mode, rk[k].start_ms, rk[k].end_ms, (int32_t)G);
-      const long long ne = rank_begin[k + 1] - rank_begin[k];
-      CK(cudaMemsetAsync(counts, 0, sizeof(int32_t) * (size_t)pa.n_buckets * G, s));
-      CK(cudaMemsetAsync(tot, 0, 32, s));
-      if (ne > 0) {
-        k_pop_count<<<grid_for(ne, 256, c->sm_count), 256, 0, s>>>(ne, gid + R + P + rank_begin[k], d_t + rank_begin[k], pa, counts, tot);
-        c->launches++;
-      }
-      k_pop_score<long long><<<grid_for(G, 256, c->sm_count), 256, 0, s>>>(pa, rk[k].mode, counts, tot, score + (size_t)k * G, present);
-      k_rank_mask<<<grid_for(G, 256, c->sm_count), 256, 0, s>>>(G, present, k, pmask);
-      c->launches += 2;
-    }
-    ar.release(counts);
-    ar.release(present);
-    fa->score = score;
-    fa->pmask = pmask;
-  }
-  // 3. properties: sorted by (group, field), stable in the triple index, so the last triple of each run wins
+  // 2. properties: sorted by (group, field), stable in the triple index, so the last triple of each run wins
   if (P > 0) {
     unsigned long long *k0, *k1;
     int32_t *v0, *v1, *pbeg, *pend;
@@ -2770,6 +2739,44 @@ static int model_fields(cco_ctx *c, Arena &ar, FormatArgs *fa, const cco_diction
     fa->ptri = vb.Current();
     fa->pbeg = pbeg;
     fa->pend = pend;
+  }
+  // 3. rankings: PopModel histograms over the groups; random ones from the popular histogram, the properties and the hash
+  fa->n_rank = n_rank;
+  if (n_rank > 0) {
+    long long *score;
+    unsigned char *pmask, *present;
+    int32_t *counts;
+    unsigned long long *tot;
+    CKR(ar.alloc(&score, (size_t)n_rank * G));
+    CKR(ar.alloc(&pmask, G));
+    CKR(ar.alloc(&present, G));
+    CKR(ar.alloc(&counts, (size_t)3 * G));
+    CKR(ar.alloc(&tot, 4));
+    CK(cudaMemsetAsync(pmask, 0, (size_t)G, s));
+    for (int k = 0; k < n_rank; ++k) {
+      const bool random = rk[k].mode == CCO_POP_RANDOM;
+      const PopArgs pa = pop_args(random ? CCO_POP_POPULAR : rk[k].mode, rk[k].start_ms, rk[k].end_ms, (int32_t)G);
+      const long long ne = rank_begin[k + 1] - rank_begin[k];
+      CK(cudaMemsetAsync(counts, 0, sizeof(int32_t) * (size_t)pa.n_buckets * G, s));
+      CK(cudaMemsetAsync(tot, 0, 32, s));
+      if (ne > 0) {
+        k_pop_count<<<grid_for(ne, 256, c->sm_count), 256, 0, s>>>(ne, gid + R + P + rank_begin[k], d_t + rank_begin[k], pa, counts, tot);
+        c->launches++;
+      }
+      if (random) {
+        k_random_score<<<grid_for(G, 256, c->sm_count), 256, 0, s>>>(G, counts, fa->pbeg, fa->pend, tb.first_sorted, key.hash,
+                                                                    rk[k].start_ms, rk[k].end_ms, score + (size_t)k * G, present);
+        fa->rank_scale[k] = 15;
+      } else {
+        k_pop_score<long long><<<grid_for(G, 256, c->sm_count), 256, 0, s>>>(pa, rk[k].mode, counts, tot, score + (size_t)k * G, present);
+      }
+      k_rank_mask<<<grid_for(G, 256, c->sm_count), 256, 0, s>>>(G, present, k, pmask);
+      c->launches += 2;
+    }
+    ar.release(counts);
+    ar.release(present);
+    fa->score = score;
+    fa->pmask = pmask;
   }
   // 4. documents of items without a row, in order of first appearance (only the result that begins at row 0 writes them)
   fa->n_extra = 0;
@@ -2837,7 +2844,8 @@ static int model_check_host(const cco_dictionary_t *row_ids, const cco_item_prop
   for (int k = 0; k < n_rank; ++k) {
     const cco_ranking_t &r = rk[k];
     if (!r.name) return set_error(CCO_E_INVALID_ARG, "ranking %d: null name", k);
-    if (r.mode < CCO_POP_POPULAR || r.mode > CCO_POP_HOT) return set_error(CCO_E_INVALID_ARG, "ranking %d: mode must be CCO_POP_POPULAR, _TRENDING or _HOT", k);
+    if (r.mode < CCO_POP_POPULAR || r.mode > CCO_POP_RANDOM)
+      return set_error(CCO_E_INVALID_ARG, "ranking %d: mode must be CCO_POP_POPULAR, _TRENDING, _HOT or _RANDOM", k);
     if (r.end_ms < r.start_ms) return set_error(CCO_E_INVALID_ARG, "ranking %d: end before start (Joda Interval would throw)", k);
     if (r.n_streams < 1 || !r.streams) return set_error(CCO_E_INVALID_ARG, "ranking %d: needs at least one stream", k);
     for (int q = 0; q < r.n_streams; ++q) {

@@ -92,11 +92,15 @@ struct FormatArgs {
   const unsigned char *pmask;                   // [n_groups] bit k: ranking k scores the group
   int32_t rank_name_off[kMaxRankings + 1];      // into names
   uint16_t rank_clash[kMaxRankings];            // bits: LATER rankings of the same name (they win); kClashId
+  uint8_t rank_scale[kMaxRankings];             // ranking k's value is score · 10^-rank_scale[k]: 0, or 15 (random)
 };
 
-// Java's Double.toString of an integer-valued double |v| < 2^53: "-"?digits".0" below 10^7, else computerised scientific
-// notation d.ddd"E"n with the trailing zeros of the digits dropped (1.0E7, 1.2345678E7).  Returns the length (<= 25).
-__device__ __forceinline__ int java_double_text(long long v, unsigned char *out) {
+// Java's Double.toString of v · 10^-scale, for scale 0 (an integer-valued double, |v| < 2^53) or scale 15 (0 <= v < 10^15).
+// Both values have at most 16 significant digits, which are their shortest round-trip digits (the decimal is the nearest
+// double's shortest text), so the text is built from v alone: plain d.ddd with at least one fraction digit for
+// 10^-3 <= |x| < 10^7, else computerised scientific notation d.ddd"E"n; trailing zeros of the digits are dropped
+// (0.0, 12.0, 1.0E7, 1.2345678E7, 0.001, 0.12, 9.99E-4, 1.0E-15).  Returns the length (<= 25).
+__device__ __forceinline__ int java_double_text(long long v, int scale, unsigned char *out) {
   unsigned long long u = v < 0 ? 0ULL - (unsigned long long)v : (unsigned long long)v;
   unsigned char d[20];
   int n = 0;
@@ -104,24 +108,35 @@ __device__ __forceinline__ int java_double_text(long long v, unsigned char *out)
     d[n++] = (unsigned char)('0' + u % 10);
     u /= 10;
   } while (u);   // d[n - 1] is the leading digit
-  int p = 0;
-  if (v < 0) out[p++] = '-';
-  if (n <= 7) {
-    for (int k = n - 1; k >= 0; --k) out[p++] = d[k];
-    out[p++] = '.';
-    out[p++] = '0';
-    return p;
-  }
+  const int e = v == 0 ? 0 : n - 1 - scale;   // decimal exponent of the leading digit
   int low = 0;   // trailing zeros after the leading digit
   while (low < n - 1 && d[low] == '0') ++low;
+  int p = 0;
+  if (v < 0) out[p++] = '-';
+  if (e >= 0 && e < 7) {          // integer digits "." fraction digits (at least one)
+    int k = n - 1;
+    for (; k >= n - 1 - e; --k) out[p++] = d[k];
+    out[p++] = '.';
+    if (k < low) out[p++] = '0';
+    for (; k >= low; --k) out[p++] = d[k];
+    return p;
+  }
+  if (e < 0 && e >= -3) {         // "0." zeros digits
+    out[p++] = '0';
+    out[p++] = '.';
+    for (int z = -1; z > e; --z) out[p++] = '0';
+    for (int k = n - 1; k >= low; --k) out[p++] = d[k];
+    return p;
+  }
   out[p++] = d[n - 1];
   out[p++] = '.';
   if (low == n - 1) out[p++] = '0';
   for (int k = n - 2; k >= low; --k) out[p++] = d[k];
   out[p++] = 'E';
-  int e = n - 1;   // 7 .. 15
-  if (e >= 10) out[p++] = (unsigned char)('0' + e / 10);
-  out[p++] = (unsigned char)('0' + e % 10);
+  if (e < 0) out[p++] = '-';
+  const int ae = e < 0 ? -e : e;   // 7 .. 15 or 4 .. 15
+  if (ae >= 10) out[p++] = (unsigned char)('0' + ae / 10);
+  out[p++] = (unsigned char)('0' + ae % 10);
   return p;
 }
 
@@ -196,7 +211,7 @@ __global__ void k_doc_len(const FormatArgs a, int32_t n_docs, long long *__restr
     for (int k = 0; k < a.n_rank; ++k) {
       if (!rank_written(a, k, mask)) continue;
       unsigned char txt[28];
-      len += (a.rank_name_off[k + 1] - a.rank_name_off[k]) + 4 + java_double_text(a.score[(size_t)k * a.n_groups + x.g], txt);
+      len += (a.rank_name_off[k + 1] - a.rank_name_off[k]) + 4 + java_double_text(a.score[(size_t)k * a.n_groups + x.g], a.rank_scale[k], txt);
     }
     doc_len[d] = len;
   }
@@ -275,7 +290,7 @@ __global__ void k_doc_write(const FormatArgs a, int32_t n_docs, const long long 
       if (!rank_written(a, k, mask)) continue;
       const int nl = a.rank_name_off[k + 1] - a.rank_name_off[k];
       unsigned char txt[28];
-      const int tl = java_double_text(a.score[(size_t)k * a.n_groups + x.g], txt);
+      const int tl = java_double_text(a.score[(size_t)k * a.n_groups + x.g], a.rank_scale[k], txt);
       warp_lit(w, ",\"", 2, lane); w += 2;
       warp_copy(w, a.names + a.rank_name_off[k], nl, lane); w += nl;
       warp_lit(w, "\":", 2, lane); w += 2;
@@ -390,6 +405,25 @@ __global__ void k_pop_score(const PopArgs a, int mode, const int32_t *__restrict
     }
     score[j] = ok ? (Score)v : (Score)0;
     present[j] = ok ? 1 : 0;
+  }
+}
+
+// ---- random (uniqueRank, PopModel.calcRandom, PopModel.scala:98-110), cco_format_model only --------------------------
+// Items: the targets of every event in [start, end) -- the ranking's streams are every event name's -- plus every item with
+// a property triple.  Value: n · 10^-15, uniform in [0, 1), from the id and the window only (the reference's unseeded
+// Random.nextDouble cannot be reproduced; these values are):
+//   h = k_str_hash of the id (mask ~0),  r = mix64(h ^ mix64(start ^ mix64(end))),  n = floor(r · 10^15 / 2^64).
+// counts = the popular histogram of the window; the group's hash is the hash of its first id in the key column.
+__global__ void k_random_score(long long n_groups, const int32_t *__restrict__ counts, const int32_t *__restrict__ pbeg,
+                               const int32_t *__restrict__ pend, const uint32_t *__restrict__ first_sorted,
+                               const uint64_t *__restrict__ hash, long long start_ms, long long end_ms, long long *__restrict__ score,
+                               unsigned char *__restrict__ present) {
+  const uint64_t window = mix64((uint64_t)start_ms ^ mix64((uint64_t)end_ms));
+  for (long long g = blockIdx.x * (long long)blockDim.x + threadIdx.x; g < n_groups; g += (long long)gridDim.x * blockDim.x) {
+    const bool ok = counts[g] > 0 || (pbeg && pend[g] > pbeg[g]);
+    const uint64_t r = mix64(hash[first_sorted[g]] ^ window);
+    score[g] = ok ? (long long)__umul64hi(r, 1000000000000000ULL) : 0;
+    present[g] = ok ? 1 : 0;
   }
 }
 

@@ -232,8 +232,10 @@ class CcoContext:
         document for every item without a row that has a property or a score (URAlgorithm.scala:351-367, URModel.scala:57-102).
         properties = (field_names, item_offsets int64[n + 1], item_bytes uint8[], field int32[n], value_offsets int64[n + 1],
         value_bytes uint8[]): n (item, field, JSON text) triples, the last of a repeated (item, field) wins.
-        rankings = [(field name, "popular" | "trending" | "hot", start_ms, end_ms, [(item_offsets, item_bytes, time_ms int64[])
-        per event name])].  Id columns in the layout of encode_ids."""
+        rankings = [(field name, "popular" | "trending" | "hot" | "random", start_ms, end_ms, [(item_offsets, item_bytes,
+        time_ms int64[]) per event name])].  A "random" ranking (uniqueRank) scores the items of its streams' events in
+        [start_ms, end_ms) plus every property item with n · 10^-15, n a hash of the id and the window (ur_model.random_rank);
+        give it every event name's stream, as calcRandom reads them all.  Id columns in the layout of encode_ids."""
         keep = []
         n, nm, rd, cds = self._format_args(names, row_ids, col_ids, keep)
         p64, p32 = C.POINTER(C.c_int64), C.POINTER(C.c_int32)

@@ -105,9 +105,11 @@ def calc_all_on_device(events: Sequence[tuple[str, str, str, int]], set_events: 
     """URAlgorithm.calcAll (URAlgorithm.scala:310-369) through URModel.save's documents, on the GPU: string events in, the
     Elasticsearch bulk body out.  events = (user id, event name, item id, time ms); set_events = (item id, {field: value}) of
     the items' `$set` events in event-time order.  Steps: cco_ingest_strings (Preparator) -> cco_train_dataset -> the
-    rankings' PopModel histograms and the property join -> cco_format_model.  "collabFiltering" writes the correlators only
-    (propertiesRDD is empty there); "backfill" (calcPop, which reads the live index) is not supported.
-    now_ms: the rankings' end when a ranking has no offsetDate (default: the wall clock)."""
+    rankings' PopModel histograms (popular, trending, hot, and random over every event name) and the property join ->
+    cco_format_model.  "collabFiltering" writes the correlators only (propertiesRDD is empty there); "backfill" (calcPop,
+    which reads the live index) is not supported.
+    now_ms: the rankings' end when a ranking has no offsetDate (default: the wall clock).  A random ranking's values are a
+    hash of the item id and the window (ur_model.random_rank): they change with now_ms and repeat for a fixed window."""
     _check_recs_model(ap)
     if ap.recsModel == "backfill":
         raise ValueError("recsModel=backfill runs calcPop against the live index; it has no train half to run here")

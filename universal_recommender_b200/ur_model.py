@@ -6,6 +6,11 @@ strings with CcoContext.format_model.
 Precedence inside a document, lowest to highest (Scala `++` and `+`: the later source wins):
   correlator fields < properties (fieldsPropMap ++ rankPropMap) < ranks (a later ranking beats an earlier one of the same
   name, getRanksRDD's foldLeft) < "id" (propsMap + ("id" -> itemId)).
+
+Random rankings (uniqueRank, PopModel.calcRandom): every item of an event in the window, of any event name, plus every item
+with a property, valued n · 10^-15 with n a hash of the id bytes and the window (random_rank) instead of the reference's
+unseeded Random.nextDouble.  The values change with the window, so with "now" as its end from train to train, as the
+reference's do; unlike the reference's, they repeat when a fixed offsetDate repeats the window.
 """
 from __future__ import annotations
 
@@ -103,6 +108,35 @@ def ranking_window(rp: RankingParams, now_ms: int) -> tuple[int, int]:
     return end - duration_seconds(rp.duration if rp.duration is not None else BACKFILL_DURATION) * 1000, end
 
 
+_M64 = (1 << 64) - 1
+
+
+def _mix64(z: int) -> int:
+    """mix64 of cco_kernels.cuh on one Python int (synth._mix64 is the numpy form)"""
+    z ^= z >> 30
+    z = (z * 0xBF58476D1CE4E5B9) & _M64
+    z ^= z >> 27
+    z = (z * 0x94D049BB133111EB) & _M64
+    return z ^ (z >> 31)
+
+
+def id_hash(item: str) -> int:
+    """the 64-bit hash k_str_hash (cco_strings.cuh, mask ~0) gives an id: mix64 over its UTF-8 bytes as little-endian 8-byte
+    words, the last one zero-padded, then over the length"""
+    b = item.encode("utf-8")
+    h = 0x243F6A8885A308D3
+    for k in range(0, len(b), 8):
+        h = (_mix64(h ^ int.from_bytes(b[k:k + 8], "little")) + 0x9E3779B97F4A7C15) & _M64
+    return _mix64(h ^ len(b))
+
+
+def random_rank(item: str, start_ms: int, end_ms: int) -> int:
+    """n of an item's random rank n · 10^-15 (0 <= n < 10^15) over the window [start_ms, end_ms):
+    r = mix64(id_hash ^ mix64(start ^ mix64(end))) as uint64, n = floor(r · 10^15 / 2^64)"""
+    window = _mix64((start_ms & _M64) ^ _mix64(end_ms & _M64))
+    return (_mix64(id_hash(item) ^ window) * 10**15) >> 64
+
+
 def pop_scores(mode: str, items: Sequence[str], times_ms: Sequence[int], start_ms: int, end_ms: int) -> dict:
     """PopModel.calcPopular / calcTrending / calcHot (PopModel.scala:113-182) per item id: {item: score} for the items the
     reference's RDD holds.  Same rules as cco_pop_model, including the empty-bucket ones."""
@@ -138,26 +172,32 @@ class Ranking:
     end_ms: int
     streams: list   # [(item ids list[str], times list[int])] one per event name
 
-    def scores(self) -> dict:
+    def scores(self, property_items: Iterable[str] = ()) -> dict:
+        """{item: score}; a random ranking also scores the items that have a property"""
         items = [i for s in self.streams for i in s[0]]
         times = [t for s in self.streams for t in s[1]]
+        if self.mode == RankingType.Random:
+            keep = [i for i, t in zip(items, times) if self.start_ms <= t < self.end_ms] + list(property_items)
+            return {i: random_rank(i, self.start_ms, self.end_ms) / 1e15 for i in dict.fromkeys(keep)}
         return pop_scores(self.mode, items, times, self.start_ms, self.end_ms)
 
 
 def rankings_for(params: Sequence[RankingParams], events_by_name: dict, now_ms: int, model_event_names: Sequence[str]) -> list[Ranking]:
-    """getRanksRDD (URAlgorithm.scala:537-560): one Ranking per histogram ranking.  A ranking reads the event store (every
-    user's events of its event names, {name: [(item, time ms)]}), not the Preparator output; without eventNames it reads the
-    first model event name.  userDefined rankings produce nothing (PopModel returns an
-    empty RDD; the field comes from the item's own properties); random (uniqueRank) is not reproducible and is refused."""
+    """getRanksRDD (URAlgorithm.scala:537-560): one Ranking per histogram or random ranking.  A ranking reads the event store
+    (every user's events of its event names, {name: [(item, time ms)]}), not the Preparator output; without eventNames it
+    reads the first model event name.  A random ranking reads every event name, in the order of events_by_name, and ignores
+    its eventNames (calcRandom, PopModel.scala:98-110).  userDefined rankings produce nothing (PopModel returns an empty RDD;
+    the field comes from the item's own properties)."""
     out = []
     for rp in params:
         t = rp.ranking_type()
-        if t == RankingType.Random:
-            raise ValueError("random rankings (uniqueRank) are not supported: pass such a rank as an item property")
-        if t not in (RankingType.Popular, RankingType.Trending, RankingType.Hot):
+        if t not in (RankingType.Popular, RankingType.Trending, RankingType.Hot, RankingType.Random):
             continue   # userDefined, or an unknown type the reference warns about and skips
         start, end = ranking_window(rp, now_ms)
-        names = rp.eventNames if rp.eventNames is not None else list(model_event_names[:1])
+        if t == RankingType.Random:
+            names = list(events_by_name)
+        else:
+            names = rp.eventNames if rp.eventNames is not None else list(model_event_names[:1])
         streams = [([i for i, _ in events_by_name.get(n, [])], [tm for _, tm in events_by_name.get(n, [])]) for n in names]
         out.append(Ranking(rp.field_name(), t, start, end, streams or [([], [])]))
     return out
@@ -243,12 +283,12 @@ def model_documents(row_ids: Sequence[str], indicators: Sequence[tuple[str, Sequ
                     properties: Sequence[tuple[str, str, object]], rankings: Sequence[Ranking]) -> list[dict]:
     """URModel.save's groupAll / getRanksRDD's fullOuterJoin as one dict per item, in the documents' order: the rows first
     (row order), then the items without a row that have a property or a score, by first appearance (property triples, then
-    the ranking streams in order).  indicators = [(event name, correlator ids per row)]; properties = (item, field, value)
-    triples, the last of a repeated (item, field) wins."""
+    the ranking streams in order).  A random ranking scores the property items too.  indicators = [(event name, correlator
+    ids per row)]; properties = (item, field, value) triples, the last of a repeated (item, field) wins."""
     props: dict = {}
     for item, f, v in properties:
         props.setdefault(item, {})[f] = v
-    scored = [(r.field, r.scores()) for r in rankings]
+    scored = [(r.field, r.scores([i for i, _, _ in properties])) for r in rankings]
     rows = set(row_ids)
     order = list(row_ids)
     seen = set()
