@@ -388,6 +388,37 @@ int cco_format_model(cco_ctx_t *ctx, const cco_result_t *res, int32_t n_names, c
                      int32_t n_rankings, const cco_ranking_t *rankings, char **out_bytes, int64_t *out_len);
 
 /*
+ * The rankings of an existing model index refreshed (calcPop, URAlgorithm.scala:375-399, recsModel "backfill"): the caller
+ * reads the index and passes it as a bulk body such as cco_format_model writes; the body is parsed on the device and every
+ * document gets the fresh rankings and properties, joined by item id the way cco_format_model joins them.  The rankings
+ * and properties are those of cco_format_model, with its host and device checks; a random ranking covers the items of its
+ * events and the property items, not the items found only in the old index.
+ * Accepted body: lines ending in '\n' (an empty body has no documents), in (action, source) pairs.  The action is a JSON
+ * object with exactly one member, "index", whose value is an object with a string member "_id" (the last "_id" if it
+ * repeats; other members such as "_index" are ignored).  The source is a JSON object.  JSON whitespace, '\r' included, may
+ * stand between tokens.  Strings must be closed and hold valid escapes and no raw byte < 0x20; scalars and the inside of
+ * values are not validated further.  Names are compared decoded (\uXXXX, surrogate pairs, \/ ...); names and values of the
+ * old documents are spliced verbatim.
+ * Precedence per document, lowest to highest: fresh properties < members of the old document < rankings (a later ranking
+ * beats an earlier one of the same name) < "id".  So a fresh property loses to an old member of the same name, and an old
+ * rank member survives when the item has no score in that ranking.  Where a member name repeats, the last one wins.
+ * Documents: the old ones in body order, then the items without an old document that have a property or a score, in order
+ * of first appearance (property items first, then the ranking streams in order), written as cco_format_model writes them.
+ * Fields of an old document: "id" (the decoded _id, escaped as every id), the old members in their order except "id", those
+ * named like a ranking present for the item and those followed by a member of the same name, then the properties in field
+ * index order except those named "id", like an old member or like a present ranking, then the rankings in order.
+ *     {"index":{"_id":"<id>"}}\n{"id":"<id>"[,<old member>]*[,"<field>":<value>]*[,"<ranking>":<number>]*}\n
+ * Errors: CCO_E_INVALID_ARG for an odd number of lines, a missing final newline, unbalanced brackets, an unterminated string,
+ * a bad escape, an action that is not "index" or has no string "_id", a source that is not an object, an _id in two
+ * documents (the message names the 0-based document; decided before anything reads through the parsed spans) and the input
+ * errors of cco_format_model; CCO_E_UNSUPPORTED for a line of 2^31 or more bytes, 2^31 - 1 or more members in the body,
+ * documents + property triples + ranking events >= 2^31, and group contexts.  out_bytes: pinned memory owned by the context,
+ * released with cco_host_free.
+ */
+int cco_rerank_model(cco_ctx_t *ctx, const char *body, int64_t body_len, const cco_item_properties_t *props /* nullable */,
+                     int32_t n_rankings, const cco_ranking_t *rankings, char **out_bytes, int64_t *out_len);
+
+/*
  * Debug/parity entry (tests only): full integer co-occurrence matrix A^T B of two canonical
  * binary matrices computed by the same accumulation kernel as cco_train, no LLR, no top-k.
  * Output CSR over the columns of A with ascending column ids, malloc'ed; free with cco_free.

@@ -12,7 +12,10 @@ Prints one JSON line:
   - gpu name and power limit, read in the same run
   - with --random: model_random_ms_median / model_random_bytes, the same call with a third ranking, uniqueRank (random) over
     every event stream, timed after the call without it; the parity sample then holds the random ranking too
-usage: python tools/model_format_bench.py --config C3 --steps 5 --warmup 1 --sample 200000 [--random]
+  - with --rerank: cco_rerank_model (calcPop) on the body format_model wrote, with the same properties and rankings,
+    alternated step by step with format_model on the same inputs: rerank_ms_median / format_alt_ms_median, the body MB in
+    and out, the H2D bytes of the call, and rerank_fixed_point (the rerank of the body equals the body)
+usage: python tools/model_format_bench.py --config C3 --steps 5 --warmup 1 --sample 200000 [--random] [--rerank]
 """
 from __future__ import annotations
 
@@ -49,6 +52,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=1)
     ap.add_argument("--sample", type=int, default=200_000, help="events per stream for the host mirror and the parity check")
     ap.add_argument("--random", action="store_true", help="also time format_model with a random (uniqueRank) ranking added")
+    ap.add_argument("--rerank", action="store_true", help="also time rerank_model on the model body, alternated with format_model")
     a = ap.parse_args()
     cfg = synth.CONFIGS[a.config]
     n_types, n_users, n_items = cfg["n_types"], cfg["n_users"], cfg["n_items"]
@@ -104,6 +108,23 @@ def main():
         extra = {"model_random_ms_median": round(float(np.median(random_ms)), 2), "model_random_ms_all": [round(x, 2) for x in random_ms],
                  "model_random_bytes": len(body_r)}
         del body_r
+    if a.rerank:
+        fmt_ms, rr_ms, out = [], [], None
+        for step in range(a.warmup + a.steps):
+            t0 = time.perf_counter()
+            ctx.format_model(h, names, ids, cols, props, rankings)
+            t1 = time.perf_counter()
+            out = ctx.rerank_model(body, props, rankings)
+            t2 = time.perf_counter()
+            if step >= a.warmup:
+                fmt_ms.append((t1 - t0) * 1e3)
+                rr_ms.append((t2 - t1) * 1e3)
+        extra.update({"rerank_ms_median": round(float(np.median(rr_ms)), 2), "rerank_ms_all": [round(x, 2) for x in rr_ms],
+                      "format_alt_ms_median": round(float(np.median(fmt_ms)), 2), "format_alt_ms_all": [round(x, 2) for x in fmt_ms],
+                      "rerank_mb_in": round(len(body) / 1e6, 2), "rerank_mb_out": round(len(out) / 1e6, 2),
+                      "rerank_h2d_bytes": int(len(body) + model_h2d),
+                      "rerank_fixed_point": out == body})
+        del out
 
     # host mirror and parity on a sample of every stream
     S = min(a.sample, per_type)

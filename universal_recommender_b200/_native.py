@@ -100,7 +100,7 @@ EXPORTS = [
     "cco_dataset_upload", "cco_train_dataset", "cco_dataset_free", "cco_timer_start", "cco_timer_stop",
     "cco_partition_rows", "cco_ingest", "cco_synth_ingest", "cco_dataset_shape", "cco_dataset_download",
     "cco_dataset_copy_to_host", "cco_format_es_bulk", "cco_ingest_strings", "cco_dataset_dictionary", "cco_pop_model",
-    "cco_format_model",
+    "cco_format_model", "cco_rerank_model",
     "cco_result_num_matrices", "cco_result_row_range", "cco_result_matrix", "cco_result_stats", "cco_result_free",
     "cco_debug_cooccurrence", "cco_debug_downsample", "cco_debug_llr", "cco_debug_string_ids", "cco_free",
 ]
@@ -147,6 +147,8 @@ def lib():
                                 p(C.c_ubyte)]
     L.cco_format_model.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, p(C.c_char_p), p(DictionaryT), p(DictionaryT), p(ItemPropertiesT),
                                    C.c_int32, p(RankingT), p(C.c_void_p), p(C.c_int64)]
+    L.cco_rerank_model.argtypes = [C.c_void_p, C.c_char_p, C.c_int64, p(ItemPropertiesT), C.c_int32, p(RankingT), p(C.c_void_p),
+                                   p(C.c_int64)]
     L.cco_dataset_shape.argtypes = [C.c_void_p, C.c_int32, p(C.c_int64), p(C.c_int32), p(C.c_int64)]
     L.cco_dataset_download.argtypes = [C.c_void_p, C.c_int32, p(p(C.c_int64)), p(p(C.c_int32))]
     L.cco_timer_start.argtypes = [C.c_void_p]

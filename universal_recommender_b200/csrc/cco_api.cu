@@ -26,6 +26,7 @@
 #include "cco_sampler.cuh"
 #include "cco_format.cuh"
 #include "cco_strings.cuh"
+#include "cco_json.cuh"
 
 namespace cco {
 
@@ -2604,22 +2605,27 @@ static PopArgs pop_args(int mode, long long start_ms, long long end_ms, int32_t 
   return a;
 }
 
-// one section of the combined key column: the row dictionary, the property items or one ranking stream
+// one section of the combined key column: the row dictionary, the property items or one ranking stream.  A device
+// section (the decoded ids of an old index, cco_rerank_model) is already in HBM: offsets from 0, nbytes bytes.
 struct KeySection {
   long long n;
   const int64_t *off;
   const char *bytes;
+  bool device = false;
+  long long nbytes = 0;
+  long long byte_count() const { return n == 0 ? 0 : device ? nbytes : off[n] - off[0]; }
 };
 
-// The model part of FormatArgs (cco_format_model): group the item ids of every source, score the rankings per group,
-// sort the properties, and list the documents of items without a row.  The caller's columns have passed str_check_host.
-static int model_fields(cco_ctx *c, Arena &ar, FormatArgs *fa, const cco_dictionary_t &row_ids, const cco_item_properties_t *props,
-                        int32_t n_rank, const cco_ranking_t *rk, bool extra_docs) {
+// The model part of FormatArgs (cco_format_model, cco_rerank_model): group the item ids of every source, score the
+// rankings per group, sort the properties, and list the documents of items without a row.  The caller's host columns have
+// passed str_check_host.  unique_rows: two rows with the same id are CCO_E_INVALID_ARG (the documents of an old index).
+static int model_fields(cco_ctx *c, Arena &ar, FormatArgs *fa, const KeySection &rows, const cco_item_properties_t *props,
+                        int32_t n_rank, const cco_ranking_t *rk, bool extra_docs, bool unique_rows = false) {
   cudaStream_t s = c->stream;
   mail_reset(c);
-  const long long R = row_ids.n, P = props ? props->n : 0;
+  const long long R = rows.n, P = props ? props->n : 0;
   std::vector<KeySection> sec;
-  sec.push_back({R, row_ids.offsets, row_ids.bytes});
+  sec.push_back(rows);
   sec.push_back({P, P > 0 ? props->item_offsets : nullptr, P > 0 ? props->item_bytes : nullptr});
   std::vector<long long> rank_begin(n_rank + 1);   // ranking k's events are key entries R + P + [rank_begin[k], rank_begin[k + 1])
   long long E = 0;
@@ -2634,7 +2640,7 @@ static int model_fields(cco_ctx *c, Arena &ar, FormatArgs *fa, const cco_diction
   rank_begin[n_rank] = E;
   const long long N = R + P + E;
   long long nb = 0;
-  for (const KeySection &k : sec) nb += k.n > 0 ? k.off[k.n] - k.off[0] : 0;
+  for (const KeySection &k : sec) nb += k.byte_count();
   DevStrCol key;
   key.n = N;
   key.base = 0;
@@ -2653,7 +2659,15 @@ static int model_fields(cco_ctx *c, Arena &ar, FormatArgs *fa, const cco_diction
   long long at = 0, byte_at = 0;
   for (const KeySection &k : sec) {
     if (k.n == 0) continue;
-    const long long kb = k.off[k.n] - k.off[0];
+    const long long kb = k.byte_count();
+    if (k.device) {
+      k_rebase<<<grid_for(k.n + 1, 256, c->sm_count), 256, 0, s>>>(k.n + 1, (const long long *)k.off, byte_at, key.off + at);
+      c->launches++;
+      if (kb > 0) CK(cudaMemcpyAsync((char *)key.w + byte_at, k.bytes, (size_t)kb, cudaMemcpyDeviceToDevice, s));
+      at += k.n;
+      byte_at += kb;
+      continue;
+    }
     CK(cudaMemcpyAsync(tmp_off, k.off, sizeof(int64_t) * ((size_t)k.n + 1), cudaMemcpyHostToDevice, s));
     k_str_check<<<grid_for(k.n, 256, c->sm_count), 256, 0, s>>>(k.n, tmp_off, bad);
     k_rebase<<<grid_for(k.n + 1, 256, c->sm_count), 256, 0, s>>>(k.n + 1, tmp_off, byte_at - k.off[0], key.off + at);
@@ -2708,6 +2722,17 @@ static int model_fields(cco_ctx *c, Arena &ar, FormatArgs *fa, const cco_diction
   StrTable tb;
   CKR(str_group(c, ar, key, nullptr, false, 0, &tb, gid));
   const long long G = tb.n_groups;
+  if (unique_rows && R > 0) {
+    unsigned long long *dup, h_dup = ~0ULL;
+    CKR(ar.alloc(&dup, 1));
+    CK(cudaMemsetAsync(dup, 0xff, 8, s));
+    k_dup_rows<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, gid, tb.first_sorted, dup);
+    c->launches++;
+    CKR(mail_fetch(c, &h_dup, dup, 8));
+    CKR(mail_wait(c));
+    if (h_dup != ~0ULL)
+      return set_error(CCO_E_INVALID_ARG, "document %llu: its _id is the _id of document %llu", h_dup >> 32, h_dup & 0xffffffffULL);
+  }
   fa->n_groups = G;
   fa->row_group = gid + fa->row_id_base;
   // 2. properties: sorted by (group, field), stable in the triple index, so the last triple of each run wins
@@ -2861,41 +2886,12 @@ static int model_check_host(const cco_dictionary_t *row_ids, const cco_item_prop
   return CCO_OK;
 }
 
-// cco_format_es_bulk == format_model without properties and rankings: one set of document kernels
-static int format_model(cco_ctx_t *ctx, const cco_result_t *res, int32_t n_names, const char *const *names, const cco_dictionary_t *row_ids,
-                        const cco_dictionary_t *col_ids, const cco_item_properties_t *props, int32_t n_rank, const cco_ranking_t *rk,
-                        char **out_bytes, int64_t *out_len, const char *range) {
-  if (!ctx || !res || !names || !row_ids || !col_ids || !out_bytes || !out_len) return set_error(CCO_E_INVALID_ARG, "null argument");
-  const int n_ind = (int)res->mats.size();
-  if (n_names != n_ind) return set_error(CCO_E_INVALID_ARG, "%d event names for %d indicators", n_names, n_ind);
-  if (n_ind < 1 || n_ind > kMaxFormatIndicators) return set_error(CCO_E_UNSUPPORTED, "1..%d indicators", kMaxFormatIndicators);
-  cco_ctx *c = ctx->members.empty() ? ctx : ctx->members[0];   // a group's merged model is formatted on its first GPU
-  const int64_t row_lo = res->mats[0].row_begin, row_hi = res->mats[0].row_end;
-  for (int i = 0; i < n_ind; ++i) {
-    const ResultMat &m = res->mats[i];
-    if (m.row_begin != row_lo || m.row_end != row_hi) return set_error(CCO_E_INVALID_ARG, "indicators cover different row ranges");
-    if (!m.row_ptr || (m.row_ptr[row_hi - row_lo] > 0 && !m.col)) return set_error(CCO_E_INVALID_ARG, "indicator %d has no column array on the host", i);
-    if (col_ids[i].n < m.n_cols) return set_error(CCO_E_INVALID_ARG, "column dictionary %d has %lld ids for %d columns", i, (long long)col_ids[i].n, m.n_cols);
-    if (!names[i]) return set_error(CCO_E_INVALID_ARG, "null event name");
-  }
-  if (row_ids->n < row_hi) return set_error(CCO_E_INVALID_ARG, "row dictionary has %lld ids, rows go up to %lld", (long long)row_ids->n, (long long)row_hi);
-  const bool model = (props && props->n > 0) || n_rank > 0;
-  if (model) CKR(model_check_host(row_ids, props, n_rank, rk));
-  const int n_fields = props ? props->n_fields : 0;
-  CK(cudaSetDevice(c->device));
+// The names of FormatArgs: event names, field names and ranking names escaped as one more tiny dictionary, and (model) who
+// beats whom where names repeat.
+static int model_names(cco_ctx *c, Arena &ar, FormatArgs *fa, int n_ind, const char *const *names, bool model,
+                       const cco_item_properties_t *props, int32_t n_rank, const cco_ranking_t *rk) {
   cudaStream_t s = c->stream;
-  Arena ar(s);
-  nvtx_push(range);
-  struct Pop { ~Pop() { nvtx_pop(); } } pop;
-  FormatArgs fa;
-  memset(&fa, 0, sizeof fa);
-  fa.n_rows = (int32_t)(row_hi - row_lo);
-  fa.row_id_base = row_lo;
-  fa.n_ind = n_ind;
-  DevDict raw;
-  CKR(upload_dict(c, ar, *row_ids, &raw));
-  CKR(escape_dict(c, ar, raw, &fa.row_ids));
-  // event names, field names and ranking names as one more tiny dictionary
+  const int n_fields = props ? props->n_fields : 0;
   std::vector<const char *> all_names(names, names + n_ind);
   if (model) {
     for (int f = 0; f < n_fields; ++f) all_names.push_back(props->field_names[f]);
@@ -2917,11 +2913,11 @@ static int format_model(cco_ctx_t *ctx, const cco_result_t *res, int32_t n_names
     CKR(escape_dict(c, ar, nraw, &nesc));
     CK(cudaMemcpyAsync(eoff.data(), nesc.off, sizeof(long long) * ((size_t)n_all + 1), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
-    fa.names = nesc.bytes;
-    for (int i = 0; i <= n_ind; ++i) fa.name_off[i] = (int32_t)eoff[i];
+    fa->names = nesc.bytes;
+    for (int i = 0; i <= n_ind; ++i) fa->name_off[i] = (int32_t)eoff[i];
     if (model) {
-      fa.field_off = nesc.off + n_ind;
-      for (int k = 0; k <= n_rank; ++k) fa.rank_name_off[k] = (int32_t)eoff[n_ind + n_fields + k];
+      fa->field_off = nesc.off + n_ind;
+      for (int k = 0; k <= n_rank; ++k) fa->rank_name_off[k] = (int32_t)eoff[n_ind + n_fields + k];
     }
   }
   if (model) {
@@ -2935,24 +2931,61 @@ static int format_model(cco_ctx_t *ctx, const cco_result_t *res, int32_t n_names
         if (same(props->field_names[f], rk[k].name)) fclash[f] |= (uint16_t)(1u << k);
     }
     for (int i = 0; i < n_ind; ++i) {
-      fa.ind_field[i] = -1;
+      fa->ind_field[i] = -1;
       for (int f = 0; f < n_fields; ++f)
-        if (same(names[i], props->field_names[f])) fa.ind_field[i] = f;
+        if (same(names[i], props->field_names[f])) fa->ind_field[i] = f;
       for (int k = 0; k < n_rank; ++k)
-        if (same(names[i], rk[k].name)) fa.ind_rank[i] |= (uint8_t)(1u << k);
+        if (same(names[i], rk[k].name)) fa->ind_rank[i] |= (uint8_t)(1u << k);
     }
     for (int k = 0; k < n_rank; ++k) {
-      if (same(rk[k].name, "id")) fa.rank_clash[k] |= kClashId;
+      if (same(rk[k].name, "id")) fa->rank_clash[k] |= kClashId;
       for (int l = k + 1; l < n_rank; ++l)
-        if (same(rk[k].name, rk[l].name)) fa.rank_clash[k] |= (uint16_t)(1u << l);
+        if (same(rk[k].name, rk[l].name)) fa->rank_clash[k] |= (uint16_t)(1u << l);
     }
     uint16_t *d_fclash;
     CKR(ar.alloc(&d_fclash, fclash.size()));
     CK(cudaMemcpyAsync(d_fclash, fclash.data(), sizeof(uint16_t) * fclash.size(), cudaMemcpyHostToDevice, s));
-    fa.field_clash = d_fclash;
-    CKR(model_fields(c, ar, &fa, *row_ids, props, n_rank, rk, row_lo == 0));
+    fa->field_clash = d_fclash;
     CK(cudaStreamSynchronize(s));   // fclash is a local
   }
+  return CCO_OK;
+}
+
+// cco_format_es_bulk == format_model without properties and rankings: one set of document kernels
+static int format_model(cco_ctx_t *ctx, const cco_result_t *res, int32_t n_names, const char *const *names, const cco_dictionary_t *row_ids,
+                        const cco_dictionary_t *col_ids, const cco_item_properties_t *props, int32_t n_rank, const cco_ranking_t *rk,
+                        char **out_bytes, int64_t *out_len, const char *range) {
+  if (!ctx || !res || !names || !row_ids || !col_ids || !out_bytes || !out_len) return set_error(CCO_E_INVALID_ARG, "null argument");
+  const int n_ind = (int)res->mats.size();
+  if (n_names != n_ind) return set_error(CCO_E_INVALID_ARG, "%d event names for %d indicators", n_names, n_ind);
+  if (n_ind < 1 || n_ind > kMaxFormatIndicators) return set_error(CCO_E_UNSUPPORTED, "1..%d indicators", kMaxFormatIndicators);
+  cco_ctx *c = ctx->members.empty() ? ctx : ctx->members[0];   // a group's merged model is formatted on its first GPU
+  const int64_t row_lo = res->mats[0].row_begin, row_hi = res->mats[0].row_end;
+  for (int i = 0; i < n_ind; ++i) {
+    const ResultMat &m = res->mats[i];
+    if (m.row_begin != row_lo || m.row_end != row_hi) return set_error(CCO_E_INVALID_ARG, "indicators cover different row ranges");
+    if (!m.row_ptr || (m.row_ptr[row_hi - row_lo] > 0 && !m.col)) return set_error(CCO_E_INVALID_ARG, "indicator %d has no column array on the host", i);
+    if (col_ids[i].n < m.n_cols) return set_error(CCO_E_INVALID_ARG, "column dictionary %d has %lld ids for %d columns", i, (long long)col_ids[i].n, m.n_cols);
+    if (!names[i]) return set_error(CCO_E_INVALID_ARG, "null event name");
+  }
+  if (row_ids->n < row_hi) return set_error(CCO_E_INVALID_ARG, "row dictionary has %lld ids, rows go up to %lld", (long long)row_ids->n, (long long)row_hi);
+  const bool model = (props && props->n > 0) || n_rank > 0;
+  if (model) CKR(model_check_host(row_ids, props, n_rank, rk));
+  CK(cudaSetDevice(c->device));
+  cudaStream_t s = c->stream;
+  Arena ar(s);
+  nvtx_push(range);
+  struct Pop { ~Pop() { nvtx_pop(); } } pop;
+  FormatArgs fa;
+  memset(&fa, 0, sizeof fa);
+  fa.n_rows = (int32_t)(row_hi - row_lo);
+  fa.row_id_base = row_lo;
+  fa.n_ind = n_ind;
+  DevDict raw;
+  CKR(upload_dict(c, ar, *row_ids, &raw));
+  CKR(escape_dict(c, ar, raw, &fa.row_ids));
+  CKR(model_names(c, ar, &fa, n_ind, names, model, props, n_rank, rk));
+  if (model) CKR(model_fields(c, ar, &fa, KeySection{row_ids->n, row_ids->offsets, row_ids->bytes}, props, n_rank, rk, row_lo == 0));
   for (int i = 0; i < n_ind; ++i) {
     const ResultMat &m = res->mats[i];
     CKR(upload_dict(c, ar, col_ids[i], &raw));
@@ -2999,7 +3032,285 @@ static int format_model(cco_ctx_t *ctx, const cco_result_t *res, int32_t n_names
   *out_len = total;
   return CCO_OK;
 }
+
+// ---- cco_rerank_model: an existing index with fresh rankings and properties (calcPop), kernels in cco_json.cuh ---------
+// the message of a tokenizer / action verdict: span = err >> 8 is a line (lines) or a document
+static int json_error(unsigned long long err, bool lines) {
+  const long long span = (long long)(err >> 8), doc = lines ? span / 2 : span;
+  const int code = (int)(err & 0xff);
+  const char *part = lines && (span & 1) ? "source" : "action";
+  if (code == kJsonLongLine) return set_error(CCO_E_UNSUPPORTED, "document %lld: the %s line is longer than 2^31 - 1 bytes", doc, part);
+  if (!lines || code == kJsonAction)
+    return set_error(CCO_E_INVALID_ARG, "document %lld: the action line is not {\"index\":{...}} with a string \"_id\" member", doc);
+  if (code == kJsonNotObject) return set_error(CCO_E_INVALID_ARG, "document %lld: the %s line is not a JSON object", doc, part);
+  if (code == kJsonString)
+    return set_error(CCO_E_INVALID_ARG, "document %lld: a string of the %s line is unterminated or holds a bad escape or a raw byte < 0x20",
+                     doc, part);
+  return set_error(CCO_E_INVALID_ARG, "document %lld: the %s line is not one JSON object (unbalanced brackets or an unexpected token)",
+                   doc, part);
+}
+// one tokenizer run over n object spans: count, verdict, write.  moff[s] = first member of span s, *total = all members
+static int json_members(cco_ctx *c, Arena &ar, long long n, const long long *sb, const long long *se, const unsigned char *body,
+                        bool lines, long long **moff_out, JMember **mem_out, long long *total_out) {
+  cudaStream_t s = c->stream;
+  long long *cnt, *moff;
+  unsigned long long *err;
+  CKR(ar.alloc(&cnt, n + 1));
+  CKR(ar.alloc(&moff, n + 1));
+  CKR(ar.alloc(&err, 1));
+  CK(cudaMemsetAsync(cnt + n, 0, 8, s));
+  CK(cudaMemsetAsync(err, 0xff, 8, s));
+  const int grid = grid_for(n * 32, 256, c->sm_count);
+  k_json_members<false><<<grid, 256, 0, s>>>(n, sb, se, body, cnt, nullptr, nullptr, err);
+  c->launches++;
+  CKR(exclusive_sum_i64(c, ar, cnt, moff, n + 1));
+  unsigned long long h_err = 0;
+  long long total = 0;
+  CKR(mail_fetch(c, &h_err, err, 8));
+  CKR(mail_fetch(c, &total, moff + n, 8));
+  CKR(mail_wait(c));
+  if (h_err != ~0ULL) return json_error(h_err, lines);
+  if (total >= 0x7fffffffLL) return set_error(CCO_E_UNSUPPORTED, "%lld members in the body, at most 2^31 - 2", total);
+  JMember *mem;
+  CKR(ar.alloc(&mem, std::max<long long>(total, 1)));
+  if (total > 0) {
+    k_json_members<true><<<grid, 256, 0, s>>>(n, sb, se, body, nullptr, moff, mem, err);
+    c->launches++;
+  }
+  ar.release(cnt);
+  *moff_out = moff;
+  *mem_out = mem;
+  *total_out = total;
+  return CCO_OK;
+}
+// the strings [m.nb, m.ne) of n members decoded into a string column (offsets from 0, 8-byte words, 16 bytes of padding)
+static int json_decode(cco_ctx *c, Arena &ar, long long n, const JMember *m, const unsigned char *body, DevStrCol *col, long long *bytes) {
+  cudaStream_t s = c->stream;
+  long long *len;
+  CKR(ar.alloc(&len, n + 1));
+  CKR(ar.alloc(&col->off, n + 1));
+  CKR(ar.alloc(&col->hash, std::max<long long>(n, 1)));
+  CK(cudaMemsetAsync(len + n, 0, 8, s));
+  const int grid = grid_for(n, 256, c->sm_count);
+  if (n > 0) k_json_unescape<false><<<grid, 256, 0, s>>>(n, m, body, len, nullptr, nullptr);
+  CKR(exclusive_sum_i64(c, ar, len, col->off, n + 1));
+  long long total = 0;
+  CKR(mail_fetch(c, &total, col->off + n, 8));
+  CKR(mail_wait(c));
+  CKR(ar.alloc(&col->w, (total + 16 + 7) / 8));
+  if (n > 0 && total > 0) k_json_unescape<true><<<grid, 256, 0, s>>>(n, m, body, nullptr, col->off, (unsigned char *)col->w);
+  c->launches += 2;
+  ar.release(len);
+  col->n = n;
+  col->base = 0;
+  *bytes = total;
+  return CCO_OK;
+}
+
+static int rerank_model(cco_ctx_t *ctx, const char *body, int64_t body_len, const cco_item_properties_t *props, int32_t n_rank,
+                        const cco_ranking_t *rk, char **out_bytes, int64_t *out_len) {
+  if (!ctx || !out_bytes || !out_len || body_len < 0 || (body_len > 0 && !body)) return set_error(CCO_E_INVALID_ARG, "null argument or negative length");
+  if (!ctx->members.empty()) return set_error(CCO_E_UNSUPPORTED, "per-GPU contexts only");
+  if (body_len > 0 && body[body_len - 1] != '\n') return set_error(CCO_E_INVALID_ARG, "the body does not end in a newline");
+  const cco_dictionary_t no_rows = {0, nullptr, nullptr};
+  CKR(model_check_host(&no_rows, props, n_rank, rk));
+  long long fresh = props ? props->n : 0;   // property triples + ranking events, checked < 2^31 by model_check_host
+  for (int k = 0; k < n_rank; ++k)
+    for (int q = 0; q < rk[k].n_streams; ++q) fresh += rk[k].streams[q].n_events;
+  cco_ctx *c = ctx;
+  CK(cudaSetDevice(c->device));
+  cudaStream_t s = c->stream;
+  Arena ar(s);
+  nvtx_push("cco:rerank_model");
+  struct Pop { ~Pop() { nvtx_pop(); } } pop;
+  mail_reset(c);
+  // 1. the body, once, into 8-byte words with 16 bytes of zero padding
+  const long long NW = (body_len + 7) / 8;
+  uint64_t *w;
+  CKR(ar.alloc(&w, NW + 2));
+  CK(cudaMemsetAsync(w + body_len / 8, 0, sizeof(uint64_t) * (size_t)(NW + 2 - body_len / 8), s));
+  if (body_len > 0) CK(cudaMemcpyAsync(w, body, (size_t)body_len, cudaMemcpyHostToDevice, s));
+  const unsigned char *bb = (const unsigned char *)w;
+  // 2. line bounds
+  long long L = 0;
+  long long *nl = nullptr;
+  if (NW > 0) {
+    const long long n_chunks = (NW + kNlChunkWords - 1) / kNlChunkWords;
+    long long *cc, *coff;
+    CKR(ar.alloc(&cc, n_chunks + 1));
+    CKR(ar.alloc(&coff, n_chunks + 1));
+    CK(cudaMemsetAsync(cc + n_chunks, 0, 8, s));
+    k_nl_count<<<grid_for(n_chunks * 32, 256, c->sm_count), 256, 0, s>>>(NW, w, cc);
+    c->launches++;
+    CKR(exclusive_sum_i64(c, ar, cc, coff, n_chunks + 1));
+    CKR(mail_fetch(c, &L, coff + n_chunks, 8));
+    CKR(mail_wait(c));
+    if (L & 1) return set_error(CCO_E_INVALID_ARG, "the body has %lld lines: lines come in (action, source) pairs", L);
+    CKR(ar.alloc(&nl, L));
+    k_nl_write<<<grid_for(n_chunks * 32, 256, c->sm_count), 256, 0, s>>>(NW, w, coff, nl);
+    c->launches++;
+  }
+  const long long D = L / 2;
+  if (D + fresh >= 0x7fffffffLL)
+    return set_error(CCO_E_UNSUPPORTED, "documents + property triples + ranking events must stay < 2^31 per call");
+  FormatArgs fa;
+  memset(&fa, 0, sizeof fa);
+  RerankArgs ra;
+  memset(&ra, 0, sizeof ra);
+  ra.body = bb;
+  DevStrCol ids, names;
+  long long ids_bytes = 0, M1 = 0;
+  if (D > 0) {
+    // 3. members of every line; the verdict on the whole body comes before anything reads through the spans
+    long long *sb, *se;
+    CKR(ar.alloc(&sb, L));
+    CKR(ar.alloc(&se, L));
+    k_line_spans<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, nl, sb, se);
+    c->launches++;
+    long long *line_moff;
+    JMember *mem;
+    CKR(json_members(c, ar, L, sb, se, bb, true, &line_moff, &mem, &M1));
+    // 4. member names decoded; each action is {"index":{...}} and its "_id" is a string
+    long long name_bytes = 0;
+    CKR(json_decode(c, ar, M1, mem, bb, &names, &name_bytes));
+    long long *ib, *ie;
+    unsigned long long *err, h_err = 0;
+    CKR(ar.alloc(&ib, D));
+    CKR(ar.alloc(&ie, D));
+    CKR(ar.alloc(&err, 1));
+    CK(cudaMemsetAsync(err, 0xff, 8, s));
+    k_action_check<<<grid_for(D, 256, c->sm_count), 256, 0, s>>>(D, line_moff, mem, names.off, (const unsigned char *)names.w, bb, ib, ie, err);
+    c->launches++;
+    CKR(mail_fetch(c, &h_err, err, 8));
+    CKR(mail_wait(c));
+    if (h_err != ~0ULL) return json_error(h_err, false);
+    long long *imoff, M2 = 0, iname_bytes = 0;
+    JMember *imem, *id_span;
+    CKR(json_members(c, ar, D, ib, ie, bb, false, &imoff, &imem, &M2));
+    DevStrCol inames;
+    CKR(json_decode(c, ar, M2, imem, bb, &inames, &iname_bytes));
+    CKR(ar.alloc(&id_span, D));
+    k_pick_id<<<grid_for(D, 256, c->sm_count), 256, 0, s>>>(D, imoff, imem, inames.off, (const unsigned char *)inames.w, bb, id_span, err);
+    c->launches++;
+    CKR(mail_fetch(c, &h_err, err, 8));
+    CKR(mail_wait(c));
+    if (h_err != ~0ULL) return json_error(h_err, false);
+    CKR(json_decode(c, ar, D, id_span, bb, &ids, &ids_bytes));
+    ra.line_moff = line_moff;
+    ra.mem = mem;
+  }
+  // 5. join: the decoded ids are the row section of the key column (a group with two of them is a repeated _id)
+  CKR(model_names(c, ar, &fa, 0, nullptr, true, props, n_rank, rk));
+  fa.n_rows = (int32_t)D;
+  const DevDict raw_ids = {ids.off, (const unsigned char *)ids.w, D};
+  CKR(escape_dict(c, ar, raw_ids, &fa.row_ids));
+  KeySection rows;
+  rows.n = D;
+  rows.off = (const int64_t *)ids.off;
+  rows.bytes = (const char *)ids.w;
+  rows.device = true;
+  rows.nbytes = ids_bytes;
+  CKR(model_fields(c, ar, &fa, rows, props, n_rank, rk, true, true));
+  // 6. member names -> the distinct names of the fields, the rankings and "id"
+  if (D > 0) {
+    std::vector<std::string> ent;
+    std::vector<int32_t> ent_field;
+    std::vector<uint8_t> ent_rank, ent_id;
+    auto entry = [&](const char *nm) {
+      for (size_t t = 0; t < ent.size(); ++t)
+        if (ent[t] == nm) return (int)t;
+      ent.push_back(nm);
+      ent_field.push_back(-1);
+      ent_rank.push_back(0);
+      ent_id.push_back(0);
+      return (int)ent.size() - 1;
+    };
+    for (int f = 0; props && f < props->n_fields; ++f) ent_field[entry(props->field_names[f])] = f;
+    for (int k = 0; k < n_rank; ++k) ent_rank[entry(rk[k].name)] |= (uint8_t)(1u << k);
+    ent_id[entry("id")] = 1;
+    const int T = (int)ent.size();
+    std::vector<int64_t> toff(T + 1, 0);
+    std::string tblob;
+    for (int t = 0; t < T; ++t) {
+      tblob += ent[t];
+      toff[t + 1] = (int64_t)tblob.size();
+    }
+    const cco_dictionary_t td = {T, toff.data(), tblob.data()};
+    DevDict traw;
+    int32_t *d_field;
+    uint8_t *d_rank, *d_id;
+    CKR(upload_dict(c, ar, td, &traw));
+    CKR(ar.alloc(&d_field, T));
+    CKR(ar.alloc(&d_rank, T));
+    CKR(ar.alloc(&d_id, T));
+    CK(cudaMemcpyAsync(d_field, ent_field.data(), sizeof(int32_t) * T, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(d_rank, ent_rank.data(), T, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(d_id, ent_id.data(), T, cudaMemcpyHostToDevice, s));
+    CK(cudaStreamSynchronize(s));   // the table is local
+    str_hash(c, names, ~0ULL);
+    int32_t *ngid, *entry_of, *ment;
+    uint8_t *mkeep;
+    CKR(ar.alloc(&ngid, std::max<long long>(M1, 1)));
+    StrTable nt;
+    CKR(str_group(c, ar, names, nullptr, false, 0, &nt, ngid));
+    CKR(ar.alloc(&entry_of, std::max<long long>(nt.n_groups, 1)));
+    CKR(ar.alloc(&ment, std::max<long long>(M1, 1)));
+    CKR(ar.alloc(&mkeep, std::max<long long>(M1, 1)));
+    if (nt.n_groups > 0)
+      k_name_entry<<<grid_for(nt.n_groups, 256, c->sm_count), 256, 0, s>>>(nt.n_groups, nt.first_sorted, names.off,
+                                                                           (const unsigned char *)names.w, T, traw.off, traw.bytes, entry_of);
+    k_member_info<<<grid_for(D * 32, 256, c->sm_count), 256, 0, s>>>(D, ra.line_moff, ngid, entry_of, d_id, ment, mkeep);
+    c->launches += 2;
+    ra.ment = ment;
+    ra.mkeep = mkeep;
+    ra.ent_field = d_field;
+    ra.ent_rank = d_rank;
+  }
+  // 7. documents: the old ones merged, then the new items' as cco_format_model writes them
+  const long long X = fa.n_extra, n_docs = D + X;
+  FormatArgs fx = fa;   // the new items only
+  fx.n_rows = 0;
+  long long *doc_len, *doc_off;
+  CKR(ar.alloc(&doc_len, n_docs + 1));
+  CKR(ar.alloc(&doc_off, n_docs + 1));
+  CK(cudaMemsetAsync(doc_len + n_docs, 0, 8, s));
+  if (D > 0) {
+    k_rerank_len<<<grid_for(D, 256, c->sm_count), 256, 0, s>>>(fa, ra, (int32_t)D, doc_len);
+    c->launches++;
+  }
+  if (X > 0) {
+    k_doc_len<<<grid_for(X, 256, c->sm_count), 256, 0, s>>>(fx, (int32_t)X, doc_len + D);
+    c->launches++;
+  }
+  CKR(exclusive_sum_i64(c, ar, doc_len, doc_off, n_docs + 1));
+  long long total = 0;
+  CKR(mail_fetch(c, &total, doc_off + n_docs, 8));
+  CKR(mail_wait(c));
+  unsigned char *d_out;
+  CKR(ar.alloc(&d_out, std::max<long long>(total, 1)));
+  if (D > 0) {
+    k_rerank_write<<<grid_for(D * 32, 256, c->sm_count), 256, 0, s>>>(fa, ra, (int32_t)D, doc_off, d_out);
+    c->launches++;
+  }
+  if (X > 0) {
+    k_doc_write<<<grid_for(X * 32, 256, c->sm_count), 256, 0, s>>>(fx, (int32_t)X, doc_off + D, d_out);
+    c->launches++;
+  }
+  char *host = (char *)ctx->pinned_get((size_t)std::max<long long>(total, 1), /*for_result=*/false);
+  if (!host) return set_error(CCO_E_OOM, "pinned host allocation failed");
+  if (total > 0) CK(cudaMemcpyAsync(host, d_out, (size_t)total, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  *out_bytes = host;
+  *out_len = total;
+  return CCO_OK;
+}
 }  // namespace cco
+
+int cco_rerank_model(cco_ctx_t *ctx, const char *body, int64_t body_len, const cco_item_properties_t *props, int32_t n_rankings,
+                     const cco_ranking_t *rankings, char **out_bytes, int64_t *out_len) {
+  return rerank_model(ctx, body, body_len, props, n_rankings, rankings, out_bytes, out_len);
+}
 
 int cco_format_es_bulk(cco_ctx_t *ctx, const cco_result_t *res, int32_t n_names, const char *const *names,
                        const cco_dictionary_t *row_ids, const cco_dictionary_t *col_ids, char **out_bytes, int64_t *out_len) {

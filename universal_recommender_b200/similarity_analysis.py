@@ -227,17 +227,9 @@ class CcoContext:
         N.check(self._L.cco_format_es_bulk(self._h, handle, n, nm, C.byref(rd), cds, C.byref(out), C.byref(ln)))
         return self._take_body(out, ln)
 
-    def format_model(self, handle, names, row_ids, col_ids, properties=None, rankings=None) -> bytes:
-        """cco_format_model: format_es_bulk plus the item properties and PopModel rankings joined in by item id, and a
-        document for every item without a row that has a property or a score (URAlgorithm.scala:351-367, URModel.scala:57-102).
-        properties = (field_names, item_offsets int64[n + 1], item_bytes uint8[], field int32[n], value_offsets int64[n + 1],
-        value_bytes uint8[]): n (item, field, JSON text) triples, the last of a repeated (item, field) wins.
-        rankings = [(field name, "popular" | "trending" | "hot" | "random", start_ms, end_ms, [(item_offsets, item_bytes,
-        time_ms int64[]) per event name])].  A "random" ranking (uniqueRank) scores the items of its streams' events in
-        [start_ms, end_ms) plus every property item with n · 10^-15, n a hash of the id and the window (ur_model.random_rank);
-        give it every event name's stream, as calcRandom reads them all.  Id columns in the layout of encode_ids."""
-        keep = []
-        n, nm, rd, cds = self._format_args(names, row_ids, col_ids, keep)
+    @staticmethod
+    def _model_args(properties, rankings, keep):
+        """format_model's properties / rankings arguments -> (ItemPropertiesT or None, rankings list, RankingT array)"""
         p64, p32 = C.POINTER(C.c_int64), C.POINTER(C.c_int32)
         arr = lambda x, dt: np.ascontiguousarray(x, dtype=dt)
         ptr = lambda b: b.ctypes.data if len(b) else None
@@ -264,9 +256,38 @@ class CcoContext:
             nb = name.encode("utf-8")
             keep.append((st, nb))
             rk[k] = N.RankingT(nb, N.POP_MODES.get(mode, -1), len(streams), int(start_ms), int(end_ms), st)
+        return props, rankings, rk
+
+    def format_model(self, handle, names, row_ids, col_ids, properties=None, rankings=None) -> bytes:
+        """cco_format_model: format_es_bulk plus the item properties and PopModel rankings joined in by item id, and a
+        document for every item without a row that has a property or a score (URAlgorithm.scala:351-367, URModel.scala:57-102).
+        properties = (field_names, item_offsets int64[n + 1], item_bytes uint8[], field int32[n], value_offsets int64[n + 1],
+        value_bytes uint8[]): n (item, field, JSON text) triples, the last of a repeated (item, field) wins.
+        rankings = [(field name, "popular" | "trending" | "hot" | "random", start_ms, end_ms, [(item_offsets, item_bytes,
+        time_ms int64[]) per event name])].  A "random" ranking (uniqueRank) scores the items of its streams' events in
+        [start_ms, end_ms) plus every property item with n · 10^-15, n a hash of the id and the window (ur_model.random_rank);
+        give it every event name's stream, as calcRandom reads them all.  Id columns in the layout of encode_ids."""
+        keep = []
+        n, nm, rd, cds = self._format_args(names, row_ids, col_ids, keep)
+        props, rankings, rk = self._model_args(properties, rankings, keep)
         out, ln = C.c_void_p(), C.c_int64()
         N.check(self._L.cco_format_model(self._h, handle, n, nm, C.byref(rd), cds, C.byref(props) if props is not None else None,
                                          len(rankings), rk, C.byref(out), C.byref(ln)))
+        return self._take_body(out, ln)
+
+    def rerank_model(self, body: bytes, properties=None, rankings=None) -> bytes:
+        """cco_rerank_model: calcPop (URAlgorithm.scala:375-399, recsModel "backfill") on an existing index.  body = the
+        Elasticsearch bulk body of the current model, as format_model writes it; properties and rankings as in format_model.
+        Every old document keeps its members and gets the rankings; a fresh property is added only where the old document
+        has no member of that name, and an old rank member stays when the item has no score in the new ranking (include/
+        cco_b200.h states the grammar, precedence and order).  Items with a property or a score but no old document are
+        appended as format_model writes them."""
+        keep = []
+        props, rankings, rk = self._model_args(properties, rankings, keep)
+        body = bytes(body)
+        out, ln = C.c_void_p(), C.c_int64()
+        N.check(self._L.cco_rerank_model(self._h, body, len(body), C.byref(props) if props is not None else None, len(rankings), rk,
+                                         C.byref(out), C.byref(ln)))
         return self._take_body(out, ln)
 
     def train_csr(self, mats: Sequence[tuple[int, int, np.ndarray, np.ndarray]], params: Sequence[tuple[int, int, Optional[float]]],

@@ -1,7 +1,8 @@
 """Mirror of the train half of URAlgorithm that reaches the hot path
 (src/main/scala/URAlgorithm.scala:130-171 params, :310-369 calcAll).
 calc_all_on_device runs the whole train half on the GPU, string events in and the Elasticsearch bulk body out.
-Everything else in URAlgorithm (calcPop, ES query building) is out of scope."""
+calc_pop_on_device runs calcPop (recsModel "backfill") on the GPU: the current index's bulk body in, the same index with
+fresh rankings out.  Everything else in URAlgorithm (ES reads and query building) is out of scope."""
 from __future__ import annotations
 
 import time
@@ -106,13 +107,13 @@ def calc_all_on_device(events: Sequence[tuple[str, str, str, int]], set_events: 
     Elasticsearch bulk body out.  events = (user id, event name, item id, time ms); set_events = (item id, {field: value}) of
     the items' `$set` events in event-time order.  Steps: cco_ingest_strings (Preparator) -> cco_train_dataset -> the
     rankings' PopModel histograms (popular, trending, hot, and random over every event name) and the property join ->
-    cco_format_model.  "collabFiltering" writes the correlators only (propertiesRDD is empty there); "backfill" (calcPop,
-    which reads the live index) is not supported.
+    cco_format_model.  "collabFiltering" writes the correlators only (propertiesRDD is empty there); "backfill" raises:
+    calcPop refreshes an existing index instead, see calc_pop_on_device.
     now_ms: the rankings' end when a ranking has no offsetDate (default: the wall clock).  A random ranking's values are a
     hash of the item id and the window (ur_model.random_rank): they change with now_ms and repeat for a fixed window."""
     _check_recs_model(ap)
     if ap.recsModel == "backfill":
-        raise ValueError("recsModel=backfill runs calcPop against the live index; it has no train half to run here")
+        raise ValueError("recsModel=backfill runs calcPop against the live index: use calc_pop_on_device with its bulk body")
     ctx = ctx or default_context()
     seed, flags = _seed_and_flags(ap, flags)
     names = ap.model_event_names()
@@ -132,15 +133,7 @@ def calc_all_on_device(events: Sequence[tuple[str, str, str, int]], set_events: 
                    ap.maxCorrelatorsPerEventType or DefaultURAlgoParams.MaxCorrelatorsPerEventType, None)] * len(actions)
     props, rankings = None, None
     if ap.recsModel == "all":
-        triples = [(i, f, extract_jvalue(f, v)) for i, f, v in aggregate_properties(set_events)]
-        fields = list(dict.fromkeys(f for _, f, _ in triples))
-        fidx = {f: k for k, f in enumerate(fields)}
-        props = (fields, *encode_ids([i for i, _, _ in triples]), [fidx[f] for _, f, _ in triples],
-                 *encode_ids([property_json(v) for _, _, v in triples]))
-        now = now_ms if now_ms is not None else int(time.time() * 1000)
-        ev_by_name = {n: [(i, t) for _, i, t in ev] for n, ev in by_name.items()}
-        rankings = [(r.field, r.mode, r.start_ms, r.end_ms, [(*encode_ids(items), times) for items, times in r.streams])
-                    for r in rankings_for(rankings_params(ap.rankings, names), ev_by_name, now, names)]
+        props, rankings = _properties_and_rankings(by_name, set_events, ap, now_ms)
     ds, _, items = ctx.ingest_strings(cols, min_events_per_user or 0)
     try:
         _, h = ctx.train_dataset(ds, params, seed, flags, keep=True)
@@ -150,3 +143,36 @@ def calc_all_on_device(events: Sequence[tuple[str, str, str, int]], set_events: 
             ctx.free_result(h)
     finally:
         ctx.free_dataset(ds)
+
+
+def _properties_and_rankings(by_name: dict, set_events: Sequence[tuple[str, dict]], ap: URAlgorithmParams, now_ms: Optional[int]):
+    """propertiesRDD's inputs in the form of CcoContext.format_model: the `$set` properties as JSON text triples and the
+    rankings of getRanksRDD over the events {event name: [(user, item, time ms)]}"""
+    names = ap.model_event_names()
+    triples = [(i, f, extract_jvalue(f, v)) for i, f, v in aggregate_properties(set_events)]
+    fields = list(dict.fromkeys(f for _, f, _ in triples))
+    fidx = {f: k for k, f in enumerate(fields)}
+    props = (fields, *encode_ids([i for i, _, _ in triples]), [fidx[f] for _, f, _ in triples],
+             *encode_ids([property_json(v) for _, _, v in triples]))
+    now = now_ms if now_ms is not None else int(time.time() * 1000)
+    ev_by_name = {n: [(i, t) for _, i, t in ev] for n, ev in by_name.items()}
+    rankings = [(r.field, r.mode, r.start_ms, r.end_ms, [(*encode_ids(items), times) for items, times in r.streams])
+                for r in rankings_for(rankings_params(ap.rankings, names), ev_by_name, now, names)]
+    return props, rankings
+
+
+def calc_pop_on_device(body: bytes, events: Sequence[tuple[str, str, str, int]], set_events: Sequence[tuple[str, dict]],
+                       ap: URAlgorithmParams, now_ms: Optional[int] = None, ctx: CcoContext | None = None) -> bytes:
+    """URAlgorithm.calcPop (URAlgorithm.scala:375-399, recsModel "backfill") on the GPU: the rankings of an existing index
+    refreshed between trains, without a CCO train.  body = the current index as an Elasticsearch bulk body (what
+    calc_all_on_device or format_model wrote; reading it from Elasticsearch stays with the caller); events and set_events as
+    in calc_all_on_device, now_ms likewise.  The properties and rankings are built as calc_all_on_device builds them and
+    joined into the old documents by cco_rerank_model: per document, fresh `$set` properties < old members < rankings <
+    "id".  So a fresh `$set` value loses to an old member of the same name, and an old rank member survives when the item
+    has no score in the new window.  Items with a property or a score and no old document are appended."""
+    ctx = ctx or default_context()
+    by_name: dict = {}
+    for u, e, i, t in events:
+        by_name.setdefault(e, []).append((u, i, t))
+    props, rankings = _properties_and_rankings(by_name, set_events, ap, now_ms)
+    return ctx.rerank_model(body, props, rankings)

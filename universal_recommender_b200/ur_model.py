@@ -312,3 +312,38 @@ def model_documents(row_ids: Sequence[str], indicators: Sequence[tuple[str, Sequ
         doc["id"] = item
         docs.append(doc)
     return docs
+
+
+def rerank_documents(old_docs: Sequence[tuple[str, dict]], properties: Sequence[tuple[str, str, object]],
+                     rankings: Sequence[Ranking]) -> list[dict]:
+    """calcPop's documents (URAlgorithm.scala:375-399): the current index `old_docs` = [(item id, {member: value})] in index
+    order joined with fresh properties and rankings the way calcPop + URModel.save join them, one dict per item in the
+    order cco_rerank_model writes the documents: the old documents first, then the items without one that have a property
+    or a score, by first appearance (property triples, then the ranking streams in order).
+    propertiesRDD = current.fullOuterJoin(ranks) gives meta ++ rank, and save's groupAll puts the fresh fields under it,
+    so per document, lowest to highest: fresh properties < old members < rankings (a later one beats an earlier one of the
+    same name) < "id".  A fresh `$set` value loses to an old member of the same name, and an old rank member survives when
+    the item has no score in the new ranking.  Random rankings cover the property items, not items only in the index."""
+    props: dict = {}
+    for item, f, v in properties:
+        props.setdefault(item, {})[f] = v
+    scored = [(r.field, r.scores([i for i, _, _ in properties])) for r in rankings]
+    have = {item for item, _ in old_docs}
+    order = list(old_docs)
+    seen = set()
+    for item in [i for i, _, _ in properties] + [i for r in rankings for s in r.streams for i in s[0]]:
+        if item in have or item in seen:
+            continue
+        seen.add(item)
+        if item in props or any(item in sc for _, sc in scored):
+            order.append((item, {}))
+    docs = []
+    for item, meta in order:
+        doc = dict(props.get(item, {}))
+        doc.update(meta)
+        for name, sc in scored:
+            if item in sc:
+                doc[name] = sc[item]
+        doc["id"] = item
+        docs.append(doc)
+    return docs
