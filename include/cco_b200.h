@@ -419,6 +419,74 @@ int cco_rerank_model(cco_ctx_t *ctx, const char *body, int64_t body_len, const c
                      int32_t n_rankings, const cco_ranking_t *rankings, char **out_bytes, int64_t *out_len);
 
 /*
+ * A PredictionIO event export read on the device: the DataSource of the reference (DataSource.scala:65-102) and the event
+ * reads of PopModel (PopModel.scala:184-195) over the interchange format `pio export` writes and `pio import` reads, JSON
+ * lines, one event per line.  Reading the event store stays with the caller.  cco_event_log_read makes one host -> device
+ * copy of the export and parses it there into a resident log (per-GPU contexts only, as every resident dataset):
+ *  - lines end in '\n' (the last one may not); a '\r' before it is JSON whitespace; every line is one JSON object (a blank
+ *    line is an error);
+ *  - members read: "event", "entityType", "entityId", "eventTime" (strings, required), "targetEntityType" and
+ *    "targetEntityId" (strings, null or absent; given together or not at all), "properties" (an object or absent); every
+ *    other member is ignored.  Names are compared decoded; where a name repeats, the last one wins.  Strings are decoded
+ *    (\uXXXX, surrogate pairs, short escapes), so ids compare as cco_ingest_strings compares them;
+ *  - eventTime: Joda's extended date-time YYYY-MM-DDThh:mm:ss, an optional fraction of 1-9 digits (digits past the third
+ *    are dropped: a floor on the time line), then Z, +hh:mm, +hhmm or +hh (sign + or -; the offset is subtracted); years
+ *    0000-9999 of the proleptic Gregorian calendar, times before 1970 included;
+ *  - training events (DataSource.scala:72-89): entityType "user" and targetEntityType "item", grouped by event name; an
+ *    empty entityId or targetEntityId there is an error ("Empty user or item ID");
+ *  - ranking events (PopModel.eventsRDD): every event with a targetEntityId, of any entity types, by event name;
+ *  - property events: "$set", "$unset" and "$delete" with entityType "item", aggregated on the device as
+ *    PEventStore.aggregateProperties does, in (eventTime, line) order -- ties go to the later line, the store's order for
+ *    them being undefined: a $set merges its members (a later value of a field wins), a $unset removes the fields it
+ *    names, a $delete drops what the item had.  An item whose final state exists keeps a document even without a field
+ *    (an "id"-only one, and a random-rank candidate), as the reference's fieldsRDD lists it.  Values are the members'
+ *    trimmed JSON text, spliced verbatim (the reference re-serialises them: number spellings and strings under a ranking
+ *    name may differ).  Items are in order of their first property event, an item's fields in the order their names
+ *    first appear among the members of $set / $unset properties;
+ *  - every other line is counted and ignored.
+ * Errors: CCO_E_INVALID_ARG for malformed JSON (nested values are checked for closed strings, valid escapes and bracket
+ * balance only, as in cco_rerank_model), a missing or mistyped member, a bad time or an empty training id -- the message
+ * names the first bad 0-based line, and the verdict comes before any kernel reads through the parsed spans;
+ * CCO_E_UNSUPPORTED for more than 2^31 - 1 lines, a line of 2^31 or more bytes, 2^31 - 1 or more ranking events of one
+ * name, 2^31 - 1 or more property members, and group contexts.  A log belongs to its context: free it before
+ * cco_destroy of that context.
+ */
+typedef struct cco_event_log cco_event_log_t;
+int cco_event_log_read(cco_ctx_t *ctx, const char *bytes, int64_t len, cco_event_log_t **out);
+typedef struct {
+  int64_t n_lines;
+  cco_dictionary_t names;          /* the distinct event names, in order of first appearance (owned by the log) */
+  const int64_t *n_training;       /* [names.n] training events of each name */
+  const int64_t *n_ranking;        /* [names.n] ranking events of each name */
+  int64_t n_property_events;       /* $set / $unset / $delete events of items */
+  int64_t n_property_items;        /* items whose final state exists (each gets a document) */
+  int64_t n_property_fields;       /* distinct fields of the aggregated properties */
+  int64_t n_ignored;               /* lines that are none of training, ranking or property events */
+} cco_event_log_info_t;
+/* arrays owned by the log, valid until cco_event_log_free */
+int cco_event_log_info(const cco_event_log_t *log, cco_event_log_info_t *out);
+/* cco_ingest_strings on the log's training events of the given names (type t = names[t]; a name without events is an
+ * empty type): the same dataset and dictionaries as cco_ingest_strings on those columns, built from the columns in HBM. */
+int cco_event_log_ingest(cco_ctx_t *ctx, const cco_event_log_t *log, int32_t n_names, const char *const *names, int32_t min_events_per_user,
+                         cco_dataset_t **out);
+typedef struct {                   /* a ranking over the log's ranking events: cco_ranking_t with event names for streams */
+  const char *name;
+  int32_t mode;                    /* CCO_POP_*; CCO_POP_RANDOM reads every event name of the log, in order of first appearance */
+  int32_t n_event_names;           /* one stream per name (ignored when random); a name the log does not hold: an empty stream */
+  int64_t start_ms, end_ms;
+  const char *const *event_names;
+} cco_log_ranking_t;
+/* cco_format_model / cco_rerank_model with the properties aggregated from the log and the ranking streams read from it,
+ * all in HBM (each stream: one event name's ranking events in line order).  Same documents, checks and errors; the log
+ * must come from the same context. */
+int cco_format_model_log(cco_ctx_t *ctx, const cco_result_t *res, int32_t n_names, const char *const *names,
+                         const cco_dictionary_t *row_ids, const cco_dictionary_t *col_ids, const cco_event_log_t *log, int32_t n_rankings,
+                         const cco_log_ranking_t *rankings, char **out_bytes, int64_t *out_len);
+int cco_rerank_model_log(cco_ctx_t *ctx, const char *body, int64_t body_len, const cco_event_log_t *log, int32_t n_rankings,
+                         const cco_log_ranking_t *rankings, char **out_bytes, int64_t *out_len);
+int cco_event_log_free(cco_event_log_t *log);
+
+/*
  * Debug/parity entry (tests only): full integer co-occurrence matrix A^T B of two canonical
  * binary matrices computed by the same accumulation kernel as cco_train, no LLR, no top-k.
  * Output CSR over the columns of A with ascending column ids, malloc'ed; free with cco_free.

@@ -12,6 +12,8 @@ Host-side mirror of the reference interface for this path:
   ur_algorithm.calc_all_on_device         <- calcAll through URModel.save's documents, on the GPU (cco_format_model)
   ur_algorithm.calc_pop_on_device         <- calcPop (recsModel "backfill"): an existing index re-ranked on the GPU
                                              (cco_rerank_model)
+  ur_algorithm.calc_all_from_events / calc_pop_from_events  <- the same from a PredictionIO event export parsed on the
+                                             GPU (cco_event_log_read: DataSource.scala:65-102); events.py is its host mirror
   ur_model                                <- propertiesRDD, getRanksRDD, groupAll (URAlgorithm.scala:351-369, 537-560;
                                              URModel.scala:57-140): the host mirror of the model documents
 """
@@ -19,16 +21,17 @@ from ._native import (CcoError, CcoInvalidArgument, FLAG_ASSUME_CANONICAL, FLAG_
                       FLAG_RESULT_NO_LLR, FLAG_ROWRATE_INTDIV, LIB_PATH)
 from .indexed_dataset import BiDictionary, IndexedDataset
 from .preparator import prepare, prepare_on_device
-from .similarity_analysis import (CcoContext, DownsamplableCrossOccurrenceDataset, SimilarityAnalysis,
+from .similarity_analysis import (CcoContext, DownsamplableCrossOccurrenceDataset, EventLog, SimilarityAnalysis,
                                   decode_ids, default_context, encode_ids)
-from .ur_algorithm import (DefaultURAlgoParams, IndicatorParams, URAlgorithmParams, calc_all, calc_all_on_device,
-                           calc_pop_on_device)
+from .ur_algorithm import (DefaultURAlgoParams, IndicatorParams, URAlgorithmParams, calc_all, calc_all_from_events, calc_all_on_device,
+                           calc_pop_from_events, calc_pop_on_device)
 from .ur_model import RankingParams
 
 __all__ = [
     "BiDictionary", "CcoContext", "CcoError", "CcoInvalidArgument", "DefaultURAlgoParams",
     "DownsamplableCrossOccurrenceDataset", "IndexedDataset", "IndicatorParams", "SimilarityAnalysis",
-    "RankingParams", "URAlgorithmParams", "calc_all", "calc_all_on_device", "calc_pop_on_device", "decode_ids", "default_context", "encode_ids", "prepare", "prepare_on_device",
+    "EventLog", "RankingParams", "URAlgorithmParams", "calc_all", "calc_all_from_events", "calc_all_on_device", "calc_pop_from_events",
+    "calc_pop_on_device", "decode_ids", "default_context", "encode_ids", "prepare", "prepare_on_device",
     "FLAG_ASSUME_CANONICAL",
     "FLAG_ENTROPY_VARARGS", "FLAG_ROWRATE_INTDIV", "FLAG_RESULT_NO_COUNT", "FLAG_RESULT_NO_LLR", "LIB_PATH",
 ]

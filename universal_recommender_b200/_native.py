@@ -84,6 +84,17 @@ class RankingT(C.Structure):
                 ("streams", C.POINTER(RankingStreamT))]
 
 
+class EventLogInfoT(C.Structure):
+    _fields_ = [("n_lines", C.c_int64), ("names", DictionaryT), ("n_training", C.POINTER(C.c_int64)), ("n_ranking", C.POINTER(C.c_int64)),
+                ("n_property_events", C.c_int64), ("n_property_items", C.c_int64), ("n_property_fields", C.c_int64),
+                ("n_ignored", C.c_int64)]
+
+
+class LogRankingT(C.Structure):
+    _fields_ = [("name", C.c_char_p), ("mode", C.c_int32), ("n_event_names", C.c_int32), ("start_ms", C.c_int64), ("end_ms", C.c_int64),
+                ("event_names", C.POINTER(C.c_char_p))]
+
+
 class StatsT(C.Structure):
     _fields_ = [("n_users", C.c_int64), ("nnz_in_total", C.c_int64),
                 ("nnz_downsampled", C.c_int64 * 16), ("products", C.c_int64 * 16),
@@ -100,7 +111,8 @@ EXPORTS = [
     "cco_dataset_upload", "cco_train_dataset", "cco_dataset_free", "cco_timer_start", "cco_timer_stop",
     "cco_partition_rows", "cco_ingest", "cco_synth_ingest", "cco_dataset_shape", "cco_dataset_download",
     "cco_dataset_copy_to_host", "cco_format_es_bulk", "cco_ingest_strings", "cco_dataset_dictionary", "cco_pop_model",
-    "cco_format_model", "cco_rerank_model",
+    "cco_format_model", "cco_rerank_model", "cco_event_log_read", "cco_event_log_info", "cco_event_log_ingest",
+    "cco_format_model_log", "cco_rerank_model_log", "cco_event_log_free",
     "cco_result_num_matrices", "cco_result_row_range", "cco_result_matrix", "cco_result_stats", "cco_result_free",
     "cco_debug_cooccurrence", "cco_debug_downsample", "cco_debug_llr", "cco_debug_string_ids", "cco_free",
 ]
@@ -149,6 +161,14 @@ def lib():
                                    C.c_int32, p(RankingT), p(C.c_void_p), p(C.c_int64)]
     L.cco_rerank_model.argtypes = [C.c_void_p, C.c_char_p, C.c_int64, p(ItemPropertiesT), C.c_int32, p(RankingT), p(C.c_void_p),
                                    p(C.c_int64)]
+    L.cco_event_log_read.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, p(C.c_void_p)]
+    L.cco_event_log_info.argtypes = [C.c_void_p, p(EventLogInfoT)]
+    L.cco_event_log_ingest.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, p(C.c_char_p), C.c_int32, p(C.c_void_p)]
+    L.cco_format_model_log.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, p(C.c_char_p), p(DictionaryT), p(DictionaryT), C.c_void_p,
+                                       C.c_int32, p(LogRankingT), p(C.c_void_p), p(C.c_int64)]
+    L.cco_rerank_model_log.argtypes = [C.c_void_p, C.c_char_p, C.c_int64, C.c_void_p, C.c_int32, p(LogRankingT), p(C.c_void_p),
+                                       p(C.c_int64)]
+    L.cco_event_log_free.argtypes = [C.c_void_p]
     L.cco_dataset_shape.argtypes = [C.c_void_p, C.c_int32, p(C.c_int64), p(C.c_int32), p(C.c_int64)]
     L.cco_dataset_download.argtypes = [C.c_void_p, C.c_int32, p(p(C.c_int64)), p(p(C.c_int32))]
     L.cco_timer_start.argtypes = [C.c_void_p]

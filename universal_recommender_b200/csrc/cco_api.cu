@@ -27,6 +27,7 @@
 #include "cco_format.cuh"
 #include "cco_strings.cuh"
 #include "cco_json.cuh"
+#include "cco_events.cuh"
 
 namespace cco {
 
@@ -302,6 +303,13 @@ struct Arena {
     ptrs.push_back(p);
     *out = (T *)p;
     return CCO_OK;
+  }
+  void take(void *p) {   // the buffer outlives the arena: its new owner frees it (never slab memory)
+    for (size_t i = 0; i < ptrs.size(); ++i)
+      if (ptrs[i] == p) {
+        ptrs.erase(ptrs.begin() + i);
+        return;
+      }
   }
   void release(void *p) {   // slab memory is simply not reused within a train
     for (size_t i = 0; i < ptrs.size(); ++i)
@@ -2277,8 +2285,10 @@ static int str_dictionary(cco_ctx *c, Arena &ar, const DevStrCol &col, const Str
   return CCO_OK;
 }
 
-static int ingest_strings_core(cco_ctx *c, int32_t n_types, const cco_string_events_t *ev, int32_t min_events_per_user,
-                               cco_dataset **out) {
+// the user and item columns of type t in HBM: uploaded from the caller's arrays, or views of an event log's columns
+using StrColumns = std::function<int(Arena &, int, DevStrCol *, DevStrCol *)>;
+
+static int ingest_strings_core(cco_ctx *c, int32_t n_types, const StrColumns &columns, int32_t min_events_per_user, cco_dataset **out) {
   CK(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   nvtx_push("cco:ingest_strings");
@@ -2301,20 +2311,10 @@ static int ingest_strings_core(cco_ctx *c, int32_t n_types, const cco_string_eve
   DevStrCol pu;   // the primary user column and its table stay resident: later types look their users up there
   StrTable ut;
   uint32_t n_users = 0;
-  int *bad;
-  CKR(ar.alloc(&bad, 1));
   for (int t = 0; t < n_types; ++t) {
-    const long long ne = ev[t].n_events;
     DevStrCol uc, ic;
-    CKR(str_upload(c, ar, ne, ev[t].user_offsets, ev[t].user_bytes, &uc));
-    CKR(str_upload(c, ar, ne, ev[t].item_offsets, ev[t].item_bytes, &ic));
-    CK(cudaMemsetAsync(bad, 0, sizeof(int), s));
-    str_check_device(c, uc, bad);
-    str_check_device(c, ic, bad);
-    int h_bad = 0;
-    CKR(mail_fetch(c, &h_bad, bad, 4));
-    CKR(mail_wait(c));
-    if (h_bad) return set_error(CCO_E_INVALID_ARG, "type %d: offsets decrease", t);
+    CKR(columns(ar, t, &uc, &ic));
+    const long long ne = uc.n;
     str_hash(c, uc, ~0ULL);
     str_hash(c, ic, ~0ULL);
     int32_t *uid, *iid;
@@ -2378,7 +2378,22 @@ int cco_ingest_strings(cco_ctx_t *c, int32_t n_types, const cco_string_events_t 
     CKR(str_check_host(ev[t].n_events, ev[t].user_offsets, ev[t].user_bytes, t, "user"));
     CKR(str_check_host(ev[t].n_events, ev[t].item_offsets, ev[t].item_bytes, t, "item"));
   }
-  return ingest_strings_core(c, n_types, ev, min_events_per_user, out);
+  const StrColumns upload = [c, ev](Arena &ar, int t, DevStrCol *uc, DevStrCol *ic) -> int {
+    const long long ne = ev[t].n_events;
+    CKR(str_upload(c, ar, ne, ev[t].user_offsets, ev[t].user_bytes, uc));
+    CKR(str_upload(c, ar, ne, ev[t].item_offsets, ev[t].item_bytes, ic));
+    int *bad;
+    CKR(ar.alloc(&bad, 1));
+    CK(cudaMemsetAsync(bad, 0, sizeof(int), c->stream));
+    str_check_device(c, *uc, bad);
+    str_check_device(c, *ic, bad);
+    int h_bad = 0;
+    CKR(mail_fetch(c, &h_bad, bad, 4));
+    CKR(mail_wait(c));
+    if (h_bad) return set_error(CCO_E_INVALID_ARG, "type %d: offsets decrease", t);
+    return CCO_OK;
+  };
+  return ingest_strings_core(c, n_types, upload, min_events_per_user, out);
 }
 
 int cco_dataset_dictionary(const cco_dataset_t *ds, int32_t which, cco_dictionary_t *out) {
@@ -2613,24 +2628,47 @@ struct KeySection {
   const char *bytes;
   bool device = false;
   long long nbytes = 0;
+  long long base = 0;   // device: off[0] (bytes points at that byte)
   long long byte_count() const { return n == 0 ? 0 : device ? nbytes : off[n] - off[0]; }
+};
+// one ranking stream of an event log (cco_format_model_log): the target ids of one event name's ranking events and their
+// times, both in HBM; per ranking, one per event name read
+struct LogStream {
+  KeySection items;
+  const long long *time;
+};
+using LogStreams = std::vector<std::vector<LogStream>>;
+// the properties of an event log (cco_format_model_log): the columns of cco_item_properties_t in HBM, built on the device
+struct DevProps {
+  KeySection items;
+  const int32_t *field;
+  const long long *voff;   // from 0
+  const unsigned char *vals;
 };
 
 // The model part of FormatArgs (cco_format_model, cco_rerank_model): group the item ids of every source, score the
 // rankings per group, sort the properties, and list the documents of items without a row.  The caller's host columns have
 // passed str_check_host.  unique_rows: two rows with the same id are CCO_E_INVALID_ARG (the documents of an old index).
 static int model_fields(cco_ctx *c, Arena &ar, FormatArgs *fa, const KeySection &rows, const cco_item_properties_t *props,
-                        int32_t n_rank, const cco_ranking_t *rk, bool extra_docs, bool unique_rows = false) {
+                        int32_t n_rank, const cco_ranking_t *rk, bool extra_docs, bool unique_rows = false, const LogStreams *ls = nullptr,
+                        const DevProps *dp = nullptr) {
   cudaStream_t s = c->stream;
   mail_reset(c);
   const long long R = rows.n, P = props ? props->n : 0;
   std::vector<KeySection> sec;
   sec.push_back(rows);
-  sec.push_back({P, P > 0 ? props->item_offsets : nullptr, P > 0 ? props->item_bytes : nullptr});
+  sec.push_back(dp ? dp->items : KeySection{P, P > 0 ? props->item_offsets : nullptr, P > 0 ? props->item_bytes : nullptr});
   std::vector<long long> rank_begin(n_rank + 1);   // ranking k's events are key entries R + P + [rank_begin[k], rank_begin[k + 1])
   long long E = 0;
   for (int k = 0; k < n_rank; ++k) {
     rank_begin[k] = E;
+    if (ls) {
+      for (const LogStream &st : (*ls)[k]) {
+        sec.push_back(st.items);
+        E += st.items.n;
+      }
+      continue;
+    }
     for (int q = 0; q < rk[k].n_streams; ++q) {
       const cco_ranking_stream_t &st = rk[k].streams[q];
       sec.push_back({st.n_events, st.item_offsets, st.item_bytes});
@@ -2661,7 +2699,7 @@ static int model_fields(cco_ctx *c, Arena &ar, FormatArgs *fa, const KeySection 
     if (k.n == 0) continue;
     const long long kb = k.byte_count();
     if (k.device) {
-      k_rebase<<<grid_for(k.n + 1, 256, c->sm_count), 256, 0, s>>>(k.n + 1, (const long long *)k.off, byte_at, key.off + at);
+      k_rebase<<<grid_for(k.n + 1, 256, c->sm_count), 256, 0, s>>>(k.n + 1, (const long long *)k.off, byte_at - k.base, key.off + at);
       c->launches++;
       if (kb > 0) CK(cudaMemcpyAsync((char *)key.w + byte_at, k.bytes, (size_t)kb, cudaMemcpyDeviceToDevice, s));
       at += k.n;
@@ -2678,7 +2716,12 @@ static int model_fields(cco_ctx *c, Arena &ar, FormatArgs *fa, const KeySection 
   }
   // property fields and values
   int32_t *d_field = nullptr;
-  if (P > 0) {
+  if (dp && P > 0) {   // built on the device: nothing to copy or check
+    d_field = (int32_t *)dp->field;
+    fa->val_off = dp->voff;
+    fa->val_base = 0;
+    fa->vals = dp->vals;
+  } else if (P > 0) {
     const long long vb = props->value_offsets[P] - props->value_offsets[0];
     long long *d_voff;
     unsigned char *d_vals;
@@ -2700,6 +2743,13 @@ static int model_fields(cco_ctx *c, Arena &ar, FormatArgs *fa, const KeySection 
   CKR(ar.alloc(&d_t, std::max<long long>(E, 1)));
   for (int k = 0; k < n_rank; ++k) {
     long long e = rank_begin[k];
+    if (ls) {
+      for (const LogStream &st : (*ls)[k]) {
+        if (st.items.n > 0) CK(cudaMemcpyAsync(d_t + e, st.time, sizeof(int64_t) * (size_t)st.items.n, cudaMemcpyDeviceToDevice, s));
+        e += st.items.n;
+      }
+      continue;
+    }
     for (int q = 0; q < rk[k].n_streams; ++q) {
       const cco_ranking_stream_t &st = rk[k].streams[q];
       if (st.n_events > 0) CK(cudaMemcpyAsync(d_t + e, st.time_ms, sizeof(int64_t) * (size_t)st.n_events, cudaMemcpyHostToDevice, s));
@@ -2846,7 +2896,8 @@ static int model_fields(cco_ctx *c, Arena &ar, FormatArgs *fa, const KeySection 
 }
 
 // host checks of the model inputs (the device checks decreasing offsets, field indices and empty values)
-static int model_check_host(const cco_dictionary_t *row_ids, const cco_item_properties_t *props, int32_t n_rank, const cco_ranking_t *rk) {
+static int model_check_host(const cco_dictionary_t *row_ids, const cco_item_properties_t *props, int32_t n_rank, const cco_ranking_t *rk,
+                            const LogStreams *ls = nullptr, bool dev_props = false) {
   if (n_rank < 0 || (n_rank > 0 && !rk)) return set_error(CCO_E_INVALID_ARG, "bad rankings");
   if (n_rank > kMaxRankings) return set_error(CCO_E_UNSUPPORTED, "%d rankings, at most %d", n_rank, kMaxRankings);
   long long total = row_ids->n;
@@ -2859,7 +2910,7 @@ static int model_check_host(const cco_dictionary_t *row_ids, const cco_item_prop
         if (!strcmp(props->field_names[h], props->field_names[f]))
           return set_error(CCO_E_INVALID_ARG, "field names %d and %d are both \"%s\"", h, f, props->field_names[f]);
     }
-    if (props->n > 0) {
+    if (props->n > 0 && !dev_props) {
       if (!props->field) return set_error(CCO_E_INVALID_ARG, "null property field indices");
       CKR(str_check_host(props->n, props->item_offsets, props->item_bytes, -1, "property item"));
       CKR(str_check_host(props->n, props->value_offsets, props->value_bytes, -1, "property value"));
@@ -2872,6 +2923,11 @@ static int model_check_host(const cco_dictionary_t *row_ids, const cco_item_prop
     if (r.mode < CCO_POP_POPULAR || r.mode > CCO_POP_RANDOM)
       return set_error(CCO_E_INVALID_ARG, "ranking %d: mode must be CCO_POP_POPULAR, _TRENDING, _HOT or _RANDOM", k);
     if (r.end_ms < r.start_ms) return set_error(CCO_E_INVALID_ARG, "ranking %d: end before start (Joda Interval would throw)", k);
+    if (ls) {   // the log's columns were built on the device
+      for (const LogStream &st : (*ls)[k]) total += st.items.n;
+      if (total >= 0x7fffffffLL) break;
+      continue;
+    }
     if (r.n_streams < 1 || !r.streams) return set_error(CCO_E_INVALID_ARG, "ranking %d: needs at least one stream", k);
     for (int q = 0; q < r.n_streams; ++q) {
       const cco_ranking_stream_t &st = r.streams[q];
@@ -2954,7 +3010,8 @@ static int model_names(cco_ctx *c, Arena &ar, FormatArgs *fa, int n_ind, const c
 // cco_format_es_bulk == format_model without properties and rankings: one set of document kernels
 static int format_model(cco_ctx_t *ctx, const cco_result_t *res, int32_t n_names, const char *const *names, const cco_dictionary_t *row_ids,
                         const cco_dictionary_t *col_ids, const cco_item_properties_t *props, int32_t n_rank, const cco_ranking_t *rk,
-                        char **out_bytes, int64_t *out_len, const char *range) {
+                        char **out_bytes, int64_t *out_len, const char *range, const LogStreams *ls = nullptr,
+                        const DevProps *dp = nullptr) {
   if (!ctx || !res || !names || !row_ids || !col_ids || !out_bytes || !out_len) return set_error(CCO_E_INVALID_ARG, "null argument");
   const int n_ind = (int)res->mats.size();
   if (n_names != n_ind) return set_error(CCO_E_INVALID_ARG, "%d event names for %d indicators", n_names, n_ind);
@@ -2970,7 +3027,7 @@ static int format_model(cco_ctx_t *ctx, const cco_result_t *res, int32_t n_names
   }
   if (row_ids->n < row_hi) return set_error(CCO_E_INVALID_ARG, "row dictionary has %lld ids, rows go up to %lld", (long long)row_ids->n, (long long)row_hi);
   const bool model = (props && props->n > 0) || n_rank > 0;
-  if (model) CKR(model_check_host(row_ids, props, n_rank, rk));
+  if (model) CKR(model_check_host(row_ids, props, n_rank, rk, ls, dp != nullptr));
   CK(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   Arena ar(s);
@@ -2985,7 +3042,7 @@ static int format_model(cco_ctx_t *ctx, const cco_result_t *res, int32_t n_names
   CKR(upload_dict(c, ar, *row_ids, &raw));
   CKR(escape_dict(c, ar, raw, &fa.row_ids));
   CKR(model_names(c, ar, &fa, n_ind, names, model, props, n_rank, rk));
-  if (model) CKR(model_fields(c, ar, &fa, KeySection{row_ids->n, row_ids->offsets, row_ids->bytes}, props, n_rank, rk, row_lo == 0));
+  if (model) CKR(model_fields(c, ar, &fa, KeySection{row_ids->n, row_ids->offsets, row_ids->bytes}, props, n_rank, rk, row_lo == 0, false, ls, dp));
   for (int i = 0; i < n_ind; ++i) {
     const ResultMat &m = res->mats[i];
     CKR(upload_dict(c, ar, col_ids[i], &raw));
@@ -3061,7 +3118,7 @@ static int json_members(cco_ctx *c, Arena &ar, long long n, const long long *sb,
   CK(cudaMemsetAsync(cnt + n, 0, 8, s));
   CK(cudaMemsetAsync(err, 0xff, 8, s));
   const int grid = grid_for(n * 32, 256, c->sm_count);
-  k_json_members<false><<<grid, 256, 0, s>>>(n, sb, se, body, cnt, nullptr, nullptr, err);
+  k_json_members<<<grid, 256, 0, s>>>(n, sb, se, body, MemberSink<false>{cnt, nullptr, nullptr}, err);
   c->launches++;
   CKR(exclusive_sum_i64(c, ar, cnt, moff, n + 1));
   unsigned long long h_err = 0;
@@ -3074,7 +3131,7 @@ static int json_members(cco_ctx *c, Arena &ar, long long n, const long long *sb,
   JMember *mem;
   CKR(ar.alloc(&mem, std::max<long long>(total, 1)));
   if (total > 0) {
-    k_json_members<true><<<grid, 256, 0, s>>>(n, sb, se, body, nullptr, moff, mem, err);
+    k_json_members<<<grid, 256, 0, s>>>(n, sb, se, body, MemberSink<true>{nullptr, moff, mem}, err);
     c->launches++;
   }
   ar.release(cnt);
@@ -3108,15 +3165,21 @@ static int json_decode(cco_ctx *c, Arena &ar, long long n, const JMember *m, con
 }
 
 static int rerank_model(cco_ctx_t *ctx, const char *body, int64_t body_len, const cco_item_properties_t *props, int32_t n_rank,
-                        const cco_ranking_t *rk, char **out_bytes, int64_t *out_len) {
+                        const cco_ranking_t *rk, char **out_bytes, int64_t *out_len, const LogStreams *ls = nullptr,
+                        const DevProps *dp = nullptr) {
   if (!ctx || !out_bytes || !out_len || body_len < 0 || (body_len > 0 && !body)) return set_error(CCO_E_INVALID_ARG, "null argument or negative length");
   if (!ctx->members.empty()) return set_error(CCO_E_UNSUPPORTED, "per-GPU contexts only");
   if (body_len > 0 && body[body_len - 1] != '\n') return set_error(CCO_E_INVALID_ARG, "the body does not end in a newline");
   const cco_dictionary_t no_rows = {0, nullptr, nullptr};
-  CKR(model_check_host(&no_rows, props, n_rank, rk));
+  CKR(model_check_host(&no_rows, props, n_rank, rk, ls, dp != nullptr));
   long long fresh = props ? props->n : 0;   // property triples + ranking events, checked < 2^31 by model_check_host
-  for (int k = 0; k < n_rank; ++k)
+  for (int k = 0; k < n_rank; ++k) {
+    if (ls) {
+      for (const LogStream &st : (*ls)[k]) fresh += st.items.n;
+      continue;
+    }
     for (int q = 0; q < rk[k].n_streams; ++q) fresh += rk[k].streams[q].n_events;
+  }
   cco_ctx *c = ctx;
   CK(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
@@ -3210,7 +3273,7 @@ static int rerank_model(cco_ctx_t *ctx, const char *body, int64_t body_len, cons
   rows.bytes = (const char *)ids.w;
   rows.device = true;
   rows.nbytes = ids_bytes;
-  CKR(model_fields(c, ar, &fa, rows, props, n_rank, rk, true, true));
+  CKR(model_fields(c, ar, &fa, rows, props, n_rank, rk, true, true, ls, dp));
   // 6. member names -> the distinct names of the fields, the rankings and "id"
   if (D > 0) {
     std::vector<std::string> ent;
@@ -3321,6 +3384,672 @@ int cco_format_model(cco_ctx_t *ctx, const cco_result_t *res, int32_t n_names, c
                      const cco_dictionary_t *col_ids, const cco_item_properties_t *props, int32_t n_rankings, const cco_ranking_t *rankings,
                      char **out_bytes, int64_t *out_len) {
   return format_model(ctx, res, n_names, names, row_ids, col_ids, props, n_rankings, rankings, out_bytes, out_len, "cco:format_model");
+}
+
+// ---- cco_event_log_*: a PredictionIO event export parsed on the device (kernels in cco_events.cuh) ---------------------
+// One string column of the log, partitioned by event name (file order inside a name): offsets from 0 and 8-byte words with
+// 16 bytes of padding, in HBM; boff[g] = the byte offset of name g's first entry (host copy, n_names + 1 entries).
+struct EvCol {
+  long long *off = nullptr;
+  uint64_t *w = nullptr;
+  std::vector<long long> boff;
+};
+struct cco_event_log {
+  cco_ctx *ctx = nullptr;
+  long long n_lines = 0, n_prop = 0, n_ignored = 0;
+  std::vector<int64_t> name_off;   // the distinct event names, first appearance order
+  std::string name_bytes;
+  std::vector<int64_t> n_train, n_rank;        // per name
+  std::vector<long long> train_at, rank_at;    // per name + 1: first event of the name in the partitioned columns
+  EvCol tu, ti, ri;                            // training users, training items, ranking items
+  long long *rtime = nullptr;                  // ranking event times, partitioned as ri
+  // the aggregated properties: n_triples (item, field, value text) triples in HBM (cco_item_properties_t's columns,
+  // offsets from 0), the field names on the host
+  long long n_prop_items = 0, n_prop_fields = 0, n_triples = 0;
+  int32_t *p_field = nullptr;
+  long long *p_voff = nullptr, *p_ioff = nullptr, p_ibytes_n = 0;
+  unsigned char *p_vals = nullptr, *p_ibytes = nullptr;
+  std::vector<std::string> field_names;
+  std::vector<void *> dev;                     // what to free
+  int code_of(const char *name) const {
+    const size_t n = strlen(name);
+    for (size_t g = 0; g + 1 < name_off.size(); ++g)
+      if ((size_t)(name_off[g + 1] - name_off[g]) == n && !memcmp(name_bytes.data() + name_off[g], name, n)) return (int)g;
+    return -1;
+  }
+  // the entries [at[g], at[g] + n) of a column as a string column the ingest and key kernels read (no copy)
+  DevStrCol view(const EvCol &col, int g, const std::vector<long long> &at, long long n) const {
+    DevStrCol v;
+    v.n = g >= 0 ? n : 0;
+    const long long b0 = g >= 0 ? col.boff[g] : 0;
+    v.base = b0 & ~7LL;
+    v.off = col.off + (g >= 0 ? at[g] : 0);
+    v.w = col.w + v.base / 8;
+    return v;
+  }
+};
+
+namespace cco {
+static void event_log_release(cco_event_log *lg) {
+  if (!lg) return;
+  cudaSetDevice(lg->ctx->device);
+  for (void *p : lg->dev) cudaFreeAsync(p, lg->ctx->stream);
+  cudaStreamSynchronize(lg->ctx->stream);
+  delete lg;
+}
+static int event_error(unsigned long long err) {
+  const long long line = (long long)(err >> 8);
+  switch ((unsigned)(err & 0xff)) {
+    case kJsonLongLine: return set_error(CCO_E_UNSUPPORTED, "line %lld: longer than 2^31 - 1 bytes", line);
+    case kJsonNotObject: return set_error(CCO_E_INVALID_ARG, "line %lld: not a JSON object (a blank line is not an event)", line);
+    case kJsonString:
+      return set_error(CCO_E_INVALID_ARG, "line %lld: a string is unterminated or holds a bad escape or a raw byte < 0x20", line);
+    case kEvMissing:
+      return set_error(CCO_E_INVALID_ARG, "line %lld: an event needs \"event\", \"entityType\", \"entityId\" and \"eventTime\"", line);
+    case kEvType:
+      return set_error(CCO_E_INVALID_ARG, "line %lld: a member has the wrong type (event, entityType, entityId, eventTime: string; "
+                       "targetEntityType, targetEntityId: string or null; properties: object)", line);
+    case kEvTime_:
+      return set_error(CCO_E_INVALID_ARG, "line %lld: eventTime is not YYYY-MM-DDThh:mm:ss[.fraction](Z|+hh:mm|+hhmm|+hh)", line);
+    case kEvEmptyId: return set_error(CCO_E_INVALID_ARG, "line %lld: Empty user or item ID", line);
+    case kEvTarget: return set_error(CCO_E_INVALID_ARG, "line %lld: targetEntityType and targetEntityId must be given together", line);
+    default:
+      return set_error(CCO_E_INVALID_ARG, "line %lld: not one JSON object (unbalanced brackets or an unexpected token)", line);
+  }
+}
+static int log_keep(Arena &ar, cco_event_log *lg, void *p) {
+  ar.take(p);
+  lg->dev.push_back(p);
+  return CCO_OK;
+}
+// the lines carrying flag bit `want` in a stable order: by event name (code != nullptr), else by line -> idx[0 .. count)
+static int event_partition(cco_ctx *c, Arena &ar, long long L, const uint8_t *flag, uint8_t want, const int32_t *code, uint32_t n_names,
+                           uint32_t **idx) {
+  cudaStream_t s = c->stream;
+  uint32_t *k0, *k1, *v0, *v1;
+  CKR(ar.alloc(&k0, L));
+  CKR(ar.alloc(&k1, L));
+  CKR(ar.alloc(&v0, L));
+  CKR(ar.alloc(&v1, L));
+  const uint32_t past = code ? n_names : 1;
+  k_event_keys<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, flag, want, code, past, k0, v0);
+  c->launches++;
+  int bits = 1;
+  while ((1u << bits) <= past) ++bits;
+  cub::DoubleBuffer<uint32_t> kb(k0, k1), vb(v0, v1);
+  size_t tbytes = 0;
+  CK(cub::DeviceRadixSort::SortPairs(nullptr, tbytes, kb, vb, L, 0, bits, s));
+  void *tmp;
+  CKR(ar.alloc((char **)&tmp, tbytes));
+  CK(cub::DeviceRadixSort::SortPairs(tmp, tbytes, kb, vb, L, 0, bits, s));
+  c->launches++;
+  ar.release(tmp);
+  *idx = vb.Current();
+  ar.release(k0);
+  ar.release(k1);
+  ar.release(vb.Alternate());
+  return CCO_OK;
+}
+// member k's string of the listed lines decoded into a column kept by the log; boff at the names' first entries
+static int event_column(cco_ctx *c, Arena &ar, cco_event_log *lg, long long n, const uint32_t *idx, int k, const long long *sb,
+                        const int2 *span, const unsigned char *body, const std::vector<long long> &at, EvCol *col) {
+  cudaStream_t s = c->stream;
+  JMember *jm;
+  CKR(ar.alloc(&jm, std::max<long long>(n, 1)));
+  if (n > 0) {
+    k_event_strings<<<grid_for(n, 256, c->sm_count), 256, 0, s>>>(n, idx, k, sb, span, body, jm);
+    c->launches++;
+  }
+  DevStrCol d;
+  long long nb = 0;
+  CKR(json_decode(c, ar, n, jm, body, &d, &nb));
+  ar.release(jm);
+  ar.release(d.hash);
+  CKR(log_keep(ar, lg, d.off));
+  CKR(log_keep(ar, lg, d.w));
+  col->off = d.off;
+  col->w = d.w;
+  col->boff.assign(at.size(), 0);
+  std::vector<uint32_t> at32(at.begin(), at.end());
+  uint32_t *d_at;
+  long long *d_b;
+  CKR(ar.alloc(&d_at, at.size()));
+  CKR(ar.alloc(&d_b, at.size()));
+  CK(cudaMemcpyAsync(d_at, at32.data(), sizeof(uint32_t) * at.size(), cudaMemcpyHostToDevice, s));
+  k_gather_i64<<<grid_for((long long)at.size(), 256, c->sm_count), 256, 0, s>>>((long long)at.size(), d_at, d.off, d_b);
+  c->launches++;
+  CK(cudaMemcpyAsync(col->boff.data(), d_b, sizeof(long long) * at.size(), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));   // at32 is a local
+  return CCO_OK;
+}
+
+// sort (key, value) pairs of n entries by the low `bits` bits of the key, stably; the sorted arrays replace *k / *v
+extern "C++" {
+template <typename K>
+int sort_pairs(cco_ctx *c, Arena &ar, long long n, K **k, uint32_t **v, int bits) {
+  cudaStream_t s = c->stream;
+  K *k1;
+  uint32_t *v1;
+  CKR(ar.alloc(&k1, std::max<long long>(n, 1)));
+  CKR(ar.alloc(&v1, std::max<long long>(n, 1)));
+  cub::DoubleBuffer<K> kb(*k, k1);
+  cub::DoubleBuffer<uint32_t> vb(*v, v1);
+  size_t tbytes = 0;
+  CK(cub::DeviceRadixSort::SortPairs(nullptr, tbytes, kb, vb, n, 0, bits, s));
+  void *tmp;
+  CKR(ar.alloc((char **)&tmp, tbytes));
+  CK(cub::DeviceRadixSort::SortPairs(tmp, tbytes, kb, vb, n, 0, bits, s));
+  c->launches++;
+  ar.release(tmp);
+  ar.release(kb.Alternate());
+  ar.release(vb.Alternate());
+  *k = kb.Current();
+  *v = vb.Current();
+  return CCO_OK;
+}
+}  // extern "C++"
+static int bits_for(long long n) {
+  int b = 1;
+  while ((1LL << b) < n) ++b;
+  return b;
+}
+// PEventStore.aggregateProperties over the property events ($set / $unset / $delete of items) of a read log, in
+// (eventTime, line) order: a $set merges its members (the later value of a field wins), a $unset removes the fields it
+// names, a $delete drops what the item had.  Result, kept by the log: (item, field, value text) triples in the order of
+// the items' first property event (line order), each item's fields in the order their names first appear among the
+// members of $set / $unset properties; an item whose final state exists without a field gets one triple of the field "id"
+// (never written: "id" wins) so that it has a document and is a random-rank candidate.  Values are the members' trimmed
+// JSON text, spliced verbatim.  Field numbers follow first appearance in the triples.
+static int event_properties(cco_ctx *c, Arena &ar, cco_event_log *lg, long long L, const uint8_t *flag, const long long *tm,
+                            const long long *sb, const int2 *span, const unsigned char *bb) {
+  cudaStream_t s = c->stream;
+  const long long NP = lg->n_prop;
+  uint32_t *pl;   // property event -> line, line order
+  CKR(event_partition(c, ar, L, flag, kEvProperty, nullptr, 0, &pl));
+  // items, grouped exactly in order of first appearance
+  EvCol pcol;
+  CKR(event_column(c, ar, lg, NP, pl, kEvEntityId, sb, span, bb, std::vector<long long>{0, NP}, &pcol));
+  DevStrCol pc;
+  pc.n = NP;
+  pc.off = pcol.off;
+  pc.w = pcol.w;
+  CKR(ar.alloc(&pc.hash, NP));
+  str_hash(c, pc, ~0ULL);
+  int32_t *pg;
+  CKR(ar.alloc(&pg, NP));
+  StrTable it;
+  CKR(str_group(c, ar, pc, nullptr, false, 0, &it, pg));
+  const long long G = it.n_groups;
+  // kinds, and each event's position in the (eventTime, line) order (a stable sort by time of events in line order)
+  uint8_t *pk;
+  long long *pt;
+  CKR(ar.alloc(&pk, NP));
+  CKR(ar.alloc(&pt, NP));
+  k_gather_u8<<<grid_for(NP, 256, c->sm_count), 256, 0, s>>>(NP, pl, flag, pk);
+  k_gather_i64<<<grid_for(NP, 256, c->sm_count), 256, 0, s>>>(NP, pl, tm, pt);
+  unsigned long long *tk;
+  uint32_t *tv;
+  CKR(ar.alloc(&tk, NP));
+  CKR(ar.alloc(&tv, NP));
+  k_prop_time_keys<<<grid_for(NP, 256, c->sm_count), 256, 0, s>>>(NP, pt, tk, tv);
+  c->launches += 3;
+  CKR(sort_pairs(c, ar, NP, &tk, &tv, 64));
+  int32_t *ord, *last_del, *last_set;
+  CKR(ar.alloc(&ord, NP));
+  CKR(ar.alloc(&last_del, G));
+  CKR(ar.alloc(&last_set, G));
+  CK(cudaMemsetAsync(last_del, 0xff, sizeof(int32_t) * (size_t)G, s));
+  CK(cudaMemsetAsync(last_set, 0xff, sizeof(int32_t) * (size_t)G, s));
+  k_prop_scatter_ord<<<grid_for(NP, 256, c->sm_count), 256, 0, s>>>(NP, tv, ord);
+  k_prop_last<<<grid_for(NP, 256, c->sm_count), 256, 0, s>>>(NP, pk, pg, ord, last_del, last_set);
+  unsigned long long *cnt, h_cnt[2] = {0, 0};
+  CKR(ar.alloc(&cnt, 2));
+  CK(cudaMemsetAsync(cnt, 0, 16, s));
+  k_prop_counts<<<grid_for(std::max(NP, G), 256, c->sm_count), 256, 0, s>>>(NP, pk, kEvPropObj, G, last_del, last_set, cnt);
+  c->launches += 3;
+  CKR(mail_fetch(c, h_cnt, cnt, 16));
+  CKR(mail_wait(c));
+  const long long Q = (long long)h_cnt[0];
+  lg->n_prop_items = (long long)h_cnt[1];
+  // members of the properties objects of $set / $unset events; the verdict names the line
+  uint32_t *qi;
+  CKR(event_partition(c, ar, NP, pk, kEvPropObj, nullptr, 0, &qi));
+  long long *qb, *qe, *mcnt, *moff;
+  unsigned long long *err, h_err = 0;
+  CKR(ar.alloc(&qb, std::max<long long>(Q, 1)));
+  CKR(ar.alloc(&qe, std::max<long long>(Q, 1)));
+  CKR(ar.alloc(&mcnt, Q + 1));
+  CKR(ar.alloc(&moff, Q + 1));
+  CKR(ar.alloc(&err, 1));
+  CK(cudaMemsetAsync(mcnt + Q, 0, 8, s));
+  CK(cudaMemsetAsync(err, 0xff, 8, s));
+  long long M = 0;
+  if (Q > 0) {
+    k_prop_spans<<<grid_for(Q, 256, c->sm_count), 256, 0, s>>>(Q, qi, pl, sb, span, qb, qe);
+    k_json_members<<<grid_for(Q * 32, 256, c->sm_count), 256, 0, s>>>(Q, qb, qe, bb, MemberSink<false>{mcnt, nullptr, nullptr}, err);
+    c->launches += 2;
+  }
+  CKR(exclusive_sum_i64(c, ar, mcnt, moff, Q + 1));
+  CKR(mail_fetch(c, &h_err, err, 8));
+  CKR(mail_fetch(c, &M, moff + Q, 8));
+  CKR(mail_wait(c));
+  if (h_err != ~0ULL) {
+    uint32_t q = 0, line = 0;
+    CK(cudaMemcpy(&q, qi + (h_err >> 8), 4, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(&line, pl + q, 4, cudaMemcpyDeviceToHost));
+    return event_error(((unsigned long long)line << 8) | (h_err & 0xff));
+  }
+  if (M + G >= 0x7fffffffLL) return set_error(CCO_E_UNSUPPORTED, "%lld property members, at most 2^31 - 2 with the items", M);
+  JMember *mem;
+  uint32_t *mev;
+  int32_t *mf;
+  CKR(ar.alloc(&mem, std::max<long long>(M, 1)));
+  CKR(ar.alloc(&mev, std::max<long long>(M, 1)));
+  CKR(ar.alloc(&mf, std::max<long long>(M, 1)));
+  if (M > 0) {
+    k_json_members<<<grid_for(Q * 32, 256, c->sm_count), 256, 0, s>>>(Q, qb, qe, bb, MemberSink<true>{nullptr, moff, mem}, err);
+    k_prop_member_event<<<grid_for(Q, 256, c->sm_count), 256, 0, s>>>(Q, moff, qi, mev);
+    c->launches += 2;
+  }
+  // field names decoded and grouped exactly; the few distinct ones go to the host once
+  DevStrCol nm;
+  long long nm_bytes = 0;
+  CKR(json_decode(c, ar, M, mem, bb, &nm, &nm_bytes));
+  str_hash(c, nm, ~0ULL);
+  StrTable ft;
+  CKR(str_group(c, ar, nm, nullptr, false, 0, &ft, mf));
+  const long long NF = ft.n_groups;
+  cco_dictionary_t fd;
+  CKR(str_dictionary(c, ar, nm, ft, &fd));
+  CK(cudaStreamSynchronize(s));
+  std::vector<std::string> fname;
+  for (long long f = 0; f < NF; ++f) fname.emplace_back(fd.bytes + fd.offsets[f], (size_t)(fd.offsets[f + 1] - fd.offsets[f]));
+  c->pinned_put((void *)fd.offsets);
+  c->pinned_put((void *)fd.bytes);
+  // members in (eventTime, line, member) order, then stably by (item, field) with one presence entry per item last
+  const long long N = M + G;
+  uint32_t *k1, *v1, *v2;
+  unsigned long long *k2;
+  CKR(ar.alloc(&k1, std::max<long long>(M, 1)));
+  CKR(ar.alloc(&v1, std::max<long long>(M, 1)));
+  CKR(ar.alloc(&k2, N + 1));
+  CKR(ar.alloc(&v2, N + 1));
+  if (M > 0) {
+    k_prop_keys1<<<grid_for(M, 256, c->sm_count), 256, 0, s>>>(M, mev, ord, k1, v1);
+    c->launches++;
+    CKR(sort_pairs(c, ar, M, &k1, &v1, bits_for(NP)));
+  }
+  k_prop_keys2<<<grid_for(N, 256, c->sm_count), 256, 0, s>>>(M, G, v1, mev, pg, mf, k2, v2);
+  c->launches++;
+  CKR(sort_pairs(c, ar, N, &k2, &v2, 32 + bits_for(G)));
+  uint32_t *keep, *pos, *has;
+  CKR(ar.alloc(&keep, N + 1));
+  CKR(ar.alloc(&pos, N + 1));
+  CKR(ar.alloc(&has, G));
+  CK(cudaMemsetAsync(has, 0, sizeof(uint32_t) * (size_t)G, s));
+  CK(cudaMemsetAsync(keep + N, 0, 4, s));
+  k_prop_win<<<grid_for(N, 256, c->sm_count), 256, 0, s>>>(M, G, k2, v2, mev, pk, ord, last_del, keep, has);
+  k_prop_presence<<<grid_for(N, 256, c->sm_count), 256, 0, s>>>(M, G, k2, last_del, last_set, has, keep);
+  c->launches += 2;
+  CKR(exclusive_sum_u32(c, ar, keep, pos, N + 1));
+  uint32_t T = 0;
+  CKR(mail_fetch(c, &T, pos + N, 4));
+  CKR(mail_wait(c));
+  lg->n_triples = T;
+  if (T == 0) return CCO_OK;
+  uint32_t *titem, *first;
+  int32_t *tfield;
+  long long *vb, *ve;
+  CKR(ar.alloc(&titem, T));
+  CKR(ar.alloc(&tfield, T));
+  CKR(ar.alloc(&vb, T));
+  CKR(ar.alloc(&ve, T));
+  CKR(ar.alloc(&first, NF + 1));
+  CK(cudaMemsetAsync(first, 0xff, sizeof(uint32_t) * (size_t)(NF + 1), s));
+  k_prop_triples<<<grid_for(N, 256, c->sm_count), 256, 0, s>>>(M, G, keep, pos, k2, v2, mev, it.first_sorted, mem, (int32_t)NF, titem, tfield,
+                                                             vb, ve, first);
+  c->launches++;
+  // field numbers by first appearance in the triples; the presence field is "id" (a property of that name included)
+  std::vector<uint32_t> h_first((size_t)NF + 1);
+  CK(cudaMemcpyAsync(h_first.data(), first, sizeof(uint32_t) * h_first.size(), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  long long f_id = NF;
+  for (long long f = 0; f < NF; ++f)
+    if (fname[f] == "id") f_id = f;
+  h_first[f_id] = std::min(h_first[f_id], h_first[NF]);
+  std::vector<long long> used;
+  for (long long f = 0; f < NF; ++f)
+    if (h_first[f] != ~0u) used.push_back(f);
+  if (f_id == NF && h_first[NF] != ~0u) used.push_back(NF);
+  std::sort(used.begin(), used.end(), [&](long long a, long long b) { return h_first[a] < h_first[b]; });
+  std::vector<int32_t> remap((size_t)NF + 1, 0);
+  lg->field_names.clear();
+  for (size_t k = 0; k < used.size(); ++k) {
+    remap[used[k]] = (int32_t)k;
+    lg->field_names.push_back(used[k] == NF ? std::string("id") : fname[used[k]]);
+  }
+  remap[NF] = remap[f_id];
+  lg->n_prop_fields = (long long)used.size() - (f_id == NF && h_first[NF] != ~0u ? 1 : 0);
+  int32_t *d_remap;
+  CKR(ar.alloc(&d_remap, NF + 1));
+  CK(cudaMemcpyAsync(d_remap, remap.data(), sizeof(int32_t) * remap.size(), cudaMemcpyHostToDevice, s));
+  k_remap_i32<<<grid_for(T, 256, c->sm_count), 256, 0, s>>>(T, d_remap, tfield);
+  // value texts and item ids of the triples as columns (offsets from 0)
+  long long *len, *voff, *ioff, vtotal = 0, itotal = 0;
+  CKR(ar.alloc(&len, (long long)T + 1));
+  CKR(ar.alloc(&voff, (long long)T + 1));
+  CKR(ar.alloc(&ioff, (long long)T + 1));
+  CK(cudaMemsetAsync(len + T, 0, 8, s));
+  k_prop_value_len<<<grid_for(T, 256, c->sm_count), 256, 0, s>>>(T, vb, ve, len);
+  CKR(exclusive_sum_i64(c, ar, len, voff, (long long)T + 1));
+  k_str_dict_len<<<grid_for(T, 256, c->sm_count), 256, 0, s>>>(T, titem, pcol.off, len);
+  CKR(exclusive_sum_i64(c, ar, len, ioff, (long long)T + 1));
+  c->launches += 3;
+  CKR(mail_fetch(c, &vtotal, voff + T, 8));
+  CKR(mail_fetch(c, &itotal, ioff + T, 8));
+  CKR(mail_wait(c));
+  unsigned char *vals, *ibytes;
+  CKR(ar.alloc(&vals, std::max<long long>(vtotal, 1)));
+  CKR(ar.alloc(&ibytes, std::max<long long>(itotal, 1)));
+  k_prop_value_copy<<<grid_for(T, 256, c->sm_count), 256, 0, s>>>(T, vb, voff, bb, vals);
+  k_str_dict_gather<<<grid_for(T, 256, c->sm_count), 256, 0, s>>>(T, titem, pcol.off, 0, (const unsigned char *)pcol.w, ioff, ibytes);
+  c->launches += 2;
+  for (void *p : {(void *)tfield, (void *)voff, (void *)vals, (void *)ioff, (void *)ibytes}) CKR(log_keep(ar, lg, p));
+  lg->p_field = tfield;
+  lg->p_voff = voff;
+  lg->p_vals = vals;
+  lg->p_ioff = ioff;
+  lg->p_ibytes = ibytes;
+  lg->p_ibytes_n = itotal;
+  return CCO_OK;
+}
+
+static int event_log_read(cco_ctx *c, const char *bytes, int64_t len, cco_event_log **out) {
+  CK(cudaSetDevice(c->device));
+  cudaStream_t s = c->stream;
+  nvtx_push("cco:event_log_read");
+  struct Pop { ~Pop() { nvtx_pop(); } } pop;
+  mail_reset(c);
+  Arena ar(s);
+  cco_event_log *lg = new cco_event_log();
+  lg->ctx = c;
+  struct G {
+    cco_event_log *l;
+    bool ok = false;
+    ~G() {
+      if (!ok) event_log_release(l);
+    }
+  } g{lg};
+  lg->name_off.assign(1, 0);
+  lg->train_at.assign(1, 0);
+  lg->rank_at.assign(1, 0);
+  // 1. the export, once, into 8-byte words with 16 bytes of zero padding
+  const long long NW = (len + 7) / 8;
+  uint64_t *w;
+  CKR(ar.alloc(&w, NW + 2));
+  CK(cudaMemsetAsync(w + len / 8, 0, sizeof(uint64_t) * (size_t)(NW + 2 - len / 8), s));
+  if (len > 0) CK(cudaMemcpyAsync(w, bytes, (size_t)len, cudaMemcpyHostToDevice, s));
+  const unsigned char *bb = (const unsigned char *)w;
+  // 2. lines: every '\n' ends one; a last line without it ends at len
+  long long L = 0;
+  const bool open_tail = len > 0 && bytes[len - 1] != '\n';
+  long long *nl;
+  long long n_chunks = (NW + kNlChunkWords - 1) / kNlChunkWords;
+  long long *cc, *coff;
+  CKR(ar.alloc(&cc, n_chunks + 1));
+  CKR(ar.alloc(&coff, n_chunks + 1));
+  CK(cudaMemsetAsync(cc + n_chunks, 0, 8, s));
+  if (NW > 0) {
+    k_nl_count<<<grid_for(n_chunks * 32, 256, c->sm_count), 256, 0, s>>>(NW, w, cc);
+    c->launches++;
+  }
+  CKR(exclusive_sum_i64(c, ar, cc, coff, n_chunks + 1));
+  CKR(mail_fetch(c, &L, coff + n_chunks, 8));
+  CKR(mail_wait(c));
+  if (L + (open_tail ? 1 : 0) > 0x7fffffffLL) return set_error(CCO_E_UNSUPPORTED, "%lld lines, at most 2^31 - 1", L + (open_tail ? 1 : 0));
+  CKR(ar.alloc(&nl, L + 1));
+  if (L > 0) {
+    k_nl_write<<<grid_for(n_chunks * 32, 256, c->sm_count), 256, 0, s>>>(NW, w, coff, nl);
+    c->launches++;
+  }
+  const long long end_pos = len;
+  if (open_tail) {
+    CK(cudaMemcpyAsync(nl + L, &end_pos, 8, cudaMemcpyHostToDevice, s));
+    ++L;
+  }
+  lg->n_lines = L;
+  if (L == 0) {
+    CK(cudaStreamSynchronize(s));
+    g.ok = true;
+    *out = lg;
+    return CCO_OK;
+  }
+  long long *sb, *se;
+  CKR(ar.alloc(&sb, L));
+  CKR(ar.alloc(&se, L));
+  k_line_spans<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, nl, sb, se);
+  c->launches++;
+  // 3. the seven members an event is read through; the tokenizer's verdict comes before anything reads the spans
+  int2 *span;
+  unsigned long long *err, h_err = 0;
+  CKR(ar.alloc(&span, L * kEvSlots));
+  CKR(ar.alloc(&err, 1));
+  CK(cudaMemsetAsync(span, 0xff, sizeof(int2) * (size_t)L * kEvSlots, s));
+  CK(cudaMemsetAsync(err, 0xff, 8, s));
+  k_json_members<<<grid_for(L * 32, 256, c->sm_count), 256, 0, s>>>(L, sb, se, bb, EventSink{span, bb}, err);
+  c->launches++;
+  CKR(mail_fetch(c, &h_err, err, 8));
+  CKR(mail_wait(c));
+  if (h_err != ~0ULL) return event_error(h_err);
+  // 4. types, times, selection
+  uint8_t *flag;
+  long long *tm;
+  CKR(ar.alloc(&flag, L));
+  CKR(ar.alloc(&tm, L));
+  k_event_check<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, sb, span, bb, flag, tm, err);
+  c->launches++;
+  CKR(mail_fetch(c, &h_err, err, 8));
+  CKR(mail_wait(c));
+  if (h_err != ~0ULL) return event_error(h_err);
+  // 5. event names: decoded, grouped exactly, numbered by first appearance; the few distinct ones go to the host
+  JMember *jm;
+  CKR(ar.alloc(&jm, L));
+  k_event_strings<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, nullptr, kEvName, sb, span, bb, jm);
+  c->launches++;
+  DevStrCol names;
+  long long name_bytes = 0;
+  CKR(json_decode(c, ar, L, jm, bb, &names, &name_bytes));
+  ar.release(jm);
+  str_hash(c, names, ~0ULL);
+  int32_t *code;
+  CKR(ar.alloc(&code, L));
+  StrTable nt;
+  CKR(str_group(c, ar, names, nullptr, false, 0, &nt, code));
+  const long long NG = nt.n_groups;
+  cco_dictionary_t nd;
+  CKR(str_dictionary(c, ar, names, nt, &nd));
+  CK(cudaStreamSynchronize(s));
+  lg->name_off.assign(nd.offsets, nd.offsets + NG + 1);
+  lg->name_bytes.assign(nd.bytes, (size_t)nd.offsets[NG]);
+  c->pinned_put((void *)nd.offsets);
+  c->pinned_put((void *)nd.bytes);
+  str_table_release(ar, nt);
+  str_release(ar, names);
+  // 6. counts per name
+  unsigned long long *cnt;
+  CKR(ar.alloc(&cnt, 2 * NG + 2));
+  CK(cudaMemsetAsync(cnt, 0, sizeof(unsigned long long) * (size_t)(2 * NG + 2), s));
+  k_event_counts<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, flag, code, (int32_t)NG, cnt);
+  c->launches++;
+  std::vector<unsigned long long> h_cnt((size_t)(2 * NG + 2));
+  CK(cudaMemcpyAsync(h_cnt.data(), cnt, sizeof(unsigned long long) * h_cnt.size(), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  lg->n_train.resize(NG);
+  lg->n_rank.resize(NG);
+  lg->train_at.assign(NG + 1, 0);
+  lg->rank_at.assign(NG + 1, 0);
+  for (long long n = 0; n < NG; ++n) {
+    lg->n_train[n] = (int64_t)h_cnt[2 * n];
+    lg->n_rank[n] = (int64_t)h_cnt[2 * n + 1];
+    if (h_cnt[2 * n + 1] >= 0x7fffffffULL)
+      return set_error(CCO_E_UNSUPPORTED, "event name %lld: %llu events, at most 2^31 - 2 per name", n, h_cnt[2 * n + 1]);
+    lg->train_at[n + 1] = lg->train_at[n] + lg->n_train[n];
+    lg->rank_at[n + 1] = lg->rank_at[n] + lg->n_rank[n];
+  }
+  lg->n_prop = (long long)h_cnt[2 * NG];
+  lg->n_ignored = (long long)h_cnt[2 * NG + 1];
+  // 7. training and ranking events partitioned by name, file order inside a name: decoded ids and times
+  uint32_t *idx;
+  CKR(event_partition(c, ar, L, flag, kEvTraining, code, (uint32_t)NG, &idx));
+  CKR(event_column(c, ar, lg, lg->train_at[NG], idx, kEvEntityId, sb, span, bb, lg->train_at, &lg->tu));
+  CKR(event_column(c, ar, lg, lg->train_at[NG], idx, kEvTargetId, sb, span, bb, lg->train_at, &lg->ti));
+  ar.release(idx);
+  CKR(event_partition(c, ar, L, flag, kEvRanking, code, (uint32_t)NG, &idx));
+  const long long NR = lg->rank_at[NG];
+  CKR(event_column(c, ar, lg, NR, idx, kEvTargetId, sb, span, bb, lg->rank_at, &lg->ri));
+  CKR(ar.alloc(&lg->rtime, std::max<long long>(NR, 1)));
+  CKR(log_keep(ar, lg, lg->rtime));
+  if (NR > 0) {
+    k_gather_i64<<<grid_for(NR, 256, c->sm_count), 256, 0, s>>>(NR, idx, tm, lg->rtime);
+    c->launches++;
+  }
+  ar.release(idx);
+  // 8. the items' properties (PEventStore.aggregateProperties), aggregated here: see event_properties
+  if (lg->n_prop > 0) CKR(event_properties(c, ar, lg, L, flag, tm, sb, span, bb));
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  g.ok = true;
+  *out = lg;
+  return CCO_OK;
+}
+
+// the rankings of cco_format_model_log / cco_rerank_model_log as cco_ranking_t (no host streams) + the log's streams
+static int log_rankings(const cco_event_log *lg, int32_t n_rank, const cco_log_ranking_t *lr, std::vector<cco_ranking_t> *rk, LogStreams *ls) {
+  if (n_rank < 0 || (n_rank > 0 && !lr)) return set_error(CCO_E_INVALID_ARG, "bad rankings");
+  rk->assign((size_t)std::max(n_rank, 0), cco_ranking_t{});
+  ls->assign((size_t)std::max(n_rank, 0), {});
+  const int NG = (int)lg->n_rank.size();
+  for (int k = 0; k < n_rank; ++k) {
+    const cco_log_ranking_t &r = lr[k];
+    (*rk)[k] = cco_ranking_t{r.name, r.mode, 0, r.start_ms, r.end_ms, nullptr};
+    std::vector<int> codes;
+    if (r.mode == CCO_POP_RANDOM) {   // calcRandom reads every event name
+      for (int g = 0; g < NG; ++g) codes.push_back(g);
+    } else {
+      if (r.n_event_names < 0 || (r.n_event_names > 0 && !r.event_names)) return set_error(CCO_E_INVALID_ARG, "ranking %d: bad event names", k);
+      for (int q = 0; q < r.n_event_names; ++q) {
+        if (!r.event_names[q]) return set_error(CCO_E_INVALID_ARG, "ranking %d: null event name", k);
+        codes.push_back(lg->code_of(r.event_names[q]));
+      }
+    }
+    for (int g : codes) {
+      if (g < 0) continue;   // a name without events: an empty stream
+      LogStream st;
+      st.items.n = lg->n_rank[g];
+      st.items.off = (const int64_t *)(lg->ri.off + lg->rank_at[g]);
+      st.items.bytes = (const char *)lg->ri.w + lg->ri.boff[g];
+      st.items.device = true;
+      st.items.base = lg->ri.boff[g];
+      st.items.nbytes = lg->ri.boff[g + 1] - lg->ri.boff[g];
+      st.time = lg->rtime + lg->rank_at[g];
+      (*ls)[k].push_back(st);
+    }
+    (*rk)[k].n_streams = (int32_t)(*ls)[k].size();
+  }
+  return CCO_OK;
+}
+}  // namespace cco
+
+int cco_event_log_read(cco_ctx_t *ctx, const char *bytes, int64_t len, cco_event_log_t **out) {
+  if (!ctx || !out || len < 0 || (len > 0 && !bytes)) return set_error(CCO_E_INVALID_ARG, "null argument or negative length");
+  *out = nullptr;
+  if (!ctx->members.empty()) return set_error(CCO_E_UNSUPPORTED, "an event log is resident on one GPU: read it on a per-GPU context");
+  return event_log_read(ctx, bytes, len, out);
+}
+
+int cco_event_log_info(const cco_event_log_t *lg, cco_event_log_info_t *out) {
+  if (!lg || !out) return set_error(CCO_E_INVALID_ARG, "null argument");
+  out->n_lines = lg->n_lines;
+  out->names = cco_dictionary_t{(int64_t)lg->n_train.size(), lg->name_off.data(), lg->name_bytes.data()};
+  out->n_training = lg->n_train.data();
+  out->n_ranking = lg->n_rank.data();
+  out->n_property_events = lg->n_prop;
+  out->n_property_items = lg->n_prop_items;
+  out->n_property_fields = lg->n_prop_fields;
+  out->n_ignored = lg->n_ignored;
+  return CCO_OK;
+}
+
+int cco_event_log_ingest(cco_ctx_t *c, const cco_event_log_t *lg, int32_t n_names, const char *const *names, int32_t min_events_per_user,
+                         cco_dataset_t **out) {
+  if (!c || !lg || !names || !out || n_names < 1) return set_error(CCO_E_INVALID_ARG, "bad argument");
+  *out = nullptr;
+  if (!c->members.empty() || lg->ctx != c) return set_error(CCO_E_UNSUPPORTED, "ingest a log on the per-GPU context that read it");
+  std::vector<int> codes(n_names);
+  for (int t = 0; t < n_names; ++t) {
+    if (!names[t]) return set_error(CCO_E_INVALID_ARG, "null event name %d", t);
+    codes[t] = lg->code_of(names[t]);
+  }
+  const StrColumns view = [lg, &codes](Arena &ar, int t, DevStrCol *uc, DevStrCol *ic) -> int {
+    const int g = codes[t];
+    const long long n = g >= 0 ? lg->n_train[g] : 0;
+    *uc = lg->view(lg->tu, g, lg->train_at, n);
+    *ic = lg->view(lg->ti, g, lg->train_at, n);
+    CKR(ar.alloc(&uc->hash, std::max<long long>(n, 1)));
+    CKR(ar.alloc(&ic->hash, std::max<long long>(n, 1)));
+    return CCO_OK;
+  };
+  return ingest_strings_core(c, n_names, view, min_events_per_user, out);
+}
+
+namespace cco {
+// the log's aggregated properties as format_model takes them: a host shell (count, field names) + the device columns
+struct LogProps {
+  std::vector<const char *> names;
+  cco_item_properties_t shell;
+  DevProps dev;
+};
+static void log_props(const cco_event_log *lg, LogProps *p) {
+  for (const std::string &f : lg->field_names) p->names.push_back(f.c_str());
+  p->shell = cco_item_properties_t{lg->n_triples, nullptr, nullptr, nullptr, nullptr, nullptr, (int32_t)p->names.size(), p->names.data()};
+  p->dev.items = KeySection{lg->n_triples, (const int64_t *)lg->p_ioff, (const char *)lg->p_ibytes, true, lg->p_ibytes_n, 0};
+  p->dev.field = lg->p_field;
+  p->dev.voff = lg->p_voff;
+  p->dev.vals = lg->p_vals;
+}
+}  // namespace cco
+
+int cco_format_model_log(cco_ctx_t *ctx, const cco_result_t *res, int32_t n_names, const char *const *names,
+                         const cco_dictionary_t *row_ids, const cco_dictionary_t *col_ids, const cco_event_log_t *lg, int32_t n_rankings,
+                         const cco_log_ranking_t *rankings, char **out_bytes, int64_t *out_len) {
+  if (!ctx || !lg) return set_error(CCO_E_INVALID_ARG, "null argument");
+  if (!ctx->members.empty() || lg->ctx != ctx) return set_error(CCO_E_UNSUPPORTED, "format on the per-GPU context that read the log");
+  std::vector<cco_ranking_t> rk;
+  LogStreams ls;
+  CKR(log_rankings(lg, n_rankings, rankings, &rk, &ls));
+  LogProps lp;
+  log_props(lg, &lp);
+  const bool any = lg->n_triples > 0;
+  return format_model(ctx, res, n_names, names, row_ids, col_ids, any ? &lp.shell : nullptr, n_rankings, rk.data(), out_bytes, out_len,
+                      "cco:format_model_log", &ls, any ? &lp.dev : nullptr);
+}
+
+int cco_rerank_model_log(cco_ctx_t *ctx, const char *body, int64_t body_len, const cco_event_log_t *lg, int32_t n_rankings,
+                         const cco_log_ranking_t *rankings, char **out_bytes, int64_t *out_len) {
+  if (!ctx || !lg) return set_error(CCO_E_INVALID_ARG, "null argument");
+  if (!ctx->members.empty() || lg->ctx != ctx) return set_error(CCO_E_UNSUPPORTED, "rerank on the per-GPU context that read the log");
+  std::vector<cco_ranking_t> rk;
+  LogStreams ls;
+  CKR(log_rankings(lg, n_rankings, rankings, &rk, &ls));
+  LogProps lp;
+  log_props(lg, &lp);
+  const bool any = lg->n_triples > 0;
+  return rerank_model(ctx, body, body_len, any ? &lp.shell : nullptr, n_rankings, rk.data(), out_bytes, out_len, &ls, any ? &lp.dev : nullptr);
+}
+
+int cco_event_log_free(cco_event_log_t *lg) {
+  event_log_release(lg);
+  return CCO_OK;
 }
 
 // ---- SURVEY.md 8f-3: PopModel rank histograms -------------------------------------------------------------------------

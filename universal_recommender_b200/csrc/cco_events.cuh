@@ -1,0 +1,384 @@
+// cco_events.cuh -- a PredictionIO event export (`pio export`: JSON lines, one event per line) parsed on the device
+// (cco_event_log_read), the DataSource of the reference (DataSource.scala:65-102) without its event store.
+//   k_json_members + EventSink     the tokenizer of cco_json.cuh with a sink that keeps, per line, the value spans of the
+//                                  seven members an event is read through (the last of a repeated name), nothing else
+//   k_event_check                  per line: member types, eventTime -> epoch ms, the selection (training / ranking /
+//                                  property event) and the empty-id rule, verdict into the error word
+//   k_event_strings                the inside of one member's string per line (or per listed line) as JMember spans for
+//                                  k_json_unescape
+//   k_event_keys / k_event_counts  partition keys by event name, per-name counts of training and ranking events
+//   k_prop_*                       PEventStore.aggregateProperties of the items' $set / $unset / $delete events: the
+//                                  (eventTime, line) order, the last $delete and $set per item, the members of the
+//                                  properties objects sorted by (item, field) after that order, the winning member per
+//                                  (item, field), one presence entry per item left without a field, the triples
+#pragma once
+
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+namespace cco {
+
+// the members of an event line that are read; every other member is skipped
+enum : int { kEvName = 0, kEvEntityType, kEvEntityId, kEvTargetType, kEvTargetId, kEvTime, kEvProps, kEvSlots };
+// error codes of an event line (after the tokenizer's kJson* codes)
+enum : unsigned { kEvMissing = 6, kEvType = 7, kEvTime_ = 8, kEvEmptyId = 9, kEvTarget = 10 };
+// line flags
+enum : uint8_t { kEvTraining = 1, kEvRanking = 2, kEvProperty = 4, kEvSet = 8, kEvUnset = 16, kEvDelete = 32, kEvPropObj = 64 };
+
+// the next decoded unit of the raw string bytes [q, e) (escapes validated by the tokenizer): a code point for an escape,
+// else the raw byte (a UTF-8 lead or continuation byte is >= 0x80 and never equals an ASCII unit)
+__device__ __forceinline__ unsigned json_next_unit(const unsigned char *__restrict__ body, long long &q) {
+  const unsigned c = body[q];
+  if (c != '\\') {
+    ++q;
+    return c;
+  }
+  const unsigned x = body[q + 1];
+  if (x != 'u') {
+    q += 2;
+    return x == 'b' ? 8 : x == 'f' ? 12 : x == 'n' ? 10 : x == 'r' ? 13 : x == 't' ? 9 : x;
+  }
+  const unsigned cp = json_hex4(body + q + 2);
+  q += 6;
+  return cp;   // a surrogate stays >= 0x80: it never equals an ASCII literal
+}
+// the raw string bytes [q, e) decode to the ASCII literal lit of n bytes
+__device__ __forceinline__ bool json_str_is(const unsigned char *__restrict__ body, long long q, long long e, const char *lit, int n) {
+  for (int k = 0; k < n; ++k) {
+    if (q >= e || json_next_unit(body, q) != (unsigned char)lit[k]) return false;
+  }
+  return q == e;
+}
+
+__device__ __forceinline__ int event_slot(const unsigned char *__restrict__ body, long long nb, long long ne) {
+  if (json_str_is(body, nb, ne, "event", 5)) return kEvName;
+  if (json_str_is(body, nb, ne, "entityType", 10)) return kEvEntityType;
+  if (json_str_is(body, nb, ne, "entityId", 8)) return kEvEntityId;
+  if (json_str_is(body, nb, ne, "targetEntityType", 16)) return kEvTargetType;
+  if (json_str_is(body, nb, ne, "targetEntityId", 14)) return kEvTargetId;
+  if (json_str_is(body, nb, ne, "eventTime", 9)) return kEvTime;
+  if (json_str_is(body, nb, ne, "properties", 10)) return kEvProps;
+  return -1;
+}
+// span[l * kEvSlots + k] = value of member k of line l relative to the line's first byte, {-1, -1} when absent (memset
+// by the caller); members arrive in order, so the last of a repeated name wins
+struct EventSink {
+  int2 *span;
+  const unsigned char *body;
+  __device__ void member(long long s, long long, long long b, const JMember &m) const {
+    const int k = event_slot(body, m.nb, m.ne);
+    if (k >= 0) span[s * kEvSlots + k] = make_int2((int)(m.vb - b), (int)(m.ve - b));
+  }
+  __device__ void end(long long, long long) const {}
+};
+
+// the value [vb, ve) is exactly one string
+__device__ __forceinline__ bool json_is_string(const unsigned char *__restrict__ body, long long vb, long long ve) {
+  if (ve - vb < 2 || body[vb] != '"') return false;
+  long long q = vb + 1;
+  while (q < ve - 1) {
+    if (body[q] == '\\') q += 2;
+    else if (body[q] == '"') return false;
+    else ++q;
+  }
+  return q == ve - 1 && body[q] == '"';
+}
+__device__ __forceinline__ bool json_is_null(const unsigned char *__restrict__ body, long long vb, long long ve) {
+  return ve - vb == 4 && body[vb] == 'n' && body[vb + 1] == 'u' && body[vb + 2] == 'l' && body[vb + 3] == 'l';
+}
+
+// Joda's extended date-time YYYY-MM-DDThh:mm:ss[.f{1,9}](Z|+hh:mm|+hhmm|+hh) (sign + or -), proleptic Gregorian,
+// years 0000-9999 -> epoch milliseconds; fraction digits past the third are dropped (a floor: the fraction is positive)
+__device__ __forceinline__ long long days_from_civil(long long y, unsigned m, unsigned d) {
+  y -= m <= 2;
+  const long long era = (y >= 0 ? y : y - 399) / 400;
+  const unsigned yoe = (unsigned)(y - era * 400);
+  const unsigned doy = (153 * (m + (m > 2 ? -3 : 9)) + 2) / 5 + d - 1;
+  const unsigned doe = yoe * 365 + yoe / 4 - yoe / 100 + doy;
+  return era * 146097 + (long long)doe - 719468;
+}
+__device__ __noinline__ bool parse_event_time(const unsigned char *__restrict__ body, long long q, long long e, long long *ms) {
+  char t[40];
+  int n = 0;
+  while (q < e) {
+    if (n == 40) return false;
+    const unsigned u = json_next_unit(body, q);
+    if (u >= 0x80) return false;
+    t[n++] = (char)u;
+  }
+  auto dig = [&](int i, int k, int *v) {
+    int x = 0;
+    for (int j = i; j < i + k; ++j) {
+      if (j >= n || t[j] < '0' || t[j] > '9') return false;
+      x = x * 10 + (t[j] - '0');
+    }
+    *v = x;
+    return true;
+  };
+  int Y, M, D, h, mi, s;
+  if (n < 20 || !dig(0, 4, &Y) || t[4] != '-' || !dig(5, 2, &M) || t[7] != '-' || !dig(8, 2, &D) || t[10] != 'T' || !dig(11, 2, &h) ||
+      t[13] != ':' || !dig(14, 2, &mi) || t[16] != ':' || !dig(17, 2, &s))
+    return false;
+  const bool leap = Y % 4 == 0 && (Y % 100 != 0 || Y % 400 == 0);
+  const int mdays = M == 2 ? (leap ? 29 : 28) : (M == 4 || M == 6 || M == 9 || M == 11) ? 30 : 31;
+  if (M < 1 || M > 12 || D < 1 || D > mdays || h > 23 || mi > 59 || s > 59) return false;
+  int i = 19, frac = 0;
+  if (t[i] == '.') {
+    int k = 0;
+    for (++i; i < n && t[i] >= '0' && t[i] <= '9'; ++i, ++k)
+      if (k < 3) frac = frac * 10 + (t[i] - '0');
+    if (k < 1 || k > 9) return false;
+    for (; k < 3; ++k) frac *= 10;
+  }
+  int off = 0;
+  if (i < n && t[i] == 'Z') {
+    ++i;
+  } else if (i < n && (t[i] == '+' || t[i] == '-')) {
+    const int sign = t[i] == '-' ? -1 : 1;
+    int oh, om = 0;
+    if (!dig(i + 1, 2, &oh)) return false;
+    i += 3;
+    if (i < n && t[i] == ':') {
+      if (!dig(i + 1, 2, &om)) return false;
+      i += 3;
+    } else if (i < n) {
+      if (!dig(i, 2, &om)) return false;
+      i += 2;
+    }
+    if (oh > 23 || om > 59) return false;
+    off = sign * (oh * 60 + om);
+  } else {
+    return false;
+  }
+  if (i != n) return false;
+  *ms = ((days_from_civil(Y, (unsigned)M, (unsigned)D) * 86400 + h * 3600 + mi * 60 + s) - (long long)off * 60) * 1000 + frac;
+  return true;
+}
+
+// per line: types, time, selection; flags and times written for every line, the verdict into err
+__global__ void k_event_check(long long n_lines, const long long *__restrict__ sb, const int2 *__restrict__ span,
+                              const unsigned char *__restrict__ body, uint8_t *__restrict__ flag, long long *__restrict__ time,
+                              unsigned long long *__restrict__ err) {
+  for (long long l = blockIdx.x * (long long)blockDim.x + threadIdx.x; l < n_lines; l += (long long)gridDim.x * blockDim.x) {
+    const long long b = sb[l];
+    const int2 *sp = span + l * kEvSlots;
+    unsigned code = 0;
+    auto vb = [&](int k) { return b + sp[k].x; };
+    auto ve = [&](int k) { return b + sp[k].y; };
+    auto present = [&](int k) { return sp[k].x >= 0; };
+    auto str = [&](int k) { return present(k) && json_is_string(body, vb(k), ve(k)); };
+    // an optional string: absent or null counts as absent
+    auto opt = [&](int k) { return present(k) && !json_is_null(body, vb(k), ve(k)); };
+    for (int k : {kEvName, kEvEntityType, kEvEntityId, kEvTime})
+      if (!code && !present(k)) code = kEvMissing;
+    for (int k : {kEvName, kEvEntityType, kEvEntityId, kEvTime})
+      if (!code && !str(k)) code = kEvType;
+    for (int k : {kEvTargetType, kEvTargetId})
+      if (!code && opt(k) && !str(k)) code = kEvType;
+    if (!code && present(kEvProps) && (body[vb(kEvProps)] != '{' || body[ve(kEvProps) - 1] != '}')) code = kEvType;
+    if (!code && opt(kEvTargetType) != opt(kEvTargetId)) code = kEvTarget;
+    long long tm = 0;
+    if (!code && !parse_event_time(body, vb(kEvTime) + 1, ve(kEvTime) - 1, &tm)) code = kEvTime_;
+    uint8_t f = 0;
+    if (!code) {
+      const bool target = opt(kEvTargetId);
+      const long long etb = vb(kEvEntityType) + 1, ete = ve(kEvEntityType) - 1;
+      if (target) {
+        f |= kEvRanking;
+        const bool train = json_str_is(body, etb, ete, "user", 4) &&
+                           json_str_is(body, vb(kEvTargetType) + 1, ve(kEvTargetType) - 1, "item", 4);
+        if (train) {
+          f |= kEvTraining;
+          if (ve(kEvEntityId) - vb(kEvEntityId) == 2 || ve(kEvTargetId) - vb(kEvTargetId) == 2) code = kEvEmptyId;
+        }
+      }
+      const long long nb = vb(kEvName) + 1, ne = ve(kEvName) - 1;
+      if (json_str_is(body, etb, ete, "item", 4)) {
+        const uint8_t kind = json_str_is(body, nb, ne, "$set", 4) ? kEvSet : json_str_is(body, nb, ne, "$unset", 6) ? kEvUnset
+                             : json_str_is(body, nb, ne, "$delete", 7) ? kEvDelete : 0;
+        if (kind) f |= kEvProperty | kind | (kind != kEvDelete && present(kEvProps) ? kEvPropObj : 0);
+      }
+    }
+    if (code) atomicMin(err, ((unsigned long long)l << 8) | code);
+    flag[l] = f;
+    time[l] = tm;
+  }
+}
+
+// out[i] = the inside of member k's string of line idx[i] (idx == nullptr: line i); absent or null -> empty
+__global__ void k_event_strings(long long n, const uint32_t *__restrict__ idx, int k, const long long *__restrict__ sb,
+                                const int2 *__restrict__ span, const unsigned char *__restrict__ body, JMember *__restrict__ out) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const long long l = idx ? (long long)idx[i] : i;
+    const int2 v = span[l * kEvSlots + k];
+    const bool s = v.x >= 0 && body[sb[l] + v.x] == '"';
+    out[i] = s ? JMember{sb[l] + v.x + 1, sb[l] + v.y - 1, 0, 0} : JMember{0, 0, 0, 0};
+  }
+}
+
+// key[l] = the line's event name code (code == nullptr: 0) if it carries flag bit `want`, else `past` (sorted after them)
+__global__ void k_event_keys(long long n_lines, const uint8_t *__restrict__ flag, uint8_t want, const int32_t *__restrict__ code,
+                             uint32_t past, uint32_t *__restrict__ key, uint32_t *__restrict__ line) {
+  for (long long l = blockIdx.x * (long long)blockDim.x + threadIdx.x; l < n_lines; l += (long long)gridDim.x * blockDim.x) {
+    key[l] = (flag[l] & want) ? (code ? (uint32_t)code[l] : 0u) : past;
+    line[l] = (uint32_t)l;
+  }
+}
+// cnt[2 g] += training events of name g, cnt[2 g + 1] += ranking events; cnt[2 n_names] += property events, cnt[2 n_names
+// + 1] += ignored lines.  Lanes of a warp that add to the same counter add once (__match_any_sync).
+__global__ void k_event_counts(long long n_lines, const uint8_t *__restrict__ flag, const int32_t *__restrict__ code, int32_t n_names,
+                               unsigned long long *__restrict__ cnt) {
+  const int lane = threadIdx.x & 31;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long base = blockIdx.x * (long long)blockDim.x; base < n_lines; base += stride) {
+    const long long l = base + threadIdx.x;
+    const uint8_t f = l < n_lines ? flag[l] : 0;
+    const int g = l < n_lines ? code[l] : -1;
+    for (int k = 0; k < 4; ++k) {
+      int slot = -1;
+      if (l < n_lines) {
+        if (k == 0 && (f & kEvTraining)) slot = 2 * g;
+        if (k == 1 && (f & kEvRanking)) slot = 2 * g + 1;
+        if (k == 2 && (f & kEvProperty)) slot = 2 * n_names;
+        if (k == 3 && !f) slot = 2 * n_names + 1;
+      }
+      const unsigned same = __match_any_sync(0xffffffffu, slot);
+      if (slot >= 0 && lane == __ffs(same) - 1) atomicAdd(&cnt[slot], (unsigned long long)__popc(same));
+    }
+  }
+}
+__global__ void k_gather_i64(long long n, const uint32_t *__restrict__ idx, const long long *__restrict__ src, long long *__restrict__ dst) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) dst[i] = src[idx[i]];
+}
+
+
+// ---- property events: PEventStore.aggregateProperties on the device ----------------------------------------------------
+// Property event i (line pl[i], line order) of item group pg[i] at position ord[i] of the (eventTime, line) order.
+__global__ void k_prop_scatter_ord(long long n, const uint32_t *__restrict__ sorted, int32_t *__restrict__ ord) {
+  for (long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x; k < n; k += (long long)gridDim.x * blockDim.x) ord[sorted[k]] = (int32_t)k;
+}
+__global__ void k_prop_time_keys(long long n, const long long *__restrict__ t, unsigned long long *__restrict__ key, uint32_t *__restrict__ val) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    key[i] = (unsigned long long)t[i] ^ 0x8000000000000000ULL;
+    val[i] = (uint32_t)i;
+  }
+}
+// last_del[g] / last_set[g] = the latest position of a $delete / $set of group g (-1: none)
+__global__ void k_prop_last(long long n, const uint8_t *__restrict__ kind, const int32_t *__restrict__ pg, const int32_t *__restrict__ ord,
+                            int32_t *__restrict__ last_del, int32_t *__restrict__ last_set) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    if (kind[i] & kEvDelete) atomicMax(&last_del[pg[i]], ord[i]);
+    if (kind[i] & kEvSet) atomicMax(&last_set[pg[i]], ord[i]);
+  }
+}
+// the properties object of event qi[s] (an index into the property events) as a span of the body
+__global__ void k_prop_spans(long long n, const uint32_t *__restrict__ qi, const uint32_t *__restrict__ pl, const long long *__restrict__ sb,
+                             const int2 *__restrict__ span, long long *__restrict__ b, long long *__restrict__ e) {
+  for (long long s = blockIdx.x * (long long)blockDim.x + threadIdx.x; s < n; s += (long long)gridDim.x * blockDim.x) {
+    const long long l = pl[qi[s]];
+    const int2 v = span[l * kEvSlots + kEvProps];
+    b[s] = sb[l] + v.x;
+    e[s] = sb[l] + v.y;
+  }
+}
+// the property event of each member: mev[m] = qi[s] for m in [moff[s], moff[s + 1])
+__global__ void k_prop_member_event(long long n, const long long *__restrict__ moff, const uint32_t *__restrict__ qi, uint32_t *__restrict__ mev) {
+  for (long long s = blockIdx.x * (long long)blockDim.x + threadIdx.x; s < n; s += (long long)gridDim.x * blockDim.x)
+    for (long long m = moff[s]; m < moff[s + 1]; ++m) mev[m] = qi[s];
+}
+// entries 0 .. M-1: members, keyed (group << 32 | field) and first ordered by the (eventTime, line) position of their event;
+// entries M .. M+G-1: one presence entry per group, keyed (group << 32 | 0xffffffff), after its fields
+__global__ void k_prop_keys1(long long M, const uint32_t *__restrict__ mev, const int32_t *__restrict__ ord, uint32_t *__restrict__ key,
+                             uint32_t *__restrict__ val) {
+  for (long long m = blockIdx.x * (long long)blockDim.x + threadIdx.x; m < M; m += (long long)gridDim.x * blockDim.x) {
+    key[m] = (uint32_t)ord[mev[m]];
+    val[m] = (uint32_t)m;
+  }
+}
+__global__ void k_prop_keys2(long long M, long long G, const uint32_t *__restrict__ by_time, const uint32_t *__restrict__ mev,
+                             const int32_t *__restrict__ pg, const int32_t *__restrict__ mf, unsigned long long *__restrict__ key,
+                             uint32_t *__restrict__ val) {
+  for (long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x; k < M + G; k += (long long)gridDim.x * blockDim.x) {
+    if (k < M) {
+      const uint32_t m = by_time[k];
+      key[k] = ((unsigned long long)(uint32_t)pg[mev[m]] << 32) | (uint32_t)mf[m];
+      val[k] = m;
+    } else {
+      key[k] = ((unsigned long long)(k - M) << 32) | 0xffffffffULL;
+      val[k] = (uint32_t)k;
+    }
+  }
+}
+// a member that ends its (group, field) run wins when its event is a $set after the group's last $delete; has[g] = 1
+__global__ void k_prop_win(long long M, long long G, const unsigned long long *__restrict__ key, const uint32_t *__restrict__ val,
+                           const uint32_t *__restrict__ mev, const uint8_t *__restrict__ kind, const int32_t *__restrict__ ord,
+                           const int32_t *__restrict__ last_del, uint32_t *__restrict__ keep, uint32_t *__restrict__ has) {
+  for (long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x; k < M + G; k += (long long)gridDim.x * blockDim.x) {
+    uint32_t w = 0;
+    if ((uint32_t)key[k] != 0xffffffffu && key[k + 1] != key[k]) {   // entry M + G - 1 is a presence entry: k + 1 exists
+      const uint32_t i = mev[val[k]];
+      const int g = (int)(key[k] >> 32);
+      if ((kind[i] & kEvSet) && ord[i] > last_del[g]) {
+        w = 1;
+        has[g] = 1;
+      }
+    }
+    keep[k] = w;
+  }
+}
+// a presence entry stays for an item whose final state exists (a $set after its last $delete) but holds no field
+__global__ void k_prop_presence(long long M, long long G, const unsigned long long *__restrict__ key, const int32_t *__restrict__ last_del,
+                                const int32_t *__restrict__ last_set, const uint32_t *__restrict__ has, uint32_t *__restrict__ keep) {
+  for (long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x; k < M + G; k += (long long)gridDim.x * blockDim.x) {
+    if ((uint32_t)key[k] != 0xffffffffu) continue;
+    const int g = (int)(key[k] >> 32);
+    keep[k] = last_set[g] > last_del[g] && !has[g] ? 1u : 0u;
+  }
+}
+// triple t (kept entry k at pos[k]): item = the item id of its event (presence: the group's first event), field, and the
+// value text span (presence: none); first[f] = min triple index of field f (presence field: index n_fields)
+__global__ void k_prop_triples(long long M, long long G, const uint32_t *__restrict__ keep, const uint32_t *__restrict__ pos,
+                               const unsigned long long *__restrict__ key, const uint32_t *__restrict__ val, const uint32_t *__restrict__ mev,
+                               const uint32_t *__restrict__ gfirst, const JMember *__restrict__ mem, int32_t n_fields,
+                               uint32_t *__restrict__ titem, int32_t *__restrict__ tfield, long long *__restrict__ vb, long long *__restrict__ ve,
+                               uint32_t *__restrict__ first) {
+  for (long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x; k < M + G; k += (long long)gridDim.x * blockDim.x) {
+    if (!keep[k]) continue;
+    const uint32_t t = pos[k];
+    const bool presence = (uint32_t)key[k] == 0xffffffffu;
+    const int f = presence ? n_fields : (int)(uint32_t)key[k];
+    titem[t] = presence ? gfirst[key[k] >> 32] : mev[val[k]];
+    tfield[t] = f;
+    vb[t] = presence ? -1 : mem[val[k]].vb;
+    ve[t] = presence ? -1 : mem[val[k]].ve;
+    atomicMin(&first[f], t);
+  }
+}
+// value text of each triple (presence: "null", never written) as a column: length pass, then copy pass
+__global__ void k_prop_value_len(long long T, const long long *__restrict__ vb, const long long *__restrict__ ve, long long *__restrict__ len) {
+  for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < T; t += (long long)gridDim.x * blockDim.x)
+    len[t] = vb[t] < 0 ? 4 : ve[t] - vb[t];
+}
+__global__ void k_prop_value_copy(long long T, const long long *__restrict__ vb, const long long *__restrict__ off, const unsigned char *__restrict__ body,
+                                  unsigned char *__restrict__ out) {
+  for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < T; t += (long long)gridDim.x * blockDim.x) {
+    const long long o = off[t], n = off[t + 1] - o;
+    for (long long j = 0; j < n; ++j) out[o + j] = vb[t] < 0 ? (unsigned char)"null"[j] : body[vb[t] + j];
+  }
+}
+__global__ void k_gather_u8(long long n, const uint32_t *__restrict__ idx, const uint8_t *__restrict__ src, uint8_t *__restrict__ dst) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) dst[i] = src[idx[i]];
+}
+// out[0] += entries with flag bit `want`; out[1] += groups whose final state exists (a $set after the last $delete)
+__global__ void k_prop_counts(long long n, const uint8_t *__restrict__ flag, uint8_t want, long long G, const int32_t *__restrict__ last_del,
+                              const int32_t *__restrict__ last_set, unsigned long long *__restrict__ out) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n || i < G; i += (long long)gridDim.x * blockDim.x) {
+    if (i < n && (flag[i] & want)) atomicAdd(&out[0], 1ULL);
+    if (i < G && last_set[i] > last_del[i]) atomicAdd(&out[1], 1ULL);
+  }
+}
+__global__ void k_remap_i32(long long n, const int32_t *__restrict__ map, int32_t *__restrict__ x) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) x[i] = map[x[i]];
+}
+
+}  // namespace cco

@@ -106,10 +106,11 @@ __device__ __noinline__ bool json_escape_ok(const unsigned char *__restrict__ bo
 //   depth          = prefix count of '{' '[' minus '}' ']' outside strings (ballot popcounts)
 // The bytes at depth <= 1 outside strings (and the quotes at depth 1) drive a small state machine, one event at a time.
 enum : int { kJBefore = 0, kJFirst, kJNext, kJName, kJColon, kJValue0, kJValue, kJDone };
-template <bool kWrite>
+// Every completed member goes to sink.member(span, index in span, span begin, member) on lane 0, and lane 0 calls
+// sink.end(span, members) once per span; a malformed span sets the error word instead (its members may be partly sunk).
+template <class Sink>
 __global__ void k_json_members(long long n_spans, const long long *__restrict__ sb, const long long *__restrict__ se,
-                               const unsigned char *__restrict__ body, long long *__restrict__ count,
-                               const long long *__restrict__ moff, JMember *__restrict__ out, unsigned long long *__restrict__ err) {
+                               const unsigned char *__restrict__ body, const Sink sink, unsigned long long *__restrict__ err) {
   const int lane = threadIdx.x & 31;
   const unsigned below = (1u << lane) - 1, upto = 0xffffffffu >> (31 - lane);
   const long long warp = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5, nwarps = ((long long)gridDim.x * blockDim.x) >> 5;
@@ -118,7 +119,6 @@ __global__ void k_json_members(long long n_spans, const long long *__restrict__ 
     int code = e - b > 0x7fffffffLL ? kJsonLongLine : 0;
     int state = kJBefore;
     long long n = 0, depth = 0, last_nonws = b - 1;
-    const long long w0 = kWrite ? moff[s] : 0;
     JMember cur = {0, 0, 0, 0};
     unsigned in_str = 0, bs_odd = 0;
     for (long long base = b; base < e && !code; base += 32) {
@@ -182,7 +182,7 @@ __global__ void k_json_members(long long n_spans, const long long *__restrict__ 
             } else {
               const unsigned lb = nwm & ((1u << i) - 1);
               cur.ve = (lb ? base + 31 - __clz(lb) : last_nonws) + 1;
-              if (kWrite && lane == 0) out[w0 + n] = cur;
+              if (lane == 0) sink.member(s, n, b, cur);
               ++n;
               state = comma ? kJNext : kJDone;
             }
@@ -201,10 +201,23 @@ __global__ void k_json_members(long long n_spans, const long long *__restrict__ 
     if (!code && state != kJDone) code = state == kJBefore ? kJsonNotObject : (in_str ? kJsonString : kJsonSyntax);
     if (lane == 0) {
       if (code) atomicMin(err, ((unsigned long long)s << 8) | (unsigned)code);
-      if (!kWrite) count[s] = n;
+      sink.end(s, n);
     }
   }
 }
+// the members of every span: count pass (count[s]) and write pass (out[moff[s] ..])
+template <bool kWrite>
+struct MemberSink {
+  long long *count;
+  const long long *moff;
+  JMember *out;
+  __device__ void member(long long s, long long n, long long, const JMember &m) const {
+    if (kWrite) out[moff[s] + n] = m;
+  }
+  __device__ void end(long long s, long long n) const {
+    if (!kWrite) count[s] = n;
+  }
+};
 
 // ---- string decoder --------------------------------------------------------------------------------------------------
 __device__ __forceinline__ unsigned json_hex4(const unsigned char *__restrict__ p) {

@@ -5,6 +5,8 @@ the hand-written sm_90a path in csrc/ -- there is no CPU implementation in this 
 from __future__ import annotations
 
 import ctypes as C
+import os
+import weakref
 from dataclasses import dataclass
 from typing import Optional, Sequence
 
@@ -58,6 +60,7 @@ class CcoContext:
         self._arena = result_arena
         self.last_stats: TrainStats | None = None
         self._pinned_addr: dict = {}
+        self._logs = weakref.WeakSet()   # an event log belongs to its context: close() frees the open ones first
         if devices is not None:
             h = C.c_void_p()
             arr = (C.c_int32 * len(devices))(*devices)
@@ -87,6 +90,8 @@ class CcoContext:
 
     def close(self):
         if getattr(self, "_h", None):
+            for log in list(getattr(self, "_logs", ())):
+                log.free()
             self._L.cco_destroy(self._h)
             self._h = None
 
@@ -258,7 +263,7 @@ class CcoContext:
             rk[k] = N.RankingT(nb, N.POP_MODES.get(mode, -1), len(streams), int(start_ms), int(end_ms), st)
         return props, rankings, rk
 
-    def format_model(self, handle, names, row_ids, col_ids, properties=None, rankings=None) -> bytes:
+    def format_model(self, handle, names, row_ids, col_ids, properties=None, rankings=None, log=None) -> bytes:
         """cco_format_model: format_es_bulk plus the item properties and PopModel rankings joined in by item id, and a
         document for every item without a row that has a property or a score (URAlgorithm.scala:351-367, URModel.scala:57-102).
         properties = (field_names, item_offsets int64[n + 1], item_bytes uint8[], field int32[n], value_offsets int64[n + 1],
@@ -266,25 +271,99 @@ class CcoContext:
         rankings = [(field name, "popular" | "trending" | "hot" | "random", start_ms, end_ms, [(item_offsets, item_bytes,
         time_ms int64[]) per event name])].  A "random" ranking (uniqueRank) scores the items of its streams' events in
         [start_ms, end_ms) plus every property item with n · 10^-15, n a hash of the id and the window (ur_model.random_rank);
-        give it every event name's stream, as calcRandom reads them all.  Id columns in the layout of encode_ids."""
+        give it every event name's stream, as calcRandom reads them all.  Id columns in the layout of encode_ids.
+        log=EventLog (cco_format_model_log): the properties are the log's, aggregated on the device (`properties` must be
+        None), the streams come from the log in HBM, and a ranking is (field name, mode, start_ms, end_ms, [event names]);
+        a "random" one reads every event name of the log."""
         keep = []
         n, nm, rd, cds = self._format_args(names, row_ids, col_ids, keep)
+        if log is not None:
+            if properties is not None:
+                raise N.CcoInvalidArgument(N.E_INVALID_ARG, "with log=, the properties are the log's")
+            rk = self._log_rankings(rankings, keep)
+            out, ln = C.c_void_p(), C.c_int64()
+            N.check(self._L.cco_format_model_log(self._h, handle, n, nm, C.byref(rd), cds, log._h, len(rankings or []), rk, C.byref(out),
+                                                 C.byref(ln)))
+            return self._take_body(out, ln)
         props, rankings, rk = self._model_args(properties, rankings, keep)
         out, ln = C.c_void_p(), C.c_int64()
         N.check(self._L.cco_format_model(self._h, handle, n, nm, C.byref(rd), cds, C.byref(props) if props is not None else None,
                                          len(rankings), rk, C.byref(out), C.byref(ln)))
         return self._take_body(out, ln)
 
-    def rerank_model(self, body: bytes, properties=None, rankings=None) -> bytes:
+    @staticmethod
+    def _log_rankings(rankings, keep):
+        """[(field name, mode, start_ms, end_ms, [event names])] -> LogRankingT array"""
+        rankings = list(rankings or [])
+        rk = (N.LogRankingT * max(len(rankings), 1))()
+        for k, (name, mode, start_ms, end_ms, event_names) in enumerate(rankings):
+            en = [x.encode("utf-8") for x in event_names]
+            arr = (C.c_char_p * max(len(en), 1))(*en)
+            nb = name.encode("utf-8")
+            keep.append((arr, en, nb))
+            rk[k] = N.LogRankingT(nb, N.POP_MODES.get(mode, -1), len(en), int(start_ms), int(end_ms), arr)
+        return rk
+
+    def read_events(self, src) -> "EventLog":
+        """cco_event_log_read: a PredictionIO event export (JSON lines, as `pio export` writes them) parsed on the device.
+        src = bytes, a buffer, or a path: a file is read straight into pinned host memory (no Python objects per line).
+        -> EventLog (free with .free(), or use it as a context manager; close() of this context frees the logs still open)."""
+        if isinstance(src, str) or hasattr(src, "__fspath__"):
+            path = os.fspath(src)
+            n = os.path.getsize(path)
+            buf = self.host_array(n, np.uint8)
+            with open(path, "rb", buffering=0) as f:
+                got = f.readinto(memoryview(buf)) if n else 0
+            if got != n:
+                self.host_free(buf)
+                raise OSError(f"{path}: read {got} of {n} bytes")
+            pinned = buf
+        else:
+            buf = np.frombuffer(src, dtype=np.uint8) if not isinstance(src, np.ndarray) else np.ascontiguousarray(src, dtype=np.uint8)
+            pinned = None
+        h = C.c_void_p()
+        try:
+            N.check(self._L.cco_event_log_read(self._h, buf.ctypes.data if len(buf) else None, len(buf), C.byref(h)))
+        except BaseException:
+            if pinned is not None:
+                self.host_free(pinned)
+            raise
+        log = EventLog(self, h, pinned)
+        self._logs.add(log)
+        return log
+
+    def ingest_event_log(self, log: "EventLog", names: Sequence[str], min_events_per_user: int = 0):
+        """cco_event_log_ingest: ingest_strings on the log's training events of `names` (type t = names[t]), from HBM.
+        -> (dataset, user ids, [item ids per type]) as ingest_strings"""
+        nm = (C.c_char_p * len(names))(*[x.encode("utf-8") for x in names])
+        ds = C.c_void_p()
+        N.check(self._L.cco_event_log_ingest(self._h, log._h, len(names), nm, int(min_events_per_user or 0), C.byref(ds)))
+        dataset = (ds, len(names))
+        try:
+            users = self.dataset_dictionary(dataset, -1)
+            items = [self.dataset_dictionary(dataset, t) for t in range(len(names))]
+        except BaseException:
+            self.free_dataset(dataset)
+            raise
+        return dataset, users, items
+
+    def rerank_model(self, body: bytes, properties=None, rankings=None, log=None) -> bytes:
         """cco_rerank_model: calcPop (URAlgorithm.scala:375-399, recsModel "backfill") on an existing index.  body = the
         Elasticsearch bulk body of the current model, as format_model writes it; properties and rankings as in format_model.
         Every old document keeps its members and gets the rankings; a fresh property is added only where the old document
         has no member of that name, and an old rank member stays when the item has no score in the new ranking (include/
         cco_b200.h states the grammar, precedence and order).  Items with a property or a score but no old document are
-        appended as format_model writes them."""
+        appended as format_model writes them.  log=EventLog: properties and rankings as in format_model(log=...)."""
         keep = []
-        props, rankings, rk = self._model_args(properties, rankings, keep)
         body = bytes(body)
+        if log is not None:
+            if properties is not None:
+                raise N.CcoInvalidArgument(N.E_INVALID_ARG, "with log=, the properties are the log's")
+            rk = self._log_rankings(rankings, keep)
+            out, ln = C.c_void_p(), C.c_int64()
+            N.check(self._L.cco_rerank_model_log(self._h, body, len(body), log._h, len(rankings or []), rk, C.byref(out), C.byref(ln)))
+            return self._take_body(out, ln)
+        props, rankings, rk = self._model_args(properties, rankings, keep)
         out, ln = C.c_void_p(), C.c_int64()
         N.check(self._L.cco_rerank_model(self._h, body, len(body), C.byref(props) if props is not None else None, len(rankings), rk,
                                          C.byref(out), C.byref(ln)))
@@ -490,6 +569,61 @@ class CcoContext:
         for p in (orp, oci, ocn):
             self._L.cco_free(p)
         return r, c, n
+
+
+@dataclass
+class EventLogInfo:
+    n_lines: int
+    names: list          # distinct event names, first appearance order
+    n_training: list     # per name
+    n_ranking: list      # per name
+    n_property_events: int
+    n_property_items: int    # items whose aggregated properties exist (each gets a document)
+    n_property_fields: int
+    n_ignored: int
+
+
+class EventLog:
+    """A PredictionIO event export resident on one GPU (cco_event_log_t), from CcoContext.read_events."""
+
+    def __init__(self, ctx: CcoContext, h, pinned: Optional[np.ndarray]):
+        self._ctx, self._h, self._pinned = ctx, h, pinned
+
+    def _info(self):
+        i = N.EventLogInfoT()
+        N.check(self._ctx._L.cco_event_log_info(self._h, C.byref(i)))
+        return i
+
+    def info(self) -> EventLogInfo:
+        i = self._info()
+        g = i.names.n
+        off = np.ctypeslib.as_array(i.names.offsets, shape=(g + 1,)).copy() if g else np.zeros(1, np.int64)
+        addr = C.c_void_p.from_buffer(i.names, N.DictionaryT.bytes.offset).value
+        names = decode_ids(off, C.string_at(addr, int(off[-1])) if off[-1] else b"")
+        per = lambda p: np.ctypeslib.as_array(p, shape=(g,)).tolist() if g else []
+        return EventLogInfo(i.n_lines, names, per(i.n_training), per(i.n_ranking), i.n_property_events, i.n_property_items,
+                            i.n_property_fields, i.n_ignored)
+
+    def free(self):
+        if getattr(self, "_h", None):
+            self._ctx._L.cco_event_log_free(self._h)
+            self._h = None
+            self._ctx._logs.discard(self)
+            if self._pinned is not None:
+                self._ctx.host_free(self._pinned)
+                self._pinned = None
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.free()
 
 
 def encode_ids(ids: Sequence[str]) -> tuple[np.ndarray, np.ndarray]:

@@ -2,7 +2,8 @@
 (src/main/scala/URAlgorithm.scala:130-171 params, :310-369 calcAll).
 calc_all_on_device runs the whole train half on the GPU, string events in and the Elasticsearch bulk body out.
 calc_pop_on_device runs calcPop (recsModel "backfill") on the GPU: the current index's bulk body in, the same index with
-fresh rankings out.  Everything else in URAlgorithm (ES reads and query building) is out of scope."""
+fresh rankings out.  calc_all_from_events / calc_pop_from_events do the same from a PredictionIO event export parsed on the
+device (CcoContext.read_events), the DataSource included.  Everything else in URAlgorithm (ES reads and query building) is out of scope."""
 from __future__ import annotations
 
 import time
@@ -11,7 +12,8 @@ from typing import Optional, Sequence
 
 from .indexed_dataset import IndexedDataset
 from .similarity_analysis import CcoContext, DownsamplableCrossOccurrenceDataset, SimilarityAnalysis, default_context, encode_ids
-from .ur_model import RankingParams, aggregate_properties, extract_jvalue, property_json, rankings_for, rankings_params
+from .ur_model import (RankingParams, RankingType, extract_jvalue, property_json, ranking_window, rankings_for,
+                       rankings_params)
 
 
 class DefaultURAlgoParams:
@@ -102,7 +104,7 @@ def _seed_and_flags(ap: URAlgorithmParams, flags: int):
 
 def calc_all_on_device(events: Sequence[tuple[str, str, str, int]], set_events: Sequence[tuple[str, dict]], ap: URAlgorithmParams,
                        min_events_per_user: Optional[int] = None, now_ms: Optional[int] = None, ctx: CcoContext | None = None,
-                       flags: int = 0) -> bytes:
+                       flags: int = 0, ranking_events: Optional[dict] = None) -> bytes:
     """URAlgorithm.calcAll (URAlgorithm.scala:310-369) through URModel.save's documents, on the GPU: string events in, the
     Elasticsearch bulk body out.  events = (user id, event name, item id, time ms); set_events = (item id, {field: value}) of
     the items' `$set` events in event-time order.  Steps: cco_ingest_strings (Preparator) -> cco_train_dataset -> the
@@ -110,7 +112,9 @@ def calc_all_on_device(events: Sequence[tuple[str, str, str, int]], set_events: 
     cco_format_model.  "collabFiltering" writes the correlators only (propertiesRDD is empty there); "backfill" raises:
     calcPop refreshes an existing index instead, see calc_pop_on_device.
     now_ms: the rankings' end when a ranking has no offsetDate (default: the wall clock).  A random ranking's values are a
-    hash of the item id and the window (ur_model.random_rank): they change with now_ms and repeat for a fixed window."""
+    hash of the item id and the window (ur_model.random_rank): they change with now_ms and repeat for a fixed window.
+    ranking_events: {event name: [(item id, time ms)]} the rankings read instead of `events` (PopModel reads events of every
+    entity type; events.read_export gives both)."""
     _check_recs_model(ap)
     if ap.recsModel == "backfill":
         raise ValueError("recsModel=backfill runs calcPop against the live index: use calc_pop_on_device with its bulk body")
@@ -124,16 +128,11 @@ def calc_all_on_device(events: Sequence[tuple[str, str, str, int]], set_events: 
     if not actions:
         raise ValueError("no events of the model's event names")
     cols = [(*encode_ids([u for u, _, _ in ev]), *encode_ids([i for _, i, _ in ev])) for _, ev in actions]
-    if ap.indicators:
-        ind = {i.name: i for i in ap.indicators}
-        params = [(ind[n].maxItemsPerUser or DefaultURAlgoParams.MaxEventsPerEventType,
-                   ind[n].maxCorrelatorsPerItem or DefaultURAlgoParams.MaxCorrelatorsPerEventType, ind[n].minLLR) for n, _ in actions]
-    else:
-        params = [(ap.maxEventsPerEventType or DefaultURAlgoParams.MaxEventsPerEventType,
-                   ap.maxCorrelatorsPerEventType or DefaultURAlgoParams.MaxCorrelatorsPerEventType, None)] * len(actions)
+    params = _indicator_params(ap, [n for n, _ in actions])
     props, rankings = None, None
     if ap.recsModel == "all":
-        props, rankings = _properties_and_rankings(by_name, set_events, ap, now_ms)
+        rank_by_name = ranking_events if ranking_events is not None else {n: [(i, t) for _, i, t in ev] for n, ev in by_name.items()}
+        props, rankings = _properties_and_rankings(rank_by_name, set_events, ap, now_ms)
     ds, _, items = ctx.ingest_strings(cols, min_events_per_user or 0)
     try:
         _, h = ctx.train_dataset(ds, params, seed, flags, keep=True)
@@ -145,24 +144,105 @@ def calc_all_on_device(events: Sequence[tuple[str, str, str, int]], set_events: 
         ctx.free_dataset(ds)
 
 
-def _properties_and_rankings(by_name: dict, set_events: Sequence[tuple[str, dict]], ap: URAlgorithmParams, now_ms: Optional[int]):
-    """propertiesRDD's inputs in the form of CcoContext.format_model: the `$set` properties as JSON text triples and the
-    rankings of getRanksRDD over the events {event name: [(user, item, time ms)]}"""
-    names = ap.model_event_names()
-    triples = [(i, f, extract_jvalue(f, v)) for i, f, v in aggregate_properties(set_events)]
+def _indicator_params(ap: URAlgorithmParams, names: Sequence[str]) -> list:
+    """(maxItemsPerUser, maxCorrelatorsPerItem, minLLR) per event name of the model (URAlgorithm.scala:323-346)"""
+    if ap.indicators:
+        ind = {i.name: i for i in ap.indicators}
+        return [(ind[n].maxItemsPerUser or DefaultURAlgoParams.MaxEventsPerEventType,
+                 ind[n].maxCorrelatorsPerItem or DefaultURAlgoParams.MaxCorrelatorsPerEventType, ind[n].minLLR) for n in names]
+    return [(ap.maxEventsPerEventType or DefaultURAlgoParams.MaxEventsPerEventType,
+             ap.maxCorrelatorsPerEventType or DefaultURAlgoParams.MaxCorrelatorsPerEventType, None)] * len(names)
+
+
+def _with_presence(set_events: Sequence[tuple[str, dict]]) -> list:
+    """ur_model.aggregate_properties, with an (item, "id", None) triple in the place of an item left with no field"""
+    props: dict = {}
+    for item, fields in set_events:
+        props.setdefault(item, {}).update(fields)
+    return [(item, k, v) for item, d in props.items() for k, v in (d.items() if d else [("id", None)])]
+
+
+def _properties(set_events: Sequence[tuple[str, dict]]):
+    """the `$set` properties as the JSON text triples of CcoContext.format_model.  An item given with no field stays a
+    property item, as the reference's fieldsRDD lists it: a triple of the field "id" (never written, the document's own
+    "id" wins) gives it an "id"-only document and makes it a random-rank candidate."""
+    triples = [(i, f, extract_jvalue(f, v)) for i, f, v in _with_presence(set_events)]
     fields = list(dict.fromkeys(f for _, f, _ in triples))
     fidx = {f: k for k, f in enumerate(fields)}
-    props = (fields, *encode_ids([i for i, _, _ in triples]), [fidx[f] for _, f, _ in triples],
-             *encode_ids([property_json(v) for _, _, v in triples]))
+    return (fields, *encode_ids([i for i, _, _ in triples]), [fidx[f] for _, f, _ in triples],
+            *encode_ids([property_json(v) for _, _, v in triples]))
+
+
+def _properties_and_rankings(ev_by_name: dict, set_events: Sequence[tuple[str, dict]], ap: URAlgorithmParams, now_ms: Optional[int]):
+    """propertiesRDD's inputs in the form of CcoContext.format_model: the `$set` properties as JSON text triples and the
+    rankings of getRanksRDD over the events {event name: [(item, time ms)]}"""
+    names = ap.model_event_names()
     now = now_ms if now_ms is not None else int(time.time() * 1000)
-    ev_by_name = {n: [(i, t) for _, i, t in ev] for n, ev in by_name.items()}
     rankings = [(r.field, r.mode, r.start_ms, r.end_ms, [(*encode_ids(items), times) for items, times in r.streams])
                 for r in rankings_for(rankings_params(ap.rankings, names), ev_by_name, now, names)]
-    return props, rankings
+    return _properties(set_events), rankings
+
+
+def _log_rankings(ap: URAlgorithmParams, now_ms: Optional[int]) -> list:
+    """getRanksRDD's rankings as CcoContext.format_model(log=...) takes them: (field, mode, start, end, event names), the
+    choices of ur_model.rankings_for (a random ranking reads every event name of the log)"""
+    names = ap.model_event_names()
+    now = now_ms if now_ms is not None else int(time.time() * 1000)
+    out = []
+    for rp in rankings_params(ap.rankings, names):
+        t = rp.ranking_type()
+        if t not in (RankingType.Popular, RankingType.Trending, RankingType.Hot, RankingType.Random):
+            continue
+        start, end = ranking_window(rp, now)
+        out.append((rp.field_name(), t, start, end, [] if t == RankingType.Random else
+                    list(rp.eventNames if rp.eventNames is not None else names[:1])))
+    return out
+
+
+def _read_log(export, ctx: CcoContext):
+    """(log, owned): an EventLog as given, or one read from bytes / a buffer / a path"""
+    from .similarity_analysis import EventLog
+    return (export, False) if isinstance(export, EventLog) else (ctx.read_events(export), True)
+
+
+def calc_all_from_events(export, ap: URAlgorithmParams, min_events_per_user: Optional[int] = None, now_ms: Optional[int] = None,
+                         ctx: CcoContext | None = None, flags: int = 0) -> bytes:
+    """calc_all_on_device from a PredictionIO event export (bytes, a buffer, a path or an EventLog of this context): the
+    export is copied to the GPU once and parsed there (the DataSource: include/cco_b200.h cco_event_log_read); the training
+    events, the ranking streams and the items' properties, aggregated there from their $set / $unset / $delete events,
+    stay in HBM.  Property values are spliced as written.  Same decisions as calc_all_on_device."""
+    _check_recs_model(ap)
+    if ap.recsModel == "backfill":
+        raise ValueError("recsModel=backfill runs calcPop against the live index: use calc_pop_from_events with its bulk body")
+    ctx = ctx or default_context()
+    seed, flags = _seed_and_flags(ap, flags)
+    log, owned = _read_log(export, ctx)
+    try:
+        info = log.info()
+        n_train = dict(zip(info.names, info.n_training))
+        actions = [n for n in ap.model_event_names() if n_train.get(n)]   # DataSource.scala:79-89 drops empty event RDDs
+        if not actions:
+            raise ValueError("no events of the model's event names")
+        params = _indicator_params(ap, actions)
+        ds, _, items = ctx.ingest_event_log(log, actions, min_events_per_user or 0)
+        try:
+            _, h = ctx.train_dataset(ds, params, seed, flags, keep=True)
+            try:
+                if ap.recsModel == "collabFiltering":   # the correlators only: propertiesRDD is empty there
+                    return ctx.format_model(h, actions, items[0], items)
+                return ctx.format_model(h, actions, items[0], items, rankings=_log_rankings(ap, now_ms), log=log)
+            finally:
+                ctx.free_result(h)
+        finally:
+            ctx.free_dataset(ds)
+    finally:
+        if owned:
+            log.free()
 
 
 def calc_pop_on_device(body: bytes, events: Sequence[tuple[str, str, str, int]], set_events: Sequence[tuple[str, dict]],
-                       ap: URAlgorithmParams, now_ms: Optional[int] = None, ctx: CcoContext | None = None) -> bytes:
+                       ap: URAlgorithmParams, now_ms: Optional[int] = None, ctx: CcoContext | None = None,
+                       ranking_events: Optional[dict] = None) -> bytes:
     """URAlgorithm.calcPop (URAlgorithm.scala:375-399, recsModel "backfill") on the GPU: the rankings of an existing index
     refreshed between trains, without a CCO train.  body = the current index as an Elasticsearch bulk body (what
     calc_all_on_device or format_model wrote; reading it from Elasticsearch stays with the caller); events and set_events as
@@ -172,7 +252,19 @@ def calc_pop_on_device(body: bytes, events: Sequence[tuple[str, str, str, int]],
     has no score in the new window.  Items with a property or a score and no old document are appended."""
     ctx = ctx or default_context()
     by_name: dict = {}
-    for u, e, i, t in events:
-        by_name.setdefault(e, []).append((u, i, t))
-    props, rankings = _properties_and_rankings(by_name, set_events, ap, now_ms)
+    for _, e, i, t in events:
+        by_name.setdefault(e, []).append((i, t))
+    props, rankings = _properties_and_rankings(ranking_events if ranking_events is not None else by_name, set_events, ap, now_ms)
     return ctx.rerank_model(body, props, rankings)
+
+
+def calc_pop_from_events(body: bytes, export, ap: URAlgorithmParams, now_ms: Optional[int] = None, ctx: CcoContext | None = None) -> bytes:
+    """calc_pop_on_device from a PredictionIO event export (as in calc_all_from_events): the ranking streams and the
+    properties of the log, both in HBM, joined into the old index by cco_rerank_model_log."""
+    ctx = ctx or default_context()
+    log, owned = _read_log(export, ctx)
+    try:
+        return ctx.rerank_model(body, None, _log_rankings(ap, now_ms), log=log)
+    finally:
+        if owned:
+            log.free()

@@ -260,8 +260,24 @@ def json_string(s: str) -> str:
     return '"' + "".join(out) + '"'
 
 
+class RawJson:
+    """a property value kept as the JSON text it was written in (an event export's member value, trimmed): spliced as is"""
+    __slots__ = ("text",)
+
+    def __init__(self, text: str):
+        self.text = text
+
+    def __eq__(self, other):
+        return isinstance(other, RawJson) and other.text == self.text
+
+    def __repr__(self):
+        return f"RawJson({self.text!r})"
+
+
 def property_json(value) -> str:
-    """a property value -> the JSON text the device splices verbatim (floats as Java's Double.toString)"""
+    """a property value -> the JSON text the device splices verbatim (floats as Java's Double.toString; RawJson as written)"""
+    if isinstance(value, RawJson):
+        return value.text
     if value is None:
         return "null"
     if isinstance(value, bool):
