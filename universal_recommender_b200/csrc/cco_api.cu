@@ -3716,6 +3716,8 @@ static int event_properties(cco_ctx *c, Arena &ar, cco_event_log *lg, long long 
   long long f_id = NF;
   for (long long f = 0; f < NF; ++f)
     if (fname[f] == "id") f_id = f;
+  // a property named "id" is a field of the aggregated properties only if some item keeps it
+  const bool id_kept = f_id < NF && h_first[f_id] != ~0u, presence = h_first[NF] != ~0u;
   h_first[f_id] = std::min(h_first[f_id], h_first[NF]);
   std::vector<long long> used;
   for (long long f = 0; f < NF; ++f)
@@ -3729,7 +3731,7 @@ static int event_properties(cco_ctx *c, Arena &ar, cco_event_log *lg, long long 
     lg->field_names.push_back(used[k] == NF ? std::string("id") : fname[used[k]]);
   }
   remap[NF] = remap[f_id];
-  lg->n_prop_fields = (long long)used.size() - (f_id == NF && h_first[NF] != ~0u ? 1 : 0);
+  lg->n_prop_fields = (long long)used.size() - (presence && !id_kept ? 1 : 0);
   int32_t *d_remap;
   CKR(ar.alloc(&d_remap, NF + 1));
   CK(cudaMemcpyAsync(d_remap, remap.data(), sizeof(int32_t) * remap.size(), cudaMemcpyHostToDevice, s));

@@ -16,9 +16,20 @@ event per line), the restatement cco_event_log_read (include/cco_b200.h) is held
 eventTime is Joda's extended date-time YYYY-MM-DDThh:mm:ss[.f{1,9}](Z|+hh:mm|+hhmm|+hh), fraction digits past the third
 dropped, proleptic Gregorian years 0000-9999.  Anything else raises ValueError naming the 0-based line.
 
-What the mirror accepts differs from the device in one way: every line goes through json.loads here, while the device
-checks nested values only for closed strings, valid escapes and bracket balance (and the members of a property event's
-properties object).  So a line such as {"event":"v",...,"tags":[tru]} raises here and is read by the device."""
+A line is strict UTF-8 text, as `pio export` writes it: a byte order mark is not whitespace, and a line that starts with
+one raises here as it does on the device.
+
+What the mirror accepts differs from the device in these ways:
+  - every line goes through json.loads here, while the device checks nested values only for closed strings, valid
+    escapes and bracket depth (and the members of a property event's properties object).  So a line such as
+    {"event":"v",...,"tags":[tru]} raises here and is read by the device, and so does a nested value whose bracket kinds
+    do not match, such as the property value {"a":{]}: the device splices its text verbatim;
+  - a byte sequence that is not UTF-8 inside a string raises here; the device copies the bytes through, so an id holds
+    them verbatim;
+  - a \\u escape of a surrogate that is not part of a pair (a high surrogate not followed by a \\u escape of a low one, or a
+    lone low one) is written by the device as the surrogate's 3-byte form (\\ud800 -> ED A0 80, Python's
+    "surrogatepass").  Here it stays a lone surrogate in the str, which encode_ids (strict UTF-8) cannot encode: such an
+    export cannot go through calc_all_on_device / calc_pop_on_device, only through the *_from_events paths."""
 from __future__ import annotations
 
 import json
@@ -119,8 +130,8 @@ class Event:
 
 def parse_line(i: int, raw: bytes) -> Event:
     """one export line -> Event, with the checks of cco_event_log_read (the last of a repeated member wins)"""
-    try:
-        obj = json.loads(raw)
+    try:   # strict UTF-8 first: json.loads(bytes) would take a leading byte order mark for utf-8-sig
+        obj = json.loads(raw.decode("utf-8"))
     except ValueError as e:
         raise ValueError(f"line {i}: not one JSON object ({e})") from None
     if not isinstance(obj, dict):
