@@ -447,12 +447,31 @@ int cco_rerank_model(cco_ctx_t *ctx, const char *body, int64_t body_len, const c
  * Errors: CCO_E_INVALID_ARG for malformed JSON (nested values are checked for closed strings, valid escapes and bracket
  * balance only, as in cco_rerank_model), a missing or mistyped member, a bad time or an empty training id -- the message
  * names the first bad 0-based line, and the verdict comes before any kernel reads through the parsed spans;
- * CCO_E_UNSUPPORTED for more than 2^31 - 1 lines, a line of 2^31 or more bytes, 2^31 - 1 or more ranking events of one
- * name, 2^31 - 1 or more property members, and group contexts.  A log belongs to its context: free it before
- * cco_destroy of that context.
+ * CCO_E_UNSUPPORTED for more than 2^31 - 1 lines in one parsed chunk (see below; the whole of cco_event_log_read is one),
+ * a line of 2^31 or more bytes, 2^31 - 1 or more ranking events of one name, 2^31 - 1 or more property members, and group
+ * contexts.  Training events of one name are limited to < 2^31 by the ingest.  A log belongs to its context: free it
+ * before cco_destroy of that context.
+ *
+ * Streamed reading: a log can be built from any split of the export's bytes, for exports larger than device or host
+ * memory and for the part files `pio export` writes.  The result -- info, ingest, format and rerank -- is identical to
+ * cco_event_log_read of the concatenated bytes, and so is the error code of a failed read; when exactly one line is bad
+ * the message is the same and names the same global 0-based line.  When several lines are bad, a streamed log may name a
+ * different one than the whole read: chunks are judged in order, each completely before the next.
+ *  - cco_event_log_begin: an empty log with chunk_bytes of device staging.
+ *  - cco_event_log_append: any number of bytes at any split point (mid-line, mid-escape, mid-UTF-8 sequence, between
+ *    '\r' and '\n'); returns once they are copied, so the caller may reuse its buffer.  Whenever the staging is full its
+ *    complete lines are parsed as one chunk and the unfinished line is carried to the next; a line longer than the
+ *    staging doubles it.  Global line numbers are 64-bit: the 2^31 - 1 line limit holds per chunk.
+ *  - cco_event_log_finish: parses the carried tail as the last line (which need not end in '\n'), lays the columns out
+ *    and aggregates the properties.  Only then do info, ingest, format_model_log and rerank_model_log accept the log.
+ * Before finish those return CCO_E_INVALID_ARG; after a failed append or finish every call but free returns
+ * CCO_E_INVALID_ARG with the failure's message.  cco_event_log_read is begin(len) + append + finish.
  */
 typedef struct cco_event_log cco_event_log_t;
 int cco_event_log_read(cco_ctx_t *ctx, const char *bytes, int64_t len, cco_event_log_t **out);
+int cco_event_log_begin(cco_ctx_t *ctx, int64_t chunk_bytes, cco_event_log_t **out);
+int cco_event_log_append(cco_event_log_t *log, const char *bytes, int64_t len);
+int cco_event_log_finish(cco_event_log_t *log);
 typedef struct {
   int64_t n_lines;
   cco_dictionary_t names;          /* the distinct event names, in order of first appearance (owned by the log) */

@@ -112,8 +112,8 @@ EXPORTS = [
     "cco_partition_rows", "cco_ingest", "cco_synth_ingest", "cco_dataset_shape", "cco_dataset_download",
     "cco_dataset_copy_to_host", "cco_format_es_bulk", "cco_ingest_strings", "cco_dataset_dictionary", "cco_pop_model",
     "cco_format_model", "cco_rerank_model", "cco_event_log_read", "cco_event_log_info", "cco_event_log_ingest",
-    "cco_format_model_log", "cco_rerank_model_log", "cco_event_log_free",
-    "cco_result_num_matrices", "cco_result_row_range", "cco_result_matrix", "cco_result_stats", "cco_result_free",
+    "cco_format_model_log", "cco_rerank_model_log", "cco_event_log_free", "cco_event_log_begin", "cco_event_log_append",
+    "cco_event_log_finish", "cco_result_num_matrices", "cco_result_row_range", "cco_result_matrix", "cco_result_stats", "cco_result_free",
     "cco_debug_cooccurrence", "cco_debug_downsample", "cco_debug_llr", "cco_debug_string_ids", "cco_free",
 ]
 
@@ -169,6 +169,9 @@ def lib():
     L.cco_rerank_model_log.argtypes = [C.c_void_p, C.c_char_p, C.c_int64, C.c_void_p, C.c_int32, p(LogRankingT), p(C.c_void_p),
                                        p(C.c_int64)]
     L.cco_event_log_free.argtypes = [C.c_void_p]
+    L.cco_event_log_begin.argtypes = [C.c_void_p, C.c_int64, p(C.c_void_p)]
+    L.cco_event_log_append.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
+    L.cco_event_log_finish.argtypes = [C.c_void_p]
     L.cco_dataset_shape.argtypes = [C.c_void_p, C.c_int32, p(C.c_int64), p(C.c_int32), p(C.c_int64)]
     L.cco_dataset_download.argtypes = [C.c_void_p, C.c_int32, p(p(C.c_int64)), p(p(C.c_int32))]
     L.cco_timer_start.argtypes = [C.c_void_p]

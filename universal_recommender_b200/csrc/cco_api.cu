@@ -19,6 +19,7 @@
 #include <mutex>
 #include <string>
 #include <thread>
+#include <unordered_map>
 #include <vector>
 
 #include "../../include/cco_b200.h"
@@ -3394,6 +3395,13 @@ struct EvCol {
   uint64_t *w = nullptr;
   std::vector<long long> boff;
 };
+// what one parsed chunk of a streamed read keeps until finish: its retained columns, partitioned by the names known when
+// it was parsed (train_at / rank_at: that many names + 1)
+struct EvSeg {
+  EvCol tu, ti, ri;
+  long long *rtime = nullptr;
+  std::vector<long long> train_at, rank_at;
+};
 struct cco_event_log {
   cco_ctx *ctx = nullptr;
   long long n_lines = 0, n_prop = 0, n_ignored = 0;
@@ -3411,6 +3419,19 @@ struct cco_event_log {
   unsigned char *p_vals = nullptr, *p_ibytes = nullptr;
   std::vector<std::string> field_names;
   std::vector<void *> dev;                     // what to free
+  // the read in progress (cco_event_log_begin / _append / _finish): staging of cap bytes (+ 24 of padding) holding
+  // `staged` bytes, the last '\n' among them at last_nl (-1: none); lines parsed so far; per chunk one segment; the
+  // property-event lines (each ending in '\n') and their global lines, aggregated at finish
+  unsigned char *stage = nullptr;
+  long long cap = 0, staged = 0, last_nl = -1;
+  std::vector<EvSeg> segs;
+  std::unordered_map<std::string, int> name_code;
+  unsigned char *pb = nullptr;
+  long long pb_len = 0, pb_cap = 0;
+  std::vector<long long> prop_line;
+  bool finished = false;
+  int fail = CCO_OK;                           // a failed append / finish: every later call returns it with fail_msg
+  std::string fail_msg;
   int code_of(const char *name) const {
     const size_t n = strlen(name);
     for (size_t g = 0; g + 1 < name_off.size(); ++g)
@@ -3461,6 +3482,15 @@ static int log_keep(Arena &ar, cco_event_log *lg, void *p) {
   ar.take(p);
   lg->dev.push_back(p);
   return CCO_OK;
+}
+// a buffer the log kept, freed before the log is
+static void log_drop(cco_event_log *lg, void *p) {
+  for (size_t i = 0; p && i < lg->dev.size(); ++i)
+    if (lg->dev[i] == p) {
+      cudaFreeAsync(p, lg->ctx->stream);
+      lg->dev.erase(lg->dev.begin() + i);
+      return;
+    }
 }
 // the lines carrying flag bit `want` in a stable order: by event name (code != nullptr), else by line -> idx[0 .. count)
 static int event_partition(cco_ctx *c, Arena &ar, long long L, const uint8_t *flag, uint8_t want, const int32_t *code, uint32_t n_names,
@@ -3559,9 +3589,10 @@ static int bits_for(long long n) {
 // the items' first property event (line order), each item's fields in the order their names first appear among the
 // members of $set / $unset properties; an item whose final state exists without a field gets one triple of the field "id"
 // (never written: "id" wins) so that it has a document and is a random-rank candidate.  Values are the members' trimmed
-// JSON text, spliced verbatim.  Field numbers follow first appearance in the triples.
+// JSON text, spliced verbatim.  Field numbers follow first appearance in the triples.  gline[l]: the global line of line l,
+// named by an error.
 static int event_properties(cco_ctx *c, Arena &ar, cco_event_log *lg, long long L, const uint8_t *flag, const long long *tm,
-                            const long long *sb, const int2 *span, const unsigned char *bb) {
+                            const long long *sb, const int2 *span, const unsigned char *bb, const long long *gline) {
   cudaStream_t s = c->stream;
   const long long NP = lg->n_prop;
   uint32_t *pl;   // property event -> line, line order
@@ -3637,7 +3668,7 @@ static int event_properties(cco_ctx *c, Arena &ar, cco_event_log *lg, long long 
     uint32_t q = 0, line = 0;
     CK(cudaMemcpy(&q, qi + (h_err >> 8), 4, cudaMemcpyDeviceToHost));
     CK(cudaMemcpy(&line, pl + q, 4, cudaMemcpyDeviceToHost));
-    return event_error(((unsigned long long)line << 8) | (h_err & 0xff));
+    return event_error(((unsigned long long)gline[line] << 8) | (h_err & 0xff));
   }
   if (M + G >= 0x7fffffffLL) return set_error(CCO_E_UNSUPPORTED, "%lld property members, at most 2^31 - 2 with the items", M);
   JMember *mem;
@@ -3766,35 +3797,22 @@ static int event_properties(cco_ctx *c, Arena &ar, cco_event_log *lg, long long 
   return CCO_OK;
 }
 
-static int event_log_read(cco_ctx *c, const char *bytes, int64_t len, cco_event_log **out) {
-  CK(cudaSetDevice(c->device));
-  cudaStream_t s = c->stream;
-  nvtx_push("cco:event_log_read");
-  struct Pop { ~Pop() { nvtx_pop(); } } pop;
-  mail_reset(c);
-  Arena ar(s);
-  cco_event_log *lg = new cco_event_log();
-  lg->ctx = c;
-  struct G {
-    cco_event_log *l;
-    bool ok = false;
-    ~G() {
-      if (!ok) event_log_release(l);
-    }
-  } g{lg};
-  lg->name_off.assign(1, 0);
-  lg->train_at.assign(1, 0);
-  lg->rank_at.assign(1, 0);
-  // 1. the export, once, into 8-byte words with 16 bytes of zero padding
-  const long long NW = (len + 7) / 8;
-  uint64_t *w;
-  CKR(ar.alloc(&w, NW + 2));
-  CK(cudaMemsetAsync(w + len / 8, 0, sizeof(uint64_t) * (size_t)(NW + 2 - len / 8), s));
-  if (len > 0) CK(cudaMemcpyAsync(w, bytes, (size_t)len, cudaMemcpyHostToDevice, s));
-  const unsigned char *bb = (const unsigned char *)w;
-  // 2. lines: every '\n' ends one; a last line without it ends at len
+// steps 2-4 of a read over the len bytes of w (bytes [len, round_up(len, 8) + 16) are zero): lines (every '\n' ends one;
+// open_tail: a last line without it ends at len), the seven members an event is read through, then types, times and the
+// selection.  Each verdict comes before anything reads through the parsed spans; an error names the global line
+// line_base + l.
+struct EvLines {
   long long L = 0;
-  const bool open_tail = len > 0 && bytes[len - 1] != '\n';
+  long long *sb = nullptr, *se = nullptr, *tm = nullptr;
+  int2 *span = nullptr;
+  uint8_t *flag = nullptr;
+};
+static int event_lines(cco_ctx *c, Arena &ar, const uint64_t *w, long long len, bool open_tail, long long line_base, EvLines *ev) {
+  cudaStream_t s = c->stream;
+  const unsigned char *bb = (const unsigned char *)w;
+  const unsigned long long base = (unsigned long long)line_base << 8;
+  const long long NW = (len + 7) / 8;
+  long long L = 0;
   long long *nl;
   long long n_chunks = (NW + kNlChunkWords - 1) / kNlChunkWords;
   long long *cc, *coff;
@@ -3808,55 +3826,69 @@ static int event_log_read(cco_ctx *c, const char *bytes, int64_t len, cco_event_
   CKR(exclusive_sum_i64(c, ar, cc, coff, n_chunks + 1));
   CKR(mail_fetch(c, &L, coff + n_chunks, 8));
   CKR(mail_wait(c));
-  if (L + (open_tail ? 1 : 0) > 0x7fffffffLL) return set_error(CCO_E_UNSUPPORTED, "%lld lines, at most 2^31 - 1", L + (open_tail ? 1 : 0));
+  if (L + (open_tail ? 1 : 0) > 0x7fffffffLL)
+    return set_error(CCO_E_UNSUPPORTED, "%lld lines in one parsed chunk, at most 2^31 - 1", L + (open_tail ? 1 : 0));
   CKR(ar.alloc(&nl, L + 1));
   if (L > 0) {
     k_nl_write<<<grid_for(n_chunks * 32, 256, c->sm_count), 256, 0, s>>>(NW, w, coff, nl);
     c->launches++;
   }
-  const long long end_pos = len;
   if (open_tail) {
-    CK(cudaMemcpyAsync(nl + L, &end_pos, 8, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(nl + L, &len, 8, cudaMemcpyHostToDevice, s));
     ++L;
   }
-  lg->n_lines = L;
-  if (L == 0) {
-    CK(cudaStreamSynchronize(s));
-    g.ok = true;
-    *out = lg;
-    return CCO_OK;
-  }
-  long long *sb, *se;
-  CKR(ar.alloc(&sb, L));
-  CKR(ar.alloc(&se, L));
-  k_line_spans<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, nl, sb, se);
+  ev->L = L;
+  if (L == 0) return CCO_OK;
+  CKR(ar.alloc(&ev->sb, L));
+  CKR(ar.alloc(&ev->se, L));
+  k_line_spans<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, nl, ev->sb, ev->se);
   c->launches++;
-  // 3. the seven members an event is read through; the tokenizer's verdict comes before anything reads the spans
-  int2 *span;
   unsigned long long *err, h_err = 0;
-  CKR(ar.alloc(&span, L * kEvSlots));
+  CKR(ar.alloc(&ev->span, L * kEvSlots));
   CKR(ar.alloc(&err, 1));
-  CK(cudaMemsetAsync(span, 0xff, sizeof(int2) * (size_t)L * kEvSlots, s));
+  CK(cudaMemsetAsync(ev->span, 0xff, sizeof(int2) * (size_t)L * kEvSlots, s));
   CK(cudaMemsetAsync(err, 0xff, 8, s));
-  k_json_members<<<grid_for(L * 32, 256, c->sm_count), 256, 0, s>>>(L, sb, se, bb, EventSink{span, bb}, err);
+  k_json_members<<<grid_for(L * 32, 256, c->sm_count), 256, 0, s>>>(L, ev->sb, ev->se, bb, EventSink{ev->span, bb}, err);
   c->launches++;
   CKR(mail_fetch(c, &h_err, err, 8));
   CKR(mail_wait(c));
-  if (h_err != ~0ULL) return event_error(h_err);
-  // 4. types, times, selection
-  uint8_t *flag;
-  long long *tm;
-  CKR(ar.alloc(&flag, L));
-  CKR(ar.alloc(&tm, L));
-  k_event_check<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, sb, span, bb, flag, tm, err);
+  if (h_err != ~0ULL) return event_error(h_err + base);
+  CKR(ar.alloc(&ev->flag, L));
+  CKR(ar.alloc(&ev->tm, L));
+  k_event_check<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, ev->sb, ev->span, bb, ev->flag, ev->tm, err);
   c->launches++;
   CKR(mail_fetch(c, &h_err, err, 8));
   CKR(mail_wait(c));
-  if (h_err != ~0ULL) return event_error(h_err);
-  // 5. event names: decoded, grouped exactly, numbered by first appearance; the few distinct ones go to the host
+  if (h_err != ~0ULL) return event_error(h_err + base);
+  return CCO_OK;
+}
+
+// zero the word that holds byte `len` of a buffer and the 16 bytes after it, so that the newline passes, which read whole
+// words, see no stale byte past len
+static int event_pad(cco_ctx *c, unsigned char *buf, long long len) {
+  CK(cudaMemsetAsync(buf + len, 0, (size_t)(((len + 7) & ~7LL) + 16 - len), c->stream));
+  return CCO_OK;
+}
+
+// one chunk of a streamed read, the first len staged bytes: every line parsed, the names numbered globally, the counts
+// added, the training and ranking events decoded into one new segment, the property-event lines appended to lg->pb
+static int event_chunk(cco_event_log *lg, long long len, bool open_tail) {
+  cco_ctx *c = lg->ctx;
+  cudaStream_t s = c->stream;
+  mail_reset(c);
+  Arena ar(s);
+  CKR(event_pad(c, lg->stage, len));
+  EvLines ev;
+  const long long base = lg->n_lines;
+  CKR(event_lines(c, ar, (const uint64_t *)lg->stage, len, open_tail, base, &ev));
+  const long long L = ev.L;
+  if (L == 0) return CCO_OK;
+  const unsigned char *bb = lg->stage;
+  // 5. event names: decoded, grouped exactly, numbered by first appearance in the chunk; the few distinct ones go to the
+  // host, where names new to the log take the next codes (chunks arrive in order: the order of the whole read)
   JMember *jm;
   CKR(ar.alloc(&jm, L));
-  k_event_strings<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, nullptr, kEvName, sb, span, bb, jm);
+  k_event_strings<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, nullptr, kEvName, ev.sb, ev.span, bb, jm);
   c->launches++;
   DevStrCol names;
   long long name_bytes = 0;
@@ -3867,61 +3899,299 @@ static int event_log_read(cco_ctx *c, const char *bytes, int64_t len, cco_event_
   CKR(ar.alloc(&code, L));
   StrTable nt;
   CKR(str_group(c, ar, names, nullptr, false, 0, &nt, code));
-  const long long NG = nt.n_groups;
+  const long long NC = nt.n_groups;
   cco_dictionary_t nd;
   CKR(str_dictionary(c, ar, names, nt, &nd));
   CK(cudaStreamSynchronize(s));
-  lg->name_off.assign(nd.offsets, nd.offsets + NG + 1);
-  lg->name_bytes.assign(nd.bytes, (size_t)nd.offsets[NG]);
+  std::vector<int32_t> remap((size_t)NC);
+  for (long long k = 0; k < NC; ++k) {
+    std::string nm(nd.bytes + nd.offsets[k], (size_t)(nd.offsets[k + 1] - nd.offsets[k]));
+    auto it = lg->name_code.find(nm);
+    if (it == lg->name_code.end()) {
+      it = lg->name_code.emplace(nm, (int)lg->name_off.size() - 1).first;
+      lg->name_bytes += nm;
+      lg->name_off.push_back((int64_t)lg->name_bytes.size());
+    }
+    remap[k] = it->second;
+  }
   c->pinned_put((void *)nd.offsets);
   c->pinned_put((void *)nd.bytes);
   str_table_release(ar, nt);
   str_release(ar, names);
+  const long long NG = (long long)lg->name_off.size() - 1;
+  int32_t *d_remap;
+  CKR(ar.alloc(&d_remap, NC));
+  CK(cudaMemcpyAsync(d_remap, remap.data(), sizeof(int32_t) * (size_t)NC, cudaMemcpyHostToDevice, s));
+  k_remap_i32<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, d_remap, code);
+  c->launches++;
   // 6. counts per name
   unsigned long long *cnt;
   CKR(ar.alloc(&cnt, 2 * NG + 2));
   CK(cudaMemsetAsync(cnt, 0, sizeof(unsigned long long) * (size_t)(2 * NG + 2), s));
-  k_event_counts<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, flag, code, (int32_t)NG, cnt);
+  k_event_counts<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, ev.flag, code, (int32_t)NG, cnt);
   c->launches++;
   std::vector<unsigned long long> h_cnt((size_t)(2 * NG + 2));
   CK(cudaMemcpyAsync(h_cnt.data(), cnt, sizeof(unsigned long long) * h_cnt.size(), cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  lg->n_train.resize(NG);
-  lg->n_rank.resize(NG);
-  lg->train_at.assign(NG + 1, 0);
-  lg->rank_at.assign(NG + 1, 0);
+  CK(cudaStreamSynchronize(s));   // remap and h_cnt are locals
+  lg->n_train.resize(NG, 0);
+  lg->n_rank.resize(NG, 0);
+  lg->segs.emplace_back();
+  EvSeg &sg = lg->segs.back();
+  sg.train_at.assign(NG + 1, 0);
+  sg.rank_at.assign(NG + 1, 0);
   for (long long n = 0; n < NG; ++n) {
-    lg->n_train[n] = (int64_t)h_cnt[2 * n];
-    lg->n_rank[n] = (int64_t)h_cnt[2 * n + 1];
-    if (h_cnt[2 * n + 1] >= 0x7fffffffULL)
-      return set_error(CCO_E_UNSUPPORTED, "event name %lld: %llu events, at most 2^31 - 2 per name", n, h_cnt[2 * n + 1]);
-    lg->train_at[n + 1] = lg->train_at[n] + lg->n_train[n];
-    lg->rank_at[n + 1] = lg->rank_at[n] + lg->n_rank[n];
+    lg->n_train[n] += (int64_t)h_cnt[2 * n];
+    lg->n_rank[n] += (int64_t)h_cnt[2 * n + 1];
+    sg.train_at[n + 1] = sg.train_at[n] + (long long)h_cnt[2 * n];
+    sg.rank_at[n + 1] = sg.rank_at[n] + (long long)h_cnt[2 * n + 1];
   }
-  lg->n_prop = (long long)h_cnt[2 * NG];
-  lg->n_ignored = (long long)h_cnt[2 * NG + 1];
+  const long long NP = (long long)h_cnt[2 * NG];
+  lg->n_prop += NP;
+  lg->n_ignored += (long long)h_cnt[2 * NG + 1];
+  lg->n_lines += L;
   // 7. training and ranking events partitioned by name, file order inside a name: decoded ids and times
   uint32_t *idx;
-  CKR(event_partition(c, ar, L, flag, kEvTraining, code, (uint32_t)NG, &idx));
-  CKR(event_column(c, ar, lg, lg->train_at[NG], idx, kEvEntityId, sb, span, bb, lg->train_at, &lg->tu));
-  CKR(event_column(c, ar, lg, lg->train_at[NG], idx, kEvTargetId, sb, span, bb, lg->train_at, &lg->ti));
+  CKR(event_partition(c, ar, L, ev.flag, kEvTraining, code, (uint32_t)NG, &idx));
+  CKR(event_column(c, ar, lg, sg.train_at[NG], idx, kEvEntityId, ev.sb, ev.span, bb, sg.train_at, &sg.tu));
+  CKR(event_column(c, ar, lg, sg.train_at[NG], idx, kEvTargetId, ev.sb, ev.span, bb, sg.train_at, &sg.ti));
   ar.release(idx);
-  CKR(event_partition(c, ar, L, flag, kEvRanking, code, (uint32_t)NG, &idx));
-  const long long NR = lg->rank_at[NG];
-  CKR(event_column(c, ar, lg, NR, idx, kEvTargetId, sb, span, bb, lg->rank_at, &lg->ri));
-  CKR(ar.alloc(&lg->rtime, std::max<long long>(NR, 1)));
-  CKR(log_keep(ar, lg, lg->rtime));
+  CKR(event_partition(c, ar, L, ev.flag, kEvRanking, code, (uint32_t)NG, &idx));
+  const long long NR = sg.rank_at[NG];
+  CKR(event_column(c, ar, lg, NR, idx, kEvTargetId, ev.sb, ev.span, bb, sg.rank_at, &sg.ri));
+  CKR(ar.alloc(&sg.rtime, std::max<long long>(NR, 1)));
+  CKR(log_keep(ar, lg, sg.rtime));
   if (NR > 0) {
-    k_gather_i64<<<grid_for(NR, 256, c->sm_count), 256, 0, s>>>(NR, idx, tm, lg->rtime);
+    k_gather_i64<<<grid_for(NR, 256, c->sm_count), 256, 0, s>>>(NR, idx, ev.tm, sg.rtime);
     c->launches++;
   }
   ar.release(idx);
-  // 8. the items' properties (PEventStore.aggregateProperties), aggregated here: see event_properties
-  if (lg->n_prop > 0) CKR(event_properties(c, ar, lg, L, flag, tm, sb, span, bb));
+  // 8. the property-event lines, in line order, for the aggregation at finish (see event_log_finish)
+  if (NP > 0) {
+    CKR(event_partition(c, ar, L, ev.flag, kEvProperty, nullptr, 0, &idx));
+    long long *len8, *off;
+    CKR(ar.alloc(&len8, NP + 1));
+    CKR(ar.alloc(&off, NP + 1));
+    CK(cudaMemsetAsync(len8 + NP, 0, 8, s));
+    k_line_len<<<grid_for(NP, 256, c->sm_count), 256, 0, s>>>(NP, idx, ev.sb, ev.se, len8);
+    c->launches++;
+    CKR(exclusive_sum_i64(c, ar, len8, off, NP + 1));
+    long long total = 0;
+    std::vector<uint32_t> h_idx((size_t)NP);
+    CK(cudaMemcpyAsync(&total, off + NP, 8, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(h_idx.data(), idx, sizeof(uint32_t) * (size_t)NP, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    if (lg->pb_len + total > lg->pb_cap) {   // grow geometrically; 24 bytes of padding for event_pad
+      const long long cap = std::max(2 * lg->pb_cap, lg->pb_len + total);
+      unsigned char *p;
+      CKR(ar.alloc(&p, cap + 24));
+      CKR(log_keep(ar, lg, p));
+      if (lg->pb_len > 0) CK(cudaMemcpyAsync(p, lg->pb, (size_t)lg->pb_len, cudaMemcpyDeviceToDevice, s));
+      log_drop(lg, lg->pb);
+      lg->pb = p;
+      lg->pb_cap = cap;
+    }
+    k_line_gather<<<grid_for(NP * 32, 256, c->sm_count), 256, 0, s>>>(NP, idx, ev.sb, ev.se, bb, off, lg->pb + lg->pb_len);
+    c->launches++;
+    lg->pb_len += total;
+    for (uint32_t l : h_idx) lg->prop_line.push_back(base + (long long)l);
+  }
   CK(cudaStreamSynchronize(s));
   CK(cudaGetLastError());
-  g.ok = true;
+  return CCO_OK;
+}
+
+// one retained column of every segment, concatenated name-major (segments in order inside a name) into *out; the
+// segments' buffers of the column are freed as soon as it is built, so that the peak stays near one column above the
+// retained bytes.  at: each segment's entry offsets per name (train_at or rank_at); gat: the same for the whole log.
+static int event_cat_column(cco_event_log *lg, EvCol EvSeg::*col, std::vector<long long> EvSeg::*at, const std::vector<long long> &gat,
+                            EvCol *out) {
+  cco_ctx *c = lg->ctx;
+  cudaStream_t s = c->stream;
+  Arena ar(s);
+  const long long NG = (long long)gat.size() - 1;
+  std::vector<CatPiece> bytes, ents;
+  out->boff.assign(NG + 1, 0);
+  long long b = 0, e = 0;
+  for (long long g = 0; g < NG; ++g) {
+    out->boff[g] = b;
+    for (EvSeg &sg : lg->segs) {
+      const std::vector<long long> &sa = sg.*at;
+      if (g + 1 >= (long long)sa.size()) continue;   // a name first seen in a later chunk
+      const EvCol &sc = sg.*col;
+      CatPiece p{sc.w, sc.off, sc.boff[g], b, sc.boff[g + 1] - sc.boff[g], sa[g], e, sa[g + 1] - sa[g], true};
+      if (p.nb > 0) bytes.push_back(p);
+      if (p.ne > 0) ents.push_back(p);
+      b += p.nb;
+      e += p.ne;
+    }
+  }
+  out->boff[NG] = b;
+  const long long NW = (b + 7) / 8 + 2;
+  CKR(ar.alloc(&out->off, e + 1));
+  CKR(ar.alloc(&out->w, NW));
+  CatPiece *d_p;
+  CKR(ar.alloc(&d_p, bytes.size() + ents.size()));
+  CK(cudaMemcpyAsync(d_p, bytes.data(), sizeof(CatPiece) * bytes.size(), cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(d_p + bytes.size(), ents.data(), sizeof(CatPiece) * ents.size(), cudaMemcpyHostToDevice, s));
+  k_cat_words<<<grid_for(NW, 256, c->sm_count), 256, 0, s>>>(NW, b, d_p, (int)bytes.size(), out->w);
+  k_cat_entries<<<grid_for(e + 1, 256, c->sm_count), 256, 0, s>>>(e, b, d_p + bytes.size(), (int)ents.size(), out->off);
+  c->launches += 2;
+  CK(cudaStreamSynchronize(s));   // the pieces are locals
+  CKR(log_keep(ar, lg, out->off));
+  CKR(log_keep(ar, lg, out->w));
+  for (EvSeg &sg : lg->segs) {
+    log_drop(lg, (sg.*col).off);
+    log_drop(lg, (sg.*col).w);
+  }
+  return CCO_OK;
+}
+// the ranking times of every segment, name-major, as the ranking items
+static int event_cat_times(cco_event_log *lg, long long **out) {
+  cco_ctx *c = lg->ctx;
+  cudaStream_t s = c->stream;
+  Arena ar(s);
+  const long long NG = (long long)lg->rank_at.size() - 1;
+  std::vector<CatPiece> ents;
+  long long e = 0;
+  for (long long g = 0; g < NG; ++g)
+    for (EvSeg &sg : lg->segs) {
+      if (g + 1 >= (long long)sg.rank_at.size() || sg.rank_at[g + 1] == sg.rank_at[g]) continue;
+      ents.push_back(CatPiece{nullptr, sg.rtime, 0, 0, 0, sg.rank_at[g], e, sg.rank_at[g + 1] - sg.rank_at[g], false});
+      e += ents.back().ne;
+    }
+  CKR(ar.alloc(out, std::max<long long>(e, 1)));
+  CatPiece *d_p;
+  CKR(ar.alloc(&d_p, ents.size()));
+  CK(cudaMemcpyAsync(d_p, ents.data(), sizeof(CatPiece) * ents.size(), cudaMemcpyHostToDevice, s));
+  if (e > 0) {
+    k_cat_entries<<<grid_for(e, 256, c->sm_count), 256, 0, s>>>(e, -1, d_p, (int)ents.size(), *out);
+    c->launches++;
+  }
+  CK(cudaStreamSynchronize(s));
+  CKR(log_keep(ar, lg, *out));
+  for (EvSeg &sg : lg->segs) log_drop(lg, sg.rtime);
+  return CCO_OK;
+}
+
+// the staging is full: parse it up to its last '\n' and carry the bytes after it to its front, or, when it holds no '\n'
+// (one line fills it), double it
+static int event_flush(cco_event_log *lg) {
+  cco_ctx *c = lg->ctx;
+  cudaStream_t s = c->stream;
+  Arena ar(s);
+  if (lg->last_nl < 0) {
+    if (lg->staged >= (1LL << 31)) return event_error(((unsigned long long)lg->n_lines << 8) | kJsonLongLine);
+    const long long cap = 2 * lg->cap;
+    unsigned char *p;
+    CKR(ar.alloc(&p, cap + 24));
+    CKR(log_keep(ar, lg, p));
+    CK(cudaMemcpyAsync(p, lg->stage, (size_t)lg->staged, cudaMemcpyDeviceToDevice, s));
+    log_drop(lg, lg->stage);
+    lg->stage = p;
+    lg->cap = cap;
+    return CCO_OK;
+  }
+  const long long P = lg->last_nl + 1, carry = lg->staged - P;
+  unsigned char *tmp = nullptr;
+  if (carry > 0) {   // through scratch: the carry may overlap its destination
+    CKR(ar.alloc(&tmp, carry));
+    CK(cudaMemcpyAsync(tmp, lg->stage + P, (size_t)carry, cudaMemcpyDeviceToDevice, s));
+  }
+  CKR(event_chunk(lg, P, false));
+  if (carry > 0) CK(cudaMemcpyAsync(lg->stage, tmp, (size_t)carry, cudaMemcpyDeviceToDevice, s));
+  lg->staged = carry;
+  lg->last_nl = -1;
+  return CCO_OK;
+}
+
+static int event_log_begin(cco_ctx *c, int64_t chunk_bytes, cco_event_log **out) {
+  CK(cudaSetDevice(c->device));
+  cco_event_log *lg = new cco_event_log();
+  lg->ctx = c;
+  lg->name_off.assign(1, 0);
+  lg->train_at.assign(1, 0);
+  lg->rank_at.assign(1, 0);
+  lg->cap = std::max<int64_t>(chunk_bytes, 1);
+  Arena ar(c->stream);
+  const int rc = ar.alloc(&lg->stage, lg->cap + 24);
+  if (rc != CCO_OK) {
+    delete lg;
+    return rc;
+  }
+  log_keep(ar, lg, lg->stage);
   *out = lg;
+  return CCO_OK;
+}
+
+static int event_log_append(cco_event_log *lg, const char *bytes, int64_t len) {
+  cco_ctx *c = lg->ctx;
+  CK(cudaSetDevice(c->device));
+  nvtx_push("cco:event_log_append");
+  struct Pop { ~Pop() { nvtx_pop(); } } pop;
+  while (len > 0) {
+    if (lg->staged == lg->cap) CKR(event_flush(lg));
+    const long long take = std::min<long long>(len, lg->cap - lg->staged);
+    CK(cudaMemcpyAsync(lg->stage + lg->staged, bytes, (size_t)take, cudaMemcpyHostToDevice, c->stream));
+    const void *nl = memrchr(bytes, '\n', (size_t)take);
+    if (nl) lg->last_nl = lg->staged + ((const char *)nl - bytes);
+    lg->staged += take;
+    bytes += take;
+    len -= take;
+  }
+  CK(cudaStreamSynchronize(c->stream));   // the bytes are copied: the caller may reuse its buffer
+  return CCO_OK;
+}
+
+// the carried tail as the last chunk (its last line need not end in '\n'), the per-name limits, the retained columns
+// name-major, then the properties: event_properties once over the property-event lines of every chunk as a small log in
+// line order, so that the (eventTime, line) rule sees them as the whole read does
+static int event_log_finish(cco_event_log *lg) {
+  cco_ctx *c = lg->ctx;
+  cudaStream_t s = c->stream;
+  CK(cudaSetDevice(c->device));
+  nvtx_push("cco:event_log_finish");
+  struct Pop { ~Pop() { nvtx_pop(); } } pop;
+  if (lg->staged > 0) CKR(event_chunk(lg, lg->staged, lg->last_nl != lg->staged - 1));
+  log_drop(lg, lg->stage);
+  lg->stage = nullptr;
+  lg->staged = 0;
+  const long long NG = (long long)lg->name_off.size() - 1;
+  lg->train_at.assign(NG + 1, 0);
+  lg->rank_at.assign(NG + 1, 0);
+  for (long long n = 0; n < NG; ++n) {
+    if (lg->n_rank[n] >= 0x7fffffffLL)
+      return set_error(CCO_E_UNSUPPORTED, "event name %lld: %lld events, at most 2^31 - 2 per name", n, (long long)lg->n_rank[n]);
+    lg->train_at[n + 1] = lg->train_at[n] + lg->n_train[n];
+    lg->rank_at[n + 1] = lg->rank_at[n] + lg->n_rank[n];
+  }
+  if (lg->segs.size() == 1) {   // one chunk: its segment is the layout
+    EvSeg &sg = lg->segs[0];
+    lg->tu = sg.tu;
+    lg->ti = sg.ti;
+    lg->ri = sg.ri;
+    lg->rtime = sg.rtime;
+  } else if (lg->segs.size() > 1) {
+    CKR(event_cat_column(lg, &EvSeg::tu, &EvSeg::train_at, lg->train_at, &lg->tu));
+    CKR(event_cat_column(lg, &EvSeg::ti, &EvSeg::train_at, lg->train_at, &lg->ti));
+    CKR(event_cat_column(lg, &EvSeg::ri, &EvSeg::rank_at, lg->rank_at, &lg->ri));
+    CKR(event_cat_times(lg, &lg->rtime));
+  }
+  lg->segs.clear();
+  if (lg->n_prop > 0) {
+    mail_reset(c);
+    Arena ar(s);
+    CKR(event_pad(c, lg->pb, lg->pb_len));
+    EvLines ev;
+    CKR(event_lines(c, ar, (const uint64_t *)lg->pb, lg->pb_len, false, 0, &ev));   // judged once already
+    CKR(event_properties(c, ar, lg, ev.L, ev.flag, ev.tm, ev.sb, ev.span, lg->pb, lg->prop_line.data()));
+    CK(cudaStreamSynchronize(s));
+  }
+  log_drop(lg, lg->pb);
+  lg->pb = nullptr;
+  lg->prop_line = std::vector<long long>();
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  lg->finished = true;
   return CCO_OK;
 }
 
@@ -3960,17 +4230,62 @@ static int log_rankings(const cco_event_log *lg, int32_t n_rank, const cco_log_r
   }
   return CCO_OK;
 }
+// a failed log answers every call with its first error's message; a log in progress is not read before finish
+static int log_state(const cco_event_log *lg, bool want_finished) {
+  if (lg->fail != CCO_OK) return set_error(CCO_E_INVALID_ARG, "the read of this log failed: %s", lg->fail_msg.c_str());
+  if (lg->finished != want_finished)
+    return set_error(CCO_E_INVALID_ARG, want_finished ? "the log is not finished (cco_event_log_finish)" : "the log is finished");
+  return CCO_OK;
+}
+static int log_fail(cco_event_log *lg, int rc) {
+  if (rc != CCO_OK) {
+    lg->fail = rc;
+    lg->fail_msg = g_err;
+  }
+  return rc;
+}
 }  // namespace cco
+
+int cco_event_log_begin(cco_ctx_t *ctx, int64_t chunk_bytes, cco_event_log_t **out) {
+  if (!ctx || !out || chunk_bytes < 1) return set_error(CCO_E_INVALID_ARG, "null argument or chunk_bytes < 1");
+  *out = nullptr;
+  if (!ctx->members.empty()) return set_error(CCO_E_UNSUPPORTED, "an event log is resident on one GPU: read it on a per-GPU context");
+  return event_log_begin(ctx, chunk_bytes, out);
+}
+
+int cco_event_log_append(cco_event_log_t *lg, const char *bytes, int64_t len) {
+  if (!lg || len < 0 || (len > 0 && !bytes)) return set_error(CCO_E_INVALID_ARG, "null argument or negative length");
+  CKR(log_state(lg, false));
+  return log_fail(lg, event_log_append(lg, bytes, len));
+}
+
+int cco_event_log_finish(cco_event_log_t *lg) {
+  if (!lg) return set_error(CCO_E_INVALID_ARG, "null argument");
+  CKR(log_state(lg, false));
+  return log_fail(lg, event_log_finish(lg));
+}
 
 int cco_event_log_read(cco_ctx_t *ctx, const char *bytes, int64_t len, cco_event_log_t **out) {
   if (!ctx || !out || len < 0 || (len > 0 && !bytes)) return set_error(CCO_E_INVALID_ARG, "null argument or negative length");
   *out = nullptr;
   if (!ctx->members.empty()) return set_error(CCO_E_UNSUPPORTED, "an event log is resident on one GPU: read it on a per-GPU context");
-  return event_log_read(ctx, bytes, len, out);
+  nvtx_push("cco:event_log_read");
+  struct Pop { ~Pop() { nvtx_pop(); } } pop;
+  cco_event_log *lg = nullptr;
+  CKR(event_log_begin(ctx, std::max<int64_t>(len, 1), &lg));
+  int rc = event_log_append(lg, bytes, len);
+  if (rc == CCO_OK) rc = event_log_finish(lg);
+  if (rc != CCO_OK) {
+    event_log_release(lg);
+    return rc;
+  }
+  *out = lg;
+  return CCO_OK;
 }
 
 int cco_event_log_info(const cco_event_log_t *lg, cco_event_log_info_t *out) {
   if (!lg || !out) return set_error(CCO_E_INVALID_ARG, "null argument");
+  CKR(log_state(lg, true));
   out->n_lines = lg->n_lines;
   out->names = cco_dictionary_t{(int64_t)lg->n_train.size(), lg->name_off.data(), lg->name_bytes.data()};
   out->n_training = lg->n_train.data();
@@ -3987,6 +4302,7 @@ int cco_event_log_ingest(cco_ctx_t *c, const cco_event_log_t *lg, int32_t n_name
   if (!c || !lg || !names || !out || n_names < 1) return set_error(CCO_E_INVALID_ARG, "bad argument");
   *out = nullptr;
   if (!c->members.empty() || lg->ctx != c) return set_error(CCO_E_UNSUPPORTED, "ingest a log on the per-GPU context that read it");
+  CKR(log_state(lg, true));
   std::vector<int> codes(n_names);
   for (int t = 0; t < n_names; ++t) {
     if (!names[t]) return set_error(CCO_E_INVALID_ARG, "null event name %d", t);
@@ -4026,6 +4342,7 @@ int cco_format_model_log(cco_ctx_t *ctx, const cco_result_t *res, int32_t n_name
                          const cco_log_ranking_t *rankings, char **out_bytes, int64_t *out_len) {
   if (!ctx || !lg) return set_error(CCO_E_INVALID_ARG, "null argument");
   if (!ctx->members.empty() || lg->ctx != ctx) return set_error(CCO_E_UNSUPPORTED, "format on the per-GPU context that read the log");
+  CKR(log_state(lg, true));
   std::vector<cco_ranking_t> rk;
   LogStreams ls;
   CKR(log_rankings(lg, n_rankings, rankings, &rk, &ls));
@@ -4040,6 +4357,7 @@ int cco_rerank_model_log(cco_ctx_t *ctx, const char *body, int64_t body_len, con
                          const cco_log_ranking_t *rankings, char **out_bytes, int64_t *out_len) {
   if (!ctx || !lg) return set_error(CCO_E_INVALID_ARG, "null argument");
   if (!ctx->members.empty() || lg->ctx != ctx) return set_error(CCO_E_UNSUPPORTED, "rerank on the per-GPU context that read the log");
+  CKR(log_state(lg, true));
   std::vector<cco_ranking_t> rk;
   LogStreams ls;
   CKR(log_rankings(lg, n_rankings, rankings, &rk, &ls));

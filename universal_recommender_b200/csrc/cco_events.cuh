@@ -11,6 +11,8 @@
 //                                  (eventTime, line) order, the last $delete and $set per item, the members of the
 //                                  properties objects sorted by (item, field) after that order, the winning member per
 //                                  (item, field), one presence entry per item left without a field, the triples
+//   k_line_len / k_line_gather     streamed reads: the property-event lines of each chunk, kept for the aggregation at finish
+//   k_cat_words / k_cat_entries    streamed reads: the chunks' name-partitioned columns concatenated name-major at finish
 #pragma once
 
 #include <cuda_runtime.h>
@@ -379,6 +381,89 @@ __global__ void k_prop_counts(long long n, const uint8_t *__restrict__ flag, uin
 }
 __global__ void k_remap_i32(long long n, const int32_t *__restrict__ map, int32_t *__restrict__ x) {
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) x[i] = map[x[i]];
+}
+
+// ---- streamed reading ------------------------------------------------------------------------------------------------
+// the property-event lines of a chunk, kept for the aggregation at finish: len[i] = bytes of line idx[i] + its '\n'
+__global__ void k_line_len(long long n, const uint32_t *__restrict__ idx, const long long *__restrict__ sb, const long long *__restrict__ se,
+                           long long *__restrict__ len) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    len[i] = se[idx[i]] - sb[idx[i]] + 1;
+}
+// one warp per listed line: its bytes to out + off[i], then a '\n' (the last line of a read may not have one)
+__global__ void k_line_gather(long long n, const uint32_t *__restrict__ idx, const long long *__restrict__ sb, const long long *__restrict__ se,
+                              const unsigned char *__restrict__ body, const long long *__restrict__ off, unsigned char *__restrict__ out) {
+  const int lane = threadIdx.x & 31;
+  const long long warp = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5, nwarps = ((long long)gridDim.x * blockDim.x) >> 5;
+  for (long long i = warp; i < n; i += nwarps) {
+    const long long b = sb[idx[i]], m = se[idx[i]] - b;
+    unsigned char *o = out + off[i];
+    for (long long j = lane; j < m; j += 32) o[j] = body[b + j];
+    if (lane == 0) o[m] = '\n';
+  }
+}
+
+// One piece of a concatenation: the bytes [src_b, src_b + nb) of a segment's words go to [dst_b, dst_b + nb) of the
+// output, and its entries [src_e, src_e + ne) of `e` to [dst_e, dst_e + ne), shifted by dst_b - src_b (offsets) or not
+// (shift false: times).  Pieces are in output order.
+struct CatPiece {
+  const uint64_t *w;
+  const long long *e;
+  long long src_b, dst_b, nb, src_e, dst_e, ne;
+  bool shift;
+};
+// the last piece whose start (`at` of the byte or the entry side) is <= x; pieces are sorted by it
+template <bool kBytes>
+__device__ __forceinline__ int cat_find(const CatPiece *__restrict__ pc, int np, long long x) {
+  int lo = 0, hi = np - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if ((kBytes ? pc[mid].dst_b : pc[mid].dst_e) <= x) lo = mid;
+    else hi = mid - 1;
+  }
+  return lo;
+}
+// output word q of the concatenated bytes (pieces with nb > 0; words past `total` bytes are zero): a word inside one piece is
+// a funnel shift of two source words (segments are not 8-byte aligned relative to each other), a word across pieces is
+// assembled byte by byte
+__global__ void k_cat_words(long long n_words, long long total, const CatPiece *__restrict__ pc, int np, uint64_t *__restrict__ out) {
+  for (long long q = blockIdx.x * (long long)blockDim.x + threadIdx.x; q < n_words; q += (long long)gridDim.x * blockDim.x) {
+    const long long pos = q * 8;
+    if (pos >= total || np == 0) {
+      out[q] = 0;
+      continue;
+    }
+    int p = cat_find<true>(pc, np, pos);
+    const CatPiece &a = pc[p];
+    if (pos + 8 <= a.dst_b + a.nb) {
+      const long long s = a.src_b + (pos - a.dst_b);
+      const int sh = (int)(s & 7) * 8;
+      const uint64_t lo = a.w[s >> 3];
+      out[q] = sh ? (lo >> sh) | (a.w[(s >> 3) + 1] << (64 - sh)) : lo;
+      continue;
+    }
+    uint64_t x = 0;
+    for (int j = 0; j < 8; ++j) {
+      const long long bp = pos + j;
+      while (p < np && bp >= pc[p].dst_b + pc[p].nb) ++p;
+      if (p == np || bp >= total) break;
+      const unsigned char *src = (const unsigned char *)pc[p].w;
+      x |= (uint64_t)src[pc[p].src_b + (bp - pc[p].dst_b)] << (8 * j);
+    }
+    out[q] = x;
+  }
+}
+// output entry i of the concatenated offsets or times (pieces with ne > 0); last >= 0: out[n] = last
+__global__ void k_cat_entries(long long n, long long last, const CatPiece *__restrict__ pc, int np, long long *__restrict__ out) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n + (last >= 0); i += (long long)gridDim.x * blockDim.x) {
+    if (i == n) {
+      out[n] = last;
+      continue;
+    }
+    const CatPiece &a = pc[cat_find<false>(pc, np, i)];
+    const long long v = a.e[a.src_e + (i - a.dst_e)];
+    out[i] = a.shift ? v - a.src_b + a.dst_b : v;
+  }
 }
 
 }  // namespace cco

@@ -33,6 +33,7 @@ What the mirror accepts differs from the device in these ways:
 from __future__ import annotations
 
 import json
+import os
 import re
 from json.decoder import scanstring
 from dataclasses import dataclass, field
@@ -200,7 +201,47 @@ class DataSourceEvents:
     property_events: list = field(default_factory=list)
 
 
-def read_export(data: bytes) -> DataSourceEvents:
+def export_parts(directory) -> list[str]:
+    """the part files of a `pio export` directory (Spark's saveAsTextFile: part-NNNNN files and a _SUCCESS marker) in name
+    order; _SUCCESS, checksum (*.crc) and hidden files and empty parts are skipped"""
+    names = sorted(n for n in os.listdir(directory) if n.startswith("part-") and not n.endswith(".crc"))
+    paths = [os.path.join(directory, n) for n in names]
+    return [p for p in paths if os.path.isfile(p) and os.path.getsize(p) > 0]
+
+
+def part_lines(path) -> int:
+    """lines of one part: every '\\n' ends one, and a last line without it counts too"""
+    n, last = 0, b"\n"
+    with open(path, "rb") as f:
+        for block in iter(lambda: f.read(1 << 24), b""):
+            n += block.count(b"\n")
+            last = block[-1:]
+    return n + (last != b"\n")
+
+
+def locate_line(counts: Sequence[int], line: int) -> tuple[int, int]:
+    """global 0-based line of parts read in order (each part's lines kept apart) -> (part index, line in that part)"""
+    for k, n in enumerate(counts):
+        if line < n:
+            return k, line
+        line -= n
+    raise ValueError("line past the last part")
+
+
+def join_parts(paths: Sequence) -> bytes:
+    """the bytes of parts read in order; a part that does not end in '\\n' is followed by one, so that parts never join lines"""
+    out = []
+    for p in paths:
+        with open(p, "rb") as f:
+            b = f.read()
+        out.append(b + b"\n" if b and not b.endswith(b"\n") else b)
+    return b"".join(out)
+
+
+def read_export(data) -> DataSourceEvents:
+    """data: the export's bytes, or the directory `pio export` writes (its parts joined as join_parts does)"""
+    if isinstance(data, (str, os.PathLike)):
+        data = join_parts(export_parts(data))
     names: dict = {}
     events, ranking, props, ignored = [], {}, [], 0
     for i, raw in enumerate(export_lines(bytes(data))):

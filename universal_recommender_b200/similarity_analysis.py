@@ -6,6 +6,9 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import queue
+import re
+import threading
 import weakref
 from dataclasses import dataclass
 from typing import Optional, Sequence
@@ -13,7 +16,24 @@ from typing import Optional, Sequence
 import numpy as np
 
 from . import _native as N
+from . import events as E
 from .indexed_dataset import IndexedDataset
+
+# device staging and host buffer size of a streamed export read (CcoContext.read_events): DESIGN.md section 8 has the
+# sweep it was chosen from
+DEFAULT_CHUNK_BYTES = 1 << 28
+
+
+def _name_part(e: Exception, paths) -> None:
+    """add the part file and its 0-based line to the message of a parse error of a multi-part read (counted only here)"""
+    m = re.search(r"line (\d+)", str(e))
+    if m is None or len(paths) < 2:
+        return
+    try:
+        k, line = E.locate_line([E.part_lines(p) for p in paths], int(m.group(1)))
+    except (OSError, ValueError):
+        return
+    e.args = (f"{e.args[0]} (part {paths[k]}, line {line})",)
 
 
 @dataclass
@@ -304,33 +324,109 @@ class CcoContext:
             rk[k] = N.LogRankingT(nb, N.POP_MODES.get(mode, -1), len(en), int(start_ms), int(end_ms), arr)
         return rk
 
-    def read_events(self, src) -> "EventLog":
-        """cco_event_log_read: a PredictionIO event export (JSON lines, as `pio export` writes them) parsed on the device.
-        src = bytes, a buffer, or a path: a file is read straight into pinned host memory (no Python objects per line).
+    def read_events(self, src, chunk_bytes: Optional[int] = None) -> "EventLog":
+        """A PredictionIO event export (JSON lines, as `pio export` writes them) parsed on the device.  src is one of
+          - bytes or a buffer: one read (cco_event_log_read), or chunks of chunk_bytes when it is given;
+          - a file path, a directory as `pio export` writes it (its part-* files in name order; events.export_parts) or a
+            sequence of paths: streamed (cco_event_log_begin / _append / _finish) through two pinned buffers of
+            chunk_bytes, one filled by a reader thread while the other is appended.  A part that does not end in '\\n' is
+            followed by one.  A parse error names the part and its 0-based line besides the global line;
+          - an iterable of buffers (a generator, say): streamed, each appended as it comes.
+        chunk_bytes defaults to DEFAULT_CHUNK_BYTES for streamed sources; it is also the device staging.  The log is the one
+        cco_event_log_read of the concatenated bytes gives.
         -> EventLog (free with .free(), or use it as a context manager; close() of this context frees the logs still open)."""
-        if isinstance(src, str) or hasattr(src, "__fspath__"):
-            path = os.fspath(src)
-            n = os.path.getsize(path)
-            buf = self.host_array(n, np.uint8)
-            with open(path, "rb", buffering=0) as f:
-                got = f.readinto(memoryview(buf)) if n else 0
-            if got != n:
-                self.host_free(buf)
-                raise OSError(f"{path}: read {got} of {n} bytes")
-            pinned = buf
-        else:
+        if isinstance(src, (bytes, bytearray, memoryview, np.ndarray)) and chunk_bytes is None:
             buf = np.frombuffer(src, dtype=np.uint8) if not isinstance(src, np.ndarray) else np.ascontiguousarray(src, dtype=np.uint8)
-            pinned = None
-        h = C.c_void_p()
-        try:
+            h = C.c_void_p()
             N.check(self._L.cco_event_log_read(self._h, buf.ctypes.data if len(buf) else None, len(buf), C.byref(h)))
+            return self._adopt_log(h)
+        chunk = int(chunk_bytes or DEFAULT_CHUNK_BYTES)
+        paths = None
+        if isinstance(src, (str, os.PathLike)):
+            p = os.fspath(src)
+            paths = E.export_parts(p) if os.path.isdir(p) else [p]
+        elif isinstance(src, (list, tuple)) and all(isinstance(x, (str, os.PathLike)) for x in src):
+            paths = [os.fspath(x) for x in src]
+        h = C.c_void_p()
+        N.check(self._L.cco_event_log_begin(self._h, chunk, C.byref(h)))
+        try:
+            if paths is not None:
+                self._append_files(h, paths, chunk)
+            else:
+                for b in ([src] if isinstance(src, (bytes, bytearray, memoryview, np.ndarray)) else src):
+                    buf = np.frombuffer(b, dtype=np.uint8) if not isinstance(b, np.ndarray) else np.ascontiguousarray(b, dtype=np.uint8)
+                    if len(buf):
+                        N.check(self._L.cco_event_log_append(h, buf.ctypes.data, len(buf)))
+            try:
+                N.check(self._L.cco_event_log_finish(h))
+            except N.CcoError as e:
+                if paths is not None:
+                    _name_part(e, paths)
+                raise
         except BaseException:
-            if pinned is not None:
-                self.host_free(pinned)
+            self._L.cco_event_log_free(h)
             raise
-        log = EventLog(self, h, pinned)
+        return self._adopt_log(h)
+
+    def _adopt_log(self, h) -> "EventLog":
+        log = EventLog(self, h, None)
         self._logs.add(log)
         return log
+
+    def _append_files(self, h, paths, chunk: int):
+        """append the files in order through two pinned buffers: a reader thread fills one while the other is appended
+        (readinto and the ctypes call both release the GIL)"""
+        bufs = [self.host_array(chunk, np.uint8) for _ in range(2)]
+        free, full = queue.Queue(), queue.Queue()
+        free.put(0)
+        free.put(1)
+
+        def reader():
+            try:
+                for path in paths:
+                    last = b"\n"
+                    with open(path, "rb", buffering=0) as f:
+                        while True:
+                            k = free.get()
+                            if k is None:
+                                return
+                            n = f.readinto(memoryview(bufs[k]))
+                            if not n:
+                                free.put(k)
+                                break
+                            last = bytes(bufs[k][n - 1:n])
+                            full.put((k, n))
+                    if last != b"\n":   # parts never join lines
+                        full.put((-1, 1))
+                full.put(None)
+            except BaseException as e:   # handed to the appending thread
+                full.put(e)
+
+        t = threading.Thread(target=reader, daemon=True)
+        t.start()
+        try:
+            while True:
+                item = full.get()
+                if item is None:
+                    break
+                if isinstance(item, BaseException):
+                    raise item
+                k, n = item
+                try:
+                    if k < 0:
+                        N.check(self._L.cco_event_log_append(h, b"\n", 1))
+                    else:
+                        N.check(self._L.cco_event_log_append(h, bufs[k].ctypes.data, n))
+                except N.CcoError as e:
+                    _name_part(e, paths)
+                    raise
+                if k >= 0:
+                    free.put(k)
+        finally:
+            free.put(None)   # a reader still waiting for a buffer stops
+            t.join()
+            for b in bufs:
+                self.host_free(b)
 
     def ingest_event_log(self, log: "EventLog", names: Sequence[str], min_events_per_user: int = 0):
         """cco_event_log_ingest: ingest_strings on the log's training events of `names` (type t = names[t]), from HBM.

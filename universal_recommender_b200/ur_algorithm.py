@@ -200,15 +200,16 @@ def _log_rankings(ap: URAlgorithmParams, now_ms: Optional[int]) -> list:
 
 
 def _read_log(export, ctx: CcoContext):
-    """(log, owned): an EventLog as given, or one read from bytes / a buffer / a path"""
+    """(log, owned): an EventLog as given, or one read by CcoContext.read_events (bytes, a buffer, a path, a `pio export`
+    directory, a sequence of paths or an iterable of buffers)"""
     from .similarity_analysis import EventLog
     return (export, False) if isinstance(export, EventLog) else (ctx.read_events(export), True)
 
 
 def calc_all_from_events(export, ap: URAlgorithmParams, min_events_per_user: Optional[int] = None, now_ms: Optional[int] = None,
                          ctx: CcoContext | None = None, flags: int = 0) -> bytes:
-    """calc_all_on_device from a PredictionIO event export (bytes, a buffer, a path or an EventLog of this context): the
-    export is copied to the GPU once and parsed there (the DataSource: include/cco_b200.h cco_event_log_read); the training
+    """calc_all_on_device from a PredictionIO event export (any source CcoContext.read_events takes, or an EventLog of this
+    context): the export is copied to the GPU and parsed there (the DataSource: include/cco_b200.h cco_event_log_read); the training
     events, the ranking streams and the items' properties, aggregated there from their $set / $unset / $delete events,
     stay in HBM.  Property values are spliced as written.  Same decisions as calc_all_on_device."""
     _check_recs_model(ap)
