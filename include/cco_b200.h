@@ -506,6 +506,37 @@ int cco_rerank_model_log(cco_ctx_t *ctx, const char *body, int64_t body_len, con
 int cco_event_log_free(cco_event_log_t *log);
 
 /*
+ * The DataSource's eventWindow (engine.json datasource.params.eventWindow, DataSource.scala:39,55,69-70): PredictionIO's
+ * SelfCleaningDataSource cleans the event store before the training read, the property aggregation and PopModel's reads,
+ * so all three selections see only the cleaned events.  Its rules, restated from PredictionIO 0.12's cleanPEvents
+ * [RECALL, unverifiable here], in this order:
+ *  - expiry (cutoff_ms > INT64_MIN): an event is kept iff eventTime > cutoff_ms (strictly), or its event is "$set" or
+ *    "$unset" whatever its time.  A "$delete" is not exempt: an expired one is dropped, so the $sets before it count again.
+ *    The caller computes cutoff_ms = now - Duration(duration).toMillis; the library parses no duration string;
+ *  - compressProperties is assumed to preserve what aggregateProperties returns: it has no field here;
+ *  - remove_duplicates: events equal in everything but eventId, eventTime and creationTime collapse to one, the one with
+ *    the latest eventTime, ties to the later line (PredictionIO keeps an arbitrary one).  The identity: event, entityType,
+ *    entityId, targetEntityType, targetEntityId and prId as decoded strings (null = absent), the text of tags (absent, null
+ *    = []) and the properties as the set of their top-level members (decoded name, trimmed value text, the last of a
+ *    repeated name; absent = {}).  Nested values compare by their trimmed text, where json4s compares numbers by value and
+ *    objects without regard to member order; a `pio export` spells equal values alike, but for the member order of nested
+ *    objects.  Since the bytes of earlier chunks are gone by finish, the identity is a 128-bit hash: two of n distinct
+ *    events collide with probability about n^2 / 2^129 (10^-21 at 10^9 lines).
+ * Parsing and checks are unchanged: an expired or duplicate line that is malformed fails as before, naming its line.  With
+ * w == NULL (cco_event_log_begin) every output is identical to a read without the window.  info counts after the window:
+ * expired and duplicate lines are in no count but the stats (n_lines still counts every line).  Any split of the bytes
+ * gives the same log and stats, duplicates across chunks included.  The cleaned events are not written back.
+ */
+typedef struct {
+  int64_t cutoff_ms;               /* INT64_MIN: nothing expires */
+  int32_t remove_duplicates;       /* 0 or 1 */
+  int32_t reserved;                /* 0 */
+} cco_event_window_t;
+int cco_event_log_begin_window(cco_ctx_t *ctx, int64_t chunk_bytes, const cco_event_window_t *w /* nullable */, cco_event_log_t **out);
+/* after finish: the lines the window dropped as expired and as duplicates */
+int cco_event_log_window_stats(const cco_event_log_t *log, int64_t *n_expired, int64_t *n_duplicates);
+
+/*
  * Debug/parity entry (tests only): full integer co-occurrence matrix A^T B of two canonical
  * binary matrices computed by the same accumulation kernel as cco_train, no LLR, no top-k.
  * Output CSR over the columns of A with ascending column ids, malloc'ed; free with cco_free.

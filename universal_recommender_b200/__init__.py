@@ -19,6 +19,7 @@ Host-side mirror of the reference interface for this path:
 """
 from ._native import (CcoError, CcoInvalidArgument, FLAG_ASSUME_CANONICAL, FLAG_ENTROPY_VARARGS, FLAG_RESULT_NO_COUNT,
                       FLAG_RESULT_NO_LLR, FLAG_ROWRATE_INTDIV, LIB_PATH)
+from .events import DataSourceParams, EventWindow
 from .indexed_dataset import BiDictionary, IndexedDataset
 from .preparator import prepare, prepare_on_device
 from .similarity_analysis import (CcoContext, DownsamplableCrossOccurrenceDataset, EventLog, SimilarityAnalysis,
@@ -28,7 +29,7 @@ from .ur_algorithm import (DefaultURAlgoParams, IndicatorParams, URAlgorithmPara
 from .ur_model import RankingParams
 
 __all__ = [
-    "BiDictionary", "CcoContext", "CcoError", "CcoInvalidArgument", "DefaultURAlgoParams",
+    "BiDictionary", "CcoContext", "CcoError", "CcoInvalidArgument", "DataSourceParams", "DefaultURAlgoParams", "EventWindow",
     "DownsamplableCrossOccurrenceDataset", "IndexedDataset", "IndicatorParams", "SimilarityAnalysis",
     "EventLog", "RankingParams", "URAlgorithmParams", "calc_all", "calc_all_from_events", "calc_all_on_device", "calc_pop_from_events",
     "calc_pop_on_device", "decode_ids", "default_context", "encode_ids", "prepare", "prepare_on_device",

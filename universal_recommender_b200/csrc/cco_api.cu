@@ -3400,6 +3400,7 @@ struct EvCol {
 struct EvSeg {
   EvCol tu, ti, ri;
   long long *rtime = nullptr;
+  long long *tline = nullptr, *rline = nullptr;   // removeDuplicates: the global line of each training / ranking entry
   std::vector<long long> train_at, rank_at;
 };
 struct cco_event_log {
@@ -3429,6 +3430,15 @@ struct cco_event_log {
   unsigned char *pb = nullptr;
   long long pb_len = 0, pb_cap = 0;
   std::vector<long long> prop_line;
+  // the eventWindow (cco_event_log_begin_window): lines at or before cutoff expire ($set / $unset excepted); with dedup
+  // each retained line leaves a WinRec (n_rec of them) for removeDuplicates at finish, and the layout keeps each
+  // retained entry's global line (tline / rline) until the columns are compacted
+  long long cutoff = INT64_MIN;
+  bool dedup = false;
+  long long n_expired = 0, n_dup = 0;
+  WinRec *rec = nullptr;
+  long long n_rec = 0, rec_cap = 0;
+  long long *tline = nullptr, *rline = nullptr;
   bool finished = false;
   int fail = CCO_OK;                           // a failed append / finish: every later call returns it with fail_msg
   std::string fail_msg;
@@ -3805,9 +3815,11 @@ struct EvLines {
   long long L = 0;
   long long *sb = nullptr, *se = nullptr, *tm = nullptr;
   int2 *span = nullptr;
+  int2 *xspan = nullptr;   // with_x: the spans of "prId" and "tags" (EventSinkX)
   uint8_t *flag = nullptr;
 };
-static int event_lines(cco_ctx *c, Arena &ar, const uint64_t *w, long long len, bool open_tail, long long line_base, EvLines *ev) {
+static int event_lines(cco_ctx *c, Arena &ar, const uint64_t *w, long long len, bool open_tail, long long line_base, EvLines *ev,
+                       bool with_x = false) {
   cudaStream_t s = c->stream;
   const unsigned char *bb = (const unsigned char *)w;
   const unsigned long long base = (unsigned long long)line_base << 8;
@@ -3848,7 +3860,13 @@ static int event_lines(cco_ctx *c, Arena &ar, const uint64_t *w, long long len, 
   CKR(ar.alloc(&err, 1));
   CK(cudaMemsetAsync(ev->span, 0xff, sizeof(int2) * (size_t)L * kEvSlots, s));
   CK(cudaMemsetAsync(err, 0xff, 8, s));
-  k_json_members<<<grid_for(L * 32, 256, c->sm_count), 256, 0, s>>>(L, ev->sb, ev->se, bb, EventSink{ev->span, bb}, err);
+  if (with_x) {
+    CKR(ar.alloc(&ev->xspan, L * kEvXSlots));
+    CK(cudaMemsetAsync(ev->xspan, 0xff, sizeof(int2) * (size_t)L * kEvXSlots, s));
+    k_json_members<<<grid_for(L * 32, 256, c->sm_count), 256, 0, s>>>(L, ev->sb, ev->se, bb, EventSinkX{ev->span, ev->xspan, bb}, err);
+  } else {
+    k_json_members<<<grid_for(L * 32, 256, c->sm_count), 256, 0, s>>>(L, ev->sb, ev->se, bb, EventSink{ev->span, bb}, err);
+  }
   c->launches++;
   CKR(mail_fetch(c, &h_err, err, 8));
   CKR(mail_wait(c));
@@ -3870,6 +3888,122 @@ static int event_pad(cco_ctx *c, unsigned char *buf, long long len) {
   return CCO_OK;
 }
 
+// removeDuplicates: the global line of each of the n entries of a chunk's column (idx: the chunk lines), kept by the log
+static int win_entry_lines(cco_event_log *lg, Arena &ar, long long n, const uint32_t *idx, long long base, long long **out) {
+  CKR(ar.alloc(out, std::max<long long>(n, 1)));
+  CKR(log_keep(ar, lg, *out));
+  if (n > 0) {
+    k_win_lines<<<grid_for(n, 256, lg->ctx->sm_count), 256, 0, lg->ctx->stream>>>(n, idx, base, *out);
+    lg->ctx->launches++;
+  }
+  return CCO_OK;
+}
+// removeDuplicates, per chunk: the identity hash of every retained line (not expired) into lg->rec.  The identity is the
+// decoded event, entityType, entityId, targetEntityType, targetEntityId and prId (null = absent), the tags text (absent,
+// null = []) and the set of the properties' top-level members (decoded name, trimmed value text; the last of a repeated
+// name; absent = {}).  A properties object the tokenizer cannot split (the line is read all the same) is its text.
+static int win_records(cco_event_log *lg, Arena &ar, const EvLines &ev, const int32_t *code, long long base) {
+  cco_ctx *c = lg->ctx;
+  cudaStream_t s = c->stream;
+  const long long L = ev.L;
+  const unsigned char *bb = lg->stage;
+  uint32_t *keep, *pos, *ridx;
+  CKR(ar.alloc(&keep, L + 1));
+  CKR(ar.alloc(&pos, L + 1));
+  CK(cudaMemsetAsync(keep + L, 0, 4, s));
+  k_win_keep_lines<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, ev.flag, keep);
+  c->launches++;
+  CKR(exclusive_sum_u32(c, ar, keep, pos, L + 1));
+  uint32_t R32 = 0;
+  CKR(mail_fetch(c, &R32, pos + L, 4));
+  CKR(mail_wait(c));
+  const long long R = R32;
+  if (R == 0) return CCO_OK;
+  CKR(ar.alloc(&ridx, R));
+  k_win_scatter<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, keep, pos, ridx);
+  // the properties' members: count pass with each span's verdict, then the members of the well-formed spans
+  long long *pb, *pe, *mcnt, *moff;
+  int *codes;
+  unsigned long long *err;
+  CKR(ar.alloc(&pb, R));
+  CKR(ar.alloc(&pe, R));
+  CKR(ar.alloc(&mcnt, R + 1));
+  CKR(ar.alloc(&moff, R + 1));
+  CKR(ar.alloc(&codes, R));
+  CKR(ar.alloc(&err, 1));
+  CK(cudaMemsetAsync(mcnt + R, 0, 8, s));
+  k_win_prop_spans<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, ridx, ev.sb, ev.span, pb, pe);
+  k_json_members<<<grid_for(R * 32, 256, c->sm_count), 256, 0, s>>>(R, pb, pe, bb, WinMemberSink<false>{mcnt, codes, nullptr, nullptr}, err);
+  c->launches += 3;
+  CKR(exclusive_sum_i64(c, ar, mcnt, moff, R + 1));
+  long long M = 0;
+  CKR(mail_fetch(c, &M, moff + R, 8));
+  CKR(mail_wait(c));
+  JMember *mem;
+  CKR(ar.alloc(&mem, std::max<long long>(M, 1)));
+  if (M > 0) {
+    k_json_members<<<grid_for(R * 32, 256, c->sm_count), 256, 0, s>>>(R, pb, pe, bb, WinMemberSink<true>{nullptr, codes, moff, mem}, err);
+    c->launches++;
+  }
+  // decoded strings (six per line, then the member names) and raw texts (tags, unsplit properties, member values), hashed
+  const long long ND = kWinStr * R + M, NR = 2 * R + M;
+  JMember *jm;
+  CKR(ar.alloc(&jm, ND));
+  k_win_strings<<<grid_for(ND, 256, c->sm_count), 256, 0, s>>>(R, ridx, ev.sb, ev.span, ev.xspan, bb, M, mem, jm);
+  c->launches++;
+  DevStrCol d;
+  long long d_bytes = 0;
+  CKR(json_decode(c, ar, ND, jm, bb, &d, &d_bytes));
+  ar.release(jm);
+  ulonglong2 *hd, *hr;
+  long long *rb, *re;
+  CKR(ar.alloc(&hd, ND));
+  CKR(ar.alloc(&hr, NR));
+  CKR(ar.alloc(&rb, NR));
+  CKR(ar.alloc(&re, NR));
+  k_win_hash<<<grid_for(ND * 32, 256, c->sm_count), 256, 0, s>>>(ND, d.off, d.off + 1, d.w, hd);
+  k_win_raw_ranges<<<grid_for(NR, 256, c->sm_count), 256, 0, s>>>(R, ridx, ev.sb, ev.span, ev.xspan, codes, M, mem, rb, re);
+  k_win_hash<<<grid_for(NR * 32, 256, c->sm_count), 256, 0, s>>>(NR, rb, re, (const uint64_t *)bb, hr);
+  c->launches += 3;
+  str_release(ar, d);
+  // the set of members: the last of each (line, name) -- sorted by name hash, then stably by line -- summed per line
+  unsigned long long *acc;
+  CKR(ar.alloc(&acc, 2 * R));
+  CK(cudaMemsetAsync(acc, 0, sizeof(unsigned long long) * 2 * (size_t)R, s));
+  if (M > 0) {
+    uint32_t *mline, *v, *k32;
+    unsigned long long *k64;
+    CKR(ar.alloc(&mline, M));
+    CKR(ar.alloc(&v, M));
+    CKR(ar.alloc(&k64, M));
+    CKR(ar.alloc(&k32, M));
+    k_win_member_line<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, moff, mline);
+    k_win_name_keys<<<grid_for(M, 256, c->sm_count), 256, 0, s>>>(M, hd + kWinStr * R, k64, v);
+    c->launches += 2;
+    CKR(sort_pairs(c, ar, M, &k64, &v, 64));
+    k_win_line_keys<<<grid_for(M, 256, c->sm_count), 256, 0, s>>>(M, v, mline, k32);
+    c->launches++;
+    CKR(sort_pairs(c, ar, M, &k32, &v, bits_for(R)));
+    k_win_props<<<grid_for(M, 256, c->sm_count), 256, 0, s>>>(M, v, mline, hd + kWinStr * R, hr + 2 * R, acc);
+    c->launches++;
+  }
+  if (lg->n_rec + R > lg->rec_cap) {   // grow geometrically
+    const long long cap = std::max(2 * lg->rec_cap, lg->n_rec + R);
+    WinRec *p;
+    CKR(ar.alloc(&p, cap));
+    CKR(log_keep(ar, lg, p));
+    if (lg->n_rec > 0) CK(cudaMemcpyAsync(p, lg->rec, sizeof(WinRec) * (size_t)lg->n_rec, cudaMemcpyDeviceToDevice, s));
+    log_drop(lg, lg->rec);
+    lg->rec = p;
+    lg->rec_cap = cap;
+  }
+  k_win_ident<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, ridx, base, ev.sb, ev.span, ev.xspan, bb, hd, hr, codes, acc, ev.tm, ev.flag,
+                                                          code, lg->rec + lg->n_rec);
+  c->launches++;
+  lg->n_rec += R;
+  return CCO_OK;
+}
+
 // one chunk of a streamed read, the first len staged bytes: every line parsed, the names numbered globally, the counts
 // added, the training and ranking events decoded into one new segment, the property-event lines appended to lg->pb
 static int event_chunk(cco_event_log *lg, long long len, bool open_tail) {
@@ -3880,10 +4014,20 @@ static int event_chunk(cco_event_log *lg, long long len, bool open_tail) {
   CKR(event_pad(c, lg->stage, len));
   EvLines ev;
   const long long base = lg->n_lines;
-  CKR(event_lines(c, ar, (const uint64_t *)lg->stage, len, open_tail, base, &ev));
+  CKR(event_lines(c, ar, (const uint64_t *)lg->stage, len, open_tail, base, &ev, lg->dedup));
   const long long L = ev.L;
   if (L == 0) return CCO_OK;
   const unsigned char *bb = lg->stage;
+  if (lg->cutoff != INT64_MIN) {   // the eventWindow's duration: expired lines lose their selection
+    unsigned long long *nx, h_nx = 0;
+    CKR(ar.alloc(&nx, 1));
+    CK(cudaMemsetAsync(nx, 0, 8, s));
+    k_win_expire<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, ev.sb, ev.span, bb, ev.tm, lg->cutoff, ev.flag, nx);
+    c->launches++;
+    CKR(mail_fetch(c, &h_nx, nx, 8));
+    CKR(mail_wait(c));
+    lg->n_expired += (long long)h_nx;
+  }
   // 5. event names: decoded, grouped exactly, numbered by first appearance in the chunk; the few distinct ones go to the
   // host, where names new to the log take the next codes (chunks arrive in order: the order of the whole read)
   JMember *jm;
@@ -3949,11 +4093,13 @@ static int event_chunk(cco_event_log *lg, long long len, bool open_tail) {
   lg->n_prop += NP;
   lg->n_ignored += (long long)h_cnt[2 * NG + 1];
   lg->n_lines += L;
+  if (lg->dedup) CKR(win_records(lg, ar, ev, code, base));
   // 7. training and ranking events partitioned by name, file order inside a name: decoded ids and times
   uint32_t *idx;
   CKR(event_partition(c, ar, L, ev.flag, kEvTraining, code, (uint32_t)NG, &idx));
   CKR(event_column(c, ar, lg, sg.train_at[NG], idx, kEvEntityId, ev.sb, ev.span, bb, sg.train_at, &sg.tu));
   CKR(event_column(c, ar, lg, sg.train_at[NG], idx, kEvTargetId, ev.sb, ev.span, bb, sg.train_at, &sg.ti));
+  if (lg->dedup) CKR(win_entry_lines(lg, ar, sg.train_at[NG], idx, base, &sg.tline));
   ar.release(idx);
   CKR(event_partition(c, ar, L, ev.flag, kEvRanking, code, (uint32_t)NG, &idx));
   const long long NR = sg.rank_at[NG];
@@ -3964,6 +4110,7 @@ static int event_chunk(cco_event_log *lg, long long len, bool open_tail) {
     k_gather_i64<<<grid_for(NR, 256, c->sm_count), 256, 0, s>>>(NR, idx, ev.tm, sg.rtime);
     c->launches++;
   }
+  if (lg->dedup) CKR(win_entry_lines(lg, ar, NR, idx, base, &sg.rline));
   ar.release(idx);
   // 8. the property-event lines, in line order, for the aggregation at finish (see event_log_finish)
   if (NP > 0) {
@@ -4045,18 +4192,21 @@ static int event_cat_column(cco_event_log *lg, EvCol EvSeg::*col, std::vector<lo
   }
   return CCO_OK;
 }
-// the ranking times of every segment, name-major, as the ranking items
-static int event_cat_times(cco_event_log *lg, long long **out) {
+// one per-entry column of every segment (the ranking times; with removeDuplicates also the entries' global lines),
+// name-major, as the string columns of the same partition (at)
+static int event_cat_times(cco_event_log *lg, long long **out, long long *EvSeg::*col = &EvSeg::rtime,
+                           std::vector<long long> EvSeg::*at = &EvSeg::rank_at) {
   cco_ctx *c = lg->ctx;
   cudaStream_t s = c->stream;
   Arena ar(s);
-  const long long NG = (long long)lg->rank_at.size() - 1;
+  const long long NG = (long long)lg->name_off.size() - 1;
   std::vector<CatPiece> ents;
   long long e = 0;
   for (long long g = 0; g < NG; ++g)
     for (EvSeg &sg : lg->segs) {
-      if (g + 1 >= (long long)sg.rank_at.size() || sg.rank_at[g + 1] == sg.rank_at[g]) continue;
-      ents.push_back(CatPiece{nullptr, sg.rtime, 0, 0, 0, sg.rank_at[g], e, sg.rank_at[g + 1] - sg.rank_at[g], false});
+      const std::vector<long long> &sa = sg.*at;
+      if (g + 1 >= (long long)sa.size() || sa[g + 1] == sa[g]) continue;
+      ents.push_back(CatPiece{nullptr, sg.*col, 0, 0, 0, sa[g], e, sa[g + 1] - sa[g], false});
       e += ents.back().ne;
     }
   CKR(ar.alloc(out, std::max<long long>(e, 1)));
@@ -4069,7 +4219,177 @@ static int event_cat_times(cco_event_log *lg, long long **out) {
   }
   CK(cudaStreamSynchronize(s));
   CKR(log_keep(ar, lg, *out));
-  for (EvSeg &sg : lg->segs) log_drop(lg, sg.rtime);
+  for (EvSeg &sg : lg->segs) log_drop(lg, sg.*col);
+  return CCO_OK;
+}
+
+// removeDuplicates at finish: the records of every chunk sorted by (hash, time desc, line desc); all but the first of each
+// run are dropped -> *bitmap over the global lines (kept by the log until finish ends); the counts of the drops
+static int win_mark(cco_event_log *lg, uint32_t **bitmap, long long *n_prop_dup) {
+  cco_ctx *c = lg->ctx;
+  cudaStream_t s = c->stream;
+  Arena ar(s);
+  const long long N = lg->n_rec, NG = (long long)lg->name_off.size() - 1, words = lg->n_lines / 32 + 1;
+  CKR(ar.alloc(bitmap, words));
+  CKR(log_keep(ar, lg, *bitmap));
+  CK(cudaMemsetAsync(*bitmap, 0, sizeof(uint32_t) * (size_t)words, s));
+  std::vector<unsigned long long> h_cnt((size_t)(2 * NG + 3), 0);
+  if (N > 1) {
+    unsigned long long *key, *cnt;
+    uint32_t *val;
+    CKR(ar.alloc(&key, N));
+    CKR(ar.alloc(&val, N));
+    k_win_key_time<<<grid_for(N, 256, c->sm_count), 256, 0, s>>>(N, lg->rec, key, val);
+    c->launches++;
+    CKR(sort_pairs(c, ar, N, &key, &val, 64));
+    for (int high : {1, 0}) {
+      k_win_key_hash<<<grid_for(N, 256, c->sm_count), 256, 0, s>>>(N, lg->rec, val, high, key);
+      c->launches++;
+      CKR(sort_pairs(c, ar, N, &key, &val, 64));
+    }
+    CKR(ar.alloc(&cnt, 2 * NG + 3));
+    CK(cudaMemsetAsync(cnt, 0, sizeof(unsigned long long) * h_cnt.size(), s));
+    k_win_mark<<<grid_for(N, 256, c->sm_count), 256, 0, s>>>(N, lg->rec, val, (int32_t)NG, *bitmap, cnt);
+    c->launches++;
+    CK(cudaMemcpyAsync(h_cnt.data(), cnt, sizeof(unsigned long long) * h_cnt.size(), cudaMemcpyDeviceToHost, s));
+  }
+  CK(cudaStreamSynchronize(s));
+  *n_prop_dup = (long long)h_cnt[2 * NG];
+  lg->n_prop -= (long long)h_cnt[2 * NG];
+  lg->n_ignored -= (long long)h_cnt[2 * NG + 1];
+  lg->n_dup = (long long)h_cnt[2 * NG + 2];
+  log_drop(lg, lg->rec);
+  lg->rec = nullptr;
+  return CCO_OK;
+}
+// a string column's entries idx[0 .. K) gathered into a new column kept by the log (the old one is freed); boff at the
+// names' first entries at
+static int win_gather_column(cco_event_log *lg, Arena &ar, long long K, const uint32_t *idx, const std::vector<long long> &at, EvCol *col) {
+  cco_ctx *c = lg->ctx;
+  cudaStream_t s = c->stream;
+  long long *len, *off, total = 0;
+  CKR(ar.alloc(&len, K + 1));
+  CKR(ar.alloc(&off, K + 1));
+  CK(cudaMemsetAsync(len + K, 0, 8, s));
+  if (K > 0) {
+    k_str_dict_len<<<grid_for(K, 256, c->sm_count), 256, 0, s>>>(K, idx, col->off, len);
+    c->launches++;
+  }
+  CKR(exclusive_sum_i64(c, ar, len, off, K + 1));
+  CK(cudaMemcpyAsync(&total, off + K, 8, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  uint64_t *w;
+  CKR(ar.alloc(&w, (total + 16 + 7) / 8));
+  if (K > 0 && total > 0) {
+    k_str_dict_gather<<<grid_for(K, 256, c->sm_count), 256, 0, s>>>(K, idx, col->off, 0, (const unsigned char *)col->w, off, (unsigned char *)w);
+    c->launches++;
+  }
+  std::vector<uint32_t> at32(at.begin(), at.end());
+  uint32_t *d_at;
+  long long *d_b;
+  CKR(ar.alloc(&d_at, at.size()));
+  CKR(ar.alloc(&d_b, at.size()));
+  CK(cudaMemcpyAsync(d_at, at32.data(), sizeof(uint32_t) * at.size(), cudaMemcpyHostToDevice, s));
+  k_gather_i64<<<grid_for((long long)at.size(), 256, c->sm_count), 256, 0, s>>>((long long)at.size(), d_at, off, d_b);
+  c->launches++;
+  col->boff.assign(at.size(), 0);
+  CK(cudaMemcpyAsync(col->boff.data(), d_b, sizeof(long long) * at.size(), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));   // at32 is a local
+  CKR(log_keep(ar, lg, off));
+  CKR(log_keep(ar, lg, w));
+  log_drop(lg, col->off);
+  log_drop(lg, col->w);
+  col->off = off;
+  col->w = w;
+  return CCO_OK;
+}
+// the name-partitioned entries whose line survives the bitmap: columns c1 (and c2), the times (nullable) and at, compacted
+static int win_compact(cco_event_log *lg, const uint32_t *bitmap, const long long *line, std::vector<long long> &at, EvCol *c1, EvCol *c2,
+                       long long **times) {
+  cco_ctx *c = lg->ctx;
+  cudaStream_t s = c->stream;
+  Arena ar(s);
+  const long long n = at.back(), NA = (long long)at.size();
+  if (n == 0) return CCO_OK;
+  uint32_t *keep, *pos, *idx;
+  CKR(ar.alloc(&keep, n + 1));
+  CKR(ar.alloc(&pos, n + 1));
+  CKR(ar.alloc(&idx, n));
+  CK(cudaMemsetAsync(keep + n, 0, 4, s));
+  k_win_entry_keep<<<grid_for(n, 256, c->sm_count), 256, 0, s>>>(n, line, bitmap, keep);
+  c->launches++;
+  CKR(exclusive_sum_u32(c, ar, keep, pos, n + 1));
+  k_win_scatter<<<grid_for(n, 256, c->sm_count), 256, 0, s>>>(n, keep, pos, idx);
+  long long *d_at, *d_nat;
+  CKR(ar.alloc(&d_at, NA));
+  CKR(ar.alloc(&d_nat, NA));
+  CK(cudaMemcpyAsync(d_at, at.data(), sizeof(long long) * (size_t)NA, cudaMemcpyHostToDevice, s));
+  k_win_at<<<grid_for(NA, 256, c->sm_count), 256, 0, s>>>(NA, d_at, pos, d_nat);
+  c->launches += 2;
+  std::vector<long long> nat((size_t)NA);
+  CK(cudaMemcpyAsync(nat.data(), d_nat, sizeof(long long) * (size_t)NA, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));   // at and nat are host vectors
+  const long long K = nat.back();
+  CKR(win_gather_column(lg, ar, K, idx, nat, c1));
+  if (c2) CKR(win_gather_column(lg, ar, K, idx, nat, c2));
+  if (times) {
+    long long *t;
+    CKR(ar.alloc(&t, std::max<long long>(K, 1)));
+    if (K > 0) {
+      k_gather_i64<<<grid_for(K, 256, c->sm_count), 256, 0, s>>>(K, idx, *times, t);
+      c->launches++;
+    }
+    CK(cudaStreamSynchronize(s));
+    CKR(log_keep(ar, lg, t));
+    log_drop(lg, *times);
+    *times = t;
+  }
+  at = nat;
+  return CCO_OK;
+}
+// the property lines gathered for finish lose their selection where dropped; first the members of every properties object
+// among them are checked, so that a dropped line fails as it fails without the window (event_properties' error)
+static int win_drop_property_lines(cco_event_log *lg, Arena &ar, const EvLines &ev, const uint32_t *bitmap) {
+  cco_ctx *c = lg->ctx;
+  cudaStream_t s = c->stream;
+  const long long L = ev.L;
+  uint32_t *keep, *pos, *qi, Q = 0;
+  CKR(ar.alloc(&keep, L + 1));
+  CKR(ar.alloc(&pos, L + 1));
+  CKR(ar.alloc(&qi, L));
+  CK(cudaMemsetAsync(keep + L, 0, 4, s));
+  k_win_flag_keep<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, ev.flag, kEvPropObj, keep);
+  c->launches++;
+  CKR(exclusive_sum_u32(c, ar, keep, pos, L + 1));
+  k_win_scatter<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, keep, pos, qi);
+  c->launches++;
+  CKR(mail_fetch(c, &Q, pos + L, 4));
+  CKR(mail_wait(c));
+  long long *gl;
+  CKR(ar.alloc(&gl, L));
+  CK(cudaMemcpyAsync(gl, lg->prop_line.data(), sizeof(long long) * (size_t)L, cudaMemcpyHostToDevice, s));
+  if (Q > 0) {
+    long long *qb, *qe, *mcnt;
+    unsigned long long *err, h_err = 0;
+    CKR(ar.alloc(&qb, Q));
+    CKR(ar.alloc(&qe, Q));
+    CKR(ar.alloc(&mcnt, Q));
+    CKR(ar.alloc(&err, 1));
+    CK(cudaMemsetAsync(err, 0xff, 8, s));
+    k_win_obj_spans<<<grid_for(Q, 256, c->sm_count), 256, 0, s>>>(Q, qi, ev.sb, ev.span, qb, qe);
+    k_json_members<<<grid_for((long long)Q * 32, 256, c->sm_count), 256, 0, s>>>(Q, qb, qe, lg->pb, MemberSink<false>{mcnt, nullptr, nullptr}, err);
+    c->launches += 2;
+    CKR(mail_fetch(c, &h_err, err, 8));
+    CKR(mail_wait(c));
+    if (h_err != ~0ULL) {
+      uint32_t line = 0;
+      CK(cudaMemcpy(&line, qi + (h_err >> 8), 4, cudaMemcpyDeviceToHost));
+      return event_error(((unsigned long long)lg->prop_line[line] << 8) | (h_err & 0xff));
+    }
+  }
+  k_win_drop_lines<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, gl, bitmap, ev.flag);
+  c->launches++;
+  CK(cudaStreamSynchronize(s));   // prop_line is read by the copy
   return CCO_OK;
 }
 
@@ -4164,28 +4484,53 @@ static int event_log_finish(cco_event_log *lg) {
     lg->train_at[n + 1] = lg->train_at[n] + lg->n_train[n];
     lg->rank_at[n + 1] = lg->rank_at[n] + lg->n_rank[n];
   }
+  uint32_t *drop = nullptr;   // removeDuplicates: the dropped global lines
+  long long n_prop_dup = 0;
+  if (lg->dedup) {
+    mail_reset(c);
+    CKR(win_mark(lg, &drop, &n_prop_dup));
+  }
   if (lg->segs.size() == 1) {   // one chunk: its segment is the layout
     EvSeg &sg = lg->segs[0];
     lg->tu = sg.tu;
     lg->ti = sg.ti;
     lg->ri = sg.ri;
     lg->rtime = sg.rtime;
+    lg->tline = sg.tline;
+    lg->rline = sg.rline;
   } else if (lg->segs.size() > 1) {
     CKR(event_cat_column(lg, &EvSeg::tu, &EvSeg::train_at, lg->train_at, &lg->tu));
     CKR(event_cat_column(lg, &EvSeg::ti, &EvSeg::train_at, lg->train_at, &lg->ti));
     CKR(event_cat_column(lg, &EvSeg::ri, &EvSeg::rank_at, lg->rank_at, &lg->ri));
     CKR(event_cat_times(lg, &lg->rtime));
+    if (lg->dedup) {
+      CKR(event_cat_times(lg, &lg->tline, &EvSeg::tline, &EvSeg::train_at));
+      CKR(event_cat_times(lg, &lg->rline, &EvSeg::rline, &EvSeg::rank_at));
+    }
   }
   lg->segs.clear();
+  if (drop && lg->n_dup > 0) {   // the retained columns without the dropped lines' entries
+    CKR(win_compact(lg, drop, lg->tline, lg->train_at, &lg->tu, &lg->ti, nullptr));
+    CKR(win_compact(lg, drop, lg->rline, lg->rank_at, &lg->ri, nullptr, &lg->rtime));
+    for (long long n = 0; n < NG; ++n) {
+      lg->n_train[n] = lg->train_at[n + 1] - lg->train_at[n];
+      lg->n_rank[n] = lg->rank_at[n + 1] - lg->rank_at[n];
+    }
+  }
+  log_drop(lg, lg->tline);
+  log_drop(lg, lg->rline);
+  lg->tline = lg->rline = nullptr;
   if (lg->n_prop > 0) {
     mail_reset(c);
     Arena ar(s);
     CKR(event_pad(c, lg->pb, lg->pb_len));
     EvLines ev;
     CKR(event_lines(c, ar, (const uint64_t *)lg->pb, lg->pb_len, false, 0, &ev));   // judged once already
+    if (n_prop_dup > 0) CKR(win_drop_property_lines(lg, ar, ev, drop));
     CKR(event_properties(c, ar, lg, ev.L, ev.flag, ev.tm, ev.sb, ev.span, lg->pb, lg->prop_line.data()));
     CK(cudaStreamSynchronize(s));
   }
+  log_drop(lg, drop);
   log_drop(lg, lg->pb);
   lg->pb = nullptr;
   lg->prop_line = std::vector<long long>();
@@ -4247,10 +4592,30 @@ static int log_fail(cco_event_log *lg, int rc) {
 }  // namespace cco
 
 int cco_event_log_begin(cco_ctx_t *ctx, int64_t chunk_bytes, cco_event_log_t **out) {
+  return cco_event_log_begin_window(ctx, chunk_bytes, nullptr, out);
+}
+
+int cco_event_log_begin_window(cco_ctx_t *ctx, int64_t chunk_bytes, const cco_event_window_t *w, cco_event_log_t **out) {
   if (!ctx || !out || chunk_bytes < 1) return set_error(CCO_E_INVALID_ARG, "null argument or chunk_bytes < 1");
   *out = nullptr;
+  if (w && (w->remove_duplicates != 0 && w->remove_duplicates != 1))
+    return set_error(CCO_E_INVALID_ARG, "remove_duplicates is %d, not 0 or 1", (int)w->remove_duplicates);
+  if (w && w->reserved != 0) return set_error(CCO_E_INVALID_ARG, "the window's reserved field must be 0");
   if (!ctx->members.empty()) return set_error(CCO_E_UNSUPPORTED, "an event log is resident on one GPU: read it on a per-GPU context");
-  return event_log_begin(ctx, chunk_bytes, out);
+  CKR(event_log_begin(ctx, chunk_bytes, out));
+  if (w) {
+    (*out)->cutoff = w->cutoff_ms;
+    (*out)->dedup = w->remove_duplicates != 0;
+  }
+  return CCO_OK;
+}
+
+int cco_event_log_window_stats(const cco_event_log_t *lg, int64_t *n_expired, int64_t *n_duplicates) {
+  if (!lg || !n_expired || !n_duplicates) return set_error(CCO_E_INVALID_ARG, "null argument");
+  CKR(log_state(lg, true));
+  *n_expired = lg->n_expired;
+  *n_duplicates = lg->n_dup;
+  return CCO_OK;
 }
 
 int cco_event_log_append(cco_event_log_t *lg, const char *bytes, int64_t len) {

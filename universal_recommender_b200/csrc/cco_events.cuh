@@ -466,4 +466,294 @@ __global__ void k_cat_entries(long long n, long long last, const CatPiece *__res
   }
 }
 
+// ---- the DataSource's eventWindow (cco_event_log_begin_window) ------------------------------------------------------------
+// PredictionIO's SelfCleaningDataSource.cleanPEvents, restated [RECALL, unverifiable here]: expiry (eventTime > cutoff, or
+// the event is $set / $unset), then removeDuplicates (events equal but for eventId, eventTime and creationTime collapse to
+// the one with the latest eventTime, ties to the later line).  Duplicates are found by a 128-bit identity hash per line
+// (the bytes of earlier chunks are gone by finish):
+//   k_win_expire                     an expired line loses its selection (flag kEvDropped) and is counted
+//   EventSinkX                       EventSink plus the spans of "prId" and "tags", captured only when duplicates go
+//   k_json_members + WinMemberSink   the top-level members of each retained line's properties, with the span's verdict
+//   k_win_strings / k_win_raw_ranges the identity's decoded strings (json_decode) and raw value texts as byte ranges
+//   k_win_hash                       128-bit hash of a byte range, one warp per range (no thread walks a long value)
+//   k_win_props                      order-insensitive sum over the properties' members, the last of a repeated name only
+//   k_win_ident                      the line's identity hash -> a WinRec (hash, time, global line, name, selection)
+//   k_win_key_* / k_win_mark         at finish: records sorted by (hash, time desc, line desc), all but the first of each
+//                                    run dropped into a bitmap over the global lines, the drops counted per selection
+//   k_win_entry_keep / k_win_scatter the retained columns and the property lines compacted through the bitmap
+enum : uint8_t { kEvDropped = 128 };   // an expired line: no selection, not ignored
+enum : int { kEvPrId = 0, kEvTags, kEvXSlots };
+constexpr int kWinStr = 6;             // decoded strings per line: event, entityType, entityId, targetEntityType, targetEntityId, prId
+
+// what removeDuplicates keeps of a retained line
+struct WinRec {
+  uint64_t h0, h1;
+  long long time, line;   // eventTime ms, global line
+  int32_t code;           // event name
+  uint32_t flag;          // selection flags
+};
+
+struct EventSinkX {
+  int2 *span, *xspan;
+  const unsigned char *body;
+  __device__ void member(long long s, long long, long long b, const JMember &m) const {
+    const int k = event_slot(body, m.nb, m.ne);
+    if (k >= 0) {
+      span[s * kEvSlots + k] = make_int2((int)(m.vb - b), (int)(m.ve - b));
+      return;
+    }
+    const int x = json_str_is(body, m.nb, m.ne, "prId", 4) ? kEvPrId : json_str_is(body, m.nb, m.ne, "tags", 4) ? kEvTags : -1;
+    if (x >= 0) xspan[s * kEvXSlots + x] = make_int2((int)(m.vb - b), (int)(m.ve - b));
+  }
+  __device__ void end(long long, long long) const {}
+};
+
+// lines at or before the cutoff whose event is neither $set nor $unset -> kEvDropped; *n_expired += them
+__global__ void k_win_expire(long long n_lines, const long long *__restrict__ sb, const int2 *__restrict__ span,
+                             const unsigned char *__restrict__ body, const long long *__restrict__ time, long long cutoff,
+                             uint8_t *__restrict__ flag, unsigned long long *__restrict__ n_expired) {
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long base = blockIdx.x * (long long)blockDim.x; base < n_lines; base += stride) {
+    const long long l = base + threadIdx.x;
+    bool x = false;
+    if (l < n_lines && time[l] <= cutoff) {
+      const int2 v = span[l * kEvSlots + kEvName];
+      const long long nb = sb[l] + v.x + 1, ne = sb[l] + v.y - 1;
+      x = !json_str_is(body, nb, ne, "$set", 4) && !json_str_is(body, nb, ne, "$unset", 6);
+      if (x) flag[l] = kEvDropped;
+    }
+    const unsigned m = __ballot_sync(0xffffffffu, x);
+    if ((threadIdx.x & 31) == 0 && m) atomicAdd(n_expired, (unsigned long long)__popc(m));
+  }
+}
+// keep[l] = line l is not expired
+__global__ void k_win_keep_lines(long long n, const uint8_t *__restrict__ flag, uint32_t *__restrict__ keep) {
+  for (long long l = blockIdx.x * (long long)blockDim.x + threadIdx.x; l < n; l += (long long)gridDim.x * blockDim.x)
+    keep[l] = flag[l] != kEvDropped;
+}
+// out[pos[i]] = i for the kept i (pos = exclusive sum of keep)
+__global__ void k_win_scatter(long long n, const uint32_t *__restrict__ keep, const uint32_t *__restrict__ pos, uint32_t *__restrict__ out) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    if (keep[i]) out[pos[i]] = (uint32_t)i;
+}
+// the properties object of retained line r (absent: an empty span, which the tokenizer calls not an object)
+__global__ void k_win_prop_spans(long long R, const uint32_t *__restrict__ ridx, const long long *__restrict__ sb, const int2 *__restrict__ span,
+                                 long long *__restrict__ b, long long *__restrict__ e) {
+  for (long long r = blockIdx.x * (long long)blockDim.x + threadIdx.x; r < R; r += (long long)gridDim.x * blockDim.x) {
+    const long long l = ridx[r];
+    const int2 v = span[l * kEvSlots + kEvProps];
+    b[r] = v.x >= 0 ? sb[l] + v.x : 0;
+    e[r] = v.x >= 0 ? sb[l] + v.y : 0;
+  }
+}
+// members of each span (count pass: count and verdict; write pass: the members of well-formed spans only)
+template <bool kWrite>
+struct WinMemberSink {
+  long long *count;
+  int *codes;
+  const long long *moff;
+  JMember *out;
+  __device__ void member(long long s, long long n, long long, const JMember &m) const {
+    if (kWrite && !codes[s]) out[moff[s] + n] = m;
+  }
+  __device__ void code(long long s, int c) const {
+    if (!kWrite) codes[s] = c;
+  }
+  __device__ void end(long long s, long long n) const {
+    if (!kWrite) count[s] = codes[s] ? 0 : n;
+  }
+};
+// string i < 6 R: slot i % 6 of retained line i / 6, its inside when a string, its text when another value, empty when
+// absent or null; string 6 R + m: the raw name of member m
+__global__ void k_win_strings(long long R, const uint32_t *__restrict__ ridx, const long long *__restrict__ sb, const int2 *__restrict__ span,
+                              const int2 *__restrict__ xspan, const unsigned char *__restrict__ body, long long M,
+                              const JMember *__restrict__ mem, JMember *__restrict__ out) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < kWinStr * R + M; i += (long long)gridDim.x * blockDim.x) {
+    if (i >= kWinStr * R) {
+      const JMember &m = mem[i - kWinStr * R];
+      out[i] = JMember{m.nb, m.ne, 0, 0};
+      continue;
+    }
+    const long long l = ridx[i / kWinStr];
+    const int k = (int)(i % kWinStr);
+    const int2 v = k < kWinStr - 1 ? span[l * kEvSlots + k] : xspan[l * kEvXSlots + kEvPrId];
+    const long long b = sb[l] + v.x, e = sb[l] + v.y;
+    const bool present = v.x >= 0 && !json_is_null(body, b, e), str = present && body[b] == '"';
+    out[i] = str ? JMember{b + 1, e - 1, 0, 0} : present ? JMember{b, e, 0, 0} : JMember{0, 0, 0, 0};
+  }
+}
+// raw byte ranges: [0, R) the tags value, [R, 2 R) the properties text of a span the tokenizer could not split, [2 R, 2 R
+// + M) the members' values (empty where unused)
+__global__ void k_win_raw_ranges(long long R, const uint32_t *__restrict__ ridx, const long long *__restrict__ sb, const int2 *__restrict__ span,
+                                 const int2 *__restrict__ xspan, const int *__restrict__ codes, long long M, const JMember *__restrict__ mem,
+                                 long long *__restrict__ rb, long long *__restrict__ re) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < 2 * R + M; i += (long long)gridDim.x * blockDim.x) {
+    long long b = 0, e = 0;
+    if (i >= 2 * R) {
+      b = mem[i - 2 * R].vb;
+      e = mem[i - 2 * R].ve;
+    } else {
+      const long long r = i < R ? i : i - R, l = ridx[r];
+      const int2 v = i < R ? xspan[l * kEvXSlots + kEvTags] : span[l * kEvSlots + kEvProps];
+      if (v.x >= 0 && (i < R || codes[r])) {
+        b = sb[l] + v.x;
+        e = sb[l] + v.y;
+      }
+    }
+    rb[i] = b;
+    re[i] = e;
+  }
+}
+// 128-bit hash of the bytes [rb[i], re[i]) of a word buffer (16 bytes of padding): the sum over its 8-byte words of a mix
+// of (word, position), then the length -- one warp per range, each lane over every 32nd word
+__device__ __forceinline__ ulonglong2 win_word(uint64_t x, uint64_t q) {
+  return make_ulonglong2(mix64(x ^ mix64(q + 0x243f6a8885a308d3ULL)), mix64(mix64(x + q * 0x9e3779b97f4a7c15ULL) ^ 0x13198a2e03707344ULL));
+}
+__global__ void k_win_hash(long long n, const long long *__restrict__ rb, const long long *__restrict__ re, const uint64_t *__restrict__ w,
+                           ulonglong2 *__restrict__ out) {
+  const int lane = threadIdx.x & 31;
+  const long long warp = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5, nwarps = ((long long)gridDim.x * blockDim.x) >> 5;
+  for (long long i = warp; i < n; i += nwarps) {
+    const long long b = rb[i], len = re[i] - b;
+    uint64_t a = 0, c = 0;
+    for (long long k = lane; k * 8 < len; k += 32) {
+      const ulonglong2 h = win_word(str_mask_tail(str_word(w, b, k), len - k * 8), (uint64_t)k);
+      a += h.x;
+      c += h.y;
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+      a += __shfl_xor_sync(0xffffffffu, a, o);
+      c += __shfl_xor_sync(0xffffffffu, c, o);
+    }
+    if (lane == 0) out[i] = make_ulonglong2(mix64(a ^ mix64((uint64_t)len ^ 0xa4093822299f31d0ULL)), mix64(c + (uint64_t)len * 0x082efa98ec4e6c89ULL));
+  }
+}
+// mline[m] = the retained line of member m
+__global__ void k_win_member_line(long long R, const long long *__restrict__ moff, uint32_t *__restrict__ mline) {
+  for (long long r = blockIdx.x * (long long)blockDim.x + threadIdx.x; r < R; r += (long long)gridDim.x * blockDim.x)
+    for (long long m = moff[r]; m < moff[r + 1]; ++m) mline[m] = (uint32_t)r;
+}
+__global__ void k_win_name_keys(long long M, const ulonglong2 *__restrict__ hname, unsigned long long *__restrict__ key, uint32_t *__restrict__ val) {
+  for (long long m = blockIdx.x * (long long)blockDim.x + threadIdx.x; m < M; m += (long long)gridDim.x * blockDim.x) {
+    key[m] = hname[m].x;
+    val[m] = (uint32_t)m;
+  }
+}
+__global__ void k_win_line_keys(long long M, const uint32_t *__restrict__ val, const uint32_t *__restrict__ mline, uint32_t *__restrict__ key) {
+  for (long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x; k < M; k += (long long)gridDim.x * blockDim.x) key[k] = mline[val[k]];
+}
+// members sorted by (line, name hash, member order): the last of each (line, name) run adds a mix of (name, value) to
+// its line's sum
+__global__ void k_win_props(long long M, const uint32_t *__restrict__ val, const uint32_t *__restrict__ mline, const ulonglong2 *__restrict__ hname,
+                            const ulonglong2 *__restrict__ hval, unsigned long long *__restrict__ acc) {
+  for (long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x; k < M; k += (long long)gridDim.x * blockDim.x) {
+    const uint32_t m = val[k], r = mline[m];
+    const ulonglong2 n = hname[m];
+    if (k + 1 < M) {
+      const uint32_t q = val[k + 1];
+      if (mline[q] == r && hname[q].x == n.x && hname[q].y == n.y) continue;
+    }
+    const ulonglong2 v = hval[m];
+    atomicAdd(&acc[2 * r], mix64(n.x ^ mix64(v.x + 0x452821e638d01377ULL)));
+    atomicAdd(&acc[2 * r + 1], mix64(n.y + mix64(v.y ^ 0xbe5466cf34e90c6cULL)));
+  }
+}
+// the identity hash of retained line r -> rec[r]
+__global__ void k_win_ident(long long R, const uint32_t *__restrict__ ridx, long long line_base, const long long *__restrict__ sb,
+                            const int2 *__restrict__ span, const int2 *__restrict__ xspan, const unsigned char *__restrict__ body,
+                            const ulonglong2 *__restrict__ hdec, const ulonglong2 *__restrict__ hraw, const int *__restrict__ codes,
+                            const unsigned long long *__restrict__ acc, const long long *__restrict__ tm, const uint8_t *__restrict__ flag,
+                            const int32_t *__restrict__ code, WinRec *__restrict__ rec) {
+  for (long long r = blockIdx.x * (long long)blockDim.x + threadIdx.x; r < R; r += (long long)gridDim.x * blockDim.x) {
+    const long long l = ridx[r], b = sb[l];
+    uint64_t a = 0x3707344a40938222ULL, c = 0x299f31d0082efa98ULL;
+    auto add = [&](uint64_t x, uint64_t y) {
+      a = mix64(a ^ x) + 0x9e3779b97f4a7c15ULL;
+      c = mix64(c + y) ^ 0xc0ac29b7c97c50ddULL;
+    };
+    unsigned kinds = 0;   // per string slot: present, a string
+    for (int k = 0; k < kWinStr; ++k) {
+      const int2 v = k < kWinStr - 1 ? span[l * kEvSlots + k] : xspan[l * kEvXSlots + kEvPrId];
+      const bool present = v.x >= 0 && !json_is_null(body, b + v.x, b + v.y);
+      kinds |= (present ? 1u : 0u) << (2 * k);
+      kinds |= (present && body[b + v.x] == '"' ? 2u : 0u) << (2 * k);
+      add(hdec[kWinStr * r + k].x, hdec[kWinStr * r + k].y);
+    }
+    add(kinds, kinds);
+    // tags: absent, null and [] are the empty list
+    const int2 t = xspan[l * kEvXSlots + kEvTags];
+    const bool no_tags = t.x < 0 || json_is_null(body, b + t.x, b + t.y) || (t.y - t.x == 2 && body[b + t.x] == '[' && body[b + t.x + 1] == ']');
+    if (no_tags) add(1, 1);
+    else add(hraw[r].x, hraw[r].y);
+    // properties: absent is {}; the text of an object the tokenizer could not split stands for it
+    const bool props = span[l * kEvSlots + kEvProps].x >= 0;
+    if (props && codes[r]) add(hraw[R + r].x ^ 2, hraw[R + r].y ^ 2);
+    else add(acc[2 * r], acc[2 * r + 1]);
+    rec[r] = WinRec{mix64(a), mix64(c ^ a), tm[l], line_base + l, code[l], flag[l]};
+  }
+}
+// at finish: keys of the (hash, time desc, line desc) order, sorted least significant first (records are in line order)
+__global__ void k_win_key_time(long long N, const WinRec *__restrict__ rec, unsigned long long *__restrict__ key, uint32_t *__restrict__ val) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < N; i += (long long)gridDim.x * blockDim.x) {
+    const long long j = N - 1 - i;
+    key[i] = ~((unsigned long long)rec[j].time ^ 0x8000000000000000ULL);
+    val[i] = (uint32_t)j;
+  }
+}
+__global__ void k_win_key_hash(long long N, const WinRec *__restrict__ rec, const uint32_t *__restrict__ val, int high,
+                               unsigned long long *__restrict__ key) {
+  for (long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x; k < N; k += (long long)gridDim.x * blockDim.x)
+    key[k] = high ? rec[val[k]].h1 : rec[val[k]].h0;
+}
+// a record whose hash equals its predecessor's is a duplicate: its line goes into the bitmap, and cnt[2 g] / cnt[2 g + 1]
+// (training / ranking events of name g), cnt[2 n_names] (property events), cnt[2 n_names + 1] (ignored lines) and
+// cnt[2 n_names + 2] (all) count it
+__global__ void k_win_mark(long long N, const WinRec *__restrict__ rec, const uint32_t *__restrict__ val, int32_t n_names,
+                           uint32_t *__restrict__ bitmap, unsigned long long *__restrict__ cnt) {
+  for (long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x; k < N; k += (long long)gridDim.x * blockDim.x) {
+    if (k == 0) continue;
+    const WinRec &x = rec[val[k]], &p = rec[val[k - 1]];
+    if (x.h0 != p.h0 || x.h1 != p.h1) continue;
+    atomicOr(&bitmap[x.line >> 5], 1u << (x.line & 31));
+    if (x.flag & kEvTraining) atomicAdd(&cnt[2 * x.code], 1ULL);
+    if (x.flag & kEvRanking) atomicAdd(&cnt[2 * x.code + 1], 1ULL);
+    if (x.flag & kEvProperty) atomicAdd(&cnt[2 * n_names], 1ULL);
+    if (!x.flag) atomicAdd(&cnt[2 * n_names + 1], 1ULL);
+    atomicAdd(&cnt[2 * n_names + 2], 1ULL);
+  }
+}
+__device__ __forceinline__ bool win_dropped(const uint32_t *__restrict__ bitmap, long long line) {
+  return (bitmap[line >> 5] >> (line & 31)) & 1;
+}
+// out[i] = base + idx[i]: the global line of each entry of a chunk's column
+__global__ void k_win_lines(long long n, const uint32_t *__restrict__ idx, long long base, long long *__restrict__ out) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) out[i] = base + idx[i];
+}
+__global__ void k_win_entry_keep(long long n, const long long *__restrict__ line, const uint32_t *__restrict__ bitmap, uint32_t *__restrict__ keep) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    keep[i] = win_dropped(bitmap, line[i]) ? 0u : 1u;
+}
+// out[g] = pos[at[g]]: the kept entries before each name's first
+__global__ void k_win_at(long long n, const long long *__restrict__ at, const uint32_t *__restrict__ pos, long long *__restrict__ out) {
+  for (long long g = blockIdx.x * (long long)blockDim.x + threadIdx.x; g < n; g += (long long)gridDim.x * blockDim.x) out[g] = pos[at[g]];
+}
+// the property lines gathered at finish: a dropped one loses its selection
+__global__ void k_win_drop_lines(long long n, const long long *__restrict__ gline, const uint32_t *__restrict__ bitmap, uint8_t *__restrict__ flag) {
+  for (long long l = blockIdx.x * (long long)blockDim.x + threadIdx.x; l < n; l += (long long)gridDim.x * blockDim.x)
+    if (win_dropped(bitmap, gline[l])) flag[l] = 0;
+}
+// the properties objects of the listed lines
+__global__ void k_win_obj_spans(long long n, const uint32_t *__restrict__ idx, const long long *__restrict__ sb, const int2 *__restrict__ span,
+                                long long *__restrict__ b, long long *__restrict__ e) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const long long l = idx[i];
+    b[i] = sb[l] + span[l * kEvSlots + kEvProps].x;
+    e[i] = sb[l] + span[l * kEvSlots + kEvProps].y;
+  }
+}
+__global__ void k_win_flag_keep(long long n, const uint8_t *__restrict__ flag, uint8_t want, uint32_t *__restrict__ keep) {
+  for (long long l = blockIdx.x * (long long)blockDim.x + threadIdx.x; l < n; l += (long long)gridDim.x * blockDim.x)
+    keep[l] = (flag[l] & want) ? 1u : 0u;
+}
+
 }  // namespace cco

@@ -106,6 +106,13 @@ __device__ __noinline__ bool json_escape_ok(const unsigned char *__restrict__ bo
 //   depth          = prefix count of '{' '[' minus '}' ']' outside strings (ballot popcounts)
 // The bytes at depth <= 1 outside strings (and the quotes at depth 1) drive a small state machine, one event at a time.
 enum : int { kJBefore = 0, kJFirst, kJNext, kJName, kJColon, kJValue0, kJValue, kJDone };
+// a sink with a code(span, code) member is told each span's verdict (0: well formed); for the others this is a no-op
+template <class Sink>
+__device__ __forceinline__ auto sink_code(const Sink &sink, long long s, int code, int) -> decltype(sink.code(s, code), void()) {
+  sink.code(s, code);
+}
+template <class Sink>
+__device__ __forceinline__ void sink_code(const Sink &, long long, int, long) {}
 // Every completed member goes to sink.member(span, index in span, span begin, member) on lane 0, and lane 0 calls
 // sink.end(span, members) once per span; a malformed span sets the error word instead (its members may be partly sunk).
 template <class Sink>
@@ -201,6 +208,7 @@ __global__ void k_json_members(long long n_spans, const long long *__restrict__ 
     if (!code && state != kJDone) code = state == kJBefore ? kJsonNotObject : (in_str ? kJsonString : kJsonSyntax);
     if (lane == 0) {
       if (code) atomicMin(err, ((unsigned long long)s << 8) | (unsigned)code);
+      sink_code(sink, s, code, 0);
       sink.end(s, n);
     }
   }

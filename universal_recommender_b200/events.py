@@ -29,7 +29,13 @@ What the mirror accepts differs from the device in these ways:
   - a \\u escape of a surrogate that is not part of a pair (a high surrogate not followed by a \\u escape of a low one, or a
     lone low one) is written by the device as the surrogate's 3-byte form (\\ud800 -> ED A0 80, Python's
     "surrogatepass").  Here it stays a lone surrogate in the str, which encode_ids (strict UTF-8) cannot encode: such an
-    export cannot go through calc_all_on_device / calc_pop_on_device, only through the *_from_events paths."""
+    export cannot go through calc_all_on_device / calc_pop_on_device, only through the *_from_events paths.
+
+The DataSource's eventWindow (read_export(window=...), cco_event_log_begin_window) cleans the events first, as PredictionIO's
+SelfCleaningDataSource does before every read [RECALL, unverifiable here]: every line is still parsed and checked; then
+an event at or before now - duration expires unless it is a $set or $unset; then, with removeDuplicates, events of equal
+identity (event_identity) collapse to the one with the latest eventTime, ties to the later line.  The training, ranking
+and property selections read what is left."""
 from __future__ import annotations
 
 import json
@@ -39,7 +45,7 @@ from json.decoder import scanstring
 from dataclasses import dataclass, field
 from typing import Optional, Sequence
 
-from .ur_model import RawJson
+from .ur_model import RawJson, duration_ms
 
 PROPERTY_EVENTS = ("$set", "$unset", "$delete")
 _WS = re.compile(r"[ \t\n\r]*")
@@ -69,6 +75,13 @@ def _members(s: str, i: int) -> tuple[list, int]:
             return out, i + 1
         else:
             raise ValueError("bad object")
+
+
+def raw_member(line: str, name: str) -> Optional[str]:
+    """the trimmed text of the last top-level member `name` of an event line, None when absent"""
+    top, _ = _members(line, _WS.match(line).end())
+    spans = [(b, e) for n, b, e in top if n == name]
+    return line[spans[-1][0]:spans[-1][1]] if spans else None
 
 
 def raw_properties(line: str) -> dict:
@@ -127,6 +140,8 @@ class Event:
     target_id: Optional[str]
     time_ms: int
     properties: dict
+    pr_id: object = None      # the decoded prId (a string), None when absent or null
+    tags: str = "[]"          # the trimmed text of tags; absent and null are "[]"
 
 
 def parse_line(i: int, raw: bytes) -> Event:
@@ -157,7 +172,10 @@ def parse_line(i: int, raw: bytes) -> Event:
         t = parse_event_time(obj["eventTime"])
     except ValueError as e:
         raise ValueError(f"line {i}: {e}") from None
-    return Event(i, obj["event"], obj["entityType"], obj["entityId"], tt, ti, t, props)
+    text = raw.decode("utf-8", "surrogatepass")
+    tags = raw_member(text, "tags") if "tags" in obj else None
+    return Event(i, obj["event"], obj["entityType"], obj["entityId"], tt, ti, t, props, obj.get("prId"),
+                 "[]" if tags in (None, "null") else tags)
 
 
 def export_lines(data: bytes) -> list[bytes]:
@@ -199,6 +217,69 @@ class DataSourceEvents:
     set_events: list                   # aggregated properties [(item, {field: value})]
     n_ignored: int = 0
     property_events: list = field(default_factory=list)
+    n_expired: int = 0                 # lines the eventWindow dropped (EventLog.window_stats)
+    n_duplicates: int = 0
+
+
+@dataclass
+class EventWindow:
+    """engine.json datasource.params.eventWindow, PredictionIO's EventWindow(duration, removeDuplicates,
+    compressProperties).  duration: a scala.concurrent.duration string (ur_model.duration_ms), None: nothing expires.
+    compressProperties rewrites each entity's $set / $unset events as one; it is assumed to leave what aggregateProperties
+    returns unchanged, so it is accepted and changes nothing here."""
+    duration: Optional[str] = None
+    removeDuplicates: bool = False
+    compressProperties: bool = False
+
+    @staticmethod
+    def from_json(d: Optional[dict]) -> Optional["EventWindow"]:
+        if d is None:
+            return None
+        return EventWindow(d.get("duration"), bool(d.get("removeDuplicates", False)), bool(d.get("compressProperties", False)))
+
+    def cutoff_ms(self, now_ms: int) -> Optional[int]:
+        """events at or before it expire ($set / $unset excepted); None without a duration"""
+        return None if self.duration is None else now_ms - duration_ms(self.duration)
+
+
+@dataclass
+class DataSourceParams:
+    """DataSourceParams (DataSource.scala:36-41): engine.json's datasource.params"""
+    appName: Optional[str] = None
+    eventNames: Optional[Sequence[str]] = None
+    eventWindow: Optional[EventWindow] = None
+    minEventsPerUser: Optional[int] = None
+
+    @staticmethod
+    def from_engine_json(params: dict) -> "DataSourceParams":
+        return DataSourceParams(params.get("appName"), params.get("eventNames"), EventWindow.from_json(params.get("eventWindow")),
+                                params.get("minEventsPerUser"))
+
+
+def event_identity(e: Event) -> tuple:
+    """what removeDuplicates compares: the event without eventId, eventTime and creationTime.  Properties are the set of
+    their top-level (name, trimmed value text) members, tags the trimmed text: nested values compare by text, as on the
+    device (json4s would compare numbers by value and objects without regard to member order)."""
+    return (e.event, e.entity_type, e.entity_id, e.target_type, e.target_id, e.pr_id, e.tags,
+            frozenset((k, v.text) for k, v in e.properties.items()))
+
+
+def clean_events(events: Sequence[Event], window: Optional[EventWindow], now_ms: Optional[int]) -> tuple[list, int, int]:
+    """the events the window keeps, in line order -> (events, expired, duplicates)"""
+    if window is None:
+        return list(events), 0, 0
+    cutoff = window.cutoff_ms(now_ms) if window.duration is not None else None
+    kept = [e for e in events if cutoff is None or e.time_ms > cutoff or e.event in ("$set", "$unset")]
+    expired = len(events) - len(kept)
+    if not window.removeDuplicates:
+        return kept, expired, 0
+    best: dict = {}
+    for e in kept:
+        k = event_identity(e)
+        if k not in best or (e.time_ms, e.line) > (best[k].time_ms, best[k].line):
+            best[k] = e
+    out = sorted(best.values(), key=lambda e: e.line)
+    return out, expired, len(kept) - len(out)
 
 
 def export_parts(directory) -> list[str]:
@@ -238,26 +319,33 @@ def join_parts(paths: Sequence) -> bytes:
     return b"".join(out)
 
 
-def read_export(data) -> DataSourceEvents:
-    """data: the export's bytes, or the directory `pio export` writes (its parts joined as join_parts does)"""
+def read_export(data, window: Optional[EventWindow] = None, now_ms: Optional[int] = None) -> DataSourceEvents:
+    """data: the export's bytes, or the directory `pio export` writes (its parts joined as join_parts does); window: the
+    eventWindow, its duration counted back from now_ms (required with a duration).  Event names are listed for every line
+    read, expired and duplicate ones included, as the device numbers them while it parses."""
     if isinstance(data, (str, os.PathLike)):
         data = join_parts(export_parts(data))
+    if window is not None and window.duration is not None and now_ms is None:
+        raise ValueError("an eventWindow with a duration needs now_ms")
     names: dict = {}
-    events, ranking, props, ignored = [], {}, [], 0
+    parsed = []
     for i, raw in enumerate(export_lines(bytes(data))):
         e = parse_line(i, raw)
+        if e.target_id is not None and e.entity_type == "user" and e.target_type == "item" and (not e.entity_id or not e.target_id):
+            raise ValueError(f"line {i}: Empty user or item ID")
         names.setdefault(e.event, None)
-        ranking.setdefault(e.event, [])
+        parsed.append(e)
+    kept, n_expired, n_dup = clean_events(parsed, window, now_ms)
+    events, ranking, props, ignored = [], {n: [] for n in names}, [], 0
+    for e in kept:
         used = False
         if e.target_id is not None:
             used = True
             ranking[e.event].append((e.target_id, e.time_ms))
             if e.entity_type == "user" and e.target_type == "item":
-                if not e.entity_id or not e.target_id:
-                    raise ValueError(f"line {i}: Empty user or item ID")
                 events.append((e.entity_id, e.event, e.target_id, e.time_ms))
         if is_property_event(e):
             used = True
             props.append(e)
         ignored += not used
-    return DataSourceEvents(list(names), events, ranking, aggregate_property_events(props), ignored, props)
+    return DataSourceEvents(list(names), events, ranking, aggregate_property_events(props), ignored, props, n_expired, n_dup)

@@ -9,6 +9,7 @@ import os
 import queue
 import re
 import threading
+import time
 import weakref
 from dataclasses import dataclass
 from typing import Optional, Sequence
@@ -324,7 +325,8 @@ class CcoContext:
             rk[k] = N.LogRankingT(nb, N.POP_MODES.get(mode, -1), len(en), int(start_ms), int(end_ms), arr)
         return rk
 
-    def read_events(self, src, chunk_bytes: Optional[int] = None) -> "EventLog":
+    def read_events(self, src, chunk_bytes: Optional[int] = None, window: Optional[E.EventWindow] = None,
+                    now_ms: Optional[int] = None) -> "EventLog":
         """A PredictionIO event export (JSON lines, as `pio export` writes them) parsed on the device.  src is one of
           - bytes or a buffer: one read (cco_event_log_read), or chunks of chunk_bytes when it is given;
           - a file path, a directory as `pio export` writes it (its part-* files in name order; events.export_parts) or a
@@ -334,13 +336,17 @@ class CcoContext:
           - an iterable of buffers (a generator, say): streamed, each appended as it comes.
         chunk_bytes defaults to DEFAULT_CHUNK_BYTES for streamed sources; it is also the device staging.  The log is the one
         cco_event_log_read of the concatenated bytes gives.
+        window: the DataSource's eventWindow (events.EventWindow; cco_event_log_begin_window), applied on the device while the
+        export is read: events at or before now_ms - duration expire ($set / $unset excepted), and with removeDuplicates
+        equal events collapse to the latest.  now_ms defaults to the wall clock; EventLog.window_stats() counts the drops.
         -> EventLog (free with .free(), or use it as a context manager; close() of this context frees the logs still open)."""
-        if isinstance(src, (bytes, bytearray, memoryview, np.ndarray)) and chunk_bytes is None:
+        whole = isinstance(src, (bytes, bytearray, memoryview, np.ndarray)) and chunk_bytes is None
+        if whole and window is None:
             buf = np.frombuffer(src, dtype=np.uint8) if not isinstance(src, np.ndarray) else np.ascontiguousarray(src, dtype=np.uint8)
             h = C.c_void_p()
             N.check(self._L.cco_event_log_read(self._h, buf.ctypes.data if len(buf) else None, len(buf), C.byref(h)))
             return self._adopt_log(h)
-        chunk = int(chunk_bytes or DEFAULT_CHUNK_BYTES)
+        chunk = int(chunk_bytes or (max(memoryview(src).nbytes, 1) if whole else DEFAULT_CHUNK_BYTES))
         paths = None
         if isinstance(src, (str, os.PathLike)):
             p = os.fspath(src)
@@ -348,7 +354,13 @@ class CcoContext:
         elif isinstance(src, (list, tuple)) and all(isinstance(x, (str, os.PathLike)) for x in src):
             paths = [os.fspath(x) for x in src]
         h = C.c_void_p()
-        N.check(self._L.cco_event_log_begin(self._h, chunk, C.byref(h)))
+        if window is None:
+            N.check(self._L.cco_event_log_begin(self._h, chunk, C.byref(h)))
+        else:
+            now = now_ms if now_ms is not None else int(time.time() * 1000)
+            cutoff = window.cutoff_ms(now)
+            w = N.EventWindowT(-(1 << 63) if cutoff is None else cutoff, 1 if window.removeDuplicates else 0, 0)
+            N.check(self._L.cco_event_log_begin_window(self._h, chunk, C.byref(w), C.byref(h)))
         try:
             if paths is not None:
                 self._append_files(h, paths, chunk)
@@ -699,6 +711,12 @@ class EventLog:
         per = lambda p: np.ctypeslib.as_array(p, shape=(g,)).tolist() if g else []
         return EventLogInfo(i.n_lines, names, per(i.n_training), per(i.n_ranking), i.n_property_events, i.n_property_items,
                             i.n_property_fields, i.n_ignored)
+
+    def window_stats(self) -> tuple[int, int]:
+        """(expired, duplicates): the lines the eventWindow dropped (both 0 for a read without one)"""
+        x, d = C.c_int64(), C.c_int64()
+        N.check(self._ctx._L.cco_event_log_window_stats(self._h, C.byref(x), C.byref(d)))
+        return x.value, d.value
 
     def free(self):
         if getattr(self, "_h", None):

@@ -199,25 +199,36 @@ def _log_rankings(ap: URAlgorithmParams, now_ms: Optional[int]) -> list:
     return out
 
 
-def _read_log(export, ctx: CcoContext):
+def _read_log(export, ctx: CcoContext, window=None, now_ms: Optional[int] = None):
     """(log, owned): an EventLog as given, or one read by CcoContext.read_events (bytes, a buffer, a path, a `pio export`
-    directory, a sequence of paths or an iterable of buffers)"""
+    directory, a sequence of paths or an iterable of buffers), through the eventWindow when one is given"""
     from .similarity_analysis import EventLog
-    return (export, False) if isinstance(export, EventLog) else (ctx.read_events(export), True)
+    if isinstance(export, EventLog):
+        if window is not None:
+            raise ValueError("the eventWindow applies while an export is read: pass the export, or read it with read_events(window=...)")
+        return export, False
+    return ctx.read_events(export, window=window, now_ms=now_ms), True
+
+
+def _now(now_ms: Optional[int]) -> int:
+    return now_ms if now_ms is not None else int(time.time() * 1000)
 
 
 def calc_all_from_events(export, ap: URAlgorithmParams, min_events_per_user: Optional[int] = None, now_ms: Optional[int] = None,
-                         ctx: CcoContext | None = None, flags: int = 0) -> bytes:
+                         ctx: CcoContext | None = None, flags: int = 0, event_window=None) -> bytes:
     """calc_all_on_device from a PredictionIO event export (any source CcoContext.read_events takes, or an EventLog of this
     context): the export is copied to the GPU and parsed there (the DataSource: include/cco_b200.h cco_event_log_read); the training
     events, the ranking streams and the items' properties, aggregated there from their $set / $unset / $delete events,
-    stay in HBM.  Property values are spliced as written.  Same decisions as calc_all_on_device."""
+    stay in HBM.  Property values are spliced as written.  Same decisions as calc_all_on_device.
+    event_window: the DataSource's eventWindow (events.EventWindow, DataSourceParams.eventWindow), applied to every
+    selection on the device; its duration counts back from the same now_ms as the rankings."""
     _check_recs_model(ap)
     if ap.recsModel == "backfill":
         raise ValueError("recsModel=backfill runs calcPop against the live index: use calc_pop_from_events with its bulk body")
     ctx = ctx or default_context()
     seed, flags = _seed_and_flags(ap, flags)
-    log, owned = _read_log(export, ctx)
+    now_ms = _now(now_ms)
+    log, owned = _read_log(export, ctx, event_window, now_ms)
     try:
         info = log.info()
         n_train = dict(zip(info.names, info.n_training))
@@ -259,11 +270,14 @@ def calc_pop_on_device(body: bytes, events: Sequence[tuple[str, str, str, int]],
     return ctx.rerank_model(body, props, rankings)
 
 
-def calc_pop_from_events(body: bytes, export, ap: URAlgorithmParams, now_ms: Optional[int] = None, ctx: CcoContext | None = None) -> bytes:
+def calc_pop_from_events(body: bytes, export, ap: URAlgorithmParams, now_ms: Optional[int] = None, ctx: CcoContext | None = None,
+                         event_window=None) -> bytes:
     """calc_pop_on_device from a PredictionIO event export (as in calc_all_from_events): the ranking streams and the
-    properties of the log, both in HBM, joined into the old index by cco_rerank_model_log."""
+    properties of the log, both in HBM, joined into the old index by cco_rerank_model_log.  event_window as in
+    calc_all_from_events."""
     ctx = ctx or default_context()
-    log, owned = _read_log(export, ctx)
+    now_ms = _now(now_ms)
+    log, owned = _read_log(export, ctx, event_window, now_ms)
     try:
         return ctx.rerank_model(body, None, _log_rankings(ap, now_ms), log=log)
     finally:

@@ -93,6 +93,44 @@ def duration_seconds(duration) -> int:
     return int(Decimal(m.group(1)) * (_UNITS[m.group(2)] if m.group(2) else 1))
 
 
+_NANOS = {**{u: 86_400_000_000_000 for u in ("d", "day", "days")}, **{u: 3_600_000_000_000 for u in ("h", "hour", "hours")},
+          **{u: 60_000_000_000 for u in ("min", "minute", "minutes")}, **{u: 1_000_000_000 for u in ("s", "sec", "secs", "second", "seconds")},
+          **{u: 1_000_000 for u in ("ms", "milli", "millis", "millisecond", "milliseconds")},
+          **{u: 1_000 for u in ("µs", "micro", "micros", "microsecond", "microseconds")},
+          **{u: 1 for u in ("ns", "nano", "nanos", "nanosecond", "nanoseconds")}}
+_DOUBLE = re.compile(r"[+-]?(?:[0-9]+\.?[0-9]*|\.[0-9]+)(?:[eE][+-]?[0-9]+)?")
+_LONG_MAX = (1 << 63) - 1
+
+
+def duration_ms(duration: str) -> int:
+    """Scala's `Duration(duration).toMillis`, as PredictionIO's EventWindow reads its duration [RECALL, unverifiable here]:
+    whitespace is removed; the unit is the trailing letters, one of scala.concurrent.duration's labels (d day, h hour,
+    min minute, s sec second, ms milli millisecond, µs micro microsecond, ns nano nanosecond; each word also with an "s");
+    the number before it is a Java double.  Up to 2^53 it is scaled to nanoseconds in double arithmetic and rounded (x +
+    0.5, truncated), beyond that it must be an integer and is scaled exactly; either way |nanoseconds| <= 2^63 - 1.  The
+    result is truncated toward zero to milliseconds.  "Inf" and the other infinite durations have no millisecond value:
+    like everything else that does not parse, they raise ValueError."""
+    s = "".join(str(duration).split())
+    unit = re.search(r"[^\W\d_]*\Z", s).group(0)
+    num = s[:len(s) - len(unit)]
+    if unit not in _NANOS or not _DOUBLE.fullmatch(num):
+        raise ValueError(f"bad duration {duration!r}")
+    value = float(num)
+    if abs(value) <= 2.0 ** 53:
+        nanos = float(_NANOS[unit]) * value
+        if not -_LONG_MAX - 1 <= nanos <= _LONG_MAX:
+            raise ValueError(f"duration {duration!r} is out of range")
+        nanos = int(nanos + 0.5)
+    else:
+        if not re.fullmatch(r"[+-]?[0-9]+", num):
+            raise ValueError(f"bad duration {duration!r}")
+        nanos = int(num) * _NANOS[unit]
+        if not -_LONG_MAX <= nanos <= _LONG_MAX:
+            raise ValueError(f"duration {duration!r} is out of range")
+    ms = abs(nanos) // 1_000_000
+    return ms if nanos >= 0 else -ms
+
+
 def ranking_window(rp: RankingParams, now_ms: int) -> tuple[int, int]:
     """PopModel.calc (PopModel.scala:57-77): end = offsetDate (ISO 8601; 'now' if it does not parse, as the reference
     warns and does), start = end - duration seconds.  Events count in [start, end)."""
