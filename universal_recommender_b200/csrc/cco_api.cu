@@ -406,16 +406,8 @@ struct DevMat {  // after canonicalise + downsample
   int32_t *marg = nullptr;  // post-sample column counts
 };
 
-static int exclusive_sum_u32(cco_ctx *c, Arena &ar, const uint32_t *in, uint32_t *out, long long n) {
-  size_t tb = 0;
-  CK(cub::DeviceScan::ExclusiveSum(nullptr, tb, in, out, n, c->stream));
-  void *tmp;
-  CKR(ar.alloc((char **)&tmp, tb));
-  CK(cub::DeviceScan::ExclusiveSum(tmp, tb, in, out, n, c->stream));
-  ar.release(tmp);
-  return CCO_OK;
-}
-static int exclusive_sum_i64(cco_ctx *c, Arena &ar, const long long *in, long long *out, long long n, cudaStream_t on = nullptr) {
+template <typename T>
+static int exclusive_sum(cco_ctx *c, Arena &ar, const T *in, T *out, long long n, cudaStream_t on = nullptr) {
   if (!on) on = c->stream;
   size_t tb = 0;
   CK(cub::DeviceScan::ExclusiveSum(nullptr, tb, in, out, n, on));
@@ -424,6 +416,34 @@ static int exclusive_sum_i64(cco_ctx *c, Arena &ar, const long long *in, long lo
   CK(cub::DeviceScan::ExclusiveSum(tmp, tb, in, out, n, on));
   ar.release(tmp);
   return CCO_OK;
+}
+// sort (key, value) pairs of n entries by the low `bits` bits of the key, stably; the sorted arrays replace *k / *v
+template <typename K, typename V>
+static int sort_pairs(cco_ctx *c, Arena &ar, long long n, K **k, V **v, int bits) {
+  cudaStream_t s = c->stream;
+  K *k1;
+  V *v1;
+  CKR(ar.alloc(&k1, std::max<long long>(n, 1)));
+  CKR(ar.alloc(&v1, std::max<long long>(n, 1)));
+  cub::DoubleBuffer<K> kb(*k, k1);
+  cub::DoubleBuffer<V> vb(*v, v1);
+  size_t tbytes = 0;
+  CK(cub::DeviceRadixSort::SortPairs(nullptr, tbytes, kb, vb, n, 0, bits, s));
+  void *tmp;
+  CKR(ar.alloc((char **)&tmp, tbytes));
+  CK(cub::DeviceRadixSort::SortPairs(tmp, tbytes, kb, vb, n, 0, bits, s));
+  c->launches++;
+  ar.release(tmp);
+  ar.release(kb.Alternate());
+  ar.release(vb.Alternate());
+  *k = kb.Current();
+  *v = vb.Current();
+  return CCO_OK;
+}
+static int bits_for(long long n) {
+  int b = 1;
+  while ((1LL << b) < n) ++b;
+  return b;
 }
 
 // canonicalisation slow path: sort (row,col) keys, drop duplicates, rebuild row_ptr
@@ -450,7 +470,7 @@ static int canonicalize_device(cco_ctx *c, Arena &ar, DevRaw &m) {
   CK(cudaMemsetAsync(flag + m.nnz, 0, 4, c->stream));
   k_unique_flags<<<grid_for(m.nnz, 256, c->sm_count), 256, 0, c->stream>>>(m.nnz, sorted, flag);
   c->launches++;
-  CKR(exclusive_sum_u32(c, ar, flag, pos, m.nnz + 1));
+  CKR(exclusive_sum(c, ar, flag, pos, m.nnz + 1));
   uint32_t n_unique = 0;
   CK(cudaMemcpyAsync(&n_unique, pos + m.nnz, 4, cudaMemcpyDeviceToHost, c->stream));
   // the canonical block is rewritten 0-based at the start of its own column storage
@@ -550,7 +570,7 @@ static int downsample_device(cco_ctx *c, Arena &ar, const DevRaw &raw, const int
   SampleScratch sc;
   CKR(sample_scratch(c, ar, raw, raw_counts, m, &sc));
   launch_count(c, raw, sc, m, seed, flags, bad, kept, out->marg);
-  CKR(exclusive_sum_u32(c, ar, kept, out->rp, raw.n_rows + 1));
+  CKR(exclusive_sum(c, ar, kept, out->rp, raw.n_rows + 1));
   CKR(launch_write(c, ar, raw, sc, out->col));
   CK(cudaGetLastError());
   ar.release(kept);
@@ -611,7 +631,7 @@ static int downsample_sharded_all(cco_ctx *c, Arena &ar, const std::vector<DevRa
   // wait, no stream-wide sync) and the gather is padded to the largest SAMPLED block only.
   std::vector<uint32_t> edge((size_t)n_mats * (W + 1), 0);
   for (int i = 0; i < n_mats; ++i) {
-    CKR(exclusive_sum_u32(c, ar, kept[i], dm[i].rp, U + 1));
+    CKR(exclusive_sum(c, ar, kept[i], dm[i].rp, U + 1));
     ar.release(kept[i]);
     for (int q = 0; q <= W; ++q) CKR(mail_fetch(c, &edge[(size_t)i * (W + 1) + q], dm[i].rp + std::min<long long>((long long)q * S, U), 4));
   }
@@ -808,7 +828,7 @@ static int enqueue_indicator(cco_ctx *c, Arena &ar, const uint32_t *at_ptr, cons
   k_row_work<<<grid_for((long long)n_items_a * kSG, 256, c->sm_count), 256, 0, ss>>>(n_items_a, at_ptr, at_users, B.rp,
                                                                                   row_work, work64, ids, nullptr);
   c->launches++;
-  CKR(exclusive_sum_i64(c, ar, (const long long *)work64, work_prefix, (long long)n_items_a + 1, ss));
+  CKR(exclusive_sum(c, ar, (const long long *)work64, work_prefix, (long long)n_items_a + 1, ss));
   if (world > 1) {
     // contiguous item ranges balanced by work prefix, identical on every rank; they never leave the device
     CKR(ar.alloc(&d_pb, world + 1));
@@ -996,7 +1016,7 @@ static int enqueue_indicator(cco_ctx *c, Arena &ar, const uint32_t *at_ptr, cons
   CKR(ar.alloc(&rec_d, 8));
   k_len_to_i64<<<grid_for((long long)n_items_a + 1, 256, c->sm_count), 256, 0, s>>>(n_items_a, o_len, d_pb, rank, len64);
   c->launches++;
-  CKR(exclusive_sum_i64(c, ar, len64, st->out_ptr, (long long)n_items_a + 1));
+  CKR(exclusive_sum(c, ar, len64, st->out_ptr, (long long)n_items_a + 1));
   // the packed size is only known on the device: the buffers take the worst case (every row of the item space full)
   CKR(ar.alloc(&st->p_col, cells));
   if (!(flags & CCO_FLAG_RESULT_NO_COUNT) || emit_all) CKR(ar.alloc(&st->p_cnt, cells));
@@ -1416,7 +1436,7 @@ static int train_dataset(cco_ctx *c, const cco_dataset *ds, const cco_indicator_
     CKR(ar.alloc(&marg_pad, n_items_a + 1));
     CK(cudaMemcpyAsync(marg_pad, dm[0].marg, sizeof(int32_t) * (size_t)n_items_a, cudaMemcpyDeviceToDevice, s));
     CK(cudaMemsetAsync(marg_pad + n_items_a, 0, 4, s));
-    CKR(exclusive_sum_u32(c, ar, marg_pad, at_ptr, (long long)n_items_a + 1));
+    CKR(exclusive_sum(c, ar, marg_pad, at_ptr, (long long)n_items_a + 1));
     ar.release(marg_pad);
   }
   CK(cudaMemcpyAsync(cursor, at_ptr, sizeof(uint32_t) * ((size_t)n_items_a + 1), cudaMemcpyDeviceToDevice, s));
@@ -1891,7 +1911,7 @@ static int ingest_csr(cco_ctx *c, Arena &ar, cco_dataset *d, int t, long long ne
     CKR(ar.alloc(&pos, kept + 1));
     CK(cudaMemsetAsync(flag + kept, 0, 4, s));
     k_unique_flags<<<grid_for((long long)kept, 256, c->sm_count), 256, 0, s>>>((long long)kept, sorted, flag);
-    CKR(exclusive_sum_u32(c, ar, flag, pos, (long long)kept + 1));
+    CKR(exclusive_sum(c, ar, flag, pos, (long long)kept + 1));
     uint32_t nuq = 0;
     CKR(mail_fetch(c, &nuq, pos + kept, 4));
     k_unique_scatter<<<grid_for((long long)kept, 256, c->sm_count), 256, 0, s>>>((long long)kept, sorted, flag, pos, other, d->col[t]);
@@ -1974,7 +1994,7 @@ static int ingest_core(cco_ctx *c, const IngestSource &src, int32_t min_events_p
       const int32_t need = min_events_per_user > 1 ? min_events_per_user : 1;
       if (n_users_raw > 0)
         k_ingest_user_flags<<<grid_for(n_users_raw, 256, c->sm_count), 256, 0, s>>>(n_users_raw, cnt, need, uflag);
-      CKR(exclusive_sum_u32(c, ar, uflag, upos, nu + 1));
+      CKR(exclusive_sum(c, ar, uflag, upos, nu + 1));
       if (n_users_raw > 0)
         k_ingest_make_map<<<grid_for(n_users_raw, 256, c->sm_count), 256, 0, s>>>(n_users_raw, uflag, upos, d_user_map);
       c->launches += 3;
@@ -1996,7 +2016,7 @@ static int ingest_core(cco_ctx *c, const IngestSource &src, int32_t min_events_p
       CK(cudaMemsetAsync(iflag, 0, sizeof(uint32_t) * ((size_t)ni + 1), s));
       if (ne > 0) k_ingest_item_flags<<<grid_for(ne, 256, c->sm_count), 256, 0, s>>>(ne, d_user, d_item, d_user_map, iflag);
     }
-    CKR(exclusive_sum_u32(c, ar, iflag, ipos, ni + 1));
+    CKR(exclusive_sum(c, ar, iflag, ipos, ni + 1));
     k_ingest_make_map<<<grid_for(ni, 256, c->sm_count), 256, 0, s>>>(src.n_items_raw[t], iflag, ipos, d_item_map);
     uint32_t n_items = 0;
     CKR(mail_fetch(c, &n_items, ipos + src.n_items_raw[t], 4));
@@ -2212,7 +2232,7 @@ static int str_group(cco_ctx *c, Arena &ar, const DevStrCol &col, const int32_t 
   CKR(ar.alloc(&pos, cap + 1));
   CK(cudaMemsetAsync(flag + cap, 0, 4, s));
   k_str_flags<<<grid_for(cap, 256, c->sm_count), 256, 0, s>>>(cap, tb->table, tb->count, need, flag);
-  CKR(exclusive_sum_u32(c, ar, flag, pos, cap + 1));
+  CKR(exclusive_sum(c, ar, flag, pos, cap + 1));
   uint32_t ng = 0;
   CKR(mail_fetch(c, &ng, pos + cap, 4));
   CKR(mail_wait(c));
@@ -2262,7 +2282,7 @@ static int str_dictionary(cco_ctx *c, Arena &ar, const DevStrCol &col, const Str
     k_str_dict_len<<<grid_for(ng, 256, c->sm_count), 256, 0, s>>>(ng, tb.first_sorted, col.off, len);
     c->launches++;
   }
-  CKR(exclusive_sum_i64(c, ar, len, off, ng + 1));
+  CKR(exclusive_sum(c, ar, len, off, ng + 1));
   long long total = 0;
   CKR(mail_fetch(c, &total, off + ng, 8));
   CKR(mail_wait(c));
@@ -2577,7 +2597,7 @@ static int escape_dict(cco_ctx *c, Arena &ar, const DevDict &raw, DevDict *esc) 
     k_escape_len<<<grid_for(raw.n, 256, c->sm_count), 256, 0, c->stream>>>(raw.n, raw.off, raw.bytes, len);
     c->launches++;
   }
-  CKR(exclusive_sum_i64(c, ar, len, off, raw.n + 1));
+  CKR(exclusive_sum(c, ar, len, off, raw.n + 1));
   long long total = 0;
   CK(cudaMemcpyAsync(&total, off + raw.n, 8, cudaMemcpyDeviceToHost, c->stream));
   CK(cudaStreamSynchronize(c->stream));
@@ -2632,13 +2652,13 @@ struct KeySection {
   long long base = 0;   // device: off[0] (bytes points at that byte)
   long long byte_count() const { return n == 0 ? 0 : device ? nbytes : off[n] - off[0]; }
 };
-// one ranking stream of an event log (cco_format_model_log): the target ids of one event name's ranking events and their
-// times, both in HBM; per ranking, one per event name read
-struct LogStream {
+// one ranking stream: the target ids of one event name's ranking events and their times, both on the host (a
+// cco_ranking_stream_t) or both in HBM (an event log's columns) as items.device says; per ranking, its streams in order
+struct Stream {
   KeySection items;
-  const long long *time;
+  const int64_t *time;
 };
-using LogStreams = std::vector<std::vector<LogStream>>;
+using Streams = std::vector<std::vector<Stream>>;
 // the properties of an event log (cco_format_model_log): the columns of cco_item_properties_t in HBM, built on the device
 struct DevProps {
   KeySection items;
@@ -2651,7 +2671,7 @@ struct DevProps {
 // rankings per group, sort the properties, and list the documents of items without a row.  The caller's host columns have
 // passed str_check_host.  unique_rows: two rows with the same id are CCO_E_INVALID_ARG (the documents of an old index).
 static int model_fields(cco_ctx *c, Arena &ar, FormatArgs *fa, const KeySection &rows, const cco_item_properties_t *props,
-                        int32_t n_rank, const cco_ranking_t *rk, bool extra_docs, bool unique_rows = false, const LogStreams *ls = nullptr,
+                        int32_t n_rank, const cco_ranking_t *rk, const Streams &st, bool extra_docs, bool unique_rows = false,
                         const DevProps *dp = nullptr) {
   cudaStream_t s = c->stream;
   mail_reset(c);
@@ -2663,17 +2683,9 @@ static int model_fields(cco_ctx *c, Arena &ar, FormatArgs *fa, const KeySection 
   long long E = 0;
   for (int k = 0; k < n_rank; ++k) {
     rank_begin[k] = E;
-    if (ls) {
-      for (const LogStream &st : (*ls)[k]) {
-        sec.push_back(st.items);
-        E += st.items.n;
-      }
-      continue;
-    }
-    for (int q = 0; q < rk[k].n_streams; ++q) {
-      const cco_ranking_stream_t &st = rk[k].streams[q];
-      sec.push_back({st.n_events, st.item_offsets, st.item_bytes});
-      E += st.n_events;
+    for (const Stream &q : st[k]) {
+      sec.push_back(q.items);
+      E += q.items.n;
     }
   }
   rank_begin[n_rank] = E;
@@ -2744,17 +2756,11 @@ static int model_fields(cco_ctx *c, Arena &ar, FormatArgs *fa, const KeySection 
   CKR(ar.alloc(&d_t, std::max<long long>(E, 1)));
   for (int k = 0; k < n_rank; ++k) {
     long long e = rank_begin[k];
-    if (ls) {
-      for (const LogStream &st : (*ls)[k]) {
-        if (st.items.n > 0) CK(cudaMemcpyAsync(d_t + e, st.time, sizeof(int64_t) * (size_t)st.items.n, cudaMemcpyDeviceToDevice, s));
-        e += st.items.n;
-      }
-      continue;
-    }
-    for (int q = 0; q < rk[k].n_streams; ++q) {
-      const cco_ranking_stream_t &st = rk[k].streams[q];
-      if (st.n_events > 0) CK(cudaMemcpyAsync(d_t + e, st.time_ms, sizeof(int64_t) * (size_t)st.n_events, cudaMemcpyHostToDevice, s));
-      e += st.n_events;
+    for (const Stream &q : st[k]) {
+      if (q.items.n > 0)
+        CK(cudaMemcpyAsync(d_t + e, q.time, sizeof(int64_t) * (size_t)q.items.n,
+                           q.items.device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, s));
+      e += q.items.n;
     }
   }
   // the device verdict comes before any kernel reads bytes through the offsets
@@ -2788,31 +2794,20 @@ static int model_fields(cco_ctx *c, Arena &ar, FormatArgs *fa, const KeySection 
   fa->row_group = gid + fa->row_id_base;
   // 2. properties: sorted by (group, field), stable in the triple index, so the last triple of each run wins
   if (P > 0) {
-    unsigned long long *k0, *k1;
-    int32_t *v0, *v1, *pbeg, *pend;
-    CKR(ar.alloc(&k0, P));
-    CKR(ar.alloc(&k1, P));
-    CKR(ar.alloc(&v0, P));
-    CKR(ar.alloc(&v1, P));
+    unsigned long long *key;
+    int32_t *tri, *pbeg, *pend;
+    CKR(ar.alloc(&key, P));
+    CKR(ar.alloc(&tri, P));
     CKR(ar.alloc(&pbeg, G));
     CKR(ar.alloc(&pend, G));
     CK(cudaMemsetAsync(pbeg, 0, sizeof(int32_t) * (size_t)G, s));
     CK(cudaMemsetAsync(pend, 0, sizeof(int32_t) * (size_t)G, s));
-    k_prop_keys<<<grid_for(P, 256, c->sm_count), 256, 0, s>>>(P, gid + R, d_field, k0, v0);
-    int gbits = 1;
-    while ((1LL << gbits) < G) ++gbits;
-    cub::DoubleBuffer<unsigned long long> kb(k0, k1);
-    cub::DoubleBuffer<int32_t> vb(v0, v1);
-    size_t tbytes = 0;
-    CK(cub::DeviceRadixSort::SortPairs(nullptr, tbytes, kb, vb, (long long)P, 0, 32 + gbits, s));
-    void *tmp;
-    CKR(ar.alloc((char **)&tmp, tbytes));
-    CK(cub::DeviceRadixSort::SortPairs(tmp, tbytes, kb, vb, (long long)P, 0, 32 + gbits, s));
-    ar.release(tmp);
-    k_prop_ranges<<<grid_for(P, 256, c->sm_count), 256, 0, s>>>(P, kb.Current(), pbeg, pend);
-    c->launches += 3;
-    fa->pkey = kb.Current();
-    fa->ptri = vb.Current();
+    k_prop_keys<<<grid_for(P, 256, c->sm_count), 256, 0, s>>>(P, gid + R, d_field, key, tri);
+    CKR(sort_pairs(c, ar, P, &key, &tri, 32 + bits_for(G)));
+    k_prop_ranges<<<grid_for(P, 256, c->sm_count), 256, 0, s>>>(P, key, pbeg, pend);
+    c->launches += 2;
+    fa->pkey = key;
+    fa->ptri = tri;
     fa->pbeg = pbeg;
     fa->pend = pend;
   }
@@ -2863,7 +2858,7 @@ static int model_fields(cco_ctx *c, Arena &ar, FormatArgs *fa, const KeySection 
     CK(cudaMemsetAsync(flag + G, 0, 4, s));
     k_extra_flags<<<grid_for(G, 256, c->sm_count), 256, 0, s>>>(G, tb.first_sorted, R, fa->pbeg, fa->pend, fa->pmask, flag);
     c->launches++;
-    CKR(exclusive_sum_u32(c, ar, flag, pos, G + 1));
+    CKR(exclusive_sum(c, ar, flag, pos, G + 1));
     uint32_t n_extra = 0;
     CKR(mail_fetch(c, &n_extra, pos + G, 4));
     CKR(mail_wait(c));
@@ -2878,7 +2873,7 @@ static int model_fields(cco_ctx *c, Arena &ar, FormatArgs *fa, const KeySection 
       k_extra_compact<<<grid_for(G, 256, c->sm_count), 256, 0, s>>>(G, flag, pos, tb.first_sorted, extra_group, extra_first);
       CK(cudaMemsetAsync(len + n_extra, 0, 8, s));
       k_str_dict_len<<<grid_for(n_extra, 256, c->sm_count), 256, 0, s>>>(n_extra, extra_first, key.off, len);
-      CKR(exclusive_sum_i64(c, ar, len, off, (long long)n_extra + 1));
+      CKR(exclusive_sum(c, ar, len, off, (long long)n_extra + 1));
       long long total = 0;
       CKR(mail_fetch(c, &total, off + n_extra, 8));
       CKR(mail_wait(c));
@@ -2896,9 +2891,10 @@ static int model_fields(cco_ctx *c, Arena &ar, FormatArgs *fa, const KeySection 
   return CCO_OK;
 }
 
-// host checks of the model inputs (the device checks decreasing offsets, field indices and empty values)
+// host checks of the model inputs (the device checks decreasing offsets, field indices and empty values).  st: the
+// rankings' streams; empty for rankings that hold their streams (cco_ranking_t), which are listed into it as they are checked
 static int model_check_host(const cco_dictionary_t *row_ids, const cco_item_properties_t *props, int32_t n_rank, const cco_ranking_t *rk,
-                            const LogStreams *ls = nullptr, bool dev_props = false) {
+                            Streams *st, bool dev_props = false) {
   if (n_rank < 0 || (n_rank > 0 && !rk)) return set_error(CCO_E_INVALID_ARG, "bad rankings");
   if (n_rank > kMaxRankings) return set_error(CCO_E_UNSUPPORTED, "%d rankings, at most %d", n_rank, kMaxRankings);
   long long total = row_ids->n;
@@ -2918,23 +2914,27 @@ static int model_check_host(const cco_dictionary_t *row_ids, const cco_item_prop
     }
     total += props->n;
   }
+  const bool listed = !st->empty();
+  st->resize(n_rank);
   for (int k = 0; k < n_rank; ++k) {
     const cco_ranking_t &r = rk[k];
     if (!r.name) return set_error(CCO_E_INVALID_ARG, "ranking %d: null name", k);
     if (r.mode < CCO_POP_POPULAR || r.mode > CCO_POP_RANDOM)
       return set_error(CCO_E_INVALID_ARG, "ranking %d: mode must be CCO_POP_POPULAR, _TRENDING, _HOT or _RANDOM", k);
     if (r.end_ms < r.start_ms) return set_error(CCO_E_INVALID_ARG, "ranking %d: end before start (Joda Interval would throw)", k);
-    if (ls) {   // the log's columns were built on the device
-      for (const LogStream &st : (*ls)[k]) total += st.items.n;
-      if (total >= 0x7fffffffLL) break;
-      continue;
+    if (!listed) {
+      if (r.n_streams < 1 || !r.streams) return set_error(CCO_E_INVALID_ARG, "ranking %d: needs at least one stream", k);
+      for (int q = 0; q < r.n_streams; ++q) {
+        const cco_ranking_stream_t &h = r.streams[q];
+        (*st)[k].push_back({{h.n_events, h.item_offsets, h.item_bytes}, h.time_ms});
+      }
     }
-    if (r.n_streams < 1 || !r.streams) return set_error(CCO_E_INVALID_ARG, "ranking %d: needs at least one stream", k);
-    for (int q = 0; q < r.n_streams; ++q) {
-      const cco_ranking_stream_t &st = r.streams[q];
-      CKR(str_check_host(st.n_events, st.item_offsets, st.item_bytes, k, "ranking item"));
-      if (st.n_events > 0 && !st.time_ms) return set_error(CCO_E_INVALID_ARG, "ranking %d: null event times", k);
-      total += st.n_events;
+    for (const Stream &q : (*st)[k]) {
+      if (!q.items.device) {
+        CKR(str_check_host(q.items.n, q.items.off, q.items.bytes, k, "ranking item"));
+        if (q.items.n > 0 && !q.time) return set_error(CCO_E_INVALID_ARG, "ranking %d: null event times", k);
+      }
+      total += q.items.n;
       if (total >= 0x7fffffffLL) break;
     }
     if (total >= 0x7fffffffLL) break;
@@ -3011,8 +3011,7 @@ static int model_names(cco_ctx *c, Arena &ar, FormatArgs *fa, int n_ind, const c
 // cco_format_es_bulk == format_model without properties and rankings: one set of document kernels
 static int format_model(cco_ctx_t *ctx, const cco_result_t *res, int32_t n_names, const char *const *names, const cco_dictionary_t *row_ids,
                         const cco_dictionary_t *col_ids, const cco_item_properties_t *props, int32_t n_rank, const cco_ranking_t *rk,
-                        char **out_bytes, int64_t *out_len, const char *range, const LogStreams *ls = nullptr,
-                        const DevProps *dp = nullptr) {
+                        char **out_bytes, int64_t *out_len, const char *range, Streams st = {}, const DevProps *dp = nullptr) {
   if (!ctx || !res || !names || !row_ids || !col_ids || !out_bytes || !out_len) return set_error(CCO_E_INVALID_ARG, "null argument");
   const int n_ind = (int)res->mats.size();
   if (n_names != n_ind) return set_error(CCO_E_INVALID_ARG, "%d event names for %d indicators", n_names, n_ind);
@@ -3028,7 +3027,7 @@ static int format_model(cco_ctx_t *ctx, const cco_result_t *res, int32_t n_names
   }
   if (row_ids->n < row_hi) return set_error(CCO_E_INVALID_ARG, "row dictionary has %lld ids, rows go up to %lld", (long long)row_ids->n, (long long)row_hi);
   const bool model = (props && props->n > 0) || n_rank > 0;
-  if (model) CKR(model_check_host(row_ids, props, n_rank, rk, ls, dp != nullptr));
+  if (model) CKR(model_check_host(row_ids, props, n_rank, rk, &st, dp != nullptr));
   CK(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   Arena ar(s);
@@ -3043,7 +3042,7 @@ static int format_model(cco_ctx_t *ctx, const cco_result_t *res, int32_t n_names
   CKR(upload_dict(c, ar, *row_ids, &raw));
   CKR(escape_dict(c, ar, raw, &fa.row_ids));
   CKR(model_names(c, ar, &fa, n_ind, names, model, props, n_rank, rk));
-  if (model) CKR(model_fields(c, ar, &fa, KeySection{row_ids->n, row_ids->offsets, row_ids->bytes}, props, n_rank, rk, row_lo == 0, false, ls, dp));
+  if (model) CKR(model_fields(c, ar, &fa, KeySection{row_ids->n, row_ids->offsets, row_ids->bytes}, props, n_rank, rk, st, row_lo == 0, false, dp));
   for (int i = 0; i < n_ind; ++i) {
     const ResultMat &m = res->mats[i];
     CKR(upload_dict(c, ar, col_ids[i], &raw));
@@ -3071,7 +3070,7 @@ static int format_model(cco_ctx_t *ctx, const cco_result_t *res, int32_t n_names
     k_doc_len<<<grid_for(n_docs, 256, c->sm_count), 256, 0, s>>>(fa, n_docs, doc_len);
     c->launches++;
   }
-  CKR(exclusive_sum_i64(c, ar, doc_len, doc_off, (long long)n_docs + 1));
+  CKR(exclusive_sum(c, ar, doc_len, doc_off, (long long)n_docs + 1));
   long long total = 0;
   CK(cudaMemcpyAsync(&total, doc_off + n_docs, 8, cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
@@ -3107,9 +3106,10 @@ static int json_error(unsigned long long err, bool lines) {
   return set_error(CCO_E_INVALID_ARG, "document %lld: the %s line is not one JSON object (unbalanced brackets or an unexpected token)",
                    doc, part);
 }
-// one tokenizer run over n object spans: count, verdict, write.  moff[s] = first member of span s, *total = all members
+// one tokenizer run over n object spans: count, verdict (*verdict = ~0: every span is one object), then, when the verdict
+// is clean and the members are fewer than limit, write.  moff[s] = first member of span s, *total = all members
 static int json_members(cco_ctx *c, Arena &ar, long long n, const long long *sb, const long long *se, const unsigned char *body,
-                        bool lines, long long **moff_out, JMember **mem_out, long long *total_out) {
+                        long long limit, unsigned long long *verdict, long long **moff_out, JMember **mem_out, long long *total_out) {
   cudaStream_t s = c->stream;
   long long *cnt, *moff;
   unsigned long long *err;
@@ -3119,16 +3119,17 @@ static int json_members(cco_ctx *c, Arena &ar, long long n, const long long *sb,
   CK(cudaMemsetAsync(cnt + n, 0, 8, s));
   CK(cudaMemsetAsync(err, 0xff, 8, s));
   const int grid = grid_for(n * 32, 256, c->sm_count);
-  k_json_members<<<grid, 256, 0, s>>>(n, sb, se, body, MemberSink<false>{cnt, nullptr, nullptr}, err);
-  c->launches++;
-  CKR(exclusive_sum_i64(c, ar, cnt, moff, n + 1));
-  unsigned long long h_err = 0;
+  if (n > 0) {
+    k_json_members<<<grid, 256, 0, s>>>(n, sb, se, body, MemberSink<false>{cnt, nullptr, nullptr}, err);
+    c->launches++;
+  }
+  CKR(exclusive_sum(c, ar, cnt, moff, n + 1));
   long long total = 0;
-  CKR(mail_fetch(c, &h_err, err, 8));
+  CKR(mail_fetch(c, verdict, err, 8));
   CKR(mail_fetch(c, &total, moff + n, 8));
   CKR(mail_wait(c));
-  if (h_err != ~0ULL) return json_error(h_err, lines);
-  if (total >= 0x7fffffffLL) return set_error(CCO_E_UNSUPPORTED, "%lld members in the body, at most 2^31 - 2", total);
+  *total_out = total;
+  if (*verdict != ~0ULL || total >= limit) return CCO_OK;
   JMember *mem;
   CKR(ar.alloc(&mem, std::max<long long>(total, 1)));
   if (total > 0) {
@@ -3138,7 +3139,40 @@ static int json_members(cco_ctx *c, Arena &ar, long long n, const long long *sb,
   ar.release(cnt);
   *moff_out = moff;
   *mem_out = mem;
-  *total_out = total;
+  return CCO_OK;
+}
+// the lines of the len bytes of w (bytes [len, round_up(len, 8) + 16) are zero): every '\n' ends one; open_tail: a last
+// line without it ends at len.  -> *L lines and, when there are any, their spans [sb, se)
+static int split_lines(cco_ctx *c, Arena &ar, const uint64_t *w, long long len, bool open_tail, long long *L, long long **sb,
+                       long long **se) {
+  cudaStream_t s = c->stream;
+  const long long NW = (len + 7) / 8, n_chunks = (NW + kNlChunkWords - 1) / kNlChunkWords;
+  long long *cc, *coff, *nl;
+  CKR(ar.alloc(&cc, n_chunks + 1));
+  CKR(ar.alloc(&coff, n_chunks + 1));
+  CK(cudaMemsetAsync(cc + n_chunks, 0, 8, s));
+  if (NW > 0) {
+    k_nl_count<<<grid_for(n_chunks * 32, 256, c->sm_count), 256, 0, s>>>(NW, w, cc);
+    c->launches++;
+  }
+  CKR(exclusive_sum(c, ar, cc, coff, n_chunks + 1));
+  *L = 0;
+  CKR(mail_fetch(c, L, coff + n_chunks, 8));
+  CKR(mail_wait(c));
+  CKR(ar.alloc(&nl, *L + 1));
+  if (*L > 0) {
+    k_nl_write<<<grid_for(n_chunks * 32, 256, c->sm_count), 256, 0, s>>>(NW, w, coff, nl);
+    c->launches++;
+  }
+  if (open_tail) {
+    CK(cudaMemcpyAsync(nl + *L, &len, 8, cudaMemcpyHostToDevice, s));
+    ++*L;
+  }
+  if (*L == 0) return CCO_OK;
+  CKR(ar.alloc(sb, *L));
+  CKR(ar.alloc(se, *L));
+  k_line_spans<<<grid_for(*L, 256, c->sm_count), 256, 0, s>>>(*L, nl, *sb, *se);
+  c->launches++;
   return CCO_OK;
 }
 // the strings [m.nb, m.ne) of n members decoded into a string column (offsets from 0, 8-byte words, 16 bytes of padding)
@@ -3151,7 +3185,7 @@ static int json_decode(cco_ctx *c, Arena &ar, long long n, const JMember *m, con
   CK(cudaMemsetAsync(len + n, 0, 8, s));
   const int grid = grid_for(n, 256, c->sm_count);
   if (n > 0) k_json_unescape<false><<<grid, 256, 0, s>>>(n, m, body, len, nullptr, nullptr);
-  CKR(exclusive_sum_i64(c, ar, len, col->off, n + 1));
+  CKR(exclusive_sum(c, ar, len, col->off, n + 1));
   long long total = 0;
   CKR(mail_fetch(c, &total, col->off + n, 8));
   CKR(mail_wait(c));
@@ -3166,21 +3200,15 @@ static int json_decode(cco_ctx *c, Arena &ar, long long n, const JMember *m, con
 }
 
 static int rerank_model(cco_ctx_t *ctx, const char *body, int64_t body_len, const cco_item_properties_t *props, int32_t n_rank,
-                        const cco_ranking_t *rk, char **out_bytes, int64_t *out_len, const LogStreams *ls = nullptr,
-                        const DevProps *dp = nullptr) {
+                        const cco_ranking_t *rk, char **out_bytes, int64_t *out_len, Streams st = {}, const DevProps *dp = nullptr) {
   if (!ctx || !out_bytes || !out_len || body_len < 0 || (body_len > 0 && !body)) return set_error(CCO_E_INVALID_ARG, "null argument or negative length");
   if (!ctx->members.empty()) return set_error(CCO_E_UNSUPPORTED, "per-GPU contexts only");
   if (body_len > 0 && body[body_len - 1] != '\n') return set_error(CCO_E_INVALID_ARG, "the body does not end in a newline");
   const cco_dictionary_t no_rows = {0, nullptr, nullptr};
-  CKR(model_check_host(&no_rows, props, n_rank, rk, ls, dp != nullptr));
+  CKR(model_check_host(&no_rows, props, n_rank, rk, &st, dp != nullptr));
   long long fresh = props ? props->n : 0;   // property triples + ranking events, checked < 2^31 by model_check_host
-  for (int k = 0; k < n_rank; ++k) {
-    if (ls) {
-      for (const LogStream &st : (*ls)[k]) fresh += st.items.n;
-      continue;
-    }
-    for (int q = 0; q < rk[k].n_streams; ++q) fresh += rk[k].streams[q].n_events;
-  }
+  for (const std::vector<Stream> &r : st)
+    for (const Stream &q : r) fresh += q.items.n;
   cco_ctx *c = ctx;
   CK(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
@@ -3196,24 +3224,9 @@ static int rerank_model(cco_ctx_t *ctx, const char *body, int64_t body_len, cons
   if (body_len > 0) CK(cudaMemcpyAsync(w, body, (size_t)body_len, cudaMemcpyHostToDevice, s));
   const unsigned char *bb = (const unsigned char *)w;
   // 2. line bounds
-  long long L = 0;
-  long long *nl = nullptr;
-  if (NW > 0) {
-    const long long n_chunks = (NW + kNlChunkWords - 1) / kNlChunkWords;
-    long long *cc, *coff;
-    CKR(ar.alloc(&cc, n_chunks + 1));
-    CKR(ar.alloc(&coff, n_chunks + 1));
-    CK(cudaMemsetAsync(cc + n_chunks, 0, 8, s));
-    k_nl_count<<<grid_for(n_chunks * 32, 256, c->sm_count), 256, 0, s>>>(NW, w, cc);
-    c->launches++;
-    CKR(exclusive_sum_i64(c, ar, cc, coff, n_chunks + 1));
-    CKR(mail_fetch(c, &L, coff + n_chunks, 8));
-    CKR(mail_wait(c));
-    if (L & 1) return set_error(CCO_E_INVALID_ARG, "the body has %lld lines: lines come in (action, source) pairs", L);
-    CKR(ar.alloc(&nl, L));
-    k_nl_write<<<grid_for(n_chunks * 32, 256, c->sm_count), 256, 0, s>>>(NW, w, coff, nl);
-    c->launches++;
-  }
+  long long L = 0, *sb = nullptr, *se = nullptr;
+  CKR(split_lines(c, ar, w, body_len, false, &L, &sb, &se));
+  if (L & 1) return set_error(CCO_E_INVALID_ARG, "the body has %lld lines: lines come in (action, source) pairs", L);
   const long long D = L / 2;
   if (D + fresh >= 0x7fffffffLL)
     return set_error(CCO_E_UNSUPPORTED, "documents + property triples + ranking events must stay < 2^31 per call");
@@ -3226,19 +3239,16 @@ static int rerank_model(cco_ctx_t *ctx, const char *body, int64_t body_len, cons
   long long ids_bytes = 0, M1 = 0;
   if (D > 0) {
     // 3. members of every line; the verdict on the whole body comes before anything reads through the spans
-    long long *sb, *se;
-    CKR(ar.alloc(&sb, L));
-    CKR(ar.alloc(&se, L));
-    k_line_spans<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, nl, sb, se);
-    c->launches++;
     long long *line_moff;
     JMember *mem;
-    CKR(json_members(c, ar, L, sb, se, bb, true, &line_moff, &mem, &M1));
+    unsigned long long *err, h_err = 0;
+    CKR(json_members(c, ar, L, sb, se, bb, 0x7fffffffLL, &h_err, &line_moff, &mem, &M1));
+    if (h_err != ~0ULL) return json_error(h_err, true);
+    if (M1 >= 0x7fffffffLL) return set_error(CCO_E_UNSUPPORTED, "%lld members in the body, at most 2^31 - 2", M1);
     // 4. member names decoded; each action is {"index":{...}} and its "_id" is a string
     long long name_bytes = 0;
     CKR(json_decode(c, ar, M1, mem, bb, &names, &name_bytes));
     long long *ib, *ie;
-    unsigned long long *err, h_err = 0;
     CKR(ar.alloc(&ib, D));
     CKR(ar.alloc(&ie, D));
     CKR(ar.alloc(&err, 1));
@@ -3250,7 +3260,9 @@ static int rerank_model(cco_ctx_t *ctx, const char *body, int64_t body_len, cons
     if (h_err != ~0ULL) return json_error(h_err, false);
     long long *imoff, M2 = 0, iname_bytes = 0;
     JMember *imem, *id_span;
-    CKR(json_members(c, ar, D, ib, ie, bb, false, &imoff, &imem, &M2));
+    CKR(json_members(c, ar, D, ib, ie, bb, 0x7fffffffLL, &h_err, &imoff, &imem, &M2));
+    if (h_err != ~0ULL) return json_error(h_err, false);
+    if (M2 >= 0x7fffffffLL) return set_error(CCO_E_UNSUPPORTED, "%lld members in the body, at most 2^31 - 2", M2);
     DevStrCol inames;
     CKR(json_decode(c, ar, M2, imem, bb, &inames, &iname_bytes));
     CKR(ar.alloc(&id_span, D));
@@ -3274,7 +3286,7 @@ static int rerank_model(cco_ctx_t *ctx, const char *body, int64_t body_len, cons
   rows.bytes = (const char *)ids.w;
   rows.device = true;
   rows.nbytes = ids_bytes;
-  CKR(model_fields(c, ar, &fa, rows, props, n_rank, rk, true, true, ls, dp));
+  CKR(model_fields(c, ar, &fa, rows, props, n_rank, rk, st, true, true, dp));
   // 6. member names -> the distinct names of the fields, the rankings and "id"
   if (D > 0) {
     std::vector<std::string> ent;
@@ -3346,7 +3358,7 @@ static int rerank_model(cco_ctx_t *ctx, const char *body, int64_t body_len, cons
     k_doc_len<<<grid_for(X, 256, c->sm_count), 256, 0, s>>>(fx, (int32_t)X, doc_len + D);
     c->launches++;
   }
-  CKR(exclusive_sum_i64(c, ar, doc_len, doc_off, n_docs + 1));
+  CKR(exclusive_sum(c, ar, doc_len, doc_off, n_docs + 1));
   long long total = 0;
   CKR(mail_fetch(c, &total, doc_off + n_docs, 8));
   CKR(mail_wait(c));
@@ -3502,32 +3514,56 @@ static void log_drop(cco_event_log *lg, void *p) {
       return;
     }
 }
-// the lines carrying flag bit `want` in a stable order: by event name (code != nullptr), else by line -> idx[0 .. count)
+// a buffer kept by the log grown to cap (+ pad) entries, its first keep entries copied; the old one is freed
+extern "C++" {
+template <typename T>
+static int log_grow(cco_event_log *lg, Arena &ar, T **buf, long long cap, long long keep, long long pad) {
+  T *p;
+  CKR(ar.alloc(&p, cap + pad));
+  CKR(log_keep(ar, lg, p));
+  if (keep > 0) CK(cudaMemcpyAsync(p, *buf, sizeof(T) * (size_t)keep, cudaMemcpyDeviceToDevice, lg->ctx->stream));
+  log_drop(lg, *buf);
+  *buf = p;
+  return CCO_OK;
+}
+}  // extern "C++"
+// the entries i < n with keep[i] != 0, in order -> idx[0 .. count); the count stays on the device in (*pos)[n].  keep
+// has n + 1 entries.
+static int select_flagged(cco_ctx *c, Arena &ar, long long n, uint32_t *keep, uint32_t **pos, uint32_t **idx) {
+  CKR(ar.alloc(pos, n + 1));
+  CKR(ar.alloc(idx, n));
+  CK(cudaMemsetAsync(keep + n, 0, 4, c->stream));
+  CKR(exclusive_sum(c, ar, (const uint32_t *)keep, *pos, n + 1));
+  k_win_scatter<<<grid_for(n, 256, c->sm_count), 256, 0, c->stream>>>(n, keep, *pos, *idx);
+  c->launches++;
+  return CCO_OK;
+}
+// the lines carrying flag bit `want` by event name, file order inside a name -> idx[0 .. count)
 static int event_partition(cco_ctx *c, Arena &ar, long long L, const uint8_t *flag, uint8_t want, const int32_t *code, uint32_t n_names,
                            uint32_t **idx) {
+  uint32_t *key;
+  CKR(ar.alloc(&key, L));
+  CKR(ar.alloc(idx, L));
+  k_event_keys<<<grid_for(L, 256, c->sm_count), 256, 0, c->stream>>>(L, flag, want, code, n_names, key, *idx);
+  c->launches++;
+  CKR(sort_pairs(c, ar, L, &key, idx, bits_for((long long)n_names + 1)));
+  ar.release(key);
+  return CCO_OK;
+}
+// boff[g] = off[at[g]]: the byte offset of each name's first entry in a column, on the host
+static int name_boff(cco_ctx *c, Arena &ar, const long long *off, const std::vector<long long> &at, std::vector<long long> *boff) {
   cudaStream_t s = c->stream;
-  uint32_t *k0, *k1, *v0, *v1;
-  CKR(ar.alloc(&k0, L));
-  CKR(ar.alloc(&k1, L));
-  CKR(ar.alloc(&v0, L));
-  CKR(ar.alloc(&v1, L));
-  const uint32_t past = code ? n_names : 1;
-  k_event_keys<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, flag, want, code, past, k0, v0);
+  boff->assign(at.size(), 0);
+  std::vector<uint32_t> at32(at.begin(), at.end());
+  uint32_t *d_at;
+  long long *d_b;
+  CKR(ar.alloc(&d_at, at.size()));
+  CKR(ar.alloc(&d_b, at.size()));
+  CK(cudaMemcpyAsync(d_at, at32.data(), sizeof(uint32_t) * at.size(), cudaMemcpyHostToDevice, s));
+  k_gather_i64<<<grid_for((long long)at.size(), 256, c->sm_count), 256, 0, s>>>((long long)at.size(), d_at, off, d_b);
   c->launches++;
-  int bits = 1;
-  while ((1u << bits) <= past) ++bits;
-  cub::DoubleBuffer<uint32_t> kb(k0, k1), vb(v0, v1);
-  size_t tbytes = 0;
-  CK(cub::DeviceRadixSort::SortPairs(nullptr, tbytes, kb, vb, L, 0, bits, s));
-  void *tmp;
-  CKR(ar.alloc((char **)&tmp, tbytes));
-  CK(cub::DeviceRadixSort::SortPairs(tmp, tbytes, kb, vb, L, 0, bits, s));
-  c->launches++;
-  ar.release(tmp);
-  *idx = vb.Current();
-  ar.release(k0);
-  ar.release(k1);
-  ar.release(vb.Alternate());
+  CK(cudaMemcpyAsync(boff->data(), d_b, sizeof(long long) * at.size(), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));   // at32 is a local
   return CCO_OK;
 }
 // member k's string of the listed lines decoded into a column kept by the log; boff at the names' first entries
@@ -3549,50 +3585,9 @@ static int event_column(cco_ctx *c, Arena &ar, cco_event_log *lg, long long n, c
   CKR(log_keep(ar, lg, d.w));
   col->off = d.off;
   col->w = d.w;
-  col->boff.assign(at.size(), 0);
-  std::vector<uint32_t> at32(at.begin(), at.end());
-  uint32_t *d_at;
-  long long *d_b;
-  CKR(ar.alloc(&d_at, at.size()));
-  CKR(ar.alloc(&d_b, at.size()));
-  CK(cudaMemcpyAsync(d_at, at32.data(), sizeof(uint32_t) * at.size(), cudaMemcpyHostToDevice, s));
-  k_gather_i64<<<grid_for((long long)at.size(), 256, c->sm_count), 256, 0, s>>>((long long)at.size(), d_at, d.off, d_b);
-  c->launches++;
-  CK(cudaMemcpyAsync(col->boff.data(), d_b, sizeof(long long) * at.size(), cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));   // at32 is a local
-  return CCO_OK;
+  return name_boff(c, ar, d.off, at, &col->boff);
 }
 
-// sort (key, value) pairs of n entries by the low `bits` bits of the key, stably; the sorted arrays replace *k / *v
-extern "C++" {
-template <typename K>
-int sort_pairs(cco_ctx *c, Arena &ar, long long n, K **k, uint32_t **v, int bits) {
-  cudaStream_t s = c->stream;
-  K *k1;
-  uint32_t *v1;
-  CKR(ar.alloc(&k1, std::max<long long>(n, 1)));
-  CKR(ar.alloc(&v1, std::max<long long>(n, 1)));
-  cub::DoubleBuffer<K> kb(*k, k1);
-  cub::DoubleBuffer<uint32_t> vb(*v, v1);
-  size_t tbytes = 0;
-  CK(cub::DeviceRadixSort::SortPairs(nullptr, tbytes, kb, vb, n, 0, bits, s));
-  void *tmp;
-  CKR(ar.alloc((char **)&tmp, tbytes));
-  CK(cub::DeviceRadixSort::SortPairs(tmp, tbytes, kb, vb, n, 0, bits, s));
-  c->launches++;
-  ar.release(tmp);
-  ar.release(kb.Alternate());
-  ar.release(vb.Alternate());
-  *k = kb.Current();
-  *v = vb.Current();
-  return CCO_OK;
-}
-}  // extern "C++"
-static int bits_for(long long n) {
-  int b = 1;
-  while ((1LL << b) < n) ++b;
-  return b;
-}
 // PEventStore.aggregateProperties over the property events ($set / $unset / $delete of items) of a read log, in
 // (eventTime, line) order: a $set merges its members (the later value of a field wins), a $unset removes the fields it
 // names, a $delete drops what the item had.  Result, kept by the log: (item, field, value text) triples in the order of
@@ -3605,8 +3600,13 @@ static int event_properties(cco_ctx *c, Arena &ar, cco_event_log *lg, long long 
                             const long long *sb, const int2 *span, const unsigned char *bb, const long long *gline) {
   cudaStream_t s = c->stream;
   const long long NP = lg->n_prop;
-  uint32_t *pl;   // property event -> line, line order
-  CKR(event_partition(c, ar, L, flag, kEvProperty, nullptr, 0, &pl));
+  uint32_t *keep, *pos, *pl;   // property event -> line, line order
+  CKR(ar.alloc(&keep, L + 1));
+  k_win_flag_keep<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, flag, kEvProperty, keep);
+  c->launches++;
+  CKR(select_flagged(c, ar, L, keep, &pos, &pl));
+  ar.release(keep);
+  ar.release(pos);
   // items, grouped exactly in order of first appearance
   EvCol pcol;
   CKR(event_column(c, ar, lg, NP, pl, kEvEntityId, sb, span, bb, std::vector<long long>{0, NP}, &pcol));
@@ -3654,26 +3654,22 @@ static int event_properties(cco_ctx *c, Arena &ar, cco_event_log *lg, long long 
   lg->n_prop_items = (long long)h_cnt[1];
   // members of the properties objects of $set / $unset events; the verdict names the line
   uint32_t *qi;
-  CKR(event_partition(c, ar, NP, pk, kEvPropObj, nullptr, 0, &qi));
-  long long *qb, *qe, *mcnt, *moff;
-  unsigned long long *err, h_err = 0;
+  CKR(ar.alloc(&keep, NP + 1));
+  k_win_flag_keep<<<grid_for(NP, 256, c->sm_count), 256, 0, s>>>(NP, pk, kEvPropObj, keep);
+  c->launches++;
+  CKR(select_flagged(c, ar, NP, keep, &pos, &qi));
+  ar.release(keep);
+  ar.release(pos);
+  long long *qb, *qe, *moff, M = 0;
+  unsigned long long h_err = 0;
   CKR(ar.alloc(&qb, std::max<long long>(Q, 1)));
   CKR(ar.alloc(&qe, std::max<long long>(Q, 1)));
-  CKR(ar.alloc(&mcnt, Q + 1));
-  CKR(ar.alloc(&moff, Q + 1));
-  CKR(ar.alloc(&err, 1));
-  CK(cudaMemsetAsync(mcnt + Q, 0, 8, s));
-  CK(cudaMemsetAsync(err, 0xff, 8, s));
-  long long M = 0;
   if (Q > 0) {
     k_prop_spans<<<grid_for(Q, 256, c->sm_count), 256, 0, s>>>(Q, qi, pl, sb, span, qb, qe);
-    k_json_members<<<grid_for(Q * 32, 256, c->sm_count), 256, 0, s>>>(Q, qb, qe, bb, MemberSink<false>{mcnt, nullptr, nullptr}, err);
-    c->launches += 2;
+    c->launches++;
   }
-  CKR(exclusive_sum_i64(c, ar, mcnt, moff, Q + 1));
-  CKR(mail_fetch(c, &h_err, err, 8));
-  CKR(mail_fetch(c, &M, moff + Q, 8));
-  CKR(mail_wait(c));
+  JMember *mem;
+  CKR(json_members(c, ar, Q, qb, qe, bb, 0x7fffffffLL - G, &h_err, &moff, &mem, &M));
   if (h_err != ~0ULL) {
     uint32_t q = 0, line = 0;
     CK(cudaMemcpy(&q, qi + (h_err >> 8), 4, cudaMemcpyDeviceToHost));
@@ -3681,16 +3677,13 @@ static int event_properties(cco_ctx *c, Arena &ar, cco_event_log *lg, long long 
     return event_error(((unsigned long long)gline[line] << 8) | (h_err & 0xff));
   }
   if (M + G >= 0x7fffffffLL) return set_error(CCO_E_UNSUPPORTED, "%lld property members, at most 2^31 - 2 with the items", M);
-  JMember *mem;
   uint32_t *mev;
   int32_t *mf;
-  CKR(ar.alloc(&mem, std::max<long long>(M, 1)));
   CKR(ar.alloc(&mev, std::max<long long>(M, 1)));
   CKR(ar.alloc(&mf, std::max<long long>(M, 1)));
   if (M > 0) {
-    k_json_members<<<grid_for(Q * 32, 256, c->sm_count), 256, 0, s>>>(Q, qb, qe, bb, MemberSink<true>{nullptr, moff, mem}, err);
     k_prop_member_event<<<grid_for(Q, 256, c->sm_count), 256, 0, s>>>(Q, moff, qi, mev);
-    c->launches += 2;
+    c->launches++;
   }
   // field names decoded and grouped exactly; the few distinct ones go to the host once
   DevStrCol nm;
@@ -3723,7 +3716,7 @@ static int event_properties(cco_ctx *c, Arena &ar, cco_event_log *lg, long long 
   k_prop_keys2<<<grid_for(N, 256, c->sm_count), 256, 0, s>>>(M, G, v1, mev, pg, mf, k2, v2);
   c->launches++;
   CKR(sort_pairs(c, ar, N, &k2, &v2, 32 + bits_for(G)));
-  uint32_t *keep, *pos, *has;
+  uint32_t *has;
   CKR(ar.alloc(&keep, N + 1));
   CKR(ar.alloc(&pos, N + 1));
   CKR(ar.alloc(&has, G));
@@ -3732,7 +3725,7 @@ static int event_properties(cco_ctx *c, Arena &ar, cco_event_log *lg, long long 
   k_prop_win<<<grid_for(N, 256, c->sm_count), 256, 0, s>>>(M, G, k2, v2, mev, pk, ord, last_del, keep, has);
   k_prop_presence<<<grid_for(N, 256, c->sm_count), 256, 0, s>>>(M, G, k2, last_del, last_set, has, keep);
   c->launches += 2;
-  CKR(exclusive_sum_u32(c, ar, keep, pos, N + 1));
+  CKR(exclusive_sum(c, ar, keep, pos, N + 1));
   uint32_t T = 0;
   CKR(mail_fetch(c, &T, pos + N, 4));
   CKR(mail_wait(c));
@@ -3784,9 +3777,9 @@ static int event_properties(cco_ctx *c, Arena &ar, cco_event_log *lg, long long 
   CKR(ar.alloc(&ioff, (long long)T + 1));
   CK(cudaMemsetAsync(len + T, 0, 8, s));
   k_prop_value_len<<<grid_for(T, 256, c->sm_count), 256, 0, s>>>(T, vb, ve, len);
-  CKR(exclusive_sum_i64(c, ar, len, voff, (long long)T + 1));
+  CKR(exclusive_sum(c, ar, len, voff, (long long)T + 1));
   k_str_dict_len<<<grid_for(T, 256, c->sm_count), 256, 0, s>>>(T, titem, pcol.off, len);
-  CKR(exclusive_sum_i64(c, ar, len, ioff, (long long)T + 1));
+  CKR(exclusive_sum(c, ar, len, ioff, (long long)T + 1));
   c->launches += 3;
   CKR(mail_fetch(c, &vtotal, voff + T, 8));
   CKR(mail_fetch(c, &itotal, ioff + T, 8));
@@ -3823,38 +3816,10 @@ static int event_lines(cco_ctx *c, Arena &ar, const uint64_t *w, long long len, 
   cudaStream_t s = c->stream;
   const unsigned char *bb = (const unsigned char *)w;
   const unsigned long long base = (unsigned long long)line_base << 8;
-  const long long NW = (len + 7) / 8;
-  long long L = 0;
-  long long *nl;
-  long long n_chunks = (NW + kNlChunkWords - 1) / kNlChunkWords;
-  long long *cc, *coff;
-  CKR(ar.alloc(&cc, n_chunks + 1));
-  CKR(ar.alloc(&coff, n_chunks + 1));
-  CK(cudaMemsetAsync(cc + n_chunks, 0, 8, s));
-  if (NW > 0) {
-    k_nl_count<<<grid_for(n_chunks * 32, 256, c->sm_count), 256, 0, s>>>(NW, w, cc);
-    c->launches++;
-  }
-  CKR(exclusive_sum_i64(c, ar, cc, coff, n_chunks + 1));
-  CKR(mail_fetch(c, &L, coff + n_chunks, 8));
-  CKR(mail_wait(c));
-  if (L + (open_tail ? 1 : 0) > 0x7fffffffLL)
-    return set_error(CCO_E_UNSUPPORTED, "%lld lines in one parsed chunk, at most 2^31 - 1", L + (open_tail ? 1 : 0));
-  CKR(ar.alloc(&nl, L + 1));
-  if (L > 0) {
-    k_nl_write<<<grid_for(n_chunks * 32, 256, c->sm_count), 256, 0, s>>>(NW, w, coff, nl);
-    c->launches++;
-  }
-  if (open_tail) {
-    CK(cudaMemcpyAsync(nl + L, &len, 8, cudaMemcpyHostToDevice, s));
-    ++L;
-  }
-  ev->L = L;
+  CKR(split_lines(c, ar, w, len, open_tail, &ev->L, &ev->sb, &ev->se));
+  const long long L = ev->L;
+  if (L > 0x7fffffffLL) return set_error(CCO_E_UNSUPPORTED, "%lld lines in one parsed chunk, at most 2^31 - 1", L);
   if (L == 0) return CCO_OK;
-  CKR(ar.alloc(&ev->sb, L));
-  CKR(ar.alloc(&ev->se, L));
-  k_line_spans<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, nl, ev->sb, ev->se);
-  c->launches++;
   unsigned long long *err, h_err = 0;
   CKR(ar.alloc(&ev->span, L * kEvSlots));
   CKR(ar.alloc(&err, 1));
@@ -3909,18 +3874,16 @@ static int win_records(cco_event_log *lg, Arena &ar, const EvLines &ev, const in
   const unsigned char *bb = lg->stage;
   uint32_t *keep, *pos, *ridx;
   CKR(ar.alloc(&keep, L + 1));
-  CKR(ar.alloc(&pos, L + 1));
-  CK(cudaMemsetAsync(keep + L, 0, 4, s));
   k_win_keep_lines<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, ev.flag, keep);
   c->launches++;
-  CKR(exclusive_sum_u32(c, ar, keep, pos, L + 1));
+  CKR(select_flagged(c, ar, L, keep, &pos, &ridx));
   uint32_t R32 = 0;
   CKR(mail_fetch(c, &R32, pos + L, 4));
   CKR(mail_wait(c));
+  ar.release(keep);
+  ar.release(pos);
   const long long R = R32;
   if (R == 0) return CCO_OK;
-  CKR(ar.alloc(&ridx, R));
-  k_win_scatter<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, keep, pos, ridx);
   // the properties' members: count pass with each span's verdict, then the members of the well-formed spans
   long long *pb, *pe, *mcnt, *moff;
   int *codes;
@@ -3934,8 +3897,8 @@ static int win_records(cco_event_log *lg, Arena &ar, const EvLines &ev, const in
   CK(cudaMemsetAsync(mcnt + R, 0, 8, s));
   k_win_prop_spans<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, ridx, ev.sb, ev.span, pb, pe);
   k_json_members<<<grid_for(R * 32, 256, c->sm_count), 256, 0, s>>>(R, pb, pe, bb, WinMemberSink<false>{mcnt, codes, nullptr, nullptr}, err);
-  c->launches += 3;
-  CKR(exclusive_sum_i64(c, ar, mcnt, moff, R + 1));
+  c->launches += 2;
+  CKR(exclusive_sum(c, ar, mcnt, moff, R + 1));
   long long M = 0;
   CKR(mail_fetch(c, &M, moff + R, 8));
   CKR(mail_wait(c));
@@ -3988,14 +3951,8 @@ static int win_records(cco_event_log *lg, Arena &ar, const EvLines &ev, const in
     c->launches++;
   }
   if (lg->n_rec + R > lg->rec_cap) {   // grow geometrically
-    const long long cap = std::max(2 * lg->rec_cap, lg->n_rec + R);
-    WinRec *p;
-    CKR(ar.alloc(&p, cap));
-    CKR(log_keep(ar, lg, p));
-    if (lg->n_rec > 0) CK(cudaMemcpyAsync(p, lg->rec, sizeof(WinRec) * (size_t)lg->n_rec, cudaMemcpyDeviceToDevice, s));
-    log_drop(lg, lg->rec);
-    lg->rec = p;
-    lg->rec_cap = cap;
+    lg->rec_cap = std::max(2 * lg->rec_cap, lg->n_rec + R);
+    CKR(log_grow(lg, ar, &lg->rec, lg->rec_cap, lg->n_rec, 0));
   }
   k_win_ident<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, ridx, base, ev.sb, ev.span, ev.xspan, bb, hd, hr, codes, acc, ev.tm, ev.flag,
                                                           code, lg->rec + lg->n_rec);
@@ -4114,28 +4071,26 @@ static int event_chunk(cco_event_log *lg, long long len, bool open_tail) {
   ar.release(idx);
   // 8. the property-event lines, in line order, for the aggregation at finish (see event_log_finish)
   if (NP > 0) {
-    CKR(event_partition(c, ar, L, ev.flag, kEvProperty, nullptr, 0, &idx));
+    uint32_t *keep, *pos;
+    CKR(ar.alloc(&keep, L + 1));
+    k_win_flag_keep<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, ev.flag, kEvProperty, keep);
+    c->launches++;
+    CKR(select_flagged(c, ar, L, keep, &pos, &idx));
     long long *len8, *off;
     CKR(ar.alloc(&len8, NP + 1));
     CKR(ar.alloc(&off, NP + 1));
     CK(cudaMemsetAsync(len8 + NP, 0, 8, s));
     k_line_len<<<grid_for(NP, 256, c->sm_count), 256, 0, s>>>(NP, idx, ev.sb, ev.se, len8);
     c->launches++;
-    CKR(exclusive_sum_i64(c, ar, len8, off, NP + 1));
+    CKR(exclusive_sum(c, ar, len8, off, NP + 1));
     long long total = 0;
     std::vector<uint32_t> h_idx((size_t)NP);
     CK(cudaMemcpyAsync(&total, off + NP, 8, cudaMemcpyDeviceToHost, s));
     CK(cudaMemcpyAsync(h_idx.data(), idx, sizeof(uint32_t) * (size_t)NP, cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
     if (lg->pb_len + total > lg->pb_cap) {   // grow geometrically; 24 bytes of padding for event_pad
-      const long long cap = std::max(2 * lg->pb_cap, lg->pb_len + total);
-      unsigned char *p;
-      CKR(ar.alloc(&p, cap + 24));
-      CKR(log_keep(ar, lg, p));
-      if (lg->pb_len > 0) CK(cudaMemcpyAsync(p, lg->pb, (size_t)lg->pb_len, cudaMemcpyDeviceToDevice, s));
-      log_drop(lg, lg->pb);
-      lg->pb = p;
-      lg->pb_cap = cap;
+      lg->pb_cap = std::max(2 * lg->pb_cap, lg->pb_len + total);
+      CKR(log_grow(lg, ar, &lg->pb, lg->pb_cap, lg->pb_len, 24));
     }
     k_line_gather<<<grid_for(NP * 32, 256, c->sm_count), 256, 0, s>>>(NP, idx, ev.sb, ev.se, bb, off, lg->pb + lg->pb_len);
     c->launches++;
@@ -4275,7 +4230,7 @@ static int win_gather_column(cco_event_log *lg, Arena &ar, long long K, const ui
     k_str_dict_len<<<grid_for(K, 256, c->sm_count), 256, 0, s>>>(K, idx, col->off, len);
     c->launches++;
   }
-  CKR(exclusive_sum_i64(c, ar, len, off, K + 1));
+  CKR(exclusive_sum(c, ar, len, off, K + 1));
   CK(cudaMemcpyAsync(&total, off + K, 8, cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
   uint64_t *w;
@@ -4284,17 +4239,7 @@ static int win_gather_column(cco_event_log *lg, Arena &ar, long long K, const ui
     k_str_dict_gather<<<grid_for(K, 256, c->sm_count), 256, 0, s>>>(K, idx, col->off, 0, (const unsigned char *)col->w, off, (unsigned char *)w);
     c->launches++;
   }
-  std::vector<uint32_t> at32(at.begin(), at.end());
-  uint32_t *d_at;
-  long long *d_b;
-  CKR(ar.alloc(&d_at, at.size()));
-  CKR(ar.alloc(&d_b, at.size()));
-  CK(cudaMemcpyAsync(d_at, at32.data(), sizeof(uint32_t) * at.size(), cudaMemcpyHostToDevice, s));
-  k_gather_i64<<<grid_for((long long)at.size(), 256, c->sm_count), 256, 0, s>>>((long long)at.size(), d_at, off, d_b);
-  c->launches++;
-  col->boff.assign(at.size(), 0);
-  CK(cudaMemcpyAsync(col->boff.data(), d_b, sizeof(long long) * at.size(), cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));   // at32 is a local
+  CKR(name_boff(c, ar, off, at, &col->boff));
   CKR(log_keep(ar, lg, off));
   CKR(log_keep(ar, lg, w));
   log_drop(lg, col->off);
@@ -4313,19 +4258,15 @@ static int win_compact(cco_event_log *lg, const uint32_t *bitmap, const long lon
   if (n == 0) return CCO_OK;
   uint32_t *keep, *pos, *idx;
   CKR(ar.alloc(&keep, n + 1));
-  CKR(ar.alloc(&pos, n + 1));
-  CKR(ar.alloc(&idx, n));
-  CK(cudaMemsetAsync(keep + n, 0, 4, s));
   k_win_entry_keep<<<grid_for(n, 256, c->sm_count), 256, 0, s>>>(n, line, bitmap, keep);
   c->launches++;
-  CKR(exclusive_sum_u32(c, ar, keep, pos, n + 1));
-  k_win_scatter<<<grid_for(n, 256, c->sm_count), 256, 0, s>>>(n, keep, pos, idx);
+  CKR(select_flagged(c, ar, n, keep, &pos, &idx));
   long long *d_at, *d_nat;
   CKR(ar.alloc(&d_at, NA));
   CKR(ar.alloc(&d_nat, NA));
   CK(cudaMemcpyAsync(d_at, at.data(), sizeof(long long) * (size_t)NA, cudaMemcpyHostToDevice, s));
   k_win_at<<<grid_for(NA, 256, c->sm_count), 256, 0, s>>>(NA, d_at, pos, d_nat);
-  c->launches += 2;
+  c->launches++;
   std::vector<long long> nat((size_t)NA);
   CK(cudaMemcpyAsync(nat.data(), d_nat, sizeof(long long) * (size_t)NA, cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));   // at and nat are host vectors
@@ -4355,14 +4296,9 @@ static int win_drop_property_lines(cco_event_log *lg, Arena &ar, const EvLines &
   const long long L = ev.L;
   uint32_t *keep, *pos, *qi, Q = 0;
   CKR(ar.alloc(&keep, L + 1));
-  CKR(ar.alloc(&pos, L + 1));
-  CKR(ar.alloc(&qi, L));
-  CK(cudaMemsetAsync(keep + L, 0, 4, s));
   k_win_flag_keep<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, ev.flag, kEvPropObj, keep);
   c->launches++;
-  CKR(exclusive_sum_u32(c, ar, keep, pos, L + 1));
-  k_win_scatter<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, keep, pos, qi);
-  c->launches++;
+  CKR(select_flagged(c, ar, L, keep, &pos, &qi));
   CKR(mail_fetch(c, &Q, pos + L, 4));
   CKR(mail_wait(c));
   long long *gl;
@@ -4401,15 +4337,8 @@ static int event_flush(cco_event_log *lg) {
   Arena ar(s);
   if (lg->last_nl < 0) {
     if (lg->staged >= (1LL << 31)) return event_error(((unsigned long long)lg->n_lines << 8) | kJsonLongLine);
-    const long long cap = 2 * lg->cap;
-    unsigned char *p;
-    CKR(ar.alloc(&p, cap + 24));
-    CKR(log_keep(ar, lg, p));
-    CK(cudaMemcpyAsync(p, lg->stage, (size_t)lg->staged, cudaMemcpyDeviceToDevice, s));
-    log_drop(lg, lg->stage);
-    lg->stage = p;
-    lg->cap = cap;
-    return CCO_OK;
+    lg->cap *= 2;
+    return log_grow(lg, ar, &lg->stage, lg->cap, lg->staged, 24);
   }
   const long long P = lg->last_nl + 1, carry = lg->staged - P;
   unsigned char *tmp = nullptr;
@@ -4540,8 +4469,8 @@ static int event_log_finish(cco_event_log *lg) {
   return CCO_OK;
 }
 
-// the rankings of cco_format_model_log / cco_rerank_model_log as cco_ranking_t (no host streams) + the log's streams
-static int log_rankings(const cco_event_log *lg, int32_t n_rank, const cco_log_ranking_t *lr, std::vector<cco_ranking_t> *rk, LogStreams *ls) {
+// the rankings of cco_format_model_log / cco_rerank_model_log as cco_ranking_t without streams + the log's streams
+static int log_rankings(const cco_event_log *lg, int32_t n_rank, const cco_log_ranking_t *lr, std::vector<cco_ranking_t> *rk, Streams *ls) {
   if (n_rank < 0 || (n_rank > 0 && !lr)) return set_error(CCO_E_INVALID_ARG, "bad rankings");
   rk->assign((size_t)std::max(n_rank, 0), cco_ranking_t{});
   ls->assign((size_t)std::max(n_rank, 0), {});
@@ -4561,17 +4490,16 @@ static int log_rankings(const cco_event_log *lg, int32_t n_rank, const cco_log_r
     }
     for (int g : codes) {
       if (g < 0) continue;   // a name without events: an empty stream
-      LogStream st;
+      Stream st;
       st.items.n = lg->n_rank[g];
       st.items.off = (const int64_t *)(lg->ri.off + lg->rank_at[g]);
       st.items.bytes = (const char *)lg->ri.w + lg->ri.boff[g];
       st.items.device = true;
       st.items.base = lg->ri.boff[g];
       st.items.nbytes = lg->ri.boff[g + 1] - lg->ri.boff[g];
-      st.time = lg->rtime + lg->rank_at[g];
+      st.time = (const int64_t *)(lg->rtime + lg->rank_at[g]);
       (*ls)[k].push_back(st);
     }
-    (*rk)[k].n_streams = (int32_t)(*ls)[k].size();
   }
   return CCO_OK;
 }
@@ -4709,13 +4637,13 @@ int cco_format_model_log(cco_ctx_t *ctx, const cco_result_t *res, int32_t n_name
   if (!ctx->members.empty() || lg->ctx != ctx) return set_error(CCO_E_UNSUPPORTED, "format on the per-GPU context that read the log");
   CKR(log_state(lg, true));
   std::vector<cco_ranking_t> rk;
-  LogStreams ls;
+  Streams ls;
   CKR(log_rankings(lg, n_rankings, rankings, &rk, &ls));
   LogProps lp;
   log_props(lg, &lp);
   const bool any = lg->n_triples > 0;
   return format_model(ctx, res, n_names, names, row_ids, col_ids, any ? &lp.shell : nullptr, n_rankings, rk.data(), out_bytes, out_len,
-                      "cco:format_model_log", &ls, any ? &lp.dev : nullptr);
+                      "cco:format_model_log", std::move(ls), any ? &lp.dev : nullptr);
 }
 
 int cco_rerank_model_log(cco_ctx_t *ctx, const char *body, int64_t body_len, const cco_event_log_t *lg, int32_t n_rankings,
@@ -4724,12 +4652,13 @@ int cco_rerank_model_log(cco_ctx_t *ctx, const char *body, int64_t body_len, con
   if (!ctx->members.empty() || lg->ctx != ctx) return set_error(CCO_E_UNSUPPORTED, "rerank on the per-GPU context that read the log");
   CKR(log_state(lg, true));
   std::vector<cco_ranking_t> rk;
-  LogStreams ls;
+  Streams ls;
   CKR(log_rankings(lg, n_rankings, rankings, &rk, &ls));
   LogProps lp;
   log_props(lg, &lp);
   const bool any = lg->n_triples > 0;
-  return rerank_model(ctx, body, body_len, any ? &lp.shell : nullptr, n_rankings, rk.data(), out_bytes, out_len, &ls, any ? &lp.dev : nullptr);
+  return rerank_model(ctx, body, body_len, any ? &lp.shell : nullptr, n_rankings, rk.data(), out_bytes, out_len, std::move(ls),
+                      any ? &lp.dev : nullptr);
 }
 
 int cco_event_log_free(cco_event_log_t *lg) {
@@ -4892,7 +4821,7 @@ int cco_debug_cooccurrence(cco_ctx_t *c, const cco_csr_t *a, const cco_csr_t *b,
   CK(cudaMemsetAsync(d_max, 0, 8, s));
   CK(cudaMemcpyAsync(marg_pad, dm[0].marg, sizeof(int32_t) * (size_t)n_items_a, cudaMemcpyDeviceToDevice, s));
   CK(cudaMemsetAsync(marg_pad + n_items_a, 0, 4, s));
-  CKR(exclusive_sum_u32(c, ar, marg_pad, at_ptr, (long long)n_items_a + 1));
+  CKR(exclusive_sum(c, ar, marg_pad, at_ptr, (long long)n_items_a + 1));
   CK(cudaMemcpyAsync(cursor, at_ptr, sizeof(uint32_t) * ((size_t)n_items_a + 1), cudaMemcpyDeviceToDevice, s));
   k_transpose_scatter<<<grid_for(a->n_rows * kSG, 256, c->sm_count), 256, 0, s>>>(a->n_rows, dm[0].rp, dm[0].col, cursor, at_users);
   if (n_items_a > 0) k_max_i32<<<grid_for(n_items_a, 256, c->sm_count, 2), 256, 0, s>>>(n_items_a, dm[0].marg, d_max);

@@ -218,11 +218,11 @@ __global__ void k_event_strings(long long n, const uint32_t *__restrict__ idx, i
   }
 }
 
-// key[l] = the line's event name code (code == nullptr: 0) if it carries flag bit `want`, else `past` (sorted after them)
+// key[l] = the line's event name code if it carries flag bit `want`, else `past` (sorted after them)
 __global__ void k_event_keys(long long n_lines, const uint8_t *__restrict__ flag, uint8_t want, const int32_t *__restrict__ code,
                              uint32_t past, uint32_t *__restrict__ key, uint32_t *__restrict__ line) {
   for (long long l = blockIdx.x * (long long)blockDim.x + threadIdx.x; l < n_lines; l += (long long)gridDim.x * blockDim.x) {
-    key[l] = (flag[l] & want) ? (code ? (uint32_t)code[l] : 0u) : past;
+    key[l] = (flag[l] & want) ? (uint32_t)code[l] : past;
     line[l] = (uint32_t)l;
   }
 }
@@ -480,7 +480,8 @@ __global__ void k_cat_entries(long long n, long long last, const CatPiece *__res
 //   k_win_ident                      the line's identity hash -> a WinRec (hash, time, global line, name, selection)
 //   k_win_key_* / k_win_mark         at finish: records sorted by (hash, time desc, line desc), all but the first of each
 //                                    run dropped into a bitmap over the global lines, the drops counted per selection
-//   k_win_entry_keep / k_win_scatter the retained columns and the property lines compacted through the bitmap
+//   k_win_entry_keep / k_win_scatter the retained columns and the property lines compacted through the bitmap; with
+//                                    k_win_flag_keep also every selection of lines by a flag bit in line order
 enum : uint8_t { kEvDropped = 128 };   // an expired line: no selection, not ignored
 enum : int { kEvPrId = 0, kEvTags, kEvXSlots };
 constexpr int kWinStr = 6;             // decoded strings per line: event, entityType, entityId, targetEntityType, targetEntityId, prId
