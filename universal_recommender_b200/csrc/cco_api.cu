@@ -677,6 +677,8 @@ struct BinCfg {
   int cbuf;     // candidate buffer entries per group
   int caux, keep_max, final_max;
   bool dense;
+  bool bitmap;    // bitmap rows (use_bitmap): slots = repeat-table words, then bm_words of bitmap and top_k singles
+  int bm_words;
   size_t region;  // shared-memory bytes per group
   size_t smem;    // per CTA
   int ctas_per_sm;
@@ -693,6 +695,8 @@ static int launch_rows_t(cco_ctx *c, const RowArgs &a, BinCfg &cfg, cudaStream_t
   constexpr int CTA = GROUP == 32 ? 64 : GROUP;   // warp-owned rows: two independent warps per CTA (fine-grained smem packing)
   int occ = 1;
   void (*kern)(const RowArgs) = cfg.dense ? k_rows<GROUP, true> : k_rows<GROUP, false>;
+  if constexpr (GROUP == 512 || GROUP == 256)
+    if (cfg.bitmap) kern = k_rows<GROUP, false, true>;
   CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg.smem));
   CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, CTA, cfg.smem));
   // 4 waves of CTAs over the work-sorted row list: a CTA that draws cheap rows retires early and the hardware
@@ -730,10 +734,30 @@ static BinCfg make_cfg(cco_ctx *c, int group, int want_slots, int top_k, int n_c
   f.slots = std::min(want_slots, max_slots);
   f.cap = f.slots / 2;  // load factor <= 1/2: higher load factors lengthen the probe chains
   f.dense = n_cols_b <= f.slots;
+  f.bitmap = false;
+  f.bm_words = 0;
   f.region = (fixed + (size_t)f.slots * 4 + 15) & ~(size_t)15;
   f.smem = f.region * groups;
   f.ctas_per_sm = 1;
   return f;
+}
+
+// Bitmap rows (DESIGN.md 3.1): a hashed CTA-owned bin whose rows all take the key path with an exact cut counts each cell's
+// first product into a bitmap over the keys and hashes only the repeats.  Its table then holds at most max_w / 2 cells at
+// load factor <= 1/2, i.e. max_w words (rounded to the per-warp segments), next to ceil(n_cols_b / 32) bitmap words and
+// top_k singles.  The bin switches only when that fits in the shared memory of its current table: same CTAs per SM.
+// Only the 512- and 256-thread bins are candidates (their gain at C3 is in DESIGN.md 3.2): the 128-thread bin's table
+// is too small to hold a 100 K-column bitmap, and the 1024-thread bins were not tried.
+static bool use_bitmap(BinCfg &f, uint32_t max_w, int top_k, int n_cols_b) {
+  if (f.dense || (f.group != 512 && f.group != 256)) return false;
+  const long long seg = 32LL * (f.group / 32);
+  const long long rep = (std::max<long long>(max_w, 64) + seg - 1) / seg * seg;
+  const long long bm = ((long long)n_cols_b + 31) / 32;
+  if (rep + bm + top_k > f.slots) return false;
+  f.bitmap = true;
+  f.slots = (int)rep;
+  f.bm_words = (int)bm;
+  return true;
 }
 
 // ---- exactness of the level-1 cut and the dominance filter under fp64 rounding (DESIGN.md 3.1) ---------------------------
@@ -886,6 +910,12 @@ static int enqueue_indicator(cco_ctx *c, Arena &ar, const uint32_t *at_ptr, cons
     h_thr[b] = lim;
     if (b > 0) h_thr[b] = std::min(h_thr[b], h_thr[b - 1]);
   }
+  // bitmap rows: the k11 = 1 cells are cut by key, so every row must be keyed (2 rowA colB < N for the largest of both)
+  // and the cut exact
+  const bool bitmap_ok = !emit_all && cut_exact(n_users, max_marg_a, max_marg_b) &&
+                         2ull * (unsigned long long)std::max(max_marg_a, 0) * (unsigned long long)std::max(max_marg_b, 0) <
+                             (unsigned long long)n_users;
+  for (int b = 1; b < kBins && bitmap_ok; ++b) use_bitmap(cfgs[b], h_thr[b - 1], k_eff, n_cols_b);
   int32_t *d_bounds;
   CKR(ar.alloc(&d_bounds, kBins + 3));
   BinThresholds bt;
@@ -1002,6 +1032,7 @@ static int enqueue_indicator(cco_ctx *c, Arena &ar, const uint32_t *at_ptr, cons
       ab.keep_max = cfgs[b].keep_max;
       ab.final_max = cfgs[b].final_max;
       ab.group_smem_bytes = (int32_t)cfgs[b].region;
+      ab.bm_words = cfgs[b].bm_words;
       CK(cudaStreamWaitEvent(c->bin_stream[b], c->bin_ev[8], 0));
       CKR(launch_rows(c, ab, cfgs[b], c->bin_stream[b]));
       CK(cudaEventRecord(c->bin_ev[b], c->bin_stream[b]));

@@ -73,6 +73,7 @@ struct RowArgs {
   unsigned long long *stat_evaluated;  // cells whose fp64 LLR was actually evaluated (after the dominance filter)
   int *err_flag;     // set to 1 if a hash table overflowed (result invalid)
   int32_t emit_all;  // debug: write every non-zero cell (col,count), no LLR/top-k
+  int32_t bm_words;  // bitmap rows (k_rows<..., BITMAP>): words of the key bitmap, ceil(n_cols_b / 32); else 0
 };
 
 constexpr uint32_t kEmpty = 0xffffffffu;
@@ -678,9 +679,12 @@ __device__ __forceinline__ void accumulate(uint32_t *table, uint32_t tsize, uint
 // Count the products [p_lo, p_hi) of a window of up to 32 users held in registers: lane l holds user l's first product
 // index `off` (non-decreasing over the lanes, lane 0's <= p_lo; unused lanes hold 0xffffffff) and the start `s` of its
 // B' row.  Each lane finds the user of its product by a 5-step shuffle search, then gathers the column.
-template <int GROUP, bool DENSE>
-__device__ __forceinline__ void count_window(const RowArgs &a, uint32_t *table, uint32_t tsize, int cbits, uint32_t n_pass,
-                                             uint32_t pass, uint32_t off, uint32_t s, uint32_t p_lo, uint32_t p_hi, int lane) {
+// BITMAP: the first product of a cell sets its bit in `seen`; only the later products of a cell reach the hash table, which
+// so holds k11 - 1 for exactly the cells with k11 >= 2.
+template <int GROUP, bool DENSE, bool BITMAP>
+__device__ __forceinline__ void count_window(const RowArgs &a, uint32_t *table, uint32_t *seen, uint32_t tsize, int cbits,
+                                             uint32_t n_pass, uint32_t pass, uint32_t off, uint32_t s, uint32_t p_lo,
+                                             uint32_t p_hi, int lane) {
   for (uint32_t p0 = p_lo; p0 < p_hi; p0 += 64) {
     // two products per lane per trip (two independent gathers in flight)
     uint32_t bb[2];
@@ -699,9 +703,18 @@ __device__ __forceinline__ void count_window(const RowArgs &a, uint32_t *table, 
       act[h] = p < p_hi;
       bb[h] = act[h] ? (uint32_t)a.b_col[sj + (p - oj)] : 0u;
     }
+    if (BITMAP) {
+      uint32_t old[2];   // both atomics issue before either result is needed
 #pragma unroll
-    for (int h = 0; h < 2; ++h)
-      if (act[h]) accumulate<GROUP, DENSE>(table, tsize, bb[h], cbits, n_pass, pass, a.err_flag);
+      for (int h = 0; h < 2; ++h) old[h] = act[h] ? atomicOr(&seen[bb[h] >> 5], 1u << (bb[h] & 31u)) : 0u;
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        if (act[h] && ((old[h] >> (bb[h] & 31u)) & 1u)) accumulate<GROUP, false>(table, tsize, bb[h], cbits, 1u, 0u, a.err_flag);
+    } else {
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        if (act[h]) accumulate<GROUP, DENSE>(table, tsize, bb[h], cbits, n_pass, pass, a.err_flag);
+    }
   }
 }
 
@@ -714,8 +727,12 @@ struct RowsMinBlocks {
   static constexpr int value = GROUP == 512 ? 2 : GROUP == 256 ? 4 : GROUP == 128 ? 8 : GROUP == 32 ? 12 : 1;
 };
 
-template <int GROUP, bool DENSE>
+// BITMAP (CTA-owned hashed bins whose rows are all on the key path with an exact cut; DESIGN.md 3.1 "bitmap rows"): the
+// count sets one bit per cell in a bitmap over the keys and hashes only the repeated products; the level-1 key cut is the
+// top_k-th set bit in key order, and only the k11 = 1 cells up to it are ever listed.
+template <int GROUP, bool DENSE, bool BITMAP = false>
 __global__ void __launch_bounds__(GROUP == 32 ? 64 : GROUP, RowsMinBlocks<GROUP>::value) k_rows(const RowArgs a) {
+  static_assert(!BITMAP || (GROUP > 32 && !DENSE), "bitmap rows are CTA-owned rows of a hashed bin");
   const int GROUPS = GROUP == 32 ? (int)(blockDim.x >> 5) : 1;  // warp-owned rows: several independent warps per CTA
   constexpr int NW = GROUP / 32;
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -731,6 +748,8 @@ __global__ void __launch_bounds__(GROUP == 32 ? 64 : GROUP, RowsMinBlocks<GROUP>
   uint32_t *wqueue = reinterpret_cast<uint32_t *>(hist + 256);  // NW * 64 queued cells awaiting evaluation
   uint32_t *h1 = reinterpret_cast<uint32_t *>(hist);   // kCutBins/2 words: u16 histogram of colB over the strongly positive k11 == 1 cells
   uint32_t *table = wqueue + NW * 64;
+  uint32_t *seen = table + a.slots;     // BITMAP: a.bm_words words, bit b = key b has a product in the row
+  uint32_t *singles = seen + a.bm_words;  // BITMAP: top_k packed words, the k11 = 1 cells up to the key cut
   volatile int *vctrl = ctrl;
 
   const int row_begin = a.bin_bounds[a.bin], row_end = a.bin_bounds[a.bin + 1];
@@ -756,8 +775,11 @@ __global__ void __launch_bounds__(GROUP == 32 ? 64 : GROUP, RowsMinBlocks<GROUP>
     uint32_t n_pass = 1, tsize = (uint32_t)a.n_cols_b;
     if (!DENSE) {
       const uint32_t w = a.row_work[item];
-      const uint32_t dbound = w < (uint32_t)a.n_cols_b ? w : (uint32_t)a.n_cols_b;
-      n_pass = (dbound + (uint32_t)a.cap - 1u) / (uint32_t)a.cap;
+      // BITMAP: the table holds only cells with k11 >= 2, each of at least two of the w products (one pass: the host
+      // sizes a.slots for the bin's largest w)
+      const uint32_t dcells = BITMAP ? w / 2u : w;
+      const uint32_t dbound = dcells < (uint32_t)a.n_cols_b ? dcells : (uint32_t)a.n_cols_b;
+      n_pass = BITMAP ? 1u : (dbound + (uint32_t)a.cap - 1u) / (uint32_t)a.cap;
       if (n_pass == 0) n_pass = 1;
       tsize = n_pass > 1 ? (uint32_t)a.slots
                          : (uint32_t)min((unsigned long long)a.slots,
@@ -776,6 +798,8 @@ __global__ void __launch_bounds__(GROUP == 32 ? 64 : GROUP, RowsMinBlocks<GROUP>
     for (uint32_t pass = 0; pass < n_pass; ++pass) {
       // ---- clear --------------------------------------------------------------------------------------
       for (uint32_t i = gtid; i < tsize; i += GROUP) table[i] = DENSE ? 0u : kEmpty;
+      if (BITMAP)
+        for (int i = gtid; i < a.bm_words; i += GROUP) seen[i] = 0u;
       group_sync<GROUP>();
       // ---- count -------------------------------------------------------------------------------------------
       if (NW == 1) {
@@ -796,7 +820,7 @@ __global__ void __launch_bounds__(GROUP == 32 ? 64 : GROUP, RowsMinBlocks<GROUP>
           }
           const uint32_t total = __shfl_sync(0xffffffffu, off, 31);
           off = i < u_end ? off - len : 0xffffffffu;  // exclusive
-          count_window<GROUP, DENSE>(a, table, tsize, cbits, n_pass, pass, off, s, 0u, total, lane);
+          count_window<GROUP, DENSE, BITMAP>(a, table, seen, tsize, cbits, n_pass, pass, off, s, 0u, total, lane);
         }
       } else {
         // CTA-owned row: the count barrier waits for the busiest warp, and B' degrees are Zipf-skewed, so the warps
@@ -844,7 +868,7 @@ __global__ void __launch_bounds__(GROUP == 32 ? 64 : GROUP, RowsMinBlocks<GROUP>
             for (uint32_t j0 = lo, p = p_lo; p < p_hi; j0 += 32) {
               const uint2 e = j0 + lane < nwin ? wofs[j0 + lane] : make_uint2(0u, 0xffffffffu);
               const uint32_t wend = min(p_hi, j0 + 32 < nwin ? wofs[j0 + 32].y : T);
-              count_window<GROUP, DENSE>(a, table, tsize, cbits, n_pass, pass, e.y, e.x, p, wend, lane);
+              count_window<GROUP, DENSE, BITMAP>(a, table, seen, tsize, cbits, n_pass, pass, e.y, e.x, p, wend, lane);
               p = wend;
             }
           }
@@ -864,12 +888,65 @@ __global__ void __launch_bounds__(GROUP == 32 ? 64 : GROUP, RowsMinBlocks<GROUP>
         const uint32_t word = DENSE ? ((idx << cbits) | w) : w;
         const unsigned m = __ballot_sync(0xffffffffu, valid);
         __syncwarp();
-        if (valid) table[seg_lo + n_mine + __popc(m & ((1u << lane) - 1u))] = word;
+        if (valid) {
+          // BITMAP: the table counted k11 - 1; the cell leaves the bitmap, which keeps the k11 = 1 cells only
+          table[seg_lo + n_mine + __popc(m & ((1u << lane) - 1u))] = BITMAP ? word + 1u : word;
+          if (BITMAP) atomicAnd(&seen[(word >> cbits) >> 5], ~(1u << ((word >> cbits) & 31u)));
+        }
         n_mine += __popc(m);
         __syncwarp();
       }
       if (lane == 0) distinct_local += n_mine;
-      if (a.emit_all) {
+      uint32_t n_list = n_mine;   // cells this warp filters: its compacted table words, then (BITMAP) its singles
+      const uint32_t *singles_mine = singles;
+      if (BITMAP) {
+        // ---- singles and the level-1 key cut (exact; DESIGN.md 3.1 "bitmap rows") -----------------------------------
+        // The bitmap now holds the k11 = 1 cells.  Without the diagonal, the first top_k set bits in key order are the
+        // cells at or below the key cut (all of them when there are fewer): one CTA prefix sum of popcounts over
+        // contiguous word ranges, and each thread lists the bits of its range that fall below top_k.
+        group_sync<GROUP>();
+        if (gtid == 0 && diag >= 0) {
+          const uint32_t bit = 1u << ((uint32_t)diag & 31u);
+          if (seen[diag >> 5] & bit) {
+            seen[diag >> 5] &= ~bit;
+            ++distinct_local;
+          }
+        }
+        group_sync<GROUP>();
+        const uint32_t nbw = (uint32_t)a.bm_words, per = (nbw + GROUP - 1u) / GROUP;
+        const uint32_t w_lo = min((uint32_t)gtid * per, nbw), w_hi = min(w_lo + per, nbw);
+        uint32_t cnt = 0;
+        for (uint32_t i = w_lo; i < w_hi; ++i) cnt += __popc(seen[i]);
+        distinct_local += cnt;
+        uint32_t incl = cnt;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+          const uint32_t v = __shfl_up_sync(0xffffffffu, incl, d);
+          if (lane >= d) incl += v;
+        }
+        int *wsum = hist;   // the select histogram is dead until the score stage
+        if (lane == 31) wsum[gw] = (int)incl;
+        __syncthreads();
+        uint32_t wpre = lane < NW ? (uint32_t)wsum[lane] : 0u;
+#pragma unroll
+        for (int d = 1; d < NW; d <<= 1) {
+          const uint32_t v = __shfl_up_sync(0xffffffffu, wpre, d);
+          if (lane >= d) wpre += v;
+        }
+        const uint32_t total = __shfl_sync(0xffffffffu, wpre, NW - 1);
+        const uint32_t before = gw == 0 ? 0u : __shfl_sync(0xffffffffu, wpre, gw - 1);
+        const uint32_t n_single = min(total, (uint32_t)a.top_k);
+        uint32_t o = before + incl - cnt;
+        for (uint32_t i = w_lo; i < w_hi && o < n_single; ++i)
+          for (uint32_t m = seen[i]; m != 0u && o < n_single; m &= m - 1u)
+            singles[o++] = (((i << 5) | (uint32_t)(__ffs(m) - 1)) << cbits) | 1u;
+        __syncthreads();   // wsum is the select histogram again; the singles are complete
+        const uint32_t s_lo = (uint32_t)((unsigned long long)n_single * gw / NW);
+        const uint32_t s_hi = (uint32_t)((unsigned long long)n_single * (gw + 1) / NW);
+        singles_mine = singles + s_lo;
+        n_list = n_mine + (s_hi - s_lo);
+      }
+      if (!BITMAP && a.emit_all) {
         // debug: every non-zero cell of the row (col, count), unordered
         int basepos = 0;
         if (lane == 0) basepos = atomicAdd(&ctrl[0], (int)n_mine);
@@ -895,8 +972,8 @@ __global__ void __launch_bounds__(GROUP == 32 ? 64 : GROUP, RowsMinBlocks<GROUP>
       // colB are ordered by column id, the output's tie order, so the cut is exact and drops ties beyond the k-th too.
       // Both hold for the COMPUTED fp64 values only when adjacent colB values are further apart than the evaluation
       // error: the host checks that once per indicator (a.cut_ok) and otherwise the row runs without the cut.
-      int cut1 = 0x7fffffff;
-      if (a.cut_ok && a.row_work[item] < 65536u) {   // u16 bins cannot overflow
+      int cut1 = 0x7fffffff;   // (BITMAP: the singles list is already cut)
+      if (!BITMAP && a.cut_ok && a.row_work[item] < 65536u) {   // u16 bins cannot overflow
         int sh = keyed ? a.key_shift : 0, hi_sh = 32;   // level: bins over key bits [sh, hi_sh) of keys matching `prefix` above
         uint32_t prefix = 0, need = (uint32_t)a.top_k;
         while (true) {
@@ -943,12 +1020,12 @@ __global__ void __launch_bounds__(GROUP == 32 ? 64 : GROUP, RowsMinBlocks<GROUP>
       uint32_t pos = 0;
       int qn = 0;
       while (true) {
-        while (qn < 32 && pos < n_mine) {
+        while (qn < 32 && pos < n_list) {
           const uint32_t q = pos + lane;
           bool surv = false;
           uint32_t word = 0;
-          if (q < n_mine) {
-            word = table[seg_lo + q];
+          if (q < n_list) {
+            word = (!BITMAP || q < n_mine) ? table[seg_lo + q] : singles_mine[q - n_mine];
             const uint32_t b = word >> cbits, k11 = word & cmask;
             if ((int)b != diag) {
               // Dominance filter (exact, DESIGN.md "dominance"): for fixed rowA and N, on the positively associated
@@ -1024,7 +1101,7 @@ __global__ void __launch_bounds__(GROUP == 32 ? 64 : GROUP, RowsMinBlocks<GROUP>
           if (pass_ok) tk[basepos + __popc(m & ((1u << lane) - 1u))] = e;
           basepos_round = basepos;
         }
-        const bool more = qn > 0 || pos < n_mine;
+        const bool more = qn > 0 || pos < n_list;
         // Both decisions of this round are taken from barrier results (CTA-uniform by construction).  Re-reading ctrl[0]
         // after the barrier raced with warps that had already looped back and appended (or with warp 0's single-warp
         // select storing the kept count): warps of one CTA could disagree on `n > prune_limit` and pair different
