@@ -547,6 +547,15 @@ int cco_debug_cooccurrence(cco_ctx_t *ctx, const cco_csr_t *a, const cco_csr_t *
 int cco_debug_downsample(cco_ctx_t *ctx, const cco_csr_t *m, int32_t max_interactions, int32_t seed,
                          uint32_t flags, int64_t **row_ptr, int32_t **col_idx, int32_t *raw_col_counts,
                          int32_t *new_col_counts);
+/* Debug/parity entry (tests only): one rank's share of the multi-GPU sampleDownAndBinarize, on one GPU.  The whole
+ * matrix is uploaded (and canonicalised unless CCO_FLAG_ASSUME_CANONICAL); the users [row_lo, row_hi) are then sampled
+ * as the rank owning that block samples them: by global user id, with raw_col_counts[n_cols] as the column counts (the
+ * whole matrix's, as the all-reduce of the ranks' histograms gives them).  Out: kept_per_row[n_rows] (indexed by global
+ * user, zero outside the block), *col_idx = the block's kept columns in order (as many as the block's kept counts sum
+ * to, malloc'ed, free with cco_free), new_col_counts[n_cols] = the block's share of the post-sample column counts. */
+int cco_debug_downsample_block(cco_ctx_t *ctx, const cco_csr_t *m, int64_t row_lo, int64_t row_hi,
+                               const int32_t *raw_col_counts, int32_t max_interactions, int32_t seed, uint32_t flags,
+                               int64_t *kept_per_row, int32_t **col_idx, int32_t *new_col_counts);
 /* Debug/parity entry (tests only): the device LLR of n cells. */
 int cco_debug_llr(cco_ctx_t *ctx, int64_t n, const int64_t *k11, const int64_t *k12, const int64_t *k21,
                   const int64_t *k22, uint32_t flags, double *out);

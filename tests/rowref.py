@@ -44,17 +44,24 @@ class Expected:
                                    self.top_k) for w, r in zip(self.work, self.ra)]
 
 
-def sampled(mats, params, seed: int, flags: int = 0):
-    """[(A' or B'_i as orc.Csr, its column marginals)] exactly as the train samples them (orc_train)."""
+def oracle_sampler(c, m: int, seed: int, flags: int = 0):
+    """The default preparation: orc_train's canonicalisation and sampler -> (sampled orc.Csr, raw counts, marginals)"""
+    return orc.downsample(orc.canonicalize(c), m, seed, flags)
+
+
+def sampled(mats, params, seed: int, flags: int = 0, sampler=None):
+    """[(A' or B'_i as orc.Csr, its column marginals)] exactly as the train samples them (orc_train).  sampler: another
+    preparation of the same shape as `oracle_sampler` (e.g. sampler_ref.csr_sampler(orc.Csr))."""
+    sampler = sampler or oracle_sampler
     out = []
     for (nr, nc, rp, ci), p in zip(mats, params):
-        d, _, marg = orc.downsample(orc.canonicalize(orc.Csr(nr, nc, rp, ci)), int(p[0]), seed, flags & 3)
+        d, _, marg = sampler(orc.Csr(nr, nc, rp, ci), int(p[0]), seed, flags & 3)
         out.append((d, marg.astype(np.int64)))
     return out
 
 
-def expected(ctx, mats, params, seed: int, flags: int = 0) -> list[Expected]:
-    sm = sampled(mats, params, seed, flags)
+def expected(ctx, mats, params, seed: int, flags: int = 0, sampler=None) -> list[Expected]:
+    sm = sampled(mats, params, seed, flags, sampler)
     a, marg_a = sm[0]
     n = int(a.n_rows)
     n_items = int(a.n_cols)

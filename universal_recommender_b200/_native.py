@@ -118,7 +118,7 @@ EXPORTS = [
     "cco_format_model", "cco_rerank_model", "cco_event_log_read", "cco_event_log_info", "cco_event_log_ingest",
     "cco_format_model_log", "cco_rerank_model_log", "cco_event_log_free", "cco_event_log_begin", "cco_event_log_append",
     "cco_event_log_finish", "cco_event_log_begin_window", "cco_event_log_window_stats", "cco_result_num_matrices", "cco_result_row_range", "cco_result_matrix", "cco_result_stats", "cco_result_free",
-    "cco_debug_cooccurrence", "cco_debug_downsample", "cco_debug_llr", "cco_debug_string_ids", "cco_free",
+    "cco_debug_cooccurrence", "cco_debug_downsample", "cco_debug_downsample_block", "cco_debug_llr", "cco_debug_string_ids", "cco_free",
 ]
 
 _lib = None
@@ -191,6 +191,8 @@ def lib():
     L.cco_debug_cooccurrence.argtypes = [C.c_void_p, p(CsrT), p(CsrT), p(p(C.c_int64)), p(p(C.c_int32)), p(p(C.c_int32))]
     L.cco_debug_downsample.argtypes = [C.c_void_p, p(CsrT), C.c_int32, C.c_int32, C.c_uint32, p(p(C.c_int64)),
                                        p(p(C.c_int32)), p(C.c_int32), p(C.c_int32)]
+    L.cco_debug_downsample_block.argtypes = [C.c_void_p, p(CsrT), C.c_int64, C.c_int64, p(C.c_int32), C.c_int32, C.c_int32, C.c_uint32,
+                                             p(C.c_int64), p(p(C.c_int32)), p(C.c_int32)]
     L.cco_debug_llr.argtypes = [C.c_void_p, C.c_int64, p(C.c_int64), p(C.c_int64), p(C.c_int64), p(C.c_int64), C.c_uint32,
                                 p(C.c_double)]
     L.cco_debug_string_ids.argtypes = [C.c_void_p, C.c_int64, p(C.c_int64), C.c_void_p, C.c_int32, p(C.c_int32)]

@@ -555,6 +555,42 @@ static int launch_write(cco_ctx *c, Arena &ar, const DevRaw &raw, const SampleSc
   return CCO_OK;
 }
 
+// Raw column counts (numNonZeroElementsPerColumn) of a block of user rows of every matrix, the one way the library counts
+// them: per matrix k_check_row_ptr (with a verdict) and k_col_histogram_flat<true> into kHistCopies replicated copies,
+// then one k_sum_copies over all matrices.  counts: kHistCopies copies of max(col_off[n], 1) zeroed words, matrix i at
+// col_off[i]; the totals land in copy 0.  ready (nullable): per matrix, the event after which its block is on the device.
+// verdict (nullable: the block is validated already): 2 ints per matrix, [2i] set for a malformed matrix.
+constexpr int kHistCopies = 16;
+static int count_raw_columns(cco_ctx *c, const std::vector<DevRaw> &raw, const std::vector<long long> &col_off, const cudaEvent_t *ready,
+                             int *verdict, int32_t *counts) {
+  cudaStream_t s = c->stream;
+  const int n_mats = (int)raw.size();
+  const long long total_cols = col_off[n_mats];
+  const long long copy_stride = std::max<long long>(total_cols, 1);
+  for (int i = 0; i < n_mats; ++i) {
+    if (ready) CK(cudaStreamWaitEvent(s, ready[i], 0));  // matrix i has landed (async upload: later ones may still be in flight)
+    if (raw[i].n_rows == 0) continue;
+    // CCO_FLAG_ASSUME_CANONICAL skips the canonicalisation, not the safety net: a malformed matrix still fails the call
+    // (until the verdict is read, the histogram skips ids outside the column space and the sampler keeps nothing)
+    int *v = verdict ? verdict + 2 * i : nullptr;
+    if (v) {
+      k_check_row_ptr<<<grid_for(raw[i].n_rows, 256, c->sm_count), 256, 0, s>>>(raw[i].n_rows, raw[i].rp, raw[i].q_base, raw[i].q_base + raw[i].nnz, v);
+      c->launches++;
+    }
+    if (raw[i].nnz > 0) {
+      // warp-aggregated (__match_any_sync) before the atomics: Zipf-hot columns take one atomic per warp instead of per lane
+      k_col_histogram_flat<true><<<grid_for(raw[i].nnz, 256, c->sm_count), 256, 0, s>>>(raw[i].nnz, raw[i].col + raw[i].q_base, raw[i].n_cols,
+                                                                                       counts + col_off[i], kHistCopies, copy_stride, v);
+      c->launches++;
+    }
+  }
+  if (total_cols > 0) {
+    k_sum_copies<<<grid_for(total_cols, 256, c->sm_count), 256, 0, s>>>(total_cols, kHistCopies, copy_stride, counts);
+    c->launches++;
+  }
+  return CCO_OK;
+}
+
 // sampleDownAndBinarize of one whole matrix on this GPU (raw column counts already final in raw_counts)
 static int downsample_device(cco_ctx *c, Arena &ar, const DevRaw &raw, const int *bad, const int32_t *raw_counts, int32_t m,
                              int32_t seed, uint32_t flags, DevMat *out) {
@@ -1400,7 +1436,6 @@ static int train_dataset(cco_ctx *c, const cco_dataset *ds, const cco_indicator_
     total_cols += raw[i].n_cols;
   }
   col_off[n_mats] = total_cols;
-  constexpr int kHistCopies = 16;
   const long long copy_stride = std::max<long long>(total_cols, 1);
   int32_t *raw_counts, *marg_all;
   int *d_check;
@@ -1410,28 +1445,7 @@ static int train_dataset(cco_ctx *c, const cco_dataset *ds, const cco_indicator_
   CK(cudaMemsetAsync(raw_counts, 0, sizeof(int32_t) * (size_t)copy_stride * kHistCopies, s));
   CK(cudaMemsetAsync(marg_all, 0, sizeof(int32_t) * (size_t)copy_stride, s));
   CK(cudaMemsetAsync(d_check, 0, sizeof(int) * 2 * n_mats, s));
-  for (int i = 0; i < n_mats; ++i) {
-    CK(cudaStreamWaitEvent(s, ds->ready[i], 0));  // matrix i has landed (async upload: later ones may still be in flight)
-    if (ds->n_local == 0) continue;
-    // CCO_FLAG_ASSUME_CANONICAL skips the canonicalisation, not the safety net: a malformed matrix still fails the call
-    // (until the verdict is read, the histogram skips ids outside the column space and the sampler keeps nothing)
-    int *verdict = ds->validated ? nullptr : d_check + 2 * i;
-    if (verdict) {
-      k_check_row_ptr<<<grid_for(raw[i].n_rows, 256, c->sm_count), 256, 0, s>>>(raw[i].n_rows, raw[i].rp, raw[i].q_base, raw[i].q_base + raw[i].nnz,
-                                                                              verdict);
-      c->launches++;
-    }
-    if (raw[i].nnz > 0) {
-      // warp-aggregated (__match_any_sync) before the atomics: Zipf-hot columns take one atomic per warp instead of per lane
-      k_col_histogram_flat<true><<<grid_for(raw[i].nnz, 256, c->sm_count), 256, 0, s>>>(raw[i].nnz, raw[i].col + raw[i].q_base, raw[i].n_cols,
-                                                                                       raw_counts + col_off[i], kHistCopies, copy_stride, verdict);
-      c->launches++;
-    }
-  }
-  if (total_cols > 0) {
-    k_sum_copies<<<grid_for(total_cols, 256, c->sm_count), 256, 0, s>>>(total_cols, kHistCopies, copy_stride, raw_counts);
-    c->launches++;
-  }
+  CKR(count_raw_columns(c, raw, col_off, ds->ready.data(), ds->validated ? nullptr : d_check, raw_counts));
   CK(mark(0));
   if (c->world > 1) {
     if (total_cols > 0)
@@ -4779,31 +4793,114 @@ int cco_debug_downsample(cco_ctx_t *c, const cco_csr_t *m, int32_t max_interacti
   CKR(dataset_upload(c, 1, m, flags, &ds));
   struct DG { cco_dataset *d; ~DG() { dataset_release(d); } } dg{ds};
   Arena ar(c->stream);
-  DevRaw raw;
-  raw.n_rows = ds->n_users; raw.n_cols = (int32_t)ds->n_cols[0]; raw.nnz = ds->nnz[0]; raw.nnz_cap = ds->nnz[0];
-  raw.rp = ds->rp[0]; raw.col = ds->col[0];
+  std::vector<DevRaw> raw(1);
+  raw[0].n_rows = ds->n_users; raw[0].n_cols = (int32_t)ds->n_cols[0]; raw[0].nnz = ds->nnz[0]; raw[0].nnz_cap = ds->nnz[0];
+  raw[0].rp = ds->rp[0]; raw[0].col = ds->col[0];
+  // the raw counts and the verdict exactly as the train makes them (count_raw_columns)
+  const std::vector<long long> col_off = {0, m->n_cols};
+  const int32_t width = std::max<int32_t>(m->n_cols, 1);
   int32_t *counts;
-  CKR(ar.alloc(&counts, std::max<int32_t>(m->n_cols, 1)));
-  CK(cudaMemsetAsync(counts, 0, sizeof(int32_t) * (size_t)std::max<int32_t>(m->n_cols, 1), c->stream));
-  if (raw.nnz > 0 && m->n_rows > 0)
-    k_col_histogram<<<grid_for(raw.nnz, 256, c->sm_count), 256, 0, c->stream>>>(0, m->n_rows, raw.rp, raw.col, raw.n_cols, counts, 1, 0);
+  int *d_check;
+  CKR(ar.alloc(&counts, (size_t)width * kHistCopies));
+  CKR(ar.alloc(&d_check, 2));
+  CK(cudaMemsetAsync(counts, 0, sizeof(int32_t) * (size_t)width * kHistCopies, c->stream));
+  CK(cudaMemsetAsync(d_check, 0, sizeof(int) * 2, c->stream));
+  int *verdict = ds->validated ? nullptr : d_check;
+  CKR(count_raw_columns(c, raw, col_off, ds->ready.data(), verdict, counts));
   DevMat dm;
-  CKR(downsample_device(c, ar, raw, nullptr, counts, max_interactions, seed, flags, &dm));
+  CKR(downsample_device(c, ar, raw[0], verdict, counts, max_interactions, seed, flags, &dm));
   std::vector<uint32_t> rp32((size_t)m->n_rows + 1);
+  int h_check = 0;
   CK(cudaMemcpyAsync(rp32.data(), dm.rp, sizeof(uint32_t) * rp32.size(), cudaMemcpyDeviceToHost, c->stream));
+  CK(cudaMemcpyAsync(&h_check, d_check, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   if (raw_col_counts && m->n_cols > 0)
     CK(cudaMemcpyAsync(raw_col_counts, counts, sizeof(int32_t) * (size_t)m->n_cols, cudaMemcpyDeviceToHost, c->stream));
   if (new_col_counts && m->n_cols > 0)
     CK(cudaMemcpyAsync(new_col_counts, dm.marg, sizeof(int32_t) * (size_t)m->n_cols, cudaMemcpyDeviceToHost, c->stream));
   CK(cudaStreamSynchronize(c->stream));
   CK(cudaGetLastError());
+  if (h_check) return set_error(CCO_E_INVALID_ARG, "row_ptr not monotone or column index out of [0, n_cols)");
   size_t nnz = rp32[m->n_rows];
   int64_t *rp = (int64_t *)malloc(sizeof(int64_t) * rp32.size());
-  int32_t *ci = (int32_t *)malloc(sizeof(int32_t) * std::max<size_t>(nnz, 1));
+  int32_t *ci = (int32_t *)calloc(std::max<size_t>(nnz, 1), sizeof(int32_t));
   if (!rp || !ci) return set_error(CCO_E_OOM, "malloc failed");
   for (size_t i = 0; i < rp32.size(); ++i) rp[i] = rp32[i];
-  if (nnz) CK(cudaMemcpy(ci, dm.col, sizeof(int32_t) * nnz, cudaMemcpyDeviceToHost));
+  // (kept counts beyond the matrix's entries show in row_ptr; the copy stays inside the sampled columns, the tail stays 0)
+  const size_t n_copy = std::min<size_t>(nnz, (size_t)raw[0].nnz);
+  if (n_copy) CK(cudaMemcpy(ci, dm.col, sizeof(int32_t) * n_copy, cudaMemcpyDeviceToHost));
   *row_ptr = rp;
+  *col_idx = ci;
+  return CCO_OK;
+}
+
+// one rank's share of downsample_sharded_all on one GPU: the rank that owns users [row_lo, row_hi) samples them with
+// row_base = row_lo, absolute entry offsets, the whole matrix's raw counts and kept counts indexed by global user
+int cco_debug_downsample_block(cco_ctx_t *c, const cco_csr_t *m, int64_t row_lo, int64_t row_hi, const int32_t *raw_col_counts,
+                               int32_t max_interactions, int32_t seed, uint32_t flags, int64_t *kept_per_row, int32_t **col_idx,
+                               int32_t *new_col_counts) {
+  if (!c || !m || !col_idx || (m->n_rows > 0 && !kept_per_row) || (m->n_cols > 0 && (!raw_col_counts || !new_col_counts)))
+    return set_error(CCO_E_INVALID_ARG, "null argument");
+  if (c->world != 1 || !c->members.empty()) return set_error(CCO_E_UNSUPPORTED, "debug entries need a single-GPU context");
+  cco_indicator_params_t prm = {max_interactions, 1, 0, 0.0};
+  CKR(validate_host(1, m, &prm));
+  if (row_lo < 0 || row_hi < row_lo || row_hi > m->n_rows)
+    return set_error(CCO_E_INVALID_ARG, "rows [%lld, %lld) outside [0, %lld)", (long long)row_lo, (long long)row_hi, (long long)m->n_rows);
+  CK(cudaSetDevice(c->device));
+  mail_reset(c);
+  cudaStream_t s = c->stream;
+  cco_dataset *ds = nullptr;
+  CKR(dataset_upload(c, 1, m, flags, &ds));
+  struct DG { cco_dataset *d; ~DG() { dataset_release(d); } } dg{ds};
+  Arena ar(s);
+  const long long U = ds->n_users;
+  const int32_t width = std::max<int32_t>(m->n_cols, 1);
+  long long q[2] = {0, 0};   // the block's entries, from the (possibly canonicalised) device row_ptr
+  CK(cudaMemcpyAsync(&q[0], ds->rp[0] + row_lo, sizeof(long long), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(&q[1], ds->rp[0] + row_hi, sizeof(long long), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  DevRaw blk;
+  blk.n_rows = row_hi - row_lo;
+  blk.row_base = row_lo;
+  blk.n_cols = m->n_cols;
+  blk.q_base = q[0];
+  blk.nnz = q[1] - q[0];
+  blk.nnz_cap = ds->nnz[0];
+  blk.rp = ds->rp[0] + row_lo;
+  blk.col = ds->col[0];   // indexable by absolute offsets, as a rank's upload is
+  int32_t *counts, *marg, *dst;
+  uint32_t *kept;
+  CKR(ar.alloc(&counts, width));
+  CKR(ar.alloc(&marg, width));
+  CKR(ar.alloc(&kept, U + 1));
+  CKR(ar.alloc(&dst, std::max<long long>(blk.nnz, 1)));
+  if (m->n_cols > 0) CK(cudaMemcpyAsync(counts, raw_col_counts, sizeof(int32_t) * (size_t)m->n_cols, cudaMemcpyHostToDevice, s));
+  CK(cudaMemsetAsync(marg, 0, sizeof(int32_t) * (size_t)width, s));
+  CK(cudaMemsetAsync(kept, 0, sizeof(uint32_t) * ((size_t)U + 1), s));
+  SampleScratch sc;
+  CKR(sample_scratch(c, ar, blk, counts, max_interactions, &sc));
+  launch_count(c, blk, sc, max_interactions, seed, flags, nullptr, kept, marg);
+  CKR(launch_write(c, ar, blk, sc, dst));
+  std::vector<uint32_t> hk((size_t)U + 1);
+  CK(cudaMemcpyAsync(hk.data(), kept, sizeof(uint32_t) * hk.size(), cudaMemcpyDeviceToHost, s));
+  if (m->n_cols > 0) CK(cudaMemcpyAsync(new_col_counts, marg, sizeof(int32_t) * (size_t)m->n_cols, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  // the train lays the block's columns out by the scanned kept counts: as many as they sum to
+  size_t n_kept = 0;
+  for (long long r = 0; r < U; ++r) {
+    kept_per_row[r] = hk[r];
+    if (r >= row_lo && r < row_hi) n_kept += hk[r];
+  }
+  int32_t *ci = (int32_t *)calloc(std::max<size_t>(n_kept, 1), sizeof(int32_t));
+  if (!ci) return set_error(CCO_E_OOM, "malloc failed");
+  const size_t n_copy = std::min<size_t>(n_kept, (size_t)blk.nnz);   // (kept counts beyond the block's entries: the tail stays 0)
+  if (n_copy) {
+    cudaError_t e = cudaMemcpy(ci, dst, sizeof(int32_t) * n_copy, cudaMemcpyDeviceToHost);
+    if (e != cudaSuccess) {
+      free(ci);
+      return set_error(CCO_E_CUDA, "cudaMemcpy: %s", cudaGetErrorString(e));
+    }
+  }
   *col_idx = ci;
   return CCO_OK;
 }
@@ -4831,16 +4928,15 @@ int cco_debug_cooccurrence(cco_ctx_t *c, const cco_csr_t *a, const cco_csr_t *b,
     raw[i].n_rows = ds->n_users; raw[i].n_cols = (int32_t)ds->n_cols[i]; raw[i].nnz = ds->nnz[i]; raw[i].nnz_cap = ds->nnz[i];
     raw[i].rp = ds->rp[i]; raw[i].col = ds->col[i];
   }
-  // identity "downsample" (m = INT_MAX) gives the device CSR + marginals
+  // identity "downsample" (m = INT_MAX) gives the device CSR + marginals; raw counts as the train makes them
+  const std::vector<long long> col_off = {0, raw[0].n_cols, (long long)raw[0].n_cols + raw[1].n_cols};
+  const long long width = std::max<long long>(col_off[2], 1);
+  int32_t *counts;
+  CKR(ar.alloc(&counts, (size_t)width * kHistCopies));
+  CK(cudaMemsetAsync(counts, 0, sizeof(int32_t) * (size_t)width * kHistCopies, s));
+  CKR(count_raw_columns(c, raw, col_off, ds->ready.data(), nullptr, counts));   // (uploaded with validation + canonicalisation)
   std::vector<DevMat> dm(2);
-  for (int i = 0; i < 2; ++i) {
-    int32_t *counts;
-    CKR(ar.alloc(&counts, std::max<int32_t>(raw[i].n_cols, 1)));
-    CK(cudaMemsetAsync(counts, 0, sizeof(int32_t) * (size_t)std::max<int32_t>(raw[i].n_cols, 1), s));
-    if (raw[i].nnz > 0 && raw[i].n_rows > 0)
-      k_col_histogram<<<grid_for(raw[i].nnz, 256, c->sm_count), 256, 0, s>>>(0, raw[i].n_rows, raw[i].rp, raw[i].col, raw[i].n_cols, counts, 1, 0);
-    CKR(downsample_device(c, ar, raw[i], nullptr, counts, 0x7fffffff, 0, 0, &dm[i]));
-  }
+  for (int i = 0; i < 2; ++i) CKR(downsample_device(c, ar, raw[i], nullptr, counts + col_off[i], 0x7fffffff, 0, 0, &dm[i]));
   const int32_t n_items_a = dm[0].n_cols;
   uint32_t *at_ptr, *cursor, *marg_pad;
   int32_t *at_users, *d_max;

@@ -21,8 +21,9 @@
 // Pass 2 is an order-preserving stream compaction by the keep bytes (cub::DeviceSelect::Flagged in cco_api.cu): kept
 // entries keep their global order, so their rank inside the block is their offset from the block's first kept entry.
 //
-// These kernels supersede k_downsample_count / k_downsample_write, which stay in cco_kernels.cuh unreferenced: bench.py
-// names the row-kernel build a line was measured on by that file's hash (source_build_id).
+// These kernels supersede k_downsample_count / k_downsample_write, and k_col_histogram_flat (the raw counts of the train and
+// of every debug entry, cco_api.cu count_raw_columns) supersedes k_col_histogram; the old ones stay in cco_kernels.cuh
+// unreferenced: bench.py names the row-kernel build a line was measured on by that file's hash (source_build_id).
 #pragma once
 
 #include <cuda_runtime.h>

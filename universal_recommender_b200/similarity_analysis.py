@@ -659,6 +659,26 @@ class CcoContext:
         self._L.cco_free(oci)
         return r, c, raw[:n_cols], new[:n_cols]
 
+    def debug_downsample_block(self, n_rows, n_cols, row_ptr, col_idx, row_lo: int, row_hi: int, raw_col_counts,
+                               max_interactions: int, seed: int, flags: int = 0):
+        """cco_debug_downsample_block: users [row_lo, row_hi) sampled as the rank owning them samples them, with the whole
+        matrix's raw column counts -> (kept per user int64[n_rows], the block's kept columns, its post-sample column counts)."""
+        rp = np.ascontiguousarray(row_ptr, dtype=np.int64)
+        ci = np.ascontiguousarray(col_idx, dtype=np.int32)
+        m = N.as_csr_t(n_rows, n_cols, rp, ci)
+        raw = np.zeros(max(n_cols, 1), np.int32)
+        raw[:n_cols] = raw_col_counts
+        kept = np.zeros(max(n_rows, 1), np.int64)
+        new = np.zeros(max(n_cols, 1), np.int32)
+        oci = C.POINTER(C.c_int32)()
+        N.check(self._L.cco_debug_downsample_block(self._h, C.byref(m), row_lo, row_hi, raw.ctypes.data_as(C.POINTER(C.c_int32)),
+                                                   max_interactions, _to_i32(seed), flags, kept.ctypes.data_as(C.POINTER(C.c_int64)),
+                                                   C.byref(oci), new.ctypes.data_as(C.POINTER(C.c_int32))))
+        n = int(kept[row_lo:row_hi].sum())
+        c = np.ctypeslib.as_array(oci, shape=(n,)).copy() if n else np.zeros(0, np.int32)
+        self._L.cco_free(oci)
+        return kept[:n_rows], c, new[:n_cols]
+
     def debug_cooccurrence(self, a, b):
         """a, b = (n_rows, n_cols, row_ptr, col_idx) canonical binary matrices -> (row_ptr, col_idx, count) of A^T B."""
         keep = []
