@@ -529,7 +529,7 @@ static int sample_scratch(cco_ctx *c, Arena &ar, const DevRaw &raw, const int32_
   return CCO_OK;
 }
 // pass 1 (k_sample_count, cco_sampler.cuh): entry-parallel; `kept` must be zero for the block's rows; `bad` (nullable) is the
-// device verdict of k_check_row_ptr / k_col_histogram_flat -- a malformed matrix keeps nothing, so pass 2 can never write more than row_ptr promises
+// device verdict of count_raw_columns -- a malformed matrix keeps nothing, so pass 2 can never write more than row_ptr promises
 static void launch_count(cco_ctx *c, const DevRaw &raw, const SampleScratch &sc, int32_t m, int32_t seed, uint32_t flags, const int *bad,
                          uint32_t *kept, int32_t *new_counts) {
   if (raw.n_rows <= 0 || raw.nnz <= 0) return;
@@ -556,22 +556,70 @@ static int launch_write(cco_ctx *c, Arena &ar, const DevRaw &raw, const SampleSc
 }
 
 // Raw column counts (numNonZeroElementsPerColumn) of a block of user rows of every matrix, the one way the library counts
-// them: per matrix k_check_row_ptr (with a verdict) and k_col_histogram_flat<true> into kHistCopies replicated copies,
-// then one k_sum_copies over all matrices.  counts: kHistCopies copies of max(col_off[n], 1) zeroed words, matrix i at
-// col_off[i]; the totals land in copy 0.  ready (nullable): per matrix, the event after which its block is on the device.
-// verdict (nullable: the block is validated already): 2 ints per matrix, [2i] set for a malformed matrix.
+// them.  Matrices whose column space fits a CTA's shared memory as 16-bit counters are counted and row_ptr-checked by
+// k_col_counts_smem, kHistSegs matrices per launch.  The others (C4: 1 M columns) take k_check_row_ptr and
+// k_col_histogram_flat<true> into kHistCopies replicated copies, folded by one k_sum_copies.  *counts (allocated here):
+// col_off[n] words, matrix i at col_off[i].  ready (nullable): per matrix, the event after which its block is on the
+// device.  verdict (nullable: the block is validated already): 2 ints per matrix, [2i] set for a malformed matrix.
 constexpr int kHistCopies = 16;
-static int count_raw_columns(cco_ctx *c, const std::vector<DevRaw> &raw, const std::vector<long long> &col_off, const cudaEvent_t *ready,
-                             int *verdict, int32_t *counts) {
+static bool hist_fits_smem(const cco_ctx *c, int32_t n_cols) { return ((size_t)n_cols + 1) / 2 * 4 <= c->smem_optin; }
+static int count_raw_columns(cco_ctx *c, Arena &ar, const std::vector<DevRaw> &raw, const std::vector<long long> &col_off, const cudaEvent_t *ready,
+                             int *verdict, int32_t **counts_out) {
   cudaStream_t s = c->stream;
   const int n_mats = (int)raw.size();
   const long long total_cols = col_off[n_mats];
   const long long copy_stride = std::max<long long>(total_cols, 1);
-  for (int i = 0; i < n_mats; ++i) {
-    if (ready) CK(cudaStreamWaitEvent(s, ready[i], 0));  // matrix i has landed (async upload: later ones may still be in flight)
-    if (raw[i].n_rows == 0) continue;
-    // CCO_FLAG_ASSUME_CANONICAL skips the canonicalisation, not the safety net: a malformed matrix still fails the call
-    // (until the verdict is read, the histogram skips ids outside the column space and the sampler keeps nothing)
+  bool copies = false;
+  for (int i = 0; i < n_mats; ++i) copies = copies || (raw[i].n_rows > 0 && !hist_fits_smem(c, raw[i].n_cols));
+  const int n_copies = copies ? kHistCopies : 1;
+  int32_t *counts;
+  CKR(ar.alloc(&counts, (size_t)copy_stride * n_copies));
+  CK(cudaMemsetAsync(counts, 0, sizeof(int32_t) * (size_t)copy_stride * n_copies, s));
+  *counts_out = counts;
+  // shared-memory path: CTAs of a batch go to its matrices in proportion to their entries, each at least
+  // kHistMinEntries, so that no CTA spends more time zeroing and flushing its counters than counting
+  std::vector<int> fit;
+  for (int i = 0; i < n_mats; ++i)
+    if (raw[i].n_rows > 0 && hist_fits_smem(c, raw[i].n_cols)) fit.push_back(i);
+  for (size_t b0 = 0; b0 < fit.size(); b0 += kHistSegs) {
+    const size_t b1 = std::min(fit.size(), b0 + kHistSegs);
+    HistBatch hb{};
+    long long nnz_sum = 0;
+    int32_t max_cols = 0;
+    for (size_t t = b0; t < b1; ++t) {
+      nnz_sum += raw[fit[t]].nnz;
+      max_cols = std::max(max_cols, raw[fit[t]].n_cols);
+    }
+    const size_t smem = ((size_t)max_cols + 1) / 2 * 4;
+    const int per_sm = std::max(1, std::min<int>(2048 / kHistThreads, (int)(c->smem_optin / std::max<size_t>(smem + 1024, 1))));
+    const long long target = (long long)c->sm_count * per_sm;
+    for (size_t t = b0; t < b1; ++t) {
+      const int i = fit[t];
+      if (ready) CK(cudaStreamWaitEvent(s, ready[i], 0));   // async upload: matrix i has landed
+      // CCO_FLAG_ASSUME_CANONICAL skips the canonicalisation, not the safety net: a malformed matrix still fails the call
+      // (until the verdict is read, the counts skip ids outside the column space and the sampler keeps nothing)
+      const long long share = nnz_sum > 0 ? (target * raw[i].nnz + nnz_sum - 1) / nnz_sum : 1;
+      const long long need = (raw[i].nnz + kHistMinEntries - 1) / kHistMinEntries;
+      HistSeg &g = hb.seg[hb.n++];
+      g.col = raw[i].col + raw[i].q_base;
+      g.rp = raw[i].rp;
+      g.nnz = raw[i].nnz;
+      g.n_rows = raw[i].n_rows;
+      g.q_lo = raw[i].q_base;
+      g.q_hi = raw[i].q_base + raw[i].nnz;
+      g.counts = counts + col_off[i];
+      g.verdict = verdict ? verdict + 2 * i : nullptr;
+      g.n_cols = raw[i].n_cols;
+      g.cta0 = hb.cta_end;
+      hb.cta_end += (int32_t)std::max(1LL, std::min(share, need));
+    }
+    CK(cudaFuncSetAttribute(k_col_counts_smem, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k_col_counts_smem<<<hb.cta_end, kHistThreads, smem, s>>>(hb);
+    c->launches++;
+  }
+  for (int i = 0; i < n_mats && copies; ++i) {
+    if (raw[i].n_rows == 0 || hist_fits_smem(c, raw[i].n_cols)) continue;
+    if (ready) CK(cudaStreamWaitEvent(s, ready[i], 0));
     int *v = verdict ? verdict + 2 * i : nullptr;
     if (v) {
       k_check_row_ptr<<<grid_for(raw[i].n_rows, 256, c->sm_count), 256, 0, s>>>(raw[i].n_rows, raw[i].rp, raw[i].q_base, raw[i].q_base + raw[i].nnz, v);
@@ -584,10 +632,12 @@ static int count_raw_columns(cco_ctx *c, const std::vector<DevRaw> &raw, const s
       c->launches++;
     }
   }
-  if (total_cols > 0) {
+  if (copies) {
     k_sum_copies<<<grid_for(total_cols, 256, c->sm_count), 256, 0, s>>>(total_cols, kHistCopies, copy_stride, counts);
     c->launches++;
   }
+  if (ready)   // every block has landed before anything after the counts reads it (also the ones with no rows)
+    for (int i = 0; i < n_mats; ++i) CK(cudaStreamWaitEvent(s, ready[i], 0));
   return CCO_OK;
 }
 
@@ -1439,13 +1489,11 @@ static int train_dataset(cco_ctx *c, const cco_dataset *ds, const cco_indicator_
   const long long copy_stride = std::max<long long>(total_cols, 1);
   int32_t *raw_counts, *marg_all;
   int *d_check;
-  CKR(ar.alloc(&raw_counts, (size_t)copy_stride * kHistCopies));
   CKR(ar.alloc(&marg_all, (size_t)copy_stride));
   CKR(ar.alloc(&d_check, 2 * n_mats));
-  CK(cudaMemsetAsync(raw_counts, 0, sizeof(int32_t) * (size_t)copy_stride * kHistCopies, s));
   CK(cudaMemsetAsync(marg_all, 0, sizeof(int32_t) * (size_t)copy_stride, s));
   CK(cudaMemsetAsync(d_check, 0, sizeof(int) * 2 * n_mats, s));
-  CKR(count_raw_columns(c, raw, col_off, ds->ready.data(), ds->validated ? nullptr : d_check, raw_counts));
+  CKR(count_raw_columns(c, ar, raw, col_off, ds->ready.data(), ds->validated ? nullptr : d_check, &raw_counts));
   CK(mark(0));
   if (c->world > 1) {
     if (total_cols > 0)
@@ -1485,7 +1533,8 @@ static int train_dataset(cco_ctx *c, const cco_dataset *ds, const cco_indicator_
     ar.release(marg_pad);
   }
   CK(cudaMemcpyAsync(cursor, at_ptr, sizeof(uint32_t) * ((size_t)n_items_a + 1), cudaMemcpyDeviceToDevice, s));
-  k_transpose_scatter<<<grid_for(n_users * kSG, 256, c->sm_count), 256, 0, s>>>(n_users, dm[0].rp, dm[0].col, cursor, at_users);
+  k_transpose_entries<<<grid_for((ds->nnz[0] + kSampleChunk - 1) / kSampleChunk * 32, 256, c->sm_count), 256, 0, s>>>(n_users, dm[0].rp,
+                                                                                                                     dm[0].col, cursor, at_users);
   c->launches++;
   for (int i = 0; i < n_mats; ++i)
     if (dm[i].n_cols > 0) {
@@ -4798,15 +4847,12 @@ int cco_debug_downsample(cco_ctx_t *c, const cco_csr_t *m, int32_t max_interacti
   raw[0].rp = ds->rp[0]; raw[0].col = ds->col[0];
   // the raw counts and the verdict exactly as the train makes them (count_raw_columns)
   const std::vector<long long> col_off = {0, m->n_cols};
-  const int32_t width = std::max<int32_t>(m->n_cols, 1);
   int32_t *counts;
   int *d_check;
-  CKR(ar.alloc(&counts, (size_t)width * kHistCopies));
   CKR(ar.alloc(&d_check, 2));
-  CK(cudaMemsetAsync(counts, 0, sizeof(int32_t) * (size_t)width * kHistCopies, c->stream));
   CK(cudaMemsetAsync(d_check, 0, sizeof(int) * 2, c->stream));
   int *verdict = ds->validated ? nullptr : d_check;
-  CKR(count_raw_columns(c, raw, col_off, ds->ready.data(), verdict, counts));
+  CKR(count_raw_columns(c, ar, raw, col_off, ds->ready.data(), verdict, &counts));
   DevMat dm;
   CKR(downsample_device(c, ar, raw[0], verdict, counts, max_interactions, seed, flags, &dm));
   std::vector<uint32_t> rp32((size_t)m->n_rows + 1);
@@ -4930,11 +4976,8 @@ int cco_debug_cooccurrence(cco_ctx_t *c, const cco_csr_t *a, const cco_csr_t *b,
   }
   // identity "downsample" (m = INT_MAX) gives the device CSR + marginals; raw counts as the train makes them
   const std::vector<long long> col_off = {0, raw[0].n_cols, (long long)raw[0].n_cols + raw[1].n_cols};
-  const long long width = std::max<long long>(col_off[2], 1);
   int32_t *counts;
-  CKR(ar.alloc(&counts, (size_t)width * kHistCopies));
-  CK(cudaMemsetAsync(counts, 0, sizeof(int32_t) * (size_t)width * kHistCopies, s));
-  CKR(count_raw_columns(c, raw, col_off, ds->ready.data(), nullptr, counts));   // (uploaded with validation + canonicalisation)
+  CKR(count_raw_columns(c, ar, raw, col_off, ds->ready.data(), nullptr, &counts));   // (uploaded with validation + canonicalisation)
   std::vector<DevMat> dm(2);
   for (int i = 0; i < 2; ++i) CKR(downsample_device(c, ar, raw[i], nullptr, counts + col_off[i], 0x7fffffff, 0, 0, &dm[i]));
   const int32_t n_items_a = dm[0].n_cols;
@@ -4950,7 +4993,8 @@ int cco_debug_cooccurrence(cco_ctx_t *c, const cco_csr_t *a, const cco_csr_t *b,
   CK(cudaMemsetAsync(marg_pad + n_items_a, 0, 4, s));
   CKR(exclusive_sum(c, ar, marg_pad, at_ptr, (long long)n_items_a + 1));
   CK(cudaMemcpyAsync(cursor, at_ptr, sizeof(uint32_t) * ((size_t)n_items_a + 1), cudaMemcpyDeviceToDevice, s));
-  k_transpose_scatter<<<grid_for(a->n_rows * kSG, 256, c->sm_count), 256, 0, s>>>(a->n_rows, dm[0].rp, dm[0].col, cursor, at_users);
+  k_transpose_entries<<<grid_for((raw[0].nnz + kSampleChunk - 1) / kSampleChunk * 32, 256, c->sm_count), 256, 0, s>>>(a->n_rows, dm[0].rp,
+                                                                                                                     dm[0].col, cursor, at_users);
   if (n_items_a > 0) k_max_i32<<<grid_for(n_items_a, 256, c->sm_count, 2), 256, 0, s>>>(n_items_a, dm[0].marg, d_max);
   if (dm[1].n_cols > 0) k_max_i32<<<grid_for(dm[1].n_cols, 256, c->sm_count, 2), 256, 0, s>>>(dm[1].n_cols, dm[1].marg, d_max + 1);
   int32_t max_marg_ab[2] = {0, 0};

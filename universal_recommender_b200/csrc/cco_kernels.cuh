@@ -6,7 +6,7 @@
 //   H2 sampleDownAndBinarize   -> k_downsample_count / k_downsample_write (row ranges: whole matrix or a rank's user block)
 //   H3 numNonZeroElementsPerColumn -> k_col_histogram (raw, before the allreduce), k_downsample_count or
 //                                 k_col_histogram_u32 (post-sample)
-//   `drmA.t`                   -> k_transpose_scatter
+//   `drmA.t`                   -> k_transpose_entries (cco_sampler.cuh)
 //   scheduling                 -> k_row_work, k_bin_bounds, k_partition_rows; column order of B' k_col_order_init /
 //                                 k_col_order / k_relabel_cols; per-column LLR constants k_col_terms
 //   H4 A'^T B' counts, H5 LLR, H6 top-k -> k_rows<GROUP, DENSE> (one fused kernel, nothing materialised)
@@ -347,18 +347,6 @@ __global__ void k_pack_blocks(int world, long long S, long long U, long long cap
     const uint32_t lo = new_ptr[u0], hi = new_ptr[u1];
     const int32_t *src = gathered + (long long)q * cap;
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < hi - lo; i += gridDim.x * blockDim.x) new_col[lo + i] = src[i];
-  }
-}
-
-// `drmA.t`: scatter users into per-item lists (order inside a list is irrelevant to the integer counts)
-__global__ void k_transpose_scatter(long long n_rows, const uint32_t *__restrict__ rp, const int32_t *__restrict__ col,
-                                    uint32_t *__restrict__ cursor, int32_t *__restrict__ users) {
-  const int lane = threadIdx.x % kSG;
-  long long row = (blockIdx.x * (long long)blockDim.x + threadIdx.x) / kSG;
-  const long long stride = (long long)gridDim.x * blockDim.x / kSG;
-  for (; row < n_rows; row += stride) {
-    uint32_t s = rp[row], e = rp[row + 1];
-    for (uint32_t q = s + lane; q < e; q += kSG) users[atomicAdd(&cursor[col[q]], 1u)] = (int32_t)row;
   }
 }
 

@@ -17,12 +17,12 @@
 //   * the owner lane counts the kept entries of its row from the ballot and a lane-range mask -- no shuffles, no atomics
 //     inside the chunk; one atomicAdd per (row, window) when the window slides or the chunk ends (rows may straddle chunks).
 // Every lane does useful work on every entry, rows of any length are split evenly over warps, and the kernel only
-// dereferences entry offsets inside [q_lo, q_hi): a malformed row_ptr (reported by k_check_row_ptr) cannot send it out of bounds.
+// dereferences entry offsets inside [q_lo, q_hi): a malformed row_ptr (reported by count_raw_columns) cannot send it out of bounds.
 // Pass 2 is an order-preserving stream compaction by the keep bytes (cub::DeviceSelect::Flagged in cco_api.cu): kept
 // entries keep their global order, so their rank inside the block is their offset from the block's first kept entry.
 //
-// These kernels supersede k_downsample_count / k_downsample_write, and k_col_histogram_flat (the raw counts of the train and
-// of every debug entry, cco_api.cu count_raw_columns) supersedes k_col_histogram; the old ones stay in cco_kernels.cuh
+// These kernels supersede k_downsample_count / k_downsample_write, and k_col_counts_smem / k_col_histogram_flat (the raw
+// counts of the train and of every debug entry, cco_api.cu count_raw_columns) supersede k_col_histogram; the old ones stay in cco_kernels.cuh
 // unreferenced: bench.py names the row-kernel build a line was measured on by that file's hash (source_build_id).
 #pragma once
 
@@ -36,12 +36,13 @@ namespace cco {
 constexpr int kSampleChunk = 256;   // stored entries per warp visit
 
 // largest r in [0, n_rows) with rp[r] <= q (the row holding entry q when row_ptr is monotone); warp-uniform
-__device__ __forceinline__ long long warp_find_row(const long long *__restrict__ rp, long long n_rows, long long q, int lane) {
+template <typename P>
+__device__ __forceinline__ long long warp_find_row(const P *__restrict__ rp, long long n_rows, long long q, int lane) {
   long long lo = 0, hi = n_rows;
   while (hi - lo > 1) {
     const long long step = (hi - lo + 31) / 32;
     const long long p = lo + lane * step;
-    const bool ok = p < hi && rp[p] <= q;
+    const bool ok = p < hi && (long long)rp[p] <= q;
     const unsigned b = __ballot_sync(0xffffffffu, ok) | 1u;   // lane 0 probes rp[lo] <= q, the loop invariant
     const int top = 31 - __clz(b);
     lo += top * step;
@@ -53,7 +54,7 @@ __device__ __forceinline__ long long warp_find_row(const long long *__restrict__
 __global__ void __launch_bounds__(256) k_sample_count(long long n_rows, long long row_base, const long long *__restrict__ rp,
                                                       const int32_t *__restrict__ col, int32_t n_cols, long long q_lo, long long q_hi,
                                                       const unsigned long long *__restrict__ col_thr, int32_t m, int32_t seed, uint32_t flags,
-                                                      const int *__restrict__ bad /* nullable: the validation verdict (k_check_row_ptr, k_col_histogram_flat) */,
+                                                      const int *__restrict__ bad /* nullable: the validation verdict (count_raw_columns) */,
                                                       uint32_t *__restrict__ kept_per_row /* zeroed */, int32_t *__restrict__ new_counts,
                                                       uint8_t *__restrict__ keep_flag) {
   const int lane = threadIdx.x & 31;
@@ -119,7 +120,7 @@ __global__ void __launch_bounds__(256) k_sample_count(long long n_rows, long lon
         const bool real_row = base + idx < n_rows;   // an entry past the last row's end (malformed row_ptr) is dropped
         bool keep = false;
         if (here) {
-          // (ids outside [0, n_cols) belong to a malformed matrix: dropped here, reported by k_col_histogram_flat)
+          // (ids outside [0, n_cols) belong to a malformed matrix: dropped here, reported by count_raw_columns)
           keep = real_row && (uint32_t)j < (uint32_t)n_cols && keep_entry_thr(t_row, t_col, x_row, (uint32_t)j);
           keep_flag[q - q_lo] = keep ? 1 : 0;   // pass 2 compacts by these decisions
           if (keep && new_counts) atomicAdd(&new_counts[j], 1);
@@ -196,6 +197,116 @@ __global__ void k_col_histogram_flat(long long n, const int32_t *__restrict__ co
     }
   }
   if (flags && bad) atomicOr(&flags[0], 1);
+}
+
+// ---- `drmA.t`, entry-parallel ----------------------------------------------------------------------------------------------
+// users[cursor[j]++] = u for every entry (u, j) of the sampled primary matrix.  A warp walks chunks of kSampleChunk
+// entries with k_sample_count's window of 32 rows (lane i holds the end of row base + i), so every lane scatters one
+// entry per batch whatever the row lengths (about 5 kept entries per user at C3).  The order of users inside an item's
+// list is not fixed; nothing downstream depends on it.
+__global__ void __launch_bounds__(256) k_transpose_entries(long long n_rows, const uint32_t *__restrict__ rp, const int32_t *__restrict__ col,
+                                                           uint32_t *__restrict__ cursor, int32_t *__restrict__ users) {
+  if (n_rows <= 0) return;
+  const int lane = threadIdx.x & 31;
+  const long long warp = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5;
+  const long long n_warps = ((long long)gridDim.x * blockDim.x) >> 5;
+  const long long nnz = rp[n_rows];
+  const long long n_chunks = (nnz + kSampleChunk - 1) / kSampleChunk;
+  for (long long chunk = warp; chunk < n_chunks; chunk += n_warps) {
+    const long long Q0 = chunk * kSampleChunk;
+    const long long Q1 = Q0 + kSampleChunk < nnz ? Q0 + kSampleChunk : nnz;
+    long long base = warp_find_row(rp, n_rows, Q0, lane);
+    long long end_i = base + lane < n_rows ? (long long)rp[base + lane + 1] : 0x7fffffffffffffffLL;
+    for (long long qb = Q0; qb < Q1; qb += 32) {
+      const long long q = qb + lane;
+      bool pending = q < Q1;
+      const int32_t j = pending ? col[q] : 0;
+      while (true) {
+        int idx = 0;   // rows of the window that end at or before q
+#pragma unroll
+        for (int step = 16; step > 0; step >>= 1) {
+          const long long v = __shfl_sync(0xffffffffu, end_i, idx + step - 1);
+          if (v <= q) idx += step;
+        }
+        if (__shfl_sync(0xffffffffu, end_i, idx & 31) <= q) idx += 1;
+        const bool here = pending && idx < 32;
+        if (here) users[atomicAdd(&cursor[j], 1u)] = (int32_t)(base + idx);
+        pending = pending && !here;
+        if (!__any_sync(0xffffffffu, pending)) break;
+        base += 32;   // entries of rows past the window (a well-formed row_ptr: they lie in rows < n_rows)
+        end_i = base + lane < n_rows ? (long long)rp[base + lane + 1] : 0x7fffffffffffffffLL;
+      }
+    }
+  }
+}
+
+// ---- raw column counts in shared memory, one launch over a batch of matrices ----------------------------------------------
+// When a matrix's column space fits a CTA's shared memory as 16-bit counters (n_cols <= ~116 K on H100), each CTA counts
+// an even slice of its matrix's entries privately and adds its counters to the global counts once, at the end: Zipf-hot
+// columns cost shared-memory atomics instead of contended L2 atomics, and nothing is replicated or summed afterwards.
+// A counter that reaches 2^15 hands 2^15 to the global count at once (hist_add), so no 16-bit counter can overflow
+// whatever the slice length.  The same CTAs check their share of the matrix's row_ptr (k_check_row_ptr's test).
+constexpr int kHistSegs = 8;                     // matrices per launch
+constexpr int kHistThreads = 1024;
+constexpr long long kHistMinEntries = 1 << 16;   // entries per CTA at least: zeroing and flushing cost ~n_cols / CTA
+struct HistSeg {
+  const int32_t *col;   // the block's first entry
+  const long long *rp;  // the block's row_ptr (n_rows + 1 values in [q_lo, q_hi] when well formed)
+  long long nnz, n_rows, q_lo, q_hi;
+  int32_t *counts;      // the matrix's raw counts: atomicAdd
+  int *verdict;         // nullable: [0] |= malformed
+  int32_t n_cols;
+  int32_t cta0;         // first CTA of the matrix; the next segment's cta0 (or HistBatch::cta_end) ends it
+};
+struct HistBatch {
+  HistSeg seg[kHistSegs];
+  int32_t n, cta_end;
+};
+__device__ __forceinline__ void hist_add(uint32_t *h, int32_t j, int32_t *g) {
+  const int sh = (j & 1) << 4;
+  const uint32_t old = atomicAdd(&h[j >> 1], 1u << sh);
+  if (((old >> sh) & 0xffffu) == 0x7fffu) {
+    // this add took the counter to 2^15: it moves 2^15 to the global count; the other threads of the CTA cannot add
+    // the further 2^15 that would overflow it before the subtraction lands
+    atomicAdd(&g[j], 0x8000);
+    atomicSub(&h[j >> 1], 0x8000u << sh);
+  }
+}
+__global__ void __launch_bounds__(kHistThreads) k_col_counts_smem(const HistBatch b) {
+  extern __shared__ uint32_t h[];   // two 16-bit counters per word: column j in word j / 2, half j % 2
+  int i = 0;
+  while (i + 1 < b.n && (int)blockIdx.x >= b.seg[i + 1].cta0) ++i;
+  const HistSeg &s = b.seg[i];
+  const long long n_ctas = (i + 1 < b.n ? b.seg[i + 1].cta0 : b.cta_end) - s.cta0, k = blockIdx.x - s.cta0;
+  const int words = (s.n_cols + 1) >> 1;
+  for (int w = threadIdx.x; w < words; w += blockDim.x) h[w] = 0;
+  int bad = 0;
+  if (s.verdict) {
+    const long long r1 = s.n_rows * (k + 1) / n_ctas;
+    for (long long r = s.n_rows * k / n_ctas + threadIdx.x; r < r1; r += blockDim.x) {
+      const long long a = s.rp[r], e = s.rp[r + 1];
+      if (e < a || a < s.q_lo || e > s.q_hi) bad = 1;
+    }
+  }
+  __syncthreads();
+  const long long q0 = s.nnz * k / n_ctas, q1 = s.nnz * (k + 1) / n_ctas;
+  constexpr int U = 8;   // loads in flight per thread
+  for (long long q = q0 + threadIdx.x; q < q1; q += U * kHistThreads) {
+    int32_t j[U];
+#pragma unroll
+    for (int u = 0; u < U; ++u) j[u] = q + u * kHistThreads < q1 ? s.col[q + u * kHistThreads] : -1;
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      if ((uint32_t)j[u] < (uint32_t)s.n_cols) hist_add(h, j[u], s.counts);
+      else if (q + u * kHistThreads < q1) bad = 1;   // outside [0, n_cols): skipped, reported
+    }
+  }
+  if (__syncthreads_or(bad) && threadIdx.x == 0 && s.verdict) atomicOr(&s.verdict[0], 1);
+  for (int w = threadIdx.x; w < words; w += blockDim.x) {
+    const uint32_t v = h[w];
+    if (v & 0xffffu) atomicAdd(&s.counts[2 * w], (int32_t)(v & 0xffffu));
+    if (v >> 16) atomicAdd(&s.counts[2 * w + 1], (int32_t)(v >> 16));
+  }
 }
 
 }  // namespace cco
