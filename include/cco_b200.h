@@ -146,9 +146,10 @@ typedef struct {
   float ms_indicator[16];       /* per indicator: row kernels only */
   int32_t n_kernel_launches;    /* kernels of this library launched by the call */
   int32_t n_mats;
-  /* breakdown of ms_prepare: [0] input check + raw column histogram  [1] all-reduce of the raw counts (multi-GPU)
+  /* breakdown of ms_prepare, the same stages on any number of GPUs (on one GPU the collectives and the pack do not run:
+   * [1] and [5] are empty and [3] holds the scans only): [0] input check + raw column histogram  [1] all-reduce of the raw counts
    * [2] sampleDownAndBinarize pass 1 (keep decisions, kept counts, marginals)  [3] kept-count all-gather + marginal
-   * all-reduce (multi-GPU) + row_ptr scans  [4] pass 2 (ordered write)  [5] column-block all-gather + pack (multi-GPU)
+   * all-reduce + row_ptr scans  [4] pass 2 (ordered write)  [5] column-block all-gather + pack
    * [6] transpose of A' + largest marginals */
   float ms_prep_stage[8];
 } cco_stats_t;

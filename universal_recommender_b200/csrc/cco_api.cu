@@ -234,7 +234,6 @@ struct cco_dataset {
   std::vector<long long *> rp;   // device, indexable by local row 0 .. n_local (values index `col`)
   std::vector<int32_t *> col;    // device, indexable by the values of rp
   std::vector<void *> rp_alloc, col_alloc;   // what to free (rp/col may be offset views of these)
-  std::vector<long long> block_cap;          // per matrix: largest raw entry count of any rank's user block
   std::vector<long long> q_lo, q_hi;         // per matrix: the offsets rp[0], rp[n_local] of the block (host-known)
   std::vector<cudaEvent_t> ready;  // per matrix: host->device copy finished (copy stream)
   bool h2d_pending = false;        // uploaded asynchronously: ms_h2d is read when the train joins
@@ -393,7 +392,6 @@ struct DevRaw {  // a block of user rows of a matrix as uploaded (int64 row_ptr 
   long long row_base = 0;   // global index of its first row
   int32_t n_cols = 0;
   long long nnz = 0;        // entries of the block
-  long long nnz_cap = 0;    // entries of the whole matrix (upper bound for the sampled matrix)
   long long q_base = 0;     // value of rp[0] (host-known): a rank's block keeps the caller's absolute offsets
   long long *rp = nullptr;  // indexable by local row
   int32_t *col = nullptr;   // indexable by rp values
@@ -446,6 +444,38 @@ static int bits_for(long long n) {
   return b;
 }
 
+// canonical CSR of n_rows rows from (row << 32 | col) keys: the n keys in k0 are radix-sorted on their low `bits` bits
+// (k1: scratch of n keys), the first n_valid sorted keys lose their duplicates into `col` and give `rp` (keys past
+// n_valid must sort after them).  The unique count comes back through the mailbox while the scatter runs.
+static int keys_to_csr(cco_ctx *c, Arena &ar, unsigned long long *k0, unsigned long long *k1, long long n, int bits, long long n_valid,
+                       long long n_rows, int32_t *col, long long *rp, long long *n_unique) {
+  cudaStream_t s = c->stream;
+  cub::DoubleBuffer<unsigned long long> db(k0, k1);
+  size_t tb = 0;
+  CK(cub::DeviceRadixSort::SortKeys(nullptr, tb, db, n, 0, bits, s));
+  void *tmp;
+  CKR(ar.alloc((char **)&tmp, tb));
+  CK(cub::DeviceRadixSort::SortKeys(tmp, tb, db, n, 0, bits, s));
+  ar.release(tmp);
+  unsigned long long *sorted = db.Current(), *other = db.Alternate();
+  uint32_t *flag, *pos;
+  CKR(ar.alloc(&flag, n_valid + 1));
+  CKR(ar.alloc(&pos, n_valid + 1));
+  CK(cudaMemsetAsync(flag + n_valid, 0, 4, s));
+  k_unique_flags<<<grid_for(n_valid, 256, c->sm_count), 256, 0, s>>>(n_valid, sorted, flag);
+  CKR(exclusive_sum(c, ar, flag, pos, n_valid + 1));
+  uint32_t nuq = 0;
+  CKR(mail_fetch(c, &nuq, pos + n_valid, 4));
+  k_unique_scatter<<<grid_for(n_valid, 256, c->sm_count), 256, 0, s>>>(n_valid, sorted, flag, pos, other, col);
+  CKR(mail_wait(c));
+  k_rowptr_from_keys<<<grid_for(n_rows + 1, 256, c->sm_count), 256, 0, s>>>(n_rows, nuq, other, rp);
+  c->launches += 3;
+  ar.release(flag);
+  ar.release(pos);
+  *n_unique = nuq;
+  return CCO_OK;
+}
+
 // canonicalisation slow path: sort (row,col) keys, drop duplicates, rebuild row_ptr
 static int canonicalize_device(cco_ctx *c, Arena &ar, DevRaw &m) {
   if (m.nnz == 0) return CCO_OK;
@@ -454,36 +484,13 @@ static int canonicalize_device(cco_ctx *c, Arena &ar, DevRaw &m) {
   CKR(ar.alloc(&k1, m.nnz));
   k_expand_keys<<<grid_for(m.n_rows * kSG, 256, c->sm_count), 256, 0, c->stream>>>(m.n_rows, m.rp, m.col, k0);
   c->launches++;
-  int row_bits = 1;
-  while ((1LL << row_bits) < m.n_rows) ++row_bits;
-  cub::DoubleBuffer<unsigned long long> db(k0, k1);
-  size_t tb = 0;
-  CK(cub::DeviceRadixSort::SortKeys(nullptr, tb, db, m.nnz, 0, 32 + row_bits, c->stream));
-  void *tmp;
-  CKR(ar.alloc((char **)&tmp, tb));
-  CK(cub::DeviceRadixSort::SortKeys(tmp, tb, db, m.nnz, 0, 32 + row_bits, c->stream));
-  ar.release(tmp);
-  unsigned long long *sorted = db.Current(), *other = db.Alternate();
-  uint32_t *flag, *pos;
-  CKR(ar.alloc(&flag, m.nnz + 1));
-  CKR(ar.alloc(&pos, m.nnz + 1));
-  CK(cudaMemsetAsync(flag + m.nnz, 0, 4, c->stream));
-  k_unique_flags<<<grid_for(m.nnz, 256, c->sm_count), 256, 0, c->stream>>>(m.nnz, sorted, flag);
-  c->launches++;
-  CKR(exclusive_sum(c, ar, flag, pos, m.nnz + 1));
-  uint32_t n_unique = 0;
-  CK(cudaMemcpyAsync(&n_unique, pos + m.nnz, 4, cudaMemcpyDeviceToHost, c->stream));
   // the canonical block is rewritten 0-based at the start of its own column storage
-  k_unique_scatter<<<grid_for(m.nnz, 256, c->sm_count), 256, 0, c->stream>>>(m.nnz, sorted, flag, pos, other, m.col + m.q_base);
-  CK(cudaStreamSynchronize(c->stream));
-  k_rowptr_from_keys<<<grid_for(m.n_rows + 1, 256, c->sm_count), 256, 0, c->stream>>>(m.n_rows, n_unique, other, m.rp);
-  c->launches += 2;
+  long long n_unique = 0;
+  CKR(keys_to_csr(c, ar, k0, k1, m.nnz, 32 + bits_for(m.n_rows), m.nnz, m.n_rows, m.col + m.q_base, m.rp, &n_unique));
   m.col += m.q_base;
   m.q_base = 0;
   m.nnz = n_unique;
   CK(cudaGetLastError());
-  ar.release(flag);
-  ar.release(pos);
   ar.release(k0);
   ar.release(k1);
   return CCO_OK;
@@ -641,51 +648,29 @@ static int count_raw_columns(cco_ctx *c, Arena &ar, const std::vector<DevRaw> &r
   return CCO_OK;
 }
 
-// sampleDownAndBinarize of one whole matrix on this GPU (raw column counts already final in raw_counts)
-static int downsample_device(cco_ctx *c, Arena &ar, const DevRaw &raw, const int *bad, const int32_t *raw_counts, int32_t m,
-                             int32_t seed, uint32_t flags, DevMat *out) {
-  out->n_rows = raw.n_rows;
-  out->n_cols = raw.n_cols;
-  uint32_t *kept;
-  CKR(ar.alloc(&kept, raw.n_rows + 1));
-  CKR(ar.alloc(&out->rp, raw.n_rows + 1));
-  if (!out->marg) CKR(ar.alloc(&out->marg, std::max<int32_t>(raw.n_cols, 1)));
-  CKR(ar.alloc(&out->col, std::max<long long>(raw.nnz, 1)));
-  CK(cudaMemsetAsync(out->marg, 0, sizeof(int32_t) * std::max<int32_t>(raw.n_cols, 1), c->stream));
-  CK(cudaMemsetAsync(kept, 0, sizeof(uint32_t) * ((size_t)raw.n_rows + 1), c->stream));
-  SampleScratch sc;
-  CKR(sample_scratch(c, ar, raw, raw_counts, m, &sc));
-  launch_count(c, raw, sc, m, seed, flags, bad, kept, out->marg);
-  CKR(exclusive_sum(c, ar, kept, out->rp, raw.n_rows + 1));
-  CKR(launch_write(c, ar, raw, sc, out->col));
-  CK(cudaGetLastError());
-  ar.release(kept);
-  ar.release(sc.col_thr);
-  ar.release(sc.keep);
-  return CCO_OK;
-}
-
 static int nccl_check(int rc, const char *what) {
   if (rc != 0) return set_error(CCO_E_NCCL, "%s: %s", what, g_nccl.GetErrorString(rc));
   return CCO_OK;
 }
 
-// Multi-GPU form of sampleDownAndBinarize.  Rank r holds (and samples) only its block of users.  Four collectives over
-// NVLink per train:
-//   (1) [caller] all-reduce of the raw column counts            -> the sampling rates
-//   (2) all-gather of the per-user kept counts (all matrices)   -> every rank scans the identical row_ptr
-//   (3) all-reduce of the post-sample column counts             -> marginals (nothing is re-counted on the gathered matrix)
-//   (4) all-gather of the sampled column blocks, each padded to the largest sampled block (the block sizes come from the
-//       scanned row_ptr through one mailbox record: an event wait, not a stream sync), then a pack kernel.
-static int downsample_sharded_all(cco_ctx *c, Arena &ar, const std::vector<DevRaw> &raw, const int *d_check /* [2 * n_mats] */,
-                                  const std::vector<long long> &block_cap,
-                                  long long U, const int32_t *raw_counts, int32_t *marg_all, const std::vector<long long> &col_off,
-                                  const cco_indicator_params_t *params, int32_t seed, uint32_t flags, std::vector<DevMat> &dm,
-                                  cudaEvent_t *stage_ev /* [4]: after pass 1, after collectives + scans, after pass 2, after gather + pack */) {
+// sampleDownAndBinarize of every matrix from the final (on several GPUs: all-reduced) raw column counts.  Rank r holds
+// and samples only its block of users; every rank ends with the whole sampled matrices.  The same steps on any number of
+// GPUs, each ending at one stage event:
+//   [0] pass 1 of every matrix: keep bytes, kept counts per user, post-sample column counts
+//   [1] on several GPUs the all-gather of the kept counts (all matrices) and the all-reduce of the post-sample column
+//       counts (the marginals: nothing is re-counted on the gathered matrix); then the row_ptr scan of every matrix
+//   [2] pass 2 of every matrix: on one GPU straight into the sampled matrix, on several into this rank's slot of a
+//       gather buffer.  NCCL's all-gather moves equal counts per rank, so the slots are padded to the largest SAMPLED
+//       block (2-3x smaller than the raw blocks at the 10M-user shapes); the block edges come from the scanned row_ptr
+//       through one mailbox record (an event wait, not a stream sync)
+//   [3] on several GPUs the all-gather of the column blocks and a pack kernel
+static int downsample_all(cco_ctx *c, Arena &ar, const std::vector<DevRaw> &raw, const int *d_check /* [2 * n_mats] */, long long U,
+                          const int32_t *raw_counts, int32_t *marg_all, const std::vector<long long> &col_off,
+                          const cco_indicator_params_t *params, int32_t seed, uint32_t flags, std::vector<DevMat> &dm,
+                          const cudaEvent_t *stage_ev /* [4] */) {
   cudaStream_t s = c->stream;
   const int W = c->world, r = c->rank, n_mats = (int)raw.size();
   const long long S = (U + W - 1) / W;
-  const long long row_base = raw[0].row_base;
   std::vector<uint32_t *> kept(n_mats, nullptr);
   std::vector<SampleScratch> sc(n_mats);
   for (int i = 0; i < n_mats; ++i) {
@@ -700,54 +685,61 @@ static int downsample_sharded_all(cco_ctx *c, Arena &ar, const std::vector<DevRa
     launch_count(c, raw[i], sc[i], params[i].max_interactions, seed, flags, d_check + 2 * i, kept[i], out->marg);
   }
   CK(cudaEventRecord(stage_ev[0], s));
-  if (S > 0) {
-    g_nccl.GroupStart();
-    for (int i = 0; i < n_mats; ++i) {
-      int rc = g_nccl.AllGather(kept[i] + (size_t)r * S, kept[i], (size_t)S, kNcclUint32, c->comm, s);
-      if (rc != 0) { g_nccl.GroupEnd(); return nccl_check(rc, "ncclAllGather(kept counts)"); }
+  if (W > 1) {
+    if (S > 0) {
+      g_nccl.GroupStart();
+      for (int i = 0; i < n_mats; ++i) {
+        int rc = g_nccl.AllGather(kept[i] + (size_t)r * S, kept[i], (size_t)S, kNcclUint32, c->comm, s);
+        if (rc != 0) { g_nccl.GroupEnd(); return nccl_check(rc, "ncclAllGather(kept counts)"); }
+      }
+      CKR(nccl_check(g_nccl.GroupEnd(), "ncclGroupEnd(kept counts)"));
     }
-    CKR(nccl_check(g_nccl.GroupEnd(), "ncclGroupEnd(kept counts)"));
+    if (col_off[n_mats] > 0)
+      CKR(nccl_check(g_nccl.AllReduce(marg_all, marg_all, (size_t)col_off[n_mats], kNcclInt32, kNcclSum, c->comm, s), "ncclAllReduce(marginals)"));
   }
-  if (col_off[n_mats] > 0)
-    CKR(nccl_check(g_nccl.AllReduce(marg_all, marg_all, (size_t)col_off[n_mats], kNcclInt32, kNcclSum, c->comm, s), "ncclAllReduce(marginals)"));
-  std::vector<int32_t *> gathered(n_mats, nullptr);
-  // NCCL's all-gather moves equal counts per rank.  The raw block size (host-known) would do as the padding, but after
-  // downsampling a block is 2-3x smaller than its raw size at the 10M-user shapes.
-  // The sampled block sizes sit in row_ptr on the device: one mailbox record per train brings them to the host (one event
-  // wait, no stream-wide sync) and the gather is padded to the largest SAMPLED block only.
   std::vector<uint32_t> edge((size_t)n_mats * (W + 1), 0);
   for (int i = 0; i < n_mats; ++i) {
     CKR(exclusive_sum(c, ar, kept[i], dm[i].rp, U + 1));
     ar.release(kept[i]);
-    for (int q = 0; q <= W; ++q) CKR(mail_fetch(c, &edge[(size_t)i * (W + 1) + q], dm[i].rp + std::min<long long>((long long)q * S, U), 4));
+    if (W > 1)
+      for (int q = 0; q <= W; ++q) CKR(mail_fetch(c, &edge[(size_t)i * (W + 1) + q], dm[i].rp + std::min<long long>((long long)q * S, U), 4));
   }
   CK(cudaEventRecord(stage_ev[1], s));
-  CKR(mail_wait(c));
+  if (W > 1) CKR(mail_wait(c));
   std::vector<long long> cap(n_mats, 0);
+  std::vector<int32_t *> gathered(n_mats, nullptr);
   for (int i = 0; i < n_mats; ++i) {
-    for (int q = 0; q < W; ++q) cap[i] = std::max<long long>(cap[i], (long long)edge[(size_t)i * (W + 1) + q + 1] - edge[(size_t)i * (W + 1) + q]);
-    CKR(ar.alloc(&dm[i].col, std::max<long long>(edge[(size_t)i * (W + 1) + W], 1)));
-    if (cap[i] == 0) continue;
-    CKR(ar.alloc(&gathered[i], (size_t)(cap[i] * W)));
-    // this rank's block goes straight into its slot of the gather buffer, relative to the block's first entry
-    CKR(launch_write(c, ar, raw[i], sc[i], gathered[i] + (size_t)r * cap[i]));
+    if (W == 1) {
+      CKR(ar.alloc(&dm[i].col, std::max<long long>(raw[i].nnz, 1)));
+      CKR(launch_write(c, ar, raw[i], sc[i], dm[i].col));
+    } else {
+      for (int q = 0; q < W; ++q) cap[i] = std::max<long long>(cap[i], (long long)edge[(size_t)i * (W + 1) + q + 1] - edge[(size_t)i * (W + 1) + q]);
+      CKR(ar.alloc(&dm[i].col, std::max<long long>(edge[(size_t)i * (W + 1) + W], 1)));
+      if (cap[i] > 0) {
+        CKR(ar.alloc(&gathered[i], (size_t)(cap[i] * W)));
+        // kept entries keep their order: this rank's block goes to its slot relative to the block's first entry
+        CKR(launch_write(c, ar, raw[i], sc[i], gathered[i] + (size_t)r * cap[i]));
+      }
+    }
     ar.release(sc[i].col_thr);
     ar.release(sc[i].keep);
   }
   CK(cudaEventRecord(stage_ev[2], s));
-  g_nccl.GroupStart();
-  for (int i = 0; i < n_mats; ++i) {
-    if (!gathered[i]) continue;
-    int rc = g_nccl.AllGather(gathered[i] + (size_t)r * cap[i], gathered[i], (size_t)cap[i], kNcclInt32, c->comm, s);
-    if (rc != 0) { g_nccl.GroupEnd(); return nccl_check(rc, "ncclAllGather(column blocks)"); }
-  }
-  CKR(nccl_check(g_nccl.GroupEnd(), "ncclGroupEnd(column blocks)"));
-  for (int i = 0; i < n_mats; ++i) {
-    if (!gathered[i]) continue;
-    dim3 grid((unsigned)std::max(1, std::min(c->sm_count * 8 / W, 1024)), (unsigned)W);
-    k_pack_blocks<<<grid, 256, 0, s>>>(W, S, U, cap[i], dm[i].rp, gathered[i], dm[i].col);
-    c->launches++;
-    ar.release(gathered[i]);
+  if (W > 1) {
+    g_nccl.GroupStart();
+    for (int i = 0; i < n_mats; ++i) {
+      if (!gathered[i]) continue;
+      int rc = g_nccl.AllGather(gathered[i] + (size_t)r * cap[i], gathered[i], (size_t)cap[i], kNcclInt32, c->comm, s);
+      if (rc != 0) { g_nccl.GroupEnd(); return nccl_check(rc, "ncclAllGather(column blocks)"); }
+    }
+    CKR(nccl_check(g_nccl.GroupEnd(), "ncclGroupEnd(column blocks)"));
+    for (int i = 0; i < n_mats; ++i) {
+      if (!gathered[i]) continue;
+      dim3 grid((unsigned)std::max(1, std::min(c->sm_count * 8 / W, 1024)), (unsigned)W);
+      k_pack_blocks<<<grid, 256, 0, s>>>(W, S, U, cap[i], dm[i].rp, gathered[i], dm[i].col);
+      c->launches++;
+      ar.release(gathered[i]);
+    }
   }
   CK(cudaEventRecord(stage_ev[3], s));
   CK(cudaGetLastError());
@@ -1291,11 +1283,25 @@ static void dataset_release(cco_dataset *d) {
   delete d;
 }
 
+// the block of user rows of matrix i that the dataset holds
+static DevRaw block_of(const cco_dataset *d, int i) {
+  DevRaw r;
+  r.n_rows = d->n_local;
+  r.row_base = d->row_base;
+  r.n_cols = (int32_t)d->n_cols[i];
+  r.q_base = d->q_lo[i];
+  r.nnz = d->q_hi[i] - d->q_lo[i];
+  r.rp = d->rp[i];
+  r.col = d->col[i];
+  return r;
+}
+
 // device check of the uploaded block(s) + canonicalisation of unsorted / duplicated rows (synchronous).  In a multi-GPU
 // job the "malformed" verdict is all-reduced so that every rank fails (or proceeds) together.
 static int dataset_validate(cco_ctx *c, cco_dataset *d, bool canonicalise) {
   cudaStream_t s = c->stream;
   const int n_mats = d->n_mats;
+  mail_reset(c);   // the canonicalisation reads its unique counts through the mailbox
   Arena ar(s);
   int *d_flags;
   CKR(ar.alloc(&d_flags, 2 * n_mats));
@@ -1303,13 +1309,7 @@ static int dataset_validate(cco_ctx *c, cco_dataset *d, bool canonicalise) {
   for (int i = 0; i < n_mats; ++i) {
     CK(cudaStreamWaitEvent(s, d->ready[i], 0));
     if (d->n_local == 0) continue;
-    DevRaw r;
-    r.n_rows = d->n_local;
-    r.n_cols = (int32_t)d->n_cols[i];
-    r.q_base = d->q_lo[i];
-    r.nnz = d->q_hi[i] - d->q_lo[i];
-    r.rp = d->rp[i];
-    r.col = d->col[i];
+    const DevRaw r = block_of(d, i);
     HeavyRows hv;
     CKR(list_heavy_rows(c, ar, r, &hv));
     launch_check(c, r, hv, d_flags + 2 * i);
@@ -1326,14 +1326,7 @@ static int dataset_validate(cco_ctx *c, cco_dataset *d, bool canonicalise) {
     for (int i = 0; i < n_mats; ++i)
       if (h[2 * i + 1] && d->n_local > 0) {
         // (the flag is all-reduced: every rank canonicalises its own block, the blocks are independent)
-        DevRaw r;
-        r.n_rows = d->n_local;
-        r.row_base = d->row_base;
-        r.n_cols = (int32_t)d->n_cols[i];
-        r.q_base = d->q_lo[i];
-        r.nnz = d->q_hi[i] - d->q_lo[i];
-        r.rp = d->rp[i];
-        r.col = d->col[i];
+        DevRaw r = block_of(d, i);
         CKR(canonicalize_device(c, ar, r));
         d->col[i] = r.col;
         d->q_lo[i] = 0;
@@ -1364,7 +1357,6 @@ static int dataset_upload(cco_ctx *c, int32_t n_mats, const cco_csr_t *mats, uin
   d->col_alloc.assign(n_mats, nullptr);
   d->n_cols.assign(n_mats, 0);
   d->nnz.assign(n_mats, 0);
-  d->block_cap.assign(n_mats, 0);
   d->q_lo.assign(n_mats, 0);
   d->q_hi.assign(n_mats, 0);
   d->ready.assign(n_mats, nullptr);
@@ -1382,11 +1374,6 @@ static int dataset_upload(cco_ctx *c, int32_t n_mats, const cco_csr_t *mats, uin
     const cco_csr_t &m = mats[i];
     d->n_cols[i] = m.n_cols;
     d->nnz[i] = m.row_ptr[m.n_rows];
-    for (int q = 0; q < c->world; ++q) {
-      long long a0, a1;
-      user_block(d->n_users, c->world, q, &a0, &a1);
-      d->block_cap[i] = std::max<long long>(d->block_cap[i], m.row_ptr[a1] - m.row_ptr[a0]);
-    }
     const long long q0 = m.row_ptr[u_lo], q1 = m.row_ptr[u_hi];
     d->q_lo[i] = q0;
     d->q_hi[i] = q1;
@@ -1426,6 +1413,98 @@ static int dataset_upload(cco_ctx *c, int32_t n_mats, const cco_csr_t *mats, uin
   return CCO_OK;
 }
 
+// The train's preparation of the dataset's matrices on this rank: raw column counts and the malformed-input verdict,
+// sampleDownAndBinarize, the transpose of A' and the largest marginals.  c->ev[1] and c->ev[2] bracket it on the stream,
+// stage[k] ends cco_stats_t.ms_prep_stage[k].  It ends in the preparation's one host round trip: the packed-word check
+// of the indicators needs the largest marginals.
+struct Prepared {
+  std::vector<DevMat> dm;          // the sampled matrices, all users
+  uint32_t *at_ptr = nullptr;      // A'^T: [n_items_a + 1] offsets into at_users
+  int32_t *at_users = nullptr;
+  int32_t *raw_counts = nullptr;   // raw column counts, matrix i at the sum of the earlier matrices' n_cols
+  std::vector<int32_t> max_marg;   // largest post-sample column count per matrix
+  std::vector<uint32_t> nnz;       // entries per sampled matrix
+  cudaEvent_t stage[7] = {};
+};
+static int prepare(cco_ctx *c, Arena &ar, const cco_dataset *ds, const cco_indicator_params_t *params, int32_t seed, uint32_t flags,
+                   Prepared *p) {
+  cudaStream_t s = c->stream;
+  const int n_mats = ds->n_mats;
+  const long long n_users = ds->n_users;
+  std::vector<DevRaw> raw(n_mats);
+  for (int i = 0; i < n_mats; ++i) raw[i] = block_of(ds, i);
+  for (auto &e : p->stage) CKR(pooled_event(c, true, &e));
+  auto mark = [&](int k) { return cudaEventRecord(p->stage[k], s); };
+  CK(cudaEventRecord(c->ev[1], s));
+  nvtx_push("cco:prepare");
+  // raw column counts: this rank histograms its user block; ONE allreduce sums all matrices' counts
+  long long total_cols = 0;
+  std::vector<long long> col_off(n_mats + 1, 0);
+  for (int i = 0; i < n_mats; ++i) {
+    col_off[i] = total_cols;
+    total_cols += raw[i].n_cols;
+  }
+  col_off[n_mats] = total_cols;
+  const long long copy_stride = std::max<long long>(total_cols, 1);
+  int32_t *marg_all;
+  int *d_check;
+  CKR(ar.alloc(&marg_all, (size_t)copy_stride));
+  CKR(ar.alloc(&d_check, 2 * n_mats));
+  CK(cudaMemsetAsync(marg_all, 0, sizeof(int32_t) * (size_t)copy_stride, s));
+  CK(cudaMemsetAsync(d_check, 0, sizeof(int) * 2 * n_mats, s));
+  CKR(count_raw_columns(c, ar, raw, col_off, ds->ready.data(), ds->validated ? nullptr : d_check, &p->raw_counts));
+  CK(mark(0));
+  if (c->world > 1) {
+    if (total_cols > 0)
+      CKR(nccl_check(g_nccl.AllReduce(p->raw_counts, p->raw_counts, (size_t)total_cols, kNcclInt32, kNcclSum, c->comm, s), "ncclAllReduce(raw counts)"));
+    CKR(nccl_check(g_nccl.AllReduce(d_check, d_check, (size_t)(2 * n_mats), kNcclInt32, kNcclMax, c->comm, s), "ncclAllReduce(check flags)"));
+  }
+  CK(mark(1));
+  // sampleDownAndBinarize every matrix
+  std::vector<DevMat> &dm = p->dm;
+  dm.assign(n_mats, DevMat());
+  CKR(downsample_all(c, ar, raw, d_check, n_users, p->raw_counts, marg_all, col_off, params, seed, flags, dm, &p->stage[2]));
+  // `drmA.t`
+  const int32_t n_items_a = dm[0].n_cols;
+  uint32_t *cursor;
+  int32_t *d_max;
+  CKR(ar.alloc(&p->at_ptr, n_items_a + 1));
+  CKR(ar.alloc(&cursor, n_items_a + 1));
+  CKR(ar.alloc(&d_max, n_mats));
+  CKR(ar.alloc(&p->at_users, std::max<long long>(ds->nnz[0], 1)));
+  CK(cudaMemsetAsync(d_max, 0, 4 * (size_t)n_mats, s));
+  {
+    uint32_t *marg_pad;
+    CKR(ar.alloc(&marg_pad, n_items_a + 1));
+    CK(cudaMemcpyAsync(marg_pad, dm[0].marg, sizeof(int32_t) * (size_t)n_items_a, cudaMemcpyDeviceToDevice, s));
+    CK(cudaMemsetAsync(marg_pad + n_items_a, 0, 4, s));
+    CKR(exclusive_sum(c, ar, marg_pad, p->at_ptr, (long long)n_items_a + 1));
+    ar.release(marg_pad);
+  }
+  CK(cudaMemcpyAsync(cursor, p->at_ptr, sizeof(uint32_t) * ((size_t)n_items_a + 1), cudaMemcpyDeviceToDevice, s));
+  k_transpose_entries<<<grid_for((ds->nnz[0] + kSampleChunk - 1) / kSampleChunk * 32, 256, c->sm_count), 256, 0, s>>>(n_users, dm[0].rp,
+                                                                                                                     dm[0].col, cursor, p->at_users);
+  c->launches++;
+  for (int i = 0; i < n_mats; ++i)
+    if (dm[i].n_cols > 0) {
+      k_max_i32<<<grid_for(dm[i].n_cols, 256, c->sm_count, 2), 256, 0, s>>>(dm[i].n_cols, dm[i].marg, d_max + i);
+      c->launches++;
+    }
+  p->max_marg.assign(n_mats, 0);
+  p->nnz.assign(n_mats, 0);
+  std::vector<int> h_check(2 * n_mats, 0);
+  CKR(mail_fetch(c, p->max_marg.data(), d_max, 4 * (size_t)n_mats));
+  CKR(mail_fetch(c, h_check.data(), d_check, sizeof(int) * 2 * (size_t)n_mats));
+  for (int i = 0; i < n_mats; ++i) CKR(mail_fetch(c, &p->nnz[i], dm[i].rp + n_users, 4));
+  CK(mark(6));
+  CK(cudaEventRecord(c->ev[2], s));
+  nvtx_pop();
+  CKR(mail_wait(c));
+  for (int i = 0; i < n_mats; ++i)
+    if (h_check[2 * i]) return set_error(CCO_E_INVALID_ARG, "matrix %d: row_ptr not monotone or column index out of [0, n_cols)", i);
+  return CCO_OK;
+}
+
 // The whole hot path on this rank, for the block of users the dataset holds.
 static int train_dataset(cco_ctx *c, const cco_dataset *ds, const cco_indicator_params_t *params, int32_t seed, uint32_t flags,
                          cco_result **out) {
@@ -1461,108 +1540,20 @@ static int train_dataset(cco_ctx *c, const cco_dataset *ds, const cco_indicator_
   st.ms_h2d = ds->ms_h2d;
   const bool h2d_pending = ds->h2d_pending;
   const long long n_users = ds->n_users;
-  std::vector<DevRaw> raw(n_mats);
-  for (int i = 0; i < n_mats; ++i) {
-    raw[i].n_rows = ds->n_local;
-    raw[i].row_base = ds->row_base;
-    raw[i].n_cols = (int32_t)ds->n_cols[i];
-    raw[i].q_base = ds->q_lo[i];
-    raw[i].nnz = ds->q_hi[i] - ds->q_lo[i];   // entries of the block
-    raw[i].nnz_cap = ds->nnz[i];
-    raw[i].rp = ds->rp[i];
-    raw[i].col = ds->col[i];
-    st.nnz_in_total += ds->nnz[i];
-  }
-  CK(cudaEventRecord(c->ev[1], s));
-  nvtx_push("cco:prepare");
-  std::vector<cudaEvent_t> sev(8, nullptr);   // stage boundaries of the preparation (cco_stats_t.ms_prep_stage)
-  for (auto &e : sev) CKR(pooled_event(c, true, &e));
-  auto mark = [&](int k) { return cudaEventRecord(sev[k], s); };
-  // raw column counts: this rank histograms its user block; ONE allreduce sums all matrices' counts
-  long long total_cols = 0;
-  std::vector<long long> col_off(n_mats + 1, 0);
-  for (int i = 0; i < n_mats; ++i) {
-    col_off[i] = total_cols;
-    total_cols += raw[i].n_cols;
-  }
-  col_off[n_mats] = total_cols;
-  const long long copy_stride = std::max<long long>(total_cols, 1);
-  int32_t *raw_counts, *marg_all;
-  int *d_check;
-  CKR(ar.alloc(&marg_all, (size_t)copy_stride));
-  CKR(ar.alloc(&d_check, 2 * n_mats));
-  CK(cudaMemsetAsync(marg_all, 0, sizeof(int32_t) * (size_t)copy_stride, s));
-  CK(cudaMemsetAsync(d_check, 0, sizeof(int) * 2 * n_mats, s));
-  CKR(count_raw_columns(c, ar, raw, col_off, ds->ready.data(), ds->validated ? nullptr : d_check, &raw_counts));
-  CK(mark(0));
-  if (c->world > 1) {
-    if (total_cols > 0)
-      CKR(nccl_check(g_nccl.AllReduce(raw_counts, raw_counts, (size_t)total_cols, kNcclInt32, kNcclSum, c->comm, s), "ncclAllReduce(raw counts)"));
-    CKR(nccl_check(g_nccl.AllReduce(d_check, d_check, (size_t)(2 * n_mats), kNcclInt32, kNcclMax, c->comm, s), "ncclAllReduce(check flags)"));
-  }
-  CK(mark(1));
-  // sampleDownAndBinarize every matrix
-  std::vector<DevMat> dm(n_mats);
-  if (c->world > 1) {
-    CKR(downsample_sharded_all(c, ar, raw, d_check, ds->block_cap, n_users, raw_counts, marg_all, col_off, params, seed, flags, dm, &sev[2]));
-  } else {
-    for (int i = 0; i < n_mats; ++i) {
-      dm[i].marg = marg_all + col_off[i];
-      CKR(downsample_device(c, ar, raw[i], d_check + 2 * i, raw_counts + col_off[i], params[i].max_interactions, seed, flags, &dm[i]));
-    }
-    CK(mark(2));   // single GPU: both passes are booked on stage 2 ... 4 as one block
-    CK(mark(3));
-    CK(mark(4));
-    CK(mark(5));
-  }
-  // `drmA.t`
-  const int32_t n_items_a = dm[0].n_cols;
-  uint32_t *at_ptr, *cursor;
-  int32_t *at_users, *d_max;
-  CKR(ar.alloc(&at_ptr, n_items_a + 1));
-  CKR(ar.alloc(&cursor, n_items_a + 1));
-  CKR(ar.alloc(&d_max, n_mats));
-  CKR(ar.alloc(&at_users, std::max<long long>(ds->nnz[0], 1)));
-  CK(cudaMemsetAsync(d_max, 0, 4 * (size_t)n_mats, s));
-  {
-    uint32_t *marg_pad;
-    CKR(ar.alloc(&marg_pad, n_items_a + 1));
-    CK(cudaMemcpyAsync(marg_pad, dm[0].marg, sizeof(int32_t) * (size_t)n_items_a, cudaMemcpyDeviceToDevice, s));
-    CK(cudaMemsetAsync(marg_pad + n_items_a, 0, 4, s));
-    CKR(exclusive_sum(c, ar, marg_pad, at_ptr, (long long)n_items_a + 1));
-    ar.release(marg_pad);
-  }
-  CK(cudaMemcpyAsync(cursor, at_ptr, sizeof(uint32_t) * ((size_t)n_items_a + 1), cudaMemcpyDeviceToDevice, s));
-  k_transpose_entries<<<grid_for((ds->nnz[0] + kSampleChunk - 1) / kSampleChunk * 32, 256, c->sm_count), 256, 0, s>>>(n_users, dm[0].rp,
-                                                                                                                     dm[0].col, cursor, at_users);
-  c->launches++;
-  for (int i = 0; i < n_mats; ++i)
-    if (dm[i].n_cols > 0) {
-      k_max_i32<<<grid_for(dm[i].n_cols, 256, c->sm_count, 2), 256, 0, s>>>(dm[i].n_cols, dm[i].marg, d_max + i);
-      c->launches++;
-    }
-  std::vector<int32_t> max_marg(n_mats, 0);
-  std::vector<uint32_t> h_nnz(n_mats);
-  std::vector<int> h_check(2 * n_mats, 0);
-  CKR(mail_fetch(c, max_marg.data(), d_max, 4 * (size_t)n_mats));
-  CKR(mail_fetch(c, h_check.data(), d_check, sizeof(int) * 2 * (size_t)n_mats));
-  for (int i = 0; i < n_mats; ++i) CKR(mail_fetch(c, &h_nnz[i], dm[i].rp + n_users, 4));
-  CK(mark(6));
-  CK(cudaEventRecord(c->ev[2], s));
-  nvtx_pop();
-  CKR(mail_wait(c));   // the one host round trip of the preparation: the packed-word check needs the largest marginals
-  for (int i = 0; i < n_mats; ++i)
-    if (h_check[2 * i]) return set_error(CCO_E_INVALID_ARG, "matrix %d: row_ptr not monotone or column index out of [0, n_cols)", i);
-  for (int i = 0; i < n_mats && i < 16; ++i) st.nnz_downsampled[i] = h_nnz[i];
+  for (int i = 0; i < n_mats; ++i) st.nnz_in_total += ds->nnz[i];
+  Prepared p;
+  CKR(prepare(c, ar, ds, params, seed, flags, &p));
+  for (int i = 0; i < n_mats && i < 16; ++i) st.nnz_downsampled[i] = p.nnz[i];
 
   // indicators, software-pipelined: indicator i+1 is on the stream before the host waits for indicator i's record
+  const int32_t n_items_a = p.dm[0].n_cols;
   std::vector<IndicatorOut> io(n_mats);
   std::vector<cudaEvent_t> ev_rows(2 * n_mats, nullptr);
   for (auto &e : ev_rows) CKR(pooled_event(c, true, &e));
   for (int i = 0; i < n_mats; ++i) {
     nvtx_push("cco:indicator");
-    CKR(enqueue_indicator(c, ar, at_ptr, at_users, n_items_a, dm[0].marg, max_marg[0], max_marg[i], dm[i], n_users, i == 0, params[i],
-                          flags, false, c->ev[2], ev_rows[2 * i], ev_rows[2 * i + 1], &ist[i]));
+    CKR(enqueue_indicator(c, ar, p.at_ptr, p.at_users, n_items_a, p.dm[0].marg, p.max_marg[0], p.max_marg[i], p.dm[i], n_users, i == 0,
+                          params[i], flags, false, c->ev[2], ev_rows[2 * i], ev_rows[2 * i + 1], &ist[i]));
     nvtx_pop();
     if (i > 0) CKR(finish_indicator(c, &ist[i - 1], flags, i - 1, &res->mats[i - 1], &io[i - 1]));
   }
@@ -1580,8 +1571,8 @@ static int train_dataset(cco_ctx *c, const cco_dataset *ds, const cco_indicator_
     CK(cudaEventElapsedTime(&st.ms_indicator[i], ev_rows[2 * i], ev_rows[2 * i + 1]));
   }
   if (h2d_pending) CK(cudaEventElapsedTime(&st.ms_h2d, c->ev[6], c->ev[7]));
-  CK(cudaEventElapsedTime(&st.ms_prep_stage[0], c->ev[1], sev[0]));
-  for (int k = 1; k <= 6; ++k) CK(cudaEventElapsedTime(&st.ms_prep_stage[k], sev[k - 1], sev[k]));
+  CK(cudaEventElapsedTime(&st.ms_prep_stage[0], c->ev[1], p.stage[0]));
+  for (int k = 1; k <= 6; ++k) CK(cudaEventElapsedTime(&st.ms_prep_stage[k], p.stage[k - 1], p.stage[k]));
   CK(cudaEventElapsedTime(&st.ms_prepare, c->ev[1], c->ev[2]));
   CK(cudaEventElapsedTime(&st.ms_cooccurrence, c->ev[2], c->ev[3]));
   CK(cudaEventElapsedTime(&st.ms_total, c->ev[1], c->ev[3]));
@@ -1961,7 +1952,6 @@ static cco_dataset *ingest_dataset_new(cco_ctx *c, int n_types) {
   d->col.assign(n_types, nullptr);
   d->rp_alloc.assign(n_types, nullptr);
   d->col_alloc.assign(n_types, nullptr);
-  d->block_cap.assign(n_types, 0);
   d->q_lo.assign(n_types, 0);
   d->q_hi.assign(n_types, 0);
   d->n_cols.assign(n_types, 0);
@@ -1988,63 +1978,29 @@ static int ingest_csr(cco_ctx *c, Arena &ar, cco_dataset *d, int t, long long ne
   d->col_alloc[t] = p;
   CK(cudaEventCreateWithFlags(&d->ready[t], cudaEventDisableTiming));
   long long n_unique = 0;
-  if (kept > 0) {
-    int row_bits = 1;
-    while ((1LL << row_bits) < (long long)n_users) ++row_bits;
-    cub::DoubleBuffer<unsigned long long> db(k0, k1);
-    size_t tb = 0;
-    // dropped events carry the key ~0 and sort to the end: all 64 bits take part
-    CK(cub::DeviceRadixSort::SortKeys(nullptr, tb, db, (long long)ne, 0, 64, s));
-    void *tmp;
-    CKR(ar.alloc((char **)&tmp, tb));
-    CK(cub::DeviceRadixSort::SortKeys(tmp, tb, db, (long long)ne, 0, 64, s));
-    ar.release(tmp);
-    unsigned long long *sorted = db.Current(), *other = db.Alternate();
-    uint32_t *flag, *pos;
-    CKR(ar.alloc(&flag, kept + 1));
-    CKR(ar.alloc(&pos, kept + 1));
-    CK(cudaMemsetAsync(flag + kept, 0, 4, s));
-    k_unique_flags<<<grid_for((long long)kept, 256, c->sm_count), 256, 0, s>>>((long long)kept, sorted, flag);
-    CKR(exclusive_sum(c, ar, flag, pos, (long long)kept + 1));
-    uint32_t nuq = 0;
-    CKR(mail_fetch(c, &nuq, pos + kept, 4));
-    k_unique_scatter<<<grid_for((long long)kept, 256, c->sm_count), 256, 0, s>>>((long long)kept, sorted, flag, pos, other, d->col[t]);
-    CKR(mail_wait(c));
-    n_unique = nuq;
-    k_rowptr_from_keys<<<grid_for((long long)n_users + 1, 256, c->sm_count), 256, 0, s>>>((long long)n_users, n_unique, other, d->rp[t]);
-    c->launches += 3;
-    ar.release(flag);
-    ar.release(pos);
-  } else {
+  if (kept > 0)   // dropped events carry the key ~0 and sort to the end: all 64 bits take part
+    CKR(keys_to_csr(c, ar, k0, k1, ne, 64, (long long)kept, n_users, d->col[t], d->rp[t], &n_unique));
+  else
     CK(cudaMemsetAsync(d->rp[t], 0, sizeof(int64_t) * ((size_t)n_users + 1), s));
-  }
   d->nnz[t] = n_unique;
   CK(cudaEventRecord(d->ready[t], s));
   return CCO_OK;
 }
 
 // every rank of a multi-GPU job builds the whole matrices (the events are all here) and then works on its block of
-// users like an uploaded dataset does; the block sizes (padding of the column-block all-gather) come from row_ptr
+// users like an uploaded dataset does; the block's entry offsets come from row_ptr
 static int ingest_blocks(cco_ctx *c, cco_dataset *d, uint32_t n_users) {
   const int n_types = d->n_mats;
   long long u_lo, u_hi;
   user_block(n_users, c->world, c->rank, &u_lo, &u_hi);
   d->row_base = u_lo;
   d->n_local = u_hi - u_lo;
-  std::vector<std::vector<long long>> edge(n_types, std::vector<long long>((size_t)c->world + 1, 0));
-  for (int t = 0; t < n_types; ++t)
-    for (int q = 0; q <= c->world; ++q) {
-      long long a0, a1;
-      user_block(n_users, c->world, std::min(q, c->world - 1), &a0, &a1);
-      CKR(mail_fetch(c, &edge[t][q], d->rp[t] + (q < c->world ? a0 : a1), 8));
-    }
-  CKR(mail_wait(c));
   for (int t = 0; t < n_types; ++t) {
-    for (int q = 0; q < c->world; ++q) d->block_cap[t] = std::max(d->block_cap[t], edge[t][q + 1] - edge[t][q]);
-    d->q_lo[t] = edge[t][c->rank];
-    d->q_hi[t] = edge[t][c->rank + 1];
-    d->rp[t] += u_lo;   // views of the block; rp_alloc / col_alloc keep the whole matrices
+    CKR(mail_fetch(c, &d->q_lo[t], d->rp[t] + u_lo, 8));
+    CKR(mail_fetch(c, &d->q_hi[t], d->rp[t] + u_hi, 8));
   }
+  CKR(mail_wait(c));
+  for (int t = 0; t < n_types; ++t) d->rp[t] += u_lo;   // views of the block; rp_alloc / col_alloc keep the whole matrices
   return CCO_OK;
 }
 
@@ -4838,48 +4794,36 @@ int cco_debug_downsample(cco_ctx_t *c, const cco_csr_t *m, int32_t max_interacti
   CKR(validate_host(1, m, &prm));
   CK(cudaSetDevice(c->device));
   mail_reset(c);
+  c->ev_timing_used = c->ev_plain_used = 0;
   cco_dataset *ds = nullptr;
   CKR(dataset_upload(c, 1, m, flags, &ds));
   struct DG { cco_dataset *d; ~DG() { dataset_release(d); } } dg{ds};
   Arena ar(c->stream);
-  std::vector<DevRaw> raw(1);
-  raw[0].n_rows = ds->n_users; raw[0].n_cols = (int32_t)ds->n_cols[0]; raw[0].nnz = ds->nnz[0]; raw[0].nnz_cap = ds->nnz[0];
-  raw[0].rp = ds->rp[0]; raw[0].col = ds->col[0];
-  // the raw counts and the verdict exactly as the train makes them (count_raw_columns)
-  const std::vector<long long> col_off = {0, m->n_cols};
-  int32_t *counts;
-  int *d_check;
-  CKR(ar.alloc(&d_check, 2));
-  CK(cudaMemsetAsync(d_check, 0, sizeof(int) * 2, c->stream));
-  int *verdict = ds->validated ? nullptr : d_check;
-  CKR(count_raw_columns(c, ar, raw, col_off, ds->ready.data(), verdict, &counts));
-  DevMat dm;
-  CKR(downsample_device(c, ar, raw[0], verdict, counts, max_interactions, seed, flags, &dm));
+  Prepared p;   // the raw counts, the verdict and the sample exactly as the train makes them
+  CKR(prepare(c, ar, ds, &prm, seed, flags, &p));
+  const DevMat &dm = p.dm[0];
   std::vector<uint32_t> rp32((size_t)m->n_rows + 1);
-  int h_check = 0;
   CK(cudaMemcpyAsync(rp32.data(), dm.rp, sizeof(uint32_t) * rp32.size(), cudaMemcpyDeviceToHost, c->stream));
-  CK(cudaMemcpyAsync(&h_check, d_check, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   if (raw_col_counts && m->n_cols > 0)
-    CK(cudaMemcpyAsync(raw_col_counts, counts, sizeof(int32_t) * (size_t)m->n_cols, cudaMemcpyDeviceToHost, c->stream));
+    CK(cudaMemcpyAsync(raw_col_counts, p.raw_counts, sizeof(int32_t) * (size_t)m->n_cols, cudaMemcpyDeviceToHost, c->stream));
   if (new_col_counts && m->n_cols > 0)
     CK(cudaMemcpyAsync(new_col_counts, dm.marg, sizeof(int32_t) * (size_t)m->n_cols, cudaMemcpyDeviceToHost, c->stream));
   CK(cudaStreamSynchronize(c->stream));
   CK(cudaGetLastError());
-  if (h_check) return set_error(CCO_E_INVALID_ARG, "row_ptr not monotone or column index out of [0, n_cols)");
   size_t nnz = rp32[m->n_rows];
   int64_t *rp = (int64_t *)malloc(sizeof(int64_t) * rp32.size());
   int32_t *ci = (int32_t *)calloc(std::max<size_t>(nnz, 1), sizeof(int32_t));
   if (!rp || !ci) return set_error(CCO_E_OOM, "malloc failed");
   for (size_t i = 0; i < rp32.size(); ++i) rp[i] = rp32[i];
   // (kept counts beyond the matrix's entries show in row_ptr; the copy stays inside the sampled columns, the tail stays 0)
-  const size_t n_copy = std::min<size_t>(nnz, (size_t)raw[0].nnz);
+  const size_t n_copy = std::min<size_t>(nnz, (size_t)ds->nnz[0]);
   if (n_copy) CK(cudaMemcpy(ci, dm.col, sizeof(int32_t) * n_copy, cudaMemcpyDeviceToHost));
   *row_ptr = rp;
   *col_idx = ci;
   return CCO_OK;
 }
 
-// one rank's share of downsample_sharded_all on one GPU: the rank that owns users [row_lo, row_hi) samples them with
+// one rank's share of downsample_all on one GPU: the rank that owns users [row_lo, row_hi) samples them with
 // row_base = row_lo, absolute entry offsets, the whole matrix's raw counts and kept counts indexed by global user
 int cco_debug_downsample_block(cco_ctx_t *c, const cco_csr_t *m, int64_t row_lo, int64_t row_hi, const int32_t *raw_col_counts,
                                int32_t max_interactions, int32_t seed, uint32_t flags, int64_t *kept_per_row, int32_t **col_idx,
@@ -4910,7 +4854,6 @@ int cco_debug_downsample_block(cco_ctx_t *c, const cco_csr_t *m, int64_t row_lo,
   blk.n_cols = m->n_cols;
   blk.q_base = q[0];
   blk.nnz = q[1] - q[0];
-  blk.nnz_cap = ds->nnz[0];
   blk.rp = ds->rp[0] + row_lo;
   blk.col = ds->col[0];   // indexable by absolute offsets, as a rank's upload is
   int32_t *counts, *marg, *dst;
@@ -4960,47 +4903,19 @@ int cco_debug_cooccurrence(cco_ctx_t *c, const cco_csr_t *a, const cco_csr_t *b,
   CKR(validate_host(2, two, prm));
   CK(cudaSetDevice(c->device));
   mail_reset(c);
-  cudaStream_t s = c->stream;
+  c->ev_timing_used = c->ev_plain_used = 0;
   cco_dataset *ds = nullptr;
   CKR(dataset_upload(c, 2, two, 0, &ds));
   struct DG { cco_dataset *d; ~DG() { dataset_release(d); } } dg{ds};
-  Arena ar(s);
+  Arena ar(c->stream);
   struct CopyJoin {
     cco_ctx *c;
     ~CopyJoin() { cudaStreamSynchronize(c->copy_stream); }
   } copy_join{c};
-  std::vector<DevRaw> raw(2);
-  for (int i = 0; i < 2; ++i) {
-    raw[i].n_rows = ds->n_users; raw[i].n_cols = (int32_t)ds->n_cols[i]; raw[i].nnz = ds->nnz[i]; raw[i].nnz_cap = ds->nnz[i];
-    raw[i].rp = ds->rp[i]; raw[i].col = ds->col[i];
-  }
-  // identity "downsample" (m = INT_MAX) gives the device CSR + marginals; raw counts as the train makes them
-  const std::vector<long long> col_off = {0, raw[0].n_cols, (long long)raw[0].n_cols + raw[1].n_cols};
-  int32_t *counts;
-  CKR(count_raw_columns(c, ar, raw, col_off, ds->ready.data(), nullptr, &counts));   // (uploaded with validation + canonicalisation)
-  std::vector<DevMat> dm(2);
-  for (int i = 0; i < 2; ++i) CKR(downsample_device(c, ar, raw[i], nullptr, counts + col_off[i], 0x7fffffff, 0, 0, &dm[i]));
-  const int32_t n_items_a = dm[0].n_cols;
-  uint32_t *at_ptr, *cursor, *marg_pad;
-  int32_t *at_users, *d_max;
-  CKR(ar.alloc(&at_ptr, n_items_a + 1));
-  CKR(ar.alloc(&cursor, n_items_a + 1));
-  CKR(ar.alloc(&marg_pad, n_items_a + 1));
-  CKR(ar.alloc(&d_max, 2));
-  CKR(ar.alloc(&at_users, std::max<long long>(raw[0].nnz, 1)));
-  CK(cudaMemsetAsync(d_max, 0, 8, s));
-  CK(cudaMemcpyAsync(marg_pad, dm[0].marg, sizeof(int32_t) * (size_t)n_items_a, cudaMemcpyDeviceToDevice, s));
-  CK(cudaMemsetAsync(marg_pad + n_items_a, 0, 4, s));
-  CKR(exclusive_sum(c, ar, marg_pad, at_ptr, (long long)n_items_a + 1));
-  CK(cudaMemcpyAsync(cursor, at_ptr, sizeof(uint32_t) * ((size_t)n_items_a + 1), cudaMemcpyDeviceToDevice, s));
-  k_transpose_entries<<<grid_for((raw[0].nnz + kSampleChunk - 1) / kSampleChunk * 32, 256, c->sm_count), 256, 0, s>>>(a->n_rows, dm[0].rp,
-                                                                                                                     dm[0].col, cursor, at_users);
-  if (n_items_a > 0) k_max_i32<<<grid_for(n_items_a, 256, c->sm_count, 2), 256, 0, s>>>(n_items_a, dm[0].marg, d_max);
-  if (dm[1].n_cols > 0) k_max_i32<<<grid_for(dm[1].n_cols, 256, c->sm_count, 2), 256, 0, s>>>(dm[1].n_cols, dm[1].marg, d_max + 1);
-  int32_t max_marg_ab[2] = {0, 0};
-  CK(cudaMemcpyAsync(max_marg_ab, d_max, 8, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  CK(cudaGetLastError());
+  // the train's preparation with the identity sample (m = INT_MAX): the device CSR, marginals and A'^T
+  Prepared prep;
+  CKR(prepare(c, ar, ds, prm, 0, 0, &prep));
+  const int32_t n_items_a = prep.dm[0].n_cols;
   ResultMat rm;
   IndicatorOut io;
   IndicatorState ist;
@@ -5010,8 +4925,8 @@ int cco_debug_cooccurrence(cco_ctx_t *c, const cco_csr_t *a, const cco_csr_t *b,
     for (void *p : {(void *)rm.row_ptr, (void *)rm.col, (void *)rm.llr, (void *)rm.cnt})
       if (p) c->pinned_put(p);
   };
-  int rc = enqueue_indicator(c, ar, at_ptr, at_users, n_items_a, dm[0].marg, max_marg_ab[0], max_marg_ab[1], dm[1], a->n_rows, false, p1,
-                             0, true, nullptr, nullptr, nullptr, &ist);
+  int rc = enqueue_indicator(c, ar, prep.at_ptr, prep.at_users, n_items_a, prep.dm[0].marg, prep.max_marg[0], prep.max_marg[1], prep.dm[1],
+                             a->n_rows, false, p1, 0, true, nullptr, nullptr, nullptr, &ist);
   if (rc == CCO_OK) rc = finish_indicator(c, &ist, 0, 0, &rm, &io);
   cudaStreamSynchronize(c->copy_stream);
   if (rc != CCO_OK) {
