@@ -538,6 +538,59 @@ int cco_event_log_begin_window(cco_ctx_t *ctx, int64_t chunk_bytes, const cco_ev
 int cco_event_log_window_stats(const cco_event_log_t *log, int64_t *n_expired, int64_t *n_duplicates);
 
 /*
+ * User queries from the log (URAlgorithm.buildQuery for Query.user, URAlgorithm.scala:563-839): one Elasticsearch query per
+ * user, built from the user's training events in HBM instead of one LEventStore.findByEntity read per user.
+ *
+ * History retention: cco_event_log_begin_ex with CCO_LOG_KEEP_HISTORY keeps each training event's eventTime and global
+ * 0-based line next to the user and item columns (16 bytes per training event).  A log read without it is what
+ * cco_event_log_begin_window reads, byte for byte and in device memory.  w as in cco_event_log_begin_window.
+ */
+enum { CCO_LOG_KEEP_HISTORY = 1 };
+int cco_event_log_begin_ex(cco_ctx_t *ctx, int64_t chunk_bytes, const cco_event_window_t *w /* nullable */, uint32_t flags,
+                           cco_event_log_t **out);
+/*
+ * The query of user u, for the query event names n_0 .. n_{k-1}:
+ *  - history of n_q: u's training events of n_q, latest first (eventTime desc, ties to the later line), the first limits[q]
+ *    of them reversed (oldest first), repeated items kept at their first position;
+ *  - blacklist: the items of every training event of u whose name is among the names and the blacklist names, latest
+ *    first, then the blacklist items, each item once (its first position);
+ *  - the body record:  header \n head ,"query":{"bool":{"should":[S],"must":[M],"must_not":[{"ids":{"values":[blacklist],
+ *    "boost":0}}(,must_not)?],"minimum_should_match":1}},"sort":sort} \n
+ *    where the terms of the first n_history_names names, {"terms":{"<n_q>":[history],"boost":<boost>}} (without "boost" when
+ *    boost is NULL) or {"terms":{"<n_q>":[history],"boost":0}} in must, come before the `should` (or `must`) fragment, all
+ *    comma-separated.  Ids and names are escaped as json4s 3.2 quotes strings: '"' and '\' get a backslash, \b \f \n \r \t
+ *    their short forms, every other code point below U+0020, in U+0080..U+009F and in U+2000..U+20FF \u%04x in lowercase.
+ * Fragments are JSON text spliced verbatim: head ({"from":F,"size":N), should (must not be empty: the reference ends should
+ * with a constant_score clause), must, must_not (may be empty), sort (an array), header (one _msearch header line).
+ * Users: n_users ids in the Arrow large_string layout (a repeated or unknown user gets its record, an unknown one with an
+ * empty history), or user_offsets == NULL: every user with a training event of a query name, in order of their first such
+ * line; *out_users then lists them (pinned offsets and bytes, each released with cco_host_free; nullable otherwise).
+ * Out: *out_body [*out_len] and *out_offsets [*out_n + 1] (record r = body[offsets[r] .. offsets[r + 1])), pinned memory
+ * owned by the context, each released with cco_host_free.
+ * Errors: CCO_E_INVALID_ARG for bad offsets in either column (decided on the device before any kernel reads bytes through
+ * them), null or empty names, negative limits, n_history_names outside [0, n_names], a null fragment, more than 64 names and
+ * a log read without CCO_LOG_KEEP_HISTORY; CCO_E_UNSUPPORTED for group contexts, 2^31 or more events of the names and a
+ * record of 2^31 or more bytes.  A name the log does not hold has no history.
+ */
+typedef struct {
+  int32_t n_names;
+  int32_t n_history_names;           /* maxQueryEvents - 1 clamped to [0, n_names] */
+  const char *const *names;          /* [n_names] the query event names */
+  const int32_t *limits;             /* [n_names] history limit per name (maxItemsPerUser) */
+  int32_t n_blacklist_names;
+  int32_t history_in_must;           /* 0: should (userBias >= 0), 1: must (userBias < 0) */
+  const char *const *blacklist_names;
+  const char *boost;                 /* JSON number text or NULL */
+  const char *head, *should, *must, *must_not, *sort, *header;
+  int64_t n_blacklist_items;
+  const int64_t *blacklist_item_offsets; /* [n + 1] */
+  const char *blacklist_item_bytes;
+} cco_user_query_t;
+int cco_event_log_user_queries(cco_ctx_t *ctx, const cco_event_log_t *log, const cco_user_query_t *q, int64_t n_users,
+                               const int64_t *user_offsets /* nullable: every user */, const char *user_bytes, char **out_body,
+                               int64_t *out_len, int64_t **out_offsets, int64_t *out_n, cco_dictionary_t *out_users /* nullable */);
+
+/*
  * Debug/parity entry (tests only): full integer co-occurrence matrix A^T B of two canonical
  * binary matrices computed by the same accumulation kernel as cco_train, no LLR, no top-k.
  * Output CSR over the columns of A with ascending column ids, malloc'ed; free with cco_free.

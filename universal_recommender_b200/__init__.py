@@ -25,14 +25,15 @@ from .preparator import prepare, prepare_on_device
 from .similarity_analysis import (CcoContext, DownsamplableCrossOccurrenceDataset, EventLog, SimilarityAnalysis,
                                   decode_ids, default_context, encode_ids)
 from .ur_algorithm import (DefaultURAlgoParams, IndicatorParams, URAlgorithmParams, calc_all, calc_all_from_events, calc_all_on_device,
-                           calc_pop_from_events, calc_pop_on_device)
+                           calc_pop_from_events, calc_pop_on_device, user_queries_from_events)
+from .ur_query import UserQuery
 from .ur_model import RankingParams
 
 __all__ = [
     "BiDictionary", "CcoContext", "CcoError", "CcoInvalidArgument", "DataSourceParams", "DefaultURAlgoParams", "EventWindow",
     "DownsamplableCrossOccurrenceDataset", "IndexedDataset", "IndicatorParams", "SimilarityAnalysis",
     "EventLog", "RankingParams", "URAlgorithmParams", "calc_all", "calc_all_from_events", "calc_all_on_device", "calc_pop_from_events",
-    "calc_pop_on_device", "decode_ids", "default_context", "encode_ids", "prepare", "prepare_on_device",
+    "calc_pop_on_device", "user_queries_from_events", "UserQuery", "decode_ids", "default_context", "encode_ids", "prepare", "prepare_on_device",
     "FLAG_ASSUME_CANONICAL",
     "FLAG_ENTROPY_VARARGS", "FLAG_ROWRATE_INTDIV", "FLAG_RESULT_NO_COUNT", "FLAG_RESULT_NO_LLR", "LIB_PATH",
 ]

@@ -94,6 +94,17 @@ class EventWindowT(C.Structure):
     _fields_ = [("cutoff_ms", C.c_int64), ("remove_duplicates", C.c_int32), ("reserved", C.c_int32)]
 
 
+LOG_KEEP_HISTORY = 1
+
+
+class UserQueryT(C.Structure):
+    _fields_ = [("n_names", C.c_int32), ("n_history_names", C.c_int32), ("names", C.POINTER(C.c_char_p)), ("limits", C.POINTER(C.c_int32)),
+                ("n_blacklist_names", C.c_int32), ("history_in_must", C.c_int32), ("blacklist_names", C.POINTER(C.c_char_p)),
+                ("boost", C.c_char_p), ("head", C.c_char_p), ("should", C.c_char_p), ("must", C.c_char_p), ("must_not", C.c_char_p),
+                ("sort", C.c_char_p), ("header", C.c_char_p), ("n_blacklist_items", C.c_int64),
+                ("blacklist_item_offsets", C.POINTER(C.c_int64)), ("blacklist_item_bytes", C.c_void_p)]
+
+
 class LogRankingT(C.Structure):
     _fields_ = [("name", C.c_char_p), ("mode", C.c_int32), ("n_event_names", C.c_int32), ("start_ms", C.c_int64), ("end_ms", C.c_int64),
                 ("event_names", C.POINTER(C.c_char_p))]
@@ -117,7 +128,8 @@ EXPORTS = [
     "cco_dataset_copy_to_host", "cco_format_es_bulk", "cco_ingest_strings", "cco_dataset_dictionary", "cco_pop_model",
     "cco_format_model", "cco_rerank_model", "cco_event_log_read", "cco_event_log_info", "cco_event_log_ingest",
     "cco_format_model_log", "cco_rerank_model_log", "cco_event_log_free", "cco_event_log_begin", "cco_event_log_append",
-    "cco_event_log_finish", "cco_event_log_begin_window", "cco_event_log_window_stats", "cco_result_num_matrices", "cco_result_row_range", "cco_result_matrix", "cco_result_stats", "cco_result_free",
+    "cco_event_log_finish", "cco_event_log_begin_window", "cco_event_log_window_stats",
+    "cco_event_log_begin_ex", "cco_event_log_user_queries", "cco_result_num_matrices", "cco_result_row_range", "cco_result_matrix", "cco_result_stats", "cco_result_free",
     "cco_debug_cooccurrence", "cco_debug_downsample", "cco_debug_downsample_block", "cco_debug_llr", "cco_debug_string_ids", "cco_free",
 ]
 
@@ -178,6 +190,9 @@ def lib():
     L.cco_event_log_finish.argtypes = [C.c_void_p]
     L.cco_event_log_begin_window.argtypes = [C.c_void_p, C.c_int64, p(EventWindowT), p(C.c_void_p)]
     L.cco_event_log_window_stats.argtypes = [C.c_void_p, p(C.c_int64), p(C.c_int64)]
+    L.cco_event_log_begin_ex.argtypes = [C.c_void_p, C.c_int64, p(EventWindowT), C.c_uint32, p(C.c_void_p)]
+    L.cco_event_log_user_queries.argtypes = [C.c_void_p, C.c_void_p, p(UserQueryT), C.c_int64, p(C.c_int64), C.c_void_p, p(C.c_void_p),
+                                             p(C.c_int64), p(C.c_void_p), p(C.c_int64), p(DictionaryT)]
     L.cco_dataset_shape.argtypes = [C.c_void_p, C.c_int32, p(C.c_int64), p(C.c_int32), p(C.c_int64)]
     L.cco_dataset_download.argtypes = [C.c_void_p, C.c_int32, p(p(C.c_int64)), p(p(C.c_int32))]
     L.cco_timer_start.argtypes = [C.c_void_p]

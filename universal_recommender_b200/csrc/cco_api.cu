@@ -29,6 +29,7 @@
 #include "cco_strings.cuh"
 #include "cco_json.cuh"
 #include "cco_events.cuh"
+#include "cco_queries.cuh"
 
 namespace cco {
 
@@ -3463,6 +3464,7 @@ struct EvSeg {
   EvCol tu, ti, ri;
   long long *rtime = nullptr;
   long long *tline = nullptr, *rline = nullptr;   // removeDuplicates: the global line of each training / ranking entry
+  long long *ttime = nullptr;                       // history retention: each training entry's time (and tline its line)
   std::vector<long long> train_at, rank_at;
 };
 struct cco_event_log {
@@ -3501,6 +3503,10 @@ struct cco_event_log {
   WinRec *rec = nullptr;
   long long n_rec = 0, rec_cap = 0;
   long long *tline = nullptr, *rline = nullptr;
+  // history retention (CCO_LOG_KEEP_HISTORY): every training entry's time and global line, partitioned as tu / ti; tline
+  // then outlives finish
+  bool history = false;
+  long long *ttime = nullptr;
   bool finished = false;
   int fail = CCO_OK;                           // a failed append / finish: every later call returns it with fail_msg
   std::string fail_msg;
@@ -4106,7 +4112,16 @@ static int event_chunk(cco_event_log *lg, long long len, bool open_tail) {
   CKR(event_partition(c, ar, L, ev.flag, kEvTraining, code, (uint32_t)NG, &idx));
   CKR(event_column(c, ar, lg, sg.train_at[NG], idx, kEvEntityId, ev.sb, ev.span, bb, sg.train_at, &sg.tu));
   CKR(event_column(c, ar, lg, sg.train_at[NG], idx, kEvTargetId, ev.sb, ev.span, bb, sg.train_at, &sg.ti));
-  if (lg->dedup) CKR(win_entry_lines(lg, ar, sg.train_at[NG], idx, base, &sg.tline));
+  if (lg->dedup || lg->history) CKR(win_entry_lines(lg, ar, sg.train_at[NG], idx, base, &sg.tline));
+  if (lg->history) {
+    const long long NT = sg.train_at[NG];
+    CKR(ar.alloc(&sg.ttime, std::max<long long>(NT, 1)));
+    CKR(log_keep(ar, lg, sg.ttime));
+    if (NT > 0) {
+      k_gather_i64<<<grid_for(NT, 256, c->sm_count), 256, 0, s>>>(NT, idx, ev.tm, sg.ttime);
+      c->launches++;
+    }
+  }
   ar.release(idx);
   CKR(event_partition(c, ar, L, ev.flag, kEvRanking, code, (uint32_t)NG, &idx));
   const long long NR = sg.rank_at[NG];
@@ -4300,7 +4315,7 @@ static int win_gather_column(cco_event_log *lg, Arena &ar, long long K, const ui
 }
 // the name-partitioned entries whose line survives the bitmap: columns c1 (and c2), the times (nullable) and at, compacted
 static int win_compact(cco_event_log *lg, const uint32_t *bitmap, const long long *line, std::vector<long long> &at, EvCol *c1, EvCol *c2,
-                       long long **times) {
+                       long long **times, long long **times2 = nullptr) {
   cco_ctx *c = lg->ctx;
   cudaStream_t s = c->stream;
   Arena ar(s);
@@ -4323,17 +4338,18 @@ static int win_compact(cco_event_log *lg, const uint32_t *bitmap, const long lon
   const long long K = nat.back();
   CKR(win_gather_column(lg, ar, K, idx, nat, c1));
   if (c2) CKR(win_gather_column(lg, ar, K, idx, nat, c2));
-  if (times) {
+  for (long long **tp : {times, times2}) {
+    if (!tp) continue;
     long long *t;
     CKR(ar.alloc(&t, std::max<long long>(K, 1)));
     if (K > 0) {
-      k_gather_i64<<<grid_for(K, 256, c->sm_count), 256, 0, s>>>(K, idx, *times, t);
+      k_gather_i64<<<grid_for(K, 256, c->sm_count), 256, 0, s>>>(K, idx, *tp, t);
       c->launches++;
     }
     CK(cudaStreamSynchronize(s));
     CKR(log_keep(ar, lg, t));
-    log_drop(lg, *times);
-    *times = t;
+    log_drop(lg, *tp);
+    *tp = t;
   }
   at = nat;
   return CCO_OK;
@@ -4477,28 +4493,32 @@ static int event_log_finish(cco_event_log *lg) {
     lg->rtime = sg.rtime;
     lg->tline = sg.tline;
     lg->rline = sg.rline;
+    lg->ttime = sg.ttime;
   } else if (lg->segs.size() > 1) {
     CKR(event_cat_column(lg, &EvSeg::tu, &EvSeg::train_at, lg->train_at, &lg->tu));
     CKR(event_cat_column(lg, &EvSeg::ti, &EvSeg::train_at, lg->train_at, &lg->ti));
     CKR(event_cat_column(lg, &EvSeg::ri, &EvSeg::rank_at, lg->rank_at, &lg->ri));
     CKR(event_cat_times(lg, &lg->rtime));
-    if (lg->dedup) {
-      CKR(event_cat_times(lg, &lg->tline, &EvSeg::tline, &EvSeg::train_at));
-      CKR(event_cat_times(lg, &lg->rline, &EvSeg::rline, &EvSeg::rank_at));
-    }
+    if (lg->dedup || lg->history) CKR(event_cat_times(lg, &lg->tline, &EvSeg::tline, &EvSeg::train_at));
+    if (lg->dedup) CKR(event_cat_times(lg, &lg->rline, &EvSeg::rline, &EvSeg::rank_at));
+    if (lg->history) CKR(event_cat_times(lg, &lg->ttime, &EvSeg::ttime, &EvSeg::train_at));
   }
   lg->segs.clear();
   if (drop && lg->n_dup > 0) {   // the retained columns without the dropped lines' entries
-    CKR(win_compact(lg, drop, lg->tline, lg->train_at, &lg->tu, &lg->ti, nullptr));
+    CKR(win_compact(lg, drop, lg->tline, lg->train_at, &lg->tu, &lg->ti, lg->history ? &lg->ttime : nullptr,
+                    lg->history ? &lg->tline : nullptr));
     CKR(win_compact(lg, drop, lg->rline, lg->rank_at, &lg->ri, nullptr, &lg->rtime));
     for (long long n = 0; n < NG; ++n) {
       lg->n_train[n] = lg->train_at[n + 1] - lg->train_at[n];
       lg->n_rank[n] = lg->rank_at[n + 1] - lg->rank_at[n];
     }
   }
-  log_drop(lg, lg->tline);
+  if (!lg->history) {
+    log_drop(lg, lg->tline);
+    lg->tline = nullptr;
+  }
   log_drop(lg, lg->rline);
-  lg->tline = lg->rline = nullptr;
+  lg->rline = nullptr;
   if (lg->n_prop > 0) {
     mail_reset(c);
     Arena ar(s);
@@ -4709,6 +4729,424 @@ int cco_rerank_model_log(cco_ctx_t *ctx, const char *body, int64_t body_len, con
   const bool any = lg->n_triples > 0;
   return rerank_model(ctx, body, body_len, any ? &lp.shell : nullptr, n_rankings, rk.data(), out_bytes, out_len, std::move(ls),
                       any ? &lp.dev : nullptr);
+}
+
+namespace cco {
+// json4s 3.2's quote of a name (the escaping of uq_escape, on the host), quotes included
+static std::string uq_quote(const char *s) {
+  std::string o = "\"";
+  const unsigned char *b = (const unsigned char *)s;
+  const size_t n = strlen(s);
+  char hex[8];
+  for (size_t i = 0; i < n; ++i) {
+    const unsigned char x = b[i];
+    unsigned cp = 0xffffffffu;
+    if (x == '"' || x == '\\') { o += '\\'; o += (char)x; continue; }
+    if (x == '\b') { o += "\\b"; continue; }
+    if (x == '\f') { o += "\\f"; continue; }
+    if (x == '\n') { o += "\\n"; continue; }
+    if (x == '\r') { o += "\\r"; continue; }
+    if (x == '\t') { o += "\\t"; continue; }
+    if (x < 0x20) cp = x;
+    else if (x == 0xC2 && i + 1 < n && b[i + 1] >= 0x80 && b[i + 1] <= 0x9F) cp = b[++i];
+    else if (x == 0xE2 && i + 2 < n && b[i + 1] >= 0x80 && b[i + 1] <= 0x83 && (b[i + 2] & 0xC0) == 0x80) {
+      cp = 0x2000u | ((unsigned)(b[i + 1] & 0x3F) << 6) | (b[i + 2] & 0x3F);
+      i += 2;
+    }
+    if (cp != 0xffffffffu) {
+      snprintf(hex, sizeof hex, "\\u%04x", cp);
+      o += hex;
+    } else {
+      o += (char)x;
+    }
+  }
+  return o + "\"";
+}
+
+// the record template: n_history_names + 2 pieces around the history lists and the blacklist (see include/cco_b200.h)
+static std::vector<std::string> uq_template(const cco_user_query_t *q) {
+  std::vector<std::string> t(1);
+  const int k = q->n_history_names;
+  auto clause = [&](const char *rest, bool hist) {
+    bool any = false;
+    for (int j = 0; hist && j < k; ++j) {
+      if (any) t.back() += ",";
+      t.back() += "{\"terms\":{" + uq_quote(q->names[j]) + ":[";
+      t.emplace_back("]");
+      if (q->history_in_must) t.back() += ",\"boost\":0";
+      else if (q->boost) t.back() += std::string(",\"boost\":") + q->boost;
+      t.back() += "}}";
+      any = true;
+    }
+    if (*rest) {
+      if (any) t.back() += ",";
+      t.back() += rest;
+    }
+  };
+  t.back() += std::string(q->header) + "\n" + q->head + ",\"query\":{\"bool\":{\"should\":[";
+  clause(q->should, !q->history_in_must);
+  t.back() += "],\"must\":[";
+  clause(q->must, q->history_in_must != 0);
+  t.back() += "],\"must_not\":[{\"ids\":{\"values\":[";
+  t.emplace_back("],\"boost\":0}}");
+  if (*q->must_not) t.back() += std::string(",") + q->must_not;
+  t.back() += std::string("],\"minimum_should_match\":1}},\"sort\":") + q->sort + "}\n";
+  return t;
+}
+
+static int uq_check_host(const cco_user_query_t *q, int64_t n_users, const int64_t *uoff, const char *ubytes) {
+  if (q->n_names < 0 || q->n_names > kUqMaxNames) return set_error(CCO_E_INVALID_ARG, "%d query event names, 0..%d", (int)q->n_names, kUqMaxNames);
+  if (q->n_names > 0 && (!q->names || !q->limits)) return set_error(CCO_E_INVALID_ARG, "null names or limits");
+  for (int k = 0; k < q->n_names; ++k) {
+    if (!q->names[k] || !*q->names[k]) return set_error(CCO_E_INVALID_ARG, "query event name %d is null or empty", k);
+    if (q->limits[k] < 0) return set_error(CCO_E_INVALID_ARG, "query event name %d: negative limit %d", k, (int)q->limits[k]);
+  }
+  if (q->n_history_names < 0 || q->n_history_names > q->n_names)
+    return set_error(CCO_E_INVALID_ARG, "n_history_names = %d is outside [0, %d]", (int)q->n_history_names, (int)q->n_names);
+  if (q->n_blacklist_names < 0 || (q->n_blacklist_names > 0 && !q->blacklist_names)) return set_error(CCO_E_INVALID_ARG, "bad blacklist names");
+  for (int b = 0; b < q->n_blacklist_names; ++b)
+    if (!q->blacklist_names[b]) return set_error(CCO_E_INVALID_ARG, "blacklist name %d is null", b);
+  if (q->history_in_must != 0 && q->history_in_must != 1) return set_error(CCO_E_INVALID_ARG, "history_in_must must be 0 or 1");
+  if (!q->head || !q->should || !q->must || !q->must_not || !q->sort || !q->header) return set_error(CCO_E_INVALID_ARG, "a null fragment");
+  if (!*q->should) return set_error(CCO_E_INVALID_ARG, "the should fragment is empty");
+  CKR(str_check_host(q->n_blacklist_items, q->blacklist_item_offsets, q->blacklist_item_bytes, 0, "blacklist item"));
+  if (uoff) CKR(str_check_host(n_users, uoff, ubytes, 0, "user"));
+  else if (n_users != 0) return set_error(CCO_E_INVALID_ARG, "n_users without user offsets");
+  return CCO_OK;
+}
+
+static int user_queries(cco_ctx *c, const cco_event_log *lg, const cco_user_query_t *q, int64_t n_users, const int64_t *uoff,
+                        const char *ubytes, char **out_body, int64_t *out_len, int64_t **out_offsets, int64_t *out_n,
+                        cco_dictionary_t *out_users) {
+  cudaStream_t s = c->stream;
+  const int nq = q->n_names;
+  std::vector<int> code(nq);
+  std::vector<uint8_t> black(std::max(nq, 1), 0);
+  for (int k = 0; k < nq; ++k) {
+    code[k] = lg->code_of(q->names[k]);
+    bool earlier = false;   // a repeated query name reads the same events: blacklist them once
+    for (int j = 0; j < k; ++j) earlier |= strcmp(q->names[j], q->names[k]) == 0;
+    for (int b = 0; b < q->n_blacklist_names && !earlier; ++b)
+      if (strcmp(q->blacklist_names[b], q->names[k]) == 0) black[k] = 1;
+  }
+  CK(cudaSetDevice(c->device));
+  mail_reset(c);
+  Arena ar(s);
+  nvtx_push("cco:user_queries");
+  struct Pop { ~Pop() { nvtx_pop(); } } pop;
+  // 1. the caller's columns, checked on the device before any kernel reads bytes through their offsets
+  DevStrCol lc, uc;
+  CKR(str_upload(c, ar, q->n_blacklist_items, q->blacklist_item_offsets, q->blacklist_item_bytes, &lc));
+  if (uoff) CKR(str_upload(c, ar, n_users, uoff, ubytes, &uc));
+  int *bad, h_bad = 0;
+  CKR(ar.alloc(&bad, 1));
+  CK(cudaMemsetAsync(bad, 0, 4, s));
+  str_check_device(c, lc, bad);
+  if (uoff) str_check_device(c, uc, bad);
+  CKR(mail_fetch(c, &h_bad, bad, 4));
+  CKR(mail_wait(c));
+  if (h_bad) return set_error(CCO_E_INVALID_ARG, "decreasing offsets in the blacklist items or the users");
+  // 2. the training events of the query names, name-major
+  std::vector<long long> qoff(nq + 1, 0), qbase(std::max(nq, 1), 0);
+  for (int k = 0; k < nq; ++k) {
+    const long long n = code[k] >= 0 ? lg->n_train[code[k]] : 0;
+    qbase[k] = code[k] >= 0 ? lg->train_at[code[k]] : 0;
+    qoff[k + 1] = qoff[k] + n;
+  }
+  const long long E = qoff[nq];
+  if (E >= 0x7fffffffLL) return set_error(CCO_E_UNSUPPORTED, "%lld training events of the query names, at most 2^31 - 2", E);
+  const long long NT = lg->train_at.back();
+  long long G = 0;
+  StrTable ut, it;
+  DevStrCol tu, ti;
+  uint32_t *ent = nullptr, *gord = nullptr, *hord = nullptr, *bord = nullptr;
+  uint8_t *qr = nullptr, *keep_h = nullptr, *keep_b = nullptr, *d_black = nullptr;
+  int32_t *uid = nullptr, *iid = nullptr, *d_limit = nullptr;
+  long long *tm = nullptr, *ln = nullptr, *hstart = nullptr, *bstart = nullptr;
+  unsigned long long *bkey = nullptr;
+  long long B = 0;
+  CKR(ar.alloc(&d_limit, std::max(nq, 1)));
+  if (nq > 0) CK(cudaMemcpyAsync(d_limit, q->limits, sizeof(int32_t) * (size_t)nq, cudaMemcpyHostToDevice, s));
+  if (E > 0) {
+    long long *d_qoff, *d_qbase;
+    CKR(ar.alloc(&d_qoff, nq + 1));
+    CKR(ar.alloc(&d_qbase, nq));
+    CKR(ar.alloc(&d_black, nq));
+    CK(cudaMemcpyAsync(d_qoff, qoff.data(), sizeof(long long) * (size_t)(nq + 1), cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(d_qbase, qbase.data(), sizeof(long long) * (size_t)nq, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(d_black, black.data(), (size_t)nq, cudaMemcpyHostToDevice, s));
+    CKR(ar.alloc(&ent, E));
+    CKR(ar.alloc(&qr, E));
+    k_uq_select<<<grid_for(E, 256, c->sm_count), 256, 0, s>>>(E, nq, d_qoff, d_qbase, ent, qr);
+    c->launches++;
+    // 3. users and items grouped exactly (hash, then bytes) over the log's columns, gated to the query names' events
+    int32_t *gate, *ugid, *igid;
+    CKR(ar.alloc(&gate, NT));
+    CK(cudaMemsetAsync(gate, 0xff, sizeof(int32_t) * (size_t)NT, s));
+    for (int k = 0; k < nq; ++k)
+      if (code[k] >= 0 && lg->n_train[code[k]] > 0)
+        CK(cudaMemsetAsync(gate + lg->train_at[code[k]], 0, sizeof(int32_t) * (size_t)lg->n_train[code[k]], s));
+    tu = lg->view(lg->tu, 0, lg->train_at, NT);
+    ti = lg->view(lg->ti, 0, lg->train_at, NT);
+    CKR(ar.alloc(&tu.hash, NT));
+    CKR(ar.alloc(&ti.hash, NT));
+    CKR(ar.alloc(&ugid, NT));
+    CKR(ar.alloc(&igid, NT));
+    str_hash(c, tu, ~0ULL);
+    str_hash(c, ti, ~0ULL);
+    CKR(str_group(c, ar, tu, gate, false, 0, &ut, ugid));
+    CKR(str_group(c, ar, ti, gate, false, 0, &it, igid));
+    G = ut.n_groups;
+    if (G * (long long)nq >= (1LL << 32)) return set_error(CCO_E_UNSUPPORTED, "%lld users x %d names, at most 2^32 segments", G, nq);
+    // 4. per event: user, item, time, line
+    CKR(ar.alloc(&uid, E));
+    CKR(ar.alloc(&iid, E));
+    CKR(ar.alloc(&tm, E));
+    CKR(ar.alloc(&ln, E));
+    k_uq_gather<<<grid_for(E, 256, c->sm_count), 256, 0, s>>>(E, ent, ugid, igid, lg->ttime, lg->tline, uid, iid, tm, ln);
+    c->launches++;
+    // 5. latest first: line desc, then stably time desc
+    unsigned long long *key;
+    CKR(ar.alloc(&key, E));
+    CKR(ar.alloc(&gord, E));
+    k_uq_key_line<<<grid_for(E, 256, c->sm_count), 256, 0, s>>>(E, lg->n_lines, ln, key, gord);
+    c->launches++;
+    CKR(sort_pairs(c, ar, E, &key, &gord, bits_for(lg->n_lines)));
+    k_uq_key_time<<<grid_for(E, 256, c->sm_count), 256, 0, s>>>(E, gord, tm, key);
+    c->launches++;
+    CKR(sort_pairs(c, ar, E, &key, &gord, 64));
+    // 6. history order: stably by (user, name rank); segment starts
+    CKR(ar.alloc(&hord, E));
+    CK(cudaMemcpyAsync(hord, gord, sizeof(uint32_t) * (size_t)E, cudaMemcpyDeviceToDevice, s));
+    k_uq_key_seg<<<grid_for(E, 256, c->sm_count), 256, 0, s>>>(E, nq, gord, uid, qr, key);
+    c->launches++;
+    CKR(sort_pairs(c, ar, E, &key, &hord, bits_for(G * nq)));
+    long long *cnt;
+    CKR(ar.alloc(&cnt, G * nq + 1));
+    CKR(ar.alloc(&hstart, G * nq + 1));
+    CK(cudaMemsetAsync(cnt, 0, sizeof(long long) * (size_t)(G * nq + 1), s));
+    k_uq_count<<<grid_for(E, 256, c->sm_count), 256, 0, s>>>(E, key, cnt);
+    c->launches++;
+    CKR(exclusive_sum(c, ar, cnt, hstart, G * nq + 1));
+    // 7. the first limit[q] of each segment, each item at its oldest position among them
+    unsigned long long *k2;
+    uint32_t *p2;
+    CKR(ar.alloc(&k2, E));
+    CKR(ar.alloc(&p2, E));
+    CKR(ar.alloc(&keep_h, E));
+    CK(cudaMemsetAsync(keep_h, 0, (size_t)E, s));
+    k_uq_hist_keys<<<grid_for(E, 256, c->sm_count), 256, 0, s>>>(E, nq, key, hstart, d_limit, hord, iid, k2, p2);
+    c->launches++;
+    CKR(sort_pairs(c, ar, E, &k2, &p2, 64));
+    k_uq_first<<<grid_for(E, 256, c->sm_count), 256, 0, s>>>(E, k2, p2, keep_h);
+    c->launches++;
+    ar.release(k2);
+    ar.release(p2);
+    // 8. blacklist: the blacklisted names' events latest first, stably by user; each item's newest position
+    uint32_t *flag, *pos, *bidx;
+    CKR(ar.alloc(&flag, E + 1));
+    k_uq_flag_black<<<grid_for(E, 256, c->sm_count), 256, 0, s>>>(E, gord, qr, d_black, flag);
+    c->launches++;
+    CKR(select_flagged(c, ar, E, flag, &pos, &bidx));
+    uint32_t B32 = 0;
+    CKR(mail_fetch(c, &B32, pos + E, 4));
+    CKR(mail_wait(c));
+    B = B32;
+    CKR(ar.alloc(&bkey, std::max<long long>(B, 1)));
+    CKR(ar.alloc(&bord, std::max<long long>(B, 1)));
+    CKR(ar.alloc(&bstart, G + 1));
+    CKR(ar.alloc(&keep_b, std::max<long long>(B, 1)));
+    long long *bcnt;
+    CKR(ar.alloc(&bcnt, G + 1));
+    CK(cudaMemsetAsync(bcnt, 0, sizeof(long long) * (size_t)(G + 1), s));
+    if (B > 0) {
+      k_uq_key_user<<<grid_for(B, 256, c->sm_count), 256, 0, s>>>(B, bidx, gord, uid, bkey, bord);
+      c->launches++;
+      CKR(sort_pairs(c, ar, B, &bkey, &bord, bits_for(G)));
+      k_uq_count<<<grid_for(B, 256, c->sm_count), 256, 0, s>>>(B, bkey, bcnt);
+      uint32_t *p3;
+      CKR(ar.alloc(&p3, B));
+      k_uq_black_keys<<<grid_for(B, 256, c->sm_count), 256, 0, s>>>(B, bord, uid, iid, bkey, p3);
+      c->launches += 2;
+      CKR(sort_pairs(c, ar, B, &bkey, &p3, 64));
+      CK(cudaMemsetAsync(keep_b, 0, (size_t)B, s));
+      k_uq_first<<<grid_for(B, 256, c->sm_count), 256, 0, s>>>(B, bkey, p3, keep_b);
+      c->launches++;
+    }
+    CKR(exclusive_sum(c, ar, bcnt, bstart, G + 1));
+  }
+  // 9. blacklistItems: item groups of the log (membership is a group test), repeats within the list dropped
+  const long long NL = q->n_blacklist_items;
+  int32_t *lgid;
+  uint8_t *keep_l;
+  CKR(ar.alloc(&lgid, std::max<long long>(NL, 1)));
+  CKR(ar.alloc(&keep_l, std::max<long long>(NL, 1)));
+  if (NL > 0) {
+    str_hash(c, lc, ~0ULL);
+    if (E > 0) {
+      k_str_lookup<<<grid_for(NL, 256, c->sm_count), 256, 0, s>>>(NL, lc.off, lc.base, lc.w, lc.hash, ti.off, ti.base, ti.w, ti.hash,
+                                                                 (uint64_t)it.cap - 1, it.table, it.rank_of_slot, lgid);
+      c->launches++;
+    } else {
+      CK(cudaMemsetAsync(lgid, 0xff, sizeof(int32_t) * (size_t)NL, s));
+    }
+    StrTable lt;
+    int32_t *lid;
+    CKR(ar.alloc(&lid, NL));
+    CKR(str_group(c, ar, lc, nullptr, false, 0, &lt, lid));
+    k_uq_list_first<<<grid_for(NL, 256, c->sm_count), 256, 0, s>>>(NL, lid, lt.first_sorted, keep_l);
+    c->launches++;
+  }
+  // 10. the records' users
+  long long R = 0;
+  int32_t *rec_uid;
+  if (uoff) {
+    R = n_users;
+    CKR(ar.alloc(&rec_uid, std::max<long long>(R, 1)));
+    if (R > 0 && E > 0) {
+      str_hash(c, uc, ~0ULL);
+      k_str_lookup<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, uc.off, uc.base, uc.w, uc.hash, tu.off, tu.base, tu.w, tu.hash,
+                                                                (uint64_t)ut.cap - 1, ut.table, ut.rank_of_slot, rec_uid);
+      c->launches++;
+    } else if (R > 0) {
+      CK(cudaMemsetAsync(rec_uid, 0xff, sizeof(int32_t) * (size_t)R, s));
+    }
+  } else {   // every user with an event of a query name, by first line
+    R = G;
+    CKR(ar.alloc(&rec_uid, std::max<long long>(R, 1)));
+    if (R > 0) {
+      unsigned long long *mn, *uk;
+      CKR(ar.alloc(&mn, G));
+      CKR(ar.alloc(&uk, G));
+      CK(cudaMemsetAsync(mn, 0xff, sizeof(unsigned long long) * (size_t)G, s));
+      k_uq_min_line<<<grid_for(E, 256, c->sm_count), 256, 0, s>>>(E, uid, ln, mn);
+      k_uq_user_keys<<<grid_for(G, 256, c->sm_count), 256, 0, s>>>(G, mn, uk, rec_uid);
+      c->launches += 2;
+      CKR(sort_pairs(c, ar, G, &uk, &rec_uid, bits_for(lg->n_lines)));
+    }
+    if (out_users) {
+      uint32_t *ue;
+      long long *len, *off, total = 0;
+      CKR(ar.alloc(&ue, std::max<long long>(R, 1)));
+      CKR(ar.alloc(&len, R + 1));
+      CKR(ar.alloc(&off, R + 1));
+      CK(cudaMemsetAsync(len + R, 0, 8, s));
+      if (R > 0) {
+        k_uq_user_entry<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, rec_uid, ut.first_sorted, ue);
+        k_str_dict_len<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, ue, tu.off, len);
+        c->launches += 2;
+      }
+      CKR(exclusive_sum(c, ar, len, off, R + 1));
+      CK(cudaMemcpyAsync(&total, off + R, 8, cudaMemcpyDeviceToHost, s));
+      CK(cudaStreamSynchronize(s));
+      unsigned char *ub;
+      CKR(ar.alloc(&ub, std::max<long long>(total, 1)));
+      if (R > 0 && total > 0) {
+        k_str_dict_gather<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, ue, tu.off, tu.base, (const unsigned char *)tu.w, off, ub);
+        c->launches++;
+      }
+      int64_t *ho = (int64_t *)c->pinned_get(sizeof(int64_t) * ((size_t)R + 1), /*for_result=*/false);
+      char *hb = (char *)c->pinned_get((size_t)std::max<long long>(total, 1), /*for_result=*/false);
+      if (!ho || !hb) return set_error(CCO_E_OOM, "pinned host allocation failed");
+      CK(cudaMemcpyAsync(ho, off, sizeof(int64_t) * ((size_t)R + 1), cudaMemcpyDeviceToHost, s));
+      if (total > 0) CK(cudaMemcpyAsync(hb, ub, (size_t)total, cudaMemcpyDeviceToHost, s));
+      *out_users = cco_dictionary_t{R, ho, hb};
+    }
+  }
+  // 11. the template, then a length pass, the record offsets and a write pass: one warp per record
+  const std::vector<std::string> tp = uq_template(q);
+  std::vector<long long> toff(tp.size() + 1, 0);
+  std::string tb;
+  for (size_t j = 0; j < tp.size(); ++j) {
+    tb += tp[j];
+    toff[j + 1] = (long long)tb.size();
+  }
+  long long *d_toff;
+  unsigned char *d_tb;
+  CKR(ar.alloc(&d_toff, (long long)toff.size()));
+  CKR(ar.alloc(&d_tb, std::max<long long>((long long)tb.size(), 1)));
+  CK(cudaMemcpyAsync(d_toff, toff.data(), sizeof(long long) * toff.size(), cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(d_tb, tb.data(), tb.size(), cudaMemcpyHostToDevice, s));
+  UqArgs a;
+  a.n_rec = R;
+  a.rec_uid = rec_uid;
+  a.nq = nq;
+  a.n_kept = q->n_history_names;
+  a.limit = d_limit;
+  a.hstart = hstart;
+  a.hord = hord;
+  a.keep_h = keep_h;
+  a.bstart = bstart;
+  a.bord = bord;
+  a.keep_b = keep_b;
+  a.bkey = bkey;
+  a.B = B;
+  a.ent = ent;
+  a.ioff = E > 0 ? lg->ti.off : nullptr;
+  a.ibytes = E > 0 ? (const unsigned char *)lg->ti.w : nullptr;
+  a.n_list = NL;
+  a.loff = lc.off;
+  a.lbase = lc.base;
+  a.lbytes = (const unsigned char *)lc.w;
+  a.lgid = lgid;
+  a.keep_l = keep_l;
+  a.toff = d_toff;
+  a.tbytes = d_tb;
+  long long *rlen, *roff;
+  CKR(ar.alloc(&rlen, R + 1));
+  CKR(ar.alloc(&roff, R + 1));
+  CK(cudaMemsetAsync(rlen + R, 0, 8, s));
+  if (R > 0) {
+    k_uq_record<false><<<grid_for(R * 32, 256, c->sm_count), 256, 0, s>>>(a, nullptr, rlen, nullptr);
+    c->launches++;
+  }
+  CKR(exclusive_sum(c, ar, rlen, roff, R + 1));
+  int64_t *ho = (int64_t *)c->pinned_get(sizeof(int64_t) * ((size_t)R + 1), /*for_result=*/false);
+  if (!ho) return set_error(CCO_E_OOM, "pinned host allocation failed");
+  CK(cudaMemcpyAsync(ho, roff, sizeof(int64_t) * ((size_t)R + 1), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  for (long long r = 0; r < R; ++r)
+    if (ho[r + 1] - ho[r] >= (1LL << 31)) {
+      c->pinned_put(ho);
+      return set_error(CCO_E_UNSUPPORTED, "record %lld has %lld bytes, at most 2^31 - 1", r, (long long)(ho[r + 1] - ho[r]));
+    }
+  const long long total = ho[R];
+  unsigned char *d_out;
+  CKR(ar.alloc(&d_out, std::max<long long>(total, 1)));
+  if (R > 0 && total > 0) {
+    k_uq_record<true><<<grid_for(R * 32, 256, c->sm_count), 256, 0, s>>>(a, roff, nullptr, d_out);
+    c->launches++;
+  }
+  char *host = (char *)c->pinned_get((size_t)std::max<long long>(total, 1), /*for_result=*/false);
+  if (!host) return set_error(CCO_E_OOM, "pinned host allocation failed");
+  if (total > 0) CK(cudaMemcpyAsync(host, d_out, (size_t)total, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  *out_body = host;
+  *out_len = total;
+  *out_offsets = ho;
+  *out_n = R;
+  return CCO_OK;
+}
+}  // namespace cco
+
+int cco_event_log_begin_ex(cco_ctx_t *ctx, int64_t chunk_bytes, const cco_event_window_t *w, uint32_t flags, cco_event_log_t **out) {
+  if (flags & ~(uint32_t)CCO_LOG_KEEP_HISTORY) return set_error(CCO_E_INVALID_ARG, "unknown flags 0x%x", (unsigned)flags);
+  CKR(cco_event_log_begin_window(ctx, chunk_bytes, w, out));
+  (*out)->history = (flags & CCO_LOG_KEEP_HISTORY) != 0;
+  return CCO_OK;
+}
+
+int cco_event_log_user_queries(cco_ctx_t *ctx, const cco_event_log_t *lg, const cco_user_query_t *q, int64_t n_users,
+                               const int64_t *user_offsets, const char *user_bytes, char **out_body, int64_t *out_len,
+                               int64_t **out_offsets, int64_t *out_n, cco_dictionary_t *out_users) {
+  if (!ctx || !lg || !q || !out_body || !out_len || !out_offsets || !out_n) return set_error(CCO_E_INVALID_ARG, "null argument");
+  if (!ctx->members.empty() || lg->ctx != ctx) return set_error(CCO_E_UNSUPPORTED, "build queries on the per-GPU context that read the log");
+  CKR(log_state(lg, true));
+  CKR(uq_check_host(q, n_users, user_offsets, user_bytes));
+  if (!lg->history) return set_error(CCO_E_INVALID_ARG, "the log was read without history retention (cco_event_log_begin_ex, CCO_LOG_KEEP_HISTORY)");
+  if (out_users) *out_users = cco_dictionary_t{0, nullptr, nullptr};
+  return user_queries(ctx, lg, q, n_users, user_offsets, user_bytes, out_body, out_len, out_offsets, out_n, out_users);
 }
 
 int cco_event_log_free(cco_event_log_t *lg) {

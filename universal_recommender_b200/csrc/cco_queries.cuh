@@ -1,0 +1,295 @@
+// cco_queries.cuh -- cco_event_log_user_queries: buildQuery (URAlgorithm.scala:563-739) for user queries over the training
+// history an event log keeps (cco_event_log_begin_ex with CCO_LOG_KEEP_HISTORY).
+//
+// e = one training event of a query event name (name rank q); its user and item are dense group ids of the log's columns.
+//   k_uq_select       e -> (log entry, name rank) over the query names' ranges of the name-partitioned columns
+//   k_uq_gather       per e: user group, item group, time and global line of its log entry
+//   k_uq_key_line / k_uq_key_time / k_uq_key_seg / k_uq_key_user   radix keys: line desc, time desc, (user, q), user
+//   k_uq_count        segment sizes (histogram) -> scan -> segment starts
+//   k_uq_hist_keys    the first `limit` of every (user, q) segment: (segment, item) keys, fed oldest first, so that the
+//                     first of each run after the stable sort is the item's oldest position (distinct after the prepend)
+//   k_uq_first        first of each run of equal keys -> keep flag
+//   k_uq_min_line     each user's first line (the record order when every user is asked for)
+//   k_uq_record       one warp per record: template pieces, history lists oldest first, the blacklist; a length pass and a
+//                     write pass (k_doc_len -> scan -> k_doc_write, as cco_format_model).  Ids are escaped as json4s
+//                     3.2 quotes them.
+#pragma once
+
+namespace cco {
+
+constexpr int kUqMaxNames = 64;
+
+__global__ void k_uq_select(long long E, int nq, const long long *__restrict__ qoff, const long long *__restrict__ qbase,
+                            uint32_t *__restrict__ ent, uint8_t *__restrict__ qr) {
+  for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < E; e += (long long)gridDim.x * blockDim.x) {
+    int lo = 0, hi = nq - 1;   // the last q with qoff[q] <= e
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (qoff[mid] <= e) lo = mid; else hi = mid - 1;
+    }
+    ent[e] = (uint32_t)(qbase[lo] + (e - qoff[lo]));
+    qr[e] = (uint8_t)lo;
+  }
+}
+
+__global__ void k_uq_gather(long long E, const uint32_t *__restrict__ ent, const int32_t *__restrict__ ugid, const int32_t *__restrict__ igid,
+                            const long long *__restrict__ ttime, const long long *__restrict__ tline, int32_t *__restrict__ uid,
+                            int32_t *__restrict__ iid, long long *__restrict__ tm, long long *__restrict__ ln) {
+  for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < E; e += (long long)gridDim.x * blockDim.x) {
+    const uint32_t x = ent[e];
+    uid[e] = ugid[x];
+    iid[e] = igid[x];
+    tm[e] = ttime[x];
+    ln[e] = tline[x];
+  }
+}
+
+// keys of the first sort (line descending) over e = 0 .. E-1
+__global__ void k_uq_key_line(long long E, long long n_lines, const long long *__restrict__ ln, unsigned long long *__restrict__ key,
+                              uint32_t *__restrict__ val) {
+  for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < E; e += (long long)gridDim.x * blockDim.x) {
+    key[e] = (unsigned long long)(n_lines - 1 - ln[e]);
+    val[e] = (uint32_t)e;
+  }
+}
+// time descending, over the current order
+__global__ void k_uq_key_time(long long E, const uint32_t *__restrict__ val, const long long *__restrict__ tm, unsigned long long *__restrict__ key) {
+  for (long long p = blockIdx.x * (long long)blockDim.x + threadIdx.x; p < E; p += (long long)gridDim.x * blockDim.x)
+    key[p] = ~((unsigned long long)tm[val[p]] ^ 0x8000000000000000ULL);
+}
+// (user, q) segment, over the current order
+__global__ void k_uq_key_seg(long long E, int nq, const uint32_t *__restrict__ val, const int32_t *__restrict__ uid,
+                             const uint8_t *__restrict__ qr, unsigned long long *__restrict__ key) {
+  for (long long p = blockIdx.x * (long long)blockDim.x + threadIdx.x; p < E; p += (long long)gridDim.x * blockDim.x) {
+    const uint32_t e = val[p];
+    key[p] = (unsigned long long)uid[e] * (unsigned long long)nq + qr[e];
+  }
+}
+// the blacklisted events (their name rank is flagged) in the current order -> keep flags
+__global__ void k_uq_flag_black(long long E, const uint32_t *__restrict__ val, const uint8_t *__restrict__ qr, const uint8_t *__restrict__ black,
+                                uint32_t *__restrict__ keep) {
+  for (long long p = blockIdx.x * (long long)blockDim.x + threadIdx.x; p < E; p += (long long)gridDim.x * blockDim.x)
+    keep[p] = black[qr[val[p]]] ? 1u : 0u;
+}
+// the selected positions' events with their user as key
+__global__ void k_uq_key_user(long long B, const uint32_t *__restrict__ idx, const uint32_t *__restrict__ order, const int32_t *__restrict__ uid,
+                              unsigned long long *__restrict__ key, uint32_t *__restrict__ val) {
+  for (long long p = blockIdx.x * (long long)blockDim.x + threadIdx.x; p < B; p += (long long)gridDim.x * blockDim.x) {
+    const uint32_t e = order[idx[p]];
+    val[p] = e;
+    key[p] = (unsigned long long)(uint32_t)uid[e];
+  }
+}
+__global__ void k_uq_count(long long n, const unsigned long long *__restrict__ key, long long *__restrict__ cnt) {
+  for (long long p = blockIdx.x * (long long)blockDim.x + threadIdx.x; p < n; p += (long long)gridDim.x * blockDim.x)
+    atomicAdd((unsigned long long *)&cnt[key[p]], 1ULL);
+}
+// history: position p of the (user, q)-sorted order is taken iff it is among the first limit[q] of its segment; the taken
+// ones get the key (segment << 32 | item), written at E - 1 - p so that the stable sort puts the oldest position first
+__global__ void k_uq_hist_keys(long long E, int nq, const unsigned long long *__restrict__ seg, const long long *__restrict__ start,
+                               const int32_t *__restrict__ limit, const uint32_t *__restrict__ val, const int32_t *__restrict__ iid,
+                               unsigned long long *__restrict__ key, uint32_t *__restrict__ pos) {
+  for (long long p = blockIdx.x * (long long)blockDim.x + threadIdx.x; p < E; p += (long long)gridDim.x * blockDim.x) {
+    const unsigned long long s = seg[p];
+    const bool taken = p - start[s] < (long long)limit[s % (unsigned long long)nq];
+    key[E - 1 - p] = taken ? (s << 32) | (uint32_t)iid[val[p]] : ~0ULL;
+    pos[E - 1 - p] = (uint32_t)p;
+  }
+}
+// blacklist: (user << 32 | item) of the user-sorted blacklisted events, position as value
+__global__ void k_uq_black_keys(long long B, const uint32_t *__restrict__ val, const int32_t *__restrict__ uid, const int32_t *__restrict__ iid,
+                                unsigned long long *__restrict__ key, uint32_t *__restrict__ pos) {
+  for (long long p = blockIdx.x * (long long)blockDim.x + threadIdx.x; p < B; p += (long long)gridDim.x * blockDim.x) {
+    const uint32_t e = val[p];
+    key[p] = ((unsigned long long)(uint32_t)uid[e] << 32) | (uint32_t)iid[e];
+    pos[p] = (uint32_t)p;
+  }
+}
+__global__ void k_uq_first(long long n, const unsigned long long *__restrict__ key, const uint32_t *__restrict__ pos, uint8_t *__restrict__ keep) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    if (key[i] != ~0ULL && (i == 0 || key[i - 1] != key[i])) keep[pos[i]] = 1;
+}
+// blacklistItems: an entry is kept iff it is its string's first appearance in the list
+__global__ void k_uq_list_first(long long n, const int32_t *__restrict__ lid, const uint32_t *__restrict__ first_sorted, uint8_t *__restrict__ keep) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    keep[i] = first_sorted[lid[i]] == (uint32_t)i ? 1 : 0;
+}
+__global__ void k_uq_min_line(long long E, const int32_t *__restrict__ uid, const long long *__restrict__ ln, unsigned long long *__restrict__ mn) {
+  for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < E; e += (long long)gridDim.x * blockDim.x)
+    atomicMin(&mn[uid[e]], (unsigned long long)ln[e]);
+}
+__global__ void k_uq_user_keys(long long G, const unsigned long long *__restrict__ mn, unsigned long long *__restrict__ key, int32_t *__restrict__ val) {
+  for (long long g = blockIdx.x * (long long)blockDim.x + threadIdx.x; g < G; g += (long long)gridDim.x * blockDim.x) {
+    key[g] = mn[g];
+    val[g] = (int32_t)g;
+  }
+}
+// the log entry that names each record's user (its group's first entry), for the users' dictionary
+__global__ void k_uq_user_entry(long long R, const int32_t *__restrict__ rec_uid, const uint32_t *__restrict__ first_sorted, uint32_t *__restrict__ e) {
+  for (long long r = blockIdx.x * (long long)blockDim.x + threadIdx.x; r < R; r += (long long)gridDim.x * blockDim.x)
+    e[r] = first_sorted[rec_uid[r]];
+}
+
+// json4s 3.2 quote: '"' and '\' get a backslash, \b \f \n \r \t their short forms, every other code point below U+0020, in
+// U+0080..U+009F (UTF-8 C2 80..C2 9F) and in U+2000..U+20FF (E2 80 80..E2 83 BF) becomes \u%04x in lowercase hex; the rest
+// passes through.  o == nullptr: the length only.
+__device__ __forceinline__ long long uq_escape(const unsigned char *__restrict__ s, long long n, unsigned char *o) {
+  long long k = 0;
+  for (long long i = 0; i < n; ++i) {
+    const unsigned char b = s[i];
+    unsigned cp = 0xffffffffu;
+    unsigned char sh = 0;
+    if (b == '"' || b == '\\') sh = b;
+    else if (b == '\b') sh = 'b';
+    else if (b == '\f') sh = 'f';
+    else if (b == '\n') sh = 'n';
+    else if (b == '\r') sh = 'r';
+    else if (b == '\t') sh = 't';
+    else if (b < 0x20) cp = b;
+    else if (b == 0xC2 && i + 1 < n && s[i + 1] >= 0x80 && s[i + 1] <= 0x9F) {
+      cp = s[i + 1];
+      i += 1;
+    } else if (b == 0xE2 && i + 2 < n && s[i + 1] >= 0x80 && s[i + 1] <= 0x83 && (s[i + 2] & 0xC0) == 0x80) {
+      cp = 0x2000u | ((unsigned)(s[i + 1] & 0x3F) << 6) | (s[i + 2] & 0x3F);
+      i += 2;
+    }
+    if (sh) {
+      if (o) {
+        o[k] = '\\';
+        o[k + 1] = sh;
+      }
+      k += 2;
+    } else if (cp != 0xffffffffu) {
+      if (o) {
+        o[k] = '\\';
+        o[k + 1] = 'u';
+        for (int d = 0; d < 4; ++d) o[k + 2 + d] = "0123456789abcdef"[(cp >> (12 - 4 * d)) & 15];
+      }
+      k += 6;
+    } else {
+      if (o) o[k] = b;
+      k += 1;
+    }
+  }
+  return k;
+}
+
+struct UqArgs {
+  long long n_rec;
+  const int32_t *rec_uid;          // [n_rec] user group, -1: a user without history
+  int nq, n_kept;                  // query names; history lists written for q < n_kept
+  const int32_t *limit;            // [nq]
+  const long long *hstart;         // [G * nq + 1] segment starts in the (user, q) order
+  const uint32_t *hord;            // [E] events in (user, q, time desc, line desc) order
+  const uint8_t *keep_h;           // [E] by position: taken and the item's oldest taken position
+  const long long *bstart;         // [G + 1]
+  const uint32_t *bord;            // [B] blacklisted events in (user, time desc, line desc) order
+  const uint8_t *keep_b;           // [B] by position: the item's newest position
+  const unsigned long long *bkey;  // [B] (user << 32 | item), sorted
+  long long B;
+  const uint32_t *ent;             // [E] log entry of each event
+  const long long *ioff;           // the log's training item column
+  const unsigned char *ibytes;
+  long long n_list;                // blacklistItems
+  const long long *loff;           // the caller's offsets: bytes at lbytes[loff[i] - lbase]
+  long long lbase;
+  const unsigned char *lbytes;
+  const int32_t *lgid;             // item group or -1
+  const uint8_t *keep_l;
+  const long long *toff;           // [n_kept + 3] template pieces
+  const unsigned char *tbytes;
+};
+
+__device__ __forceinline__ bool uq_has(const UqArgs &a, int32_t u, int32_t g) {
+  const unsigned long long x = ((unsigned long long)(uint32_t)u << 32) | (uint32_t)g;
+  long long lo = a.bstart[u], hi = a.bstart[u + 1];
+  while (lo < hi) {
+    const long long mid = (lo + hi) >> 1;
+    if (a.bkey[mid] < x) lo = mid + 1; else hi = mid;
+  }
+  return lo < a.bstart[u + 1] && a.bkey[lo] == x;
+}
+
+// one list of quoted, comma-separated ids from n candidates; get(i, &ptr, &len) == false skips candidate i.  cur and
+// first are warp-uniform.
+template <class Get>
+__device__ __forceinline__ void uq_list(long long n, const Get &get, unsigned char *o, long long &cur, bool &first) {
+  const int lane = threadIdx.x & 31;
+  for (long long b = 0; b < n; b += 32) {
+    const long long i = b + lane;
+    const unsigned char *p = nullptr;
+    long long len = 0;
+    const bool keep = i < n && get(i, &p, &len);
+    const unsigned ball = __ballot_sync(0xffffffffu, keep);
+    if (!ball) continue;
+    const bool lead = first && lane == __ffs(ball) - 1;
+    const long long el = keep ? uq_escape(p, len, nullptr) + 2 + (lead ? 0 : 1) : 0;
+    long long x = el;
+    for (int d = 1; d < 32; d <<= 1) {
+      const long long y = __shfl_up_sync(0xffffffffu, x, d);
+      if (lane >= d) x += y;
+    }
+    if (o && keep) {
+      unsigned char *q = o + cur + x - el;
+      if (!lead) *q++ = ',';
+      *q++ = '"';
+      q += uq_escape(p, len, q);
+      *q = '"';
+    }
+    cur += __shfl_sync(0xffffffffu, x, 31);
+    first = false;
+  }
+}
+
+template <bool WRITE>
+__global__ void __launch_bounds__(256) k_uq_record(UqArgs a, const long long *__restrict__ rec_off, long long *__restrict__ rec_len,
+                                                   unsigned char *__restrict__ out) {
+  const int lane = threadIdx.x & 31;
+  const long long warps = (long long)gridDim.x * (blockDim.x >> 5);
+  for (long long r = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5; r < a.n_rec; r += warps) {
+    const int32_t u = a.rec_uid[r];
+    unsigned char *o = WRITE ? out + rec_off[r] : nullptr;
+    long long cur = 0;
+    for (int j = 0; j <= a.n_kept + 1; ++j) {
+      const long long t0 = a.toff[j], tl = a.toff[j + 1] - t0;
+      if (WRITE)
+        for (long long k = lane; k < tl; k += 32) o[cur + k] = a.tbytes[t0 + k];
+      cur += tl;
+      if (j > a.n_kept) break;
+      bool first = true;
+      if (j < a.n_kept) {   // the history of name j, oldest first, each item at its first position
+        if (u < 0) continue;
+        const unsigned long long s = (unsigned long long)u * a.nq + j;
+        const long long h0 = a.hstart[s], cnt = min(a.hstart[s + 1] - h0, (long long)a.limit[j]);
+        uq_list(cnt, [&](long long i, const unsigned char **p, long long *len) {
+          const long long pos = h0 + cnt - 1 - i;
+          if (!a.keep_h[pos]) return false;
+          const uint32_t e = a.ent[a.hord[pos]];
+          *p = a.ibytes + a.ioff[e];
+          *len = a.ioff[e + 1] - a.ioff[e];
+          return true;
+        }, o, cur, first);
+      } else {   // the blacklist: the user's blacklisted items newest first, then blacklistItems, distinct
+        if (u >= 0) {
+          const long long b0 = a.bstart[u];
+          uq_list(a.bstart[u + 1] - b0, [&](long long i, const unsigned char **p, long long *len) {
+            if (!a.keep_b[b0 + i]) return false;
+            const uint32_t e = a.ent[a.bord[b0 + i]];
+            *p = a.ibytes + a.ioff[e];
+            *len = a.ioff[e + 1] - a.ioff[e];
+            return true;
+          }, o, cur, first);
+        }
+        uq_list(a.n_list, [&](long long i, const unsigned char **p, long long *len) {
+          if (!a.keep_l[i] || (u >= 0 && a.lgid[i] >= 0 && uq_has(a, u, a.lgid[i]))) return false;
+          *p = a.lbytes + (a.loff[i] - a.lbase);
+          *len = a.loff[i + 1] - a.loff[i];
+          return true;
+        }, o, cur, first);
+      }
+    }
+    if (!WRITE && lane == 0) rec_len[r] = cur;
+  }
+}
+
+}  // namespace cco

@@ -326,7 +326,7 @@ class CcoContext:
         return rk
 
     def read_events(self, src, chunk_bytes: Optional[int] = None, window: Optional[E.EventWindow] = None,
-                    now_ms: Optional[int] = None) -> "EventLog":
+                    now_ms: Optional[int] = None, keep_history: bool = False) -> "EventLog":
         """A PredictionIO event export (JSON lines, as `pio export` writes them) parsed on the device.  src is one of
           - bytes or a buffer: one read (cco_event_log_read), or chunks of chunk_bytes when it is given;
           - a file path, a directory as `pio export` writes it (its part-* files in name order; events.export_parts) or a
@@ -339,9 +339,11 @@ class CcoContext:
         window: the DataSource's eventWindow (events.EventWindow; cco_event_log_begin_window), applied on the device while the
         export is read: events at or before now_ms - duration expire ($set / $unset excepted), and with removeDuplicates
         equal events collapse to the latest.  now_ms defaults to the wall clock; EventLog.window_stats() counts the drops.
+        keep_history: keep every training event's time and line (cco_event_log_begin_ex, CCO_LOG_KEEP_HISTORY), which
+        user_queries reads; a log read without it is exactly the log read before the option existed.
         -> EventLog (free with .free(), or use it as a context manager; close() of this context frees the logs still open)."""
         whole = isinstance(src, (bytes, bytearray, memoryview, np.ndarray)) and chunk_bytes is None
-        if whole and window is None:
+        if whole and window is None and not keep_history:
             buf = np.frombuffer(src, dtype=np.uint8) if not isinstance(src, np.ndarray) else np.ascontiguousarray(src, dtype=np.uint8)
             h = C.c_void_p()
             N.check(self._L.cco_event_log_read(self._h, buf.ctypes.data if len(buf) else None, len(buf), C.byref(h)))
@@ -354,12 +356,16 @@ class CcoContext:
         elif isinstance(src, (list, tuple)) and all(isinstance(x, (str, os.PathLike)) for x in src):
             paths = [os.fspath(x) for x in src]
         h = C.c_void_p()
-        if window is None:
-            N.check(self._L.cco_event_log_begin(self._h, chunk, C.byref(h)))
-        else:
+        w = None
+        if window is not None:
             now = now_ms if now_ms is not None else int(time.time() * 1000)
             cutoff = window.cutoff_ms(now)
             w = N.EventWindowT(-(1 << 63) if cutoff is None else cutoff, 1 if window.removeDuplicates else 0, 0)
+        if keep_history:
+            N.check(self._L.cco_event_log_begin_ex(self._h, chunk, C.byref(w) if w is not None else None, N.LOG_KEEP_HISTORY, C.byref(h)))
+        elif w is None:
+            N.check(self._L.cco_event_log_begin(self._h, chunk, C.byref(h)))
+        else:
             N.check(self._L.cco_event_log_begin_window(self._h, chunk, C.byref(w), C.byref(h)))
         try:
             if paths is not None:
@@ -454,6 +460,48 @@ class CcoContext:
             self.free_dataset(dataset)
             raise
         return dataset, users, items
+
+    def user_queries(self, log: "EventLog", ap, query=None, users=None, now_ms: Optional[int] = None, header: str = "{}"):
+        """cco_event_log_user_queries: URAlgorithm.buildQuery for every user (ur_query.py restates it), from the history of a
+        log read with keep_history=True.  ap: ur_algorithm.URAlgorithmParams; query: ur_query.UserQuery (None: defaults);
+        users: the user ids, or None for every user with a training event of a query event name, by first line.
+        -> (body, offsets int64[n + 1]): `header\nquery\n` records, the _msearch body; record r = body[offsets[r]:offsets[r + 1]].
+        With users=None -> (body, offsets, users)."""
+        from . import ur_query as Q
+        plan = Q.plan(ap, query or Q.UserQuery(), now_ms)
+        enc = lambda xs: [x.encode("utf-8", "surrogatepass") for x in xs]
+        names, black = enc(plan.names), enc(plan.blacklist)
+        nm = (C.c_char_p * max(len(names), 1))(*names)
+        bl = (C.c_char_p * max(len(black), 1))(*black)
+        lim = np.ascontiguousarray(plan.limits, dtype=np.int32) if plan.names else np.zeros(1, np.int32)
+        lo, lb = encode_ids(list(plan.blacklist_items))
+        qt = N.UserQueryT(len(names), plan.n_history, nm, lim.ctypes.data_as(C.POINTER(C.c_int32)), len(black), 1 if plan.in_must else 0, bl,
+                          None if plan.boost is None else plan.boost.encode(), plan.head.encode("utf-8", "surrogatepass"),
+                          plan.should.encode("utf-8", "surrogatepass"), plan.must.encode("utf-8", "surrogatepass"),
+                          plan.must_not.encode("utf-8", "surrogatepass"), plan.sort.encode("utf-8", "surrogatepass"),
+                          header.encode("utf-8", "surrogatepass"), len(lo) - 1, lo.ctypes.data_as(C.POINTER(C.c_int64)),
+                          lb.ctypes.data if len(lb) else None)
+        out, ln, off, n = C.c_void_p(), C.c_int64(), C.c_void_p(), C.c_int64()
+        ud = N.DictionaryT()
+        if users is None:
+            N.check(self._L.cco_event_log_user_queries(self._h, log._h, C.byref(qt), 0, None, None, C.byref(out), C.byref(ln), C.byref(off),
+                                                       C.byref(n), C.byref(ud)))
+        else:
+            uo, ub = encode_ids(list(users))
+            N.check(self._L.cco_event_log_user_queries(self._h, log._h, C.byref(qt), len(uo) - 1, uo.ctypes.data_as(C.POINTER(C.c_int64)),
+                                                       ub.ctypes.data if len(ub) else None, C.byref(out), C.byref(ln), C.byref(off),
+                                                       C.byref(n), None))
+        offsets = np.ctypeslib.as_array(C.cast(off, C.POINTER(C.c_int64)), shape=(n.value + 1,)).copy()
+        self._L.cco_host_free(self._h, off)
+        body = self._take_body(out, ln)
+        if users is not None:
+            return body, offsets
+        uoff = np.ctypeslib.as_array(ud.offsets, shape=(ud.n + 1,)).copy()
+        addr = C.c_void_p.from_buffer(ud, N.DictionaryT.bytes.offset).value
+        ids = decode_ids(uoff, C.string_at(addr, int(uoff[-1])) if uoff[-1] else b"")
+        self._L.cco_host_free(self._h, C.cast(ud.offsets, C.c_void_p))
+        self._L.cco_host_free(self._h, C.c_void_p(addr))
+        return body, offsets, ids
 
     def rerank_model(self, body: bytes, properties=None, rankings=None, log=None) -> bytes:
         """cco_rerank_model: calcPop (URAlgorithm.scala:375-399, recsModel "backfill") on an existing index.  body = the

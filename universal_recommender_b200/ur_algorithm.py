@@ -3,7 +3,10 @@
 calc_all_on_device runs the whole train half on the GPU, string events in and the Elasticsearch bulk body out.
 calc_pop_on_device runs calcPop (recsModel "backfill") on the GPU: the current index's bulk body in, the same index with
 fresh rankings out.  calc_all_from_events / calc_pop_from_events do the same from a PredictionIO event export parsed on the
-device (CcoContext.read_events), the DataSource included.  Everything else in URAlgorithm (ES reads and query building) is out of scope."""
+device (CcoContext.read_events), the DataSource included.  user_queries_from_events builds buildQuery's user queries for a
+whole user base from the same export (ur_query.py restates buildQuery).  Out of scope: item and item-set queries (they need
+each item's correlators, which a kept train result could supply), Elasticsearch's scoring, reading the index and the HTTP
+call."""
 from __future__ import annotations
 
 import time
@@ -12,6 +15,7 @@ from typing import Optional, Sequence
 
 from .indexed_dataset import IndexedDataset
 from .similarity_analysis import CcoContext, DownsamplableCrossOccurrenceDataset, SimilarityAnalysis, default_context, encode_ids
+from .ur_query import Field, UserQuery
 from .ur_model import (RankingParams, RankingType, extract_jvalue, property_json, ranking_window, rankings_for,
                        rankings_params)
 
@@ -45,6 +49,16 @@ class URAlgorithmParams:
     # sampleDownAndBinarize (SURVEY.md A.1; every interaction of a user above maxItemsPerUser is dropped) instead of the
     # real division min(m, d) / d this build defaults to (INTEGRATION.md "Deviation to know about")
     rowRateIntDiv: bool = False
+    # query-side keys (buildQuery, ur_query.py); the train ignores them
+    blacklistEvents: Optional[Sequence[str]] = None
+    maxQueryEvents: Optional[int] = None
+    num: Optional[int] = None
+    userBias: Optional[float] = None
+    fields: Optional[Sequence[Field]] = None
+    availableDateName: Optional[str] = None
+    expireDateName: Optional[str] = None
+    dateName: Optional[str] = None
+    indexName: Optional[str] = None
 
     @staticmethod
     def from_engine_json(algo_params: dict) -> "URAlgorithmParams":
@@ -57,7 +71,12 @@ class URAlgorithmParams:
                                                                  i.get("maxCorrelatorsPerItem"), i.get("minLLR")) for i in ind],
             seed=algo_params.get("seed"), recsModel=algo_params.get("recsModel", "all"),
             rankings=None if algo_params.get("rankings") is None else [RankingParams.from_json(r) for r in algo_params["rankings"]],
-            rowRateIntDiv=bool(algo_params.get("rowRateIntDiv", False)))
+            rowRateIntDiv=bool(algo_params.get("rowRateIntDiv", False)),
+            blacklistEvents=algo_params.get("blacklistEvents"), maxQueryEvents=algo_params.get("maxQueryEvents"),
+            num=algo_params.get("num"), userBias=algo_params.get("userBias"),
+            fields=None if algo_params.get("fields") is None else [Field.from_json(f) for f in algo_params["fields"]],
+            availableDateName=algo_params.get("availableDateName"), expireDateName=algo_params.get("expireDateName"),
+            dateName=algo_params.get("dateName"), indexName=algo_params.get("indexName"))
 
     def model_event_names(self) -> list[str]:
         """URAlgorithm.scala:230-235: the indicator names if given, else eventNames"""
@@ -283,3 +302,24 @@ def calc_pop_from_events(body: bytes, export, ap: URAlgorithmParams, now_ms: Opt
     finally:
         if owned:
             log.free()
+
+
+def user_queries_from_events(export, ap: URAlgorithmParams, query: Optional[UserQuery] = None, users=None, now_ms: Optional[int] = None,
+                             ctx: CcoContext | None = None, event_window=None, header: str = "{}"):
+    """buildQuery (URAlgorithm.scala:563-839) for every user of `users` (None: every user with a training event of a query
+    event name, by first line) from a PredictionIO event export read on the device with history retention: one
+    `header\nquery\n` record per user, the body of an Elasticsearch _msearch.  -> (body, offsets) as CcoContext.user_queries
+    ((body, offsets, users) for users=None).  now_ms: "now" of the available / expire date filter and of the eventWindow.
+    The query event names, limits, blacklist and fragments are ur_query.plan's."""
+    ctx = ctx or default_context()
+    now_ms = _now(now_ms)
+    from .similarity_analysis import EventLog
+    if isinstance(export, EventLog):
+        if event_window is not None:
+            raise ValueError("the eventWindow applies while an export is read")
+        return ctx.user_queries(export, ap, query, users, now_ms, header)
+    log = ctx.read_events(export, window=event_window, now_ms=now_ms, keep_history=True)
+    try:
+        return ctx.user_queries(log, ap, query, users, now_ms, header)
+    finally:
+        log.free()

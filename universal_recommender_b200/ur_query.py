@@ -1,0 +1,279 @@
+"""URAlgorithm.buildQuery for user queries (Query.user set; item, itemSet and withRanks absent), restated from
+src/main/scala/URAlgorithm.scala:195-267 (parameters), :563-767 (should / must / must_not / sort), :795-839
+(getBiasedRecentUserActions) and :872-953 (date filters).  The query is the text the reference posts to Elasticsearch;
+scoring stays with Elasticsearch.
+
+plan() renders what every user's query shares (the fragments CcoContext.user_queries hands to the device);
+user_queries() is the host mirror over events.read_export's output, the whole body built here.
+
+Quirks of the reference, kept on purpose:
+  * the per-name history limit is DefaultIndicatorParams().maxItemsPerUser = 100 whenever `eventNames` is given, even
+    next to `indicators`, and otherwise the indicator's maxItemsPerUser or 500 (:213-224); a query event name without an
+    entry raises KeyError, as the reference throws NoSuchElementException;
+  * maxQueryEvents with indicators is the sum of their maxItemsPerUser (100 each by default) times 10 (:202-210), and
+    only the first maxQueryEvents - 1 *names* get a terms clause: the slice is over names, not events (:575, :665);
+  * the should / must choice tests the algorithm's userBias, not the query's (:572, :660); the boost itself is the
+    query's userBias, else the algorithm's, written only when b > 0 and b != 1 (:823-824);
+  * the metadata signs are inverted between query and engine.json: boosts are query fields with bias > 0 plus params
+    fields with bias < 0, filters the other way round, exclusions bias == 0 of both (:844-867), each list distinct;
+  * a dateRange whose `after` or `before` is given writes one range clause even when the value is "", and leaves the
+    empty bound out (:878-918); otherwise availableDateName and expireDateName both set give the lte / gt pair against
+    currentDate, the query's or "now" as Joda's DateTime.toDateTimeISO.toString in UTC (yyyy-MM-ddTHH:mm:ss.SSSZ)
+    [RECALL: Joda 2.9];
+  * the history is the latest `limit` events of each name, prepended one by one (oldest first) and then `distinct`: an
+    item stays at its oldest position among them; a name without history still writes [] (:826-836);
+  * the blacklist is the targets of *all* the user's events of the query names that are also blacklistEvents (default:
+    the first model event name; [] means none), newest first, then blacklistItems, distinct (:742-767);
+  * sort is [] under recsModel "collabFiltering" (:730-738).
+Rendering is json4s 3.2.x compact(render(...)) [RECALL]: a Float is widened to Double and printed by Double.toString (a
+bias of 1.05 prints 1.0499999523162842, 2 prints 2.0), ints print plainly, and strings escape '"' and '\\', use the short
+forms \\b \\f \\n \\r \\t, and write every other code point below U+0020, in U+0080..U+009F and in U+2000..U+20FF as
+\\u%04x in lowercase hex.  Any valid escaping gives Elasticsearch the same query; the rule is fixed so that bytes compare.
+Date values and sort field names are interpolated into JSON text and parsed again by the reference; here they are written
+as escaped strings, the same text for every value that needs no escape.
+LEventStore.findByEntity is taken to read every event of the user, unlimited, latest first [RECALL: PredictionIO 0.12].
+
+Deviations:
+  * the history is the log's training events (entityType "user" -> targetEntityType "item"); findByEntity has no
+    target-type filter, so events aimed at other entity types, which the reference would read, are not read here;
+  * where the reference would throw on a target-less event of a query name, no such event exists here.
+"""
+from __future__ import annotations
+
+import datetime as _dt
+from dataclasses import dataclass, field
+from typing import Optional, Sequence
+
+import numpy as np
+
+from .ur_model import java_double, rankings_params
+
+MAX_QUERY_EVENTS = 100          # DefaultURAlgoParams.MaxQueryEvents (URAlgorithm.scala:57)
+MAX_EVENTS_PER_EVENT_TYPE = 500
+NUM_RESULTS = 20
+CONSTANT_SCORE = '{"constant_score":{"filter":{"match_all":{}},"boost":0}}'
+
+
+@dataclass
+class Field:
+    """Engine.scala:53-58: bias > 0 boosts, < 0 filters, 0 excludes (signs inverted for engine.json fields)"""
+    name: str
+    values: Sequence[str]
+    bias: float
+
+    @staticmethod
+    def from_json(d: dict) -> "Field":
+        return Field(d["name"], list(d["values"]), float(d["bias"]))
+
+
+@dataclass
+class DateRange:
+    """Engine.scala:61-65"""
+    name: str
+    before: Optional[str] = None
+    after: Optional[str] = None
+
+
+@dataclass
+class UserQuery:
+    """the user-query members of Query (Engine.scala:32-50); the user itself is the record's"""
+    userBias: Optional[float] = None
+    fields: Optional[Sequence[Field]] = None
+    currentDate: Optional[str] = None
+    dateRange: Optional[DateRange] = None
+    blacklistItems: Optional[Sequence[str]] = None
+    num: Optional[int] = None
+    from_: Optional[int] = None
+    eventNames: Optional[Sequence[str]] = None
+
+    @staticmethod
+    def from_json(d: dict) -> "UserQuery":
+        dr = d.get("dateRange")
+        return UserQuery(d.get("userBias"), None if d.get("fields") is None else [Field.from_json(f) for f in d["fields"]],
+                         d.get("currentDate"), None if dr is None else DateRange(dr["name"], dr.get("before"), dr.get("after")),
+                         d.get("blacklistItems"), d.get("num"), d.get("from"), d.get("eventNames"))
+
+
+def f32(x: float) -> float:
+    return float(np.float32(x))
+
+
+def json_string(s: str) -> str:
+    """json4s 3.2's quote, quotes included"""
+    out = ['"']
+    for ch in s:
+        c = ord(ch)
+        if ch in '"\\':
+            out.append("\\" + ch)
+        elif ch in "\b\f\n\r\t":
+            out.append({"\b": "\\b", "\f": "\\f", "\n": "\\n", "\r": "\\r", "\t": "\\t"}[ch])
+        elif c < 0x20 or 0x80 <= c < 0xA0 or 0x2000 <= c < 0x2100:
+            out.append("\\u%04x" % c)
+        else:
+            out.append(ch)
+    out.append('"')
+    return "".join(out)
+
+
+def jfloat(x: float) -> str:
+    """a Scala Float rendered by json4s: widened to Double, Double.toString"""
+    return java_double(f32(x))
+
+
+def iso_utc(ms: int) -> str:
+    """Joda DateTime.toDateTimeISO.toString in UTC"""
+    t = _dt.datetime(1970, 1, 1, tzinfo=_dt.timezone.utc) + _dt.timedelta(milliseconds=int(ms))
+    return t.strftime("%Y-%m-%dT%H:%M:%S.") + "%03dZ" % (t.microsecond // 1000)
+
+
+def terms(name: str, values: Sequence[str], boost: Optional[str]) -> str:
+    b = "" if boost is None else ',"boost":' + boost
+    return '{"terms":{' + json_string(name) + ":[" + ",".join(json_string(v) for v in values) + "]" + b + "}}"
+
+
+def _distinct(xs):
+    out = []
+    for x in xs:
+        if x not in out:
+            out.append(x)
+    return out
+
+
+@dataclass
+class Plan:
+    """what every user's query shares"""
+    names: list                 # query event names
+    limits: list                # per name
+    blacklist: list             # blacklistEvents
+    boost: Optional[str]        # the history boost's text, None: no "boost"
+    in_must: bool               # the algorithm's userBias < 0
+    n_history: int              # names with a terms clause: maxQueryEvents - 1, clamped
+    head: str                   # {"from":F,"size":N
+    should: str                 # should elements after the history
+    must: str                   # must elements after the history
+    must_not: str               # must_not elements after the ids clause
+    sort: str
+    blacklist_items: list = field(default_factory=list)
+
+
+def query_event_limits(ap, names: Sequence[str]) -> list:
+    """indicatorParams(action).maxItemsPerUser (URAlgorithm.scala:213-224)"""
+    if ap.eventNames is not None:
+        table = {n: MAX_QUERY_EVENTS for n in ap.eventNames}
+    elif ap.indicators:
+        table = {i.name: i.maxItemsPerUser or MAX_EVENTS_PER_EVENT_TYPE for i in ap.indicators}
+    else:
+        raise ValueError('Must have either "eventNames" or "indicators" in algorithm parameters.')
+    out = []
+    for n in names:
+        if n not in table:
+            raise KeyError(f"key not found: {n}")   # NoSuchElementException
+        out.append(table[n])
+    return out
+
+
+def max_query_events(ap) -> int:
+    if not ap.indicators:
+        return ap.maxQueryEvents if ap.maxQueryEvents is not None else MAX_QUERY_EVENTS
+    return sum(i.maxItemsPerUser or MAX_QUERY_EVENTS for i in ap.indicators) * 10
+
+
+def plan(ap, query: UserQuery, now_ms: Optional[int] = None) -> Plan:
+    model_names = ap.model_event_names()
+    names = list(query.eventNames) if query.eventNames is not None else list(model_names)
+    limits = query_event_limits(ap, names)
+    blacklist = list(ap.blacklistEvents) if ap.blacklistEvents is not None else list(model_names[:1])
+    algo_bias = f32(ap.userBias) if ap.userBias is not None else 1.0
+    b = f32(query.userBias) if query.userBias is not None else algo_bias
+    boost = java_double(b) if b > 0 and b != 1 else None
+    n_history = max(0, min(max_query_events(ap) - 1, len(names)))
+    size = query.num if query.num is not None else (ap.num if ap.num is not None else NUM_RESULTS)
+    head = '{"from":%d,"size":%d' % (query.from_ or 0, size)
+    qf, pf = list(query.fields or []), list(ap.fields or [])
+    boosted = _distinct([(f.name, list(f.values), f32(f.bias)) for f in [f for f in qf if f32(f.bias) > 0] + [f for f in pf if f32(f.bias) < 0]])
+    filters = _distinct([(f.name, list(f.values)) for f in [f for f in qf if f32(f.bias) < 0] + [f for f in pf if f32(f.bias) > 0]])
+    excluded = _distinct([(f.name, list(f.values)) for f in [f for f in qf if f32(f.bias) == 0] + [f for f in pf if f32(f.bias) == 0]])
+    should = [terms(n, v, java_double(x)) for n, v, x in boosted] + [CONSTANT_SCORE]
+    must = [terms(n, v, "0") for n, v in filters] + date_filters(ap, query, now_ms)
+    must_not = ['{"terms":{' + json_string(n) + ":[" + ",".join(json_string(x) for x in v) + "]}}" for n, v in excluded]
+    if ap.recsModel in ("all", "backfill"):
+        ranks = [rp.field_name() for rp in rankings_params(ap.rankings, model_names)]
+        sort = "[" + ",".join(['{"_score":{"order":"desc"}}'] + ["{" + json_string(r) + ':{"unmapped_type":"double","order":"desc"}}'
+                                                                  for r in ranks]) + "]"
+    else:
+        sort = "[]"
+    return Plan(names, limits, blacklist, boost, algo_bias < 0, n_history, head, ",".join(should), ",".join(must), ",".join(must_not),
+                sort, list(query.blacklistItems or []))
+
+
+def _range(name: str, bounds: Sequence[tuple[str, str]]) -> str:
+    return ('{"constant_score":{"filter":{"range":{' + json_string(name) + ":{" + ",".join(json_string(k) + ":" + json_string(v) for k, v in bounds)
+            + '}}},"boost":0}}')
+
+
+def date_filters(ap, query: UserQuery, now_ms: Optional[int]) -> list:
+    """getFilteringDateRange (URAlgorithm.scala:872-953)"""
+    dr = query.dateRange
+    if dr is not None and (dr.after is not None or dr.before is not None):
+        bounds = []
+        if dr.after:
+            bounds.append(("gt", dr.after))
+        if dr.before:
+            bounds.append(("lt", dr.before))
+        return [_range(dr.name, bounds)]
+    if ap.availableDateName is not None and ap.expireDateName is not None:
+        if query.currentDate is not None:
+            current = query.currentDate
+        else:
+            if now_ms is None:
+                raise ValueError("the available / expire date filter needs now_ms or the query's currentDate")
+            current = iso_utc(now_ms)
+        return [_range(ap.availableDateName, [("lte", current)]), _range(ap.expireDateName, [("gt", current)])]
+    return []
+
+
+def user_history(recent: Sequence[tuple[str, str]], p: Plan) -> tuple[list, list]:
+    """getBiasedRecentUserActions + getExcludedItems on one user's events [(event name, item)], latest first:
+    -> ([items per query name], blacklist)"""
+    hist = []
+    for name, limit in zip(p.names, p.limits):
+        items: list = []
+        for ev, item in recent:
+            if ev == name and len(items) < limit:
+                items = [item] + items
+        hist.append(list(dict.fromkeys(items)))
+    black = [item for ev, item in recent if ev in p.blacklist] + list(p.blacklist_items)
+    return hist, list(dict.fromkeys(black))
+
+
+def render(p: Plan, hist: Sequence[Sequence[str]], black: Sequence[str]) -> str:
+    """buildQuery's document (URAlgorithm.scala:599-610) in json4s' compact rendering"""
+    h = [terms(n, items, "0" if p.in_must else p.boost) for n, items in zip(p.names[:p.n_history], hist)]
+    should = ([] if p.in_must else h) + [p.should]
+    must = (h if p.in_must else []) + ([p.must] if p.must else [])
+    must_not = ['{"ids":{"values":[' + ",".join(json_string(x) for x in black) + '],"boost":0}}'] + ([p.must_not] if p.must_not else [])
+    return (p.head + ',"query":{"bool":{"should":[' + ",".join(should) + '],"must":[' + ",".join(must) + '],"must_not":['
+            + ",".join(must_not) + '],"minimum_should_match":1}},"sort":' + p.sort + "}")
+
+
+def user_queries(events, ap, query: Optional[UserQuery] = None, users: Optional[Sequence[str]] = None, now_ms: Optional[int] = None,
+                 header: str = "{}"):
+    """the host mirror of CcoContext.user_queries over events.read_export's output (its training events, line order):
+    -> (body, offsets), or (body, offsets, users) for users=None (every user with a training event of a query event
+    name, in order of their first such line)"""
+    p = plan(ap, query or UserQuery(), now_ms)
+    qn = set(p.names)
+    by_user: dict = {}
+    for line, (u, ev, item, t) in enumerate(events.events):
+        if ev in qn:
+            by_user.setdefault(u, []).append((t, line, ev, item))
+    who = list(by_user) if users is None else list(users)
+    recs = []
+    for u in who:
+        recent = [(ev, item) for _, _, ev, item in sorted(by_user.get(u, []), key=lambda x: (-x[0], -x[1]))]
+        hist, black = user_history(recent, p)
+        recs.append((header + "\n" + render(p, hist, black) + "\n").encode("utf-8", "surrogatepass"))
+    offsets = np.zeros(len(recs) + 1, dtype=np.int64)
+    np.cumsum([len(r) for r in recs], out=offsets[1:])
+    body = b"".join(recs)
+    return (body, offsets) if users is not None else (body, offsets, who)
