@@ -591,6 +591,56 @@ int cco_event_log_user_queries(cco_ctx_t *ctx, const cco_event_log_t *log, const
                                int64_t *out_len, int64_t **out_offsets, int64_t *out_n, cco_dictionary_t *out_users /* nullable */);
 
 /*
+ * Item queries from a model index (URAlgorithm.buildQuery for Query.item, user and itemSet absent, URAlgorithm.scala:563-792):
+ * one Elasticsearch query per item, its similar items read from the index body instead of one EsClient.getSource round
+ * trip per item.  index_body is an Elasticsearch bulk body as cco_format_model, cco_format_model_log and cco_rerank_model
+ * write it, with cco_rerank_model's grammar, checks and messages (actions {"index":{..., "_id":"<string>"}}, sources JSON
+ * objects, names compared decoded, the last of a repeated member name wins).
+ *  - Documents by _id: a requested item matches the document whose decoded _id has the same bytes (UTF-8; a lone surrogate
+ *    in its 3-byte form).  item_offsets == NULL: one record per document, in body order; *out_items then lists their
+ *    decoded _ids (pinned offsets and bytes, each released with cco_host_free; nullable otherwise).  A repeated item gets a
+ *    record each time.
+ *  - Similar items: when the item has a document whose source has at least one member, one clause per model event name
+ *    n_j, {"terms":{"<n_j>":[elements]}}, where the elements are those of the source's last member named n_j, which must be
+ *    '[' string (',' string)* ']' or '[]' (JSON whitespace between tokens); a source without that member gives [].  A list
+ *    of at most max_query_events elements is kept whole, a longer one keeps its first max_query_events - 1.  The clause ends
+ *    in ,"boost":<similar_boost> when similar_boost is not NULL; with similar_in_must the clauses go to must instead, each
+ *    with ,"boost":0.  An unknown item, or a document whose source is {}, has no similar-items clause.
+ *  - Excluded ids: blacklistItems in order, each once, then the item itself when exclude_self and it is not among them.
+ *  - The body record:
+ *      header \n head ,"query":{"bool":{"should":[should_head, SIMILAR?, should],"must":[must_head, SIMILAR?, must],
+ *      "must_not":[{"ids":{"values":[excluded],"boost":0}}(,must_not)?],"minimum_should_match":1}},"sort":sort} \n
+ *    where SIMILAR stands in should unless similar_in_must, and in must then; the elements of each list are comma-separated
+ *    and an empty piece leaves no comma.  Ids, elements and names are escaped as in cco_event_log_user_queries.
+ * Fragments are JSON text spliced verbatim: head ({"from":F,"size":N), should_head / must_head (the clauses before the
+ * similar items, e.g. buildQuery's empty user-history clauses; may be empty), should, must, must_not (may be empty), sort
+ * (an array), header (one _msearch header line).  Items: n_items ids in the Arrow large_string layout.
+ * Out: *out_body [*out_len] and *out_offsets [*out_n + 1] (record r = body[offsets[r] .. offsets[r + 1])), pinned memory
+ * owned by the context, each released with cco_host_free.
+ * Errors: CCO_E_INVALID_ARG for everything cco_rerank_model refuses in the body (same messages), an _id in two documents,
+ * bad offsets in the items or the blacklist items (decided on the device before any kernel reads bytes through them), null
+ * or empty names, more than 64 names, a null fragment, max_query_events < 1, and a queried document whose model-name
+ * member is not an array of strings (the message names the 0-based document and the member; decided before anything reads
+ * through the elements; an unqueried document is not checked); CCO_E_UNSUPPORTED for group contexts, documents + items +
+ * blacklist items >= 2^31 and a record of 2^31 or more bytes.
+ */
+typedef struct {
+  int32_t n_names;
+  const char *const *names;          /* [n_names] the model event names = the index's indicator fields */
+  int32_t max_query_events;          /* a longer list keeps its first max_query_events - 1 */
+  int32_t similar_in_must;           /* 0: should (algorithm itemBias >= 0), 1: must (itemBias < 0) */
+  const char *similar_boost;         /* JSON number text or NULL */
+  int32_t exclude_self;              /* 1: the item is excluded (!returnSelf) */
+  const char *head, *should_head, *should, *must_head, *must, *must_not, *sort, *header;  /* *_head may be "" */
+  int64_t n_blacklist_items;
+  const int64_t *blacklist_item_offsets; /* [n + 1] */
+  const char *blacklist_item_bytes;
+} cco_item_query_t;
+int cco_item_queries(cco_ctx_t *ctx, const char *index_body, int64_t index_len, const cco_item_query_t *q, int64_t n_items,
+                     const int64_t *item_offsets /* nullable: every document */, const char *item_bytes, char **out_body,
+                     int64_t *out_len, int64_t **out_offsets, int64_t *out_n, cco_dictionary_t *out_items /* nullable */);
+
+/*
  * Debug/parity entry (tests only): full integer co-occurrence matrix A^T B of two canonical
  * binary matrices computed by the same accumulation kernel as cco_train, no LLR, no top-k.
  * Output CSR over the columns of A with ascending column ids, malloc'ed; free with cco_free.

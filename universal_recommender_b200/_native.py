@@ -105,6 +105,14 @@ class UserQueryT(C.Structure):
                 ("blacklist_item_offsets", C.POINTER(C.c_int64)), ("blacklist_item_bytes", C.c_void_p)]
 
 
+class ItemQueryT(C.Structure):
+    _fields_ = [("n_names", C.c_int32), ("names", C.POINTER(C.c_char_p)), ("max_query_events", C.c_int32), ("similar_in_must", C.c_int32),
+                ("similar_boost", C.c_char_p), ("exclude_self", C.c_int32), ("head", C.c_char_p), ("should_head", C.c_char_p),
+                ("should", C.c_char_p), ("must_head", C.c_char_p), ("must", C.c_char_p), ("must_not", C.c_char_p), ("sort", C.c_char_p),
+                ("header", C.c_char_p), ("n_blacklist_items", C.c_int64), ("blacklist_item_offsets", C.POINTER(C.c_int64)),
+                ("blacklist_item_bytes", C.c_void_p)]
+
+
 class LogRankingT(C.Structure):
     _fields_ = [("name", C.c_char_p), ("mode", C.c_int32), ("n_event_names", C.c_int32), ("start_ms", C.c_int64), ("end_ms", C.c_int64),
                 ("event_names", C.POINTER(C.c_char_p))]
@@ -129,7 +137,7 @@ EXPORTS = [
     "cco_format_model", "cco_rerank_model", "cco_event_log_read", "cco_event_log_info", "cco_event_log_ingest",
     "cco_format_model_log", "cco_rerank_model_log", "cco_event_log_free", "cco_event_log_begin", "cco_event_log_append",
     "cco_event_log_finish", "cco_event_log_begin_window", "cco_event_log_window_stats",
-    "cco_event_log_begin_ex", "cco_event_log_user_queries", "cco_result_num_matrices", "cco_result_row_range", "cco_result_matrix", "cco_result_stats", "cco_result_free",
+    "cco_event_log_begin_ex", "cco_event_log_user_queries", "cco_item_queries", "cco_result_num_matrices", "cco_result_row_range", "cco_result_matrix", "cco_result_stats", "cco_result_free",
     "cco_debug_cooccurrence", "cco_debug_downsample", "cco_debug_downsample_block", "cco_debug_llr", "cco_debug_string_ids", "cco_free",
 ]
 
@@ -193,6 +201,8 @@ def lib():
     L.cco_event_log_begin_ex.argtypes = [C.c_void_p, C.c_int64, p(EventWindowT), C.c_uint32, p(C.c_void_p)]
     L.cco_event_log_user_queries.argtypes = [C.c_void_p, C.c_void_p, p(UserQueryT), C.c_int64, p(C.c_int64), C.c_void_p, p(C.c_void_p),
                                              p(C.c_int64), p(C.c_void_p), p(C.c_int64), p(DictionaryT)]
+    L.cco_item_queries.argtypes = [C.c_void_p, C.c_char_p, C.c_int64, p(ItemQueryT), C.c_int64, p(C.c_int64), C.c_void_p, p(C.c_void_p),
+                                   p(C.c_int64), p(C.c_void_p), p(C.c_int64), p(DictionaryT)]
     L.cco_dataset_shape.argtypes = [C.c_void_p, C.c_int32, p(C.c_int64), p(C.c_int32), p(C.c_int64)]
     L.cco_dataset_download.argtypes = [C.c_void_p, C.c_int32, p(p(C.c_int64)), p(p(C.c_int32))]
     L.cco_timer_start.argtypes = [C.c_void_p]

@@ -3250,6 +3250,70 @@ static int json_decode(cco_ctx *c, Arena &ar, long long n, const JMember *m, con
   return CCO_OK;
 }
 
+// the documents of an index body parsed on the device: its lines' members and the decoded member names and _ids
+struct BulkDocs {
+  const unsigned char *body = nullptr;   // the body as 8-byte words with 16 bytes of zero padding
+  long long D = 0, M1 = 0;               // documents, members of all lines
+  long long *line_moff = nullptr;        // [2 D + 1]: line l's members are [line_moff[l], line_moff[l + 1])
+  JMember *mem = nullptr;                // [M1]
+  DevStrCol names, ids;                  // decoded member names [M1] and _ids [D] (offsets from 0)
+  long long ids_bytes = 0;
+};
+// upload, line split, members, the action / _id checks and the decoded names and ids (cco_rerank_model's grammar; the
+// messages name the 0-based document).  extra entries share the 2^31 limit with the documents; `what` names them.
+static int bulk_parse(cco_ctx *c, Arena &ar, const char *body, int64_t body_len, long long extra, const char *what, BulkDocs *bd) {
+  cudaStream_t s = c->stream;
+  // 1. the body, once, into 8-byte words with 16 bytes of zero padding
+  const long long NW = (body_len + 7) / 8;
+  uint64_t *w;
+  CKR(ar.alloc(&w, NW + 2));
+  CK(cudaMemsetAsync(w + body_len / 8, 0, sizeof(uint64_t) * (size_t)(NW + 2 - body_len / 8), s));
+  if (body_len > 0) CK(cudaMemcpyAsync(w, body, (size_t)body_len, cudaMemcpyHostToDevice, s));
+  const unsigned char *bb = (const unsigned char *)w;
+  bd->body = bb;
+  // 2. line bounds
+  long long L = 0, *sb = nullptr, *se = nullptr;
+  CKR(split_lines(c, ar, w, body_len, false, &L, &sb, &se));
+  if (L & 1) return set_error(CCO_E_INVALID_ARG, "the body has %lld lines: lines come in (action, source) pairs", L);
+  const long long D = L / 2;
+  if (D + extra >= 0x7fffffffLL) return set_error(CCO_E_UNSUPPORTED, "documents + %s must stay < 2^31 per call", what);
+  bd->D = D;
+  if (D == 0) return CCO_OK;
+  // 3. members of every line; the verdict on the whole body comes before anything reads through the spans
+  unsigned long long *err, h_err = 0;
+  CKR(json_members(c, ar, L, sb, se, bb, 0x7fffffffLL, &h_err, &bd->line_moff, &bd->mem, &bd->M1));
+  if (h_err != ~0ULL) return json_error(h_err, true);
+  if (bd->M1 >= 0x7fffffffLL) return set_error(CCO_E_UNSUPPORTED, "%lld members in the body, at most 2^31 - 2", bd->M1);
+  // 4. member names decoded; each action is {"index":{...}} and its "_id" is a string
+  long long name_bytes = 0;
+  CKR(json_decode(c, ar, bd->M1, bd->mem, bb, &bd->names, &name_bytes));
+  long long *ib, *ie;
+  CKR(ar.alloc(&ib, D));
+  CKR(ar.alloc(&ie, D));
+  CKR(ar.alloc(&err, 1));
+  CK(cudaMemsetAsync(err, 0xff, 8, s));
+  k_action_check<<<grid_for(D, 256, c->sm_count), 256, 0, s>>>(D, bd->line_moff, bd->mem, bd->names.off, (const unsigned char *)bd->names.w,
+                                                               bb, ib, ie, err);
+  c->launches++;
+  CKR(mail_fetch(c, &h_err, err, 8));
+  CKR(mail_wait(c));
+  if (h_err != ~0ULL) return json_error(h_err, false);
+  long long *imoff, M2 = 0, iname_bytes = 0;
+  JMember *imem, *id_span;
+  CKR(json_members(c, ar, D, ib, ie, bb, 0x7fffffffLL, &h_err, &imoff, &imem, &M2));
+  if (h_err != ~0ULL) return json_error(h_err, false);
+  if (M2 >= 0x7fffffffLL) return set_error(CCO_E_UNSUPPORTED, "%lld members in the body, at most 2^31 - 2", M2);
+  DevStrCol inames;
+  CKR(json_decode(c, ar, M2, imem, bb, &inames, &iname_bytes));
+  CKR(ar.alloc(&id_span, D));
+  k_pick_id<<<grid_for(D, 256, c->sm_count), 256, 0, s>>>(D, imoff, imem, inames.off, (const unsigned char *)inames.w, bb, id_span, err);
+  c->launches++;
+  CKR(mail_fetch(c, &h_err, err, 8));
+  CKR(mail_wait(c));
+  if (h_err != ~0ULL) return json_error(h_err, false);
+  return json_decode(c, ar, D, id_span, bb, &bd->ids, &bd->ids_bytes);
+}
+
 static int rerank_model(cco_ctx_t *ctx, const char *body, int64_t body_len, const cco_item_properties_t *props, int32_t n_rank,
                         const cco_ranking_t *rk, char **out_bytes, int64_t *out_len, Streams st = {}, const DevProps *dp = nullptr) {
   if (!ctx || !out_bytes || !out_len || body_len < 0 || (body_len > 0 && !body)) return set_error(CCO_E_INVALID_ARG, "null argument or negative length");
@@ -3267,65 +3331,20 @@ static int rerank_model(cco_ctx_t *ctx, const char *body, int64_t body_len, cons
   nvtx_push("cco:rerank_model");
   struct Pop { ~Pop() { nvtx_pop(); } } pop;
   mail_reset(c);
-  // 1. the body, once, into 8-byte words with 16 bytes of zero padding
-  const long long NW = (body_len + 7) / 8;
-  uint64_t *w;
-  CKR(ar.alloc(&w, NW + 2));
-  CK(cudaMemsetAsync(w + body_len / 8, 0, sizeof(uint64_t) * (size_t)(NW + 2 - body_len / 8), s));
-  if (body_len > 0) CK(cudaMemcpyAsync(w, body, (size_t)body_len, cudaMemcpyHostToDevice, s));
-  const unsigned char *bb = (const unsigned char *)w;
-  // 2. line bounds
-  long long L = 0, *sb = nullptr, *se = nullptr;
-  CKR(split_lines(c, ar, w, body_len, false, &L, &sb, &se));
-  if (L & 1) return set_error(CCO_E_INVALID_ARG, "the body has %lld lines: lines come in (action, source) pairs", L);
-  const long long D = L / 2;
-  if (D + fresh >= 0x7fffffffLL)
-    return set_error(CCO_E_UNSUPPORTED, "documents + property triples + ranking events must stay < 2^31 per call");
+  // 1-4. the documents: members, decoded names and _ids
+  BulkDocs bd;
+  CKR(bulk_parse(c, ar, body, body_len, fresh, "property triples + ranking events", &bd));
+  const long long D = bd.D, M1 = bd.M1;
+  const unsigned char *bb = bd.body;
   FormatArgs fa;
   memset(&fa, 0, sizeof fa);
   RerankArgs ra;
   memset(&ra, 0, sizeof ra);
   ra.body = bb;
-  DevStrCol ids, names;
-  long long ids_bytes = 0, M1 = 0;
-  if (D > 0) {
-    // 3. members of every line; the verdict on the whole body comes before anything reads through the spans
-    long long *line_moff;
-    JMember *mem;
-    unsigned long long *err, h_err = 0;
-    CKR(json_members(c, ar, L, sb, se, bb, 0x7fffffffLL, &h_err, &line_moff, &mem, &M1));
-    if (h_err != ~0ULL) return json_error(h_err, true);
-    if (M1 >= 0x7fffffffLL) return set_error(CCO_E_UNSUPPORTED, "%lld members in the body, at most 2^31 - 2", M1);
-    // 4. member names decoded; each action is {"index":{...}} and its "_id" is a string
-    long long name_bytes = 0;
-    CKR(json_decode(c, ar, M1, mem, bb, &names, &name_bytes));
-    long long *ib, *ie;
-    CKR(ar.alloc(&ib, D));
-    CKR(ar.alloc(&ie, D));
-    CKR(ar.alloc(&err, 1));
-    CK(cudaMemsetAsync(err, 0xff, 8, s));
-    k_action_check<<<grid_for(D, 256, c->sm_count), 256, 0, s>>>(D, line_moff, mem, names.off, (const unsigned char *)names.w, bb, ib, ie, err);
-    c->launches++;
-    CKR(mail_fetch(c, &h_err, err, 8));
-    CKR(mail_wait(c));
-    if (h_err != ~0ULL) return json_error(h_err, false);
-    long long *imoff, M2 = 0, iname_bytes = 0;
-    JMember *imem, *id_span;
-    CKR(json_members(c, ar, D, ib, ie, bb, 0x7fffffffLL, &h_err, &imoff, &imem, &M2));
-    if (h_err != ~0ULL) return json_error(h_err, false);
-    if (M2 >= 0x7fffffffLL) return set_error(CCO_E_UNSUPPORTED, "%lld members in the body, at most 2^31 - 2", M2);
-    DevStrCol inames;
-    CKR(json_decode(c, ar, M2, imem, bb, &inames, &iname_bytes));
-    CKR(ar.alloc(&id_span, D));
-    k_pick_id<<<grid_for(D, 256, c->sm_count), 256, 0, s>>>(D, imoff, imem, inames.off, (const unsigned char *)inames.w, bb, id_span, err);
-    c->launches++;
-    CKR(mail_fetch(c, &h_err, err, 8));
-    CKR(mail_wait(c));
-    if (h_err != ~0ULL) return json_error(h_err, false);
-    CKR(json_decode(c, ar, D, id_span, bb, &ids, &ids_bytes));
-    ra.line_moff = line_moff;
-    ra.mem = mem;
-  }
+  DevStrCol &ids = bd.ids, &names = bd.names;
+  const long long ids_bytes = bd.ids_bytes;
+  ra.line_moff = bd.line_moff;
+  ra.mem = bd.mem;
   // 5. join: the decoded ids are the row section of the key column (a group with two of them is a repeated _id)
   CKR(model_names(c, ar, &fa, 0, nullptr, true, props, n_rank, rk));
   fa.n_rows = (int32_t)D;
@@ -5147,6 +5166,298 @@ int cco_event_log_user_queries(cco_ctx_t *ctx, const cco_event_log_t *lg, const 
   if (!lg->history) return set_error(CCO_E_INVALID_ARG, "the log was read without history retention (cco_event_log_begin_ex, CCO_LOG_KEEP_HISTORY)");
   if (out_users) *out_users = cco_dictionary_t{0, nullptr, nullptr};
   return user_queries(ctx, lg, q, n_users, user_offsets, user_bytes, out_body, out_len, out_offsets, out_n, out_users);
+}
+
+namespace cco {
+// the record template of an item query, 9 + n_names pieces: 0 head and "should":[, 1 should_head, 2 should, 3 "must":[,
+// 4 must_head, 5 must, 6 the ids clause up to its values, 7 the rest of the record, 8 the end of a similar-items clause,
+// 9 + j the start of model name j's clause (see include/cco_b200.h)
+static std::vector<std::string> iq_template(const cco_item_query_t *q) {
+  std::vector<std::string> t(9 + q->n_names);
+  t[0] = std::string(q->header) + "\n" + q->head + ",\"query\":{\"bool\":{\"should\":[";
+  t[1] = q->should_head;
+  t[2] = q->should;
+  t[3] = "],\"must\":[";
+  t[4] = q->must_head;
+  t[5] = q->must;
+  t[6] = "],\"must_not\":[{\"ids\":{\"values\":[";
+  t[7] = std::string("],\"boost\":0}}") + (*q->must_not ? std::string(",") + q->must_not : std::string()) +
+         "],\"minimum_should_match\":1}},\"sort\":" + q->sort + "}\n";
+  t[8] = q->similar_in_must ? "],\"boost\":0}}" : q->similar_boost ? std::string("],\"boost\":") + q->similar_boost + "}}" : "]}}";
+  for (int j = 0; j < q->n_names; ++j) t[9 + j] = "{\"terms\":{" + uq_quote(q->names[j]) + ":[";
+  return t;
+}
+
+static int iq_check_host(const cco_item_query_t *q, int64_t n_items, const int64_t *ioff, const char *ibytes) {
+  if (q->n_names < 1 || q->n_names > kUqMaxNames) return set_error(CCO_E_INVALID_ARG, "%d model event names, 1..%d", (int)q->n_names, kUqMaxNames);
+  if (!q->names) return set_error(CCO_E_INVALID_ARG, "null names");
+  for (int k = 0; k < q->n_names; ++k)
+    if (!q->names[k] || !*q->names[k]) return set_error(CCO_E_INVALID_ARG, "model event name %d is null or empty", k);
+  if (q->max_query_events < 1) return set_error(CCO_E_INVALID_ARG, "max_query_events = %d, at least 1", (int)q->max_query_events);
+  if ((q->similar_in_must != 0 && q->similar_in_must != 1) || (q->exclude_self != 0 && q->exclude_self != 1))
+    return set_error(CCO_E_INVALID_ARG, "similar_in_must and exclude_self must be 0 or 1");
+  if (!q->head || !q->should_head || !q->should || !q->must_head || !q->must || !q->must_not || !q->sort || !q->header)
+    return set_error(CCO_E_INVALID_ARG, "a null fragment");
+  CKR(str_check_host(q->n_blacklist_items, q->blacklist_item_offsets, q->blacklist_item_bytes, 0, "blacklist item"));
+  if (ioff) CKR(str_check_host(n_items, ioff, ibytes, 0, "item"));
+  else if (n_items != 0) return set_error(CCO_E_INVALID_ARG, "n_items without item offsets");
+  return CCO_OK;
+}
+
+static int item_queries(cco_ctx *c, const char *body, int64_t body_len, const cco_item_query_t *q, int64_t n_items, const int64_t *ioff,
+                        const char *ibytes, char **out_body, int64_t *out_len, int64_t **out_offsets, int64_t *out_n,
+                        cco_dictionary_t *out_items) {
+  cudaStream_t s = c->stream;
+  CK(cudaSetDevice(c->device));
+  Arena ar(s);
+  nvtx_push("cco:item_queries");
+  struct Pop { ~Pop() { nvtx_pop(); } } pop;
+  mail_reset(c);
+  const bool all = ioff == nullptr;
+  const long long NI = all ? 0 : n_items, NL = q->n_blacklist_items;
+  // 1-4. the documents: members, decoded names and _ids
+  BulkDocs bd;
+  CKR(bulk_parse(c, ar, body, body_len, NI + NL, "items + blacklist items", &bd));
+  const long long D = bd.D, R = all ? D : NI;
+  // 5. one key column: the decoded _ids, the items, blacklistItems; the caller's offsets are checked on the device before
+  //    any kernel reads bytes through them
+  const long long NK = D + NI + NL;
+  const long long nb = bd.ids_bytes + (NI > 0 ? ioff[NI] - ioff[0] : 0) +
+                       (NL > 0 ? q->blacklist_item_offsets[NL] - q->blacklist_item_offsets[0] : 0);
+  DevStrCol key;
+  key.n = NK;
+  key.base = 0;
+  CKR(ar.alloc(&key.off, NK + 1));
+  CKR(ar.alloc(&key.w, (nb + 16 + 7) / 8));
+  CKR(ar.alloc(&key.hash, std::max<long long>(NK, 1)));
+  CK(cudaMemsetAsync(key.off, 0, 8, s));
+  int *bad, h_bad = 0;
+  CKR(ar.alloc(&bad, 1));
+  CK(cudaMemsetAsync(bad, 0, sizeof(int), s));
+  long long at = 0, byte_at = 0;
+  if (D > 0) {
+    k_rebase<<<grid_for(D + 1, 256, c->sm_count), 256, 0, s>>>(D + 1, bd.ids.off, 0, key.off);
+    c->launches++;
+    if (bd.ids_bytes > 0) CK(cudaMemcpyAsync(key.w, bd.ids.w, (size_t)bd.ids_bytes, cudaMemcpyDeviceToDevice, s));
+    at = D;
+    byte_at = bd.ids_bytes;
+  }
+  for (int k = 0; k < 2; ++k) {
+    const long long n = k ? NL : NI;
+    const int64_t *off = k ? q->blacklist_item_offsets : ioff;
+    const char *bytes = k ? q->blacklist_item_bytes : ibytes;
+    if (n == 0) continue;
+    long long *tmp;
+    CKR(ar.alloc(&tmp, n + 1));
+    CK(cudaMemcpyAsync(tmp, off, sizeof(int64_t) * ((size_t)n + 1), cudaMemcpyHostToDevice, s));
+    k_str_check<<<grid_for(n, 256, c->sm_count), 256, 0, s>>>(n, tmp, bad);
+    k_rebase<<<grid_for(n + 1, 256, c->sm_count), 256, 0, s>>>(n + 1, tmp, byte_at - off[0], key.off + at);
+    c->launches += 2;
+    const long long kb = off[n] - off[0];
+    if (kb > 0) CK(cudaMemcpyAsync((char *)key.w + byte_at, bytes + off[0], (size_t)kb, cudaMemcpyHostToDevice, s));
+    at += n;
+    byte_at += kb;
+  }
+  CKR(mail_fetch(c, &h_bad, bad, 4));
+  CKR(mail_wait(c));
+  if (h_bad) return set_error(CCO_E_INVALID_ARG, "decreasing offsets in the items or the blacklist items");
+  // 6. one exact grouping over the key column; a group that holds two documents is a repeated _id
+  str_hash(c, key, ~0ULL);
+  int32_t *gid;
+  CKR(ar.alloc(&gid, std::max<long long>(NK, 1)));
+  StrTable tb;
+  CKR(str_group(c, ar, key, nullptr, false, 0, &tb, gid));
+  if (D > 0) {
+    unsigned long long *dup, h_dup = ~0ULL;
+    CKR(ar.alloc(&dup, 1));
+    CK(cudaMemsetAsync(dup, 0xff, 8, s));
+    k_dup_rows<<<grid_for(D, 256, c->sm_count), 256, 0, s>>>(D, gid, tb.first_sorted, dup);
+    c->launches++;
+    CKR(mail_fetch(c, &h_dup, dup, 8));
+    CKR(mail_wait(c));
+    if (h_dup != ~0ULL)
+      return set_error(CCO_E_INVALID_ARG, "document %llu: its _id is the _id of document %llu", h_dup >> 32, h_dup & 0xffffffffULL);
+  }
+  // 7. blacklistItems: each group's first list index (membership and repeats are group tests)
+  const long long G = tb.n_groups;
+  uint32_t *first_in_list;
+  CKR(ar.alloc(&first_in_list, std::max<long long>(G, 1)));
+  CK(cudaMemsetAsync(first_in_list, 0xff, sizeof(uint32_t) * (size_t)std::max<long long>(G, 1), s));
+  if (NL > 0) {
+    k_iq_black<<<grid_for(NL, 256, c->sm_count), 256, 0, s>>>(NL, D + NI, gid, first_in_list);
+    c->launches++;
+  }
+  // 8. the records' documents; the queried documents
+  int32_t *rec_doc, *rec_key;
+  uint8_t *queried;
+  CKR(ar.alloc(&rec_doc, std::max<long long>(R, 1)));
+  CKR(ar.alloc(&rec_key, std::max<long long>(R, 1)));
+  CKR(ar.alloc(&queried, std::max<long long>(D, 1)));
+  CK(cudaMemsetAsync(queried, 0, (size_t)std::max<long long>(D, 1), s));
+  if (R > 0) {
+    k_iq_rec<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, D, all, gid, tb.first_sorted, rec_doc, rec_key, queried);
+    c->launches++;
+  }
+  // 9. the distinct model names; per document the last source member of each
+  std::vector<std::string> ent;
+  std::vector<int32_t> name_entry(q->n_names);
+  for (int j = 0; j < q->n_names; ++j) {
+    size_t t = 0;
+    while (t < ent.size() && ent[t] != q->names[j]) ++t;
+    if (t == ent.size()) ent.push_back(q->names[j]);
+    name_entry[j] = (int32_t)t;
+  }
+  const int T = (int)ent.size();
+  const long long DT = D * T;
+  long long *eoff;
+  CKR(ar.alloc(&eoff, DT + 1));
+  CK(cudaMemsetAsync(eoff, 0, sizeof(long long) * (size_t)(DT + 1), s));
+  DevStrCol dec;
+  if (D > 0) {
+    std::vector<int64_t> toff(T + 1, 0);
+    std::string tblob;
+    for (int t = 0; t < T; ++t) {
+      tblob += ent[t];
+      toff[t + 1] = (int64_t)tblob.size();
+    }
+    const cco_dictionary_t td = {T, toff.data(), tblob.data()};
+    DevDict traw;
+    CKR(upload_dict(c, ar, td, &traw));
+    CK(cudaStreamSynchronize(s));   // the table is local
+    str_hash(c, bd.names, ~0ULL);
+    int32_t *ngid, *entry_of, *pick;
+    CKR(ar.alloc(&ngid, std::max<long long>(bd.M1, 1)));
+    StrTable nt;
+    CKR(str_group(c, ar, bd.names, nullptr, false, 0, &nt, ngid));
+    CKR(ar.alloc(&entry_of, std::max<long long>(nt.n_groups, 1)));
+    CKR(ar.alloc(&pick, DT));
+    if (nt.n_groups > 0)
+      k_name_entry<<<grid_for(nt.n_groups, 256, c->sm_count), 256, 0, s>>>(nt.n_groups, nt.first_sorted, bd.names.off,
+                                                                           (const unsigned char *)bd.names.w, T, traw.off, traw.bytes, entry_of);
+    k_iq_pick<<<grid_for(D, 256, c->sm_count), 256, 0, s>>>(D, T, bd.line_moff, ngid, entry_of, pick);
+    c->launches += 2;
+    // 10. the queried documents' picked values: the verdict comes before anything reads through the element spans
+    long long *cnt, NE = 0;
+    unsigned long long *err, h_err = ~0ULL;
+    CKR(ar.alloc(&cnt, DT + 1));
+    CKR(ar.alloc(&err, 1));
+    CK(cudaMemsetAsync(cnt + DT, 0, 8, s));
+    CK(cudaMemsetAsync(err, 0xff, 8, s));
+    const int agrid = grid_for(DT * 32, 256, c->sm_count);
+    k_iq_array<false><<<agrid, 256, 0, s>>>(DT, T, queried, pick, bd.mem, bd.body, cnt, nullptr, nullptr, err);
+    c->launches++;
+    CKR(exclusive_sum(c, ar, cnt, eoff, DT + 1));
+    CKR(mail_fetch(c, &h_err, err, 8));
+    CKR(mail_fetch(c, &NE, eoff + DT, 8));
+    CKR(mail_wait(c));
+    if (h_err != ~0ULL)
+      return set_error(CCO_E_INVALID_ARG, "document %lld: its \"%s\" member is not an array of strings", (long long)(h_err / T),
+                       ent[h_err % T].c_str());
+    JMember *elem;
+    CKR(ar.alloc(&elem, std::max<long long>(NE, 1)));
+    if (NE > 0) {
+      k_iq_array<true><<<agrid, 256, 0, s>>>(DT, T, queried, pick, bd.mem, bd.body, nullptr, eoff, elem, err);
+      c->launches++;
+    }
+    long long dec_bytes = 0;
+    CKR(json_decode(c, ar, NE, elem, bd.body, &dec, &dec_bytes));
+  }
+  // 11. the template, then a length pass, the record offsets and a write pass: one warp per record
+  const std::vector<std::string> tp = iq_template(q);
+  std::vector<long long> toff(tp.size() + 1, 0);
+  std::string tbl;
+  for (size_t j = 0; j < tp.size(); ++j) {
+    tbl += tp[j];
+    toff[j + 1] = (long long)tbl.size();
+  }
+  long long *d_toff;
+  unsigned char *d_tb;
+  int32_t *d_entry;
+  CKR(ar.alloc(&d_toff, (long long)toff.size()));
+  CKR(ar.alloc(&d_tb, std::max<long long>((long long)tbl.size(), 1)));
+  CKR(ar.alloc(&d_entry, q->n_names));
+  CK(cudaMemcpyAsync(d_toff, toff.data(), sizeof(long long) * toff.size(), cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(d_tb, tbl.data(), tbl.size(), cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(d_entry, name_entry.data(), sizeof(int32_t) * (size_t)q->n_names, cudaMemcpyHostToDevice, s));
+  IqArgs a;
+  a.n_rec = R;
+  a.rec_doc = rec_doc;
+  a.rec_key = rec_key;
+  a.kgid = gid;
+  a.koff = key.off;
+  a.kbytes = (const unsigned char *)key.w;
+  a.line_moff = bd.line_moff;
+  a.T = T;
+  a.n_names = q->n_names;
+  a.name_entry = d_entry;
+  a.eoff = eoff;
+  a.doff = dec.off;
+  a.dbytes = (const unsigned char *)dec.w;
+  a.slice = q->max_query_events;
+  a.in_must = q->similar_in_must;
+  a.exclude_self = q->exclude_self;
+  a.n_list = NL;
+  a.list_at = D + NI;
+  a.first_in_list = first_in_list;
+  a.toff = d_toff;
+  a.tbytes = d_tb;
+  long long *rlen, *roff;
+  CKR(ar.alloc(&rlen, R + 1));
+  CKR(ar.alloc(&roff, R + 1));
+  CK(cudaMemsetAsync(rlen + R, 0, 8, s));
+  if (R > 0) {
+    k_iq_record<false><<<grid_for(R * 32, 256, c->sm_count), 256, 0, s>>>(a, nullptr, rlen, nullptr);
+    c->launches++;
+  }
+  CKR(exclusive_sum(c, ar, rlen, roff, R + 1));
+  int64_t *ho = (int64_t *)c->pinned_get(sizeof(int64_t) * ((size_t)R + 1), /*for_result=*/false);
+  if (!ho) return set_error(CCO_E_OOM, "pinned host allocation failed");
+  CK(cudaMemcpyAsync(ho, roff, sizeof(int64_t) * ((size_t)R + 1), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  for (long long r = 0; r < R; ++r)
+    if (ho[r + 1] - ho[r] >= (1LL << 31)) {
+      c->pinned_put(ho);
+      return set_error(CCO_E_UNSUPPORTED, "record %lld has %lld bytes, at most 2^31 - 1", r, (long long)(ho[r + 1] - ho[r]));
+    }
+  const long long total = ho[R];
+  unsigned char *d_out;
+  CKR(ar.alloc(&d_out, std::max<long long>(total, 1)));
+  if (R > 0 && total > 0) {
+    k_iq_record<true><<<grid_for(R * 32, 256, c->sm_count), 256, 0, s>>>(a, roff, nullptr, d_out);
+    c->launches++;
+  }
+  char *host = (char *)c->pinned_get((size_t)std::max<long long>(total, 1), /*for_result=*/false);
+  if (!host) return set_error(CCO_E_OOM, "pinned host allocation failed");
+  if (total > 0) CK(cudaMemcpyAsync(host, d_out, (size_t)total, cudaMemcpyDeviceToHost, s));
+  if (all && out_items) {   // the documents' decoded _ids, in body order
+    int64_t *io = (int64_t *)c->pinned_get(sizeof(int64_t) * ((size_t)D + 1), /*for_result=*/false);
+    char *ib = (char *)c->pinned_get((size_t)std::max<long long>(bd.ids_bytes, 1), /*for_result=*/false);
+    if (!io || !ib) return set_error(CCO_E_OOM, "pinned host allocation failed");
+    io[0] = 0;
+    if (D > 0) CK(cudaMemcpyAsync(io, bd.ids.off, sizeof(int64_t) * ((size_t)D + 1), cudaMemcpyDeviceToHost, s));
+    if (bd.ids_bytes > 0) CK(cudaMemcpyAsync(ib, bd.ids.w, (size_t)bd.ids_bytes, cudaMemcpyDeviceToHost, s));
+    *out_items = cco_dictionary_t{D, io, ib};
+  }
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  *out_body = host;
+  *out_len = total;
+  *out_offsets = ho;
+  *out_n = R;
+  return CCO_OK;
+}
+}  // namespace cco
+
+int cco_item_queries(cco_ctx_t *ctx, const char *index_body, int64_t index_len, const cco_item_query_t *q, int64_t n_items,
+                     const int64_t *item_offsets, const char *item_bytes, char **out_body, int64_t *out_len, int64_t **out_offsets,
+                     int64_t *out_n, cco_dictionary_t *out_items) {
+  if (!ctx || !q || !out_body || !out_len || !out_offsets || !out_n || index_len < 0 || (index_len > 0 && !index_body))
+    return set_error(CCO_E_INVALID_ARG, "null argument or negative length");
+  if (!ctx->members.empty()) return set_error(CCO_E_UNSUPPORTED, "per-GPU contexts only");
+  if (index_len > 0 && index_body[index_len - 1] != '\n') return set_error(CCO_E_INVALID_ARG, "the body does not end in a newline");
+  CKR(iq_check_host(q, n_items, item_offsets, item_bytes));
+  if (out_items) *out_items = cco_dictionary_t{0, nullptr, nullptr};
+  return item_queries(ctx, index_body, index_len, q, n_items, item_offsets, item_bytes, out_body, out_len, out_offsets, out_n, out_items);
 }
 
 int cco_event_log_free(cco_event_log_t *lg) {

@@ -1,5 +1,6 @@
 // cco_queries.cuh -- cco_event_log_user_queries: buildQuery (URAlgorithm.scala:563-739) for user queries over the training
-// history an event log keeps (cco_event_log_begin_ex with CCO_LOG_KEEP_HISTORY).
+// history an event log keeps (cco_event_log_begin_ex with CCO_LOG_KEEP_HISTORY); cco_item_queries: the same for item
+// queries over a model index body (its kernels are listed with them, below the user-query ones).
 //
 // e = one training event of a query event name (name rank q); its user and item are dense group ids of the log's columns.
 //   k_uq_select       e -> (log entry, name rank) over the query names' ranges of the name-partitioned columns
@@ -288,6 +289,200 @@ __global__ void __launch_bounds__(256) k_uq_record(UqArgs a, const long long *__
         }, o, cur, first);
       }
     }
+    if (!WRITE && lane == 0) rec_len[r] = cur;
+  }
+}
+
+// ---- cco_item_queries: buildQuery for item queries over a model index body (parsed by cco_json.cuh) ----------------------
+//   k_iq_pick      per document: the last source member of each model name (T distinct names), -1
+//   k_iq_black     blacklistItems: the first list index of each key group (membership and distinct are group tests)
+//   k_iq_rec       per record: its document (-1: none) and key entry; the queried documents flagged
+//   k_iq_array     one warp per (queried document, name) value span: the array-of-strings grammar and the raw element spans,
+//                  a count pass and a write pass; an error word for the first bad span
+//   k_iq_record    one warp per record: template pieces, the sliced similar-items lists and the exclusion list, a length
+//                  pass and a write pass (as k_uq_record)
+__global__ void k_iq_pick(long long n_docs, int T, const long long *__restrict__ line_moff, const int32_t *__restrict__ ngid,
+                          const int32_t *__restrict__ entry_of, int32_t *__restrict__ pick) {
+  for (long long d = blockIdx.x * (long long)blockDim.x + threadIdx.x; d < n_docs; d += (long long)gridDim.x * blockDim.x) {
+    int32_t *p = pick + d * T;
+    for (int t = 0; t < T; ++t) p[t] = -1;
+    for (long long m = line_moff[2 * d + 1]; m < line_moff[2 * d + 2]; ++m) {
+      const int32_t t = entry_of[ngid[m]];
+      if (t >= 0) p[t] = (int32_t)m;
+    }
+  }
+}
+__global__ void k_iq_black(long long n, long long at, const int32_t *__restrict__ gid, uint32_t *__restrict__ first_in_list) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    atomicMin(&first_in_list[gid[at + i]], (uint32_t)i);
+}
+// every document (all): record r is document r; else record r is key entry n_docs + r, found when its group's first entry
+// is a document (the documents come first in the key column)
+__global__ void k_iq_rec(long long R, long long n_docs, bool all, const int32_t *__restrict__ gid, const uint32_t *__restrict__ first_sorted,
+                         int32_t *__restrict__ rec_doc, int32_t *__restrict__ rec_key, uint8_t *__restrict__ queried) {
+  for (long long r = blockIdx.x * (long long)blockDim.x + threadIdx.x; r < R; r += (long long)gridDim.x * blockDim.x) {
+    const long long k = all ? r : n_docs + r;
+    const uint32_t f = first_sorted[gid[k]];
+    const int32_t d = (long long)f < n_docs ? (int32_t)f : -1;
+    rec_doc[r] = d;
+    rec_key[r] = (int32_t)k;
+    if (d >= 0) queried[d] = 1;
+  }
+}
+
+// Grammar of a picked value: '[' ws* ( ']' | string (ws* ',' ws* string)* ws* ']' ) -- the span is trimmed, its strings were
+// validated by k_json_members.  The string and escape masks are k_json_members': escaped byte = an odd run of backslashes
+// right before it, in string = prefix XOR of the unescaped quotes.  Events are the unescaped quotes and the non-whitespace
+// bytes outside strings.  x = d * T + t; a span that is not queried or not picked counts 0 elements.
+enum : int { kIaOpen = 0, kIaFirst, kIaString, kIaAfter, kIaNext, kIaDone };
+template <bool kWrite>
+__global__ void __launch_bounds__(256) k_iq_array(long long n, int T, const uint8_t *__restrict__ queried, const int32_t *__restrict__ pick,
+                                                  const JMember *__restrict__ mem, const unsigned char *__restrict__ body,
+                                                  long long *__restrict__ cnt, const long long *__restrict__ eoff, JMember *__restrict__ elem,
+                                                  unsigned long long *__restrict__ err) {
+  const int lane = threadIdx.x & 31;
+  const unsigned below = (1u << lane) - 1, upto = 0xffffffffu >> (31 - lane);
+  const long long warp = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5, nwarps = ((long long)gridDim.x * blockDim.x) >> 5;
+  for (long long x = warp; x < n; x += nwarps) {
+    const int32_t m = queried[x / T] ? pick[x] : -1;
+    if (m < 0) {
+      if (!kWrite && lane == 0) cnt[x] = 0;
+      continue;
+    }
+    const long long b = mem[m].vb, e = mem[m].ve;
+    const long long at = kWrite ? eoff[x] : 0;
+    int state = kIaOpen;
+    long long k = 0, sb = 0;
+    unsigned in_str = 0, bs_odd = 0;
+    for (long long base = b; base < e && state >= 0; base += 32) {
+      const long long p = base + lane;
+      const unsigned c = p < e ? body[p] : ' ';
+      const unsigned bsm = __ballot_sync(0xffffffffu, c == '\\');
+      const unsigned nb = ~bsm & below;
+      const unsigned esc = (nb ? lane - 1 - (31 - __clz(nb)) : lane + bs_odd) & 1;
+      const unsigned qm = __ballot_sync(0xffffffffu, c == '"' && !esc);
+      const bool uq = (qm >> lane) & 1;
+      const bool S = (in_str ^ __popc(qm & upto)) & 1;
+      const unsigned Sm = __ballot_sync(0xffffffffu, S);
+      unsigned evm = __ballot_sync(0xffffffffu, uq || (p < e && !S && !json_ws(c)));
+      while (evm && state >= 0) {
+        const int i = __ffs(evm) - 1;
+        evm &= evm - 1;
+        const unsigned ci = __shfl_sync(0xffffffffu, c, i);
+        const bool qi = (qm >> i) & 1, open_q = qi && ((Sm >> i) & 1);
+        const long long pi = base + i;
+        if (state == kIaOpen) {
+          state = ci == '[' ? kIaFirst : -1;
+        } else if (state == kIaFirst || state == kIaNext) {
+          if (open_q) {
+            sb = pi + 1;
+            state = kIaString;
+          } else {
+            state = state == kIaFirst && ci == ']' ? kIaDone : -1;
+          }
+        } else if (state == kIaString) {   // the only event inside a string is its closing quote
+          if (kWrite && lane == 0) elem[at + k] = JMember{sb, pi, 0, 0};
+          ++k;
+          state = kIaAfter;
+        } else if (state == kIaAfter) {
+          state = qi ? -1 : ci == ',' ? kIaNext : ci == ']' ? kIaDone : -1;
+        } else {
+          state = -1;   // anything after the closing bracket
+        }
+      }
+      in_str = (in_str ^ __popc(qm)) & 1;
+      if (~bsm) bs_odd = __clz(~bsm) & 1;
+    }
+    if (lane == 0) {
+      if (state != kIaDone) atomicMin(err, (unsigned long long)x);
+      if (!kWrite) cnt[x] = state == kIaDone ? k : 0;
+    }
+  }
+}
+
+struct IqArgs {
+  long long n_rec;
+  const int32_t *rec_doc;          // [n_rec] document, -1
+  const int32_t *rec_key;          // [n_rec] key entry of the record's item
+  const int32_t *kgid;             // key column: decoded _ids, the items, blacklistItems; group per entry
+  const long long *koff;
+  const unsigned char *kbytes;
+  const long long *line_moff;      // the source of document d has members iff line_moff[2 d + 2] > line_moff[2 d + 1]
+  int T, n_names;                  // distinct model names; model names
+  const int32_t *name_entry;       // [n_names] distinct entry of each model name
+  const long long *eoff;           // [D * T + 1] first element of (d, t)
+  const long long *doff;           // decoded elements
+  const unsigned char *dbytes;
+  long long slice;                 // max_query_events
+  int in_must, exclude_self;
+  long long n_list, list_at;       // blacklistItems are key entries list_at + i
+  const uint32_t *first_in_list;   // per group: first list index, ~0
+  const long long *toff;           // [n_names + 10] template pieces (see iq_template)
+  const unsigned char *tbytes;
+};
+
+template <bool WRITE>
+__global__ void __launch_bounds__(256) k_iq_record(IqArgs a, const long long *__restrict__ rec_off, long long *__restrict__ rec_len,
+                                                   unsigned char *__restrict__ out) {
+  const int lane = threadIdx.x & 31;
+  const long long warps = (long long)gridDim.x * (blockDim.x >> 5);
+  for (long long r = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5; r < a.n_rec; r += warps) {
+    const int32_t d = a.rec_doc[r], key = a.rec_key[r];
+    const bool similar = d >= 0 && a.line_moff[2 * (long long)d + 2] > a.line_moff[2 * (long long)d + 1];
+    unsigned char *o = WRITE ? out + rec_off[r] : nullptr;
+    long long cur = 0;
+    auto piece = [&](int j) {
+      const long long t0 = a.toff[j], tl = a.toff[j + 1] - t0;
+      if (WRITE)
+        for (long long k = lane; k < tl; k += 32) o[cur + k] = a.tbytes[t0 + k];
+      cur += tl;
+      return tl > 0;
+    };
+    auto comma = [&]() {
+      if (WRITE && lane == 0) o[cur] = ',';
+      cur += 1;
+    };
+    // a clause list: head fragment, the similar items (when here), tail fragment, comma-separated
+    auto section = [&](int head, bool here, int tail) {
+      bool any = piece(head);
+      for (int j = 0; here && similar && j < a.n_names; ++j) {
+        if (any) comma();
+        piece(9 + j);
+        const long long x = (long long)d * a.T + a.name_entry[j], e0 = a.eoff[x], n = a.eoff[x + 1] - e0;
+        bool first = true;
+        uq_list(n <= a.slice ? n : a.slice - 1, [&](long long i, const unsigned char **p, long long *len) {
+          *p = a.dbytes + a.doff[e0 + i];
+          *len = a.doff[e0 + i + 1] - a.doff[e0 + i];
+          return true;
+        }, o, cur, first);
+        piece(8);
+        any = true;
+      }
+      if (a.toff[tail + 1] > a.toff[tail]) {
+        if (any) comma();
+        piece(tail);
+      }
+    };
+    piece(0);
+    section(1, !a.in_must, 2);
+    piece(3);
+    section(4, a.in_must, 5);
+    piece(6);
+    bool first = true;   // blacklistItems, each once, then the item unless it is among them
+    uq_list(a.n_list, [&](long long i, const unsigned char **p, long long *len) {
+      const long long k = a.list_at + i;
+      if (a.first_in_list[a.kgid[k]] != (uint32_t)i) return false;
+      *p = a.kbytes + a.koff[k];
+      *len = a.koff[k + 1] - a.koff[k];
+      return true;
+    }, o, cur, first);
+    if (a.exclude_self && a.first_in_list[a.kgid[key]] == ~0u)
+      uq_list(1, [&](long long, const unsigned char **p, long long *len) {
+        *p = a.kbytes + a.koff[key];
+        *len = a.koff[key + 1] - a.koff[key];
+        return true;
+      }, o, cur, first);
+    piece(7);
     if (!WRITE && lane == 0) rec_len[r] = cur;
   }
 }

@@ -503,6 +503,57 @@ class CcoContext:
         self._L.cco_host_free(self._h, C.c_void_p(addr))
         return body, offsets, ids
 
+    def item_queries(self, index_body: bytes, ap, query=None, items=None, now_ms: Optional[int] = None, header: str = "{}"):
+        """cco_item_queries: URAlgorithm.buildQuery for item queries (ur_query.py restates it), the similar items read from a
+        model index bulk body (as format_model / rerank_model write it).  ap: ur_algorithm.URAlgorithmParams; query:
+        ur_query.ItemQuery (None: defaults); items: the item ids, or None for every document, in body order.
+        -> (body, offsets int64[n + 1]): `header\nquery\n` records, the _msearch body; record r = body[offsets[r]:offsets[r + 1]].
+        With items=None -> (body, offsets, items)."""
+        from . import ur_query as Q
+        p = Q.item_plan(ap, query, now_ms)
+        enc = lambda x: x.encode("utf-8", "surrogatepass")
+        names = [enc(n) for n in p.names]
+        nm = (C.c_char_p * max(len(names), 1))(*names)
+        def column(ids):   # ids compare as UTF-8 bytes, a lone surrogate in its 3-byte form
+            b = [enc(x) for x in ids]
+            o = np.zeros(len(b) + 1, dtype=np.int64)
+            np.cumsum([len(x) for x in b], out=o[1:])
+            return o, np.frombuffer(b"".join(b), dtype=np.uint8)
+
+        def text(b: bytes) -> str:
+            try:
+                return b.decode("utf-8", "surrogatepass")
+            except UnicodeDecodeError:
+                return b.decode("utf-8", "surrogateescape")
+        lo, lb = column(p.blacklist_items)
+        qt = N.ItemQueryT(len(names), nm, p.max_query_events, 1 if p.in_must else 0, None if p.boost is None else p.boost.encode(),
+                          1 if p.exclude_self else 0, enc(p.head), enc(p.should_head), enc(p.should), enc(p.must_head), enc(p.must),
+                          enc(p.must_not), enc(p.sort), enc(header), len(lo) - 1, lo.ctypes.data_as(C.POINTER(C.c_int64)),
+                          lb.ctypes.data if len(lb) else None)
+        index_body = bytes(index_body)
+        out, ln, off, n = C.c_void_p(), C.c_int64(), C.c_void_p(), C.c_int64()
+        idd = N.DictionaryT()
+        if items is None:
+            N.check(self._L.cco_item_queries(self._h, index_body, len(index_body), C.byref(qt), 0, None, None, C.byref(out), C.byref(ln),
+                                             C.byref(off), C.byref(n), C.byref(idd)))
+        else:
+            io, ib = column(list(items))
+            N.check(self._L.cco_item_queries(self._h, index_body, len(index_body), C.byref(qt), len(io) - 1,
+                                             io.ctypes.data_as(C.POINTER(C.c_int64)), ib.ctypes.data if len(ib) else None, C.byref(out),
+                                             C.byref(ln), C.byref(off), C.byref(n), None))
+        offsets = np.ctypeslib.as_array(C.cast(off, C.POINTER(C.c_int64)), shape=(n.value + 1,)).copy()
+        self._L.cco_host_free(self._h, off)
+        body = self._take_body(out, ln)
+        if items is not None:
+            return body, offsets
+        ioff = np.ctypeslib.as_array(idd.offsets, shape=(idd.n + 1,)).copy()
+        addr = C.c_void_p.from_buffer(idd, N.DictionaryT.bytes.offset).value
+        blob = C.string_at(addr, int(ioff[-1])) if ioff[-1] else b""
+        ids = [text(blob[a:b]) for a, b in zip(ioff[:-1].tolist(), ioff[1:].tolist())]
+        self._L.cco_host_free(self._h, C.cast(idd.offsets, C.c_void_p))
+        self._L.cco_host_free(self._h, C.c_void_p(addr))
+        return body, offsets, ids
+
     def rerank_model(self, body: bytes, properties=None, rankings=None, log=None) -> bytes:
         """cco_rerank_model: calcPop (URAlgorithm.scala:375-399, recsModel "backfill") on an existing index.  body = the
         Elasticsearch bulk body of the current model, as format_model writes it; properties and rankings as in format_model.

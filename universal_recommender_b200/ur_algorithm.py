@@ -4,8 +4,8 @@ calc_all_on_device runs the whole train half on the GPU, string events in and th
 calc_pop_on_device runs calcPop (recsModel "backfill") on the GPU: the current index's bulk body in, the same index with
 fresh rankings out.  calc_all_from_events / calc_pop_from_events do the same from a PredictionIO event export parsed on the
 device (CcoContext.read_events), the DataSource included.  user_queries_from_events builds buildQuery's user queries for a
-whole user base from the same export (ur_query.py restates buildQuery).  Out of scope: item and item-set queries (they need
-each item's correlators, which a kept train result could supply), Elasticsearch's scoring, reading the index and the HTTP
+whole user base from the same export (ur_query.py restates buildQuery); item_queries builds its item queries for every
+item of a model index body.  Out of scope: item-set queries, Elasticsearch's scoring, reading the index and the HTTP
 call."""
 from __future__ import annotations
 
@@ -15,7 +15,7 @@ from typing import Optional, Sequence
 
 from .indexed_dataset import IndexedDataset
 from .similarity_analysis import CcoContext, DownsamplableCrossOccurrenceDataset, SimilarityAnalysis, default_context, encode_ids
-from .ur_query import Field, UserQuery
+from .ur_query import Field, ItemQuery, UserQuery
 from .ur_model import (RankingParams, RankingType, extract_jvalue, property_json, ranking_window, rankings_for,
                        rankings_params)
 
@@ -54,6 +54,8 @@ class URAlgorithmParams:
     maxQueryEvents: Optional[int] = None
     num: Optional[int] = None
     userBias: Optional[float] = None
+    itemBias: Optional[float] = None
+    returnSelf: Optional[bool] = None
     fields: Optional[Sequence[Field]] = None
     availableDateName: Optional[str] = None
     expireDateName: Optional[str] = None
@@ -73,7 +75,8 @@ class URAlgorithmParams:
             rankings=None if algo_params.get("rankings") is None else [RankingParams.from_json(r) for r in algo_params["rankings"]],
             rowRateIntDiv=bool(algo_params.get("rowRateIntDiv", False)),
             blacklistEvents=algo_params.get("blacklistEvents"), maxQueryEvents=algo_params.get("maxQueryEvents"),
-            num=algo_params.get("num"), userBias=algo_params.get("userBias"),
+            num=algo_params.get("num"), userBias=algo_params.get("userBias"), itemBias=algo_params.get("itemBias"),
+            returnSelf=algo_params.get("returnSelf"),
             fields=None if algo_params.get("fields") is None else [Field.from_json(f) for f in algo_params["fields"]],
             availableDateName=algo_params.get("availableDateName"), expireDateName=algo_params.get("expireDateName"),
             dateName=algo_params.get("dateName"), indexName=algo_params.get("indexName"))
@@ -323,3 +326,14 @@ def user_queries_from_events(export, ap: URAlgorithmParams, query: Optional[User
         return ctx.user_queries(log, ap, query, users, now_ms, header)
     finally:
         log.free()
+
+
+def item_queries(index_body: bytes, ap: URAlgorithmParams, query: Optional[ItemQuery] = None, items=None, now_ms: Optional[int] = None,
+                 ctx: CcoContext | None = None, header: str = "{}"):
+    """buildQuery (URAlgorithm.scala:563-792) for every item of `items` (None: every document of the index, in body order),
+    the similar items read from the model index body (what calc_all_from_events, calc_all_on_device or a calcPop wrote;
+    reading it from Elasticsearch stays with the caller) on the device: one `header\nquery\n` record per item, the body of
+    an Elasticsearch _msearch.  -> (body, offsets) as CcoContext.item_queries ((body, offsets, items) for items=None).
+    now_ms: "now" of the available / expire date filter (default: the wall clock).  The fragments are ur_query.item_plan's."""
+    ctx = ctx or default_context()
+    return ctx.item_queries(index_body, ap, query, items, _now(now_ms), header)

@@ -37,6 +37,31 @@ Deviations:
   * the history is the log's training events (entityType "user" -> targetEntityType "item"); findByEntity has no
     target-type filter, so events aimed at other entity types, which the reference would read, are not read here;
   * where the reference would throw on a target-less event of a query name, no such event exists here.
+
+Item queries (Query.item set; user, itemSet and withRanks absent): item_plan() renders what every item's query shares (the
+fragments CcoContext.item_queries hands to the device); item_queries() is the host mirror over a model index body (what
+CcoContext.format_model / rerank_model write).  Quirks of the reference, kept on purpose:
+  * history clauses are still written: getBiasedRecentUserActions (:795-839) evaluates query.user.get inside its try, the
+    NoSuchElementException is caught, and every query event name (query eventNames, else the model names) gets a terms
+    clause with [] -- the first maxQueryEvents - 1 names (:624, :690), in should with the user boost or in must with
+    "boost":0 when the algorithm's userBias < 0, as plan() renders them for a user without history.  No event is read, so
+    indicatorParams is never consulted: a query event name without an entry raises nothing here;
+  * similar items (getBiasedSimilarItems, :770-792) are one clause per *model* event name, not per query eventName; the
+    document is EsClient.getSource by _id (EsClient.scala:394-442), and a missing document (a 404 reaches Map.empty
+    through the caught ResponseException [RECALL: ES 5 low-level client]) or a source without members (m.nonEmpty, :776)
+    adds no clause at all, while a document without the name's field writes {"terms":{"<name>":[]}} (an item with only
+    $set events has such a document);
+  * a list with size <= maxQueryEvents is kept whole, a longer one keeps its first maxQueryEvents - 1 (:782); elements
+    keep the document's order, no distinct;
+  * the should / must choice tests the algorithm's itemBias (:630, :695-697); the boost is the query's itemBias, else the
+    algorithm's, written only when > 0 and != 1, a Float widened to Double (:777-779); in must it is "boost":0;
+  * clause order: should = history, similar items, boosted metadata, constant_score (:653, :681); must = history filter,
+    similar-items filter, filtering metadata, date filters (:703-709);
+  * must_not ids (:741-767): blacklistItems, then the item itself unless query.returnSelf.getOrElse(ap.returnSelf)
+    (default false, :237, :759), then distinct -- an item already in blacklistItems is not repeated;
+  * getSource casts the source unchecked to Map[String, List[String]] (EsClient.scala:435): a queried document whose
+    model-name member is not an array of strings makes that query fail; here it raises, naming the document.
+Deviation: the reference's GET for an empty item id addresses the type, not a document; here "" is looked up as any id.
 """
 from __future__ import annotations
 
@@ -92,6 +117,18 @@ class UserQuery:
         return UserQuery(d.get("userBias"), None if d.get("fields") is None else [Field.from_json(f) for f in d["fields"]],
                          d.get("currentDate"), None if dr is None else DateRange(dr["name"], dr.get("before"), dr.get("after")),
                          d.get("blacklistItems"), d.get("num"), d.get("from"), d.get("eventNames"))
+
+
+@dataclass
+class ItemQuery(UserQuery):
+    """the item-query members of Query (Engine.scala:32-50); the item itself is the record's"""
+    itemBias: Optional[float] = None
+    returnSelf: Optional[bool] = None
+
+    @staticmethod
+    def from_json(d: dict) -> "ItemQuery":
+        u = UserQuery.from_json(d)
+        return ItemQuery(**{k: getattr(u, k) for k in u.__dataclass_fields__}, itemBias=d.get("itemBias"), returnSelf=d.get("returnSelf"))
 
 
 def f32(x: float) -> float:
@@ -178,10 +215,11 @@ def max_query_events(ap) -> int:
     return sum(i.maxItemsPerUser or MAX_QUERY_EVENTS for i in ap.indicators) * 10
 
 
-def plan(ap, query: UserQuery, now_ms: Optional[int] = None) -> Plan:
+def plan(ap, query: UserQuery, now_ms: Optional[int] = None, with_limits: bool = True) -> Plan:
+    """with_limits=False: no per-name limits (an item query reads no history, so indicatorParams is never consulted)"""
     model_names = ap.model_event_names()
     names = list(query.eventNames) if query.eventNames is not None else list(model_names)
-    limits = query_event_limits(ap, names)
+    limits = query_event_limits(ap, names) if with_limits else []
     blacklist = list(ap.blacklistEvents) if ap.blacklistEvents is not None else list(model_names[:1])
     algo_bias = f32(ap.userBias) if ap.userBias is not None else 1.0
     b = f32(query.userBias) if query.userBias is not None else algo_bias
@@ -277,3 +315,100 @@ def user_queries(events, ap, query: Optional[UserQuery] = None, users: Optional[
     np.cumsum([len(r) for r in recs], out=offsets[1:])
     body = b"".join(recs)
     return (body, offsets) if users is not None else (body, offsets, who)
+
+
+@dataclass
+class ItemPlan:
+    """what every item's query shares"""
+    names: list                 # model event names: one similar-items clause each
+    max_query_events: int       # slice bound: a longer list keeps its first max_query_events - 1
+    in_must: bool               # the algorithm's itemBias < 0
+    boost: Optional[str]        # the similar items' boost text, None: no "boost"
+    exclude_self: bool          # not returnSelf
+    head: str
+    should_head: str            # the empty history clauses when they go to should, else ""
+    should: str
+    must_head: str              # the same in must
+    must: str
+    must_not: str
+    sort: str
+    blacklist_items: list = field(default_factory=list)
+
+
+def item_plan(ap, query: Optional[ItemQuery] = None, now_ms: Optional[int] = None) -> ItemPlan:
+    query = query or ItemQuery()
+    p = plan(ap, query, now_ms, with_limits=False)
+    history = ",".join(terms(n, [], "0" if p.in_must else p.boost) for n in p.names[:p.n_history])
+    algo_bias = f32(ap.itemBias) if ap.itemBias is not None else 1.0
+    b = f32(query.itemBias) if query.itemBias is not None else algo_bias
+    return_self = query.returnSelf if query.returnSelf is not None else bool(ap.returnSelf)
+    return ItemPlan(list(ap.model_event_names()), max_query_events(ap), algo_bias < 0, java_double(b) if b > 0 and b != 1 else None,
+                    not return_self, p.head, "" if p.in_must else history, p.should, history if p.in_must else "", p.must,
+                    p.must_not, p.sort, p.blacklist_items)
+
+
+def index_documents(index_body: bytes) -> list:
+    """a model index bulk body -> [(decoded _id, source dict)] in body order; json's last-member-wins for repeated names"""
+    if not index_body:
+        return []
+    if not index_body.endswith(b"\n"):
+        raise ValueError("the body does not end in a newline")
+    import json
+    lines = index_body[:-1].decode("utf-8", "surrogatepass").split("\n")
+    if len(lines) % 2:
+        raise ValueError(f"the body has {len(lines)} lines: lines come in (action, source) pairs")
+    docs, seen = [], {}
+    for d in range(len(lines) // 2):
+        action, source = json.loads(lines[2 * d]), json.loads(lines[2 * d + 1])
+        if not isinstance(action, dict) or list(action) != ["index"] or not isinstance(action["index"], dict) \
+                or not isinstance(action["index"].get("_id"), str):
+            raise ValueError(f"document {d}: the action line is not {{\"index\":{{...}}}} with a string \"_id\" member")
+        if not isinstance(source, dict):
+            raise ValueError(f"document {d}: the source line is not a JSON object")
+        i = action["index"]["_id"]
+        if i in seen:
+            raise ValueError(f"document {d}: its _id is the _id of document {seen[i]}")
+        seen[i] = d
+        docs.append((i, source))
+    return docs
+
+
+def similar_items(p: ItemPlan, d: int, source: dict) -> list:
+    """getBiasedSimilarItems on one document's source -> [terms clause per model name]"""
+    out = []
+    for n in p.names:
+        v = source.get(n, [])
+        if not isinstance(v, list) or not all(isinstance(x, str) for x in v):
+            raise ValueError(f'document {d}: its "{n}" member is not an array of strings')
+        v = v if len(v) <= p.max_query_events else v[:p.max_query_events - 1]
+        out.append(terms(n, v, "0" if p.in_must else p.boost))
+    return out
+
+
+def item_render(p: ItemPlan, similar: Sequence[str], excluded: Sequence[str]) -> str:
+    """buildQuery's document for an item query (URAlgorithm.scala:594-606) in json4s' compact rendering"""
+    should = [x for x in [p.should_head] if x] + ([] if p.in_must else list(similar)) + [x for x in [p.should] if x]
+    must = [x for x in [p.must_head] if x] + (list(similar) if p.in_must else []) + [x for x in [p.must] if x]
+    must_not = ['{"ids":{"values":[' + ",".join(json_string(x) for x in excluded) + '],"boost":0}}'] + ([p.must_not] if p.must_not else [])
+    return (p.head + ',"query":{"bool":{"should":[' + ",".join(should) + '],"must":[' + ",".join(must) + '],"must_not":['
+            + ",".join(must_not) + '],"minimum_should_match":1}},"sort":' + p.sort + "}")
+
+
+def item_queries(index_body: bytes, ap, query: Optional[ItemQuery] = None, items: Optional[Sequence[str]] = None,
+                 now_ms: Optional[int] = None, header: str = "{}"):
+    """the host mirror of CcoContext.item_queries over a model index bulk body -> (body, offsets), or (body, offsets, items)
+    for items=None (every document, in body order)"""
+    p = item_plan(ap, query, now_ms)
+    docs = index_documents(bytes(index_body))
+    by_id = {i: (d, src) for d, (i, src) in enumerate(docs)}
+    who = [i for i, _ in docs] if items is None else list(items)
+    recs = []
+    for it in who:
+        d, src = by_id.get(it, (-1, {}))
+        similar = similar_items(p, d, src) if src else []
+        excluded = _distinct(list(p.blacklist_items) + ([it] if p.exclude_self else []))
+        recs.append((header + "\n" + item_render(p, similar, excluded) + "\n").encode("utf-8", "surrogatepass"))
+    offsets = np.zeros(len(recs) + 1, dtype=np.int64)
+    np.cumsum([len(r) for r in recs], out=offsets[1:])
+    body = b"".join(recs)
+    return (body, offsets) if items is not None else (body, offsets, who)
