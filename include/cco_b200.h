@@ -667,6 +667,11 @@ int cco_debug_llr(cco_ctx_t *ctx, int64_t n, const int64_t *k11, const int64_t *
  * truncated to hash_bits (0..64) bits so that distinct ids collide on purpose.  ids[e] = dictionary id of id e, the
  * dictionary ordered by first appearance; the result is the same for every hash_bits. */
 int cco_debug_string_ids(cco_ctx_t *ctx, int64_t n, const int64_t *offsets, const char *bytes, int32_t hash_bits, int32_t *ids);
+/* Debug/parity entry (tests only): the rank number text of cco_format_model, Java's Double.toString of v[i] * 10^-scale,
+ * written by the device routine the document kernels call, once per value.  scale 0 (a histogram rank: |v[i]| < 2^53) or
+ * 15 (a random rank: 0 <= v[i] < 10^15).  Text i = bytes[offsets[i] .. offsets[i + 1]), offsets[0] = 0; offsets holds
+ * n + 1 entries and bytes 32 * n bytes, both the caller's (a text is at most 25 bytes long). */
+int cco_debug_rank_text(cco_ctx_t *ctx, int64_t n, const int64_t *v, int32_t scale, int64_t *offsets, char *bytes);
 void cco_free(void *p);
 
 #ifdef __cplusplus

@@ -1,4 +1,4 @@
-/* Plain-C consumer of the complete-model entry of include/cco_b200.h: its structs fill from C99 and the call type-checks.
+/* Plain-C consumer of the complete-model entries of include/cco_b200.h: their structs fill from C99 and the calls type-check.
  * Compiled by tests/test_model_docs.py. */
 #include <stddef.h>
 
@@ -15,4 +15,9 @@ int format_with_properties_and_rankings(cco_ctx_t *ctx, const cco_result_t *res,
   cco_ranking_stream_t stream = {2, ev_off, "item-1item-3", ev_time};
   cco_ranking_t ranking = {"popRank", CCO_POP_POPULAR, 1, 0, 5000, &stream};
   return cco_format_model(ctx, res, 1, names, rows, cols, &props, 1, &ranking, out, len);
+}
+
+int rank_texts(cco_ctx_t *ctx, char *bytes /* 32 * 3 */, int64_t offsets[4]) {
+  static const int64_t v[3] = {9999999, 10000000, -12000000};
+  return cco_debug_rank_text(ctx, 3, v, 0, offsets, bytes);
 }

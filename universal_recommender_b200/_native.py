@@ -138,7 +138,7 @@ EXPORTS = [
     "cco_format_model_log", "cco_rerank_model_log", "cco_event_log_free", "cco_event_log_begin", "cco_event_log_append",
     "cco_event_log_finish", "cco_event_log_begin_window", "cco_event_log_window_stats",
     "cco_event_log_begin_ex", "cco_event_log_user_queries", "cco_item_queries", "cco_result_num_matrices", "cco_result_row_range", "cco_result_matrix", "cco_result_stats", "cco_result_free",
-    "cco_debug_cooccurrence", "cco_debug_downsample", "cco_debug_downsample_block", "cco_debug_llr", "cco_debug_string_ids", "cco_free",
+    "cco_debug_cooccurrence", "cco_debug_downsample", "cco_debug_downsample_block", "cco_debug_llr", "cco_debug_string_ids", "cco_debug_rank_text", "cco_free",
 ]
 
 _lib = None
@@ -221,6 +221,7 @@ def lib():
     L.cco_debug_llr.argtypes = [C.c_void_p, C.c_int64, p(C.c_int64), p(C.c_int64), p(C.c_int64), p(C.c_int64), C.c_uint32,
                                 p(C.c_double)]
     L.cco_debug_string_ids.argtypes = [C.c_void_p, C.c_int64, p(C.c_int64), C.c_void_p, C.c_int32, p(C.c_int32)]
+    L.cco_debug_rank_text.argtypes = [C.c_void_p, C.c_int64, p(C.c_int64), C.c_int32, p(C.c_int64), C.c_void_p]
     L.cco_free.argtypes = [C.c_void_p]
     L.cco_free.restype = None
     _lib = L

@@ -5535,6 +5535,39 @@ int cco_debug_llr(cco_ctx_t *c, int64_t n, const int64_t *k11, const int64_t *k1
   return CCO_OK;
 }
 
+int cco_debug_rank_text(cco_ctx_t *c, int64_t n, const int64_t *v, int32_t scale, int64_t *offsets, char *bytes) {
+  if (!c || n < 0 || !offsets || (n > 0 && (!v || !bytes))) return set_error(CCO_E_INVALID_ARG, "bad argument");
+  if (scale != 0 && scale != 15) return set_error(CCO_E_INVALID_ARG, "scale %d is neither 0 nor 15", scale);
+  for (int64_t i = 0; i < n; ++i)
+    if (scale == 0 ? (v[i] <= -(1LL << 53) || v[i] >= (1LL << 53)) : (v[i] < 0 || v[i] >= 1000000000000000LL))
+      return set_error(CCO_E_INVALID_ARG, "value %lld at %lld is outside the range of scale %d", (long long)v[i], (long long)i, scale);
+  offsets[0] = 0;
+  if (n == 0) return CCO_OK;
+  CK(cudaSetDevice(c->device));
+  cudaStream_t s = c->stream;
+  Arena ar(s);
+  long long *d_v;
+  unsigned char *d_slot;
+  int32_t *d_len;
+  CKR(ar.alloc(&d_v, n));
+  CKR(ar.alloc(&d_slot, 32 * n));
+  CKR(ar.alloc(&d_len, n));
+  CK(cudaMemcpyAsync(d_v, v, sizeof(int64_t) * (size_t)n, cudaMemcpyHostToDevice, s));
+  k_debug_rank_text<<<grid_for(n, 256, c->sm_count), 256, 0, s>>>(n, d_v, scale, d_slot, d_len);
+  std::vector<unsigned char> slot((size_t)32 * n);
+  std::vector<int32_t> len((size_t)n);
+  CK(cudaMemcpyAsync(slot.data(), d_slot, slot.size(), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(len.data(), d_len, sizeof(int32_t) * (size_t)n, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  for (int64_t i = 0; i < n; ++i) {
+    if (len[i] < 1 || len[i] > 32) return set_error(CCO_E_CUDA, "text %lld has length %d", (long long)i, len[i]);
+    memcpy(bytes + offsets[i], slot.data() + 32 * (size_t)i, (size_t)len[i]);
+    offsets[i + 1] = offsets[i] + len[i];
+  }
+  return CCO_OK;
+}
+
 int cco_debug_downsample(cco_ctx_t *c, const cco_csr_t *m, int32_t max_interactions, int32_t seed, uint32_t flags,
                          int64_t **row_ptr, int32_t **col_idx, int32_t *raw_col_counts, int32_t *new_col_counts) {
   if (!c || !m || !row_ptr || !col_idx) return set_error(CCO_E_INVALID_ARG, "null argument");

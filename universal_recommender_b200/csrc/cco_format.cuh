@@ -140,6 +140,17 @@ __device__ __forceinline__ int java_double_text(long long v, int scale, unsigned
   return p;
 }
 
+// java_double_text of every value, one text per 32-byte slot (cco_debug_rank_text)
+__global__ void k_debug_rank_text(long long n, const long long *__restrict__ v, int scale, unsigned char *__restrict__ slot,
+                                  int32_t *__restrict__ len) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    unsigned char txt[32];
+    const int l = java_double_text(v[i], scale, txt);
+    for (int k = 0; k < l; ++k) slot[i * 32 + k] = txt[k];
+    len[i] = l;
+  }
+}
+
 // one document: a row of the slice (r >= 0) or an item without a row (r = -1); g = item group, -1 without one
 struct DocRef {
   const unsigned char *id;

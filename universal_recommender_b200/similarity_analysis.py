@@ -741,6 +741,16 @@ class CcoContext:
                                              hash_bits, ids.ctypes.data_as(C.POINTER(C.c_int32))))
         return ids[:len(off) - 1]
 
+    def debug_rank_text(self, values, scale: int = 0):
+        """cco_debug_rank_text: the model index's rank number text of every values[i] * 10^-scale (scale 0 or 15), as the
+        document kernels write it -> (offsets int64[n + 1], bytes uint8[])"""
+        v = np.ascontiguousarray(values, dtype=np.int64)
+        off = np.zeros(len(v) + 1, dtype=np.int64)
+        b = np.zeros(max(32 * len(v), 1), dtype=np.uint8)
+        N.check(self._L.cco_debug_rank_text(self._h, len(v), v.ctypes.data_as(C.POINTER(C.c_int64)), scale,
+                                            off.ctypes.data_as(C.POINTER(C.c_int64)), b.ctypes.data))
+        return off, b[:off[-1]]
+
     def debug_downsample(self, n_rows, n_cols, row_ptr, col_idx, max_interactions: int, seed: int, flags: int = 0):
         rp = np.ascontiguousarray(row_ptr, dtype=np.int64)
         ci = np.ascontiguousarray(col_idx, dtype=np.int32)
