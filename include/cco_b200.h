@@ -641,6 +641,46 @@ int cco_item_queries(cco_ctx_t *ctx, const char *index_body, int64_t index_len, 
                      int64_t *out_len, int64_t **out_offsets, int64_t *out_n, cco_dictionary_t *out_items /* nullable */);
 
 /*
+ * Item-set queries (URAlgorithm.buildQuery for Query.itemSet, user and item absent, URAlgorithm.scala:563-767): one
+ * Elasticsearch query per item set ("shopping cart"), built for a whole batch of sets.  The sets are the caller's input;
+ * nothing is read from a model or a history.
+ *  - Sets: the Arrow list<large_string> layout.  Set s holds the elements [set_offsets[s], set_offsets[s + 1]) of a
+ *    large_string column of n_elements ids; element e = elem_bytes[elem_offsets[e] .. elem_offsets[e + 1]).  Only the
+ *    elements [set_offsets[0], set_offsets[n_sets]) are read.
+ *  - The set clause, when with_set: {"terms":{"<name>":[elements]}}, the set's elements exactly as given (order and repeats
+ *    kept, no slicing), ending in ,"boost":<boost> when boost is not NULL.  It always goes to should.
+ *  - Excluded ids: blacklistItems in order, each once, then each element of the set that is not among them and did not
+ *    appear earlier in the set (ids compare as bytes).  A repeated element is written twice in the set clause and once here.
+ *  - The body record:
+ *      header \n head ,"query":{"bool":{"should":[should_head, SET?, should_tail],"must":[must],
+ *      "must_not":[{"ids":{"values":[excluded],"boost":0}}(,must_not)?],"minimum_should_match":1}},"sort":sort} \n
+ *    where SET stands when with_set; the elements of should are comma-separated and an empty piece leaves no comma.  Ids,
+ *    elements and the name are escaped as in cco_event_log_user_queries.
+ * Fragments are JSON text spliced verbatim: head ({"from":F,"size":N), should_head (buildQuery's empty user-history clauses
+ * when they go to should, then the boosted metadata; may be empty), should_tail (the constant_score clause), must (the
+ * empty history clauses when they go to must, the filtering metadata and the date filters; may be empty), must_not (may be
+ * empty), sort (an array), header (one _msearch header line).
+ * Out: *out_body [*out_len] and *out_offsets [*out_n + 1] (record s = body[offsets[s] .. offsets[s + 1])), pinned memory
+ * owned by the context, each released with cco_host_free.
+ * Errors: CCO_E_INVALID_ARG for bad offsets in any column (set offsets that decrease or leave [0, n_elements], element or
+ * blacklist item offsets that decrease; decided on the device before any kernel reads bytes through them), a null
+ * fragment, and a null or empty name while with_set; CCO_E_UNSUPPORTED for group contexts, 2^31 or more sets, elements +
+ * blacklist items >= 2^31 and a record of 2^31 or more bytes.
+ */
+typedef struct {
+  const char *name;                  /* the set clause's field: the first model event name (may be NULL without with_set) */
+  int32_t with_set;                  /* 0: no set clause (itemSetBias 0), 1: the clause is written */
+  const char *boost;                 /* JSON number text or NULL */
+  const char *head, *should_head, *should_tail, *must, *must_not, *sort, *header;  /* should_head, must may be "" */
+  int64_t n_blacklist_items;
+  const int64_t *blacklist_item_offsets; /* [n + 1] */
+  const char *blacklist_item_bytes;
+} cco_item_set_query_t;
+int cco_item_set_queries(cco_ctx_t *ctx, const cco_item_set_query_t *q, int64_t n_sets, const int64_t *set_offsets, int64_t n_elements,
+                         const int64_t *elem_offsets, const char *elem_bytes, char **out_body, int64_t *out_len, int64_t **out_offsets,
+                         int64_t *out_n);
+
+/*
  * Debug/parity entry (tests only): full integer co-occurrence matrix A^T B of two canonical
  * binary matrices computed by the same accumulation kernel as cco_train, no LLR, no top-k.
  * Output CSR over the columns of A with ascending column ids, malloc'ed; free with cco_free.

@@ -14,8 +14,9 @@ Host-side mirror of the reference interface for this path:
                                              (cco_rerank_model)
   ur_algorithm.calc_all_from_events / calc_pop_from_events  <- the same from a PredictionIO event export parsed on the
                                              GPU (cco_event_log_read: DataSource.scala:65-102); events.py is its host mirror
-  ur_algorithm.user_queries_from_events / item_queries  <- buildQuery for every user of an export / every item of a model
-                                             index, on the GPU (cco_event_log_user_queries, cco_item_queries); ur_query.py
+  ur_algorithm.user_queries_from_events / item_queries / item_set_queries  <- buildQuery for every user of an export /
+                                             every item of a model index / every item set of a batch, on the GPU
+                                             (cco_event_log_user_queries, cco_item_queries, cco_item_set_queries); ur_query.py
   ur_model                                <- propertiesRDD, getRanksRDD, groupAll (URAlgorithm.scala:351-369, 537-560;
                                              URModel.scala:57-140): the host mirror of the model documents
 """
@@ -27,15 +28,15 @@ from .preparator import prepare, prepare_on_device
 from .similarity_analysis import (CcoContext, DownsamplableCrossOccurrenceDataset, EventLog, SimilarityAnalysis,
                                   decode_ids, default_context, encode_ids)
 from .ur_algorithm import (DefaultURAlgoParams, IndicatorParams, URAlgorithmParams, calc_all, calc_all_from_events, calc_all_on_device,
-                           calc_pop_from_events, calc_pop_on_device, item_queries, user_queries_from_events)
-from .ur_query import ItemQuery, UserQuery
+                           calc_pop_from_events, calc_pop_on_device, item_queries, item_set_queries, user_queries_from_events)
+from .ur_query import ItemQuery, ItemSetQuery, UserQuery
 from .ur_model import RankingParams
 
 __all__ = [
     "BiDictionary", "CcoContext", "CcoError", "CcoInvalidArgument", "DataSourceParams", "DefaultURAlgoParams", "EventWindow",
     "DownsamplableCrossOccurrenceDataset", "IndexedDataset", "IndicatorParams", "SimilarityAnalysis",
     "EventLog", "RankingParams", "URAlgorithmParams", "calc_all", "calc_all_from_events", "calc_all_on_device", "calc_pop_from_events",
-    "calc_pop_on_device", "item_queries", "user_queries_from_events", "ItemQuery", "UserQuery", "decode_ids", "default_context", "encode_ids", "prepare", "prepare_on_device",
+    "calc_pop_on_device", "item_queries", "item_set_queries", "user_queries_from_events", "ItemQuery", "ItemSetQuery", "UserQuery", "decode_ids", "default_context", "encode_ids", "prepare", "prepare_on_device",
     "FLAG_ASSUME_CANONICAL",
     "FLAG_ENTROPY_VARARGS", "FLAG_ROWRATE_INTDIV", "FLAG_RESULT_NO_COUNT", "FLAG_RESULT_NO_LLR", "LIB_PATH",
 ]

@@ -5460,6 +5460,201 @@ int cco_item_queries(cco_ctx_t *ctx, const char *index_body, int64_t index_len, 
   return item_queries(ctx, index_body, index_len, q, n_items, item_offsets, item_bytes, out_body, out_len, out_offsets, out_n, out_items);
 }
 
+namespace cco {
+// the record template of an item-set query, 7 pieces: 0 head and "should":[, 1 should_head, 2 the start of the set clause,
+// 3 its end, 4 should_tail, 5 must up to the ids clause's values, 6 the rest of the record (see include/cco_b200.h)
+static std::vector<std::string> is_template(const cco_item_set_query_t *q) {
+  std::vector<std::string> t(7);
+  t[0] = std::string(q->header) + "\n" + q->head + ",\"query\":{\"bool\":{\"should\":[";
+  t[1] = q->should_head;
+  if (q->with_set) {
+    t[2] = "{\"terms\":{" + uq_quote(q->name) + ":[";
+    t[3] = q->boost ? std::string("],\"boost\":") + q->boost + "}}" : "]}}";
+  }
+  t[4] = q->should_tail;
+  t[5] = std::string("],\"must\":[") + q->must + "],\"must_not\":[{\"ids\":{\"values\":[";
+  t[6] = std::string("],\"boost\":0}}") + (*q->must_not ? std::string(",") + q->must_not : std::string()) +
+         "],\"minimum_should_match\":1}},\"sort\":" + q->sort + "}\n";
+  return t;
+}
+
+static int is_check_host(const cco_item_set_query_t *q, long long n_sets, const int64_t *soff, long long n_elements, const int64_t *eoff,
+                         const char *ebytes) {
+  if (q->with_set != 0 && q->with_set != 1) return set_error(CCO_E_INVALID_ARG, "with_set must be 0 or 1");
+  if (q->with_set && (!q->name || !*q->name)) return set_error(CCO_E_INVALID_ARG, "the set clause's name is null or empty");
+  if (!q->head || !q->should_head || !q->should_tail || !q->must || !q->must_not || !q->sort || !q->header)
+    return set_error(CCO_E_INVALID_ARG, "a null fragment");
+  CKR(str_check_host(q->n_blacklist_items, q->blacklist_item_offsets, q->blacklist_item_bytes, 0, "blacklist item"));
+  if (n_sets < 0 || n_elements < 0) return set_error(CCO_E_INVALID_ARG, "negative set or element count");
+  if (n_sets >= 0x7fffffffLL) return set_error(CCO_E_UNSUPPORTED, "%lld sets, at most 2^31 - 2", n_sets);
+  if (!soff) return set_error(CCO_E_INVALID_ARG, "null set offsets");
+  if (soff[0] < 0 || soff[0] > soff[n_sets] || soff[n_sets] > n_elements)
+    return set_error(CCO_E_INVALID_ARG, "set offsets [0] = %lld and [n_sets] = %lld are not within [0, n_elements = %lld] in order",
+                     (long long)soff[0], (long long)soff[n_sets], n_elements);
+  const long long NE = soff[n_sets] - soff[0];
+  if (NE + q->n_blacklist_items >= 0x7fffffffLL)
+    return set_error(CCO_E_UNSUPPORTED, "%lld elements + %lld blacklist items, at most 2^31 - 2", NE, (long long)q->n_blacklist_items);
+  if (NE > 0) CKR(str_check_host(NE, eoff ? eoff + soff[0] : nullptr, ebytes, 0, "element"));
+  return CCO_OK;
+}
+
+static int item_set_queries(cco_ctx *c, const cco_item_set_query_t *q, long long n_sets, const int64_t *set_off, const int64_t *eoff,
+                            const char *ebytes, char **out_body, int64_t *out_len, int64_t **out_offsets, int64_t *out_n) {
+  cudaStream_t s = c->stream;
+  CK(cudaSetDevice(c->device));
+  Arena ar(s);
+  nvtx_push("cco:item_set_queries");
+  struct Pop { ~Pop() { nvtx_pop(); } } pop;
+  mail_reset(c);
+  const long long S = n_sets, s0 = set_off[0], NE = set_off[S] - s0, NL = q->n_blacklist_items;
+  // 1. one key column: blacklistItems, then the sets' elements; the set offsets 0-based.  Every column's offsets are
+  //    checked on the device before any kernel reads bytes through them
+  const long long NK = NL + NE;
+  const long long nb = (NL > 0 ? q->blacklist_item_offsets[NL] - q->blacklist_item_offsets[0] : 0) + (NE > 0 ? eoff[s0 + NE] - eoff[s0] : 0);
+  DevStrCol key;
+  key.n = NK;
+  key.base = 0;
+  CKR(ar.alloc(&key.off, NK + 1));
+  CKR(ar.alloc(&key.w, (nb + 16 + 7) / 8));
+  CKR(ar.alloc(&key.hash, std::max<long long>(NK, 1)));
+  CK(cudaMemsetAsync(key.off, 0, 8, s));
+  int *bad, h_bad = 0;
+  CKR(ar.alloc(&bad, 1));
+  CK(cudaMemsetAsync(bad, 0, sizeof(int), s));
+  long long *soff, *stmp;
+  CKR(ar.alloc(&soff, S + 1));
+  CKR(ar.alloc(&stmp, S + 1));
+  CK(cudaMemcpyAsync(stmp, set_off, sizeof(int64_t) * ((size_t)S + 1), cudaMemcpyHostToDevice, s));
+  if (S > 0) {
+    k_str_check<<<grid_for(S, 256, c->sm_count), 256, 0, s>>>(S, stmp, bad);
+    c->launches++;
+  }
+  k_rebase<<<grid_for(S + 1, 256, c->sm_count), 256, 0, s>>>(S + 1, stmp, -s0, soff);
+  c->launches++;
+  long long at = 0, byte_at = 0;
+  for (int k = 0; k < 2; ++k) {
+    const long long n = k ? NE : NL;
+    const int64_t *off = k ? eoff + s0 : q->blacklist_item_offsets;
+    const char *bytes = k ? ebytes : q->blacklist_item_bytes;
+    if (n == 0) continue;
+    long long *tmp;
+    CKR(ar.alloc(&tmp, n + 1));
+    CK(cudaMemcpyAsync(tmp, off, sizeof(int64_t) * ((size_t)n + 1), cudaMemcpyHostToDevice, s));
+    k_str_check<<<grid_for(n, 256, c->sm_count), 256, 0, s>>>(n, tmp, bad);
+    k_rebase<<<grid_for(n + 1, 256, c->sm_count), 256, 0, s>>>(n + 1, tmp, byte_at - off[0], key.off + at);
+    c->launches += 2;
+    const long long kb = off[n] - off[0];
+    if (kb > 0) CK(cudaMemcpyAsync((char *)key.w + byte_at, bytes + off[0], (size_t)kb, cudaMemcpyHostToDevice, s));
+    at += n;
+    byte_at += kb;
+  }
+  CKR(mail_fetch(c, &h_bad, bad, 4));
+  CKR(mail_wait(c));
+  if (h_bad) return set_error(CCO_E_INVALID_ARG, "decreasing offsets in the sets, the elements or the blacklist items");
+  // 2. one exact grouping over the key column; blacklistItems: each group's first list index (membership is a group test)
+  str_hash(c, key, ~0ULL);
+  int32_t *gid;
+  CKR(ar.alloc(&gid, std::max<long long>(NK, 1)));
+  StrTable tb;
+  CKR(str_group(c, ar, key, nullptr, false, 0, &tb, gid));
+  const long long G = tb.n_groups;
+  uint32_t *first_in_list;
+  CKR(ar.alloc(&first_in_list, std::max<long long>(G, 1)));
+  CK(cudaMemsetAsync(first_in_list, 0xff, sizeof(uint32_t) * (size_t)std::max<long long>(G, 1), s));
+  if (NL > 0) {
+    k_iq_black<<<grid_for(NL, 256, c->sm_count), 256, 0, s>>>(NL, 0, gid, first_in_list);
+    c->launches++;
+  }
+  // 3. each element's first occurrence within its set: the first of each run of (set, group) keys after a stable sort
+  uint8_t *first_in_set;
+  CKR(ar.alloc(&first_in_set, std::max<long long>(NE, 1)));
+  if (NE > 0) {
+    unsigned long long *k2;
+    uint32_t *p2;
+    CKR(ar.alloc(&k2, NE));
+    CKR(ar.alloc(&p2, NE));
+    CK(cudaMemsetAsync(first_in_set, 0, (size_t)NE, s));
+    k_is_keys<<<grid_for(NE, 256, c->sm_count), 256, 0, s>>>(NE, S, soff, gid + NL, k2, p2);
+    c->launches++;
+    CKR(sort_pairs(c, ar, NE, &k2, &p2, 32 + bits_for(S)));
+    k_uq_first<<<grid_for(NE, 256, c->sm_count), 256, 0, s>>>(NE, k2, p2, first_in_set);
+    c->launches++;
+    ar.release(k2);
+    ar.release(p2);
+  }
+  // 4. the template, then a length pass, the record offsets and a write pass: one warp per set
+  const std::vector<std::string> tp = is_template(q);
+  std::vector<long long> toff(tp.size() + 1, 0);
+  std::string tbl;
+  for (size_t j = 0; j < tp.size(); ++j) {
+    tbl += tp[j];
+    toff[j + 1] = (long long)tbl.size();
+  }
+  long long *d_toff;
+  unsigned char *d_tb;
+  CKR(ar.alloc(&d_toff, (long long)toff.size()));
+  CKR(ar.alloc(&d_tb, std::max<long long>((long long)tbl.size(), 1)));
+  CK(cudaMemcpyAsync(d_toff, toff.data(), sizeof(long long) * toff.size(), cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(d_tb, tbl.data(), tbl.size(), cudaMemcpyHostToDevice, s));
+  IsArgs a;
+  a.n_sets = S;
+  a.soff = soff;
+  a.kgid = gid;
+  a.koff = key.off;
+  a.kbytes = (const unsigned char *)key.w;
+  a.n_list = NL;
+  a.first_in_list = first_in_list;
+  a.first_in_set = first_in_set;
+  a.with_set = q->with_set;
+  a.toff = d_toff;
+  a.tbytes = d_tb;
+  long long *rlen, *roff;
+  CKR(ar.alloc(&rlen, S + 1));
+  CKR(ar.alloc(&roff, S + 1));
+  CK(cudaMemsetAsync(rlen + S, 0, 8, s));
+  if (S > 0) {
+    k_is_record<false><<<grid_for(S * 32, 256, c->sm_count), 256, 0, s>>>(a, nullptr, rlen, nullptr);
+    c->launches++;
+  }
+  CKR(exclusive_sum(c, ar, rlen, roff, S + 1));
+  int64_t *ho = (int64_t *)c->pinned_get(sizeof(int64_t) * ((size_t)S + 1), /*for_result=*/false);
+  if (!ho) return set_error(CCO_E_OOM, "pinned host allocation failed");
+  CK(cudaMemcpyAsync(ho, roff, sizeof(int64_t) * ((size_t)S + 1), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  for (long long r = 0; r < S; ++r)
+    if (ho[r + 1] - ho[r] >= (1LL << 31)) {
+      c->pinned_put(ho);
+      return set_error(CCO_E_UNSUPPORTED, "record %lld has %lld bytes, at most 2^31 - 1", r, (long long)(ho[r + 1] - ho[r]));
+    }
+  const long long total = ho[S];
+  unsigned char *d_out;
+  CKR(ar.alloc(&d_out, std::max<long long>(total, 1)));
+  if (S > 0 && total > 0) {
+    k_is_record<true><<<grid_for(S * 32, 256, c->sm_count), 256, 0, s>>>(a, roff, nullptr, d_out);
+    c->launches++;
+  }
+  char *host = (char *)c->pinned_get((size_t)std::max<long long>(total, 1), /*for_result=*/false);
+  if (!host) return set_error(CCO_E_OOM, "pinned host allocation failed");
+  if (total > 0) CK(cudaMemcpyAsync(host, d_out, (size_t)total, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  *out_body = host;
+  *out_len = total;
+  *out_offsets = ho;
+  *out_n = S;
+  return CCO_OK;
+}
+}  // namespace cco
+
+int cco_item_set_queries(cco_ctx_t *ctx, const cco_item_set_query_t *q, int64_t n_sets, const int64_t *set_offsets, int64_t n_elements,
+                         const int64_t *elem_offsets, const char *elem_bytes, char **out_body, int64_t *out_len, int64_t **out_offsets,
+                         int64_t *out_n) {
+  if (!ctx || !q || !out_body || !out_len || !out_offsets || !out_n) return set_error(CCO_E_INVALID_ARG, "null argument");
+  if (!ctx->members.empty()) return set_error(CCO_E_UNSUPPORTED, "per-GPU contexts only");
+  CKR(is_check_host(q, n_sets, set_offsets, n_elements, elem_offsets, elem_bytes));
+  return item_set_queries(ctx, q, n_sets, set_offsets, elem_offsets, elem_bytes, out_body, out_len, out_offsets, out_n);
+}
+
 int cco_event_log_free(cco_event_log_t *lg) {
   event_log_release(lg);
   return CCO_OK;

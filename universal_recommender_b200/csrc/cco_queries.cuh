@@ -1,6 +1,7 @@
 // cco_queries.cuh -- cco_event_log_user_queries: buildQuery (URAlgorithm.scala:563-739) for user queries over the training
 // history an event log keeps (cco_event_log_begin_ex with CCO_LOG_KEEP_HISTORY); cco_item_queries: the same for item
-// queries over a model index body (its kernels are listed with them, below the user-query ones).
+// queries over a model index body; cco_item_set_queries: the same for item-set queries over the caller's sets (the kernels
+// of each are listed with them, below the user-query ones).
 //
 // e = one training event of a query event name (name rank q); its user and item are dense group ids of the log's columns.
 //   k_uq_select       e -> (log entry, name rank) over the query names' ranges of the name-partitioned columns
@@ -483,6 +484,99 @@ __global__ void __launch_bounds__(256) k_iq_record(IqArgs a, const long long *__
         return true;
       }, o, cur, first);
     piece(7);
+    if (!WRITE && lane == 0) rec_len[r] = cur;
+  }
+}
+
+// ---- cco_item_set_queries: buildQuery for item-set queries over the caller's sets ----------------------------------------
+// The key column is blacklistItems ++ the elements, grouped exactly by str_group; blacklist membership is k_iq_black's
+// first_in_list, and "first occurrence within its set" is the first of each run of (set << 32 | group) keys after one stable
+// sort (k_uq_first).
+//   k_is_keys      per element: the key (set << 32 | group), its position as value (the set by a search of the set offsets)
+//   k_is_record    one warp per set: template pieces, the set clause's elements as given, the exclusion list, a length pass
+//                  and a write pass (as k_uq_record)
+__global__ void k_is_keys(long long NE, long long n_sets, const long long *__restrict__ soff, const int32_t *__restrict__ egid,
+                          unsigned long long *__restrict__ key, uint32_t *__restrict__ pos) {
+  for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < NE; e += (long long)gridDim.x * blockDim.x) {
+    long long lo = 0, hi = n_sets - 1;   // the last s with soff[s] <= e (the set holding e: soff[s] <= e < soff[s + 1])
+    while (lo < hi) {
+      const long long mid = (lo + hi + 1) >> 1;
+      if (soff[mid] <= e) lo = mid; else hi = mid - 1;
+    }
+    key[e] = ((unsigned long long)lo << 32) | (uint32_t)egid[e];
+    pos[e] = (uint32_t)e;
+  }
+}
+
+struct IsArgs {
+  long long n_sets;
+  const long long *soff;           // [n_sets + 1] element index of each set's start, 0-based
+  const int32_t *kgid;             // key column: blacklistItems, then the elements; group per entry
+  const long long *koff;
+  const unsigned char *kbytes;
+  long long n_list;                // blacklistItems are key entries 0 .. n_list - 1, element e is entry n_list + e
+  const uint32_t *first_in_list;   // per group: first list index, ~0
+  const uint8_t *first_in_set;     // [n_elements] the element is its string's first occurrence in its set
+  int with_set;
+  const long long *toff;           // [8] template pieces (see is_template)
+  const unsigned char *tbytes;
+};
+
+// (256, 1): without the minimum, ptxas holds the length pass to 32 registers and spills its loop state; with it the two
+// passes take 36 and 46 registers and spill nothing
+template <bool WRITE>
+__global__ void __launch_bounds__(256, 1) k_is_record(IsArgs a, const long long *__restrict__ rec_off, long long *__restrict__ rec_len,
+                                                   unsigned char *__restrict__ out) {
+  const int lane = threadIdx.x & 31;
+  const long long warps = (long long)gridDim.x * (blockDim.x >> 5);
+  for (long long r = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5; r < a.n_sets; r += warps) {
+    const long long e0 = a.soff[r], n = a.soff[r + 1] - e0, k0 = a.n_list + e0;
+    unsigned char *o = WRITE ? out + rec_off[r] : nullptr;
+    long long cur = 0;
+    auto piece = [&](int j) {
+      const long long t0 = a.toff[j], tl = a.toff[j + 1] - t0;
+      if (WRITE)
+        for (long long k = lane; k < tl; k += 32) o[cur + k] = a.tbytes[t0 + k];
+      cur += tl;
+      return tl > 0;
+    };
+    auto comma = [&]() {
+      if (WRITE && lane == 0) o[cur] = ',';
+      cur += 1;
+    };
+    piece(0);
+    bool any = piece(1);   // should: should_head, the set clause, should_tail
+    if (a.with_set) {
+      if (any) comma();
+      piece(2);
+      bool first = true;   // every element as given
+      uq_list(n, [&](long long i, const unsigned char **p, long long *len) {
+        *p = a.kbytes + a.koff[k0 + i];
+        *len = a.koff[k0 + i + 1] - a.koff[k0 + i];
+        return true;
+      }, o, cur, first);
+      piece(3);
+      any = true;
+    }
+    if (a.toff[5] > a.toff[4]) {
+      if (any) comma();
+      piece(4);
+    }
+    piece(5);
+    bool first = true;   // blacklistItems, each once, then the set's first occurrences that are not among them
+    uq_list(a.n_list, [&](long long i, const unsigned char **p, long long *len) {
+      if (a.first_in_list[a.kgid[i]] != (uint32_t)i) return false;
+      *p = a.kbytes + a.koff[i];
+      *len = a.koff[i + 1] - a.koff[i];
+      return true;
+    }, o, cur, first);
+    uq_list(n, [&](long long i, const unsigned char **p, long long *len) {
+      if (!a.first_in_set[e0 + i] || a.first_in_list[a.kgid[k0 + i]] != ~0u) return false;
+      *p = a.kbytes + a.koff[k0 + i];
+      *len = a.koff[k0 + i + 1] - a.koff[k0 + i];
+      return true;
+    }, o, cur, first);
+    piece(6);
     if (!WRITE && lane == 0) rec_len[r] = cur;
   }
 }

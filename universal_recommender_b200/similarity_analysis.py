@@ -554,6 +554,41 @@ class CcoContext:
         self._L.cco_host_free(self._h, C.c_void_p(addr))
         return body, offsets, ids
 
+    def item_set_queries(self, sets, ap, query=None, now_ms: Optional[int] = None, header: str = "{}"):
+        """cco_item_set_queries: URAlgorithm.buildQuery for item-set ("shopping cart") queries (ur_query.py restates it), one
+        per set.  sets: a sequence of sequences of str, or the Arrow list<large_string> buffers (set_offsets int64[n + 1],
+        elem_offsets int64[m + 1], elem_bytes) of a batch too large to pass as Python strings.  ap:
+        ur_algorithm.URAlgorithmParams; query: ur_query.ItemSetQuery (None: defaults).
+        -> (body, offsets int64[n + 1]): `header\nquery\n` records, the _msearch body; record s = body[offsets[s]:offsets[s + 1]]."""
+        from . import ur_query as Q
+        p = Q.item_set_plan(ap, query, now_ms)
+        enc = lambda x: x.encode("utf-8", "surrogatepass")
+
+        def column(ids):   # ids compare as UTF-8 bytes, a lone surrogate in its 3-byte form
+            b = [enc(x) for x in ids]
+            o = np.zeros(len(b) + 1, dtype=np.int64)
+            np.cumsum([len(x) for x in b], out=o[1:])
+            return o, np.frombuffer(b"".join(b), dtype=np.uint8)
+        if isinstance(sets, tuple) and len(sets) == 3 and isinstance(sets[0], np.ndarray):
+            so, eo, eb = np.ascontiguousarray(sets[0], dtype=np.int64), np.ascontiguousarray(sets[1], dtype=np.int64), sets[2]
+            eb = np.frombuffer(eb, dtype=np.uint8) if isinstance(eb, (bytes, bytearray, memoryview)) else np.ascontiguousarray(eb, dtype=np.uint8)
+        else:
+            sets = [list(s) for s in sets]
+            so = np.zeros(len(sets) + 1, dtype=np.int64)
+            np.cumsum([len(s) for s in sets], out=so[1:])
+            eo, eb = column([x for s in sets for x in s])
+        lo, lb = column(p.blacklist_items)
+        qt = N.ItemSetQueryT(None if p.name is None else enc(p.name), 1 if p.with_set else 0, None if p.boost is None else p.boost.encode(),
+                             enc(p.head), enc(p.should_head), enc(p.should_tail), enc(p.must), enc(p.must_not), enc(p.sort), enc(header),
+                             len(lo) - 1, lo.ctypes.data_as(C.POINTER(C.c_int64)), lb.ctypes.data if len(lb) else None)
+        out, ln, off, n = C.c_void_p(), C.c_int64(), C.c_void_p(), C.c_int64()
+        N.check(self._L.cco_item_set_queries(self._h, C.byref(qt), len(so) - 1, so.ctypes.data_as(C.POINTER(C.c_int64)), len(eo) - 1,
+                                             eo.ctypes.data_as(C.POINTER(C.c_int64)), eb.ctypes.data if len(eb) else None, C.byref(out),
+                                             C.byref(ln), C.byref(off), C.byref(n)))
+        offsets = np.ctypeslib.as_array(C.cast(off, C.POINTER(C.c_int64)), shape=(n.value + 1,)).copy()
+        self._L.cco_host_free(self._h, off)
+        return self._take_body(out, ln), offsets
+
     def rerank_model(self, body: bytes, properties=None, rankings=None, log=None) -> bytes:
         """cco_rerank_model: calcPop (URAlgorithm.scala:375-399, recsModel "backfill") on an existing index.  body = the
         Elasticsearch bulk body of the current model, as format_model writes it; properties and rankings as in format_model.

@@ -5,7 +5,8 @@ calc_pop_on_device runs calcPop (recsModel "backfill") on the GPU: the current i
 fresh rankings out.  calc_all_from_events / calc_pop_from_events do the same from a PredictionIO event export parsed on the
 device (CcoContext.read_events), the DataSource included.  user_queries_from_events builds buildQuery's user queries for a
 whole user base from the same export (ur_query.py restates buildQuery); item_queries builds its item queries for every
-item of a model index body.  Out of scope: item-set queries, Elasticsearch's scoring, reading the index and the HTTP
+item of a model index body; item_set_queries builds its item-set ("shopping cart") queries for a batch of sets.  Out of
+scope: mixed queries (user, item and itemSet together), withRanks, Elasticsearch's scoring, reading the index and the HTTP
 call."""
 from __future__ import annotations
 
@@ -15,7 +16,7 @@ from typing import Optional, Sequence
 
 from .indexed_dataset import IndexedDataset
 from .similarity_analysis import CcoContext, DownsamplableCrossOccurrenceDataset, SimilarityAnalysis, default_context, encode_ids
-from .ur_query import Field, ItemQuery, UserQuery
+from .ur_query import Field, ItemQuery, ItemSetQuery, UserQuery
 from .ur_model import (RankingParams, RankingType, extract_jvalue, property_json, ranking_window, rankings_for,
                        rankings_params)
 
@@ -337,3 +338,14 @@ def item_queries(index_body: bytes, ap: URAlgorithmParams, query: Optional[ItemQ
     now_ms: "now" of the available / expire date filter (default: the wall clock).  The fragments are ur_query.item_plan's."""
     ctx = ctx or default_context()
     return ctx.item_queries(index_body, ap, query, items, _now(now_ms), header)
+
+
+def item_set_queries(sets, ap: URAlgorithmParams, query: Optional[ItemSetQuery] = None, now_ms: Optional[int] = None,
+                     ctx: CcoContext | None = None, header: str = "{}"):
+    """buildQuery (URAlgorithm.scala:563-767) for every item set ("shopping cart") of `sets` on the device: one
+    `header\nquery\n` record per set, the body of an Elasticsearch _msearch.  sets: a sequence of sequences of str, or the
+    Arrow list<large_string> buffers (set_offsets, elem_offsets, elem_bytes).  -> (body, offsets) as
+    CcoContext.item_set_queries.  now_ms: "now" of the available / expire date filter (default: the wall clock).  The
+    fragments are ur_query.item_set_plan's; ValueError without a model event name (the set clause's field)."""
+    ctx = ctx or default_context()
+    return ctx.item_set_queries(sets, ap, query, _now(now_ms), header)

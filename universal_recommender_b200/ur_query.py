@@ -1,4 +1,5 @@
-"""URAlgorithm.buildQuery for user queries (Query.user set; item, itemSet and withRanks absent), restated from
+"""URAlgorithm.buildQuery for user queries (Query.user set; item, itemSet and withRanks absent), item queries and
+item-set queries (both below), restated from
 src/main/scala/URAlgorithm.scala:195-267 (parameters), :563-767 (should / must / must_not / sort), :795-839
 (getBiasedRecentUserActions) and :872-953 (date filters).  The query is the text the reference posts to Elasticsearch;
 scoring stays with Elasticsearch.
@@ -62,6 +63,27 @@ CcoContext.format_model / rerank_model write).  Quirks of the reference, kept on
   * getSource casts the source unchecked to Map[String, List[String]] (EsClient.scala:435): a queried document whose
     model-name member is not an array of strings makes that query fail; here it raises, naming the document.
 Deviation: the reference's GET for an empty item id addresses the type, not a document; here "" is looked up as any id.
+
+Item-set queries (Query.itemSet set: "shopping cart" recommendations; user, item and withRanks absent): item_set_plan()
+renders what every set's query shares (the fragments CcoContext.item_set_queries hands to the device); item_set_queries()
+is the host mirror over a list of sets.  Nothing is read: the set is the caller's.  Quirks of the reference, kept on purpose:
+  * history clauses are still written, empty, exactly as for item queries (getBiasedRecentUserActions, :795-839): the
+    first maxQueryEvents - 1 query event names (query eventNames, else the model names), in should with the user boost or
+    in must with "boost":0 when the algorithm's userBias < 0; indicatorParams is never consulted;
+  * no similar items (query.item is empty, :630, :695);
+  * the set clause is BoostableCorrelators(modelEventNames.head, itemSet, query.itemSetBias) (:640-648): its field is the
+    *first model event name*, not a query eventName, and with no model event name the reference's .head throws (here
+    ValueError); its elements are the set exactly as given -- order and repeats kept, no maxQueryEvents slice;
+  * its boost is query.itemSetBias only, a Float widened to Double, with no algorithm-level fallback (Engine.scala:38's
+    comment says otherwise) and no > 0 / != 1 test: None writes no "boost", 1 writes "boost":1.0, -1 writes "boost":-1.0
+    in should; boost.getOrElse(1f) != 0f (:656-659) drops the clause for 0 and -0.0; an empty set ("itemSet": [] is
+    Some(Nil)) still writes {"terms":{"<name>":[]}};
+  * clause order: should = history, boosted metadata, the set clause, constant_score (:653, :681); must = history filter,
+    filtering metadata, date filters (:703-709); the set clause never goes to must;
+  * must_not ids (getExcludedItems, :741-767): distinct(blacklistItems ++ itemSet) -- the blacklist first, each once, then
+    each set element not among them and not earlier in the set: a repeated element is written twice in the set clause and
+    once here.
+Out of scope: mixed queries (user or item next to itemSet, :641-644), withRanks (it only changes how results are read).
 """
 from __future__ import annotations
 
@@ -131,6 +153,17 @@ class ItemQuery(UserQuery):
         return ItemQuery(**{k: getattr(u, k) for k in u.__dataclass_fields__}, itemBias=d.get("itemBias"), returnSelf=d.get("returnSelf"))
 
 
+@dataclass
+class ItemSetQuery(UserQuery):
+    """the item-set-query members of Query (Engine.scala:32-50); the set itself is the record's"""
+    itemSetBias: Optional[float] = None
+
+    @staticmethod
+    def from_json(d: dict) -> "ItemSetQuery":
+        u = UserQuery.from_json(d)
+        return ItemSetQuery(**{k: getattr(u, k) for k in u.__dataclass_fields__}, itemSetBias=d.get("itemSetBias"))
+
+
 def f32(x: float) -> float:
     return float(np.float32(x))
 
@@ -191,6 +224,7 @@ class Plan:
     must_not: str               # must_not elements after the ids clause
     sort: str
     blacklist_items: list = field(default_factory=list)
+    boosted: str = ""           # the boosted metadata clauses of `should`, without the constant_score clause
 
 
 def query_event_limits(ap, names: Sequence[str]) -> list:
@@ -241,7 +275,7 @@ def plan(ap, query: UserQuery, now_ms: Optional[int] = None, with_limits: bool =
     else:
         sort = "[]"
     return Plan(names, limits, blacklist, boost, algo_bias < 0, n_history, head, ",".join(should), ",".join(must), ",".join(must_not),
-                sort, list(query.blacklistItems or []))
+                sort, list(query.blacklistItems or []), ",".join(should[:-1]))
 
 
 def _range(name: str, bounds: Sequence[tuple[str, str]]) -> str:
@@ -412,3 +446,51 @@ def item_queries(index_body: bytes, ap, query: Optional[ItemQuery] = None, items
     np.cumsum([len(r) for r in recs], out=offsets[1:])
     body = b"".join(recs)
     return (body, offsets) if items is not None else (body, offsets, who)
+
+
+@dataclass
+class ItemSetPlan:
+    """what every item set's query shares"""
+    name: Optional[str]         # the set clause's field: the first model event name
+    with_set: bool              # itemSetBias != 0: the set clause is written
+    boost: Optional[str]        # the set clause's boost text (the query's itemSetBias), None: no "boost"
+    head: str
+    should_head: str            # the empty history clauses when they go to should, then the boosted metadata
+    should_tail: str            # the constant_score clause
+    must: str                   # the empty history clauses when they go to must, the filtering metadata, the date filters
+    must_not: str
+    sort: str
+    blacklist_items: list = field(default_factory=list)
+
+
+def item_set_plan(ap, query: Optional[ItemSetQuery] = None, now_ms: Optional[int] = None) -> ItemSetPlan:
+    query = query or ItemSetQuery()
+    model_names = ap.model_event_names()
+    if not model_names:
+        raise ValueError("an item-set query needs a model event name: the set clause's field is the first one")
+    p = plan(ap, query, now_ms, with_limits=False)
+    history = [terms(n, [], "0" if p.in_must else p.boost) for n in p.names[:p.n_history]]
+    b = None if query.itemSetBias is None else f32(query.itemSetBias)
+    should_head = ([] if p.in_must else history) + ([p.boosted] if p.boosted else [])
+    must = (history if p.in_must else []) + ([p.must] if p.must else [])
+    return ItemSetPlan(model_names[0], b is None or b != 0, None if b is None else java_double(b), p.head, ",".join(should_head),
+                       CONSTANT_SCORE, ",".join(must), p.must_not, p.sort, p.blacklist_items)
+
+
+def item_set_render(p: ItemSetPlan, item_set: Sequence[str]) -> str:
+    """buildQuery's document for an item-set query (URAlgorithm.scala:594-606) in json4s' compact rendering"""
+    should = [x for x in [p.should_head] if x] + ([terms(p.name, item_set, p.boost)] if p.with_set else []) + [x for x in [p.should_tail] if x]
+    excluded = list(dict.fromkeys(list(p.blacklist_items) + list(item_set)))   # distinct, first position
+    must_not = ['{"ids":{"values":[' + ",".join(json_string(x) for x in excluded) + '],"boost":0}}'] + ([p.must_not] if p.must_not else [])
+    return (p.head + ',"query":{"bool":{"should":[' + ",".join(should) + '],"must":[' + p.must + '],"must_not":['
+            + ",".join(must_not) + '],"minimum_should_match":1}},"sort":' + p.sort + "}")
+
+
+def item_set_queries(sets: Sequence[Sequence[str]], ap, query: Optional[ItemSetQuery] = None, now_ms: Optional[int] = None,
+                     header: str = "{}"):
+    """the host mirror of CcoContext.item_set_queries: one record per set, in order -> (body, offsets)"""
+    p = item_set_plan(ap, query, now_ms)
+    recs = [(header + "\n" + item_set_render(p, list(s)) + "\n").encode("utf-8", "surrogatepass") for s in sets]
+    offsets = np.zeros(len(recs) + 1, dtype=np.int64)
+    np.cumsum([len(r) for r in recs], out=offsets[1:])
+    return b"".join(recs), offsets
