@@ -337,6 +337,10 @@ static int pooled_event(cco_ctx *c, bool timing, cudaEvent_t *out) {
 // NVTX ranges per stage (SURVEY.md section 5: tracing); header-only NVTX3, a no-op unless a profiler is attached
 static inline void nvtx_push(const char *name) { nvtxRangePushA(name); }
 static inline void nvtx_pop() { nvtxRangePop(); }
+struct NvtxRange {   // a range over one scope
+  explicit NvtxRange(const char *name) { nvtx_push(name); }
+  ~NvtxRange() { nvtx_pop(); }
+};
 
 static inline int grid_for(long long work_items, int block, int sm_count, int waves = 8) {
   long long g = (work_items + block - 1) / block;
@@ -2363,8 +2367,7 @@ using StrColumns = std::function<int(Arena &, int, DevStrCol *, DevStrCol *)>;
 static int ingest_strings_core(cco_ctx *c, int32_t n_types, const StrColumns &columns, int32_t min_events_per_user, cco_dataset **out) {
   CK(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
-  nvtx_push("cco:ingest_strings");
-  struct Pop { ~Pop() { nvtx_pop(); } } pop;
+  NvtxRange nvtx("cco:ingest_strings");
   mail_reset(c);
   Arena ar(s);
   cco_dataset *d = ingest_dataset_new(c, n_types);
@@ -2638,6 +2641,18 @@ static int upload_dict(cco_ctx *c, Arena &ar, const cco_dictionary_t &d, DevDict
   raw->n = d.n;
   return CCO_OK;
 }
+// a few host strings as a device dictionary; waits for the copies, since the flattened strings are local
+static int upload_strings(cco_ctx *c, Arena &ar, const std::vector<std::string> &strs, DevDict *raw) {
+  std::vector<int64_t> off(strs.size() + 1, 0);
+  std::string blob;
+  for (size_t i = 0; i < strs.size(); ++i) {
+    blob += strs[i];
+    off[i + 1] = (int64_t)blob.size();
+  }
+  CKR(upload_dict(c, ar, cco_dictionary_t{(int64_t)strs.size(), off.data(), blob.data()}, raw));
+  CK(cudaStreamSynchronize(c->stream));
+  return CCO_OK;
+}
 // JSON-escape every string of a device dictionary (two passes: lengths, scan, bytes)
 static int escape_dict(cco_ctx *c, Arena &ar, const DevDict &raw, DevDict *esc) {
   long long *len, *off;
@@ -2692,8 +2707,8 @@ static PopArgs pop_args(int mode, long long start_ms, long long end_ms, int32_t 
   return a;
 }
 
-// one section of the combined key column: the row dictionary, the property items or one ranking stream.  A device
-// section (the decoded ids of an old index, cco_rerank_model) is already in HBM: offsets from 0, nbytes bytes.
+// one section of a combined key column (key_column), e.g. the row dictionary, the property items or one ranking stream.  A
+// device section (the decoded ids of an index body) is already in HBM: offsets from 0, nbytes bytes.
 struct KeySection {
   long long n;
   const int64_t *off;
@@ -2718,6 +2733,50 @@ struct DevProps {
   const unsigned char *vals;
 };
 
+// One string column of the sections in order: offsets from 0, bytes as 8-byte words with 16 bytes of padding.  A host
+// section's offsets are checked on the device into *bad; the caller reads that verdict before any kernel reads bytes
+// through the key column.
+static int key_column(cco_ctx *c, Arena &ar, const std::vector<KeySection> &sec, int *bad, DevStrCol *key) {
+  cudaStream_t s = c->stream;
+  long long N = 0, nb = 0, max_n = 0;
+  for (const KeySection &k : sec) {
+    N += k.n;
+    nb += k.byte_count();
+    max_n = std::max(max_n, k.n);
+  }
+  key->n = N;
+  key->base = 0;
+  CKR(ar.alloc(&key->off, N + 1));
+  CKR(ar.alloc(&key->w, (nb + 16 + 7) / 8));
+  CKR(ar.alloc(&key->hash, std::max<long long>(N, 1)));
+  CK(cudaMemsetAsync(key->off, 0, 8, s));
+  long long *tmp_off;
+  CKR(ar.alloc(&tmp_off, max_n + 1));
+  // every section: raw offsets -> decreasing check -> rebased into the key column; bytes appended to the word buffer
+  long long at = 0, byte_at = 0;
+  for (const KeySection &k : sec) {
+    if (k.n == 0) continue;
+    const long long kb = k.byte_count();
+    if (k.device) {
+      k_rebase<<<grid_for(k.n + 1, 256, c->sm_count), 256, 0, s>>>(k.n + 1, (const long long *)k.off, byte_at - k.base, key->off + at);
+      c->launches++;
+      if (kb > 0) CK(cudaMemcpyAsync((char *)key->w + byte_at, k.bytes, (size_t)kb, cudaMemcpyDeviceToDevice, s));
+      at += k.n;
+      byte_at += kb;
+      continue;
+    }
+    CK(cudaMemcpyAsync(tmp_off, k.off, sizeof(int64_t) * ((size_t)k.n + 1), cudaMemcpyHostToDevice, s));
+    k_str_check<<<grid_for(k.n, 256, c->sm_count), 256, 0, s>>>(k.n, tmp_off, bad);
+    k_rebase<<<grid_for(k.n + 1, 256, c->sm_count), 256, 0, s>>>(k.n + 1, tmp_off, byte_at - k.off[0], key->off + at);
+    c->launches += 2;
+    if (kb > 0) CK(cudaMemcpyAsync((char *)key->w + byte_at, k.bytes + k.off[0], (size_t)kb, cudaMemcpyHostToDevice, s));
+    at += k.n;
+    byte_at += kb;
+  }
+  ar.release(tmp_off);
+  return CCO_OK;
+}
+
 // The model part of FormatArgs (cco_format_model, cco_rerank_model): group the item ids of every source, score the
 // rankings per group, sort the properties, and list the documents of items without a row.  The caller's host columns have
 // passed str_check_host.  unique_rows: two rows with the same id are CCO_E_INVALID_ARG (the documents of an old index).
@@ -2741,43 +2800,11 @@ static int model_fields(cco_ctx *c, Arena &ar, FormatArgs *fa, const KeySection 
   }
   rank_begin[n_rank] = E;
   const long long N = R + P + E;
-  long long nb = 0;
-  for (const KeySection &k : sec) nb += k.byte_count();
-  DevStrCol key;
-  key.n = N;
-  key.base = 0;
-  CKR(ar.alloc(&key.off, N + 1));
-  CKR(ar.alloc(&key.w, (nb + 16 + 7) / 8));
-  CKR(ar.alloc(&key.hash, std::max<long long>(N, 1)));
-  CK(cudaMemsetAsync(key.off, 0, 8, s));
   int *bad;
   CKR(ar.alloc(&bad, 1));
   CK(cudaMemsetAsync(bad, 0, sizeof(int), s));
-  long long *tmp_off;
-  long long max_n = 0;
-  for (const KeySection &k : sec) max_n = std::max(max_n, k.n);
-  CKR(ar.alloc(&tmp_off, max_n + 1));
-  // every section: raw offsets -> decreasing check -> rebased into the key column; bytes appended to the word buffer
-  long long at = 0, byte_at = 0;
-  for (const KeySection &k : sec) {
-    if (k.n == 0) continue;
-    const long long kb = k.byte_count();
-    if (k.device) {
-      k_rebase<<<grid_for(k.n + 1, 256, c->sm_count), 256, 0, s>>>(k.n + 1, (const long long *)k.off, byte_at - k.base, key.off + at);
-      c->launches++;
-      if (kb > 0) CK(cudaMemcpyAsync((char *)key.w + byte_at, k.bytes, (size_t)kb, cudaMemcpyDeviceToDevice, s));
-      at += k.n;
-      byte_at += kb;
-      continue;
-    }
-    CK(cudaMemcpyAsync(tmp_off, k.off, sizeof(int64_t) * ((size_t)k.n + 1), cudaMemcpyHostToDevice, s));
-    k_str_check<<<grid_for(k.n, 256, c->sm_count), 256, 0, s>>>(k.n, tmp_off, bad);
-    k_rebase<<<grid_for(k.n + 1, 256, c->sm_count), 256, 0, s>>>(k.n + 1, tmp_off, byte_at - k.off[0], key.off + at);
-    c->launches += 2;
-    if (kb > 0) CK(cudaMemcpyAsync((char *)key.w + byte_at, k.bytes + k.off[0], (size_t)kb, cudaMemcpyHostToDevice, s));
-    at += k.n;
-    byte_at += kb;
-  }
+  DevStrCol key;
+  CKR(key_column(c, ar, sec, bad, &key));
   // property fields and values
   int32_t *d_field = nullptr;
   if (dp && P > 0) {   // built on the device: nothing to copy or check
@@ -2821,7 +2848,6 @@ static int model_fields(cco_ctx *c, Arena &ar, FormatArgs *fa, const KeySection 
   if (h_bad & 1) return set_error(CCO_E_INVALID_ARG, "offsets decrease");
   if (h_bad & 2) return set_error(CCO_E_INVALID_ARG, "a property field index is outside [0, %d)", props->n_fields);
   if (h_bad & 4) return set_error(CCO_E_INVALID_ARG, "an empty property value (values are JSON text)");
-  ar.release(tmp_off);
 
   // 1. item key space: one exact grouping by string over every source, numbered by first appearance
   str_hash(c, key, ~0ULL);
@@ -3000,33 +3026,23 @@ static int model_names(cco_ctx *c, Arena &ar, FormatArgs *fa, int n_ind, const c
                        const cco_item_properties_t *props, int32_t n_rank, const cco_ranking_t *rk) {
   cudaStream_t s = c->stream;
   const int n_fields = props ? props->n_fields : 0;
-  std::vector<const char *> all_names(names, names + n_ind);
+  std::vector<std::string> all_names(names, names + n_ind);
   if (model) {
     for (int f = 0; f < n_fields; ++f) all_names.push_back(props->field_names[f]);
     for (int k = 0; k < n_rank; ++k) all_names.push_back(rk[k].name);
   }
   const int n_all = (int)all_names.size();
   std::vector<long long> eoff(n_all + 1);
-  {
-    std::vector<int64_t> noff(n_all + 1, 0);
-    std::string blob;
-    for (int i = 0; i < n_all; ++i) {
-      blob += all_names[i];
-      noff[i + 1] = (int64_t)blob.size();
-    }
-    cco_dictionary_t nd = {n_all, noff.data(), blob.data()};
-    DevDict nraw, nesc;
-    CKR(upload_dict(c, ar, nd, &nraw));
-    CK(cudaStreamSynchronize(s));   // noff / blob are locals
-    CKR(escape_dict(c, ar, nraw, &nesc));
-    CK(cudaMemcpyAsync(eoff.data(), nesc.off, sizeof(long long) * ((size_t)n_all + 1), cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    fa->names = nesc.bytes;
-    for (int i = 0; i <= n_ind; ++i) fa->name_off[i] = (int32_t)eoff[i];
-    if (model) {
-      fa->field_off = nesc.off + n_ind;
-      for (int k = 0; k <= n_rank; ++k) fa->rank_name_off[k] = (int32_t)eoff[n_ind + n_fields + k];
-    }
+  DevDict nraw, nesc;
+  CKR(upload_strings(c, ar, all_names, &nraw));
+  CKR(escape_dict(c, ar, nraw, &nesc));
+  CK(cudaMemcpyAsync(eoff.data(), nesc.off, sizeof(long long) * ((size_t)n_all + 1), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  fa->names = nesc.bytes;
+  for (int i = 0; i <= n_ind; ++i) fa->name_off[i] = (int32_t)eoff[i];
+  if (model) {
+    fa->field_off = nesc.off + n_ind;
+    for (int k = 0; k <= n_rank; ++k) fa->rank_name_off[k] = (int32_t)eoff[n_ind + n_fields + k];
   }
   if (model) {
     // precedence, lowest to highest: indicators < properties < rankings (a later ranking beats an earlier one) < "id".
@@ -3059,6 +3075,28 @@ static int model_names(cco_ctx *c, Arena &ar, FormatArgs *fa, int n_ind, const c
   return CCO_OK;
 }
 
+// The total bytes at d_out into pinned memory of `owner` (released with cco_host_free on that context), then the wait for
+// stream s; `also` may enqueue more copies before the wait.  On failure the pinned memory is given back.
+static int body_to_host(cco_ctx *owner, cudaStream_t s, const unsigned char *d_out, long long total, char **out_bytes, int64_t *out_len,
+                        const std::function<int()> &also = nullptr) {
+  char *host = (char *)owner->pinned_get((size_t)std::max<long long>(total, 1), /*for_result=*/false);
+  if (!host) return set_error(CCO_E_OOM, "pinned host allocation failed");
+  const int st = [&]() -> int {
+    if (total > 0) CK(cudaMemcpyAsync(host, d_out, (size_t)total, cudaMemcpyDeviceToHost, s));
+    if (also) CKR(also());
+    CK(cudaStreamSynchronize(s));
+    CK(cudaGetLastError());
+    return CCO_OK;
+  }();
+  if (st != CCO_OK) {
+    owner->pinned_put(host);
+    return st;
+  }
+  *out_bytes = host;
+  *out_len = total;
+  return CCO_OK;
+}
+
 // cco_format_es_bulk == format_model without properties and rankings: one set of document kernels
 static int format_model(cco_ctx_t *ctx, const cco_result_t *res, int32_t n_names, const char *const *names, const cco_dictionary_t *row_ids,
                         const cco_dictionary_t *col_ids, const cco_item_properties_t *props, int32_t n_rank, const cco_ranking_t *rk,
@@ -3082,8 +3120,7 @@ static int format_model(cco_ctx_t *ctx, const cco_result_t *res, int32_t n_names
   CK(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   Arena ar(s);
-  nvtx_push(range);
-  struct Pop { ~Pop() { nvtx_pop(); } } pop;
+  NvtxRange nvtx(range);
   FormatArgs fa;
   memset(&fa, 0, sizeof fa);
   fa.n_rows = (int32_t)(row_hi - row_lo);
@@ -3131,14 +3168,7 @@ static int format_model(cco_ctx_t *ctx, const cco_result_t *res, int32_t n_names
     k_doc_write<<<grid_for((long long)n_docs * 32, 256, c->sm_count), 256, 0, s>>>(fa, n_docs, doc_off, d_out);
     c->launches++;
   }
-  char *host = (char *)ctx->pinned_get((size_t)std::max<long long>(total, 1), /*for_result=*/false);
-  if (!host) return set_error(CCO_E_OOM, "pinned host allocation failed");
-  if (total > 0) CK(cudaMemcpyAsync(host, d_out, (size_t)total, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  CK(cudaGetLastError());
-  *out_bytes = host;
-  *out_len = total;
-  return CCO_OK;
+  return body_to_host(ctx, s, d_out, total, out_bytes, out_len);
 }
 
 // ---- cco_rerank_model: an existing index with fresh rankings and properties (calcPop), kernels in cco_json.cuh ---------
@@ -3313,6 +3343,24 @@ static int bulk_parse(cco_ctx *c, Arena &ar, const char *body, int64_t body_len,
   if (h_err != ~0ULL) return json_error(h_err, false);
   return json_decode(c, ar, D, id_span, bb, &bd->ids, &bd->ids_bytes);
 }
+// the decoded member names of a body against a small host table of names: *ngid = each member's name group, *entry_of =
+// each group's table entry (-1: not in the table)
+static int member_entries(cco_ctx *c, Arena &ar, const DevStrCol &names, const std::vector<std::string> &entries, int32_t **ngid,
+                          int32_t **entry_of) {
+  DevDict traw;
+  CKR(upload_strings(c, ar, entries, &traw));
+  str_hash(c, names, ~0ULL);
+  CKR(ar.alloc(ngid, std::max<long long>(names.n, 1)));
+  StrTable nt;
+  CKR(str_group(c, ar, names, nullptr, false, 0, &nt, *ngid));
+  CKR(ar.alloc(entry_of, std::max<long long>(nt.n_groups, 1)));
+  if (nt.n_groups > 0) {
+    k_name_entry<<<grid_for(nt.n_groups, 256, c->sm_count), 256, 0, c->stream>>>(nt.n_groups, nt.first_sorted, names.off, (const unsigned char *)names.w,
+                                                                                (int)entries.size(), traw.off, traw.bytes, *entry_of);
+    c->launches++;
+  }
+  return CCO_OK;
+}
 
 static int rerank_model(cco_ctx_t *ctx, const char *body, int64_t body_len, const cco_item_properties_t *props, int32_t n_rank,
                         const cco_ranking_t *rk, char **out_bytes, int64_t *out_len, Streams st = {}, const DevProps *dp = nullptr) {
@@ -3328,8 +3376,7 @@ static int rerank_model(cco_ctx_t *ctx, const char *body, int64_t body_len, cons
   CK(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   Arena ar(s);
-  nvtx_push("cco:rerank_model");
-  struct Pop { ~Pop() { nvtx_pop(); } } pop;
+  NvtxRange nvtx("cco:rerank_model");
   mail_reset(c);
   // 1-4. the documents: members, decoded names and _ids
   BulkDocs bd;
@@ -3350,12 +3397,7 @@ static int rerank_model(cco_ctx_t *ctx, const char *body, int64_t body_len, cons
   fa.n_rows = (int32_t)D;
   const DevDict raw_ids = {ids.off, (const unsigned char *)ids.w, D};
   CKR(escape_dict(c, ar, raw_ids, &fa.row_ids));
-  KeySection rows;
-  rows.n = D;
-  rows.off = (const int64_t *)ids.off;
-  rows.bytes = (const char *)ids.w;
-  rows.device = true;
-  rows.nbytes = ids_bytes;
+  const KeySection rows{D, (const int64_t *)ids.off, (const char *)ids.w, true, ids_bytes};
   CKR(model_fields(c, ar, &fa, rows, props, n_rank, rk, st, true, true, dp));
   // 6. member names -> the distinct names of the fields, the rankings and "id"
   if (D > 0) {
@@ -3375,38 +3417,19 @@ static int rerank_model(cco_ctx_t *ctx, const char *body, int64_t body_len, cons
     for (int k = 0; k < n_rank; ++k) ent_rank[entry(rk[k].name)] |= (uint8_t)(1u << k);
     ent_id[entry("id")] = 1;
     const int T = (int)ent.size();
-    std::vector<int64_t> toff(T + 1, 0);
-    std::string tblob;
-    for (int t = 0; t < T; ++t) {
-      tblob += ent[t];
-      toff[t + 1] = (int64_t)tblob.size();
-    }
-    const cco_dictionary_t td = {T, toff.data(), tblob.data()};
-    DevDict traw;
-    int32_t *d_field;
-    uint8_t *d_rank, *d_id;
-    CKR(upload_dict(c, ar, td, &traw));
+    int32_t *d_field, *ngid, *entry_of, *ment;
+    uint8_t *d_rank, *d_id, *mkeep;
     CKR(ar.alloc(&d_field, T));
     CKR(ar.alloc(&d_rank, T));
     CKR(ar.alloc(&d_id, T));
     CK(cudaMemcpyAsync(d_field, ent_field.data(), sizeof(int32_t) * T, cudaMemcpyHostToDevice, s));
     CK(cudaMemcpyAsync(d_rank, ent_rank.data(), T, cudaMemcpyHostToDevice, s));
     CK(cudaMemcpyAsync(d_id, ent_id.data(), T, cudaMemcpyHostToDevice, s));
-    CK(cudaStreamSynchronize(s));   // the table is local
-    str_hash(c, names, ~0ULL);
-    int32_t *ngid, *entry_of, *ment;
-    uint8_t *mkeep;
-    CKR(ar.alloc(&ngid, std::max<long long>(M1, 1)));
-    StrTable nt;
-    CKR(str_group(c, ar, names, nullptr, false, 0, &nt, ngid));
-    CKR(ar.alloc(&entry_of, std::max<long long>(nt.n_groups, 1)));
+    CKR(member_entries(c, ar, names, ent, &ngid, &entry_of));   // its wait for the upload also covers these local tables
     CKR(ar.alloc(&ment, std::max<long long>(M1, 1)));
     CKR(ar.alloc(&mkeep, std::max<long long>(M1, 1)));
-    if (nt.n_groups > 0)
-      k_name_entry<<<grid_for(nt.n_groups, 256, c->sm_count), 256, 0, s>>>(nt.n_groups, nt.first_sorted, names.off,
-                                                                           (const unsigned char *)names.w, T, traw.off, traw.bytes, entry_of);
     k_member_info<<<grid_for(D * 32, 256, c->sm_count), 256, 0, s>>>(D, ra.line_moff, ngid, entry_of, d_id, ment, mkeep);
-    c->launches += 2;
+    c->launches++;
     ra.ment = ment;
     ra.mkeep = mkeep;
     ra.ent_field = d_field;
@@ -3442,14 +3465,7 @@ static int rerank_model(cco_ctx_t *ctx, const char *body, int64_t body_len, cons
     k_doc_write<<<grid_for(X * 32, 256, c->sm_count), 256, 0, s>>>(fx, (int32_t)X, doc_off + D, d_out);
     c->launches++;
   }
-  char *host = (char *)ctx->pinned_get((size_t)std::max<long long>(total, 1), /*for_result=*/false);
-  if (!host) return set_error(CCO_E_OOM, "pinned host allocation failed");
-  if (total > 0) CK(cudaMemcpyAsync(host, d_out, (size_t)total, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  CK(cudaGetLastError());
-  *out_bytes = host;
-  *out_len = total;
-  return CCO_OK;
+  return body_to_host(c, s, d_out, total, out_bytes, out_len);
 }
 }  // namespace cco
 
@@ -4460,8 +4476,7 @@ static int event_log_begin(cco_ctx *c, int64_t chunk_bytes, cco_event_log **out)
 static int event_log_append(cco_event_log *lg, const char *bytes, int64_t len) {
   cco_ctx *c = lg->ctx;
   CK(cudaSetDevice(c->device));
-  nvtx_push("cco:event_log_append");
-  struct Pop { ~Pop() { nvtx_pop(); } } pop;
+  NvtxRange nvtx("cco:event_log_append");
   while (len > 0) {
     if (lg->staged == lg->cap) CKR(event_flush(lg));
     const long long take = std::min<long long>(len, lg->cap - lg->staged);
@@ -4483,8 +4498,7 @@ static int event_log_finish(cco_event_log *lg) {
   cco_ctx *c = lg->ctx;
   cudaStream_t s = c->stream;
   CK(cudaSetDevice(c->device));
-  nvtx_push("cco:event_log_finish");
-  struct Pop { ~Pop() { nvtx_pop(); } } pop;
+  NvtxRange nvtx("cco:event_log_finish");
   if (lg->staged > 0) CKR(event_chunk(lg, lg->staged, lg->last_nl != lg->staged - 1));
   log_drop(lg, lg->stage);
   lg->stage = nullptr;
@@ -4651,8 +4665,7 @@ int cco_event_log_read(cco_ctx_t *ctx, const char *bytes, int64_t len, cco_event
   if (!ctx || !out || len < 0 || (len > 0 && !bytes)) return set_error(CCO_E_INVALID_ARG, "null argument or negative length");
   *out = nullptr;
   if (!ctx->members.empty()) return set_error(CCO_E_UNSUPPORTED, "an event log is resident on one GPU: read it on a per-GPU context");
-  nvtx_push("cco:event_log_read");
-  struct Pop { ~Pop() { nvtx_pop(); } } pop;
+  NvtxRange nvtx("cco:event_log_read");
   cco_event_log *lg = nullptr;
   CKR(event_log_begin(ctx, std::max<int64_t>(len, 1), &lg));
   int rc = event_log_append(lg, bytes, len);
@@ -4782,6 +4795,61 @@ static std::string uq_quote(const char *s) {
   return o + "\"";
 }
 
+// the text every query template starts with (up to the should clauses), and the one after the must_not ids
+static std::string query_head(const char *header, const char *head) {
+  return std::string(header) + "\n" + head + ",\"query\":{\"bool\":{\"should\":[";
+}
+static std::string query_tail(const char *must_not, const char *sort) {
+  return std::string("],\"boost\":0}}") + (*must_not ? std::string(",") + must_not : std::string()) +
+         "],\"minimum_should_match\":1}},\"sort\":" + sort + "}\n";
+}
+
+// The R records of a query builder, one warp each: the length pass, the record offsets (each record < 2^31 bytes) on the
+// host, the write pass and the body on the host; `also` as in body_to_host.  On failure every pinned buffer taken here is
+// given back.
+extern "C++" {
+template <class Args>
+static int emit_records(cco_ctx *c, Arena &ar, long long R, void (*len_pass)(Args, const long long *, long long *, unsigned char *),
+                        void (*write_pass)(Args, const long long *, long long *, unsigned char *), const Args &a, char **out_body,
+                        int64_t *out_len, int64_t **out_offsets, int64_t *out_n, const std::function<int()> &also = nullptr) {
+  cudaStream_t s = c->stream;
+  const int grid = grid_for(R * 32, 256, c->sm_count);
+  long long *rlen, *roff;
+  CKR(ar.alloc(&rlen, R + 1));
+  CKR(ar.alloc(&roff, R + 1));
+  CK(cudaMemsetAsync(rlen + R, 0, 8, s));
+  if (R > 0) {
+    len_pass<<<grid, 256, 0, s>>>(a, nullptr, rlen, nullptr);
+    c->launches++;
+  }
+  CKR(exclusive_sum(c, ar, rlen, roff, R + 1));
+  int64_t *ho = (int64_t *)c->pinned_get(sizeof(int64_t) * ((size_t)R + 1), /*for_result=*/false);
+  if (!ho) return set_error(CCO_E_OOM, "pinned host allocation failed");
+  const int st = [&]() -> int {
+    CK(cudaMemcpyAsync(ho, roff, sizeof(int64_t) * ((size_t)R + 1), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    for (long long r = 0; r < R; ++r)
+      if (ho[r + 1] - ho[r] >= (1LL << 31))
+        return set_error(CCO_E_UNSUPPORTED, "record %lld has %lld bytes, at most 2^31 - 1", r, (long long)(ho[r + 1] - ho[r]));
+    const long long total = ho[R];
+    unsigned char *d_out;
+    CKR(ar.alloc(&d_out, std::max<long long>(total, 1)));
+    if (R > 0 && total > 0) {
+      write_pass<<<grid, 256, 0, s>>>(a, roff, nullptr, d_out);
+      c->launches++;
+    }
+    return body_to_host(c, s, d_out, total, out_body, out_len, also);
+  }();
+  if (st != CCO_OK) {
+    c->pinned_put(ho);
+    return st;
+  }
+  *out_offsets = ho;
+  *out_n = R;
+  return CCO_OK;
+}
+}  // extern "C++"
+
 // the record template: n_history_names + 2 pieces around the history lists and the blacklist (see include/cco_b200.h)
 static std::vector<std::string> uq_template(const cco_user_query_t *q) {
   std::vector<std::string> t(1);
@@ -4802,14 +4870,12 @@ static std::vector<std::string> uq_template(const cco_user_query_t *q) {
       t.back() += rest;
     }
   };
-  t.back() += std::string(q->header) + "\n" + q->head + ",\"query\":{\"bool\":{\"should\":[";
+  t.back() += query_head(q->header, q->head);
   clause(q->should, !q->history_in_must);
   t.back() += "],\"must\":[";
   clause(q->must, q->history_in_must != 0);
   t.back() += "],\"must_not\":[{\"ids\":{\"values\":[";
-  t.emplace_back("],\"boost\":0}}");
-  if (*q->must_not) t.back() += std::string(",") + q->must_not;
-  t.back() += std::string("],\"minimum_should_match\":1}},\"sort\":") + q->sort + "}\n";
+  t.push_back(query_tail(q->must_not, q->sort));
   return t;
 }
 
@@ -4851,8 +4917,7 @@ static int user_queries(cco_ctx *c, const cco_event_log *lg, const cco_user_quer
   CK(cudaSetDevice(c->device));
   mail_reset(c);
   Arena ar(s);
-  nvtx_push("cco:user_queries");
-  struct Pop { ~Pop() { nvtx_pop(); } } pop;
+  NvtxRange nvtx("cco:user_queries");
   // 1. the caller's columns, checked on the device before any kernel reads bytes through their offsets
   DevStrCol lc, uc;
   CKR(str_upload(c, ar, q->n_blacklist_items, q->blacklist_item_offsets, q->blacklist_item_bytes, &lc));
@@ -5073,19 +5138,8 @@ static int user_queries(cco_ctx *c, const cco_event_log *lg, const cco_user_quer
     }
   }
   // 11. the template, then a length pass, the record offsets and a write pass: one warp per record
-  const std::vector<std::string> tp = uq_template(q);
-  std::vector<long long> toff(tp.size() + 1, 0);
-  std::string tb;
-  for (size_t j = 0; j < tp.size(); ++j) {
-    tb += tp[j];
-    toff[j + 1] = (long long)tb.size();
-  }
-  long long *d_toff;
-  unsigned char *d_tb;
-  CKR(ar.alloc(&d_toff, (long long)toff.size()));
-  CKR(ar.alloc(&d_tb, std::max<long long>((long long)tb.size(), 1)));
-  CK(cudaMemcpyAsync(d_toff, toff.data(), sizeof(long long) * toff.size(), cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(d_tb, tb.data(), tb.size(), cudaMemcpyHostToDevice, s));
+  DevDict tp;
+  CKR(upload_strings(c, ar, uq_template(q), &tp));
   UqArgs a;
   a.n_rec = R;
   a.rec_uid = rec_uid;
@@ -5109,43 +5163,9 @@ static int user_queries(cco_ctx *c, const cco_event_log *lg, const cco_user_quer
   a.lbytes = (const unsigned char *)lc.w;
   a.lgid = lgid;
   a.keep_l = keep_l;
-  a.toff = d_toff;
-  a.tbytes = d_tb;
-  long long *rlen, *roff;
-  CKR(ar.alloc(&rlen, R + 1));
-  CKR(ar.alloc(&roff, R + 1));
-  CK(cudaMemsetAsync(rlen + R, 0, 8, s));
-  if (R > 0) {
-    k_uq_record<false><<<grid_for(R * 32, 256, c->sm_count), 256, 0, s>>>(a, nullptr, rlen, nullptr);
-    c->launches++;
-  }
-  CKR(exclusive_sum(c, ar, rlen, roff, R + 1));
-  int64_t *ho = (int64_t *)c->pinned_get(sizeof(int64_t) * ((size_t)R + 1), /*for_result=*/false);
-  if (!ho) return set_error(CCO_E_OOM, "pinned host allocation failed");
-  CK(cudaMemcpyAsync(ho, roff, sizeof(int64_t) * ((size_t)R + 1), cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  for (long long r = 0; r < R; ++r)
-    if (ho[r + 1] - ho[r] >= (1LL << 31)) {
-      c->pinned_put(ho);
-      return set_error(CCO_E_UNSUPPORTED, "record %lld has %lld bytes, at most 2^31 - 1", r, (long long)(ho[r + 1] - ho[r]));
-    }
-  const long long total = ho[R];
-  unsigned char *d_out;
-  CKR(ar.alloc(&d_out, std::max<long long>(total, 1)));
-  if (R > 0 && total > 0) {
-    k_uq_record<true><<<grid_for(R * 32, 256, c->sm_count), 256, 0, s>>>(a, roff, nullptr, d_out);
-    c->launches++;
-  }
-  char *host = (char *)c->pinned_get((size_t)std::max<long long>(total, 1), /*for_result=*/false);
-  if (!host) return set_error(CCO_E_OOM, "pinned host allocation failed");
-  if (total > 0) CK(cudaMemcpyAsync(host, d_out, (size_t)total, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  CK(cudaGetLastError());
-  *out_body = host;
-  *out_len = total;
-  *out_offsets = ho;
-  *out_n = R;
-  return CCO_OK;
+  a.toff = tp.off;
+  a.tbytes = tp.bytes;
+  return emit_records(c, ar, R, k_uq_record<false>, k_uq_record<true>, a, out_body, out_len, out_offsets, out_n);
 }
 }  // namespace cco
 
@@ -5174,15 +5194,14 @@ namespace cco {
 // 9 + j the start of model name j's clause (see include/cco_b200.h)
 static std::vector<std::string> iq_template(const cco_item_query_t *q) {
   std::vector<std::string> t(9 + q->n_names);
-  t[0] = std::string(q->header) + "\n" + q->head + ",\"query\":{\"bool\":{\"should\":[";
+  t[0] = query_head(q->header, q->head);
   t[1] = q->should_head;
   t[2] = q->should;
   t[3] = "],\"must\":[";
   t[4] = q->must_head;
   t[5] = q->must;
   t[6] = "],\"must_not\":[{\"ids\":{\"values\":[";
-  t[7] = std::string("],\"boost\":0}}") + (*q->must_not ? std::string(",") + q->must_not : std::string()) +
-         "],\"minimum_should_match\":1}},\"sort\":" + q->sort + "}\n";
+  t[7] = query_tail(q->must_not, q->sort);
   t[8] = q->similar_in_must ? "],\"boost\":0}}" : q->similar_boost ? std::string("],\"boost\":") + q->similar_boost + "}}" : "]}}";
   for (int j = 0; j < q->n_names; ++j) t[9 + j] = "{\"terms\":{" + uq_quote(q->names[j]) + ":[";
   return t;
@@ -5210,8 +5229,7 @@ static int item_queries(cco_ctx *c, const char *body, int64_t body_len, const cc
   cudaStream_t s = c->stream;
   CK(cudaSetDevice(c->device));
   Arena ar(s);
-  nvtx_push("cco:item_queries");
-  struct Pop { ~Pop() { nvtx_pop(); } } pop;
+  NvtxRange nvtx("cco:item_queries");
   mail_reset(c);
   const bool all = ioff == nullptr;
   const long long NI = all ? 0 : n_items, NL = q->n_blacklist_items;
@@ -5221,50 +5239,19 @@ static int item_queries(cco_ctx *c, const char *body, int64_t body_len, const cc
   const long long D = bd.D, R = all ? D : NI;
   // 5. one key column: the decoded _ids, the items, blacklistItems; the caller's offsets are checked on the device before
   //    any kernel reads bytes through them
-  const long long NK = D + NI + NL;
-  const long long nb = bd.ids_bytes + (NI > 0 ? ioff[NI] - ioff[0] : 0) +
-                       (NL > 0 ? q->blacklist_item_offsets[NL] - q->blacklist_item_offsets[0] : 0);
-  DevStrCol key;
-  key.n = NK;
-  key.base = 0;
-  CKR(ar.alloc(&key.off, NK + 1));
-  CKR(ar.alloc(&key.w, (nb + 16 + 7) / 8));
-  CKR(ar.alloc(&key.hash, std::max<long long>(NK, 1)));
-  CK(cudaMemsetAsync(key.off, 0, 8, s));
   int *bad, h_bad = 0;
   CKR(ar.alloc(&bad, 1));
   CK(cudaMemsetAsync(bad, 0, sizeof(int), s));
-  long long at = 0, byte_at = 0;
-  if (D > 0) {
-    k_rebase<<<grid_for(D + 1, 256, c->sm_count), 256, 0, s>>>(D + 1, bd.ids.off, 0, key.off);
-    c->launches++;
-    if (bd.ids_bytes > 0) CK(cudaMemcpyAsync(key.w, bd.ids.w, (size_t)bd.ids_bytes, cudaMemcpyDeviceToDevice, s));
-    at = D;
-    byte_at = bd.ids_bytes;
-  }
-  for (int k = 0; k < 2; ++k) {
-    const long long n = k ? NL : NI;
-    const int64_t *off = k ? q->blacklist_item_offsets : ioff;
-    const char *bytes = k ? q->blacklist_item_bytes : ibytes;
-    if (n == 0) continue;
-    long long *tmp;
-    CKR(ar.alloc(&tmp, n + 1));
-    CK(cudaMemcpyAsync(tmp, off, sizeof(int64_t) * ((size_t)n + 1), cudaMemcpyHostToDevice, s));
-    k_str_check<<<grid_for(n, 256, c->sm_count), 256, 0, s>>>(n, tmp, bad);
-    k_rebase<<<grid_for(n + 1, 256, c->sm_count), 256, 0, s>>>(n + 1, tmp, byte_at - off[0], key.off + at);
-    c->launches += 2;
-    const long long kb = off[n] - off[0];
-    if (kb > 0) CK(cudaMemcpyAsync((char *)key.w + byte_at, bytes + off[0], (size_t)kb, cudaMemcpyHostToDevice, s));
-    at += n;
-    byte_at += kb;
-  }
+  DevStrCol key;
+  CKR(key_column(c, ar, {KeySection{D, (const int64_t *)bd.ids.off, (const char *)bd.ids.w, true, bd.ids_bytes}, KeySection{NI, ioff, ibytes},
+                         KeySection{NL, q->blacklist_item_offsets, q->blacklist_item_bytes}}, bad, &key));
   CKR(mail_fetch(c, &h_bad, bad, 4));
   CKR(mail_wait(c));
   if (h_bad) return set_error(CCO_E_INVALID_ARG, "decreasing offsets in the items or the blacklist items");
   // 6. one exact grouping over the key column; a group that holds two documents is a repeated _id
   str_hash(c, key, ~0ULL);
   int32_t *gid;
-  CKR(ar.alloc(&gid, std::max<long long>(NK, 1)));
+  CKR(ar.alloc(&gid, std::max<long long>(key.n, 1)));
   StrTable tb;
   CKR(str_group(c, ar, key, nullptr, false, 0, &tb, gid));
   if (D > 0) {
@@ -5314,28 +5301,11 @@ static int item_queries(cco_ctx *c, const char *body, int64_t body_len, const cc
   CK(cudaMemsetAsync(eoff, 0, sizeof(long long) * (size_t)(DT + 1), s));
   DevStrCol dec;
   if (D > 0) {
-    std::vector<int64_t> toff(T + 1, 0);
-    std::string tblob;
-    for (int t = 0; t < T; ++t) {
-      tblob += ent[t];
-      toff[t + 1] = (int64_t)tblob.size();
-    }
-    const cco_dictionary_t td = {T, toff.data(), tblob.data()};
-    DevDict traw;
-    CKR(upload_dict(c, ar, td, &traw));
-    CK(cudaStreamSynchronize(s));   // the table is local
-    str_hash(c, bd.names, ~0ULL);
     int32_t *ngid, *entry_of, *pick;
-    CKR(ar.alloc(&ngid, std::max<long long>(bd.M1, 1)));
-    StrTable nt;
-    CKR(str_group(c, ar, bd.names, nullptr, false, 0, &nt, ngid));
-    CKR(ar.alloc(&entry_of, std::max<long long>(nt.n_groups, 1)));
+    CKR(member_entries(c, ar, bd.names, ent, &ngid, &entry_of));
     CKR(ar.alloc(&pick, DT));
-    if (nt.n_groups > 0)
-      k_name_entry<<<grid_for(nt.n_groups, 256, c->sm_count), 256, 0, s>>>(nt.n_groups, nt.first_sorted, bd.names.off,
-                                                                           (const unsigned char *)bd.names.w, T, traw.off, traw.bytes, entry_of);
     k_iq_pick<<<grid_for(D, 256, c->sm_count), 256, 0, s>>>(D, T, bd.line_moff, ngid, entry_of, pick);
-    c->launches += 2;
+    c->launches++;
     // 10. the queried documents' picked values: the verdict comes before anything reads through the element spans
     long long *cnt, NE = 0;
     unsigned long long *err, h_err = ~0ULL;
@@ -5363,22 +5333,11 @@ static int item_queries(cco_ctx *c, const char *body, int64_t body_len, const cc
     CKR(json_decode(c, ar, NE, elem, bd.body, &dec, &dec_bytes));
   }
   // 11. the template, then a length pass, the record offsets and a write pass: one warp per record
-  const std::vector<std::string> tp = iq_template(q);
-  std::vector<long long> toff(tp.size() + 1, 0);
-  std::string tbl;
-  for (size_t j = 0; j < tp.size(); ++j) {
-    tbl += tp[j];
-    toff[j + 1] = (long long)tbl.size();
-  }
-  long long *d_toff;
-  unsigned char *d_tb;
   int32_t *d_entry;
-  CKR(ar.alloc(&d_toff, (long long)toff.size()));
-  CKR(ar.alloc(&d_tb, std::max<long long>((long long)tbl.size(), 1)));
   CKR(ar.alloc(&d_entry, q->n_names));
-  CK(cudaMemcpyAsync(d_toff, toff.data(), sizeof(long long) * toff.size(), cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(d_tb, tbl.data(), tbl.size(), cudaMemcpyHostToDevice, s));
   CK(cudaMemcpyAsync(d_entry, name_entry.data(), sizeof(int32_t) * (size_t)q->n_names, cudaMemcpyHostToDevice, s));
+  DevDict tp;
+  CKR(upload_strings(c, ar, iq_template(q), &tp));
   IqArgs a;
   a.n_rec = R;
   a.rec_doc = rec_doc;
@@ -5399,37 +5358,11 @@ static int item_queries(cco_ctx *c, const char *body, int64_t body_len, const cc
   a.n_list = NL;
   a.list_at = D + NI;
   a.first_in_list = first_in_list;
-  a.toff = d_toff;
-  a.tbytes = d_tb;
-  long long *rlen, *roff;
-  CKR(ar.alloc(&rlen, R + 1));
-  CKR(ar.alloc(&roff, R + 1));
-  CK(cudaMemsetAsync(rlen + R, 0, 8, s));
-  if (R > 0) {
-    k_iq_record<false><<<grid_for(R * 32, 256, c->sm_count), 256, 0, s>>>(a, nullptr, rlen, nullptr);
-    c->launches++;
-  }
-  CKR(exclusive_sum(c, ar, rlen, roff, R + 1));
-  int64_t *ho = (int64_t *)c->pinned_get(sizeof(int64_t) * ((size_t)R + 1), /*for_result=*/false);
-  if (!ho) return set_error(CCO_E_OOM, "pinned host allocation failed");
-  CK(cudaMemcpyAsync(ho, roff, sizeof(int64_t) * ((size_t)R + 1), cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  for (long long r = 0; r < R; ++r)
-    if (ho[r + 1] - ho[r] >= (1LL << 31)) {
-      c->pinned_put(ho);
-      return set_error(CCO_E_UNSUPPORTED, "record %lld has %lld bytes, at most 2^31 - 1", r, (long long)(ho[r + 1] - ho[r]));
-    }
-  const long long total = ho[R];
-  unsigned char *d_out;
-  CKR(ar.alloc(&d_out, std::max<long long>(total, 1)));
-  if (R > 0 && total > 0) {
-    k_iq_record<true><<<grid_for(R * 32, 256, c->sm_count), 256, 0, s>>>(a, roff, nullptr, d_out);
-    c->launches++;
-  }
-  char *host = (char *)c->pinned_get((size_t)std::max<long long>(total, 1), /*for_result=*/false);
-  if (!host) return set_error(CCO_E_OOM, "pinned host allocation failed");
-  if (total > 0) CK(cudaMemcpyAsync(host, d_out, (size_t)total, cudaMemcpyDeviceToHost, s));
-  if (all && out_items) {   // the documents' decoded _ids, in body order
+  a.toff = tp.off;
+  a.tbytes = tp.bytes;
+  return emit_records(c, ar, R, k_iq_record<false>, k_iq_record<true>, a, out_body, out_len, out_offsets, out_n, [&]() -> int {
+    if (!all || !out_items) return CCO_OK;
+    // the documents' decoded _ids, in body order
     int64_t *io = (int64_t *)c->pinned_get(sizeof(int64_t) * ((size_t)D + 1), /*for_result=*/false);
     char *ib = (char *)c->pinned_get((size_t)std::max<long long>(bd.ids_bytes, 1), /*for_result=*/false);
     if (!io || !ib) return set_error(CCO_E_OOM, "pinned host allocation failed");
@@ -5437,14 +5370,8 @@ static int item_queries(cco_ctx *c, const char *body, int64_t body_len, const cc
     if (D > 0) CK(cudaMemcpyAsync(io, bd.ids.off, sizeof(int64_t) * ((size_t)D + 1), cudaMemcpyDeviceToHost, s));
     if (bd.ids_bytes > 0) CK(cudaMemcpyAsync(ib, bd.ids.w, (size_t)bd.ids_bytes, cudaMemcpyDeviceToHost, s));
     *out_items = cco_dictionary_t{D, io, ib};
-  }
-  CK(cudaStreamSynchronize(s));
-  CK(cudaGetLastError());
-  *out_body = host;
-  *out_len = total;
-  *out_offsets = ho;
-  *out_n = R;
-  return CCO_OK;
+    return CCO_OK;
+  });
 }
 }  // namespace cco
 
@@ -5465,7 +5392,7 @@ namespace cco {
 // 3 its end, 4 should_tail, 5 must up to the ids clause's values, 6 the rest of the record (see include/cco_b200.h)
 static std::vector<std::string> is_template(const cco_item_set_query_t *q) {
   std::vector<std::string> t(7);
-  t[0] = std::string(q->header) + "\n" + q->head + ",\"query\":{\"bool\":{\"should\":[";
+  t[0] = query_head(q->header, q->head);
   t[1] = q->should_head;
   if (q->with_set) {
     t[2] = "{\"terms\":{" + uq_quote(q->name) + ":[";
@@ -5473,8 +5400,7 @@ static std::vector<std::string> is_template(const cco_item_set_query_t *q) {
   }
   t[4] = q->should_tail;
   t[5] = std::string("],\"must\":[") + q->must + "],\"must_not\":[{\"ids\":{\"values\":[";
-  t[6] = std::string("],\"boost\":0}}") + (*q->must_not ? std::string(",") + q->must_not : std::string()) +
-         "],\"minimum_should_match\":1}},\"sort\":" + q->sort + "}\n";
+  t[6] = query_tail(q->must_not, q->sort);
   return t;
 }
 
@@ -5503,21 +5429,11 @@ static int item_set_queries(cco_ctx *c, const cco_item_set_query_t *q, long long
   cudaStream_t s = c->stream;
   CK(cudaSetDevice(c->device));
   Arena ar(s);
-  nvtx_push("cco:item_set_queries");
-  struct Pop { ~Pop() { nvtx_pop(); } } pop;
+  NvtxRange nvtx("cco:item_set_queries");
   mail_reset(c);
   const long long S = n_sets, s0 = set_off[0], NE = set_off[S] - s0, NL = q->n_blacklist_items;
   // 1. one key column: blacklistItems, then the sets' elements; the set offsets 0-based.  Every column's offsets are
   //    checked on the device before any kernel reads bytes through them
-  const long long NK = NL + NE;
-  const long long nb = (NL > 0 ? q->blacklist_item_offsets[NL] - q->blacklist_item_offsets[0] : 0) + (NE > 0 ? eoff[s0 + NE] - eoff[s0] : 0);
-  DevStrCol key;
-  key.n = NK;
-  key.base = 0;
-  CKR(ar.alloc(&key.off, NK + 1));
-  CKR(ar.alloc(&key.w, (nb + 16 + 7) / 8));
-  CKR(ar.alloc(&key.hash, std::max<long long>(NK, 1)));
-  CK(cudaMemsetAsync(key.off, 0, 8, s));
   int *bad, h_bad = 0;
   CKR(ar.alloc(&bad, 1));
   CK(cudaMemsetAsync(bad, 0, sizeof(int), s));
@@ -5531,30 +5447,15 @@ static int item_set_queries(cco_ctx *c, const cco_item_set_query_t *q, long long
   }
   k_rebase<<<grid_for(S + 1, 256, c->sm_count), 256, 0, s>>>(S + 1, stmp, -s0, soff);
   c->launches++;
-  long long at = 0, byte_at = 0;
-  for (int k = 0; k < 2; ++k) {
-    const long long n = k ? NE : NL;
-    const int64_t *off = k ? eoff + s0 : q->blacklist_item_offsets;
-    const char *bytes = k ? ebytes : q->blacklist_item_bytes;
-    if (n == 0) continue;
-    long long *tmp;
-    CKR(ar.alloc(&tmp, n + 1));
-    CK(cudaMemcpyAsync(tmp, off, sizeof(int64_t) * ((size_t)n + 1), cudaMemcpyHostToDevice, s));
-    k_str_check<<<grid_for(n, 256, c->sm_count), 256, 0, s>>>(n, tmp, bad);
-    k_rebase<<<grid_for(n + 1, 256, c->sm_count), 256, 0, s>>>(n + 1, tmp, byte_at - off[0], key.off + at);
-    c->launches += 2;
-    const long long kb = off[n] - off[0];
-    if (kb > 0) CK(cudaMemcpyAsync((char *)key.w + byte_at, bytes + off[0], (size_t)kb, cudaMemcpyHostToDevice, s));
-    at += n;
-    byte_at += kb;
-  }
+  DevStrCol key;
+  CKR(key_column(c, ar, {KeySection{NL, q->blacklist_item_offsets, q->blacklist_item_bytes}, KeySection{NE, eoff + s0, ebytes}}, bad, &key));
   CKR(mail_fetch(c, &h_bad, bad, 4));
   CKR(mail_wait(c));
   if (h_bad) return set_error(CCO_E_INVALID_ARG, "decreasing offsets in the sets, the elements or the blacklist items");
   // 2. one exact grouping over the key column; blacklistItems: each group's first list index (membership is a group test)
   str_hash(c, key, ~0ULL);
   int32_t *gid;
-  CKR(ar.alloc(&gid, std::max<long long>(NK, 1)));
+  CKR(ar.alloc(&gid, std::max<long long>(key.n, 1)));
   StrTable tb;
   CKR(str_group(c, ar, key, nullptr, false, 0, &tb, gid));
   const long long G = tb.n_groups;
@@ -5583,19 +5484,8 @@ static int item_set_queries(cco_ctx *c, const cco_item_set_query_t *q, long long
     ar.release(p2);
   }
   // 4. the template, then a length pass, the record offsets and a write pass: one warp per set
-  const std::vector<std::string> tp = is_template(q);
-  std::vector<long long> toff(tp.size() + 1, 0);
-  std::string tbl;
-  for (size_t j = 0; j < tp.size(); ++j) {
-    tbl += tp[j];
-    toff[j + 1] = (long long)tbl.size();
-  }
-  long long *d_toff;
-  unsigned char *d_tb;
-  CKR(ar.alloc(&d_toff, (long long)toff.size()));
-  CKR(ar.alloc(&d_tb, std::max<long long>((long long)tbl.size(), 1)));
-  CK(cudaMemcpyAsync(d_toff, toff.data(), sizeof(long long) * toff.size(), cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(d_tb, tbl.data(), tbl.size(), cudaMemcpyHostToDevice, s));
+  DevDict tp;
+  CKR(upload_strings(c, ar, is_template(q), &tp));
   IsArgs a;
   a.n_sets = S;
   a.soff = soff;
@@ -5606,43 +5496,9 @@ static int item_set_queries(cco_ctx *c, const cco_item_set_query_t *q, long long
   a.first_in_list = first_in_list;
   a.first_in_set = first_in_set;
   a.with_set = q->with_set;
-  a.toff = d_toff;
-  a.tbytes = d_tb;
-  long long *rlen, *roff;
-  CKR(ar.alloc(&rlen, S + 1));
-  CKR(ar.alloc(&roff, S + 1));
-  CK(cudaMemsetAsync(rlen + S, 0, 8, s));
-  if (S > 0) {
-    k_is_record<false><<<grid_for(S * 32, 256, c->sm_count), 256, 0, s>>>(a, nullptr, rlen, nullptr);
-    c->launches++;
-  }
-  CKR(exclusive_sum(c, ar, rlen, roff, S + 1));
-  int64_t *ho = (int64_t *)c->pinned_get(sizeof(int64_t) * ((size_t)S + 1), /*for_result=*/false);
-  if (!ho) return set_error(CCO_E_OOM, "pinned host allocation failed");
-  CK(cudaMemcpyAsync(ho, roff, sizeof(int64_t) * ((size_t)S + 1), cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  for (long long r = 0; r < S; ++r)
-    if (ho[r + 1] - ho[r] >= (1LL << 31)) {
-      c->pinned_put(ho);
-      return set_error(CCO_E_UNSUPPORTED, "record %lld has %lld bytes, at most 2^31 - 1", r, (long long)(ho[r + 1] - ho[r]));
-    }
-  const long long total = ho[S];
-  unsigned char *d_out;
-  CKR(ar.alloc(&d_out, std::max<long long>(total, 1)));
-  if (S > 0 && total > 0) {
-    k_is_record<true><<<grid_for(S * 32, 256, c->sm_count), 256, 0, s>>>(a, roff, nullptr, d_out);
-    c->launches++;
-  }
-  char *host = (char *)c->pinned_get((size_t)std::max<long long>(total, 1), /*for_result=*/false);
-  if (!host) return set_error(CCO_E_OOM, "pinned host allocation failed");
-  if (total > 0) CK(cudaMemcpyAsync(host, d_out, (size_t)total, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  CK(cudaGetLastError());
-  *out_body = host;
-  *out_len = total;
-  *out_offsets = ho;
-  *out_n = S;
-  return CCO_OK;
+  a.toff = tp.off;
+  a.tbytes = tp.bytes;
+  return emit_records(c, ar, S, k_is_record<false>, k_is_record<true>, a, out_body, out_len, out_offsets, out_n);
 }
 }  // namespace cco
 
@@ -5672,8 +5528,7 @@ int cco_pop_model(cco_ctx_t *ctx, int32_t mode, int64_t n_events, const int32_t 
   CK(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   Arena ar(s);
-  nvtx_push("cco:pop_model");
-  struct Pop { ~Pop() { nvtx_pop(); } } pop;
+  NvtxRange nvtx("cco:pop_model");
   const PopArgs a = pop_args(mode, start_ms, end_ms, n_items);
   int32_t *d_item, *d_counts;
   long long *d_t;

@@ -212,36 +212,57 @@ __device__ __forceinline__ bool uq_has(const UqArgs &a, int32_t u, int32_t g) {
   return lo < a.bstart[u + 1] && a.bkey[lo] == x;
 }
 
-// one list of quoted, comma-separated ids from n candidates; get(i, &ptr, &len) == false skips candidate i.  cur and
-// first are warp-uniform.
-template <class Get>
-__device__ __forceinline__ void uq_list(long long n, const Get &get, unsigned char *o, long long &cur, bool &first) {
-  const int lane = threadIdx.x & 31;
-  for (long long b = 0; b < n; b += 32) {
-    const long long i = b + lane;
-    const unsigned char *p = nullptr;
-    long long len = 0;
-    const bool keep = i < n && get(i, &p, &len);
-    const unsigned ball = __ballot_sync(0xffffffffu, keep);
-    if (!ball) continue;
-    const bool lead = first && lane == __ffs(ball) - 1;
-    const long long el = keep ? uq_escape(p, len, nullptr) + 2 + (lead ? 0 : 1) : 0;
-    long long x = el;
-    for (int d = 1; d < 32; d <<= 1) {
-      const long long y = __shfl_up_sync(0xffffffffu, x, d);
-      if (lane >= d) x += y;
-    }
-    if (o && keep) {
-      unsigned char *q = o + cur + x - el;
-      if (!lead) *q++ = ',';
-      *q++ = '"';
-      q += uq_escape(p, len, q);
-      *q = '"';
-    }
-    cur += __shfl_sync(0xffffffffu, x, 31);
-    first = false;
+// One record of a query builder, written by one warp at o (the write pass) or only measured (o == nullptr): cur is the
+// warp-uniform byte count so far.
+template <bool WRITE>
+struct RecordOut {
+  unsigned char *o;
+  long long cur;
+  int lane;
+  // template piece j of the kernel's arguments (a.toff / a.tbytes, rendered on the host); whether it is not empty
+  template <class Args>
+  __device__ __forceinline__ bool piece(const Args &a, int j) {
+    const long long t0 = a.toff[j], tl = a.toff[j + 1] - t0;
+    if (WRITE)
+      for (long long k = lane; k < tl; k += 32) o[cur + k] = a.tbytes[t0 + k];
+    cur += tl;
+    return tl > 0;
   }
-}
+  __device__ __forceinline__ void comma() {
+    if (WRITE && lane == 0) o[cur] = ',';
+    cur += 1;
+  }
+  // one list of quoted, comma-separated ids from n candidates; get(i, &ptr, &len) == false skips candidate i.  first is
+  // warp-uniform.  The write tests o, not WRITE: with WRITE, ptxas holds k_iq_record's write pass to 40 registers and
+  // spills.
+  template <class Get>
+  __device__ __forceinline__ void list(long long n, const Get &get, bool &first) {
+    for (long long b = 0; b < n; b += 32) {
+      const long long i = b + lane;
+      const unsigned char *p = nullptr;
+      long long len = 0;
+      const bool keep = i < n && get(i, &p, &len);
+      const unsigned ball = __ballot_sync(0xffffffffu, keep);
+      if (!ball) continue;
+      const bool lead = first && lane == __ffs(ball) - 1;
+      const long long el = keep ? uq_escape(p, len, nullptr) + 2 + (lead ? 0 : 1) : 0;
+      long long x = el;
+      for (int d = 1; d < 32; d <<= 1) {
+        const long long y = __shfl_up_sync(0xffffffffu, x, d);
+        if (lane >= d) x += y;
+      }
+      if (o && keep) {
+        unsigned char *q = o + cur + x - el;
+        if (!lead) *q++ = ',';
+        *q++ = '"';
+        q += uq_escape(p, len, q);
+        *q = '"';
+      }
+      cur += __shfl_sync(0xffffffffu, x, 31);
+      first = false;
+    }
+  }
+};
 
 template <bool WRITE>
 __global__ void __launch_bounds__(256) k_uq_record(UqArgs a, const long long *__restrict__ rec_off, long long *__restrict__ rec_len,
@@ -250,47 +271,43 @@ __global__ void __launch_bounds__(256) k_uq_record(UqArgs a, const long long *__
   const long long warps = (long long)gridDim.x * (blockDim.x >> 5);
   for (long long r = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5; r < a.n_rec; r += warps) {
     const int32_t u = a.rec_uid[r];
-    unsigned char *o = WRITE ? out + rec_off[r] : nullptr;
-    long long cur = 0;
+    RecordOut<WRITE> w{WRITE ? out + rec_off[r] : nullptr, 0, lane};
     for (int j = 0; j <= a.n_kept + 1; ++j) {
-      const long long t0 = a.toff[j], tl = a.toff[j + 1] - t0;
-      if (WRITE)
-        for (long long k = lane; k < tl; k += 32) o[cur + k] = a.tbytes[t0 + k];
-      cur += tl;
+      w.piece(a, j);
       if (j > a.n_kept) break;
       bool first = true;
       if (j < a.n_kept) {   // the history of name j, oldest first, each item at its first position
         if (u < 0) continue;
         const unsigned long long s = (unsigned long long)u * a.nq + j;
         const long long h0 = a.hstart[s], cnt = min(a.hstart[s + 1] - h0, (long long)a.limit[j]);
-        uq_list(cnt, [&](long long i, const unsigned char **p, long long *len) {
+        w.list(cnt, [&](long long i, const unsigned char **p, long long *len) {
           const long long pos = h0 + cnt - 1 - i;
           if (!a.keep_h[pos]) return false;
           const uint32_t e = a.ent[a.hord[pos]];
           *p = a.ibytes + a.ioff[e];
           *len = a.ioff[e + 1] - a.ioff[e];
           return true;
-        }, o, cur, first);
+        }, first);
       } else {   // the blacklist: the user's blacklisted items newest first, then blacklistItems, distinct
         if (u >= 0) {
           const long long b0 = a.bstart[u];
-          uq_list(a.bstart[u + 1] - b0, [&](long long i, const unsigned char **p, long long *len) {
+          w.list(a.bstart[u + 1] - b0, [&](long long i, const unsigned char **p, long long *len) {
             if (!a.keep_b[b0 + i]) return false;
             const uint32_t e = a.ent[a.bord[b0 + i]];
             *p = a.ibytes + a.ioff[e];
             *len = a.ioff[e + 1] - a.ioff[e];
             return true;
-          }, o, cur, first);
+          }, first);
         }
-        uq_list(a.n_list, [&](long long i, const unsigned char **p, long long *len) {
+        w.list(a.n_list, [&](long long i, const unsigned char **p, long long *len) {
           if (!a.keep_l[i] || (u >= 0 && a.lgid[i] >= 0 && uq_has(a, u, a.lgid[i]))) return false;
           *p = a.lbytes + (a.loff[i] - a.lbase);
           *len = a.loff[i + 1] - a.loff[i];
           return true;
-        }, o, cur, first);
+        }, first);
       }
     }
-    if (!WRITE && lane == 0) rec_len[r] = cur;
+    if (!WRITE && lane == 0) rec_len[r] = w.cur;
   }
 }
 
@@ -430,61 +447,49 @@ __global__ void __launch_bounds__(256) k_iq_record(IqArgs a, const long long *__
   for (long long r = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5; r < a.n_rec; r += warps) {
     const int32_t d = a.rec_doc[r], key = a.rec_key[r];
     const bool similar = d >= 0 && a.line_moff[2 * (long long)d + 2] > a.line_moff[2 * (long long)d + 1];
-    unsigned char *o = WRITE ? out + rec_off[r] : nullptr;
-    long long cur = 0;
-    auto piece = [&](int j) {
-      const long long t0 = a.toff[j], tl = a.toff[j + 1] - t0;
-      if (WRITE)
-        for (long long k = lane; k < tl; k += 32) o[cur + k] = a.tbytes[t0 + k];
-      cur += tl;
-      return tl > 0;
-    };
-    auto comma = [&]() {
-      if (WRITE && lane == 0) o[cur] = ',';
-      cur += 1;
-    };
+    RecordOut<WRITE> w{WRITE ? out + rec_off[r] : nullptr, 0, lane};
     // a clause list: head fragment, the similar items (when here), tail fragment, comma-separated
     auto section = [&](int head, bool here, int tail) {
-      bool any = piece(head);
+      bool any = w.piece(a, head);
       for (int j = 0; here && similar && j < a.n_names; ++j) {
-        if (any) comma();
-        piece(9 + j);
+        if (any) w.comma();
+        w.piece(a, 9 + j);
         const long long x = (long long)d * a.T + a.name_entry[j], e0 = a.eoff[x], n = a.eoff[x + 1] - e0;
         bool first = true;
-        uq_list(n <= a.slice ? n : a.slice - 1, [&](long long i, const unsigned char **p, long long *len) {
+        w.list(n <= a.slice ? n : a.slice - 1, [&](long long i, const unsigned char **p, long long *len) {
           *p = a.dbytes + a.doff[e0 + i];
           *len = a.doff[e0 + i + 1] - a.doff[e0 + i];
           return true;
-        }, o, cur, first);
-        piece(8);
+        }, first);
+        w.piece(a, 8);
         any = true;
       }
       if (a.toff[tail + 1] > a.toff[tail]) {
-        if (any) comma();
-        piece(tail);
+        if (any) w.comma();
+        w.piece(a, tail);
       }
     };
-    piece(0);
+    w.piece(a, 0);
     section(1, !a.in_must, 2);
-    piece(3);
+    w.piece(a, 3);
     section(4, a.in_must, 5);
-    piece(6);
+    w.piece(a, 6);
     bool first = true;   // blacklistItems, each once, then the item unless it is among them
-    uq_list(a.n_list, [&](long long i, const unsigned char **p, long long *len) {
+    w.list(a.n_list, [&](long long i, const unsigned char **p, long long *len) {
       const long long k = a.list_at + i;
       if (a.first_in_list[a.kgid[k]] != (uint32_t)i) return false;
       *p = a.kbytes + a.koff[k];
       *len = a.koff[k + 1] - a.koff[k];
       return true;
-    }, o, cur, first);
+    }, first);
     if (a.exclude_self && a.first_in_list[a.kgid[key]] == ~0u)
-      uq_list(1, [&](long long, const unsigned char **p, long long *len) {
+      w.list(1, [&](long long, const unsigned char **p, long long *len) {
         *p = a.kbytes + a.koff[key];
         *len = a.koff[key + 1] - a.koff[key];
         return true;
-      }, o, cur, first);
-    piece(7);
-    if (!WRITE && lane == 0) rec_len[r] = cur;
+      }, first);
+    w.piece(a, 7);
+    if (!WRITE && lane == 0) rec_len[r] = w.cur;
   }
 }
 
@@ -531,53 +536,41 @@ __global__ void __launch_bounds__(256, 1) k_is_record(IsArgs a, const long long 
   const long long warps = (long long)gridDim.x * (blockDim.x >> 5);
   for (long long r = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5; r < a.n_sets; r += warps) {
     const long long e0 = a.soff[r], n = a.soff[r + 1] - e0, k0 = a.n_list + e0;
-    unsigned char *o = WRITE ? out + rec_off[r] : nullptr;
-    long long cur = 0;
-    auto piece = [&](int j) {
-      const long long t0 = a.toff[j], tl = a.toff[j + 1] - t0;
-      if (WRITE)
-        for (long long k = lane; k < tl; k += 32) o[cur + k] = a.tbytes[t0 + k];
-      cur += tl;
-      return tl > 0;
-    };
-    auto comma = [&]() {
-      if (WRITE && lane == 0) o[cur] = ',';
-      cur += 1;
-    };
-    piece(0);
-    bool any = piece(1);   // should: should_head, the set clause, should_tail
+    RecordOut<WRITE> w{WRITE ? out + rec_off[r] : nullptr, 0, lane};
+    w.piece(a, 0);
+    bool any = w.piece(a, 1);   // should: should_head, the set clause, should_tail
     if (a.with_set) {
-      if (any) comma();
-      piece(2);
+      if (any) w.comma();
+      w.piece(a, 2);
       bool first = true;   // every element as given
-      uq_list(n, [&](long long i, const unsigned char **p, long long *len) {
+      w.list(n, [&](long long i, const unsigned char **p, long long *len) {
         *p = a.kbytes + a.koff[k0 + i];
         *len = a.koff[k0 + i + 1] - a.koff[k0 + i];
         return true;
-      }, o, cur, first);
-      piece(3);
+      }, first);
+      w.piece(a, 3);
       any = true;
     }
     if (a.toff[5] > a.toff[4]) {
-      if (any) comma();
-      piece(4);
+      if (any) w.comma();
+      w.piece(a, 4);
     }
-    piece(5);
+    w.piece(a, 5);
     bool first = true;   // blacklistItems, each once, then the set's first occurrences that are not among them
-    uq_list(a.n_list, [&](long long i, const unsigned char **p, long long *len) {
+    w.list(a.n_list, [&](long long i, const unsigned char **p, long long *len) {
       if (a.first_in_list[a.kgid[i]] != (uint32_t)i) return false;
       *p = a.kbytes + a.koff[i];
       *len = a.koff[i + 1] - a.koff[i];
       return true;
-    }, o, cur, first);
-    uq_list(n, [&](long long i, const unsigned char **p, long long *len) {
+    }, first);
+    w.list(n, [&](long long i, const unsigned char **p, long long *len) {
       if (!a.first_in_set[e0 + i] || a.first_in_list[a.kgid[k0 + i]] != ~0u) return false;
       *p = a.kbytes + a.koff[k0 + i];
       *len = a.koff[k0 + i + 1] - a.koff[k0 + i];
       return true;
-    }, o, cur, first);
-    piece(6);
-    if (!WRITE && lane == 0) rec_len[r] = cur;
+    }, first);
+    w.piece(a, 6);
+    if (!WRITE && lane == 0) rec_len[r] = w.cur;
   }
 }
 

@@ -243,6 +243,21 @@ class CcoContext:
         finally:
             self._L.cco_host_free(self._h, out)
 
+    def _take_records(self, out, ln, off, n):
+        """-> (body, offsets int64[n + 1]) of a query builder's output, both buffers freed"""
+        offsets = np.ctypeslib.as_array(C.cast(off, C.POINTER(C.c_int64)), shape=(n.value + 1,)).copy()
+        self._L.cco_host_free(self._h, off)
+        return self._take_body(out, ln), offsets
+
+    def _take_dictionary(self, d, decode) -> list[str]:
+        """the ids of a cco_dictionary_t the library returned, as decode(offsets, blob) reads them; both buffers freed"""
+        off = np.ctypeslib.as_array(d.offsets, shape=(d.n + 1,)).copy()
+        addr = C.c_void_p.from_buffer(d, N.DictionaryT.bytes.offset).value
+        ids = decode(off, C.string_at(addr, int(off[-1])) if off[-1] else b"")
+        self._L.cco_host_free(self._h, C.cast(d.offsets, C.c_void_p))
+        self._L.cco_host_free(self._h, C.c_void_p(addr))
+        return ids
+
     def format_es_bulk(self, handle, names, row_ids, col_ids) -> bytes:
         """cco_format_es_bulk on a kept result (train_csr(..., keep=True)): one Elasticsearch bulk index action per row,
         `{"index":{"_id":id}}\\n{"id":id,"<event>":[ordered correlator ids],...}\\n` -- what toStringMapRDD + URModel.save +
@@ -491,17 +506,10 @@ class CcoContext:
             N.check(self._L.cco_event_log_user_queries(self._h, log._h, C.byref(qt), len(uo) - 1, uo.ctypes.data_as(C.POINTER(C.c_int64)),
                                                        ub.ctypes.data if len(ub) else None, C.byref(out), C.byref(ln), C.byref(off),
                                                        C.byref(n), None))
-        offsets = np.ctypeslib.as_array(C.cast(off, C.POINTER(C.c_int64)), shape=(n.value + 1,)).copy()
-        self._L.cco_host_free(self._h, off)
-        body = self._take_body(out, ln)
+        body, offsets = self._take_records(out, ln, off, n)
         if users is not None:
             return body, offsets
-        uoff = np.ctypeslib.as_array(ud.offsets, shape=(ud.n + 1,)).copy()
-        addr = C.c_void_p.from_buffer(ud, N.DictionaryT.bytes.offset).value
-        ids = decode_ids(uoff, C.string_at(addr, int(uoff[-1])) if uoff[-1] else b"")
-        self._L.cco_host_free(self._h, C.cast(ud.offsets, C.c_void_p))
-        self._L.cco_host_free(self._h, C.c_void_p(addr))
-        return body, offsets, ids
+        return body, offsets, self._take_dictionary(ud, decode_ids)
 
     def item_queries(self, index_body: bytes, ap, query=None, items=None, now_ms: Optional[int] = None, header: str = "{}"):
         """cco_item_queries: URAlgorithm.buildQuery for item queries (ur_query.py restates it), the similar items read from a
@@ -514,18 +522,16 @@ class CcoContext:
         enc = lambda x: x.encode("utf-8", "surrogatepass")
         names = [enc(n) for n in p.names]
         nm = (C.c_char_p * max(len(names), 1))(*names)
-        def column(ids):   # ids compare as UTF-8 bytes, a lone surrogate in its 3-byte form
-            b = [enc(x) for x in ids]
-            o = np.zeros(len(b) + 1, dtype=np.int64)
-            np.cumsum([len(x) for x in b], out=o[1:])
-            return o, np.frombuffer(b"".join(b), dtype=np.uint8)
 
         def text(b: bytes) -> str:
             try:
                 return b.decode("utf-8", "surrogatepass")
             except UnicodeDecodeError:
                 return b.decode("utf-8", "surrogateescape")
-        lo, lb = column(p.blacklist_items)
+
+        def decode(o, blob: bytes) -> list[str]:
+            return [text(blob[a:b]) for a, b in zip(o[:-1].tolist(), o[1:].tolist())]
+        lo, lb = _column(p.blacklist_items)
         qt = N.ItemQueryT(len(names), nm, p.max_query_events, 1 if p.in_must else 0, None if p.boost is None else p.boost.encode(),
                           1 if p.exclude_self else 0, enc(p.head), enc(p.should_head), enc(p.should), enc(p.must_head), enc(p.must),
                           enc(p.must_not), enc(p.sort), enc(header), len(lo) - 1, lo.ctypes.data_as(C.POINTER(C.c_int64)),
@@ -537,22 +543,14 @@ class CcoContext:
             N.check(self._L.cco_item_queries(self._h, index_body, len(index_body), C.byref(qt), 0, None, None, C.byref(out), C.byref(ln),
                                              C.byref(off), C.byref(n), C.byref(idd)))
         else:
-            io, ib = column(list(items))
+            io, ib = _column(list(items))
             N.check(self._L.cco_item_queries(self._h, index_body, len(index_body), C.byref(qt), len(io) - 1,
                                              io.ctypes.data_as(C.POINTER(C.c_int64)), ib.ctypes.data if len(ib) else None, C.byref(out),
                                              C.byref(ln), C.byref(off), C.byref(n), None))
-        offsets = np.ctypeslib.as_array(C.cast(off, C.POINTER(C.c_int64)), shape=(n.value + 1,)).copy()
-        self._L.cco_host_free(self._h, off)
-        body = self._take_body(out, ln)
+        body, offsets = self._take_records(out, ln, off, n)
         if items is not None:
             return body, offsets
-        ioff = np.ctypeslib.as_array(idd.offsets, shape=(idd.n + 1,)).copy()
-        addr = C.c_void_p.from_buffer(idd, N.DictionaryT.bytes.offset).value
-        blob = C.string_at(addr, int(ioff[-1])) if ioff[-1] else b""
-        ids = [text(blob[a:b]) for a, b in zip(ioff[:-1].tolist(), ioff[1:].tolist())]
-        self._L.cco_host_free(self._h, C.cast(idd.offsets, C.c_void_p))
-        self._L.cco_host_free(self._h, C.c_void_p(addr))
-        return body, offsets, ids
+        return body, offsets, self._take_dictionary(idd, decode)
 
     def item_set_queries(self, sets, ap, query=None, now_ms: Optional[int] = None, header: str = "{}"):
         """cco_item_set_queries: URAlgorithm.buildQuery for item-set ("shopping cart") queries (ur_query.py restates it), one
@@ -563,12 +561,6 @@ class CcoContext:
         from . import ur_query as Q
         p = Q.item_set_plan(ap, query, now_ms)
         enc = lambda x: x.encode("utf-8", "surrogatepass")
-
-        def column(ids):   # ids compare as UTF-8 bytes, a lone surrogate in its 3-byte form
-            b = [enc(x) for x in ids]
-            o = np.zeros(len(b) + 1, dtype=np.int64)
-            np.cumsum([len(x) for x in b], out=o[1:])
-            return o, np.frombuffer(b"".join(b), dtype=np.uint8)
         if isinstance(sets, tuple) and len(sets) == 3 and isinstance(sets[0], np.ndarray):
             so, eo, eb = np.ascontiguousarray(sets[0], dtype=np.int64), np.ascontiguousarray(sets[1], dtype=np.int64), sets[2]
             eb = np.frombuffer(eb, dtype=np.uint8) if isinstance(eb, (bytes, bytearray, memoryview)) else np.ascontiguousarray(eb, dtype=np.uint8)
@@ -576,8 +568,8 @@ class CcoContext:
             sets = [list(s) for s in sets]
             so = np.zeros(len(sets) + 1, dtype=np.int64)
             np.cumsum([len(s) for s in sets], out=so[1:])
-            eo, eb = column([x for s in sets for x in s])
-        lo, lb = column(p.blacklist_items)
+            eo, eb = _column([x for s in sets for x in s])
+        lo, lb = _column(p.blacklist_items)
         qt = N.ItemSetQueryT(None if p.name is None else enc(p.name), 1 if p.with_set else 0, None if p.boost is None else p.boost.encode(),
                              enc(p.head), enc(p.should_head), enc(p.should_tail), enc(p.must), enc(p.must_not), enc(p.sort), enc(header),
                              len(lo) - 1, lo.ctypes.data_as(C.POINTER(C.c_int64)), lb.ctypes.data if len(lb) else None)
@@ -585,9 +577,7 @@ class CcoContext:
         N.check(self._L.cco_item_set_queries(self._h, C.byref(qt), len(so) - 1, so.ctypes.data_as(C.POINTER(C.c_int64)), len(eo) - 1,
                                              eo.ctypes.data_as(C.POINTER(C.c_int64)), eb.ctypes.data if len(eb) else None, C.byref(out),
                                              C.byref(ln), C.byref(off), C.byref(n)))
-        offsets = np.ctypeslib.as_array(C.cast(off, C.POINTER(C.c_int64)), shape=(n.value + 1,)).copy()
-        self._L.cco_host_free(self._h, off)
-        return self._take_body(out, ln), offsets
+        return self._take_records(out, ln, off, n)
 
     def rerank_model(self, body: bytes, properties=None, rankings=None, log=None) -> bytes:
         """cco_rerank_model: calcPop (URAlgorithm.scala:375-399, recsModel "backfill") on an existing index.  body = the
@@ -919,6 +909,14 @@ def encode_ids(ids: Sequence[str]) -> tuple[np.ndarray, np.ndarray]:
     off = np.zeros(len(ids) + 1, dtype=np.int64)
     np.cumsum(lens, out=off[1:])
     return off, np.frombuffer(blob, dtype=np.uint8)
+
+
+def _column(ids) -> tuple[np.ndarray, np.ndarray]:
+    """encode_ids for the item query builders: ids compare as UTF-8 bytes, a lone surrogate in its 3-byte form"""
+    b = [x.encode("utf-8", "surrogatepass") for x in ids]
+    o = np.zeros(len(b) + 1, dtype=np.int64)
+    np.cumsum([len(x) for x in b], out=o[1:])
+    return o, np.frombuffer(b"".join(b), dtype=np.uint8)
 
 
 def decode_ids(offsets: np.ndarray, blob: bytes) -> list[str]:
