@@ -681,6 +681,78 @@ int cco_item_set_queries(cco_ctx_t *ctx, const cco_item_set_query_t *q, int64_t 
                          int64_t *out_n);
 
 /*
+ * Mixed queries (URAlgorithm.buildQuery for any combination of Query.user, Query.item and Query.itemSet,
+ * URAlgorithm.scala:563-839): one Elasticsearch query per row, where each row of the batch may have a user, an item and an
+ * item set, or any subset of them.  The batch shares one template.
+ *  - Rows: n_rows; three optional columns, each with an optional validity bitmap (Arrow: LSB-first, bit r = 1 when row r
+ *    has the member; NULL: every row has it).  A NULL offsets pointer means no row has the member.  users and items are
+ *    large_string columns of n_rows ids; sets are list<large_string> as in cco_item_set_queries (set_offsets [n_rows + 1]
+ *    into an element column of n_elements ids).  An absent set writes nothing; a present empty set writes [].
+ *  - History (the row's user, as in cco_event_log_user_queries, from a log read with CCO_LOG_KEEP_HISTORY): the first
+ *    n_history_names names get a terms clause, with the user's list, or [] for a row without a user or with a user the log
+ *    does not know.  In should with history_boost (none when NULL), or in must with "boost":0 when history_in_must.
+ *  - Similar items (the row's item, as in cco_item_queries, from index_body): one clause per model name when the item has a
+ *    document whose source has a member; sliced to max_query_events; in should with similar_boost, or in must with
+ *    "boost":0 when similar_in_must.
+ *  - The set clause (as in cco_item_set_queries): {"terms":{"<set_name>":[elements]}} with ,"boost":<set_boost> when
+ *    set_boost is not NULL, when with_set and the row has a set.
+ *  - Excluded ids: the user's blacklisted items (newest first), blacklistItems, the item when exclude_self, the set's
+ *    elements; each id once, at its first position (ids compare as bytes).
+ *  - The body record:
+ *      header \n head ,"query":{"bool":{"should":[HISTORY?, SIMILAR?, boosted, SET?, should_tail],"must":[HISTORY?,
+ *      SIMILAR?, must],"must_not":[{"ids":{"values":[excluded],"boost":0}}(,must_not)?],"minimum_should_match":1}},
+ *      "sort":sort} \n
+ *    where the elements of should and must are comma-separated and an empty piece leaves no comma.  Ids, elements and
+ *    names are escaped as in cco_event_log_user_queries.
+ * log may be NULL when no row has a user; index_body may be NULL when no row has an item (index_len 0 with a non-NULL
+ * body is an empty index: every item is unknown).  A given body is parsed with cco_item_queries' grammar and checks.
+ * limits may be NULL when user_offsets is NULL.
+ * Fragments are JSON text spliced verbatim: head ({"from":F,"size":N), boosted (the boosted metadata; may be empty),
+ * should_tail (the constant_score clause), must (the filtering metadata and the date filters; may be empty), must_not (may
+ * be empty), sort (an array), header (one _msearch header line).
+ * Out: *out_body [*out_len] and *out_offsets [*out_n + 1] (record r = body[offsets[r] .. offsets[r + 1])), pinned memory
+ * owned by the context, each released with cco_host_free.
+ * Errors: CCO_E_INVALID_ARG for everything the three builders refuse (same messages where the cause is the same), a row
+ * with a user but no log or a log without history, a log of another context, a row with an item but no index body, and
+ * bad offsets in any column (decided on the device before any kernel reads through them); CCO_E_UNSUPPORTED for group
+ * contexts, 2^31 or more rows, documents + items + blacklist items + elements >= 2^31, 2^31 or more training events of
+ * the names and a record of 2^31 or more bytes.
+ */
+typedef struct {
+  /* the history: cco_user_query_t's members */
+  int32_t n_names;
+  int32_t n_history_names;           /* maxQueryEvents - 1 clamped to [0, n_names] */
+  const char *const *names;          /* [n_names] the query event names */
+  const int32_t *limits;             /* [n_names] history limit per name; may be NULL without a user column */
+  int32_t n_blacklist_names;
+  int32_t history_in_must;           /* 0: should (userBias >= 0), 1: must (userBias < 0) */
+  const char *const *blacklist_names;
+  const char *history_boost;         /* JSON number text or NULL */
+  /* the similar items: cco_item_query_t's members */
+  int32_t n_model_names;
+  const char *const *model_names;    /* [n_model_names] the index's indicator fields */
+  int32_t max_query_events;
+  int32_t similar_in_must;           /* 0: should (algorithm itemBias >= 0), 1: must (itemBias < 0) */
+  const char *similar_boost;         /* JSON number text or NULL */
+  int32_t exclude_self;              /* 1: the item is excluded (!returnSelf) */
+  /* the set clause: cco_item_set_query_t's members */
+  const char *set_name;              /* the first model event name (may be NULL without with_set) */
+  int32_t with_set;                  /* 0: no set clause (itemSetBias 0), 1: the clause is written */
+  const char *set_boost;             /* JSON number text or NULL */
+  const char *head, *boosted, *should_tail, *must, *must_not, *sort, *header;  /* boosted, must may be "" */
+  int64_t n_blacklist_items;
+  const int64_t *blacklist_item_offsets; /* [n + 1] */
+  const char *blacklist_item_bytes;
+} cco_mixed_query_t;
+int cco_mixed_queries(cco_ctx_t *ctx, const cco_event_log_t *log /* nullable */, const char *index_body /* nullable */, int64_t index_len,
+                      const cco_mixed_query_t *q, int64_t n_rows,
+                      const int64_t *user_offsets /* nullable */, const char *user_bytes, const uint8_t *user_validity /* nullable */,
+                      const int64_t *item_offsets /* nullable */, const char *item_bytes, const uint8_t *item_validity /* nullable */,
+                      const int64_t *set_offsets /* nullable */, int64_t n_elements, const int64_t *elem_offsets, const char *elem_bytes,
+                      const uint8_t *set_validity /* nullable */, char **out_body, int64_t *out_len, int64_t **out_offsets,
+                      int64_t *out_n);
+
+/*
  * Debug/parity entry (tests only): full integer co-occurrence matrix A^T B of two canonical
  * binary matrices computed by the same accumulation kernel as cco_train, no LLR, no top-k.
  * Output CSR over the columns of A with ascending column ids, malloc'ed; free with cco_free.

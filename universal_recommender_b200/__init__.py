@@ -17,6 +17,8 @@ Host-side mirror of the reference interface for this path:
   ur_algorithm.user_queries_from_events / item_queries / item_set_queries  <- buildQuery for every user of an export /
                                              every item of a model index / every item set of a batch, on the GPU
                                              (cco_event_log_user_queries, cco_item_queries, cco_item_set_queries); ur_query.py
+  ur_algorithm.mixed_queries_from_events  <- buildQuery for rows with any subset of {user, item, item set}, on the GPU
+                                             (cco_mixed_queries); ur_query.py
   ur_model                                <- propertiesRDD, getRanksRDD, groupAll (URAlgorithm.scala:351-369, 537-560;
                                              URModel.scala:57-140): the host mirror of the model documents
 """
@@ -28,15 +30,16 @@ from .preparator import prepare, prepare_on_device
 from .similarity_analysis import (CcoContext, DownsamplableCrossOccurrenceDataset, EventLog, SimilarityAnalysis,
                                   decode_ids, default_context, encode_ids)
 from .ur_algorithm import (DefaultURAlgoParams, IndicatorParams, URAlgorithmParams, calc_all, calc_all_from_events, calc_all_on_device,
-                           calc_pop_from_events, calc_pop_on_device, item_queries, item_set_queries, user_queries_from_events)
-from .ur_query import ItemQuery, ItemSetQuery, UserQuery
+                           calc_pop_from_events, calc_pop_on_device, item_queries, item_set_queries, mixed_queries_from_events,
+                           user_queries_from_events)
+from .ur_query import ItemQuery, ItemSetQuery, MixedQuery, UserQuery
 from .ur_model import RankingParams
 
 __all__ = [
     "BiDictionary", "CcoContext", "CcoError", "CcoInvalidArgument", "DataSourceParams", "DefaultURAlgoParams", "EventWindow",
     "DownsamplableCrossOccurrenceDataset", "IndexedDataset", "IndicatorParams", "SimilarityAnalysis",
     "EventLog", "RankingParams", "URAlgorithmParams", "calc_all", "calc_all_from_events", "calc_all_on_device", "calc_pop_from_events",
-    "calc_pop_on_device", "item_queries", "item_set_queries", "user_queries_from_events", "ItemQuery", "ItemSetQuery", "UserQuery", "decode_ids", "default_context", "encode_ids", "prepare", "prepare_on_device",
+    "calc_pop_on_device", "item_queries", "item_set_queries", "mixed_queries_from_events", "user_queries_from_events", "ItemQuery", "ItemSetQuery", "MixedQuery", "UserQuery", "decode_ids", "default_context", "encode_ids", "prepare", "prepare_on_device",
     "FLAG_ASSUME_CANONICAL",
     "FLAG_ENTROPY_VARARGS", "FLAG_ROWRATE_INTDIV", "FLAG_RESULT_NO_COUNT", "FLAG_RESULT_NO_LLR", "LIB_PATH",
 ]

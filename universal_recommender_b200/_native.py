@@ -119,6 +119,16 @@ class ItemSetQueryT(C.Structure):
                 ("n_blacklist_items", C.c_int64), ("blacklist_item_offsets", C.POINTER(C.c_int64)), ("blacklist_item_bytes", C.c_void_p)]
 
 
+class MixedQueryT(C.Structure):
+    _fields_ = [("n_names", C.c_int32), ("n_history_names", C.c_int32), ("names", C.POINTER(C.c_char_p)), ("limits", C.POINTER(C.c_int32)),
+                ("n_blacklist_names", C.c_int32), ("history_in_must", C.c_int32), ("blacklist_names", C.POINTER(C.c_char_p)),
+                ("history_boost", C.c_char_p), ("n_model_names", C.c_int32), ("model_names", C.POINTER(C.c_char_p)),
+                ("max_query_events", C.c_int32), ("similar_in_must", C.c_int32), ("similar_boost", C.c_char_p), ("exclude_self", C.c_int32),
+                ("set_name", C.c_char_p), ("with_set", C.c_int32), ("set_boost", C.c_char_p), ("head", C.c_char_p), ("boosted", C.c_char_p),
+                ("should_tail", C.c_char_p), ("must", C.c_char_p), ("must_not", C.c_char_p), ("sort", C.c_char_p), ("header", C.c_char_p),
+                ("n_blacklist_items", C.c_int64), ("blacklist_item_offsets", C.POINTER(C.c_int64)), ("blacklist_item_bytes", C.c_void_p)]
+
+
 class LogRankingT(C.Structure):
     _fields_ = [("name", C.c_char_p), ("mode", C.c_int32), ("n_event_names", C.c_int32), ("start_ms", C.c_int64), ("end_ms", C.c_int64),
                 ("event_names", C.POINTER(C.c_char_p))]
@@ -143,7 +153,7 @@ EXPORTS = [
     "cco_format_model", "cco_rerank_model", "cco_event_log_read", "cco_event_log_info", "cco_event_log_ingest",
     "cco_format_model_log", "cco_rerank_model_log", "cco_event_log_free", "cco_event_log_begin", "cco_event_log_append",
     "cco_event_log_finish", "cco_event_log_begin_window", "cco_event_log_window_stats",
-    "cco_event_log_begin_ex", "cco_event_log_user_queries", "cco_item_queries", "cco_item_set_queries", "cco_result_num_matrices", "cco_result_row_range", "cco_result_matrix", "cco_result_stats", "cco_result_free",
+    "cco_event_log_begin_ex", "cco_event_log_user_queries", "cco_item_queries", "cco_item_set_queries", "cco_mixed_queries", "cco_result_num_matrices", "cco_result_row_range", "cco_result_matrix", "cco_result_stats", "cco_result_free",
     "cco_debug_cooccurrence", "cco_debug_downsample", "cco_debug_downsample_block", "cco_debug_llr", "cco_debug_string_ids", "cco_debug_rank_text", "cco_free",
 ]
 
@@ -211,6 +221,10 @@ def lib():
                                    p(C.c_int64), p(C.c_void_p), p(C.c_int64), p(DictionaryT)]
     L.cco_item_set_queries.argtypes = [C.c_void_p, p(ItemSetQueryT), C.c_int64, p(C.c_int64), C.c_int64, p(C.c_int64), C.c_void_p,
                                        p(C.c_void_p), p(C.c_int64), p(C.c_void_p), p(C.c_int64)]
+    L.cco_mixed_queries.argtypes = [C.c_void_p, C.c_void_p, C.c_char_p, C.c_int64, p(MixedQueryT), C.c_int64,
+                                    p(C.c_int64), C.c_void_p, C.c_void_p, p(C.c_int64), C.c_void_p, C.c_void_p,
+                                    p(C.c_int64), C.c_int64, p(C.c_int64), C.c_void_p, C.c_void_p,
+                                    p(C.c_void_p), p(C.c_int64), p(C.c_void_p), p(C.c_int64)]
     L.cco_dataset_shape.argtypes = [C.c_void_p, C.c_int32, p(C.c_int64), p(C.c_int32), p(C.c_int64)]
     L.cco_dataset_download.argtypes = [C.c_void_p, C.c_int32, p(p(C.c_int64)), p(p(C.c_int32))]
     L.cco_timer_start.argtypes = [C.c_void_p]

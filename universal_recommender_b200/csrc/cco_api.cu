@@ -4900,36 +4900,31 @@ static int uq_check_host(const cco_user_query_t *q, int64_t n_users, const int64
   return CCO_OK;
 }
 
-static int user_queries(cco_ctx *c, const cco_event_log *lg, const cco_user_query_t *q, int64_t n_users, const int64_t *uoff,
-                        const char *ubytes, char **out_body, int64_t *out_len, int64_t **out_offsets, int64_t *out_n,
-                        cco_dictionary_t *out_users) {
+// The history stage of the user-query builders: every training event of the query names, the users' history lists and
+// their blacklisted items, in HBM.  The log's users and items are grouped exactly; the groups number the user table (ut)
+// and the item table (it) that records and ids are looked up in.
+struct UqHistory {
+  long long E = 0, G = 0, B = 0;   // events of the query names, users among them, blacklisted events
+  StrTable ut, it;
+  DevStrCol tu, ti;                // the log's training user and item columns (hashed when E > 0)
+  uint32_t *ent = nullptr, *hord = nullptr, *bord = nullptr, *gord = nullptr;
+  uint8_t *keep_h = nullptr, *keep_b = nullptr;
+  int32_t *uid = nullptr, *iid = nullptr, *d_limit = nullptr;
+  long long *ln = nullptr, *hstart = nullptr, *bstart = nullptr;
+  unsigned long long *bkey = nullptr;
+};
+static int uq_history(cco_ctx *c, Arena &ar, const cco_event_log *lg, int nq, const char *const *names, const int32_t *limits,
+                      int n_blacklist_names, const char *const *blacklist_names, UqHistory *h) {
   cudaStream_t s = c->stream;
-  const int nq = q->n_names;
   std::vector<int> code(nq);
   std::vector<uint8_t> black(std::max(nq, 1), 0);
   for (int k = 0; k < nq; ++k) {
-    code[k] = lg->code_of(q->names[k]);
+    code[k] = lg->code_of(names[k]);
     bool earlier = false;   // a repeated query name reads the same events: blacklist them once
-    for (int j = 0; j < k; ++j) earlier |= strcmp(q->names[j], q->names[k]) == 0;
-    for (int b = 0; b < q->n_blacklist_names && !earlier; ++b)
-      if (strcmp(q->blacklist_names[b], q->names[k]) == 0) black[k] = 1;
+    for (int j = 0; j < k; ++j) earlier |= strcmp(names[j], names[k]) == 0;
+    for (int b = 0; b < n_blacklist_names && !earlier; ++b)
+      if (strcmp(blacklist_names[b], names[k]) == 0) black[k] = 1;
   }
-  CK(cudaSetDevice(c->device));
-  mail_reset(c);
-  Arena ar(s);
-  NvtxRange nvtx("cco:user_queries");
-  // 1. the caller's columns, checked on the device before any kernel reads bytes through their offsets
-  DevStrCol lc, uc;
-  CKR(str_upload(c, ar, q->n_blacklist_items, q->blacklist_item_offsets, q->blacklist_item_bytes, &lc));
-  if (uoff) CKR(str_upload(c, ar, n_users, uoff, ubytes, &uc));
-  int *bad, h_bad = 0;
-  CKR(ar.alloc(&bad, 1));
-  CK(cudaMemsetAsync(bad, 0, 4, s));
-  str_check_device(c, lc, bad);
-  if (uoff) str_check_device(c, uc, bad);
-  CKR(mail_fetch(c, &h_bad, bad, 4));
-  CKR(mail_wait(c));
-  if (h_bad) return set_error(CCO_E_INVALID_ARG, "decreasing offsets in the blacklist items or the users");
   // 2. the training events of the query names, name-major
   std::vector<long long> qoff(nq + 1, 0), qbase(std::max(nq, 1), 0);
   for (int k = 0; k < nq; ++k) {
@@ -4940,17 +4935,17 @@ static int user_queries(cco_ctx *c, const cco_event_log *lg, const cco_user_quer
   const long long E = qoff[nq];
   if (E >= 0x7fffffffLL) return set_error(CCO_E_UNSUPPORTED, "%lld training events of the query names, at most 2^31 - 2", E);
   const long long NT = lg->train_at.back();
-  long long G = 0;
-  StrTable ut, it;
-  DevStrCol tu, ti;
-  uint32_t *ent = nullptr, *gord = nullptr, *hord = nullptr, *bord = nullptr;
-  uint8_t *qr = nullptr, *keep_h = nullptr, *keep_b = nullptr, *d_black = nullptr;
-  int32_t *uid = nullptr, *iid = nullptr, *d_limit = nullptr;
-  long long *tm = nullptr, *ln = nullptr, *hstart = nullptr, *bstart = nullptr;
-  unsigned long long *bkey = nullptr;
-  long long B = 0;
+  h->E = E;
+  long long &G = h->G, &B = h->B;
+  StrTable &ut = h->ut, &it = h->it;
+  DevStrCol &tu = h->tu, &ti = h->ti;
+  uint32_t *&ent = h->ent, *&gord = h->gord, *&hord = h->hord, *&bord = h->bord;
+  uint8_t *qr = nullptr, *&keep_h = h->keep_h, *&keep_b = h->keep_b, *d_black = nullptr;
+  int32_t *&uid = h->uid, *&iid = h->iid, *&d_limit = h->d_limit;
+  long long *tm = nullptr, *&ln = h->ln, *&hstart = h->hstart, *&bstart = h->bstart;
+  unsigned long long *&bkey = h->bkey;
   CKR(ar.alloc(&d_limit, std::max(nq, 1)));
-  if (nq > 0) CK(cudaMemcpyAsync(d_limit, q->limits, sizeof(int32_t) * (size_t)nq, cudaMemcpyHostToDevice, s));
+  if (nq > 0) CK(cudaMemcpyAsync(d_limit, limits, sizeof(int32_t) * (size_t)nq, cudaMemcpyHostToDevice, s));
   if (E > 0) {
     long long *d_qoff, *d_qbase;
     CKR(ar.alloc(&d_qoff, nq + 1));
@@ -5059,6 +5054,68 @@ static int user_queries(cco_ctx *c, const cco_event_log *lg, const cco_user_quer
     }
     CKR(exclusive_sum(c, ar, bcnt, bstart, G + 1));
   }
+  return CCO_OK;
+}
+// the user group of each of R records (-1: no training event of a query name); uc holds the records' user ids
+static int uq_record_users(cco_ctx *c, const UqHistory &h, const DevStrCol &uc, long long R, int32_t *rec_uid) {
+  cudaStream_t s = c->stream;
+  if (R > 0 && h.E > 0) {
+    str_hash(c, uc, ~0ULL);
+    k_str_lookup<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, uc.off, uc.base, uc.w, uc.hash, h.tu.off, h.tu.base, h.tu.w, h.tu.hash,
+                                                              (uint64_t)h.ut.cap - 1, h.ut.table, h.ut.rank_of_slot, rec_uid);
+    c->launches++;
+  } else if (R > 0) {
+    CK(cudaMemsetAsync(rec_uid, 0xff, sizeof(int32_t) * (size_t)R, s));
+  }
+  return CCO_OK;
+}
+// the history members of a record kernel's UqArgs; the records, the list and the template are the caller's
+static UqArgs uq_args(const UqHistory &h, const cco_event_log *lg, int nq, int n_kept) {
+  UqArgs a{};
+  a.nq = nq;
+  a.n_kept = n_kept;
+  a.limit = h.d_limit;
+  a.hstart = h.hstart;
+  a.hord = h.hord;
+  a.keep_h = h.keep_h;
+  a.bstart = h.bstart;
+  a.bord = h.bord;
+  a.keep_b = h.keep_b;
+  a.bkey = h.bkey;
+  a.B = h.B;
+  a.ent = h.ent;
+  a.ioff = h.E > 0 ? lg->ti.off : nullptr;
+  a.ibytes = h.E > 0 ? (const unsigned char *)lg->ti.w : nullptr;
+  return a;
+}
+
+static int user_queries(cco_ctx *c, const cco_event_log *lg, const cco_user_query_t *q, int64_t n_users, const int64_t *uoff,
+                        const char *ubytes, char **out_body, int64_t *out_len, int64_t **out_offsets, int64_t *out_n,
+                        cco_dictionary_t *out_users) {
+  cudaStream_t s = c->stream;
+  const int nq = q->n_names;
+  CK(cudaSetDevice(c->device));
+  mail_reset(c);
+  Arena ar(s);
+  NvtxRange nvtx("cco:user_queries");
+  // 1. the caller's columns, checked on the device before any kernel reads bytes through their offsets
+  DevStrCol lc, uc;
+  CKR(str_upload(c, ar, q->n_blacklist_items, q->blacklist_item_offsets, q->blacklist_item_bytes, &lc));
+  if (uoff) CKR(str_upload(c, ar, n_users, uoff, ubytes, &uc));
+  int *bad, h_bad = 0;
+  CKR(ar.alloc(&bad, 1));
+  CK(cudaMemsetAsync(bad, 0, 4, s));
+  str_check_device(c, lc, bad);
+  if (uoff) str_check_device(c, uc, bad);
+  CKR(mail_fetch(c, &h_bad, bad, 4));
+  CKR(mail_wait(c));
+  if (h_bad) return set_error(CCO_E_INVALID_ARG, "decreasing offsets in the blacklist items or the users");
+  // 2-8. the history
+  UqHistory h;
+  CKR(uq_history(c, ar, lg, nq, q->names, q->limits, q->n_blacklist_names, q->blacklist_names, &h));
+  const long long E = h.E, G = h.G;
+  const StrTable &ut = h.ut, &it = h.it;
+  const DevStrCol &tu = h.tu, &ti = h.ti;
   // 9. blacklistItems: item groups of the log (membership is a group test), repeats within the list dropped
   const long long NL = q->n_blacklist_items;
   int32_t *lgid;
@@ -5087,14 +5144,7 @@ static int user_queries(cco_ctx *c, const cco_event_log *lg, const cco_user_quer
   if (uoff) {
     R = n_users;
     CKR(ar.alloc(&rec_uid, std::max<long long>(R, 1)));
-    if (R > 0 && E > 0) {
-      str_hash(c, uc, ~0ULL);
-      k_str_lookup<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, uc.off, uc.base, uc.w, uc.hash, tu.off, tu.base, tu.w, tu.hash,
-                                                                (uint64_t)ut.cap - 1, ut.table, ut.rank_of_slot, rec_uid);
-      c->launches++;
-    } else if (R > 0) {
-      CK(cudaMemsetAsync(rec_uid, 0xff, sizeof(int32_t) * (size_t)R, s));
-    }
+    CKR(uq_record_users(c, h, uc, R, rec_uid));
   } else {   // every user with an event of a query name, by first line
     R = G;
     CKR(ar.alloc(&rec_uid, std::max<long long>(R, 1)));
@@ -5103,7 +5153,7 @@ static int user_queries(cco_ctx *c, const cco_event_log *lg, const cco_user_quer
       CKR(ar.alloc(&mn, G));
       CKR(ar.alloc(&uk, G));
       CK(cudaMemsetAsync(mn, 0xff, sizeof(unsigned long long) * (size_t)G, s));
-      k_uq_min_line<<<grid_for(E, 256, c->sm_count), 256, 0, s>>>(E, uid, ln, mn);
+      k_uq_min_line<<<grid_for(E, 256, c->sm_count), 256, 0, s>>>(E, h.uid, h.ln, mn);
       k_uq_user_keys<<<grid_for(G, 256, c->sm_count), 256, 0, s>>>(G, mn, uk, rec_uid);
       c->launches += 2;
       CKR(sort_pairs(c, ar, G, &uk, &rec_uid, bits_for(lg->n_lines)));
@@ -5140,23 +5190,9 @@ static int user_queries(cco_ctx *c, const cco_event_log *lg, const cco_user_quer
   // 11. the template, then a length pass, the record offsets and a write pass: one warp per record
   DevDict tp;
   CKR(upload_strings(c, ar, uq_template(q), &tp));
-  UqArgs a;
+  UqArgs a = uq_args(h, lg, nq, q->n_history_names);
   a.n_rec = R;
   a.rec_uid = rec_uid;
-  a.nq = nq;
-  a.n_kept = q->n_history_names;
-  a.limit = d_limit;
-  a.hstart = hstart;
-  a.hord = hord;
-  a.keep_h = keep_h;
-  a.bstart = bstart;
-  a.bord = bord;
-  a.keep_b = keep_b;
-  a.bkey = bkey;
-  a.B = B;
-  a.ent = ent;
-  a.ioff = E > 0 ? lg->ti.off : nullptr;
-  a.ibytes = E > 0 ? (const unsigned char *)lg->ti.w : nullptr;
   a.n_list = NL;
   a.loff = lc.off;
   a.lbase = lc.base;
@@ -5223,37 +5259,9 @@ static int iq_check_host(const cco_item_query_t *q, int64_t n_items, const int64
   return CCO_OK;
 }
 
-static int item_queries(cco_ctx *c, const char *body, int64_t body_len, const cco_item_query_t *q, int64_t n_items, const int64_t *ioff,
-                        const char *ibytes, char **out_body, int64_t *out_len, int64_t **out_offsets, int64_t *out_n,
-                        cco_dictionary_t *out_items) {
+// the documents' side of an item query: _ids are unique (gid: the key column's groups, the documents first)
+static int iq_unique_ids(cco_ctx *c, Arena &ar, long long D, const int32_t *gid, const StrTable &tb) {
   cudaStream_t s = c->stream;
-  CK(cudaSetDevice(c->device));
-  Arena ar(s);
-  NvtxRange nvtx("cco:item_queries");
-  mail_reset(c);
-  const bool all = ioff == nullptr;
-  const long long NI = all ? 0 : n_items, NL = q->n_blacklist_items;
-  // 1-4. the documents: members, decoded names and _ids
-  BulkDocs bd;
-  CKR(bulk_parse(c, ar, body, body_len, NI + NL, "items + blacklist items", &bd));
-  const long long D = bd.D, R = all ? D : NI;
-  // 5. one key column: the decoded _ids, the items, blacklistItems; the caller's offsets are checked on the device before
-  //    any kernel reads bytes through them
-  int *bad, h_bad = 0;
-  CKR(ar.alloc(&bad, 1));
-  CK(cudaMemsetAsync(bad, 0, sizeof(int), s));
-  DevStrCol key;
-  CKR(key_column(c, ar, {KeySection{D, (const int64_t *)bd.ids.off, (const char *)bd.ids.w, true, bd.ids_bytes}, KeySection{NI, ioff, ibytes},
-                         KeySection{NL, q->blacklist_item_offsets, q->blacklist_item_bytes}}, bad, &key));
-  CKR(mail_fetch(c, &h_bad, bad, 4));
-  CKR(mail_wait(c));
-  if (h_bad) return set_error(CCO_E_INVALID_ARG, "decreasing offsets in the items or the blacklist items");
-  // 6. one exact grouping over the key column; a group that holds two documents is a repeated _id
-  str_hash(c, key, ~0ULL);
-  int32_t *gid;
-  CKR(ar.alloc(&gid, std::max<long long>(key.n, 1)));
-  StrTable tb;
-  CKR(str_group(c, ar, key, nullptr, false, 0, &tb, gid));
   if (D > 0) {
     unsigned long long *dup, h_dup = ~0ULL;
     CKR(ar.alloc(&dup, 1));
@@ -5265,41 +5273,37 @@ static int item_queries(cco_ctx *c, const char *body, int64_t body_len, const cc
     if (h_dup != ~0ULL)
       return set_error(CCO_E_INVALID_ARG, "document %llu: its _id is the _id of document %llu", h_dup >> 32, h_dup & 0xffffffffULL);
   }
-  // 7. blacklistItems: each group's first list index (membership and repeats are group tests)
-  const long long G = tb.n_groups;
-  uint32_t *first_in_list;
-  CKR(ar.alloc(&first_in_list, std::max<long long>(G, 1)));
-  CK(cudaMemsetAsync(first_in_list, 0xff, sizeof(uint32_t) * (size_t)std::max<long long>(G, 1), s));
-  if (NL > 0) {
-    k_iq_black<<<grid_for(NL, 256, c->sm_count), 256, 0, s>>>(NL, D + NI, gid, first_in_list);
-    c->launches++;
-  }
-  // 8. the records' documents; the queried documents
-  int32_t *rec_doc, *rec_key;
-  uint8_t *queried;
-  CKR(ar.alloc(&rec_doc, std::max<long long>(R, 1)));
-  CKR(ar.alloc(&rec_key, std::max<long long>(R, 1)));
-  CKR(ar.alloc(&queried, std::max<long long>(D, 1)));
-  CK(cudaMemsetAsync(queried, 0, (size_t)std::max<long long>(D, 1), s));
-  if (R > 0) {
-    k_iq_rec<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, D, all, gid, tb.first_sorted, rec_doc, rec_key, queried);
-    c->launches++;
-  }
+  return CCO_OK;
+}
+// The similar-items lists of the queried documents: per document the last source member of each distinct model name,
+// checked as an array of strings (only where queried[d]) and its elements decoded.  Element list (d, t) is
+// dec[eoff[d * T + t] .. eoff[d * T + t + 1]); model name j is distinct name name_entry[j].
+struct IqDocs {
+  int T = 0;
+  std::vector<int32_t> name_entry;
+  long long *eoff = nullptr;   // [D * T + 1]
+  DevStrCol dec;
+};
+static int iq_documents(cco_ctx *c, Arena &ar, const BulkDocs &bd, int n_names, const char *const *names, const uint8_t *queried,
+                        IqDocs *o) {
+  cudaStream_t s = c->stream;
   // 9. the distinct model names; per document the last source member of each
   std::vector<std::string> ent;
-  std::vector<int32_t> name_entry(q->n_names);
-  for (int j = 0; j < q->n_names; ++j) {
+  std::vector<int32_t> &name_entry = o->name_entry;
+  name_entry.assign(n_names, 0);
+  for (int j = 0; j < n_names; ++j) {
     size_t t = 0;
-    while (t < ent.size() && ent[t] != q->names[j]) ++t;
-    if (t == ent.size()) ent.push_back(q->names[j]);
+    while (t < ent.size() && ent[t] != names[j]) ++t;
+    if (t == ent.size()) ent.push_back(names[j]);
     name_entry[j] = (int32_t)t;
   }
   const int T = (int)ent.size();
-  const long long DT = D * T;
-  long long *eoff;
+  o->T = T;
+  const long long D = bd.D, DT = D * T;
+  long long *&eoff = o->eoff;
   CKR(ar.alloc(&eoff, DT + 1));
   CK(cudaMemsetAsync(eoff, 0, sizeof(long long) * (size_t)(DT + 1), s));
-  DevStrCol dec;
+  DevStrCol &dec = o->dec;
   if (D > 0) {
     int32_t *ngid, *entry_of, *pick;
     CKR(member_entries(c, ar, bd.names, ent, &ngid, &entry_of));
@@ -5332,10 +5336,68 @@ static int item_queries(cco_ctx *c, const char *body, int64_t body_len, const cc
     long long dec_bytes = 0;
     CKR(json_decode(c, ar, NE, elem, bd.body, &dec, &dec_bytes));
   }
+  return CCO_OK;
+}
+
+static int item_queries(cco_ctx *c, const char *body, int64_t body_len, const cco_item_query_t *q, int64_t n_items, const int64_t *ioff,
+                        const char *ibytes, char **out_body, int64_t *out_len, int64_t **out_offsets, int64_t *out_n,
+                        cco_dictionary_t *out_items) {
+  cudaStream_t s = c->stream;
+  CK(cudaSetDevice(c->device));
+  Arena ar(s);
+  NvtxRange nvtx("cco:item_queries");
+  mail_reset(c);
+  const bool all = ioff == nullptr;
+  const long long NI = all ? 0 : n_items, NL = q->n_blacklist_items;
+  // 1-4. the documents: members, decoded names and _ids
+  BulkDocs bd;
+  CKR(bulk_parse(c, ar, body, body_len, NI + NL, "items + blacklist items", &bd));
+  const long long D = bd.D, R = all ? D : NI;
+  // 5. one key column: the decoded _ids, the items, blacklistItems; the caller's offsets are checked on the device before
+  //    any kernel reads bytes through them
+  int *bad, h_bad = 0;
+  CKR(ar.alloc(&bad, 1));
+  CK(cudaMemsetAsync(bad, 0, sizeof(int), s));
+  DevStrCol key;
+  CKR(key_column(c, ar, {KeySection{D, (const int64_t *)bd.ids.off, (const char *)bd.ids.w, true, bd.ids_bytes}, KeySection{NI, ioff, ibytes},
+                         KeySection{NL, q->blacklist_item_offsets, q->blacklist_item_bytes}}, bad, &key));
+  CKR(mail_fetch(c, &h_bad, bad, 4));
+  CKR(mail_wait(c));
+  if (h_bad) return set_error(CCO_E_INVALID_ARG, "decreasing offsets in the items or the blacklist items");
+  // 6. one exact grouping over the key column; a group that holds two documents is a repeated _id
+  str_hash(c, key, ~0ULL);
+  int32_t *gid;
+  CKR(ar.alloc(&gid, std::max<long long>(key.n, 1)));
+  StrTable tb;
+  CKR(str_group(c, ar, key, nullptr, false, 0, &tb, gid));
+  CKR(iq_unique_ids(c, ar, D, gid, tb));
+  // 7. blacklistItems: each group's first list index (membership and repeats are group tests)
+  const long long G = tb.n_groups;
+  uint32_t *first_in_list;
+  CKR(ar.alloc(&first_in_list, std::max<long long>(G, 1)));
+  CK(cudaMemsetAsync(first_in_list, 0xff, sizeof(uint32_t) * (size_t)std::max<long long>(G, 1), s));
+  if (NL > 0) {
+    k_iq_black<<<grid_for(NL, 256, c->sm_count), 256, 0, s>>>(NL, D + NI, gid, first_in_list);
+    c->launches++;
+  }
+  // 8. the records' documents; the queried documents
+  int32_t *rec_doc, *rec_key;
+  uint8_t *queried;
+  CKR(ar.alloc(&rec_doc, std::max<long long>(R, 1)));
+  CKR(ar.alloc(&rec_key, std::max<long long>(R, 1)));
+  CKR(ar.alloc(&queried, std::max<long long>(D, 1)));
+  CK(cudaMemsetAsync(queried, 0, (size_t)std::max<long long>(D, 1), s));
+  if (R > 0) {
+    k_iq_rec<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, D, all, gid, tb.first_sorted, rec_doc, rec_key, queried);
+    c->launches++;
+  }
+  // 9-10. the queried documents' similar-items lists
+  IqDocs docs;
+  CKR(iq_documents(c, ar, bd, q->n_names, q->names, queried, &docs));
   // 11. the template, then a length pass, the record offsets and a write pass: one warp per record
   int32_t *d_entry;
   CKR(ar.alloc(&d_entry, q->n_names));
-  CK(cudaMemcpyAsync(d_entry, name_entry.data(), sizeof(int32_t) * (size_t)q->n_names, cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(d_entry, docs.name_entry.data(), sizeof(int32_t) * (size_t)q->n_names, cudaMemcpyHostToDevice, s));
   DevDict tp;
   CKR(upload_strings(c, ar, iq_template(q), &tp));
   IqArgs a;
@@ -5346,12 +5408,12 @@ static int item_queries(cco_ctx *c, const char *body, int64_t body_len, const cc
   a.koff = key.off;
   a.kbytes = (const unsigned char *)key.w;
   a.line_moff = bd.line_moff;
-  a.T = T;
+  a.T = docs.T;
   a.n_names = q->n_names;
   a.name_entry = d_entry;
-  a.eoff = eoff;
-  a.doff = dec.off;
-  a.dbytes = (const unsigned char *)dec.w;
+  a.eoff = docs.eoff;
+  a.doff = docs.dec.off;
+  a.dbytes = (const unsigned char *)docs.dec.w;
   a.slice = q->max_query_events;
   a.in_must = q->similar_in_must;
   a.exclude_self = q->exclude_self;
@@ -5509,6 +5571,278 @@ int cco_item_set_queries(cco_ctx_t *ctx, const cco_item_set_query_t *q, int64_t 
   if (!ctx->members.empty()) return set_error(CCO_E_UNSUPPORTED, "per-GPU contexts only");
   CKR(is_check_host(q, n_sets, set_offsets, n_elements, elem_offsets, elem_bytes));
   return item_set_queries(ctx, q, n_sets, set_offsets, elem_offsets, elem_bytes, out_body, out_len, out_offsets, out_n);
+}
+
+namespace cco {
+// the record template of a mixed query, 11 + n_history_names + n_model_names pieces: 0 head and "should":[, 1 boosted,
+// 2 should_tail, 3 must, 4 "],"must":[, 5 the ids clause up to its values, 6 the rest of the record, 7 the end of a history
+// clause, 8 the end of a similar-items clause, 9 / 10 the start / end of the set clause, 11 + j the start of query name j's
+// history clause, 11 + n_history_names + j the start of model name j's similar-items clause (see include/cco_b200.h)
+static std::vector<std::string> mq_template(const cco_mixed_query_t *q) {
+  auto end = [](bool in_must, const char *boost) {
+    return in_must ? std::string("],\"boost\":0}}") : boost ? std::string("],\"boost\":") + boost + "}}" : std::string("]}}");
+  };
+  std::vector<std::string> t(11);
+  t[0] = query_head(q->header, q->head);
+  t[1] = q->boosted;
+  t[2] = q->should_tail;
+  t[3] = q->must;
+  t[4] = "],\"must\":[";
+  t[5] = "],\"must_not\":[{\"ids\":{\"values\":[";
+  t[6] = query_tail(q->must_not, q->sort);
+  t[7] = end(q->history_in_must != 0, q->history_boost);
+  t[8] = end(q->similar_in_must != 0, q->similar_boost);
+  if (q->with_set) {
+    t[9] = "{\"terms\":{" + uq_quote(q->set_name) + ":[";
+    t[10] = end(false, q->set_boost);
+  }
+  for (int j = 0; j < q->n_history_names; ++j) t.push_back("{\"terms\":{" + uq_quote(q->names[j]) + ":[");
+  for (int j = 0; j < q->n_model_names; ++j) t.push_back("{\"terms\":{" + uq_quote(q->model_names[j]) + ":[");
+  return t;
+}
+
+// whether any of the R rows has the member: a column is given and its bitmap (nullptr: every row) has a bit set
+static bool mq_any(long long R, const int64_t *off, const uint8_t *valid) {
+  if (!off || R == 0) return false;
+  if (!valid) return true;
+  for (long long r = 0; r < R; ++r)
+    if ((valid[r >> 3] >> (r & 7)) & 1) return true;
+  return false;
+}
+
+static int mq_check_host(const cco_mixed_query_t *q, long long R, const int64_t *uoff, const char *ubytes, const int64_t *ioff,
+                         const char *ibytes, const int64_t *soff, long long n_elements, const int64_t *eoff, const char *ebytes) {
+  // the history, as uq_check_host
+  if (q->n_names < 0 || q->n_names > kUqMaxNames) return set_error(CCO_E_INVALID_ARG, "%d query event names, 0..%d", (int)q->n_names, kUqMaxNames);
+  if (q->n_names > 0 && (!q->names || (uoff && !q->limits))) return set_error(CCO_E_INVALID_ARG, "null names or limits");
+  for (int k = 0; k < q->n_names; ++k) {
+    if (!q->names[k] || !*q->names[k]) return set_error(CCO_E_INVALID_ARG, "query event name %d is null or empty", k);
+    if (uoff && q->limits[k] < 0) return set_error(CCO_E_INVALID_ARG, "query event name %d: negative limit %d", k, (int)q->limits[k]);
+  }
+  if (q->n_history_names < 0 || q->n_history_names > q->n_names)
+    return set_error(CCO_E_INVALID_ARG, "n_history_names = %d is outside [0, %d]", (int)q->n_history_names, (int)q->n_names);
+  if (q->n_blacklist_names < 0 || (q->n_blacklist_names > 0 && !q->blacklist_names)) return set_error(CCO_E_INVALID_ARG, "bad blacklist names");
+  for (int b = 0; b < q->n_blacklist_names; ++b)
+    if (!q->blacklist_names[b]) return set_error(CCO_E_INVALID_ARG, "blacklist name %d is null", b);
+  if (q->history_in_must != 0 && q->history_in_must != 1) return set_error(CCO_E_INVALID_ARG, "history_in_must must be 0 or 1");
+  // the similar items, as iq_check_host; an item column needs a model name
+  if (q->n_model_names < (ioff ? 1 : 0) || q->n_model_names > kUqMaxNames)
+    return set_error(CCO_E_INVALID_ARG, "%d model event names, %d..%d", (int)q->n_model_names, ioff ? 1 : 0, kUqMaxNames);
+  if (q->n_model_names > 0 && !q->model_names) return set_error(CCO_E_INVALID_ARG, "null names");
+  for (int k = 0; k < q->n_model_names; ++k)
+    if (!q->model_names[k] || !*q->model_names[k]) return set_error(CCO_E_INVALID_ARG, "model event name %d is null or empty", k);
+  if (q->max_query_events < 1) return set_error(CCO_E_INVALID_ARG, "max_query_events = %d, at least 1", (int)q->max_query_events);
+  if ((q->similar_in_must != 0 && q->similar_in_must != 1) || (q->exclude_self != 0 && q->exclude_self != 1))
+    return set_error(CCO_E_INVALID_ARG, "similar_in_must and exclude_self must be 0 or 1");
+  // the set clause, as is_check_host
+  if (q->with_set != 0 && q->with_set != 1) return set_error(CCO_E_INVALID_ARG, "with_set must be 0 or 1");
+  if (q->with_set && (!q->set_name || !*q->set_name)) return set_error(CCO_E_INVALID_ARG, "the set clause's name is null or empty");
+  if (!q->head || !q->boosted || !q->should_tail || !q->must || !q->must_not || !q->sort || !q->header)
+    return set_error(CCO_E_INVALID_ARG, "a null fragment");
+  CKR(str_check_host(q->n_blacklist_items, q->blacklist_item_offsets, q->blacklist_item_bytes, 0, "blacklist item"));
+  // the rows
+  if (R < 0 || n_elements < 0) return set_error(CCO_E_INVALID_ARG, "negative row or element count");
+  if (R >= 0x7fffffffLL) return set_error(CCO_E_UNSUPPORTED, "%lld rows, at most 2^31 - 2", R);
+  if (uoff) CKR(str_check_host(R, uoff, ubytes, 0, "user"));
+  if (ioff) CKR(str_check_host(R, ioff, ibytes, 0, "item"));
+  long long NE = 0;
+  if (soff) {
+    if (soff[0] < 0 || soff[0] > soff[R] || soff[R] > n_elements)
+      return set_error(CCO_E_INVALID_ARG, "set offsets [0] = %lld and [n_sets] = %lld are not within [0, n_elements = %lld] in order",
+                       (long long)soff[0], (long long)soff[R], n_elements);
+    NE = soff[R] - soff[0];
+    if (NE > 0) CKR(str_check_host(NE, eoff ? eoff + soff[0] : nullptr, ebytes, 0, "element"));
+  }
+  const long long NI = ioff ? R : 0;
+  if (NI + q->n_blacklist_items + NE >= 0x7fffffffLL)
+    return set_error(CCO_E_UNSUPPORTED, "%lld items + %lld blacklist items + %lld elements, at most 2^31 - 2", NI, (long long)q->n_blacklist_items, NE);
+  return CCO_OK;
+}
+
+static int mixed_queries(cco_ctx *c, const cco_event_log *lg, const char *body, int64_t body_len, const cco_mixed_query_t *q, long long R,
+                         const int64_t *uoff, const char *ubytes, const uint8_t *uval, const int64_t *ioff, const char *ibytes,
+                         const uint8_t *ival, const int64_t *set_off, const int64_t *eoff, const char *ebytes, const uint8_t *sval,
+                         bool any_user, char **out_body, int64_t *out_len, int64_t **out_offsets, int64_t *out_n) {
+  cudaStream_t s = c->stream;
+  CK(cudaSetDevice(c->device));
+  Arena ar(s);
+  NvtxRange nvtx("cco:mixed_queries");
+  mail_reset(c);
+  const long long NI = ioff ? R : 0, NL = q->n_blacklist_items, s0 = set_off ? set_off[0] : 0, NE = set_off ? set_off[R] - s0 : 0;
+  // 1. the documents of the index body: members, decoded names and _ids
+  BulkDocs bd;
+  if (body) CKR(bulk_parse(c, ar, body, body_len, NI + NL + NE, "items + blacklist items + elements", &bd));
+  const long long D = bd.D;
+  // 2. the users, the validity bitmaps, the set offsets 0-based and one key column of the decoded _ids, the items,
+  //    blacklistItems and the elements.  Every column's offsets are checked on the device before any kernel reads through them
+  int *bad, h_bad = 0;
+  CKR(ar.alloc(&bad, 1));
+  CK(cudaMemsetAsync(bad, 0, sizeof(int), s));
+  DevStrCol uc;
+  if (uoff) {
+    CKR(str_upload(c, ar, R, uoff, ubytes, &uc));
+    str_check_device(c, uc, bad);
+  }
+  uint8_t *d_valid[3] = {nullptr, nullptr, nullptr};
+  const uint8_t *h_valid[3] = {uval, ival, sval};
+  for (int k = 0; k < 3; ++k)
+    if (h_valid[k] && R > 0) {
+      CKR(ar.alloc(&d_valid[k], (R + 7) / 8));
+      CK(cudaMemcpyAsync(d_valid[k], h_valid[k], (size_t)(R + 7) / 8, cudaMemcpyHostToDevice, s));
+    }
+  long long *soff;
+  CKR(ar.alloc(&soff, R + 1));
+  if (set_off) {
+    long long *stmp;
+    CKR(ar.alloc(&stmp, R + 1));
+    CK(cudaMemcpyAsync(stmp, set_off, sizeof(int64_t) * ((size_t)R + 1), cudaMemcpyHostToDevice, s));
+    if (R > 0) {
+      k_str_check<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, stmp, bad);
+      c->launches++;
+    }
+    k_rebase<<<grid_for(R + 1, 256, c->sm_count), 256, 0, s>>>(R + 1, stmp, -s0, soff);
+    c->launches++;
+  } else {
+    CK(cudaMemsetAsync(soff, 0, sizeof(long long) * ((size_t)R + 1), s));
+  }
+  DevStrCol key;
+  CKR(key_column(c, ar, {KeySection{D, (const int64_t *)bd.ids.off, (const char *)bd.ids.w, true, bd.ids_bytes}, KeySection{NI, ioff, ibytes},
+                         KeySection{NL, q->blacklist_item_offsets, q->blacklist_item_bytes}, KeySection{NE, eoff ? eoff + s0 : nullptr, ebytes}},
+                     bad, &key));
+  CKR(mail_fetch(c, &h_bad, bad, 4));
+  CKR(mail_wait(c));
+  if (h_bad) return set_error(CCO_E_INVALID_ARG, "decreasing offsets in the users, the items, the sets, the elements or the blacklist items");
+  // 3. one exact grouping over the key column: _ids are unique; blacklistItems: each group's first list index
+  str_hash(c, key, ~0ULL);
+  int32_t *gid;
+  CKR(ar.alloc(&gid, std::max<long long>(key.n, 1)));
+  StrTable tb;
+  CKR(str_group(c, ar, key, nullptr, false, 0, &tb, gid));
+  CKR(iq_unique_ids(c, ar, D, gid, tb));
+  const long long G = tb.n_groups;
+  uint32_t *first_in_list;
+  CKR(ar.alloc(&first_in_list, std::max<long long>(G, 1)));
+  CK(cudaMemsetAsync(first_in_list, 0xff, sizeof(uint32_t) * (size_t)std::max<long long>(G, 1), s));
+  if (NL > 0) {
+    k_iq_black<<<grid_for(NL, 256, c->sm_count), 256, 0, s>>>(NL, D + NI, gid, first_in_list);
+    c->launches++;
+  }
+  // 4. the history, when a row has a user, and each row's user group
+  UqHistory h;
+  int32_t *rec_uid;
+  CKR(ar.alloc(&rec_uid, std::max<long long>(R, 1)));
+  if (any_user) {
+    CKR(uq_history(c, ar, lg, q->n_names, q->names, q->limits, q->n_blacklist_names, q->blacklist_names, &h));
+    CKR(uq_record_users(c, h, uc, R, rec_uid));
+  } else if (R > 0) {
+    CK(cudaMemsetAsync(rec_uid, 0xff, sizeof(int32_t) * (size_t)R, s));
+  }
+  // 5. each row's members and document; the queried documents
+  int32_t *rec_doc, *rec_key;
+  uint8_t *rec_set, *queried;
+  CKR(ar.alloc(&rec_doc, std::max<long long>(R, 1)));
+  CKR(ar.alloc(&rec_key, std::max<long long>(R, 1)));
+  CKR(ar.alloc(&rec_set, std::max<long long>(R, 1)));
+  CKR(ar.alloc(&queried, std::max<long long>(D, 1)));
+  CK(cudaMemsetAsync(queried, 0, (size_t)std::max<long long>(D, 1), s));
+  if (R > 0) {
+    k_mq_rows<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, d_valid[0], d_valid[1], d_valid[2], uoff != nullptr, ioff != nullptr,
+                                                           set_off != nullptr, D, D, gid, tb.first_sorted, rec_uid, rec_doc, rec_key,
+                                                           rec_set, queried);
+    c->launches++;
+  }
+  // 6. the queried documents' similar-items lists
+  IqDocs docs;
+  CKR(iq_documents(c, ar, bd, q->n_model_names, q->model_names, queried, &docs));
+  // 7. the items, blacklistItems and elements in the log's item table: the user's blacklist is a group test there
+  int32_t *klog;
+  CKR(ar.alloc(&klog, std::max<long long>(key.n, 1)));
+  CK(cudaMemsetAsync(klog, 0xff, sizeof(int32_t) * (size_t)std::max<long long>(key.n, 1), s));
+  if (h.E > 0 && key.n > D) {
+    k_str_lookup<<<grid_for(key.n - D, 256, c->sm_count), 256, 0, s>>>(key.n - D, key.off + D, key.base, key.w, key.hash + D, h.ti.off, h.ti.base,
+                                                                       h.ti.w, h.ti.hash, (uint64_t)h.it.cap - 1, h.it.table,
+                                                                       h.it.rank_of_slot, klog + D);
+    c->launches++;
+  }
+  // 8. each element's first occurrence within its set: the first of each run of (row, group) keys after a stable sort
+  uint8_t *first_in_set;
+  CKR(ar.alloc(&first_in_set, std::max<long long>(NE, 1)));
+  if (NE > 0) {
+    unsigned long long *k2;
+    uint32_t *p2;
+    CKR(ar.alloc(&k2, NE));
+    CKR(ar.alloc(&p2, NE));
+    CK(cudaMemsetAsync(first_in_set, 0, (size_t)NE, s));
+    k_is_keys<<<grid_for(NE, 256, c->sm_count), 256, 0, s>>>(NE, R, soff, gid + D + NI + NL, k2, p2);
+    c->launches++;
+    CKR(sort_pairs(c, ar, NE, &k2, &p2, 32 + bits_for(R)));
+    k_uq_first<<<grid_for(NE, 256, c->sm_count), 256, 0, s>>>(NE, k2, p2, first_in_set);
+    c->launches++;
+    ar.release(k2);
+    ar.release(p2);
+  }
+  // 9. the template, then a length pass, the record offsets and a write pass: one warp per row
+  int32_t *d_entry;
+  CKR(ar.alloc(&d_entry, std::max(q->n_model_names, 1)));
+  if (q->n_model_names > 0)
+    CK(cudaMemcpyAsync(d_entry, docs.name_entry.data(), sizeof(int32_t) * (size_t)q->n_model_names, cudaMemcpyHostToDevice, s));
+  DevDict tp;
+  CKR(upload_strings(c, ar, mq_template(q), &tp));
+  MqArgs a{};
+  a.n_rec = R;
+  a.rec_uid = rec_uid;
+  a.rec_doc = rec_doc;
+  a.rec_key = rec_key;
+  a.rec_set = rec_set;
+  a.h = uq_args(h, lg, q->n_names, q->n_history_names);
+  a.hist_in_must = q->history_in_must;
+  a.similar_in_must = q->similar_in_must;
+  a.exclude_self = q->exclude_self;
+  a.with_set = q->with_set;
+  a.kgid = gid;
+  a.koff = key.off;
+  a.kbytes = (const unsigned char *)key.w;
+  a.klog = klog;
+  a.line_moff = bd.line_moff;
+  a.T = docs.T;
+  a.n_names = q->n_model_names;
+  a.name_entry = d_entry;
+  a.eoff = docs.eoff;
+  a.doff = docs.dec.off;
+  a.dbytes = (const unsigned char *)docs.dec.w;
+  a.slice = q->max_query_events;
+  a.n_list = NL;
+  a.list_at = D + NI;
+  a.first_in_list = first_in_list;
+  a.soff = soff;
+  a.elem_at = D + NI + NL;
+  a.first_in_set = first_in_set;
+  a.toff = tp.off;
+  a.tbytes = tp.bytes;
+  return emit_records(c, ar, R, k_mq_record<false>, k_mq_record<true>, a, out_body, out_len, out_offsets, out_n);
+}
+}  // namespace cco
+
+int cco_mixed_queries(cco_ctx_t *ctx, const cco_event_log_t *lg, const char *index_body, int64_t index_len, const cco_mixed_query_t *q,
+                      int64_t n_rows, const int64_t *user_offsets, const char *user_bytes, const uint8_t *user_validity,
+                      const int64_t *item_offsets, const char *item_bytes, const uint8_t *item_validity, const int64_t *set_offsets,
+                      int64_t n_elements, const int64_t *elem_offsets, const char *elem_bytes, const uint8_t *set_validity, char **out_body,
+                      int64_t *out_len, int64_t **out_offsets, int64_t *out_n) {
+  if (!ctx || !q || !out_body || !out_len || !out_offsets || !out_n || index_len < 0 || (index_len > 0 && !index_body))
+    return set_error(CCO_E_INVALID_ARG, "null argument or negative length");
+  if (!ctx->members.empty()) return set_error(CCO_E_UNSUPPORTED, "per-GPU contexts only");
+  if (lg && lg->ctx != ctx) return set_error(CCO_E_INVALID_ARG, "the log was read on another context");
+  if (lg) CKR(log_state(lg, true));
+  if (index_len > 0 && index_body[index_len - 1] != '\n') return set_error(CCO_E_INVALID_ARG, "the body does not end in a newline");
+  CKR(mq_check_host(q, n_rows, user_offsets, user_bytes, item_offsets, item_bytes, set_offsets, n_elements, elem_offsets, elem_bytes));
+  const bool any_user = mq_any(n_rows, user_offsets, user_validity);
+  if (any_user && !lg) return set_error(CCO_E_INVALID_ARG, "a row has a user: its history needs a log (cco_event_log_begin_ex, CCO_LOG_KEEP_HISTORY)");
+  if (any_user && !lg->history)
+    return set_error(CCO_E_INVALID_ARG, "the log was read without history retention (cco_event_log_begin_ex, CCO_LOG_KEEP_HISTORY)");
+  if (mq_any(n_rows, item_offsets, item_validity) && !index_body)
+    return set_error(CCO_E_INVALID_ARG, "a row has an item: its similar items need an index body");
+  return mixed_queries(ctx, lg, index_body, index_len, q, n_rows, user_offsets, user_bytes, user_validity, item_offsets, item_bytes,
+                       item_validity, set_offsets, elem_offsets, elem_bytes, set_validity, any_user, out_body, out_len, out_offsets, out_n);
 }
 
 int cco_event_log_free(cco_event_log_t *lg) {

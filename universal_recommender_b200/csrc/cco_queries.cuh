@@ -574,4 +574,182 @@ __global__ void __launch_bounds__(256, 1) k_is_record(IsArgs a, const long long 
   }
 }
 
+// ---- cco_mixed_queries: buildQuery for rows with any subset of {user, item, item set} --------------------------------------
+// The history comes from cco_event_log_user_queries' stage (UqHistory), the similar items from cco_item_queries' (IqDocs).
+// One key column holds the decoded _ids, the items, blacklistItems and the set elements, grouped exactly; the items,
+// blacklistItems and elements are also probed into the log's item table, so that every test of the exclusion list
+// distinct(userBlacklisted ++ blacklistItems :+ item ++ itemSet) is a group test: the user's blacklist by uq_has,
+// blacklistItems by first_in_list, the item by group equality, earlier in the set by first_in_set.
+//   k_mq_rows      per row: which members it has (LSB-first validity bitmaps, nullptr: every row); its document; the queried
+//                  documents flagged
+//   k_mq_record    one warp per row: template pieces, history lists, similar-items lists, the set clause and the exclusion
+//                  list, a length pass and a write pass (as k_uq_record)
+__device__ __forceinline__ bool mq_valid(const uint8_t *v, long long r) { return !v || ((v[r >> 3] >> (r & 7)) & 1); }
+
+__global__ void k_mq_rows(long long R, const uint8_t *__restrict__ uvalid, const uint8_t *__restrict__ ivalid,
+                          const uint8_t *__restrict__ svalid, int has_users, int has_items, int has_sets, long long D, long long item_at,
+                          const int32_t *__restrict__ gid, const uint32_t *__restrict__ first_sorted, int32_t *__restrict__ rec_uid,
+                          int32_t *__restrict__ rec_doc, int32_t *__restrict__ rec_key, uint8_t *__restrict__ rec_set,
+                          uint8_t *__restrict__ queried) {
+  for (long long r = blockIdx.x * (long long)blockDim.x + threadIdx.x; r < R; r += (long long)gridDim.x * blockDim.x) {
+    if (!has_users || !mq_valid(uvalid, r)) rec_uid[r] = -1;
+    int32_t d = -1, k = -1;
+    if (has_items && mq_valid(ivalid, r)) {
+      k = (int32_t)(item_at + r);
+      const uint32_t f = first_sorted[gid[k]];
+      if ((long long)f < D) d = (int32_t)f;
+    }
+    rec_doc[r] = d;
+    rec_key[r] = k;
+    if (d >= 0) queried[d] = 1;
+    rec_set[r] = has_sets && mq_valid(svalid, r) ? 1 : 0;
+  }
+}
+
+struct MqArgs {
+  long long n_rec;
+  const int32_t *rec_uid;          // [n_rec] user group of the history, -1: no user or no history
+  const int32_t *rec_doc;          // [n_rec] document, -1
+  const int32_t *rec_key;          // [n_rec] key entry of the item, -1: no item
+  const uint8_t *rec_set;          // [n_rec] the row has a set
+  UqArgs h;                        // the history and the users' blacklists (h.n_list and the list members unused)
+  int hist_in_must, similar_in_must, exclude_self, with_set;
+  const int32_t *kgid;             // key column: decoded _ids, items, blacklistItems, elements; group per entry
+  const long long *koff;
+  const unsigned char *kbytes;
+  const int32_t *klog;             // per key entry: the log's item group, -1 (documents and unknown ids)
+  const long long *line_moff;      // the source of document d has members iff line_moff[2 d + 2] > line_moff[2 d + 1]
+  int T, n_names;                  // distinct model names; model names
+  const int32_t *name_entry;
+  const long long *eoff;           // [D * T + 1]
+  const long long *doff;           // decoded elements of the documents
+  const unsigned char *dbytes;
+  long long slice;                 // max_query_events
+  long long n_list, list_at;       // blacklistItems are key entries list_at + i
+  const uint32_t *first_in_list;   // per group: first list index, ~0
+  const long long *soff;           // [n_rec + 1] 0-based element index of each row's set
+  long long elem_at;               // element e is key entry elem_at + e
+  const uint8_t *first_in_set;     // [elements] the element is its string's first occurrence in its set
+  const long long *toff;           // [11 + n_kept + n_names] template pieces (see mq_template)
+  const unsigned char *tbytes;
+};
+
+template <bool WRITE>
+__global__ void __launch_bounds__(256, 1) k_mq_record(MqArgs a, const long long *__restrict__ rec_off, long long *__restrict__ rec_len,
+                                                   unsigned char *__restrict__ out) {
+  const int lane = threadIdx.x & 31;
+  const long long warps = (long long)gridDim.x * (blockDim.x >> 5);
+  for (long long r = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5; r < a.n_rec; r += warps) {
+    const int32_t u = a.rec_uid[r], d = a.rec_doc[r], key = a.rec_key[r];
+    const bool similar = d >= 0 && a.line_moff[2 * (long long)d + 2] > a.line_moff[2 * (long long)d + 1];
+    const long long e0 = a.soff[r], ne = a.rec_set[r] ? a.soff[r + 1] - e0 : 0, k0 = a.elem_at + e0;
+    const bool set_clause = a.with_set && a.rec_set[r];
+    RecordOut<WRITE> w{WRITE ? out + rec_off[r] : nullptr, 0, lane};
+    // should (must = false) or must: history, similar items, then should's boosted metadata, set clause and constant_score,
+    // or must's tail, comma-separated
+    auto section = [&](bool must) {
+      bool any = false;
+      for (int j = 0; (a.hist_in_must != 0) == must && j < a.h.n_kept; ++j) {
+        if (any) w.comma();
+        w.piece(a, 11 + j);
+        bool first = true;   // the history of name j, oldest first, each item at its first position
+        if (u >= 0) {
+          const unsigned long long s = (unsigned long long)u * a.h.nq + j;
+          const long long h0 = a.h.hstart[s], cnt = min(a.h.hstart[s + 1] - h0, (long long)a.h.limit[j]);
+          w.list(cnt, [&](long long i, const unsigned char **p, long long *len) {
+            const long long pos = h0 + cnt - 1 - i;
+            if (!a.h.keep_h[pos]) return false;
+            const uint32_t e = a.h.ent[a.h.hord[pos]];
+            *p = a.h.ibytes + a.h.ioff[e];
+            *len = a.h.ioff[e + 1] - a.h.ioff[e];
+            return true;
+          }, first);
+        }
+        w.piece(a, 7);
+        any = true;
+      }
+      for (int j = 0; similar && (a.similar_in_must != 0) == must && j < a.n_names; ++j) {
+        if (any) w.comma();
+        w.piece(a, 11 + a.h.n_kept + j);
+        const long long x = (long long)d * a.T + a.name_entry[j], x0 = a.eoff[x], n = a.eoff[x + 1] - x0;
+        bool first = true;
+        w.list(n <= a.slice ? n : a.slice - 1, [&](long long i, const unsigned char **p, long long *len) {
+          *p = a.dbytes + a.doff[x0 + i];
+          *len = a.doff[x0 + i + 1] - a.doff[x0 + i];
+          return true;
+        }, first);
+        w.piece(a, 8);
+        any = true;
+      }
+      const int tail = must ? 3 : 1;   // must's tail, or should's boosted metadata
+      if (a.toff[tail + 1] > a.toff[tail]) {
+        if (any) w.comma();
+        w.piece(a, tail);
+        any = true;
+      }
+      if (must) return;
+      if (set_clause) {   // every element as given
+        if (any) w.comma();
+        w.piece(a, 9);
+        bool first = true;
+        w.list(ne, [&](long long i, const unsigned char **p, long long *len) {
+          *p = a.kbytes + a.koff[k0 + i];
+          *len = a.koff[k0 + i + 1] - a.koff[k0 + i];
+          return true;
+        }, first);
+        w.piece(a, 10);
+        any = true;
+      }
+      if (a.toff[3] > a.toff[2]) {
+        if (any) w.comma();
+        w.piece(a, 2);
+      }
+    };
+    w.piece(a, 0);
+    section(false);
+    w.piece(a, 4);
+    section(true);
+    w.piece(a, 5);
+    // the exclusion list: the user's blacklisted items newest first, blacklistItems, the item, the set; each id once
+    auto in_user = [&](long long k) {
+      const int32_t g = a.klog[k];
+      return u >= 0 && g >= 0 && uq_has(a.h, u, g);
+    };
+    bool first = true;
+    if (u >= 0) {
+      const long long b0 = a.h.bstart[u];
+      w.list(a.h.bstart[u + 1] - b0, [&](long long i, const unsigned char **p, long long *len) {
+        if (!a.h.keep_b[b0 + i]) return false;
+        const uint32_t e = a.h.ent[a.h.bord[b0 + i]];
+        *p = a.h.ibytes + a.h.ioff[e];
+        *len = a.h.ioff[e + 1] - a.h.ioff[e];
+        return true;
+      }, first);
+    }
+    w.list(a.n_list, [&](long long i, const unsigned char **p, long long *len) {
+      const long long k = a.list_at + i;
+      if (a.first_in_list[a.kgid[k]] != (uint32_t)i || in_user(k)) return false;
+      *p = a.kbytes + a.koff[k];
+      *len = a.koff[k + 1] - a.koff[k];
+      return true;
+    }, first);
+    const bool self = a.exclude_self && key >= 0;
+    if (self && a.first_in_list[a.kgid[key]] == ~0u && !in_user(key))
+      w.list(1, [&](long long, const unsigned char **p, long long *len) {
+        *p = a.kbytes + a.koff[key];
+        *len = a.koff[key + 1] - a.koff[key];
+        return true;
+      }, first);
+    w.list(ne, [&](long long i, const unsigned char **p, long long *len) {
+      const long long k = k0 + i;
+      if (!a.first_in_set[e0 + i] || a.first_in_list[a.kgid[k]] != ~0u || (self && a.kgid[k] == a.kgid[key]) || in_user(k)) return false;
+      *p = a.kbytes + a.koff[k];
+      *len = a.koff[k + 1] - a.koff[k];
+      return true;
+    }, first);
+    w.piece(a, 6);
+    if (!WRITE && lane == 0) rec_len[r] = w.cur;
+  }
+}
+
 }  // namespace cco

@@ -579,6 +579,80 @@ class CcoContext:
                                              C.byref(ln), C.byref(off), C.byref(n)))
         return self._take_records(out, ln, off, n)
 
+    def mixed_queries(self, log: Optional["EventLog"], index_body: Optional[bytes], ap, query=None, users=None, items=None, item_sets=None,
+                      now_ms: Optional[int] = None, header: str = "{}"):
+        """cco_mixed_queries: URAlgorithm.buildQuery for rows that may each have a user, an item and an item set (ur_query.py
+        restates it).  log: read with keep_history=True (None when no row has a user); index_body: a model index bulk body
+        (None when no row has an item).  users, items: a sequence of str or None per row, or the Arrow large_string buffers
+        (offsets int64[n + 1], bytes, validity bitmap or None); item_sets: a sequence of (sequence of str) or None per row, or
+        the Arrow list<large_string> buffers (set_offsets int64[n + 1], elem_offsets, elem_bytes, validity or None).  A column
+        that is None: no row has the member.  Per-name limits are consulted exactly when users is given (ur_query.mixed_plan).
+        ap: ur_algorithm.URAlgorithmParams; query: ur_query.MixedQuery (None: defaults).
+        -> (body, offsets int64[n + 1]): `header\nquery\n` records, the _msearch body; record r = body[offsets[r]:offsets[r + 1]]."""
+        from . import ur_query as Q
+        p = Q.mixed_plan(ap, query, now_ms, with_limits=users is not None)
+        enc = lambda x: x.encode("utf-8", "surrogatepass")
+        def bitmap(present):
+            if all(present):
+                return None
+            return np.packbits(np.asarray(present, dtype=bool), bitorder="little")
+
+        def strings(col):   # -> (offsets, bytes, validity) or None
+            if col is None:
+                return None
+            if isinstance(col, tuple) and len(col) == 3 and isinstance(col[0], np.ndarray):
+                return np.ascontiguousarray(col[0], dtype=np.int64), _bytes(col[1]), None if col[2] is None else _bytes(col[2])
+            col = list(col)
+            o, b = _column(["" if x is None else x for x in col])
+            return o, b, bitmap([x is not None for x in col])
+
+        def sets(col):      # -> (set offsets, elem offsets, elem bytes, validity) or None
+            if col is None:
+                return None
+            if isinstance(col, tuple) and len(col) == 4 and isinstance(col[0], np.ndarray):
+                return (np.ascontiguousarray(col[0], dtype=np.int64), np.ascontiguousarray(col[1], dtype=np.int64), _bytes(col[2]),
+                        None if col[3] is None else _bytes(col[3]))
+            col = [None if s is None else list(s) for s in col]
+            so = np.zeros(len(col) + 1, dtype=np.int64)
+            np.cumsum([0 if s is None else len(s) for s in col], out=so[1:])
+            eo, eb = _column([x for s in col if s is not None for x in s])
+            return so, eo, eb, bitmap([s is not None for s in col])
+        uc, ic, sc = strings(users), strings(items), sets(item_sets)
+        lens = [len(c[0]) - 1 for c in (uc, ic, sc) if c is not None]
+        if any(x != lens[0] for x in lens):
+            raise ValueError("the user, item and item-set columns have different lengths")
+        n_rows = lens[0] if lens else 0
+        with_set = p.with_set
+        if p.set_name is None:
+            if sc is not None and n_rows > 0 and with_set and (sc[3] is None or np.unpackbits(sc[3], bitorder="little")[:n_rows].any()):
+                raise ValueError("an item-set query needs a model event name: the set clause's field is the first one")
+            with_set = False
+        u, it = p.user, p.item
+        names, black, model = [enc(x) for x in u.names], [enc(x) for x in u.blacklist], [enc(x) for x in it.names]
+        nm = (C.c_char_p * max(len(names), 1))(*names)
+        bl = (C.c_char_p * max(len(black), 1))(*black)
+        mn = (C.c_char_p * max(len(model), 1))(*model)
+        lim = np.ascontiguousarray(u.limits, dtype=np.int32) if u.limits else np.zeros(1, np.int32)
+        lo, lb = _column(u.blacklist_items)
+        qt = N.MixedQueryT(len(names), u.n_history, nm, lim.ctypes.data_as(C.POINTER(C.c_int32)), len(black), 1 if u.in_must else 0, bl,
+                           None if u.boost is None else u.boost.encode(), len(model), mn, it.max_query_events, 1 if it.in_must else 0,
+                           None if it.boost is None else it.boost.encode(), 1 if it.exclude_self else 0,
+                           None if p.set_name is None else enc(p.set_name), 1 if with_set else 0, None if p.set_boost is None else p.set_boost.encode(),
+                           enc(u.head), enc(u.boosted), enc(Q.CONSTANT_SCORE), enc(u.must), enc(u.must_not), enc(u.sort), enc(header),
+                           len(lo) - 1, lo.ctypes.data_as(C.POINTER(C.c_int64)), lb.ctypes.data if len(lb) else None)
+        p64 = lambda a: None if a is None else a.ctypes.data_as(C.POINTER(C.c_int64))
+        ptr = lambda a: None if a is None or len(a) == 0 else a.ctypes.data
+        empty = np.zeros(1, dtype=np.int64)
+        body = None if index_body is None else bytes(index_body)
+        out, ln, off, n = C.c_void_p(), C.c_int64(), C.c_void_p(), C.c_int64()
+        N.check(self._L.cco_mixed_queries(self._h, None if log is None else log._h, body, 0 if body is None else len(body), C.byref(qt), n_rows,
+                                          p64(uc[0]) if uc else None, ptr(uc[1]) if uc else None, ptr(uc[2]) if uc else None,
+                                          p64(ic[0]) if ic else None, ptr(ic[1]) if ic else None, ptr(ic[2]) if ic else None,
+                                          p64(sc[0]) if sc else None, len(sc[1]) - 1 if sc else 0, p64(sc[1]) if sc else p64(empty),
+                                          ptr(sc[2]) if sc else None, ptr(sc[3]) if sc else None,
+                                          C.byref(out), C.byref(ln), C.byref(off), C.byref(n)))
+        return self._take_records(out, ln, off, n)
+
     def rerank_model(self, body: bytes, properties=None, rankings=None, log=None) -> bytes:
         """cco_rerank_model: calcPop (URAlgorithm.scala:375-399, recsModel "backfill") on an existing index.  body = the
         Elasticsearch bulk body of the current model, as format_model writes it; properties and rankings as in format_model.
@@ -917,6 +991,13 @@ def _column(ids) -> tuple[np.ndarray, np.ndarray]:
     o = np.zeros(len(b) + 1, dtype=np.int64)
     np.cumsum([len(x) for x in b], out=o[1:])
     return o, np.frombuffer(b"".join(b), dtype=np.uint8)
+
+
+def _bytes(b) -> np.ndarray:
+    """a byte buffer (bytes, bytearray, memoryview or array) as a contiguous uint8 array"""
+    if isinstance(b, (bytes, bytearray, memoryview)):
+        return np.frombuffer(b, dtype=np.uint8)
+    return np.ascontiguousarray(b, dtype=np.uint8)
 
 
 def decode_ids(offsets: np.ndarray, blob: bytes) -> list[str]:

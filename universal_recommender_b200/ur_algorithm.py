@@ -5,9 +5,9 @@ calc_pop_on_device runs calcPop (recsModel "backfill") on the GPU: the current i
 fresh rankings out.  calc_all_from_events / calc_pop_from_events do the same from a PredictionIO event export parsed on the
 device (CcoContext.read_events), the DataSource included.  user_queries_from_events builds buildQuery's user queries for a
 whole user base from the same export (ur_query.py restates buildQuery); item_queries builds its item queries for every
-item of a model index body; item_set_queries builds its item-set ("shopping cart") queries for a batch of sets.  Out of
-scope: mixed queries (user, item and itemSet together), withRanks, Elasticsearch's scoring, reading the index and the HTTP
-call."""
+item of a model index body; item_set_queries builds its item-set ("shopping cart") queries for a batch of sets;
+mixed_queries_from_events builds its queries for rows with any subset of user, item and item set.  Out of scope:
+withRanks, a different template per query, Elasticsearch's scoring, reading the index and the HTTP call."""
 from __future__ import annotations
 
 import time
@@ -16,7 +16,7 @@ from typing import Optional, Sequence
 
 from .indexed_dataset import IndexedDataset
 from .similarity_analysis import CcoContext, DownsamplableCrossOccurrenceDataset, SimilarityAnalysis, default_context, encode_ids
-from .ur_query import Field, ItemQuery, ItemSetQuery, UserQuery
+from .ur_query import Field, ItemQuery, ItemSetQuery, MixedQuery, UserQuery
 from .ur_model import (RankingParams, RankingType, extract_jvalue, property_json, ranking_window, rankings_for,
                        rankings_params)
 
@@ -325,6 +325,30 @@ def user_queries_from_events(export, ap: URAlgorithmParams, query: Optional[User
     log = ctx.read_events(export, window=event_window, now_ms=now_ms, keep_history=True)
     try:
         return ctx.user_queries(log, ap, query, users, now_ms, header)
+    finally:
+        log.free()
+
+
+def mixed_queries_from_events(export, index_body: Optional[bytes], ap: URAlgorithmParams, query: Optional[MixedQuery] = None, users=None,
+                              items=None, item_sets=None, now_ms: Optional[int] = None, ctx: CcoContext | None = None, event_window=None,
+                              header: str = "{}"):
+    """buildQuery (URAlgorithm.scala:563-839) for rows that may each have a user, an item and an item set ("this user, on
+    this product page", "this user, with this cart"): the users' histories from a PredictionIO event export read on the
+    device with history retention (or an EventLog read with keep_history=True; None when no row has a user), the similar
+    items from a model index body (None when no row has an item).  One `header\nquery\n` record per row, the body of an
+    Elasticsearch _msearch.  users, items, item_sets as in CcoContext.mixed_queries: a column that is None has no member in
+    any row, a row's None has none in that row.  -> (body, offsets).  now_ms: "now" of the available / expire date filter
+    and of the eventWindow.  The fragments are ur_query.mixed_plan's."""
+    ctx = ctx or default_context()
+    now_ms = _now(now_ms)
+    from .similarity_analysis import EventLog
+    if export is None or isinstance(export, EventLog):
+        if event_window is not None:
+            raise ValueError("the eventWindow applies while an export is read")
+        return ctx.mixed_queries(export, index_body, ap, query, users, items, item_sets, now_ms, header)
+    log = ctx.read_events(export, window=event_window, now_ms=now_ms, keep_history=True)
+    try:
+        return ctx.mixed_queries(log, index_body, ap, query, users, items, item_sets, now_ms, header)
     finally:
         log.free()
 

@@ -83,7 +83,27 @@ is the host mirror over a list of sets.  Nothing is read: the set is the caller'
   * must_not ids (getExcludedItems, :741-767): distinct(blacklistItems ++ itemSet) -- the blacklist first, each once, then
     each set element not among them and not earlier in the set: a repeated element is written twice in the set clause and
     once here.
-Out of scope: mixed queries (user or item next to itemSet, :641-644), withRanks (it only changes how results are read).
+
+Mixed queries (any subset of Query.user, Query.item and Query.itemSet in one query; withRanks absent): mixed_plan()
+renders what every row's query shares (the fragments CcoContext.mixed_queries hands to the device); mixed_queries() is the
+host mirror over an event export, an index body and three columns in which an absent member is None.  buildQuery composes
+the three shapes above; quirks of the reference, kept on purpose:
+  * history (getBiasedRecentUserActions, :795-839): a row with a user gets that user's lists, exactly as a user query (the
+    per-name limits, latest first then reversed, distinct); a row without one evaluates query.user.get, the
+    NoSuchElementException is caught, and each of the first maxQueryEvents - 1 query names still writes [] -- as an
+    unknown user does.  Per-name limits are consulted exactly when the batch has a user column (mixed_plan's with_limits):
+    then a query event name without an indicatorParams entry raises KeyError, as plan() does, even for rows without a user;
+  * should (:653): the history (the algorithm's userBias >= 0), the similar items (the algorithm's itemBias >= 0; one
+    clause per model name from the item's document, sliced, none for a missing document or a {} source), the boosted
+    metadata, the set clause (the first model name, the set as given, boost = the query's itemSetBias only, dropped for 0
+    and -0.0, [] for an empty set, nothing for an absent one), constant_score;
+  * must (:703-709): the history filter (userBias < 0), the similar-items filter (itemBias < 0), the filtering metadata,
+    the date filters;
+  * must_not ids (getExcludedItems, :741-767): distinct(userBlacklisted ++ blacklistItems :+ item (unless returnSelf) ++
+    itemSet), where userBlacklisted is the items of the user's events of blacklisted query names, latest first; distinct
+    keeps each id's first position across the four sources;
+  * "ItemSets should not be mixed with user or item queries" (:641-644) is only a log line: the query is built anyway.
+Out of scope: withRanks (it only changes how results are read), a different template per query.
 """
 from __future__ import annotations
 
@@ -162,6 +182,18 @@ class ItemSetQuery(UserQuery):
     def from_json(d: dict) -> "ItemSetQuery":
         u = UserQuery.from_json(d)
         return ItemSetQuery(**{k: getattr(u, k) for k in u.__dataclass_fields__}, itemSetBias=d.get("itemSetBias"))
+
+
+@dataclass
+class MixedQuery(ItemQuery):
+    """the template members of Query (Engine.scala:32-50) for rows that may have a user, an item and an item set: the union
+    of UserQuery, ItemQuery and ItemSetQuery; the user, item and set themselves are the row's"""
+    itemSetBias: Optional[float] = None
+
+    @staticmethod
+    def from_json(d: dict) -> "MixedQuery":
+        i = ItemQuery.from_json(d)
+        return MixedQuery(**{k: getattr(i, k) for k in i.__dataclass_fields__}, itemSetBias=d.get("itemSetBias"))
 
 
 def f32(x: float) -> float:
@@ -491,6 +523,90 @@ def item_set_queries(sets: Sequence[Sequence[str]], ap, query: Optional[ItemSetQ
     """the host mirror of CcoContext.item_set_queries: one record per set, in order -> (body, offsets)"""
     p = item_set_plan(ap, query, now_ms)
     recs = [(header + "\n" + item_set_render(p, list(s)) + "\n").encode("utf-8", "surrogatepass") for s in sets]
+    offsets = np.zeros(len(recs) + 1, dtype=np.int64)
+    np.cumsum([len(r) for r in recs], out=offsets[1:])
+    return b"".join(recs), offsets
+
+
+@dataclass
+class MixedPlan:
+    """what every row of a mixed batch shares: the user-query plan (history, blacklist names, fragments), the item-query
+    plan (similar items) and the set clause"""
+    user: Plan
+    item: ItemPlan
+    set_name: Optional[str]     # the first model event name, None without one
+    with_set: bool              # itemSetBias != 0: the set clause is written for a row with a set
+    set_boost: Optional[str]    # the query's itemSetBias text, None: no "boost"
+
+
+def mixed_plan(ap, query: Optional[MixedQuery] = None, now_ms: Optional[int] = None, with_limits: bool = True) -> MixedPlan:
+    """with_limits: consult the per-name limits (indicatorParams), as plan() does; pass whether the batch has a user column,
+    so a batch without users never raises KeyError for a query event name without an entry"""
+    query = query or MixedQuery()
+    model_names = ap.model_event_names()
+    b = None if query.itemSetBias is None else f32(query.itemSetBias)
+    return MixedPlan(plan(ap, query, now_ms, with_limits), item_plan(ap, query, now_ms), model_names[0] if model_names else None,
+                     b is None or b != 0, None if b is None else java_double(b))
+
+
+def mixed_render(p: MixedPlan, hist: Sequence[Sequence[str]], similar: Sequence[str], item_set: Optional[Sequence[str]],
+                 excluded: Sequence[str]) -> str:
+    """buildQuery's document for a row with any subset of user, item and item set (URAlgorithm.scala:594-606) in json4s'
+    compact rendering: hist = the history list of each of the first n_history names, similar = the rendered similar-items
+    clauses, item_set = None for a row without a set"""
+    u, i = p.user, p.item
+    h = [terms(n, items, "0" if u.in_must else u.boost) for n, items in zip(u.names[:u.n_history], hist)]
+    if item_set is not None and p.with_set and p.set_name is None:
+        raise ValueError("an item-set query needs a model event name: the set clause's field is the first one")
+    set_clause = [terms(p.set_name, item_set, p.set_boost)] if item_set is not None and p.with_set else []
+    should = ([] if u.in_must else h) + ([] if i.in_must else list(similar)) + ([u.boosted] if u.boosted else []) + set_clause + [CONSTANT_SCORE]
+    must = (h if u.in_must else []) + (list(similar) if i.in_must else []) + ([u.must] if u.must else [])
+    must_not = ['{"ids":{"values":[' + ",".join(json_string(x) for x in excluded) + '],"boost":0}}'] + ([u.must_not] if u.must_not else [])
+    return (u.head + ',"query":{"bool":{"should":[' + ",".join(should) + '],"must":[' + ",".join(must) + '],"must_not":['
+            + ",".join(must_not) + '],"minimum_should_match":1}},"sort":' + u.sort + "}")
+
+
+def mixed_queries(events, index_body: Optional[bytes], ap, query: Optional[MixedQuery] = None, users: Optional[Sequence] = None,
+                  items: Optional[Sequence] = None, item_sets: Optional[Sequence] = None, now_ms: Optional[int] = None,
+                  header: str = "{}"):
+    """the host mirror of CcoContext.mixed_queries: one record per row -> (body, offsets).  users, items: a str or None per
+    row; item_sets: a sequence of str or None per row; a column that is None has no member in any row.  events:
+    events.read_export's output (None when no row has a user); index_body: a model index bulk body (None when no row has an
+    item)."""
+    cols = [c for c in (users, items, item_sets) if c is not None]
+    n = len(cols[0]) if cols else 0
+    if any(len(c) != n for c in cols):
+        raise ValueError("the user, item and item-set columns have different lengths")
+    p = mixed_plan(ap, query, now_ms, with_limits=users is not None)
+    by_user: dict = {}
+    if users is not None and any(x is not None for x in users):
+        if events is None:
+            raise ValueError("a row has a user: its history needs the events")
+        qn = set(p.user.names)
+        for line, (u, ev, item, t) in enumerate(events.events):
+            if ev in qn:
+                by_user.setdefault(u, []).append((t, line, ev, item))
+    by_id: dict = {}
+    if items is not None and any(x is not None for x in items):
+        if index_body is None:
+            raise ValueError("a row has an item: its similar items need an index body")
+        by_id = {i: (d, src) for d, (i, src) in enumerate(index_documents(bytes(index_body)))}
+    recs = []
+    for r in range(n):
+        u = None if users is None else users[r]
+        it = None if items is None else items[r]
+        s = None if item_sets is None or item_sets[r] is None else list(item_sets[r])
+        if u is not None:
+            recent = [(ev, item) for _, _, ev, item in sorted(by_user.get(u, []), key=lambda x: (-x[0], -x[1]))]
+            hist, black = user_history(recent, p.user)   # black = distinct(userBlacklisted ++ blacklistItems)
+        else:
+            hist, black = [[] for _ in p.user.names[:p.user.n_history]], list(p.user.blacklist_items)
+        similar = []
+        if it is not None:
+            d, src = by_id.get(it, (-1, {}))
+            similar = similar_items(p.item, d, src) if src else []
+        excluded = list(dict.fromkeys(list(black) + ([it] if it is not None and p.item.exclude_self else []) + (s or [])))
+        recs.append((header + "\n" + mixed_render(p, hist, similar, s, excluded) + "\n").encode("utf-8", "surrogatepass"))
     offsets = np.zeros(len(recs) + 1, dtype=np.int64)
     np.cumsum([len(r) for r in recs], out=offsets[1:])
     return b"".join(recs), offsets
