@@ -753,6 +753,42 @@ int cco_mixed_queries(cco_ctx_t *ctx, const cco_event_log_t *log /* nullable */,
                       int64_t *out_n);
 
 /*
+ * Batchpredict query files: one Query JSON object per line (`pio batchpredict --input`), each line with its own members.
+ * Record r of the body is line r's query, exactly what cco_mixed_queries writes for a one-row batch whose template is the
+ * line's members.
+ *  - cco_query_file_read parses the file on the device with the event reader's line split and tokenizer: lines end at '\n'
+ *    (a final one opens no line; an empty or blank line is an error), member names compare decoded, null is an absent
+ *    member, unknown members are ignored, a repeated known member is an error.  The row members are checked and decoded
+ *    there: user and item (a string), itemSet and blacklistItems (an array of strings); withRanks must be true or false and
+ *    is otherwise ignored.  The other known members (fields, dateRange, currentDate, returnSelf, num, from, eventNames,
+ *    userBias, itemBias, itemSetBias) form the line's template key: each member's raw value text in that order, '\0'
+ *    between them, an absent one empty.  Keys get template ids by first appearance.
+ *  - cco_query_file_templates hands out the T distinct keys (key t = key_bytes[key_offsets[t] .. key_offsets[t + 1])),
+ *    the first line of each and first_member_line[3 t + k], the first line of template t with a user (k = 0), an item
+ *    (k = 1) and a set (k = 2), -1 for none.  The pointers stay valid until cco_query_file_free.  The caller decodes and
+ *    type-checks each key and renders its cco_mixed_query_t (limits are required for a template with a user; its
+ *    blacklist items must be empty: the lines carry their own).
+ *  - cco_query_file_queries renders every line with its template's fragments in one length pass and one write pass:
+ *    the history is built once over the union of the query names of the templates with a user (at most 64; a name has
+ *    one limit), the user's blacklist once per distinct mask of (template names x blacklist names), and each line's
+ *    blacklistItems is its own list (each id once, at its first position across the four sources, as in
+ *    cco_mixed_queries).  The model names and max_query_events must be the same in every template.
+ * Errors name the 0-based line: CCO_E_INVALID_ARG for malformed JSON, a non-object line, a wrong type, a repeated member,
+ * a line with a user but no log with history or with an item but no index body, and everything cco_mixed_queries
+ * refuses; CCO_E_UNSUPPORTED for group contexts, 2^31 lines, lines + blacklist items + elements >= 2^31, a line or a
+ * record of 2^31 bytes and more than 64 distinct query names.  Outputs as in cco_mixed_queries.
+ */
+typedef struct cco_query_file cco_query_file_t;
+int cco_query_file_read(cco_ctx_t *ctx, const char *bytes, int64_t len, cco_query_file_t **out);
+int cco_query_file_templates(const cco_query_file_t *qf, int64_t *n_lines, int64_t *n_templates, const int64_t **key_offsets,
+                             const char **key_bytes, const int64_t **first_line, const int64_t **first_member_line);
+int cco_query_file_queries(cco_ctx_t *ctx, const cco_query_file_t *qf, const cco_event_log_t *log /* nullable */,
+                           const char *index_body /* nullable */, int64_t index_len, int64_t n_templates,
+                           const cco_mixed_query_t *templates, char **out_body, int64_t *out_len, int64_t **out_offsets,
+                           int64_t *out_n);
+int cco_query_file_free(cco_query_file_t *qf);
+
+/*
  * Debug/parity entry (tests only): full integer co-occurrence matrix A^T B of two canonical
  * binary matrices computed by the same accumulation kernel as cco_train, no LLR, no top-k.
  * Output CSR over the columns of A with ascending column ids, malloc'ed; free with cco_free.

@@ -19,6 +19,8 @@ Host-side mirror of the reference interface for this path:
                                              (cco_event_log_user_queries, cco_item_queries, cco_item_set_queries); ur_query.py
   ur_algorithm.mixed_queries_from_events  <- buildQuery for rows with any subset of {user, item, item set}, on the GPU
                                              (cco_mixed_queries); ur_query.py
+  ur_algorithm.queries_from_file          <- the same for a batchpredict query file (one Query per line, each with its own
+                                             template): read and rendered on the GPU (cco_query_file_*); ur_query.query_file
   ur_model                                <- propertiesRDD, getRanksRDD, groupAll (URAlgorithm.scala:351-369, 537-560;
                                              URModel.scala:57-140): the host mirror of the model documents
 """
@@ -31,7 +33,7 @@ from .similarity_analysis import (CcoContext, DownsamplableCrossOccurrenceDatase
                                   decode_ids, default_context, encode_ids)
 from .ur_algorithm import (DefaultURAlgoParams, IndicatorParams, URAlgorithmParams, calc_all, calc_all_from_events, calc_all_on_device,
                            calc_pop_from_events, calc_pop_on_device, item_queries, item_set_queries, mixed_queries_from_events,
-                           user_queries_from_events)
+                           queries_from_file, user_queries_from_events)
 from .ur_query import ItemQuery, ItemSetQuery, MixedQuery, UserQuery
 from .ur_model import RankingParams
 
@@ -39,7 +41,7 @@ __all__ = [
     "BiDictionary", "CcoContext", "CcoError", "CcoInvalidArgument", "DataSourceParams", "DefaultURAlgoParams", "EventWindow",
     "DownsamplableCrossOccurrenceDataset", "IndexedDataset", "IndicatorParams", "SimilarityAnalysis",
     "EventLog", "RankingParams", "URAlgorithmParams", "calc_all", "calc_all_from_events", "calc_all_on_device", "calc_pop_from_events",
-    "calc_pop_on_device", "item_queries", "item_set_queries", "mixed_queries_from_events", "user_queries_from_events", "ItemQuery", "ItemSetQuery", "MixedQuery", "UserQuery", "decode_ids", "default_context", "encode_ids", "prepare", "prepare_on_device",
+    "calc_pop_on_device", "item_queries", "item_set_queries", "mixed_queries_from_events", "queries_from_file", "user_queries_from_events", "ItemQuery", "ItemSetQuery", "MixedQuery", "UserQuery", "decode_ids", "default_context", "encode_ids", "prepare", "prepare_on_device",
     "FLAG_ASSUME_CANONICAL",
     "FLAG_ENTROPY_VARARGS", "FLAG_ROWRATE_INTDIV", "FLAG_RESULT_NO_COUNT", "FLAG_RESULT_NO_LLR", "LIB_PATH",
 ]

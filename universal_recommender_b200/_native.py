@@ -153,7 +153,7 @@ EXPORTS = [
     "cco_format_model", "cco_rerank_model", "cco_event_log_read", "cco_event_log_info", "cco_event_log_ingest",
     "cco_format_model_log", "cco_rerank_model_log", "cco_event_log_free", "cco_event_log_begin", "cco_event_log_append",
     "cco_event_log_finish", "cco_event_log_begin_window", "cco_event_log_window_stats",
-    "cco_event_log_begin_ex", "cco_event_log_user_queries", "cco_item_queries", "cco_item_set_queries", "cco_mixed_queries", "cco_result_num_matrices", "cco_result_row_range", "cco_result_matrix", "cco_result_stats", "cco_result_free",
+    "cco_event_log_begin_ex", "cco_event_log_user_queries", "cco_item_queries", "cco_item_set_queries", "cco_mixed_queries", "cco_query_file_read", "cco_query_file_templates", "cco_query_file_queries", "cco_query_file_free", "cco_result_num_matrices", "cco_result_row_range", "cco_result_matrix", "cco_result_stats", "cco_result_free",
     "cco_debug_cooccurrence", "cco_debug_downsample", "cco_debug_downsample_block", "cco_debug_llr", "cco_debug_string_ids", "cco_debug_rank_text", "cco_free",
 ]
 
@@ -221,6 +221,12 @@ def lib():
                                    p(C.c_int64), p(C.c_void_p), p(C.c_int64), p(DictionaryT)]
     L.cco_item_set_queries.argtypes = [C.c_void_p, p(ItemSetQueryT), C.c_int64, p(C.c_int64), C.c_int64, p(C.c_int64), C.c_void_p,
                                        p(C.c_void_p), p(C.c_int64), p(C.c_void_p), p(C.c_int64)]
+    L.cco_query_file_read.argtypes = [C.c_void_p, C.c_char_p, C.c_int64, p(C.c_void_p)]
+    L.cco_query_file_templates.argtypes = [C.c_void_p, p(C.c_int64), p(C.c_int64), p(p(C.c_int64)), p(C.c_void_p), p(p(C.c_int64)),
+                                           p(p(C.c_int64))]
+    L.cco_query_file_queries.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_char_p, C.c_int64, C.c_int64, p(MixedQueryT),
+                                         p(C.c_void_p), p(C.c_int64), p(C.c_void_p), p(C.c_int64)]
+    L.cco_query_file_free.argtypes = [C.c_void_p]
     L.cco_mixed_queries.argtypes = [C.c_void_p, C.c_void_p, C.c_char_p, C.c_int64, p(MixedQueryT), C.c_int64,
                                     p(C.c_int64), C.c_void_p, C.c_void_p, p(C.c_int64), C.c_void_p, C.c_void_p,
                                     p(C.c_int64), C.c_int64, p(C.c_int64), C.c_void_p, C.c_void_p,

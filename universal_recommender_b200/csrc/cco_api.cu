@@ -4908,23 +4908,28 @@ struct UqHistory {
   StrTable ut, it;
   DevStrCol tu, ti;                // the log's training user and item columns (hashed when E > 0)
   uint32_t *ent = nullptr, *hord = nullptr, *bord = nullptr, *gord = nullptr;
-  uint8_t *keep_h = nullptr, *keep_b = nullptr;
+  uint8_t *keep_h = nullptr, *keep_b = nullptr, *qr = nullptr;
   int32_t *uid = nullptr, *iid = nullptr, *d_limit = nullptr;
   long long *ln = nullptr, *hstart = nullptr, *bstart = nullptr;
   unsigned long long *bkey = nullptr;
 };
-static int uq_history(cco_ctx *c, Arena &ar, const cco_event_log *lg, int nq, const char *const *names, const int32_t *limits,
-                      int n_blacklist_names, const char *const *blacklist_names, UqHistory *h) {
-  cudaStream_t s = c->stream;
-  std::vector<int> code(nq);
+// per query name: its events are blacklisted (a blacklist name; a repeated query name reads the same events: once)
+static std::vector<uint8_t> uq_black_names(int nq, const char *const *names, int n_blacklist_names, const char *const *blacklist_names) {
   std::vector<uint8_t> black(std::max(nq, 1), 0);
   for (int k = 0; k < nq; ++k) {
-    code[k] = lg->code_of(names[k]);
-    bool earlier = false;   // a repeated query name reads the same events: blacklist them once
+    bool earlier = false;
     for (int j = 0; j < k; ++j) earlier |= strcmp(names[j], names[k]) == 0;
     for (int b = 0; b < n_blacklist_names && !earlier; ++b)
       if (strcmp(blacklist_names[b], names[k]) == 0) black[k] = 1;
   }
+  return black;
+}
+static int uq_blacklist(cco_ctx *c, Arena &ar, int nq, const std::vector<uint8_t> &black, UqHistory *h);
+static int uq_history(cco_ctx *c, Arena &ar, const cco_event_log *lg, int nq, const char *const *names, const int32_t *limits,
+                      const std::vector<uint8_t> &black, UqHistory *h) {
+  cudaStream_t s = c->stream;
+  std::vector<int> code(nq);
+  for (int k = 0; k < nq; ++k) code[k] = lg->code_of(names[k]);
   // 2. the training events of the query names, name-major
   std::vector<long long> qoff(nq + 1, 0), qbase(std::max(nq, 1), 0);
   for (int k = 0; k < nq; ++k) {
@@ -4936,24 +4941,21 @@ static int uq_history(cco_ctx *c, Arena &ar, const cco_event_log *lg, int nq, co
   if (E >= 0x7fffffffLL) return set_error(CCO_E_UNSUPPORTED, "%lld training events of the query names, at most 2^31 - 2", E);
   const long long NT = lg->train_at.back();
   h->E = E;
-  long long &G = h->G, &B = h->B;
+  long long &G = h->G;
   StrTable &ut = h->ut, &it = h->it;
   DevStrCol &tu = h->tu, &ti = h->ti;
-  uint32_t *&ent = h->ent, *&gord = h->gord, *&hord = h->hord, *&bord = h->bord;
-  uint8_t *qr = nullptr, *&keep_h = h->keep_h, *&keep_b = h->keep_b, *d_black = nullptr;
+  uint32_t *&ent = h->ent, *&gord = h->gord, *&hord = h->hord;
+  uint8_t *&qr = h->qr, *&keep_h = h->keep_h;
   int32_t *&uid = h->uid, *&iid = h->iid, *&d_limit = h->d_limit;
-  long long *tm = nullptr, *&ln = h->ln, *&hstart = h->hstart, *&bstart = h->bstart;
-  unsigned long long *&bkey = h->bkey;
+  long long *tm = nullptr, *&ln = h->ln, *&hstart = h->hstart;
   CKR(ar.alloc(&d_limit, std::max(nq, 1)));
   if (nq > 0) CK(cudaMemcpyAsync(d_limit, limits, sizeof(int32_t) * (size_t)nq, cudaMemcpyHostToDevice, s));
   if (E > 0) {
     long long *d_qoff, *d_qbase;
     CKR(ar.alloc(&d_qoff, nq + 1));
     CKR(ar.alloc(&d_qbase, nq));
-    CKR(ar.alloc(&d_black, nq));
     CK(cudaMemcpyAsync(d_qoff, qoff.data(), sizeof(long long) * (size_t)(nq + 1), cudaMemcpyHostToDevice, s));
     CK(cudaMemcpyAsync(d_qbase, qbase.data(), sizeof(long long) * (size_t)nq, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(d_black, black.data(), (size_t)nq, cudaMemcpyHostToDevice, s));
     CKR(ar.alloc(&ent, E));
     CKR(ar.alloc(&qr, E));
     k_uq_select<<<grid_for(E, 256, c->sm_count), 256, 0, s>>>(E, nq, d_qoff, d_qbase, ent, qr);
@@ -5021,10 +5023,26 @@ static int uq_history(cco_ctx *c, Arena &ar, const cco_event_log *lg, int nq, co
     c->launches++;
     ar.release(k2);
     ar.release(p2);
-    // 8. blacklist: the blacklisted names' events latest first, stably by user; each item's newest position
+  }
+  return uq_blacklist(c, ar, nq, black, h);
+}
+// 8. blacklist: the events of the names flagged in black latest first, stably by user; each item's newest position (into
+//    h's bstart, bord, keep_b, bkey, B)
+static int uq_blacklist(cco_ctx *c, Arena &ar, int nq, const std::vector<uint8_t> &black, UqHistory *h) {
+  cudaStream_t s = c->stream;
+  const long long E = h->E, G = h->G;
+  long long &B = h->B;
+  uint32_t *&bord = h->bord, *gord = h->gord;
+  uint8_t *&keep_b = h->keep_b;
+  long long *&bstart = h->bstart;
+  unsigned long long *&bkey = h->bkey;
+  if (E > 0) {
+    uint8_t *d_black;
+    CKR(ar.alloc(&d_black, nq));
+    CK(cudaMemcpyAsync(d_black, black.data(), (size_t)nq, cudaMemcpyHostToDevice, s));
     uint32_t *flag, *pos, *bidx;
     CKR(ar.alloc(&flag, E + 1));
-    k_uq_flag_black<<<grid_for(E, 256, c->sm_count), 256, 0, s>>>(E, gord, qr, d_black, flag);
+    k_uq_flag_black<<<grid_for(E, 256, c->sm_count), 256, 0, s>>>(E, gord, h->qr, d_black, flag);
     c->launches++;
     CKR(select_flagged(c, ar, E, flag, &pos, &bidx));
     uint32_t B32 = 0;
@@ -5039,13 +5057,13 @@ static int uq_history(cco_ctx *c, Arena &ar, const cco_event_log *lg, int nq, co
     CKR(ar.alloc(&bcnt, G + 1));
     CK(cudaMemsetAsync(bcnt, 0, sizeof(long long) * (size_t)(G + 1), s));
     if (B > 0) {
-      k_uq_key_user<<<grid_for(B, 256, c->sm_count), 256, 0, s>>>(B, bidx, gord, uid, bkey, bord);
+      k_uq_key_user<<<grid_for(B, 256, c->sm_count), 256, 0, s>>>(B, bidx, gord, h->uid, bkey, bord);
       c->launches++;
       CKR(sort_pairs(c, ar, B, &bkey, &bord, bits_for(G)));
       k_uq_count<<<grid_for(B, 256, c->sm_count), 256, 0, s>>>(B, bkey, bcnt);
       uint32_t *p3;
       CKR(ar.alloc(&p3, B));
-      k_uq_black_keys<<<grid_for(B, 256, c->sm_count), 256, 0, s>>>(B, bord, uid, iid, bkey, p3);
+      k_uq_black_keys<<<grid_for(B, 256, c->sm_count), 256, 0, s>>>(B, bord, h->uid, h->iid, bkey, p3);
       c->launches += 2;
       CKR(sort_pairs(c, ar, B, &bkey, &p3, 64));
       CK(cudaMemsetAsync(keep_b, 0, (size_t)B, s));
@@ -5112,7 +5130,7 @@ static int user_queries(cco_ctx *c, const cco_event_log *lg, const cco_user_quer
   if (h_bad) return set_error(CCO_E_INVALID_ARG, "decreasing offsets in the blacklist items or the users");
   // 2-8. the history
   UqHistory h;
-  CKR(uq_history(c, ar, lg, nq, q->names, q->limits, q->n_blacklist_names, q->blacklist_names, &h));
+  CKR(uq_history(c, ar, lg, nq, q->names, q->limits, uq_black_names(nq, q->names, q->n_blacklist_names, q->blacklist_names), &h));
   const long long E = h.E, G = h.G;
   const StrTable &ut = h.ut, &it = h.it;
   const DevStrCol &tu = h.tu, &ti = h.ti;
@@ -5659,85 +5677,152 @@ static int mq_check_host(const cco_mixed_query_t *q, long long R, const int64_t 
   return CCO_OK;
 }
 
-static int mixed_queries(cco_ctx *c, const cco_event_log *lg, const char *body, int64_t body_len, const cco_mixed_query_t *q, long long R,
-                         const int64_t *uoff, const char *ubytes, const uint8_t *uval, const int64_t *ioff, const char *ibytes,
-                         const uint8_t *ival, const int64_t *set_off, const int64_t *eoff, const char *ebytes, const uint8_t *sval,
-                         bool any_user, char **out_body, int64_t *out_len, int64_t **out_offsets, int64_t *out_n) {
+// The rows of a mixed batch in HBM, as the two callers stage them: cco_mixed_queries' columns (one template, one shared
+// blacklistItems list) and a query file's lines (a template and a blacklistItems list per row).
+struct MqRows {
+  long long R = 0, NI = 0, NL = 0, NE = 0;   // rows; key entries of the items (R or 0), the lists and the elements
+  std::vector<KeySection> sec;              // the items, the lists' entries, the elements (the key column after the _ids)
+  DevStrCol uc;                             // the users (uc.n = R when a user column is given)
+  bool col[3] = {false, false, false};      // a user, item, set column is given
+  const uint8_t *valid[3] = {nullptr, nullptr, nullptr};   // device LSB-first bitmaps, nullptr: every row
+  long long *soff = nullptr;                // [R + 1] 0-based element index of each row's set
+  long long *loff = nullptr;                // [lists + 1] entry index of each list
+  bool list_shared = true;                  // one list for every row, else list r is row r's
+  int32_t *rec_tpl = nullptr;               // [R] template of each row
+  std::vector<uint8_t> tpl_user;            // per template: a row with a user reads it
+};
+
+// the union of the query names of the templates a row with a user reads, their limits, each template's history names in
+// it and each distinct blacklist name mask over it (template -> mask)
+struct MqNames {
+  std::vector<const char *> names;
+  std::vector<int32_t> limits, hbeg{0}, hname, tmask;
+  std::vector<std::vector<uint8_t>> masks;
+};
+static int mq_names(const std::vector<const cco_mixed_query_t *> &tq, const std::vector<uint8_t> &tpl_user, bool single, MqNames *o) {
+  const int T = (int)tq.size();
+  auto find = [&](const char *n) {
+    for (size_t k = 0; k < o->names.size(); ++k)
+      if (strcmp(o->names[k], n) == 0) return (int)k;
+    return -1;
+  };
+  for (int t = 0; t < T; ++t) {   // the union: cco_mixed_queries keeps its names as given (a repeated one reads the same events)
+    if (!tpl_user[t]) continue;
+    const cco_mixed_query_t *q = tq[t];
+    for (int j = 0; j < q->n_names; ++j) {
+      const int x = single ? -1 : find(q->names[j]);
+      if (x >= 0) {
+        if (o->limits[x] != q->limits[j])
+          return set_error(CCO_E_INVALID_ARG, "template %d: query event name \"%s\" has limit %d, another template %d", t, q->names[j],
+                           (int)q->limits[j], (int)o->limits[x]);
+        continue;
+      }
+      if ((int)o->names.size() == kUqMaxNames)
+        return set_error(CCO_E_UNSUPPORTED, "more than %d distinct query event names over the templates with a user", kUqMaxNames);
+      o->names.push_back(q->names[j]);
+      o->limits.push_back(q->limits[j]);
+    }
+  }
+  for (int t = 0; t < T; ++t) {
+    const cco_mixed_query_t *q = tq[t];
+    for (int j = 0; j < q->n_history_names; ++j) o->hname.push_back(!tpl_user[t] ? -1 : single ? j : find(q->names[j]));
+    o->hbeg.push_back((int32_t)o->hname.size());
+  }
+  // masks: the union names that are this template's query names and blacklist names (first occurrence only)
+  const int nq = (int)o->names.size();
+  o->tmask.assign(T, 0);
+  for (int t = 0; t < T; ++t) {
+    if (!tpl_user[t]) continue;
+    const cco_mixed_query_t *q = tq[t];
+    std::vector<uint8_t> m(std::max(nq, 1), 0);
+    if (single) {
+      m = uq_black_names(q->n_names, q->names, q->n_blacklist_names, q->blacklist_names);
+    } else {
+      for (int k = 0; k < nq; ++k) {
+        bool in_q = false, in_b = false;
+        for (int j = 0; j < q->n_names && !in_q; ++j) in_q = strcmp(q->names[j], o->names[k]) == 0;
+        for (int b = 0; b < q->n_blacklist_names && !in_b; ++b) in_b = strcmp(q->blacklist_names[b], o->names[k]) == 0;
+        m[k] = in_q && in_b;
+      }
+    }
+    size_t x = 0;
+    while (x < o->masks.size() && o->masks[x] != m) ++x;
+    if (x == o->masks.size()) o->masks.push_back(m);
+    o->tmask[t] = (int32_t)x;
+  }
+  return CCO_OK;
+}
+
+// Steps shared by cco_mixed_queries (T = 1) and cco_query_file_queries: the documents, one key column (_ids, items,
+// blacklistItems, elements), the history over the union of the templates' names, each row's members, the lists' and sets'
+// first occurrences, and the records.  *bad holds the device verdict on the caller's offsets so far.
+static int mixed_render(cco_ctx *c, Arena &ar, const cco_event_log *lg, const char *body, int64_t body_len,
+                        const std::vector<const cco_mixed_query_t *> &tq, MqRows &in, int *bad, char **out_body, int64_t *out_len,
+                        int64_t **out_offsets, int64_t *out_n) {
   cudaStream_t s = c->stream;
-  CK(cudaSetDevice(c->device));
-  Arena ar(s);
-  NvtxRange nvtx("cco:mixed_queries");
-  mail_reset(c);
-  const long long NI = ioff ? R : 0, NL = q->n_blacklist_items, s0 = set_off ? set_off[0] : 0, NE = set_off ? set_off[R] - s0 : 0;
+  const long long R = in.R, NI = in.NI, NL = in.NL, NE = in.NE;
+  const cco_mixed_query_t *q0 = tq[0];
+  const int T = (int)tq.size();
+  bool any_user = false;
+  for (uint8_t x : in.tpl_user) any_user |= x != 0;
   // 1. the documents of the index body: members, decoded names and _ids
   BulkDocs bd;
   if (body) CKR(bulk_parse(c, ar, body, body_len, NI + NL + NE, "items + blacklist items + elements", &bd));
   const long long D = bd.D;
-  // 2. the users, the validity bitmaps, the set offsets 0-based and one key column of the decoded _ids, the items,
-  //    blacklistItems and the elements.  Every column's offsets are checked on the device before any kernel reads through them
-  int *bad, h_bad = 0;
-  CKR(ar.alloc(&bad, 1));
-  CK(cudaMemsetAsync(bad, 0, sizeof(int), s));
-  DevStrCol uc;
-  if (uoff) {
-    CKR(str_upload(c, ar, R, uoff, ubytes, &uc));
-    str_check_device(c, uc, bad);
-  }
-  uint8_t *d_valid[3] = {nullptr, nullptr, nullptr};
-  const uint8_t *h_valid[3] = {uval, ival, sval};
-  for (int k = 0; k < 3; ++k)
-    if (h_valid[k] && R > 0) {
-      CKR(ar.alloc(&d_valid[k], (R + 7) / 8));
-      CK(cudaMemcpyAsync(d_valid[k], h_valid[k], (size_t)(R + 7) / 8, cudaMemcpyHostToDevice, s));
-    }
-  long long *soff;
-  CKR(ar.alloc(&soff, R + 1));
-  if (set_off) {
-    long long *stmp;
-    CKR(ar.alloc(&stmp, R + 1));
-    CK(cudaMemcpyAsync(stmp, set_off, sizeof(int64_t) * ((size_t)R + 1), cudaMemcpyHostToDevice, s));
-    if (R > 0) {
-      k_str_check<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, stmp, bad);
-      c->launches++;
-    }
-    k_rebase<<<grid_for(R + 1, 256, c->sm_count), 256, 0, s>>>(R + 1, stmp, -s0, soff);
-    c->launches++;
-  } else {
-    CK(cudaMemsetAsync(soff, 0, sizeof(long long) * ((size_t)R + 1), s));
-  }
+  // 2. one key column of the decoded _ids, the items, blacklistItems and the elements
+  std::vector<KeySection> sec{KeySection{D, (const int64_t *)bd.ids.off, (const char *)bd.ids.w, true, bd.ids_bytes}};
+  sec.insert(sec.end(), in.sec.begin(), in.sec.end());
   DevStrCol key;
-  CKR(key_column(c, ar, {KeySection{D, (const int64_t *)bd.ids.off, (const char *)bd.ids.w, true, bd.ids_bytes}, KeySection{NI, ioff, ibytes},
-                         KeySection{NL, q->blacklist_item_offsets, q->blacklist_item_bytes}, KeySection{NE, eoff ? eoff + s0 : nullptr, ebytes}},
-                     bad, &key));
+  int h_bad = 0;
+  CKR(key_column(c, ar, sec, bad, &key));
   CKR(mail_fetch(c, &h_bad, bad, 4));
   CKR(mail_wait(c));
   if (h_bad) return set_error(CCO_E_INVALID_ARG, "decreasing offsets in the users, the items, the sets, the elements or the blacklist items");
-  // 3. one exact grouping over the key column: _ids are unique; blacklistItems: each group's first list index
+  // 3. one exact grouping over the key column: _ids are unique
   str_hash(c, key, ~0ULL);
   int32_t *gid;
   CKR(ar.alloc(&gid, std::max<long long>(key.n, 1)));
   StrTable tb;
   CKR(str_group(c, ar, key, nullptr, false, 0, &tb, gid));
   CKR(iq_unique_ids(c, ar, D, gid, tb));
-  const long long G = tb.n_groups;
-  uint32_t *first_in_list;
-  CKR(ar.alloc(&first_in_list, std::max<long long>(G, 1)));
-  CK(cudaMemsetAsync(first_in_list, 0xff, sizeof(uint32_t) * (size_t)std::max<long long>(G, 1), s));
+  // 4. blacklistItems: each entry's first occurrence within its list and each list's sorted (list << 32 | group) keys,
+  //    from one stable sort (membership is a search of the row's list)
+  const long long n_lists = in.list_shared ? 1 : R;
+  uint8_t *first_in_list;
+  unsigned long long *lkey;
+  CKR(ar.alloc(&first_in_list, std::max<long long>(NL, 1)));
+  CKR(ar.alloc(&lkey, std::max<long long>(NL, 1)));
   if (NL > 0) {
-    k_iq_black<<<grid_for(NL, 256, c->sm_count), 256, 0, s>>>(NL, D + NI, gid, first_in_list);
+    uint32_t *p2;
+    CKR(ar.alloc(&p2, NL));
+    CK(cudaMemsetAsync(first_in_list, 0, (size_t)NL, s));
+    k_is_keys<<<grid_for(NL, 256, c->sm_count), 256, 0, s>>>(NL, n_lists, in.loff, gid + D + NI, lkey, p2);
+    c->launches++;
+    CKR(sort_pairs(c, ar, NL, &lkey, &p2, 32 + bits_for(n_lists)));
+    k_uq_first<<<grid_for(NL, 256, c->sm_count), 256, 0, s>>>(NL, lkey, p2, first_in_list);
     c->launches++;
   }
-  // 4. the history, when a row has a user, and each row's user group
+  // 5. the history over the union of names, when a row has a user; each row's user group; one user blacklist per mask
+  MqNames nm;
+  CKR(mq_names(tq, in.tpl_user, T == 1 && in.list_shared, &nm));
+  const int nq = (int)nm.names.size();
   UqHistory h;
+  std::vector<MqBlack> hb;
   int32_t *rec_uid;
   CKR(ar.alloc(&rec_uid, std::max<long long>(R, 1)));
   if (any_user) {
-    CKR(uq_history(c, ar, lg, q->n_names, q->names, q->limits, q->n_blacklist_names, q->blacklist_names, &h));
-    CKR(uq_record_users(c, h, uc, R, rec_uid));
+    CKR(uq_history(c, ar, lg, nq, nm.names.data(), nm.limits.data(), nm.masks[0], &h));
+    hb.push_back(MqBlack{h.bstart, h.bkey, h.bord, h.keep_b});
+    for (size_t m = 1; m < nm.masks.size(); ++m) {
+      CKR(uq_blacklist(c, ar, nq, nm.masks[m], &h));
+      hb.push_back(MqBlack{h.bstart, h.bkey, h.bord, h.keep_b});
+    }
+    CKR(uq_record_users(c, h, in.uc, R, rec_uid));
   } else if (R > 0) {
     CK(cudaMemsetAsync(rec_uid, 0xff, sizeof(int32_t) * (size_t)R, s));
   }
-  // 5. each row's members and document; the queried documents
+  if (hb.empty()) hb.push_back(MqBlack{nullptr, nullptr, nullptr, nullptr});
+  // 6. each row's members and document; the queried documents
   int32_t *rec_doc, *rec_key;
   uint8_t *rec_set, *queried;
   CKR(ar.alloc(&rec_doc, std::max<long long>(R, 1)));
@@ -5746,15 +5831,14 @@ static int mixed_queries(cco_ctx *c, const cco_event_log *lg, const char *body, 
   CKR(ar.alloc(&queried, std::max<long long>(D, 1)));
   CK(cudaMemsetAsync(queried, 0, (size_t)std::max<long long>(D, 1), s));
   if (R > 0) {
-    k_mq_rows<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, d_valid[0], d_valid[1], d_valid[2], uoff != nullptr, ioff != nullptr,
-                                                           set_off != nullptr, D, D, gid, tb.first_sorted, rec_uid, rec_doc, rec_key,
-                                                           rec_set, queried);
+    k_mq_rows<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, in.valid[0], in.valid[1], in.valid[2], in.col[0], in.col[1], in.col[2], D, D,
+                                                           gid, tb.first_sorted, rec_uid, rec_doc, rec_key, rec_set, queried);
     c->launches++;
   }
-  // 6. the queried documents' similar-items lists
+  // 7. the queried documents' similar-items lists (the model names are the algorithm's: every template has the same)
   IqDocs docs;
-  CKR(iq_documents(c, ar, bd, q->n_model_names, q->model_names, queried, &docs));
-  // 7. the items, blacklistItems and elements in the log's item table: the user's blacklist is a group test there
+  CKR(iq_documents(c, ar, bd, q0->n_model_names, q0->model_names, queried, &docs));
+  // 8. the items, blacklistItems and elements in the log's item table: the user's blacklist is a group test there
   int32_t *klog;
   CKR(ar.alloc(&klog, std::max<long long>(key.n, 1)));
   CK(cudaMemsetAsync(klog, 0xff, sizeof(int32_t) * (size_t)std::max<long long>(key.n, 1), s));
@@ -5764,7 +5848,7 @@ static int mixed_queries(cco_ctx *c, const cco_event_log *lg, const char *body, 
                                                                        h.it.rank_of_slot, klog + D);
     c->launches++;
   }
-  // 8. each element's first occurrence within its set: the first of each run of (row, group) keys after a stable sort
+  // 9. each element's first occurrence within its set: the first of each run of (row, group) keys after a stable sort
   uint8_t *first_in_set;
   CKR(ar.alloc(&first_in_set, std::max<long long>(NE, 1)));
   if (NE > 0) {
@@ -5773,7 +5857,7 @@ static int mixed_queries(cco_ctx *c, const cco_event_log *lg, const char *body, 
     CKR(ar.alloc(&k2, NE));
     CKR(ar.alloc(&p2, NE));
     CK(cudaMemsetAsync(first_in_set, 0, (size_t)NE, s));
-    k_is_keys<<<grid_for(NE, 256, c->sm_count), 256, 0, s>>>(NE, R, soff, gid + D + NI + NL, k2, p2);
+    k_is_keys<<<grid_for(NE, 256, c->sm_count), 256, 0, s>>>(NE, R, in.soff, gid + D + NI + NL, k2, p2);
     c->launches++;
     CKR(sort_pairs(c, ar, NE, &k2, &p2, 32 + bits_for(R)));
     k_uq_first<<<grid_for(NE, 256, c->sm_count), 256, 0, s>>>(NE, k2, p2, first_in_set);
@@ -5781,45 +5865,134 @@ static int mixed_queries(cco_ctx *c, const cco_event_log *lg, const char *body, 
     ar.release(k2);
     ar.release(p2);
   }
-  // 9. the template, then a length pass, the record offsets and a write pass: one warp per row
-  int32_t *d_entry;
-  CKR(ar.alloc(&d_entry, std::max(q->n_model_names, 1)));
-  if (q->n_model_names > 0)
-    CK(cudaMemcpyAsync(d_entry, docs.name_entry.data(), sizeof(int32_t) * (size_t)q->n_model_names, cudaMemcpyHostToDevice, s));
+  // 10. every template's pieces and per-template arrays, then a length pass, the record offsets and a write pass: one warp
+  //     per row
+  std::vector<std::string> pieces;
+  std::vector<int32_t> tpiece(T);
+  std::vector<uint8_t> tflag(T);
+  for (int t = 0; t < T; ++t) {
+    const cco_mixed_query_t *q = tq[t];
+    tpiece[t] = (int32_t)pieces.size();
+    std::vector<std::string> p = mq_template(q);
+    pieces.insert(pieces.end(), p.begin(), p.end());
+    tflag[t] = (uint8_t)((q->history_in_must ? kMqHistInMust : 0) | (q->similar_in_must ? kMqSimilarInMust : 0) |
+                         (q->exclude_self ? kMqExcludeSelf : 0) | (q->with_set ? kMqWithSet : 0));
+  }
+  int32_t *d_entry, *d_tpiece, *d_hbeg, *d_hname, *d_tmask;
+  uint8_t *d_tflag;
+  MqBlack *d_black;
+  auto up = [&](auto **dst, const auto &v) -> int {
+    CKR(ar.alloc(dst, std::max<size_t>(v.size(), 1)));
+    if (!v.empty()) CK(cudaMemcpyAsync(*dst, v.data(), sizeof(v[0]) * v.size(), cudaMemcpyHostToDevice, s));
+    return CCO_OK;
+  };
+  CKR(up(&d_entry, docs.name_entry));
+  CKR(up(&d_tpiece, tpiece));
+  CKR(up(&d_hbeg, nm.hbeg));
+  CKR(up(&d_hname, nm.hname));
+  CKR(up(&d_tmask, nm.tmask));
+  CKR(up(&d_tflag, tflag));
+  CKR(up(&d_black, hb));
   DevDict tp;
-  CKR(upload_strings(c, ar, mq_template(q), &tp));
+  CKR(upload_strings(c, ar, pieces, &tp));   // waits for the copies above too: the host vectors are local
   MqArgs a{};
   a.n_rec = R;
   a.rec_uid = rec_uid;
   a.rec_doc = rec_doc;
   a.rec_key = rec_key;
   a.rec_set = rec_set;
-  a.h = uq_args(h, lg, q->n_names, q->n_history_names);
-  a.hist_in_must = q->history_in_must;
-  a.similar_in_must = q->similar_in_must;
-  a.exclude_self = q->exclude_self;
-  a.with_set = q->with_set;
+  a.rec_tpl = in.rec_tpl;
+  a.h = uq_args(h, lg, nq, 0);
+  a.tpiece = d_tpiece;
+  a.hbeg = d_hbeg;
+  a.hname = d_hname;
+  a.tflag = d_tflag;
+  a.tmask = d_tmask;
+  a.black = d_black;
   a.kgid = gid;
   a.koff = key.off;
   a.kbytes = (const unsigned char *)key.w;
   a.klog = klog;
   a.line_moff = bd.line_moff;
   a.T = docs.T;
-  a.n_names = q->n_model_names;
+  a.n_names = q0->n_model_names;
   a.name_entry = d_entry;
   a.eoff = docs.eoff;
   a.doff = docs.dec.off;
   a.dbytes = (const unsigned char *)docs.dec.w;
-  a.slice = q->max_query_events;
-  a.n_list = NL;
+  a.slice = q0->max_query_events;
   a.list_at = D + NI;
+  a.loff = in.loff;
+  a.list_shared = in.list_shared;
   a.first_in_list = first_in_list;
-  a.soff = soff;
+  a.lkey = lkey;
+  a.soff = in.soff;
   a.elem_at = D + NI + NL;
   a.first_in_set = first_in_set;
   a.toff = tp.off;
   a.tbytes = tp.bytes;
   return emit_records(c, ar, R, k_mq_record<false>, k_mq_record<true>, a, out_body, out_len, out_offsets, out_n);
+}
+
+static int mixed_queries(cco_ctx *c, const cco_event_log *lg, const char *body, int64_t body_len, const cco_mixed_query_t *q, long long R,
+                         const int64_t *uoff, const char *ubytes, const uint8_t *uval, const int64_t *ioff, const char *ibytes,
+                         const uint8_t *ival, const int64_t *set_off, const int64_t *eoff, const char *ebytes, const uint8_t *sval,
+                         bool any_user, char **out_body, int64_t *out_len, int64_t **out_offsets, int64_t *out_n) {
+  cudaStream_t s = c->stream;
+  CK(cudaSetDevice(c->device));
+  Arena ar(s);
+  NvtxRange nvtx("cco:mixed_queries");
+  mail_reset(c);
+  MqRows in;
+  in.R = R;
+  in.NI = ioff ? R : 0;
+  in.NL = q->n_blacklist_items;
+  const long long s0 = set_off ? set_off[0] : 0;
+  in.NE = set_off ? set_off[R] - s0 : 0;
+  // the users, the validity bitmaps, the set offsets 0-based and the one shared list; every column's offsets are checked
+  // on the device before any kernel reads through them
+  int *bad;
+  CKR(ar.alloc(&bad, 1));
+  CK(cudaMemsetAsync(bad, 0, sizeof(int), s));
+  if (uoff) {
+    CKR(str_upload(c, ar, R, uoff, ubytes, &in.uc));
+    str_check_device(c, in.uc, bad);
+  }
+  const uint8_t *h_valid[3] = {uval, ival, sval};
+  for (int k = 0; k < 3; ++k)
+    if (h_valid[k] && R > 0) {
+      uint8_t *d;
+      CKR(ar.alloc(&d, (R + 7) / 8));
+      CK(cudaMemcpyAsync(d, h_valid[k], (size_t)(R + 7) / 8, cudaMemcpyHostToDevice, s));
+      in.valid[k] = d;
+    }
+  in.col[0] = uoff != nullptr;
+  in.col[1] = ioff != nullptr;
+  in.col[2] = set_off != nullptr;
+  CKR(ar.alloc(&in.soff, R + 1));
+  if (set_off) {
+    long long *stmp;
+    CKR(ar.alloc(&stmp, R + 1));
+    CK(cudaMemcpyAsync(stmp, set_off, sizeof(int64_t) * ((size_t)R + 1), cudaMemcpyHostToDevice, s));
+    if (R > 0) {
+      k_str_check<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, stmp, bad);
+      c->launches++;
+    }
+    k_rebase<<<grid_for(R + 1, 256, c->sm_count), 256, 0, s>>>(R + 1, stmp, -s0, in.soff);
+    c->launches++;
+  } else {
+    CK(cudaMemsetAsync(in.soff, 0, sizeof(long long) * ((size_t)R + 1), s));
+  }
+  const long long lo[2] = {0, in.NL};
+  CKR(ar.alloc(&in.loff, 2));
+  CK(cudaMemcpyAsync(in.loff, lo, sizeof lo, cudaMemcpyHostToDevice, s));
+  CKR(ar.alloc(&in.rec_tpl, std::max<long long>(R, 1)));
+  CK(cudaMemsetAsync(in.rec_tpl, 0, sizeof(int32_t) * (size_t)std::max<long long>(R, 1), s));
+  in.sec = {KeySection{in.NI, ioff, ibytes}, KeySection{in.NL, q->blacklist_item_offsets, q->blacklist_item_bytes},
+            KeySection{in.NE, eoff ? eoff + s0 : nullptr, ebytes}};
+  in.tpl_user = {(uint8_t)(any_user ? 1 : 0)};
+  CK(cudaStreamSynchronize(s));   // lo is local
+  return mixed_render(c, ar, lg, body, body_len, {q}, in, bad, out_body, out_len, out_offsets, out_n);
 }
 }  // namespace cco
 
@@ -5843,6 +6016,321 @@ int cco_mixed_queries(cco_ctx_t *ctx, const cco_event_log_t *lg, const char *ind
     return set_error(CCO_E_INVALID_ARG, "a row has an item: its similar items need an index body");
   return mixed_queries(ctx, lg, index_body, index_len, q, n_rows, user_offsets, user_bytes, user_validity, item_offsets, item_bytes,
                        item_validity, set_offsets, elem_offsets, elem_bytes, set_validity, any_user, out_body, out_len, out_offsets, out_n);
+}
+
+// ---- batchpredict query files: the lines read on the device, the templates planned by the caller, the rows rendered -----
+struct cco_query_file {
+  cco_ctx *ctx = nullptr;
+  long long L = 0, NL = 0, NE = 0, rows_bytes = 0;
+  std::vector<void *> dev;
+  DevStrCol uc, rows;                  // decoded users [L]; decoded items [L], blacklistItems entries [NL], elements [NE]
+  long long *soff = nullptr, *loff = nullptr;
+  uint8_t *bits = nullptr;             // 3 LSB-first bitmaps of (L + 7) / 8 bytes: user, item, set present
+  int32_t *tid = nullptr;              // [L] template by first appearance
+  std::vector<int64_t> key_off, first_line, first_member;   // first_member: [3 T] first line with a user, item, set; -1
+  std::string key_bytes;
+};
+
+namespace cco {
+static const char *const kQfNames[kQfMembers] = {"user", "item", "itemSet", "blacklistItems", "withRanks", "fields", "dateRange",
+                                                 "currentDate", "returnSelf", "num", "from", "eventNames", "userBias", "itemBias",
+                                                 "itemSetBias"};
+static int qf_line_error(unsigned long long err) {
+  const long long line = (long long)(err >> 8);
+  switch ((unsigned)(err & 0xff)) {
+    case kJsonLongLine: return set_error(CCO_E_UNSUPPORTED, "line %lld: longer than 2^31 - 1 bytes", line);
+    case kJsonNotObject: return set_error(CCO_E_INVALID_ARG, "line %lld: not a JSON object (an empty line is not a query)", line);
+    case kJsonString:
+      return set_error(CCO_E_INVALID_ARG, "line %lld: not one JSON object (a string is unterminated or holds a bad escape or a raw byte < 0x20)", line);
+    default: return set_error(CCO_E_INVALID_ARG, "line %lld: not one JSON object", line);
+  }
+}
+static int qf_keep(Arena &ar, cco_query_file *qf, void *p) {
+  ar.take(p);
+  qf->dev.push_back(p);
+  return CCO_OK;
+}
+// the array members of every line picked in pick (-1: none) -> element spans at elem, per-line offsets eoff [L + 1]
+static int qf_arrays(cco_ctx *c, Arena &ar, long long L, const uint8_t *ones, const int32_t *pick, const JMember *mem, const unsigned char *bb,
+                     const char *what, long long **eoff, long long *n, JMember **elem) {
+  cudaStream_t s = c->stream;
+  long long *cnt;
+  unsigned long long *err, h_err = ~0ULL;
+  CKR(ar.alloc(&cnt, L + 1));
+  CKR(ar.alloc(eoff, L + 1));
+  CKR(ar.alloc(&err, 1));
+  CK(cudaMemsetAsync(cnt + L, 0, 8, s));
+  CK(cudaMemsetAsync(err, 0xff, 8, s));
+  const int grid = grid_for(L * 32, 256, c->sm_count);
+  if (L > 0) k_iq_array<false><<<grid, 256, 0, s>>>(L, 1, ones, pick, mem, bb, cnt, nullptr, nullptr, err);
+  CKR(exclusive_sum(c, ar, cnt, *eoff, L + 1));
+  CKR(mail_fetch(c, &h_err, err, 8));
+  CKR(mail_fetch(c, n, *eoff + L, 8));
+  CKR(mail_wait(c));
+  if (h_err != ~0ULL) return set_error(CCO_E_INVALID_ARG, "line %lld: \"%s\" is not an array of strings", (long long)h_err, what);
+  CKR(ar.alloc(elem, std::max<long long>(*n, 1)));
+  if (*n > 0) k_iq_array<true><<<grid, 256, 0, s>>>(L, 1, ones, pick, mem, bb, nullptr, *eoff, *elem, err);
+  c->launches += 2;
+  return CCO_OK;
+}
+static int query_file_read(cco_ctx *c, const char *bytes, int64_t len, cco_query_file *qf) {
+  cudaStream_t s = c->stream;
+  CK(cudaSetDevice(c->device));
+  Arena ar(s);
+  NvtxRange nvtx("cco:query_file_read");
+  mail_reset(c);
+  // 1. the file as 8-byte words with 16 bytes of zero padding; its lines (a final '\n' opens none)
+  const long long NW = (len + 7) / 8;
+  uint64_t *w;
+  CKR(ar.alloc(&w, NW + 2));
+  CK(cudaMemsetAsync(w + len / 8, 0, sizeof(uint64_t) * (size_t)(NW + 2 - len / 8), s));
+  if (len > 0) CK(cudaMemcpyAsync(w, bytes, (size_t)len, cudaMemcpyHostToDevice, s));
+  const unsigned char *bb = (const unsigned char *)w;
+  long long L = 0, *sb = nullptr, *se = nullptr;
+  CKR(split_lines(c, ar, w, len, len > 0 && bytes[len - 1] != '\n', &L, &sb, &se));
+  if (L >= 0x7fffffffLL) return set_error(CCO_E_UNSUPPORTED, "%lld lines, at most 2^31 - 2", L);
+  qf->L = L;
+  // 2. every line one object (the verdict before anything reads through the spans); member names decoded and matched
+  long long *moff = nullptr, M = 0;
+  JMember *mem = nullptr;
+  unsigned long long h_err = ~0ULL;
+  if (L > 0) {
+    CKR(json_members(c, ar, L, sb, se, bb, 0x7fffffffLL, &h_err, &moff, &mem, &M));
+    if (h_err != ~0ULL) return qf_line_error(h_err);
+    if (M >= 0x7fffffffLL) return set_error(CCO_E_UNSUPPORTED, "%lld members in the file, at most 2^31 - 2", M);
+  }
+  DevStrCol names;
+  long long name_bytes = 0;
+  CKR(json_decode(c, ar, M, mem, bb, &names, &name_bytes));
+  int32_t *ngid, *entry_of;
+  CKR(member_entries(c, ar, names, std::vector<std::string>(kQfNames, kQfNames + kQfMembers), &ngid, &entry_of));
+  // 3. per line: the known members, once each, null = absent; user and item are strings
+  JMember *uspan;
+  int32_t *pick_set, *pick_list, *tmem;
+  uint8_t *has, *ones;
+  unsigned long long *err;
+  const long long L1 = std::max<long long>(L, 1);
+  CKR(ar.alloc(&uspan, L1));
+  CKR(ar.alloc(&pick_set, L1));
+  CKR(ar.alloc(&pick_list, L1));
+  CKR(ar.alloc(&tmem, L1 * kQfTemplateMembers));
+  CKR(ar.alloc(&has, L1));
+  CKR(ar.alloc(&ones, L1));
+  CKR(ar.alloc(&err, 1));
+  CK(cudaMemsetAsync(ones, 1, (size_t)L1, s));
+  CK(cudaMemsetAsync(err, 0xff, 8, s));
+  // the item spans go first in the decoded row column, the list entries and the elements after them (sized below)
+  JMember *ispan;
+  CKR(ar.alloc(&ispan, L1));
+  if (L > 0) {
+    k_qf_lines<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, moff, mem, ngid, entry_of, bb, uspan, ispan, pick_set, pick_list, tmem, has, err);
+    c->launches++;
+  }
+  CKR(mail_fetch(c, &h_err, err, 8));
+  CKR(mail_wait(c));
+  if (h_err != ~0ULL) {
+    const long long line = (long long)(h_err >> 16);
+    const int t = (int)((h_err >> 8) & 0xff);
+    if ((h_err & 0xff) == kQfRepeated) return set_error(CCO_E_INVALID_ARG, "line %lld: the member \"%s\" is repeated", line, kQfNames[t]);
+    if (t == kQfWithRanks) return set_error(CCO_E_INVALID_ARG, "line %lld: \"withRanks\" is not true or false", line);
+    return set_error(CCO_E_INVALID_ARG, "line %lld: \"%s\" is not a string", line, kQfNames[t]);
+  }
+  // 4. blacklistItems and itemSet: arrays of strings, their element spans
+  JMember *lel, *sel;
+  CKR(qf_arrays(c, ar, L, ones, pick_list, mem, bb, "blacklistItems", &qf->loff, &qf->NL, &lel));
+  CKR(qf_arrays(c, ar, L, ones, pick_set, mem, bb, "itemSet", &qf->soff, &qf->NE, &sel));
+  if (L + qf->NL + qf->NE >= 0x7fffffffLL)
+    return set_error(CCO_E_UNSUPPORTED, "%lld lines + %lld blacklist items + %lld elements, at most 2^31 - 2", L, qf->NL, qf->NE);
+  // 5. the strings decoded: the users; the items, the blacklistItems entries and the elements in one column
+  JMember *rs;
+  const long long NR = L + qf->NL + qf->NE;
+  CKR(ar.alloc(&rs, std::max<long long>(NR, 1)));
+  if (L > 0) CK(cudaMemcpyAsync(rs, ispan, sizeof(JMember) * (size_t)L, cudaMemcpyDeviceToDevice, s));
+  if (qf->NL > 0) CK(cudaMemcpyAsync(rs + L, lel, sizeof(JMember) * (size_t)qf->NL, cudaMemcpyDeviceToDevice, s));
+  if (qf->NE > 0) CK(cudaMemcpyAsync(rs + L + qf->NL, sel, sizeof(JMember) * (size_t)qf->NE, cudaMemcpyDeviceToDevice, s));
+  long long ub = 0;
+  CKR(json_decode(c, ar, L, uspan, bb, &qf->uc, &ub));
+  CKR(json_decode(c, ar, NR, rs, bb, &qf->rows, &qf->rows_bytes));
+  // 6. template keys: the template members' raw spans in order, '\0' between them; template ids by first appearance
+  DevStrCol key;
+  long long *klen, total = 0;
+  CKR(ar.alloc(&klen, L + 1));
+  CKR(ar.alloc(&key.off, L + 1));
+  CKR(ar.alloc(&key.hash, L1));
+  CK(cudaMemsetAsync(klen + L, 0, 8, s));
+  if (L > 0) k_qf_key<false><<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, tmem, mem, bb, klen, nullptr, nullptr);
+  CKR(exclusive_sum(c, ar, klen, key.off, L + 1));
+  CKR(mail_fetch(c, &total, key.off + L, 8));
+  CKR(mail_wait(c));
+  CKR(ar.alloc(&key.w, (total + 16 + 7) / 8));
+  if (L > 0 && total > 0) k_qf_key<true><<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, tmem, mem, bb, nullptr, key.off, (unsigned char *)key.w);
+  c->launches += 2;
+  key.n = L;
+  str_hash(c, key, ~0ULL);
+  CKR(ar.alloc(&qf->tid, L1));
+  StrTable tb;
+  CKR(str_group(c, ar, key, nullptr, false, 0, &tb, qf->tid));
+  const long long T = tb.n_groups;
+  // 7. per template: the key, its first line, its first line with a user, an item, a set; the rows' validity bitmaps
+  long long *first, *dlen, *doff;
+  CKR(ar.alloc(&first, std::max<long long>(3 * T, 1)));
+  CKR(ar.alloc(&dlen, T + 1));
+  CKR(ar.alloc(&doff, T + 1));
+  CK(cudaMemsetAsync(first, 0xff, sizeof(long long) * (size_t)std::max<long long>(3 * T, 1), s));
+  CK(cudaMemsetAsync(dlen + T, 0, 8, s));
+  CKR(ar.alloc(&qf->bits, 3 * ((L + 7) / 8) + 1));
+  if (L > 0) {
+    k_qf_first<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, qf->tid, has, first);
+    k_qf_bits<<<grid_for((L + 7) / 8, 256, c->sm_count), 256, 0, s>>>(L, has, qf->bits);
+    k_str_dict_len<<<grid_for(T, 256, c->sm_count), 256, 0, s>>>(T, tb.first_sorted, key.off, dlen);
+    c->launches += 3;
+  }
+  CKR(exclusive_sum(c, ar, dlen, doff, T + 1));
+  qf->key_off.assign(T + 1, 0);
+  CK(cudaMemcpyAsync(qf->key_off.data(), doff, sizeof(int64_t) * (size_t)(T + 1), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  unsigned char *kb;
+  CKR(ar.alloc(&kb, std::max<long long>(qf->key_off[T], 1)));
+  if (T > 0 && qf->key_off[T] > 0) {
+    k_str_dict_gather<<<grid_for(T, 256, c->sm_count), 256, 0, s>>>(T, tb.first_sorted, key.off, key.base, (const unsigned char *)key.w, doff, kb);
+    c->launches++;
+  }
+  qf->key_bytes.resize((size_t)qf->key_off[T]);
+  std::vector<uint32_t> fs(T);
+  qf->first_member.assign(3 * T, -1);
+  if (qf->key_off[T] > 0) CK(cudaMemcpyAsync(&qf->key_bytes[0], kb, (size_t)qf->key_off[T], cudaMemcpyDeviceToHost, s));
+  if (T > 0) {
+    CK(cudaMemcpyAsync(fs.data(), tb.first_sorted, sizeof(uint32_t) * (size_t)T, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(qf->first_member.data(), first, sizeof(int64_t) * (size_t)(3 * T), cudaMemcpyDeviceToHost, s));
+  }
+  CK(cudaStreamSynchronize(s));
+  qf->first_line.assign(fs.begin(), fs.end());
+  for (void *p : {(void *)qf->uc.off, (void *)qf->uc.w, (void *)qf->uc.hash, (void *)qf->rows.off, (void *)qf->rows.w, (void *)qf->rows.hash,
+                  (void *)qf->soff, (void *)qf->loff, (void *)qf->bits, (void *)qf->tid})
+    CKR(qf_keep(ar, qf, p));
+  return CCO_OK;
+}
+
+static int query_file_queries(cco_ctx *c, const cco_query_file *qf, const cco_event_log *lg, const char *body, int64_t body_len,
+                              const std::vector<const cco_mixed_query_t *> &tq, char **out_body, int64_t *out_len, int64_t **out_offsets,
+                              int64_t *out_n) {
+  cudaStream_t s = c->stream;
+  CK(cudaSetDevice(c->device));
+  Arena ar(s);
+  NvtxRange nvtx("cco:query_file_queries");
+  mail_reset(c);
+  const long long L = qf->L, T = (long long)tq.size();
+  if (L == 0) {   // no line: an empty body
+    int64_t *ho = (int64_t *)c->pinned_get(sizeof(int64_t), /*for_result=*/false);
+    if (!ho) return set_error(CCO_E_OOM, "pinned host allocation failed");
+    ho[0] = 0;
+    const int st = body_to_host(c, s, nullptr, 0, out_body, out_len);
+    if (st != CCO_OK) {
+      c->pinned_put(ho);
+      return st;
+    }
+    *out_offsets = ho;
+    *out_n = 0;
+    return CCO_OK;
+  }
+  MqRows in;
+  in.R = L;
+  in.NI = L;
+  in.NL = qf->NL;
+  in.NE = qf->NE;
+  in.sec = {KeySection{L + qf->NL + qf->NE, (const int64_t *)qf->rows.off, (const char *)qf->rows.w, true, qf->rows_bytes}};
+  in.uc = qf->uc;
+  const long long nb = (L + 7) / 8;
+  for (int k = 0; k < 3; ++k) {
+    in.col[k] = true;
+    in.valid[k] = qf->bits + k * nb;
+  }
+  in.soff = qf->soff;
+  in.loff = qf->loff;
+  in.list_shared = false;
+  in.rec_tpl = qf->tid;
+  in.tpl_user.resize(T);
+  for (long long t = 0; t < T; ++t) in.tpl_user[t] = qf->first_member[3 * t] >= 0;
+  int *bad;
+  CKR(ar.alloc(&bad, 1));
+  CK(cudaMemsetAsync(bad, 0, sizeof(int), s));
+  return mixed_render(c, ar, lg, body, body_len, tq, in, bad, out_body, out_len, out_offsets, out_n);
+}
+}  // namespace cco
+
+int cco_query_file_read(cco_ctx_t *ctx, const char *bytes, int64_t len, cco_query_file_t **out) {
+  if (!ctx || !out || len < 0 || (len > 0 && !bytes)) return set_error(CCO_E_INVALID_ARG, "null argument or negative length");
+  if (!ctx->members.empty()) return set_error(CCO_E_UNSUPPORTED, "per-GPU contexts only");
+  *out = nullptr;
+  cco_query_file *qf = new cco_query_file();
+  qf->ctx = ctx;
+  const int st = query_file_read(ctx, bytes, len, qf);
+  if (st != CCO_OK) {
+    cco_query_file_free(qf);
+    return st;
+  }
+  *out = qf;
+  return CCO_OK;
+}
+
+int cco_query_file_templates(const cco_query_file_t *qf, int64_t *n_lines, int64_t *n_templates, const int64_t **key_offsets,
+                             const char **key_bytes, const int64_t **first_line, const int64_t **first_member_line) {
+  if (!qf || !n_lines || !n_templates || !key_offsets || !key_bytes || !first_line || !first_member_line)
+    return set_error(CCO_E_INVALID_ARG, "null argument");
+  *n_lines = qf->L;
+  *n_templates = (int64_t)qf->first_line.size();
+  *key_offsets = qf->key_off.data();
+  *key_bytes = qf->key_bytes.data();
+  *first_line = qf->first_line.data();
+  *first_member_line = qf->first_member.data();
+  return CCO_OK;
+}
+
+int cco_query_file_queries(cco_ctx_t *ctx, const cco_query_file_t *qf, const cco_event_log_t *lg, const char *index_body, int64_t index_len,
+                           int64_t n_templates, const cco_mixed_query_t *templates, char **out_body, int64_t *out_len, int64_t **out_offsets,
+                           int64_t *out_n) {
+  if (!ctx || !qf || !out_body || !out_len || !out_offsets || !out_n || index_len < 0 || (index_len > 0 && !index_body) ||
+      (n_templates > 0 && !templates))
+    return set_error(CCO_E_INVALID_ARG, "null argument or negative length");
+  if (qf->ctx != ctx) return set_error(CCO_E_INVALID_ARG, "the query file was read on another context");
+  if (lg && lg->ctx != ctx) return set_error(CCO_E_INVALID_ARG, "the log was read on another context");
+  if (lg) CKR(log_state(lg, true));
+  if (index_len > 0 && index_body[index_len - 1] != '\n') return set_error(CCO_E_INVALID_ARG, "the body does not end in a newline");
+  const long long T = (long long)qf->first_line.size();
+  if (n_templates != T) return set_error(CCO_E_INVALID_ARG, "%lld templates given, the file has %lld", (long long)n_templates, T);
+  static const int64_t zero[1] = {0};
+  std::vector<const cco_mixed_query_t *> tq;
+  long long user_line = -1, item_line = -1;
+  for (long long t = 0; t < T; ++t) {
+    const cco_mixed_query_t *q = &templates[t];
+    const long long fu = qf->first_member[3 * t], fi = qf->first_member[3 * t + 1];
+    const int st = mq_check_host(q, 0, fu >= 0 ? zero : nullptr, nullptr, fi >= 0 ? zero : nullptr, nullptr, nullptr, 0, nullptr, nullptr);
+    if (st != CCO_OK) return set_error(st, "line %lld: %s", (long long)qf->first_line[t], std::string(cco_last_error()).c_str());
+    if (q->n_blacklist_items != 0) return set_error(CCO_E_INVALID_ARG, "template %lld: blacklistItems are the lines' own", t);
+    if (q->n_model_names != templates[0].n_model_names || q->max_query_events != templates[0].max_query_events)
+      return set_error(CCO_E_INVALID_ARG, "template %lld: the model names and max_query_events are the algorithm's, the same in every template", t);
+    for (int k = 0; k < q->n_model_names; ++k)
+      if (strcmp(q->model_names[k], templates[0].model_names[k]) != 0)
+        return set_error(CCO_E_INVALID_ARG, "template %lld: the model names are the algorithm's, the same in every template", t);
+    if (fu >= 0 && (user_line < 0 || fu < user_line)) user_line = fu;
+    if (fi >= 0 && (item_line < 0 || fi < item_line)) item_line = fi;
+    tq.push_back(q);
+  }
+  if (user_line >= 0 && !lg)
+    return set_error(CCO_E_INVALID_ARG, "line %lld: a row has a user: its history needs a log (cco_event_log_begin_ex, CCO_LOG_KEEP_HISTORY)", user_line);
+  if (user_line >= 0 && !lg->history)
+    return set_error(CCO_E_INVALID_ARG, "line %lld: the log was read without history retention (cco_event_log_begin_ex, CCO_LOG_KEEP_HISTORY)", user_line);
+  if (item_line >= 0 && !index_body) return set_error(CCO_E_INVALID_ARG, "line %lld: a row has an item: its similar items need an index body", item_line);
+  return query_file_queries(ctx, qf, lg, index_body, index_len, tq, out_body, out_len, out_offsets, out_n);
+}
+
+int cco_query_file_free(cco_query_file_t *qf) {
+  if (!qf) return CCO_OK;
+  cudaSetDevice(qf->ctx->device);
+  for (void *p : qf->dev) cudaFreeAsync(p, qf->ctx->stream);
+  cudaStreamSynchronize(qf->ctx->stream);
+  delete qf;
+  return CCO_OK;
 }
 
 int cco_event_log_free(cco_event_log_t *lg) {

@@ -202,7 +202,9 @@ struct UqArgs {
   const unsigned char *tbytes;
 };
 
-__device__ __forceinline__ bool uq_has(const UqArgs &a, int32_t u, int32_t g) {
+// whether user u's blacklisted items hold item group g; B: UqArgs or MqBlack (bstart, bkey)
+template <class B>
+__device__ __forceinline__ bool uq_has(const B &a, int32_t u, int32_t g) {
   const unsigned long long x = ((unsigned long long)(uint32_t)u << 32) | (uint32_t)g;
   long long lo = a.bstart[u], hi = a.bstart[u + 1];
   while (lo < hi) {
@@ -606,14 +608,32 @@ __global__ void k_mq_rows(long long R, const uint8_t *__restrict__ uvalid, const
   }
 }
 
+// the blacklisted items of the users under one set of blacklisted query names (uq_blacklist)
+struct MqBlack {
+  const long long *bstart;         // [G + 1]
+  const unsigned long long *bkey;  // [B] (user << 32 | item), sorted
+  const uint32_t *bord;            // [B] blacklisted events in (user, time desc, line desc) order
+  const uint8_t *keep_b;           // [B] by position: the item's newest position
+};
+
+// A row reads everything that is not its own through its template tp = rec_tpl[r]: the template pieces from tpiece[tp] on
+// (see mq_template), its history names hname[hbeg[tp] .. hbeg[tp + 1]) (indices into the union of query names that the
+// history segments were built over), its flags and its user blacklist black[tmask[tp]].
+enum : uint8_t { kMqHistInMust = 1, kMqSimilarInMust = 2, kMqExcludeSelf = 4, kMqWithSet = 8 };
 struct MqArgs {
   long long n_rec;
   const int32_t *rec_uid;          // [n_rec] user group of the history, -1: no user or no history
   const int32_t *rec_doc;          // [n_rec] document, -1
   const int32_t *rec_key;          // [n_rec] key entry of the item, -1: no item
   const uint8_t *rec_set;          // [n_rec] the row has a set
-  UqArgs h;                        // the history and the users' blacklists (h.n_list and the list members unused)
-  int hist_in_must, similar_in_must, exclude_self, with_set;
+  const int32_t *rec_tpl;          // [n_rec] template
+  UqArgs h;                        // the history over the union of names (h.n_kept, the blacklist and list members unused)
+  const int32_t *tpiece;           // [T] first template piece
+  const int32_t *hbeg;             // [T + 1]
+  const int32_t *hname;            // [hbeg[T]] union name index, -1 for a template no row with a user reads
+  const uint8_t *tflag;            // [T] kMq* bits
+  const int32_t *tmask;            // [T] blacklist of the template's rows
+  const MqBlack *black;
   const int32_t *kgid;             // key column: decoded _ids, items, blacklistItems, elements; group per entry
   const long long *koff;
   const unsigned char *kbytes;
@@ -625,12 +645,15 @@ struct MqArgs {
   const long long *doff;           // decoded elements of the documents
   const unsigned char *dbytes;
   long long slice;                 // max_query_events
-  long long n_list, list_at;       // blacklistItems are key entries list_at + i
-  const uint32_t *first_in_list;   // per group: first list index, ~0
+  long long list_at;               // blacklistItems entry i is key entry list_at + i
+  const long long *loff;           // list l is entries [loff[l], loff[l + 1]); row r reads list 0 (list_shared) or r
+  int list_shared;
+  const uint8_t *first_in_list;    // [entries] the entry is its string's first occurrence in its list
+  const unsigned long long *lkey;  // [entries] (list << 32 | group), sorted: each list's groups, for membership
   const long long *soff;           // [n_rec + 1] 0-based element index of each row's set
   long long elem_at;               // element e is key entry elem_at + e
   const uint8_t *first_in_set;     // [elements] the element is its string's first occurrence in its set
-  const long long *toff;           // [11 + n_kept + n_names] template pieces (see mq_template)
+  const long long *toff;           // template pieces of every template (see mq_template)
   const unsigned char *tbytes;
 };
 
@@ -640,22 +663,25 @@ __global__ void __launch_bounds__(256, 1) k_mq_record(MqArgs a, const long long 
   const int lane = threadIdx.x & 31;
   const long long warps = (long long)gridDim.x * (blockDim.x >> 5);
   for (long long r = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5; r < a.n_rec; r += warps) {
-    const int32_t u = a.rec_uid[r], d = a.rec_doc[r], key = a.rec_key[r];
+    const int32_t u = a.rec_uid[r], d = a.rec_doc[r], key = a.rec_key[r], tp = a.rec_tpl[r];
+    const int pb = a.tpiece[tp], h0n = a.hbeg[tp], n_kept = a.hbeg[tp + 1] - h0n;
+    const unsigned fl = a.tflag[tp];
     const bool similar = d >= 0 && a.line_moff[2 * (long long)d + 2] > a.line_moff[2 * (long long)d + 1];
     const long long e0 = a.soff[r], ne = a.rec_set[r] ? a.soff[r + 1] - e0 : 0, k0 = a.elem_at + e0;
-    const bool set_clause = a.with_set && a.rec_set[r];
+    const bool set_clause = (fl & kMqWithSet) && a.rec_set[r];
     RecordOut<WRITE> w{WRITE ? out + rec_off[r] : nullptr, 0, lane};
     // should (must = false) or must: history, similar items, then should's boosted metadata, set clause and constant_score,
     // or must's tail, comma-separated
     auto section = [&](bool must) {
       bool any = false;
-      for (int j = 0; (a.hist_in_must != 0) == must && j < a.h.n_kept; ++j) {
+      for (int j = 0; ((fl & kMqHistInMust) != 0) == must && j < n_kept; ++j) {
         if (any) w.comma();
-        w.piece(a, 11 + j);
+        w.piece(a, pb + 11 + j);
         bool first = true;   // the history of name j, oldest first, each item at its first position
         if (u >= 0) {
-          const unsigned long long s = (unsigned long long)u * a.h.nq + j;
-          const long long h0 = a.h.hstart[s], cnt = min(a.h.hstart[s + 1] - h0, (long long)a.h.limit[j]);
+          const int q = a.hname[h0n + j];
+          const unsigned long long s = (unsigned long long)u * a.h.nq + q;
+          const long long h0 = a.h.hstart[s], cnt = min(a.h.hstart[s + 1] - h0, (long long)a.h.limit[q]);
           w.list(cnt, [&](long long i, const unsigned char **p, long long *len) {
             const long long pos = h0 + cnt - 1 - i;
             if (!a.h.keep_h[pos]) return false;
@@ -665,12 +691,12 @@ __global__ void __launch_bounds__(256, 1) k_mq_record(MqArgs a, const long long 
             return true;
           }, first);
         }
-        w.piece(a, 7);
+        w.piece(a, pb + 7);
         any = true;
       }
-      for (int j = 0; similar && (a.similar_in_must != 0) == must && j < a.n_names; ++j) {
+      for (int j = 0; similar && ((fl & kMqSimilarInMust) != 0) == must && j < a.n_names; ++j) {
         if (any) w.comma();
-        w.piece(a, 11 + a.h.n_kept + j);
+        w.piece(a, pb + 11 + n_kept + j);
         const long long x = (long long)d * a.T + a.name_entry[j], x0 = a.eoff[x], n = a.eoff[x + 1] - x0;
         bool first = true;
         w.list(n <= a.slice ? n : a.slice - 1, [&](long long i, const unsigned char **p, long long *len) {
@@ -678,10 +704,10 @@ __global__ void __launch_bounds__(256, 1) k_mq_record(MqArgs a, const long long 
           *len = a.doff[x0 + i + 1] - a.doff[x0 + i];
           return true;
         }, first);
-        w.piece(a, 8);
+        w.piece(a, pb + 8);
         any = true;
       }
-      const int tail = must ? 3 : 1;   // must's tail, or should's boosted metadata
+      const int tail = pb + (must ? 3 : 1);   // must's tail, or should's boosted metadata
       if (a.toff[tail + 1] > a.toff[tail]) {
         if (any) w.comma();
         w.piece(a, tail);
@@ -690,51 +716,62 @@ __global__ void __launch_bounds__(256, 1) k_mq_record(MqArgs a, const long long 
       if (must) return;
       if (set_clause) {   // every element as given
         if (any) w.comma();
-        w.piece(a, 9);
+        w.piece(a, pb + 9);
         bool first = true;
         w.list(ne, [&](long long i, const unsigned char **p, long long *len) {
           *p = a.kbytes + a.koff[k0 + i];
           *len = a.koff[k0 + i + 1] - a.koff[k0 + i];
           return true;
         }, first);
-        w.piece(a, 10);
+        w.piece(a, pb + 10);
         any = true;
       }
-      if (a.toff[3] > a.toff[2]) {
+      if (a.toff[pb + 3] > a.toff[pb + 2]) {
         if (any) w.comma();
-        w.piece(a, 2);
+        w.piece(a, pb + 2);
       }
     };
-    w.piece(a, 0);
+    w.piece(a, pb + 0);
     section(false);
-    w.piece(a, 4);
+    w.piece(a, pb + 4);
     section(true);
-    w.piece(a, 5);
+    w.piece(a, pb + 5);
     // the exclusion list: the user's blacklisted items newest first, blacklistItems, the item, the set; each id once
+    const MqBlack bl = a.black[u >= 0 ? a.tmask[tp] : 0];
     auto in_user = [&](long long k) {
       const int32_t g = a.klog[k];
-      return u >= 0 && g >= 0 && uq_has(a.h, u, g);
+      return u >= 0 && g >= 0 && uq_has(bl, u, g);
+    };
+    const long long lr = a.list_shared ? 0 : r, l0 = a.loff[lr], l1 = a.loff[lr + 1];
+    auto in_list = [&](int32_t g) {   // g is in the row's blacklistItems
+      const unsigned long long x = ((unsigned long long)lr << 32) | (uint32_t)g;
+      long long lo = l0, hi = l1;
+      while (lo < hi) {
+        const long long mid = (lo + hi) >> 1;
+        if (a.lkey[mid] < x) lo = mid + 1; else hi = mid;
+      }
+      return lo < l1 && a.lkey[lo] == x;
     };
     bool first = true;
     if (u >= 0) {
-      const long long b0 = a.h.bstart[u];
-      w.list(a.h.bstart[u + 1] - b0, [&](long long i, const unsigned char **p, long long *len) {
-        if (!a.h.keep_b[b0 + i]) return false;
-        const uint32_t e = a.h.ent[a.h.bord[b0 + i]];
+      const long long b0 = bl.bstart[u];
+      w.list(bl.bstart[u + 1] - b0, [&](long long i, const unsigned char **p, long long *len) {
+        if (!bl.keep_b[b0 + i]) return false;
+        const uint32_t e = a.h.ent[bl.bord[b0 + i]];
         *p = a.h.ibytes + a.h.ioff[e];
         *len = a.h.ioff[e + 1] - a.h.ioff[e];
         return true;
       }, first);
     }
-    w.list(a.n_list, [&](long long i, const unsigned char **p, long long *len) {
-      const long long k = a.list_at + i;
-      if (a.first_in_list[a.kgid[k]] != (uint32_t)i || in_user(k)) return false;
+    w.list(l1 - l0, [&](long long i, const unsigned char **p, long long *len) {
+      const long long k = a.list_at + l0 + i;
+      if (!a.first_in_list[l0 + i] || in_user(k)) return false;
       *p = a.kbytes + a.koff[k];
       *len = a.koff[k + 1] - a.koff[k];
       return true;
     }, first);
-    const bool self = a.exclude_self && key >= 0;
-    if (self && a.first_in_list[a.kgid[key]] == ~0u && !in_user(key))
+    const bool self = (fl & kMqExcludeSelf) && key >= 0;
+    if (self && !in_list(a.kgid[key]) && !in_user(key))
       w.list(1, [&](long long, const unsigned char **p, long long *len) {
         *p = a.kbytes + a.koff[key];
         *len = a.koff[key + 1] - a.koff[key];
@@ -742,14 +779,113 @@ __global__ void __launch_bounds__(256, 1) k_mq_record(MqArgs a, const long long 
       }, first);
     w.list(ne, [&](long long i, const unsigned char **p, long long *len) {
       const long long k = k0 + i;
-      if (!a.first_in_set[e0 + i] || a.first_in_list[a.kgid[k]] != ~0u || (self && a.kgid[k] == a.kgid[key]) || in_user(k)) return false;
+      if (!a.first_in_set[e0 + i] || (self && a.kgid[k] == a.kgid[key]) || in_list(a.kgid[k]) || in_user(k)) return false;
       *p = a.kbytes + a.koff[k];
       *len = a.koff[k + 1] - a.koff[k];
       return true;
     }, first);
-    w.piece(a, 6);
+    w.piece(a, pb + 6);
     if (!WRITE && lane == 0) rec_len[r] = w.cur;
   }
+}
+
+// ---- cco_query_file_read: the lines of a batchpredict query file (tokenized by k_json_members) ------------------------
+// Known members, by table entry (kQf*): the four row members, withRanks, then the template members in their fixed order.
+//   k_qf_lines     one thread per line: each known member once, null = absent; user / item must be one string (its inside
+//                  becomes a span for the decoder), itemSet / blacklistItems are picked for k_iq_array, withRanks must be
+//                  true / false; the template members' raw value spans
+//   k_qf_key<>     the template key of each line: the raw spans of the template members in order, separated by '\0' (an
+//                  absent member leaves its place empty), a length pass and a write pass
+//   k_qf_bits      per-line member flags -> LSB-first validity bitmaps (for k_mq_rows)
+//   k_qf_first     per template: its first line with a user, with an item and with a set
+enum : int { kQfUser = 0, kQfItem, kQfItemSet, kQfBlacklistItems, kQfWithRanks, kQfTemplate0 };
+constexpr int kQfTemplateMembers = 10, kQfMembers = kQfTemplate0 + kQfTemplateMembers;
+enum : unsigned { kQfRepeated = 16, kQfType = 17 };   // error codes next to the tokenizer's; the member entry rides in bits 8..15
+
+__device__ __forceinline__ bool qf_literal(const unsigned char *b, const JMember &m, const char *lit, int n) {
+  if (m.ve - m.vb != n) return false;
+  for (int k = 0; k < n; ++k)
+    if (b[m.vb + k] != (unsigned char)lit[k]) return false;
+  return true;
+}
+__global__ void k_qf_lines(long long L, const long long *__restrict__ moff, const JMember *__restrict__ mem, const int32_t *__restrict__ ngid,
+                           const int32_t *__restrict__ entry_of, const unsigned char *__restrict__ body, JMember *__restrict__ uspan,
+                           JMember *__restrict__ ispan, int32_t *__restrict__ pick_set, int32_t *__restrict__ pick_list,
+                           int32_t *__restrict__ tmem, uint8_t *__restrict__ has, unsigned long long *__restrict__ err) {
+  for (long long l = blockIdx.x * (long long)blockDim.x + threadIdx.x; l < L; l += (long long)gridDim.x * blockDim.x) {
+    int32_t at[kQfMembers];
+    for (int t = 0; t < kQfMembers; ++t) at[t] = -1;
+    unsigned seen = 0, code = 0, bad_t = 0;
+    for (long long m = moff[l]; m < moff[l + 1] && !code; ++m) {
+      const int32_t t = entry_of[ngid[m]];
+      if (t < 0) continue;
+      if ((seen >> t) & 1) {
+        code = kQfRepeated;
+        bad_t = t;
+      }
+      seen |= 1u << t;
+      if (!qf_literal(body, mem[m], "null", 4)) at[t] = (int32_t)m;
+    }
+    for (int t = 0; t < 2 && !code; ++t) {   // user, item: one string
+      const int32_t m = at[t];
+      if (m < 0) continue;
+      const long long b = mem[m].vb, e = mem[m].ve - 1;
+      bool ok = body[b] == '"' && e > b && body[e] == '"';
+      long long q = b + 1;
+      while (ok && q < e) {
+        if (body[q] == '\\') q += 2;
+        else if (body[q] == '"') ok = false;
+        else ++q;
+      }
+      ok = ok && q == e;
+      if (!ok) {
+        code = kQfType;
+        bad_t = t;
+      }
+    }
+    if (!code && at[kQfWithRanks] >= 0 && !qf_literal(body, mem[at[kQfWithRanks]], "true", 4) && !qf_literal(body, mem[at[kQfWithRanks]], "false", 5)) {
+      code = kQfType;
+      bad_t = kQfWithRanks;
+    }
+    if (code) atomicMin(err, ((unsigned long long)l << 16) | (bad_t << 8) | code);
+    uspan[l] = at[kQfUser] >= 0 ? JMember{mem[at[kQfUser]].vb + 1, mem[at[kQfUser]].ve - 1, 0, 0} : JMember{0, 0, 0, 0};
+    ispan[l] = at[kQfItem] >= 0 ? JMember{mem[at[kQfItem]].vb + 1, mem[at[kQfItem]].ve - 1, 0, 0} : JMember{0, 0, 0, 0};
+    pick_set[l] = at[kQfItemSet];
+    pick_list[l] = at[kQfBlacklistItems];
+    for (int k = 0; k < kQfTemplateMembers; ++k) tmem[l * kQfTemplateMembers + k] = at[kQfTemplate0 + k];
+    has[l] = (at[kQfUser] >= 0 ? 1 : 0) | (at[kQfItem] >= 0 ? 2 : 0) | (at[kQfItemSet] >= 0 ? 4 : 0);
+  }
+}
+template <bool kWrite>
+__global__ void k_qf_key(long long L, const int32_t *__restrict__ tmem, const JMember *__restrict__ mem, const unsigned char *__restrict__ body,
+                         long long *__restrict__ len, const long long *__restrict__ off, unsigned char *__restrict__ out) {
+  for (long long l = blockIdx.x * (long long)blockDim.x + threadIdx.x; l < L; l += (long long)gridDim.x * blockDim.x) {
+    long long k = kWrite ? off[l] : 0;
+    for (int t = 0; t < kQfTemplateMembers; ++t) {
+      if (t) {
+        if (kWrite) out[k] = 0;
+        ++k;
+      }
+      const int32_t m = tmem[l * kQfTemplateMembers + t];
+      if (m < 0) continue;
+      for (long long p = mem[m].vb; p < mem[m].ve; ++p, ++k)
+        if (kWrite) out[k] = body[p];
+    }
+    if (!kWrite) len[l] = k;
+  }
+}
+__global__ void k_qf_bits(long long L, const uint8_t *__restrict__ has, uint8_t *__restrict__ bits) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < (L + 7) / 8; i += (long long)gridDim.x * blockDim.x)
+    for (int b = 0; b < 3; ++b) {
+      unsigned v = 0;
+      for (int j = 0; j < 8 && i * 8 + j < L; ++j) v |= (unsigned)((has[i * 8 + j] >> b) & 1) << j;
+      bits[b * ((L + 7) / 8) + i] = (uint8_t)v;
+    }
+}
+__global__ void k_qf_first(long long L, const int32_t *__restrict__ tid, const uint8_t *__restrict__ has, long long *__restrict__ first) {
+  for (long long l = blockIdx.x * (long long)blockDim.x + threadIdx.x; l < L; l += (long long)gridDim.x * blockDim.x)
+    for (int b = 0; b < 3; ++b)
+      if ((has[l] >> b) & 1) atomicMin((unsigned long long *)&first[3 * (long long)tid[l] + b], (unsigned long long)l);
 }
 
 }  // namespace cco

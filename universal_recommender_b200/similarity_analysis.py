@@ -653,6 +653,84 @@ class CcoContext:
                                           C.byref(out), C.byref(ln), C.byref(off), C.byref(n)))
         return self._take_records(out, ln, off, n)
 
+    def query_file(self, log: Optional["EventLog"], index_body: Optional[bytes], ap, lines, now_ms: Optional[int] = None,
+                   header: str = "{}", timings: Optional[dict] = None):
+        """URAlgorithm.buildQuery for every line of a batchpredict query file (one Query JSON object per line, each with its
+        own members; ur_query.parse_query_line lists the extraction rules).  lines: the file's bytes (or a buffer), or a
+        path.  log: read with keep_history=True (None when no line has a user); index_body: a model index bulk body (None
+        when no line has an item).  The file is read on the device (cco_query_file_read: the lines, their row members and
+        a template id per line); each distinct template is decoded and planned here (ur_query.mixed_plan, O(templates)
+        host work); every line is rendered on the device in one pass (cco_query_file_queries).  Errors name the 0-based
+        line.  timings: a dict that gets the wall-clock ms of the read, the plans and the render ("read_ms", "plans_ms",
+        "render_ms"); each native step returns after its device work.
+        -> (body, offsets int64[n_lines + 1]): record r, body[offsets[r]:offsets[r + 1]], is line r's."""
+        from . import ur_query as Q
+        if isinstance(lines, (str, os.PathLike)):
+            with open(lines, "rb") as f:
+                lines = f.read()
+        data = bytes(lines)
+        qf = C.c_void_p()
+        clock = [time.perf_counter()]
+        def lap(name):
+            now = time.perf_counter()
+            if timings is not None:
+                timings[name] = (now - clock[0]) * 1e3
+            clock[0] = now
+        N.check(self._L.cco_query_file_read(self._h, data, len(data), C.byref(qf)))
+        lap("read_ms")
+        try:
+            n_lines, T = C.c_int64(), C.c_int64()
+            ko, kb, fl, fm = C.POINTER(C.c_int64)(), C.c_void_p(), C.POINTER(C.c_int64)(), C.POINTER(C.c_int64)()
+            N.check(self._L.cco_query_file_templates(qf, C.byref(n_lines), C.byref(T), C.byref(ko), C.byref(kb), C.byref(fl), C.byref(fm)))
+            T = T.value
+            koff = np.ctypeslib.as_array(ko, shape=(T + 1,)).copy() if T else np.zeros(1, np.int64)
+            keys = C.string_at(kb.value, int(koff[-1])) if koff[-1] else b""
+            first = np.ctypeslib.as_array(fl, shape=(T,)).copy() if T else np.zeros(0, np.int64)
+            fmem = np.ctypeslib.as_array(fm, shape=(3 * T,)).copy().reshape(T, 3) if T else np.zeros((0, 3), np.int64)
+            # every template decoded and planned; the error of the earliest line wins, as line by line
+            errs, plans = [], []
+            for t in range(T):
+                try:
+                    q = Q.template_from_key(keys[koff[t]:koff[t + 1]], int(first[t]))
+                except ValueError as e:
+                    errs.append((int(first[t]), e))
+                    plans.append(None)
+                    continue
+                fu, fi, fs = (int(x) for x in fmem[t])
+                try:
+                    p = Q.mixed_plan(ap, q, now_ms, with_limits=fu >= 0)
+                except KeyError as e:
+                    errs.append((fu, ValueError(f"line {fu}: {e.args[0]}")))
+                    plans.append(None)
+                    continue
+                except ValueError as e:
+                    errs.append((int(first[t]), ValueError(f"line {int(first[t])}: {e}")))
+                    plans.append(None)
+                    continue
+                if fu >= 0 and log is None:
+                    errs.append((fu, ValueError(f"line {fu}: a row has a user: its history needs the events")))
+                if fi >= 0 and index_body is None:
+                    errs.append((fi, ValueError(f"line {fi}: a row has an item: its similar items need an index body")))
+                if fs >= 0 and p.with_set and p.set_name is None:
+                    errs.append((fs, ValueError(f"line {fs}: an item-set query needs a model event name: the set clause's field is the first one")))
+                plans.append(p)
+            if errs:
+                raise min(errs, key=lambda x: x[0])[1]
+            keep = []
+            qts = (N.MixedQueryT * max(T, 1))()
+            for t, p in enumerate(plans):
+                qts[t] = _mixed_query_t(p, fmem[t][2] >= 0, header, keep)
+            body = None if index_body is None else bytes(index_body)
+            lap("plans_ms")
+            out, ln, off, n = C.c_void_p(), C.c_int64(), C.c_void_p(), C.c_int64()
+            N.check(self._L.cco_query_file_queries(self._h, qf, None if log is None else log._h, body, 0 if body is None else len(body), T, qts,
+                                                   C.byref(out), C.byref(ln), C.byref(off), C.byref(n)))
+            records = self._take_records(out, ln, off, n)
+            lap("render_ms")
+            return records
+        finally:
+            self._L.cco_query_file_free(qf)
+
     def rerank_model(self, body: bytes, properties=None, rankings=None, log=None) -> bytes:
         """cco_rerank_model: calcPop (URAlgorithm.scala:375-399, recsModel "backfill") on an existing index.  body = the
         Elasticsearch bulk body of the current model, as format_model writes it; properties and rankings as in format_model.
@@ -983,6 +1061,27 @@ def encode_ids(ids: Sequence[str]) -> tuple[np.ndarray, np.ndarray]:
     off = np.zeros(len(ids) + 1, dtype=np.int64)
     np.cumsum(lens, out=off[1:])
     return off, np.frombuffer(blob, dtype=np.uint8)
+
+
+def _mixed_query_t(p, with_rows_sets: bool, header: str, keep: list):
+    """a ur_query.MixedPlan as cco_mixed_query_t, without blacklist items (a query file's lines carry their own); the
+    buffers it points into go to keep"""
+    from . import ur_query as Q
+    enc = lambda x: x.encode("utf-8", "surrogatepass")
+    u, it = p.user, p.item
+    names, black, model = [enc(x) for x in u.names], [enc(x) for x in u.blacklist], [enc(x) for x in it.names]
+    nm = (C.c_char_p * max(len(names), 1))(*names)
+    bl = (C.c_char_p * max(len(black), 1))(*black)
+    mn = (C.c_char_p * max(len(model), 1))(*model)
+    lim = np.ascontiguousarray(u.limits, dtype=np.int32) if u.limits else np.zeros(1, np.int32)
+    with_set = p.with_set and p.set_name is not None
+    strs = [None if u.boost is None else u.boost.encode(), None if it.boost is None else it.boost.encode(),
+            None if p.set_name is None else enc(p.set_name), None if p.set_boost is None else p.set_boost.encode(), enc(u.head),
+            enc(u.boosted), enc(Q.CONSTANT_SCORE), enc(u.must), enc(u.must_not), enc(u.sort), enc(header)]
+    keep += [names, black, model, nm, bl, mn, lim, strs]
+    return N.MixedQueryT(len(names), u.n_history, nm, lim.ctypes.data_as(C.POINTER(C.c_int32)), len(black), 1 if u.in_must else 0, bl,
+                         strs[0], len(model), mn, it.max_query_events, 1 if it.in_must else 0, strs[1], 1 if it.exclude_self else 0,
+                         strs[2], 1 if with_set else 0, strs[3], *strs[4:], 0, None, None)
 
 
 def _column(ids) -> tuple[np.ndarray, np.ndarray]:

@@ -6,8 +6,9 @@ fresh rankings out.  calc_all_from_events / calc_pop_from_events do the same fro
 device (CcoContext.read_events), the DataSource included.  user_queries_from_events builds buildQuery's user queries for a
 whole user base from the same export (ur_query.py restates buildQuery); item_queries builds its item queries for every
 item of a model index body; item_set_queries builds its item-set ("shopping cart") queries for a batch of sets;
-mixed_queries_from_events builds its queries for rows with any subset of user, item and item set.  Out of scope:
-withRanks, a different template per query, Elasticsearch's scoring, reading the index and the HTTP call."""
+mixed_queries_from_events builds its queries for rows with any subset of user, item and item set; queries_from_file
+builds them for a batchpredict query file, each line with its own template.  Out of scope: withRanks, Elasticsearch's
+scoring, reading the index and the HTTP call."""
 from __future__ import annotations
 
 import time
@@ -349,6 +350,27 @@ def mixed_queries_from_events(export, index_body: Optional[bytes], ap: URAlgorit
     log = ctx.read_events(export, window=event_window, now_ms=now_ms, keep_history=True)
     try:
         return ctx.mixed_queries(log, index_body, ap, query, users, items, item_sets, now_ms, header)
+    finally:
+        log.free()
+
+
+def queries_from_file(query_file, export, index_body: Optional[bytes], ap: URAlgorithmParams, now_ms: Optional[int] = None,
+                      ctx: CcoContext | None = None, event_window=None, header: str = "{}"):
+    """buildQuery (URAlgorithm.scala:563-839) for every line of a batchpredict query file (`pio batchpredict --input`: one
+    Query JSON object per line, each with its own members), as CcoContext.query_file: the bytes or a path; export: a
+    PredictionIO event export read on the device with history retention, or an EventLog read with keep_history=True, or
+    None when no line has a user; index_body: a model index body (None when no line has an item).  -> (body, offsets),
+    record r is line r's.  now_ms: "now" of the available / expire date filter and of the eventWindow."""
+    ctx = ctx or default_context()
+    now_ms = _now(now_ms)
+    from .similarity_analysis import EventLog
+    if export is None or isinstance(export, EventLog):
+        if event_window is not None:
+            raise ValueError("the eventWindow applies while an export is read")
+        return ctx.query_file(export, index_body, ap, query_file, now_ms, header)
+    log = ctx.read_events(export, window=event_window, now_ms=now_ms, keep_history=True)
+    try:
+        return ctx.query_file(log, index_body, ap, query_file, now_ms, header)
     finally:
         log.free()
 

@@ -103,7 +103,10 @@ the three shapes above; quirks of the reference, kept on purpose:
     itemSet), where userBlacklisted is the items of the user's events of blacklisted query names, latest first; distinct
     keeps each id's first position across the four sources;
   * "ItemSets should not be mixed with user or item queries" (:641-644) is only a log line: the query is built anyway.
-Out of scope: withRanks (it only changes how results are read), a different template per query.
+Query files (a batchpredict input: one Query object per line, each with its own template): query_file() is the host
+mirror of CcoContext.query_file, mixed_queries() for each line as a one-row batch; the extraction rules are listed above
+parse_query_line().
+Out of scope: withRanks (it only changes how results are read).
 """
 from __future__ import annotations
 
@@ -609,4 +612,199 @@ def mixed_queries(events, index_body: Optional[bytes], ap, query: Optional[Mixed
         recs.append((header + "\n" + mixed_render(p, hist, similar, s, excluded) + "\n").encode("utf-8", "surrogatepass"))
     offsets = np.zeros(len(recs) + 1, dtype=np.int64)
     np.cumsum([len(r) for r in recs], out=offsets[1:])
+    return b"".join(recs), offsets
+
+
+# ---- batchpredict query files ----------------------------------------------------------------------------------------
+# A query file (`pio batchpredict --input`) holds one Query JSON object per line, each with its own members.  Record r of
+# its body is the buildQuery of line r: mixed_queries() for a one-row batch whose template is that line's members.
+# Extraction restates PIO's json4s extract[Query] (Engine.scala:32-65); CcoContext.query_file applies the same rules on the
+# device (cco_query_file_read) and decodes each distinct template with template_from_key:
+#   * lines are separated by "\n"; a final "\n" opens no empty line; JSON whitespace ("\r" included) may surround the
+#     object; an empty or whitespace-only line is an error, as json4s' parse("") fails and the batch job with it;
+#   * members compare by their decoded name.  user, item, currentDate: a string; itemSet, blacklistItems, eventNames: an
+#     array of strings; userBias, itemBias, itemSetBias: a JSON number, read as a double and rounded to float (JDouble ->
+#     Float, f32(float(x))); num, from: an integer literal in Int32 range, a fraction or an exponent is an error [RECALL];
+#     returnSelf, withRanks: true or false; fields: an array of {"name": string, "values": [strings], "bias": number}, all
+#     three required; dateRange: {"name": string, "before"?: string, "after"?: string};
+#   * null is an absent member (an Option is None); unknown members are ignored [RECALL: json4s extraction ignores extra
+#     fields]; withRanks is checked and then ignored (it only changes how results are read);
+#   * deviation: a repeated known member is an error (json4s keeps both, and which one it extracts is not verifiable here).
+#   * the row members are user, item, itemSet and blacklistItems; every other known member is the line's template;
+#   * deviations of the device reader (CcoContext.query_file): the inside of an unknown member's value is checked only for
+#     its strings and bracket balance, and bytes are not checked as UTF-8; a template member's value that is not JSON is
+#     an error naming the member.
+ROW_MEMBERS = ("user", "item", "itemSet", "blacklistItems")
+TEMPLATE_MEMBERS = ("fields", "dateRange", "currentDate", "returnSelf", "num", "from", "eventNames", "userBias", "itemBias", "itemSetBias")
+KNOWN_MEMBERS = frozenset(ROW_MEMBERS + TEMPLATE_MEMBERS + ("withRanks",))
+
+
+class _Obj(dict):
+    """a decoded JSON object that remembers its member names in order (json's last-wins dict drops repeats)"""
+    def __init__(self, pairs):
+        super().__init__(pairs)
+        self.names = [k for k, _ in pairs]
+
+
+def _no_constant(x):
+    raise ValueError(f"{x} is not JSON")
+
+
+def query_file_lines(data) -> list:
+    """the lines of a query file's bytes: "\\n"-separated, a final "\\n" opens no line"""
+    data = bytes(data)
+    if not data:
+        return []
+    lines = data.split(b"\n")
+    return lines[:-1] if data.endswith(b"\n") else lines
+
+
+def parse_query_line(raw: bytes, r: int):
+    """one line of a query file -> (template key, MixedQuery, user, item, item set); ValueError naming line r"""
+    import json
+    def bad(what):
+        return ValueError(f"line {r}: {what}")
+    try:
+        text = raw.decode("utf-8", "surrogatepass")
+    except UnicodeDecodeError:
+        raise bad("not UTF-8") from None
+    if not text.strip(" \t\r"):
+        raise bad("not a JSON object (an empty line is not a query)")
+    try:
+        d = json.loads(text, object_pairs_hook=_Obj, parse_constant=_no_constant)
+    except ValueError as e:
+        raise bad(f"not one JSON object ({e})") from None
+    if not isinstance(d, _Obj):
+        raise bad("not a JSON object")
+    seen = set()
+    for n in d.names:
+        if n in KNOWN_MEMBERS and n in seen:
+            raise bad(f'the member "{n}" is repeated')
+        seen.add(n)
+    m = {k: d[k] for k in KNOWN_MEMBERS if d.get(k) is not None}
+    if "withRanks" in m and not isinstance(m["withRanks"], bool):
+        raise bad('"withRanks" is not true or false')
+    for k in ("user", "item"):
+        if k in m and not isinstance(m[k], str):
+            raise bad(f'"{k}" is not a string')
+    for k in ("blacklistItems", "itemSet"):
+        if k in m and (not isinstance(m[k], list) or not all(isinstance(x, str) for x in m[k])):
+            raise bad(f'"{k}" is not an array of strings')
+    q = template_query(m, r)
+    q.blacklistItems = list(m["blacklistItems"]) if "blacklistItems" in m else None
+    key = json.dumps([m.get(k) for k in TEMPLATE_MEMBERS])
+    return key, q, m.get("user"), m.get("item"), None if "itemSet" not in m else list(m["itemSet"])
+
+
+def template_query(m: dict, r: int) -> MixedQuery:
+    """the template members of a line (decoded, null dropped) -> MixedQuery without blacklistItems; ValueError naming line r"""
+    def bad(what):
+        return ValueError(f"line {r}: {what}")
+
+    def string(k, v):
+        if not isinstance(v, str):
+            raise bad(f'"{k}" is not a string')
+        return v
+
+    def strings(k, v):
+        if not isinstance(v, list) or not all(isinstance(x, str) for x in v):
+            raise bad(f'"{k}" is not an array of strings')
+        return list(v)
+
+    def number(k, v):
+        if isinstance(v, bool) or not isinstance(v, (int, float)):
+            raise bad(f'"{k}" is not a number')
+        try:
+            return float(v)
+        except OverflowError:
+            raise bad(f'"{k}" is out of the range of a double') from None
+
+    def int32(k, v):
+        if isinstance(v, bool) or not isinstance(v, int):
+            raise bad(f'"{k}" is not an integer literal')
+        if not -2**31 <= v < 2**31:
+            raise bad(f'"{k}" is outside the Int32 range')
+        return v
+
+    def boolean(k, v):
+        if not isinstance(v, bool):
+            raise bad(f'"{k}" is not true or false')
+        return v
+
+    def fields(v):
+        if not isinstance(v, list):
+            raise bad('"fields" is not an array')
+        out = []
+        for f in v:
+            if not isinstance(f, dict) or any(f.get(x) is None for x in ("name", "values", "bias")):
+                raise bad('a "fields" element is not {"name": string, "values": [strings], "bias": number}')
+            out.append(Field(string("fields.name", f["name"]), strings("fields.values", f["values"]), number("fields.bias", f["bias"])))
+        return out
+
+    def date_range(v):
+        if not isinstance(v, dict) or v.get("name") is None:
+            raise bad('"dateRange" is not {"name": string, "before"?: string, "after"?: string}')
+        return DateRange(string("dateRange.name", v["name"]), *[None if v.get(x) is None else string("dateRange." + x, v[x]) for x in ("before", "after")])
+
+    return MixedQuery(userBias=number("userBias", m["userBias"]) if "userBias" in m else None,
+                   fields=fields(m["fields"]) if "fields" in m else None,
+                   currentDate=string("currentDate", m["currentDate"]) if "currentDate" in m else None,
+                   dateRange=date_range(m["dateRange"]) if "dateRange" in m else None,
+                   num=int32("num", m["num"]) if "num" in m else None,
+                   from_=int32("from", m["from"]) if "from" in m else None,
+                   eventNames=strings("eventNames", m["eventNames"]) if "eventNames" in m else None,
+                   itemBias=number("itemBias", m["itemBias"]) if "itemBias" in m else None,
+                   returnSelf=boolean("returnSelf", m["returnSelf"]) if "returnSelf" in m else None,
+                   itemSetBias=number("itemSetBias", m["itemSetBias"]) if "itemSetBias" in m else None)
+
+
+def template_from_key(key: bytes, r: int) -> MixedQuery:
+    """a template key of cco_query_file_read (the template members' raw values in TEMPLATE_MEMBERS order, '\\0' between
+    them, an absent one empty) -> MixedQuery; ValueError naming line r (the template's first line)"""
+    import json
+    parts = key.split(b"\0")
+    m = {}
+    for k, raw in zip(TEMPLATE_MEMBERS, parts):
+        if not raw:
+            continue
+        try:
+            m[k] = json.loads(raw.decode("utf-8", "surrogatepass"), object_pairs_hook=_Obj, parse_constant=_no_constant)
+        except ValueError:
+            raise ValueError(f'line {r}: "{k}" is not JSON') from None
+    return template_query(m, r)
+
+
+def query_file_line_check(ap, q: MixedQuery, r: int, user, item, item_set, now_ms, have_events: bool, have_index: bool):
+    """the errors mixed_queries() raises for line r as a one-row batch, with the line named; -> its MixedPlan"""
+    try:
+        p = mixed_plan(ap, q, now_ms, with_limits=user is not None)
+    except KeyError as e:
+        raise ValueError(f"line {r}: {e.args[0]}") from None
+    except ValueError as e:
+        raise ValueError(f"line {r}: {e}") from None
+    if user is not None and not have_events:
+        raise ValueError(f"line {r}: a row has a user: its history needs the events")
+    if item is not None and not have_index:
+        raise ValueError(f"line {r}: a row has an item: its similar items need an index body")
+    if item_set is not None and p.with_set and p.set_name is None:
+        raise ValueError(f"line {r}: an item-set query needs a model event name: the set clause's field is the first one")
+    return p
+
+
+def query_file(events, index_body: Optional[bytes], ap, lines, now_ms: Optional[int] = None, header: str = "{}"):
+    """the host mirror of CcoContext.query_file: one record per line of a batchpredict query file (bytes), the line's
+    buildQuery as mixed_queries() writes it for a one-row batch with the line's members as its template -> (body, offsets)"""
+    recs = []
+    for r, raw in enumerate(query_file_lines(lines)):
+        _, q, u, it, s = parse_query_line(raw, r)
+        query_file_line_check(ap, q, r, u, it, s, now_ms, events is not None, index_body is not None)
+        try:
+            # the set column is always given (a line may have no member), so the batch has its one row
+            body, _ = mixed_queries(events, index_body, ap, q, None if u is None else [u], None if it is None else [it], [s], now_ms,
+                                    header)
+        except ValueError as e:
+            raise ValueError(f"line {r}: {e}") from None
+        recs.append(body)
+    offsets = np.zeros(len(recs) + 1, dtype=np.int64)
+    np.cumsum([len(x) for x in recs], out=offsets[1:])
     return b"".join(recs), offsets
