@@ -3,7 +3,7 @@ test_gpu_query_edges.py on the device).
 
 json4s_quote_ref and history_ref restate, independently of ur_query, the two rules the device kernels implement on their
 own: the json4s 3.2 quote (uq_escape on the device, uq_quote on the host) and one user's history lists and blacklist
-(k_uq_hist_keys, k_uq_first, k_uq_record).  The generators write the directed index bodies and event exports; each returns
+(k_uq_hist_keys, k_uq_first, k_mq_record).  The generators write the directed index bodies and event exports; each returns
 the body or export with the structure the queries must carry, which does not depend on the escaping."""
 from __future__ import annotations
 

@@ -117,7 +117,7 @@ def test_every_code_point_in_model_names(ctx):
               "c": None, "d": {}}
     dev = item_check(ctx, body, ap, None, None, expect)
     text = dev[0].decode("utf-8", "surrogatepass")
-    for n in names:   # iq_template's uq_quote
+    for n in names:   # mq_template's uq_quote
         assert "{" + '"terms":' + "{" + R.json4s_quote_ref(n) + ":[" in text
     item_check(ctx, body, ap, Q.ItemQuery(blacklistItems=["a", "x0"]), ["a", "b", "zz", "a"], expect)
 
@@ -129,7 +129,7 @@ def test_every_code_point_in_user_query_names_and_items(ctx):
     dev = user_check(ctx, data, ap, None, None)
     assert len(dev[2]) == 7
     text = dev[0].decode("utf-8", "surrogatepass")
-    for n in names:   # uq_template's uq_quote
+    for n in names:   # mq_template's uq_quote
         assert '{"terms":{' + R.json4s_quote_ref(n) + ":[" in text
     for k, s in enumerate(R.codepoint_strings() + R.EDGE_STRINGS):   # the items of the query names' events, through uq_escape
         if k % 3 < 2:

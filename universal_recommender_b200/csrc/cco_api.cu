@@ -4850,35 +4850,6 @@ static int emit_records(cco_ctx *c, Arena &ar, long long R, void (*len_pass)(Arg
 }
 }  // extern "C++"
 
-// the record template: n_history_names + 2 pieces around the history lists and the blacklist (see include/cco_b200.h)
-static std::vector<std::string> uq_template(const cco_user_query_t *q) {
-  std::vector<std::string> t(1);
-  const int k = q->n_history_names;
-  auto clause = [&](const char *rest, bool hist) {
-    bool any = false;
-    for (int j = 0; hist && j < k; ++j) {
-      if (any) t.back() += ",";
-      t.back() += "{\"terms\":{" + uq_quote(q->names[j]) + ":[";
-      t.emplace_back("]");
-      if (q->history_in_must) t.back() += ",\"boost\":0";
-      else if (q->boost) t.back() += std::string(",\"boost\":") + q->boost;
-      t.back() += "}}";
-      any = true;
-    }
-    if (*rest) {
-      if (any) t.back() += ",";
-      t.back() += rest;
-    }
-  };
-  t.back() += query_head(q->header, q->head);
-  clause(q->should, !q->history_in_must);
-  t.back() += "],\"must\":[";
-  clause(q->must, q->history_in_must != 0);
-  t.back() += "],\"must_not\":[{\"ids\":{\"values\":[";
-  t.push_back(query_tail(q->must_not, q->sort));
-  return t;
-}
-
 static int uq_check_host(const cco_user_query_t *q, int64_t n_users, const int64_t *uoff, const char *ubytes) {
   if (q->n_names < 0 || q->n_names > kUqMaxNames) return set_error(CCO_E_INVALID_ARG, "%d query event names, 0..%d", (int)q->n_names, kUqMaxNames);
   if (q->n_names > 0 && (!q->names || !q->limits)) return set_error(CCO_E_INVALID_ARG, "null names or limits");
@@ -5087,139 +5058,62 @@ static int uq_record_users(cco_ctx *c, const UqHistory &h, const DevStrCol &uc, 
   }
   return CCO_OK;
 }
-// the history members of a record kernel's UqArgs; the records, the list and the template are the caller's
-static UqArgs uq_args(const UqHistory &h, const cco_event_log *lg, int nq, int n_kept) {
+// the history lists as the record kernel reads them
+static UqArgs uq_args(const UqHistory &h, const cco_event_log *lg, int nq) {
   UqArgs a{};
   a.nq = nq;
-  a.n_kept = n_kept;
   a.limit = h.d_limit;
   a.hstart = h.hstart;
   a.hord = h.hord;
   a.keep_h = h.keep_h;
-  a.bstart = h.bstart;
-  a.bord = h.bord;
-  a.keep_b = h.keep_b;
-  a.bkey = h.bkey;
-  a.B = h.B;
   a.ent = h.ent;
   a.ioff = h.E > 0 ? lg->ti.off : nullptr;
   a.ibytes = h.E > 0 ? (const unsigned char *)lg->ti.w : nullptr;
   return a;
 }
-
-static int user_queries(cco_ctx *c, const cco_event_log *lg, const cco_user_query_t *q, int64_t n_users, const int64_t *uoff,
-                        const char *ubytes, char **out_body, int64_t *out_len, int64_t **out_offsets, int64_t *out_n,
-                        cco_dictionary_t *out_users) {
+// every user with an event of a query name, in order of their first line: the rows' user groups (*rec_uid [h.G]) and, when
+// users is not null, their ids
+static int uq_every_user(cco_ctx *c, Arena &ar, const cco_event_log *lg, const UqHistory &h, int32_t **rec_uid, cco_dictionary_t *users) {
   cudaStream_t s = c->stream;
-  const int nq = q->n_names;
-  CK(cudaSetDevice(c->device));
-  mail_reset(c);
-  Arena ar(s);
-  NvtxRange nvtx("cco:user_queries");
-  // 1. the caller's columns, checked on the device before any kernel reads bytes through their offsets
-  DevStrCol lc, uc;
-  CKR(str_upload(c, ar, q->n_blacklist_items, q->blacklist_item_offsets, q->blacklist_item_bytes, &lc));
-  if (uoff) CKR(str_upload(c, ar, n_users, uoff, ubytes, &uc));
-  int *bad, h_bad = 0;
-  CKR(ar.alloc(&bad, 1));
-  CK(cudaMemsetAsync(bad, 0, 4, s));
-  str_check_device(c, lc, bad);
-  if (uoff) str_check_device(c, uc, bad);
-  CKR(mail_fetch(c, &h_bad, bad, 4));
-  CKR(mail_wait(c));
-  if (h_bad) return set_error(CCO_E_INVALID_ARG, "decreasing offsets in the blacklist items or the users");
-  // 2-8. the history
-  UqHistory h;
-  CKR(uq_history(c, ar, lg, nq, q->names, q->limits, uq_black_names(nq, q->names, q->n_blacklist_names, q->blacklist_names), &h));
-  const long long E = h.E, G = h.G;
-  const StrTable &ut = h.ut, &it = h.it;
-  const DevStrCol &tu = h.tu, &ti = h.ti;
-  // 9. blacklistItems: item groups of the log (membership is a group test), repeats within the list dropped
-  const long long NL = q->n_blacklist_items;
-  int32_t *lgid;
-  uint8_t *keep_l;
-  CKR(ar.alloc(&lgid, std::max<long long>(NL, 1)));
-  CKR(ar.alloc(&keep_l, std::max<long long>(NL, 1)));
-  if (NL > 0) {
-    str_hash(c, lc, ~0ULL);
-    if (E > 0) {
-      k_str_lookup<<<grid_for(NL, 256, c->sm_count), 256, 0, s>>>(NL, lc.off, lc.base, lc.w, lc.hash, ti.off, ti.base, ti.w, ti.hash,
-                                                                 (uint64_t)it.cap - 1, it.table, it.rank_of_slot, lgid);
-      c->launches++;
-    } else {
-      CK(cudaMemsetAsync(lgid, 0xff, sizeof(int32_t) * (size_t)NL, s));
-    }
-    StrTable lt;
-    int32_t *lid;
-    CKR(ar.alloc(&lid, NL));
-    CKR(str_group(c, ar, lc, nullptr, false, 0, &lt, lid));
-    k_uq_list_first<<<grid_for(NL, 256, c->sm_count), 256, 0, s>>>(NL, lid, lt.first_sorted, keep_l);
+  const long long R = h.G;
+  if (R > 0) {
+    unsigned long long *mn, *uk;
+    CKR(ar.alloc(&mn, R));
+    CKR(ar.alloc(&uk, R));
+    CK(cudaMemsetAsync(mn, 0xff, sizeof(unsigned long long) * (size_t)R, s));
+    k_uq_min_line<<<grid_for(h.E, 256, c->sm_count), 256, 0, s>>>(h.E, h.uid, h.ln, mn);
+    k_uq_user_keys<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, mn, uk, *rec_uid);
+    c->launches += 2;
+    CKR(sort_pairs(c, ar, R, &uk, rec_uid, bits_for(lg->n_lines)));
+  }
+  if (!users) return CCO_OK;
+  uint32_t *ue;
+  long long *len, *off, total = 0;
+  CKR(ar.alloc(&ue, std::max<long long>(R, 1)));
+  CKR(ar.alloc(&len, R + 1));
+  CKR(ar.alloc(&off, R + 1));
+  CK(cudaMemsetAsync(len + R, 0, 8, s));
+  if (R > 0) {
+    k_uq_user_entry<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, *rec_uid, h.ut.first_sorted, ue);
+    k_str_dict_len<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, ue, h.tu.off, len);
+    c->launches += 2;
+  }
+  CKR(exclusive_sum(c, ar, len, off, R + 1));
+  CK(cudaMemcpyAsync(&total, off + R, 8, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  unsigned char *ub;
+  CKR(ar.alloc(&ub, std::max<long long>(total, 1)));
+  if (R > 0 && total > 0) {
+    k_str_dict_gather<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, ue, h.tu.off, h.tu.base, (const unsigned char *)h.tu.w, off, ub);
     c->launches++;
   }
-  // 10. the records' users
-  long long R = 0;
-  int32_t *rec_uid;
-  if (uoff) {
-    R = n_users;
-    CKR(ar.alloc(&rec_uid, std::max<long long>(R, 1)));
-    CKR(uq_record_users(c, h, uc, R, rec_uid));
-  } else {   // every user with an event of a query name, by first line
-    R = G;
-    CKR(ar.alloc(&rec_uid, std::max<long long>(R, 1)));
-    if (R > 0) {
-      unsigned long long *mn, *uk;
-      CKR(ar.alloc(&mn, G));
-      CKR(ar.alloc(&uk, G));
-      CK(cudaMemsetAsync(mn, 0xff, sizeof(unsigned long long) * (size_t)G, s));
-      k_uq_min_line<<<grid_for(E, 256, c->sm_count), 256, 0, s>>>(E, h.uid, h.ln, mn);
-      k_uq_user_keys<<<grid_for(G, 256, c->sm_count), 256, 0, s>>>(G, mn, uk, rec_uid);
-      c->launches += 2;
-      CKR(sort_pairs(c, ar, G, &uk, &rec_uid, bits_for(lg->n_lines)));
-    }
-    if (out_users) {
-      uint32_t *ue;
-      long long *len, *off, total = 0;
-      CKR(ar.alloc(&ue, std::max<long long>(R, 1)));
-      CKR(ar.alloc(&len, R + 1));
-      CKR(ar.alloc(&off, R + 1));
-      CK(cudaMemsetAsync(len + R, 0, 8, s));
-      if (R > 0) {
-        k_uq_user_entry<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, rec_uid, ut.first_sorted, ue);
-        k_str_dict_len<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, ue, tu.off, len);
-        c->launches += 2;
-      }
-      CKR(exclusive_sum(c, ar, len, off, R + 1));
-      CK(cudaMemcpyAsync(&total, off + R, 8, cudaMemcpyDeviceToHost, s));
-      CK(cudaStreamSynchronize(s));
-      unsigned char *ub;
-      CKR(ar.alloc(&ub, std::max<long long>(total, 1)));
-      if (R > 0 && total > 0) {
-        k_str_dict_gather<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, ue, tu.off, tu.base, (const unsigned char *)tu.w, off, ub);
-        c->launches++;
-      }
-      int64_t *ho = (int64_t *)c->pinned_get(sizeof(int64_t) * ((size_t)R + 1), /*for_result=*/false);
-      char *hb = (char *)c->pinned_get((size_t)std::max<long long>(total, 1), /*for_result=*/false);
-      if (!ho || !hb) return set_error(CCO_E_OOM, "pinned host allocation failed");
-      CK(cudaMemcpyAsync(ho, off, sizeof(int64_t) * ((size_t)R + 1), cudaMemcpyDeviceToHost, s));
-      if (total > 0) CK(cudaMemcpyAsync(hb, ub, (size_t)total, cudaMemcpyDeviceToHost, s));
-      *out_users = cco_dictionary_t{R, ho, hb};
-    }
-  }
-  // 11. the template, then a length pass, the record offsets and a write pass: one warp per record
-  DevDict tp;
-  CKR(upload_strings(c, ar, uq_template(q), &tp));
-  UqArgs a = uq_args(h, lg, nq, q->n_history_names);
-  a.n_rec = R;
-  a.rec_uid = rec_uid;
-  a.n_list = NL;
-  a.loff = lc.off;
-  a.lbase = lc.base;
-  a.lbytes = (const unsigned char *)lc.w;
-  a.lgid = lgid;
-  a.keep_l = keep_l;
-  a.toff = tp.off;
-  a.tbytes = tp.bytes;
-  return emit_records(c, ar, R, k_uq_record<false>, k_uq_record<true>, a, out_body, out_len, out_offsets, out_n);
+  int64_t *ho = (int64_t *)c->pinned_get(sizeof(int64_t) * ((size_t)R + 1), /*for_result=*/false);
+  char *hb = (char *)c->pinned_get((size_t)std::max<long long>(total, 1), /*for_result=*/false);
+  if (!ho || !hb) return set_error(CCO_E_OOM, "pinned host allocation failed");
+  CK(cudaMemcpyAsync(ho, off, sizeof(int64_t) * ((size_t)R + 1), cudaMemcpyDeviceToHost, s));
+  if (total > 0) CK(cudaMemcpyAsync(hb, ub, (size_t)total, cudaMemcpyDeviceToHost, s));
+  *users = cco_dictionary_t{R, ho, hb};
+  return CCO_OK;
 }
 }  // namespace cco
 
@@ -5230,37 +5124,7 @@ int cco_event_log_begin_ex(cco_ctx_t *ctx, int64_t chunk_bytes, const cco_event_
   return CCO_OK;
 }
 
-int cco_event_log_user_queries(cco_ctx_t *ctx, const cco_event_log_t *lg, const cco_user_query_t *q, int64_t n_users,
-                               const int64_t *user_offsets, const char *user_bytes, char **out_body, int64_t *out_len,
-                               int64_t **out_offsets, int64_t *out_n, cco_dictionary_t *out_users) {
-  if (!ctx || !lg || !q || !out_body || !out_len || !out_offsets || !out_n) return set_error(CCO_E_INVALID_ARG, "null argument");
-  if (!ctx->members.empty() || lg->ctx != ctx) return set_error(CCO_E_UNSUPPORTED, "build queries on the per-GPU context that read the log");
-  CKR(log_state(lg, true));
-  CKR(uq_check_host(q, n_users, user_offsets, user_bytes));
-  if (!lg->history) return set_error(CCO_E_INVALID_ARG, "the log was read without history retention (cco_event_log_begin_ex, CCO_LOG_KEEP_HISTORY)");
-  if (out_users) *out_users = cco_dictionary_t{0, nullptr, nullptr};
-  return user_queries(ctx, lg, q, n_users, user_offsets, user_bytes, out_body, out_len, out_offsets, out_n, out_users);
-}
-
 namespace cco {
-// the record template of an item query, 9 + n_names pieces: 0 head and "should":[, 1 should_head, 2 should, 3 "must":[,
-// 4 must_head, 5 must, 6 the ids clause up to its values, 7 the rest of the record, 8 the end of a similar-items clause,
-// 9 + j the start of model name j's clause (see include/cco_b200.h)
-static std::vector<std::string> iq_template(const cco_item_query_t *q) {
-  std::vector<std::string> t(9 + q->n_names);
-  t[0] = query_head(q->header, q->head);
-  t[1] = q->should_head;
-  t[2] = q->should;
-  t[3] = "],\"must\":[";
-  t[4] = q->must_head;
-  t[5] = q->must;
-  t[6] = "],\"must_not\":[{\"ids\":{\"values\":[";
-  t[7] = query_tail(q->must_not, q->sort);
-  t[8] = q->similar_in_must ? "],\"boost\":0}}" : q->similar_boost ? std::string("],\"boost\":") + q->similar_boost + "}}" : "]}}";
-  for (int j = 0; j < q->n_names; ++j) t[9 + j] = "{\"terms\":{" + uq_quote(q->names[j]) + ":[";
-  return t;
-}
-
 static int iq_check_host(const cco_item_query_t *q, int64_t n_items, const int64_t *ioff, const char *ibytes) {
   if (q->n_names < 1 || q->n_names > kUqMaxNames) return set_error(CCO_E_INVALID_ARG, "%d model event names, 1..%d", (int)q->n_names, kUqMaxNames);
   if (!q->names) return set_error(CCO_E_INVALID_ARG, "null names");
@@ -5357,133 +5221,6 @@ static int iq_documents(cco_ctx *c, Arena &ar, const BulkDocs &bd, int n_names, 
   return CCO_OK;
 }
 
-static int item_queries(cco_ctx *c, const char *body, int64_t body_len, const cco_item_query_t *q, int64_t n_items, const int64_t *ioff,
-                        const char *ibytes, char **out_body, int64_t *out_len, int64_t **out_offsets, int64_t *out_n,
-                        cco_dictionary_t *out_items) {
-  cudaStream_t s = c->stream;
-  CK(cudaSetDevice(c->device));
-  Arena ar(s);
-  NvtxRange nvtx("cco:item_queries");
-  mail_reset(c);
-  const bool all = ioff == nullptr;
-  const long long NI = all ? 0 : n_items, NL = q->n_blacklist_items;
-  // 1-4. the documents: members, decoded names and _ids
-  BulkDocs bd;
-  CKR(bulk_parse(c, ar, body, body_len, NI + NL, "items + blacklist items", &bd));
-  const long long D = bd.D, R = all ? D : NI;
-  // 5. one key column: the decoded _ids, the items, blacklistItems; the caller's offsets are checked on the device before
-  //    any kernel reads bytes through them
-  int *bad, h_bad = 0;
-  CKR(ar.alloc(&bad, 1));
-  CK(cudaMemsetAsync(bad, 0, sizeof(int), s));
-  DevStrCol key;
-  CKR(key_column(c, ar, {KeySection{D, (const int64_t *)bd.ids.off, (const char *)bd.ids.w, true, bd.ids_bytes}, KeySection{NI, ioff, ibytes},
-                         KeySection{NL, q->blacklist_item_offsets, q->blacklist_item_bytes}}, bad, &key));
-  CKR(mail_fetch(c, &h_bad, bad, 4));
-  CKR(mail_wait(c));
-  if (h_bad) return set_error(CCO_E_INVALID_ARG, "decreasing offsets in the items or the blacklist items");
-  // 6. one exact grouping over the key column; a group that holds two documents is a repeated _id
-  str_hash(c, key, ~0ULL);
-  int32_t *gid;
-  CKR(ar.alloc(&gid, std::max<long long>(key.n, 1)));
-  StrTable tb;
-  CKR(str_group(c, ar, key, nullptr, false, 0, &tb, gid));
-  CKR(iq_unique_ids(c, ar, D, gid, tb));
-  // 7. blacklistItems: each group's first list index (membership and repeats are group tests)
-  const long long G = tb.n_groups;
-  uint32_t *first_in_list;
-  CKR(ar.alloc(&first_in_list, std::max<long long>(G, 1)));
-  CK(cudaMemsetAsync(first_in_list, 0xff, sizeof(uint32_t) * (size_t)std::max<long long>(G, 1), s));
-  if (NL > 0) {
-    k_iq_black<<<grid_for(NL, 256, c->sm_count), 256, 0, s>>>(NL, D + NI, gid, first_in_list);
-    c->launches++;
-  }
-  // 8. the records' documents; the queried documents
-  int32_t *rec_doc, *rec_key;
-  uint8_t *queried;
-  CKR(ar.alloc(&rec_doc, std::max<long long>(R, 1)));
-  CKR(ar.alloc(&rec_key, std::max<long long>(R, 1)));
-  CKR(ar.alloc(&queried, std::max<long long>(D, 1)));
-  CK(cudaMemsetAsync(queried, 0, (size_t)std::max<long long>(D, 1), s));
-  if (R > 0) {
-    k_iq_rec<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, D, all, gid, tb.first_sorted, rec_doc, rec_key, queried);
-    c->launches++;
-  }
-  // 9-10. the queried documents' similar-items lists
-  IqDocs docs;
-  CKR(iq_documents(c, ar, bd, q->n_names, q->names, queried, &docs));
-  // 11. the template, then a length pass, the record offsets and a write pass: one warp per record
-  int32_t *d_entry;
-  CKR(ar.alloc(&d_entry, q->n_names));
-  CK(cudaMemcpyAsync(d_entry, docs.name_entry.data(), sizeof(int32_t) * (size_t)q->n_names, cudaMemcpyHostToDevice, s));
-  DevDict tp;
-  CKR(upload_strings(c, ar, iq_template(q), &tp));
-  IqArgs a;
-  a.n_rec = R;
-  a.rec_doc = rec_doc;
-  a.rec_key = rec_key;
-  a.kgid = gid;
-  a.koff = key.off;
-  a.kbytes = (const unsigned char *)key.w;
-  a.line_moff = bd.line_moff;
-  a.T = docs.T;
-  a.n_names = q->n_names;
-  a.name_entry = d_entry;
-  a.eoff = docs.eoff;
-  a.doff = docs.dec.off;
-  a.dbytes = (const unsigned char *)docs.dec.w;
-  a.slice = q->max_query_events;
-  a.in_must = q->similar_in_must;
-  a.exclude_self = q->exclude_self;
-  a.n_list = NL;
-  a.list_at = D + NI;
-  a.first_in_list = first_in_list;
-  a.toff = tp.off;
-  a.tbytes = tp.bytes;
-  return emit_records(c, ar, R, k_iq_record<false>, k_iq_record<true>, a, out_body, out_len, out_offsets, out_n, [&]() -> int {
-    if (!all || !out_items) return CCO_OK;
-    // the documents' decoded _ids, in body order
-    int64_t *io = (int64_t *)c->pinned_get(sizeof(int64_t) * ((size_t)D + 1), /*for_result=*/false);
-    char *ib = (char *)c->pinned_get((size_t)std::max<long long>(bd.ids_bytes, 1), /*for_result=*/false);
-    if (!io || !ib) return set_error(CCO_E_OOM, "pinned host allocation failed");
-    io[0] = 0;
-    if (D > 0) CK(cudaMemcpyAsync(io, bd.ids.off, sizeof(int64_t) * ((size_t)D + 1), cudaMemcpyDeviceToHost, s));
-    if (bd.ids_bytes > 0) CK(cudaMemcpyAsync(ib, bd.ids.w, (size_t)bd.ids_bytes, cudaMemcpyDeviceToHost, s));
-    *out_items = cco_dictionary_t{D, io, ib};
-    return CCO_OK;
-  });
-}
-}  // namespace cco
-
-int cco_item_queries(cco_ctx_t *ctx, const char *index_body, int64_t index_len, const cco_item_query_t *q, int64_t n_items,
-                     const int64_t *item_offsets, const char *item_bytes, char **out_body, int64_t *out_len, int64_t **out_offsets,
-                     int64_t *out_n, cco_dictionary_t *out_items) {
-  if (!ctx || !q || !out_body || !out_len || !out_offsets || !out_n || index_len < 0 || (index_len > 0 && !index_body))
-    return set_error(CCO_E_INVALID_ARG, "null argument or negative length");
-  if (!ctx->members.empty()) return set_error(CCO_E_UNSUPPORTED, "per-GPU contexts only");
-  if (index_len > 0 && index_body[index_len - 1] != '\n') return set_error(CCO_E_INVALID_ARG, "the body does not end in a newline");
-  CKR(iq_check_host(q, n_items, item_offsets, item_bytes));
-  if (out_items) *out_items = cco_dictionary_t{0, nullptr, nullptr};
-  return item_queries(ctx, index_body, index_len, q, n_items, item_offsets, item_bytes, out_body, out_len, out_offsets, out_n, out_items);
-}
-
-namespace cco {
-// the record template of an item-set query, 7 pieces: 0 head and "should":[, 1 should_head, 2 the start of the set clause,
-// 3 its end, 4 should_tail, 5 must up to the ids clause's values, 6 the rest of the record (see include/cco_b200.h)
-static std::vector<std::string> is_template(const cco_item_set_query_t *q) {
-  std::vector<std::string> t(7);
-  t[0] = query_head(q->header, q->head);
-  t[1] = q->should_head;
-  if (q->with_set) {
-    t[2] = "{\"terms\":{" + uq_quote(q->name) + ":[";
-    t[3] = q->boost ? std::string("],\"boost\":") + q->boost + "}}" : "]}}";
-  }
-  t[4] = q->should_tail;
-  t[5] = std::string("],\"must\":[") + q->must + "],\"must_not\":[{\"ids\":{\"values\":[";
-  t[6] = query_tail(q->must_not, q->sort);
-  return t;
-}
-
 static int is_check_host(const cco_item_set_query_t *q, long long n_sets, const int64_t *soff, long long n_elements, const int64_t *eoff,
                          const char *ebytes) {
   if (q->with_set != 0 && q->with_set != 1) return set_error(CCO_E_INVALID_ARG, "with_set must be 0 or 1");
@@ -5504,103 +5241,30 @@ static int is_check_host(const cco_item_set_query_t *q, long long n_sets, const 
   return CCO_OK;
 }
 
-static int item_set_queries(cco_ctx *c, const cco_item_set_query_t *q, long long n_sets, const int64_t *set_off, const int64_t *eoff,
-                            const char *ebytes, char **out_body, int64_t *out_len, int64_t **out_offsets, int64_t *out_n) {
-  cudaStream_t s = c->stream;
-  CK(cudaSetDevice(c->device));
-  Arena ar(s);
-  NvtxRange nvtx("cco:item_set_queries");
-  mail_reset(c);
-  const long long S = n_sets, s0 = set_off[0], NE = set_off[S] - s0, NL = q->n_blacklist_items;
-  // 1. one key column: blacklistItems, then the sets' elements; the set offsets 0-based.  Every column's offsets are
-  //    checked on the device before any kernel reads bytes through them
-  int *bad, h_bad = 0;
-  CKR(ar.alloc(&bad, 1));
-  CK(cudaMemsetAsync(bad, 0, sizeof(int), s));
-  long long *soff, *stmp;
-  CKR(ar.alloc(&soff, S + 1));
-  CKR(ar.alloc(&stmp, S + 1));
-  CK(cudaMemcpyAsync(stmp, set_off, sizeof(int64_t) * ((size_t)S + 1), cudaMemcpyHostToDevice, s));
-  if (S > 0) {
-    k_str_check<<<grid_for(S, 256, c->sm_count), 256, 0, s>>>(S, stmp, bad);
-    c->launches++;
-  }
-  k_rebase<<<grid_for(S + 1, 256, c->sm_count), 256, 0, s>>>(S + 1, stmp, -s0, soff);
-  c->launches++;
-  DevStrCol key;
-  CKR(key_column(c, ar, {KeySection{NL, q->blacklist_item_offsets, q->blacklist_item_bytes}, KeySection{NE, eoff + s0, ebytes}}, bad, &key));
-  CKR(mail_fetch(c, &h_bad, bad, 4));
-  CKR(mail_wait(c));
-  if (h_bad) return set_error(CCO_E_INVALID_ARG, "decreasing offsets in the sets, the elements or the blacklist items");
-  // 2. one exact grouping over the key column; blacklistItems: each group's first list index (membership is a group test)
-  str_hash(c, key, ~0ULL);
-  int32_t *gid;
-  CKR(ar.alloc(&gid, std::max<long long>(key.n, 1)));
-  StrTable tb;
-  CKR(str_group(c, ar, key, nullptr, false, 0, &tb, gid));
-  const long long G = tb.n_groups;
-  uint32_t *first_in_list;
-  CKR(ar.alloc(&first_in_list, std::max<long long>(G, 1)));
-  CK(cudaMemsetAsync(first_in_list, 0xff, sizeof(uint32_t) * (size_t)std::max<long long>(G, 1), s));
-  if (NL > 0) {
-    k_iq_black<<<grid_for(NL, 256, c->sm_count), 256, 0, s>>>(NL, 0, gid, first_in_list);
-    c->launches++;
-  }
-  // 3. each element's first occurrence within its set: the first of each run of (set, group) keys after a stable sort
-  uint8_t *first_in_set;
-  CKR(ar.alloc(&first_in_set, std::max<long long>(NE, 1)));
-  if (NE > 0) {
-    unsigned long long *k2;
-    uint32_t *p2;
-    CKR(ar.alloc(&k2, NE));
-    CKR(ar.alloc(&p2, NE));
-    CK(cudaMemsetAsync(first_in_set, 0, (size_t)NE, s));
-    k_is_keys<<<grid_for(NE, 256, c->sm_count), 256, 0, s>>>(NE, S, soff, gid + NL, k2, p2);
-    c->launches++;
-    CKR(sort_pairs(c, ar, NE, &k2, &p2, 32 + bits_for(S)));
-    k_uq_first<<<grid_for(NE, 256, c->sm_count), 256, 0, s>>>(NE, k2, p2, first_in_set);
-    c->launches++;
-    ar.release(k2);
-    ar.release(p2);
-  }
-  // 4. the template, then a length pass, the record offsets and a write pass: one warp per set
-  DevDict tp;
-  CKR(upload_strings(c, ar, is_template(q), &tp));
-  IsArgs a;
-  a.n_sets = S;
-  a.soff = soff;
-  a.kgid = gid;
-  a.koff = key.off;
-  a.kbytes = (const unsigned char *)key.w;
-  a.n_list = NL;
-  a.first_in_list = first_in_list;
-  a.first_in_set = first_in_set;
-  a.with_set = q->with_set;
-  a.toff = tp.off;
-  a.tbytes = tp.bytes;
-  return emit_records(c, ar, S, k_is_record<false>, k_is_record<true>, a, out_body, out_len, out_offsets, out_n);
-}
-}  // namespace cco
+// What cco_event_log_user_queries, cco_item_queries and cco_item_set_queries add when they render their queries as rows of
+// a mixed batch, each row with one member: the NVTX range; an item query's head clauses, written before the history and
+// the similar items of should and must; the members the body's size check names; and a row source that is not a column,
+// every user of the history or every document of the body, whose rows are fixed once they are known, with *keys (nullable)
+// listing them.
+enum : int { kMqColumns = 0, kMqEveryUser, kMqEveryDoc };
+struct MqSingle {
+  const char *range = "cco:mixed_queries";
+  const char *should_head = "", *must_head = "";
+  const char *what = "items + blacklist items + elements";
+  int rows = kMqColumns;
+  cco_dictionary_t *keys = nullptr;
+};
 
-int cco_item_set_queries(cco_ctx_t *ctx, const cco_item_set_query_t *q, int64_t n_sets, const int64_t *set_offsets, int64_t n_elements,
-                         const int64_t *elem_offsets, const char *elem_bytes, char **out_body, int64_t *out_len, int64_t **out_offsets,
-                         int64_t *out_n) {
-  if (!ctx || !q || !out_body || !out_len || !out_offsets || !out_n) return set_error(CCO_E_INVALID_ARG, "null argument");
-  if (!ctx->members.empty()) return set_error(CCO_E_UNSUPPORTED, "per-GPU contexts only");
-  CKR(is_check_host(q, n_sets, set_offsets, n_elements, elem_offsets, elem_bytes));
-  return item_set_queries(ctx, q, n_sets, set_offsets, elem_offsets, elem_bytes, out_body, out_len, out_offsets, out_n);
-}
-
-namespace cco {
-// the record template of a mixed query, 11 + n_history_names + n_model_names pieces: 0 head and "should":[, 1 boosted,
+// the record template of a mixed query, 13 + n_history_names + n_model_names pieces: 0 head and "should":[, 1 boosted,
 // 2 should_tail, 3 must, 4 "],"must":[, 5 the ids clause up to its values, 6 the rest of the record, 7 the end of a history
-// clause, 8 the end of a similar-items clause, 9 / 10 the start / end of the set clause, 11 + j the start of query name j's
-// history clause, 11 + n_history_names + j the start of model name j's similar-items clause (see include/cco_b200.h)
-static std::vector<std::string> mq_template(const cco_mixed_query_t *q) {
+// clause, 8 the end of a similar-items clause, 9 / 10 the start / end of the set clause, 11 / 12 should's / must's head,
+// 13 + j the start of query name j's history clause, 13 + n_history_names + j the start of model name j's similar-items
+// clause (see include/cco_b200.h)
+static std::vector<std::string> mq_template(const cco_mixed_query_t *q, const MqSingle &x) {
   auto end = [](bool in_must, const char *boost) {
     return in_must ? std::string("],\"boost\":0}}") : boost ? std::string("],\"boost\":") + boost + "}}" : std::string("]}}");
   };
-  std::vector<std::string> t(11);
+  std::vector<std::string> t(13);
   t[0] = query_head(q->header, q->head);
   t[1] = q->boosted;
   t[2] = q->should_tail;
@@ -5614,6 +5278,8 @@ static std::vector<std::string> mq_template(const cco_mixed_query_t *q) {
     t[9] = "{\"terms\":{" + uq_quote(q->set_name) + ":[";
     t[10] = end(false, q->set_boost);
   }
+  t[11] = x.should_head;
+  t[12] = x.must_head;
   for (int j = 0; j < q->n_history_names; ++j) t.push_back("{\"terms\":{" + uq_quote(q->names[j]) + ":[");
   for (int j = 0; j < q->n_model_names; ++j) t.push_back("{\"terms\":{" + uq_quote(q->model_names[j]) + ":[");
   return t;
@@ -5677,7 +5343,7 @@ static int mq_check_host(const cco_mixed_query_t *q, long long R, const int64_t 
   return CCO_OK;
 }
 
-// The rows of a mixed batch in HBM, as the two callers stage them: cco_mixed_queries' columns (one template, one shared
+// The rows of a mixed batch in HBM, as the two callers stage them: mixed_queries' columns (one template, one shared
 // blacklistItems list) and a query file's lines (a template and a blacklistItems list per row).
 struct MqRows {
   long long R = 0, NI = 0, NL = 0, NE = 0;   // rows; key entries of the items (R or 0), the lists and the elements
@@ -5685,11 +5351,12 @@ struct MqRows {
   DevStrCol uc;                             // the users (uc.n = R when a user column is given)
   bool col[3] = {false, false, false};      // a user, item, set column is given
   const uint8_t *valid[3] = {nullptr, nullptr, nullptr};   // device LSB-first bitmaps, nullptr: every row
-  long long *soff = nullptr;                // [R + 1] 0-based element index of each row's set
+  long long *soff = nullptr;                // [R + 1] 0-based element index of each row's set, nullptr: all 0
   long long *loff = nullptr;                // [lists + 1] entry index of each list
   bool list_shared = true;                  // one list for every row, else list r is row r's
-  int32_t *rec_tpl = nullptr;               // [R] template of each row
+  int32_t *rec_tpl = nullptr;               // [R] template of each row, nullptr: all 0
   std::vector<uint8_t> tpl_user;            // per template: a row with a user reads it
+  MqSingle one;
 };
 
 // the union of the query names of the templates a row with a user reads, their limits, each template's history names in
@@ -5753,22 +5420,24 @@ static int mq_names(const std::vector<const cco_mixed_query_t *> &tq, const std:
   return CCO_OK;
 }
 
-// Steps shared by cco_mixed_queries (T = 1) and cco_query_file_queries: the documents, one key column (_ids, items,
-// blacklistItems, elements), the history over the union of the templates' names, each row's members, the lists' and sets'
-// first occurrences, and the records.  *bad holds the device verdict on the caller's offsets so far.
+// Steps shared by every query builder: the documents, one key column (_ids, items, blacklistItems, elements), the history
+// over the union of the templates' names, each row's members, the lists' and sets' first occurrences, and the records.
+// *bad holds the device verdict on the caller's offsets so far.
 static int mixed_render(cco_ctx *c, Arena &ar, const cco_event_log *lg, const char *body, int64_t body_len,
                         const std::vector<const cco_mixed_query_t *> &tq, MqRows &in, int *bad, char **out_body, int64_t *out_len,
                         int64_t **out_offsets, int64_t *out_n) {
   cudaStream_t s = c->stream;
-  const long long R = in.R, NI = in.NI, NL = in.NL, NE = in.NE;
+  const long long NI = in.NI, NL = in.NL, NE = in.NE;
+  long long R = in.R;
   const cco_mixed_query_t *q0 = tq[0];
   const int T = (int)tq.size();
   bool any_user = false;
   for (uint8_t x : in.tpl_user) any_user |= x != 0;
   // 1. the documents of the index body: members, decoded names and _ids
   BulkDocs bd;
-  if (body) CKR(bulk_parse(c, ar, body, body_len, NI + NL + NE, "items + blacklist items + elements", &bd));
+  if (body) CKR(bulk_parse(c, ar, body, body_len, NI + NL + NE, in.one.what, &bd));
   const long long D = bd.D;
+  if (in.one.rows == kMqEveryDoc) R = D;   // row r is document r, its item key entry r (its own _id)
   // 2. one key column of the decoded _ids, the items, blacklistItems and the elements
   std::vector<KeySection> sec{KeySection{D, (const int64_t *)bd.ids.off, (const char *)bd.ids.w, true, bd.ids_bytes}};
   sec.insert(sec.end(), in.sec.begin(), in.sec.end());
@@ -5808,8 +5477,6 @@ static int mixed_render(cco_ctx *c, Arena &ar, const cco_event_log *lg, const ch
   const int nq = (int)nm.names.size();
   UqHistory h;
   std::vector<MqBlack> hb;
-  int32_t *rec_uid;
-  CKR(ar.alloc(&rec_uid, std::max<long long>(R, 1)));
   if (any_user) {
     CKR(uq_history(c, ar, lg, nq, nm.names.data(), nm.limits.data(), nm.masks[0], &h));
     hb.push_back(MqBlack{h.bstart, h.bkey, h.bord, h.keep_b});
@@ -5817,11 +5484,25 @@ static int mixed_render(cco_ctx *c, Arena &ar, const cco_event_log *lg, const ch
       CKR(uq_blacklist(c, ar, nq, nm.masks[m], &h));
       hb.push_back(MqBlack{h.bstart, h.bkey, h.bord, h.keep_b});
     }
-    CKR(uq_record_users(c, h, in.uc, R, rec_uid));
-  } else if (R > 0) {
-    CK(cudaMemsetAsync(rec_uid, 0xff, sizeof(int32_t) * (size_t)R, s));
   }
   if (hb.empty()) hb.push_back(MqBlack{nullptr, nullptr, nullptr, nullptr});
+  if (in.one.rows == kMqEveryUser) R = h.G;
+  int32_t *rec_uid;
+  CKR(ar.alloc(&rec_uid, std::max<long long>(R, 1)));
+  if (in.one.rows == kMqEveryUser) CKR(uq_every_user(c, ar, lg, h, &rec_uid, in.one.keys));
+  else if (any_user) CKR(uq_record_users(c, h, in.uc, R, rec_uid));
+  else if (R > 0) CK(cudaMemsetAsync(rec_uid, 0xff, sizeof(int32_t) * (size_t)R, s));
+  // a caller without sets or templates: every row's set is empty and its template 0
+  long long *soff = in.soff;
+  int32_t *rec_tpl = in.rec_tpl;
+  if (!soff) {
+    CKR(ar.alloc(&soff, R + 1));
+    CK(cudaMemsetAsync(soff, 0, sizeof(long long) * ((size_t)R + 1), s));
+  }
+  if (!rec_tpl) {
+    CKR(ar.alloc(&rec_tpl, std::max<long long>(R, 1)));
+    CK(cudaMemsetAsync(rec_tpl, 0, sizeof(int32_t) * (size_t)std::max<long long>(R, 1), s));
+  }
   // 6. each row's members and document; the queried documents
   int32_t *rec_doc, *rec_key;
   uint8_t *rec_set, *queried;
@@ -5831,8 +5512,9 @@ static int mixed_render(cco_ctx *c, Arena &ar, const cco_event_log *lg, const ch
   CKR(ar.alloc(&queried, std::max<long long>(D, 1)));
   CK(cudaMemsetAsync(queried, 0, (size_t)std::max<long long>(D, 1), s));
   if (R > 0) {
-    k_mq_rows<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, in.valid[0], in.valid[1], in.valid[2], in.col[0], in.col[1], in.col[2], D, D,
-                                                           gid, tb.first_sorted, rec_uid, rec_doc, rec_key, rec_set, queried);
+    k_mq_rows<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, in.valid[0], in.valid[1], in.valid[2], in.col[0], in.col[1], in.col[2], D,
+                                                           in.one.rows == kMqEveryDoc ? 0 : D, gid, tb.first_sorted, rec_uid, rec_doc,
+                                                           rec_key, rec_set, queried);
     c->launches++;
   }
   // 7. the queried documents' similar-items lists (the model names are the algorithm's: every template has the same)
@@ -5857,7 +5539,7 @@ static int mixed_render(cco_ctx *c, Arena &ar, const cco_event_log *lg, const ch
     CKR(ar.alloc(&k2, NE));
     CKR(ar.alloc(&p2, NE));
     CK(cudaMemsetAsync(first_in_set, 0, (size_t)NE, s));
-    k_is_keys<<<grid_for(NE, 256, c->sm_count), 256, 0, s>>>(NE, R, in.soff, gid + D + NI + NL, k2, p2);
+    k_is_keys<<<grid_for(NE, 256, c->sm_count), 256, 0, s>>>(NE, R, soff, gid + D + NI + NL, k2, p2);
     c->launches++;
     CKR(sort_pairs(c, ar, NE, &k2, &p2, 32 + bits_for(R)));
     k_uq_first<<<grid_for(NE, 256, c->sm_count), 256, 0, s>>>(NE, k2, p2, first_in_set);
@@ -5873,7 +5555,7 @@ static int mixed_render(cco_ctx *c, Arena &ar, const cco_event_log *lg, const ch
   for (int t = 0; t < T; ++t) {
     const cco_mixed_query_t *q = tq[t];
     tpiece[t] = (int32_t)pieces.size();
-    std::vector<std::string> p = mq_template(q);
+    std::vector<std::string> p = mq_template(q, in.one);
     pieces.insert(pieces.end(), p.begin(), p.end());
     tflag[t] = (uint8_t)((q->history_in_must ? kMqHistInMust : 0) | (q->similar_in_must ? kMqSimilarInMust : 0) |
                          (q->exclude_self ? kMqExcludeSelf : 0) | (q->with_set ? kMqWithSet : 0));
@@ -5901,8 +5583,8 @@ static int mixed_render(cco_ctx *c, Arena &ar, const cco_event_log *lg, const ch
   a.rec_doc = rec_doc;
   a.rec_key = rec_key;
   a.rec_set = rec_set;
-  a.rec_tpl = in.rec_tpl;
-  a.h = uq_args(h, lg, nq, 0);
+  a.rec_tpl = rec_tpl;
+  a.h = uq_args(h, lg, nq);
   a.tpiece = d_tpiece;
   a.hbeg = d_hbeg;
   a.hname = d_hname;
@@ -5926,24 +5608,36 @@ static int mixed_render(cco_ctx *c, Arena &ar, const cco_event_log *lg, const ch
   a.list_shared = in.list_shared;
   a.first_in_list = first_in_list;
   a.lkey = lkey;
-  a.soff = in.soff;
+  a.soff = soff;
   a.elem_at = D + NI + NL;
   a.first_in_set = first_in_set;
   a.toff = tp.off;
   a.tbytes = tp.bytes;
-  return emit_records(c, ar, R, k_mq_record<false>, k_mq_record<true>, a, out_body, out_len, out_offsets, out_n);
+  return emit_records(c, ar, R, k_mq_record<false>, k_mq_record<true>, a, out_body, out_len, out_offsets, out_n, [&]() -> int {
+    if (in.one.rows != kMqEveryDoc || !in.one.keys) return CCO_OK;
+    // the documents' decoded _ids, in body order
+    int64_t *io = (int64_t *)c->pinned_get(sizeof(int64_t) * ((size_t)D + 1), /*for_result=*/false);
+    char *ib = (char *)c->pinned_get((size_t)std::max<long long>(bd.ids_bytes, 1), /*for_result=*/false);
+    if (!io || !ib) return set_error(CCO_E_OOM, "pinned host allocation failed");
+    io[0] = 0;
+    if (D > 0) CK(cudaMemcpyAsync(io, bd.ids.off, sizeof(int64_t) * ((size_t)D + 1), cudaMemcpyDeviceToHost, s));
+    if (bd.ids_bytes > 0) CK(cudaMemcpyAsync(ib, bd.ids.w, (size_t)bd.ids_bytes, cudaMemcpyDeviceToHost, s));
+    *in.one.keys = cco_dictionary_t{D, io, ib};
+    return CCO_OK;
+  });
 }
 
 static int mixed_queries(cco_ctx *c, const cco_event_log *lg, const char *body, int64_t body_len, const cco_mixed_query_t *q, long long R,
                          const int64_t *uoff, const char *ubytes, const uint8_t *uval, const int64_t *ioff, const char *ibytes,
                          const uint8_t *ival, const int64_t *set_off, const int64_t *eoff, const char *ebytes, const uint8_t *sval,
-                         bool any_user, char **out_body, int64_t *out_len, int64_t **out_offsets, int64_t *out_n) {
+                         bool any_user, const MqSingle &one, char **out_body, int64_t *out_len, int64_t **out_offsets, int64_t *out_n) {
   cudaStream_t s = c->stream;
   CK(cudaSetDevice(c->device));
   Arena ar(s);
-  NvtxRange nvtx("cco:mixed_queries");
+  NvtxRange nvtx(one.range);
   mail_reset(c);
   MqRows in;
+  in.one = one;
   in.R = R;
   in.NI = ioff ? R : 0;
   in.NL = q->n_blacklist_items;
@@ -5966,12 +5660,12 @@ static int mixed_queries(cco_ctx *c, const cco_event_log *lg, const char *body, 
       CK(cudaMemcpyAsync(d, h_valid[k], (size_t)(R + 7) / 8, cudaMemcpyHostToDevice, s));
       in.valid[k] = d;
     }
-  in.col[0] = uoff != nullptr;
-  in.col[1] = ioff != nullptr;
+  in.col[0] = uoff != nullptr || one.rows == kMqEveryUser;
+  in.col[1] = ioff != nullptr || one.rows == kMqEveryDoc;
   in.col[2] = set_off != nullptr;
-  CKR(ar.alloc(&in.soff, R + 1));
   if (set_off) {
     long long *stmp;
+    CKR(ar.alloc(&in.soff, R + 1));
     CKR(ar.alloc(&stmp, R + 1));
     CK(cudaMemcpyAsync(stmp, set_off, sizeof(int64_t) * ((size_t)R + 1), cudaMemcpyHostToDevice, s));
     if (R > 0) {
@@ -5980,14 +5674,10 @@ static int mixed_queries(cco_ctx *c, const cco_event_log *lg, const char *body, 
     }
     k_rebase<<<grid_for(R + 1, 256, c->sm_count), 256, 0, s>>>(R + 1, stmp, -s0, in.soff);
     c->launches++;
-  } else {
-    CK(cudaMemsetAsync(in.soff, 0, sizeof(long long) * ((size_t)R + 1), s));
   }
   const long long lo[2] = {0, in.NL};
   CKR(ar.alloc(&in.loff, 2));
   CK(cudaMemcpyAsync(in.loff, lo, sizeof lo, cudaMemcpyHostToDevice, s));
-  CKR(ar.alloc(&in.rec_tpl, std::max<long long>(R, 1)));
-  CK(cudaMemsetAsync(in.rec_tpl, 0, sizeof(int32_t) * (size_t)std::max<long long>(R, 1), s));
   in.sec = {KeySection{in.NI, ioff, ibytes}, KeySection{in.NL, q->blacklist_item_offsets, q->blacklist_item_bytes},
             KeySection{in.NE, eoff ? eoff + s0 : nullptr, ebytes}};
   in.tpl_user = {(uint8_t)(any_user ? 1 : 0)};
@@ -6015,7 +5705,117 @@ int cco_mixed_queries(cco_ctx_t *ctx, const cco_event_log_t *lg, const char *ind
   if (mq_any(n_rows, item_offsets, item_validity) && !index_body)
     return set_error(CCO_E_INVALID_ARG, "a row has an item: its similar items need an index body");
   return mixed_queries(ctx, lg, index_body, index_len, q, n_rows, user_offsets, user_bytes, user_validity, item_offsets, item_bytes,
-                       item_validity, set_offsets, elem_offsets, elem_bytes, set_validity, any_user, out_body, out_len, out_offsets, out_n);
+                       item_validity, set_offsets, elem_offsets, elem_bytes, set_validity, any_user, MqSingle{}, out_body, out_len,
+                       out_offsets, out_n);
+}
+
+// ---- the single builders: each query a row of a mixed batch with one member -------------------------------------------
+int cco_event_log_user_queries(cco_ctx_t *ctx, const cco_event_log_t *lg, const cco_user_query_t *q, int64_t n_users,
+                               const int64_t *user_offsets, const char *user_bytes, char **out_body, int64_t *out_len,
+                               int64_t **out_offsets, int64_t *out_n, cco_dictionary_t *out_users) {
+  if (!ctx || !lg || !q || !out_body || !out_len || !out_offsets || !out_n) return set_error(CCO_E_INVALID_ARG, "null argument");
+  if (!ctx->members.empty() || lg->ctx != ctx) return set_error(CCO_E_UNSUPPORTED, "build queries on the per-GPU context that read the log");
+  CKR(log_state(lg, true));
+  CKR(uq_check_host(q, n_users, user_offsets, user_bytes));
+  if (!lg->history) return set_error(CCO_E_INVALID_ARG, "the log was read without history retention (cco_event_log_begin_ex, CCO_LOG_KEEP_HISTORY)");
+  if (out_users) *out_users = cco_dictionary_t{0, nullptr, nullptr};
+  cco_mixed_query_t m{};
+  m.n_names = q->n_names;
+  m.n_history_names = q->n_history_names;
+  m.names = q->names;
+  m.limits = q->limits;
+  m.n_blacklist_names = q->n_blacklist_names;
+  m.history_in_must = q->history_in_must;
+  m.blacklist_names = q->blacklist_names;
+  m.history_boost = q->boost;
+  m.max_query_events = 1;
+  m.head = q->head;
+  m.boosted = q->should;
+  m.should_tail = "";
+  m.must = q->must;
+  m.must_not = q->must_not;
+  m.sort = q->sort;
+  m.header = q->header;
+  m.n_blacklist_items = q->n_blacklist_items;
+  m.blacklist_item_offsets = q->blacklist_item_offsets;
+  m.blacklist_item_bytes = q->blacklist_item_bytes;
+  MqSingle one;
+  one.range = "cco:user_queries";
+  if (!user_offsets) {
+    one.rows = kMqEveryUser;
+    one.keys = out_users;
+  }
+  // the history is built even for no row
+  return mixed_queries(ctx, lg, nullptr, 0, &m, user_offsets ? n_users : 0, user_offsets, user_bytes, nullptr, nullptr, nullptr, nullptr,
+                       nullptr, nullptr, nullptr, nullptr, true, one, out_body, out_len, out_offsets, out_n);
+}
+
+int cco_item_queries(cco_ctx_t *ctx, const char *index_body, int64_t index_len, const cco_item_query_t *q, int64_t n_items,
+                     const int64_t *item_offsets, const char *item_bytes, char **out_body, int64_t *out_len, int64_t **out_offsets,
+                     int64_t *out_n, cco_dictionary_t *out_items) {
+  if (!ctx || !q || !out_body || !out_len || !out_offsets || !out_n || index_len < 0 || (index_len > 0 && !index_body))
+    return set_error(CCO_E_INVALID_ARG, "null argument or negative length");
+  if (!ctx->members.empty()) return set_error(CCO_E_UNSUPPORTED, "per-GPU contexts only");
+  if (index_len > 0 && index_body[index_len - 1] != '\n') return set_error(CCO_E_INVALID_ARG, "the body does not end in a newline");
+  CKR(iq_check_host(q, n_items, item_offsets, item_bytes));
+  if (out_items) *out_items = cco_dictionary_t{0, nullptr, nullptr};
+  cco_mixed_query_t m{};
+  m.n_model_names = q->n_names;
+  m.model_names = q->names;
+  m.max_query_events = q->max_query_events;
+  m.similar_in_must = q->similar_in_must;
+  m.similar_boost = q->similar_boost;
+  m.exclude_self = q->exclude_self;
+  m.head = q->head;
+  m.boosted = "";
+  m.should_tail = q->should;
+  m.must = q->must;
+  m.must_not = q->must_not;
+  m.sort = q->sort;
+  m.header = q->header;
+  m.n_blacklist_items = q->n_blacklist_items;
+  m.blacklist_item_offsets = q->blacklist_item_offsets;
+  m.blacklist_item_bytes = q->blacklist_item_bytes;
+  MqSingle one;
+  one.range = "cco:item_queries";
+  one.should_head = q->should_head;
+  one.must_head = q->must_head;
+  one.what = "items + blacklist items";
+  if (!item_offsets) {
+    one.rows = kMqEveryDoc;
+    one.keys = out_items;
+  }
+  // an empty body, NULL or not, holds no document
+  return mixed_queries(ctx, nullptr, index_len > 0 ? index_body : "", index_len, &m, item_offsets ? n_items : 0, nullptr, nullptr, nullptr,
+                       item_offsets, item_bytes, nullptr, nullptr, nullptr, nullptr, nullptr, false, one, out_body, out_len, out_offsets,
+                       out_n);
+}
+
+int cco_item_set_queries(cco_ctx_t *ctx, const cco_item_set_query_t *q, int64_t n_sets, const int64_t *set_offsets, int64_t n_elements,
+                         const int64_t *elem_offsets, const char *elem_bytes, char **out_body, int64_t *out_len, int64_t **out_offsets,
+                         int64_t *out_n) {
+  if (!ctx || !q || !out_body || !out_len || !out_offsets || !out_n) return set_error(CCO_E_INVALID_ARG, "null argument");
+  if (!ctx->members.empty()) return set_error(CCO_E_UNSUPPORTED, "per-GPU contexts only");
+  CKR(is_check_host(q, n_sets, set_offsets, n_elements, elem_offsets, elem_bytes));
+  cco_mixed_query_t m{};
+  m.max_query_events = 1;
+  m.set_name = q->name;
+  m.with_set = q->with_set;
+  m.set_boost = q->boost;
+  m.head = q->head;
+  m.boosted = q->should_head;
+  m.should_tail = q->should_tail;
+  m.must = q->must;
+  m.must_not = q->must_not;
+  m.sort = q->sort;
+  m.header = q->header;
+  m.n_blacklist_items = q->n_blacklist_items;
+  m.blacklist_item_offsets = q->blacklist_item_offsets;
+  m.blacklist_item_bytes = q->blacklist_item_bytes;
+  MqSingle one;
+  one.range = "cco:item_set_queries";
+  return mixed_queries(ctx, nullptr, nullptr, 0, &m, n_sets, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, set_offsets, elem_offsets,
+                       elem_bytes, nullptr, false, one, out_body, out_len, out_offsets, out_n);
 }
 
 // ---- batchpredict query files: the lines read on the device, the templates planned by the caller, the rows rendered -----

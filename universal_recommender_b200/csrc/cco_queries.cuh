@@ -1,7 +1,8 @@
-// cco_queries.cuh -- cco_event_log_user_queries: buildQuery (URAlgorithm.scala:563-739) for user queries over the training
-// history an event log keeps (cco_event_log_begin_ex with CCO_LOG_KEEP_HISTORY); cco_item_queries: the same for item
-// queries over a model index body; cco_item_set_queries: the same for item-set queries over the caller's sets (the kernels
-// of each are listed with them, below the user-query ones).
+// cco_queries.cuh -- buildQuery (URAlgorithm.scala:563-839) on the device.  Every query builder renders its records as rows
+// of a mixed batch (k_mq_record): cco_event_log_user_queries, cco_item_queries and cco_item_set_queries as rows with one
+// member, cco_mixed_queries and cco_query_file_queries as rows with any.  The stages that feed it are listed with them: the
+// training history an event log keeps (cco_event_log_begin_ex with CCO_LOG_KEEP_HISTORY), the similar items of a model
+// index body, the set elements, then the mixed rows and the query file's lines.
 //
 // e = one training event of a query event name (name rank q); its user and item are dense group ids of the log's columns.
 //   k_uq_select       e -> (log entry, name rank) over the query names' ranges of the name-partitioned columns
@@ -11,10 +12,9 @@
 //   k_uq_hist_keys    the first `limit` of every (user, q) segment: (segment, item) keys, fed oldest first, so that the
 //                     first of each run after the stable sort is the item's oldest position (distinct after the prepend)
 //   k_uq_first        first of each run of equal keys -> keep flag
-//   k_uq_min_line     each user's first line (the record order when every user is asked for)
-//   k_uq_record       one warp per record: template pieces, history lists oldest first, the blacklist; a length pass and a
-//                     write pass (k_doc_len -> scan -> k_doc_write, as cco_format_model).  Ids are escaped as json4s
-//                     3.2 quotes them.
+//   k_uq_min_line     each user's first line (the row order when every user is asked for)
+//   k_uq_user_keys    (first line, user) pairs for that order's sort
+//   k_uq_user_entry   the log entry that names each row's user, for the users' dictionary
 #pragma once
 
 namespace cco {
@@ -111,11 +111,6 @@ __global__ void k_uq_first(long long n, const unsigned long long *__restrict__ k
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
     if (key[i] != ~0ULL && (i == 0 || key[i - 1] != key[i])) keep[pos[i]] = 1;
 }
-// blacklistItems: an entry is kept iff it is its string's first appearance in the list
-__global__ void k_uq_list_first(long long n, const int32_t *__restrict__ lid, const uint32_t *__restrict__ first_sorted, uint8_t *__restrict__ keep) {
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-    keep[i] = first_sorted[lid[i]] == (uint32_t)i ? 1 : 0;
-}
 __global__ void k_uq_min_line(long long E, const int32_t *__restrict__ uid, const long long *__restrict__ ln, unsigned long long *__restrict__ mn) {
   for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < E; e += (long long)gridDim.x * blockDim.x)
     atomicMin(&mn[uid[e]], (unsigned long long)ln[e]);
@@ -176,35 +171,28 @@ __device__ __forceinline__ long long uq_escape(const unsigned char *__restrict__
   return k;
 }
 
+// the users' history lists
 struct UqArgs {
-  long long n_rec;
-  const int32_t *rec_uid;          // [n_rec] user group, -1: a user without history
-  int nq, n_kept;                  // query names; history lists written for q < n_kept
+  int nq;                          // query names
   const int32_t *limit;            // [nq]
   const long long *hstart;         // [G * nq + 1] segment starts in the (user, q) order
   const uint32_t *hord;            // [E] events in (user, q, time desc, line desc) order
   const uint8_t *keep_h;           // [E] by position: taken and the item's oldest taken position
-  const long long *bstart;         // [G + 1]
-  const uint32_t *bord;            // [B] blacklisted events in (user, time desc, line desc) order
-  const uint8_t *keep_b;           // [B] by position: the item's newest position
-  const unsigned long long *bkey;  // [B] (user << 32 | item), sorted
-  long long B;
   const uint32_t *ent;             // [E] log entry of each event
   const long long *ioff;           // the log's training item column
   const unsigned char *ibytes;
-  long long n_list;                // blacklistItems
-  const long long *loff;           // the caller's offsets: bytes at lbytes[loff[i] - lbase]
-  long long lbase;
-  const unsigned char *lbytes;
-  const int32_t *lgid;             // item group or -1
-  const uint8_t *keep_l;
-  const long long *toff;           // [n_kept + 3] template pieces
-  const unsigned char *tbytes;
 };
 
-// whether user u's blacklisted items hold item group g; B: UqArgs or MqBlack (bstart, bkey)
-template <class B>
-__device__ __forceinline__ bool uq_has(const B &a, int32_t u, int32_t g) {
+// the blacklisted items of the users under one set of blacklisted query names (uq_blacklist)
+struct MqBlack {
+  const long long *bstart;         // [G + 1]
+  const unsigned long long *bkey;  // [B] (user << 32 | item), sorted
+  const uint32_t *bord;            // [B] blacklisted events in (user, time desc, line desc) order
+  const uint8_t *keep_b;           // [B] by position: the item's newest position
+};
+
+// whether user u's blacklisted items hold item group g
+__device__ __forceinline__ bool uq_has(const MqBlack &a, int32_t u, int32_t g) {
   const unsigned long long x = ((unsigned long long)(uint32_t)u << 32) | (uint32_t)g;
   long long lo = a.bstart[u], hi = a.bstart[u + 1];
   while (lo < hi) {
@@ -214,8 +202,8 @@ __device__ __forceinline__ bool uq_has(const B &a, int32_t u, int32_t g) {
   return lo < a.bstart[u + 1] && a.bkey[lo] == x;
 }
 
-// One record of a query builder, written by one warp at o (the write pass) or only measured (o == nullptr): cur is the
-// warp-uniform byte count so far.
+// One record, written by one warp at o (the write pass) or only measured (o == nullptr): cur is the warp-uniform byte count
+// so far.
 template <bool WRITE>
 struct RecordOut {
   unsigned char *o;
@@ -235,8 +223,7 @@ struct RecordOut {
     cur += 1;
   }
   // one list of quoted, comma-separated ids from n candidates; get(i, &ptr, &len) == false skips candidate i.  first is
-  // warp-uniform.  The write tests o, not WRITE: with WRITE, ptxas holds k_iq_record's write pass to 40 registers and
-  // spills.
+  // warp-uniform.  The write tests o, not WRITE: testing WRITE here has made ptxas spill in a record kernel's write pass.
   template <class Get>
   __device__ __forceinline__ void list(long long n, const Get &get, bool &first) {
     for (long long b = 0; b < n; b += 32) {
@@ -266,61 +253,10 @@ struct RecordOut {
   }
 };
 
-template <bool WRITE>
-__global__ void __launch_bounds__(256) k_uq_record(UqArgs a, const long long *__restrict__ rec_off, long long *__restrict__ rec_len,
-                                                   unsigned char *__restrict__ out) {
-  const int lane = threadIdx.x & 31;
-  const long long warps = (long long)gridDim.x * (blockDim.x >> 5);
-  for (long long r = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5; r < a.n_rec; r += warps) {
-    const int32_t u = a.rec_uid[r];
-    RecordOut<WRITE> w{WRITE ? out + rec_off[r] : nullptr, 0, lane};
-    for (int j = 0; j <= a.n_kept + 1; ++j) {
-      w.piece(a, j);
-      if (j > a.n_kept) break;
-      bool first = true;
-      if (j < a.n_kept) {   // the history of name j, oldest first, each item at its first position
-        if (u < 0) continue;
-        const unsigned long long s = (unsigned long long)u * a.nq + j;
-        const long long h0 = a.hstart[s], cnt = min(a.hstart[s + 1] - h0, (long long)a.limit[j]);
-        w.list(cnt, [&](long long i, const unsigned char **p, long long *len) {
-          const long long pos = h0 + cnt - 1 - i;
-          if (!a.keep_h[pos]) return false;
-          const uint32_t e = a.ent[a.hord[pos]];
-          *p = a.ibytes + a.ioff[e];
-          *len = a.ioff[e + 1] - a.ioff[e];
-          return true;
-        }, first);
-      } else {   // the blacklist: the user's blacklisted items newest first, then blacklistItems, distinct
-        if (u >= 0) {
-          const long long b0 = a.bstart[u];
-          w.list(a.bstart[u + 1] - b0, [&](long long i, const unsigned char **p, long long *len) {
-            if (!a.keep_b[b0 + i]) return false;
-            const uint32_t e = a.ent[a.bord[b0 + i]];
-            *p = a.ibytes + a.ioff[e];
-            *len = a.ioff[e + 1] - a.ioff[e];
-            return true;
-          }, first);
-        }
-        w.list(a.n_list, [&](long long i, const unsigned char **p, long long *len) {
-          if (!a.keep_l[i] || (u >= 0 && a.lgid[i] >= 0 && uq_has(a, u, a.lgid[i]))) return false;
-          *p = a.lbytes + (a.loff[i] - a.lbase);
-          *len = a.loff[i + 1] - a.loff[i];
-          return true;
-        }, first);
-      }
-    }
-    if (!WRITE && lane == 0) rec_len[r] = w.cur;
-  }
-}
-
-// ---- cco_item_queries: buildQuery for item queries over a model index body (parsed by cco_json.cuh) ----------------------
+// ---- the similar items of a model index body (parsed by cco_json.cuh) -------------------------------------------------
 //   k_iq_pick      per document: the last source member of each model name (T distinct names), -1
-//   k_iq_black     blacklistItems: the first list index of each key group (membership and distinct are group tests)
-//   k_iq_rec       per record: its document (-1: none) and key entry; the queried documents flagged
 //   k_iq_array     one warp per (queried document, name) value span: the array-of-strings grammar and the raw element spans,
 //                  a count pass and a write pass; an error word for the first bad span
-//   k_iq_record    one warp per record: template pieces, the sliced similar-items lists and the exclusion list, a length
-//                  pass and a write pass (as k_uq_record)
 __global__ void k_iq_pick(long long n_docs, int T, const long long *__restrict__ line_moff, const int32_t *__restrict__ ngid,
                           const int32_t *__restrict__ entry_of, int32_t *__restrict__ pick) {
   for (long long d = blockIdx.x * (long long)blockDim.x + threadIdx.x; d < n_docs; d += (long long)gridDim.x * blockDim.x) {
@@ -332,24 +268,6 @@ __global__ void k_iq_pick(long long n_docs, int T, const long long *__restrict__
     }
   }
 }
-__global__ void k_iq_black(long long n, long long at, const int32_t *__restrict__ gid, uint32_t *__restrict__ first_in_list) {
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-    atomicMin(&first_in_list[gid[at + i]], (uint32_t)i);
-}
-// every document (all): record r is document r; else record r is key entry n_docs + r, found when its group's first entry
-// is a document (the documents come first in the key column)
-__global__ void k_iq_rec(long long R, long long n_docs, bool all, const int32_t *__restrict__ gid, const uint32_t *__restrict__ first_sorted,
-                         int32_t *__restrict__ rec_doc, int32_t *__restrict__ rec_key, uint8_t *__restrict__ queried) {
-  for (long long r = blockIdx.x * (long long)blockDim.x + threadIdx.x; r < R; r += (long long)gridDim.x * blockDim.x) {
-    const long long k = all ? r : n_docs + r;
-    const uint32_t f = first_sorted[gid[k]];
-    const int32_t d = (long long)f < n_docs ? (int32_t)f : -1;
-    rec_doc[r] = d;
-    rec_key[r] = (int32_t)k;
-    if (d >= 0) queried[d] = 1;
-  }
-}
-
 // Grammar of a picked value: '[' ws* ( ']' | string (ws* ',' ws* string)* ws* ']' ) -- the span is trimmed, its strings were
 // validated by k_json_members.  The string and escape masks are k_json_members': escaped byte = an odd run of backslashes
 // right before it, in string = prefix XOR of the unescaped quotes.  Events are the unescaped quotes and the non-whitespace
@@ -420,88 +338,10 @@ __global__ void __launch_bounds__(256) k_iq_array(long long n, int T, const uint
   }
 }
 
-struct IqArgs {
-  long long n_rec;
-  const int32_t *rec_doc;          // [n_rec] document, -1
-  const int32_t *rec_key;          // [n_rec] key entry of the record's item
-  const int32_t *kgid;             // key column: decoded _ids, the items, blacklistItems; group per entry
-  const long long *koff;
-  const unsigned char *kbytes;
-  const long long *line_moff;      // the source of document d has members iff line_moff[2 d + 2] > line_moff[2 d + 1]
-  int T, n_names;                  // distinct model names; model names
-  const int32_t *name_entry;       // [n_names] distinct entry of each model name
-  const long long *eoff;           // [D * T + 1] first element of (d, t)
-  const long long *doff;           // decoded elements
-  const unsigned char *dbytes;
-  long long slice;                 // max_query_events
-  int in_must, exclude_self;
-  long long n_list, list_at;       // blacklistItems are key entries list_at + i
-  const uint32_t *first_in_list;   // per group: first list index, ~0
-  const long long *toff;           // [n_names + 10] template pieces (see iq_template)
-  const unsigned char *tbytes;
-};
-
-template <bool WRITE>
-__global__ void __launch_bounds__(256) k_iq_record(IqArgs a, const long long *__restrict__ rec_off, long long *__restrict__ rec_len,
-                                                   unsigned char *__restrict__ out) {
-  const int lane = threadIdx.x & 31;
-  const long long warps = (long long)gridDim.x * (blockDim.x >> 5);
-  for (long long r = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5; r < a.n_rec; r += warps) {
-    const int32_t d = a.rec_doc[r], key = a.rec_key[r];
-    const bool similar = d >= 0 && a.line_moff[2 * (long long)d + 2] > a.line_moff[2 * (long long)d + 1];
-    RecordOut<WRITE> w{WRITE ? out + rec_off[r] : nullptr, 0, lane};
-    // a clause list: head fragment, the similar items (when here), tail fragment, comma-separated
-    auto section = [&](int head, bool here, int tail) {
-      bool any = w.piece(a, head);
-      for (int j = 0; here && similar && j < a.n_names; ++j) {
-        if (any) w.comma();
-        w.piece(a, 9 + j);
-        const long long x = (long long)d * a.T + a.name_entry[j], e0 = a.eoff[x], n = a.eoff[x + 1] - e0;
-        bool first = true;
-        w.list(n <= a.slice ? n : a.slice - 1, [&](long long i, const unsigned char **p, long long *len) {
-          *p = a.dbytes + a.doff[e0 + i];
-          *len = a.doff[e0 + i + 1] - a.doff[e0 + i];
-          return true;
-        }, first);
-        w.piece(a, 8);
-        any = true;
-      }
-      if (a.toff[tail + 1] > a.toff[tail]) {
-        if (any) w.comma();
-        w.piece(a, tail);
-      }
-    };
-    w.piece(a, 0);
-    section(1, !a.in_must, 2);
-    w.piece(a, 3);
-    section(4, a.in_must, 5);
-    w.piece(a, 6);
-    bool first = true;   // blacklistItems, each once, then the item unless it is among them
-    w.list(a.n_list, [&](long long i, const unsigned char **p, long long *len) {
-      const long long k = a.list_at + i;
-      if (a.first_in_list[a.kgid[k]] != (uint32_t)i) return false;
-      *p = a.kbytes + a.koff[k];
-      *len = a.koff[k + 1] - a.koff[k];
-      return true;
-    }, first);
-    if (a.exclude_self && a.first_in_list[a.kgid[key]] == ~0u)
-      w.list(1, [&](long long, const unsigned char **p, long long *len) {
-        *p = a.kbytes + a.koff[key];
-        *len = a.koff[key + 1] - a.koff[key];
-        return true;
-      }, first);
-    w.piece(a, 7);
-    if (!WRITE && lane == 0) rec_len[r] = w.cur;
-  }
-}
-
-// ---- cco_item_set_queries: buildQuery for item-set queries over the caller's sets ----------------------------------------
-// The key column is blacklistItems ++ the elements, grouped exactly by str_group; blacklist membership is k_iq_black's
-// first_in_list, and "first occurrence within its set" is the first of each run of (set << 32 | group) keys after one stable
-// sort (k_uq_first).
+// ---- the sets' elements and the blacklistItems lists ------------------------------------------------------------------
+// "First occurrence within its set (list)" is the first of each run of (set << 32 | group) keys after one stable sort
+// (k_uq_first).
 //   k_is_keys      per element: the key (set << 32 | group), its position as value (the set by a search of the set offsets)
-//   k_is_record    one warp per set: template pieces, the set clause's elements as given, the exclusion list, a length pass
-//                  and a write pass (as k_uq_record)
 __global__ void k_is_keys(long long NE, long long n_sets, const long long *__restrict__ soff, const int32_t *__restrict__ egid,
                           unsigned long long *__restrict__ key, uint32_t *__restrict__ pos) {
   for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < NE; e += (long long)gridDim.x * blockDim.x) {
@@ -515,69 +355,8 @@ __global__ void k_is_keys(long long NE, long long n_sets, const long long *__res
   }
 }
 
-struct IsArgs {
-  long long n_sets;
-  const long long *soff;           // [n_sets + 1] element index of each set's start, 0-based
-  const int32_t *kgid;             // key column: blacklistItems, then the elements; group per entry
-  const long long *koff;
-  const unsigned char *kbytes;
-  long long n_list;                // blacklistItems are key entries 0 .. n_list - 1, element e is entry n_list + e
-  const uint32_t *first_in_list;   // per group: first list index, ~0
-  const uint8_t *first_in_set;     // [n_elements] the element is its string's first occurrence in its set
-  int with_set;
-  const long long *toff;           // [8] template pieces (see is_template)
-  const unsigned char *tbytes;
-};
-
-// (256, 1): without the minimum, ptxas holds the length pass to 32 registers and spills its loop state; with it the two
-// passes take 36 and 46 registers and spill nothing
-template <bool WRITE>
-__global__ void __launch_bounds__(256, 1) k_is_record(IsArgs a, const long long *__restrict__ rec_off, long long *__restrict__ rec_len,
-                                                   unsigned char *__restrict__ out) {
-  const int lane = threadIdx.x & 31;
-  const long long warps = (long long)gridDim.x * (blockDim.x >> 5);
-  for (long long r = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5; r < a.n_sets; r += warps) {
-    const long long e0 = a.soff[r], n = a.soff[r + 1] - e0, k0 = a.n_list + e0;
-    RecordOut<WRITE> w{WRITE ? out + rec_off[r] : nullptr, 0, lane};
-    w.piece(a, 0);
-    bool any = w.piece(a, 1);   // should: should_head, the set clause, should_tail
-    if (a.with_set) {
-      if (any) w.comma();
-      w.piece(a, 2);
-      bool first = true;   // every element as given
-      w.list(n, [&](long long i, const unsigned char **p, long long *len) {
-        *p = a.kbytes + a.koff[k0 + i];
-        *len = a.koff[k0 + i + 1] - a.koff[k0 + i];
-        return true;
-      }, first);
-      w.piece(a, 3);
-      any = true;
-    }
-    if (a.toff[5] > a.toff[4]) {
-      if (any) w.comma();
-      w.piece(a, 4);
-    }
-    w.piece(a, 5);
-    bool first = true;   // blacklistItems, each once, then the set's first occurrences that are not among them
-    w.list(a.n_list, [&](long long i, const unsigned char **p, long long *len) {
-      if (a.first_in_list[a.kgid[i]] != (uint32_t)i) return false;
-      *p = a.kbytes + a.koff[i];
-      *len = a.koff[i + 1] - a.koff[i];
-      return true;
-    }, first);
-    w.list(n, [&](long long i, const unsigned char **p, long long *len) {
-      if (!a.first_in_set[e0 + i] || a.first_in_list[a.kgid[k0 + i]] != ~0u) return false;
-      *p = a.kbytes + a.koff[k0 + i];
-      *len = a.koff[k0 + i + 1] - a.koff[k0 + i];
-      return true;
-    }, first);
-    w.piece(a, 6);
-    if (!WRITE && lane == 0) rec_len[r] = w.cur;
-  }
-}
-
-// ---- cco_mixed_queries: buildQuery for rows with any subset of {user, item, item set} --------------------------------------
-// The history comes from cco_event_log_user_queries' stage (UqHistory), the similar items from cco_item_queries' (IqDocs).
+// ---- the records: buildQuery for rows with any subset of {user, item, item set} ------------------------------------------
+// The history comes from the history stage (UqHistory), the similar items from the documents' stage (IqDocs).
 // One key column holds the decoded _ids, the items, blacklistItems and the set elements, grouped exactly; the items,
 // blacklistItems and elements are also probed into the log's item table, so that every test of the exclusion list
 // distinct(userBlacklisted ++ blacklistItems :+ item ++ itemSet) is a group test: the user's blacklist by uq_has,
@@ -585,7 +364,8 @@ __global__ void __launch_bounds__(256, 1) k_is_record(IsArgs a, const long long 
 //   k_mq_rows      per row: which members it has (LSB-first validity bitmaps, nullptr: every row); its document; the queried
 //                  documents flagged
 //   k_mq_record    one warp per row: template pieces, history lists, similar-items lists, the set clause and the exclusion
-//                  list, a length pass and a write pass (as k_uq_record)
+//                  list; a length pass and a write pass (k_doc_len -> scan -> k_doc_write, as cco_format_model).  Ids
+//                  are escaped as json4s 3.2 quotes them.
 __device__ __forceinline__ bool mq_valid(const uint8_t *v, long long r) { return !v || ((v[r >> 3] >> (r & 7)) & 1); }
 
 __global__ void k_mq_rows(long long R, const uint8_t *__restrict__ uvalid, const uint8_t *__restrict__ ivalid,
@@ -608,14 +388,6 @@ __global__ void k_mq_rows(long long R, const uint8_t *__restrict__ uvalid, const
   }
 }
 
-// the blacklisted items of the users under one set of blacklisted query names (uq_blacklist)
-struct MqBlack {
-  const long long *bstart;         // [G + 1]
-  const unsigned long long *bkey;  // [B] (user << 32 | item), sorted
-  const uint32_t *bord;            // [B] blacklisted events in (user, time desc, line desc) order
-  const uint8_t *keep_b;           // [B] by position: the item's newest position
-};
-
 // A row reads everything that is not its own through its template tp = rec_tpl[r]: the template pieces from tpiece[tp] on
 // (see mq_template), its history names hname[hbeg[tp] .. hbeg[tp + 1]) (indices into the union of query names that the
 // history segments were built over), its flags and its user blacklist black[tmask[tp]].
@@ -627,7 +399,7 @@ struct MqArgs {
   const int32_t *rec_key;          // [n_rec] key entry of the item, -1: no item
   const uint8_t *rec_set;          // [n_rec] the row has a set
   const int32_t *rec_tpl;          // [n_rec] template
-  UqArgs h;                        // the history over the union of names (h.n_kept, the blacklist and list members unused)
+  UqArgs h;                        // the history over the union of names
   const int32_t *tpiece;           // [T] first template piece
   const int32_t *hbeg;             // [T + 1]
   const int32_t *hname;            // [hbeg[T]] union name index, -1 for a template no row with a user reads
@@ -670,13 +442,13 @@ __global__ void __launch_bounds__(256, 1) k_mq_record(MqArgs a, const long long 
     const long long e0 = a.soff[r], ne = a.rec_set[r] ? a.soff[r + 1] - e0 : 0, k0 = a.elem_at + e0;
     const bool set_clause = (fl & kMqWithSet) && a.rec_set[r];
     RecordOut<WRITE> w{WRITE ? out + rec_off[r] : nullptr, 0, lane};
-    // should (must = false) or must: history, similar items, then should's boosted metadata, set clause and constant_score,
-    // or must's tail, comma-separated
+    // should (must = false) or must: the head, history, similar items, then should's boosted metadata, set clause and
+    // constant_score, or must's tail, comma-separated
     auto section = [&](bool must) {
-      bool any = false;
+      bool any = w.piece(a, pb + (must ? 12 : 11));
       for (int j = 0; ((fl & kMqHistInMust) != 0) == must && j < n_kept; ++j) {
         if (any) w.comma();
-        w.piece(a, pb + 11 + j);
+        w.piece(a, pb + 13 + j);
         bool first = true;   // the history of name j, oldest first, each item at its first position
         if (u >= 0) {
           const int q = a.hname[h0n + j];
@@ -696,7 +468,7 @@ __global__ void __launch_bounds__(256, 1) k_mq_record(MqArgs a, const long long 
       }
       for (int j = 0; similar && ((fl & kMqSimilarInMust) != 0) == must && j < a.n_names; ++j) {
         if (any) w.comma();
-        w.piece(a, pb + 11 + n_kept + j);
+        w.piece(a, pb + 13 + n_kept + j);
         const long long x = (long long)d * a.T + a.name_entry[j], x0 = a.eoff[x], n = a.eoff[x + 1] - x0;
         bool first = true;
         w.list(n <= a.slice ? n : a.slice - 1, [&](long long i, const unsigned char **p, long long *len) {
