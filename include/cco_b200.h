@@ -789,6 +789,75 @@ int cco_query_file_queries(cco_ctx_t *ctx, const cco_query_file_t *qf, const cco
 int cco_query_file_free(cco_query_file_t *qf);
 
 /*
+ * Search results: the Elasticsearch _msearch responses to query bodies read on the device into what URAlgorithm.predict
+ * returns for each query (URAlgorithm.scala:484-529, EsClient.scala:370-385, Serving.scala:25-29).  Record r is element r
+ * of a body's "responses" array, numbered across appends:
+ *  - an element with an "error" member, or a "status" other than 200, has no hits (the reference's None);
+ *  - otherwise every element of hits.hits, in order, is one hit: its _id decoded, its _score as the double nearest to
+ *    ES's text (a JSON integer too), and for a withRanks record each ranking member of its "_source" that is a number
+ *    (absent or null: none).  A missing or null hits.hits has no hits;
+ *  - total is hits.total (a number, or ES 7's {"value": ...}), -1 when absent; status is the element's "status", 0 when
+ *    absent.  Of a repeated member other than _id and _score the first counts.
+ * With CCO_SR_TEXT the PredictedResult of every record is rendered as PredictionIO serves it:
+ * {"itemScores":[{"item":"<id>","score":<double>,"ranks":{"<name>":<double>,...}}]}, ids and names through json4s' quote,
+ * doubles as Java's Double.toString over the shortest digits, ranks in the order of the names and left out when a hit has
+ * none.  Numbers with at most 15 significant digits and a decimal exponent within +-22 are converted on the device; the
+ * others (n_exact) on the host, exactly.
+ * Streaming: begin, any number of appends (one complete response body each; the next body's copy to the device overlaps
+ * the read of the previous one, so a body's error may be returned by the next append or by finish), finish, free.  After
+ * a failed append or finish every call but free fails with the same message.
+ *  - n_records: the elements the body must hold (the queries of its _msearch request); -1: any number;
+ *  - with_ranks: LSB-first bitmap over the body's records (nullable: CCO_SR_WITH_RANKS of params for every record);
+ *  - line_offsets[n_records + 1] / line_bytes (nullable; then with_ranks must be NULL): the query-file lines of the body's
+ *    records, line r = line_bytes[line_offsets[r] .. line_offsets[r + 1]).  Each line must be one JSON object; its
+ *    withRanks, as cco_query_file_read reads it (true or false, null = absent, at most once), is the record's.  With
+ *    CCO_SR_BATCHPREDICT record r's text is PredictionIO's BatchPredict output line [RECALL] without its newline:
+ *    {"query":<line r re-rendered by json4s>,"prediction":<the PredictedResult>}.  The echo drops insignificant
+ *    whitespace, decodes and re-quotes strings (json4s' quote), prints integer literals as BigInt does (-0 -> 0) and other
+ *    numbers as the scores are printed; member order and repeated members are kept.  A line is checked for JSON syntax
+ *    and nests at most 64 levels; its errors name the record.
+ * Errors: CCO_E_INVALID_ARG for malformed JSON and a top level that is not an object with one "responses" array (with the
+ * body's byte offset), a count mismatch, and, naming the record (and hit), a responses or hits.hits element that is not an
+ * object, hits.hits that is neither an array nor null, a status that is not a 32-bit integer, a hit without a string _id,
+ * a repeated _id or _score, a _score that is missing, null or not a number, a rank that is present but neither a number
+ * nor null, and a number out of the range of a double.  Strings are checked for valid escapes and raw bytes where the reads
+ * go (member names up to _source's, ids); what _source's values hold is checked for closed strings and bracket balance
+ * only.  CCO_E_UNSUPPORTED for group contexts, a body larger than a quarter of the device's memory, and 2^31 or more
+ * records or hits in one body.
+ * Outputs (finish): pinned memory owned by the context, each array released with cco_host_free:
+ *   hit_offsets[n_records + 1], status[n_records], total[n_records]; per hit the ids as an Arrow large_string (id_offsets
+ *   [n_hits + 1], id_bytes), score[n_hits] and ranks[n_hits * n_rankings] (NaN where a hit has no such rank); with
+ *   CCO_SR_TEXT text_offsets[n_records + 1] and text (record r = text[text_offsets[r] .. text_offsets[r + 1])), else NULL.
+ */
+#define CCO_SR_WITH_RANKS 1u         /* every record is a withRanks query */
+#define CCO_SR_TEXT 2u               /* render the PredictedResult text */
+#define CCO_SR_BATCHPREDICT 4u       /* with CCO_SR_TEXT: render batchpredict output lines (every append gives query lines) */
+typedef struct {
+  int32_t n_rankings;                /* 0 .. CCO_MAX_RANKINGS names, in ur_model.rankings_params order; a repeat is one member (the first) */
+  const char *const *ranking_names;  /* UTF-8 */
+  uint32_t flags;
+} cco_search_results_params_t;
+typedef struct {
+  int64_t n_records, n_hits;
+  int32_t n_rankings, reserved;
+  int64_t n_exact;                   /* numbers converted on the host */
+  int64_t *hit_offsets;
+  int32_t *status;
+  int64_t *total;
+  int64_t *id_offsets;
+  char *id_bytes;
+  double *score, *ranks;
+  int64_t *text_offsets;
+  char *text;
+} cco_search_results_out_t;
+typedef struct cco_search_results cco_search_results_t;
+int cco_search_results_begin(cco_ctx_t *ctx, const cco_search_results_params_t *params, cco_search_results_t **out);
+int cco_search_results_append(cco_search_results_t *h, const char *body, int64_t len, int64_t n_records,
+                              const int64_t *line_offsets /* nullable */, const char *line_bytes, const uint8_t *with_ranks /* nullable */);
+int cco_search_results_finish(cco_search_results_t *h, cco_search_results_out_t *out);
+int cco_search_results_free(cco_search_results_t *h);
+
+/*
  * Debug/parity entry (tests only): full integer co-occurrence matrix A^T B of two canonical
  * binary matrices computed by the same accumulation kernel as cco_train, no LLR, no top-k.
  * Output CSR over the columns of A with ascending column ids, malloc'ed; free with cco_free.

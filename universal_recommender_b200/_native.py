@@ -129,6 +129,23 @@ class MixedQueryT(C.Structure):
                 ("n_blacklist_items", C.c_int64), ("blacklist_item_offsets", C.POINTER(C.c_int64)), ("blacklist_item_bytes", C.c_void_p)]
 
 
+class SearchResultsParamsT(C.Structure):
+    _fields_ = [("n_rankings", C.c_int32), ("ranking_names", C.POINTER(C.c_char_p)), ("flags", C.c_uint32)]
+
+
+class SearchResultsOutT(C.Structure):
+    _fields_ = [("n_records", C.c_int64), ("n_hits", C.c_int64), ("n_rankings", C.c_int32), ("reserved", C.c_int32),
+                ("n_exact", C.c_int64), ("hit_offsets", C.POINTER(C.c_int64)), ("status", C.POINTER(C.c_int32)),
+                ("total", C.POINTER(C.c_int64)), ("id_offsets", C.POINTER(C.c_int64)), ("id_bytes", C.c_void_p),
+                ("score", C.POINTER(C.c_double)), ("ranks", C.POINTER(C.c_double)), ("text_offsets", C.POINTER(C.c_int64)),
+                ("text", C.c_void_p)]
+
+
+SR_WITH_RANKS = 1
+SR_TEXT = 2
+SR_BATCHPREDICT = 4
+
+
 class LogRankingT(C.Structure):
     _fields_ = [("name", C.c_char_p), ("mode", C.c_int32), ("n_event_names", C.c_int32), ("start_ms", C.c_int64), ("end_ms", C.c_int64),
                 ("event_names", C.POINTER(C.c_char_p))]
@@ -153,7 +170,7 @@ EXPORTS = [
     "cco_format_model", "cco_rerank_model", "cco_event_log_read", "cco_event_log_info", "cco_event_log_ingest",
     "cco_format_model_log", "cco_rerank_model_log", "cco_event_log_free", "cco_event_log_begin", "cco_event_log_append",
     "cco_event_log_finish", "cco_event_log_begin_window", "cco_event_log_window_stats",
-    "cco_event_log_begin_ex", "cco_event_log_user_queries", "cco_item_queries", "cco_item_set_queries", "cco_mixed_queries", "cco_query_file_read", "cco_query_file_templates", "cco_query_file_queries", "cco_query_file_free", "cco_result_num_matrices", "cco_result_row_range", "cco_result_matrix", "cco_result_stats", "cco_result_free",
+    "cco_event_log_begin_ex", "cco_event_log_user_queries", "cco_item_queries", "cco_item_set_queries", "cco_mixed_queries", "cco_query_file_read", "cco_query_file_templates", "cco_query_file_queries", "cco_query_file_free", "cco_search_results_begin", "cco_search_results_append", "cco_search_results_finish", "cco_search_results_free", "cco_result_num_matrices", "cco_result_row_range", "cco_result_matrix", "cco_result_stats", "cco_result_free",
     "cco_debug_cooccurrence", "cco_debug_downsample", "cco_debug_downsample_block", "cco_debug_llr", "cco_debug_string_ids", "cco_debug_rank_text", "cco_free",
 ]
 
@@ -227,6 +244,10 @@ def lib():
     L.cco_query_file_queries.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_char_p, C.c_int64, C.c_int64, p(MixedQueryT),
                                          p(C.c_void_p), p(C.c_int64), p(C.c_void_p), p(C.c_int64)]
     L.cco_query_file_free.argtypes = [C.c_void_p]
+    L.cco_search_results_begin.argtypes = [C.c_void_p, p(SearchResultsParamsT), p(C.c_void_p)]
+    L.cco_search_results_append.argtypes = [C.c_void_p, C.c_char_p, C.c_int64, C.c_int64, C.c_void_p, C.c_char_p, C.c_void_p]
+    L.cco_search_results_finish.argtypes = [C.c_void_p, p(SearchResultsOutT)]
+    L.cco_search_results_free.argtypes = [C.c_void_p]
     L.cco_mixed_queries.argtypes = [C.c_void_p, C.c_void_p, C.c_char_p, C.c_int64, p(MixedQueryT), C.c_int64,
                                     p(C.c_int64), C.c_void_p, C.c_void_p, p(C.c_int64), C.c_void_p, C.c_void_p,
                                     p(C.c_int64), C.c_int64, p(C.c_int64), C.c_void_p, C.c_void_p,

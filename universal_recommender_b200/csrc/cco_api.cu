@@ -30,6 +30,7 @@
 #include "cco_json.cuh"
 #include "cco_events.cuh"
 #include "cco_queries.cuh"
+#include "cco_results.cuh"
 
 namespace cco {
 
@@ -6412,6 +6413,623 @@ int cco_debug_cooccurrence(cco_ctx_t *c, const cco_csr_t *a, const cco_csr_t *b,
   *row_ptr = rp;
   *col_idx = ci;
   *count = cn;
+  return CCO_OK;
+}
+
+// ---- cco_search_results: _msearch response bodies -> PredictedResults, kernels in cco_results.cuh ----------------------
+struct cco_search_results {
+  cco_ctx *ctx = nullptr;
+  int n_rank = 0;
+  uint32_t flags = 0;
+  std::string names, qnames;           // ranking names (UTF-8) and their json4s quotes, each followed by ':'
+  int name_off[9] = {}, qname_off[9] = {};
+  char *stage[2] = {};                 // pinned staging of the last two bodies
+  size_t stage_cap[2] = {};
+  unsigned char *dbody[2] = {};        // their device copies
+  size_t dcap[2] = {};
+  cudaEvent_t copied[2] = {};
+  long long n_bodies = 0;
+  bool pending = false;                // the last appended body is copied, not yet read
+  long long p_len = 0, p_rec = 0;
+  std::vector<uint8_t> p_ranks;        // its records' withRanks, one byte each (without query lines)
+  bool p_has_lines = false;            // its records' query lines (rebased offsets and bytes, copied at append)
+  std::vector<int64_t> p_loff;
+  std::string p_lines;
+  bool failed = false, finished = false;
+  std::string fail_msg;
+  int fail_code = CCO_OK;
+  // what the read bodies gave, records and hits numbered across bodies
+  std::vector<int64_t> hit_off{0}, total, id_off{0}, text_off{0};
+  std::vector<int32_t> status;
+  std::vector<double> score, ranks;
+  std::string id_bytes, text;
+  long long n_exact = 0;
+};
+
+extern "C++" {
+namespace cco {
+
+static const char *sr_message(int code) {
+  switch (code) {
+    case kSrSyntax: return "malformed JSON";
+    case kSrString: return "a string holds a bad escape or a raw byte < 0x20";
+    case kSrUnbalanced: return "unbalanced or mismatched brackets";
+    case kSrNoResponses: return "the top level is not an object with one \"responses\" array";
+    case kSrElement: return "a responses element is not an object";
+    case kSrStatus: return "status is not a 32-bit integer";
+    case kSrHitsNotArray: return "hits.hits is not an array";
+    case kSrHitNotObject: return "a hits.hits element is not an object";
+    case kSrNoId: return "the hit has no string _id";
+    case kSrRepeated: return "a repeated _id or _score";
+    case kSrNoScore: return "_score is missing, null or not a number";
+    case kSrBadRank: return "a rank is not a number";
+    case kSrLine: return "the query line is not one JSON object";
+    case kSrWithRanks: return "the query line's withRanks is not true, false or null";
+    case kSrLineRepeated: return "the query line repeats withRanks";
+    case kSrLineDeep: return "the query line nests deeper than 64 levels";
+  }
+  return "malformed response";
+}
+static int sr_count_check(long long n, const char *what) {
+  if (n >= (1LL << 31)) return set_error(CCO_E_UNSUPPORTED, "%lld %s in one body: at most 2^31 - 1", n, what);
+  return CCO_OK;
+}
+// the exact path: strtod (correctly rounded) and the shortest %.*e digits that give the same double back
+static int sr_exact_value(const char *t, long long n, SrNum *o) {
+  std::string s(t, (size_t)n);
+  const double v = strtod(s.c_str(), nullptr);
+  if (std::isinf(v)) return 1;
+  SrNum r = {v, 0ULL, 0, 0, s[0] == '-', 0};
+  if (v != 0) {
+    char buf[40];
+    const double a = std::fabs(v);
+    for (int p = 1; p <= 17; ++p) {
+      snprintf(buf, sizeof buf, "%.*e", p - 1, a);
+      if (strtod(buf, nullptr) == a) break;
+    }
+    const char *e = strchr(buf, 'e');
+    unsigned long long dig = 0;
+    int nd = 0;
+    for (const char *q = buf; q < e; ++q)
+      if (*q != '.') {
+        dig = dig * 10 + (unsigned)(*q - '0');
+        ++nd;
+      }
+    int e10 = atoi(e + 1) - (nd - 1);
+    while (dig % 10 == 0) {
+      dig /= 10;
+      ++e10;
+      --nd;
+    }
+    r.dig = dig;
+    r.e10 = e10;
+    r.nd = nd;
+  }
+  *o = r;
+  return 0;
+}
+template <typename T>
+static void sr_append(std::vector<T> &dst, const T *src, long long n, T delta = T()) {
+  const size_t at = dst.size();
+  dst.resize(at + (size_t)n);
+  for (long long i = 0; i < n; ++i) dst[at + i] = src[i] + delta;
+}
+// the compaction of the index entries with lo_dep <= dep <= hi_dep strictly between entries lo and hi
+static int sr_select(cco_ctx *c, Arena &ar, long long m, const unsigned char *dep, int lo_dep, int hi_dep, long long lo, long long hi,
+                     long long **out, long long *n) {
+  cudaStream_t s = c->stream;
+  long long *flag, *off;
+  CKR(ar.alloc(&flag, m + 1));
+  CKR(ar.alloc(&off, m + 1));
+  CK(cudaMemsetAsync(flag + m, 0, 8, s));
+  if (m > 0) k_sr_flag<<<grid_for(m, 256, c->sm_count), 256, 0, s>>>(m, dep, lo_dep, hi_dep, lo, hi, flag);
+  CKR(exclusive_sum(c, ar, flag, off, m + 1));
+  CKR(mail_fetch(c, n, off + m, 8));
+  CKR(mail_wait(c));
+  CKR(ar.alloc(out, *n + 1));
+  if (m > 0) k_sr_compact<<<grid_for(m, 256, c->sm_count), 256, 0, s>>>(m, flag, off, *out);
+  c->launches += 2;
+  ar.release(flag);
+  ar.release(off);
+  return CCO_OK;
+}
+
+// Read the pending body (device slot h->n_bodies - 1 & 1): its records go after the ones read so far.
+static int sr_read(cco_search_results *h) {
+  cco_ctx *c = h->ctx;
+  cudaStream_t s = c->stream;
+  const int slot = (int)((h->n_bodies - 1) & 1);
+  const long long len = h->p_len, body_no = h->n_bodies - 1, rec_base = (long long)h->status.size(),
+                  hit_base = h->hit_off.back();
+  const unsigned char *body = h->dbody[slot];
+  const char *hbody = h->stage[slot];
+  CK(cudaStreamWaitEvent(s, h->copied[slot], 0));
+  mail_reset(c);   // every fetch below is waited for before the next body
+  Arena ar(s);
+  NvtxRange nvtx("cco:search_results");
+  auto byte_error = [&](unsigned long long e) {
+    return set_error(CCO_E_INVALID_ARG, "response body %lld, byte %lld: %s", body_no, (long long)(e >> 8), sr_message((int)(e & 0xff)));
+  };
+  // the structural index
+  const long long NW = (len + 63) / 64, n_chunks = (NW + kSrChunkWords - 1) / kSrChunkWords;
+  unsigned long long *err;
+  CKR(ar.alloc(&err, 4));
+  CK(cudaMemsetAsync(err, 0xff, 32, s));
+  SrFun *fun, *pre;
+  long long *cnt, *coff;
+  CKR(ar.alloc(&fun, n_chunks + 1));
+  CKR(ar.alloc(&pre, n_chunks + 1));
+  CKR(ar.alloc(&cnt, n_chunks + 1));
+  CKR(ar.alloc(&coff, n_chunks + 1));
+  CK(cudaMemsetAsync(cnt + n_chunks, 0, 8, s));
+  SrFun fin = sr_identity();
+  long long m = 0;
+  if (n_chunks > 0) {
+    const int grid = grid_for(n_chunks * 32, 256, c->sm_count);
+    k_sr_chunk<<<grid, 256, 0, s>>>(NW, (const uint4 *)body, fun);
+    k_sr_scan<<<1, kSrScanThreads, 0, s>>>(n_chunks, fun, pre);
+    k_sr_index<false><<<grid, 256, 0, s>>>(NW, (const uint4 *)body, pre, cnt, nullptr, nullptr, nullptr, err);
+    c->launches += 3;
+    CKR(mail_fetch(c, &fin, pre + n_chunks - 1, sizeof(SrFun)));
+  }
+  CKR(exclusive_sum(c, ar, cnt, coff, n_chunks + 1));
+  unsigned long long e0 = ~0ULL;
+  CKR(mail_fetch(c, &m, coff + n_chunks, 8));
+  CKR(mail_fetch(c, &e0, err, 8));
+  CKR(mail_wait(c));
+  if (e0 != ~0ULL) return byte_error(e0);
+  if (fin.f[0] >> 1) return set_error(CCO_E_INVALID_ARG, "response body %lld, byte %lld: %s", body_no, len, "a string is not closed");
+  if (fin.d[0] != 0) return set_error(CCO_E_INVALID_ARG, "response body %lld, byte %lld: %s", body_no, len, sr_message(kSrUnbalanced));
+  long long *pos;
+  unsigned char *dep;
+  CKR(ar.alloc(&pos, m + 1));
+  CKR(ar.alloc(&dep, m + 1));
+  if (m > 0) {
+    k_sr_index<true><<<grid_for(n_chunks * 32, 256, c->sm_count), 256, 0, s>>>(NW, (const uint4 *)body, pre, nullptr, coff, pos, dep, err);
+    c->launches++;
+  }
+  // the top level and the responses array
+  long long *top, nt = 0, ends[2] = {-1, -1}, *d_ends;
+  CKR(sr_select(c, ar, m, dep, 0, 1, -1, m, &top, &nt));
+  CKR(ar.alloc(&d_ends, 2));
+  k_sr_top<<<1, 32, 0, s>>>(SrIdx{pos, dep, body, top}, nt, len, d_ends, err);
+  c->launches++;
+  CKR(mail_fetch(c, &e0, err, 8));
+  CKR(mail_fetch(c, ends, d_ends, 16));
+  CKR(mail_wait(c));
+  if (e0 != ~0ULL) return byte_error(e0);
+  // one record per element
+  long long *el, n2 = 0;
+  CKR(sr_select(c, ar, m, dep, 2, 2, ends[0], ends[1], &el, &n2));
+  long long *eflag, *erank, n_rec = 0;
+  CKR(ar.alloc(&eflag, n2 + 1));
+  CKR(ar.alloc(&erank, n2 + 1));
+  CK(cudaMemsetAsync(eflag + n2, 0, 8, s));
+  k_sr_elems<<<grid_for(n2 + 1, 256, c->sm_count), 256, 0, s>>>(SrIdx{pos, dep, body, el}, n2, ends[0], ends[1], eflag, err);
+  c->launches++;
+  CKR(exclusive_sum(c, ar, eflag, erank, n2 + 1));
+  CKR(mail_fetch(c, &e0, err, 8));
+  CKR(mail_fetch(c, &n_rec, erank + n2, 8));
+  CKR(mail_wait(c));
+  if (e0 != ~0ULL) return byte_error(e0);
+  CKR(sr_count_check(n_rec, "records"));
+  if (h->p_rec >= 0 && n_rec != h->p_rec)
+    return set_error(CCO_E_INVALID_ARG, "response body %lld: %lld response elements for %lld records", body_no, n_rec, h->p_rec);
+  if (h->p_rec < 0) h->p_ranks.assign((size_t)n_rec, (h->flags & CCO_SR_WITH_RANKS) ? 1 : 0);
+  // the query lines: checked, their withRanks read, numbers beyond the fast path converted here
+  SrLines q = {nullptr, nullptr, nullptr, nullptr, 0};
+  uint8_t *wr;
+  CKR(ar.alloc(&wr, n_rec + 1));
+  if (h->p_has_lines) {
+    const long long lb = (long long)h->p_lines.size(), cap = lb / 2 + 1;
+    unsigned char *d_lines;
+    long long *d_loff;
+    SrExact *lx;
+    CKR(ar.alloc(&d_lines, lb + 1));
+    CKR(ar.alloc(&d_loff, n_rec + 1));
+    CKR(ar.alloc(&lx, cap));
+    if (lb > 0) CK(cudaMemcpyAsync(d_lines, h->p_lines.data(), (size_t)lb, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(d_loff, h->p_loff.data(), 8 * ((size_t)n_rec + 1), cudaMemcpyHostToDevice, s));
+    CK(cudaMemsetAsync(err + 3, 0, 8, s));
+    q.bytes = d_lines;
+    q.off = d_loff;
+    if (n_rec > 0) {
+      k_sr_lines<<<grid_for(n_rec, 128, c->sm_count), 128, 0, s>>>(n_rec, q, wr, lx, err + 3, err + 2);
+      c->launches++;
+    }
+    unsigned long long e2 = ~0ULL, nx = 0;
+    CKR(mail_fetch(c, &e2, err + 2, 8));
+    CKR(mail_fetch(c, &nx, err + 3, 8));
+    CKR(mail_wait(c));
+    if (e2 != ~0ULL)
+      return set_error(CCO_E_INVALID_ARG, "record %lld: %s", rec_base + (long long)(e2 >> 8), sr_message((int)(e2 & 0xff)));
+    if (nx > 0) {
+      std::vector<SrExact> xs((size_t)nx);
+      CK(cudaMemcpyAsync(xs.data(), lx, sizeof(SrExact) * (size_t)nx, cudaMemcpyDeviceToHost, s));
+      CK(cudaStreamSynchronize(s));
+      std::sort(xs.begin(), xs.end(), [](const SrExact &x, const SrExact &y) { return x.b < y.b; });
+      std::vector<long long> xpos((size_t)nx);
+      std::vector<SrNum> xval((size_t)nx);
+      for (size_t i = 0; i < xs.size(); ++i) {
+        xpos[i] = xs[i].b;
+        if (sr_exact_value(h->p_lines.data() + xs[i].b, xs[i].e - xs[i].b, &xval[i])) {
+          const long long r = (long long)(std::upper_bound(h->p_loff.begin(), h->p_loff.end(), (int64_t)xs[i].b) - h->p_loff.begin()) - 1;
+          return set_error(CCO_E_INVALID_ARG, "record %lld: the query line's %.*s is out of the range of a double", rec_base + r,
+                           (int)std::min<long long>(xs[i].e - xs[i].b, 64), h->p_lines.data() + xs[i].b);
+        }
+      }
+      long long *d_xpos;
+      SrNum *d_xval;
+      CKR(ar.alloc(&d_xpos, (long long)nx));
+      CKR(ar.alloc(&d_xval, (long long)nx));
+      CK(cudaMemcpyAsync(d_xpos, xpos.data(), 8 * (size_t)nx, cudaMemcpyHostToDevice, s));
+      CK(cudaMemcpyAsync(d_xval, xval.data(), sizeof(SrNum) * (size_t)nx, cudaMemcpyHostToDevice, s));
+      CK(cudaStreamSynchronize(s));   // the host vectors go out of scope
+      q.xpos = d_xpos;
+      q.xval = d_xval;
+      q.nx = (long long)nx;
+      h->n_exact += (long long)nx;
+    }
+  } else if (n_rec > 0) {
+    CK(cudaMemcpyAsync(wr, h->p_ranks.data(), (size_t)n_rec, cudaMemcpyHostToDevice, s));
+  }
+  SrArgs a;
+  memset(&a, 0, sizeof a);
+  a.x = SrIdx{pos, dep, body, nullptr};
+  a.n_rec = n_rec;
+  a.n_rank = h->n_rank;
+  memcpy(a.name_off, h->name_off, sizeof a.name_off);
+  long long *ropen, *rclose, *nh, *hoff;
+  int32_t *st;
+  long long *tot;
+  unsigned char *names;
+  CKR(ar.alloc(&ropen, n_rec + 1));
+  CKR(ar.alloc(&rclose, n_rec + 1));
+  CKR(ar.alloc(&nh, n_rec + 1));
+  CKR(ar.alloc(&hoff, n_rec + 1));
+  CKR(ar.alloc(&st, n_rec + 1));
+  CKR(ar.alloc(&tot, n_rec + 1));
+  CKR(ar.alloc(&names, h->names.size() + 1));
+  if (!h->names.empty()) CK(cudaMemcpyAsync(names, h->names.data(), h->names.size(), cudaMemcpyHostToDevice, s));
+  a.ropen = ropen;
+  a.rclose = rclose;
+  a.with_ranks = wr;
+  a.names = names;
+  CK(cudaMemsetAsync(nh + n_rec, 0, 8, s));
+  if (n2 > 0) k_sr_records<<<grid_for(n2, 256, c->sm_count), 256, 0, s>>>(n2, el, eflag, erank, ropen, rclose);
+  const int rgrid = grid_for(n_rec * 32, 256, c->sm_count);
+  if (n_rec > 0) k_sr_resp<false><<<rgrid, 256, 0, s>>>(a, st, tot, nh, nullptr, nullptr, nullptr, nullptr, err + 1);
+  c->launches += 2;
+  CKR(exclusive_sum(c, ar, nh, hoff, n_rec + 1));
+  long long n_hits = 0;
+  unsigned long long e1 = ~0ULL;
+  CKR(mail_fetch(c, &e1, err + 1, 8));
+  CKR(mail_fetch(c, &n_hits, hoff + n_rec, 8));
+  CKR(mail_wait(c));
+  if (e1 != ~0ULL)
+    return set_error(CCO_E_INVALID_ARG, "record %lld: %s", rec_base + (long long)(e1 >> 8), sr_message((int)(e1 & 0xff)));
+  CKR(sr_count_check(n_hits, "hits"));
+  long long *hopen, *hclose;
+  int32_t *hrec;
+  JMember *idm;
+  SrNum *sc, *rk;
+  uint8_t *hr;
+  SrExact *xl;
+  const long long n_slots = n_hits * (1 + h->n_rank);
+  CKR(ar.alloc(&hopen, n_hits + 1));
+  CKR(ar.alloc(&hclose, n_hits + 1));
+  CKR(ar.alloc(&hrec, n_hits + 1));
+  CKR(ar.alloc(&idm, n_hits + 1));
+  CKR(ar.alloc(&sc, n_hits + 1));
+  CKR(ar.alloc(&rk, n_hits * h->n_rank + 1));
+  CKR(ar.alloc(&hr, n_hits + 1));
+  CKR(ar.alloc(&xl, n_slots + 1));
+  CK(cudaMemsetAsync(err + 3, 0, 8, s));   // the exact-path count
+  if (n_rec > 0 && n_hits > 0) {
+    k_sr_resp<true><<<rgrid, 256, 0, s>>>(a, nullptr, nullptr, nullptr, hoff, hopen, hclose, hrec, err + 1);
+    k_sr_hit<<<grid_for(n_hits * 32, 256, c->sm_count), 256, 0, s>>>(a, n_hits, hopen, hclose, hrec, idm, sc, rk, hr, xl, err + 3, err + 2);
+    c->launches += 2;
+  }
+  unsigned long long e2 = ~0ULL, nx = 0;
+  CKR(mail_fetch(c, &e2, err + 2, 8));
+  CKR(mail_fetch(c, &nx, err + 3, 8));
+  CKR(mail_wait(c));
+  std::vector<int64_t> hh((size_t)n_rec + 1);
+  CK(cudaMemcpyAsync(hh.data(), hoff, 8 * ((size_t)n_rec + 1), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  auto hit_where = [&](long long hit, char *buf, size_t n) {
+    const long long r = (long long)(std::upper_bound(hh.begin(), hh.end(), (int64_t)hit) - hh.begin()) - 1;
+    snprintf(buf, n, "record %lld hit %lld", rec_base + r, hit - hh[(size_t)r]);
+  };
+  char where[96];
+  if (e2 != ~0ULL) {
+    hit_where((long long)(e2 >> 8), where, sizeof where);
+    return set_error(CCO_E_INVALID_ARG, "%s: %s", where, sr_message((int)(e2 & 0xff)));
+  }
+  // numbers beyond the fast path, on the host
+  if (nx > 0) {
+    std::vector<SrExact> xs((size_t)nx);
+    CK(cudaMemcpyAsync(xs.data(), xl, sizeof(SrExact) * (size_t)nx, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    std::vector<long long> slot_h((size_t)nx);
+    std::vector<SrNum> val((size_t)nx);
+    for (size_t i = 0; i < xs.size(); ++i) {
+      slot_h[i] = xs[i].slot;
+      if (sr_exact_value(hbody + xs[i].b, xs[i].e - xs[i].b, &val[i])) {
+        hit_where(xs[i].slot < n_hits ? xs[i].slot : (xs[i].slot - n_hits) / std::max(h->n_rank, 1), where, sizeof where);
+        return set_error(CCO_E_INVALID_ARG, "%s: %.*s is out of the range of a double", where, (int)std::min<long long>(xs[i].e - xs[i].b, 64),
+                         hbody + xs[i].b);
+      }
+    }
+    long long *d_slot;
+    SrNum *d_val;
+    CKR(ar.alloc(&d_slot, (long long)nx));
+    CKR(ar.alloc(&d_val, (long long)nx));
+    CK(cudaMemcpyAsync(d_slot, slot_h.data(), 8 * (size_t)nx, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(d_val, val.data(), sizeof(SrNum) * (size_t)nx, cudaMemcpyHostToDevice, s));
+    k_sr_exact_put<<<grid_for((long long)nx, 256, c->sm_count), 256, 0, s>>>((long long)nx, d_slot, d_val, n_hits, sc, rk);
+    c->launches++;
+    CK(cudaStreamSynchronize(s));   // the host vectors go out of scope
+    h->n_exact += (long long)nx;
+  }
+  // the ids decoded, the value columns
+  DevStrCol ids;
+  long long id_total = 0;
+  CKR(json_decode(c, ar, n_hits, idm, body, &ids, &id_total));
+  double *sv, *rv;
+  CKR(ar.alloc(&sv, n_hits + 1));
+  CKR(ar.alloc(&rv, n_hits * h->n_rank + 1));
+  if (n_hits > 0) {
+    k_sr_values<<<grid_for(n_hits, 256, c->sm_count), 256, 0, s>>>(n_hits, h->n_rank, sc, rk, hr, sv, rv);
+    c->launches++;
+  }
+  // the text
+  long long text_total = 0, *rec_off = nullptr;
+  unsigned char *d_text = nullptr;
+  if (h->flags & CCO_SR_TEXT) {
+    SrText t;
+    memset(&t, 0, sizeof t);
+    unsigned char *qn;
+    CKR(ar.alloc(&qn, h->qnames.size() + 1));
+    if (!h->qnames.empty()) CK(cudaMemcpyAsync(qn, h->qnames.data(), h->qnames.size(), cudaMemcpyHostToDevice, s));
+    t.id_off = ids.off;
+    t.id_bytes = (const unsigned char *)ids.w;
+    t.score = sc;
+    t.rank = rk;
+    t.has_rank = hr;
+    t.hrec = hrec;
+    t.rec_hoff = hoff;
+    t.n_rank = h->n_rank;
+    t.qnames = qn;
+    memcpy(t.qname_off, h->qname_off, sizeof t.qname_off);
+    long long *tl, *toff;
+    CKR(ar.alloc(&tl, n_hits + 1));
+    CKR(ar.alloc(&toff, n_hits + 1));
+    CKR(ar.alloc(&rec_off, n_rec + 1));
+    CK(cudaMemsetAsync(tl + n_hits, 0, 8, s));
+    const int hgrid = grid_for(n_hits, 256, c->sm_count), rg = grid_for(n_rec + 1, 256, c->sm_count);
+    long long *eoff = nullptr;   // batchpredict lines: the echoes' offsets
+    if (h->flags & CCO_SR_BATCHPREDICT) {
+      long long *el;
+      CKR(ar.alloc(&el, n_rec + 1));
+      CKR(ar.alloc(&eoff, n_rec + 1));
+      CK(cudaMemsetAsync(el + n_rec, 0, 8, s));
+      if (n_rec > 0) k_sr_echo_len<<<grid_for(n_rec, 128, c->sm_count), 128, 0, s>>>(n_rec, q, el);
+      CKR(exclusive_sum(c, ar, el, eoff, n_rec + 1));
+      c->launches++;
+    }
+    if (n_hits > 0) k_sr_hit_text<false><<<hgrid, 256, 0, s>>>(t, eoff, n_hits, tl, nullptr, nullptr, nullptr);
+    CKR(exclusive_sum(c, ar, tl, toff, n_hits + 1));
+    k_sr_rec_text<false><<<rg, 256, 0, s>>>(n_rec, hoff, toff, eoff, q, rec_off, nullptr);
+    CKR(mail_fetch(c, &text_total, rec_off + n_rec, 8));
+    CKR(mail_wait(c));
+    CKR(ar.alloc(&d_text, text_total + 1));
+    if (n_hits > 0) k_sr_hit_text<true><<<hgrid, 256, 0, s>>>(t, eoff, n_hits, nullptr, toff, rec_off, d_text);
+    k_sr_rec_text<true><<<rg, 256, 0, s>>>(n_rec, hoff, toff, eoff, q, rec_off, d_text);
+    c->launches += 4;
+  }
+  // to the host, after the records read so far
+  std::vector<int64_t> idoff((size_t)n_hits + 1), toff_h((size_t)n_rec + 1), tot_h((size_t)n_rec);
+  std::vector<int32_t> st_h((size_t)n_rec);
+  const size_t at_id = h->id_bytes.size(), at_text = h->text.size(), at_sc = h->score.size(), at_rk = h->ranks.size();
+  h->id_bytes.resize(at_id + (size_t)id_total);
+  h->score.resize(at_sc + (size_t)n_hits);
+  h->ranks.resize(at_rk + (size_t)(n_hits * h->n_rank));
+  h->text.resize(at_text + (size_t)text_total);
+  CK(cudaMemcpyAsync(idoff.data(), ids.off, 8 * ((size_t)n_hits + 1), cudaMemcpyDeviceToHost, s));
+  if (id_total > 0) CK(cudaMemcpyAsync(&h->id_bytes[at_id], ids.w, (size_t)id_total, cudaMemcpyDeviceToHost, s));
+  if (n_hits > 0) CK(cudaMemcpyAsync(&h->score[at_sc], sv, 8 * (size_t)n_hits, cudaMemcpyDeviceToHost, s));
+  if (n_hits * h->n_rank > 0) CK(cudaMemcpyAsync(&h->ranks[at_rk], rv, 8 * (size_t)(n_hits * h->n_rank), cudaMemcpyDeviceToHost, s));
+  if (n_rec > 0) {
+    CK(cudaMemcpyAsync(st_h.data(), st, 4 * (size_t)n_rec, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(tot_h.data(), tot, 8 * (size_t)n_rec, cudaMemcpyDeviceToHost, s));
+  }
+  if (rec_off) {
+    CK(cudaMemcpyAsync(toff_h.data(), rec_off, 8 * ((size_t)n_rec + 1), cudaMemcpyDeviceToHost, s));
+    if (text_total > 0) CK(cudaMemcpyAsync(&h->text[at_text], d_text, (size_t)text_total, cudaMemcpyDeviceToHost, s));
+  }
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  sr_append(h->hit_off, hh.data() + 1, n_rec, (int64_t)hit_base);
+  sr_append(h->status, st_h.data(), n_rec);
+  sr_append(h->total, tot_h.data(), n_rec);
+  sr_append(h->id_off, idoff.data() + 1, n_hits, (int64_t)at_id);
+  if (rec_off) sr_append(h->text_off, toff_h.data() + 1, n_rec, (int64_t)at_text);
+  return CCO_OK;
+}
+static int sr_fail_with(cco_search_results *h, int st) {
+  h->failed = true;
+  h->fail_code = st;
+  h->fail_msg = cco_last_error();
+  return st;
+}
+static int sr_state(const cco_search_results *h) {
+  if (h->failed) return set_error(h->fail_code == CCO_OK ? CCO_E_INVALID_ARG : h->fail_code, "%s", h->fail_msg.c_str());
+  if (h->finished) return set_error(CCO_E_INVALID_ARG, "the results are finished");
+  return CCO_OK;
+}
+
+}  // namespace cco
+}  // extern "C++"
+
+int cco_search_results_begin(cco_ctx_t *ctx, const cco_search_results_params_t *params, cco_search_results_t **out) {
+  if (!ctx || !params || !out || (params->n_rankings > 0 && !params->ranking_names)) return set_error(CCO_E_INVALID_ARG, "null argument");
+  if (!ctx->members.empty()) return set_error(CCO_E_UNSUPPORTED, "per-GPU contexts only");
+  if (params->n_rankings < 0 || params->n_rankings > CCO_MAX_RANKINGS)
+    return set_error(CCO_E_INVALID_ARG, "%d rankings: 0 .. %d", params->n_rankings, CCO_MAX_RANKINGS);
+  if (params->flags & ~(uint32_t)(CCO_SR_WITH_RANKS | CCO_SR_TEXT | CCO_SR_BATCHPREDICT))
+    return set_error(CCO_E_INVALID_ARG, "unknown flags %#x", params->flags);
+  *out = nullptr;
+  CK(cudaSetDevice(ctx->device));
+  cco_search_results *h = new cco_search_results();
+  h->ctx = ctx;
+  h->flags = params->flags;
+  for (int k = 0; k < params->n_rankings; ++k) {
+    const char *nm = params->ranking_names[k];
+    if (!nm) {
+      delete h;
+      return set_error(CCO_E_INVALID_ARG, "null ranking name");
+    }
+    bool repeat = false;   // a name listed twice is one member, at its first place
+    for (int j = 0; j < k; ++j) repeat = repeat || !strcmp(nm, params->ranking_names[j]);
+    if (repeat) continue;
+    const int at = h->n_rank++;
+    h->names += nm;
+    h->name_off[at + 1] = (int)h->names.size();
+    std::string q(strlen(nm) * 6 + 3, '\0');   // json4s' quote of the name, then ':'
+    q[0] = '"';
+    const long long n = uq_escape((const unsigned char *)nm, (long long)strlen(nm), (unsigned char *)&q[1]);
+    q.resize((size_t)n + 1);
+    q += "\":";
+    h->qnames += q;
+    h->qname_off[at + 1] = (int)h->qnames.size();
+  }
+  for (int i = 0; i < 2; ++i)
+    if (cudaEventCreateWithFlags(&h->copied[i], cudaEventDisableTiming) != cudaSuccess) {
+      cco_search_results_free(h);
+      return set_error(CCO_E_CUDA, "cudaEventCreate failed");
+    }
+  *out = h;
+  return CCO_OK;
+}
+
+int cco_search_results_append(cco_search_results_t *h, const char *body, int64_t len, int64_t n_records, const int64_t *line_offsets,
+                              const char *line_bytes, const uint8_t *with_ranks) {
+  if (!h || len < 0 || (len > 0 && !body) || (with_ranks && n_records < 0)) return set_error(CCO_E_INVALID_ARG, "null argument or negative length");
+  CKR(sr_state(h));
+  if (n_records >= (1LL << 31)) return sr_fail_with(h, set_error(CCO_E_UNSUPPORTED, "%lld records in one body: at most 2^31 - 1", (long long)n_records));
+  if (line_offsets && (n_records < 0 || with_ranks)) return set_error(CCO_E_INVALID_ARG, "query lines need n_records >= 0 and no with_ranks bitmap");
+  if ((h->flags & CCO_SR_BATCHPREDICT) && !line_offsets) return set_error(CCO_E_INVALID_ARG, "batchpredict lines need the query lines");
+  if (line_offsets) {
+    for (long long r = 0; r < n_records; ++r)
+      if (line_offsets[r + 1] < line_offsets[r]) return set_error(CCO_E_INVALID_ARG, "query line %lld: decreasing offsets", r);
+    if (line_offsets[n_records] > line_offsets[0] && !line_bytes) return set_error(CCO_E_INVALID_ARG, "null line bytes");
+  }
+  cco_ctx *c = h->ctx;
+  CK(cudaSetDevice(c->device));
+  const int slot = (int)(h->n_bodies & 1);
+  const size_t padded = (size_t)((len + 63) / 64 * 64) + 64;
+  size_t free_b = 0, total_b = 0;
+  CK(cudaMemGetInfo(&free_b, &total_b));
+  if (padded > total_b / 4)
+    return sr_fail_with(h, set_error(CCO_E_UNSUPPORTED, "a response body of %lld bytes: at most a quarter of the device's memory", (long long)len));
+  // staging and device buffers of this slot were last used by the body before the previous one, which has been read
+  if (h->stage_cap[slot] < padded) {
+    if (h->stage[slot]) cudaFreeHost(h->stage[slot]);
+    h->stage[slot] = nullptr;
+    h->stage_cap[slot] = 0;
+    if (cudaHostAlloc((void **)&h->stage[slot], padded, cudaHostAllocPortable) != cudaSuccess)
+      return sr_fail_with(h, set_error(CCO_E_OOM, "cudaHostAlloc(%zu) failed", padded));
+    h->stage_cap[slot] = padded;
+  }
+  if (h->dcap[slot] < padded) {
+    if (h->dbody[slot]) cudaFree(h->dbody[slot]);
+    h->dbody[slot] = nullptr;
+    h->dcap[slot] = 0;
+    if (cudaMalloc((void **)&h->dbody[slot], padded) != cudaSuccess)
+      return sr_fail_with(h, set_error(CCO_E_UNSUPPORTED, "a response body of %lld bytes does not fit the device", (long long)len));
+    h->dcap[slot] = padded;
+  }
+  if (len > 0) memcpy(h->stage[slot], body, (size_t)len);
+  memset(h->stage[slot] + len, ' ', padded - (size_t)len);
+  if (cudaMemcpyAsync(h->dbody[slot], h->stage[slot], padded, cudaMemcpyHostToDevice, c->copy_stream) != cudaSuccess ||
+      cudaEventRecord(h->copied[slot], c->copy_stream) != cudaSuccess)
+    return sr_fail_with(h, set_error(CCO_E_CUDA, "the copy of response body %lld failed", (long long)h->n_bodies));
+  // the previous body is read while this one is copied
+  if (h->pending) {
+    const int st = sr_read(h);
+    if (st != CCO_OK) return sr_fail_with(h, st);
+  }
+  ++h->n_bodies;
+  h->pending = true;
+  h->p_len = len;
+  h->p_rec = n_records;
+  h->p_ranks.clear();
+  h->p_has_lines = line_offsets != nullptr;
+  h->p_loff.clear();
+  h->p_lines.clear();
+  if (line_offsets) {
+    h->p_loff.resize((size_t)n_records + 1);
+    for (long long r = 0; r <= n_records; ++r) h->p_loff[(size_t)r] = line_offsets[r] - line_offsets[0];
+    h->p_lines.assign(line_bytes ? line_bytes + line_offsets[0] : "", (size_t)(line_offsets[n_records] - line_offsets[0]));
+  } else if (n_records >= 0) {
+    h->p_ranks.resize((size_t)n_records);
+    for (long long r = 0; r < n_records; ++r)
+      h->p_ranks[(size_t)r] = with_ranks ? (with_ranks[r >> 3] >> (r & 7)) & 1 : ((h->flags & CCO_SR_WITH_RANKS) ? 1 : 0);
+  }
+  return CCO_OK;
+}
+
+int cco_search_results_finish(cco_search_results_t *h, cco_search_results_out_t *out) {
+  if (!h || !out) return set_error(CCO_E_INVALID_ARG, "null argument");
+  CKR(sr_state(h));
+  cco_ctx *c = h->ctx;
+  CK(cudaSetDevice(c->device));
+  if (h->pending) {
+    const int st = sr_read(h);
+    if (st != CCO_OK) return sr_fail_with(h, st);
+    h->pending = false;
+  }
+  h->finished = true;
+  memset(out, 0, sizeof *out);
+  const long long R = (long long)h->status.size(), H = h->hit_off.back();
+  std::vector<void *> got;
+  auto give = [&](void **dst, const void *src, size_t n) {
+    void *p = c->pinned_get(std::max<size_t>(n, 1), /*for_result=*/false);
+    if (!p) return false;
+    if (n) memcpy(p, src, n);
+    got.push_back(p);
+    *dst = p;
+    return true;
+  };
+  bool ok = give((void **)&out->hit_offsets, h->hit_off.data(), 8 * (size_t)(R + 1)) && give((void **)&out->status, h->status.data(), 4 * (size_t)R) &&
+            give((void **)&out->total, h->total.data(), 8 * (size_t)R) && give((void **)&out->id_offsets, h->id_off.data(), 8 * (size_t)(H + 1)) &&
+            give((void **)&out->id_bytes, h->id_bytes.data(), h->id_bytes.size()) && give((void **)&out->score, h->score.data(), 8 * (size_t)H) &&
+            give((void **)&out->ranks, h->ranks.data(), 8 * h->ranks.size());
+  if (ok && (h->flags & CCO_SR_TEXT))
+    ok = give((void **)&out->text_offsets, h->text_off.data(), 8 * (size_t)(R + 1)) && give((void **)&out->text, h->text.data(), h->text.size());
+  if (!ok) {
+    for (void *p : got) c->pinned_put(p);
+    memset(out, 0, sizeof *out);
+    return set_error(CCO_E_OOM, "pinned host allocation failed");
+  }
+  out->n_records = R;
+  out->n_hits = H;
+  out->n_rankings = h->n_rank;
+  out->n_exact = h->n_exact;
+  return CCO_OK;
+}
+
+int cco_search_results_free(cco_search_results_t *h) {
+  if (!h) return CCO_OK;
+  cudaSetDevice(h->ctx->device);
+  cudaStreamSynchronize(h->ctx->copy_stream);
+  for (int i = 0; i < 2; ++i) {
+    if (h->stage[i]) cudaFreeHost(h->stage[i]);
+    if (h->dbody[i]) cudaFree(h->dbody[i]);
+    if (h->copied[i]) cudaEventDestroy(h->copied[i]);
+  }
+  delete h;
   return CCO_OK;
 }
 

@@ -130,7 +130,7 @@ __global__ void k_uq_user_entry(long long R, const int32_t *__restrict__ rec_uid
 // json4s 3.2 quote: '"' and '\' get a backslash, \b \f \n \r \t their short forms, every other code point below U+0020, in
 // U+0080..U+009F (UTF-8 C2 80..C2 9F) and in U+2000..U+20FF (E2 80 80..E2 83 BF) becomes \u%04x in lowercase hex; the rest
 // passes through.  o == nullptr: the length only.
-__device__ __forceinline__ long long uq_escape(const unsigned char *__restrict__ s, long long n, unsigned char *o) {
+__host__ __device__ __forceinline__ long long uq_escape(const unsigned char *__restrict__ s, long long n, unsigned char *o) {
   long long k = 0;
   for (long long i = 0; i < n; ++i) {
     const unsigned char b = s[i];

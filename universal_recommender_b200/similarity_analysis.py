@@ -731,6 +731,65 @@ class CcoContext:
         finally:
             self._L.cco_query_file_free(qf)
 
+    def search_results(self, responses, ap, with_ranks=False, counts=None, text: bool = True, query_lines=None) -> "SearchResults":
+        """URAlgorithm.predict's reading of the search hits (URAlgorithm.scala:484-529) for every element of Elasticsearch
+        _msearch response bodies, on the device (cco_search_results_*; ur_predict restates the rules).  responses: one
+        body (bytes or a path), or a list or generator of bodies; the next body is copied to the device while the previous
+        one is read.  ap: URAlgorithmParams (its ranking field names) or a list of ranking names.  with_ranks: a bool for
+        every record, or one bool per record over all bodies.  counts: the elements each body must hold (None: any number;
+        needed for several bodies when the records carry per-record flags or query lines).  text: render the
+        PredictedResult JSON.  query_lines: the batchpredict query file (bytes or a path) or its lines, line r for record
+        r: each record's withRanks is its line's, and the text is the batchpredict output lines."""
+        from . import ur_predict as P
+        names = list(ap) if isinstance(ap, (list, tuple)) else P.ranking_names(ap)
+        if isinstance(responses, (bytes, bytearray, memoryview, str, os.PathLike)):
+            responses = [responses]
+        if query_lines is not None:
+            query_lines = P.query_file_lines(query_lines)
+            if not isinstance(with_ranks, bool) or with_ranks:
+                raise ValueError("with query lines, each record's withRanks is its line's")
+        per_record = not isinstance(with_ranks, bool)
+        flags_all = list(map(bool, with_ranks)) if per_record else None
+        n_all = len(flags_all) if per_record else len(query_lines) if query_lines is not None else None
+        enc = [n.encode("utf-8") for n in names]
+        flags = (N.SR_WITH_RANKS if with_ranks is True else 0) | (N.SR_TEXT if text else 0)
+        if query_lines is not None and text:
+            flags |= N.SR_BATCHPREDICT
+        prm = N.SearchResultsParamsT(len(enc), (C.c_char_p * max(len(enc), 1))(*enc), flags)
+        h = C.c_void_p()
+        N.check(self._L.cco_search_results_begin(self._h, C.byref(prm), C.byref(h)))
+        try:
+            counts_it = iter(counts) if counts is not None else None
+            done = 0
+            for body in responses:
+                if isinstance(body, (str, os.PathLike)):
+                    with open(body, "rb") as f:
+                        body = f.read()
+                body = bytes(body)
+                n = next(counts_it) if counts_it is not None else -1
+                if n < 0 and n_all is not None:
+                    n = n_all
+                bitmap, loff, lbytes = None, None, None
+                if per_record:
+                    bits = np.zeros(8 * ((n + 7) // 8), dtype=np.uint8)
+                    bits[:n] = flags_all[done:done + n]
+                    bitmap = np.packbits(bits, bitorder="little")
+                if query_lines is not None:
+                    mine = query_lines[done:done + n]
+                    if len(mine) != n:
+                        raise ValueError(f"{len(query_lines)} query lines for more records")
+                    loff = np.zeros(n + 1, dtype=np.int64)
+                    np.cumsum([len(x) for x in mine], out=loff[1:])
+                    lbytes = b"".join(mine)
+                N.check(self._L.cco_search_results_append(h, body, len(body), n, None if loff is None else loff.ctypes.data, lbytes,
+                                                          None if bitmap is None else bitmap.ctypes.data))
+                done += max(n, 0)
+            out = N.SearchResultsOutT()
+            N.check(self._L.cco_search_results_finish(h, C.byref(out)))
+            return SearchResults(self, out, P._unique(names))
+        finally:
+            self._L.cco_search_results_free(h)
+
     def rerank_model(self, body: bytes, properties=None, rankings=None, log=None) -> bytes:
         """cco_rerank_model: calcPop (URAlgorithm.scala:375-399, recsModel "backfill") on an existing index.  body = the
         Elasticsearch bulk body of the current model, as format_model writes it; properties and rankings as in format_model.
@@ -983,6 +1042,47 @@ class CcoContext:
         for p in (orp, oci, ocn):
             self._L.cco_free(p)
         return r, c, n
+
+
+class SearchResults:
+    """What CcoContext.search_results read: per record hit_offsets[n + 1], status and total; per hit ids, scores and
+    ranks [n_hits, n_rankings] (NaN where absent); n_exact numbers were converted on the host's exact path."""
+
+    def __init__(self, ctx: "CcoContext", out, names):
+        L, h = ctx._L, ctx._h
+        R, H, K = out.n_records, out.n_hits, out.n_rankings
+        arr = lambda p, n: np.ctypeslib.as_array(p, shape=(n,)).copy() if n else np.zeros(0, p._type_)
+        self.ranking_names = list(names)
+        self.n_exact = out.n_exact
+        self.hit_offsets = arr(out.hit_offsets, R + 1)
+        self.status = arr(out.status, R)
+        self.total = arr(out.total, R)
+        id_off = arr(out.id_offsets, H + 1)
+        self.scores = arr(out.score, H)
+        self.ranks = arr(out.ranks, H * K).reshape(H, K)
+        blob = C.string_at(out.id_bytes, int(id_off[-1])) if H and id_off[-1] else b""
+        self.ids = [blob[id_off[i]:id_off[i + 1]].decode("utf-8", "surrogatepass") for i in range(H)]
+        self.text_offsets, self._text = None, None
+        if out.text_offsets:
+            self.text_offsets = arr(out.text_offsets, R + 1)
+            self._text = C.string_at(out.text, int(self.text_offsets[-1])) if self.text_offsets[-1] else b""
+        for p in (out.hit_offsets, out.status, out.total, out.id_offsets, out.id_bytes, out.score, out.ranks, out.text_offsets, out.text):
+            if p:
+                L.cco_host_free(h, C.cast(p, C.c_void_p))
+
+    def __len__(self) -> int:
+        return len(self.status)
+
+    def records(self) -> list[str]:
+        """the PredictedResult JSON of every record"""
+        if self._text is None:
+            raise ValueError("the results were read without text")
+        t, o = self._text, self.text_offsets
+        return [t[o[r]:o[r + 1]].decode("utf-8", "surrogatepass") for r in range(len(self))]
+
+    def text(self) -> bytes:
+        """every record's PredictedResult, one per line"""
+        return b"".join(self._text[self.text_offsets[r]:self.text_offsets[r + 1]] + b"\n" for r in range(len(self)))
 
 
 @dataclass

@@ -375,6 +375,30 @@ def queries_from_file(query_file, export, index_body: Optional[bytes], ap: URAlg
         log.free()
 
 
+def predictions_from_responses(responses, ap: URAlgorithmParams, with_ranks=False, counts=None, ctx: CcoContext | None = None):
+    """URAlgorithm.predict's second half (URAlgorithm.scala:484-529, Serving.scala:25-29) for every element of Elasticsearch
+    _msearch response bodies -- the responses to the bodies the query builders write -- on the device, as
+    CcoContext.search_results: one body or a list or generator of them (bytes or paths), with_ranks for every record or
+    one per record, counts the elements of each body.  -> SearchResults: .records() are the PredictedResult JSON texts."""
+    ctx = ctx or default_context()
+    return ctx.search_results(responses, ap, with_ranks=with_ranks, counts=counts)
+
+
+def batchpredict_output(query_file, responses, ap: URAlgorithmParams, out=None, counts=None, ctx: CcoContext | None = None):
+    """`pio batchpredict --output` on the device: line r of the query file (bytes or a path; one Query JSON object per
+    line, as queries_from_file reads it) paired with record r of the _msearch responses to the body queries_from_file
+    built from it (one body or a list or generator of bodies; counts the records of each when there are several).  Each
+    record's withRanks is its line's.  -> the output lines as bytes, each ending in a newline ([RECALL] PredictionIO's
+    {"query":...,"prediction":...}), or None after writing them to the path `out`."""
+    ctx = ctx or default_context()
+    text = ctx.search_results(responses, ap, counts=counts, query_lines=query_file).text()
+    if out is None:
+        return text
+    with open(out, "wb") as f:
+        f.write(text)
+    return None
+
+
 def item_queries(index_body: bytes, ap: URAlgorithmParams, query: Optional[ItemQuery] = None, items=None, now_ms: Optional[int] = None,
                  ctx: CcoContext | None = None, header: str = "{}"):
     """buildQuery (URAlgorithm.scala:563-792) for every item of `items` (None: every document of the index, in body order),
