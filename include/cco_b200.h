@@ -858,6 +858,46 @@ int cco_search_results_finish(cco_search_results_t *h, cco_search_results_out_t 
 int cco_search_results_free(cco_search_results_t *h);
 
 /*
+ * Index pages: the model index read back from Elasticsearch, as calcPop reads it (EsClient.getRDD / esJsonRDD,
+ * EsClient.scala:464-470) and the item queries read a document (EsClient.getSource, EsClient.scala:394-442), turned into the
+ * bulk body cco_format_model writes, which cco_rerank_model, cco_item_queries, cco_mixed_queries and cco_query_file_queries
+ * take.  A page is one complete _search or _search/scroll response body (ES 5 .. 8, compact or ?pretty).  For every hit of
+ * every page, in order, the body holds
+ *   {"index":{"_id":"<_id>"}}\n<_source>\n
+ *  - <_id> is the decoded _id (UTF-8, a lone surrogate in its 3-byte form) escaped as cco_format_model escapes ids;
+ *  - <_source> is the hit's _source with the whitespace (space, \t, \n, \r) outside strings dropped: member order, repeated
+ *    members, number spellings and string escapes are kept, so a compact _source is copied byte for byte.
+ * A body this library wrote, paged as Elasticsearch returns it with compact sources, is read back byte for byte.  The
+ * reader reads _scroll_id, error, status, timed_out, _shards.failed, hits.total and hits.hits of a page (of a repeated
+ * member the first) and _id and _source of a hit (of a repeated _source the first); other members are skipped by depth.
+ * Streaming: begin, an append per page, finish, free.  append returns the page's hit count and its decoded _scroll_id
+ * (valid until the next call on h; NULL when absent), so a scroll loop is while (n_hits) append(the next scroll page).
+ * The page's documents are written by the next append or by finish, so a page's later errors may come from either; after
+ * a failed append or finish every call but free fails with the same message.
+ * Errors, naming the 0-based page, and the hit or the byte offset where they apply: CCO_E_INVALID_ARG for malformed JSON,
+ * a top level that is not an object, a top-level "error" member (with the page's status when it has one), timed_out true,
+ * _shards.failed other than 0, hits.hits that is neither an array nor absent (null), a hit that is not an object, has no
+ * string _id or a repeated _id, a hit without _source (_source disabled in the mapping or the request) or whose _source is
+ * not an object, and a _source string with a bad escape or a raw byte < 0x20 (cco_rerank_model's string rules).  Inside
+ * _source only the strings and the bracket balance are checked; the consumers read its members.  An _id on two pages is
+ * not checked here: every consumer rejects it.  CCO_E_UNSUPPORTED for group contexts, a page larger than a quarter of the
+ * device's memory, 2^31 or more hits in one page and a document line of 2^31 bytes or more.
+ */
+typedef struct cco_index_pages cco_index_pages_t;
+typedef struct {
+  int64_t n_docs;        /* documents written = hits read over all pages */
+  int64_t total;         /* the first page's hits.total when exact (ES 7: relation "eq"), else -1 */
+  char *body;            /* pinned, owned by the context, released with cco_host_free */
+  int64_t body_len;
+} cco_index_pages_out_t;
+int cco_index_pages_begin(cco_ctx_t *ctx, cco_index_pages_t **out);
+int cco_index_pages_append(cco_index_pages_t *h, const char *page, int64_t len, int64_t *n_hits,
+                           const char **scroll_id /* decoded, valid until the next call on h; NULL if absent */,
+                           int64_t *scroll_id_len);
+int cco_index_pages_finish(cco_index_pages_t *h, cco_index_pages_out_t *out);
+int cco_index_pages_free(cco_index_pages_t *h);
+
+/*
  * Debug/parity entry (tests only): full integer co-occurrence matrix A^T B of two canonical
  * binary matrices computed by the same accumulation kernel as cco_train, no LLR, no top-k.
  * Output CSR over the columns of A with ascending column ids, malloc'ed; free with cco_free.

@@ -31,6 +31,7 @@
 #include "cco_events.cuh"
 #include "cco_queries.cuh"
 #include "cco_results.cuh"
+#include "cco_index_pages.cuh"
 
 namespace cco {
 
@@ -6568,7 +6569,7 @@ static int sr_read(cco_search_results *h) {
     const int grid = grid_for(n_chunks * 32, 256, c->sm_count);
     k_sr_chunk<<<grid, 256, 0, s>>>(NW, (const uint4 *)body, fun);
     k_sr_scan<<<1, kSrScanThreads, 0, s>>>(n_chunks, fun, pre);
-    k_sr_index<false><<<grid, 256, 0, s>>>(NW, (const uint4 *)body, pre, cnt, nullptr, nullptr, nullptr, err);
+    k_sr_index<false><<<grid, 256, 0, s>>>(NW, (const uint4 *)body, pre, kSrMaxDepth, cnt, nullptr, nullptr, nullptr, err);
     c->launches += 3;
     CKR(mail_fetch(c, &fin, pre + n_chunks - 1, sizeof(SrFun)));
   }
@@ -6585,7 +6586,7 @@ static int sr_read(cco_search_results *h) {
   CKR(ar.alloc(&pos, m + 1));
   CKR(ar.alloc(&dep, m + 1));
   if (m > 0) {
-    k_sr_index<true><<<grid_for(n_chunks * 32, 256, c->sm_count), 256, 0, s>>>(NW, (const uint4 *)body, pre, nullptr, coff, pos, dep, err);
+    k_sr_index<true><<<grid_for(n_chunks * 32, 256, c->sm_count), 256, 0, s>>>(NW, (const uint4 *)body, pre, kSrMaxDepth, nullptr, coff, pos, dep, err);
     c->launches++;
   }
   // the top level and the responses array
@@ -7029,6 +7030,392 @@ int cco_search_results_free(cco_search_results_t *h) {
     if (h->dbody[i]) cudaFree(h->dbody[i]);
     if (h->copied[i]) cudaEventDestroy(h->copied[i]);
   }
+  delete h;
+  return CCO_OK;
+}
+
+// ---- cco_index_pages: _search / _search/scroll response pages -> the model index's bulk body, kernels in
+// cco_index_pages.cuh ----------------------------------------------------------------------------------------------------
+struct cco_index_pages {
+  cco_ctx *ctx = nullptr;
+  char *stage[2] = {};                 // pinned staging of the last two pages
+  size_t stage_cap[2] = {};
+  unsigned char *dpage[2] = {};        // their device copies
+  size_t dcap[2] = {};
+  cudaEvent_t copied[2] = {};
+  long long n_pages = 0;
+  // the pending page (the last appended): its hits are known, its documents are written by the next append or by finish
+  bool pending = false;
+  Arena *p_ar = nullptr;               // its index and hit brackets
+  long long p_len = 0, p_hits = 0;
+  const long long *p_pos = nullptr, *p_hopen = nullptr, *p_hclose = nullptr;
+  const unsigned char *p_dep = nullptr;
+  std::string scroll_id;               // the last page's, decoded
+  long long total = -1, n_docs = 0;
+  char *out = nullptr;                 // the documents so far (the context's pinned memory, handed to the caller by finish)
+  size_t out_cap = 0, out_len = 0;
+  bool failed = false, finished = false;
+  std::string fail_msg;
+  int fail_code = CCO_OK;
+};
+
+extern "C++" {
+namespace cco {
+
+static const char *ip_message(int code) {
+  switch (code) {
+    case kIpNotObject: return "the top level is not an object";
+    case kIpError: return "Elasticsearch returned an error";
+    case kIpTimedOut: return "the search timed out (timed_out is true)";
+    case kIpShards: return "_shards.failed is not 0";
+    case kIpHitsNotArray: return "hits.hits is neither an array nor absent";
+    case kSrHitNotObject: return "a hits.hits element is not an object";
+    case kSrNoId: return "the hit has no string _id";
+    case kIpRepeatedId: return "a repeated _id";
+    case kIpNoSource: return "the hit has no _source";
+    case kIpSourceNotObject: return "_source is not an object";
+    case kSrString: return "a string holds a bad escape or a raw byte < 0x20";
+  }
+  return sr_message(code);
+}
+// a valid raw JSON string as UTF-8, a surrogate that is not part of a pair in its 3-byte form (k_json_unescape's rules)
+static std::string ip_unescape(const char *p, long long n) {
+  std::string o;
+  auto hex4 = [](const char *q) { return (unsigned)strtoul(std::string(q, 4).c_str(), nullptr, 16); };
+  for (long long i = 0; i < n;) {
+    if (p[i] != '\\') {
+      o += p[i++];
+      continue;
+    }
+    const char x = p[i + 1];
+    if (x != 'u') {
+      o += x == 'b' ? '\b' : x == 'f' ? '\f' : x == 'n' ? '\n' : x == 'r' ? '\r' : x == 't' ? '\t' : x;
+      i += 2;
+      continue;
+    }
+    unsigned cp = hex4(p + i + 2);
+    i += 6;
+    if (cp >= 0xd800 && cp < 0xdc00 && i + 6 <= n && p[i] == '\\' && p[i + 1] == 'u') {
+      const unsigned lo = hex4(p + i + 2);
+      if (lo >= 0xdc00 && lo < 0xe000) {
+        cp = 0x10000 + ((cp - 0xd800) << 10) + (lo - 0xdc00);
+        i += 6;
+      }
+    }
+    if (cp < 0x80) {
+      o += (char)cp;
+    } else if (cp < 0x800) {
+      o += (char)(0xc0 | cp >> 6);
+      o += (char)(0x80 | (cp & 0x3f));
+    } else if (cp < 0x10000) {
+      o += (char)(0xe0 | cp >> 12);
+      o += (char)(0x80 | (cp >> 6 & 0x3f));
+      o += (char)(0x80 | (cp & 0x3f));
+    } else {
+      o += (char)(0xf0 | cp >> 18);
+      o += (char)(0x80 | (cp >> 12 & 0x3f));
+      o += (char)(0x80 | (cp >> 6 & 0x3f));
+      o += (char)(0x80 | (cp & 0x3f));
+    }
+  }
+  return o;
+}
+
+// The new page (slot h->n_pages & 1, copied on the copy stream): its structural index down to the _source brackets and the
+// top walk.  Leaves it pending with its hit count; *sid = its _scroll_id's raw inside (sid[0] < 0: absent).
+static int ip_top(cco_index_pages *h, long long len, long long *n_hits, long long sid[2]) {
+  cco_ctx *c = h->ctx;
+  cudaStream_t s = c->stream;
+  const int slot = (int)(h->n_pages & 1);
+  const long long page_no = h->n_pages;
+  const unsigned char *page = h->dpage[slot];
+  CK(cudaStreamWaitEvent(s, h->copied[slot], 0));
+  mail_reset(c);
+  h->p_ar = new Arena(s);
+  Arena &ar = *h->p_ar;
+  NvtxRange nvtx("cco:index_pages");
+  auto byte_error = [&](long long at, int code) {
+    return set_error(CCO_E_INVALID_ARG, "page %lld, byte %lld: %s", page_no, at, ip_message(code));
+  };
+  const long long NW = (len + 63) / 64, n_chunks = (NW + kSrChunkWords - 1) / kSrChunkWords;
+  unsigned long long *err;
+  CKR(ar.alloc(&err, 1));
+  CK(cudaMemsetAsync(err, 0xff, 8, s));
+  SrFun *fun, *pre;
+  long long *cnt, *coff;
+  CKR(ar.alloc(&fun, n_chunks + 1));
+  CKR(ar.alloc(&pre, n_chunks + 1));
+  CKR(ar.alloc(&cnt, n_chunks + 1));
+  CKR(ar.alloc(&coff, n_chunks + 1));
+  CK(cudaMemsetAsync(cnt + n_chunks, 0, 8, s));
+  SrFun fin = sr_identity();
+  long long m = 0;
+  if (n_chunks > 0) {
+    const int grid = grid_for(n_chunks * 32, 256, c->sm_count);
+    k_sr_chunk<<<grid, 256, 0, s>>>(NW, (const uint4 *)page, fun);
+    k_sr_scan<<<1, kSrScanThreads, 0, s>>>(n_chunks, fun, pre);
+    k_sr_index<false><<<grid, 256, 0, s>>>(NW, (const uint4 *)page, pre, kIpMaxDepth, cnt, nullptr, nullptr, nullptr, err);
+    c->launches += 3;
+    CKR(mail_fetch(c, &fin, pre + n_chunks - 1, sizeof(SrFun)));
+  }
+  CKR(exclusive_sum(c, ar, cnt, coff, n_chunks + 1));
+  unsigned long long e0 = ~0ULL;
+  CKR(mail_fetch(c, &m, coff + n_chunks, 8));
+  CKR(mail_fetch(c, &e0, err, 8));
+  CKR(mail_wait(c));
+  if (e0 != ~0ULL) return byte_error((long long)(e0 >> 8), (int)(e0 & 0xff));
+  if (fin.f[0] >> 1) return set_error(CCO_E_INVALID_ARG, "page %lld, byte %lld: a string is not closed", page_no, len);
+  if (fin.d[0] != 0) return byte_error(len, kSrUnbalanced);
+  long long *pos;
+  unsigned char *dep;
+  CKR(ar.alloc(&pos, m + 1));
+  CKR(ar.alloc(&dep, m + 1));
+  if (m > 0) {
+    k_sr_index<true><<<grid_for(n_chunks * 32, 256, c->sm_count), 256, 0, s>>>(NW, (const uint4 *)page, pre, kIpMaxDepth, nullptr, coff, pos, dep, err);
+    c->launches++;
+  }
+  ar.release(fun);
+  ar.release(pre);
+  ar.release(cnt);
+  ar.release(coff);
+  // the top walk over the entries down to the hits' brackets
+  long long *top, nt = 0, *hopen, *hclose;
+  CKR(sr_select(c, ar, m, dep, 0, kIpTopDepth, -1, m, &top, &nt));
+  CKR(ar.alloc(&hopen, nt / 2 + 1));
+  CKR(ar.alloc(&hclose, nt / 2 + 1));
+  IpTop *d_top, r;
+  CKR(ar.alloc(&d_top, 1));
+  k_ip_top<<<1, 32, 0, s>>>(SrIdx{pos, dep, page, top}, nt, len, d_top, hopen, hclose);
+  c->launches++;
+  CKR(mail_fetch(c, &r, d_top, sizeof r));
+  CKR(mail_wait(c));
+  ar.release(top);
+  if (r.code == kIpNotObject || r.code == kIpTimedOut || r.code == kIpShards || r.code == kIpHitsNotArray)
+    return set_error(CCO_E_INVALID_ARG, "page %lld: %s", page_no, ip_message(r.code));
+  if (r.code == kIpError) {
+    if (r.has_status) return set_error(CCO_E_INVALID_ARG, "page %lld: %s (status %lld)", page_no, ip_message(r.code), r.status);
+    return set_error(CCO_E_INVALID_ARG, "page %lld: %s", page_no, ip_message(r.code));
+  }
+  if (r.code) return byte_error(r.bad, r.code);
+  if (r.n_hits >= (1LL << 31)) return set_error(CCO_E_UNSUPPORTED, "page %lld: %lld hits in one page: at most 2^31 - 1", page_no, r.n_hits);
+  if (page_no == 0) h->total = r.total;
+  h->p_len = len;
+  h->p_hits = r.n_hits;
+  h->p_pos = pos;
+  h->p_dep = dep;
+  h->p_hopen = hopen;
+  h->p_hclose = hclose;
+  h->pending = true;
+  *n_hits = r.n_hits;
+  sid[0] = r.sid_b;
+  sid[1] = r.sid_e;
+  return CCO_OK;
+}
+
+// The pending page's documents: each hit's _id and _source, the documents written on the device and appended to h->out.
+static int ip_docs(cco_index_pages *h) {
+  cco_ctx *c = h->ctx;
+  cudaStream_t s = c->stream;
+  const long long page_no = h->n_pages - 1, n = h->p_hits;
+  const unsigned char *page = h->dpage[page_no & 1];
+  h->pending = false;
+  Arena &ar = *h->p_ar;
+  mail_reset(c);
+  NvtxRange nvtx("cco:index_pages");
+  if (n > 0) {
+    unsigned long long *err;
+    CKR(ar.alloc(&err, 4));
+    CK(cudaMemsetAsync(err, 0xff, 24, s));
+    CK(cudaMemsetAsync(err + 3, 0, 8, s));
+    JMember *idm;
+    long long *sb, *se;
+    CKR(ar.alloc(&idm, n));
+    CKR(ar.alloc(&sb, n));
+    CKR(ar.alloc(&se, n));
+    k_ip_hit<<<grid_for(n * 32, 256, c->sm_count), 256, 0, s>>>(SrIdx{h->p_pos, h->p_dep, page, nullptr}, n, h->p_hopen, h->p_hclose, idm, sb, se,
+                                                                err, err + 1);
+    c->launches++;
+    unsigned long long e_hit = ~0ULL, e_byte = ~0ULL;
+    CKR(mail_fetch(c, &e_hit, err, 8));
+    CKR(mail_fetch(c, &e_byte, err + 1, 8));
+    DevStrCol ids;
+    long long id_total = 0;
+    CKR(json_decode(c, ar, n, idm, page, &ids, &id_total));   // waits for the fetches above
+    if (e_byte != ~0ULL)
+      return set_error(CCO_E_INVALID_ARG, "page %lld, byte %lld: %s", page_no, (long long)(e_byte >> 8), ip_message((int)(e_byte & 0xff)));
+    if (e_hit != ~0ULL) return set_error(CCO_E_INVALID_ARG, "page %lld, hit %lld: %s", page_no, (long long)(e_hit >> 8), ip_message((int)(e_hit & 0xff)));
+    IpDocs a = {page, sb, se, ids.off, (const unsigned char *)ids.w};
+    long long *len, *off;
+    CKR(ar.alloc(&len, n + 1));
+    CKR(ar.alloc(&off, n + 1));
+    CK(cudaMemsetAsync(len + n, 0, 8, s));
+    const int grid = grid_for(n * 32, 256, c->sm_count);
+    k_ip_doc<false><<<grid, 256, 0, s>>>(a, n, len, nullptr, nullptr, err + 2, err + 3);
+    c->launches++;
+    CKR(exclusive_sum(c, ar, len, off, n + 1));
+    long long total = 0;
+    unsigned long long e_str = ~0ULL, max_line = 0;
+    CKR(mail_fetch(c, &total, off + n, 8));
+    CKR(mail_fetch(c, &e_str, err + 2, 8));
+    CKR(mail_fetch(c, &max_line, err + 3, 8));
+    CKR(mail_wait(c));
+    if (e_str != ~0ULL) {
+      const long long at = (long long)(e_str >> 8);
+      std::vector<long long> sb_h((size_t)n);
+      CK(cudaMemcpyAsync(sb_h.data(), sb, 8 * (size_t)n, cudaMemcpyDeviceToHost, s));
+      CK(cudaStreamSynchronize(s));
+      const long long hit = (long long)(std::upper_bound(sb_h.begin(), sb_h.end(), at) - sb_h.begin()) - 1;
+      return set_error(CCO_E_INVALID_ARG, "page %lld, hit %lld, byte %lld: a _source string holds a bad escape or a raw byte < 0x20", page_no,
+                       hit, at);
+    }
+    if (max_line >= (1ULL << 31))
+      return set_error(CCO_E_UNSUPPORTED, "page %lld: a document line of %llu bytes: at most 2^31 - 1", page_no, max_line);
+    if (h->out_len + (size_t)total > h->out_cap) {   // from the context's pinned pool, so a later read reuses it
+      const size_t cap = std::max<size_t>(h->out_cap * 2, std::max<size_t>(h->out_len + (size_t)total, 1u << 20));
+      char *p = (char *)c->pinned_get(cap, /*for_result=*/false);
+      if (!p) return set_error(CCO_E_OOM, "pinned host allocation of %zu bytes failed", cap);
+      if (h->out_len) memcpy(p, h->out, h->out_len);
+      if (h->out) c->pinned_put(h->out);
+      h->out = p;
+      h->out_cap = cap;
+    }
+    unsigned char *d_out;
+    CKR(ar.alloc(&d_out, total + 1));
+    k_ip_doc<true><<<grid, 256, 0, s>>>(a, n, nullptr, off, d_out, nullptr, nullptr);
+    c->launches++;
+    CK(cudaMemcpyAsync(h->out + h->out_len, d_out, (size_t)total, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    CK(cudaGetLastError());
+    h->out_len += (size_t)total;
+    h->n_docs += n;
+  }
+  delete h->p_ar;   // the page's index is freed in stream order
+  h->p_ar = nullptr;
+  return CCO_OK;
+}
+static int ip_fail_with(cco_index_pages *h, int st) {
+  h->failed = true;
+  h->fail_code = st;
+  h->fail_msg = cco_last_error();
+  return st;
+}
+static int ip_state(const cco_index_pages *h) {
+  if (h->failed) return set_error(h->fail_code == CCO_OK ? CCO_E_INVALID_ARG : h->fail_code, "%s", h->fail_msg.c_str());
+  if (h->finished) return set_error(CCO_E_INVALID_ARG, "the index pages are finished");
+  return CCO_OK;
+}
+
+}  // namespace cco
+}  // extern "C++"
+
+int cco_index_pages_begin(cco_ctx_t *ctx, cco_index_pages_t **out) {
+  if (!ctx || !out) return set_error(CCO_E_INVALID_ARG, "null argument");
+  if (!ctx->members.empty()) return set_error(CCO_E_UNSUPPORTED, "per-GPU contexts only");
+  *out = nullptr;
+  CK(cudaSetDevice(ctx->device));
+  cco_index_pages *h = new cco_index_pages();
+  h->ctx = ctx;
+  for (int i = 0; i < 2; ++i)
+    if (cudaEventCreateWithFlags(&h->copied[i], cudaEventDisableTiming) != cudaSuccess) {
+      cco_index_pages_free(h);
+      return set_error(CCO_E_CUDA, "cudaEventCreate failed");
+    }
+  *out = h;
+  return CCO_OK;
+}
+
+int cco_index_pages_append(cco_index_pages_t *h, const char *page, int64_t len, int64_t *n_hits, const char **scroll_id,
+                           int64_t *scroll_id_len) {
+  if (!h || len < 0 || (len > 0 && !page) || !n_hits || !scroll_id || !scroll_id_len)
+    return set_error(CCO_E_INVALID_ARG, "null argument or negative length");
+  CKR(ip_state(h));
+  *n_hits = 0;
+  *scroll_id = nullptr;
+  *scroll_id_len = 0;
+  cco_ctx *c = h->ctx;
+  CK(cudaSetDevice(c->device));
+  const int slot = (int)(h->n_pages & 1);
+  const size_t padded = (size_t)((len + 63) / 64 * 64) + 64;
+  size_t free_b = 0, total_b = 0;
+  CK(cudaMemGetInfo(&free_b, &total_b));
+  if (padded > total_b / 4)
+    return ip_fail_with(h, set_error(CCO_E_UNSUPPORTED, "page %lld of %lld bytes: at most a quarter of the device's memory", h->n_pages, (long long)len));
+  // this slot last held the page before the previous one, whose documents are written
+  if (h->stage_cap[slot] < padded) {
+    if (h->stage[slot]) cudaFreeHost(h->stage[slot]);
+    h->stage[slot] = nullptr;
+    h->stage_cap[slot] = 0;
+    if (cudaHostAlloc((void **)&h->stage[slot], padded, cudaHostAllocPortable) != cudaSuccess)
+      return ip_fail_with(h, set_error(CCO_E_OOM, "cudaHostAlloc(%zu) failed", padded));
+    h->stage_cap[slot] = padded;
+  }
+  if (h->dcap[slot] < padded) {
+    if (h->dpage[slot]) cudaFree(h->dpage[slot]);
+    h->dpage[slot] = nullptr;
+    h->dcap[slot] = 0;
+    if (cudaMalloc((void **)&h->dpage[slot], padded) != cudaSuccess)
+      return ip_fail_with(h, set_error(CCO_E_UNSUPPORTED, "page %lld of %lld bytes does not fit the device", h->n_pages, (long long)len));
+    h->dcap[slot] = padded;
+  }
+  if (len > 0) memcpy(h->stage[slot], page, (size_t)len);
+  memset(h->stage[slot] + len, ' ', padded - (size_t)len);
+  if (cudaMemcpyAsync(h->dpage[slot], h->stage[slot], padded, cudaMemcpyHostToDevice, c->copy_stream) != cudaSuccess ||
+      cudaEventRecord(h->copied[slot], c->copy_stream) != cudaSuccess)
+    return ip_fail_with(h, set_error(CCO_E_CUDA, "the copy of page %lld failed", h->n_pages));
+  // the previous page's documents are written while this one is copied
+  if (h->pending) {
+    const int st = ip_docs(h);
+    if (st != CCO_OK) return ip_fail_with(h, st);
+  }
+  long long n = 0, sid[2] = {-1, -1};
+  const int st = ip_top(h, len, &n, sid);
+  ++h->n_pages;
+  if (st != CCO_OK) return ip_fail_with(h, st);
+  *n_hits = n;
+  if (sid[0] >= 0) {
+    h->scroll_id = ip_unescape(h->stage[slot] + sid[0], sid[1] - sid[0]);
+    *scroll_id = h->scroll_id.data();
+    *scroll_id_len = (int64_t)h->scroll_id.size();
+  }
+  return CCO_OK;
+}
+
+int cco_index_pages_finish(cco_index_pages_t *h, cco_index_pages_out_t *out) {
+  if (!h || !out) return set_error(CCO_E_INVALID_ARG, "null argument");
+  CKR(ip_state(h));
+  cco_ctx *c = h->ctx;
+  CK(cudaSetDevice(c->device));
+  if (h->pending) {
+    const int st = ip_docs(h);
+    if (st != CCO_OK) return ip_fail_with(h, st);
+  }
+  memset(out, 0, sizeof *out);
+  if (!h->out) {   // an empty index: an empty body
+    h->out = (char *)c->pinned_get(1, /*for_result=*/false);
+    if (!h->out) return set_error(CCO_E_OOM, "pinned host allocation failed");
+  }
+  h->finished = true;
+  out->n_docs = h->n_docs;
+  out->total = h->total;
+  out->body = h->out;
+  out->body_len = (int64_t)h->out_len;
+  h->out = nullptr;
+  h->out_cap = h->out_len = 0;
+  return CCO_OK;
+}
+
+int cco_index_pages_free(cco_index_pages_t *h) {
+  if (!h) return CCO_OK;
+  cudaSetDevice(h->ctx->device);
+  cudaStreamSynchronize(h->ctx->copy_stream);
+  cudaStreamSynchronize(h->ctx->stream);
+  delete h->p_ar;
+  for (int i = 0; i < 2; ++i) {
+    if (h->stage[i]) cudaFreeHost(h->stage[i]);
+    if (h->dpage[i]) cudaFree(h->dpage[i]);
+    if (h->copied[i]) cudaEventDestroy(h->copied[i]);
+  }
+  if (h->out) h->ctx->pinned_put(h->out);
   delete h;
   return CCO_OK;
 }

@@ -1,8 +1,9 @@
 // cco_json.cuh -- the Elasticsearch bulk body of an existing model index, parsed on the device (cco_rerank_model).
 //
 // What the reference does with it (calcPop, URAlgorithm.scala:375-399): read the live index, join the fresh rankings and
-// properties into every document by item id (URModel.scala:47-102) and write the index again.  Reading the index stays
-// with the caller; this file splits the bulk body it hands in into documents and top-level members:
+// properties into every document by item id (URModel.scala:47-102) and write the index again.  The caller reads the index
+// (cco_index_pages turns Elasticsearch's pages into the bulk body); this file splits that body into documents and
+// top-level members:
 //   k_nl_count / k_nl_write        '\n' positions: one warp per 2 KB chunk of the body's 8-byte words, a count pass and a
 //                                  write pass around an exclusive scan of the chunk counts
 //   k_json_members                 structural tokenizer, one warp per object span (a line, or the value of an action's

@@ -211,10 +211,11 @@ __global__ void __launch_bounds__(kSrScanThreads) k_sr_scan(long long n, const S
   }
 }
 
-// count pass (cnt[chunk]) and write pass (pos / dep from coff[chunk]); pre = inclusive scan of the chunk functions.
+// count pass (cnt[chunk]) and write pass (pos / dep from coff[chunk]) of the entries at depth <= max_depth (kSrMaxDepth
+// for an _msearch body); pre = inclusive scan of the chunk functions.
 // A closing bracket with nothing open sets err (byte offset, kSrUnbalanced).
 template <bool kWrite>
-__global__ void k_sr_index(long long n_words, const uint4 *__restrict__ body, const SrFun *__restrict__ pre, long long *__restrict__ cnt,
+__global__ void k_sr_index(long long n_words, const uint4 *__restrict__ body, const SrFun *__restrict__ pre, int max_depth, long long *__restrict__ cnt,
                            const long long *__restrict__ coff, long long *__restrict__ pos, unsigned char *__restrict__ dep,
                            unsigned long long *__restrict__ err) {
   const int lane = threadIdx.x & 31;
@@ -250,9 +251,9 @@ __global__ void k_sr_index(long long n_words, const uint4 *__restrict__ body, co
         const int i = __ffsll((long long)s2) - 1;
         s2 &= s2 - 1;
         const uint64_t bit = 1ULL << i;
-        if (o.m.op & bit & ~ins) k += dd++ <= kSrMaxDepth;
-        else if (o.m.cl & bit & ~ins) k += --dd <= kSrMaxDepth && dd >= 0;
-        else k += dd <= kSrMaxDepth;
+        if (o.m.op & bit & ~ins) k += dd++ <= max_depth;
+        else if (o.m.cl & bit & ~ins) k += --dd <= max_depth && dd >= 0;
+        else k += dd <= max_depth;
       }
       long long x = k;
 #pragma unroll
@@ -279,7 +280,7 @@ __global__ void k_sr_index(long long n_words, const uint4 *__restrict__ body, co
       } else {
         e = d;
       }
-      if (e > kSrMaxDepth) continue;
+      if (e > max_depth) continue;
       if (kWrite) {
         pos[at] = p;
         dep[at] = (unsigned char)e;

@@ -790,6 +790,12 @@ class CcoContext:
         finally:
             self._L.cco_search_results_free(h)
 
+    def index_pages(self) -> "IndexPages":
+        """A reader of the model index read back from Elasticsearch (cco_index_pages_*; ur_model.index_from_pages restates
+        the rules): append each _search / _search/scroll response page in order, then finish() gives the bulk body
+        format_model writes, which rerank_model and the query builders take.  Use it as a context manager, or free()."""
+        return IndexPages(self)
+
     def rerank_model(self, body: bytes, properties=None, rankings=None, log=None) -> bytes:
         """cco_rerank_model: calcPop (URAlgorithm.scala:375-399, recsModel "backfill") on an existing index.  body = the
         Elasticsearch bulk body of the current model, as format_model writes it; properties and rankings as in format_model.
@@ -1042,6 +1048,57 @@ class CcoContext:
         for p in (orp, oci, ocn):
             self._L.cco_free(p)
         return r, c, n
+
+
+class IndexPages:
+    """CcoContext.index_pages(): one model index read page by page.  append(page) -> (n_hits, scroll_id or None), the
+    page's hit count and its decoded _scroll_id, known before the next page is needed, so a scroll loop is
+    `while n: n, sid = r.append(scroll(sid))`; the page's documents are written on the device by the next append or by
+    finish, so a page's later error may come from either, and after an error every call but free() raises it again.
+    finish() -> the bulk body; .n_docs and .total (the first page's exact hits.total, -1) are set by it."""
+
+    def __init__(self, ctx: "CcoContext"):
+        self._ctx = ctx
+        self._h = C.c_void_p()
+        self.n_docs, self.total = 0, -1
+        N.check(ctx._L.cco_index_pages_begin(ctx._h, C.byref(self._h)))
+
+    def append(self, page) -> tuple:
+        """one page (bytes, a buffer or a path) -> (n_hits, scroll_id | None)"""
+        if isinstance(page, (str, os.PathLike)):
+            with open(page, "rb") as f:
+                page = f.read()
+        page = bytes(page)
+        n, sid, sid_len = C.c_int64(), C.c_void_p(), C.c_int64()
+        N.check(self._ctx._L.cco_index_pages_append(self._h, page, len(page), C.byref(n), C.byref(sid), C.byref(sid_len)))
+        scroll_id = C.string_at(sid.value, sid_len.value).decode("utf-8", "surrogatepass") if sid.value else None
+        return n.value, scroll_id
+
+    def finish(self) -> bytes:
+        out = N.IndexPagesOutT()
+        N.check(self._ctx._L.cco_index_pages_finish(self._h, C.byref(out)))
+        self.n_docs, self.total = out.n_docs, out.total
+        try:
+            return C.string_at(out.body, out.body_len)
+        finally:
+            self._ctx._L.cco_host_free(self._ctx._h, C.c_void_p(out.body))
+
+    def free(self) -> None:
+        if self._h:
+            self._ctx._L.cco_index_pages_free(self._h)
+            self._h = C.c_void_p()
+
+    def __enter__(self) -> "IndexPages":
+        return self
+
+    def __exit__(self, *exc) -> None:
+        self.free()
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:   # interpreter shutdown
+            pass
 
 
 class SearchResults:

@@ -7,10 +7,11 @@ device (CcoContext.read_events), the DataSource included.  user_queries_from_eve
 whole user base from the same export (ur_query.py restates buildQuery); item_queries builds its item queries for every
 item of a model index body; item_set_queries builds its item-set ("shopping cart") queries for a batch of sets;
 mixed_queries_from_events builds its queries for rows with any subset of user, item and item set; queries_from_file
-builds them for a batchpredict query file, each line with its own template.  Out of scope: withRanks, Elasticsearch's
-scoring, reading the index and the HTTP call."""
+builds them for a batchpredict query file, each line with its own template; index_from_pages reads the model index back
+from Elasticsearch's _search / scroll pages.  Out of scope: Elasticsearch's scoring and the HTTP calls."""
 from __future__ import annotations
 
+import os
 import time
 from dataclasses import dataclass, field
 from typing import Optional, Sequence
@@ -281,7 +282,7 @@ def calc_pop_on_device(body: bytes, events: Sequence[tuple[str, str, str, int]],
                        ranking_events: Optional[dict] = None) -> bytes:
     """URAlgorithm.calcPop (URAlgorithm.scala:375-399, recsModel "backfill") on the GPU: the rankings of an existing index
     refreshed between trains, without a CCO train.  body = the current index as an Elasticsearch bulk body (what
-    calc_all_on_device or format_model wrote; reading it from Elasticsearch stays with the caller); events and set_events as
+    calc_all_on_device or format_model wrote, or index_from_pages read back from Elasticsearch); events and set_events as
     in calc_all_on_device, now_ms likewise.  The properties and rankings are built as calc_all_on_device builds them and
     joined into the old documents by cco_rerank_model: per document, fresh `$set` properties < old members < rankings <
     "id".  So a fresh `$set` value loses to an old member of the same name, and an old rank member survives when the item
@@ -384,6 +385,24 @@ def predictions_from_responses(responses, ap: URAlgorithmParams, with_ranks=Fals
     return ctx.search_results(responses, ap, with_ranks=with_ranks, counts=counts)
 
 
+def index_from_pages(pages, ctx: CcoContext | None = None) -> bytes:
+    """The model index read back from Elasticsearch, as calcPop (EsClient.getRDD, EsClient.scala:464-470) and the item
+    queries (EsClient.getSource, EsClient.scala:394-442) read it, on the device (CcoContext.index_pages): one _search /
+    _search/scroll response page, or a list or generator of them (bytes or paths), in order.  -> the bulk body
+    format_model writes, which calc_pop_from_events, calc_pop_on_device and the query builders take.  Raises when the
+    first page's hits.total is exact and differs from the documents read: the scroll ended early."""
+    ctx = ctx or default_context()
+    if isinstance(pages, (bytes, bytearray, memoryview, str, os.PathLike)):
+        pages = [pages]
+    with ctx.index_pages() as r:
+        for page in pages:
+            r.append(page)
+        body = r.finish()
+        if r.total >= 0 and r.total != r.n_docs:
+            raise ValueError(f"hits.total is {r.total} but the pages hold {r.n_docs} documents: the scroll ended early")
+    return body
+
+
 def batchpredict_output(query_file, responses, ap: URAlgorithmParams, out=None, counts=None, ctx: CcoContext | None = None):
     """`pio batchpredict --output` on the device: line r of the query file (bytes or a path; one Query JSON object per
     line, as queries_from_file reads it) paired with record r of the _msearch responses to the body queries_from_file
@@ -402,8 +421,8 @@ def batchpredict_output(query_file, responses, ap: URAlgorithmParams, out=None, 
 def item_queries(index_body: bytes, ap: URAlgorithmParams, query: Optional[ItemQuery] = None, items=None, now_ms: Optional[int] = None,
                  ctx: CcoContext | None = None, header: str = "{}"):
     """buildQuery (URAlgorithm.scala:563-792) for every item of `items` (None: every document of the index, in body order),
-    the similar items read from the model index body (what calc_all_from_events, calc_all_on_device or a calcPop wrote;
-    reading it from Elasticsearch stays with the caller) on the device: one `header\nquery\n` record per item, the body of
+    the similar items read from the model index body (what calc_all_from_events, calc_all_on_device or a calcPop wrote,
+    or index_from_pages read back from Elasticsearch) on the device: one `header\nquery\n` record per item, the body of
     an Elasticsearch _msearch.  -> (body, offsets) as CcoContext.item_queries ((body, offsets, items) for items=None).
     now_ms: "now" of the available / expire date filter (default: the wall clock).  The fragments are ur_query.item_plan's."""
     ctx = ctx or default_context()

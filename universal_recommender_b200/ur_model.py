@@ -15,6 +15,7 @@ reference's do; unlike the reference's, they repeat when a fixed offsetDate repe
 from __future__ import annotations
 
 import datetime
+import json
 import re
 from collections import Counter
 from dataclasses import dataclass
@@ -401,3 +402,258 @@ def rerank_documents(old_docs: Sequence[tuple[str, dict]], properties: Sequence[
         doc["id"] = item
         docs.append(doc)
     return docs
+
+
+# ---- the index read back from Elasticsearch -------------------------------------------------------------------------------
+# EsClient.getRDD (esJsonRDD, EsClient.scala:464-470) scrolls the index for calcPop, EsClient.getSource (EsClient.scala:
+# 394-442) reads one document for the item queries.  index_from_pages is the host mirror of cco_index_pages_*: the pages
+# of a _search / _search/scroll turned back into the bulk body above, one `{"index":{"_id":"<id>"}}\n<_source>\n` per hit.
+_WS = b" \t\n\r"
+_STRING = re.compile(rb'"(?:[^"\\]|\\.)*"', re.S)
+_STRUCT = re.compile(rb'"(?:[^"\\]|\\.)*"|\\.|"|[{}\[\]]', re.S)       # a string, an escape pair outside one, a lone quote, a bracket
+_GOOD_STRING = re.compile(rb'"(?:[^"\\\x00-\x1f]|\\["\\/bfnrt]|\\u[0-9a-fA-F]{4})*"')
+_NUMBER = re.compile(rb"-?(?:0|[1-9][0-9]*)(?:\.[0-9]+)?(?:[eE][+-]?[0-9]+)?\Z")
+_INTEGER = re.compile(rb"-?(?:0|[1-9][0-9]*)\Z")
+_COMPACT = re.compile(rb'("(?:[^"\\]|\\.)*")|[ \t\n\r]+', re.S)
+
+
+class _PageError(ValueError):
+    pass
+
+
+def _string_bad(b: bytes, i: int, e: int) -> int:
+    """the first bad byte of the raw string inside b[i:e] (a raw byte < 0x20, a bad escape), -1"""
+    while i < e:
+        c = b[i]
+        if c < 0x20:
+            return i
+        if c != 0x5C:
+            i += 1
+        elif b[i + 1:i + 2] in (b'"', b"\\", b"/", b"b", b"f", b"n", b"r", b"t"):
+            i += 2
+        elif b[i + 1:i + 2] == b"u" and re.fullmatch(rb"[0-9a-fA-F]{4}", b[i + 2:min(i + 6, e)]):
+            i += 6
+        else:
+            return i
+    return -1
+
+
+class _Walk:
+    """one page: the levels the reader reads are parsed strictly, every other value is skipped by its brackets"""
+
+    def __init__(self, b: bytes, page: int):
+        self.b, self.page = b, page
+
+    def fail(self, at: int, what: str):
+        raise _PageError(f"page {self.page}, byte {at}: {what}")
+
+    def ws(self, i: int) -> int:
+        while i < len(self.b) and self.b[i] in _WS:
+            i += 1
+        return i
+
+    def string(self, i: int) -> int:
+        """b[i] is a quote: the end of the string (its raw inside checked)"""
+        m = _STRING.match(self.b, i)
+        if not m:
+            self.fail(len(self.b), "a string is not closed")
+        if _string_bad(self.b, i + 1, m.end() - 1) >= 0:
+            self.fail(i + 1, "a string holds a bad escape or a raw byte < 0x20")
+        return m.end()
+
+    def skip(self, i: int) -> int:
+        """b[i] opens an object or an array: the end of its matching close, which must be of its kind"""
+        depth = 0
+        for m in _STRUCT.finditer(self.b, i):
+            t = m.group()
+            if t in (b"{", b"["):
+                depth += 1
+            elif t in (b"}", b"]"):
+                depth -= 1
+                if depth == 0:
+                    if t != (b"}" if self.b[i] == 0x7B else b"]"):
+                        self.fail(m.start(), "unbalanced or mismatched brackets")
+                    return m.end()
+        self.fail(len(self.b), "unbalanced or mismatched brackets")
+
+    def value(self, i: int):
+        """a member value at b[i] (not whitespace) -> (kind, start, end): 'string' (the quotes included), 'object',
+        'array' or 'scalar' (true, false, null or a number)"""
+        c = self.b[i:i + 1]
+        if c == b'"':
+            return "string", i, self.string(i)
+        if c in (b"{", b"["):
+            return ("object" if c == b"{" else "array"), i, self.skip(i)
+        j = i
+        while j < len(self.b) and self.b[j] not in b',}]{["' and self.b[j] not in _WS:
+            j += 1
+        t = self.b[i:j]
+        if not (t in (b"true", b"false", b"null") or _NUMBER.match(t)):
+            self.fail(i, "malformed JSON")
+        return "scalar", i, j
+
+    def members(self, i: int) -> list:
+        """the object opening at b[i] -> [(decoded name, kind, start, end)]"""
+        out = []
+        j = self.ws(i + 1)
+        if self.b[j:j + 1] == b"}":
+            return out
+        while True:
+            if self.b[j:j + 1] != b'"':
+                self.fail(j, "malformed JSON")
+            ne = self.string(j)
+            name = json.loads(self.b[j:ne].decode("utf-8", "surrogatepass"))
+            j = self.ws(ne)
+            if self.b[j:j + 1] != b":":
+                self.fail(j, "malformed JSON")
+            j = self.ws(j + 1)
+            if j >= len(self.b) or self.b[j] in b",}]":
+                self.fail(j, "malformed JSON")
+            kind, vb, ve = self.value(j)
+            out.append((name, kind, vb, ve))
+            j = self.ws(ve)
+            if self.b[j:j + 1] == b"}":
+                return out
+            if self.b[j:j + 1] != b",":
+                self.fail(j, "unbalanced or mismatched brackets" if self.b[j:j + 1] == b"]" else "malformed JSON")
+            j = self.ws(j + 1)
+
+    def elements(self, i: int) -> list:
+        """the array opening at b[i], every element an object -> [(start, end)]"""
+        out = []
+        j = self.ws(i + 1)
+        if self.b[j:j + 1] == b"]":
+            return out
+        while True:
+            c = self.b[j:j + 1]
+            if c != b"{":
+                self.fail(j, "malformed JSON" if c in (b",", b"]") else "a hits.hits element is not an object")
+            e = self.skip(j)
+            out.append((j, e))
+            j = self.ws(e)
+            if self.b[j:j + 1] == b"]":
+                return out
+            if self.b[j:j + 1] != b",":
+                self.fail(j, "a hits.hits element is not an object" if self.b[j:j + 1] != b"}" else "malformed JSON")
+            j = self.ws(j + 1)
+
+
+def _first(members, name):
+    for m in members:
+        if m[0] == name:
+            return m
+    return None
+
+
+def _structure(b: bytes, page: int) -> None:
+    """the whole page: no closing bracket without an opening one, every string closed, the brackets balanced"""
+    depth = 0
+    for m in _STRUCT.finditer(b):
+        t = m.group()
+        if t == b'"':
+            raise _PageError(f"page {page}, byte {len(b)}: a string is not closed")
+        if t in (b"{", b"["):
+            depth += 1
+        elif t in (b"}", b"]"):
+            depth -= 1
+            if depth < 0:
+                raise _PageError(f"page {page}, byte {m.start()}: unbalanced or mismatched brackets")
+    if depth:
+        raise _PageError(f"page {page}, byte {len(b)}: unbalanced or mismatched brackets")
+
+
+def index_page(b: bytes, page: int = 0):
+    """one _search / _search/scroll response page -> (documents as bytes, n_hits, scroll_id or None, hits.total when
+    exact else -1); ValueError names the page, and the hit or the byte offset"""
+    b = bytes(b)
+    _structure(b, page)
+    w = _Walk(b, page)
+    first = w.ws(0)
+    if b[first:first + 1] != b"{":
+        raise _PageError(f"page {page}: the top level is not an object")
+    end = w.skip(first)
+    if w.ws(end) != len(b):
+        w.fail(end, "malformed JSON")
+    top = w.members(first)
+    scroll_id, total, status, hits_arr = None, -1, None, None
+    timed_out = shards_failed = hits_bad = False
+    seen = set()
+    for name, kind, vb, ve in top:   # the nested levels in member order, the first of a repeated member
+        if name in seen:
+            continue
+        seen.add(name)
+        if name == "_shards" and kind == "object":
+            f = _first(w.members(vb), "failed")
+            shards_failed = f is not None and not (f[1] == "scalar" and _INTEGER.match(b[f[2]:f[3]]) and int(b[f[2]:f[3]]) == 0)
+        elif name == "hits" and kind == "object":
+            inner = w.members(vb)
+            t = _first(inner, "total")
+            if t is not None and t[1] == "scalar":
+                text = b[t[2]:t[3]]
+                total = int(text) if _INTEGER.match(text) and -2 ** 63 < int(text) < 2 ** 63 else -1
+            elif t is not None and t[1] == "object":   # ES 7: {"value": n, "relation": "eq" | "gte"}
+                tm = w.members(t[2])
+                v, r = _first(tm, "value"), _first(tm, "relation")
+                exact = v is not None and v[1] == "scalar" and _INTEGER.match(b[v[2]:v[3]]) is not None \
+                    and -2 ** 63 < int(b[v[2]:v[3]]) < 2 ** 63
+                if r is not None:
+                    exact = exact and r[1] == "string" and json.loads(b[r[2]:r[3]].decode("utf-8", "surrogatepass")) == "eq"
+                total = int(b[v[2]:v[3]]) if exact else -1
+            h = _first(inner, "hits")
+            if h is not None and not (h[1] == "scalar" and b[h[2]:h[3]] == b"null"):
+                hits_arr = h if h[1] == "array" else None
+                hits_bad = h[1] != "array"
+    sid = _first(top, "_scroll_id")
+    if sid is not None and sid[1] == "string":
+        scroll_id = json.loads(b[sid[2]:sid[3]].decode("utf-8", "surrogatepass"))
+    st = _first(top, "status")
+    if st is not None and st[1] == "scalar" and _INTEGER.match(b[st[2]:st[3]]) and -2 ** 31 <= int(b[st[2]:st[3]]) < 2 ** 31:
+        status = int(b[st[2]:st[3]])
+    to = _first(top, "timed_out")
+    timed_out = to is not None and to[1] == "scalar" and b[to[2]:to[3]] == b"true"
+    if _first(top, "error") is not None:
+        raise _PageError(f"page {page}: Elasticsearch returned an error" + (f" (status {status})" if status is not None else ""))
+    if timed_out:
+        raise _PageError(f"page {page}: the search timed out (timed_out is true)")
+    if shards_failed:
+        raise _PageError(f"page {page}: _shards.failed is not 0")
+    if hits_bad:
+        raise _PageError(f"page {page}: hits.hits is neither an array nor absent")
+    hits = [w.members(hb) for hb, _ in w.elements(hits_arr[2])] if hits_arr is not None else []
+    docs = []
+    for k, hit in enumerate(hits):
+        ids = [m for m in hit if m[0] == "_id"]
+        if not ids or any(m[1] != "string" for m in ids):
+            raise _PageError(f"page {page}, hit {k}: the hit has no string _id")
+        if len(ids) > 1:
+            raise _PageError(f"page {page}, hit {k}: a repeated _id")
+        src = _first(hit, "_source")
+        if src is None:
+            raise _PageError(f"page {page}, hit {k}: the hit has no _source")
+        if src[1] != "object":
+            raise _PageError(f"page {page}, hit {k}: _source is not an object")
+        docs.append((json.loads(b[ids[0][2]:ids[0][3]].decode("utf-8", "surrogatepass")), src[2], src[3]))
+    out = bytearray()
+    for k, (item, sb, se) in enumerate(docs):
+        for m in re.finditer(rb'"(?:[^"\\]|\\.)*"|\\', b[sb:se], re.S):   # the source's strings, and backslashes outside them
+            bad = sb + m.start() if m.group() == b"\\" else _string_bad(b, sb + m.start() + 1, sb + m.end() - 1)
+            if bad >= 0:
+                raise _PageError(f"page {page}, hit {k}, byte {bad}: a _source string holds a bad escape or a raw byte < 0x20")
+        out += b'{"index":{"_id":' + json_string(item).encode("utf-8", "surrogatepass") + b'}}\n'
+        out += _COMPACT.sub(lambda m: m.group(1) or b"", b[sb:se]) + b"\n"
+    return bytes(out), len(docs), scroll_id, total
+
+
+def index_from_pages(pages) -> tuple:
+    """the model index read back from the pages of an Elasticsearch _search / scroll (each bytes), in order -> (bulk body,
+    n_docs, total): one `{"index":{"_id":"<_id>"}}\\n<_source>\\n` per hit, the _id decoded and escaped as format_model
+    escapes ids (json_string), _source with the whitespace outside strings dropped; total is the first page's hits.total
+    when exact, else -1"""
+    body, n_docs, total = bytearray(), 0, -1
+    for p, page in enumerate(pages):
+        docs, n, _, t = index_page(page, p)
+        body += docs
+        n_docs += n
+        if p == 0:
+            total = t
+    return bytes(body), n_docs, total
