@@ -11,6 +11,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <charconv>
 #include <cmath>
 #include <functional>
 #include <cub/cub.cuh>
@@ -6475,7 +6476,8 @@ static int sr_count_check(long long n, const char *what) {
   if (n >= (1LL << 31)) return set_error(CCO_E_UNSUPPORTED, "%lld %s in one body: at most 2^31 - 1", n, what);
   return CCO_OK;
 }
-// the exact path: strtod (correctly rounded) and the shortest %.*e digits that give the same double back
+// the exact path: strtod (correctly rounded; an underflow is a zero, not an error) and std::to_chars' digits, the
+// shortest that give the same double back and of those the nearest to it (what Python's repr prints)
 static int sr_exact_value(const char *t, long long n, SrNum *o) {
   std::string s(t, (size_t)n);
   const double v = strtod(s.c_str(), nullptr);
@@ -6483,11 +6485,8 @@ static int sr_exact_value(const char *t, long long n, SrNum *o) {
   SrNum r = {v, 0ULL, 0, 0, s[0] == '-', 0};
   if (v != 0) {
     char buf[40];
-    const double a = std::fabs(v);
-    for (int p = 1; p <= 17; ++p) {
-      snprintf(buf, sizeof buf, "%.*e", p - 1, a);
-      if (strtod(buf, nullptr) == a) break;
-    }
+    const std::to_chars_result tc = std::to_chars(buf, buf + sizeof buf - 1, std::fabs(v), std::chars_format::scientific);
+    *tc.ptr = 0;
     const char *e = strchr(buf, 'e');
     unsigned long long dig = 0;
     int nd = 0;

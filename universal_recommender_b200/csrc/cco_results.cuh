@@ -402,9 +402,12 @@ struct SrNum {
   int e10, nd;
   int neg, exact;   // exact: the host computes v, dig, e10 and nd from the text
 };
-// false when [p, e) is not a JSON number
+// false when [p, e) is not a JSON number.  The exponent and the offset the mantissa's digits carry are summed in 64 bits;
+// the exponent literal saturates at 2^59, beyond any digit offset, so a sum inside the fast path's window is exact, and a
+// number outside it goes to the host, which reads the text itself.
 __device__ __forceinline__ bool sr_number(const unsigned char *__restrict__ b, long long p, long long e, SrNum *o) {
   SrNum r = {0.0, 0ULL, 0, 0, 0, 0};
+  long long e10 = 0;
   if (p < e && b[p] == '-') {
     r.neg = 1;
     ++p;
@@ -413,15 +416,15 @@ __device__ __forceinline__ bool sr_number(const unsigned char *__restrict__ b, l
   bool lost = false;
   auto digit = [&](unsigned d, bool frac) {
     if (r.dig == 0 && d == 0) {
-      if (frac) --r.e10;
+      if (frac) --e10;
       return;
     }
     if (r.nd < 19) {
       r.dig = r.dig * 10 + d;
       ++r.nd;
-      if (frac) --r.e10;
+      if (frac) --e10;
     } else {
-      if (!frac) ++r.e10;
+      if (!frac) ++e10;
       if (d) lost = true;
     }
   };
@@ -445,25 +448,25 @@ __device__ __forceinline__ bool sr_number(const unsigned char *__restrict__ b, l
     if (p >= e || b[p] - '0' >= 10u) return false;
     long long x = 0;
     while (p < e && b[p] - '0' < 10u) {
-      x = x * 10 + (b[p++] - '0');
-      if (x > 100000) x = 100000;
+      const unsigned d = b[p++] - '0';
+      if (x < (1LL << 59)) x = x * 10 + d;   // x * 10 + 9 still fits
     }
-    r.e10 += (int)(sg * x);
+    e10 += sg * x;
   }
   if (p != e) return false;
   if (r.dig == 0) {
     if (is_int) r.neg = 0;   // a JSON integer is a JInt: -0 is 0
-    r.e10 = 0;
     r.v = r.neg ? -0.0 : 0.0;
     *o = r;
     return true;
   }
   while (r.dig % 10 == 0) {
     r.dig /= 10;
-    ++r.e10;
+    ++e10;
     --r.nd;
   }
-  if (!lost && r.nd <= 15 && r.e10 >= -22 && r.e10 <= 22) {   // Clinger: both operands exact, one rounding
+  if (!lost && r.nd <= 15 && e10 >= -22 && e10 <= 22) {   // Clinger: both operands exact, one rounding
+    r.e10 = (int)e10;
     const double p10[23] = {1e0, 1e1, 1e2, 1e3, 1e4, 1e5, 1e6, 1e7, 1e8, 1e9, 1e10, 1e11, 1e12, 1e13, 1e14, 1e15,
                             1e16, 1e17, 1e18, 1e19, 1e20, 1e21, 1e22};
     const double m = (double)r.dig;

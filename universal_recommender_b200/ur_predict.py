@@ -60,9 +60,11 @@ def loads(text) -> object:
 
 
 def number_value(text: str) -> float:
-    """the double nearest to a JSON number's text (Python's float() rounds exactly); an integer literal is a JInt, so -0
-    is 0.0; out of range is an error"""
-    v = float(int(text)) if _is_integer(text) else float(text)
+    """the double nearest to a JSON number's text (Python's float() rounds exactly, integer literals of any length
+    included); an integer literal is a JInt, so -0 is 0.0; out of range is a ValueError"""
+    v = float(text)
+    if v == 0 and _is_integer(text):
+        v = 0.0
     if v in (float("inf"), float("-inf")):
         raise ValueError(f"{text} is out of the range of a double")
     return v
@@ -237,7 +239,7 @@ def batchpredict_line(line, prediction_text: str) -> str:
 def render(v) -> str:
     """json4s compact rendering of a parsed value"""
     if isinstance(v, Num):
-        return str(int(v)) if _is_integer(v) else number_text(v)
+        return ("0" if v == "-0" else str(v)) if _is_integer(v) else number_text(v)   # BigInt prints a JSON integer as it is
     if isinstance(v, str):
         return json_string(v)
     if isinstance(v, _Obj):
