@@ -764,6 +764,7 @@ struct BinCfg {
   int caux, keep_max, final_max;
   bool dense;
   bool bitmap;    // bitmap rows (use_bitmap): slots = repeat-table words, then bm_words of bitmap and top_k singles
+  bool sorted;    // sorted rows (use_sorted): the table holds a row's keys and the radix sort's second buffer
   int bm_words;
   size_t region;  // shared-memory bytes per group
   size_t smem;    // per CTA
@@ -783,6 +784,8 @@ static int launch_rows_t(cco_ctx *c, const RowArgs &a, BinCfg &cfg, cudaStream_t
   void (*kern)(const RowArgs) = cfg.dense ? k_rows<GROUP, true> : k_rows<GROUP, false>;
   if constexpr (GROUP == 512 || GROUP == 256)
     if (cfg.bitmap) kern = k_rows<GROUP, false, true>;
+  if constexpr (GROUP == 32)
+    if (cfg.sorted) kern = k_rows<32, false, false, true>;
   CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg.smem));
   CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, CTA, cfg.smem));
   // 4 waves of CTAs over the work-sorted row list: a CTA that draws cheap rows retires early and the hardware
@@ -821,6 +824,7 @@ static BinCfg make_cfg(cco_ctx *c, int group, int want_slots, int top_k, int n_c
   f.cap = f.slots / 2;  // load factor <= 1/2: higher load factors lengthen the probe chains
   f.dense = n_cols_b <= f.slots;
   f.bitmap = false;
+  f.sorted = false;
   f.bm_words = 0;
   f.region = (fixed + (size_t)f.slots * 4 + 15) & ~(size_t)15;
   f.smem = f.region * groups;
@@ -843,6 +847,26 @@ static bool use_bitmap(BinCfg &f, uint32_t max_w, int top_k, int n_cols_b) {
   f.bitmap = true;
   f.slots = (int)rep;
   f.bm_words = (int)bm;
+  return true;
+}
+
+// Sorted rows (DESIGN.md 3.1): a hashed warp-owned bin whose rows all take the key path with an exact cut sorts each row's
+// keys instead of hashing them.  The radix sort ping-pongs between two max_w-word halves that end where the table ends and
+// reach back over the select histogram and the evaluation queues (256 + 64 words, dead while a row counts); the second half,
+// which holds the cells the score stage reads, stays inside the table.  The table so shrinks to max(2 max_w - 320, max_w)
+// words -- bin 5 (max_w 1024) from 2048 to 1728, one more CTA per SM.  One packed u16 histogram per key digit lives in the
+// candidate buffer (also dead while a row counts).  Digits as sort_digits (cco_kernels.cuh): ceil(key bits / 9) passes.
+static bool use_sorted(BinCfg &f, uint32_t max_w, int count_bits) {
+  constexpr int kAliased = 256 + 64;   // k_rows: hist + wqueue (NW = 1) lie right below the table
+  if (f.dense || f.group != 32 || max_w > 1024u) return false;
+  const int slots = std::max(2 * (int)max_w - kAliased, (int)max_w);
+  const int kb = 32 - count_bits, passes = (kb + 8) / 9;
+  const int dbits = std::max((kb + passes - 1) / passes, 6);
+  if (slots > f.slots || (long long)passes << (dbits - 1) > 4LL * f.cbuf) return false;
+  f.sorted = true;
+  f.region -= (size_t)(f.slots - slots) * 4;
+  f.smem = f.region * 2;
+  f.slots = slots;
   return true;
 }
 
@@ -996,12 +1020,15 @@ static int enqueue_indicator(cco_ctx *c, Arena &ar, const uint32_t *at_ptr, cons
     h_thr[b] = lim;
     if (b > 0) h_thr[b] = std::min(h_thr[b], h_thr[b - 1]);
   }
-  // bitmap rows: the k11 = 1 cells are cut by key, so every row must be keyed (2 rowA colB < N for the largest of both)
+  // bitmap and sorted rows: the k11 = 1 cells are cut by key, so every row must be keyed (2 rowA colB < N for the largest of both)
   // and the cut exact
   const bool bitmap_ok = !emit_all && cut_exact(n_users, max_marg_a, max_marg_b) &&
                          2ull * (unsigned long long)std::max(max_marg_a, 0) * (unsigned long long)std::max(max_marg_b, 0) <
                              (unsigned long long)n_users;
-  for (int b = 1; b < kBins && bitmap_ok; ++b) use_bitmap(cfgs[b], h_thr[b - 1], k_eff, n_cols_b);
+  for (int b = 1; b < kBins && bitmap_ok; ++b) {
+    use_bitmap(cfgs[b], h_thr[b - 1], k_eff, n_cols_b);
+    use_sorted(cfgs[b], h_thr[b - 1], count_bits);
+  }
   int32_t *d_bounds;
   CKR(ar.alloc(&d_bounds, kBins + 3));
   BinThresholds bt;

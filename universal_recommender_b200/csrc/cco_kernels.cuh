@@ -706,10 +706,151 @@ __device__ __forceinline__ void count_window(const RowArgs &a, uint32_t *table, 
   }
 }
 
+// ---- sorted rows (warp-owned rows keyed with an exact cut; DESIGN.md 3.1 "sorted rows") ------------------------------------
+// The row's keys are sorted by an LSD radix sort over `passes` digits of `dbits` bits.  Each digit has a histogram of
+// 2^dbits u16 bins packed two to a word (a warp-owned row has at most 1024 products); all of them are counted while the
+// keys are gathered.
+struct SortDigits {
+  int passes, dbits, hwords;   // hwords = 2^(dbits - 1): words of one digit's histogram, 32 .. 256
+};
+__device__ __forceinline__ SortDigits sort_digits(int cbits) {
+  const int kb = 32 - cbits;
+  SortDigits d;
+  d.passes = (kb + 8) / 9;
+  d.dbits = max((kb + d.passes - 1) / d.passes, 6);
+  d.hwords = 1 << (d.dbits - 1);
+  return d;
+}
+__device__ __forceinline__ void digit_count(uint32_t *h, const SortDigits &sd, uint32_t b) {
+  for (int p = 0; p < sd.passes; ++p) {
+    const uint32_t dg = (b >> (p * sd.dbits)) & ((1u << sd.dbits) - 1u);
+    atomicAdd(&h[p * sd.hwords + (dg >> 1)], 1u << (16u * (dg & 1u)));
+  }
+}
+
+// Gather the products [0, p_hi) of a window of up to 32 users (registers as in count_window) to keys[p] in product order,
+// counting every digit of every key into the histograms h.  Nothing waits on a gathered key here (no probe), so each lane
+// keeps kGatherDepth gathers in flight.
+constexpr int kGatherDepth = 4;
+__device__ __forceinline__ void gather_window(const RowArgs &a, uint32_t *keys, uint32_t *h, const SortDigits &sd, uint32_t off,
+                                              uint32_t s, uint32_t p_hi, int lane) {
+  for (uint32_t p0 = 0; p0 < p_hi; p0 += 32 * kGatherDepth) {
+    uint32_t bb[kGatherDepth];
+    bool act[kGatherDepth];
+#pragma unroll
+    for (int hh = 0; hh < kGatherDepth; ++hh) {
+      const uint32_t p = p0 + hh * 32 + lane;
+      int j = 0;
+#pragma unroll
+      for (int st = 16; st > 0; st >>= 1) {
+        const int c = j + st;
+        const uint32_t v = __shfl_sync(0xffffffffu, off, c);
+        if (v <= p) j = c;
+      }
+      const uint32_t sj = __shfl_sync(0xffffffffu, s, j), oj = __shfl_sync(0xffffffffu, off, j);
+      act[hh] = p < p_hi;
+      bb[hh] = act[hh] ? (uint32_t)a.b_col[sj + (p - oj)] : 0u;
+    }
+#pragma unroll
+    for (int hh = 0; hh < kGatherDepth; ++hh)
+      if (act[hh]) {
+        keys[p0 + hh * 32 + lane] = bb[hh];
+        digit_count(h, sd, bb[hh]);
+      }
+  }
+}
+
+// One warp: the counts of a packed u16 histogram of hwords words -> exclusive prefix sums, in place
+__device__ __forceinline__ void digit_scan(uint32_t *h, int hwords, int lane) {
+  const int per = hwords >> 5;
+  uint32_t sum = 0;
+  for (int j = 0; j < per; ++j) { const uint32_t v = h[lane * per + j]; sum += (v & 0xffffu) + (v >> 16); }
+  uint32_t incl = sum;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const uint32_t v = __shfl_up_sync(0xffffffffu, incl, d);
+    if (lane >= d) incl += v;
+  }
+  uint32_t run = incl - sum;
+  for (int j = 0; j < per; ++j) {
+    const uint32_t v = h[lane * per + j], lo = v & 0xffffu;
+    h[lane * per + j] = run | ((run + lo) << 16);
+    run += lo + (v >> 16);
+  }
+  __syncwarp();
+}
+
+// Sorted rows: the row's w <= 1024 keys are in keys[0, w), keys[w, 2 w) is free, and h holds every digit's counts.  A
+// stable LSD radix sort orders them (equal digits of one 32-key batch keep their lane order: match.any ranks them), and
+// one pass over the sorted keys turns each run of equal keys into the packed word (key << cbits) | k11 at its last key,
+// compacted to keys[w, w + n) -- the cells the filter reads.  The diagonal is dropped (the filter would skip it), and so
+// is every k11 = 1 cell after the top_k-th other one: the singles are in key order, so those are exactly the cells
+// beyond the level-1 key cut.  Returns n; *n_runs = the distinct cells.
+__device__ uint32_t sort_runs(uint32_t *keys, uint32_t w, uint32_t *h, const SortDigits &sd, int cbits, int diag, int top_k,
+                              uint32_t *n_runs, int lane) {
+  const unsigned lt = (1u << lane) - 1u, le = (2u << lane) - 1u;
+  uint32_t *src = keys, *dst = keys + w;
+  for (int p = 0; p < sd.passes; ++p) {
+    uint32_t *hp = h + p * sd.hwords;
+    digit_scan(hp, sd.hwords, lane);
+    const int sh = p * sd.dbits;
+    for (uint32_t i0 = 0; i0 < w; i0 += 32) {
+      const uint32_t i = i0 + lane;
+      const bool valid = i < w;
+      const uint32_t k = valid ? src[i] : 0u;
+      const uint32_t dg = valid ? (k >> sh) & ((1u << sd.dbits) - 1u) : 0xffffffffu;
+      const unsigned peers = __match_any_sync(0xffffffffu, dg);
+      const uint32_t hsh = 16u * (dg & 1u);
+      const uint32_t base = valid ? (hp[dg >> 1] >> hsh) & 0xffffu : 0u;
+      __syncwarp();   // every lane has read its digit's offset before the batch's first lane of it moves it on
+      if (valid) {
+        const uint32_t r = __popc(peers & lt);
+        dst[base + r] = k;
+        if (r == 0) atomicAdd(&hp[dg >> 1], (uint32_t)__popc(peers) << hsh);
+      }
+      __syncwarp();
+    }
+    uint32_t *t = src; src = dst; dst = t;
+  }
+  // runs -> packed words at keys[w, w + n).  After an even number of passes that half is free; after an odd number it is
+  // src itself, and the compaction is in place: the words of a batch go below the batch's last key (one word per run that
+  // ends in or before it), and every later read is at or beyond the next batch.
+  uint32_t *out = keys + w;
+  uint32_t n = 0, n_single = 0, nr = 0, prev_key = kEmpty, head_pos = 0;
+  for (uint32_t i0 = 0; i0 < w; i0 += 32) {
+    const uint32_t i = i0 + lane;
+    const bool valid = i < w;
+    const uint32_t k = valid ? src[i] : kEmpty;   // keys are < 2^key_bits - 1: never kEmpty
+    const uint32_t nk = i + 1 < w ? src[i + 1] : kEmpty;
+    uint32_t pk = __shfl_up_sync(0xffffffffu, k, 1);
+    if (lane == 0) pk = prev_key;
+    const unsigned hm = __ballot_sync(0xffffffffu, valid && k != pk);
+    nr += __popc(hm);
+    const unsigned mine = hm & le;   // heads at or below this lane: the last one starts its run
+    const uint32_t hpos = mine ? i0 + 31u - (uint32_t)__clz(mine) : head_pos;
+    const uint32_t len = i + 1u - hpos;
+    const bool off_diag = valid && k != nk && (int)k != diag;   // run ends here
+    const bool single = off_diag && len == 1u;
+    const unsigned sm = __ballot_sync(0xffffffffu, single);
+    const bool keep = off_diag && (len > 1u || n_single + __popc(sm & lt) < (uint32_t)top_k);
+    n_single += __popc(sm);
+    const unsigned km = __ballot_sync(0xffffffffu, keep);
+    prev_key = __shfl_sync(0xffffffffu, k, 31);
+    head_pos = __shfl_sync(0xffffffffu, hpos, 31);
+    __syncwarp();
+    if (keep) out[n + __popc(km & lt)] = (k << cbits) | len;
+    n += __popc(km);
+    __syncwarp();
+  }
+  *n_runs = nr;
+  return n;
+}
+
 // Minimum resident CTAs per SM that the register allocation must allow.  At top_k 50 make_cfg (cco_api.cu) fits 2 / 4 / 9
 // hashed 512 / 256 / 128-thread CTAs per SM in shared memory; 8 instead of 9 keeps 64 registers (9 forces 56 and measured
 // no faster).  Warp-owned rows run as 64-thread CTAs whose three bins fit 8 / 13 / 16 per SM: 12 is what their spill-free
-// 80 registers allow, and a 16-CTA bound (64 registers) measured no faster.  DESIGN.md 3.2 lists registers and spills.
+// 80 registers allow, and a 16-CTA bound (64 registers) measured no faster.  Sorted rows need 72 registers (14 CTAs per
+// SM) and their smaller tables fit 9 / 15 / 19.  DESIGN.md 3.2 lists registers and spills.
 template <int GROUP>
 struct RowsMinBlocks {
   static constexpr int value = GROUP == 512 ? 2 : GROUP == 256 ? 4 : GROUP == 128 ? 8 : GROUP == 32 ? 12 : 1;
@@ -718,9 +859,14 @@ struct RowsMinBlocks {
 // BITMAP (CTA-owned hashed bins whose rows are all on the key path with an exact cut; DESIGN.md 3.1 "bitmap rows"): the
 // count sets one bit per cell in a bitmap over the keys and hashes only the repeated products; the level-1 key cut is the
 // top_k-th set bit in key order, and only the k11 = 1 cells up to it are ever listed.
-template <int GROUP, bool DENSE, bool BITMAP = false>
+//
+// SORTED (warp-owned hashed bins whose rows are all on the key path with an exact cut; DESIGN.md 3.1 "sorted rows"): the
+// row's keys are gathered and sorted instead of hashed (sort_runs), which yields the counts, the compacted list and the
+// level-1 key cut at once.
+template <int GROUP, bool DENSE, bool BITMAP = false, bool SORTED = false>
 __global__ void __launch_bounds__(GROUP == 32 ? 64 : GROUP, RowsMinBlocks<GROUP>::value) k_rows(const RowArgs a) {
   static_assert(!BITMAP || (GROUP > 32 && !DENSE), "bitmap rows are CTA-owned rows of a hashed bin");
+  static_assert(!SORTED || (GROUP == 32 && !DENSE && !BITMAP), "sorted rows are warp-owned rows of a hashed bin");
   const int GROUPS = GROUP == 32 ? (int)(blockDim.x >> 5) : 1;  // warp-owned rows: several independent warps per CTA
   constexpr int NW = GROUP / 32;
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -749,6 +895,8 @@ __global__ void __launch_bounds__(GROUP == 32 ? 64 : GROUP, RowsMinBlocks<GROUP>
   const double xN = xlogx(N);
   unsigned long long distinct_local = 0, evaluated_local = 0;
   if (gtid < 32) x11tab[gtid] = xlogx((long long)gtid);
+  uint32_t *dhist = reinterpret_cast<uint32_t *>(tk);   // SORTED: the digit histograms (the candidates are dead until the score stage)
+  const SortDigits sd = sort_digits(cbits);
 
   for (int ri = row_begin + blockIdx.x * GROUPS + gid; ri < row_end; ri += gridDim.x * GROUPS) {
     const int item = a.rows_sorted[ri];
@@ -761,7 +909,7 @@ __global__ void __launch_bounds__(GROUP == 32 ? 64 : GROUP, RowsMinBlocks<GROUP>
     const bool keyed = 2ull * (unsigned long long)ra * (unsigned long long)a.max_marg_b < (unsigned long long)N;
     // table sized to the row: load factor <= 1/2 of the distinct-cell bound D = min(w, n_cols_b)
     uint32_t n_pass = 1, tsize = (uint32_t)a.n_cols_b;
-    if (!DENSE) {
+    if (!DENSE && !SORTED) {
       const uint32_t w = a.row_work[item];
       // BITMAP: the table holds only cells with k11 >= 2, each of at least two of the w products (one pass: the host
       // sizes a.slots for the bin's largest w)
@@ -785,11 +933,19 @@ __global__ void __launch_bounds__(GROUP == 32 ? 64 : GROUP, RowsMinBlocks<GROUP>
 
     for (uint32_t pass = 0; pass < n_pass; ++pass) {
       // ---- clear --------------------------------------------------------------------------------------
-      for (uint32_t i = gtid; i < tsize; i += GROUP) table[i] = DENSE ? 0u : kEmpty;
+      if (SORTED)
+        for (int i = lane; i < sd.passes * sd.hwords; i += 32) dhist[i] = 0u;
+      else
+        for (uint32_t i = gtid; i < tsize; i += GROUP) table[i] = DENSE ? 0u : kEmpty;
       if (BITMAP)
         for (int i = gtid; i < a.bm_words; i += GROUP) seen[i] = 0u;
       group_sync<GROUP>();
       // ---- count -------------------------------------------------------------------------------------------
+      // SORTED: the row's w keys and the sort's second half end where the table ends, reaching back over the dead select
+      // histogram and evaluation queues (the host sizes a.slots >= max(2 max_w - 320, max_w)); the cells the filter reads
+      // end up in the second half, inside the table
+      uint32_t *keys = table + a.slots - 2u * (SORTED ? a.row_work[item] : 0u);
+      uint32_t n_keys = 0;   // SORTED: the keys gathered so far
       if (NW == 1) {
         // warp-owned row: 32-user chunks, the products of a chunk flattened over the lanes by a warp prefix sum
         for (uint32_t c0 = u_begin; c0 < u_end; c0 += 32) {
@@ -808,7 +964,12 @@ __global__ void __launch_bounds__(GROUP == 32 ? 64 : GROUP, RowsMinBlocks<GROUP>
           }
           const uint32_t total = __shfl_sync(0xffffffffu, off, 31);
           off = i < u_end ? off - len : 0xffffffffu;  // exclusive
-          count_window<GROUP, DENSE, BITMAP>(a, table, seen, tsize, cbits, n_pass, pass, off, s, 0u, total, lane);
+          if (SORTED) {
+            gather_window(a, keys + n_keys, dhist, sd, off, s, total, lane);
+            n_keys += total;
+          } else {
+            count_window<GROUP, DENSE, BITMAP>(a, table, seen, tsize, cbits, n_pass, pass, off, s, 0u, total, lane);
+          }
         }
       } else {
         // CTA-owned row: the count barrier waits for the busiest warp, and B' degrees are Zipf-skewed, so the warps
@@ -868,7 +1029,14 @@ __global__ void __launch_bounds__(GROUP == 32 ? 64 : GROUP, RowsMinBlocks<GROUP>
       const uint32_t seg = (((tsize + NW - 1) / NW) + 31u) & ~31u;
       const uint32_t seg_lo = min((uint32_t)gw * seg, tsize), seg_hi = min(seg_lo + seg, tsize);
       uint32_t n_mine = 0;
-      for (uint32_t pos = seg_lo; pos < seg_hi; pos += 32) {
+      const uint32_t *list = table;   // the cells the filter reads (SORTED: the second half of the sort)
+      if (SORTED) {
+        uint32_t n_runs;
+        n_mine = sort_runs(keys, n_keys, dhist, sd, cbits, diag, a.top_k, &n_runs, lane);
+        list = keys + n_keys;
+        if (lane == 0) distinct_local += n_runs;
+      }
+      for (uint32_t pos = seg_lo; pos < seg_hi && !SORTED; pos += 32) {
         const uint32_t idx = pos + lane;
         uint32_t w = DENSE ? 0u : kEmpty;
         if (idx < seg_hi) w = table[idx];
@@ -884,7 +1052,7 @@ __global__ void __launch_bounds__(GROUP == 32 ? 64 : GROUP, RowsMinBlocks<GROUP>
         n_mine += __popc(m);
         __syncwarp();
       }
-      if (lane == 0) distinct_local += n_mine;
+      if (lane == 0 && !SORTED) distinct_local += n_mine;
       uint32_t n_list = n_mine;   // cells this warp filters: its compacted table words, then (BITMAP) its singles
       const uint32_t *singles_mine = singles;
       if (BITMAP) {
@@ -934,7 +1102,7 @@ __global__ void __launch_bounds__(GROUP == 32 ? 64 : GROUP, RowsMinBlocks<GROUP>
         singles_mine = singles + s_lo;
         n_list = n_mine + (s_hi - s_lo);
       }
-      if (!BITMAP && a.emit_all) {
+      if (!BITMAP && !SORTED && a.emit_all) {
         // debug: every non-zero cell of the row (col, count), unordered
         int basepos = 0;
         if (lane == 0) basepos = atomicAdd(&ctrl[0], (int)n_mine);
@@ -960,8 +1128,8 @@ __global__ void __launch_bounds__(GROUP == 32 ? 64 : GROUP, RowsMinBlocks<GROUP>
       // colB are ordered by column id, the output's tie order, so the cut is exact and drops ties beyond the k-th too.
       // Both hold for the COMPUTED fp64 values only when adjacent colB values are further apart than the evaluation
       // error: the host checks that once per indicator (a.cut_ok) and otherwise the row runs without the cut.
-      int cut1 = 0x7fffffff;   // (BITMAP: the singles list is already cut)
-      if (!BITMAP && a.cut_ok && a.row_work[item] < 65536u) {   // u16 bins cannot overflow
+      int cut1 = 0x7fffffff;   // (BITMAP, SORTED: the singles list is already cut)
+      if (!BITMAP && !SORTED && a.cut_ok && a.row_work[item] < 65536u) {   // u16 bins cannot overflow
         int sh = keyed ? a.key_shift : 0, hi_sh = 32;   // level: bins over key bits [sh, hi_sh) of keys matching `prefix` above
         uint32_t prefix = 0, need = (uint32_t)a.top_k;
         while (true) {
@@ -1013,7 +1181,7 @@ __global__ void __launch_bounds__(GROUP == 32 ? 64 : GROUP, RowsMinBlocks<GROUP>
           bool surv = false;
           uint32_t word = 0;
           if (q < n_list) {
-            word = (!BITMAP || q < n_mine) ? table[seg_lo + q] : singles_mine[q - n_mine];
+            word = (!BITMAP || q < n_mine) ? list[seg_lo + q] : singles_mine[q - n_mine];
             const uint32_t b = word >> cbits, k11 = word & cmask;
             if ((int)b != diag) {
               // Dominance filter (exact, DESIGN.md "dominance"): for fixed rowA and N, on the positively associated
