@@ -898,6 +898,74 @@ int cco_index_pages_finish(cco_index_pages_t *h, cco_index_pages_out_t *out);
 int cco_index_pages_free(cco_index_pages_t *h);
 
 /*
+ * Index write: the model index written into Elasticsearch as URModel.save and EsClient.hotSwap write it (URModel.scala:
+ * 47-84, EsClient.scala:168-246, 257-362), every part that reads the body or the answers.  The HTTP calls stay with the
+ * caller: it sends the byte ranges of the body as POST /<index>/<type>/_bulk requests and hands each response body back.
+ *  - begin: the body, in the form cco_format_model, cco_rerank_model and cco_index_pages write ({"index":{..."_id":"<s>"...}}
+ *    and one object line per document, each line ending in '\n'), checked with cco_rerank_model's rules (a repeated _id
+ *    included); CCO_E_INVALID_ARG names the 0-based document.  The body stays on the device for the session.
+ *  - fields: esFields (URModel.scala:78), every distinct decoded member name of the document lines in order of first
+ *    appearance (document order, then member order), each escaped as cco_format_model escapes names; "id", which save
+ *    adds to every document, goes last when no document line has it (and there is a document).
+ *  - requests: the greedy cut of the body into _bulk requests of at most max_docs documents and max_bytes bytes (action and
+ *    document lines); a document larger than max_bytes is a request of its own.  Request q holds the documents
+ *    [doc_begin[q], doc_begin[q + 1]) and the bytes [byte_begin[q], byte_begin[q + 1]) of the body.
+ *  - response: the body of the response to request q.  Requests are answered in any order, each once.  The response is
+ *    one object whose "items" array holds one item per document of the request, in order; item i is {"index":{...}} with a
+ *    string _id equal to document i's decoded _id, a 32-bit integer status and, for an error, error.type and error.reason
+ *    (strings; caused_by and every other member are skipped).  ES 5 .. 8 shapes, compact or ?pretty, any member order.
+ *    Each document's latest status is kept on the device.
+ *  - retry: the documents whose latest status is 429, their lines in document order as a new body, cut by the same rule
+ *    into requests numbered from first_request on; their responses are handed to response like the others.
+ *  - finish: the latest status per document (0: never answered), the counts, and for every document whose latest status
+ *    is not 2xx its index and the decoded error.type and error.reason of its latest error (empty when it had none).
+ * Errors: CCO_E_INVALID_ARG naming the request (and the item or the byte offset where they apply) for malformed JSON, a
+ * top level that is not an object, a top-level "error" member (with the response's status when it has one), a missing or
+ * non-array "items", an item count other than the request's documents, an item that is not {"index":{...}}, a missing,
+ * repeated or non-string _id, an _id that is not the document's, a missing, repeated or non-integer status, a request
+ * number out of range and a request answered twice.  CCO_E_UNSUPPORTED for group contexts, a body or a response larger
+ * than a quarter of the device's memory, and 2^31 or more documents or members.  After a failed call every call but free
+ * fails with the same message.  Every pointer an out-structure receives is pinned memory of the context, released with
+ * cco_host_free.
+ */
+typedef struct cco_index_write cco_index_write_t;
+typedef struct {
+  int64_t max_docs;      /* documents per request, >= 1 (elasticsearch-hadoop es.batch.size.entries: 1000) */
+  int64_t max_bytes;     /* bytes per request, >= 1 (es.batch.size.bytes: 1 MiB) */
+} cco_index_write_params_t;
+typedef struct {
+  int64_t n_docs;        /* documents to send again */
+  int64_t *doc;          /* [n_docs] their indexes, ascending */
+  char *body;            /* their lines, in document order */
+  int64_t body_len;
+  int64_t first_request; /* the number of the first retry request */
+  int64_t n_requests;
+  int64_t *doc_begin;    /* [n_requests + 1] positions in doc[] */
+  int64_t *byte_begin;   /* [n_requests + 1] offsets in body */
+} cco_index_write_retry_t;
+typedef struct {
+  int64_t n_docs;
+  int32_t *status;       /* [n_docs] the latest status, 0 if never answered */
+  int64_t n_ok;          /* 2xx */
+  int64_t n_rejected;    /* 429 */
+  int64_t n_failed;      /* anything else, never answered included */
+  int64_t n_errors;      /* n_rejected + n_failed */
+  int64_t *error_doc;    /* [n_errors] ascending */
+  int64_t *type_offsets; /* [n_errors + 1], Arrow large_string */
+  char *type_bytes;
+  int64_t *reason_offsets;
+  char *reason_bytes;
+} cco_index_write_out_t;
+int cco_index_write_begin(cco_ctx_t *ctx, const char *body, int64_t len, const cco_index_write_params_t *params,
+                          cco_index_write_t **out);
+int cco_index_write_fields(cco_index_write_t *h, int64_t *n, int64_t **name_offsets, char **name_bytes);
+int cco_index_write_requests(cco_index_write_t *h, int64_t *n_requests, int64_t **doc_begin, int64_t **byte_begin);
+int cco_index_write_response(cco_index_write_t *h, int64_t request, const char *resp, int64_t len);
+int cco_index_write_retry(cco_index_write_t *h, cco_index_write_retry_t *out);
+int cco_index_write_finish(cco_index_write_t *h, cco_index_write_out_t *out);
+int cco_index_write_free(cco_index_write_t *h);
+
+/*
  * Debug/parity entry (tests only): full integer co-occurrence matrix A^T B of two canonical
  * binary matrices computed by the same accumulation kernel as cco_train, no LLR, no top-k.
  * Output CSR over the columns of A with ascending column ids, malloc'ed; free with cco_free.

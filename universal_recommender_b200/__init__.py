@@ -24,6 +24,9 @@ Host-side mirror of the reference interface for this path:
   ur_algorithm.index_from_pages           <- EsClient.getRDD / esJsonRDD (calcPop) and EsClient.getSource (item queries):
                                              the model index read back from Elasticsearch _search / scroll pages into the
                                              bulk body, on the GPU (cco_index_pages_*); ur_model.index_from_pages
+  ur_algorithm.write_index                <- URModel.save -> EsClient.hotSwap: the mapping, bounded _bulk requests, their
+                                             responses read on the GPU (cco_index_write_*), 429 retries and the alias swap,
+                                             over a caller-supplied request function; ur_model.index_mapping / alias_actions
   ur_model                                <- propertiesRDD, getRanksRDD, groupAll (URAlgorithm.scala:351-369, 537-560;
                                              URModel.scala:57-140): the host mirror of the model documents
 """
@@ -32,10 +35,10 @@ from ._native import (CcoError, CcoInvalidArgument, FLAG_ASSUME_CANONICAL, FLAG_
 from .events import DataSourceParams, EventWindow
 from .indexed_dataset import BiDictionary, IndexedDataset
 from .preparator import prepare, prepare_on_device
-from .similarity_analysis import (CcoContext, DownsamplableCrossOccurrenceDataset, EventLog, IndexPages, SearchResults, SimilarityAnalysis,
+from .similarity_analysis import (CcoContext, DownsamplableCrossOccurrenceDataset, EventLog, IndexPages, IndexWrite, IndexWriteResult, SearchResults, SimilarityAnalysis,
                                   decode_ids, default_context, encode_ids)
 from .ur_algorithm import (DefaultURAlgoParams, IndicatorParams, URAlgorithmParams, calc_all, calc_all_from_events, calc_all_on_device,
-                           batchpredict_output, calc_pop_from_events, calc_pop_on_device, index_from_pages, item_queries, item_set_queries, mixed_queries_from_events,
+                           batchpredict_output, calc_pop_from_events, calc_pop_on_device, index_from_pages, IndexWriteError, write_index, item_queries, item_set_queries, mixed_queries_from_events,
                            predictions_from_responses, queries_from_file, user_queries_from_events)
 from .ur_query import ItemQuery, ItemSetQuery, MixedQuery, UserQuery
 from .ur_model import RankingParams
@@ -44,7 +47,7 @@ __all__ = [
     "BiDictionary", "CcoContext", "CcoError", "CcoInvalidArgument", "DataSourceParams", "DefaultURAlgoParams", "EventWindow",
     "DownsamplableCrossOccurrenceDataset", "IndexedDataset", "IndicatorParams", "SimilarityAnalysis",
     "EventLog", "RankingParams", "URAlgorithmParams", "calc_all", "calc_all_from_events", "calc_all_on_device", "calc_pop_from_events",
-    "batchpredict_output", "calc_pop_on_device", "item_queries", "item_set_queries", "mixed_queries_from_events", "predictions_from_responses", "queries_from_file", "SearchResults", "IndexPages", "index_from_pages", "user_queries_from_events", "ItemQuery", "ItemSetQuery", "MixedQuery", "UserQuery", "decode_ids", "default_context", "encode_ids", "prepare", "prepare_on_device",
+    "batchpredict_output", "calc_pop_on_device", "item_queries", "item_set_queries", "mixed_queries_from_events", "predictions_from_responses", "queries_from_file", "SearchResults", "IndexPages", "index_from_pages", "IndexWrite", "IndexWriteResult", "IndexWriteError", "write_index", "user_queries_from_events", "ItemQuery", "ItemSetQuery", "MixedQuery", "UserQuery", "decode_ids", "default_context", "encode_ids", "prepare", "prepare_on_device",
     "FLAG_ASSUME_CANONICAL",
     "FLAG_ENTROPY_VARARGS", "FLAG_ROWRATE_INTDIV", "FLAG_RESULT_NO_COUNT", "FLAG_RESULT_NO_LLR", "LIB_PATH",
 ]

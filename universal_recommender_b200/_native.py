@@ -145,6 +145,23 @@ class IndexPagesOutT(C.Structure):
     _fields_ = [("n_docs", C.c_int64), ("total", C.c_int64), ("body", C.c_void_p), ("body_len", C.c_int64)]
 
 
+class IndexWriteParamsT(C.Structure):
+    _fields_ = [("max_docs", C.c_int64), ("max_bytes", C.c_int64)]
+
+
+class IndexWriteRetryT(C.Structure):
+    _fields_ = [("n_docs", C.c_int64), ("doc", C.POINTER(C.c_int64)), ("body", C.c_void_p), ("body_len", C.c_int64),
+                ("first_request", C.c_int64), ("n_requests", C.c_int64), ("doc_begin", C.POINTER(C.c_int64)),
+                ("byte_begin", C.POINTER(C.c_int64))]
+
+
+class IndexWriteOutT(C.Structure):
+    _fields_ = [("n_docs", C.c_int64), ("status", C.POINTER(C.c_int32)), ("n_ok", C.c_int64), ("n_rejected", C.c_int64),
+                ("n_failed", C.c_int64), ("n_errors", C.c_int64), ("error_doc", C.POINTER(C.c_int64)),
+                ("type_offsets", C.POINTER(C.c_int64)), ("type_bytes", C.c_void_p), ("reason_offsets", C.POINTER(C.c_int64)),
+                ("reason_bytes", C.c_void_p)]
+
+
 SR_WITH_RANKS = 1
 SR_TEXT = 2
 SR_BATCHPREDICT = 4
@@ -174,7 +191,7 @@ EXPORTS = [
     "cco_format_model", "cco_rerank_model", "cco_event_log_read", "cco_event_log_info", "cco_event_log_ingest",
     "cco_format_model_log", "cco_rerank_model_log", "cco_event_log_free", "cco_event_log_begin", "cco_event_log_append",
     "cco_event_log_finish", "cco_event_log_begin_window", "cco_event_log_window_stats",
-    "cco_event_log_begin_ex", "cco_event_log_user_queries", "cco_item_queries", "cco_item_set_queries", "cco_mixed_queries", "cco_query_file_read", "cco_query_file_templates", "cco_query_file_queries", "cco_query_file_free", "cco_search_results_begin", "cco_search_results_append", "cco_search_results_finish", "cco_search_results_free", "cco_index_pages_begin", "cco_index_pages_append", "cco_index_pages_finish", "cco_index_pages_free", "cco_result_num_matrices", "cco_result_row_range", "cco_result_matrix", "cco_result_stats", "cco_result_free",
+    "cco_event_log_begin_ex", "cco_event_log_user_queries", "cco_item_queries", "cco_item_set_queries", "cco_mixed_queries", "cco_query_file_read", "cco_query_file_templates", "cco_query_file_queries", "cco_query_file_free", "cco_search_results_begin", "cco_search_results_append", "cco_search_results_finish", "cco_search_results_free", "cco_index_pages_begin", "cco_index_pages_append", "cco_index_pages_finish", "cco_index_pages_free", "cco_index_write_begin", "cco_index_write_fields", "cco_index_write_requests", "cco_index_write_response", "cco_index_write_retry", "cco_index_write_finish", "cco_index_write_free", "cco_result_num_matrices", "cco_result_row_range", "cco_result_matrix", "cco_result_stats", "cco_result_free",
     "cco_debug_cooccurrence", "cco_debug_downsample", "cco_debug_downsample_block", "cco_debug_llr", "cco_debug_string_ids", "cco_debug_rank_text", "cco_free",
 ]
 
@@ -256,6 +273,13 @@ def lib():
     L.cco_index_pages_append.argtypes = [C.c_void_p, C.c_char_p, C.c_int64, p(C.c_int64), p(C.c_void_p), p(C.c_int64)]
     L.cco_index_pages_finish.argtypes = [C.c_void_p, p(IndexPagesOutT)]
     L.cco_index_pages_free.argtypes = [C.c_void_p]
+    L.cco_index_write_begin.argtypes = [C.c_void_p, C.c_char_p, C.c_int64, p(IndexWriteParamsT), p(C.c_void_p)]
+    L.cco_index_write_fields.argtypes = [C.c_void_p, p(C.c_int64), p(p(C.c_int64)), p(C.c_void_p)]
+    L.cco_index_write_requests.argtypes = [C.c_void_p, p(C.c_int64), p(p(C.c_int64)), p(p(C.c_int64))]
+    L.cco_index_write_response.argtypes = [C.c_void_p, C.c_int64, C.c_char_p, C.c_int64]
+    L.cco_index_write_retry.argtypes = [C.c_void_p, p(IndexWriteRetryT)]
+    L.cco_index_write_finish.argtypes = [C.c_void_p, p(IndexWriteOutT)]
+    L.cco_index_write_free.argtypes = [C.c_void_p]
     L.cco_mixed_queries.argtypes = [C.c_void_p, C.c_void_p, C.c_char_p, C.c_int64, p(MixedQueryT), C.c_int64,
                                     p(C.c_int64), C.c_void_p, C.c_void_p, p(C.c_int64), C.c_void_p, C.c_void_p,
                                     p(C.c_int64), C.c_int64, p(C.c_int64), C.c_void_p, C.c_void_p,

@@ -33,6 +33,7 @@
 #include "cco_queries.cuh"
 #include "cco_results.cuh"
 #include "cco_index_pages.cuh"
+#include "cco_index_write.cuh"
 
 namespace cco {
 
@@ -3318,6 +3319,7 @@ struct BulkDocs {
   JMember *mem = nullptr;                // [M1]
   DevStrCol names, ids;                  // decoded member names [M1] and _ids [D] (offsets from 0)
   long long ids_bytes = 0;
+  const long long *line_b = nullptr;     // [2 D]: the first byte of each line
 };
 // upload, line split, members, the action / _id checks and the decoded names and ids (cco_rerank_model's grammar; the
 // messages name the 0-based document).  extra entries share the 2^31 limit with the documents; `what` names them.
@@ -3338,6 +3340,7 @@ static int bulk_parse(cco_ctx *c, Arena &ar, const char *body, int64_t body_len,
   const long long D = L / 2;
   if (D + extra >= 0x7fffffffLL) return set_error(CCO_E_UNSUPPORTED, "documents + %s must stay < 2^31 per call", what);
   bd->D = D;
+  bd->line_b = sb;
   if (D == 0) return CCO_OK;
   // 3. members of every line; the verdict on the whole body comes before anything reads through the spans
   unsigned long long *err, h_err = 0;
@@ -7445,5 +7448,492 @@ int cco_index_pages_free(cco_index_pages_t *h) {
   delete h;
   return CCO_OK;
 }
+
+// ---- cco_index_write: the model index written into Elasticsearch (URModel.save, EsClient.hotSwap), kernels in
+// cco_index_write.cuh ----------------------------------------------------------------------------------------------------
+struct cco_index_write {
+  cco_ctx *ctx = nullptr;
+  Arena *ar = nullptr;                 // the body, its parse, the statuses and the retry lists, for the session
+  BulkDocs bd;
+  int32_t *status = nullptr;           // [D] on the device: each document's latest status, 0 if never answered
+  char *hbody = nullptr;               // the body in pinned memory: retry bodies are gathered from it
+  long long len = 0, max_docs = 0, max_bytes = 0;
+  std::vector<long long> doc_b;        // [D + 1]: the first byte of each document's action line, len at D
+  struct Req {
+    int round;                         // -1: the documents [b, e); else the positions [b, e) of retry round `round`
+    long long b, e;
+    bool answered;
+  };
+  std::vector<Req> reqs;
+  long long n_first = 0;               // requests of the body itself
+  std::vector<long long> first_db, first_bb;
+  std::vector<std::vector<long long>> round_docs;   // the documents of each retry round, ascending
+  std::vector<long long *> round_ddocs;             // their device copies
+  std::unordered_map<long long, std::pair<std::string, std::string>> errors;   // each document's latest error.type, .reason
+  bool failed = false, finished = false;
+  std::string fail_msg;
+  int fail_code = CCO_OK;
+};
+
+extern "C++" {
+namespace cco {
+
+static const char *iw_message(int code) {
+  switch (code) {
+    case kIwNotObject: return "the top level is not an object";
+    case kIwError: return "Elasticsearch returned an error";
+    case kIwNoItems: return "the response has no \"items\" array";
+    case kIwItemNotObject: return "an items element is not an object";
+    case kIwNotIndex: return "the item is not {\"index\":{...}}";
+    case kIwNoId: return "the item has no string _id";
+    case kIwRepeatedId: return "a repeated _id";
+    case kIwIdMismatch: return "the item's _id is not the document's _id";
+    case kIwNoStatus: return "the item has no status";
+    case kIwRepeatedStatus: return "a repeated status";
+    case kIwBadStatus: return "the status is not a 32-bit integer";
+  }
+  return sr_message(code);
+}
+// The greedy cut of documents of the given sizes into requests of at most max_docs documents and max_bytes bytes; a
+// document larger than max_bytes is a request of its own.  db / bb: the requests' first document and byte, then the ends.
+static void iw_cut(const std::vector<long long> &size, long long max_docs, long long max_bytes, std::vector<long long> &db,
+                   std::vector<long long> &bb) {
+  db.assign(1, 0);
+  bb.assign(1, 0);
+  long long n = 0, bytes = 0, at = 0;
+  for (size_t k = 0; k < size.size(); ++k) {
+    if (n > 0 && (n == max_docs || bytes + size[k] > max_bytes)) {
+      db.push_back((long long)k);
+      bb.push_back(at);
+      n = 0;
+      bytes = 0;
+    }
+    ++n;
+    bytes += size[k];
+    at += size[k];
+  }
+  if (n > 0) {
+    db.push_back((long long)size.size());
+    bb.push_back(at);
+  }
+}
+template <typename T>
+static T *iw_pinned(cco_ctx *c, size_t n) {
+  return (T *)c->pinned_get(sizeof(T) * std::max<size_t>(n, 1), /*for_result=*/false);
+}
+template <typename T>
+static int iw_put(cco_ctx *c, const std::vector<T> &v, T **out) {
+  *out = iw_pinned<T>(c, v.size());
+  if (!*out) return set_error(CCO_E_OOM, "pinned host allocation failed");
+  if (!v.empty()) memcpy(*out, v.data(), sizeof(T) * v.size());
+  return CCO_OK;
+}
+
+// The body on the device: its documents checked as cco_rerank_model checks them (a repeated _id included), the documents'
+// first bytes on the host, and the requests of the body itself.
+static int iw_begin(cco_index_write *h, const char *body, long long len) {
+  cco_ctx *c = h->ctx;
+  cudaStream_t s = c->stream;
+  h->ar = new Arena(s);
+  Arena &ar = *h->ar;
+  NvtxRange nvtx("cco:index_write");
+  mail_reset(c);
+  BulkDocs &bd = h->bd;
+  CKR(bulk_parse(c, ar, body, len, 0, "nothing", &bd));
+  const long long D = bd.D;
+  h->doc_b.assign((size_t)D + 1, len);
+  CKR(ar.alloc(&h->status, std::max<long long>(D, 1)));
+  CK(cudaMemsetAsync(h->status, 0, sizeof(int32_t) * (size_t)std::max<long long>(D, 1), s));
+  if (D > 0) {
+    str_hash(c, bd.ids, ~0ULL);
+    int32_t *gid;
+    CKR(ar.alloc(&gid, D));
+    StrTable tb;
+    CKR(str_group(c, ar, bd.ids, nullptr, false, 0, &tb, gid));
+    CKR(iq_unique_ids(c, ar, D, gid, tb));
+    str_table_release(ar, tb);
+    ar.release(gid);
+    CK(cudaMemcpy2DAsync(h->doc_b.data(), sizeof(long long), bd.line_b, 2 * sizeof(long long), sizeof(long long), (size_t)D,
+                         cudaMemcpyDeviceToHost, s));
+  }
+  h->hbody = iw_pinned<char>(c, (size_t)len);
+  if (!h->hbody) return set_error(CCO_E_OOM, "pinned host allocation of %lld bytes failed", len);
+  if (len > 0) memcpy(h->hbody, body, (size_t)len);
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  std::vector<long long> size((size_t)D);
+  for (long long d = 0; d < D; ++d) size[d] = h->doc_b[d + 1] - h->doc_b[d];
+  iw_cut(size, h->max_docs, h->max_bytes, h->first_db, h->first_bb);
+  h->n_first = (long long)h->first_db.size() - 1;
+  for (long long q = 0; q < h->n_first; ++q) h->reqs.push_back({-1, h->first_db[q], h->first_db[q + 1], false});
+  return CCO_OK;
+}
+
+// esFields: the distinct decoded names of the document lines' members in first-appearance order, escaped; "id" last when
+// no document line has it.
+static int iw_fields(cco_index_write *h, int64_t *n_out, int64_t **name_offsets, char **name_bytes) {
+  cco_ctx *c = h->ctx;
+  cudaStream_t s = c->stream;
+  Arena ar(s);
+  NvtxRange nvtx("cco:index_write");
+  mail_reset(c);
+  const BulkDocs &bd = h->bd;
+  const long long D = bd.D;
+  long long ng = 0, total = 0;
+  DevDict esc = {nullptr, nullptr, 0};
+  if (D > 0 && bd.M1 > 0) {
+    int32_t *gate, *gid;
+    CKR(ar.alloc(&gate, bd.M1));
+    CKR(ar.alloc(&gid, bd.M1));
+    k_iw_gate<<<grid_for(2 * D, 256, c->sm_count), 256, 0, s>>>(2 * D, bd.line_moff, gate);
+    c->launches++;
+    str_hash(c, bd.names, ~0ULL);
+    StrTable tb;
+    CKR(str_group(c, ar, bd.names, gate, false, 0, &tb, gid));
+    ng = tb.n_groups;
+    long long *len, *off;
+    CKR(ar.alloc(&len, ng + 1));
+    CKR(ar.alloc(&off, ng + 1));
+    CK(cudaMemsetAsync(len + ng, 0, 8, s));
+    if (ng > 0) {
+      k_str_dict_len<<<grid_for(ng, 256, c->sm_count), 256, 0, s>>>(ng, tb.first_sorted, bd.names.off, len);
+      c->launches++;
+    }
+    CKR(exclusive_sum(c, ar, len, off, ng + 1));
+    long long raw_total = 0;
+    CKR(mail_fetch(c, &raw_total, off + ng, 8));
+    CKR(mail_wait(c));
+    unsigned char *raw;
+    CKR(ar.alloc(&raw, std::max<long long>(raw_total, 1)));
+    if (ng > 0 && raw_total > 0) {
+      k_str_dict_gather<<<grid_for(ng, 256, c->sm_count), 256, 0, s>>>(ng, tb.first_sorted, bd.names.off, bd.names.base,
+                                                                      (const unsigned char *)bd.names.w, off, raw);
+      c->launches++;
+    }
+    CKR(escape_dict(c, ar, DevDict{off, raw, ng}, &esc));   // waits for its total
+    CK(cudaMemcpyAsync(&total, esc.off + ng, 8, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+  }
+  int64_t *ho = iw_pinned<int64_t>(c, (size_t)ng + 2);
+  char *hb = iw_pinned<char>(c, (size_t)total + 2);
+  if (!ho || !hb) return set_error(CCO_E_OOM, "pinned host allocation failed");
+  ho[0] = 0;
+  if (ng > 0) {
+    CK(cudaMemcpyAsync(ho, esc.off, sizeof(int64_t) * ((size_t)ng + 1), cudaMemcpyDeviceToHost, s));
+    if (total > 0) CK(cudaMemcpyAsync(hb, esc.bytes, (size_t)total, cudaMemcpyDeviceToHost, s));
+  }
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  bool has_id = false;
+  for (long long k = 0; k < ng && !has_id; ++k) has_id = ho[k + 1] - ho[k] == 2 && hb[ho[k]] == 'i' && hb[ho[k] + 1] == 'd';
+  if (D > 0 && !has_id) {   // save adds "id" to every document (URModel.scala:73)
+    hb[total] = 'i';
+    hb[total + 1] = 'd';
+    ho[++ng] = total + 2;
+  }
+  *n_out = ng;
+  *name_offsets = ho;
+  *name_bytes = hb;
+  return CCO_OK;
+}
+
+// One _bulk response body for request q: its structural index, the top walk, one warp per item.
+static int iw_response(cco_index_write *h, long long q, const char *resp, long long len) {
+  cco_ctx *c = h->ctx;
+  cudaStream_t s = c->stream;
+  if (q < 0 || q >= (long long)h->reqs.size())
+    return set_error(CCO_E_INVALID_ARG, "request %lld is out of range: there are %lld requests", q, (long long)h->reqs.size());
+  cco_index_write::Req &rq = h->reqs[q];
+  if (rq.answered) return set_error(CCO_E_INVALID_ARG, "request %lld is answered twice", q);
+  const long long n_docs = rq.e - rq.b;
+  const size_t padded = (size_t)((len + 63) / 64 * 64) + 64;
+  size_t free_b = 0, total_b = 0;
+  CK(cudaMemGetInfo(&free_b, &total_b));
+  if (padded > total_b / 4)
+    return set_error(CCO_E_UNSUPPORTED, "request %lld: a response of %lld bytes: at most a quarter of the device's memory", q, len);
+  Arena ar(s);
+  NvtxRange nvtx("cco:index_write");
+  mail_reset(c);
+  auto byte_error = [&](long long at, int code) {
+    return set_error(CCO_E_INVALID_ARG, "request %lld, byte %lld: %s", q, at, iw_message(code));
+  };
+  unsigned char *page;
+  CKR(ar.alloc(&page, padded));
+  if (len > 0) CK(cudaMemcpyAsync(page, resp, (size_t)len, cudaMemcpyHostToDevice, s));
+  CK(cudaMemsetAsync(page + len, ' ', padded - (size_t)len, s));
+  // the structural index down to the members of an item's error
+  const long long NW = (len + 63) / 64, n_chunks = (NW + kSrChunkWords - 1) / kSrChunkWords;
+  unsigned long long *err;
+  CKR(ar.alloc(&err, 4));
+  CK(cudaMemsetAsync(err, 0xff, 24, s));
+  CK(cudaMemsetAsync(err + 3, 0, 8, s));
+  SrFun *fun, *pre;
+  long long *cnt, *coff;
+  CKR(ar.alloc(&fun, n_chunks + 1));
+  CKR(ar.alloc(&pre, n_chunks + 1));
+  CKR(ar.alloc(&cnt, n_chunks + 1));
+  CKR(ar.alloc(&coff, n_chunks + 1));
+  CK(cudaMemsetAsync(cnt + n_chunks, 0, 8, s));
+  SrFun fin = sr_identity();
+  long long m = 0;
+  if (n_chunks > 0) {
+    const int grid = grid_for(n_chunks * 32, 256, c->sm_count);
+    k_sr_chunk<<<grid, 256, 0, s>>>(NW, (const uint4 *)page, fun);
+    k_sr_scan<<<1, kSrScanThreads, 0, s>>>(n_chunks, fun, pre);
+    k_sr_index<false><<<grid, 256, 0, s>>>(NW, (const uint4 *)page, pre, kIwMaxDepth, cnt, nullptr, nullptr, nullptr, err);
+    c->launches += 3;
+    CKR(mail_fetch(c, &fin, pre + n_chunks - 1, sizeof(SrFun)));
+  }
+  CKR(exclusive_sum(c, ar, cnt, coff, n_chunks + 1));
+  unsigned long long e0 = ~0ULL;
+  CKR(mail_fetch(c, &m, coff + n_chunks, 8));
+  CKR(mail_fetch(c, &e0, err, 8));
+  CKR(mail_wait(c));
+  if (e0 != ~0ULL) return byte_error((long long)(e0 >> 8), (int)(e0 & 0xff));
+  if (fin.f[0] >> 1) return set_error(CCO_E_INVALID_ARG, "request %lld, byte %lld: a string is not closed", q, len);
+  if (fin.d[0] != 0) return byte_error(len, kSrUnbalanced);
+  long long *pos;
+  unsigned char *dep;
+  CKR(ar.alloc(&pos, m + 1));
+  CKR(ar.alloc(&dep, m + 1));
+  if (m > 0) {
+    k_sr_index<true><<<grid_for(n_chunks * 32, 256, c->sm_count), 256, 0, s>>>(NW, (const uint4 *)page, pre, kIwMaxDepth, nullptr, coff, pos, dep, err);
+    c->launches++;
+  }
+  // the top walk over the entries down to the items' brackets
+  long long *top, nt = 0, *iopen, *iclose;
+  CKR(sr_select(c, ar, m, dep, 0, kIwTopDepth, -1, m, &top, &nt));
+  CKR(ar.alloc(&iopen, nt / 2 + 1));
+  CKR(ar.alloc(&iclose, nt / 2 + 1));
+  IwTop *d_top, r;
+  CKR(ar.alloc(&d_top, 1));
+  k_iw_top<<<1, 32, 0, s>>>(SrIdx{pos, dep, page, top}, nt, len, d_top, iopen, iclose);
+  c->launches++;
+  CKR(mail_fetch(c, &r, d_top, sizeof r));
+  CKR(mail_wait(c));
+  if (r.code == kIwNotObject || r.code == kIwNoItems) return set_error(CCO_E_INVALID_ARG, "request %lld: %s", q, iw_message(r.code));
+  if (r.code == kIwError) {
+    if (r.has_status) return set_error(CCO_E_INVALID_ARG, "request %lld: %s (status %lld)", q, iw_message(r.code), r.status);
+    return set_error(CCO_E_INVALID_ARG, "request %lld: %s", q, iw_message(r.code));
+  }
+  if (r.code) return byte_error(r.bad, r.code);
+  if (r.n_items != n_docs)
+    return set_error(CCO_E_INVALID_ARG, "request %lld: %lld items for %lld documents", q, r.n_items, n_docs);
+  if (n_docs > 0) {
+    const long long *ddocs = rq.round < 0 ? nullptr : h->round_ddocs[rq.round] + rq.b;
+    const IwItems it = {ddocs, rq.round < 0 ? rq.b : 0, h->bd.ids.off, (const unsigned char *)h->bd.ids.w};
+    IwFail *fail;
+    CKR(ar.alloc(&fail, n_docs));
+    k_iw_item<<<grid_for(n_docs * 32, 256, c->sm_count), 256, 0, s>>>(SrIdx{pos, dep, page, nullptr}, n_docs, iopen, iclose, it, h->status, fail,
+                                                                      err + 3, err + 1, err + 2);
+    c->launches++;
+    unsigned long long e_item = ~0ULL, e_byte = ~0ULL, nf = 0;
+    CKR(mail_fetch(c, &e_item, err + 1, 8));
+    CKR(mail_fetch(c, &e_byte, err + 2, 8));
+    CKR(mail_fetch(c, &nf, err + 3, 8));
+    CKR(mail_wait(c));
+    if (e_byte != ~0ULL) return byte_error((long long)(e_byte >> 8), (int)(e_byte & 0xff));
+    if (e_item != ~0ULL)
+      return set_error(CCO_E_INVALID_ARG, "request %lld, item %lld: %s", q, (long long)(e_item >> 8), iw_message((int)(e_item & 0xff)));
+    if (nf > 0) {   // failures are few: their error texts are decoded on the host, from the caller's response
+      std::vector<IwFail> hf((size_t)nf);
+      CK(cudaMemcpyAsync(hf.data(), fail, sizeof(IwFail) * (size_t)nf, cudaMemcpyDeviceToHost, s));
+      CK(cudaStreamSynchronize(s));
+      for (const IwFail &f : hf) {
+        const long long doc = rq.round < 0 ? rq.b + f.item : h->round_docs[rq.round][rq.b + f.item];
+        h->errors[doc] = {f.tb < 0 ? std::string() : ip_unescape(resp + f.tb, f.te - f.tb),
+                          f.rb < 0 ? std::string() : ip_unescape(resp + f.rb, f.re - f.rb)};
+      }
+    }
+  }
+  CK(cudaGetLastError());
+  rq.answered = true;
+  return CCO_OK;
+}
+
+static int iw_statuses(cco_index_write *h, int32_t *out) {
+  if (h->bd.D > 0) CK(cudaMemcpyAsync(out, h->status, sizeof(int32_t) * (size_t)h->bd.D, cudaMemcpyDeviceToHost, h->ctx->stream));
+  CK(cudaStreamSynchronize(h->ctx->stream));
+  return CCO_OK;
+}
+
+// The documents whose latest status is 429 as a new body, gathered from the pinned copy, and its requests.
+static int iw_retry(cco_index_write *h, cco_index_write_retry_t *out) {
+  cco_ctx *c = h->ctx;
+  const long long D = h->bd.D;
+  std::vector<int32_t> st((size_t)D);
+  CKR(iw_statuses(h, st.data()));
+  std::vector<long long> docs, size;
+  for (long long d = 0; d < D; ++d)
+    if (st[d] == 429) {
+      docs.push_back(d);
+      size.push_back(h->doc_b[d + 1] - h->doc_b[d]);
+    }
+  std::vector<long long> db, bb;
+  iw_cut(size, h->max_docs, h->max_bytes, db, bb);
+  char *body = iw_pinned<char>(c, (size_t)bb.back());
+  if (!body) return set_error(CCO_E_OOM, "pinned host allocation failed");
+  long long at = 0;
+  for (size_t k = 0; k < docs.size(); ++k) {
+    memcpy(body + at, h->hbody + h->doc_b[docs[k]], (size_t)size[k]);
+    at += size[k];
+  }
+  long long *dd = nullptr;
+  if (!docs.empty()) {
+    CKR(h->ar->alloc(&dd, docs.size()));
+    CK(cudaMemcpyAsync(dd, docs.data(), sizeof(long long) * docs.size(), cudaMemcpyHostToDevice, c->stream));
+    CK(cudaStreamSynchronize(c->stream));
+  }
+  const int round = (int)h->round_docs.size();
+  h->round_docs.push_back(docs);
+  h->round_ddocs.push_back(dd);
+  memset(out, 0, sizeof *out);
+  out->first_request = (int64_t)h->reqs.size();
+  for (size_t k = 0; k + 1 < db.size(); ++k) h->reqs.push_back({round, db[k], db[k + 1], false});
+  out->n_docs = (int64_t)docs.size();
+  out->body = body;
+  out->body_len = at;
+  out->n_requests = (int64_t)db.size() - 1;
+  std::vector<int64_t> docs64(docs.begin(), docs.end()), db64(db.begin(), db.end()), bb64(bb.begin(), bb.end());
+  CKR(iw_put(c, docs64, &out->doc));
+  CKR(iw_put(c, db64, &out->doc_begin));
+  CKR(iw_put(c, bb64, &out->byte_begin));
+  return CCO_OK;
+}
+
+static int iw_finish(cco_index_write *h, cco_index_write_out_t *out) {
+  cco_ctx *c = h->ctx;
+  const long long D = h->bd.D;
+  memset(out, 0, sizeof *out);
+  int32_t *st = iw_pinned<int32_t>(c, (size_t)D);
+  if (!st) return set_error(CCO_E_OOM, "pinned host allocation failed");
+  out->status = st;
+  CKR(iw_statuses(h, st));
+  std::vector<int64_t> edoc, toff{0}, roff{0};
+  std::string tb, rb;
+  for (long long d = 0; d < D; ++d) {
+    if (st[d] >= 200 && st[d] < 300) {
+      ++out->n_ok;
+      continue;
+    }
+    ++(st[d] == 429 ? out->n_rejected : out->n_failed);
+    edoc.push_back(d);
+    auto e = h->errors.find(d);
+    if (e != h->errors.end()) {
+      tb += e->second.first;
+      rb += e->second.second;
+    }
+    toff.push_back((int64_t)tb.size());
+    roff.push_back((int64_t)rb.size());
+  }
+  out->n_docs = D;
+  out->n_errors = (int64_t)edoc.size();
+  CKR(iw_put(c, edoc, &out->error_doc));
+  CKR(iw_put(c, toff, &out->type_offsets));
+  CKR(iw_put(c, roff, &out->reason_offsets));
+  CKR(iw_put(c, std::vector<char>(tb.begin(), tb.end()), &out->type_bytes));
+  CKR(iw_put(c, std::vector<char>(rb.begin(), rb.end()), &out->reason_bytes));
+  return CCO_OK;
+}
+
+static int iw_fail_with(cco_index_write *h, int st) {
+  h->failed = true;
+  h->fail_code = st;
+  h->fail_msg = cco_last_error();
+  return st;
+}
+static int iw_state(const cco_index_write *h) {
+  if (h->failed) return set_error(h->fail_code == CCO_OK ? CCO_E_INVALID_ARG : h->fail_code, "%s", h->fail_msg.c_str());
+  if (h->finished) return set_error(CCO_E_INVALID_ARG, "the index write is finished");
+  return CCO_OK;
+}
+
+}  // namespace cco
+}  // extern "C++"
+
+int cco_index_write_begin(cco_ctx_t *ctx, const char *body, int64_t len, const cco_index_write_params_t *params, cco_index_write_t **out) {
+  if (!ctx || !out || !params || len < 0 || (len > 0 && !body)) return set_error(CCO_E_INVALID_ARG, "null argument or negative length");
+  *out = nullptr;
+  if (params->max_docs < 1 || params->max_bytes < 1)
+    return set_error(CCO_E_INVALID_ARG, "max_docs = %lld and max_bytes = %lld: both must be at least 1", (long long)params->max_docs,
+                     (long long)params->max_bytes);
+  if (!ctx->members.empty()) return set_error(CCO_E_UNSUPPORTED, "per-GPU contexts only");
+  if (len > 0 && body[len - 1] != '\n') return set_error(CCO_E_INVALID_ARG, "the body does not end in a newline");
+  CK(cudaSetDevice(ctx->device));
+  size_t free_b = 0, total_b = 0;
+  CK(cudaMemGetInfo(&free_b, &total_b));
+  if ((size_t)len > total_b / 4)
+    return set_error(CCO_E_UNSUPPORTED, "a body of %lld bytes: at most a quarter of the device's memory", (long long)len);
+  cco_index_write *h = new cco_index_write();
+  h->ctx = ctx;
+  h->len = len;
+  h->max_docs = params->max_docs;
+  h->max_bytes = params->max_bytes;
+  const int st = iw_begin(h, body, len);
+  if (st != CCO_OK) {
+    const std::string msg = cco_last_error();
+    cco_index_write_free(h);
+    return set_error(st, "%s", msg.c_str());
+  }
+  *out = h;
+  return CCO_OK;
+}
+
+int cco_index_write_fields(cco_index_write_t *h, int64_t *n, int64_t **name_offsets, char **name_bytes) {
+  if (!h || !n || !name_offsets || !name_bytes) return set_error(CCO_E_INVALID_ARG, "null argument");
+  CKR(iw_state(h));
+  CK(cudaSetDevice(h->ctx->device));
+  const int st = iw_fields(h, n, name_offsets, name_bytes);
+  return st == CCO_OK ? st : iw_fail_with(h, st);
+}
+
+int cco_index_write_requests(cco_index_write_t *h, int64_t *n_requests, int64_t **doc_begin, int64_t **byte_begin) {
+  if (!h || !n_requests || !doc_begin || !byte_begin) return set_error(CCO_E_INVALID_ARG, "null argument");
+  CKR(iw_state(h));
+  std::vector<int64_t> db(h->first_db.begin(), h->first_db.end()), bb(h->first_bb.begin(), h->first_bb.end());
+  int st = iw_put(h->ctx, db, doc_begin);
+  if (st == CCO_OK) st = iw_put(h->ctx, bb, byte_begin);
+  if (st != CCO_OK) return iw_fail_with(h, st);
+  *n_requests = h->n_first;
+  return CCO_OK;
+}
+
+int cco_index_write_response(cco_index_write_t *h, int64_t request, const char *resp, int64_t len) {
+  if (!h || len < 0 || (len > 0 && !resp)) return set_error(CCO_E_INVALID_ARG, "null argument or negative length");
+  CKR(iw_state(h));
+  CK(cudaSetDevice(h->ctx->device));
+  const int st = iw_response(h, request, resp, len);
+  return st == CCO_OK ? st : iw_fail_with(h, st);
+}
+
+int cco_index_write_retry(cco_index_write_t *h, cco_index_write_retry_t *out) {
+  if (!h || !out) return set_error(CCO_E_INVALID_ARG, "null argument");
+  CKR(iw_state(h));
+  CK(cudaSetDevice(h->ctx->device));
+  const int st = iw_retry(h, out);
+  return st == CCO_OK ? st : iw_fail_with(h, st);
+}
+
+int cco_index_write_finish(cco_index_write_t *h, cco_index_write_out_t *out) {
+  if (!h || !out) return set_error(CCO_E_INVALID_ARG, "null argument");
+  CKR(iw_state(h));
+  CK(cudaSetDevice(h->ctx->device));
+  const int st = iw_finish(h, out);
+  if (st != CCO_OK) return iw_fail_with(h, st);
+  h->finished = true;
+  return CCO_OK;
+}
+
+int cco_index_write_free(cco_index_write_t *h) {
+  if (!h) return CCO_OK;
+  cudaSetDevice(h->ctx->device);
+  cudaStreamSynchronize(h->ctx->stream);
+  delete h->ar;
+  cudaStreamSynchronize(h->ctx->stream);
+  if (h->hbody) h->ctx->pinned_put(h->hbody);
+  delete h;
+  return CCO_OK;
+}
+
 
 }  // extern "C"

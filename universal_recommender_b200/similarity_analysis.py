@@ -796,6 +796,13 @@ class CcoContext:
         format_model writes, which rerank_model and the query builders take.  Use it as a context manager, or free()."""
         return IndexPages(self)
 
+    def index_write(self, body: bytes, max_docs: int = 1000, max_bytes: int = 1 << 20) -> "IndexWrite":
+        """A session that writes the model index body into Elasticsearch as URModel.save / EsClient.hotSwap do
+        (cco_index_write_*): the fields the mapping names, the _bulk requests, and the responses read on the device.
+        max_docs / max_bytes bound each request (elasticsearch-hadoop's es.batch.size.entries / .bytes).  The HTTP calls
+        are the caller's; ur_algorithm.write_index drives the whole sequence.  Use it as a context manager, or free()."""
+        return IndexWrite(self, body, max_docs, max_bytes)
+
     def rerank_model(self, body: bytes, properties=None, rankings=None, log=None) -> bytes:
         """cco_rerank_model: calcPop (URAlgorithm.scala:375-399, recsModel "backfill") on an existing index.  body = the
         Elasticsearch bulk body of the current model, as format_model writes it; properties and rankings as in format_model.
@@ -1048,6 +1055,107 @@ class CcoContext:
         for p in (orp, oci, ocn):
             self._L.cco_free(p)
         return r, c, n
+
+
+class IndexWrite:
+    """CcoContext.index_write(body): the model index body on the device for one write.  fields() -> esFields (the names
+    the mapping lists); requests() -> the byte slices of the body, one per _bulk request; response(q, body) reads the
+    response to request q (any order, each once); retry() -> (first request number, [(doc indexes, bytes)] per request)
+    for the documents whose latest status is 429; finish() -> IndexWriteResult.  After an error every call but free()
+    raises it again."""
+
+    def __init__(self, ctx: "CcoContext", body: bytes, max_docs: int = 1000, max_bytes: int = 1 << 20):
+        self._ctx = ctx
+        self._h = C.c_void_p()
+        self._body = bytes(body)
+        prm = N.IndexWriteParamsT(int(max_docs), int(max_bytes))
+        N.check(ctx._L.cco_index_write_begin(ctx._h, self._body, len(self._body), C.byref(prm), C.byref(self._h)))
+
+    def _take(self, ptr, n: int, dtype) -> np.ndarray:
+        try:
+            return np.ctypeslib.as_array(ptr, shape=(n,)).copy() if n else np.zeros(0, dtype)
+        finally:
+            self._ctx._L.cco_host_free(self._ctx._h, C.cast(ptr, C.c_void_p))
+
+    def _take_bytes(self, addr, n: int) -> bytes:
+        try:
+            return C.string_at(addr, n) if n else b""
+        finally:
+            self._ctx._L.cco_host_free(self._ctx._h, C.c_void_p(addr))
+
+    def fields(self) -> list[str]:
+        n, off, b = C.c_int64(), C.POINTER(C.c_int64)(), C.c_void_p()
+        N.check(self._ctx._L.cco_index_write_fields(self._h, C.byref(n), C.byref(off), C.byref(b)))
+        o = self._take(off, n.value + 1, np.int64)
+        blob = self._take_bytes(b.value, int(o[-1]))
+        return [blob[o[k]:o[k + 1]].decode("utf-8", "surrogatepass") for k in range(n.value)]
+
+    def cuts(self) -> tuple:
+        """(doc_begin, byte_begin): request q holds documents [doc_begin[q], doc_begin[q + 1]) and body bytes
+        [byte_begin[q], byte_begin[q + 1])"""
+        n, db, bb = C.c_int64(), C.POINTER(C.c_int64)(), C.POINTER(C.c_int64)()
+        N.check(self._ctx._L.cco_index_write_requests(self._h, C.byref(n), C.byref(db), C.byref(bb)))
+        return self._take(db, n.value + 1, np.int64), self._take(bb, n.value + 1, np.int64)
+
+    def requests(self) -> list[bytes]:
+        _, bb = self.cuts()
+        return [self._body[bb[q]:bb[q + 1]] for q in range(len(bb) - 1)]
+
+    def response(self, request: int, body: bytes) -> None:
+        body = bytes(body)
+        N.check(self._ctx._L.cco_index_write_response(self._h, int(request), body, len(body)))
+
+    def retry(self) -> tuple:
+        """-> (first request number, [(document indexes int64[], request bytes)]): the documents whose latest status is
+        429, cut into requests by the same rule; their responses go to response() under those numbers"""
+        out = N.IndexWriteRetryT()
+        N.check(self._ctx._L.cco_index_write_retry(self._h, C.byref(out)))
+        docs = self._take(out.doc, out.n_docs, np.int64)
+        db = self._take(out.doc_begin, out.n_requests + 1, np.int64)
+        bb = self._take(out.byte_begin, out.n_requests + 1, np.int64)
+        body = self._take_bytes(out.body, out.body_len)
+        return out.first_request, [(docs[db[k]:db[k + 1]], body[bb[k]:bb[k + 1]]) for k in range(out.n_requests)]
+
+    def finish(self) -> "IndexWriteResult":
+        out = N.IndexWriteOutT()
+        N.check(self._ctx._L.cco_index_write_finish(self._h, C.byref(out)))
+        status = self._take(out.status, out.n_docs, np.int32)
+        edoc = self._take(out.error_doc, out.n_errors, np.int64)
+        to = self._take(out.type_offsets, out.n_errors + 1, np.int64)
+        ro = self._take(out.reason_offsets, out.n_errors + 1, np.int64)
+        tb = self._take_bytes(out.type_bytes, int(to[-1]))
+        rb = self._take_bytes(out.reason_bytes, int(ro[-1]))
+        errors = [(int(edoc[k]), tb[to[k]:to[k + 1]].decode("utf-8", "surrogatepass"), rb[ro[k]:ro[k + 1]].decode("utf-8", "surrogatepass"))
+                  for k in range(out.n_errors)]
+        return IndexWriteResult(status, out.n_ok, out.n_rejected, out.n_failed, errors)
+
+    def free(self) -> None:
+        if self._h:
+            self._ctx._L.cco_index_write_free(self._h)
+            self._h = C.c_void_p()
+
+    def __enter__(self) -> "IndexWrite":
+        return self
+
+    def __exit__(self, *exc) -> None:
+        self.free()
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass
+
+
+@dataclass
+class IndexWriteResult:
+    """IndexWrite.finish(): the latest status per document (0: never answered), the counts of 2xx, 429 and every other
+    status, and (document index, error.type, error.reason) for every document whose latest status is not 2xx"""
+    status: np.ndarray
+    n_ok: int
+    n_rejected: int
+    n_failed: int
+    errors: list
 
 
 class IndexPages:

@@ -8,9 +8,11 @@ whole user base from the same export (ur_query.py restates buildQuery); item_que
 item of a model index body; item_set_queries builds its item-set ("shopping cart") queries for a batch of sets;
 mixed_queries_from_events builds its queries for rows with any subset of user, item and item set; queries_from_file
 builds them for a batchpredict query file, each line with its own template; index_from_pages reads the model index back
-from Elasticsearch's _search / scroll pages.  Out of scope: Elasticsearch's scoring and the HTTP calls."""
+from Elasticsearch's _search / scroll pages; write_index writes a model index body into Elasticsearch as hotSwap does, over a
+request function the caller supplies.  Out of scope: Elasticsearch's scoring and the HTTP client."""
 from __future__ import annotations
 
+import json
 import os
 import time
 from dataclasses import dataclass, field
@@ -19,8 +21,8 @@ from typing import Optional, Sequence
 from .indexed_dataset import IndexedDataset
 from .similarity_analysis import CcoContext, DownsamplableCrossOccurrenceDataset, SimilarityAnalysis, default_context, encode_ids
 from .ur_query import Field, ItemQuery, ItemSetQuery, MixedQuery, UserQuery
-from .ur_model import (RankingParams, RankingType, extract_jvalue, property_json, ranking_window, rankings_for,
-                       rankings_params)
+from .ur_model import (RankingParams, RankingType, alias_actions, extract_jvalue, index_mapping, new_index_name, property_json,
+                       ranking_window, rankings_for, rankings_params)
 
 
 class DefaultURAlgoParams:
@@ -64,6 +66,7 @@ class URAlgorithmParams:
     expireDateName: Optional[str] = None
     dateName: Optional[str] = None
     indexName: Optional[str] = None
+    typeName: Optional[str] = None   # the Elasticsearch type of the documents (write_index)
 
     @staticmethod
     def from_engine_json(algo_params: dict) -> "URAlgorithmParams":
@@ -82,7 +85,8 @@ class URAlgorithmParams:
             returnSelf=algo_params.get("returnSelf"),
             fields=None if algo_params.get("fields") is None else [Field.from_json(f) for f in algo_params["fields"]],
             availableDateName=algo_params.get("availableDateName"), expireDateName=algo_params.get("expireDateName"),
-            dateName=algo_params.get("dateName"), indexName=algo_params.get("indexName"))
+            dateName=algo_params.get("dateName"), indexName=algo_params.get("indexName"),
+            typeName=algo_params.get("typeName"))
 
     def model_event_names(self) -> list[str]:
         """URAlgorithm.scala:230-235: the indicator names if given, else eventNames"""
@@ -438,3 +442,90 @@ def item_set_queries(sets, ap: URAlgorithmParams, query: Optional[ItemSetQuery] 
     fragments are ur_query.item_set_plan's; ValueError without a model event name (the set clause's field)."""
     ctx = ctx or default_context()
     return ctx.item_set_queries(sets, ap, query, _now(now_ms), header)
+
+
+class IndexWriteError(RuntimeError):
+    """write_index stopped before the alias swap: the alias still serves the old index; the new one is left in place"""
+
+    def __init__(self, message: str, new_index: str, result=None):
+        super().__init__(message)
+        self.new_index = new_index
+        self.result = result
+
+
+def _bulk_ids(body: bytes, docs) -> dict:
+    """{document index: decoded _id} of the given documents of a model index body"""
+    want, out = set(int(d) for d in docs), {}
+    at = 0
+    for d in range(max(want) + 1 if want else 0):
+        end = body.index(b"\n", at)
+        if d in want:
+            out[d] = json.loads(body[at:end].decode("utf-8", "surrogatepass"))["index"]["_id"]
+        at = body.index(b"\n", end + 1) + 1
+    return out
+
+
+def write_index(body: bytes, ap: URAlgorithmParams, request, now_ms: Optional[int] = None, max_docs: int = 1000,
+                max_bytes: int = 1 << 20, retries: int = 3, retry_wait_s: float = 10.0, ctx: CcoContext | None = None):
+    """URModel.save -> EsClient.hotSwap (URModel.scala:47-84, EsClient.scala:168-246, 257-362) for a model index body
+    (what calc_all_from_events or a calcPop wrote), over request(method, path, body bytes or None) -> (HTTP status, response
+    bytes), one request at a time:
+      1. HEAD /<new>, which must be 404 (new = <indexName>_<now_ms>);  2. PUT /<new> with index_mapping(esFields);
+      3. POST /<new>/_refresh;  4. POST /<new>/<typeName>/_bulk for every request of at most max_docs documents and
+      max_bytes bytes, each response read on the device (CcoContext.index_write);  5. up to `retries` rounds that send
+      again the documents rejected with 429, retry_wait_s apart (elasticsearch-hadoop's es.batch.write.retry.count /
+      .wait);  6. HEAD and GET /_alias/<indexName>, HEAD of its old index, POST /_aliases (add, remove_index), DELETE of
+      the old indexes.
+    An HTTP status other than 200 on steps 2-4, any item failure other than 429, or 429s left after the last round raise
+    IndexWriteError before step 6, naming the first documents' ids with Elasticsearch's error type and reason: the alias
+    keeps serving the old index and the new index is left in place.  -> (new index name, IndexWriteResult)."""
+    if not ap.indexName or not ap.typeName:
+        raise ValueError("write_index needs indexName and typeName in the algorithm params")
+    ctx = ctx or default_context()
+    body = bytes(body)
+    alias, type_name = ap.indexName, ap.typeName
+    new = new_index_name(alias, _now(now_ms))
+
+    def call(method: str, path: str, data: Optional[bytes] = None, ok=(200,)):
+        status, resp = request(method, path, data)
+        if ok is not None and status not in ok:
+            raise IndexWriteError(f"{method} {path} answered HTTP {status}: {bytes(resp or b'')[:500]!r}", new)
+        return status, resp
+
+    with ctx.index_write(body, max_docs, max_bytes) as w:
+        mapping = index_mapping(w.fields(), ap, type_name)
+        call("HEAD", f"/{new}", ok=(404,))
+        call("PUT", f"/{new}", mapping)
+        call("POST", f"/{new}/_refresh")
+        bulk = f"/{new}/{type_name}/_bulk"
+        for q, part in enumerate(w.requests()):
+            w.response(q, call("POST", bulk, part)[1])
+        for _ in range(retries):
+            first, parts = w.retry()
+            if not parts:
+                break
+            time.sleep(retry_wait_s)
+            for k, (_, part) in enumerate(parts):
+                w.response(first + k, call("POST", bulk, part)[1])
+        result = w.finish()
+    if result.errors:
+        shown = result.errors[:5]
+        ids = _bulk_ids(body, [d for d, _, _ in shown])
+        lines = "; ".join(f"{ids[d]!r}: {t or '-'}: {r or '-'}" for d, t, r in shown)
+        raise IndexWriteError(f"{len(result.errors)} documents were not written to {new} ({result.n_rejected} still rejected "
+                              f"with 429, {result.n_failed} failed), the alias {alias} is unchanged: {lines}", new, result)
+    old_set, old = [], None
+    if call("HEAD", f"/_alias/{alias}", ok=None)[0] == 200:
+        old_set = list(json.loads(bytes(call("GET", f"/_alias/{alias}")[1]).decode("utf-8")).keys())
+        if old_set and call("HEAD", f"/{old_set[0]}", ok=None)[0] == 200:
+            old = old_set[0]
+        else:
+            old_set = []
+    call("POST", "/_aliases", alias_actions(alias, new, old))
+    for name in old_set:   # deleteIndex: HEAD, then DELETE when it still exists
+        st = call("HEAD", f"/{name}", ok=None)[0]
+        if st == 200:
+            call("DELETE", f"/{name}", ok=None)
+        elif st != 404:
+            raise IndexWriteError(f"HEAD /{name} answered HTTP {st}", new, result)
+    return new, result

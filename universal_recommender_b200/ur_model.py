@@ -657,3 +657,151 @@ def index_from_pages(pages) -> tuple:
         if p == 0:
             total = t
     return bytes(body), n_docs, total
+
+
+# ---- the index written into Elasticsearch -----------------------------------------------------------------------------------
+# URModel.save (URModel.scala:47-84) hands EsClient.hotSwap (EsClient.scala:257-362) the documents and esFields;
+# createIndex (EsClient.scala:168-246) PUTs the mapping, saveToEs sends the _bulk requests, _aliases swaps the alias.  The
+# bodies below restate the Scala string construction; index_fields, bulk_requests and bulk_item_statuses are the host mirrors
+# of cco_index_write_*, written over json.
+def index_mapping(fields: Sequence[str], ap, type_name: str) -> bytes:
+    """the mapping createIndex PUTs for the fields (each as IndexWrite.fields / index_fields spell it: escaped), typed by
+    getMappings (URAlgorithm.scala:955-967): its Map `++` order lets the date names override the event names and those
+    the ranking names; every other field is a keyword.  The tail's unused "last" property closes the object without a
+    trailing comma, so a field really named "last" is written twice, as the reference writes it."""
+    names = ap.model_event_names()
+    dates = list(dict.fromkeys(d for d in (ap.dateName, ap.availableDateName, ap.expireDateName) if d is not None))
+    types = {**{rp.field_name(): "float" for rp in rankings_params(ap.rankings, names)}, **{e: "keyword" for e in names},
+             **{d: "date" for d in dates}}
+    types = {json_string(k)[1:-1]: v for k, v in types.items()}
+    out = '{ "mappings": {    "%s": {      "properties": {            ' % type_name
+    for f in fields:
+        out += '"%s"    : {      "type": "%s"    },            ' % (f, types.get(f, "keyword"))
+    out += '    "last": {      "type": "keyword"    }}}}}            '
+    return out.encode("utf-8", "surrogatepass")
+
+
+def alias_actions(alias: str, new_index: str, old_index: Optional[str] = None) -> bytes:
+    """hotSwap's _aliases body: add the alias to the new index and, when the alias names an existing index, remove that
+    index (remove_index)"""
+    remove = ',{ "remove_index": { "index": "%s"}}' % old_index if old_index is not None else ""
+    return ('{    "actions" : [        { "add":  { "index": "%s", "alias": "%s" } }        %s    ]}      '
+            % (new_index, alias, remove)).encode("utf-8", "surrogatepass")
+
+
+def new_index_name(index_name: str, now_ms: int) -> str:
+    """hotSwap's new index: the alias, '_', the wall clock in milliseconds"""
+    return f"{index_name}_{now_ms}"
+
+
+class _Obj(list):
+    """a JSON object as its (name, value) pairs in order, repeated names kept"""
+
+
+def _pairs(text: bytes):
+    return json.loads(text.decode("utf-8", "surrogatepass"), object_pairs_hook=_Obj)
+
+
+def bulk_documents(body: bytes) -> list:
+    """the documents of a model index body -> [(decoded _id, first byte, end byte, [(decoded name, value)])]"""
+    body = bytes(body)
+    if body and not body.endswith(b"\n"):
+        raise ValueError("the body does not end in a newline")
+    docs, at = [], 0
+    lines = body.split(b"\n")[:-1] if body else []
+    if len(lines) % 2:
+        raise ValueError(f"the body has {len(lines)} lines: lines come in (action, source) pairs")
+    for d in range(0, len(lines), 2):
+        action, source = _pairs(lines[d]), _pairs(lines[d + 1])
+        end = at + len(lines[d]) + len(lines[d + 1]) + 2
+        if not isinstance(action, _Obj) or not isinstance(source, _Obj):
+            raise ValueError(f"document {d // 2}: a line is not a JSON object")
+        index = [v for k, v in action if k == "index"]
+        ids = [v for k, v in index[0] if k == "_id"] if index and isinstance(index[0], _Obj) else []
+        if not ids or not isinstance(ids[0], str):
+            raise ValueError(f"document {d // 2}: the action line is not {{\"index\":{{...}}}} with a string \"_id\" member")
+        docs.append((ids[0], at, end, source))
+        at = end
+    return docs
+
+
+def index_fields(body: bytes) -> list:
+    """esFields (URModel.scala:78) as cco_index_write_fields gives them: the distinct decoded member names of the document
+    lines in first-appearance order, escaped as format_model escapes names; "id", which save adds to every document, last
+    when no document line has it"""
+    docs = bulk_documents(body)
+    seen = dict.fromkeys(name for _, _, _, members in docs for name, _ in members)
+    if docs and "id" not in seen:
+        seen["id"] = None
+    return [json_string(n)[1:-1] for n in seen]
+
+
+def bulk_requests(body: bytes, max_docs: int, max_bytes: int) -> tuple:
+    """elasticsearch-hadoop's batching of the documents into _bulk requests of at most max_docs documents and max_bytes
+    bytes, a larger document alone -> (doc_begin, byte_begin), each with one entry past the last request"""
+    docs = bulk_documents(body)
+    doc_begin, byte_begin, n, size = [0], [0], 0, 0
+    for d, (_, b, e, _) in enumerate(docs):
+        if n and (n == max_docs or size + (e - b) > max_bytes):
+            doc_begin.append(d)
+            byte_begin.append(b)
+            n = size = 0
+        n += 1
+        size += e - b
+    if n:
+        doc_begin.append(len(docs))
+        byte_begin.append(docs[-1][2])
+    return doc_begin, byte_begin
+
+
+def bulk_item_statuses(response: bytes, ids: Sequence[str]) -> list:
+    """one _bulk response for the documents of `ids` -> [(status, error.type, error.reason)] per item ("" where the item
+    has no such string).  ValueError for the errors cco_index_write_response reports."""
+    top = _pairs(bytes(response))
+    if not isinstance(top, _Obj):
+        raise ValueError("the top level is not an object")
+    if any(k == "error" for k, _ in top):
+        status = _first_pair(top, "status")
+        ok = isinstance(status, int) and not isinstance(status, bool) and -2 ** 31 <= status < 2 ** 31
+        raise ValueError("Elasticsearch returned an error" + (f" (status {status})" if ok else ""))
+    items = _first_pair(top, "items", None)
+    if not isinstance(items, list) or isinstance(items, _Obj):
+        raise ValueError('the response has no "items" array')
+    if any(not isinstance(x, _Obj) for x in items):
+        raise ValueError("an items element is not an object")
+    if len(items) != len(ids):
+        raise ValueError(f"{len(items)} items for {len(ids)} documents")
+    out = []
+    for i, item in enumerate(items):
+        if len(item) != 1 or item[0][0] != "index" or not isinstance(item[0][1], _Obj):
+            raise ValueError(f"item {i}: the item is not {{\"index\":{{...}}}}")
+        members = item[0][1]
+        got_id = [v for k, v in members if k == "_id"]
+        status = [v for k, v in members if k == "status"]
+        if not got_id or any(not isinstance(v, str) for v in got_id):
+            raise ValueError(f"item {i}: the item has no string _id")
+        if len(got_id) > 1:
+            raise ValueError(f"item {i}: a repeated _id")
+        if not status:
+            raise ValueError(f"item {i}: the item has no status")
+        if len(status) > 1:
+            raise ValueError(f"item {i}: a repeated status")
+        if not (isinstance(status[0], int) and not isinstance(status[0], bool) and -2 ** 31 <= status[0] < 2 ** 31):
+            raise ValueError(f"item {i}: the status is not a 32-bit integer")
+        if got_id[0] != ids[i]:
+            raise ValueError(f"item {i}: the item's _id is not the document's _id")
+        err = _first_pair(members, "error")
+        kind = reason = ""
+        if isinstance(err, _Obj):
+            t, r = _first_pair(err, "type"), _first_pair(err, "reason")
+            kind = t if isinstance(t, str) else ""
+            reason = r if isinstance(r, str) else ""
+        out.append((status[0], kind, reason))
+    return out
+
+
+def _first_pair(pairs: list, name: str, default=None):
+    for k, v in pairs:
+        if k == name:
+            return v
+    return default
