@@ -75,7 +75,9 @@ typedef struct {
  *    32 bits.  count <= min(largest primary-item marginal, largest column marginal of this event type) must fit next to
  *    the column id: bitlen(n_cols + 1) + bitlen(max count) <= 32.  After the reference's default downsampling (500) every
  *    marginal is <= ~560, i.e. 10 bits: item spaces up to 4M columns.  Without downsampling (m huge) a 1M-column space
- *    allows counts < 4096.
+ *    allows counts < 4096.  Without CCO_FLAG_KEY_RANGES an indicator past this bound is refused (CCO_E_UNSUPPORTED,
+ *    the remedy named: lower maxItemsPerUser / maxEventsPerEventType); with it, the indicator is trained in column key
+ *    ranges that each fit the word, bit for bit the result an unlimited word would give (see the flag).
  */
 
 /* cco_train flags */
@@ -95,7 +97,17 @@ enum {
    * drops the LLR values, nothing reads k11): NO_COUNT skips the count array (cco_result_matrix returns NULL for it),
    * NO_LLR skips the LLR array too -- 80 instead of 321 MB come back per train at C3. */
   CCO_FLAG_RESULT_NO_COUNT = 16,
-  CCO_FLAG_RESULT_NO_LLR = 32
+  CCO_FLAG_RESULT_NO_LLR = 32,
+  /* An indicator whose counts do not fit the packed accumulator word ("Limits") is trained in key ranges instead of
+   * being refused: the columns, numbered by (colB ascending, column id ascending), are cut into the fewest contiguous
+   * ranges whose counts fit, each range is scored on its own and the ranges' top-k lists are merged on the device.  The
+   * result is bit for bit the unsplit one (LLR depends only on k11, colA, colB and N; ties keep the column-id order).
+   * A flag, not automatic: the refusal is a documented contract, and without downsampling the number of ranges has no
+   * useful bound (counts of 2^20 leave 12 key bits per range, each range a pass over B'), so the caller accepts that
+   * cost.  Indicators whose word fits run exactly as without the flag.  Honoured by cco_train, cco_train_dataset,
+   * cco_cooccurrences_idss, group contexts and multi-process ranks (every rank cuts the same plan).
+   * llr_evaluated may differ from the unsplit run: the key cut and the dominance filter work per range. */
+  CCO_FLAG_KEY_RANGES = 64
 };
 
 /*
@@ -272,6 +284,8 @@ int cco_result_matrix(const cco_result_t *r, int32_t i, int64_t *n_rows, int32_t
                       const int64_t **row_ptr, const int32_t **col_idx, const double **llr,
                       const int32_t **count);
 int cco_result_stats(const cco_result_t *r, cco_stats_t *out);
+/* the number of key ranges indicator i ran in (CCO_FLAG_KEY_RANGES): 1 when its counts fit the packed word */
+int cco_result_key_ranges(const cco_result_t *r, int32_t i, int32_t *n_ranges);
 int cco_result_free(cco_result_t *r);
 
 /*
@@ -972,6 +986,10 @@ int cco_index_write_free(cco_index_write_t *h);
  */
 int cco_debug_cooccurrence(cco_ctx_t *ctx, const cco_csr_t *a, const cco_csr_t *b, int64_t **row_ptr,
                            int32_t **col_idx, int32_t **count);
+/* Debug entry (tests only): cap every key range (CCO_FLAG_KEY_RANGES) of this context's trains and debug entries at
+ * max_keys keys, even where the packed word fits and without the flag, so that every row path can be run split; 0 = off.
+ * On a group context it applies to every GPU of the group. */
+int cco_debug_key_range_cap(cco_ctx_t *ctx, int32_t max_keys);
 /* Debug/parity entry (tests only): sampleDownAndBinarize of one matrix on the device. */
 int cco_debug_downsample(cco_ctx_t *ctx, const cco_csr_t *m, int32_t max_interactions, int32_t seed,
                          uint32_t flags, int64_t **row_ptr, int32_t **col_idx, int32_t *raw_col_counts,

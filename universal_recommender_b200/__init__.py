@@ -30,7 +30,7 @@ Host-side mirror of the reference interface for this path:
   ur_model                                <- propertiesRDD, getRanksRDD, groupAll (URAlgorithm.scala:351-369, 537-560;
                                              URModel.scala:57-140): the host mirror of the model documents
 """
-from ._native import (CcoError, CcoInvalidArgument, FLAG_ASSUME_CANONICAL, FLAG_ENTROPY_VARARGS, FLAG_RESULT_NO_COUNT,
+from ._native import (CcoError, CcoInvalidArgument, FLAG_ASSUME_CANONICAL, FLAG_ENTROPY_VARARGS, FLAG_KEY_RANGES, FLAG_RESULT_NO_COUNT,
                       FLAG_RESULT_NO_LLR, FLAG_ROWRATE_INTDIV, LIB_PATH)
 from .events import DataSourceParams, EventWindow
 from .indexed_dataset import BiDictionary, IndexedDataset
@@ -49,5 +49,5 @@ __all__ = [
     "EventLog", "RankingParams", "URAlgorithmParams", "calc_all", "calc_all_from_events", "calc_all_on_device", "calc_pop_from_events",
     "batchpredict_output", "calc_pop_on_device", "item_queries", "item_set_queries", "mixed_queries_from_events", "predictions_from_responses", "queries_from_file", "SearchResults", "IndexPages", "index_from_pages", "IndexWrite", "IndexWriteResult", "IndexWriteError", "write_index", "user_queries_from_events", "ItemQuery", "ItemSetQuery", "MixedQuery", "UserQuery", "decode_ids", "default_context", "encode_ids", "prepare", "prepare_on_device",
     "FLAG_ASSUME_CANONICAL",
-    "FLAG_ENTROPY_VARARGS", "FLAG_ROWRATE_INTDIV", "FLAG_RESULT_NO_COUNT", "FLAG_RESULT_NO_LLR", "LIB_PATH",
+    "FLAG_ENTROPY_VARARGS", "FLAG_KEY_RANGES", "FLAG_ROWRATE_INTDIV", "FLAG_RESULT_NO_COUNT", "FLAG_RESULT_NO_LLR", "LIB_PATH",
 ]

@@ -18,6 +18,7 @@ FLAG_ASSUME_CANONICAL = 4
 FLAG_RESULT_ON_DEVICE = 8
 FLAG_RESULT_NO_COUNT = 16
 FLAG_RESULT_NO_LLR = 32
+FLAG_KEY_RANGES = 64
 MAX_TOP_K = 2048
 MAX_RANKINGS = 8
 POP_MODES = {"popular": 0, "trending": 1, "hot": 2, "random": 3}   # random: cco_format_model only
@@ -191,8 +192,8 @@ EXPORTS = [
     "cco_format_model", "cco_rerank_model", "cco_event_log_read", "cco_event_log_info", "cco_event_log_ingest",
     "cco_format_model_log", "cco_rerank_model_log", "cco_event_log_free", "cco_event_log_begin", "cco_event_log_append",
     "cco_event_log_finish", "cco_event_log_begin_window", "cco_event_log_window_stats",
-    "cco_event_log_begin_ex", "cco_event_log_user_queries", "cco_item_queries", "cco_item_set_queries", "cco_mixed_queries", "cco_query_file_read", "cco_query_file_templates", "cco_query_file_queries", "cco_query_file_free", "cco_search_results_begin", "cco_search_results_append", "cco_search_results_finish", "cco_search_results_free", "cco_index_pages_begin", "cco_index_pages_append", "cco_index_pages_finish", "cco_index_pages_free", "cco_index_write_begin", "cco_index_write_fields", "cco_index_write_requests", "cco_index_write_response", "cco_index_write_retry", "cco_index_write_finish", "cco_index_write_free", "cco_result_num_matrices", "cco_result_row_range", "cco_result_matrix", "cco_result_stats", "cco_result_free",
-    "cco_debug_cooccurrence", "cco_debug_downsample", "cco_debug_downsample_block", "cco_debug_llr", "cco_debug_string_ids", "cco_debug_rank_text", "cco_free",
+    "cco_event_log_begin_ex", "cco_event_log_user_queries", "cco_item_queries", "cco_item_set_queries", "cco_mixed_queries", "cco_query_file_read", "cco_query_file_templates", "cco_query_file_queries", "cco_query_file_free", "cco_search_results_begin", "cco_search_results_append", "cco_search_results_finish", "cco_search_results_free", "cco_index_pages_begin", "cco_index_pages_append", "cco_index_pages_finish", "cco_index_pages_free", "cco_index_write_begin", "cco_index_write_fields", "cco_index_write_requests", "cco_index_write_response", "cco_index_write_retry", "cco_index_write_finish", "cco_index_write_free", "cco_result_num_matrices", "cco_result_row_range", "cco_result_matrix", "cco_result_stats", "cco_result_key_ranges", "cco_result_free",
+    "cco_debug_cooccurrence", "cco_debug_key_range_cap", "cco_debug_downsample", "cco_debug_downsample_block", "cco_debug_llr", "cco_debug_string_ids", "cco_debug_rank_text", "cco_free",
 ]
 
 _lib = None
@@ -293,8 +294,10 @@ def lib():
     L.cco_result_matrix.argtypes = [C.c_void_p, C.c_int32, p(C.c_int64), p(C.c_int32), p(p(C.c_int64)),
                                     p(p(C.c_int32)), p(p(C.c_double)), p(p(C.c_int32))]
     L.cco_result_stats.argtypes = [C.c_void_p, p(StatsT)]
+    L.cco_result_key_ranges.argtypes = [C.c_void_p, C.c_int32, p(C.c_int32)]
     L.cco_result_free.argtypes = [C.c_void_p]
     L.cco_debug_cooccurrence.argtypes = [C.c_void_p, p(CsrT), p(CsrT), p(p(C.c_int64)), p(p(C.c_int32)), p(p(C.c_int32))]
+    L.cco_debug_key_range_cap.argtypes = [C.c_void_p, C.c_int32]
     L.cco_debug_downsample.argtypes = [C.c_void_p, p(CsrT), C.c_int32, C.c_int32, C.c_uint32, p(p(C.c_int64)),
                                        p(p(C.c_int32)), p(C.c_int32), p(C.c_int32)]
     L.cco_debug_downsample_block.argtypes = [C.c_void_p, p(CsrT), C.c_int64, C.c_int64, p(C.c_int32), C.c_int32, C.c_int32, C.c_uint32,

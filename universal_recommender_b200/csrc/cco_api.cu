@@ -158,6 +158,7 @@ struct cco_ctx {
   std::mutex mu;
   ncclComm_t comm = nullptr;
   int launches = 0;
+  int32_t key_range_cap = 0;   // cco_debug_key_range_cap: at most this many keys per key range (0 = off)
   // mailbox for small device -> host results (mapped pinned memory written by k_mail_bytes).  Records are closed into
   // groups; a group is complete when its event has fired, so the host can wait for indicator i's numbers while the GPU
   // already runs indicator i + 1 (no stream-wide synchronisation).
@@ -227,6 +228,7 @@ struct ResultMat {
   int32_t *col = nullptr;
   double *llr = nullptr;
   int32_t *cnt = nullptr;
+  int32_t key_ranges = 1;   // key ranges the indicator ran in
 };
 // A dataset holds, per event type, the block of user rows this context works on: the whole matrix on a single GPU,
 // this rank's user block [row_base, row_base + n_local) in a multi-GPU job (each GPU uploads 1/N of the rows).
@@ -905,6 +907,132 @@ static bool cut_exact(long long n_users, int32_t max_marg_a, int32_t max_marg_b)
   return g > 2.0 * llr_error_bound(n_users);
 }
 
+// ---- bins of one indicator (or of one key range of it) -----------------------------------------------------------------
+struct BinPlan {
+  std::vector<BinCfg> cfgs;
+  int32_t *d_bounds = nullptr;   // [bins + 3] row-list bounds, filled on the device by k_bin_bounds (allocated if null)
+};
+// the packed (key << count_bits | count) word for keys 0 .. n_keys - 1 and counts up to k11_max: false = it does not fit
+static bool packed_bits(long long n_keys, long long k11_max, int *key_bits, int *count_bits) {
+  int kb = 1;
+  while (((1LL << kb) - 1) <= n_keys) ++kb;  // keys <= 2^kb - 2
+  *key_bits = kb;
+  *count_bits = 32 - kb;
+  return *count_bits >= 1 && k11_max < (1LL << *count_bits);
+}
+static int plan_bins(cco_ctx *c, Arena &ar, int32_t n_items_a, int32_t n_cols_b, int count_bits, int32_t max_marg_a,
+                     int32_t max_marg_b, long long n_users, int k_eff, bool emit_all, const uint32_t *sorted_work, cudaStream_t ss,
+                     BinPlan *bp) {
+  const bool warp_ok = k_eff + 32 <= 256;  // warp-owned rows keep a 256-entry candidate buffer
+  // Work bins, largest rows first.  {threads that own a row, table words, largest row work w the bin takes}.
+  // Bin 0 is the multi-pass bin (same config as bin 1).  Rows up to 1024 products are WARP-owned: no CTA barrier
+  // anywhere in their count / compact / score / select pipeline; larger rows need the table and the parallelism of a CTA.
+  struct BinSpec { int group, slots; uint32_t max_w; };
+  std::vector<BinSpec> spec = {{1024, 1 << 20, 0xffffffffu}, {1024, 1 << 20, 0xffffffffu}, {512, 16384, 8192u}, {256, 8192, 4096u}};
+  if (warp_ok) {
+    // rows of 1025..2048 products: a 128-thread CTA shares one 4096-word table -- a warp-owned 4096-word table leaves
+    // too few warps per SM; up to 1024 products rows are warp-owned
+    spec.push_back({128, 4096, 2048u});
+    spec.push_back({32, 2048, 1024u});
+    spec.push_back({32, 1024, 512u});
+    spec.push_back({32, 512, 256u});
+  } else {
+    spec.push_back({128, 4096, 2048u});
+  }
+  const int kBins = (int)spec.size();
+  std::vector<BinCfg> &cfgs = bp->cfgs;
+  cfgs.resize(kBins);
+  for (int b = 0; b < kBins; ++b) cfgs[b] = make_cfg(c, spec[b].group, spec[b].slots, k_eff, n_cols_b);
+  // thresholds on w, descending: bin b takes rows with h_thr[b-1] >= w > h_thr[b]; a hashed table also needs w <= cap
+  std::vector<uint32_t> h_thr(kBins);
+  for (int b = 0; b < kBins; ++b) {
+    const BinCfg &f = cfgs[std::min(b + 1, kBins - 1)];   // h_thr[b] = upper limit of bin b+1
+    uint32_t lim = b + 1 < kBins ? spec[b + 1].max_w : 0u;
+    if (b + 1 < kBins && !f.dense) lim = std::min<uint32_t>(lim, (uint32_t)f.cap);
+    h_thr[b] = lim;
+    if (b > 0) h_thr[b] = std::min(h_thr[b], h_thr[b - 1]);
+  }
+  // bitmap and sorted rows: the k11 = 1 cells are cut by key, so every row must be keyed (2 rowA colB < N for the largest of both)
+  // and the cut exact
+  const bool bitmap_ok = !emit_all && cut_exact(n_users, max_marg_a, max_marg_b) &&
+                         2ull * (unsigned long long)std::max(max_marg_a, 0) * (unsigned long long)std::max(max_marg_b, 0) <
+                             (unsigned long long)n_users;
+  for (int b = 1; b < kBins && bitmap_ok; ++b) {
+    use_bitmap(cfgs[b], h_thr[b - 1], k_eff, n_cols_b);
+    use_sorted(cfgs[b], h_thr[b - 1], count_bits);
+  }
+  if (!bp->d_bounds) CKR(ar.alloc(&bp->d_bounds, kBins + 3));   // key ranges reuse one across ranges
+  BinThresholds bt;
+  memset(&bt, 0, sizeof bt);
+  for (int b = 0; b < kBins; ++b) bt.t[b] = h_thr[b];
+  k_bin_bounds<<<1, 32, 0, ss>>>(n_items_a, sorted_work, kBins, bt, bp->d_bounds);
+  c->launches++;
+  return CCO_OK;
+}
+// the bins touch disjoint rows: run them concurrently (tails of one bin overlap the bulk of another); s joins them all
+static int launch_bins(cco_ctx *c, const RowArgs &a, BinPlan &bp, cudaStream_t s) {
+  std::vector<BinCfg> &cfgs = bp.cfgs;
+  CK(cudaEventRecord(c->bin_ev[8], s));
+  for (int b = 0; b < (int)cfgs.size(); ++b) {
+    if (b == 0 && cfgs[1].dense) continue;                 // dense L takes every large row in bin 1
+    RowArgs ab = a;
+    ab.bin_bounds = bp.d_bounds;
+    ab.bin = b;
+    ab.slots = cfgs[b].slots;
+    ab.cap = cfgs[b].cap;
+    ab.tsize_x16 = 32;
+    ab.cbuf = cfgs[b].cbuf;
+    ab.caux = cfgs[b].caux;
+    ab.keep_max = cfgs[b].keep_max;
+    ab.final_max = cfgs[b].final_max;
+    ab.group_smem_bytes = (int32_t)cfgs[b].region;
+    ab.bm_words = cfgs[b].bm_words;
+    CK(cudaStreamWaitEvent(c->bin_stream[b], c->bin_ev[8], 0));
+    CKR(launch_rows(c, ab, cfgs[b], c->bin_stream[b]));
+    CK(cudaEventRecord(c->bin_ev[b], c->bin_stream[b]));
+    CK(cudaStreamWaitEvent(s, c->bin_ev[b], 0));
+  }
+  return CCO_OK;
+}
+
+// (n_cols_b - 1) >> key_shift < kCutBins: the first level of the key cut
+static int key_shift_for(int32_t n_cols_b) {
+  int sh = 0;
+  while (((long long)std::max(n_cols_b - 1, 0) >> sh) >= kCutBins) ++sh;
+  return sh;
+}
+
+// ---- key ranges (DESIGN.md 3.1 "key ranges") -----------------------------------------------------------------------------
+// Keys number B' columns by (colB ascending, column id ascending), so colB never decreases with the key and a key range
+// [k0, k1) has its largest colB at k1 - 1.  The range's counts fit the packed word when bitlen(k1 - k0 + 1) +
+// bitlen(min(max rowA, colB(k1 - 1))) <= 32 (packed_bits).  Any sub-range of a range that fits fits too, so cutting
+// greedily from key 0 upward, each range as long as it fits (and at most max_keys keys when max_keys > 0), gives the
+// fewest ranges.  first_key_of_cb[c] (c in [0, max_marg_b + 1]) = first key whose colB >= c, as k_col_order builds it.
+// False when a single key's counts do not fit.
+struct KeyRange { int32_t k0, k1, max_marg; };
+static bool plan_key_ranges(const int32_t *first_key_of_cb, int32_t max_marg_b, int32_t n_keys, int32_t max_marg_a,
+                            int32_t max_keys, std::vector<KeyRange> *plan) {
+  const int32_t *fk_end = first_key_of_cb + (size_t)max_marg_b + 2;
+  auto marg = [&](int32_t k) { return (int32_t)(std::upper_bound(first_key_of_cb, fk_end, k) - first_key_of_cb) - 1; };
+  auto fits = [&](int32_t k0, int32_t k1) {
+    int kb, cb;
+    return packed_bits((long long)k1 - k0, std::min<long long>(max_marg_a, marg(k1 - 1)), &kb, &cb);
+  };
+  plan->clear();
+  for (int32_t k0 = 0; k0 < n_keys;) {
+    const int32_t top = max_keys > 0 ? (int32_t)std::min<long long>(n_keys, (long long)k0 + max_keys) : n_keys;
+    if (!fits(k0, k0 + 1)) return false;
+    int32_t lo = k0 + 1, hi = top;   // the largest k1 in [lo, hi] that fits
+    while (lo < hi) {
+      const int32_t mid = lo + (hi - lo + 1) / 2;
+      if (fits(k0, mid)) lo = mid; else hi = mid - 1;
+    }
+    plan->push_back({k0, lo, marg(lo - 1)});
+    k0 = lo;
+  }
+  return true;
+}
+
 // ---- one indicator = rows [lo, hi) of A'^T B' on this rank ---------------------------------------------------------------
 // enqueue_indicator puts everything of one indicator on the stream without a single host round trip (the rank partition,
 // the bin bounds and the packed sizes stay on the device); finish_indicator waits for that indicator's mailbox record
@@ -917,6 +1045,7 @@ struct IndicatorState {
   int32_t *p_col = nullptr, *p_cnt = nullptr;
   double *p_llr = nullptr;
   int32_t n_items_a = 0, n_cols_b = 0;
+  int n_ranges = 1;                            // key ranges the indicator ran in
   bool emit_all = false;
 };
 
@@ -978,65 +1107,25 @@ static int enqueue_indicator(cco_ctx *c, Arena &ar, const uint32_t *at_ptr, cons
     CK(cub::DeviceRadixSort::SortPairsDescending(tmp, sort_tb, masked, sorted_work, ids, rows_sorted, n_items_a, 0, 32, ss));
     ar.release(tmp);
   }
-  // 2. bins -----------------------------------------------------------------------------------------
+  // 2. packed word and bins -------------------------------------------------------------------------
   const int k_eff = emit_all ? 1 : prm.top_k;
-  const bool warp_ok = k_eff + 32 <= 256;  // warp-owned rows keep a 256-entry candidate buffer
-  // Work bins, largest rows first.  {threads that own a row, table words, largest row work w the bin takes}.
-  // Bin 0 is the multi-pass bin (same config as bin 1).  Rows up to 1024 products are WARP-owned: no CTA barrier
-  // anywhere in their count / compact / score / select pipeline; larger rows need the table and the parallelism of a CTA.
-  struct BinSpec { int group, slots; uint32_t max_w; };
-  std::vector<BinSpec> spec = {{1024, 1 << 20, 0xffffffffu}, {1024, 1 << 20, 0xffffffffu}, {512, 16384, 8192u}, {256, 8192, 4096u}};
-  if (warp_ok) {
-    // rows of 1025..2048 products: a 128-thread CTA shares one 4096-word table -- a warp-owned 4096-word table leaves
-    // too few warps per SM; up to 1024 products rows are warp-owned
-    spec.push_back({128, 4096, 2048u});
-    spec.push_back({32, 2048, 1024u});
-    spec.push_back({32, 1024, 512u});
-    spec.push_back({32, 512, 256u});
-  } else {
-    spec.push_back({128, 4096, 2048u});
-  }
-  const int kBins = (int)spec.size();
-  std::vector<BinCfg> cfgs(kBins);
-  for (int b = 0; b < kBins; ++b) cfgs[b] = make_cfg(c, spec[b].group, spec[b].slots, k_eff, n_cols_b);
-  BinCfg &cfgL = cfgs[1];
-  // packed word: key bits must leave room for the largest possible count
-  int key_bits = 1;
-  while (((1LL << key_bits) - 1) <= (long long)n_cols_b) ++key_bits;  // keys <= 2^kb - 2
-  int count_bits = 32 - key_bits;
   // a co-occurrence count is bounded by both marginals: k11 <= min(rowA, colB) <= min(max rowA, max colB).  With the
   // reference's default downsampling (m = 500) that is ~560, i.e. 10 count bits next to 22 key bits (4M columns).
+  int key_bits, count_bits;
   const long long k11_max = std::min<long long>(max_marg_a, max_marg_b);
-  if (count_bits < 1 || k11_max >= (1LL << count_bits))
+  const bool fits = packed_bits(n_cols_b, k11_max, &key_bits, &count_bits);
+  // key ranges: the counts do not fit and the caller accepts the ranges' cost, or the debug cap forces them
+  const bool split = n_cols_b > 0 && (c->key_range_cap > 0 || (!fits && (flags & CCO_FLAG_KEY_RANGES)));
+  if (!fits && !split)
     return set_error(CCO_E_UNSUPPORTED,
                      "co-occurrence counts up to %lld over %d columns do not fit the packed 32-bit accumulator word "
-                     "(key %d bits + count %d bits): lower maxItemsPerUser/maxEventsPerEventType for this event type "
-                     "(\"Limits\" in include/cco_b200.h)", k11_max, n_cols_b, key_bits, count_bits);
-  // thresholds on w, descending: bin b takes rows with h_thr[b-1] >= w > h_thr[b]; a hashed table also needs w <= cap
-  std::vector<uint32_t> h_thr(kBins);
-  for (int b = 0; b < kBins; ++b) {
-    const BinCfg &f = cfgs[std::min(b + 1, kBins - 1)];   // h_thr[b] = upper limit of bin b+1
-    uint32_t lim = b + 1 < kBins ? spec[b + 1].max_w : 0u;
-    if (b + 1 < kBins && !f.dense) lim = std::min<uint32_t>(lim, (uint32_t)f.cap);
-    h_thr[b] = lim;
-    if (b > 0) h_thr[b] = std::min(h_thr[b], h_thr[b - 1]);
-  }
-  // bitmap and sorted rows: the k11 = 1 cells are cut by key, so every row must be keyed (2 rowA colB < N for the largest of both)
-  // and the cut exact
-  const bool bitmap_ok = !emit_all && cut_exact(n_users, max_marg_a, max_marg_b) &&
-                         2ull * (unsigned long long)std::max(max_marg_a, 0) * (unsigned long long)std::max(max_marg_b, 0) <
-                             (unsigned long long)n_users;
-  for (int b = 1; b < kBins && bitmap_ok; ++b) {
-    use_bitmap(cfgs[b], h_thr[b - 1], k_eff, n_cols_b);
-    use_sorted(cfgs[b], h_thr[b - 1], count_bits);
-  }
-  int32_t *d_bounds;
-  CKR(ar.alloc(&d_bounds, kBins + 3));
-  BinThresholds bt;
-  memset(&bt, 0, sizeof bt);
-  for (int b = 0; b < kBins; ++b) bt.t[b] = h_thr[b];
-  k_bin_bounds<<<1, 32, 0, ss>>>(n_items_a, sorted_work, kBins, bt, d_bounds);
-  c->launches++;
+                     "(key %d bits + count %d bits): lower maxItemsPerUser/maxEventsPerEventType for this event type, "
+                     "or train it in key ranges with CCO_FLAG_KEY_RANGES (\"Limits\" in include/cco_b200.h)",
+                     k11_max, n_cols_b, key_bits, count_bits);
+  st->n_ranges = 1;
+  BinPlan bins;
+  if (!split)
+    CKR(plan_bins(c, ar, n_items_a, n_cols_b, count_bits, max_marg_a, max_marg_b, n_users, k_eff, emit_all, sorted_work, ss, &bins));
   // column order of B' (DESIGN.md 3.1, step 3): key = rank under (colB ascending, column id ascending), from a stable
   // sort of the final post-sample marginals (identical on every rank).  B' is relabelled to keys IN PLACE: every B' is
   // this train's own sampled copy, and A' (the B' of the self indicator) has already been transposed.  Like the
@@ -1104,13 +1193,11 @@ static int enqueue_indicator(cco_ctx *c, Arena &ar, const uint32_t *at_ptr, cons
   a.marg_b = marg_key;
   a.key_of_col = key_of_col;
   a.first_key_of_cb = first_key_of_cb;
-  a.key_shift = 0;
-  while (((long long)std::max(n_cols_b - 1, 0) >> a.key_shift) >= kCutBins) ++a.key_shift;
+  a.key_shift = key_shift_for(n_cols_b);
   a.max_marg_b = max_marg_b;
   a.col_terms = col_terms;
   a.rows_sorted = rows_sorted;
   a.row_work = row_work;
-  a.bin_bounds = d_bounds;
   a.n_cols_b = n_cols_b;
   a.n_users = n_users;
   a.self = self ? 1 : 0;
@@ -1130,27 +1217,98 @@ static int enqueue_indicator(cco_ctx *c, Arena &ar, const uint32_t *at_ptr, cons
   a.stat_evaluated = d_distinct + 1;
   a.err_flag = d_err;
   a.emit_all = emit_all ? 1 : 0;
+  a.key_base = 0;
   if (ev_begin) CK(cudaEventRecord(ev_begin, s));
-  if (n_items_a > 0) {
-    // the bins touch disjoint rows: run them concurrently (tails of one bin overlap the bulk of another)
-    CK(cudaEventRecord(c->bin_ev[8], s));
-    for (int b = 0; b < kBins; ++b) {
-      if (b == 0 && cfgL.dense) continue;                 // dense L takes every large row in bin 1
-      RowArgs ab = a;
-      ab.bin = b;
-      ab.slots = cfgs[b].slots;
-      ab.cap = cfgs[b].cap;
-      ab.tsize_x16 = 32;
-      ab.cbuf = cfgs[b].cbuf;
-      ab.caux = cfgs[b].caux;
-      ab.keep_max = cfgs[b].keep_max;
-      ab.final_max = cfgs[b].final_max;
-      ab.group_smem_bytes = (int32_t)cfgs[b].region;
-      ab.bm_words = cfgs[b].bm_words;
-      CK(cudaStreamWaitEvent(c->bin_stream[b], c->bin_ev[8], 0));
-      CKR(launch_rows(c, ab, cfgs[b], c->bin_stream[b]));
-      CK(cudaEventRecord(c->bin_ev[b], c->bin_stream[b]));
-      CK(cudaStreamWaitEvent(s, c->bin_ev[b], 0));
+  if (!split) {
+    if (n_items_a > 0) CKR(launch_bins(c, a, bins, s));
+  } else {
+    // 2b. key ranges (DESIGN.md 3.1 "key ranges"): the plan is cut on the host from first_key_of_cb, read together with
+    // nnz(B') in one round trip (a plain copy: max colB + 2 ints can outgrow the mailbox).  The marginals are all-reduced,
+    // so every rank cuts the same plan.
+    const int32_t n_fk = max_marg_b + 2;
+    int32_t *h_fk = (int32_t *)c->pinned_get(sizeof(int32_t) * ((size_t)n_fk + 1), false);
+    if (!h_fk) return set_error(CCO_E_OOM, "pinned host allocation failed");
+    struct PutBack { cco_ctx *c; void *p; ~PutBack() { c->pinned_put(p); } } put_back{c, h_fk};
+    CK(cudaMemcpyAsync(h_fk, first_key_of_cb, sizeof(int32_t) * (size_t)n_fk, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(h_fk + n_fk, B.rp + B.n_rows, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    std::vector<KeyRange> plan;
+    if (!plan_key_ranges(h_fk, max_marg_b, n_cols_b, max_marg_a, c->key_range_cap, &plan))
+      return set_error(CCO_E_UNSUPPORTED,
+                       "co-occurrence counts up to %lld do not fit the packed 32-bit accumulator word even in a key range of one "
+                       "column (at most 2^30 - 1): lower maxItemsPerUser/maxEventsPerEventType for this event type "
+                       "(\"Limits\" in include/cco_b200.h)", k11_max);
+    const long long nnz_b = (long long)(uint32_t)h_fk[n_fk], U = B.n_rows;
+    st->n_ranges = (int)plan.size();
+    // Everything the ranges need is allocated once, here: one range's B'_r at a time, the running top-k next to one
+    // range's rows, and one set of scratch (scan and sort storage, the range's first_key_of_cb, the bin bounds) reused
+    // by every range -- memory does not grow with the number of ranges.
+    uint32_t *r_cnt, *r_ptr;
+    int32_t *r_col, *fk_r, *t_col = nullptr, *t_cnt = nullptr, *t_len = nullptr;
+    double *t_llr = nullptr;
+    void *scan_tmp, *sort_tmp;
+    size_t scan_tb = 0;
+    CKR(ar.alloc(&r_cnt, U + 1));
+    CKR(ar.alloc(&r_ptr, U + 1));
+    CK(cub::DeviceScan::ExclusiveSum(nullptr, scan_tb, r_cnt, r_ptr, U + 1, s));
+    CKR(ar.alloc(&r_col, std::max<long long>(nnz_b, 1)));
+    CKR(ar.alloc(&fk_r, (size_t)max_marg_b + 2));
+    CKR(ar.alloc((char **)&scan_tmp, scan_tb));
+    CKR(ar.alloc((char **)&sort_tmp, sort_tb));
+    BinPlan bp;
+    if (plan.size() > 1) {
+      CKR(ar.alloc(&t_col, cells));
+      CKR(ar.alloc(&t_cnt, cells));
+      if (!emit_all) CKR(ar.alloc(&t_llr, cells));
+      CKR(ar.alloc(&t_len, n_items_a + 1));
+    }
+    const int split_grid = grid_for(U * 32, 256, c->sm_count);
+    for (size_t r = 0; r < plan.size(); ++r) {
+      const KeyRange kr = plan[r];
+      const int32_t n_r = kr.k1 - kr.k0;
+      k_split_range<false><<<split_grid, 256, 0, s>>>(U, B.rp, B.col, kr.k0, kr.k1, r_cnt, nullptr);
+      CK(cub::DeviceScan::ExclusiveSum(scan_tmp, scan_tb, r_cnt, r_ptr, U + 1, s));
+      k_split_range<true><<<split_grid, 256, 0, s>>>(U, B.rp, B.col, kr.k0, kr.k1, r_ptr, r_col);
+      c->launches += 2;
+      // the range's schedule: products per row over B'_r, masked to this rank's rows (the partition of the whole B')
+      k_row_work<<<grid_for((long long)n_items_a * kSG, 256, c->sm_count), 256, 0, s>>>(n_items_a, at_ptr, at_users, r_ptr, row_work,
+                                                                                     work64, ids, nullptr);
+      k_mask_work<<<grid_for(n_items_a, 256, c->sm_count), 256, 0, s>>>(n_items_a, row_work, d_pb, rank, masked);
+      c->launches += 2;
+      if (n_items_a > 0)
+        CK(cub::DeviceRadixSort::SortPairsDescending(sort_tmp, sort_tb, masked, sorted_work, ids, rows_sorted, n_items_a, 0, 32, s));
+      k_range_first_keys<<<grid_for((long long)kr.max_marg + 2, 256, c->sm_count), 256, 0, s>>>(kr.max_marg + 2, first_key_of_cb, kr.k0,
+                                                                                             n_r, fk_r);
+      c->launches++;
+      int kb_r, cbits_r;
+      packed_bits(n_r, std::min<long long>(max_marg_a, kr.max_marg), &kb_r, &cbits_r);
+      CKR(plan_bins(c, ar, n_items_a, n_r, cbits_r, max_marg_a, kr.max_marg, n_users, k_eff, emit_all, sorted_work, s, &bp));
+      // the range as a view of B': keys rebased by k0, the per-key tables offset by k0 (the output keeps column ids)
+      RowArgs ar_r = a;
+      ar_r.b_ptr = r_ptr;
+      ar_r.b_col = r_col;
+      ar_r.marg_b = marg_key + kr.k0;
+      ar_r.col_terms = col_terms + kr.k0;
+      ar_r.first_key_of_cb = fk_r;
+      ar_r.key_base = kr.k0;
+      ar_r.key_shift = key_shift_for(n_r);
+      ar_r.max_marg_b = kr.max_marg;
+      ar_r.n_cols_b = n_r;
+      ar_r.cut_ok = cut_exact(n_users, max_marg_a, kr.max_marg) ? 1 : 0;
+      ar_r.count_bits = cbits_r;
+      if (r > 0) {   // later ranges write beside the running result and are merged into it
+        ar_r.out_col = t_col;
+        ar_r.out_llr = t_llr;
+        ar_r.out_cnt = t_cnt;
+        ar_r.out_len = t_len;
+        CK(cudaMemsetAsync(t_len, 0, sizeof(int32_t) * ((size_t)n_items_a + 1), s));
+      }
+      if (n_items_a > 0) CKR(launch_bins(c, ar_r, bp, s));
+      if (r > 0 && n_items_a > 0) {
+        k_merge_range<<<grid_for((long long)n_items_a * 32, 256, c->sm_count), 256, 0, s>>>(n_items_a, stride, k_eff, emit_all ? 1 : 0, o_col,
+                                                                                         o_llr, o_cnt, o_len, t_col, t_llr, t_cnt, t_len);
+        c->launches++;
+      }
     }
   }
   if (ev_end) CK(cudaEventRecord(ev_end, s));
@@ -1233,6 +1391,7 @@ static int finish_indicator(cco_ctx *c, IndicatorState *st, uint32_t flags, int 
       mm.col = (int32_t *)owner->pinned_get(sizeof(int32_t) * (size_t)std::max<long long>(grand, 1));
       if (st->p_cnt) mm.cnt = (int32_t *)owner->pinned_get(sizeof(int32_t) * (size_t)std::max<long long>(grand, 1));
       if (st->p_llr) mm.llr = (double *)owner->pinned_get(sizeof(double) * (size_t)std::max<long long>(grand, 1));
+      mm.key_ranges = st->n_ranges;   // every rank cuts the same plan
     }
     gs->barrier();
     if (!mm.row_ptr || !mm.col || (st->p_cnt && !mm.cnt) || (st->p_llr && !mm.llr)) return set_error(CCO_E_OOM, "pinned host allocation failed");
@@ -1247,10 +1406,12 @@ static int finish_indicator(cco_ctx *c, IndicatorState *st, uint32_t flags, int 
     rm->row_begin = lo;   // the member's own record (stats only; the arrays belong to the merged result)
     rm->row_end = hi;
     rm->n_cols = st->n_cols_b;
+    rm->key_ranges = st->n_ranges;
   } else {
     rm->row_begin = lo;
     rm->row_end = hi;
     rm->n_cols = st->n_cols_b;
+    rm->key_ranges = st->n_ranges;
     rm->row_ptr = (int64_t *)c->pinned_get(sizeof(int64_t) * ((size_t)n_my + 1));
     rm->col = (int32_t *)c->pinned_get(sizeof(int32_t) * (size_t)std::max<long long>(total, 1));
     if (st->p_cnt) rm->cnt = (int32_t *)c->pinned_get(sizeof(int32_t) * (size_t)std::max<long long>(total, 1));
@@ -2620,6 +2781,12 @@ int cco_result_row_range(const cco_result_t *r, int32_t i, int64_t *row_begin, i
   if (!r || i < 0 || i >= (int)r->mats.size()) return set_error(CCO_E_INVALID_ARG, "bad result/index");
   if (row_begin) *row_begin = r->mats[i].row_begin;
   if (row_end) *row_end = r->mats[i].row_end;
+  return CCO_OK;
+}
+
+int cco_result_key_ranges(const cco_result_t *r, int32_t i, int32_t *n_ranges) {
+  if (!r || i < 0 || i >= (int)r->mats.size() || !n_ranges) return set_error(CCO_E_INVALID_ARG, "bad result/index");
+  *n_ranges = r->mats[i].key_ranges;
   return CCO_OK;
 }
 
@@ -6378,6 +6545,13 @@ int cco_debug_downsample_block(cco_ctx_t *c, const cco_csr_t *m, int64_t row_lo,
     }
   }
   *col_idx = ci;
+  return CCO_OK;
+}
+
+int cco_debug_key_range_cap(cco_ctx_t *c, int32_t max_keys) {
+  if (!c || max_keys < 0) return set_error(CCO_E_INVALID_ARG, "null context or negative cap");
+  c->key_range_cap = max_keys;
+  for (cco_ctx *m : c->members) m->key_range_cap = max_keys;
   return CCO_OK;
 }
 

@@ -74,6 +74,7 @@ struct RowArgs {
   int *err_flag;     // set to 1 if a hash table overflowed (result invalid)
   int32_t emit_all;  // debug: write every non-zero cell (col,count), no LLR/top-k
   int32_t bm_words;  // bitmap rows (k_rows<..., BITMAP>): words of the key bitmap, ceil(n_cols_b / 32); else 0
+  int32_t key_base;  // key ranges (DESIGN.md 3.1): first global key of this view; its keys are key_of_col - key_base
 };
 
 constexpr uint32_t kEmpty = 0xffffffffu;
@@ -902,7 +903,11 @@ __global__ void __launch_bounds__(GROUP == 32 ? 64 : GROUP, RowsMinBlocks<GROUP>
     const int item = a.rows_sorted[ri];
     const uint32_t u_begin = a.at_ptr[item], u_end = a.at_ptr[item + 1];
     const long long ra = a.marg_a[item];
-    const int diag = a.self ? a.key_of_col[item] : -1;   // the key of the A'^T A' diagonal cell
+    int diag = -1;   // the key of the A'^T A' diagonal cell, -1 when it lies outside this key range
+    if (a.self) {
+      const int d = a.key_of_col[item] - a.key_base;
+      if ((unsigned)d < (unsigned)a.n_cols_b) diag = d;
+    }
     // Key path: 2 rowA colB < N for every column of B' (every row at C3 / C4), so every cell is strongly positive and both
     // the level-1 cut and the dominance filter are monotone in colB -- hence in the key.  They compare keys, and no cell
     // gathers its colB.  Other rows read colB from marg_b[key].
@@ -1344,6 +1349,89 @@ __global__ void k_compact_rows(int32_t n_items, int32_t stride, const long long 
       if (p_llr) p_llr[o + i] = llr[src + i];
       if (p_cnt) p_cnt[o + i] = cnt[src + i];
     }
+  }
+}
+
+// ---- key ranges (DESIGN.md 3.1): an indicator whose counts do not fit the packed word runs once per key range ----------
+// B'_r = the entries of B' whose key lies in [k0, k1), rebased to key - k0, over the same users.  One warp per user row;
+// WRITE = false counts them into r_ptr[u] (and r_ptr[n_rows] = 0, so an exclusive scan turns the counts into row pointers),
+// WRITE = true writes them at r_ptr[u] in the order of B'[u].
+template <bool WRITE>
+__global__ void k_split_range(long long n_rows, const uint32_t *__restrict__ b_ptr, const int32_t *__restrict__ b_col, int32_t k0,
+                              int32_t k1, uint32_t *__restrict__ r_ptr, int32_t *__restrict__ r_col) {
+  const int lane = threadIdx.x & 31;
+  const long long stride = (long long)gridDim.x * blockDim.x / 32;
+  if (!WRITE && blockIdx.x == 0 && threadIdx.x == 0) r_ptr[n_rows] = 0u;
+  for (long long u = (blockIdx.x * (long long)blockDim.x + threadIdx.x) / 32; u < n_rows; u += stride) {
+    const uint32_t s = b_ptr[u], e = b_ptr[u + 1];
+    uint32_t w = WRITE ? r_ptr[u] : 0u;
+    for (uint32_t q0 = s; q0 < e; q0 += 32) {
+      const uint32_t q = q0 + lane;
+      const int32_t key = q < e ? b_col[q] : -1;
+      const bool in = key >= k0 && key < k1;
+      const unsigned m = __ballot_sync(0xffffffffu, in);
+      if (WRITE && in) r_col[w + __popc(m & ((1u << lane) - 1u))] = key - k0;
+      w += __popc(m);
+    }
+    if (!WRITE && lane == 0) r_ptr[u] = w;
+  }
+}
+// first_key_of_cb of a key range: [c] = first key of the range whose colB >= c, for c in [0, max colB of the range + 1]
+__global__ void k_range_first_keys(int32_t n, const int32_t *__restrict__ first_key_of_cb, int32_t k0, int32_t n_keys,
+                                   int32_t *__restrict__ out) {
+  for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < n; c += gridDim.x * blockDim.x)
+    out[c] = min(max(first_key_of_cb[c] - k0, 0), n_keys);
+}
+// Merge range r's strided rows (r_*) into the running result (col / llr / cnt / len), in place, one warp per row.
+// Top-k rows: both lists are sorted by (llr desc, col asc) and hold distinct columns, so the first min(top_k, la + lb)
+// entries of their merge are the top-k over both ranges.  Output position p takes A[i] or B[p - i], i = the merge-path
+// co-rank of p; positions are filled from the end, 32 at a time, and every read of a chunk lies at or below its positions
+// while every later write lies below the chunk: the merge can overwrite A in place.
+// emit_all rows: the ranges' cells are appended (that mode's rows are unordered).
+__device__ __forceinline__ bool merge_before(double la, int32_t ca, double lb, int32_t cb) {
+  return la > lb || (la == lb && ca < cb);
+}
+__global__ void k_merge_range(int32_t n_items, int32_t stride, int32_t top_k, int32_t emit_all, int32_t *__restrict__ col,
+                              double *__restrict__ llr, int32_t *__restrict__ cnt, int32_t *__restrict__ len,
+                              const int32_t *__restrict__ r_col, const double *__restrict__ r_llr, const int32_t *__restrict__ r_cnt,
+                              const int32_t *__restrict__ r_len) {
+  const int lane = threadIdx.x & 31;
+  const int nwarps = (gridDim.x * blockDim.x) >> 5;
+  for (int item = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; item < n_items; item += nwarps) {
+    const int la = len[item], lb = r_len[item];
+    if (lb == 0) continue;
+    int32_t *A_col = col + (size_t)item * stride, *A_cnt = cnt + (size_t)item * stride;
+    const int32_t *B_col = r_col + (size_t)item * stride, *B_cnt = r_cnt + (size_t)item * stride;
+    if (emit_all) {
+      for (int j = lane; j < lb; j += 32) {
+        A_col[la + j] = B_col[j];
+        A_cnt[la + j] = B_cnt[j];
+      }
+      if (lane == 0) len[item] = la + lb;
+      continue;
+    }
+    double *A_llr = llr + (size_t)item * stride;
+    const double *B_llr = r_llr + (size_t)item * stride;
+    const int n = min(top_k, la + lb);
+    for (int base = (n - 1) & ~31; base >= 0; base -= 32) {
+      const int p = base + lane;
+      int32_t oc = 0, on = 0;
+      double ol = 0.0;
+      if (p < n) {
+        int lo = max(0, p - lb), hi = min(p, la);
+        while (lo < hi) {   // co-rank: the number of A entries among the first p outputs
+          const int mid = (lo + hi) >> 1;
+          if (merge_before(A_llr[mid], A_col[mid], B_llr[p - 1 - mid], B_col[p - 1 - mid])) lo = mid + 1; else hi = mid;
+        }
+        const int i = lo, j = p - lo;
+        const bool from_a = j >= lb || (i < la && merge_before(A_llr[i], A_col[i], B_llr[j], B_col[j]));
+        if (from_a) { oc = A_col[i]; ol = A_llr[i]; on = A_cnt[i]; } else { oc = B_col[j]; ol = B_llr[j]; on = B_cnt[j]; }
+      }
+      __syncwarp();
+      if (p < n) { A_col[p] = oc; A_llr[p] = ol; A_cnt[p] = on; }
+      __syncwarp();
+    }
+    if (lane == 0) len[item] = n;
   }
 }
 

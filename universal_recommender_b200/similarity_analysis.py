@@ -80,6 +80,7 @@ class CcoContext:
         self._uid = None
         self._arena = result_arena
         self.last_stats: TrainStats | None = None
+        self.last_key_ranges: list[int] | None = None   # per indicator of the last train: key ranges it ran in (FLAG_KEY_RANGES)
         self._pinned_addr: dict = {}
         self._logs = weakref.WeakSet()   # an event log belongs to its context: close() frees the open ones first
         if devices is not None:
@@ -166,7 +167,15 @@ class CcoContext:
         L = self._L
         try:
             out = []
+            ranges = []
+            # libcco_b200.so always exports it; only a stand-in for the result entry points (tests/test_string_ids.py's
+            # _StubLib answers row_range / matrix / stats / free) lacks it, and last_key_ranges is then None
+            key_ranges = getattr(L, "cco_result_key_ranges", None)
             for i in range(n):
+                if key_ranges is not None:
+                    kr = C.c_int32()
+                    N.check(key_ranges(res, i, C.byref(kr)))
+                    ranges.append(kr.value)
                 rb, re_ = C.c_int64(), C.c_int64()
                 N.check(L.cco_result_row_range(res, i, C.byref(rb), C.byref(re_)))
                 nr, nc = C.c_int64(), C.c_int32()
@@ -190,6 +199,7 @@ class CcoContext:
             self.last_stats = TrainStats(st.n_users, st.nnz_in_total, list(st.nnz_downsampled)[:n], list(st.products)[:n],
                                          list(st.distinct_cells)[:n], list(st.out_nnz)[:n], list(st.llr_evaluated)[:n], st.ms_h2d, st.ms_prepare,
                                          st.ms_cooccurrence, st.ms_total, list(st.ms_indicator)[:n], st.n_kernel_launches, list(st.ms_prep_stage))
+            self.last_key_ranges = ranges if key_ranges is not None else None
             if keep:
                 h, res = res, None
                 return out, h
@@ -1055,6 +1065,11 @@ class CcoContext:
         for p in (orp, oci, ocn):
             self._L.cco_free(p)
         return r, c, n
+
+    def debug_key_range_cap(self, max_keys: int):
+        """Tests only: cap every key range of this context's trains and debug entries at max_keys keys, even where the
+        packed word fits and without FLAG_KEY_RANGES (0 = off); last_key_ranges shows the ranges a train ran in."""
+        N.check(self._L.cco_debug_key_range_cap(self._h, int(max_keys)))
 
 
 class IndexWrite:
