@@ -559,9 +559,49 @@ int cco_event_log_window_stats(const cco_event_log_t *log, int64_t *n_expired, i
  * 0-based line next to the user and item columns (16 bytes per training event).  A log read without it is what
  * cco_event_log_begin_window reads, byte for byte and in device memory.  w as in cco_event_log_begin_window.
  */
-enum { CCO_LOG_KEEP_HISTORY = 1 };
+enum { CCO_LOG_KEEP_HISTORY = 1, CCO_LOG_EXTENDABLE = 2 };
 int cco_event_log_begin_ex(cco_ctx_t *ctx, int64_t chunk_bytes, const cco_event_window_t *w /* nullable */, uint32_t flags,
                            cco_event_log_t **out);
+
+/*
+ * Extendable logs: a resident log that takes the newest lines of an export and a later cutoff without a re-read, for a
+ * trainer that retrains on a schedule with a sliding eventWindow.  cco_event_log_begin_ex with CCO_LOG_EXTENDABLE (it
+ * combines with CCO_LOG_KEEP_HISTORY) keeps, besides what the log holds anyway: each retained line's record (40 bytes:
+ * its identity hash under remove_duplicates, eventTime, global line, name and selection), the global line of each
+ * training and ranking entry (8 bytes each), the retained property-event lines (their bytes) and, under
+ * remove_duplicates, the eventTime of each line dropped as a duplicate whose event is neither $set nor $unset (8 bytes).
+ * A log read without the flag is what cco_event_log_begin_ex reads without it, byte for byte and in device memory.
+ *
+ * cco_event_log_extend reopens a finished extendable log for cco_event_log_append / cco_event_log_finish, staged in the
+ * chunk_bytes the log was begun with; w == NULL keeps the current window.  Reading bytes A with window w1, then
+ * extending with w2 and appending bytes B, gives after finish the log one read of A followed by B under w2 gives: info,
+ * window_stats and every consumer's output (ingest, format_model_log, rerank_model_log, user_queries, mixed_queries,
+ * query_file_queries).  B's first byte starts a line, as if A ended in '\n'; B's lines are numbered after A's, in
+ * messages, in the (eventTime, line) rules and in history order.  Extends compose; one with no bytes only slides the
+ * window.  Expiry comes first, then removeDuplicates (cco_event_log_begin_window), and three consequences follow:
+ *  - duplicates across the seam: a line of B can drop a retained line of A, or be dropped for it, in either time order;
+ *    at equal eventTime the later line, B's, stays.  So the record of every retained line survives finish, ignored and
+ *    property-event lines included, since the counts of info name them;
+ *  - stats re-attribution: a line dropped as a duplicate under the old cutoff whose eventTime is at or before the new one
+ *    (and whose event is neither $set nor $unset) is an expired line for a whole read under the new cutoff; it moves from
+ *    the duplicates to the expired lines of window_stats;
+ *  - properties: a $delete that expires under the new cutoff lets the $sets before it count again, so the retained
+ *    property-event lines stay resident and the aggregation runs again at every finish over old and new lines.  $set
+ *    and $unset never expire.
+ * All of it is exact because cutoffs only move forward: a line dropped under w1 is dropped under w2.  At finish only B
+ * is parsed; the retained records, entries and property lines at or before the new cutoff are dropped and freed, the
+ * retained records are deduplicated together with B's (one sort of all of them: the three 64-bit passes of removeDuplicates,
+ * O(retained + new) per finish), the columns are concatenated name-major (the retained layout first, names new in B
+ * after) and compacted, and the properties are aggregated again.
+ * Errors: CCO_E_INVALID_ARG for a null log, a log read without CCO_LOG_EXTENDABLE, a log not finished or failed, a cutoff
+ * below the current one, a remove_duplicates other than the first read's and a nonzero reserved field.  A failed append
+ * or finish during an extend fails the log as it does any read: its resident state is lost, and every call but free
+ * returns CCO_E_INVALID_ARG with the failure's message.
+ * cco_event_log_resident_bytes: the device bytes a finished log holds (bounded by its retained lines, not by every line
+ * ever appended).
+ */
+int cco_event_log_extend(cco_event_log_t *log, const cco_event_window_t *w /* nullable: keep the current window */);
+int cco_event_log_resident_bytes(const cco_event_log_t *log, int64_t *bytes);
 /*
  * The query of user u, for the query event names n_0 .. n_{k-1}:
  *  - history of n_q: u's training events of n_q, latest first (eventTime desc, ties to the later line), the first limits[q]

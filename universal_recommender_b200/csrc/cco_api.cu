@@ -264,6 +264,7 @@ struct Arena {
   cudaStream_t s;
   cco_ctx *c;   // non-null: buffers up to kSlabMax bytes are bump-allocated from the context's slabs
   std::vector<void *> ptrs;
+  std::vector<size_t> sizes;   // bytes of each of ptrs
   static constexpr size_t kSlabMax = 8u << 20, kSlabBytes = 64u << 20;
   explicit Arena(cudaStream_t st, cco_ctx *ctx = nullptr) : s(st), c(ctx && !ctx->slab_busy ? ctx : nullptr) {
     if (c) {
@@ -308,21 +309,27 @@ struct Arena {
     cudaError_t e = cudaMallocAsync(&p, bytes, s);
     if (e != cudaSuccess) return set_error(CCO_E_OOM, "cudaMallocAsync(%zu bytes): %s", bytes, cudaGetErrorString(e));
     ptrs.push_back(p);
+    sizes.push_back(bytes);
     *out = (T *)p;
     return CCO_OK;
   }
-  void take(void *p) {   // the buffer outlives the arena: its new owner frees it (never slab memory)
+  // the buffer outlives the arena: its new owner frees it (never slab memory); -> its bytes
+  size_t take(void *p) {
     for (size_t i = 0; i < ptrs.size(); ++i)
       if (ptrs[i] == p) {
+        const size_t b = sizes[i];
         ptrs.erase(ptrs.begin() + i);
-        return;
+        sizes.erase(sizes.begin() + i);
+        return b;
       }
+    return 0;
   }
   void release(void *p) {   // slab memory is simply not reused within a train
     for (size_t i = 0; i < ptrs.size(); ++i)
       if (ptrs[i] == p) {
         cudaFreeAsync(p, s);
         ptrs.erase(ptrs.begin() + i);
+        sizes.erase(sizes.begin() + i);
         return;
       }
   }
@@ -3719,6 +3726,7 @@ struct cco_event_log {
   unsigned char *p_vals = nullptr, *p_ibytes = nullptr;
   std::vector<std::string> field_names;
   std::vector<void *> dev;                     // what to free
+  std::vector<size_t> dev_bytes;               // the bytes of each (cco_event_log_resident_bytes)
   // the read in progress (cco_event_log_begin / _append / _finish): staging of cap bytes (+ 24 of padding) holding
   // `staged` bytes, the last '\n' among them at last_nl (-1: none); lines parsed so far; per chunk one segment; the
   // property-event lines (each ending in '\n') and their global lines, aggregated at finish
@@ -3742,6 +3750,13 @@ struct cco_event_log {
   // then outlives finish
   bool history = false;
   long long *ttime = nullptr;
+  // extendable logs (CCO_LOG_EXTENDABLE): rec (one record per retained line, with or without dedup), tline / rline and the
+  // property lines (pb, prop_line) outlive finish; dup_time holds the eventTimes of the non-exempt lines removeDuplicates
+  // dropped, which a later cutoff turns into expired lines; chunk0 is the staging cco_event_log_extend reopens with
+  bool extendable = false;
+  long long chunk0 = 0;
+  long long *dup_time = nullptr;
+  long long n_dup_time = 0;
   bool finished = false;
   int fail = CCO_OK;                           // a failed append / finish: every later call returns it with fail_msg
   std::string fail_msg;
@@ -3792,7 +3807,7 @@ static int event_error(unsigned long long err) {
   }
 }
 static int log_keep(Arena &ar, cco_event_log *lg, void *p) {
-  ar.take(p);
+  lg->dev_bytes.push_back(ar.take(p));
   lg->dev.push_back(p);
   return CCO_OK;
 }
@@ -3802,6 +3817,7 @@ static void log_drop(cco_event_log *lg, void *p) {
     if (lg->dev[i] == p) {
       cudaFreeAsync(p, lg->ctx->stream);
       lg->dev.erase(lg->dev.begin() + i);
+      lg->dev_bytes.erase(lg->dev_bytes.begin() + i);
       return;
     }
 }
@@ -4021,7 +4037,15 @@ static int event_properties(cco_ctx *c, Arena &ar, cco_event_log *lg, long long 
   CKR(mail_fetch(c, &T, pos + N, 4));
   CKR(mail_wait(c));
   lg->n_triples = T;
-  if (T == 0) return CCO_OK;
+  auto drop_items = [&] {   // an extendable log aggregates at every finish: the item column goes once the triples are built
+    if (!lg->extendable) return;
+    log_drop(lg, pcol.off);
+    log_drop(lg, pcol.w);
+  };
+  if (T == 0) {
+    drop_items();
+    return CCO_OK;
+  }
   uint32_t *titem, *first;
   int32_t *tfield;
   long long *vb, *ve;
@@ -4088,6 +4112,7 @@ static int event_properties(cco_ctx *c, Arena &ar, cco_event_log *lg, long long 
   lg->p_ioff = ioff;
   lg->p_ibytes = ibytes;
   lg->p_ibytes_n = itotal;
+  drop_items();
   return CCO_OK;
 }
 
@@ -4251,6 +4276,29 @@ static int win_records(cco_event_log *lg, Arena &ar, const EvLines &ev, const in
   lg->n_rec += R;
   return CCO_OK;
 }
+// extendable logs without removeDuplicates, per chunk: what expiry needs of every retained line (a WinRec without a hash)
+static int ext_records(cco_event_log *lg, Arena &ar, const EvLines &ev, const int32_t *code, long long base) {
+  cco_ctx *c = lg->ctx;
+  cudaStream_t s = c->stream;
+  const long long L = ev.L;
+  uint32_t *keep, *pos, *ridx, R32 = 0;
+  CKR(ar.alloc(&keep, L + 1));
+  k_win_keep_lines<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, ev.flag, keep);
+  c->launches++;
+  CKR(select_flagged(c, ar, L, keep, &pos, &ridx));
+  CKR(mail_fetch(c, &R32, pos + L, 4));
+  CKR(mail_wait(c));
+  const long long R = R32;
+  if (R == 0) return CCO_OK;
+  if (lg->n_rec + R > lg->rec_cap) {   // grow geometrically
+    lg->rec_cap = std::max(2 * lg->rec_cap, lg->n_rec + R);
+    CKR(log_grow(lg, ar, &lg->rec, lg->rec_cap, lg->n_rec, 0));
+  }
+  k_ext_line_recs<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, ridx, base, ev.tm, ev.flag, code, lg->rec + lg->n_rec);
+  c->launches++;
+  lg->n_rec += R;
+  return CCO_OK;
+}
 
 // one chunk of a streamed read, the first len staged bytes: every line parsed, the names numbered globally, the counts
 // added, the training and ranking events decoded into one new segment, the property-event lines appended to lg->pb
@@ -4342,12 +4390,13 @@ static int event_chunk(cco_event_log *lg, long long len, bool open_tail) {
   lg->n_ignored += (long long)h_cnt[2 * NG + 1];
   lg->n_lines += L;
   if (lg->dedup) CKR(win_records(lg, ar, ev, code, base));
+  else if (lg->extendable) CKR(ext_records(lg, ar, ev, code, base));
   // 7. training and ranking events partitioned by name, file order inside a name: decoded ids and times
   uint32_t *idx;
   CKR(event_partition(c, ar, L, ev.flag, kEvTraining, code, (uint32_t)NG, &idx));
   CKR(event_column(c, ar, lg, sg.train_at[NG], idx, kEvEntityId, ev.sb, ev.span, bb, sg.train_at, &sg.tu));
   CKR(event_column(c, ar, lg, sg.train_at[NG], idx, kEvTargetId, ev.sb, ev.span, bb, sg.train_at, &sg.ti));
-  if (lg->dedup || lg->history) CKR(win_entry_lines(lg, ar, sg.train_at[NG], idx, base, &sg.tline));
+  if (lg->dedup || lg->history || lg->extendable) CKR(win_entry_lines(lg, ar, sg.train_at[NG], idx, base, &sg.tline));
   if (lg->history) {
     const long long NT = sg.train_at[NG];
     CKR(ar.alloc(&sg.ttime, std::max<long long>(NT, 1)));
@@ -4367,7 +4416,7 @@ static int event_chunk(cco_event_log *lg, long long len, bool open_tail) {
     k_gather_i64<<<grid_for(NR, 256, c->sm_count), 256, 0, s>>>(NR, idx, ev.tm, sg.rtime);
     c->launches++;
   }
-  if (lg->dedup) CKR(win_entry_lines(lg, ar, NR, idx, base, &sg.rline));
+  if (lg->dedup || lg->extendable) CKR(win_entry_lines(lg, ar, NR, idx, base, &sg.rline));
   ar.release(idx);
   // 8. the property-event lines, in line order, for the aggregation at finish (see event_log_finish)
   if (NP > 0) {
@@ -4478,16 +4527,24 @@ static int event_cat_times(cco_event_log *lg, long long **out, long long *EvSeg:
   return CCO_OK;
 }
 
+// the drop bitmap over the global lines, kept by the log until finish ends
+static int win_bitmap(cco_event_log *lg, Arena &ar, uint32_t **bitmap) {
+  const long long words = lg->n_lines / 32 + 1;
+  CKR(ar.alloc(bitmap, words));
+  CKR(log_keep(ar, lg, *bitmap));
+  CK(cudaMemsetAsync(*bitmap, 0, sizeof(uint32_t) * (size_t)words, lg->ctx->stream));
+  return CCO_OK;
+}
 // removeDuplicates at finish: the records of every chunk sorted by (hash, time desc, line desc); all but the first of each
-// run are dropped -> *bitmap over the global lines (kept by the log until finish ends); the counts of the drops
-static int win_mark(cco_event_log *lg, uint32_t **bitmap, long long *n_prop_dup) {
+// run are dropped -> *bitmap over the global lines (made here when null); *n_prop_drop += the property lines among the
+// drops, *n_new = all of them.
+// An extendable log keeps its records (ext_split_records takes the dropped ones out).
+static int win_mark(cco_event_log *lg, uint32_t **bitmap, long long *n_prop_drop, long long *n_new) {
   cco_ctx *c = lg->ctx;
   cudaStream_t s = c->stream;
   Arena ar(s);
-  const long long N = lg->n_rec, NG = (long long)lg->name_off.size() - 1, words = lg->n_lines / 32 + 1;
-  CKR(ar.alloc(bitmap, words));
-  CKR(log_keep(ar, lg, *bitmap));
-  CK(cudaMemsetAsync(*bitmap, 0, sizeof(uint32_t) * (size_t)words, s));
+  const long long N = lg->n_rec, NG = (long long)lg->name_off.size() - 1;
+  if (!*bitmap) CKR(win_bitmap(lg, ar, bitmap));
   std::vector<unsigned long long> h_cnt((size_t)(2 * NG + 3), 0);
   if (N > 1) {
     unsigned long long *key, *cnt;
@@ -4509,12 +4566,170 @@ static int win_mark(cco_event_log *lg, uint32_t **bitmap, long long *n_prop_dup)
     CK(cudaMemcpyAsync(h_cnt.data(), cnt, sizeof(unsigned long long) * h_cnt.size(), cudaMemcpyDeviceToHost, s));
   }
   CK(cudaStreamSynchronize(s));
-  *n_prop_dup = (long long)h_cnt[2 * NG];
+  *n_prop_drop += (long long)h_cnt[2 * NG];
   lg->n_prop -= (long long)h_cnt[2 * NG];
   lg->n_ignored -= (long long)h_cnt[2 * NG + 1];
-  lg->n_dup = (long long)h_cnt[2 * NG + 2];
+  *n_new = (long long)h_cnt[2 * NG + 2];
+  lg->n_dup += *n_new;
+  if (!lg->extendable) {
+    log_drop(lg, lg->rec);
+    lg->rec = nullptr;
+  }
+  return CCO_OK;
+}
+
+// ---- extendable logs: the retained part under a later cutoff (kernels k_ext_* in cco_events.cuh) ---------------------------
+// per event name: 1 for "$set" and "$unset", which never expire
+static int ext_exempt(cco_event_log *lg, Arena &ar, uint8_t **out) {
+  const long long NG = (long long)lg->name_off.size() - 1;
+  std::vector<uint8_t> h((size_t)std::max<long long>(NG, 1), 0);
+  for (long long g = 0; g < NG; ++g) {
+    const std::string nm(lg->name_bytes.data() + lg->name_off[g], (size_t)(lg->name_off[g + 1] - lg->name_off[g]));
+    h[g] = nm == "$set" || nm == "$unset";
+  }
+  CKR(ar.alloc(out, h.size()));
+  CK(cudaMemcpyAsync(*out, h.data(), h.size(), cudaMemcpyHostToDevice, lg->ctx->stream));
+  CK(cudaStreamSynchronize(lg->ctx->stream));   // h is a local
+  return CCO_OK;
+}
+// the records idx[0 .. K) become the log's records (an exact fit: expired and dropped ones are freed)
+static int ext_keep_records(cco_event_log *lg, Arena &ar, long long K, const uint32_t *idx) {
+  cco_ctx *c = lg->ctx;
+  WinRec *r;
+  CKR(ar.alloc(&r, std::max<long long>(K, 1)));
+  if (K > 0) {
+    k_ext_gather_rec<<<grid_for(K, 256, c->sm_count), 256, 0, c->stream>>>(K, idx, lg->rec, r);
+    c->launches++;
+  }
+  CKR(log_keep(ar, lg, r));
   log_drop(lg, lg->rec);
-  lg->rec = nullptr;
+  lg->rec = r;
+  lg->n_rec = lg->rec_cap = K;
+  return CCO_OK;
+}
+// the cutoff applied to what earlier finishes retained: a record at or before it whose name is not exempt expires (its
+// line goes into *bitmap, made here), and an earlier duplicate drop at or before it counts as expired from now on, as a
+// whole read under this cutoff counts it.  *n_x: the lines that expired, *n_px: of them property events.  The lines
+// parsed since the last finish were judged under this cutoff already and pass unchanged.
+static int ext_expire(cco_event_log *lg, const uint8_t *exempt, uint32_t **bitmap, long long *n_x, long long *n_px) {
+  cco_ctx *c = lg->ctx;
+  cudaStream_t s = c->stream;
+  Arena ar(s);
+  CKR(win_bitmap(lg, ar, bitmap));
+  *n_x = *n_px = 0;
+  const long long N = lg->n_rec, D = lg->n_dup_time;
+  if (lg->cutoff == INT64_MIN || (N == 0 && D == 0)) return CCO_OK;
+  unsigned long long *cnt, h_cnt[4] = {0, 0, 0, 0};
+  uint32_t *keep, *pos, *idx, *dkeep, *dpos, *didx, K = 0, KD = 0;
+  CKR(ar.alloc(&cnt, 4));
+  CK(cudaMemsetAsync(cnt, 0, sizeof(h_cnt), s));
+  CKR(ar.alloc(&keep, N + 1));
+  CKR(ar.alloc(&dkeep, D + 1));
+  if (N > 0) {
+    k_ext_expire<<<grid_for(N, 256, c->sm_count), 256, 0, s>>>(N, lg->rec, lg->cutoff, exempt, *bitmap, keep, cnt);
+    c->launches++;
+  }
+  CKR(select_flagged(c, ar, N, keep, &pos, &idx));
+  if (D > 0) {
+    k_ext_expire_times<<<grid_for(D, 256, c->sm_count), 256, 0, s>>>(D, lg->dup_time, lg->cutoff, dkeep, cnt + 3);
+    c->launches++;
+  }
+  CKR(select_flagged(c, ar, D, dkeep, &dpos, &didx));
+  CK(cudaMemcpyAsync(h_cnt, cnt, sizeof(h_cnt), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(&K, pos + N, 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(&KD, dpos + D, 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  if (h_cnt[0] > 0) CKR(ext_keep_records(lg, ar, K, idx));
+  if (h_cnt[3] > 0) {
+    long long *t;
+    CKR(ar.alloc(&t, std::max<uint32_t>(KD, 1)));
+    if (KD > 0) {
+      k_gather_i64<<<grid_for(KD, 256, c->sm_count), 256, 0, s>>>(KD, didx, lg->dup_time, t);
+      c->launches++;
+    }
+    CKR(log_keep(ar, lg, t));
+    log_drop(lg, lg->dup_time);
+    lg->dup_time = t;
+    lg->n_dup_time = KD;
+  }
+  CK(cudaStreamSynchronize(s));
+  *n_x = (long long)h_cnt[0];
+  *n_px = (long long)h_cnt[1];
+  lg->n_expired += (long long)(h_cnt[0] + h_cnt[3]);
+  lg->n_dup -= (long long)h_cnt[3];
+  lg->n_prop -= (long long)h_cnt[1];
+  lg->n_ignored -= (long long)h_cnt[2];
+  return CCO_OK;
+}
+// after win_mark: the records whose line it dropped leave the log; the eventTimes of the non-exempt ones join dup_time
+static int ext_split_records(cco_event_log *lg, const uint8_t *exempt, const uint32_t *bitmap) {
+  cco_ctx *c = lg->ctx;
+  cudaStream_t s = c->stream;
+  Arena ar(s);
+  const long long N = lg->n_rec;
+  uint32_t *keep, *dup, *pos, *idx, *dpos, *didx, K = 0, KD = 0;
+  long long *tm;
+  CKR(ar.alloc(&keep, N + 1));
+  CKR(ar.alloc(&dup, N + 1));
+  CKR(ar.alloc(&tm, N));
+  k_ext_dup_split<<<grid_for(N, 256, c->sm_count), 256, 0, s>>>(N, lg->rec, bitmap, exempt, keep, dup, tm);
+  c->launches++;
+  CKR(select_flagged(c, ar, N, keep, &pos, &idx));
+  CKR(select_flagged(c, ar, N, dup, &dpos, &didx));
+  CK(cudaMemcpyAsync(&K, pos + N, 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(&KD, dpos + N, 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  CKR(ext_keep_records(lg, ar, K, idx));
+  if (KD > 0) {
+    CKR(log_grow(lg, ar, &lg->dup_time, lg->n_dup_time + KD, lg->n_dup_time, 0));
+    k_gather_i64<<<grid_for(KD, 256, c->sm_count), 256, 0, s>>>(KD, didx, tm, lg->dup_time + lg->n_dup_time);
+    c->launches++;
+    lg->n_dup_time += KD;
+  }
+  CK(cudaStreamSynchronize(s));
+  return CCO_OK;
+}
+// after the aggregation: the property lines that are still selected (ev: pb parsed, dropped lines with flag 0) become pb,
+// an exact fit, and prop_line follows them
+static int ext_keep_property_lines(cco_event_log *lg, Arena &ar, const EvLines &ev) {
+  cco_ctx *c = lg->ctx;
+  cudaStream_t s = c->stream;
+  const long long L = ev.L;
+  uint32_t *keep, *pos, *idx, K = 0;
+  CKR(ar.alloc(&keep, L + 1));
+  k_win_flag_keep<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, ev.flag, kEvProperty, keep);
+  c->launches++;
+  CKR(select_flagged(c, ar, L, keep, &pos, &idx));
+  CK(cudaMemcpyAsync(&K, pos + L, 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  if (K == (uint32_t)L) return CCO_OK;   // nothing left the window
+  long long *len8, *off, total = 0;
+  CKR(ar.alloc(&len8, (long long)K + 1));
+  CKR(ar.alloc(&off, (long long)K + 1));
+  CK(cudaMemsetAsync(len8 + K, 0, 8, s));
+  if (K > 0) {
+    k_line_len<<<grid_for(K, 256, c->sm_count), 256, 0, s>>>(K, idx, ev.sb, ev.se, len8);
+    c->launches++;
+  }
+  CKR(exclusive_sum(c, ar, len8, off, (long long)K + 1));
+  std::vector<uint32_t> h_idx((size_t)K);
+  CK(cudaMemcpyAsync(&total, off + K, 8, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(h_idx.data(), idx, sizeof(uint32_t) * (size_t)K, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  unsigned char *pb;
+  CKR(ar.alloc(&pb, total + 24));
+  if (K > 0) {
+    k_line_gather<<<grid_for((long long)K * 32, 256, c->sm_count), 256, 0, s>>>(K, idx, ev.sb, ev.se, lg->pb, off, pb);
+    c->launches++;
+  }
+  CKR(log_keep(ar, lg, pb));
+  log_drop(lg, lg->pb);
+  lg->pb = pb;
+  lg->pb_len = lg->pb_cap = total;
+  std::vector<long long> pl((size_t)K);
+  for (uint32_t k = 0; k < K; ++k) pl[k] = lg->prop_line[h_idx[k]];
+  lg->prop_line.swap(pl);
+  CK(cudaStreamSynchronize(s));
   return CCO_OK;
 }
 // a string column's entries idx[0 .. K) gathered into a new column kept by the log (the old one is freed); boff at the
@@ -4661,7 +4876,7 @@ static int event_log_begin(cco_ctx *c, int64_t chunk_bytes, cco_event_log **out)
   lg->name_off.assign(1, 0);
   lg->train_at.assign(1, 0);
   lg->rank_at.assign(1, 0);
-  lg->cap = std::max<int64_t>(chunk_bytes, 1);
+  lg->cap = lg->chunk0 = std::max<int64_t>(chunk_bytes, 1);
   Arena ar(c->stream);
   const int rc = ar.alloc(&lg->stage, lg->cap + 24);
   if (rc != CCO_OK) {
@@ -4712,11 +4927,23 @@ static int event_log_finish(cco_event_log *lg) {
     lg->train_at[n + 1] = lg->train_at[n] + lg->n_train[n];
     lg->rank_at[n + 1] = lg->rank_at[n] + lg->n_rank[n];
   }
-  uint32_t *drop = nullptr;   // removeDuplicates: the dropped global lines
-  long long n_prop_dup = 0;
+  uint32_t *drop = nullptr;   // removeDuplicates (and an extendable log's expiry): the dropped global lines
+  long long n_prop_drop = 0, n_drop = 0;   // dropped property lines, all dropped lines
+  Arena ear(s);
+  uint8_t *exempt = nullptr;
+  if (lg->extendable) {   // what earlier finishes retained, under the current cutoff
+    long long n_x = 0, n_px = 0;
+    CKR(ext_exempt(lg, ear, &exempt));
+    CKR(ext_expire(lg, exempt, &drop, &n_x, &n_px));
+    n_drop += n_x;
+    n_prop_drop += n_px;
+  }
   if (lg->dedup) {
+    long long n_new = 0;
     mail_reset(c);
-    CKR(win_mark(lg, &drop, &n_prop_dup));
+    CKR(win_mark(lg, &drop, &n_prop_drop, &n_new));
+    n_drop += n_new;
+    if (lg->extendable && n_new > 0) CKR(ext_split_records(lg, exempt, drop));
   }
   if (lg->segs.size() == 1) {   // one chunk: its segment is the layout
     EvSeg &sg = lg->segs[0];
@@ -4732,43 +4959,84 @@ static int event_log_finish(cco_event_log *lg) {
     CKR(event_cat_column(lg, &EvSeg::ti, &EvSeg::train_at, lg->train_at, &lg->ti));
     CKR(event_cat_column(lg, &EvSeg::ri, &EvSeg::rank_at, lg->rank_at, &lg->ri));
     CKR(event_cat_times(lg, &lg->rtime));
-    if (lg->dedup || lg->history) CKR(event_cat_times(lg, &lg->tline, &EvSeg::tline, &EvSeg::train_at));
-    if (lg->dedup) CKR(event_cat_times(lg, &lg->rline, &EvSeg::rline, &EvSeg::rank_at));
+    if (lg->dedup || lg->history || lg->extendable) CKR(event_cat_times(lg, &lg->tline, &EvSeg::tline, &EvSeg::train_at));
+    if (lg->dedup || lg->extendable) CKR(event_cat_times(lg, &lg->rline, &EvSeg::rline, &EvSeg::rank_at));
     if (lg->history) CKR(event_cat_times(lg, &lg->ttime, &EvSeg::ttime, &EvSeg::train_at));
   }
   lg->segs.clear();
-  if (drop && lg->n_dup > 0) {   // the retained columns without the dropped lines' entries
+  if (drop && n_drop > 0) {   // the retained columns without the dropped lines' entries
     CKR(win_compact(lg, drop, lg->tline, lg->train_at, &lg->tu, &lg->ti, lg->history ? &lg->ttime : nullptr,
-                    lg->history ? &lg->tline : nullptr));
-    CKR(win_compact(lg, drop, lg->rline, lg->rank_at, &lg->ri, nullptr, &lg->rtime));
+                    lg->history || lg->extendable ? &lg->tline : nullptr));
+    CKR(win_compact(lg, drop, lg->rline, lg->rank_at, &lg->ri, nullptr, &lg->rtime, lg->extendable ? &lg->rline : nullptr));
     for (long long n = 0; n < NG; ++n) {
       lg->n_train[n] = lg->train_at[n + 1] - lg->train_at[n];
       lg->n_rank[n] = lg->rank_at[n + 1] - lg->rank_at[n];
     }
   }
-  if (!lg->history) {
+  if (!lg->history && !lg->extendable) {
     log_drop(lg, lg->tline);
     lg->tline = nullptr;
   }
-  log_drop(lg, lg->rline);
-  lg->rline = nullptr;
+  if (!lg->extendable) {
+    log_drop(lg, lg->rline);
+    lg->rline = nullptr;
+  }
   if (lg->n_prop > 0) {
     mail_reset(c);
     Arena ar(s);
     CKR(event_pad(c, lg->pb, lg->pb_len));
     EvLines ev;
     CKR(event_lines(c, ar, (const uint64_t *)lg->pb, lg->pb_len, false, 0, &ev));   // judged once already
-    if (n_prop_dup > 0) CKR(win_drop_property_lines(lg, ar, ev, drop));
+    if (n_prop_drop > 0) CKR(win_drop_property_lines(lg, ar, ev, drop));
     CKR(event_properties(c, ar, lg, ev.L, ev.flag, ev.tm, ev.sb, ev.span, lg->pb, lg->prop_line.data()));
+    if (lg->extendable) CKR(ext_keep_property_lines(lg, ar, ev));
     CK(cudaStreamSynchronize(s));
   }
   log_drop(lg, drop);
-  log_drop(lg, lg->pb);
-  lg->pb = nullptr;
-  lg->prop_line = std::vector<long long>();
+  if (!lg->extendable || lg->n_prop == 0) {
+    log_drop(lg, lg->pb);
+    lg->pb = nullptr;
+    lg->pb_len = lg->pb_cap = 0;
+    lg->prop_line = std::vector<long long>();
+  }
   CK(cudaStreamSynchronize(s));
   CK(cudaGetLastError());
   lg->finished = true;
+  return CCO_OK;
+}
+
+// a finished extendable log reopened for append / finish: its retained layout becomes the first segment of the next
+// finish, which concatenates the new chunks' segments after it name-major, re-expires it under the new cutoff and
+// deduplicates it together with them; the aggregated properties are rebuilt then
+static int event_log_extend(cco_event_log *lg, const cco_event_window_t *w) {
+  cco_ctx *c = lg->ctx;
+  CK(cudaSetDevice(c->device));
+  NvtxRange nvtx("cco:event_log_extend");
+  Arena ar(c->stream);
+  lg->cap = lg->chunk0;
+  CKR(ar.alloc(&lg->stage, lg->cap + 24));
+  CKR(log_keep(ar, lg, lg->stage));
+  lg->staged = 0;
+  lg->last_nl = -1;
+  if (w) lg->cutoff = w->cutoff_ms;
+  EvSeg sg;
+  sg.tu = lg->tu;
+  sg.ti = lg->ti;
+  sg.ri = lg->ri;
+  sg.rtime = lg->rtime;
+  sg.tline = lg->tline;
+  sg.rline = lg->rline;
+  sg.ttime = lg->ttime;
+  sg.train_at = lg->train_at;
+  sg.rank_at = lg->rank_at;
+  lg->segs.assign(1, sg);
+  for (void *p : {(void *)lg->p_field, (void *)lg->p_voff, (void *)lg->p_vals, (void *)lg->p_ioff, (void *)lg->p_ibytes}) log_drop(lg, p);
+  lg->p_field = nullptr;
+  lg->p_voff = lg->p_ioff = nullptr;
+  lg->p_vals = lg->p_ibytes = nullptr;
+  lg->p_ibytes_n = lg->n_triples = lg->n_prop_items = lg->n_prop_fields = 0;
+  lg->field_names.clear();
+  lg->finished = false;
   return CCO_OK;
 }
 
@@ -4859,6 +5127,29 @@ int cco_event_log_finish(cco_event_log_t *lg) {
   if (!lg) return set_error(CCO_E_INVALID_ARG, "null argument");
   CKR(log_state(lg, false));
   return log_fail(lg, event_log_finish(lg));
+}
+
+int cco_event_log_extend(cco_event_log_t *lg, const cco_event_window_t *w) {
+  if (!lg) return set_error(CCO_E_INVALID_ARG, "null argument");
+  CKR(log_state(lg, true));
+  if (!lg->extendable) return set_error(CCO_E_INVALID_ARG, "the log was read without CCO_LOG_EXTENDABLE (cco_event_log_begin_ex)");
+  if (w) {
+    if (w->reserved != 0) return set_error(CCO_E_INVALID_ARG, "the window's reserved field must be 0");
+    if ((w->remove_duplicates != 0) != lg->dedup || (w->remove_duplicates != 0 && w->remove_duplicates != 1))
+      return set_error(CCO_E_INVALID_ARG, "remove_duplicates is %d: an extend keeps the first read's (%d)", (int)w->remove_duplicates, (int)lg->dedup);
+    if (w->cutoff_ms < lg->cutoff)
+      return set_error(CCO_E_INVALID_ARG, "cutoff %lld is before the log's %lld: expired lines are gone", (long long)w->cutoff_ms, lg->cutoff);
+  }
+  return log_fail(lg, event_log_extend(lg, w));
+}
+
+int cco_event_log_resident_bytes(const cco_event_log_t *lg, int64_t *bytes) {
+  if (!lg || !bytes) return set_error(CCO_E_INVALID_ARG, "null argument");
+  CKR(log_state(lg, true));
+  int64_t b = 0;
+  for (size_t x : lg->dev_bytes) b += (int64_t)x;
+  *bytes = b;
+  return CCO_OK;
 }
 
 int cco_event_log_read(cco_ctx_t *ctx, const char *bytes, int64_t len, cco_event_log_t **out) {
@@ -5318,9 +5609,10 @@ static int uq_every_user(cco_ctx *c, Arena &ar, const cco_event_log *lg, const U
 }  // namespace cco
 
 int cco_event_log_begin_ex(cco_ctx_t *ctx, int64_t chunk_bytes, const cco_event_window_t *w, uint32_t flags, cco_event_log_t **out) {
-  if (flags & ~(uint32_t)CCO_LOG_KEEP_HISTORY) return set_error(CCO_E_INVALID_ARG, "unknown flags 0x%x", (unsigned)flags);
+  if (flags & ~(uint32_t)(CCO_LOG_KEEP_HISTORY | CCO_LOG_EXTENDABLE)) return set_error(CCO_E_INVALID_ARG, "unknown flags 0x%x", (unsigned)flags);
   CKR(cco_event_log_begin_window(ctx, chunk_bytes, w, out));
   (*out)->history = (flags & CCO_LOG_KEEP_HISTORY) != 0;
+  (*out)->extendable = (flags & CCO_LOG_EXTENDABLE) != 0;
   return CCO_OK;
 }
 

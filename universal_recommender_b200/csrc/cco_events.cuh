@@ -13,6 +13,7 @@
 //                                  (item, field), one presence entry per item left without a field, the triples
 //   k_line_len / k_line_gather     streamed reads: the property-event lines of each chunk, kept for the aggregation at finish
 //   k_cat_words / k_cat_entries    streamed reads: the chunks' name-partitioned columns concatenated name-major at finish
+//   k_ext_*                        extendable logs: the retained part re-expired under a later cutoff at each finish
 #pragma once
 
 #include <cuda_runtime.h>
@@ -755,6 +756,72 @@ __global__ void k_win_obj_spans(long long n, const uint32_t *__restrict__ idx, c
 __global__ void k_win_flag_keep(long long n, const uint8_t *__restrict__ flag, uint8_t want, uint32_t *__restrict__ keep) {
   for (long long l = blockIdx.x * (long long)blockDim.x + threadIdx.x; l < n; l += (long long)gridDim.x * blockDim.x)
     keep[l] = (flag[l] & want) ? 1u : 0u;
+}
+
+// ---- extendable logs (CCO_LOG_EXTENDABLE, cco_event_log_extend) ------------------------------------------------------------
+// A finished extendable log keeps one WinRec per retained line (without removeDuplicates its hash is 0), the global line of
+// every training and ranking entry and the retained property-event lines.  At each finish:
+//   k_ext_line_recs      per chunk, without removeDuplicates: the WinRec of every retained line (time, line, name, selection)
+//   k_ext_expire         the records at or before the cutoff whose name is not exempt ($set / $unset) expire: their lines go
+//                        into the drop bitmap, counted per selection; the rest are kept
+//   k_ext_gather_rec     the kept records, in line order
+//   k_ext_expire_times   the eventTimes of earlier duplicate drops (exempt names excluded) at or before the cutoff: a whole
+//                        read under this cutoff calls those lines expired
+//   k_ext_dup_split      after k_win_mark: the records whose line it dropped leave, and the times of the non-exempt ones stay
+//                        for k_ext_expire_times
+__global__ void k_ext_line_recs(long long R, const uint32_t *__restrict__ ridx, long long line_base, const long long *__restrict__ tm,
+                                const uint8_t *__restrict__ flag, const int32_t *__restrict__ code, WinRec *__restrict__ rec) {
+  for (long long r = blockIdx.x * (long long)blockDim.x + threadIdx.x; r < R; r += (long long)gridDim.x * blockDim.x) {
+    const long long l = ridx[r];
+    rec[r] = WinRec{0, 0, tm[l], line_base + l, code[l], flag[l]};
+  }
+}
+// cnt[0] += expired records, cnt[1] += of them property events, cnt[2] += ignored lines
+__global__ void k_ext_expire(long long N, const WinRec *__restrict__ rec, long long cutoff, const uint8_t *__restrict__ exempt,
+                             uint32_t *__restrict__ bitmap, uint32_t *__restrict__ keep, unsigned long long *__restrict__ cnt) {
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long base = blockIdx.x * (long long)blockDim.x; base < N; base += stride) {
+    const long long i = base + threadIdx.x;
+    bool x = false;
+    if (i < N) {
+      const WinRec &r = rec[i];
+      x = r.time <= cutoff && !exempt[r.code];
+      keep[i] = x ? 0u : 1u;
+      if (x) {
+        atomicOr(&bitmap[r.line >> 5], 1u << (r.line & 31));
+        if (r.flag & kEvProperty) atomicAdd(&cnt[1], 1ULL);
+        if (!r.flag) atomicAdd(&cnt[2], 1ULL);
+      }
+    }
+    const unsigned m = __ballot_sync(0xffffffffu, x);
+    if ((threadIdx.x & 31) == 0 && m) atomicAdd(&cnt[0], (unsigned long long)__popc(m));
+  }
+}
+__global__ void k_ext_gather_rec(long long n, const uint32_t *__restrict__ idx, const WinRec *__restrict__ src, WinRec *__restrict__ dst) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) dst[i] = src[idx[i]];
+}
+// keep[i] = time[i] > cutoff; *n_out += the others
+__global__ void k_ext_expire_times(long long n, const long long *__restrict__ time, long long cutoff, uint32_t *__restrict__ keep,
+                                   unsigned long long *__restrict__ n_out) {
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long base = blockIdx.x * (long long)blockDim.x; base < n; base += stride) {
+    const long long i = base + threadIdx.x;
+    const bool x = i < n && time[i] <= cutoff;
+    if (i < n) keep[i] = x ? 0u : 1u;
+    const unsigned m = __ballot_sync(0xffffffffu, x);
+    if ((threadIdx.x & 31) == 0 && m) atomicAdd(n_out, (unsigned long long)__popc(m));
+  }
+}
+// keep[i] = record i's line survived k_win_mark; dup[i] = it did not and its name is not exempt; time[i] its eventTime
+__global__ void k_ext_dup_split(long long N, const WinRec *__restrict__ rec, const uint32_t *__restrict__ bitmap, const uint8_t *__restrict__ exempt,
+                                uint32_t *__restrict__ keep, uint32_t *__restrict__ dup, long long *__restrict__ time) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < N; i += (long long)gridDim.x * blockDim.x) {
+    const WinRec &r = rec[i];
+    const bool d = win_dropped(bitmap, r.line);
+    keep[i] = d ? 0u : 1u;
+    dup[i] = d && !exempt[r.code] ? 1u : 0u;
+    time[i] = r.time;
+  }
 }
 
 }  // namespace cco

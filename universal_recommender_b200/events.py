@@ -282,6 +282,60 @@ def clean_events(events: Sequence[Event], window: Optional[EventWindow], now_ms:
     return out, expired, len(kept) - len(out)
 
 
+@dataclass
+class KeptEvents:
+    """what an extendable log keeps of the lines read so far (CcoContext.read_events(extendable=True)): the events the window
+    kept, the drop counts, and the eventTimes of the events removeDuplicates dropped that are neither $set nor $unset (a
+    later cutoff turns those into expired events).  cutoff: the window's, None when nothing expires."""
+    events: list = field(default_factory=list)
+    n_expired: int = 0
+    n_duplicates: int = 0
+    dup_times: list = field(default_factory=list)
+    cutoff: Optional[int] = None
+    remove_duplicates: Optional[bool] = None   # None: nothing read yet
+
+
+def extend_clean(kept: KeptEvents, new_events: Sequence[Event], window: Optional[EventWindow], now_ms: Optional[int]) -> KeptEvents:
+    """the mirror of EventLog.extend: kept (the state after events A under an earlier window) with the events B that follow
+    them (lines numbered after A's) under `window`.  The contract: extend_clean(clean_kept(A, w1), B, w2) gives the events
+    and counts of clean_events(A + B, w2) whenever w2's cutoff is at or after w1's and removeDuplicates is the same.  It
+    holds because an event dropped under the earlier cutoff is dropped under the later one: among equal events the kept
+    one is the latest, so when it expires all of them have, and a duplicate drop at or before the new cutoff is an expired
+    event of the whole read.  A cutoff before kept.cutoff raises: the events it would bring back are gone."""
+    cutoff = window.cutoff_ms(now_ms) if window is not None and window.duration is not None else None
+    if kept.cutoff is not None and (cutoff is None or cutoff < kept.cutoff):
+        raise ValueError("the cutoff cannot move back: the events it expired are gone")
+    dedup = window is not None and window.removeDuplicates
+    if kept.remove_duplicates is not None and dedup != kept.remove_duplicates:
+        raise ValueError("removeDuplicates cannot change between reads")
+    exempt = lambda e: e.event in ("$set", "$unset")
+    gone = lambda t: cutoff is not None and t <= cutoff
+    old = [e for e in kept.events if exempt(e) or not gone(e.time_ms)]
+    new = [e for e in new_events if exempt(e) or not gone(e.time_ms)]
+    moved = sum(1 for t in kept.dup_times if gone(t))
+    n_expired = kept.n_expired + (len(kept.events) - len(old)) + (len(new_events) - len(new)) + moved
+    n_dup = kept.n_duplicates - moved
+    dup_times = [t for t in kept.dup_times if not gone(t)]
+    out = old + new
+    if dedup:
+        best: dict = {}
+        for e in out:
+            k = event_identity(e)
+            if k not in best or (e.time_ms, e.line) > (best[k].time_ms, best[k].line):
+                best[k] = e
+        stay = {id(e) for e in best.values()}
+        dropped = [e for e in out if id(e) not in stay]
+        n_dup += len(dropped)
+        dup_times += [e.time_ms for e in dropped if not exempt(e)]
+        out = [e for e in out if id(e) in stay]
+    return KeptEvents(out, n_expired, n_dup, dup_times, cutoff, dedup)
+
+
+def clean_kept(events: Sequence[Event], window: Optional[EventWindow], now_ms: Optional[int]) -> KeptEvents:
+    """clean_events as the state an extendable log keeps: the extend of nothing"""
+    return extend_clean(KeptEvents(), events, window, now_ms)
+
+
 def export_parts(directory) -> list[str]:
     """the part files of a `pio export` directory (Spark's saveAsTextFile: part-NNNNN files and a _SUCCESS marker) in name
     order; _SUCCESS, checksum (*.crc) and hidden files and empty parts are skipped"""

@@ -25,16 +25,25 @@ from .indexed_dataset import IndexedDataset
 DEFAULT_CHUNK_BYTES = 1 << 28
 
 
-def _name_part(e: Exception, paths) -> None:
-    """add the part file and its 0-based line to the message of a parse error of a multi-part read (counted only here)"""
+def _name_part(e: Exception, paths, line_base: int = 0) -> None:
+    """add the part file and its 0-based line to the message of a parse error of a multi-part read (counted only here);
+    line_base: the lines the log held before these parts"""
     m = re.search(r"line (\d+)", str(e))
     if m is None or len(paths) < 2:
         return
     try:
-        k, line = E.locate_line([E.part_lines(p) for p in paths], int(m.group(1)))
+        k, line = E.locate_line([E.part_lines(p) for p in paths], int(m.group(1)) - line_base)
     except (OSError, ValueError):
         return
     e.args = (f"{e.args[0]} (part {paths[k]}, line {line})",)
+
+
+def _window_t(window: Optional[E.EventWindow], now_ms: Optional[int]):
+    """EventWindow + now (the wall clock by default) -> cco_event_window_t, None without a window"""
+    if window is None:
+        return None
+    cutoff = window.cutoff_ms(now_ms if now_ms is not None else int(time.time() * 1000))
+    return N.EventWindowT(-(1 << 63) if cutoff is None else cutoff, 1 if window.removeDuplicates else 0, 0)
 
 
 @dataclass
@@ -351,7 +360,7 @@ class CcoContext:
         return rk
 
     def read_events(self, src, chunk_bytes: Optional[int] = None, window: Optional[E.EventWindow] = None,
-                    now_ms: Optional[int] = None, keep_history: bool = False) -> "EventLog":
+                    now_ms: Optional[int] = None, keep_history: bool = False, extendable: bool = False) -> "EventLog":
         """A PredictionIO event export (JSON lines, as `pio export` writes them) parsed on the device.  src is one of
           - bytes or a buffer: one read (cco_event_log_read), or chunks of chunk_bytes when it is given;
           - a file path, a directory as `pio export` writes it (its part-* files in name order; events.export_parts) or a
@@ -366,57 +375,60 @@ class CcoContext:
         equal events collapse to the latest.  now_ms defaults to the wall clock; EventLog.window_stats() counts the drops.
         keep_history: keep every training event's time and line (cco_event_log_begin_ex, CCO_LOG_KEEP_HISTORY), which
         user_queries reads; a log read without it is exactly the log read before the option existed.
+        extendable: keep what EventLog.extend needs to take new lines and a later cutoff without a re-read
+        (cco_event_log_begin_ex, CCO_LOG_EXTENDABLE); the device staging of later extends is this read's chunk_bytes.
         -> EventLog (free with .free(), or use it as a context manager; close() of this context frees the logs still open)."""
         whole = isinstance(src, (bytes, bytearray, memoryview, np.ndarray)) and chunk_bytes is None
-        if whole and window is None and not keep_history:
+        if whole and window is None and not keep_history and not extendable:
             buf = np.frombuffer(src, dtype=np.uint8) if not isinstance(src, np.ndarray) else np.ascontiguousarray(src, dtype=np.uint8)
             h = C.c_void_p()
             N.check(self._L.cco_event_log_read(self._h, buf.ctypes.data if len(buf) else None, len(buf), C.byref(h)))
             return self._adopt_log(h)
         chunk = int(chunk_bytes or (max(memoryview(src).nbytes, 1) if whole else DEFAULT_CHUNK_BYTES))
+        h = C.c_void_p()
+        w = _window_t(window, now_ms)
+        flags = (N.LOG_KEEP_HISTORY if keep_history else 0) | (N.LOG_EXTENDABLE if extendable else 0)
+        if flags:
+            N.check(self._L.cco_event_log_begin_ex(self._h, chunk, C.byref(w) if w is not None else None, flags, C.byref(h)))
+        elif w is None:
+            N.check(self._L.cco_event_log_begin(self._h, chunk, C.byref(h)))
+        else:
+            N.check(self._L.cco_event_log_begin_window(self._h, chunk, C.byref(w), C.byref(h)))
+        try:
+            self._append_finish(h, src, chunk)
+        except BaseException:
+            self._L.cco_event_log_free(h)
+            raise
+        return self._adopt_log(h)
+
+    def _append_finish(self, h, src, chunk: int, line_base: int = 0):
+        """append every byte of a read_events source to an open log (holding line_base lines), then finish it"""
         paths = None
         if isinstance(src, (str, os.PathLike)):
             p = os.fspath(src)
             paths = E.export_parts(p) if os.path.isdir(p) else [p]
         elif isinstance(src, (list, tuple)) and all(isinstance(x, (str, os.PathLike)) for x in src):
             paths = [os.fspath(x) for x in src]
-        h = C.c_void_p()
-        w = None
-        if window is not None:
-            now = now_ms if now_ms is not None else int(time.time() * 1000)
-            cutoff = window.cutoff_ms(now)
-            w = N.EventWindowT(-(1 << 63) if cutoff is None else cutoff, 1 if window.removeDuplicates else 0, 0)
-        if keep_history:
-            N.check(self._L.cco_event_log_begin_ex(self._h, chunk, C.byref(w) if w is not None else None, N.LOG_KEEP_HISTORY, C.byref(h)))
-        elif w is None:
-            N.check(self._L.cco_event_log_begin(self._h, chunk, C.byref(h)))
+        if paths is not None:
+            self._append_files(h, paths, chunk, line_base)
         else:
-            N.check(self._L.cco_event_log_begin_window(self._h, chunk, C.byref(w), C.byref(h)))
+            for b in ([src] if isinstance(src, (bytes, bytearray, memoryview, np.ndarray)) else src):
+                buf = np.frombuffer(b, dtype=np.uint8) if not isinstance(b, np.ndarray) else np.ascontiguousarray(b, dtype=np.uint8)
+                if len(buf):
+                    N.check(self._L.cco_event_log_append(h, buf.ctypes.data, len(buf)))
         try:
+            N.check(self._L.cco_event_log_finish(h))
+        except N.CcoError as e:
             if paths is not None:
-                self._append_files(h, paths, chunk)
-            else:
-                for b in ([src] if isinstance(src, (bytes, bytearray, memoryview, np.ndarray)) else src):
-                    buf = np.frombuffer(b, dtype=np.uint8) if not isinstance(b, np.ndarray) else np.ascontiguousarray(b, dtype=np.uint8)
-                    if len(buf):
-                        N.check(self._L.cco_event_log_append(h, buf.ctypes.data, len(buf)))
-            try:
-                N.check(self._L.cco_event_log_finish(h))
-            except N.CcoError as e:
-                if paths is not None:
-                    _name_part(e, paths)
-                raise
-        except BaseException:
-            self._L.cco_event_log_free(h)
+                _name_part(e, paths, line_base)
             raise
-        return self._adopt_log(h)
 
     def _adopt_log(self, h) -> "EventLog":
         log = EventLog(self, h, None)
         self._logs.add(log)
         return log
 
-    def _append_files(self, h, paths, chunk: int):
+    def _append_files(self, h, paths, chunk: int, line_base: int = 0):
         """append the files in order through two pinned buffers: a reader thread fills one while the other is appended
         (readinto and the ctypes call both release the GIL)"""
         bufs = [self.host_array(chunk, np.uint8) for _ in range(2)]
@@ -461,7 +473,7 @@ class CcoContext:
                     else:
                         N.check(self._L.cco_event_log_append(h, bufs[k].ctypes.data, n))
                 except N.CcoError as e:
-                    _name_part(e, paths)
+                    _name_part(e, paths, line_base)
                     raise
                 if k >= 0:
                     free.put(k)
@@ -1303,6 +1315,27 @@ class EventLog:
         x, d = C.c_int64(), C.c_int64()
         N.check(self._ctx._L.cco_event_log_window_stats(self._h, C.byref(x), C.byref(d)))
         return x.value, d.value
+
+    def extend(self, src, window: Optional[E.EventWindow] = None, now_ms: Optional[int] = None,
+               chunk_bytes: Optional[int] = None) -> "EventLog":
+        """cco_event_log_extend: the newest lines of the export and a later cutoff, without reading the rest again.  The log
+        (read with extendable=True) becomes the one read_events gives for its bytes followed by src's under `window`: src's
+        first byte starts a line, and its lines are numbered after the log's.  src: any source read_events takes; window:
+        events.EventWindow, its cutoff counted back from now_ms (the wall clock by default), None keeps the current window.
+        The cutoff may not move back and removeDuplicates may not change.  chunk_bytes: the host blocks of file sources
+        (DEFAULT_CHUNK_BYTES); the device staging stays the read's.  A failed extend fails the log, which must then be freed.
+        -> self"""
+        w = _window_t(window, now_ms)
+        n_lines = self._info().n_lines
+        N.check(self._ctx._L.cco_event_log_extend(self._h, C.byref(w) if w is not None else None))
+        self._ctx._append_finish(self._h, src, int(chunk_bytes or DEFAULT_CHUNK_BYTES), n_lines)
+        return self
+
+    def resident_bytes(self) -> int:
+        """cco_event_log_resident_bytes: the device bytes the finished log holds"""
+        b = C.c_int64()
+        N.check(self._ctx._L.cco_event_log_resident_bytes(self._h, C.byref(b)))
+        return b.value
 
     def free(self):
         if getattr(self, "_h", None):
