@@ -1020,6 +1020,66 @@ int cco_index_write_finish(cco_index_write_t *h, cco_index_write_out_t *out);
 int cco_index_write_free(cco_index_write_t *h);
 
 /*
+ * Item properties refreshed in the live model index without a retrain: a `$set`, `$unset` or `$delete` reaches the
+ * documents in place, and only the documents it changes are written again.  This is not calcPop (cco_rerank_model keeps
+ * the reference's precedence, where an old member beats a fresh property); here the fresh properties win, and rankings and
+ * correlators are never recomputed.
+ * Inputs: the current index as a bulk body, with cco_rerank_model's grammar, checks and messages (a repeated _id is an
+ * error); params: the correlator names (the model's event names) and the computed ranking names (the fields of the
+ * popular, trending, hot and random rankings; a userDefined ranking's field is an ordinary property); the fresh
+ * properties as (item, field, value) triples (cco_item_properties_t, as cco_format_model takes them), or a finished event
+ * log's aggregated properties (cco_refresh_properties_log).
+ * The rule, one document at a time.  An old document with id x is rewritten as
+ *   {"index":{"_id":"<x>"}}\n{"id":"<x>"[,<correlator member>]*[,"<field>":<value>]*[,<ranking member>]*}\n
+ *  1. "id" and x as cco_rerank_model writes them (the decoded _id, escaped as every id);
+ *  2. its members named like a correlator, verbatim and in order;
+ *  3. x's fresh properties by cco_format_model's rules: field index order, the last triple of an (item, field) wins, field
+ *     "id" only marks that the item exists, and a field named like a computed ranking is not written;
+ *  4. its members named like a computed ranking, verbatim and in order.
+ * Every other old member is an old property and is dropped.  "id" and a member followed by a member of the same name are
+ * skipped (json4s keeps the last).  A property field named like a correlator is CCO_E_UNSUPPORTED, naming the field:
+ * cco_format_model would let it replace the correlator array, and a refresh has no array to put back.
+ * Each document is then one of
+ *  - deleted: the item has no triple and its rewritten document has no member besides "id" (cco_format_model would not
+ *    write it);
+ *  - changed: its rewritten source line differs from the old one byte for byte;
+ *  - new: an item with a triple and no old document, written as cco_format_model writes a property-only item, in order of
+ *    first appearance among the triples;
+ *  - unchanged: everything else.
+ * Outputs: body = the refreshed full index (the old documents in order without the deleted ones, then the new ones), which
+ * the caller keeps for the next refresh, calcPop and item queries; delta = the changed and new documents, in the body's
+ * order, which cco_index_write_begin takes; deletes = one {"delete":{"_id":"<id>"}} line per deleted document, the id
+ * escaped as every id; changed / deleted = the old document numbers (0-based, ascending).  With params and properties
+ * that made the body (the same triples cco_format_model was given, no random ranking), body is the input byte for byte
+ * and delta and deletes are empty.  A new item gets no random (uniqueRank) value until the next calcPop.
+ * Errors: those of cco_rerank_model on the body and of cco_format_model on the properties; CCO_E_INVALID_ARG for null
+ * name arrays or names; CCO_E_UNSUPPORTED for a property named like a correlator, group contexts and documents + triples
+ * >= 2^31.  Every pointer the out-structure receives is pinned memory of the context, released with cco_host_free.
+ */
+typedef struct {
+  int32_t n_correlators;
+  const char *const *correlators;   /* [n_correlators] NUL-terminated UTF-8 */
+  int32_t n_rankings;
+  const char *const *rankings;      /* [n_rankings] */
+} cco_refresh_params_t;
+typedef struct {
+  int64_t n_docs;                   /* documents of body */
+  int64_t n_changed, n_new, n_deleted, n_unchanged;
+  char *body;
+  int64_t body_len;
+  char *delta;
+  int64_t delta_len;
+  char *deletes;
+  int64_t deletes_len;
+  int64_t *changed;                 /* [n_changed] */
+  int64_t *deleted;                 /* [n_deleted] */
+} cco_refresh_out_t;
+int cco_refresh_properties(cco_ctx_t *ctx, const char *body, int64_t body_len, const cco_item_properties_t *props /* nullable */,
+                           const cco_refresh_params_t *params, cco_refresh_out_t *out);
+int cco_refresh_properties_log(cco_ctx_t *ctx, const char *body, int64_t body_len, const cco_event_log_t *log,
+                               const cco_refresh_params_t *params, cco_refresh_out_t *out);
+
+/*
  * Debug/parity entry (tests only): full integer co-occurrence matrix A^T B of two canonical
  * binary matrices computed by the same accumulation kernel as cco_train, no LLR, no top-k.
  * Output CSR over the columns of A with ascending column ids, malloc'ed; free with cco_free.

@@ -27,6 +27,10 @@ Host-side mirror of the reference interface for this path:
   ur_algorithm.write_index                <- URModel.save -> EsClient.hotSwap: the mapping, bounded _bulk requests, their
                                              responses read on the GPU (cco_index_write_*), 429 retries and the alias swap,
                                              over a caller-supplied request function; ur_model.index_mapping / alias_actions
+  ur_algorithm.refresh_properties_from_events / update_index  <- item properties ($set / $unset / $delete) written into
+                                             the live index in place, without a retrain: the changed documents built on the
+                                             GPU (cco_refresh_properties), then _bulk index and delete requests;
+                                             ur_model.refresh_documents
   ur_model                                <- propertiesRDD, getRanksRDD, groupAll (URAlgorithm.scala:351-369, 537-560;
                                              URModel.scala:57-140): the host mirror of the model documents
 """
@@ -39,15 +43,16 @@ from .similarity_analysis import (CcoContext, DownsamplableCrossOccurrenceDatase
                                   decode_ids, default_context, encode_ids)
 from .ur_algorithm import (DefaultURAlgoParams, IndicatorParams, URAlgorithmParams, calc_all, calc_all_from_events, calc_all_on_device,
                            batchpredict_output, calc_pop_from_events, calc_pop_on_device, index_from_pages, IndexWriteError, write_index, item_queries, item_set_queries, mixed_queries_from_events,
-                           predictions_from_responses, queries_from_file, user_queries_from_events)
+                           predictions_from_responses, queries_from_file, refresh_properties_from_events, refresh_properties_on_device,
+                           update_index, user_queries_from_events)
 from .ur_query import ItemQuery, ItemSetQuery, MixedQuery, UserQuery
-from .ur_model import RankingParams
+from .ur_model import RankingParams, RefreshedIndex
 
 __all__ = [
     "BiDictionary", "CcoContext", "CcoError", "CcoInvalidArgument", "DataSourceParams", "DefaultURAlgoParams", "EventWindow",
     "DownsamplableCrossOccurrenceDataset", "IndexedDataset", "IndicatorParams", "SimilarityAnalysis",
     "EventLog", "RankingParams", "URAlgorithmParams", "calc_all", "calc_all_from_events", "calc_all_on_device", "calc_pop_from_events",
-    "batchpredict_output", "calc_pop_on_device", "item_queries", "item_set_queries", "mixed_queries_from_events", "predictions_from_responses", "queries_from_file", "SearchResults", "IndexPages", "index_from_pages", "IndexWrite", "IndexWriteResult", "IndexWriteError", "write_index", "user_queries_from_events", "ItemQuery", "ItemSetQuery", "MixedQuery", "UserQuery", "decode_ids", "default_context", "encode_ids", "prepare", "prepare_on_device",
+    "batchpredict_output", "calc_pop_on_device", "item_queries", "item_set_queries", "mixed_queries_from_events", "predictions_from_responses", "queries_from_file", "SearchResults", "IndexPages", "index_from_pages", "IndexWrite", "IndexWriteResult", "IndexWriteError", "write_index", "refresh_properties_from_events", "refresh_properties_on_device", "update_index", "RefreshedIndex", "user_queries_from_events", "ItemQuery", "ItemSetQuery", "MixedQuery", "UserQuery", "decode_ids", "default_context", "encode_ids", "prepare", "prepare_on_device",
     "FLAG_ASSUME_CANONICAL",
     "FLAG_ENTROPY_VARARGS", "FLAG_KEY_RANGES", "FLAG_ROWRATE_INTDIV", "FLAG_RESULT_NO_COUNT", "FLAG_RESULT_NO_LLR", "LIB_PATH",
 ]

@@ -164,6 +164,18 @@ class IndexWriteOutT(C.Structure):
                 ("reason_bytes", C.c_void_p)]
 
 
+class RefreshParamsT(C.Structure):
+    _fields_ = [("n_correlators", C.c_int32), ("correlators", C.POINTER(C.c_char_p)), ("n_rankings", C.c_int32),
+                ("rankings", C.POINTER(C.c_char_p))]
+
+
+class RefreshOutT(C.Structure):
+    _fields_ = [("n_docs", C.c_int64), ("n_changed", C.c_int64), ("n_new", C.c_int64), ("n_deleted", C.c_int64),
+                ("n_unchanged", C.c_int64), ("body", C.c_void_p), ("body_len", C.c_int64), ("delta", C.c_void_p),
+                ("delta_len", C.c_int64), ("deletes", C.c_void_p), ("deletes_len", C.c_int64),
+                ("changed", C.POINTER(C.c_int64)), ("deleted", C.POINTER(C.c_int64))]
+
+
 SR_WITH_RANKS = 1
 SR_TEXT = 2
 SR_BATCHPREDICT = 4
@@ -193,7 +205,7 @@ EXPORTS = [
     "cco_format_model", "cco_rerank_model", "cco_event_log_read", "cco_event_log_info", "cco_event_log_ingest",
     "cco_format_model_log", "cco_rerank_model_log", "cco_event_log_free", "cco_event_log_begin", "cco_event_log_append",
     "cco_event_log_finish", "cco_event_log_begin_window", "cco_event_log_window_stats",
-    "cco_event_log_begin_ex", "cco_event_log_extend", "cco_event_log_resident_bytes", "cco_event_log_user_queries", "cco_item_queries", "cco_item_set_queries", "cco_mixed_queries", "cco_query_file_read", "cco_query_file_templates", "cco_query_file_queries", "cco_query_file_free", "cco_search_results_begin", "cco_search_results_append", "cco_search_results_finish", "cco_search_results_free", "cco_index_pages_begin", "cco_index_pages_append", "cco_index_pages_finish", "cco_index_pages_free", "cco_index_write_begin", "cco_index_write_fields", "cco_index_write_requests", "cco_index_write_response", "cco_index_write_retry", "cco_index_write_finish", "cco_index_write_free", "cco_result_num_matrices", "cco_result_row_range", "cco_result_matrix", "cco_result_stats", "cco_result_key_ranges", "cco_result_free",
+    "cco_event_log_begin_ex", "cco_event_log_extend", "cco_event_log_resident_bytes", "cco_event_log_user_queries", "cco_item_queries", "cco_item_set_queries", "cco_mixed_queries", "cco_query_file_read", "cco_query_file_templates", "cco_query_file_queries", "cco_query_file_free", "cco_search_results_begin", "cco_search_results_append", "cco_search_results_finish", "cco_search_results_free", "cco_index_pages_begin", "cco_index_pages_append", "cco_index_pages_finish", "cco_index_pages_free", "cco_index_write_begin", "cco_index_write_fields", "cco_index_write_requests", "cco_index_write_response", "cco_index_write_retry", "cco_index_write_finish", "cco_index_write_free", "cco_refresh_properties", "cco_refresh_properties_log", "cco_result_num_matrices", "cco_result_row_range", "cco_result_matrix", "cco_result_stats", "cco_result_key_ranges", "cco_result_free",
     "cco_debug_cooccurrence", "cco_debug_key_range_cap", "cco_debug_downsample", "cco_debug_downsample_block", "cco_debug_llr", "cco_debug_string_ids", "cco_debug_rank_text", "cco_free",
 ]
 
@@ -284,6 +296,8 @@ def lib():
     L.cco_index_write_retry.argtypes = [C.c_void_p, p(IndexWriteRetryT)]
     L.cco_index_write_finish.argtypes = [C.c_void_p, p(IndexWriteOutT)]
     L.cco_index_write_free.argtypes = [C.c_void_p]
+    L.cco_refresh_properties.argtypes = [C.c_void_p, C.c_char_p, C.c_int64, p(ItemPropertiesT), p(RefreshParamsT), p(RefreshOutT)]
+    L.cco_refresh_properties_log.argtypes = [C.c_void_p, C.c_char_p, C.c_int64, C.c_void_p, p(RefreshParamsT), p(RefreshOutT)]
     L.cco_mixed_queries.argtypes = [C.c_void_p, C.c_void_p, C.c_char_p, C.c_int64, p(MixedQueryT), C.c_int64,
                                     p(C.c_int64), C.c_void_p, C.c_void_p, p(C.c_int64), C.c_void_p, C.c_void_p,
                                     p(C.c_int64), C.c_int64, p(C.c_int64), C.c_void_p, C.c_void_p,

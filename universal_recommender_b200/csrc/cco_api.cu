@@ -34,6 +34,7 @@
 #include "cco_results.cuh"
 #include "cco_index_pages.cuh"
 #include "cco_index_write.cuh"
+#include "cco_refresh.cuh"
 
 namespace cco {
 
@@ -5252,6 +5253,238 @@ int cco_rerank_model_log(cco_ctx_t *ctx, const char *body, int64_t body_len, con
   const bool any = lg->n_triples > 0;
   return rerank_model(ctx, body, body_len, any ? &lp.shell : nullptr, n_rankings, rk.data(), out_bytes, out_len, std::move(ls),
                       any ? &lp.dev : nullptr);
+}
+
+// ---- cco_refresh_properties: fresh item properties written into the old documents, kernels in cco_refresh.cuh ----------
+namespace cco {
+static int refresh_names(int32_t n, const char *const *names, const char *what) {
+  if (n < 0 || (n > 0 && !names)) return set_error(CCO_E_INVALID_ARG, "bad %s names", what);
+  for (int k = 0; k < n; ++k)
+    if (!names[k]) return set_error(CCO_E_INVALID_ARG, "%s name %d is null", what, k);
+  return CCO_OK;
+}
+// the outputs into pinned memory of c, one device-to-host copy each, then one wait; on failure every buffer goes back
+static int refresh_to_host(cco_ctx *c, const unsigned char *const src[5], const long long bytes[5], void *dst[5]) {
+  cudaStream_t s = c->stream;
+  for (int k = 0; k < 5; ++k) dst[k] = nullptr;
+  const int st = [&]() -> int {
+    for (int k = 0; k < 5; ++k) {
+      dst[k] = c->pinned_get((size_t)std::max<long long>(bytes[k], 1), /*for_result=*/false);
+      if (!dst[k]) return set_error(CCO_E_OOM, "pinned host allocation failed");
+      if (bytes[k] > 0) CK(cudaMemcpyAsync(dst[k], src[k], (size_t)bytes[k], cudaMemcpyDeviceToHost, s));
+    }
+    CK(cudaStreamSynchronize(s));
+    CK(cudaGetLastError());
+    return CCO_OK;
+  }();
+  if (st != CCO_OK)
+    for (int k = 0; k < 5; ++k)
+      if (dst[k]) c->pinned_put(dst[k]);
+  return st;
+}
+
+static int refresh_properties(cco_ctx_t *ctx, const char *body, int64_t body_len, const cco_item_properties_t *props,
+                              const cco_refresh_params_t *prm, cco_refresh_out_t *out, const DevProps *dp = nullptr) {
+  if (!ctx || !prm || !out || body_len < 0 || (body_len > 0 && !body)) return set_error(CCO_E_INVALID_ARG, "null argument or negative length");
+  memset(out, 0, sizeof *out);
+  if (!ctx->members.empty()) return set_error(CCO_E_UNSUPPORTED, "per-GPU contexts only");
+  if (body_len > 0 && body[body_len - 1] != '\n') return set_error(CCO_E_INVALID_ARG, "the body does not end in a newline");
+  CKR(refresh_names(prm->n_correlators, prm->correlators, "correlator"));
+  CKR(refresh_names(prm->n_rankings, prm->rankings, "ranking"));
+  const cco_dictionary_t no_rows = {0, nullptr, nullptr};
+  Streams st;
+  CKR(model_check_host(&no_rows, props, 0, nullptr, &st, dp != nullptr));
+  const int n_fields = props ? props->n_fields : 0;
+  for (int f = 0; f < n_fields; ++f)   // cco_format_model would let it replace the array; a refresh has none to put back
+    for (int i = 0; i < prm->n_correlators; ++i)
+      if (!strcmp(props->field_names[f], prm->correlators[i]))
+        return set_error(CCO_E_UNSUPPORTED, "property field \"%s\" is named like a correlator: a refresh keeps the correlator arrays",
+                         props->field_names[f]);
+  cco_ctx *c = ctx;
+  CK(cudaSetDevice(c->device));
+  cudaStream_t s = c->stream;
+  Arena ar(s);
+  NvtxRange nvtx("cco:refresh_properties");
+  mail_reset(c);
+  // 1. the old documents: members, decoded names and _ids (cco_rerank_model's grammar and checks)
+  BulkDocs bd;
+  CKR(bulk_parse(c, ar, body, body_len, props ? props->n : 0, "property triples", &bd));
+  const long long D = bd.D, M1 = bd.M1;
+  // 2. join: the decoded ids are the row section of the key column, the properties sorted per item as cco_format_model
+  FormatArgs fa;
+  memset(&fa, 0, sizeof fa);
+  CKR(model_names(c, ar, &fa, 0, nullptr, true, props, 0, nullptr));
+  fa.n_rows = (int32_t)D;
+  const DevDict raw_ids = {bd.ids.off, (const unsigned char *)bd.ids.w, D};
+  CKR(escape_dict(c, ar, raw_ids, &fa.row_ids));
+  const KeySection rows{D, (const int64_t *)bd.ids.off, (const char *)bd.ids.w, true, bd.ids_bytes};
+  CKR(model_fields(c, ar, &fa, rows, props, 0, nullptr, st, true, true, dp));
+  // a field named "id" or like a computed ranking is not written (kClashId: prop_written skips it)
+  std::vector<uint16_t> fclash(std::max(n_fields, 1), 0);
+  for (int f = 0; f < n_fields; ++f) {
+    if (!strcmp(props->field_names[f], "id")) fclash[f] = kClashId;
+    for (int k = 0; k < prm->n_rankings; ++k)
+      if (!strcmp(props->field_names[f], prm->rankings[k])) fclash[f] = kClashId;
+  }
+  uint16_t *d_fclash;
+  CKR(ar.alloc(&d_fclash, fclash.size()));
+  CK(cudaMemcpyAsync(d_fclash, fclash.data(), sizeof(uint16_t) * fclash.size(), cudaMemcpyHostToDevice, s));
+  fa.field_clash = d_fclash;
+  // 3. member names -> correlator, computed ranking or other; "id" and members followed by one of the same name are skipped
+  RefreshArgs ra;
+  memset(&ra, 0, sizeof ra);
+  ra.body = bd.body;
+  ra.line_moff = bd.line_moff;
+  ra.mem = bd.mem;
+  ra.line_b = bd.line_b;
+  ra.body_len = body_len;
+  std::vector<std::string> ent;
+  std::vector<uint8_t> ent_cls, ent_id;
+  auto entry = [&](const char *nm, uint8_t cls, uint8_t id) {
+    for (size_t t = 0; t < ent.size(); ++t)
+      if (ent[t] == nm) return;
+    ent.push_back(nm);
+    ent_cls.push_back(cls);
+    ent_id.push_back(id);
+  };
+  entry("id", kRefreshOther, 1);
+  for (int i = 0; i < prm->n_correlators; ++i) entry(prm->correlators[i], kRefreshCorrelator, 0);
+  for (int k = 0; k < prm->n_rankings; ++k) entry(prm->rankings[k], kRefreshRanking, 0);
+  if (D > 0) {
+    const int T = (int)ent.size();
+    int32_t *ngid, *entry_of, *ment;
+    uint8_t *d_cls, *d_id, *mkeep;
+    CKR(ar.alloc(&d_cls, T));
+    CKR(ar.alloc(&d_id, T));
+    CK(cudaMemcpyAsync(d_cls, ent_cls.data(), T, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(d_id, ent_id.data(), T, cudaMemcpyHostToDevice, s));
+    CKR(member_entries(c, ar, bd.names, ent, &ngid, &entry_of));   // its wait for the upload also covers these local tables
+    CKR(ar.alloc(&ment, std::max<long long>(M1, 1)));
+    CKR(ar.alloc(&mkeep, std::max<long long>(M1, 1)));
+    k_member_info<<<grid_for(D * 32, 256, c->sm_count), 256, 0, s>>>(D, ra.line_moff, ngid, entry_of, d_id, ment, mkeep);
+    c->launches++;
+    ra.ment = ment;
+    ra.mkeep = mkeep;
+    ra.ent_cls = d_cls;
+  }
+  CK(cudaStreamSynchronize(s));   // fclash, ent_cls and ent_id are locals
+  // 4. the refreshed body: the old documents rewritten (deleted ones: 0 bytes), then the new items as cco_format_model writes them
+  const long long X = fa.n_extra, N = D + X;
+  FormatArgs fx = fa;   // the new items only
+  fx.n_rows = 0;
+  long long *doc_len, *doc_off;
+  CKR(ar.alloc(&doc_len, N + 1));
+  CKR(ar.alloc(&doc_off, N + 1));
+  CK(cudaMemsetAsync(doc_len + N, 0, 8, s));
+  if (D > 0) k_refresh_len<<<grid_for(D * 32, 256, c->sm_count), 256, 0, s>>>(fa, ra, (int32_t)D, doc_len);
+  if (X > 0) k_doc_len<<<grid_for(X, 256, c->sm_count), 256, 0, s>>>(fx, (int32_t)X, doc_len + D);
+  c->launches += (D > 0) + (X > 0);
+  CKR(exclusive_sum(c, ar, doc_len, doc_off, N + 1));
+  long long total = 0;
+  CKR(mail_fetch(c, &total, doc_off + N, 8));
+  CKR(mail_wait(c));
+  unsigned char *d_full;
+  CKR(ar.alloc(&d_full, std::max<long long>(total, 1)));
+  if (D > 0) k_refresh_write<<<grid_for(D * 32, 256, c->sm_count), 256, 0, s>>>(fa, ra, (int32_t)D, doc_off, d_full);
+  if (X > 0) k_doc_write<<<grid_for(X * 32, 256, c->sm_count), 256, 0, s>>>(fx, (int32_t)X, doc_off + D, d_full);
+  c->launches += (D > 0) + (X > 0);
+  // 5. the diff against the old source lines, the delta and deleted lists
+  uint32_t *flag, *fpos, *del, *dpos;
+  CKR(ar.alloc(&flag, N + 1));
+  CKR(ar.alloc(&fpos, N + 1));
+  CKR(ar.alloc(&del, N + 1));
+  CKR(ar.alloc(&dpos, N + 1));
+  CK(cudaMemsetAsync(flag, 0, sizeof(uint32_t) * (size_t)(N + 1), s));
+  CK(cudaMemsetAsync(del, 0, sizeof(uint32_t) * (size_t)(N + 1), s));
+  if (N > 0) {
+    k_refresh_diff<<<grid_for(N * 32, 256, c->sm_count), 256, 0, s>>>(fa, ra, (int32_t)D, (int32_t)N, doc_off, d_full, flag, del);
+    c->launches++;
+  }
+  CKR(exclusive_sum(c, ar, flag, fpos, N + 1));
+  CKR(exclusive_sum(c, ar, del, dpos, N + 1));
+  uint32_t n_delta = 0, n_changed = 0, n_deleted = 0;
+  CKR(mail_fetch(c, &n_delta, fpos + N, 4));
+  CKR(mail_fetch(c, &n_changed, fpos + D, 4));
+  CKR(mail_fetch(c, &n_deleted, dpos + N, 4));
+  CKR(mail_wait(c));
+  uint32_t *pick;
+  long long *se, *dlen, *doff, *xlen, *xoff;
+  int64_t *changed, *deleted;
+  CKR(ar.alloc(&pick, std::max<long long>(n_delta, 1)));
+  CKR(ar.alloc(&se, std::max<long long>(N, 1)));
+  CKR(ar.alloc(&changed, std::max<long long>(n_changed, 1)));
+  CKR(ar.alloc(&deleted, std::max<long long>(n_deleted, 1)));
+  CKR(ar.alloc(&dlen, (long long)n_delta + 1));
+  CKR(ar.alloc(&doff, (long long)n_delta + 1));
+  CKR(ar.alloc(&xlen, (long long)n_deleted + 1));
+  CKR(ar.alloc(&xoff, (long long)n_deleted + 1));
+  CK(cudaMemsetAsync(dlen + n_delta, 0, 8, s));
+  CK(cudaMemsetAsync(xlen + n_deleted, 0, 8, s));
+  if (N > 0) {
+    k_refresh_lists<<<grid_for(N, 256, c->sm_count), 256, 0, s>>>((int32_t)D, (int32_t)N, flag, fpos, del, dpos, doc_off, pick, se, changed, deleted);
+    c->launches++;
+  }
+  if (n_delta > 0) {
+    k_line_len<<<grid_for(n_delta, 256, c->sm_count), 256, 0, s>>>(n_delta, pick, doc_off, se, dlen);
+    c->launches++;
+  }
+  if (n_deleted > 0) {
+    k_refresh_del_len<<<grid_for(n_deleted, 256, c->sm_count), 256, 0, s>>>(n_deleted, deleted, fa.row_ids, xlen);
+    c->launches++;
+  }
+  CKR(exclusive_sum(c, ar, dlen, doff, (long long)n_delta + 1));
+  CKR(exclusive_sum(c, ar, xlen, xoff, (long long)n_deleted + 1));
+  long long delta_bytes = 0, del_bytes = 0;
+  CKR(mail_fetch(c, &delta_bytes, doff + n_delta, 8));
+  CKR(mail_fetch(c, &del_bytes, xoff + n_deleted, 8));
+  CKR(mail_wait(c));
+  unsigned char *d_delta, *d_del;
+  CKR(ar.alloc(&d_delta, std::max<long long>(delta_bytes, 1)));
+  CKR(ar.alloc(&d_del, std::max<long long>(del_bytes, 1)));
+  if (n_delta > 0) {
+    k_line_gather<<<grid_for((long long)n_delta * 32, 256, c->sm_count), 256, 0, s>>>(n_delta, pick, doc_off, se, d_full, doff, d_delta);
+    c->launches++;
+  }
+  if (n_deleted > 0) {
+    k_refresh_del_write<<<grid_for((long long)n_deleted * 32, 256, c->sm_count), 256, 0, s>>>(n_deleted, deleted, fa.row_ids, xoff, d_del);
+    c->launches++;
+  }
+  // 6. one device-to-host copy per output
+  const unsigned char *src[5] = {d_full, d_delta, d_del, (const unsigned char *)changed, (const unsigned char *)deleted};
+  const long long bytes[5] = {total, delta_bytes, del_bytes, 8LL * n_changed, 8LL * n_deleted};
+  void *dst[5];
+  CKR(refresh_to_host(c, src, bytes, dst));
+  out->n_docs = N - n_deleted;
+  out->n_changed = n_changed;
+  out->n_new = X;
+  out->n_deleted = n_deleted;
+  out->n_unchanged = D - n_deleted - n_changed;
+  out->body = (char *)dst[0];
+  out->body_len = total;
+  out->delta = (char *)dst[1];
+  out->delta_len = delta_bytes;
+  out->deletes = (char *)dst[2];
+  out->deletes_len = del_bytes;
+  out->changed = (int64_t *)dst[3];
+  out->deleted = (int64_t *)dst[4];
+  return CCO_OK;
+}
+}  // namespace cco
+
+int cco_refresh_properties(cco_ctx_t *ctx, const char *body, int64_t body_len, const cco_item_properties_t *props,
+                           const cco_refresh_params_t *params, cco_refresh_out_t *out) {
+  return refresh_properties(ctx, body, body_len, props, params, out);
+}
+
+int cco_refresh_properties_log(cco_ctx_t *ctx, const char *body, int64_t body_len, const cco_event_log_t *lg,
+                               const cco_refresh_params_t *params, cco_refresh_out_t *out) {
+  if (!ctx || !lg) return set_error(CCO_E_INVALID_ARG, "null argument");
+  if (!ctx->members.empty() || lg->ctx != ctx) return set_error(CCO_E_UNSUPPORTED, "refresh on the per-GPU context that read the log");
+  CKR(log_state(lg, true));
+  LogProps lp;
+  log_props(lg, &lp);
+  const bool any = lg->n_triples > 0;
+  return refresh_properties(ctx, body, body_len, any ? &lp.shell : nullptr, params, out, any ? &lp.dev : nullptr);
 }
 
 namespace cco {

@@ -847,6 +847,41 @@ class CcoContext:
                                          C.byref(out), C.byref(ln)))
         return self._take_body(out, ln)
 
+    def refresh_properties(self, body: bytes, correlators, rankings, properties=None, log=None):
+        """cco_refresh_properties: fresh item properties written into the documents of the current index `body`, without
+        a retrain.  correlators: the model's event names; rankings: the field names of the computed rankings (popular,
+        trending, hot, random).  Per old document: "id", its correlator members, the item's fresh properties, its ranking
+        members; every other old member is dropped (include/cco_b200.h states the rule).  properties as in format_model
+        (the triples), or log=EventLog: its aggregated properties, in HBM.  -> ur_model.RefreshedIndex: the refreshed
+        full body, the delta (changed and new documents, a bulk body), the delete lines, the counts and the old document
+        numbers of the changed and deleted documents."""
+        from .ur_model import RefreshedIndex
+        keep = []
+        body = bytes(body)
+        cn = [x.encode("utf-8") for x in correlators]
+        rn = [x.encode("utf-8") for x in rankings]
+        ca, ra = (C.c_char_p * max(len(cn), 1))(*cn), (C.c_char_p * max(len(rn), 1))(*rn)
+        prm = N.RefreshParamsT(len(cn), ca, len(rn), ra)
+        out = N.RefreshOutT()
+        if log is not None:
+            if properties is not None:
+                raise N.CcoInvalidArgument(N.E_INVALID_ARG, "with log=, the properties are the log's")
+            N.check(self._L.cco_refresh_properties_log(self._h, body, len(body), log._h, C.byref(prm), C.byref(out)))
+        else:
+            props, _, _ = self._model_args(properties, None, keep)
+            N.check(self._L.cco_refresh_properties(self._h, body, len(body), C.byref(props) if props is not None else None, C.byref(prm),
+                                                   C.byref(out)))
+        addrs = [out.body, out.delta, out.deletes, C.cast(out.changed, C.c_void_p).value, C.cast(out.deleted, C.c_void_p).value]
+        try:
+            full, delta, deletes, changed, deleted = (C.string_at(a, n) if n else b"" for a, n in zip(
+                addrs, (out.body_len, out.delta_len, out.deletes_len, 8 * out.n_changed, 8 * out.n_deleted)))
+            changed = np.frombuffer(changed, dtype=np.int64).tolist()
+            deleted = np.frombuffer(deleted, dtype=np.int64).tolist()
+        finally:
+            for addr in addrs:
+                self._L.cco_host_free(self._h, C.c_void_p(addr))
+        return RefreshedIndex(full, delta, deletes, out.n_docs, out.n_changed, out.n_new, out.n_deleted, out.n_unchanged, changed, deleted)
+
     def train_csr(self, mats: Sequence[tuple[int, int, np.ndarray, np.ndarray]], params: Sequence[tuple[int, int, Optional[float]]],
                   seed: int, flags: int = 0, copy_arrays: bool = True, keep: bool = False):
         """Raw entry (cco_train): mats = [(n_rows, n_cols, row_ptr int64, col_idx int32)], params = [(m, k, minLLR|None)].

@@ -21,8 +21,8 @@ from typing import Optional, Sequence
 from .indexed_dataset import IndexedDataset
 from .similarity_analysis import CcoContext, DownsamplableCrossOccurrenceDataset, SimilarityAnalysis, default_context, encode_ids
 from .ur_query import Field, ItemQuery, ItemSetQuery, MixedQuery, UserQuery
-from .ur_model import (RankingParams, RankingType, alias_actions, extract_jvalue, index_mapping, new_index_name, property_json,
-                       ranking_window, rankings_for, rankings_params)
+from .ur_model import (RankingParams, RankingType, RefreshedIndex, alias_actions, bulk_item_statuses, extract_jvalue, index_mapping,
+                       mapping_additions, new_index_name, property_json, ranking_window, rankings_for, rankings_params)
 
 
 class DefaultURAlgoParams:
@@ -314,6 +314,41 @@ def calc_pop_from_events(body: bytes, export, ap: URAlgorithmParams, now_ms: Opt
             log.free()
 
 
+def _refresh_names(ap: URAlgorithmParams) -> tuple:
+    """(correlator names, computed ranking names) of a refresh: the model's event names, and the fields of the rankings
+    _log_rankings lists (popular, trending, hot, random; a userDefined field is an ordinary property)"""
+    return ap.model_event_names(), [r[0] for r in _log_rankings(ap, 0)]
+
+
+def refresh_properties_from_events(body: bytes, export, ap: URAlgorithmParams, now_ms: Optional[int] = None, event_window=None,
+                                   ctx: CcoContext | None = None) -> RefreshedIndex:
+    """The item properties of the live index refreshed without a retrain (CcoContext.refresh_properties): the properties
+    aggregated from a PredictionIO event export on the device (as in calc_all_from_events; an EventLog is used as given, not
+    freed, so a resident log extended with new lines serves every refresh) written into the documents of the current index
+    `body`.  Fresh properties win: a `$set` value replaces the old one, an `$unset` field leaves the document, a `$delete`d
+    item loses its properties and, when it has no correlator or ranking member either, its document.  Correlators and
+    rankings are kept as they are, never recomputed.  now_ms and event_window as in calc_all_from_events.  -> RefreshedIndex;
+    update_index writes its delta and deletes in place."""
+    ctx = ctx or default_context()
+    now_ms = _now(now_ms)
+    correlators, rankings = _refresh_names(ap)
+    log, owned = _read_log(export, ctx, event_window, now_ms)
+    try:
+        return ctx.refresh_properties(body, correlators, rankings, log=log)
+    finally:
+        if owned:
+            log.free()
+
+
+def refresh_properties_on_device(body: bytes, set_events: Sequence[tuple[str, dict]], ap: URAlgorithmParams,
+                                 ctx: CcoContext | None = None) -> RefreshedIndex:
+    """refresh_properties_from_events with the properties given as calc_pop_on_device takes them: set_events = the `$set`
+    events [(item, {field: value})] in event-time order, the later value of a field winning"""
+    ctx = ctx or default_context()
+    correlators, rankings = _refresh_names(ap)
+    return ctx.refresh_properties(body, correlators, rankings, properties=_properties(set_events))
+
+
 def user_queries_from_events(export, ap: URAlgorithmParams, query: Optional[UserQuery] = None, users=None, now_ms: Optional[int] = None,
                              ctx: CcoContext | None = None, event_window=None, header: str = "{}"):
     """buildQuery (URAlgorithm.scala:563-839) for every user of `users` (None: every user with a training event of a query
@@ -529,3 +564,84 @@ def write_index(body: bytes, ap: URAlgorithmParams, request, now_ms: Optional[in
         elif st != 404:
             raise IndexWriteError(f"HEAD /{name} answered HTTP {st}", new, result)
     return new, result
+
+
+def _delete_requests(deletes: bytes, max_docs: int, max_bytes: int) -> list:
+    """the delete lines cut as bulk_requests cuts documents -> [(decoded ids, request bytes)]"""
+    lines = [ln + b"\n" for ln in bytes(deletes).split(b"\n")[:-1]]
+    out, cur = [], []
+    for ln in lines:
+        if cur and (len(cur) == max_docs or sum(map(len, cur)) + len(ln) > max_bytes):
+            out.append(cur)
+            cur = []
+        cur.append(ln)
+    if cur:
+        out.append(cur)
+    ids = lambda part: [json.loads(ln.decode("utf-8", "surrogatepass"))["delete"]["_id"] for ln in part]
+    return [(ids(part), b"".join(part)) for part in out]
+
+
+def update_index(refresh: RefreshedIndex, ap: URAlgorithmParams, request, max_docs: int = 1000, max_bytes: int = 1 << 20,
+                 retries: int = 3, retry_wait_s: float = 10.0, ctx: CcoContext | None = None):
+    """A refresh (refresh_properties_from_events) written into the live index in place, over request(method, path, body
+    bytes or None) -> (HTTP status, response bytes), as for write_index:
+      1. GET /_alias/<indexName>, which must name exactly one index;  2. GET /<index>/_mapping/<typeName>, then one PUT of
+      the same path adding the delta's fields the mapping lacks, typed as index_mapping types them (Elasticsearch would
+      map a new property as analysed text);  3. POST /<index>/<typeName>/_bulk for the delta, at most max_docs documents
+      and max_bytes bytes per request, the responses read on the device with up to `retries` rounds for 429s, retry_wait_s
+      apart (write_index's steps 4-5);  4. the delete lines as _bulk requests cut by the same limits, a delete answered 200
+      or 404 (already gone) being success;  5. POST /<index>/_refresh.
+    No index is created, no alias moves, nothing but the deleted documents is removed.  Every action writes or deletes a
+    whole document, so running the update again after a partial failure converges on the same index.  A status other
+    than 200, an item failure or 429s left after the last round raise IndexWriteError naming the index.
+    -> (index name, IndexWriteResult of the delta, or None when the delta is empty)."""
+    if not ap.indexName or not ap.typeName:
+        raise ValueError("update_index needs indexName and typeName in the algorithm params")
+    ctx = ctx or default_context()
+    alias, type_name = ap.indexName, ap.typeName
+    index = None
+
+    def call(method: str, path: str, data: Optional[bytes] = None, ok=(200,)):
+        status, resp = request(method, path, data)
+        if status not in ok:
+            raise IndexWriteError(f"{method} {path} answered HTTP {status}: {bytes(resp or b'')[:500]!r}", index)
+        return bytes(resp or b"")
+
+    names = list(json.loads(call("GET", f"/_alias/{alias}").decode("utf-8")).keys())
+    if len(names) != 1:
+        raise IndexWriteError(f"the alias {alias} names {len(names)} indexes ({', '.join(names) or 'none'}): an update writes into one", None)
+    index = names[0]
+    mapping_path = f"/{index}/_mapping/{type_name}"
+    known: set = set()
+    for idx in json.loads(call("GET", mapping_path).decode("utf-8")).values():
+        known.update(((idx.get("mappings") or {}).get(type_name) or {}).get("properties") or {})
+    result = None
+    if refresh.delta:
+        with ctx.index_write(refresh.delta, max_docs, max_bytes) as w:
+            missing = [f for f in w.fields() if json.loads('"' + f + '"') not in known]
+            if missing:
+                call("PUT", mapping_path, mapping_additions(missing, ap))
+            bulk = f"/{index}/{type_name}/_bulk"
+            for q, part in enumerate(w.requests()):
+                w.response(q, call("POST", bulk, part))
+            for _ in range(retries):
+                first, parts = w.retry()
+                if not parts:
+                    break
+                time.sleep(retry_wait_s)
+                for k, (_, part) in enumerate(parts):
+                    w.response(first + k, call("POST", bulk, part))
+            result = w.finish()
+        if result.errors:
+            shown = result.errors[:5]
+            ids = _bulk_ids(refresh.delta, [d for d, _, _ in shown])
+            lines = "; ".join(f"{ids[d]!r}: {t or '-'}: {r or '-'}" for d, t, r in shown)
+            raise IndexWriteError(f"{len(result.errors)} documents were not written to {index} ({result.n_rejected} still rejected "
+                                  f"with 429, {result.n_failed} failed): {lines}", index, result)
+    for ids, part in _delete_requests(refresh.deletes, max_docs, max_bytes):
+        statuses = bulk_item_statuses(call("POST", f"/{index}/{type_name}/_bulk", part), ids, action="delete")
+        bad = [(i, st) for i, (st, _, _) in zip(ids, statuses) if st not in (200, 404)]
+        if bad:
+            raise IndexWriteError(f"{len(bad)} deletes failed on {index}: " + "; ".join(f"{i!r}: HTTP {st}" for i, st in bad[:5]), index, result)
+    call("POST", f"/{index}/_refresh")
+    return index, result

@@ -669,16 +669,30 @@ def index_mapping(fields: Sequence[str], ap, type_name: str) -> bytes:
     getMappings (URAlgorithm.scala:955-967): its Map `++` order lets the date names override the event names and those
     the ranking names; every other field is a keyword.  The tail's unused "last" property closes the object without a
     trailing comma, so a field really named "last" is written twice, as the reference writes it."""
-    names = ap.model_event_names()
-    dates = list(dict.fromkeys(d for d in (ap.dateName, ap.availableDateName, ap.expireDateName) if d is not None))
-    types = {**{rp.field_name(): "float" for rp in rankings_params(ap.rankings, names)}, **{e: "keyword" for e in names},
-             **{d: "date" for d in dates}}
-    types = {json_string(k)[1:-1]: v for k, v in types.items()}
+    types = index_field_types(ap)
     out = '{ "mappings": {    "%s": {      "properties": {            ' % type_name
     for f in fields:
         out += '"%s"    : {      "type": "%s"    },            ' % (f, types.get(f, "keyword"))
     out += '    "last": {      "type": "keyword"    }}}}}            '
     return out.encode("utf-8", "surrogatepass")
+
+
+def index_field_types(ap) -> dict:
+    """getMappings' types by escaped field name (index_mapping's rule): date names over event names over ranking names; a
+    field not listed is a keyword"""
+    names = ap.model_event_names()
+    dates = list(dict.fromkeys(d for d in (ap.dateName, ap.availableDateName, ap.expireDateName) if d is not None))
+    types = {**{rp.field_name(): "float" for rp in rankings_params(ap.rankings, names)}, **{e: "keyword" for e in names},
+             **{d: "date" for d in dates}}
+    return {json_string(k)[1:-1]: v for k, v in types.items()}
+
+
+def mapping_additions(fields: Sequence[str], ap) -> bytes:
+    """the body of PUT /<index>/_mapping/<type> that adds the fields (escaped, as IndexWrite.fields gives them) to a live
+    index, typed as index_mapping types them"""
+    types = index_field_types(ap)
+    return ('{"properties":{' + ",".join('"%s":{"type":"%s"}' % (f, types.get(f, "keyword")) for f in fields)
+            + "}}").encode("utf-8", "surrogatepass")
 
 
 def alias_actions(alias: str, new_index: str, old_index: Optional[str] = None) -> bytes:
@@ -754,9 +768,10 @@ def bulk_requests(body: bytes, max_docs: int, max_bytes: int) -> tuple:
     return doc_begin, byte_begin
 
 
-def bulk_item_statuses(response: bytes, ids: Sequence[str]) -> list:
+def bulk_item_statuses(response: bytes, ids: Sequence[str], action: str = "index") -> list:
     """one _bulk response for the documents of `ids` -> [(status, error.type, error.reason)] per item ("" where the item
-    has no such string).  ValueError for the errors cco_index_write_response reports."""
+    has no such string).  ValueError for the errors cco_index_write_response reports.  action="delete" reads the response
+    to `delete` actions, whose items are {"delete":{...}} with the same members."""
     top = _pairs(bytes(response))
     if not isinstance(top, _Obj):
         raise ValueError("the top level is not an object")
@@ -773,8 +788,8 @@ def bulk_item_statuses(response: bytes, ids: Sequence[str]) -> list:
         raise ValueError(f"{len(items)} items for {len(ids)} documents")
     out = []
     for i, item in enumerate(items):
-        if len(item) != 1 or item[0][0] != "index" or not isinstance(item[0][1], _Obj):
-            raise ValueError(f"item {i}: the item is not {{\"index\":{{...}}}}")
+        if len(item) != 1 or item[0][0] != action or not isinstance(item[0][1], _Obj):
+            raise ValueError(f"item {i}: the item is not {{\"{action}\":{{...}}}}")
         members = item[0][1]
         got_id = [v for k, v in members if k == "_id"]
         status = [v for k, v in members if k == "status"]
@@ -805,3 +820,115 @@ def _first_pair(pairs: list, name: str, default=None):
         if k == name:
             return v
     return default
+
+
+# ---- item properties refreshed in the live index ----------------------------------------------------------------------------
+# The host mirror of cco_refresh_properties (include/cco_b200.h states the rule): fresh properties win, the correlator and
+# computed ranking members of an old document are kept verbatim, every other old member is dropped.
+@dataclass
+class RefreshedIndex:
+    """A refresh of the model index: body = the refreshed full index; delta = the changed and new documents (a bulk body);
+    deletes = one {"delete":{"_id":...}} line per deleted document; changed / deleted = their old document numbers."""
+    body: bytes
+    delta: bytes
+    deletes: bytes
+    n_docs: int
+    n_changed: int
+    n_new: int
+    n_deleted: int
+    n_unchanged: int
+    changed: list
+    deleted: list
+
+    @property
+    def changed_ids(self) -> list:
+        """the decoded ids of the changed documents (the first n_changed documents of the delta)"""
+        lines = self.delta.split(b"\n")
+        return [_pairs(lines[2 * k])[0][1][0][1] for k in range(self.n_changed)]
+
+    @property
+    def deleted_ids(self) -> list:
+        return [_pairs(line)[0][1][0][1] for line in self.deletes.split(b"\n")[:-1]]
+
+
+def _raw_members(line: bytes) -> list:
+    """the members of a source line -> [(decoded name, raw name bytes between the quotes, trimmed raw value bytes)]"""
+    w = _Walk(line, 0)
+    i = w.ws(0)
+    out = []
+    j = w.ws(i + 1)
+    if line[j:j + 1] == b"}":
+        return out
+    while True:
+        name_b, ne = j, w.string(j)
+        name = json.loads(line[j:ne].decode("utf-8", "surrogatepass"))
+        j = w.ws(ne)
+        _, vb, ve = w.value(w.ws(j + 1))
+        out.append((name, line[name_b + 1:ne - 1], line[vb:ve]))
+        j = w.ws(ve)
+        if line[j:j + 1] == b"}":
+            return out
+        j = w.ws(j + 1)
+
+
+def refresh_documents(body: bytes, correlators: Sequence[str], rankings: Sequence[str],
+                      triples: Sequence[tuple[str, str, object]]) -> RefreshedIndex:
+    """cco_refresh_properties on the host.  body: the current index (bulk_documents' grammar, an _id in two documents is a
+    ValueError); correlators: the model's event names; rankings: the field names of the computed (popular, trending, hot,
+    random) rankings; triples: the fresh (item, field, value) properties, values as property_json writes them, fields
+    numbered by first appearance, the last triple of an (item, field) wins.  An old document becomes "id", its members
+    named like a correlator, the item's fresh properties (not "id", not named like a computed ranking), its members named
+    like a computed ranking; "id" and a member followed by one of the same name are skipped.  A document with neither a
+    triple nor a kept member is deleted; an item with a triple and no document is new.  ValueError for a property named
+    like a correlator."""
+    body = bytes(body)
+    docs = bulk_documents(body)
+    corr, rank = set(correlators), set(rankings) - set(correlators)
+    fields = list(dict.fromkeys(f for _, f, _ in triples))
+    for f in fields:
+        if f in corr:
+            raise ValueError(f'property field "{f}" is named like a correlator: a refresh keeps the correlator arrays')
+    fnum = {f: k for k, f in enumerate(fields)}
+    props: dict = {}
+    for item, f, v in triples:
+        props.setdefault(item, {})[f] = v
+    enc = lambda s: s.encode("utf-8", "surrogatepass")
+
+    def prop_bytes(item) -> bytes:
+        d = props.get(item, {})
+        return b"".join(b"," + enc(json_string(f)) + b":" + enc(property_json(d[f]))
+                        for f in sorted(d, key=fnum.get) if f != "id" and f not in rank)
+
+    def doc_bytes(item, src: bytes) -> bytes:
+        return b'{"index":{"_id":' + enc(json_string(item)) + b"}}\n" + src + b"\n"
+
+    first: dict = {}
+    full, delta, deletes = bytearray(), bytearray(), bytearray()
+    changed, deleted = [], []
+    for d, (_, b, e, _) in enumerate(docs):
+        index = _first_pair(_pairs(body[b:e].split(b"\n")[0]), "index")
+        item = [v for k, v in index if k == "_id"][-1]   # of a repeated _id the last, as cco_rerank_model reads it
+        if item in first:
+            raise ValueError(f"document {d}: its _id is the _id of document {first[item]}")
+        first[item] = d
+        old = body[b:e].split(b"\n")[1]
+        members = _raw_members(old)
+        kept = [m for k, m in enumerate(members) if m[0] != "id" and all(m2[0] != m[0] for m2 in members[k + 1:])]
+        cm = b"".join(b',"' + raw + b'":' + val for name, raw, val in kept if name in corr)
+        rm = b"".join(b',"' + raw + b'":' + val for name, raw, val in kept if name in rank)
+        if item not in props and not cm and not rm:
+            deleted.append(d)
+            deletes += b'{"delete":{"_id":' + enc(json_string(item)) + b"}}\n"
+            continue
+        src = b'{"id":' + enc(json_string(item)) + cm + prop_bytes(item) + rm + b"}"
+        full += doc_bytes(item, src)
+        if src != old:
+            changed.append(d)
+            delta += doc_bytes(item, src)
+    new = [item for item in props if item not in first]
+    for item in new:
+        doc = doc_bytes(item, b'{"id":' + enc(json_string(item)) + prop_bytes(item) + b"}")
+        full += doc
+        delta += doc
+    return RefreshedIndex(bytes(full), bytes(delta), bytes(deletes), len(docs) - len(deleted) + len(new), len(changed), len(new),
+                          len(deleted), len(docs) - len(deleted) - len(changed), changed, deleted)
