@@ -602,6 +602,33 @@ int cco_event_log_begin_ex(cco_ctx_t *ctx, int64_t chunk_bytes, const cco_event_
  */
 int cco_event_log_extend(cco_event_log_t *log, const cco_event_window_t *w /* nullable: keep the current window */);
 int cco_event_log_resident_bytes(const cco_event_log_t *log, int64_t *bytes);
+
+/*
+ * Interned logs: retrains from a resident log at a cost set by its new lines plus integer passes.  cco_event_log_begin_ex
+ * with CCO_LOG_INTERN_IDS (it combines with CCO_LOG_KEEP_HISTORY, CCO_LOG_EXTENDABLE and a window) gives every distinct
+ * user id and item id of the training entries a 32-bit key as the lines are read: one table for the users (entityId),
+ * one for the items (targetEntityId, shared by every event name).  Each chunk, and each extend, interns only its own
+ * lines, and cco_event_log_ingest on the log then groups keys instead of strings.
+ *
+ * The invariant: for any export, window, chunking and sequence of extends, cco_event_log_ingest of an interned log, with
+ * any names and any min_events_per_user, gives the dataset the same lines read once without the flag under the same
+ * final window give -- the same dictionaries byte for byte and in the same order, the same matrices.  Every other
+ * consumer (info, window_stats, format_model_log, rerank_model_log, user and mixed queries, query files,
+ * refresh_properties_log) gives what it gives on that log.  After every finish, of a read or of an extend, the tables
+ * hold exactly the distinct ids of the retained training entries (those of expired and duplicate lines are gone), and
+ * their sizes are a fixed function of those counts and bytes: an extended interned log and a fresh interned extendable
+ * read of the same lines hold the same bytes.  Key numbering is internal.
+ *
+ * Added device memory: 8 bytes per retained training entry (its user and item keys), and per table 24 to 32 bytes per
+ * key (its string offset and hash, 8 bytes each, and 2 to 4 table slots of 4 bytes; at least 64 slots) plus the keys'
+ * string bytes and 16 bytes of padding.
+ *
+ * cco_event_log_intern_stats: the live key counts of a finished interned log.  Errors: CCO_E_INVALID_ARG for a null
+ * argument, a log not finished or failed, and a log read without CCO_LOG_INTERN_IDS; CCO_E_UNSUPPORTED for 2^31 or more
+ * distinct ids in one table; group contexts refuse logs as before.
+ */
+enum { CCO_LOG_INTERN_IDS = 4 };
+int cco_event_log_intern_stats(const cco_event_log_t *log, int64_t *n_user_keys, int64_t *n_item_keys);
 /*
  * The query of user u, for the query event names n_0 .. n_{k-1}:
  *  - history of n_q: u's training events of n_q, latest first (eventTime desc, ties to the later line), the first limits[q]
@@ -1090,6 +1117,9 @@ int cco_debug_cooccurrence(cco_ctx_t *ctx, const cco_csr_t *a, const cco_csr_t *
  * max_keys keys, even where the packed word fits and without the flag, so that every row path can be run split; 0 = off.
  * On a group context it applies to every GPU of the group. */
 int cco_debug_key_range_cap(cco_ctx_t *ctx, int32_t max_keys);
+/* Debug entry (tests only): truncate the intern hash (CCO_LOG_INTERN_IDS) of the logs this context begins from now on to
+ * its low `bits` bits (0..64; 64 = off), so that inserts collide and every key is found by its bytes. */
+int cco_debug_intern_hash_bits(cco_ctx_t *ctx, int32_t bits);
 /* Debug/parity entry (tests only): sampleDownAndBinarize of one matrix on the device. */
 int cco_debug_downsample(cco_ctx_t *ctx, const cco_csr_t *m, int32_t max_interactions, int32_t seed,
                          uint32_t flags, int64_t **row_ptr, int32_t **col_idx, int32_t *raw_col_counts,

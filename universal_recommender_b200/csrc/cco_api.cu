@@ -35,6 +35,7 @@
 #include "cco_index_pages.cuh"
 #include "cco_index_write.cuh"
 #include "cco_refresh.cuh"
+#include "cco_intern.cuh"
 
 namespace cco {
 
@@ -160,6 +161,7 @@ struct cco_ctx {
   ncclComm_t comm = nullptr;
   int launches = 0;
   int32_t key_range_cap = 0;   // cco_debug_key_range_cap: at most this many keys per key range (0 = off)
+  uint64_t intern_mask = ~0ULL;   // cco_debug_intern_hash_bits: the intern hash of the logs begun from now on, truncated
   // mailbox for small device -> host results (mapped pinned memory written by k_mail_bytes).  Records are closed into
   // groups; a group is complete when its event has fired, so the host can wait for indicator i's numbers while the GPU
   // already runs indicator i + 1 (no stream-wide synchronisation).
@@ -2561,6 +2563,30 @@ static int str_dictionary(cco_ctx *c, Arena &ar, const DevStrCol &col, const Str
   return CCO_OK;
 }
 
+// type t of the dataset from each event's user and item dictionary ids (-1: dropped): the (user, item) keys, then the
+// CSR; uid and iid are released
+static int ingest_ids_csr(cco_ctx *c, Arena &ar, cco_dataset *d, int t, long long ne, uint32_t n_users, int32_t *uid, int32_t *iid) {
+  cudaStream_t s = c->stream;
+  unsigned long long *k0, *k1, *d_kept;
+  CKR(ar.alloc(&k0, std::max<long long>(ne, 1)));
+  CKR(ar.alloc(&k1, std::max<long long>(ne, 1)));
+  CKR(ar.alloc(&d_kept, 1));
+  CK(cudaMemsetAsync(d_kept, 0, 8, s));
+  if (ne > 0) {
+    k_str_keys<<<grid_for(ne, 256, c->sm_count), 256, 0, s>>>(ne, uid, iid, k0, d_kept);
+    c->launches++;
+  }
+  unsigned long long kept = 0;
+  CKR(mail_fetch(c, &kept, d_kept, 8));
+  CKR(mail_wait(c));
+  ar.release(uid);
+  ar.release(iid);
+  CKR(ingest_csr(c, ar, d, t, ne, n_users, k0, k1, kept));
+  ar.release(k0);
+  ar.release(k1);
+  return CCO_OK;
+}
+
 // the user and item columns of type t in HBM: uploaded from the caller's arrays, or views of an event log's columns
 using StrColumns = std::function<int(Arena &, int, DevStrCol *, DevStrCol *)>;
 
@@ -2618,23 +2644,7 @@ static int ingest_strings_core(cco_ctx *c, int32_t n_types, const StrColumns &co
     str_table_release(ar, it);
     if (t > 0) str_release(ar, uc);
     str_release(ar, ic);
-    unsigned long long *k0, *k1, *d_kept;
-    CKR(ar.alloc(&k0, std::max<long long>(ne, 1)));
-    CKR(ar.alloc(&k1, std::max<long long>(ne, 1)));
-    CKR(ar.alloc(&d_kept, 1));
-    CK(cudaMemsetAsync(d_kept, 0, 8, s));
-    if (ne > 0) {
-      k_str_keys<<<grid_for(ne, 256, c->sm_count), 256, 0, s>>>(ne, uid, iid, k0, d_kept);
-      c->launches++;
-    }
-    unsigned long long kept = 0;
-    CKR(mail_fetch(c, &kept, d_kept, 8));
-    CKR(mail_wait(c));
-    ar.release(uid);
-    ar.release(iid);
-    CKR(ingest_csr(c, ar, d, t, ne, n_users, k0, k1, kept));
-    ar.release(k0);
-    ar.release(k1);
+    CKR(ingest_ids_csr(c, ar, d, t, ne, n_users, uid, iid));
   }
   CKR(ingest_blocks(c, d, n_users));
   CK(cudaStreamSynchronize(s));
@@ -3708,7 +3718,25 @@ struct EvSeg {
   long long *rtime = nullptr;
   long long *tline = nullptr, *rline = nullptr;   // removeDuplicates: the global line of each training / ranking entry
   long long *ttime = nullptr;                       // history retention: each training entry's time (and tline its line)
+  long long *tkey = nullptr;                        // interned ids: each training entry's (user key << 32 | item key)
   std::vector<long long> train_at, rank_at;
+};
+// the intern table of one id column (CCO_LOG_INTERN_IDS; kernels in cco_intern.cuh): key k's string is the heap's bytes
+// [off[k], off[k + 1]) (words w, 16 bytes of padding), its hash hash[k]; table: cap slots, each a key or kStrEmpty
+struct InternTable {
+  long long n = 0, kcap = 0;        // keys; capacity of off (+ 1) and hash
+  long long bytes = 0, bcap = 0;    // heap bytes; capacity of w (+ 16 bytes)
+  long long cap = 0;
+  long long *off = nullptr;
+  uint64_t *w = nullptr, *hash = nullptr;
+  uint32_t *table = nullptr;
+  DevStrCol heap() const {
+    DevStrCol v;
+    v.n = n;
+    v.off = off;
+    v.w = w;
+    return v;
+  }
 };
 struct cco_event_log {
   cco_ctx *ctx = nullptr;
@@ -3751,6 +3779,13 @@ struct cco_event_log {
   // then outlives finish
   bool history = false;
   long long *ttime = nullptr;
+  // interned ids (CCO_LOG_INTERN_IDS): one table for the users and one for the items of the training entries, and tkey
+  // (user key << 32 | item key) per training entry, partitioned as tu / ti.  After every finish the tables hold exactly
+  // the ids of the retained entries.  intern_mask: the context's cco_debug_intern_hash_bits when the read began.
+  bool intern = false;
+  uint64_t intern_mask = ~0ULL;
+  InternTable users, items;
+  long long *tkey = nullptr;
   // extendable logs (CCO_LOG_EXTENDABLE): rec (one record per retained line, with or without dedup), tline / rline and the
   // property lines (pb, prop_line) outlive finish; dup_time holds the eventTimes of the non-exempt lines removeDuplicates
   // dropped, which a later cutoff turns into expired lines; chunk0 is the staging cco_event_log_extend reopens with
@@ -4301,6 +4336,153 @@ static int ext_records(cco_event_log *lg, Arena &ar, const EvLines &ev, const in
   return CCO_OK;
 }
 
+// ---- interned logs: intern tables per chunk and their refit at finish (kernels in cco_intern.cuh) --------------------------
+// the slots of a table for n keys: a power of two, at most half full
+static long long intern_slots(long long n) {
+  long long cap = 64;
+  while (cap < 2 * n) cap <<= 1;
+  return cap;
+}
+// tb's keys in a new table of cap slots, inserted from their stored hashes; the old table is freed
+static int intern_rehash(cco_event_log *lg, Arena &ar, InternTable *tb, long long cap) {
+  cco_ctx *c = lg->ctx;
+  uint32_t *t;
+  CKR(ar.alloc(&t, cap));
+  CKR(log_keep(ar, lg, t));
+  CK(cudaMemsetAsync(t, 0xff, sizeof(uint32_t) * (size_t)cap, c->stream));
+  if (tb->n > 0) {
+    k_intern_rehash<<<grid_for(tb->n, 256, c->sm_count), 256, 0, c->stream>>>(tb->n, tb->hash, (uint64_t)cap - 1, t);
+    c->launches++;
+  }
+  log_drop(lg, tb->table);
+  tb->table = t;
+  tb->cap = cap;
+  return CCO_OK;
+}
+// the n ids of one column of a chunk's segment interned into tb: the strings new to tb take the next keys in the order
+// of their first entry, their bytes join the heap; each entry's key -> half[2 i]
+static int intern_column(cco_event_log *lg, Arena &ar, InternTable *tb, const EvCol &col, long long n, uint32_t *half) {
+  if (n == 0) return CCO_OK;
+  cco_ctx *c = lg->ctx;
+  cudaStream_t s = c->stream;
+  if (intern_slots(tb->n + n) > tb->cap) CKR(intern_rehash(lg, ar, tb, intern_slots(tb->n + n)));
+  uint64_t *hash;
+  uint32_t *slot_of, *flag, *pos, *idx, K = 0;
+  CKR(ar.alloc(&hash, n));
+  CKR(ar.alloc(&slot_of, n));
+  CKR(ar.alloc(&flag, n + 1));
+  k_str_hash<<<grid_for(n, 256, c->sm_count), 256, 0, s>>>(n, col.off, 0, col.w, lg->intern_mask, hash);
+  k_intern_claim<<<grid_for(n, 256, c->sm_count), 256, 0, s>>>(n, col.off, col.w, hash, tb->off, tb->w, tb->hash, (uint64_t)tb->cap - 1,
+                                                               tb->table, slot_of);
+  k_intern_first<<<grid_for(n, 256, c->sm_count), 256, 0, s>>>(n, slot_of, tb->table, flag);
+  c->launches += 3;
+  CKR(select_flagged(c, ar, n, flag, &pos, &idx));
+  CKR(mail_fetch(c, &K, pos + n, 4));
+  CKR(mail_wait(c));
+  if (tb->n + K >= (long long)kInternNew) return set_error(CCO_E_UNSUPPORTED, "%lld distinct ids: an interned log takes < 2^31", tb->n + K);
+  if (K > 0) {
+    long long *len, *noff, total = 0;
+    CKR(ar.alloc(&len, (long long)K + 1));
+    CKR(ar.alloc(&noff, (long long)K + 1));
+    CK(cudaMemsetAsync(len + K, 0, 8, s));
+    k_str_dict_len<<<grid_for(K, 256, c->sm_count), 256, 0, s>>>(K, idx, col.off, len);
+    c->launches++;
+    CKR(exclusive_sum(c, ar, len, noff, (long long)K + 1));
+    CKR(mail_fetch(c, &total, noff + K, 8));
+    CKR(mail_wait(c));
+    if (tb->n + K > tb->kcap) {   // grow geometrically
+      const long long kc = std::max(2 * tb->kcap, tb->n + K);
+      CKR(log_grow(lg, ar, &tb->off, kc, tb->n > 0 ? tb->n + 1 : 0, 1));
+      CKR(log_grow(lg, ar, &tb->hash, kc, tb->n, 0));
+      tb->kcap = kc;
+    }
+    if (tb->bytes + total > tb->bcap) {
+      const long long bc = std::max(2 * tb->bcap, tb->bytes + total);
+      CKR(log_grow(lg, ar, &tb->w, (bc + 7) / 8, (tb->bytes + 7) / 8, 2));
+      tb->bcap = bc;
+    }
+    k_intern_new<<<grid_for(K, 256, c->sm_count), 256, 0, s>>>(K, idx, slot_of, hash, (uint32_t)tb->n, tb->table, tb->hash);
+    k_intern_heap_off<<<grid_for((long long)K + 1, 256, c->sm_count), 256, 0, s>>>(K, noff, tb->bytes, tb->off + tb->n);
+    c->launches += 2;
+    if (total > 0) {
+      k_str_dict_gather<<<grid_for(K, 256, c->sm_count), 256, 0, s>>>(K, idx, col.off, 0, (const unsigned char *)col.w, noff,
+                                                                      (unsigned char *)tb->w + tb->bytes);
+      c->launches++;
+    }
+    tb->n += K;
+    tb->bytes += total;
+  }
+  k_intern_keys<<<grid_for(n, 256, c->sm_count), 256, 0, s>>>(n, slot_of, tb->table, half);
+  c->launches++;
+  CK(cudaStreamSynchronize(s));
+  return CCO_OK;
+}
+// the keys live[k] != 0 of tb kept, renumbered in key order (pos: their new numbers, idx: the old key of each new one):
+// the heap and hashes gathered as exact fits, the table rebuilt at intern_slots of the count
+static int intern_refit_table(cco_event_log *lg, Arena &ar, InternTable *tb, const uint32_t *pos, const uint32_t *idx) {
+  cco_ctx *c = lg->ctx;
+  cudaStream_t s = c->stream;
+  uint32_t K = 0;
+  long long total = 0;
+  CK(cudaMemcpyAsync(&K, pos + tb->n, 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  long long *len, *off;
+  uint64_t *w, *h;
+  CKR(ar.alloc(&len, (long long)K + 1));
+  CKR(ar.alloc(&off, (long long)K + 1));
+  CK(cudaMemsetAsync(len + K, 0, 8, s));
+  if (K > 0) {
+    k_str_dict_len<<<grid_for(K, 256, c->sm_count), 256, 0, s>>>(K, idx, tb->off, len);
+    c->launches++;
+  }
+  CKR(exclusive_sum(c, ar, len, off, (long long)K + 1));
+  CK(cudaMemcpyAsync(&total, off + K, 8, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  CKR(ar.alloc(&w, (total + 16 + 7) / 8));
+  CKR(ar.alloc(&h, std::max<long long>(K, 1)));
+  if (K > 0) {
+    if (total > 0) {
+      k_str_dict_gather<<<grid_for(K, 256, c->sm_count), 256, 0, s>>>(K, idx, tb->off, 0, (const unsigned char *)tb->w, off, (unsigned char *)w);
+      c->launches++;
+    }
+    k_gather_i64<<<grid_for(K, 256, c->sm_count), 256, 0, s>>>(K, idx, (const long long *)tb->hash, (long long *)h);
+    c->launches++;
+  }
+  for (void *p : {(void *)off, (void *)w, (void *)h}) CKR(log_keep(ar, lg, p));
+  for (void *p : {(void *)tb->off, (void *)tb->w, (void *)tb->hash}) log_drop(lg, p);
+  tb->off = off;
+  tb->w = w;
+  tb->hash = h;
+  tb->n = tb->kcap = K;
+  tb->bytes = tb->bcap = total;
+  return intern_rehash(lg, ar, tb, intern_slots(K));
+}
+// at the end of every finish: the tables keep exactly the ids of the retained training entries, sized by their counts only
+static int intern_refit(cco_event_log *lg) {
+  cco_ctx *c = lg->ctx;
+  cudaStream_t s = c->stream;
+  Arena ar(s);
+  const long long E = lg->train_at.back();
+  InternTable *tbs[2] = {&lg->users, &lg->items};
+  uint32_t *live[2], *pos[2], *idx[2];
+  for (int x = 0; x < 2; ++x) {
+    CKR(ar.alloc(&live[x], tbs[x]->n + 1));
+    CK(cudaMemsetAsync(live[x], 0, sizeof(uint32_t) * (size_t)(tbs[x]->n + 1), s));
+  }
+  if (E > 0) {
+    k_intern_live<<<grid_for(E, 256, c->sm_count), 256, 0, s>>>(E, (const unsigned long long *)lg->tkey, live[0], live[1]);
+    c->launches++;
+  }
+  for (int x = 0; x < 2; ++x) CKR(select_flagged(c, ar, tbs[x]->n, live[x], &pos[x], &idx[x]));
+  if (E > 0) {
+    k_intern_remap<<<grid_for(E, 256, c->sm_count), 256, 0, s>>>(E, pos[0], pos[1], (unsigned long long *)lg->tkey);
+    c->launches++;
+  }
+  for (int x = 0; x < 2; ++x) CKR(intern_refit_table(lg, ar, tbs[x], pos[x], idx[x]));
+  CK(cudaStreamSynchronize(s));
+  return CCO_OK;
+}
+
 // one chunk of a streamed read, the first len staged bytes: every line parsed, the names numbered globally, the counts
 // added, the training and ranking events decoded into one new segment, the property-event lines appended to lg->pb
 static int event_chunk(cco_event_log *lg, long long len, bool open_tail) {
@@ -4398,6 +4580,13 @@ static int event_chunk(cco_event_log *lg, long long len, bool open_tail) {
   CKR(event_column(c, ar, lg, sg.train_at[NG], idx, kEvEntityId, ev.sb, ev.span, bb, sg.train_at, &sg.tu));
   CKR(event_column(c, ar, lg, sg.train_at[NG], idx, kEvTargetId, ev.sb, ev.span, bb, sg.train_at, &sg.ti));
   if (lg->dedup || lg->history || lg->extendable) CKR(win_entry_lines(lg, ar, sg.train_at[NG], idx, base, &sg.tline));
+  if (lg->intern) {   // the chunk's lines have their verdicts: its training ids take their keys
+    const long long NT = sg.train_at[NG];
+    CKR(ar.alloc(&sg.tkey, std::max<long long>(NT, 1)));
+    CKR(log_keep(ar, lg, sg.tkey));
+    CKR(intern_column(lg, ar, &lg->users, sg.tu, NT, (uint32_t *)sg.tkey + 1));
+    CKR(intern_column(lg, ar, &lg->items, sg.ti, NT, (uint32_t *)sg.tkey));
+  }
   if (lg->history) {
     const long long NT = sg.train_at[NG];
     CKR(ar.alloc(&sg.ttime, std::max<long long>(NT, 1)));
@@ -4766,7 +4955,7 @@ static int win_gather_column(cco_event_log *lg, Arena &ar, long long K, const ui
 }
 // the name-partitioned entries whose line survives the bitmap: columns c1 (and c2), the times (nullable) and at, compacted
 static int win_compact(cco_event_log *lg, const uint32_t *bitmap, const long long *line, std::vector<long long> &at, EvCol *c1, EvCol *c2,
-                       long long **times, long long **times2 = nullptr) {
+                       long long **times, long long **times2 = nullptr, long long **times3 = nullptr) {
   cco_ctx *c = lg->ctx;
   cudaStream_t s = c->stream;
   Arena ar(s);
@@ -4789,7 +4978,7 @@ static int win_compact(cco_event_log *lg, const uint32_t *bitmap, const long lon
   const long long K = nat.back();
   CKR(win_gather_column(lg, ar, K, idx, nat, c1));
   if (c2) CKR(win_gather_column(lg, ar, K, idx, nat, c2));
-  for (long long **tp : {times, times2}) {
+  for (long long **tp : {times, times2, times3}) {
     if (!tp) continue;
     long long *t;
     CKR(ar.alloc(&t, std::max<long long>(K, 1)));
@@ -4955,6 +5144,7 @@ static int event_log_finish(cco_event_log *lg) {
     lg->tline = sg.tline;
     lg->rline = sg.rline;
     lg->ttime = sg.ttime;
+    lg->tkey = sg.tkey;
   } else if (lg->segs.size() > 1) {
     CKR(event_cat_column(lg, &EvSeg::tu, &EvSeg::train_at, lg->train_at, &lg->tu));
     CKR(event_cat_column(lg, &EvSeg::ti, &EvSeg::train_at, lg->train_at, &lg->ti));
@@ -4963,11 +5153,12 @@ static int event_log_finish(cco_event_log *lg) {
     if (lg->dedup || lg->history || lg->extendable) CKR(event_cat_times(lg, &lg->tline, &EvSeg::tline, &EvSeg::train_at));
     if (lg->dedup || lg->extendable) CKR(event_cat_times(lg, &lg->rline, &EvSeg::rline, &EvSeg::rank_at));
     if (lg->history) CKR(event_cat_times(lg, &lg->ttime, &EvSeg::ttime, &EvSeg::train_at));
+    if (lg->intern) CKR(event_cat_times(lg, &lg->tkey, &EvSeg::tkey, &EvSeg::train_at));
   }
   lg->segs.clear();
   if (drop && n_drop > 0) {   // the retained columns without the dropped lines' entries
     CKR(win_compact(lg, drop, lg->tline, lg->train_at, &lg->tu, &lg->ti, lg->history ? &lg->ttime : nullptr,
-                    lg->history || lg->extendable ? &lg->tline : nullptr));
+                    lg->history || lg->extendable ? &lg->tline : nullptr, lg->intern ? &lg->tkey : nullptr));
     CKR(win_compact(lg, drop, lg->rline, lg->rank_at, &lg->ri, nullptr, &lg->rtime, lg->extendable ? &lg->rline : nullptr));
     for (long long n = 0; n < NG; ++n) {
       lg->n_train[n] = lg->train_at[n + 1] - lg->train_at[n];
@@ -4978,6 +5169,7 @@ static int event_log_finish(cco_event_log *lg) {
     log_drop(lg, lg->tline);
     lg->tline = nullptr;
   }
+  if (lg->intern) CKR(intern_refit(lg));
   if (!lg->extendable) {
     log_drop(lg, lg->rline);
     lg->rline = nullptr;
@@ -5028,6 +5220,7 @@ static int event_log_extend(cco_event_log *lg, const cco_event_window_t *w) {
   sg.tline = lg->tline;
   sg.rline = lg->rline;
   sg.ttime = lg->ttime;
+  sg.tkey = lg->tkey;
   sg.train_at = lg->train_at;
   sg.rank_at = lg->rank_at;
   lg->segs.assign(1, sg);
@@ -5144,6 +5337,15 @@ int cco_event_log_extend(cco_event_log_t *lg, const cco_event_window_t *w) {
   return log_fail(lg, event_log_extend(lg, w));
 }
 
+int cco_event_log_intern_stats(const cco_event_log_t *lg, int64_t *n_user_keys, int64_t *n_item_keys) {
+  if (!lg || !n_user_keys || !n_item_keys) return set_error(CCO_E_INVALID_ARG, "null argument");
+  CKR(log_state(lg, true));
+  if (!lg->intern) return set_error(CCO_E_INVALID_ARG, "the log was read without CCO_LOG_INTERN_IDS (cco_event_log_begin_ex)");
+  *n_user_keys = lg->users.n;
+  *n_item_keys = lg->items.n;
+  return CCO_OK;
+}
+
 int cco_event_log_resident_bytes(const cco_event_log_t *lg, int64_t *bytes) {
   if (!lg || !bytes) return set_error(CCO_E_INVALID_ARG, "null argument");
   CKR(log_state(lg, true));
@@ -5184,6 +5386,127 @@ int cco_event_log_info(const cco_event_log_t *lg, cco_event_log_info_t *out) {
   return CCO_OK;
 }
 
+namespace cco {
+// the entries [0, n) of one key column (entry e's key: key2[2 e] < n_keys) grouped by key, gated entries (gate[e] < 0)
+// left out: the keys with >= need entries (counting; duplicates count) or every key met, numbered by their first entry
+// -> rank[key] (-1: not numbered), id[e] (-1: gated or not numbered), the keys in dictionary order (tb->first_sorted, as
+// str_dictionary reads it: the heap's strings are indexed by key)
+static int key_group(cco_ctx *c, Arena &ar, long long n, const uint32_t *key2, long long n_keys, const int32_t *gate, bool counting,
+                     uint32_t need, StrTable *tb, int32_t *rank, int32_t *id) {
+  cudaStream_t s = c->stream;
+  uint32_t *first, *count = nullptr, *flag, *pos;
+  CKR(ar.alloc(&first, std::max<long long>(n_keys, 1)));
+  CK(cudaMemsetAsync(first, 0xff, sizeof(uint32_t) * (size_t)n_keys, s));
+  if (counting) {
+    CKR(ar.alloc(&count, std::max<long long>(n_keys, 1)));
+    CK(cudaMemsetAsync(count, 0, sizeof(uint32_t) * (size_t)n_keys, s));
+  }
+  CK(cudaMemsetAsync(rank, 0xff, sizeof(int32_t) * (size_t)n_keys, s));
+  if (n > 0) {
+    k_intern_first_count<<<grid_for(n, 256, c->sm_count), 256, 0, s>>>(n, key2, gate, first, count);
+    c->launches++;
+  }
+  CKR(ar.alloc(&flag, n_keys + 1));
+  CKR(ar.alloc(&pos, n_keys + 1));
+  CK(cudaMemsetAsync(flag + n_keys, 0, 4, s));
+  if (n_keys > 0) {
+    k_str_flags<<<grid_for(n_keys, 256, c->sm_count), 256, 0, s>>>(n_keys, first, count, need, flag);   // first: kStrEmpty = no entry
+    c->launches++;
+  }
+  CKR(exclusive_sum(c, ar, flag, pos, n_keys + 1));
+  uint32_t ng = 0;
+  CKR(mail_fetch(c, &ng, pos + n_keys, 4));
+  CKR(mail_wait(c));
+  tb->n_groups = ng;
+  if (ng > 0) {
+    uint32_t *k0, *v0;
+    CKR(ar.alloc(&k0, ng));
+    CKR(ar.alloc(&v0, ng));
+    k_str_compact<<<grid_for(n_keys, 256, c->sm_count), 256, 0, s>>>(n_keys, flag, pos, first, k0, v0);
+    c->launches++;
+    CKR(sort_pairs(c, ar, ng, &k0, &v0, bits_for(n)));   // first entries are distinct: the sort by them is the dictionary order
+    k_str_rank<<<grid_for(ng, 256, c->sm_count), 256, 0, s>>>(ng, v0, rank);
+    c->launches++;
+    ar.release(k0);
+    tb->first_sorted = v0;
+  }
+  if (n > 0) {
+    k_intern_ids<<<grid_for(n, 256, c->sm_count), 256, 0, s>>>(n, key2, gate, rank, id);
+    c->launches++;
+  }
+  ar.release(first);
+  ar.release(count);
+  ar.release(flag);
+  ar.release(pos);
+  return CCO_OK;
+}
+// cco_event_log_ingest on an interned log: ingest_strings_core's rules over the entries' keys, integer passes only; the
+// dictionaries are the heaps' strings gathered in dictionary order
+static int ingest_keys_core(cco_ctx *c, const cco_event_log *lg, const std::vector<int> &codes, int32_t min_events_per_user, cco_dataset **out) {
+  CK(cudaSetDevice(c->device));
+  cudaStream_t s = c->stream;
+  NvtxRange nvtx("cco:ingest_keys");
+  mail_reset(c);
+  Arena ar(s);
+  const int n_types = (int)codes.size();
+  cco_dataset *d = ingest_dataset_new(c, n_types);
+  d->dicts.assign((size_t)n_types + 1, cco_dictionary_t{0, nullptr, nullptr});
+  struct G {
+    cco_dataset *d;
+    bool ok = false;
+    ~G() {
+      if (!ok) {
+        cudaStreamSynchronize(d->ctx->stream);   // no dictionary copy still writes the pinned buffers released here
+        dataset_release(d);
+      }
+    }
+  } g{d};
+  const uint32_t need = min_events_per_user > 1 ? (uint32_t)min_events_per_user : 1u;
+  const long long NU = lg->users.n, NI = lg->items.n;
+  int32_t *urank, *irank;
+  CKR(ar.alloc(&urank, std::max<long long>(NU, 1)));
+  CKR(ar.alloc(&irank, std::max<long long>(NI, 1)));
+  uint32_t n_users = 0;
+  for (int t = 0; t < n_types; ++t) {
+    const int gc = codes[t];
+    const long long ne = gc >= 0 ? lg->n_train[gc] : 0;
+    // entry e's item key at k2[2 e], its user key at k2[2 e + 1]
+    const uint32_t *k2 = ne > 0 ? (const uint32_t *)(lg->tkey + lg->train_at[gc]) : nullptr;
+    int32_t *uid, *iid;
+    CKR(ar.alloc(&uid, std::max<long long>(ne, 1)));
+    CKR(ar.alloc(&iid, std::max<long long>(ne, 1)));
+    if (t == 0) {
+      // user dictionary: primary users with >= need events (duplicates count, Preparator.scala:129-132), first appearance order
+      StrTable ut;
+      CKR(key_group(c, ar, ne, k2 ? k2 + 1 : nullptr, NU, nullptr, true, need, &ut, urank, uid));
+      if (ut.n_groups >= 0x7fffffffLL) return set_error(CCO_E_UNSUPPORTED, "%lld users: the user space must stay < 2^31 - 1", ut.n_groups);
+      n_users = (uint32_t)ut.n_groups;
+      d->n_users = n_users;
+      CKR(str_dictionary(c, ar, lg->users.heap(), ut, &d->dicts[0]));
+      ar.release(ut.first_sorted);
+    } else if (ne > 0) {
+      // secondary events of users outside the dictionary are dropped (Preparator.scala:175-178)
+      k_intern_ids<<<grid_for(ne, 256, c->sm_count), 256, 0, s>>>(ne, k2 + 1, nullptr, urank, uid);
+      c->launches++;
+    }
+    // item dictionary of type t: items with a surviving event, ordered by first surviving appearance
+    StrTable it;
+    CKR(key_group(c, ar, ne, k2, NI, uid, false, 0, &it, irank, iid));
+    if (it.n_groups >= 0x7ffffffeLL) return set_error(CCO_E_UNSUPPORTED, "type %d: %lld items, at most 2^31 - 2", t, it.n_groups);
+    d->n_cols[t] = it.n_groups;
+    CKR(str_dictionary(c, ar, lg->items.heap(), it, &d->dicts[1 + t]));
+    ar.release(it.first_sorted);
+    CKR(ingest_ids_csr(c, ar, d, t, ne, n_users, uid, iid));
+  }
+  CKR(ingest_blocks(c, d, n_users));
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  g.ok = true;
+  *out = d;
+  return CCO_OK;
+}
+}  // namespace cco
+
 int cco_event_log_ingest(cco_ctx_t *c, const cco_event_log_t *lg, int32_t n_names, const char *const *names, int32_t min_events_per_user,
                          cco_dataset_t **out) {
   if (!c || !lg || !names || !out || n_names < 1) return set_error(CCO_E_INVALID_ARG, "bad argument");
@@ -5195,6 +5518,7 @@ int cco_event_log_ingest(cco_ctx_t *c, const cco_event_log_t *lg, int32_t n_name
     if (!names[t]) return set_error(CCO_E_INVALID_ARG, "null event name %d", t);
     codes[t] = lg->code_of(names[t]);
   }
+  if (lg->intern) return ingest_keys_core(c, lg, codes, min_events_per_user, out);
   const StrColumns view = [lg, &codes](Arena &ar, int t, DevStrCol *uc, DevStrCol *ic) -> int {
     const int g = codes[t];
     const long long n = g >= 0 ? lg->n_train[g] : 0;
@@ -5842,10 +6166,13 @@ static int uq_every_user(cco_ctx *c, Arena &ar, const cco_event_log *lg, const U
 }  // namespace cco
 
 int cco_event_log_begin_ex(cco_ctx_t *ctx, int64_t chunk_bytes, const cco_event_window_t *w, uint32_t flags, cco_event_log_t **out) {
-  if (flags & ~(uint32_t)(CCO_LOG_KEEP_HISTORY | CCO_LOG_EXTENDABLE)) return set_error(CCO_E_INVALID_ARG, "unknown flags 0x%x", (unsigned)flags);
+  if (flags & ~(uint32_t)(CCO_LOG_KEEP_HISTORY | CCO_LOG_EXTENDABLE | CCO_LOG_INTERN_IDS))
+    return set_error(CCO_E_INVALID_ARG, "unknown flags 0x%x", (unsigned)flags);
   CKR(cco_event_log_begin_window(ctx, chunk_bytes, w, out));
   (*out)->history = (flags & CCO_LOG_KEEP_HISTORY) != 0;
   (*out)->extendable = (flags & CCO_LOG_EXTENDABLE) != 0;
+  (*out)->intern = (flags & CCO_LOG_INTERN_IDS) != 0;
+  (*out)->intern_mask = ctx->intern_mask;
   return CCO_OK;
 }
 
@@ -7077,6 +7404,12 @@ int cco_debug_key_range_cap(cco_ctx_t *c, int32_t max_keys) {
   if (!c || max_keys < 0) return set_error(CCO_E_INVALID_ARG, "null context or negative cap");
   c->key_range_cap = max_keys;
   for (cco_ctx *m : c->members) m->key_range_cap = max_keys;
+  return CCO_OK;
+}
+
+int cco_debug_intern_hash_bits(cco_ctx_t *c, int32_t bits) {
+  if (!c || bits < 0 || bits > 64) return set_error(CCO_E_INVALID_ARG, "null context or hash bits %d not in [0, 64]", bits);
+  c->intern_mask = bits == 64 ? ~0ULL : (1ULL << bits) - 1;
   return CCO_OK;
 }
 

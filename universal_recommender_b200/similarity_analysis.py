@@ -360,7 +360,8 @@ class CcoContext:
         return rk
 
     def read_events(self, src, chunk_bytes: Optional[int] = None, window: Optional[E.EventWindow] = None,
-                    now_ms: Optional[int] = None, keep_history: bool = False, extendable: bool = False) -> "EventLog":
+                    now_ms: Optional[int] = None, keep_history: bool = False, extendable: bool = False,
+                    intern_ids: bool = False) -> "EventLog":
         """A PredictionIO event export (JSON lines, as `pio export` writes them) parsed on the device.  src is one of
           - bytes or a buffer: one read (cco_event_log_read), or chunks of chunk_bytes when it is given;
           - a file path, a directory as `pio export` writes it (its part-* files in name order; events.export_parts) or a
@@ -377,9 +378,12 @@ class CcoContext:
         user_queries reads; a log read without it is exactly the log read before the option existed.
         extendable: keep what EventLog.extend needs to take new lines and a later cutoff without a re-read
         (cco_event_log_begin_ex, CCO_LOG_EXTENDABLE); the device staging of later extends is this read's chunk_bytes.
+        intern_ids: give every distinct user and item id of the training events a 32-bit key as the lines are read
+        (cco_event_log_begin_ex, CCO_LOG_INTERN_IDS), so that ingest_event_log (and calc_all_from_events) groups keys, not
+        strings, with the same result; an extend interns only its new lines.
         -> EventLog (free with .free(), or use it as a context manager; close() of this context frees the logs still open)."""
         whole = isinstance(src, (bytes, bytearray, memoryview, np.ndarray)) and chunk_bytes is None
-        if whole and window is None and not keep_history and not extendable:
+        if whole and window is None and not keep_history and not extendable and not intern_ids:
             buf = np.frombuffer(src, dtype=np.uint8) if not isinstance(src, np.ndarray) else np.ascontiguousarray(src, dtype=np.uint8)
             h = C.c_void_p()
             N.check(self._L.cco_event_log_read(self._h, buf.ctypes.data if len(buf) else None, len(buf), C.byref(h)))
@@ -387,7 +391,8 @@ class CcoContext:
         chunk = int(chunk_bytes or (max(memoryview(src).nbytes, 1) if whole else DEFAULT_CHUNK_BYTES))
         h = C.c_void_p()
         w = _window_t(window, now_ms)
-        flags = (N.LOG_KEEP_HISTORY if keep_history else 0) | (N.LOG_EXTENDABLE if extendable else 0)
+        flags = ((N.LOG_KEEP_HISTORY if keep_history else 0) | (N.LOG_EXTENDABLE if extendable else 0)
+                 | (N.LOG_INTERN_IDS if intern_ids else 0))
         if flags:
             N.check(self._L.cco_event_log_begin_ex(self._h, chunk, C.byref(w) if w is not None else None, flags, C.byref(h)))
         elif w is None:
@@ -484,7 +489,8 @@ class CcoContext:
                 self.host_free(b)
 
     def ingest_event_log(self, log: "EventLog", names: Sequence[str], min_events_per_user: int = 0):
-        """cco_event_log_ingest: ingest_strings on the log's training events of `names` (type t = names[t]), from HBM.
+        """cco_event_log_ingest: ingest_strings on the log's training events of `names` (type t = names[t]), from HBM; on a
+        log read with intern_ids=True it groups the ids' keys instead, with the same result.
         -> (dataset, user ids, [item ids per type]) as ingest_strings"""
         nm = (C.c_char_p * len(names))(*[x.encode("utf-8") for x in names])
         ds = C.c_void_p()
@@ -1118,6 +1124,11 @@ class CcoContext:
         packed word fits and without FLAG_KEY_RANGES (0 = off); last_key_ranges shows the ranges a train ran in."""
         N.check(self._L.cco_debug_key_range_cap(self._h, int(max_keys)))
 
+    def debug_intern_hash_bits(self, bits: int):
+        """Tests only: truncate the intern hash of the logs read_events(intern_ids=True) begins from now on to `bits` bits
+        (64 = off), so that ids collide in the intern tables and are told apart by their bytes."""
+        N.check(self._L.cco_debug_intern_hash_bits(self._h, int(bits)))
+
 
 class IndexWrite:
     """CcoContext.index_write(body): the model index body on the device for one write.  fields() -> esFields (the names
@@ -1365,6 +1376,13 @@ class EventLog:
         N.check(self._ctx._L.cco_event_log_extend(self._h, C.byref(w) if w is not None else None))
         self._ctx._append_finish(self._h, src, int(chunk_bytes or DEFAULT_CHUNK_BYTES), n_lines)
         return self
+
+    def intern_stats(self) -> tuple[int, int]:
+        """cco_event_log_intern_stats: (user keys, item keys) of a log read with intern_ids=True -- the distinct ids of its
+        retained training events"""
+        u, i = C.c_int64(), C.c_int64()
+        N.check(self._ctx._L.cco_event_log_intern_stats(self._h, C.byref(u), C.byref(i)))
+        return u.value, i.value
 
     def resident_bytes(self) -> int:
         """cco_event_log_resident_bytes: the device bytes the finished log holds"""
