@@ -4,6 +4,7 @@ import numpy as np
 import pytest
 
 import universal_recommender_b200 as ur
+from test_gpu_parity import assert_llr_close
 
 pytestmark = pytest.mark.gpu
 
@@ -30,9 +31,9 @@ def test_ingest_matches_oracle(orc, ctx, min_ev):
     params = [(500, 20, None)] * 3
     got = ctx.train_dataset(ds, params, seed=9, flags=ur.FLAG_ASSUME_CANONICAL)
     ref = orc.train(mats, [orc.Params(*p) for p in params], 9)
-    for g, r in zip(got, ref):
+    for i, (g, r) in enumerate(zip(got, ref)):
         assert np.array_equal(g[3], r.row_ptr) and np.array_equal(g[4], r.col_idx) and np.array_equal(g[6], r.count)
-        assert np.allclose(g[5], r.llr, rtol=1e-6, atol=0)
+        assert_llr_close(g[5], r.llr, mats[0].n_rows, f"indicator {i}")
     ctx.free_dataset(ds)
 
 

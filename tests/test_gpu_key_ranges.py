@@ -144,7 +144,7 @@ def test_cap_splits_a_run_of_equal_colb_with_the_cut_on_a_tie(capped, orc):
         _, _, _, rp, ci, ll, _ = got[1]
         assert list(ci[rp[0]:rp[1]]) == [0, 1, 2, 3, 4, 5]
         assert len(set(ll[rp[0]:rp[1]].tolist())) == 1
-    assert_indicators_equal(oracle_train(orc, [a, b], params, 1), got, "tie run")
+    assert_indicators_equal(oracle_train(orc, [a, b], params, 1), got, a[0], "tie run")
 
 
 def test_forced_ranges_golden_fixtures(capped):
@@ -243,7 +243,7 @@ def _check_past_limit(orc, ctx, mats, params, seed, want_ranges, tag, brute=True
     if brute:
         rowref.assert_matches(rowref.expected(ctx, mats, params, seed), got, tag)
     ref = oracle_train(orc, mats, params, seed)
-    assert_indicators_equal(ref, got, tag)
+    assert_indicators_equal(ref, got, mats[0][0], tag)
     assert ctx.last_stats.products == [r.products for r in ref] and ctx.last_stats.distinct_cells == [r.distinct_cells for r in ref]
     return got
 

@@ -36,7 +36,7 @@ def run(orc, ctx, mats, params, seed=1, flags=0, tag=""):
     got = ctx.train_csr(mats, params, seed=seed, flags=flags)
     exp = rowref.expected(ctx, mats, params, seed, flags)
     rowref.assert_matches(exp, got, tag)
-    assert_indicators_equal(oracle_train(orc, mats, params, seed, flags & 3), got, tag)
+    assert_indicators_equal(oracle_train(orc, mats, params, seed, flags & 3), got, mats[0][0], tag)
     assert ctx.last_stats.distinct_cells == [e.distinct for e in exp]
     paths = [e.paths() for e in exp]
     for ps in paths:

@@ -4,12 +4,13 @@ The cut and the filter rely on the LLR being monotone in colB and k11.  The real
 not, once adjacent colB values are closer than the evaluation error.  These tests pin instances of that (with the
 oracle's own evaluation order and glibc log), show with 50-digit arithmetic that the real values are monotone there,
 and check that the host's exactness test (cco_api.cu cut_exact) rejects those shapes and accepts C3 and C4."""
-from decimal import Decimal, getcontext
+from decimal import Decimal
 
 import numpy as np
 import pytest
 
 import row_paths as rp
+from llr_exact import cut_c_max, llr_exact
 
 
 # ---- the path model ---------------------------------------------------------------------------------------------------
@@ -80,17 +81,6 @@ def llr_k1(orc, n, ra, cb, k=1):
     return orc.llr(k, ra - k, cb - k, n - ra - cb + k)
 
 
-def llr_exact(n, ra, cb, k=1):
-    """The real LLR, 50 significant digits."""
-    getcontext().prec = 50
-    xl = lambda x: Decimal(0) if x == 0 else Decimal(x) * Decimal(x).ln()
-    k12, k21, k22 = ra - k, cb - k, n - ra - cb + k
-    row = xl(n) - xl(k + k12) - xl(k21 + k22)
-    col = xl(n) - xl(k + k21) - xl(k12 + k22)
-    mat = xl(n) - xl(k) - xl(k12) - xl(k21) - xl(k22)
-    return 2 * (row + col - mat)
-
-
 def test_key_cut_tie_instance(orc):
     # N = 2e7, rowA = 1, k11 = 1: two adjacent colB values give the same fp64 LLR; the real values differ by ~2.2e-7
     n = 20_000_000
@@ -147,14 +137,7 @@ def test_cut_exact_bound_holds_where_it_admits_the_cut(orc, n, ra):
     # the largest max colB that cut_exact admits for this rowA (on the strongly positive side): computed values
     # strictly decrease right up to it
     eps = rp.llr_error_bound(n)
-    lo, hi = 1, (n - 1) // (2 * ra) - 1
-    assert rp.cut_exact(n, ra, lo)
-    if rp.cut_exact(n, ra, hi):
-        lo = hi
-    while hi - lo > 1:                                   # cut_exact is monotone in max colB
-        mid = (lo + hi) // 2
-        lo, hi = (mid, hi) if rp.cut_exact(n, ra, mid) else (lo, mid)
-    c_max = lo
+    c_max = cut_c_max(n, ra)
     assert first_non_decreasing(orc, n, ra, max(1, c_max - 3000), c_max) is None
     # and the real gap there is above the bound's 2 eps
     assert float(llr_exact(n, ra, c_max - 1) - llr_exact(n, ra, c_max)) > 2 * eps

@@ -132,16 +132,6 @@ __device__ __forceinline__ double llr_cells(long long k11, long long k12, long l
   if (s < mat_e) return 0.0;  // round off error
   return __dmul_rn(2.0, __dsub_rn(s, mat_e));
 }
-// fused form used by the row kernel: row entropy hoisted per row (bit-identical sub-expression)
-__device__ __forceinline__ double llr_hoisted(long long k11, long long ra, long long cb, long long n, double row_e,
-                                              bool varargs) {
-  long long k12 = ra - k11, k21 = cb - k11, k22 = n - ra - cb + k11;
-  double col_e = entropy2(cb, n - cb, varargs);
-  double mat_e = entropy4(k11, k12, k21, k22, varargs);
-  double s = __dadd_rn(row_e, col_e);
-  if (s < mat_e) return 0.0;
-  return __dmul_rn(2.0, __dsub_rn(s, mat_e));
-}
 
 __global__ void k_debug_llr(long long n, const long long *k11, const long long *k12, const long long *k21,
                             const long long *k22, uint32_t flags, double *out) {
