@@ -7480,38 +7480,86 @@ int cco_debug_cooccurrence(cco_ctx_t *c, const cco_csr_t *a, const cco_csr_t *b,
   return CCO_OK;
 }
 
-// ---- cco_search_results: _msearch response bodies -> PredictedResults, kernels in cco_results.cuh ----------------------
-struct cco_search_results {
-  cco_ctx *ctx = nullptr;
-  int n_rank = 0;
-  uint32_t flags = 0;
-  std::string names, qnames;           // ranking names (UTF-8) and their json4s quotes, each followed by ':'
-  int name_off[9] = {}, qname_off[9] = {};
-  char *stage[2] = {};                 // pinned staging of the last two bodies
-  size_t stage_cap[2] = {};
-  unsigned char *dbody[2] = {};        // their device copies
-  size_t dcap[2] = {};
-  cudaEvent_t copied[2] = {};
-  long long n_bodies = 0;
-  bool pending = false;                // the last appended body is copied, not yet read
-  long long p_len = 0, p_rec = 0;
-  std::vector<uint8_t> p_ranks;        // its records' withRanks, one byte each (without query lines)
-  bool p_has_lines = false;            // its records' query lines (rebased offsets and bytes, copied at append)
-  std::vector<int64_t> p_loff;
-  std::string p_lines;
-  bool failed = false, finished = false;
-  std::string fail_msg;
-  int fail_code = CCO_OK;
-  // what the read bodies gave, records and hits numbered across bodies
-  std::vector<int64_t> hit_off{0}, total, id_off{0}, text_off{0};
-  std::vector<int32_t> status;
-  std::vector<double> score, ranks;
-  std::string id_bytes, text;
-  long long n_exact = 0;
-};
-
+// ---- what the readers of Elasticsearch responses share (search results, index pages, index write) ---------------------
 extern "C++" {
 namespace cco {
+
+// A reader's first failure, repeated by every later call but free; a finished reader refuses every call but free.
+struct ReaderLatch {
+  bool failed = false, finished = false;
+  std::string msg;
+  int code = CCO_OK;
+  int fail(int st) {
+    failed = true;
+    code = st;
+    msg = cco_last_error();
+    return st;
+  }
+  int state(const char *finished_msg) const {
+    if (failed) return set_error(code == CCO_OK ? CCO_E_INVALID_ARG : code, "%s", msg.c_str());
+    if (finished) return set_error(CCO_E_INVALID_ARG, "%s", finished_msg);
+    return CCO_OK;
+  }
+};
+
+// Response bodies on their way to the device, in one or two slots: per slot a pinned staging buffer and a device buffer,
+// each grown to the largest body so far, and the event of the copy.  A body is padded with spaces to whole 64-byte words
+// and one word more, as the structural passes read it, and copied on the copy stream.  A slot's next put reuses its
+// buffers, so the slot's last body must have been read by then.
+struct BodyStage {
+  char *pinned[2] = {};
+  size_t pinned_cap[2] = {};
+  unsigned char *dev[2] = {};
+  size_t dev_cap[2] = {};
+  cudaEvent_t copied[2] = {};
+
+  int init() {
+    for (cudaEvent_t &e : copied)
+      if (cudaEventCreateWithFlags(&e, cudaEventDisableTiming) != cudaSuccess) return set_error(CCO_E_CUDA, "cudaEventCreate failed");
+    return CCO_OK;
+  }
+  // what names the body in a refusal ("page 3 of 812 bytes"), copy_of in a failed copy ("page 3")
+  int put(cco_ctx *c, int slot, const char *bytes, long long len, const char *what, const char *copy_of) {
+    const size_t padded = (size_t)((len + 63) / 64 * 64) + 64;
+    size_t free_b = 0, total_b = 0;
+    CK(cudaMemGetInfo(&free_b, &total_b));
+    if (padded > total_b / 4) return set_error(CCO_E_UNSUPPORTED, "%s: at most a quarter of the device's memory", what);
+    if (pinned_cap[slot] < padded) {
+      if (pinned[slot]) cudaFreeHost(pinned[slot]);
+      pinned[slot] = nullptr;
+      pinned_cap[slot] = 0;
+      if (cudaHostAlloc((void **)&pinned[slot], padded, cudaHostAllocPortable) != cudaSuccess)
+        return set_error(CCO_E_OOM, "cudaHostAlloc(%zu) failed", padded);
+      pinned_cap[slot] = padded;
+    }
+    if (dev_cap[slot] < padded) {
+      if (dev[slot]) cudaFree(dev[slot]);
+      dev[slot] = nullptr;
+      dev_cap[slot] = 0;
+      if (cudaMalloc((void **)&dev[slot], padded) != cudaSuccess) return set_error(CCO_E_UNSUPPORTED, "%s does not fit the device", what);
+      dev_cap[slot] = padded;
+    }
+    if (len > 0) memcpy(pinned[slot], bytes, (size_t)len);
+    memset(pinned[slot] + len, ' ', padded - (size_t)len);
+    if (cudaMemcpyAsync(dev[slot], pinned[slot], padded, cudaMemcpyHostToDevice, c->copy_stream) != cudaSuccess ||
+        cudaEventRecord(copied[slot], c->copy_stream) != cudaSuccess)
+      return set_error(CCO_E_CUDA, "the copy of %s failed", copy_of);
+    return CCO_OK;
+  }
+  int wait(cudaStream_t s, int slot) const {
+    CK(cudaStreamWaitEvent(s, copied[slot], 0));
+    return CCO_OK;
+  }
+  const char *host(int slot) const { return pinned[slot]; }
+  void release(cco_ctx *c) {
+    cudaStreamSynchronize(c->copy_stream);
+    for (int i = 0; i < 2; ++i) {
+      if (pinned[i]) cudaFreeHost(pinned[i]);
+      if (dev[i]) cudaFree(dev[i]);
+      if (copied[i]) cudaEventDestroy(copied[i]);
+    }
+  }
+};
 
 static const char *sr_message(int code) {
   switch (code) {
@@ -7531,9 +7579,161 @@ static const char *sr_message(int code) {
     case kSrWithRanks: return "the query line's withRanks is not true, false or null";
     case kSrLineRepeated: return "the query line repeats withRanks";
     case kSrLineDeep: return "the query line nests deeper than 64 levels";
+    case kSrOpenString: return "a string is not closed";
+    case kSrNotObject: return "the top level is not an object";
+    case kSrEsError: return "Elasticsearch returned an error";
+    case kSrRepeatedId: return "a repeated _id";
+    case kIpTimedOut: return "the search timed out (timed_out is true)";
+    case kIpShards: return "_shards.failed is not 0";
+    case kIpHitsNotArray: return "hits.hits is neither an array nor absent";
+    case kIpNoSource: return "the hit has no _source";
+    case kIpSourceNotObject: return "_source is not an object";
+    case kIwNoItems: return "the response has no \"items\" array";
+    case kIwItemNotObject: return "an items element is not an object";
+    case kIwNotIndex: return "the item is not {\"index\":{...}}";
+    case kIwNoId: return "the item has no string _id";
+    case kIwIdMismatch: return "the item's _id is not the document's _id";
+    case kIwNoStatus: return "the item has no status";
+    case kIwRepeatedStatus: return "a repeated status";
+    case kIwBadStatus: return "the status is not a 32-bit integer";
   }
   return "malformed response";
 }
+
+// The structural index of a body on the device, padded as BodyStage pads it: the byte positions pos[m] and depths dep[m]
+// (in ar) of the entries at depth <= max_depth.  *bad = ~0, or (byte offset << 8 | kSr* code) of a malformed body.  The
+// passes' scratch is released before it returns.
+struct SrIndex {
+  long long *pos = nullptr;
+  unsigned char *dep = nullptr;
+  long long m = 0;
+};
+static int sr_index(cco_ctx *c, Arena &ar, const unsigned char *body, long long len, int max_depth, SrIndex *ix, unsigned long long *bad) {
+  cudaStream_t s = c->stream;
+  const long long NW = (len + 63) / 64, n_chunks = (NW + kSrChunkWords - 1) / kSrChunkWords;
+  unsigned long long *err;
+  SrFun *fun, *pre;
+  long long *cnt, *coff;
+  CKR(ar.alloc(&err, 1));
+  CKR(ar.alloc(&fun, n_chunks + 1));
+  CKR(ar.alloc(&pre, n_chunks + 1));
+  CKR(ar.alloc(&cnt, n_chunks + 1));
+  CKR(ar.alloc(&coff, n_chunks + 1));
+  CK(cudaMemsetAsync(err, 0xff, 8, s));
+  CK(cudaMemsetAsync(cnt + n_chunks, 0, 8, s));
+  SrFun fin = sr_identity();
+  if (n_chunks > 0) {
+    const int grid = grid_for(n_chunks * 32, 256, c->sm_count);
+    k_sr_chunk<<<grid, 256, 0, s>>>(NW, (const uint4 *)body, fun);
+    k_sr_scan<<<1, kSrScanThreads, 0, s>>>(n_chunks, fun, pre);
+    k_sr_index<false><<<grid, 256, 0, s>>>(NW, (const uint4 *)body, pre, max_depth, cnt, nullptr, nullptr, nullptr, err);
+    c->launches += 3;
+    CKR(mail_fetch(c, &fin, pre + n_chunks - 1, sizeof(SrFun)));
+  }
+  CKR(exclusive_sum(c, ar, cnt, coff, n_chunks + 1));
+  ix->m = 0;
+  *bad = ~0ULL;
+  CKR(mail_fetch(c, &ix->m, coff + n_chunks, 8));
+  CKR(mail_fetch(c, bad, err, 8));
+  CKR(mail_wait(c));
+  if (*bad == ~0ULL && (fin.f[0] >> 1)) *bad = (unsigned long long)len << 8 | kSrOpenString;
+  if (*bad == ~0ULL && fin.d[0] != 0) *bad = (unsigned long long)len << 8 | kSrUnbalanced;
+  if (*bad == ~0ULL) {
+    CKR(ar.alloc(&ix->pos, ix->m + 1));
+    CKR(ar.alloc(&ix->dep, ix->m + 1));
+    if (ix->m > 0) {
+      k_sr_index<true><<<grid_for(n_chunks * 32, 256, c->sm_count), 256, 0, s>>>(NW, (const uint4 *)body, pre, max_depth, nullptr, coff, ix->pos,
+                                                                                  ix->dep, err);
+      c->launches++;
+    }
+  }
+  for (void *p : {(void *)err, (void *)fun, (void *)pre, (void *)cnt, (void *)coff}) ar.release(p);
+  return CCO_OK;
+}
+
+// A buffer of n bytes from the context's pinned pool for the caller, who frees it with cco_host_free: a copy of src, or
+// left for the caller to fill when src is null.
+template <typename T>
+static int pinned_give(cco_ctx *c, T **out, const void *src, size_t n) {
+  *out = (T *)c->pinned_get(std::max<size_t>(n, 1), /*for_result=*/false);
+  if (!*out) return set_error(CCO_E_OOM, "pinned host allocation failed");
+  if (src && n) memcpy(*out, src, n);
+  return CCO_OK;
+}
+
+// a valid raw JSON string as UTF-8, a surrogate that is not part of a pair in its 3-byte form (k_json_unescape's rules)
+static std::string sr_unescape(const char *p, long long n) {
+  std::string o;
+  auto hex4 = [](const char *q) { return (unsigned)strtoul(std::string(q, 4).c_str(), nullptr, 16); };
+  for (long long i = 0; i < n;) {
+    if (p[i] != '\\') {
+      o += p[i++];
+      continue;
+    }
+    const char x = p[i + 1];
+    if (x != 'u') {
+      o += x == 'b' ? '\b' : x == 'f' ? '\f' : x == 'n' ? '\n' : x == 'r' ? '\r' : x == 't' ? '\t' : x;
+      i += 2;
+      continue;
+    }
+    unsigned cp = hex4(p + i + 2);
+    i += 6;
+    if (cp >= 0xd800 && cp < 0xdc00 && i + 6 <= n && p[i] == '\\' && p[i + 1] == 'u') {
+      const unsigned lo = hex4(p + i + 2);
+      if (lo >= 0xdc00 && lo < 0xe000) {
+        cp = 0x10000 + ((cp - 0xd800) << 10) + (lo - 0xdc00);
+        i += 6;
+      }
+    }
+    if (cp < 0x80) {
+      o += (char)cp;
+    } else if (cp < 0x800) {
+      o += (char)(0xc0 | cp >> 6);
+      o += (char)(0x80 | (cp & 0x3f));
+    } else if (cp < 0x10000) {
+      o += (char)(0xe0 | cp >> 12);
+      o += (char)(0x80 | (cp >> 6 & 0x3f));
+      o += (char)(0x80 | (cp & 0x3f));
+    } else {
+      o += (char)(0xf0 | cp >> 18);
+      o += (char)(0x80 | (cp >> 12 & 0x3f));
+      o += (char)(0x80 | (cp >> 6 & 0x3f));
+      o += (char)(0x80 | (cp & 0x3f));
+    }
+  }
+  return o;
+}
+
+}  // namespace cco
+}  // extern "C++"
+
+// ---- cco_search_results: _msearch response bodies -> PredictedResults, kernels in cco_results.cuh ----------------------
+struct cco_search_results {
+  cco_ctx *ctx = nullptr;
+  int n_rank = 0;
+  uint32_t flags = 0;
+  std::string names, qnames;           // ranking names (UTF-8) and their json4s quotes, each followed by ':'
+  int name_off[9] = {}, qname_off[9] = {};
+  BodyStage stage;                     // the last two bodies
+  long long n_bodies = 0;
+  bool pending = false;                // the last appended body is copied, not yet read
+  long long p_len = 0, p_rec = 0;
+  std::vector<uint8_t> p_ranks;        // its records' withRanks, one byte each (without query lines)
+  bool p_has_lines = false;            // its records' query lines (rebased offsets and bytes, copied at append)
+  std::vector<int64_t> p_loff;
+  std::string p_lines;
+  ReaderLatch latch;
+  // what the read bodies gave, records and hits numbered across bodies
+  std::vector<int64_t> hit_off{0}, total, id_off{0}, text_off{0};
+  std::vector<int32_t> status;
+  std::vector<double> score, ranks;
+  std::string id_bytes, text;
+  long long n_exact = 0;
+};
+
+extern "C++" {
+namespace cco {
+
 static int sr_count_check(long long n, const char *what) {
   if (n >= (1LL << 31)) return set_error(CCO_E_UNSUPPORTED, "%lld %s in one body: at most 2^31 - 1", n, what);
   return CCO_OK;
@@ -7570,6 +7770,13 @@ static int sr_exact_value(const char *t, long long n, SrNum *o) {
   *o = r;
   return 0;
 }
+// the exact path's spans [b, e) of text converted into val -> the first entry out of the range of a double, or -1
+static long long sr_exact_values(const char *text, const std::vector<SrExact> &xs, std::vector<SrNum> &val) {
+  val.resize(xs.size());
+  for (size_t i = 0; i < xs.size(); ++i)
+    if (sr_exact_value(text + xs[i].b, xs[i].e - xs[i].b, &val[i])) return (long long)i;
+  return -1;
+}
 template <typename T>
 static void sr_append(std::vector<T> &dst, const T *src, long long n, T delta = T()) {
   const size_t at = dst.size();
@@ -7603,53 +7810,24 @@ static int sr_read(cco_search_results *h) {
   const int slot = (int)((h->n_bodies - 1) & 1);
   const long long len = h->p_len, body_no = h->n_bodies - 1, rec_base = (long long)h->status.size(),
                   hit_base = h->hit_off.back();
-  const unsigned char *body = h->dbody[slot];
-  const char *hbody = h->stage[slot];
-  CK(cudaStreamWaitEvent(s, h->copied[slot], 0));
+  const unsigned char *body = h->stage.dev[slot];
+  const char *hbody = h->stage.host(slot);
+  CKR(h->stage.wait(s, slot));
   mail_reset(c);   // every fetch below is waited for before the next body
   Arena ar(s);
   NvtxRange nvtx("cco:search_results");
   auto byte_error = [&](unsigned long long e) {
     return set_error(CCO_E_INVALID_ARG, "response body %lld, byte %lld: %s", body_no, (long long)(e >> 8), sr_message((int)(e & 0xff)));
   };
-  // the structural index
-  const long long NW = (len + 63) / 64, n_chunks = (NW + kSrChunkWords - 1) / kSrChunkWords;
+  SrIndex ix;
+  unsigned long long e0 = ~0ULL;
+  CKR(sr_index(c, ar, body, len, kSrMaxDepth, &ix, &e0));
+  if (e0 != ~0ULL) return byte_error(e0);
+  const long long m = ix.m, *pos = ix.pos;
+  const unsigned char *dep = ix.dep;
   unsigned long long *err;
   CKR(ar.alloc(&err, 4));
   CK(cudaMemsetAsync(err, 0xff, 32, s));
-  SrFun *fun, *pre;
-  long long *cnt, *coff;
-  CKR(ar.alloc(&fun, n_chunks + 1));
-  CKR(ar.alloc(&pre, n_chunks + 1));
-  CKR(ar.alloc(&cnt, n_chunks + 1));
-  CKR(ar.alloc(&coff, n_chunks + 1));
-  CK(cudaMemsetAsync(cnt + n_chunks, 0, 8, s));
-  SrFun fin = sr_identity();
-  long long m = 0;
-  if (n_chunks > 0) {
-    const int grid = grid_for(n_chunks * 32, 256, c->sm_count);
-    k_sr_chunk<<<grid, 256, 0, s>>>(NW, (const uint4 *)body, fun);
-    k_sr_scan<<<1, kSrScanThreads, 0, s>>>(n_chunks, fun, pre);
-    k_sr_index<false><<<grid, 256, 0, s>>>(NW, (const uint4 *)body, pre, kSrMaxDepth, cnt, nullptr, nullptr, nullptr, err);
-    c->launches += 3;
-    CKR(mail_fetch(c, &fin, pre + n_chunks - 1, sizeof(SrFun)));
-  }
-  CKR(exclusive_sum(c, ar, cnt, coff, n_chunks + 1));
-  unsigned long long e0 = ~0ULL;
-  CKR(mail_fetch(c, &m, coff + n_chunks, 8));
-  CKR(mail_fetch(c, &e0, err, 8));
-  CKR(mail_wait(c));
-  if (e0 != ~0ULL) return byte_error(e0);
-  if (fin.f[0] >> 1) return set_error(CCO_E_INVALID_ARG, "response body %lld, byte %lld: %s", body_no, len, "a string is not closed");
-  if (fin.d[0] != 0) return set_error(CCO_E_INVALID_ARG, "response body %lld, byte %lld: %s", body_no, len, sr_message(kSrUnbalanced));
-  long long *pos;
-  unsigned char *dep;
-  CKR(ar.alloc(&pos, m + 1));
-  CKR(ar.alloc(&dep, m + 1));
-  if (m > 0) {
-    k_sr_index<true><<<grid_for(n_chunks * 32, 256, c->sm_count), 256, 0, s>>>(NW, (const uint4 *)body, pre, kSrMaxDepth, nullptr, coff, pos, dep, err);
-    c->launches++;
-  }
   // the top level and the responses array
   long long *top, nt = 0, ends[2] = {-1, -1}, *d_ends;
   CKR(sr_select(c, ar, m, dep, 0, 1, -1, m, &top, &nt));
@@ -7710,16 +7888,16 @@ static int sr_read(cco_search_results *h) {
       CK(cudaMemcpyAsync(xs.data(), lx, sizeof(SrExact) * (size_t)nx, cudaMemcpyDeviceToHost, s));
       CK(cudaStreamSynchronize(s));
       std::sort(xs.begin(), xs.end(), [](const SrExact &x, const SrExact &y) { return x.b < y.b; });
-      std::vector<long long> xpos((size_t)nx);
-      std::vector<SrNum> xval((size_t)nx);
-      for (size_t i = 0; i < xs.size(); ++i) {
-        xpos[i] = xs[i].b;
-        if (sr_exact_value(h->p_lines.data() + xs[i].b, xs[i].e - xs[i].b, &xval[i])) {
-          const long long r = (long long)(std::upper_bound(h->p_loff.begin(), h->p_loff.end(), (int64_t)xs[i].b) - h->p_loff.begin()) - 1;
-          return set_error(CCO_E_INVALID_ARG, "record %lld: the query line's %.*s is out of the range of a double", rec_base + r,
-                           (int)std::min<long long>(xs[i].e - xs[i].b, 64), h->p_lines.data() + xs[i].b);
-        }
+      std::vector<SrNum> xval;
+      const long long bad = sr_exact_values(h->p_lines.data(), xs, xval);
+      if (bad >= 0) {
+        const SrExact &x = xs[(size_t)bad];
+        const long long r = (long long)(std::upper_bound(h->p_loff.begin(), h->p_loff.end(), (int64_t)x.b) - h->p_loff.begin()) - 1;
+        return set_error(CCO_E_INVALID_ARG, "record %lld: the query line's %.*s is out of the range of a double", rec_base + r,
+                         (int)std::min<long long>(x.e - x.b, 64), h->p_lines.data() + x.b);
       }
+      std::vector<long long> xpos((size_t)nx);
+      for (size_t i = 0; i < xs.size(); ++i) xpos[i] = xs[i].b;
       long long *d_xpos;
       SrNum *d_xval;
       CKR(ar.alloc(&d_xpos, (long long)nx));
@@ -7813,16 +7991,15 @@ static int sr_read(cco_search_results *h) {
     std::vector<SrExact> xs((size_t)nx);
     CK(cudaMemcpyAsync(xs.data(), xl, sizeof(SrExact) * (size_t)nx, cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
-    std::vector<long long> slot_h((size_t)nx);
-    std::vector<SrNum> val((size_t)nx);
-    for (size_t i = 0; i < xs.size(); ++i) {
-      slot_h[i] = xs[i].slot;
-      if (sr_exact_value(hbody + xs[i].b, xs[i].e - xs[i].b, &val[i])) {
-        hit_where(xs[i].slot < n_hits ? xs[i].slot : (xs[i].slot - n_hits) / std::max(h->n_rank, 1), where, sizeof where);
-        return set_error(CCO_E_INVALID_ARG, "%s: %.*s is out of the range of a double", where, (int)std::min<long long>(xs[i].e - xs[i].b, 64),
-                         hbody + xs[i].b);
-      }
+    std::vector<SrNum> val;
+    const long long bad = sr_exact_values(hbody, xs, val);
+    if (bad >= 0) {
+      const SrExact &x = xs[(size_t)bad];
+      hit_where(x.slot < n_hits ? x.slot : (x.slot - n_hits) / std::max(h->n_rank, 1), where, sizeof where);
+      return set_error(CCO_E_INVALID_ARG, "%s: %.*s is out of the range of a double", where, (int)std::min<long long>(x.e - x.b, 64), hbody + x.b);
     }
+    std::vector<long long> slot_h((size_t)nx);
+    for (size_t i = 0; i < xs.size(); ++i) slot_h[i] = xs[i].slot;
     long long *d_slot;
     SrNum *d_val;
     CKR(ar.alloc(&d_slot, (long long)nx));
@@ -7919,17 +8096,6 @@ static int sr_read(cco_search_results *h) {
   if (rec_off) sr_append(h->text_off, toff_h.data() + 1, n_rec, (int64_t)at_text);
   return CCO_OK;
 }
-static int sr_fail_with(cco_search_results *h, int st) {
-  h->failed = true;
-  h->fail_code = st;
-  h->fail_msg = cco_last_error();
-  return st;
-}
-static int sr_state(const cco_search_results *h) {
-  if (h->failed) return set_error(h->fail_code == CCO_OK ? CCO_E_INVALID_ARG : h->fail_code, "%s", h->fail_msg.c_str());
-  if (h->finished) return set_error(CCO_E_INVALID_ARG, "the results are finished");
-  return CCO_OK;
-}
 
 }  // namespace cco
 }  // extern "C++"
@@ -7966,11 +8132,10 @@ int cco_search_results_begin(cco_ctx_t *ctx, const cco_search_results_params_t *
     h->qnames += q;
     h->qname_off[at + 1] = (int)h->qnames.size();
   }
-  for (int i = 0; i < 2; ++i)
-    if (cudaEventCreateWithFlags(&h->copied[i], cudaEventDisableTiming) != cudaSuccess) {
-      cco_search_results_free(h);
-      return set_error(CCO_E_CUDA, "cudaEventCreate failed");
-    }
+  if (h->stage.init() != CCO_OK) {
+    cco_search_results_free(h);
+    return set_error(CCO_E_CUDA, "cudaEventCreate failed");
+  }
   *out = h;
   return CCO_OK;
 }
@@ -7978,8 +8143,8 @@ int cco_search_results_begin(cco_ctx_t *ctx, const cco_search_results_params_t *
 int cco_search_results_append(cco_search_results_t *h, const char *body, int64_t len, int64_t n_records, const int64_t *line_offsets,
                               const char *line_bytes, const uint8_t *with_ranks) {
   if (!h || len < 0 || (len > 0 && !body) || (with_ranks && n_records < 0)) return set_error(CCO_E_INVALID_ARG, "null argument or negative length");
-  CKR(sr_state(h));
-  if (n_records >= (1LL << 31)) return sr_fail_with(h, set_error(CCO_E_UNSUPPORTED, "%lld records in one body: at most 2^31 - 1", (long long)n_records));
+  CKR(h->latch.state("the results are finished"));
+  if (n_records >= (1LL << 31)) return h->latch.fail(set_error(CCO_E_UNSUPPORTED, "%lld records in one body: at most 2^31 - 1", (long long)n_records));
   if (line_offsets && (n_records < 0 || with_ranks)) return set_error(CCO_E_INVALID_ARG, "query lines need n_records >= 0 and no with_ranks bitmap");
   if ((h->flags & CCO_SR_BATCHPREDICT) && !line_offsets) return set_error(CCO_E_INVALID_ARG, "batchpredict lines need the query lines");
   if (line_offsets) {
@@ -7989,39 +8154,14 @@ int cco_search_results_append(cco_search_results_t *h, const char *body, int64_t
   }
   cco_ctx *c = h->ctx;
   CK(cudaSetDevice(c->device));
-  const int slot = (int)(h->n_bodies & 1);
-  const size_t padded = (size_t)((len + 63) / 64 * 64) + 64;
-  size_t free_b = 0, total_b = 0;
-  CK(cudaMemGetInfo(&free_b, &total_b));
-  if (padded > total_b / 4)
-    return sr_fail_with(h, set_error(CCO_E_UNSUPPORTED, "a response body of %lld bytes: at most a quarter of the device's memory", (long long)len));
-  // staging and device buffers of this slot were last used by the body before the previous one, which has been read
-  if (h->stage_cap[slot] < padded) {
-    if (h->stage[slot]) cudaFreeHost(h->stage[slot]);
-    h->stage[slot] = nullptr;
-    h->stage_cap[slot] = 0;
-    if (cudaHostAlloc((void **)&h->stage[slot], padded, cudaHostAllocPortable) != cudaSuccess)
-      return sr_fail_with(h, set_error(CCO_E_OOM, "cudaHostAlloc(%zu) failed", padded));
-    h->stage_cap[slot] = padded;
-  }
-  if (h->dcap[slot] < padded) {
-    if (h->dbody[slot]) cudaFree(h->dbody[slot]);
-    h->dbody[slot] = nullptr;
-    h->dcap[slot] = 0;
-    if (cudaMalloc((void **)&h->dbody[slot], padded) != cudaSuccess)
-      return sr_fail_with(h, set_error(CCO_E_UNSUPPORTED, "a response body of %lld bytes does not fit the device", (long long)len));
-    h->dcap[slot] = padded;
-  }
-  if (len > 0) memcpy(h->stage[slot], body, (size_t)len);
-  memset(h->stage[slot] + len, ' ', padded - (size_t)len);
-  if (cudaMemcpyAsync(h->dbody[slot], h->stage[slot], padded, cudaMemcpyHostToDevice, c->copy_stream) != cudaSuccess ||
-      cudaEventRecord(h->copied[slot], c->copy_stream) != cudaSuccess)
-    return sr_fail_with(h, set_error(CCO_E_CUDA, "the copy of response body %lld failed", (long long)h->n_bodies));
+  // this slot last held the body before the previous one, which has been read
+  char what[64], copy_of[48];
+  snprintf(what, sizeof what, "a response body of %lld bytes", (long long)len);
+  snprintf(copy_of, sizeof copy_of, "response body %lld", h->n_bodies);
+  int st = h->stage.put(c, (int)(h->n_bodies & 1), body, len, what, copy_of);
   // the previous body is read while this one is copied
-  if (h->pending) {
-    const int st = sr_read(h);
-    if (st != CCO_OK) return sr_fail_with(h, st);
-  }
+  if (st == CCO_OK && h->pending) st = sr_read(h);
+  if (st != CCO_OK) return h->latch.fail(st);
   ++h->n_bodies;
   h->pending = true;
   h->p_len = len;
@@ -8044,24 +8184,21 @@ int cco_search_results_append(cco_search_results_t *h, const char *body, int64_t
 
 int cco_search_results_finish(cco_search_results_t *h, cco_search_results_out_t *out) {
   if (!h || !out) return set_error(CCO_E_INVALID_ARG, "null argument");
-  CKR(sr_state(h));
+  CKR(h->latch.state("the results are finished"));
   cco_ctx *c = h->ctx;
   CK(cudaSetDevice(c->device));
   if (h->pending) {
     const int st = sr_read(h);
-    if (st != CCO_OK) return sr_fail_with(h, st);
+    if (st != CCO_OK) return h->latch.fail(st);
     h->pending = false;
   }
-  h->finished = true;
+  h->latch.finished = true;
   memset(out, 0, sizeof *out);
   const long long R = (long long)h->status.size(), H = h->hit_off.back();
-  std::vector<void *> got;
+  std::vector<void *> got;   // handed back to the pool when a later one fails
   auto give = [&](void **dst, const void *src, size_t n) {
-    void *p = c->pinned_get(std::max<size_t>(n, 1), /*for_result=*/false);
-    if (!p) return false;
-    if (n) memcpy(p, src, n);
-    got.push_back(p);
-    *dst = p;
+    if (pinned_give(c, dst, src, n) != CCO_OK) return false;
+    got.push_back(*dst);
     return true;
   };
   bool ok = give((void **)&out->hit_offsets, h->hit_off.data(), 8 * (size_t)(R + 1)) && give((void **)&out->status, h->status.data(), 4 * (size_t)R) &&
@@ -8085,12 +8222,7 @@ int cco_search_results_finish(cco_search_results_t *h, cco_search_results_out_t 
 int cco_search_results_free(cco_search_results_t *h) {
   if (!h) return CCO_OK;
   cudaSetDevice(h->ctx->device);
-  cudaStreamSynchronize(h->ctx->copy_stream);
-  for (int i = 0; i < 2; ++i) {
-    if (h->stage[i]) cudaFreeHost(h->stage[i]);
-    if (h->dbody[i]) cudaFree(h->dbody[i]);
-    if (h->copied[i]) cudaEventDestroy(h->copied[i]);
-  }
+  h->stage.release(h->ctx);
   delete h;
   return CCO_OK;
 }
@@ -8099,11 +8231,7 @@ int cco_search_results_free(cco_search_results_t *h) {
 // cco_index_pages.cuh ----------------------------------------------------------------------------------------------------
 struct cco_index_pages {
   cco_ctx *ctx = nullptr;
-  char *stage[2] = {};                 // pinned staging of the last two pages
-  size_t stage_cap[2] = {};
-  unsigned char *dpage[2] = {};        // their device copies
-  size_t dcap[2] = {};
-  cudaEvent_t copied[2] = {};
+  BodyStage stage;                     // the last two pages
   long long n_pages = 0;
   // the pending page (the last appended): its hits are known, its documents are written by the next append or by finish
   bool pending = false;
@@ -8115,72 +8243,11 @@ struct cco_index_pages {
   long long total = -1, n_docs = 0;
   char *out = nullptr;                 // the documents so far (the context's pinned memory, handed to the caller by finish)
   size_t out_cap = 0, out_len = 0;
-  bool failed = false, finished = false;
-  std::string fail_msg;
-  int fail_code = CCO_OK;
+  ReaderLatch latch;
 };
 
 extern "C++" {
 namespace cco {
-
-static const char *ip_message(int code) {
-  switch (code) {
-    case kIpNotObject: return "the top level is not an object";
-    case kIpError: return "Elasticsearch returned an error";
-    case kIpTimedOut: return "the search timed out (timed_out is true)";
-    case kIpShards: return "_shards.failed is not 0";
-    case kIpHitsNotArray: return "hits.hits is neither an array nor absent";
-    case kSrHitNotObject: return "a hits.hits element is not an object";
-    case kSrNoId: return "the hit has no string _id";
-    case kIpRepeatedId: return "a repeated _id";
-    case kIpNoSource: return "the hit has no _source";
-    case kIpSourceNotObject: return "_source is not an object";
-    case kSrString: return "a string holds a bad escape or a raw byte < 0x20";
-  }
-  return sr_message(code);
-}
-// a valid raw JSON string as UTF-8, a surrogate that is not part of a pair in its 3-byte form (k_json_unescape's rules)
-static std::string ip_unescape(const char *p, long long n) {
-  std::string o;
-  auto hex4 = [](const char *q) { return (unsigned)strtoul(std::string(q, 4).c_str(), nullptr, 16); };
-  for (long long i = 0; i < n;) {
-    if (p[i] != '\\') {
-      o += p[i++];
-      continue;
-    }
-    const char x = p[i + 1];
-    if (x != 'u') {
-      o += x == 'b' ? '\b' : x == 'f' ? '\f' : x == 'n' ? '\n' : x == 'r' ? '\r' : x == 't' ? '\t' : x;
-      i += 2;
-      continue;
-    }
-    unsigned cp = hex4(p + i + 2);
-    i += 6;
-    if (cp >= 0xd800 && cp < 0xdc00 && i + 6 <= n && p[i] == '\\' && p[i + 1] == 'u') {
-      const unsigned lo = hex4(p + i + 2);
-      if (lo >= 0xdc00 && lo < 0xe000) {
-        cp = 0x10000 + ((cp - 0xd800) << 10) + (lo - 0xdc00);
-        i += 6;
-      }
-    }
-    if (cp < 0x80) {
-      o += (char)cp;
-    } else if (cp < 0x800) {
-      o += (char)(0xc0 | cp >> 6);
-      o += (char)(0x80 | (cp & 0x3f));
-    } else if (cp < 0x10000) {
-      o += (char)(0xe0 | cp >> 12);
-      o += (char)(0x80 | (cp >> 6 & 0x3f));
-      o += (char)(0x80 | (cp & 0x3f));
-    } else {
-      o += (char)(0xf0 | cp >> 18);
-      o += (char)(0x80 | (cp >> 12 & 0x3f));
-      o += (char)(0x80 | (cp >> 6 & 0x3f));
-      o += (char)(0x80 | (cp & 0x3f));
-    }
-  }
-  return o;
-}
 
 // The new page (slot h->n_pages & 1, copied on the copy stream): its structural index down to the _source brackets and the
 // top walk.  Leaves it pending with its hit count; *sid = its _scroll_id's raw inside (sid[0] < 0: absent).
@@ -8189,56 +8256,21 @@ static int ip_top(cco_index_pages *h, long long len, long long *n_hits, long lon
   cudaStream_t s = c->stream;
   const int slot = (int)(h->n_pages & 1);
   const long long page_no = h->n_pages;
-  const unsigned char *page = h->dpage[slot];
-  CK(cudaStreamWaitEvent(s, h->copied[slot], 0));
+  const unsigned char *page = h->stage.dev[slot];
+  CKR(h->stage.wait(s, slot));
   mail_reset(c);
   h->p_ar = new Arena(s);
   Arena &ar = *h->p_ar;
   NvtxRange nvtx("cco:index_pages");
   auto byte_error = [&](long long at, int code) {
-    return set_error(CCO_E_INVALID_ARG, "page %lld, byte %lld: %s", page_no, at, ip_message(code));
+    return set_error(CCO_E_INVALID_ARG, "page %lld, byte %lld: %s", page_no, at, sr_message(code));
   };
-  const long long NW = (len + 63) / 64, n_chunks = (NW + kSrChunkWords - 1) / kSrChunkWords;
-  unsigned long long *err;
-  CKR(ar.alloc(&err, 1));
-  CK(cudaMemsetAsync(err, 0xff, 8, s));
-  SrFun *fun, *pre;
-  long long *cnt, *coff;
-  CKR(ar.alloc(&fun, n_chunks + 1));
-  CKR(ar.alloc(&pre, n_chunks + 1));
-  CKR(ar.alloc(&cnt, n_chunks + 1));
-  CKR(ar.alloc(&coff, n_chunks + 1));
-  CK(cudaMemsetAsync(cnt + n_chunks, 0, 8, s));
-  SrFun fin = sr_identity();
-  long long m = 0;
-  if (n_chunks > 0) {
-    const int grid = grid_for(n_chunks * 32, 256, c->sm_count);
-    k_sr_chunk<<<grid, 256, 0, s>>>(NW, (const uint4 *)page, fun);
-    k_sr_scan<<<1, kSrScanThreads, 0, s>>>(n_chunks, fun, pre);
-    k_sr_index<false><<<grid, 256, 0, s>>>(NW, (const uint4 *)page, pre, kIpMaxDepth, cnt, nullptr, nullptr, nullptr, err);
-    c->launches += 3;
-    CKR(mail_fetch(c, &fin, pre + n_chunks - 1, sizeof(SrFun)));
-  }
-  CKR(exclusive_sum(c, ar, cnt, coff, n_chunks + 1));
+  SrIndex ix;
   unsigned long long e0 = ~0ULL;
-  CKR(mail_fetch(c, &m, coff + n_chunks, 8));
-  CKR(mail_fetch(c, &e0, err, 8));
-  CKR(mail_wait(c));
+  CKR(sr_index(c, ar, page, len, kIpMaxDepth, &ix, &e0));
   if (e0 != ~0ULL) return byte_error((long long)(e0 >> 8), (int)(e0 & 0xff));
-  if (fin.f[0] >> 1) return set_error(CCO_E_INVALID_ARG, "page %lld, byte %lld: a string is not closed", page_no, len);
-  if (fin.d[0] != 0) return byte_error(len, kSrUnbalanced);
-  long long *pos;
-  unsigned char *dep;
-  CKR(ar.alloc(&pos, m + 1));
-  CKR(ar.alloc(&dep, m + 1));
-  if (m > 0) {
-    k_sr_index<true><<<grid_for(n_chunks * 32, 256, c->sm_count), 256, 0, s>>>(NW, (const uint4 *)page, pre, kIpMaxDepth, nullptr, coff, pos, dep, err);
-    c->launches++;
-  }
-  ar.release(fun);
-  ar.release(pre);
-  ar.release(cnt);
-  ar.release(coff);
+  const long long m = ix.m, *pos = ix.pos;
+  const unsigned char *dep = ix.dep;
   // the top walk over the entries down to the hits' brackets
   long long *top, nt = 0, *hopen, *hclose;
   CKR(sr_select(c, ar, m, dep, 0, kIpTopDepth, -1, m, &top, &nt));
@@ -8251,11 +8283,11 @@ static int ip_top(cco_index_pages *h, long long len, long long *n_hits, long lon
   CKR(mail_fetch(c, &r, d_top, sizeof r));
   CKR(mail_wait(c));
   ar.release(top);
-  if (r.code == kIpNotObject || r.code == kIpTimedOut || r.code == kIpShards || r.code == kIpHitsNotArray)
-    return set_error(CCO_E_INVALID_ARG, "page %lld: %s", page_no, ip_message(r.code));
-  if (r.code == kIpError) {
-    if (r.has_status) return set_error(CCO_E_INVALID_ARG, "page %lld: %s (status %lld)", page_no, ip_message(r.code), r.status);
-    return set_error(CCO_E_INVALID_ARG, "page %lld: %s", page_no, ip_message(r.code));
+  if (r.code == kSrNotObject || r.code == kIpTimedOut || r.code == kIpShards || r.code == kIpHitsNotArray)
+    return set_error(CCO_E_INVALID_ARG, "page %lld: %s", page_no, sr_message(r.code));
+  if (r.code == kSrEsError) {
+    if (r.has_status) return set_error(CCO_E_INVALID_ARG, "page %lld: %s (status %lld)", page_no, sr_message(r.code), r.status);
+    return set_error(CCO_E_INVALID_ARG, "page %lld: %s", page_no, sr_message(r.code));
   }
   if (r.code) return byte_error(r.bad, r.code);
   if (r.n_hits >= (1LL << 31)) return set_error(CCO_E_UNSUPPORTED, "page %lld: %lld hits in one page: at most 2^31 - 1", page_no, r.n_hits);
@@ -8278,7 +8310,7 @@ static int ip_docs(cco_index_pages *h) {
   cco_ctx *c = h->ctx;
   cudaStream_t s = c->stream;
   const long long page_no = h->n_pages - 1, n = h->p_hits;
-  const unsigned char *page = h->dpage[page_no & 1];
+  const unsigned char *page = h->stage.dev[page_no & 1];
   h->pending = false;
   Arena &ar = *h->p_ar;
   mail_reset(c);
@@ -8303,8 +8335,8 @@ static int ip_docs(cco_index_pages *h) {
     long long id_total = 0;
     CKR(json_decode(c, ar, n, idm, page, &ids, &id_total));   // waits for the fetches above
     if (e_byte != ~0ULL)
-      return set_error(CCO_E_INVALID_ARG, "page %lld, byte %lld: %s", page_no, (long long)(e_byte >> 8), ip_message((int)(e_byte & 0xff)));
-    if (e_hit != ~0ULL) return set_error(CCO_E_INVALID_ARG, "page %lld, hit %lld: %s", page_no, (long long)(e_hit >> 8), ip_message((int)(e_hit & 0xff)));
+      return set_error(CCO_E_INVALID_ARG, "page %lld, byte %lld: %s", page_no, (long long)(e_byte >> 8), sr_message((int)(e_byte & 0xff)));
+    if (e_hit != ~0ULL) return set_error(CCO_E_INVALID_ARG, "page %lld, hit %lld: %s", page_no, (long long)(e_hit >> 8), sr_message((int)(e_hit & 0xff)));
     IpDocs a = {page, sb, se, ids.off, (const unsigned char *)ids.w};
     long long *len, *off;
     CKR(ar.alloc(&len, n + 1));
@@ -8354,18 +8386,6 @@ static int ip_docs(cco_index_pages *h) {
   h->p_ar = nullptr;
   return CCO_OK;
 }
-static int ip_fail_with(cco_index_pages *h, int st) {
-  h->failed = true;
-  h->fail_code = st;
-  h->fail_msg = cco_last_error();
-  return st;
-}
-static int ip_state(const cco_index_pages *h) {
-  if (h->failed) return set_error(h->fail_code == CCO_OK ? CCO_E_INVALID_ARG : h->fail_code, "%s", h->fail_msg.c_str());
-  if (h->finished) return set_error(CCO_E_INVALID_ARG, "the index pages are finished");
-  return CCO_OK;
-}
-
 }  // namespace cco
 }  // extern "C++"
 
@@ -8376,11 +8396,10 @@ int cco_index_pages_begin(cco_ctx_t *ctx, cco_index_pages_t **out) {
   CK(cudaSetDevice(ctx->device));
   cco_index_pages *h = new cco_index_pages();
   h->ctx = ctx;
-  for (int i = 0; i < 2; ++i)
-    if (cudaEventCreateWithFlags(&h->copied[i], cudaEventDisableTiming) != cudaSuccess) {
-      cco_index_pages_free(h);
-      return set_error(CCO_E_CUDA, "cudaEventCreate failed");
-    }
+  if (h->stage.init() != CCO_OK) {
+    cco_index_pages_free(h);
+    return set_error(CCO_E_CUDA, "cudaEventCreate failed");
+  }
   *out = h;
   return CCO_OK;
 }
@@ -8389,52 +8408,28 @@ int cco_index_pages_append(cco_index_pages_t *h, const char *page, int64_t len, 
                            int64_t *scroll_id_len) {
   if (!h || len < 0 || (len > 0 && !page) || !n_hits || !scroll_id || !scroll_id_len)
     return set_error(CCO_E_INVALID_ARG, "null argument or negative length");
-  CKR(ip_state(h));
+  CKR(h->latch.state("the index pages are finished"));
   *n_hits = 0;
   *scroll_id = nullptr;
   *scroll_id_len = 0;
   cco_ctx *c = h->ctx;
   CK(cudaSetDevice(c->device));
-  const int slot = (int)(h->n_pages & 1);
-  const size_t padded = (size_t)((len + 63) / 64 * 64) + 64;
-  size_t free_b = 0, total_b = 0;
-  CK(cudaMemGetInfo(&free_b, &total_b));
-  if (padded > total_b / 4)
-    return ip_fail_with(h, set_error(CCO_E_UNSUPPORTED, "page %lld of %lld bytes: at most a quarter of the device's memory", h->n_pages, (long long)len));
   // this slot last held the page before the previous one, whose documents are written
-  if (h->stage_cap[slot] < padded) {
-    if (h->stage[slot]) cudaFreeHost(h->stage[slot]);
-    h->stage[slot] = nullptr;
-    h->stage_cap[slot] = 0;
-    if (cudaHostAlloc((void **)&h->stage[slot], padded, cudaHostAllocPortable) != cudaSuccess)
-      return ip_fail_with(h, set_error(CCO_E_OOM, "cudaHostAlloc(%zu) failed", padded));
-    h->stage_cap[slot] = padded;
-  }
-  if (h->dcap[slot] < padded) {
-    if (h->dpage[slot]) cudaFree(h->dpage[slot]);
-    h->dpage[slot] = nullptr;
-    h->dcap[slot] = 0;
-    if (cudaMalloc((void **)&h->dpage[slot], padded) != cudaSuccess)
-      return ip_fail_with(h, set_error(CCO_E_UNSUPPORTED, "page %lld of %lld bytes does not fit the device", h->n_pages, (long long)len));
-    h->dcap[slot] = padded;
-  }
-  if (len > 0) memcpy(h->stage[slot], page, (size_t)len);
-  memset(h->stage[slot] + len, ' ', padded - (size_t)len);
-  if (cudaMemcpyAsync(h->dpage[slot], h->stage[slot], padded, cudaMemcpyHostToDevice, c->copy_stream) != cudaSuccess ||
-      cudaEventRecord(h->copied[slot], c->copy_stream) != cudaSuccess)
-    return ip_fail_with(h, set_error(CCO_E_CUDA, "the copy of page %lld failed", h->n_pages));
+  const int slot = (int)(h->n_pages & 1);
+  char what[80], copy_of[48];
+  snprintf(what, sizeof what, "page %lld of %lld bytes", h->n_pages, (long long)len);
+  snprintf(copy_of, sizeof copy_of, "page %lld", h->n_pages);
+  int st = h->stage.put(c, slot, page, len, what, copy_of);
   // the previous page's documents are written while this one is copied
-  if (h->pending) {
-    const int st = ip_docs(h);
-    if (st != CCO_OK) return ip_fail_with(h, st);
-  }
+  if (st == CCO_OK && h->pending) st = ip_docs(h);
+  if (st != CCO_OK) return h->latch.fail(st);
   long long n = 0, sid[2] = {-1, -1};
-  const int st = ip_top(h, len, &n, sid);
+  st = ip_top(h, len, &n, sid);
   ++h->n_pages;
-  if (st != CCO_OK) return ip_fail_with(h, st);
+  if (st != CCO_OK) return h->latch.fail(st);
   *n_hits = n;
   if (sid[0] >= 0) {
-    h->scroll_id = ip_unescape(h->stage[slot] + sid[0], sid[1] - sid[0]);
+    h->scroll_id = sr_unescape(h->stage.host(slot) + sid[0], sid[1] - sid[0]);
     *scroll_id = h->scroll_id.data();
     *scroll_id_len = (int64_t)h->scroll_id.size();
   }
@@ -8443,19 +8438,19 @@ int cco_index_pages_append(cco_index_pages_t *h, const char *page, int64_t len, 
 
 int cco_index_pages_finish(cco_index_pages_t *h, cco_index_pages_out_t *out) {
   if (!h || !out) return set_error(CCO_E_INVALID_ARG, "null argument");
-  CKR(ip_state(h));
+  CKR(h->latch.state("the index pages are finished"));
   cco_ctx *c = h->ctx;
   CK(cudaSetDevice(c->device));
   if (h->pending) {
     const int st = ip_docs(h);
-    if (st != CCO_OK) return ip_fail_with(h, st);
+    if (st != CCO_OK) return h->latch.fail(st);
   }
   memset(out, 0, sizeof *out);
   if (!h->out) {   // an empty index: an empty body
     h->out = (char *)c->pinned_get(1, /*for_result=*/false);
     if (!h->out) return set_error(CCO_E_OOM, "pinned host allocation failed");
   }
-  h->finished = true;
+  h->latch.finished = true;
   out->n_docs = h->n_docs;
   out->total = h->total;
   out->body = h->out;
@@ -8468,14 +8463,9 @@ int cco_index_pages_finish(cco_index_pages_t *h, cco_index_pages_out_t *out) {
 int cco_index_pages_free(cco_index_pages_t *h) {
   if (!h) return CCO_OK;
   cudaSetDevice(h->ctx->device);
-  cudaStreamSynchronize(h->ctx->copy_stream);
   cudaStreamSynchronize(h->ctx->stream);
   delete h->p_ar;
-  for (int i = 0; i < 2; ++i) {
-    if (h->stage[i]) cudaFreeHost(h->stage[i]);
-    if (h->dpage[i]) cudaFree(h->dpage[i]);
-    if (h->copied[i]) cudaEventDestroy(h->copied[i]);
-  }
+  h->stage.release(h->ctx);
   if (h->out) h->ctx->pinned_put(h->out);
   delete h;
   return CCO_OK;
@@ -8486,6 +8476,7 @@ int cco_index_pages_free(cco_index_pages_t *h) {
 struct cco_index_write {
   cco_ctx *ctx = nullptr;
   Arena *ar = nullptr;                 // the body, its parse, the statuses and the retry lists, for the session
+  BodyStage stage;                     // the response being read, in slot 0
   BulkDocs bd;
   int32_t *status = nullptr;           // [D] on the device: each document's latest status, 0 if never answered
   char *hbody = nullptr;               // the body in pinned memory: retry bodies are gathered from it
@@ -8502,30 +8493,12 @@ struct cco_index_write {
   std::vector<std::vector<long long>> round_docs;   // the documents of each retry round, ascending
   std::vector<long long *> round_ddocs;             // their device copies
   std::unordered_map<long long, std::pair<std::string, std::string>> errors;   // each document's latest error.type, .reason
-  bool failed = false, finished = false;
-  std::string fail_msg;
-  int fail_code = CCO_OK;
+  ReaderLatch latch;
 };
 
 extern "C++" {
 namespace cco {
 
-static const char *iw_message(int code) {
-  switch (code) {
-    case kIwNotObject: return "the top level is not an object";
-    case kIwError: return "Elasticsearch returned an error";
-    case kIwNoItems: return "the response has no \"items\" array";
-    case kIwItemNotObject: return "an items element is not an object";
-    case kIwNotIndex: return "the item is not {\"index\":{...}}";
-    case kIwNoId: return "the item has no string _id";
-    case kIwRepeatedId: return "a repeated _id";
-    case kIwIdMismatch: return "the item's _id is not the document's _id";
-    case kIwNoStatus: return "the item has no status";
-    case kIwRepeatedStatus: return "a repeated status";
-    case kIwBadStatus: return "the status is not a 32-bit integer";
-  }
-  return sr_message(code);
-}
 // The greedy cut of documents of the given sizes into requests of at most max_docs documents and max_bytes bytes; a
 // document larger than max_bytes is a request of its own.  db / bb: the requests' first document and byte, then the ends.
 static void iw_cut(const std::vector<long long> &size, long long max_docs, long long max_bytes, std::vector<long long> &db,
@@ -8549,18 +8522,6 @@ static void iw_cut(const std::vector<long long> &size, long long max_docs, long 
     bb.push_back(at);
   }
 }
-template <typename T>
-static T *iw_pinned(cco_ctx *c, size_t n) {
-  return (T *)c->pinned_get(sizeof(T) * std::max<size_t>(n, 1), /*for_result=*/false);
-}
-template <typename T>
-static int iw_put(cco_ctx *c, const std::vector<T> &v, T **out) {
-  *out = iw_pinned<T>(c, v.size());
-  if (!*out) return set_error(CCO_E_OOM, "pinned host allocation failed");
-  if (!v.empty()) memcpy(*out, v.data(), sizeof(T) * v.size());
-  return CCO_OK;
-}
-
 // The body on the device: its documents checked as cco_rerank_model checks them (a repeated _id included), the documents'
 // first bytes on the host, and the requests of the body itself.
 static int iw_begin(cco_index_write *h, const char *body, long long len) {
@@ -8588,9 +8549,7 @@ static int iw_begin(cco_index_write *h, const char *body, long long len) {
     CK(cudaMemcpy2DAsync(h->doc_b.data(), sizeof(long long), bd.line_b, 2 * sizeof(long long), sizeof(long long), (size_t)D,
                          cudaMemcpyDeviceToHost, s));
   }
-  h->hbody = iw_pinned<char>(c, (size_t)len);
-  if (!h->hbody) return set_error(CCO_E_OOM, "pinned host allocation of %lld bytes failed", len);
-  if (len > 0) memcpy(h->hbody, body, (size_t)len);
+  if (pinned_give(c, &h->hbody, body, (size_t)len) != CCO_OK) return set_error(CCO_E_OOM, "pinned host allocation of %lld bytes failed", len);
   CK(cudaStreamSynchronize(s));
   CK(cudaGetLastError());
   std::vector<long long> size((size_t)D);
@@ -8646,9 +8605,10 @@ static int iw_fields(cco_index_write *h, int64_t *n_out, int64_t **name_offsets,
     CK(cudaMemcpyAsync(&total, esc.off + ng, 8, cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
   }
-  int64_t *ho = iw_pinned<int64_t>(c, (size_t)ng + 2);
-  char *hb = iw_pinned<char>(c, (size_t)total + 2);
-  if (!ho || !hb) return set_error(CCO_E_OOM, "pinned host allocation failed");
+  int64_t *ho;
+  char *hb;
+  CKR(pinned_give(c, &ho, nullptr, sizeof(int64_t) * ((size_t)ng + 2)));
+  CKR(pinned_give(c, &hb, nullptr, (size_t)total + 2));
   ho[0] = 0;
   if (ng > 0) {
     CK(cudaMemcpyAsync(ho, esc.off, sizeof(int64_t) * ((size_t)ng + 1), cudaMemcpyDeviceToHost, s));
@@ -8678,60 +8638,25 @@ static int iw_response(cco_index_write *h, long long q, const char *resp, long l
   cco_index_write::Req &rq = h->reqs[q];
   if (rq.answered) return set_error(CCO_E_INVALID_ARG, "request %lld is answered twice", q);
   const long long n_docs = rq.e - rq.b;
-  const size_t padded = (size_t)((len + 63) / 64 * 64) + 64;
-  size_t free_b = 0, total_b = 0;
-  CK(cudaMemGetInfo(&free_b, &total_b));
-  if (padded > total_b / 4)
-    return set_error(CCO_E_UNSUPPORTED, "request %lld: a response of %lld bytes: at most a quarter of the device's memory", q, len);
+  char what[96], copy_of[48];
+  snprintf(what, sizeof what, "request %lld: a response of %lld bytes", q, len);
+  snprintf(copy_of, sizeof copy_of, "the response to request %lld", q);
+  CKR(h->stage.put(c, 0, resp, len, what, copy_of));
+  CKR(h->stage.wait(s, 0));
+  const unsigned char *page = h->stage.dev[0];
   Arena ar(s);
   NvtxRange nvtx("cco:index_write");
   mail_reset(c);
   auto byte_error = [&](long long at, int code) {
-    return set_error(CCO_E_INVALID_ARG, "request %lld, byte %lld: %s", q, at, iw_message(code));
+    return set_error(CCO_E_INVALID_ARG, "request %lld, byte %lld: %s", q, at, sr_message(code));
   };
-  unsigned char *page;
-  CKR(ar.alloc(&page, padded));
-  if (len > 0) CK(cudaMemcpyAsync(page, resp, (size_t)len, cudaMemcpyHostToDevice, s));
-  CK(cudaMemsetAsync(page + len, ' ', padded - (size_t)len, s));
   // the structural index down to the members of an item's error
-  const long long NW = (len + 63) / 64, n_chunks = (NW + kSrChunkWords - 1) / kSrChunkWords;
-  unsigned long long *err;
-  CKR(ar.alloc(&err, 4));
-  CK(cudaMemsetAsync(err, 0xff, 24, s));
-  CK(cudaMemsetAsync(err + 3, 0, 8, s));
-  SrFun *fun, *pre;
-  long long *cnt, *coff;
-  CKR(ar.alloc(&fun, n_chunks + 1));
-  CKR(ar.alloc(&pre, n_chunks + 1));
-  CKR(ar.alloc(&cnt, n_chunks + 1));
-  CKR(ar.alloc(&coff, n_chunks + 1));
-  CK(cudaMemsetAsync(cnt + n_chunks, 0, 8, s));
-  SrFun fin = sr_identity();
-  long long m = 0;
-  if (n_chunks > 0) {
-    const int grid = grid_for(n_chunks * 32, 256, c->sm_count);
-    k_sr_chunk<<<grid, 256, 0, s>>>(NW, (const uint4 *)page, fun);
-    k_sr_scan<<<1, kSrScanThreads, 0, s>>>(n_chunks, fun, pre);
-    k_sr_index<false><<<grid, 256, 0, s>>>(NW, (const uint4 *)page, pre, kIwMaxDepth, cnt, nullptr, nullptr, nullptr, err);
-    c->launches += 3;
-    CKR(mail_fetch(c, &fin, pre + n_chunks - 1, sizeof(SrFun)));
-  }
-  CKR(exclusive_sum(c, ar, cnt, coff, n_chunks + 1));
+  SrIndex ix;
   unsigned long long e0 = ~0ULL;
-  CKR(mail_fetch(c, &m, coff + n_chunks, 8));
-  CKR(mail_fetch(c, &e0, err, 8));
-  CKR(mail_wait(c));
+  CKR(sr_index(c, ar, page, len, kIwMaxDepth, &ix, &e0));
   if (e0 != ~0ULL) return byte_error((long long)(e0 >> 8), (int)(e0 & 0xff));
-  if (fin.f[0] >> 1) return set_error(CCO_E_INVALID_ARG, "request %lld, byte %lld: a string is not closed", q, len);
-  if (fin.d[0] != 0) return byte_error(len, kSrUnbalanced);
-  long long *pos;
-  unsigned char *dep;
-  CKR(ar.alloc(&pos, m + 1));
-  CKR(ar.alloc(&dep, m + 1));
-  if (m > 0) {
-    k_sr_index<true><<<grid_for(n_chunks * 32, 256, c->sm_count), 256, 0, s>>>(NW, (const uint4 *)page, pre, kIwMaxDepth, nullptr, coff, pos, dep, err);
-    c->launches++;
-  }
+  const long long m = ix.m, *pos = ix.pos;
+  const unsigned char *dep = ix.dep;
   // the top walk over the entries down to the items' brackets
   long long *top, nt = 0, *iopen, *iclose;
   CKR(sr_select(c, ar, m, dep, 0, kIwTopDepth, -1, m, &top, &nt));
@@ -8743,10 +8668,10 @@ static int iw_response(cco_index_write *h, long long q, const char *resp, long l
   c->launches++;
   CKR(mail_fetch(c, &r, d_top, sizeof r));
   CKR(mail_wait(c));
-  if (r.code == kIwNotObject || r.code == kIwNoItems) return set_error(CCO_E_INVALID_ARG, "request %lld: %s", q, iw_message(r.code));
-  if (r.code == kIwError) {
-    if (r.has_status) return set_error(CCO_E_INVALID_ARG, "request %lld: %s (status %lld)", q, iw_message(r.code), r.status);
-    return set_error(CCO_E_INVALID_ARG, "request %lld: %s", q, iw_message(r.code));
+  if (r.code == kSrNotObject || r.code == kIwNoItems) return set_error(CCO_E_INVALID_ARG, "request %lld: %s", q, sr_message(r.code));
+  if (r.code == kSrEsError) {
+    if (r.has_status) return set_error(CCO_E_INVALID_ARG, "request %lld: %s (status %lld)", q, sr_message(r.code), r.status);
+    return set_error(CCO_E_INVALID_ARG, "request %lld: %s", q, sr_message(r.code));
   }
   if (r.code) return byte_error(r.bad, r.code);
   if (r.n_items != n_docs)
@@ -8754,8 +8679,12 @@ static int iw_response(cco_index_write *h, long long q, const char *resp, long l
   if (n_docs > 0) {
     const long long *ddocs = rq.round < 0 ? nullptr : h->round_ddocs[rq.round] + rq.b;
     const IwItems it = {ddocs, rq.round < 0 ? rq.b : 0, h->bd.ids.off, (const unsigned char *)h->bd.ids.w};
+    unsigned long long *err;
     IwFail *fail;
+    CKR(ar.alloc(&err, 4));
     CKR(ar.alloc(&fail, n_docs));
+    CK(cudaMemsetAsync(err, 0xff, 24, s));
+    CK(cudaMemsetAsync(err + 3, 0, 8, s));
     k_iw_item<<<grid_for(n_docs * 32, 256, c->sm_count), 256, 0, s>>>(SrIdx{pos, dep, page, nullptr}, n_docs, iopen, iclose, it, h->status, fail,
                                                                       err + 3, err + 1, err + 2);
     c->launches++;
@@ -8766,15 +8695,15 @@ static int iw_response(cco_index_write *h, long long q, const char *resp, long l
     CKR(mail_wait(c));
     if (e_byte != ~0ULL) return byte_error((long long)(e_byte >> 8), (int)(e_byte & 0xff));
     if (e_item != ~0ULL)
-      return set_error(CCO_E_INVALID_ARG, "request %lld, item %lld: %s", q, (long long)(e_item >> 8), iw_message((int)(e_item & 0xff)));
+      return set_error(CCO_E_INVALID_ARG, "request %lld, item %lld: %s", q, (long long)(e_item >> 8), sr_message((int)(e_item & 0xff)));
     if (nf > 0) {   // failures are few: their error texts are decoded on the host, from the caller's response
       std::vector<IwFail> hf((size_t)nf);
       CK(cudaMemcpyAsync(hf.data(), fail, sizeof(IwFail) * (size_t)nf, cudaMemcpyDeviceToHost, s));
       CK(cudaStreamSynchronize(s));
       for (const IwFail &f : hf) {
         const long long doc = rq.round < 0 ? rq.b + f.item : h->round_docs[rq.round][rq.b + f.item];
-        h->errors[doc] = {f.tb < 0 ? std::string() : ip_unescape(resp + f.tb, f.te - f.tb),
-                          f.rb < 0 ? std::string() : ip_unescape(resp + f.rb, f.re - f.rb)};
+        h->errors[doc] = {f.tb < 0 ? std::string() : sr_unescape(resp + f.tb, f.te - f.tb),
+                          f.rb < 0 ? std::string() : sr_unescape(resp + f.rb, f.re - f.rb)};
       }
     }
   }
@@ -8803,8 +8732,8 @@ static int iw_retry(cco_index_write *h, cco_index_write_retry_t *out) {
     }
   std::vector<long long> db, bb;
   iw_cut(size, h->max_docs, h->max_bytes, db, bb);
-  char *body = iw_pinned<char>(c, (size_t)bb.back());
-  if (!body) return set_error(CCO_E_OOM, "pinned host allocation failed");
+  char *body;
+  CKR(pinned_give(c, &body, nullptr, (size_t)bb.back()));
   long long at = 0;
   for (size_t k = 0; k < docs.size(); ++k) {
     memcpy(body + at, h->hbody + h->doc_b[docs[k]], (size_t)size[k]);
@@ -8826,10 +8755,9 @@ static int iw_retry(cco_index_write *h, cco_index_write_retry_t *out) {
   out->body = body;
   out->body_len = at;
   out->n_requests = (int64_t)db.size() - 1;
-  std::vector<int64_t> docs64(docs.begin(), docs.end()), db64(db.begin(), db.end()), bb64(bb.begin(), bb.end());
-  CKR(iw_put(c, docs64, &out->doc));
-  CKR(iw_put(c, db64, &out->doc_begin));
-  CKR(iw_put(c, bb64, &out->byte_begin));
+  CKR(pinned_give(c, &out->doc, docs.data(), sizeof(int64_t) * docs.size()));
+  CKR(pinned_give(c, &out->doc_begin, db.data(), sizeof(int64_t) * db.size()));
+  CKR(pinned_give(c, &out->byte_begin, bb.data(), sizeof(int64_t) * bb.size()));
   return CCO_OK;
 }
 
@@ -8837,8 +8765,8 @@ static int iw_finish(cco_index_write *h, cco_index_write_out_t *out) {
   cco_ctx *c = h->ctx;
   const long long D = h->bd.D;
   memset(out, 0, sizeof *out);
-  int32_t *st = iw_pinned<int32_t>(c, (size_t)D);
-  if (!st) return set_error(CCO_E_OOM, "pinned host allocation failed");
+  int32_t *st;
+  CKR(pinned_give(c, &st, nullptr, sizeof(int32_t) * (size_t)D));
   out->status = st;
   CKR(iw_statuses(h, st));
   std::vector<int64_t> edoc, toff{0}, roff{0};
@@ -8860,23 +8788,11 @@ static int iw_finish(cco_index_write *h, cco_index_write_out_t *out) {
   }
   out->n_docs = D;
   out->n_errors = (int64_t)edoc.size();
-  CKR(iw_put(c, edoc, &out->error_doc));
-  CKR(iw_put(c, toff, &out->type_offsets));
-  CKR(iw_put(c, roff, &out->reason_offsets));
-  CKR(iw_put(c, std::vector<char>(tb.begin(), tb.end()), &out->type_bytes));
-  CKR(iw_put(c, std::vector<char>(rb.begin(), rb.end()), &out->reason_bytes));
-  return CCO_OK;
-}
-
-static int iw_fail_with(cco_index_write *h, int st) {
-  h->failed = true;
-  h->fail_code = st;
-  h->fail_msg = cco_last_error();
-  return st;
-}
-static int iw_state(const cco_index_write *h) {
-  if (h->failed) return set_error(h->fail_code == CCO_OK ? CCO_E_INVALID_ARG : h->fail_code, "%s", h->fail_msg.c_str());
-  if (h->finished) return set_error(CCO_E_INVALID_ARG, "the index write is finished");
+  CKR(pinned_give(c, &out->error_doc, edoc.data(), sizeof(int64_t) * edoc.size()));
+  CKR(pinned_give(c, &out->type_offsets, toff.data(), sizeof(int64_t) * toff.size()));
+  CKR(pinned_give(c, &out->reason_offsets, roff.data(), sizeof(int64_t) * roff.size()));
+  CKR(pinned_give(c, &out->type_bytes, tb.data(), tb.size()));
+  CKR(pinned_give(c, &out->reason_bytes, rb.data(), rb.size()));
   return CCO_OK;
 }
 
@@ -8901,7 +8817,8 @@ int cco_index_write_begin(cco_ctx_t *ctx, const char *body, int64_t len, const c
   h->len = len;
   h->max_docs = params->max_docs;
   h->max_bytes = params->max_bytes;
-  const int st = iw_begin(h, body, len);
+  int st = h->stage.init();
+  if (st == CCO_OK) st = iw_begin(h, body, len);
   if (st != CCO_OK) {
     const std::string msg = cco_last_error();
     cco_index_write_free(h);
@@ -8913,46 +8830,45 @@ int cco_index_write_begin(cco_ctx_t *ctx, const char *body, int64_t len, const c
 
 int cco_index_write_fields(cco_index_write_t *h, int64_t *n, int64_t **name_offsets, char **name_bytes) {
   if (!h || !n || !name_offsets || !name_bytes) return set_error(CCO_E_INVALID_ARG, "null argument");
-  CKR(iw_state(h));
+  CKR(h->latch.state("the index write is finished"));
   CK(cudaSetDevice(h->ctx->device));
   const int st = iw_fields(h, n, name_offsets, name_bytes);
-  return st == CCO_OK ? st : iw_fail_with(h, st);
+  return st == CCO_OK ? st : h->latch.fail(st);
 }
 
 int cco_index_write_requests(cco_index_write_t *h, int64_t *n_requests, int64_t **doc_begin, int64_t **byte_begin) {
   if (!h || !n_requests || !doc_begin || !byte_begin) return set_error(CCO_E_INVALID_ARG, "null argument");
-  CKR(iw_state(h));
-  std::vector<int64_t> db(h->first_db.begin(), h->first_db.end()), bb(h->first_bb.begin(), h->first_bb.end());
-  int st = iw_put(h->ctx, db, doc_begin);
-  if (st == CCO_OK) st = iw_put(h->ctx, bb, byte_begin);
-  if (st != CCO_OK) return iw_fail_with(h, st);
+  CKR(h->latch.state("the index write is finished"));
+  int st = pinned_give(h->ctx, doc_begin, h->first_db.data(), sizeof(int64_t) * h->first_db.size());
+  if (st == CCO_OK) st = pinned_give(h->ctx, byte_begin, h->first_bb.data(), sizeof(int64_t) * h->first_bb.size());
+  if (st != CCO_OK) return h->latch.fail(st);
   *n_requests = h->n_first;
   return CCO_OK;
 }
 
 int cco_index_write_response(cco_index_write_t *h, int64_t request, const char *resp, int64_t len) {
   if (!h || len < 0 || (len > 0 && !resp)) return set_error(CCO_E_INVALID_ARG, "null argument or negative length");
-  CKR(iw_state(h));
+  CKR(h->latch.state("the index write is finished"));
   CK(cudaSetDevice(h->ctx->device));
   const int st = iw_response(h, request, resp, len);
-  return st == CCO_OK ? st : iw_fail_with(h, st);
+  return st == CCO_OK ? st : h->latch.fail(st);
 }
 
 int cco_index_write_retry(cco_index_write_t *h, cco_index_write_retry_t *out) {
   if (!h || !out) return set_error(CCO_E_INVALID_ARG, "null argument");
-  CKR(iw_state(h));
+  CKR(h->latch.state("the index write is finished"));
   CK(cudaSetDevice(h->ctx->device));
   const int st = iw_retry(h, out);
-  return st == CCO_OK ? st : iw_fail_with(h, st);
+  return st == CCO_OK ? st : h->latch.fail(st);
 }
 
 int cco_index_write_finish(cco_index_write_t *h, cco_index_write_out_t *out) {
   if (!h || !out) return set_error(CCO_E_INVALID_ARG, "null argument");
-  CKR(iw_state(h));
+  CKR(h->latch.state("the index write is finished"));
   CK(cudaSetDevice(h->ctx->device));
   const int st = iw_finish(h, out);
-  if (st != CCO_OK) return iw_fail_with(h, st);
-  h->finished = true;
+  if (st != CCO_OK) return h->latch.fail(st);
+  h->latch.finished = true;
   return CCO_OK;
 }
 
@@ -8962,6 +8878,7 @@ int cco_index_write_free(cco_index_write_t *h) {
   cudaStreamSynchronize(h->ctx->stream);
   delete h->ar;
   cudaStreamSynchronize(h->ctx->stream);
+  h->stage.release(h->ctx);
   if (h->hbody) h->ctx->pinned_put(h->hbody);
   delete h;
   return CCO_OK;

@@ -23,12 +23,9 @@ constexpr int kIpTopDepth = 3;   // the top walk: down to the hits' brackets
 
 // what is wrong with a page, beyond the kSr* codes of the walks
 enum {
-  kIpNotObject = 32,    // the top level is not an object
-  kIpError,             // a top-level "error" member
-  kIpTimedOut,          // timed_out is true
+  kIpTimedOut = 32,     // timed_out is true
   kIpShards,            // _shards.failed is not 0
   kIpHitsNotArray,      // hits.hits is neither an array nor absent (null)
-  kIpRepeatedId,        // a hit with two _id members
   kIpNoSource,          // a hit without _source
   kIpSourceNotObject,   // a hit whose _source is not an object
 };
@@ -40,20 +37,9 @@ struct IpTop {
   long long sid_b, sid_e;   // the raw inside of _scroll_id; sid_b < 0: absent
   long long status;         // the first "status" member, when it is a 32-bit integer (has_status)
   int has_status;
-  int code;                 // 0, a kSr* code at byte `bad`, or a kIp* code
+  int code;                 // 0, a kSr* code at byte `bad`, kSrNotObject, kSrEsError or a kIp* code
   long long bad;
 };
-
-// walk-order index of index entry e in the sorted entry list src[0 .. n)
-__device__ __forceinline__ long long ip_walk_at(const long long *__restrict__ src, long long n, long long e) {
-  long long lo = 0, hi = n - 1;
-  while (lo < hi) {
-    const long long mid = (lo + hi) >> 1;
-    if (src[mid] < e) lo = mid + 1;
-    else hi = mid;
-  }
-  return lo;
-}
 
 // One warp over the entries at depth <= kIpTopDepth (the list x.src[0 .. n)): the page is ws* '{' members '}' ws*.  Of a
 // repeated member the first counts, except "error", which fails the page wherever it is.  hopen / hclose (n / 2 + 1
@@ -67,7 +53,7 @@ __global__ void k_ip_top(SrIdx x, long long n, long long len, IpTop *__restrict_
   long long first = 0;
   while (first < len && sr_ws(b[first])) ++first;
   if (n < 2 || x.pos[x.at(0)] != first || b[first] != '{') {
-    r.code = kIpNotObject;
+    r.code = kSrNotObject;
   } else if (x.dep[x.at(n - 1)] != 0 || b[x.pos[x.at(n - 1)]] != '}' || !sr_gap_ws(b, x.pos[x.at(n - 1)] + 1, len)) {
     r.code = kSrSyntax;
     r.bad = x.pos[x.at(n - 1)] + 1;
@@ -102,7 +88,7 @@ __global__ void k_ip_top(SrIdx x, long long n, long long len, IpTop *__restrict_
         if (v.kind != kVObject) return true;
         long long bad2 = 0;
         bool seen_failed = false;
-        nested(sr_members(x, ip_walk_at(x.src, n, v.ob), ip_walk_at(x.src, n, v.oe), 2, &bad2, [&](long long nb2, long long ne2, const SrVal &w) {
+        nested(sr_members(x, sr_walk_at(x.src, n, v.ob), sr_walk_at(x.src, n, v.oe), 2, &bad2, [&](long long nb2, long long ne2, const SrVal &w) {
                  if (!seen_failed && sr_is(b, nb2, ne2, "failed", 6)) {
                    seen_failed = true;
                    long long f = 1;
@@ -116,7 +102,7 @@ __global__ void k_ip_top(SrIdx x, long long n, long long len, IpTop *__restrict_
         if (v.kind != kVObject) return true;
         long long bad2 = 0;
         bool seen_total = false, seen_inner = false;
-        nested(sr_members(x, ip_walk_at(x.src, n, v.ob), ip_walk_at(x.src, n, v.oe), 2, &bad2, [&](long long nb2, long long ne2, const SrVal &w) {
+        nested(sr_members(x, sr_walk_at(x.src, n, v.ob), sr_walk_at(x.src, n, v.oe), 2, &bad2, [&](long long nb2, long long ne2, const SrVal &w) {
                  if (sr_is(b, nb2, ne2, "total", 5) && !seen_total) {
                    seen_total = true;
                    if (w.kind == kVScalar) {
@@ -124,7 +110,7 @@ __global__ void k_ip_top(SrIdx x, long long n, long long len, IpTop *__restrict_
                    } else if (w.kind == kVObject) {   // ES 7: {"value": n, "relation": "eq" | "gte"}
                      long long bad3 = 0, value = -1;
                      bool seen_value = false, seen_rel = false, exact = true;
-                     nested(sr_members(x, ip_walk_at(x.src, n, w.ob), ip_walk_at(x.src, n, w.oe), 3, &bad3,
+                     nested(sr_members(x, sr_walk_at(x.src, n, w.ob), sr_walk_at(x.src, n, w.oe), 3, &bad3,
                                        [&](long long nb3, long long ne3, const SrVal &u) {
                                          if (!seen_value && sr_is(b, nb3, ne3, "value", 5)) {
                                            seen_value = true;
@@ -159,7 +145,7 @@ __global__ void k_ip_top(SrIdx x, long long n, long long len, IpTop *__restrict_
       r.code = code;
       r.bad = nbad;
     } else if (has_error) {
-      r.code = kIpError;
+      r.code = kSrEsError;
     } else if (timed_out) {
       r.code = kIpTimedOut;
     } else if (shards_failed) {
@@ -168,7 +154,7 @@ __global__ void k_ip_top(SrIdx x, long long n, long long len, IpTop *__restrict_
       r.code = kIpHitsNotArray;
     } else if (hits_kind == kVArray) {
       long long nh = 0;
-      r.code = sr_objects(x, ip_walk_at(x.src, n, ha), ip_walk_at(x.src, n, hb), 3, kSrHitNotObject, &bad, &nh,
+      r.code = sr_objects(x, sr_walk_at(x.src, n, ha), sr_walk_at(x.src, n, hb), 3, kSrHitNotObject, &bad, &nh,
                           [&](long long k, long long o, long long c) {
                             if (lane == 0) {
                               hopen[k] = o;
@@ -208,7 +194,7 @@ __global__ void k_ip_hit(SrIdx x, long long n_hits, const long long *__restrict_
       }
       return true;
     });
-    const int code = rc ? 0 : !n_id || !id_str ? kSrNoId : n_id > 1 ? kIpRepeatedId : !n_src ? kIpNoSource : !src_obj ? kIpSourceNotObject : 0;
+    const int code = rc ? 0 : !n_id || !id_str ? kSrNoId : n_id > 1 ? kSrRepeatedId : !n_src ? kIpNoSource : !src_obj ? kIpSourceNotObject : 0;
     if (lane == 0) {
       if (rc) sr_fail(byte_err, bad, rc);
       if (code) sr_fail(err, h, code);

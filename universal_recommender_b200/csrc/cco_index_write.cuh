@@ -19,13 +19,10 @@ constexpr int kIwTopDepth = 2;   // the top walk: down to the items' brackets
 
 // what is wrong with a _bulk response, beyond the kSr* codes of the walks
 enum {
-  kIwNotObject = 48,     // the top level is not an object
-  kIwError,              // a top-level "error" member
-  kIwNoItems,            // no "items" member, or it is not an array
+  kIwNoItems = 48,       // no "items" member, or it is not an array
   kIwItemNotObject,      // an items element that is not an object
   kIwNotIndex,           // an item whose one member is not an "index" object
   kIwNoId,               // an item without a string index._id
-  kIwRepeatedId,         // an item with two index._id members
   kIwIdMismatch,         // index._id is not the document's _id
   kIwNoStatus,           // an item without index.status
   kIwRepeatedStatus,     // an item with two index.status members
@@ -37,7 +34,7 @@ struct IwTop {
   long long n_items;
   long long status;   // the first "status" member, when it is a 32-bit integer (has_status)
   int has_status;
-  int code;           // 0, a kSr* code at byte `bad`, or a kIw* code
+  int code;           // 0, a kSr* code at byte `bad`, kSrNotObject, kSrEsError or a kIw* code
   long long bad;
 };
 
@@ -74,7 +71,7 @@ __global__ void k_iw_top(SrIdx x, long long n, long long len, IwTop *__restrict_
   long long first = 0;
   while (first < len && sr_ws(b[first])) ++first;
   if (n < 2 || x.pos[x.at(0)] != first || b[first] != '{') {
-    r.code = kIwNotObject;
+    r.code = kSrNotObject;
   } else if (x.dep[x.at(n - 1)] != 0 || b[x.pos[x.at(n - 1)]] != '}' || !sr_gap_ws(b, x.pos[x.at(n - 1)] + 1, len)) {
     r.code = kSrSyntax;
     r.bad = x.pos[x.at(n - 1)] + 1;
@@ -100,12 +97,12 @@ __global__ void k_iw_top(SrIdx x, long long n, long long len, IwTop *__restrict_
       r.code = rc;
       r.bad = bad;
     } else if (has_error) {
-      r.code = kIwError;
+      r.code = kSrEsError;
     } else if (items_kind != kVArray) {
       r.code = kIwNoItems;
     } else {
       long long ni = 0;
-      r.code = sr_objects(x, ip_walk_at(x.src, n, ia), ip_walk_at(x.src, n, ib), 2, kIwItemNotObject, &bad, &ni,
+      r.code = sr_objects(x, sr_walk_at(x.src, n, ia), sr_walk_at(x.src, n, ib), 2, kIwItemNotObject, &bad, &ni,
                           [&](long long k, long long o, long long c) {
                             if (lane == 0) {
                               iopen[k] = o;
@@ -187,7 +184,7 @@ __global__ void k_iw_item(SrIdx x, long long n_items, const long long *__restric
       const long long i0 = it.id_off[doc], i1 = it.id_off[doc + 1];
       code = !index_obj || n_members != 1 ? kIwNotIndex
              : !n_id || !id_str          ? kIwNoId
-             : n_id > 1                  ? kIwRepeatedId
+             : n_id > 1                  ? kSrRepeatedId
              : !n_status                 ? kIwNoStatus
              : n_status > 1              ? kIwRepeatedStatus
              : !status_ok                ? kIwBadStatus

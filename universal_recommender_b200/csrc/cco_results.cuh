@@ -40,6 +40,13 @@ enum {
   kSrNoScore,           // a hit whose _score is missing, null or not a number
   kSrBadRank,           // a ranking member that is present but neither a number nor null
 };
+// codes every reader shares (line errors take 16 .. 19, index pages 32 .., index write 48 ..)
+enum {
+  kSrOpenString = 20,   // the body ends inside a string
+  kSrNotObject,         // the top level is not an object (index pages, index write)
+  kSrEsError,           // a top-level "error" member (index pages, index write)
+  kSrRepeatedId,        // a hit or item with two _id members (index pages, index write)
+};
 
 __device__ __forceinline__ void sr_fail(unsigned long long *w, long long key, int code) {
   atomicMin(w, ((unsigned long long)key << 8) | (unsigned)code);
@@ -321,6 +328,16 @@ __device__ __forceinline__ bool sr_gap_ws(const unsigned char *__restrict__ b, l
   for (; p < e; ++p)
     if (!sr_ws(b[p])) return false;
   return true;
+}
+// walk-order index of index entry e in the sorted entry list src[0 .. n)
+__device__ __forceinline__ long long sr_walk_at(const long long *__restrict__ src, long long n, long long e) {
+  long long lo = 0, hi = n - 1;
+  while (lo < hi) {
+    const long long mid = (lo + hi) >> 1;
+    if (src[mid] < e) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo;
 }
 // the raw inside of a string: valid escapes, no raw byte < 0x20
 __device__ __forceinline__ bool sr_string_ok(const unsigned char *__restrict__ b, long long p, long long e) {
