@@ -629,6 +629,62 @@ int cco_event_log_resident_bytes(const cco_event_log_t *log, int64_t *bytes);
  */
 enum { CCO_LOG_INTERN_IDS = 4 };
 int cco_event_log_intern_stats(const cco_event_log_t *log, int64_t *n_user_keys, int64_t *n_item_keys);
+
+/*
+ * Snapshots: a finished log saved as one binary image and loaded back, so that a trainer restarts (after a deploy, a crash,
+ * or on another GPU machine) without reading its export again.  The loaded log is the saved one: info, window_stats,
+ * resident_bytes, intern_stats and every consumer's output are equal, and a loaded extendable log extends as the saved
+ * one would.  Both sides stream in chunks, so neither needs the whole image in host memory.
+ *  - cco_event_log_save_size: the image's exact length.  The image is built at the first save call after a finish
+ *    (a hash pass over the device sections) and kept until the log is extended or freed.
+ *  - cco_event_log_save: bytes [offset, offset + len) of the image into dst, any split; the device sections are copied on
+ *    the context's copy stream through its pinned staging.
+ *  - cco_event_log_load_begin / _append / _finish: a new log from the image's bytes, any split.  The sections are copied
+ *    into their device buffers as they arrive; finish checks the whole image and builds the log.
+ * Refused with CCO_E_INVALID_ARG: saving a log that is not finished or has failed.
+ *
+ * Layout (version CCO_SNAPSHOT_VERSION; integers little-endian; offsets from the image's first byte):
+ *  - header, bytes [0, 64): the magic "CCOLOGSN" (8 bytes); u32 format version; u32 CCO_ABI_VERSION; u32 n_sections;
+ *    u32 0; i64 total bytes; u64 the checksum of bytes [0, 64 + 40 n_sections) with these 8 bytes read as 0; 24 bytes 0.
+ *  - section table, bytes [64, 64 + 40 n_sections): per section u32 kind; u32 0; i64 offset; i64 length; i64 device
+ *    bytes (the buffer the loader allocates for it: its length plus the log's padding or growth room; 0 for a host
+ *    section); u64 checksum.  Kinds ascend; offsets are multiples of 256 and sections do not overlap the table or each
+ *    other; the last section ends at the total.  Bytes between sections are padding (zero when saved, not read).
+ *  - checksum of n bytes: mix(n) + sum over words i of mix(w_i ^ (i * 0x9e3779b97f4a7c15)) mod 2^64, w_i the i-th 8-byte
+ *    word (the last one zero-filled) and mix splitmix64's finaliser (x ^= x >> 30; x *= 0xbf58476d1ce4e5b9; x ^= x >> 27;
+ *    x *= 0x94d049bb133111eb; x ^= x >> 31).
+ *  - host sections (lists of strings: i64 n, i64 offsets [n + 1] from 0, the bytes):
+ *      1 state: 16 i64: flags (CCO_LOG_*), remove_duplicates, cutoff_ms, chunk_bytes, n_lines, property events, ignored
+ *        lines, property items, property fields, expired lines, duplicate lines, the intern hash mask, 4 zeros;
+ *      2 names: the event names (a string list); 3 counts: training then ranking events per name (i64 each);
+ *      4 fields: the aggregated properties' field names (a string list);
+ *      5 property_lines: the global line of each retained property-event line (i64; CCO_LOG_EXTENDABLE).
+ *  - device sections, present where the log holds the buffer (string columns: i64 offsets [n + 1] from 0 and the bytes):
+ *      6-11 the training users, training items and ranking items (name-major, file order inside a name); 12 rank_times;
+ *      13 train_lines (KEEP_HISTORY or EXTENDABLE); 14 rank_lines (EXTENDABLE); 15 train_times (KEEP_HISTORY);
+ *      16 train_keys (INTERN_IDS: user key << 32 | item key); 17 records (EXTENDABLE: 40 bytes per retained line);
+ *      18 duplicate_times (EXTENDABLE with remove_duplicates); 19 property_bytes (EXTENDABLE: the retained property-event
+ *      lines); 20-24 the aggregated properties (i32 field of each triple, value offsets, values, item offsets, item
+ *      bytes); 25-26 property_items (the property events' item ids a log without EXTENDABLE keeps); 27-30 the user and
+ *      item keys' strings (INTERN_IDS; key k is string k).  The intern hash tables are not stored: the loader rebuilds
+ *      them from the strings, so a snapshot of a log is independent of where its tables placed the keys.
+ *
+ * A snapshot is untrusted input: every damaged or inconsistent image is refused with CCO_E_INVALID_ARG and a message that
+ * names the header or the section, and no kernel reads a byte through a stored offset before the host has the verdict
+ * on it.  Refused: a wrong magic, format version or ABI version; a section table out of order, overlapping or past the
+ * end; bytes past the end; an image shorter than its total at finish; a checksum mismatch; and any structural violation --
+ * decreasing offsets or offsets that disagree with their bytes, name or field numbers out of range, keys >= their table's
+ * count, an id stored twice in a key table, lines >= the line count, records out of line order, column lengths that
+ * disagree with the counts, a section the flags do not allow or a missing one.  A failed load frees the device memory it
+ * took; the log then answers every call but free with the failure's message.  CCO_E_UNSUPPORTED: group contexts, as for
+ * every log.  A different format version is refused, never converted.
+ */
+#define CCO_SNAPSHOT_VERSION 1
+int cco_event_log_save_size(cco_event_log_t *log, int64_t *bytes);
+int cco_event_log_save(cco_event_log_t *log, int64_t offset, void *dst, int64_t len);
+int cco_event_log_load_begin(cco_ctx_t *ctx, cco_event_log_t **out);
+int cco_event_log_load_append(cco_event_log_t *log, const void *bytes, int64_t len);
+int cco_event_log_load_finish(cco_event_log_t *log);
 /*
  * The query of user u, for the query event names n_0 .. n_{k-1}:
  *  - history of n_q: u's training events of n_q, latest first (eventTime desc, ties to the later line), the first limits[q]

@@ -14,6 +14,7 @@
 #include <charconv>
 #include <cmath>
 #include <functional>
+#include <memory>
 #include <cub/cub.cuh>
 #include <nvtx3/nvToolsExt.h>
 #include <condition_variable>
@@ -36,6 +37,7 @@
 #include "cco_index_write.cuh"
 #include "cco_refresh.cuh"
 #include "cco_intern.cuh"
+#include "cco_snapshot.cuh"
 
 namespace cco {
 
@@ -3738,6 +3740,18 @@ struct InternTable {
     return v;
   }
 };
+extern "C++" {
+namespace cco {
+struct SnapImage;
+struct SnapLoad;
+void snap_delete(SnapImage *);
+void snap_delete(SnapLoad *);
+struct SnapFree {
+  template <typename T>
+  void operator()(T *p) const { snap_delete(p); }
+};
+}  // namespace cco
+}  // extern "C++"
 struct cco_event_log {
   cco_ctx *ctx = nullptr;
   long long n_lines = 0, n_prop = 0, n_ignored = 0;
@@ -3793,6 +3807,13 @@ struct cco_event_log {
   long long chunk0 = 0;
   long long *dup_time = nullptr;
   long long n_dup_time = 0;
+  // the property events' item ids, which a log read without CCO_LOG_EXTENDABLE keeps after the aggregation (a snapshot
+  // carries them, so that a loaded log holds the bytes the saved one holds)
+  EvCol pitem;
+  // snapshots (cco_event_log_save / cco_event_log_load_*): the image of the finished log, built at the first save call
+  // after a finish; the state of a load in progress
+  std::unique_ptr<cco::SnapImage, cco::SnapFree> snap;
+  std::unique_ptr<cco::SnapLoad, cco::SnapFree> load;
   bool finished = false;
   int fail = CCO_OK;                           // a failed append / finish: every later call returns it with fail_msg
   std::string fail_msg;
@@ -4074,7 +4095,11 @@ static int event_properties(cco_ctx *c, Arena &ar, cco_event_log *lg, long long 
   CKR(mail_wait(c));
   lg->n_triples = T;
   auto drop_items = [&] {   // an extendable log aggregates at every finish: the item column goes once the triples are built
-    if (!lg->extendable) return;
+    if (!lg->extendable) {
+      lg->pitem.off = pcol.off;
+      lg->pitem.w = pcol.w;
+      return;
+    }
     log_drop(lg, pcol.off);
     log_drop(lg, pcol.w);
   };
@@ -5271,6 +5296,7 @@ static int log_rankings(const cco_event_log *lg, int32_t n_rank, const cco_log_r
 // a failed log answers every call with its first error's message; a log in progress is not read before finish
 static int log_state(const cco_event_log *lg, bool want_finished) {
   if (lg->fail != CCO_OK) return set_error(CCO_E_INVALID_ARG, "the read of this log failed: %s", lg->fail_msg.c_str());
+  if (lg->load) return set_error(CCO_E_INVALID_ARG, "the log is being loaded (cco_event_log_load_finish)");
   if (lg->finished != want_finished)
     return set_error(CCO_E_INVALID_ARG, want_finished ? "the log is not finished (cco_event_log_finish)" : "the log is finished");
   return CCO_OK;
@@ -5327,6 +5353,7 @@ int cco_event_log_extend(cco_event_log_t *lg, const cco_event_window_t *w) {
   if (!lg) return set_error(CCO_E_INVALID_ARG, "null argument");
   CKR(log_state(lg, true));
   if (!lg->extendable) return set_error(CCO_E_INVALID_ARG, "the log was read without CCO_LOG_EXTENDABLE (cco_event_log_begin_ex)");
+  lg->snap.reset();   // the image is of the log as it was finished
   if (w) {
     if (w->reserved != 0) return set_error(CCO_E_INVALID_ARG, "the window's reserved field must be 0");
     if ((w->remove_duplicates != 0) != lg->dedup || (w->remove_duplicates != 0 && w->remove_duplicates != 1))
@@ -7188,6 +7215,747 @@ int cco_query_file_free(cco_query_file_t *qf) {
 int cco_event_log_free(cco_event_log_t *lg) {
   event_log_release(lg);
   return CCO_OK;
+}
+
+// ---- event log snapshots (cco_event_log_save / cco_event_log_load_*; layout in include/cco_b200.h) --------------------
+namespace cco {
+constexpr char kSnapMagic[8] = {'C', 'C', 'O', 'L', 'O', 'G', 'S', 'N'};
+constexpr uint32_t kSnapVersion = CCO_SNAPSHOT_VERSION;
+constexpr long long kSnapHead = 64, kSnapEntry = 40, kSnapAlign = 256, kSnapStateWords = 16;
+constexpr long long kSnapStage = 32LL << 20;   // pinned staging of a save, per buffer (two)
+enum SnapKind : uint32_t {
+  kSnState = 1, kSnNames, kSnCounts, kSnFields, kSnPropLines,   // host sections
+  kSnTuOff, kSnTuBytes, kSnTiOff, kSnTiBytes, kSnRiOff, kSnRiBytes, kSnRtime, kSnTline, kSnRline, kSnTtime, kSnTkey, kSnRecords,
+  kSnDupTime, kSnPropBytes, kSnPField, kSnPVoff, kSnPVals, kSnPIoff, kSnPIbytes, kSnPItemOff, kSnPItemBytes, kSnUserOff,
+  kSnUserBytes, kSnItemOff, kSnItemBytes,
+  kSnEnd
+};
+static const char *const kSnName[kSnEnd] = {"", "state", "names", "counts", "fields", "property_lines", "train_users.offsets",
+  "train_users.bytes", "train_items.offsets", "train_items.bytes", "rank_items.offsets", "rank_items.bytes", "rank_times",
+  "train_lines", "rank_lines", "train_times", "train_keys", "records", "duplicate_times", "property_bytes", "properties.fields",
+  "properties.value_offsets", "properties.values", "properties.item_offsets", "properties.item_bytes",
+  "property_items.offsets", "property_items.bytes", "user_keys.offsets", "user_keys.bytes", "item_keys.offsets",
+  "item_keys.bytes"};
+static bool snap_host_kind(uint32_t k) { return k >= kSnState && k <= kSnPropLines; }
+// string bytes carry 16 bytes of padding past a whole word, the property lines 24 (event_pad)
+static bool snap_str_bytes(uint32_t k) {
+  return k == kSnTuBytes || k == kSnTiBytes || k == kSnRiBytes || k == kSnPItemBytes || k == kSnUserBytes || k == kSnItemBytes;
+}
+// the least device bytes a section of len bytes takes (what the log allocates for it)
+static long long snap_need(uint32_t k, long long len) {
+  if (snap_str_bytes(k)) return std::max<long long>((len + 23) / 8 * 8, 16);
+  if (k == kSnPropBytes) return len + 24;
+  return std::max<long long>(len, k == kSnRecords ? (long long)sizeof(WinRec) : 16);
+}
+
+struct SnapSec {
+  uint32_t kind = 0;
+  long long off = 0, len = 0, alloc = 0;   // alloc: device bytes (0: a host section)
+  uint64_t sum = 0;
+  unsigned char *dev = nullptr;
+  std::string host;
+};
+struct SnapImage {
+  std::string head;   // header + table, zero-padded to the first section
+  std::vector<SnapSec> secs;
+  long long total = 0;
+};
+struct SnapLoad {
+  std::string head;
+  long long pos = 0, total = -1, n_sec = 0;
+  bool table = false;
+  std::vector<SnapSec> secs;
+  long long pb_newlines = 0;
+  unsigned char pb_last = 0;
+};
+}  // namespace cco
+extern "C++" {
+namespace cco {
+void snap_delete(SnapImage *p) { delete p; }
+void snap_delete(SnapLoad *p) { delete p; }
+template <typename T>
+static void snap_put(std::string *s, T v) {
+  s->append((const char *)&v, sizeof v);
+}
+template <typename T>
+static T snap_get(const std::string &s, long long at) {
+  T v;
+  memcpy(&v, s.data() + at, sizeof v);
+  return v;
+}
+}  // namespace cco
+}  // extern "C++"
+namespace cco {
+
+static uint64_t snap_sum_host(const unsigned char *p, long long len) {
+  uint64_t h = snap_mix((uint64_t)len);
+  for (long long i = 0; i * 8 < len; ++i) {
+    uint64_t w = 0;
+    memcpy(&w, p + 8 * i, (size_t)std::min<long long>(8, len - 8 * i));
+    h += snap_mix(w ^ (uint64_t)i * kSnapGolden);
+  }
+  return h;
+}
+// a list of strings: n, offsets [n + 1] from 0, bytes
+static std::string snap_strings(const std::vector<std::string> &v) {
+  std::string s;
+  snap_put<int64_t>(&s, (int64_t)v.size());
+  int64_t o = 0;
+  snap_put<int64_t>(&s, 0);
+  for (const std::string &x : v) snap_put<int64_t>(&s, o += (int64_t)x.size());
+  for (const std::string &x : v) s += x;
+  return s;
+}
+static int snap_unstrings(const SnapSec &sc, std::vector<std::string> *out) {
+  const std::string &s = sc.host;
+  const long long L = (long long)s.size();
+  const int64_t n = L >= 8 ? snap_get<int64_t>(s, 0) : -1;
+  if (n < 0 || n > (L - 16) / 8) return set_error(CCO_E_INVALID_ARG, "snapshot section %s: a bad string count", kSnName[sc.kind]);
+  const long long b0 = 16 + 8 * n;
+  int64_t prev = 0;
+  out->clear();
+  for (int64_t i = 0; i < n; ++i) {
+    const int64_t o = snap_get<int64_t>(s, 8 * (i + 2));
+    if (o < prev || b0 + o > L) return set_error(CCO_E_INVALID_ARG, "snapshot section %s: string %lld has a bad offset", kSnName[sc.kind], (long long)i);
+    out->emplace_back(s.data() + b0 + prev, (size_t)(o - prev));
+    prev = o;
+  }
+  if (snap_get<int64_t>(s, 8) != 0 || b0 + prev != L)
+    return set_error(CCO_E_INVALID_ARG, "snapshot section %s: the offsets disagree with its length", kSnName[sc.kind]);
+  return CCO_OK;
+}
+// the log field a device section fills
+static void **snap_slot(cco_event_log *lg, uint32_t k) {
+  switch (k) {
+    case kSnTuOff: return (void **)&lg->tu.off;
+    case kSnTuBytes: return (void **)&lg->tu.w;
+    case kSnTiOff: return (void **)&lg->ti.off;
+    case kSnTiBytes: return (void **)&lg->ti.w;
+    case kSnRiOff: return (void **)&lg->ri.off;
+    case kSnRiBytes: return (void **)&lg->ri.w;
+    case kSnRtime: return (void **)&lg->rtime;
+    case kSnTline: return (void **)&lg->tline;
+    case kSnRline: return (void **)&lg->rline;
+    case kSnTtime: return (void **)&lg->ttime;
+    case kSnTkey: return (void **)&lg->tkey;
+    case kSnRecords: return (void **)&lg->rec;
+    case kSnDupTime: return (void **)&lg->dup_time;
+    case kSnPropBytes: return (void **)&lg->pb;
+    case kSnPField: return (void **)&lg->p_field;
+    case kSnPVoff: return (void **)&lg->p_voff;
+    case kSnPVals: return (void **)&lg->p_vals;
+    case kSnPIoff: return (void **)&lg->p_ioff;
+    case kSnPIbytes: return (void **)&lg->p_ibytes;
+    case kSnPItemOff: return (void **)&lg->pitem.off;
+    case kSnPItemBytes: return (void **)&lg->pitem.w;
+    case kSnUserOff: return (void **)&lg->users.off;
+    case kSnUserBytes: return (void **)&lg->users.w;
+    case kSnItemOff: return (void **)&lg->items.off;
+    case kSnItemBytes: return (void **)&lg->items.w;
+    default: return nullptr;
+  }
+}
+// the offsets section paired with a bytes section
+static uint32_t snap_off_of(uint32_t k) {
+  switch (k) {
+    case kSnTuBytes: case kSnTiBytes: case kSnRiBytes: case kSnPVals: case kSnPIbytes: case kSnPItemBytes: case kSnUserBytes:
+    case kSnItemBytes: return k - 1;
+    default: return 0;
+  }
+}
+
+// the checksums of the device sections, one k_snap_sum pass over all of them
+static int snap_device_sums(cco_ctx *c, std::vector<SnapSec *> &secs) {
+  cudaStream_t s = c->stream;
+  std::vector<SnapSpan> sp;
+  long long at = 0;
+  for (SnapSec *x : secs) {
+    sp.push_back(SnapSpan{x->dev, x->len, at});
+    at += ((x->len + 7) / 8 + 31) / 32 * 32;
+  }
+  if (sp.empty()) return CCO_OK;
+  Arena ar(s);
+  SnapSpan *d_sp;
+  unsigned long long *d_sum;
+  CKR(ar.alloc(&d_sp, sp.size()));
+  CKR(ar.alloc(&d_sum, sp.size()));
+  std::vector<unsigned long long> h((size_t)sp.size(), 0);
+  CK(cudaMemcpyAsync(d_sp, sp.data(), sizeof(SnapSpan) * sp.size(), cudaMemcpyHostToDevice, s));
+  CK(cudaMemsetAsync(d_sum, 0, sizeof(unsigned long long) * sp.size(), s));
+  if (at > 0) {
+    k_snap_sum<<<grid_for(at, 256, c->sm_count), 256, 0, s>>>((int)sp.size(), d_sp, at, d_sum);
+    c->launches++;
+  }
+  CK(cudaMemcpyAsync(h.data(), d_sum, sizeof(unsigned long long) * h.size(), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  for (size_t i = 0; i < secs.size(); ++i) secs[i]->sum = h[i] + snap_mix((uint64_t)secs[i]->len);
+  return CCO_OK;
+}
+
+// the image of a finished log: host sections serialised, device sections measured and hashed, the layout and header
+static int snap_image(cco_event_log *lg) {
+  if (lg->snap) return CCO_OK;
+  cco_ctx *c = lg->ctx;
+  cudaStream_t s = c->stream;
+  CK(cudaStreamSynchronize(s));
+  std::unique_ptr<SnapImage, SnapFree> im(new SnapImage());
+  auto host = [&](uint32_t k, std::string v) {
+    SnapSec x;
+    x.kind = k;
+    x.len = (long long)v.size();
+    x.host = std::move(v);
+    x.sum = snap_sum_host((const unsigned char *)x.host.data(), x.len);
+    im->secs.push_back(std::move(x));
+  };
+  std::string st;
+  const int64_t flags = (lg->history ? CCO_LOG_KEEP_HISTORY : 0) | (lg->extendable ? CCO_LOG_EXTENDABLE : 0) | (lg->intern ? CCO_LOG_INTERN_IDS : 0);
+  const int64_t w[kSnapStateWords] = {flags, lg->dedup, lg->cutoff, lg->chunk0, lg->n_lines, lg->n_prop, lg->n_ignored, lg->n_prop_items,
+                                      lg->n_prop_fields, lg->n_expired, lg->n_dup, (int64_t)lg->intern_mask, 0, 0, 0, 0};
+  st.assign((const char *)w, sizeof w);
+  host(kSnState, st);
+  const long long NG = (long long)lg->name_off.size() - 1;
+  std::vector<std::string> names;
+  for (long long g = 0; g < NG; ++g) names.emplace_back(lg->name_bytes.data() + lg->name_off[g], (size_t)(lg->name_off[g + 1] - lg->name_off[g]));
+  host(kSnNames, snap_strings(names));
+  std::string cnt;
+  for (int64_t v : lg->n_train) snap_put<int64_t>(&cnt, v);
+  for (int64_t v : lg->n_rank) snap_put<int64_t>(&cnt, v);
+  host(kSnCounts, cnt);
+  host(kSnFields, snap_strings(lg->field_names));
+  if (lg->pb) host(kSnPropLines, std::string((const char *)lg->prop_line.data(), sizeof(long long) * lg->prop_line.size()));
+  // device sections: entries from the counters, string bytes from the last offset
+  const long long NT = lg->train_at.back(), NR = lg->rank_at.back(), T = lg->n_triples;
+  auto last_off = [&](const long long *off, long long n, long long *v) -> int {
+    CK(cudaMemcpy(v, off + n, 8, cudaMemcpyDeviceToHost));
+    return CCO_OK;
+  };
+  std::vector<SnapSec *> dev;
+  for (uint32_t k = kSnTuOff; k < kSnEnd; ++k) {
+    void *p = *snap_slot(lg, k);
+    if (!p) continue;
+    long long n = 0;
+    switch (k) {
+      case kSnTuOff: case kSnTiOff: n = 8 * (NT + 1); break;
+      case kSnRiOff: n = 8 * (NR + 1); break;
+      case kSnRtime: case kSnRline: n = 8 * NR; break;
+      case kSnTline: case kSnTtime: case kSnTkey: n = 8 * NT; break;
+      case kSnRecords: n = (long long)sizeof(WinRec) * lg->n_rec; break;
+      case kSnDupTime: n = 8 * lg->n_dup_time; break;
+      case kSnPropBytes: n = lg->pb_len; break;
+      case kSnPField: n = 4 * T; break;
+      case kSnPVoff: case kSnPIoff: n = 8 * (T + 1); break;
+      case kSnPItemOff: n = 8 * (lg->n_prop + 1); break;
+      case kSnUserOff: n = 8 * (lg->users.n + 1); break;
+      case kSnItemOff: n = 8 * (lg->items.n + 1); break;
+      default: CKR(last_off((const long long *)*snap_slot(lg, snap_off_of(k)), im->secs.back().len / 8 - 1, &n));
+    }
+    SnapSec x;
+    x.kind = k;
+    x.len = n;
+    x.dev = (unsigned char *)p;
+    for (size_t i = 0; i < lg->dev.size(); ++i)
+      if (lg->dev[i] == p) x.alloc = (long long)lg->dev_bytes[i];
+    if (x.alloc < snap_need(k, n)) return set_error(CCO_E_CUDA, "internal: section %s holds %lld bytes of %lld", kSnName[k], x.alloc, n);
+    im->secs.push_back(std::move(x));
+  }
+  for (SnapSec &x : im->secs)
+    if (x.dev) dev.push_back(&x);
+  CKR(snap_device_sums(c, dev));
+  const long long NS = (long long)im->secs.size();
+  long long at = (kSnapHead + kSnapEntry * NS + kSnapAlign - 1) / kSnapAlign * kSnapAlign;
+  for (SnapSec &x : im->secs) {
+    x.off = at;
+    at = (at + x.len + kSnapAlign - 1) / kSnapAlign * kSnapAlign;
+  }
+  im->total = im->secs.back().off + im->secs.back().len;
+  std::string &h = im->head;
+  h.append(kSnapMagic, 8);
+  snap_put<uint32_t>(&h, kSnapVersion);
+  snap_put<uint32_t>(&h, CCO_ABI_VERSION);
+  snap_put<uint32_t>(&h, (uint32_t)NS);
+  snap_put<uint32_t>(&h, 0);
+  snap_put<int64_t>(&h, im->total);
+  h.resize(kSnapHead, '\0');
+  for (const SnapSec &x : im->secs) {
+    snap_put<uint32_t>(&h, x.kind);
+    snap_put<uint32_t>(&h, 0);
+    snap_put<int64_t>(&h, x.off);
+    snap_put<int64_t>(&h, x.len);
+    snap_put<int64_t>(&h, x.alloc);
+    snap_put<uint64_t>(&h, x.sum);
+  }
+  const uint64_t hs = snap_sum_host((const unsigned char *)h.data(), (long long)h.size());
+  memcpy(&h[32], &hs, 8);
+  h.resize((size_t)im->secs[0].off, '\0');
+  lg->snap = std::move(im);
+  return CCO_OK;
+}
+
+// bytes [offset, offset + len) of the image -> dst; device sections through two pinned buffers on the copy stream
+static int snap_save(cco_event_log *lg, long long offset, unsigned char *dst, long long len) {
+  cco_ctx *c = lg->ctx;
+  const SnapImage &im = *lg->snap;
+  const long long end = offset + len;
+  long long cur = offset;   // dst holds the image's bytes [offset, cur)
+  auto gap = [&](long long a) {   // zeros up to a (the padding before a section)
+    a = std::min(a, end);
+    if (a > cur) memset(dst + (cur - offset), 0, (size_t)(a - cur));
+    cur = std::max(cur, a);
+  };
+  if (offset < (long long)im.head.size()) {
+    cur = std::min(end, (long long)im.head.size());
+    memcpy(dst, im.head.data() + offset, (size_t)(cur - offset));
+  }
+  for (const SnapSec &x : im.secs) {
+    const long long a = std::max(x.off, cur), b = std::min(x.off + x.len, end);
+    if (a >= b) continue;
+    gap(a);
+    if (!x.dev) {
+      memcpy(dst + (a - offset), x.host.data() + (a - x.off), (size_t)(b - a));
+      cur = b;
+      continue;
+    }
+    const long long piece = std::min(kSnapStage, b - a);
+    unsigned char *buf[2] = {(unsigned char *)c->pinned_get((size_t)piece, false), nullptr};
+    if (b - a > piece) buf[1] = (unsigned char *)c->pinned_get((size_t)piece, false);
+    struct Put {
+      cco_ctx *c;
+      unsigned char **b;
+      ~Put() {
+        for (int i = 0; i < 2; ++i)
+          if (b[i]) c->pinned_put(b[i]);
+      }
+    } put{c, buf};
+    if (!buf[0] || (b - a > piece && !buf[1])) return set_error(CCO_E_OOM, "pinned host allocation failed");
+    long long prev = -1, prev_n = 0;
+    int j = 0;
+    for (long long q = a; q < b; q += piece, ++j) {
+      const long long n = std::min(piece, b - q);
+      CK(cudaMemcpyAsync(buf[j & 1], x.dev + (q - x.off), (size_t)n, cudaMemcpyDeviceToHost, c->copy_stream));
+      CK(cudaEventRecord(c->copy_ev[j & 1], c->copy_stream));
+      if (prev >= 0) {
+        CK(cudaEventSynchronize(c->copy_ev[(j - 1) & 1]));
+        memcpy(dst + (prev - offset), buf[(j - 1) & 1], (size_t)prev_n);
+      }
+      prev = q;
+      prev_n = n;
+    }
+    CK(cudaEventSynchronize(c->copy_ev[(j - 1) & 1]));
+    memcpy(dst + (prev - offset), buf[(j - 1) & 1], (size_t)prev_n);
+    cur = b;
+  }
+  gap(end);
+  return CCO_OK;
+}
+
+// ---- load ---------------------------------------------------------------------------------------------------------------
+static const char *snap_name(uint32_t k) { return k > 0 && k < kSnEnd ? kSnName[k] : "?"; }
+// the header and the section table, complete: checked before anything is allocated; then the device sections' buffers
+static int snap_table(cco_event_log *lg) {
+  SnapLoad &ld = *lg->load;
+  const std::string &h = ld.head;
+  const long long NS = ld.n_sec, tab = kSnapHead + kSnapEntry * NS;
+  std::string z = h;
+  memset(&z[32], 0, 8);
+  if (snap_sum_host((const unsigned char *)z.data(), tab) != snap_get<uint64_t>(h, 32))
+    return set_error(CCO_E_INVALID_ARG, "snapshot header: checksum mismatch");
+  long long prev_end = tab;
+  uint32_t prev_kind = 0;
+  for (long long i = 0; i < NS; ++i) {
+    const long long e = kSnapHead + kSnapEntry * i;
+    SnapSec x;
+    x.kind = snap_get<uint32_t>(h, e);
+    x.off = snap_get<int64_t>(h, e + 8);
+    x.len = snap_get<int64_t>(h, e + 16);
+    x.alloc = snap_get<int64_t>(h, e + 24);
+    x.sum = snap_get<uint64_t>(h, e + 32);
+    const char *nm = snap_name(x.kind);
+    if (x.kind <= prev_kind || x.kind >= kSnEnd || snap_get<uint32_t>(h, e + 4) != 0)
+      return set_error(CCO_E_INVALID_ARG, "snapshot section table: entry %lld has kind %u (unknown, repeated or out of order)", i, x.kind);
+    if (x.off % kSnapAlign != 0) return set_error(CCO_E_INVALID_ARG, "snapshot section %s: offset %lld is not 256-byte aligned", nm, x.off);
+    if (x.off < prev_end) return set_error(CCO_E_INVALID_ARG, "snapshot section %s: overlaps the section table or the section before it", nm);
+    if (x.len < 0 || x.len > ld.total - x.off)
+      return set_error(CCO_E_INVALID_ARG, "snapshot section %s: [%lld, +%lld) runs past the end (%lld bytes)", nm, x.off, x.len, ld.total);
+    if (snap_host_kind(x.kind) ? x.alloc != 0 : (x.alloc < snap_need(x.kind, x.len) || x.alloc > 2 * snap_need(x.kind, x.len) + 4096))
+      return set_error(CCO_E_INVALID_ARG, "snapshot section %s: %lld device bytes for %lld bytes", nm, x.alloc, x.len);
+    prev_end = x.off + x.len;
+    prev_kind = x.kind;
+    ld.secs.push_back(std::move(x));
+  }
+  if (prev_end != ld.total) return set_error(CCO_E_INVALID_ARG, "snapshot: %lld bytes, its last section ends at %lld", ld.total, prev_end);
+  cco_ctx *c = lg->ctx;
+  Arena ar(c->stream);
+  for (SnapSec &x : ld.secs) {
+    if (!x.alloc) {
+      x.host.reserve((size_t)x.len);
+      continue;
+    }
+    CKR(ar.alloc(&x.dev, (size_t)x.alloc));
+    CKR(log_keep(ar, lg, x.dev));
+  }
+  CK(cudaStreamSynchronize(c->stream));   // the copies run on the copy stream
+  for (SnapSec &x : ld.secs)
+    if (x.dev) CK(cudaMemsetAsync(x.dev, 0, (size_t)x.alloc, c->copy_stream));
+  ld.table = true;
+  return CCO_OK;
+}
+static int snap_append(cco_event_log *lg, const unsigned char *bytes, long long len) {
+  cco_ctx *c = lg->ctx;
+  CK(cudaSetDevice(c->device));
+  SnapLoad &ld = *lg->load;
+  while (len > 0 && !ld.table) {
+    const long long want = ld.head.size() < (size_t)kSnapHead ? kSnapHead : kSnapHead + kSnapEntry * ld.n_sec;
+    const long long take = std::min(len, want - (long long)ld.head.size());
+    ld.head.append((const char *)bytes, (size_t)take);
+    ld.pos += take;
+    bytes += take;
+    len -= take;
+    if ((long long)ld.head.size() == kSnapHead && want == kSnapHead) {
+      const std::string &h = ld.head;
+      if (memcmp(h.data(), kSnapMagic, 8) != 0) return set_error(CCO_E_INVALID_ARG, "snapshot header: not an event log snapshot (bad magic)");
+      if (snap_get<uint32_t>(h, 8) != kSnapVersion)
+        return set_error(CCO_E_INVALID_ARG, "snapshot header: format version %u, this library reads %u", snap_get<uint32_t>(h, 8), kSnapVersion);
+      if (snap_get<uint32_t>(h, 12) != CCO_ABI_VERSION)
+        return set_error(CCO_E_INVALID_ARG, "snapshot header: ABI version %u, this library is %u", snap_get<uint32_t>(h, 12), (unsigned)CCO_ABI_VERSION);
+      ld.n_sec = snap_get<uint32_t>(h, 16);
+      ld.total = snap_get<int64_t>(h, 24);
+      if (ld.n_sec < 1 || ld.n_sec >= kSnEnd) return set_error(CCO_E_INVALID_ARG, "snapshot header: %lld sections", ld.n_sec);
+      if (ld.total < kSnapHead + kSnapEntry * ld.n_sec) return set_error(CCO_E_INVALID_ARG, "snapshot header: %lld bytes, shorter than its section table", ld.total);
+    }
+    if ((long long)ld.head.size() == kSnapHead + kSnapEntry * ld.n_sec && ld.n_sec > 0) CKR(snap_table(lg));
+  }
+  if (len == 0) return CCO_OK;
+  if (len > ld.total - ld.pos) return set_error(CCO_E_INVALID_ARG, "snapshot: bytes past its end (%lld bytes)", ld.total);
+  const long long a = ld.pos, b = a + len;
+  for (SnapSec &x : ld.secs) {
+    const long long p = std::max(a, x.off), q = std::min(b, x.off + x.len);
+    if (p >= q) continue;
+    const unsigned char *src = bytes + (p - a);
+    if (!x.dev) {
+      x.host.append((const char *)src, (size_t)(q - p));
+      continue;
+    }
+    CK(cudaMemcpyAsync(x.dev + (p - x.off), src, (size_t)(q - p), cudaMemcpyHostToDevice, c->copy_stream));
+    if (x.kind == kSnPropBytes) {   // the lines a later finish parses: counted here, checked against property_lines
+      for (const unsigned char *r = src, *e = src + (q - p); (r = (const unsigned char *)memchr(r, '\n', (size_t)(e - r))); ++r) ++ld.pb_newlines;
+      ld.pb_last = src[q - p - 1];
+    }
+  }
+  ld.pos = b;
+  CK(cudaStreamSynchronize(c->copy_stream));   // the bytes are copied: the caller may reuse its buffer
+  return CCO_OK;
+}
+
+// the checks of a complete snapshot and the log built from it
+static int snap_finish(cco_event_log *lg) {
+  cco_ctx *c = lg->ctx;
+  cudaStream_t s = c->stream;
+  CK(cudaSetDevice(c->device));
+  NvtxRange nvtx("cco:event_log_load");
+  SnapLoad &ld = *lg->load;
+  if (!ld.table) return set_error(CCO_E_INVALID_ARG, "snapshot truncated at byte %lld: the header and section table are incomplete", ld.pos);
+  if (ld.pos < ld.total) {
+    for (const SnapSec &x : ld.secs)
+      if (x.off + x.len > ld.pos)
+        return set_error(CCO_E_INVALID_ARG, "snapshot truncated at byte %lld of %lld: section %s is incomplete", ld.pos, ld.total, kSnName[x.kind]);
+  }
+  CK(cudaStreamSynchronize(c->copy_stream));
+  SnapSec *sec[kSnEnd] = {};
+  std::vector<SnapSec *> dev;
+  for (SnapSec &x : ld.secs) {
+    sec[x.kind] = &x;
+    if (x.dev) dev.push_back(&x);
+  }
+  std::vector<uint64_t> want;
+  for (SnapSec *x : dev) want.push_back(x->sum);
+  for (SnapSec &x : ld.secs)
+    if (!x.dev && snap_sum_host((const unsigned char *)x.host.data(), x.len) != x.sum)
+      return set_error(CCO_E_INVALID_ARG, "snapshot section %s: checksum mismatch", kSnName[x.kind]);
+  mail_reset(c);
+  CKR(snap_device_sums(c, dev));
+  for (size_t i = 0; i < dev.size(); ++i)
+    if (dev[i]->sum != want[i]) return set_error(CCO_E_INVALID_ARG, "snapshot section %s: checksum mismatch", kSnName[dev[i]->kind]);
+  // host state
+  for (uint32_t k : {kSnState, kSnNames, kSnCounts, kSnFields})
+    if (!sec[k]) return set_error(CCO_E_INVALID_ARG, "snapshot section %s: missing", kSnName[k]);
+  if (sec[kSnState]->len != 8 * kSnapStateWords) return set_error(CCO_E_INVALID_ARG, "snapshot section state: %lld bytes, not %lld", sec[kSnState]->len, 8 * kSnapStateWords);
+  int64_t st[kSnapStateWords];
+  memcpy(st, sec[kSnState]->host.data(), sizeof st);
+  const int64_t flags = st[0];
+  if (flags & ~(int64_t)(CCO_LOG_KEEP_HISTORY | CCO_LOG_EXTENDABLE | CCO_LOG_INTERN_IDS))
+    return set_error(CCO_E_INVALID_ARG, "snapshot section state: unknown flags 0x%llx", (long long)flags);
+  bool counters_ok = (st[1] == 0 || st[1] == 1) && st[3] >= 1;
+  for (int i = 4; i <= 10; ++i) counters_ok = counters_ok && st[i] >= 0;
+  for (int i = 12; i < kSnapStateWords; ++i) counters_ok = counters_ok && st[i] == 0;
+  if (!counters_ok) return set_error(CCO_E_INVALID_ARG, "snapshot section state: a counter is out of range");
+  lg->history = flags & CCO_LOG_KEEP_HISTORY;
+  lg->extendable = flags & CCO_LOG_EXTENDABLE;
+  lg->intern = flags & CCO_LOG_INTERN_IDS;
+  lg->dedup = st[1] != 0;
+  lg->cutoff = st[2];
+  lg->chunk0 = st[3];
+  lg->n_lines = st[4];
+  lg->n_prop = st[5];
+  lg->n_ignored = st[6];
+  lg->n_prop_items = st[7];
+  lg->n_prop_fields = st[8];
+  lg->n_expired = st[9];
+  lg->n_dup = st[10];
+  lg->intern_mask = (uint64_t)st[11];
+  std::vector<std::string> names;
+  CKR(snap_unstrings(*sec[kSnNames], &names));
+  const long long NG = (long long)names.size();
+  for (long long g = 0; g < NG; ++g) {
+    if (!lg->name_code.emplace(names[g], (int)g).second)
+      return set_error(CCO_E_INVALID_ARG, "snapshot section names: name %lld repeats an earlier one", g);
+    lg->name_bytes += names[g];
+    lg->name_off.push_back((int64_t)lg->name_bytes.size());
+  }
+  if (sec[kSnCounts]->len != 16 * NG) return set_error(CCO_E_INVALID_ARG, "snapshot section counts: %lld bytes for %lld names", sec[kSnCounts]->len, NG);
+  lg->n_train.resize(NG);
+  lg->n_rank.resize(NG);
+  memcpy(lg->n_train.data(), sec[kSnCounts]->host.data(), 8 * (size_t)NG);
+  memcpy(lg->n_rank.data(), sec[kSnCounts]->host.data() + 8 * NG, 8 * (size_t)NG);
+  lg->train_at.assign(NG + 1, 0);
+  lg->rank_at.assign(NG + 1, 0);
+  for (long long g = 0; g < NG; ++g) {
+    if (lg->n_train[g] < 0 || lg->n_train[g] >= 0x7fffffffLL || lg->n_rank[g] < 0 || lg->n_rank[g] >= 0x7fffffffLL)
+      return set_error(CCO_E_INVALID_ARG, "snapshot section counts: name %lld has %lld training and %lld ranking events", g, (long long)lg->n_train[g],
+                       (long long)lg->n_rank[g]);
+    lg->train_at[g + 1] = lg->train_at[g] + lg->n_train[g];
+    lg->rank_at[g + 1] = lg->rank_at[g] + lg->n_rank[g];
+  }
+  CKR(snap_unstrings(*sec[kSnFields], &lg->field_names));
+  for (size_t f = 0; f < lg->field_names.size(); ++f)
+    for (size_t g = 0; g < f; ++g)
+      if (lg->field_names[f] == lg->field_names[g]) return set_error(CCO_E_INVALID_ARG, "snapshot section fields: field %zu repeats an earlier one", f);
+  if (lg->n_prop_fields > (long long)lg->field_names.size()) return set_error(CCO_E_INVALID_ARG, "snapshot section state: more property fields than field names");
+  // which sections the flags allow, and the length each must have
+  const long long NT = lg->train_at.back(), NR = lg->rank_at.back();
+  const long long T = sec[kSnPField] ? sec[kSnPField]->len / 4 : 0;
+  const long long UK = sec[kSnUserOff] ? sec[kSnUserOff]->len / 8 - 1 : 0, IK = sec[kSnItemOff] ? sec[kSnItemOff]->len / 8 - 1 : 0;
+  for (uint32_t k = kSnPropLines; k < kSnEnd; ++k) {
+    bool allowed = true;
+    long long want_len = -1, n_entries = -1;   // -1: any length (the paired offsets decide the bytes)
+    switch (k) {
+      case kSnPropLines: case kSnPropBytes: case kSnRecords: case kSnRline: allowed = lg->extendable; break;
+      case kSnDupTime: allowed = lg->extendable && lg->dedup; break;
+      case kSnTline: allowed = lg->history || lg->extendable; break;
+      case kSnTtime: allowed = lg->history; break;
+      case kSnTkey: case kSnUserOff: case kSnUserBytes: case kSnItemOff: case kSnItemBytes: allowed = lg->intern; break;
+      case kSnPItemOff: case kSnPItemBytes: allowed = !lg->extendable; break;
+      default: break;
+    }
+    switch (k) {
+      case kSnTuOff: case kSnTiOff: n_entries = NT; want_len = 8 * (NT + 1); break;
+      case kSnRiOff: n_entries = NR; want_len = 8 * (NR + 1); break;
+      case kSnRtime: case kSnRline: n_entries = NR; want_len = 8 * NR; break;
+      case kSnTline: case kSnTtime: case kSnTkey: n_entries = NT; want_len = 8 * NT; break;
+      case kSnPVoff: case kSnPIoff: n_entries = T; want_len = 8 * (T + 1); break;
+      case kSnPItemOff: n_entries = lg->n_prop; want_len = 8 * (lg->n_prop + 1); break;
+      case kSnPropLines: n_entries = lg->n_prop; want_len = 8 * lg->n_prop; break;
+      default: break;
+    }
+    SnapSec *x = sec[k];
+    const char *nm = kSnName[k];
+    if (x && !allowed) return set_error(CCO_E_INVALID_ARG, "snapshot section %s: not part of a log with flags 0x%llx", nm, (long long)flags);
+    if (!x) {   // an absent column holds no entries
+      const uint32_t ko = snap_off_of(k);
+      if (allowed && (n_entries > 0 || (ko && sec[ko]) || (lg->intern && (k == kSnUserOff || k == kSnItemOff))))
+        return set_error(CCO_E_INVALID_ARG, "snapshot section %s: missing", nm);
+      continue;
+    }
+    if (snap_off_of(k) && !sec[snap_off_of(k)]) return set_error(CCO_E_INVALID_ARG, "snapshot section %s: its offsets are missing", nm);
+    if ((k == kSnPVoff || k == kSnPIoff || k == kSnPVals || k == kSnPIbytes) && !sec[kSnPField])
+      return set_error(CCO_E_INVALID_ARG, "snapshot section %s: the property fields are missing", nm);
+    if (want_len >= 0 && x->len != want_len)
+      return set_error(CCO_E_INVALID_ARG, "snapshot section %s: %lld bytes, its counters give %lld", nm, x->len, want_len);
+    const long long unit = k == kSnRecords ? (long long)sizeof(WinRec) : k == kSnPField ? 4 : (k == kSnUserOff || k == kSnItemOff || k == kSnDupTime) ? 8 : 1;
+    if (x->len % unit != 0 || ((k == kSnUserOff || k == kSnItemOff) && x->len < 8))
+      return set_error(CCO_E_INVALID_ARG, "snapshot section %s: %lld bytes is not a whole number of entries", nm, x->len);
+    if (k == kSnPField && T == 0) return set_error(CCO_E_INVALID_ARG, "snapshot section %s: present without entries", nm);
+  }
+  if (sec[kSnPropBytes]) {
+    const long long NP = sec[kSnPropLines] ? sec[kSnPropLines]->len / 8 : 0;
+    if (ld.pb_newlines != NP || ld.pb_last != '\n' || NP == 0)
+      return set_error(CCO_E_INVALID_ARG, "snapshot section property_bytes: its lines disagree with property_lines");
+  } else if (lg->extendable && lg->n_prop > 0) {
+    return set_error(CCO_E_INVALID_ARG, "snapshot section property_bytes: missing");
+  }
+  if (sec[kSnPropLines]) {
+    lg->prop_line.resize((size_t)lg->n_prop);
+    memcpy(lg->prop_line.data(), sec[kSnPropLines]->host.data(), 8 * (size_t)lg->n_prop);
+    for (long long i = 0; i < lg->n_prop; ++i)
+      if (lg->prop_line[i] < 0 || lg->prop_line[i] >= lg->n_lines || (i > 0 && lg->prop_line[i] <= lg->prop_line[i - 1]))
+        return set_error(CCO_E_INVALID_ARG, "snapshot section property_lines: line %lld is out of order or >= the line count", i);
+  }
+  // device checks: one k_snap_check over every checked section, its verdict before anything reads through an offset
+  std::vector<SnapTask> tk;
+  std::vector<uint32_t> tkind;
+  long long at = 0;
+  auto task = [&](uint32_t k, int kind, long long n, long long bound, long long bound2) {
+    if (!sec[k] || n <= 0) return;
+    tk.push_back(SnapTask{sec[k]->dev, n, at, bound, bound2, kind});
+    tkind.push_back(k);
+    at += n;
+  };
+  for (uint32_t k : {kSnTuBytes, kSnTiBytes, kSnRiBytes, kSnPVals, kSnPIbytes, kSnPItemBytes, kSnUserBytes, kSnItemBytes}) {
+    const uint32_t ko = snap_off_of(k);
+    if (sec[ko]) task(ko, kSnapOffsets, sec[ko]->len / 8, sec[k] ? sec[k]->len : 0, 0);
+  }
+  task(kSnTline, kSnapBelow, NT, lg->n_lines, 0);
+  task(kSnRline, kSnapBelow, NR, lg->n_lines, 0);
+  task(kSnTkey, kSnapKeys, NT, UK, IK);
+  task(kSnPField, kSnapFields, T, (long long)lg->field_names.size(), 0);
+  task(kSnRecords, kSnapRecords, sec[kSnRecords] ? sec[kSnRecords]->len / (long long)sizeof(WinRec) : 0, lg->n_lines, NG);
+  if (!tk.empty()) {
+    Arena ar(s);
+    SnapTask *d_tk;
+    unsigned long long *bad, h_bad = ~0ULL;
+    CKR(ar.alloc(&d_tk, tk.size()));
+    CKR(ar.alloc(&bad, 1));
+    CK(cudaMemcpyAsync(d_tk, tk.data(), sizeof(SnapTask) * tk.size(), cudaMemcpyHostToDevice, s));
+    CK(cudaMemsetAsync(bad, 0xff, 8, s));
+    k_snap_check<<<grid_for(at, 256, c->sm_count), 256, 0, s>>>((int)tk.size(), d_tk, at, bad);
+    c->launches++;
+    CKR(mail_fetch(c, &h_bad, bad, 8));
+    CKR(mail_wait(c));
+    if (h_bad != ~0ULL) {
+      const SnapTask &t = tk[h_bad >> 40];
+      const long long i = (long long)(h_bad & ((1ULL << 40) - 1));
+      const char *nm = kSnName[tkind[h_bad >> 40]];
+      switch (t.kind) {
+        case kSnapOffsets:
+          return set_error(CCO_E_INVALID_ARG, "snapshot section %s: offset %lld decreases, does not start at 0 or does not end at the %lld bytes", nm, i, t.bound);
+        case kSnapBelow: return set_error(CCO_E_INVALID_ARG, "snapshot section %s: entry %lld is not a line of the log (%lld lines)", nm, i, t.bound);
+        case kSnapKeys: return set_error(CCO_E_INVALID_ARG, "snapshot section %s: entry %lld holds a key >= its table's key count", nm, i);
+        case kSnapFields: return set_error(CCO_E_INVALID_ARG, "snapshot section %s: entry %lld is not a field of the %lld names", nm, i, t.bound);
+        default:
+          return set_error(CCO_E_INVALID_ARG, "snapshot section %s: record %lld is out of line order, >= the line count or of a name >= %lld", nm, i, t.bound2);
+      }
+    }
+  }
+  // the log: the sections are its buffers
+  for (SnapSec *x : dev) *snap_slot(lg, x->kind) = x->dev;
+  lg->n_triples = T;
+  lg->p_ibytes_n = sec[kSnPIbytes] ? sec[kSnPIbytes]->len : 0;
+  if (sec[kSnRecords]) {
+    lg->n_rec = sec[kSnRecords]->len / (long long)sizeof(WinRec);
+    lg->rec_cap = sec[kSnRecords]->alloc / (long long)sizeof(WinRec);
+  }
+  lg->n_dup_time = sec[kSnDupTime] ? sec[kSnDupTime]->len / 8 : 0;
+  if (sec[kSnPropBytes]) {
+    lg->pb_len = sec[kSnPropBytes]->len;
+    lg->pb_cap = sec[kSnPropBytes]->alloc - 24;
+  }
+  Arena ar(s);
+  for (auto cl : {std::make_pair(&lg->tu, &lg->train_at), std::make_pair(&lg->ti, &lg->train_at), std::make_pair(&lg->ri, &lg->rank_at)}) {
+    if (cl.first->off) CKR(name_boff(c, ar, cl.first->off, *cl.second, &cl.first->boff));
+    else cl.first->boff.assign(NG + 1, 0);
+  }
+  // the intern tables: the stored strings hashed and claimed into empty tables, each its own key; a string stored twice
+  // would claim one slot for both
+  if (lg->intern) {
+    InternTable *tbs[2] = {&lg->users, &lg->items};
+    for (int x = 0; x < 2; ++x) {
+      InternTable *tb = tbs[x];
+      const uint32_t ko = x == 0 ? kSnUserOff : kSnItemOff;
+      const long long K = sec[ko]->len / 8 - 1;
+      tb->n = tb->kcap = K;
+      tb->bytes = tb->bcap = sec[ko + 1]->len;
+      tb->cap = intern_slots(K);
+      CKR(ar.alloc(&tb->hash, std::max<long long>(K, 1)));
+      CKR(log_keep(ar, lg, tb->hash));
+      CKR(ar.alloc(&tb->table, tb->cap));
+      CKR(log_keep(ar, lg, tb->table));
+      CK(cudaMemsetAsync(tb->table, 0xff, sizeof(uint32_t) * (size_t)tb->cap, s));
+      if (K == 0) continue;
+      uint64_t *hash;
+      uint32_t *slot_of, *flag, *pos, *idx, KN = 0;
+      CKR(ar.alloc(&hash, K));
+      CKR(ar.alloc(&slot_of, K));
+      CKR(ar.alloc(&flag, K + 1));
+      k_str_hash<<<grid_for(K, 256, c->sm_count), 256, 0, s>>>(K, tb->off, 0, tb->w, lg->intern_mask, hash);
+      k_intern_claim<<<grid_for(K, 256, c->sm_count), 256, 0, s>>>(K, tb->off, tb->w, hash, tb->off, tb->w, tb->hash, (uint64_t)tb->cap - 1,
+                                                                   tb->table, slot_of);
+      k_intern_first<<<grid_for(K, 256, c->sm_count), 256, 0, s>>>(K, slot_of, tb->table, flag);
+      c->launches += 3;
+      CKR(select_flagged(c, ar, K, flag, &pos, &idx));
+      CKR(mail_fetch(c, &KN, pos + K, 4));
+      CKR(mail_wait(c));
+      if (KN != (uint32_t)K) return set_error(CCO_E_INVALID_ARG, "snapshot section %s: an id is stored twice", kSnName[ko + 1]);
+      k_intern_new<<<grid_for(K, 256, c->sm_count), 256, 0, s>>>(K, idx, slot_of, hash, 0, tb->table, tb->hash);
+      c->launches++;
+    }
+  }
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  lg->load.reset();
+  lg->finished = true;
+  return CCO_OK;
+}
+// a failed load keeps no device memory: the log answers with its message until it is freed
+static int snap_fail(cco_event_log *lg, int rc) {
+  if (rc == CCO_OK) return rc;
+  log_fail(lg, rc);
+  cudaSetDevice(lg->ctx->device);
+  cudaStreamSynchronize(lg->ctx->copy_stream);
+  for (void *p : lg->dev) cudaFreeAsync(p, lg->ctx->stream);
+  cudaStreamSynchronize(lg->ctx->stream);
+  lg->dev.clear();
+  lg->dev_bytes.clear();
+  lg->load.reset();
+  return rc;
+}
+}  // namespace cco
+
+int cco_event_log_save_size(cco_event_log_t *lg, int64_t *bytes) {
+  if (!lg || !bytes) return set_error(CCO_E_INVALID_ARG, "null argument");
+  CKR(log_state(lg, true));
+  CK(cudaSetDevice(lg->ctx->device));
+  CKR(snap_image(lg));
+  *bytes = lg->snap->total;
+  return CCO_OK;
+}
+
+int cco_event_log_save(cco_event_log_t *lg, int64_t offset, void *dst, int64_t len) {
+  if (!lg || offset < 0 || len < 0 || (len > 0 && !dst)) return set_error(CCO_E_INVALID_ARG, "null argument, or a negative offset or length");
+  CKR(log_state(lg, true));
+  CK(cudaSetDevice(lg->ctx->device));
+  NvtxRange nvtx("cco:event_log_save");
+  CKR(snap_image(lg));
+  if (len > lg->snap->total - offset)
+    return set_error(CCO_E_INVALID_ARG, "bytes [%lld, %lld) of a %lld-byte snapshot", (long long)offset, (long long)(offset + len), lg->snap->total);
+  return snap_save(lg, offset, (unsigned char *)dst, len);
+}
+
+int cco_event_log_load_begin(cco_ctx_t *ctx, cco_event_log_t **out) {
+  if (!ctx || !out) return set_error(CCO_E_INVALID_ARG, "null argument");
+  *out = nullptr;
+  if (!ctx->members.empty()) return set_error(CCO_E_UNSUPPORTED, "an event log is resident on one GPU: load it on a per-GPU context");
+  CK(cudaSetDevice(ctx->device));
+  cco_event_log *lg = new cco_event_log();
+  lg->ctx = ctx;
+  lg->name_off.assign(1, 0);
+  lg->train_at.assign(1, 0);
+  lg->rank_at.assign(1, 0);
+  lg->load.reset(new SnapLoad());
+  *out = lg;
+  return CCO_OK;
+}
+
+int cco_event_log_load_append(cco_event_log_t *lg, const void *bytes, int64_t len) {
+  if (!lg || len < 0 || (len > 0 && !bytes)) return set_error(CCO_E_INVALID_ARG, "null argument or negative length");
+  if (lg->fail != CCO_OK) return set_error(CCO_E_INVALID_ARG, "the load of this log failed: %s", lg->fail_msg.c_str());
+  if (!lg->load) return set_error(CCO_E_INVALID_ARG, "the log is not being loaded (cco_event_log_load_begin)");
+  return snap_fail(lg, snap_append(lg, (const unsigned char *)bytes, len));
+}
+
+int cco_event_log_load_finish(cco_event_log_t *lg) {
+  if (!lg) return set_error(CCO_E_INVALID_ARG, "null argument");
+  if (lg->fail != CCO_OK) return set_error(CCO_E_INVALID_ARG, "the load of this log failed: %s", lg->fail_msg.c_str());
+  if (!lg->load) return set_error(CCO_E_INVALID_ARG, "the log is not being loaded (cco_event_log_load_begin)");
+  return snap_fail(lg, snap_finish(lg));
 }
 
 // ---- SURVEY.md 8f-3: PopModel rank histograms -------------------------------------------------------------------------

@@ -406,6 +406,37 @@ class CcoContext:
             raise
         return self._adopt_log(h)
 
+    def load_events(self, src, chunk_bytes: Optional[int] = None) -> "EventLog":
+        """A log saved with EventLog.save, loaded back onto this context's GPU (cco_event_log_load_begin / _append /
+        _finish): the log that was saved, without reading its export again.  src is a file path (read in blocks of
+        chunk_bytes, DEFAULT_CHUNK_BYTES by default, through one pinned buffer), a buffer (bytes, bytearray, memoryview or a
+        uint8 array: one append, or blocks of chunk_bytes when it is given) or an iterable of buffers, each appended as it
+        comes.  A damaged or inconsistent snapshot raises CcoError (CCO_E_INVALID_ARG) naming its section; nothing of it
+        stays on the device.  -> EventLog"""
+        h = C.c_void_p()
+        N.check(self._L.cco_event_log_load_begin(self._h, C.byref(h)))
+        try:
+            if isinstance(src, (str, os.PathLike)):
+                buf = self.host_array(int(chunk_bytes or DEFAULT_CHUNK_BYTES), np.uint8)
+                try:
+                    with open(os.fspath(src), "rb", buffering=0) as f:
+                        while n := f.readinto(memoryview(buf)):
+                            N.check(self._L.cco_event_log_load_append(h, buf.ctypes.data, n))
+                finally:
+                    self.host_free(buf)
+            else:
+                whole = isinstance(src, (bytes, bytearray, memoryview, np.ndarray))
+                for b in ([src] if whole else src):
+                    a = np.frombuffer(b, dtype=np.uint8) if not isinstance(b, np.ndarray) else np.ascontiguousarray(b).view(np.uint8).reshape(-1)
+                    step = int(chunk_bytes or max(len(a), 1)) if whole else max(len(a), 1)
+                    for k in range(0, len(a), step):
+                        N.check(self._L.cco_event_log_load_append(h, a[k:k + step].ctypes.data, len(a[k:k + step])))
+            N.check(self._L.cco_event_log_load_finish(h))
+        except BaseException:
+            self._L.cco_event_log_free(h)
+            raise
+        return self._adopt_log(h)
+
     def _append_finish(self, h, src, chunk: int, line_base: int = 0):
         """append every byte of a read_events source to an open log (holding line_base lines), then finish it"""
         paths = None
@@ -1389,6 +1420,30 @@ class EventLog:
         b = C.c_int64()
         N.check(self._ctx._L.cco_event_log_resident_bytes(self._h, C.byref(b)))
         return b.value
+
+    def save_size(self) -> int:
+        """cco_event_log_save_size: the length of the log's snapshot"""
+        b = C.c_int64()
+        N.check(self._ctx._L.cco_event_log_save_size(self._h, C.byref(b)))
+        return b.value
+
+    def save(self, dst, chunk_bytes: Optional[int] = None) -> int:
+        """the log's snapshot (cco_event_log_save; the layout is in include/cco_b200.h) written to dst, a file path or a
+        binary file object, in blocks of chunk_bytes (DEFAULT_CHUNK_BYTES by default); CcoContext.load_events reads it
+        back.  The log must be finished.  -> the snapshot's length in bytes"""
+        total = self.save_size()
+        step = max(1, min(int(chunk_bytes or DEFAULT_CHUNK_BYTES), total))
+        buf = np.empty(step, np.uint8)
+        f = open(os.fspath(dst), "wb") if isinstance(dst, (str, os.PathLike)) else dst
+        try:
+            for off in range(0, total, step):
+                n = min(step, total - off)
+                N.check(self._ctx._L.cco_event_log_save(self._h, off, buf.ctypes.data, n))
+                f.write(memoryview(buf)[:n])
+        finally:
+            if f is not dst:
+                f.close()
+        return total
 
     def free(self):
         if getattr(self, "_h", None):
