@@ -685,6 +685,54 @@ int cco_event_log_save(cco_event_log_t *log, int64_t offset, void *dst, int64_t 
 int cco_event_log_load_begin(cco_ctx_t *ctx, cco_event_log_t **out);
 int cco_event_log_load_append(cco_event_log_t *log, const void *bytes, int64_t len);
 int cco_event_log_load_finish(cco_event_log_t *log);
+
+/*
+ * Clean write-back: an extendable log's cleaned events written out as a compacted export, the part of PredictionIO's
+ * SelfCleaningDataSource.cleanPersistedPEvents that writes the cleaned set back [RECALL, unverifiable here], so that the
+ * export a trainer reads stops growing.  The log keeps one record per retained line (CCO_LOG_EXTENDABLE); the cleaner
+ * reads the source bytes a second time and copies out exactly those lines, verbatim, each ending in '\n' (a last line or
+ * a part without one gets one).  No resident state is added to the log, and the log is unchanged by a clean: its info,
+ * window_stats, resident bytes, snapshot image and every consumer's output are the same before and after.
+ *  - cco_event_log_clean_begin: a cleaner of a finished extendable log (read, extended or loaded).  It marks the log's
+ *    retained lines in a bitmap of one bit per line read, and stages chunks as the log's read did.
+ *  - cco_event_log_clean_append: the bytes the log has read, in order -- the first read's source, then each extend's --
+ *    split anywhere.  *out / *out_len: the kept lines completed in this append, in pinned memory owned by the cleaner and
+ *    valid until its next call.
+ *  - cco_event_log_clean_finish: the rest; *stats as below.
+ * The contract (events.clean_export is its host statement): reading the output under any later window w' (a cutoff at or
+ * after the log's, the same removeDuplicates) gives the training events, the ranking events per name and the aggregated
+ * properties that reading the whole source under w' gives, and without compression n_ignored and the order of
+ * property-only items as well.
+ * CCO_CLEAN_COMPRESS_PROPERTIES (compressProperties) folds, at begin, the $set / $unset lines of each item (entityType
+ * "item") whose lines the log retained: an item with a retained $delete, with a $set / $unset that carries a target, or
+ * with a single such line keeps its lines verbatim in place; every other item's lines become one line, written at finish
+ * after all verbatim lines in the order of each item's first line: a $set of its aggregated state (or, for an item that
+ * only unsets, an $unset of the union of the names, each with its last value), eventTime the last folded event's text,
+ * strings through json4s' quote, values their trimmed text, no eventId.  Other entity types' lines are never folded: the
+ * log keeps only the items' property lines, and no read looks at the others.  The folded lines are the log's own, so the
+ * source's property members are not compared with them beyond the record check below.
+ * The source is checked against the log as it is read: every line is parsed and checked as a read checks it, and each
+ * kept line's eventTime, event name and selection must equal its record, and under remove_duplicates its 128-bit
+ * identity too (without remove_duplicates the check does not cover ids, properties or other members).  A mismatch, a
+ * line past the log's count, an event name the log did not read and a source that ends short at finish fail the cleaner
+ * with CCO_E_INVALID_ARG naming the global 0-based line.
+ * Errors: CCO_E_INVALID_ARG for a null argument, a log read without CCO_LOG_EXTENDABLE, not finished or failed, and
+ * unknown flags; CCO_E_UNSUPPORTED for group contexts, as for every log.  While a cleaner of a log is open,
+ * cco_event_log_extend and cco_event_log_free of the log refuse with CCO_E_INVALID_ARG: a caller frees every cleaner
+ * before its log (the log would otherwise stay allocated), and every log before cco_destroy of its context.  A failed cleaner answers every
+ * later call but free with its message.
+ */
+typedef struct cco_event_clean cco_event_clean_t;
+enum { CCO_CLEAN_COMPRESS_PROPERTIES = 1 };
+typedef struct {
+  int64_t n_lines, n_written, n_expired, n_duplicates;   /* lines read; lines out; the log's window_stats */
+  int64_t n_folded, n_compressed, n_bytes;               /* property lines folded; lines they became; bytes out (all three
+                                                            in the output: n_written counts the lines they became) */
+} cco_event_clean_stats_t;
+int cco_event_log_clean_begin(cco_event_log_t *log, uint32_t flags, cco_event_clean_t **out);
+int cco_event_log_clean_append(cco_event_clean_t *x, const char *bytes, int64_t len, const char **out, int64_t *out_len);
+int cco_event_log_clean_finish(cco_event_clean_t *x, const char **out, int64_t *out_len, cco_event_clean_stats_t *stats);
+int cco_event_log_clean_free(cco_event_clean_t *x);
 /*
  * The query of user u, for the query event names n_0 .. n_{k-1}:
  *  - history of n_q: u's training events of n_q, latest first (eventTime desc, ties to the later line), the first limits[q]

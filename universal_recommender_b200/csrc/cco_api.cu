@@ -38,6 +38,7 @@
 #include "cco_refresh.cuh"
 #include "cco_intern.cuh"
 #include "cco_snapshot.cuh"
+#include "cco_clean.cuh"
 
 namespace cco {
 
@@ -3815,6 +3816,7 @@ struct cco_event_log {
   std::unique_ptr<cco::SnapImage, cco::SnapFree> snap;
   std::unique_ptr<cco::SnapLoad, cco::SnapFree> load;
   bool finished = false;
+  int cleaners = 0;                            // open cco_event_log_clean_begin cleaners: extend and free refuse meanwhile
   int fail = CCO_OK;                           // a failed append / finish: every later call returns it with fail_msg
   std::string fail_msg;
   int code_of(const char *name) const {
@@ -4244,11 +4246,13 @@ static int win_entry_lines(cco_event_log *lg, Arena &ar, long long n, const uint
 // decoded event, entityType, entityId, targetEntityType, targetEntityId and prId (null = absent), the tags text (absent,
 // null = []) and the set of the properties' top-level members (decoded name, trimmed value text; the last of a repeated
 // name; absent = {}).  A properties object the tokenizer cannot split (the line is read all the same) is its text.
+// win_idents: the records of the R chunk lines ridx (bytes bb) -> out[0 .. R); win_records also in the event log's cleaner
+static int win_idents(cco_ctx *c, Arena &ar, const EvLines &ev, const unsigned char *bb, const int32_t *code, long long base, long long R,
+                      const uint32_t *ridx, WinRec *out);
 static int win_records(cco_event_log *lg, Arena &ar, const EvLines &ev, const int32_t *code, long long base) {
   cco_ctx *c = lg->ctx;
   cudaStream_t s = c->stream;
   const long long L = ev.L;
-  const unsigned char *bb = lg->stage;
   uint32_t *keep, *pos, *ridx;
   CKR(ar.alloc(&keep, L + 1));
   k_win_keep_lines<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, ev.flag, keep);
@@ -4261,6 +4265,17 @@ static int win_records(cco_event_log *lg, Arena &ar, const EvLines &ev, const in
   ar.release(pos);
   const long long R = R32;
   if (R == 0) return CCO_OK;
+  if (lg->n_rec + R > lg->rec_cap) {   // grow geometrically
+    lg->rec_cap = std::max(2 * lg->rec_cap, lg->n_rec + R);
+    CKR(log_grow(lg, ar, &lg->rec, lg->rec_cap, lg->n_rec, 0));
+  }
+  CKR(win_idents(c, ar, ev, lg->stage, code, base, R, ridx, lg->rec + lg->n_rec));
+  lg->n_rec += R;
+  return CCO_OK;
+}
+static int win_idents(cco_ctx *c, Arena &ar, const EvLines &ev, const unsigned char *bb, const int32_t *code, long long base, long long R,
+                      const uint32_t *ridx, WinRec *out) {
+  cudaStream_t s = c->stream;
   // the properties' members: count pass with each span's verdict, then the members of the well-formed spans
   long long *pb, *pe, *mcnt, *moff;
   int *codes;
@@ -4327,14 +4342,9 @@ static int win_records(cco_event_log *lg, Arena &ar, const EvLines &ev, const in
     k_win_props<<<grid_for(M, 256, c->sm_count), 256, 0, s>>>(M, v, mline, hd + kWinStr * R, hr + 2 * R, acc);
     c->launches++;
   }
-  if (lg->n_rec + R > lg->rec_cap) {   // grow geometrically
-    lg->rec_cap = std::max(2 * lg->rec_cap, lg->n_rec + R);
-    CKR(log_grow(lg, ar, &lg->rec, lg->rec_cap, lg->n_rec, 0));
-  }
   k_win_ident<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, ridx, base, ev.sb, ev.span, ev.xspan, bb, hd, hr, codes, acc, ev.tm, ev.flag,
-                                                          code, lg->rec + lg->n_rec);
+                                                          code, out);
   c->launches++;
-  lg->n_rec += R;
   return CCO_OK;
 }
 // extendable logs without removeDuplicates, per chunk: what expiry needs of every retained line (a WinRec without a hash)
@@ -4508,6 +4518,46 @@ static int intern_refit(cco_event_log *lg) {
   return CCO_OK;
 }
 
+// the event names of a chunk's lines: decoded and grouped exactly -> *code (each line's group, numbered by first
+// appearance in the chunk) and the groups' names on the host
+static int chunk_names(cco_ctx *c, Arena &ar, const EvLines &ev, const unsigned char *bb, int32_t **code, std::vector<std::string> *out) {
+  cudaStream_t s = c->stream;
+  const long long L = ev.L;
+  JMember *jm;
+  CKR(ar.alloc(&jm, L));
+  k_event_strings<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, nullptr, kEvName, ev.sb, ev.span, bb, jm);
+  c->launches++;
+  DevStrCol names;
+  long long name_bytes = 0;
+  CKR(json_decode(c, ar, L, jm, bb, &names, &name_bytes));
+  ar.release(jm);
+  str_hash(c, names, ~0ULL);
+  CKR(ar.alloc(code, L));
+  StrTable nt;
+  CKR(str_group(c, ar, names, nullptr, false, 0, &nt, *code));
+  const long long NC = nt.n_groups;
+  cco_dictionary_t nd;
+  CKR(str_dictionary(c, ar, names, nt, &nd));
+  CK(cudaStreamSynchronize(s));
+  out->clear();
+  for (long long k = 0; k < NC; ++k) out->emplace_back(nd.bytes + nd.offsets[k], (size_t)(nd.offsets[k + 1] - nd.offsets[k]));
+  c->pinned_put((void *)nd.offsets);
+  c->pinned_put((void *)nd.bytes);
+  str_table_release(ar, nt);
+  str_release(ar, names);
+  return CCO_OK;
+}
+// code[l] = remap[code[l]] for the L lines of a chunk
+static int chunk_remap(cco_ctx *c, Arena &ar, long long L, const std::vector<int32_t> &remap, int32_t *code) {
+  cudaStream_t s = c->stream;
+  int32_t *d_remap;
+  CKR(ar.alloc(&d_remap, (long long)remap.size()));
+  CK(cudaMemcpyAsync(d_remap, remap.data(), sizeof(int32_t) * remap.size(), cudaMemcpyHostToDevice, s));
+  k_remap_i32<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, d_remap, code);
+  c->launches++;
+  return CCO_OK;
+}
+
 // one chunk of a streamed read, the first len staged bytes: every line parsed, the names numbered globally, the counts
 // added, the training and ranking events decoded into one new segment, the property-event lines appended to lg->pb
 static int event_chunk(cco_event_log *lg, long long len, bool open_tail) {
@@ -4534,26 +4584,12 @@ static int event_chunk(cco_event_log *lg, long long len, bool open_tail) {
   }
   // 5. event names: decoded, grouped exactly, numbered by first appearance in the chunk; the few distinct ones go to the
   // host, where names new to the log take the next codes (chunks arrive in order: the order of the whole read)
-  JMember *jm;
-  CKR(ar.alloc(&jm, L));
-  k_event_strings<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, nullptr, kEvName, ev.sb, ev.span, bb, jm);
-  c->launches++;
-  DevStrCol names;
-  long long name_bytes = 0;
-  CKR(json_decode(c, ar, L, jm, bb, &names, &name_bytes));
-  ar.release(jm);
-  str_hash(c, names, ~0ULL);
   int32_t *code;
-  CKR(ar.alloc(&code, L));
-  StrTable nt;
-  CKR(str_group(c, ar, names, nullptr, false, 0, &nt, code));
-  const long long NC = nt.n_groups;
-  cco_dictionary_t nd;
-  CKR(str_dictionary(c, ar, names, nt, &nd));
-  CK(cudaStreamSynchronize(s));
-  std::vector<int32_t> remap((size_t)NC);
-  for (long long k = 0; k < NC; ++k) {
-    std::string nm(nd.bytes + nd.offsets[k], (size_t)(nd.offsets[k + 1] - nd.offsets[k]));
+  std::vector<std::string> cnames;
+  CKR(chunk_names(c, ar, ev, bb, &code, &cnames));
+  std::vector<int32_t> remap(cnames.size());
+  for (size_t k = 0; k < cnames.size(); ++k) {
+    const std::string &nm = cnames[k];
     auto it = lg->name_code.find(nm);
     if (it == lg->name_code.end()) {
       it = lg->name_code.emplace(nm, (int)lg->name_off.size() - 1).first;
@@ -4562,16 +4598,8 @@ static int event_chunk(cco_event_log *lg, long long len, bool open_tail) {
     }
     remap[k] = it->second;
   }
-  c->pinned_put((void *)nd.offsets);
-  c->pinned_put((void *)nd.bytes);
-  str_table_release(ar, nt);
-  str_release(ar, names);
   const long long NG = (long long)lg->name_off.size() - 1;
-  int32_t *d_remap;
-  CKR(ar.alloc(&d_remap, NC));
-  CK(cudaMemcpyAsync(d_remap, remap.data(), sizeof(int32_t) * (size_t)NC, cudaMemcpyHostToDevice, s));
-  k_remap_i32<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, d_remap, code);
-  c->launches++;
+  CKR(chunk_remap(c, ar, L, remap, code));
   // 6. counts per name
   unsigned long long *cnt;
   CKR(ar.alloc(&cnt, 2 * NG + 2));
@@ -5353,6 +5381,7 @@ int cco_event_log_extend(cco_event_log_t *lg, const cco_event_window_t *w) {
   if (!lg) return set_error(CCO_E_INVALID_ARG, "null argument");
   CKR(log_state(lg, true));
   if (!lg->extendable) return set_error(CCO_E_INVALID_ARG, "the log was read without CCO_LOG_EXTENDABLE (cco_event_log_begin_ex)");
+  if (lg->cleaners > 0) return set_error(CCO_E_INVALID_ARG, "a cleaner of the log is open (cco_event_log_clean_free)");
   lg->snap.reset();   // the image is of the log as it was finished
   if (w) {
     if (w->reserved != 0) return set_error(CCO_E_INVALID_ARG, "the window's reserved field must be 0");
@@ -7213,7 +7242,519 @@ int cco_query_file_free(cco_query_file_t *qf) {
 }
 
 int cco_event_log_free(cco_event_log_t *lg) {
+  if (lg && lg->cleaners > 0) return set_error(CCO_E_INVALID_ARG, "a cleaner of the log is open (cco_event_log_clean_free)");
   event_log_release(lg);
+  return CCO_OK;
+}
+
+// ---- cco_event_log_clean_*: the log's kept lines copied out of its source bytes (kernels in cco_clean.cuh) ------------------
+struct cco_event_clean {
+  cco_event_log *lg = nullptr;
+  uint32_t flags = 0;
+  // the staging, as the log's read stages (cap bytes + 24 of padding, `staged` of them, the last '\n' at last_nl)
+  unsigned char *stage = nullptr;
+  long long cap = 0, staged = 0, last_nl = -1;
+  uint32_t *keep_bits = nullptr;   // one bit per global line of the log: set for the line of every retained record
+  uint32_t *fold_bits = nullptr;   // compressProperties: the same, set for the lines folded into fold_out
+  std::string fold_out;            // compressProperties: the folded lines, rendered at begin, written at finish
+  long long n_read = 0;            // lines read so far
+  long long n_rec_done = 0;        // records matched so far (the kept lines read)
+  std::vector<int32_t> name_remap; // the log's code of each name, by its chunk-local number (rebuilt per chunk)
+  // pinned output of the current call (from the context's pool): out_len bytes of out_cap
+  unsigned char *out = nullptr;
+  long long out_len = 0, out_cap = 0;
+  cco_event_clean_stats_t stats{};
+  bool finished = false;
+  int fail = CCO_OK;
+  std::string fail_msg;
+  std::vector<void *> dev;
+};
+
+namespace cco {
+static void clean_release(cco_event_clean *x) {
+  cco_ctx *c = x->lg->ctx;
+  cudaSetDevice(c->device);
+  for (void *p : x->dev) cudaFreeAsync(p, c->stream);
+  cudaStreamSynchronize(c->stream);
+  if (x->out) c->pinned_put(x->out);
+  x->lg->cleaners--;
+  delete x;
+}
+// room for n more bytes in the pinned output, its first out_len bytes kept
+static int clean_out_room(cco_event_clean *x, long long n) {
+  if (x->out_len + n <= x->out_cap) return CCO_OK;
+  const long long cap = std::max(2 * x->out_cap, x->out_len + n);
+  cco_ctx *c = x->lg->ctx;
+  unsigned char *p = (unsigned char *)c->pinned_get((size_t)cap, false);   // the context's pool: reused by the next clean
+  if (!p) return set_error(CCO_E_OOM, "cudaHostAlloc(%lld bytes) for the cleaned lines failed", cap);
+  if (x->out_len > 0) memcpy(p, x->out, (size_t)x->out_len);
+  if (x->out) c->pinned_put(x->out);
+  x->out = p;
+  x->out_cap = cap;
+  return CCO_OK;
+}
+static int clean_mismatch(unsigned long long err) {
+  const long long line = (long long)(err >> 8);
+  const char *what = (err & 0xff) == kClTime ? "eventTime" : (err & 0xff) == kClName ? "event name"
+                     : (err & 0xff) == kClSelection ? "selection (entity and target types, ids, event kind)" : "identity";
+  return set_error(CCO_E_INVALID_ARG, "line %lld: its %s differs from the log's record of the line: the source is not what the log read",
+                   line, what);
+}
+// one chunk, the first len staged bytes: parsed and checked as the read parses them, the kept lines checked against their
+// records and appended to the pinned output
+static int clean_chunk(cco_event_clean *x, long long len, bool open_tail) {
+  cco_event_log *lg = x->lg;
+  cco_ctx *c = lg->ctx;
+  cudaStream_t s = c->stream;
+  mail_reset(c);
+  Arena ar(s);
+  CKR(event_pad(c, x->stage, len));
+  EvLines ev;
+  const long long base = x->n_read;
+  CKR(event_lines(c, ar, (const uint64_t *)x->stage, len, open_tail, base, &ev, lg->dedup));
+  const long long L = ev.L;
+  if (L == 0) return CCO_OK;
+  if (base + L > lg->n_lines)
+    return set_error(CCO_E_INVALID_ARG, "line %lld: past the %lld lines the log read", lg->n_lines, lg->n_lines);
+  const unsigned char *bb = x->stage;
+  int32_t *code;
+  std::vector<std::string> cnames;
+  CKR(chunk_names(c, ar, ev, bb, &code, &cnames));
+  x->name_remap.assign(cnames.size(), 0);
+  for (size_t k = 0; k < cnames.size(); ++k) {
+    auto it = lg->name_code.find(cnames[k]);
+    if (it == lg->name_code.end()) {   // the first line of the name: found on the device
+      unsigned long long *first;
+      CKR(ar.alloc(&first, 1));
+      CK(cudaMemsetAsync(first, 0xff, 8, s));
+      k_clean_first_code<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, code, (int32_t)k, first);
+      c->launches++;
+      unsigned long long h_first = 0;
+      CKR(mail_fetch(c, &h_first, first, 8));
+      CKR(mail_wait(c));
+      return set_error(CCO_E_INVALID_ARG, "line %lld: an event name the log did not read: the source is not what the log read",
+                       base + (long long)h_first);
+    }
+    x->name_remap[k] = it->second;
+  }
+  CKR(chunk_remap(c, ar, L, x->name_remap, code));
+  // the kept lines of the chunk and their records
+  uint32_t *keep, *pos, *kidx, K32 = 0;
+  CKR(ar.alloc(&keep, L + 1));
+  k_clean_keep<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, base, x->keep_bits, keep);
+  c->launches++;
+  CKR(select_flagged(c, ar, L, keep, &pos, &kidx));
+  CKR(mail_fetch(c, &K32, pos + L, 4));
+  CKR(mail_wait(c));
+  const long long K = K32;
+  x->n_read += L;
+  if (K == 0) return CCO_OK;
+  WinRec *ident = nullptr;
+  if (lg->dedup) {
+    CKR(ar.alloc(&ident, K));
+    CKR(win_idents(c, ar, ev, bb, code, base, K, kidx, ident));
+  }
+  unsigned long long *err, h_err = 0;
+  CKR(ar.alloc(&err, 1));
+  CK(cudaMemsetAsync(err, 0xff, 8, s));
+  k_clean_check<<<grid_for(K, 256, c->sm_count), 256, 0, s>>>(K, kidx, base, lg->rec + x->n_rec_done, ev.tm, ev.flag, code, ident, err);
+  c->launches++;
+  CKR(mail_fetch(c, &h_err, err, 8));
+  // the compaction: each kept line and its '\n'
+  long long *len8, *off, total = 0;
+  CKR(ar.alloc(&len8, K + 1));
+  CKR(ar.alloc(&off, K + 1));
+  CK(cudaMemsetAsync(len8 + K, 0, 8, s));
+  k_clean_len<<<grid_for(K, 256, c->sm_count), 256, 0, s>>>(K, kidx, base, ev.sb, ev.se, x->fold_bits, len8);
+  c->launches++;
+  CKR(exclusive_sum(c, ar, len8, off, K + 1));
+  CKR(mail_fetch(c, &total, off + K, 8));
+  CKR(mail_wait(c));
+  if (h_err != ~0ULL) return clean_mismatch(h_err);
+  x->n_rec_done += K;
+  if (total == 0) return CCO_OK;
+  unsigned char *d_out;
+  CKR(ar.alloc(&d_out, (total + 7) / 8 * 8));
+  k_clean_compact<<<grid_for(K * 32, 256, c->sm_count), 256, 0, s>>>(K, kidx, ev.sb, ev.se, (const uint64_t *)bb, off, d_out);
+  c->launches++;
+  CKR(clean_out_room(x, total));
+  CK(cudaMemcpyAsync(x->out + x->out_len, d_out, (size_t)total, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  x->out_len += total;
+  x->stats.n_bytes += total;
+  return CCO_OK;
+}
+// the staging is full: as event_flush, through clean_chunk
+static int clean_flush(cco_event_clean *x) {
+  cco_ctx *c = x->lg->ctx;
+  cudaStream_t s = c->stream;
+  Arena ar(s);
+  if (x->last_nl < 0) {
+    if (x->staged >= (1LL << 31)) return event_error(((unsigned long long)x->n_read << 8) | kJsonLongLine);
+    unsigned char *p;
+    CKR(ar.alloc(&p, 2 * x->cap + 24));
+    ar.take(p);
+    CK(cudaMemcpyAsync(p, x->stage, (size_t)x->staged, cudaMemcpyDeviceToDevice, s));
+    for (void *&d : x->dev)
+      if (d == x->stage) d = p;
+    cudaFreeAsync(x->stage, s);
+    x->stage = p;
+    x->cap *= 2;
+    return CCO_OK;
+  }
+  const long long P = x->last_nl + 1, carry = x->staged - P;
+  unsigned char *tmp = nullptr;
+  if (carry > 0) {
+    CKR(ar.alloc(&tmp, carry));
+    CK(cudaMemcpyAsync(tmp, x->stage + P, (size_t)carry, cudaMemcpyDeviceToDevice, s));
+  }
+  CKR(clean_chunk(x, P, false));
+  if (carry > 0) CK(cudaMemcpyAsync(x->stage, tmp, (size_t)carry, cudaMemcpyDeviceToDevice, s));
+  x->staged = carry;
+  x->last_nl = -1;
+  return CCO_OK;
+}
+// compressProperties over the log's retained item property lines (lg->pb, their global lines lg->prop_line): the $set /
+// $unset lines of each foldable entity marked in fold_bits and rendered as one line each into fold_out (kernels k_fold_*)
+static int clean_fold(cco_event_clean *x) {
+  cco_event_log *lg = x->lg;
+  cco_ctx *c = lg->ctx;
+  cudaStream_t s = c->stream;
+  mail_reset(c);
+  Arena ar(s);
+  CKR(event_pad(c, lg->pb, lg->pb_len));
+  EvLines ev;
+  CKR(event_lines(c, ar, (const uint64_t *)lg->pb, lg->pb_len, false, 0, &ev));   // judged when the log read them
+  const long long L = ev.L;
+  if (L == 0) return CCO_OK;
+  if (L != (long long)lg->prop_line.size()) return set_error(CCO_E_INVALID_ARG, "internal: %lld property lines, %zu line numbers", L, lg->prop_line.size());
+  const unsigned char *pb = lg->pb;
+  // 1. the entities: decoded entityIds grouped exactly (hash, then the strings compared), numbered by first line
+  JMember *jm;
+  CKR(ar.alloc(&jm, L));
+  k_event_strings<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, nullptr, kEvEntityId, ev.sb, ev.span, pb, jm);
+  c->launches++;
+  DevStrCol ids;
+  long long id_bytes = 0;
+  CKR(json_decode(c, ar, L, jm, pb, &ids, &id_bytes));
+  str_hash(c, ids, ~0ULL);
+  int32_t *gcode;
+  CKR(ar.alloc(&gcode, L));
+  StrTable gt;
+  CKR(str_group(c, ar, ids, nullptr, false, 0, &gt, gcode));
+  const long long G = gt.n_groups;
+  // 2. foldable groups (no pin, two or more $set / $unset lines), ranked in order of their first line; their lines
+  uint32_t *cnt, *pin, *gkeep, *gpos, *gidx, R32 = 0;
+  CKR(ar.alloc(&cnt, G));
+  CKR(ar.alloc(&pin, G));
+  CKR(ar.alloc(&gkeep, G + 1));
+  CK(cudaMemsetAsync(cnt, 0, sizeof(uint32_t) * (size_t)G, s));
+  CK(cudaMemsetAsync(pin, 0, sizeof(uint32_t) * (size_t)G, s));
+  k_fold_count<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, ev.flag, gcode, cnt, pin);
+  k_fold_groups<<<grid_for(G, 256, c->sm_count), 256, 0, s>>>(G, cnt, pin, gkeep);
+  c->launches += 2;
+  CKR(select_flagged(c, ar, G, gkeep, &gpos, &gidx));
+  long long *gline;
+  uint8_t *fl;
+  CKR(ar.alloc(&gline, L));
+  CKR(ar.alloc(&fl, L + 1));
+  CK(cudaMemcpyAsync(gline, lg->prop_line.data(), sizeof(long long) * (size_t)L, cudaMemcpyHostToDevice, s));
+  k_fold_lines<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, ev.flag, gcode, gkeep, gline, fl, x->fold_bits);
+  c->launches++;
+  CKR(mail_fetch(c, &R32, gpos + G, 4));
+  CKR(mail_wait(c));
+  const long long R = R32;
+  if (R == 0) return CCO_OK;
+  uint32_t *lkeep, *lpos, *idx, F32 = 0;
+  CKR(ar.alloc(&lkeep, L + 1));
+  k_win_flag_keep<<<grid_for(L, 256, c->sm_count), 256, 0, s>>>(L, fl, kFoldLine, lkeep);
+  c->launches++;
+  CKR(select_flagged(c, ar, L, lkeep, &lpos, &idx));
+  CKR(mail_fetch(c, &F32, lpos + L, 4));
+  CKR(mail_wait(c));
+  const long long F = F32;
+  // 3. the fold order: (group rank, eventTime, line) -- sorted by time, then stably by rank (idx is in line order)
+  unsigned long long *k1;
+  uint32_t *k2, *v, *gr;
+  CKR(ar.alloc(&k1, F));
+  CKR(ar.alloc(&k2, F));
+  CKR(ar.alloc(&v, F));
+  CKR(ar.alloc(&gr, F));
+  k_fold_keys<<<grid_for(F, 256, c->sm_count), 256, 0, s>>>(F, idx, ev.tm, gcode, gpos, k1, k2, v);
+  c->launches++;
+  CKR(sort_pairs(c, ar, F, &k1, &v, 64));
+  k_fold_key2<<<grid_for(F, 256, c->sm_count), 256, 0, s>>>(F, v, k2, gr);
+  c->launches++;
+  CKR(sort_pairs(c, ar, F, &gr, &v, bits_for(R)));
+  uint32_t *place, *first_set, *last;
+  const uint32_t *rank_of_line = k2;   // each folded line's group rank, in folded-line order
+  CKR(ar.alloc(&place, F));
+  CKR(ar.alloc(&first_set, R));
+  CKR(ar.alloc(&last, R));
+  CK(cudaMemsetAsync(first_set, 0xff, sizeof(uint32_t) * (size_t)R, s));
+  k_fold_first<<<grid_for(F, 256, c->sm_count), 256, 0, s>>>(F, v, gr, idx, fl, place, first_set, last);
+  c->launches++;
+  // 4. the members of the folded lines' properties (count pass with each object's verdict, then the members)
+  long long *ob, *oe, *mcnt, *moff;
+  int *codes;
+  unsigned long long *err;
+  CKR(ar.alloc(&ob, F));
+  CKR(ar.alloc(&oe, F));
+  CKR(ar.alloc(&mcnt, F + 1));
+  CKR(ar.alloc(&moff, F + 1));
+  CKR(ar.alloc(&codes, F));
+  CKR(ar.alloc(&err, 1));
+  CK(cudaMemsetAsync(mcnt + F, 0, 8, s));
+  k_win_prop_spans<<<grid_for(F, 256, c->sm_count), 256, 0, s>>>(F, idx, ev.sb, ev.span, ob, oe);
+  k_json_members<<<grid_for(F * 32, 256, c->sm_count), 256, 0, s>>>(F, ob, oe, pb, WinMemberSink<false>{mcnt, codes, nullptr, nullptr}, err);
+  c->launches += 2;
+  CKR(exclusive_sum(c, ar, mcnt, moff, F + 1));
+  long long M = 0;
+  CKR(mail_fetch(c, &M, moff + F, 8));
+  CKR(mail_wait(c));
+  JMember *mem;
+  CKR(ar.alloc(&mem, std::max<long long>(M, 1)));
+  uint32_t *members = nullptr, P32 = 0;
+  long long *gmoff;
+  CKR(ar.alloc(&gmoff, R + 1));
+  CK(cudaMemsetAsync(gmoff, 0, sizeof(long long) * (size_t)(R + 1), s));
+  DevStrCol names;
+  if (M > 0) {
+    k_json_members<<<grid_for(F * 32, 256, c->sm_count), 256, 0, s>>>(F, ob, oe, pb, WinMemberSink<true>{nullptr, codes, moff, mem}, err);
+    c->launches++;
+    // 5. the names, decoded and grouped exactly; members sorted by (rank, name, place, index)
+    JMember *nm;
+    CKR(ar.alloc(&nm, M));
+    k_win_strings<<<grid_for(M, 256, c->sm_count), 256, 0, s>>>(0, nullptr, nullptr, nullptr, nullptr, pb, M, mem, nm);
+    c->launches++;
+    long long name_bytes = 0;
+    CKR(json_decode(c, ar, M, nm, pb, &names, &name_bytes));
+    str_hash(c, names, ~0ULL);
+    int32_t *ncode;
+    CKR(ar.alloc(&ncode, M));
+    StrTable nt;
+    CKR(str_group(c, ar, names, nullptr, false, 0, &nt, ncode));
+    uint32_t *mline, *mv, *keep, *kpos, *kidx;
+    unsigned long long *mk1, *mk2, *mk2s, *ins;
+    CKR(ar.alloc(&mline, M));
+    CKR(ar.alloc(&mv, M));
+    CKR(ar.alloc(&mk1, M));
+    CKR(ar.alloc(&mk2, M));
+    CKR(ar.alloc(&mk2s, M));
+    k_win_member_line<<<grid_for(F, 256, c->sm_count), 256, 0, s>>>(F, moff, mline);
+    k_fold_mkeys<<<grid_for(M, 256, c->sm_count), 256, 0, s>>>(M, mline, moff, place, rank_of_line, ncode, mk1, mk2, mv);
+    c->launches += 2;
+    CKR(sort_pairs(c, ar, M, &mk1, &mv, 64));
+    k_fold_mkey2<<<grid_for(M, 256, c->sm_count), 256, 0, s>>>(M, mv, mk2, mk2s);
+    c->launches++;
+    CKR(sort_pairs(c, ar, M, &mk2s, &mv, 64));
+    // 6. per (group, name) run: in the line or not, where inserted, which value; then the members in insertion order
+    CKR(ar.alloc(&keep, M + 1));
+    CKR(ar.alloc(&ins, M));
+    uint32_t *vm;
+    CKR(ar.alloc(&vm, M));
+    k_fold_runs<<<grid_for(M, 256, c->sm_count), 256, 0, s>>>(M, mk2s, mv, mline, moff, place, idx, fl, first_set, keep, ins, vm);
+    c->launches++;
+    CKR(select_flagged(c, ar, M, keep, &kpos, &kidx));
+    CKR(mail_fetch(c, &P32, kpos + M, 4));
+    CKR(mail_wait(c));
+    const long long P = P32;
+    if (P > 0) {
+      // sorted by insertion, then stably by rank: each folded line's members in insertion order
+      unsigned long long *ok1;
+      uint32_t *or32, *om, *perm, *r2, *ocnt;
+      CKR(ar.alloc(&ok1, P));
+      CKR(ar.alloc(&or32, P));
+      CKR(ar.alloc(&om, P));
+      CKR(ar.alloc(&perm, P));
+      CKR(ar.alloc(&r2, P));
+      CKR(ar.alloc(&members, P));
+      CKR(ar.alloc(&ocnt, R + 1));
+      CK(cudaMemsetAsync(ocnt, 0, sizeof(uint32_t) * (size_t)(R + 1), s));
+      k_fold_okeys<<<grid_for(P, 256, c->sm_count), 256, 0, s>>>(P, kidx, mk2s, ins, vm, ok1, or32, om, perm, ocnt);
+      c->launches++;
+      CKR(sort_pairs(c, ar, P, &ok1, &perm, 64));
+      k_fold_gather2<<<grid_for(P, 256, c->sm_count), 256, 0, s>>>(P, perm, or32, om, r2, members);
+      c->launches++;
+      CKR(sort_pairs(c, ar, P, &r2, &members, bits_for(R)));
+      long long *c64;
+      CKR(ar.alloc(&c64, R + 1));
+      k_fold_count64<<<grid_for(R + 1, 256, c->sm_count), 256, 0, s>>>(R, ocnt, c64);
+      c->launches++;
+      CKR(exclusive_sum(c, ar, c64, gmoff, R + 1));
+    }
+  }
+  // 7. the entity id of each folded group (its first line's) and the two render passes
+  DevDict gid;
+  {
+    uint32_t *first_line;
+    long long *len, *goff;
+    CKR(ar.alloc(&first_line, R));
+    CKR(ar.alloc(&len, R + 1));
+    CKR(ar.alloc(&goff, R + 1));
+    k_fold_group_line<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, gidx, gt.first_sorted, first_line, ids.off, len);
+    c->launches++;
+    CK(cudaMemsetAsync(len + R, 0, 8, s));
+    CKR(exclusive_sum(c, ar, len, goff, R + 1));
+    long long total = 0;
+    CKR(mail_fetch(c, &total, goff + R, 8));
+    CKR(mail_wait(c));
+    unsigned char *gb;
+    CKR(ar.alloc(&gb, std::max<long long>(total, 1)));
+    k_str_dict_gather<<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, first_line, ids.off, 0, (const unsigned char *)ids.w, goff, gb);
+    c->launches++;
+    gid = DevDict{goff, gb, R};
+  }
+  long long *rlen, *roff, total = 0;
+  CKR(ar.alloc(&rlen, R + 1));
+  CKR(ar.alloc(&roff, R + 1));
+  CK(cudaMemsetAsync(rlen + R, 0, 8, s));
+  const long long *noff = M > 0 ? names.off : nullptr;
+  const unsigned char *nb = M > 0 ? (const unsigned char *)names.w : nullptr;
+  k_fold_render<false><<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, last, first_set, idx, ev.sb, ev.span, pb, gid.off, gid.bytes, gmoff, members,
+                                                                     noff, nb, mem, nullptr, rlen, nullptr);
+  c->launches++;
+  CKR(exclusive_sum(c, ar, rlen, roff, R + 1));
+  CKR(mail_fetch(c, &total, roff + R, 8));
+  CKR(mail_wait(c));
+  unsigned char *d_out;
+  CKR(ar.alloc(&d_out, std::max<long long>(total, 1)));
+  k_fold_render<true><<<grid_for(R, 256, c->sm_count), 256, 0, s>>>(R, last, first_set, idx, ev.sb, ev.span, pb, gid.off, gid.bytes, gmoff, members,
+                                                                    noff, nb, mem, roff, nullptr, d_out);
+  c->launches++;
+  x->fold_out.resize((size_t)total);
+  CK(cudaMemcpyAsync(&x->fold_out[0], d_out, (size_t)total, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  x->stats.n_folded = F;
+  x->stats.n_compressed = R;
+  return CCO_OK;
+}
+static int clean_begin(cco_event_log *lg, uint32_t flags, cco_event_clean **out) {
+  cco_ctx *c = lg->ctx;
+  cudaStream_t s = c->stream;
+  CK(cudaSetDevice(c->device));
+  NvtxRange nvtx("cco:event_clean");
+  std::unique_ptr<cco_event_clean> x(new cco_event_clean());
+  x->lg = lg;
+  x->flags = flags;
+  x->cap = lg->chunk0;
+  Arena ar(s);
+  const long long NB = (lg->n_lines + 31) / 32;
+  CKR(ar.alloc(&x->stage, x->cap + 24));
+  CKR(ar.alloc(&x->keep_bits, std::max<long long>(NB, 1)));
+  for (void *p : {(void *)x->stage, (void *)x->keep_bits}) {
+    ar.take(p);
+    x->dev.push_back(p);
+  }
+  CK(cudaMemsetAsync(x->keep_bits, 0, sizeof(uint32_t) * (size_t)std::max<long long>(NB, 1), s));
+  if (lg->n_rec > 0) {
+    k_clean_bitmap<<<grid_for(lg->n_rec, 256, c->sm_count), 256, 0, s>>>(lg->n_rec, lg->rec, x->keep_bits);
+    c->launches++;
+  }
+  CK(cudaStreamSynchronize(s));
+  if ((flags & CCO_CLEAN_COMPRESS_PROPERTIES) && lg->n_prop > 0) {
+    CKR(ar.alloc(&x->fold_bits, std::max<long long>(NB, 1)));
+    ar.take(x->fold_bits);
+    x->dev.push_back(x->fold_bits);
+    CK(cudaMemsetAsync(x->fold_bits, 0, sizeof(uint32_t) * (size_t)std::max<long long>(NB, 1), s));
+    CKR(clean_fold(x.get()));
+  }
+  x->stats.n_expired = lg->n_expired;
+  x->stats.n_duplicates = lg->n_dup;
+  lg->cleaners++;
+  *out = x.release();
+  return CCO_OK;
+}
+static int clean_append(cco_event_clean *x, const char *bytes, int64_t len) {
+  cco_ctx *c = x->lg->ctx;
+  CK(cudaSetDevice(c->device));
+  NvtxRange nvtx("cco:event_clean");
+  x->out_len = 0;
+  while (len > 0) {
+    if (x->staged == x->cap) CKR(clean_flush(x));
+    const long long take = std::min<long long>(len, x->cap - x->staged);
+    CK(cudaMemcpyAsync(x->stage + x->staged, bytes, (size_t)take, cudaMemcpyHostToDevice, c->stream));
+    const void *nl = memrchr(bytes, '\n', (size_t)take);
+    if (nl) x->last_nl = x->staged + ((const char *)nl - bytes);
+    x->staged += take;
+    bytes += take;
+    len -= take;
+  }
+  CK(cudaStreamSynchronize(c->stream));   // the bytes are copied: the caller may reuse its buffer
+  return CCO_OK;
+}
+static int clean_finish(cco_event_clean *x) {
+  cco_event_log *lg = x->lg;
+  CK(cudaSetDevice(lg->ctx->device));
+  NvtxRange nvtx("cco:event_clean");
+  x->out_len = 0;
+  if (x->staged > 0) CKR(clean_chunk(x, x->staged, x->last_nl != x->staged - 1));
+  x->staged = 0;
+  if (x->n_read != lg->n_lines)
+    return set_error(CCO_E_INVALID_ARG, "line %lld: the source ends after %lld lines, the log read %lld", x->n_read, x->n_read, lg->n_lines);
+  const long long F = (long long)x->fold_out.size();
+  if (F > 0) {
+    CKR(clean_out_room(x, F));
+    memcpy(x->out + x->out_len, x->fold_out.data(), (size_t)F);
+    x->out_len += F;
+    x->stats.n_bytes += F;
+  }
+  x->stats.n_lines = x->n_read;
+  x->stats.n_written = lg->n_rec - x->stats.n_folded + x->stats.n_compressed;
+  x->finished = true;
+  return CCO_OK;
+}
+static int clean_state(const cco_event_clean *x) {
+  if (x->fail != CCO_OK) return set_error(CCO_E_INVALID_ARG, "the cleaner failed: %s", x->fail_msg.c_str());
+  if (x->finished) return set_error(CCO_E_INVALID_ARG, "the cleaner is finished");
+  return CCO_OK;
+}
+static int clean_fail(cco_event_clean *x, int rc) {
+  if (rc != CCO_OK) {
+    x->fail = rc;
+    x->fail_msg = g_err;
+  }
+  return rc;
+}
+}  // namespace cco
+
+int cco_event_log_clean_begin(cco_event_log_t *lg, uint32_t flags, cco_event_clean_t **out) {
+  if (!lg || !out) return set_error(CCO_E_INVALID_ARG, "null argument");
+  *out = nullptr;
+  if (flags & ~(uint32_t)CCO_CLEAN_COMPRESS_PROPERTIES) return set_error(CCO_E_INVALID_ARG, "unknown flags 0x%x", (unsigned)flags);
+  if (!lg->ctx->members.empty()) return set_error(CCO_E_UNSUPPORTED, "an event log is resident on one GPU");
+  CKR(log_state(lg, true));
+  if (!lg->extendable) return set_error(CCO_E_INVALID_ARG, "the log was read without CCO_LOG_EXTENDABLE (cco_event_log_begin_ex)");
+  return clean_begin(lg, flags, out);
+}
+
+int cco_event_log_clean_append(cco_event_clean_t *x, const char *bytes, int64_t len, const char **out, int64_t *out_len) {
+  if (!x || len < 0 || (len > 0 && !bytes) || !out || !out_len) return set_error(CCO_E_INVALID_ARG, "null argument or negative length");
+  *out = nullptr;
+  *out_len = 0;
+  CKR(clean_state(x));
+  CKR(clean_fail(x, clean_append(x, bytes, len)));
+  *out = (const char *)x->out;
+  *out_len = x->out_len;
+  return CCO_OK;
+}
+
+int cco_event_log_clean_finish(cco_event_clean_t *x, const char **out, int64_t *out_len, cco_event_clean_stats_t *stats) {
+  if (!x || !out || !out_len || !stats) return set_error(CCO_E_INVALID_ARG, "null argument");
+  *out = nullptr;
+  *out_len = 0;
+  CKR(clean_state(x));
+  CKR(clean_fail(x, clean_finish(x)));
+  *out = (const char *)x->out;
+  *out_len = x->out_len;
+  *stats = x->stats;
+  return CCO_OK;
+}
+
+int cco_event_log_clean_free(cco_event_clean_t *x) {
+  if (x) clean_release(x);
   return CCO_OK;
 }
 

@@ -225,8 +225,9 @@ class DataSourceEvents:
 class EventWindow:
     """engine.json datasource.params.eventWindow, PredictionIO's EventWindow(duration, removeDuplicates,
     compressProperties).  duration: a scala.concurrent.duration string (ur_model.duration_ms), None: nothing expires.
-    compressProperties rewrites each entity's $set / $unset events as one; it is assumed to leave what aggregateProperties
-    returns unchanged, so it is accepted and changes nothing here."""
+    compressProperties applies to the cleaned events written back (clean_export, ur.clean_export): each item's $set /
+    $unset lines are folded into one where that leaves what aggregateProperties returns unchanged.  A read does not
+    rewrite events, so it changes nothing in read_export or CcoContext.read_events."""
     duration: Optional[str] = None
     removeDuplicates: bool = False
     compressProperties: bool = False
@@ -334,6 +335,78 @@ def extend_clean(kept: KeptEvents, new_events: Sequence[Event], window: Optional
 def clean_kept(events: Sequence[Event], window: Optional[EventWindow], now_ms: Optional[int]) -> KeptEvents:
     """clean_events as the state an extendable log keeps: the extend of nothing"""
     return extend_clean(KeptEvents(), events, window, now_ms)
+
+
+def _fold_line(group: Sequence[Event], lines: Sequence[bytes]) -> bytes:
+    """one $set / $unset line for a group of one entity's property lines (no $delete, no target): the fold in (eventTime,
+    line) order.  With a $set, aggregate_property_events' state (None at first, so an $unset before the first $set does
+    nothing) as a $set, members in dict insertion order; with only $unsets, one $unset of the union of the names, each with
+    its last value text.  eventTime: the last folded event's eventTime text."""
+    from .ur_query import json_string
+    order = sorted(group, key=lambda e: (e.time_ms, e.line))
+    if any(e.event == "$set" for e in order):
+        state = None
+        for e in order:
+            if e.event == "$set":
+                state = {**state, **e.properties} if state is not None else dict(e.properties)
+            elif state is not None:
+                state = {k: v for k, v in state.items() if k not in e.properties}
+        name, props = "$set", state
+    else:
+        props: dict = {}
+        for e in order:
+            props.update(e.properties)
+        name = "$unset"
+    last = order[-1]
+    time_text = raw_member(lines[last.line].decode("utf-8", "surrogatepass"), "eventTime")
+    members = ",".join(f"{json_string(k)}:{v.text}" for k, v in props.items())
+    text = (f'{{"event":{json_string(name)},"entityType":{json_string(last.entity_type)},"entityId":{json_string(last.entity_id)},'
+            f'"properties":{{{members}}},"eventTime":{time_text}}}')
+    return text.encode("utf-8", "surrogatepass") + b"\n"
+
+
+def clean_export(data, window: Optional[EventWindow], now_ms: Optional[int], compress_properties: bool = False) -> bytes:
+    """PredictionIO's cleanPersistedPEvents as a compacted export [RECALL, unverifiable here]: the lines clean_events keeps,
+    in line order, each copied byte for byte and ending in '\\n' (as join_parts ends a part).  data: as read_export takes it.
+
+    compress_properties: the kept $set / $unset lines of items (entityType "item", the property events a read aggregates)
+    are grouped by decoded entityId.  Other entity types' lines stay verbatim: a resident log keeps the item property
+    lines only, so those are what the device can group before the source streams past, and no read looks at the others.
+    These stay verbatim in place: the property lines of an entity with a kept $delete line, of an entity with a kept
+    $set / $unset that carries a target entity (that line is also a ranking event, and a fold around it would move it in
+    the (eventTime, line) order), and the line of an entity with only one.  Every other group becomes one line (_fold_line),
+    written after all verbatim lines in the order of each group's first line.
+
+    The contract: for any later window w' (cutoff at or after this one's, the same removeDuplicates) and now',
+    read_export(clean_export(X, w, now, p), w', now') gives the training events and the ranking events per name (names left
+    without events aside) that read_export(X, w', now') gives, and the same aggregated properties as {item: {field: text}};
+    without compress_properties also n_ignored and the order of the property-only items.  It holds because a line dropped
+    under w is dropped under w' (extend_clean), $set / $unset never expire, and an entity whose $delete could expire
+    later is never folded.
+
+    Deviations from PredictionIO (whose compressPProperties is recalled, not read): PIO folds every entity type; PIO folds across $delete, which changes
+    what aggregateProperties returns; PIO's fold keeps the first event's name and eventId, this one writes a new $set or
+    $unset without eventId, creationTime, prId or tags; members are in insertion order, not Scala Map order; the folded
+    lines come last, as an export has no order the store keeps."""
+    if isinstance(data, (str, os.PathLike)):
+        data = join_parts(export_parts(data))
+    if window is not None and window.duration is not None and now_ms is None:
+        raise ValueError("an eventWindow with a duration needs now_ms")
+    lines = export_lines(bytes(data))
+    kept, _, _ = clean_events([parse_line(i, raw) for i, raw in enumerate(lines)], window, now_ms)
+    folded: dict = {}
+    if compress_properties:
+        ent = lambda e: (e.entity_type, e.entity_id)
+        props = [e for e in kept if is_property_event(e)]
+        pinned = {ent(e) for e in props if e.event == "$delete" or e.target_id is not None}
+        for e in props:
+            if e.event in ("$set", "$unset") and ent(e) not in pinned:
+                folded.setdefault(ent(e), []).append(e)
+        folded = {k: g for k, g in folded.items() if len(g) > 1}
+    gone = {e.line for g in folded.values() for e in g}
+    out = [lines[e.line] + b"\n" for e in kept if e.line not in gone]
+    out += [_fold_line(g, lines) for g in folded.values()]
+    return b"".join(out)
 
 
 def export_parts(directory) -> list[str]:

@@ -437,8 +437,11 @@ class CcoContext:
             raise
         return self._adopt_log(h)
 
-    def _append_finish(self, h, src, chunk: int, line_base: int = 0):
-        """append every byte of a read_events source to an open log (holding line_base lines), then finish it"""
+    def _append_finish(self, h, src, chunk: int, line_base: int = 0, append=None, finish=None):
+        """append every byte of a read_events source to an open log (holding line_base lines), then finish it; append(ptr,
+        n) / finish() stand in for cco_event_log_append / _finish of h (EventLog.write_clean passes its cleaner's)"""
+        append = append or (lambda ptr, n: N.check(self._L.cco_event_log_append(h, ptr, n)))
+        finish = finish or (lambda: N.check(self._L.cco_event_log_finish(h)))
         paths = None
         if isinstance(src, (str, os.PathLike)):
             p = os.fspath(src)
@@ -446,14 +449,14 @@ class CcoContext:
         elif isinstance(src, (list, tuple)) and all(isinstance(x, (str, os.PathLike)) for x in src):
             paths = [os.fspath(x) for x in src]
         if paths is not None:
-            self._append_files(h, paths, chunk, line_base)
+            self._append_files(paths, chunk, line_base, append)
         else:
             for b in ([src] if isinstance(src, (bytes, bytearray, memoryview, np.ndarray)) else src):
                 buf = np.frombuffer(b, dtype=np.uint8) if not isinstance(b, np.ndarray) else np.ascontiguousarray(b, dtype=np.uint8)
                 if len(buf):
-                    N.check(self._L.cco_event_log_append(h, buf.ctypes.data, len(buf)))
+                    append(buf.ctypes.data, len(buf))
         try:
-            N.check(self._L.cco_event_log_finish(h))
+            finish()
         except N.CcoError as e:
             if paths is not None:
                 _name_part(e, paths, line_base)
@@ -464,7 +467,7 @@ class CcoContext:
         self._logs.add(log)
         return log
 
-    def _append_files(self, h, paths, chunk: int, line_base: int = 0):
+    def _append_files(self, paths, chunk: int, line_base: int, append):
         """append the files in order through two pinned buffers: a reader thread fills one while the other is appended
         (readinto and the ctypes call both release the GIL)"""
         bufs = [self.host_array(chunk, np.uint8) for _ in range(2)]
@@ -505,9 +508,9 @@ class CcoContext:
                 k, n = item
                 try:
                     if k < 0:
-                        N.check(self._L.cco_event_log_append(h, b"\n", 1))
+                        append(b"\n", 1)
                     else:
-                        N.check(self._L.cco_event_log_append(h, bufs[k].ctypes.data, n))
+                        append(bufs[k].ctypes.data, n)
                 except N.CcoError as e:
                     _name_part(e, paths, line_base)
                     raise
@@ -1366,6 +1369,18 @@ class EventLogInfo:
     n_ignored: int
 
 
+@dataclass
+class CleanStats:
+    """cco_event_clean_stats_t: what EventLog.write_clean read and wrote"""
+    n_lines: int         # lines read
+    n_written: int       # lines written
+    n_expired: int       # the log's window_stats
+    n_duplicates: int
+    n_folded: int        # property lines folded (compress_properties)
+    n_compressed: int    # the lines they became
+    n_bytes: int         # bytes written
+
+
 class EventLog:
     """A PredictionIO event export resident on one GPU (cco_event_log_t), from CcoContext.read_events."""
 
@@ -1444,6 +1459,63 @@ class EventLog:
             if f is not dst:
                 f.close()
         return total
+
+    def write_clean(self, src, out, compress_properties: bool = False, chunk_bytes: Optional[int] = None) -> "CleanStats":
+        """The log's cleaned events written back as a compacted export (cco_event_log_clean_*): the lines the log keeps,
+        copied verbatim out of src on the device, each ending in '\\n' -- events.clean_export's output for the log's
+        window.  The log must have been read with extendable=True (then extended or loaded, or not) and is unchanged.
+        src: what the log has read, in order (the first read's source, then each extend's), as any source read_events takes;
+        a file source's part that does not end in '\\n' is followed by one.  Each kept line is checked against the log's
+        record of it (eventTime, event name, selection, and under removeDuplicates its identity): a source that is not what
+        the log read raises CcoError naming the line, and the part and its line for a multi-part source.
+        out: a path, written under a temporary name beside it and renamed over it only when the whole export is written
+        (so a failure leaves no partial export), or a binary file object.  compress_properties: events.clean_export's fold of
+        each item's $set / $unset lines (compressProperties), computed on the device from the log's property lines.  chunk_bytes: the host
+        blocks of file sources (DEFAULT_CHUNK_BYTES); the device staging is the log's.  -> CleanStats"""
+        L = self._ctx._L
+        x = C.c_void_p()
+        N.check(L.cco_event_log_clean_begin(self._h, N.CLEAN_COMPRESS_PROPERTIES if compress_properties else 0, C.byref(x)))
+        path = os.fspath(out) if isinstance(out, (str, os.PathLike)) else None
+        tmp, f = None, out
+        o, n, st = C.c_void_p(), C.c_int64(), N.EventCleanStatsT()
+
+        def emit():
+            if n.value:
+                f.write(memoryview((C.c_char * n.value).from_address(o.value)))
+
+        step = max(1, int(chunk_bytes or DEFAULT_CHUNK_BYTES))
+
+        def append(ptr, k):   # a large buffer in steps, so that each call's output stays near one chunk
+            for at in range(0, k, step):
+                m = min(step, k - at)
+                N.check(L.cco_event_log_clean_append(x, ptr + at if at else ptr, m, C.byref(o), C.byref(n)))
+                emit()
+
+        def finish():
+            N.check(L.cco_event_log_clean_finish(x, C.byref(o), C.byref(n), C.byref(st)))
+            emit()
+
+        try:
+            if path is not None:
+                d, b = os.path.split(os.path.abspath(path))
+                tmp = os.path.join(d, f".{b}.{os.getpid()}.tmp")
+                f = open(tmp, "wb")
+            self._ctx._append_finish(None, src, int(chunk_bytes or DEFAULT_CHUNK_BYTES), 0, append, finish)
+            if path is not None:
+                f.flush()
+                os.fsync(f.fileno())
+                f.close()
+                os.replace(tmp, path)
+                tmp = None
+        finally:
+            L.cco_event_log_clean_free(x)
+            if tmp is not None:
+                f.close()
+                try:
+                    os.remove(tmp)
+                except OSError:
+                    pass
+        return CleanStats(st.n_lines, st.n_written, st.n_expired, st.n_duplicates, st.n_folded, st.n_compressed, st.n_bytes)
 
     def free(self):
         if getattr(self, "_h", None):

@@ -320,6 +320,20 @@ def _refresh_names(ap: URAlgorithmParams) -> tuple:
     return ap.model_event_names(), [r[0] for r in _log_rankings(ap, 0)]
 
 
+def clean_export(src, out, window, now_ms: Optional[int] = None, chunk_bytes: Optional[int] = None, ctx: CcoContext | None = None):
+    """PredictionIO's cleanPersistedPEvents in one call [RECALL, unverifiable here]: the export src read on the device with
+    the eventWindow `window` (events.EventWindow; its cutoff counted back from now_ms, the wall clock by default) as an
+    extendable log, its cleaned events written to out (EventLog.write_clean, compressProperties from the window), and the
+    log freed.  src is read twice, so it must be a path, a part directory, a list of paths or a buffer, not a generator.
+    The caller imports out into the event store (`pio import`).  -> CleanStats"""
+    ctx = ctx or default_context()
+    log = ctx.read_events(src, chunk_bytes, window, _now(now_ms), extendable=True)
+    try:
+        return log.write_clean(src, out, window is not None and window.compressProperties, chunk_bytes)
+    finally:
+        log.free()
+
+
 def refresh_properties_from_events(body: bytes, export, ap: URAlgorithmParams, now_ms: Optional[int] = None, event_window=None,
                                    ctx: CcoContext | None = None) -> RefreshedIndex:
     """The item properties of the live index refreshed without a retrain (CcoContext.refresh_properties): the properties
