@@ -655,7 +655,9 @@ int cco_event_log_intern_stats(const cco_event_log_t *log, int64_t *n_user_keys,
  *    x *= 0x94d049bb133111eb; x ^= x >> 31).
  *  - host sections (lists of strings: i64 n, i64 offsets [n + 1] from 0, the bytes):
  *      1 state: 16 i64: flags (CCO_LOG_*), remove_duplicates, cutoff_ms, chunk_bytes, n_lines, property events, ignored
- *        lines, property items, property fields, expired lines, duplicate lines, the intern hash mask, 4 zeros;
+ *        lines, property items, property fields, expired lines, duplicate lines, the intern hash mask, erased lines
+ *        (cco_event_log_erased, >= 0; a reserved zero before erasure existed, so a library older than it refuses an image
+ *        with erased lines: "a counter is out of range"), 3 zeros;
  *      2 names: the event names (a string list); 3 counts: training then ranking events per name (i64 each);
  *      4 fields: the aggregated properties' field names (a string list);
  *      5 property_lines: the global line of each retained property-event line (i64; CCO_LOG_EXTENDABLE).
@@ -733,6 +735,51 @@ int cco_event_log_clean_begin(cco_event_log_t *log, uint32_t flags, cco_event_cl
 int cco_event_log_clean_append(cco_event_clean_t *x, const char *bytes, int64_t len, const char **out, int64_t *out_len);
 int cco_event_log_clean_finish(cco_event_clean_t *x, const char **out, int64_t *out_len, cco_event_clean_stats_t *stats);
 int cco_event_log_clean_free(cco_event_clean_t *x);
+/*
+ * Erasure: the lines of given users and items taken out of a finished extendable log (read, extended or loaded), for bot
+ * and test users, deletion requests and withdrawn products, without a re-read.  events.erased_line is the host statement
+ * of which lines go.  A line is erased, whole (its training entry, ranking entry, property line, record and history
+ * time), when
+ *  1. it is a training event (entityType "user", targetEntityType "item") whose entityId is one of the users;
+ *  2. its targetEntityId is one of the items, whatever its types (PopModel reads ranking events by id);
+ *  3. it is a property event ($set / $unset / $delete of entityType "item") whose entityId is one of the items.
+ * Ids compare decoded, as the log compares them; ids are bytes in the Arrow layout (id i = bytes[offsets[i] - offsets[0],
+ * offsets[i + 1] - offsets[0])).  The rule is made of whole removeDuplicates groups (their identity holds entityId and
+ * targetEntityId), and from that:
+ *  - consumers: erasing set E from a log read from X under window w gives every consumer's output a fresh read of X - E
+ *    (the export without E's lines) gives under w: ingest, format_model_log, rerank_model_log, user, mixed and query-file
+ *    queries, refresh_properties_log and intern_stats.  An extend after the erase gives what a fresh read of (X - E) + B
+ *    gives.  Erasure is not a block list: later extends read new lines of erased ids as any others;
+ *  - counters: info's n_lines and window_stats are unchanged by an erase; info's training, ranking and property counts
+ *    follow the retained lines; cco_event_log_erased counts the erased lines over the log's life, so that lines read =
+ *    retained + expired + duplicates + erased holds for every log and across extends;
+ *  - write-back: cco_event_log_clean_* of X after the erase writes events.clean_export(X - E, w, now, compress), byte for
+ *    byte, with and without CCO_CLEAN_COMPRESS_PROPERTIES;
+ *  - resident bytes: those of the fresh read, plus 8 for each duplicate eventTime the log keeps of a dropped duplicate of
+ *    an erased line (the log holds no id for those lines; they still turn into expired lines under a later cutoff).
+ * Limits: the log holds no entityId for a user's lines without an item target (a user $set, an event on a "user" or
+ * "category" target) nor for lines that name an item only as entityId and are not property events, so these are not
+ * erased and a write-back keeps them; a caller who must remove them filters the export.
+ * On the device: the ids become two intern tables (users, items; cco_intern.cuh's table, exact byte compares); the
+ * training entries are probed by string, or on an interned log by their keys (the ids looked up in the log's tables,
+ * then 8 bytes per entry); the ranking entries and the retained property lines' entityIds are probed against the items.
+ * The marked lines leave through the extend's finish: records, columns, property lines, aggregation and intern refit.
+ * Ids the log does not hold, repeated ids and empty lists are fine; an erase that marks nothing leaves the log bit for
+ * bit as it was, its snapshot image included.  Otherwise the saved image is rebuilt at the next save.
+ * *stats (nullable): the lines erased, and the training, ranking and property events among them.
+ * Errors: CCO_E_INVALID_ARG for a null log, null offsets with a positive count, null bytes with offsets that span bytes,
+ * a negative count ("users: a negative count"), offsets[0] < 0 ("items: offsets[0] = -1 is negative"), decreasing
+ * offsets ("users: offsets[3] = 2 decreases"), a log read without CCO_LOG_EXTENDABLE, a log not finished or failed, and a
+ * log with an open cleaner (as cco_event_log_extend); CCO_E_UNSUPPORTED for group contexts, as for every log.  A failed
+ * erase fails the log as a failed extend does.  cco_event_log_erased: CCO_E_INVALID_ARG for a null argument and a log
+ * not finished or failed (0 for a log that never erased).
+ */
+typedef struct {
+  int64_t n_lines, n_training, n_ranking, n_property_events;
+} cco_event_erase_stats_t;
+int cco_event_log_erase(cco_event_log_t *log, int64_t n_users, const int64_t *user_offsets, const char *user_bytes, int64_t n_items,
+                        const int64_t *item_offsets, const char *item_bytes, cco_event_erase_stats_t *stats /* nullable */);
+int cco_event_log_erased(const cco_event_log_t *log, int64_t *n_erased);
 /*
  * The query of user u, for the query event names n_0 .. n_{k-1}:
  *  - history of n_q: u's training events of n_q, latest first (eventTime desc, ties to the later line), the first limits[q]

@@ -39,7 +39,7 @@ from ._native import (CcoError, CcoInvalidArgument, FLAG_ASSUME_CANONICAL, FLAG_
 from .events import DataSourceParams, EventWindow
 from .indexed_dataset import BiDictionary, IndexedDataset
 from .preparator import prepare, prepare_on_device
-from .similarity_analysis import (CcoContext, CleanStats, DownsamplableCrossOccurrenceDataset, EventLog, IndexPages, IndexWrite, IndexWriteResult, SearchResults, SimilarityAnalysis,
+from .similarity_analysis import (CcoContext, CleanStats, EraseStats, DownsamplableCrossOccurrenceDataset, EventLog, IndexPages, IndexWrite, IndexWriteResult, SearchResults, SimilarityAnalysis,
                                   decode_ids, default_context, encode_ids)
 from .ur_algorithm import (DefaultURAlgoParams, IndicatorParams, URAlgorithmParams, calc_all, calc_all_from_events, calc_all_on_device,
                            batchpredict_output, calc_pop_from_events, clean_export, calc_pop_on_device, index_from_pages, IndexWriteError, write_index, item_queries, item_set_queries, mixed_queries_from_events,
@@ -51,7 +51,7 @@ from .ur_model import RankingParams, RefreshedIndex
 __all__ = [
     "BiDictionary", "CcoContext", "CcoError", "CcoInvalidArgument", "DataSourceParams", "DefaultURAlgoParams", "EventWindow",
     "DownsamplableCrossOccurrenceDataset", "IndexedDataset", "IndicatorParams", "SimilarityAnalysis",
-    "EventLog", "RankingParams", "URAlgorithmParams", "calc_all", "calc_all_from_events", "calc_all_on_device", "calc_pop_from_events", "clean_export", "CleanStats",
+    "EventLog", "RankingParams", "URAlgorithmParams", "calc_all", "calc_all_from_events", "calc_all_on_device", "calc_pop_from_events", "clean_export", "CleanStats", "EraseStats",
     "batchpredict_output", "calc_pop_on_device", "item_queries", "item_set_queries", "mixed_queries_from_events", "predictions_from_responses", "queries_from_file", "SearchResults", "IndexPages", "index_from_pages", "IndexWrite", "IndexWriteResult", "IndexWriteError", "write_index", "refresh_properties_from_events", "refresh_properties_on_device", "update_index", "RefreshedIndex", "user_queries_from_events", "ItemQuery", "ItemSetQuery", "MixedQuery", "UserQuery", "decode_ids", "default_context", "encode_ids", "prepare", "prepare_on_device",
     "FLAG_ASSUME_CANONICAL",
     "FLAG_ENTROPY_VARARGS", "FLAG_KEY_RANGES", "FLAG_ROWRATE_INTDIV", "FLAG_RESULT_NO_COUNT", "FLAG_RESULT_NO_LLR", "LIB_PATH",

@@ -106,6 +106,10 @@ class EventCleanStatsT(C.Structure):
                 ("n_folded", C.c_int64), ("n_compressed", C.c_int64), ("n_bytes", C.c_int64)]
 
 
+class EventEraseStatsT(C.Structure):
+    _fields_ = [("n_lines", C.c_int64), ("n_training", C.c_int64), ("n_ranking", C.c_int64), ("n_property_events", C.c_int64)]
+
+
 class UserQueryT(C.Structure):
     _fields_ = [("n_names", C.c_int32), ("n_history_names", C.c_int32), ("names", C.POINTER(C.c_char_p)), ("limits", C.POINTER(C.c_int32)),
                 ("n_blacklist_names", C.c_int32), ("history_in_must", C.c_int32), ("blacklist_names", C.POINTER(C.c_char_p)),
@@ -212,7 +216,7 @@ EXPORTS = [
     "cco_format_model", "cco_rerank_model", "cco_event_log_read", "cco_event_log_info", "cco_event_log_ingest",
     "cco_format_model_log", "cco_rerank_model_log", "cco_event_log_free", "cco_event_log_begin", "cco_event_log_append",
     "cco_event_log_finish", "cco_event_log_begin_window", "cco_event_log_window_stats",
-    "cco_event_log_begin_ex", "cco_event_log_extend", "cco_event_log_resident_bytes", "cco_event_log_intern_stats", "cco_event_log_save_size", "cco_event_log_save", "cco_event_log_load_begin", "cco_event_log_load_append", "cco_event_log_load_finish", "cco_event_log_clean_begin", "cco_event_log_clean_append", "cco_event_log_clean_finish", "cco_event_log_clean_free", "cco_event_log_user_queries", "cco_item_queries", "cco_item_set_queries", "cco_mixed_queries", "cco_query_file_read", "cco_query_file_templates", "cco_query_file_queries", "cco_query_file_free", "cco_search_results_begin", "cco_search_results_append", "cco_search_results_finish", "cco_search_results_free", "cco_index_pages_begin", "cco_index_pages_append", "cco_index_pages_finish", "cco_index_pages_free", "cco_index_write_begin", "cco_index_write_fields", "cco_index_write_requests", "cco_index_write_response", "cco_index_write_retry", "cco_index_write_finish", "cco_index_write_free", "cco_refresh_properties", "cco_refresh_properties_log", "cco_result_num_matrices", "cco_result_row_range", "cco_result_matrix", "cco_result_stats", "cco_result_key_ranges", "cco_result_free",
+    "cco_event_log_begin_ex", "cco_event_log_extend", "cco_event_log_resident_bytes", "cco_event_log_intern_stats", "cco_event_log_save_size", "cco_event_log_save", "cco_event_log_load_begin", "cco_event_log_load_append", "cco_event_log_load_finish", "cco_event_log_clean_begin", "cco_event_log_clean_append", "cco_event_log_clean_finish", "cco_event_log_clean_free", "cco_event_log_erase", "cco_event_log_erased", "cco_event_log_user_queries", "cco_item_queries", "cco_item_set_queries", "cco_mixed_queries", "cco_query_file_read", "cco_query_file_templates", "cco_query_file_queries", "cco_query_file_free", "cco_search_results_begin", "cco_search_results_append", "cco_search_results_finish", "cco_search_results_free", "cco_index_pages_begin", "cco_index_pages_append", "cco_index_pages_finish", "cco_index_pages_free", "cco_index_write_begin", "cco_index_write_fields", "cco_index_write_requests", "cco_index_write_response", "cco_index_write_retry", "cco_index_write_finish", "cco_index_write_free", "cco_refresh_properties", "cco_refresh_properties_log", "cco_result_num_matrices", "cco_result_row_range", "cco_result_matrix", "cco_result_stats", "cco_result_key_ranges", "cco_result_free",
     "cco_debug_cooccurrence", "cco_debug_key_range_cap", "cco_debug_intern_hash_bits", "cco_debug_downsample", "cco_debug_downsample_block", "cco_debug_llr", "cco_debug_string_ids", "cco_debug_rank_text", "cco_free",
 ]
 
@@ -286,6 +290,9 @@ def lib():
     L.cco_event_log_clean_append.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, p(C.c_void_p), p(C.c_int64)]
     L.cco_event_log_clean_finish.argtypes = [C.c_void_p, p(C.c_void_p), p(C.c_int64), p(EventCleanStatsT)]
     L.cco_event_log_clean_free.argtypes = [C.c_void_p]
+    L.cco_event_log_erase.argtypes = [C.c_void_p, C.c_int64, p(C.c_int64), C.c_void_p, C.c_int64, p(C.c_int64), C.c_void_p,
+                                      p(EventEraseStatsT)]
+    L.cco_event_log_erased.argtypes = [C.c_void_p, p(C.c_int64)]
     L.cco_event_log_user_queries.argtypes = [C.c_void_p, C.c_void_p, p(UserQueryT), C.c_int64, p(C.c_int64), C.c_void_p, p(C.c_void_p),
                                              p(C.c_int64), p(C.c_void_p), p(C.c_int64), p(DictionaryT)]
     L.cco_item_queries.argtypes = [C.c_void_p, C.c_char_p, C.c_int64, p(ItemQueryT), C.c_int64, p(C.c_int64), C.c_void_p, p(C.c_void_p),

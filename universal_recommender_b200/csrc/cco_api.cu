@@ -39,6 +39,7 @@
 #include "cco_intern.cuh"
 #include "cco_snapshot.cuh"
 #include "cco_clean.cuh"
+#include "cco_erase.cuh"
 
 namespace cco {
 
@@ -3808,6 +3809,7 @@ struct cco_event_log {
   long long chunk0 = 0;
   long long *dup_time = nullptr;
   long long n_dup_time = 0;
+  long long n_erased = 0;                      // retained lines cco_event_log_erase took out, over the log's life
   // the property events' item ids, which a log read without CCO_LOG_EXTENDABLE keeps after the aggregation (a snapshot
   // carries them, so that a loaded log holds the bytes the saved one holds)
   EvCol pitem;
@@ -5287,6 +5289,165 @@ static int event_log_extend(cco_event_log *lg, const cco_event_window_t *w) {
   return CCO_OK;
 }
 
+// ---- cco_event_log_erase: the lines of erased users and items taken out of a finished extendable log (cco_erase.cuh) ----
+// one id list of the caller (Arrow layout, checked on the host) on the device as a column with offsets from 0
+static int erase_upload(cco_ctx *c, Arena &ar, int64_t n, const int64_t *off, const char *bytes, EvCol *col) {
+  std::vector<long long> o((size_t)n + 1, 0);
+  for (int64_t i = 1; i <= n; ++i) o[i] = off[i] - off[0];
+  CKR(ar.alloc(&col->off, n + 1));
+  CKR(ar.alloc(&col->w, (o[n] + 16 + 7) / 8));
+  CK(cudaMemcpyAsync(col->off, o.data(), sizeof(long long) * o.size(), cudaMemcpyHostToDevice, c->stream));
+  if (o[n] > 0) CK(cudaMemcpyAsync(col->w, bytes + off[0], (size_t)o[n], cudaMemcpyHostToDevice, c->stream));
+  CK(cudaStreamSynchronize(c->stream));   // o is a local
+  return CCO_OK;
+}
+// the n ids of col probed in table tb: bit line[i] of bits for each found id (line null: the bit of its key)
+static void erase_probe(cco_event_log *lg, long long n, const long long *off, const uint64_t *w, const InternTable &tb, const long long *line,
+                        uint32_t *bits) {
+  if (n == 0 || tb.n == 0) return;
+  cco_ctx *c = lg->ctx;
+  k_erase_probe<<<grid_for(n, 256, c->sm_count), 256, 0, c->stream>>>(n, off, w, lg->intern_mask, tb.off, tb.w, tb.hash, (uint64_t)tb.cap - 1,
+                                                                       tb.table, line, bits);
+  c->launches++;
+}
+// a zeroed bitmap of n bits in the arena
+static int erase_bits(cco_ctx *c, Arena &ar, long long n, uint32_t **bits) {
+  const long long words = n / 32 + 1;
+  CKR(ar.alloc(bits, words));
+  CK(cudaMemsetAsync(*bits, 0, sizeof(uint32_t) * (size_t)words, c->stream));
+  return CCO_OK;
+}
+// Mark, then drop through the extend's finish pipeline: the records, the training and ranking columns, the property lines and
+// their aggregation, the intern tables.  Nothing marked: the log is left untouched, its snapshot image included.
+static int event_log_erase(cco_event_log *lg, int64_t n_users, const int64_t *user_off, const char *user_bytes, int64_t n_items,
+                           const int64_t *item_off, const char *item_bytes, cco_event_erase_stats_t *stats) {
+  cco_ctx *c = lg->ctx;
+  cudaStream_t s = c->stream;
+  CK(cudaSetDevice(c->device));
+  NvtxRange nvtx("cco:event_log_erase");
+  mail_reset(c);
+  Arena ar(s);
+  EvCol eu, ei;
+  CKR(erase_upload(c, ar, n_users, user_off, user_bytes, &eu));
+  CKR(erase_upload(c, ar, n_items, item_off, item_bytes, &ei));
+  uint32_t *drop = nullptr;
+  CKR(win_bitmap(lg, ar, &drop));
+  // the erase sets: intern tables of the ids, their buffers the log's until the erase ends
+  InternTable su, si;
+  uint32_t *half;
+  CKR(ar.alloc(&half, 2 * std::max<int64_t>(std::max(n_users, n_items), 1)));
+  auto drop_set = [&](InternTable &tb) {
+    for (void *p : {(void *)tb.off, (void *)tb.w, (void *)tb.hash, (void *)tb.table}) log_drop(lg, p);
+  };
+  auto release = [&] {
+    drop_set(su);
+    drop_set(si);
+    log_drop(lg, drop);
+  };
+  int rc = [&]() -> int {
+    const long long E = lg->train_at.back(), R = lg->rank_at.back();
+    CKR(intern_column(lg, ar, &si, ei, n_items, half));
+    if (lg->intern) {   // the erase ids' keys in the log's own tables, then 8 bytes per training entry
+      uint32_t *ub, *ib;
+      CKR(erase_bits(c, ar, lg->users.n, &ub));
+      CKR(erase_bits(c, ar, lg->items.n, &ib));
+      erase_probe(lg, n_users, eu.off, eu.w, lg->users, nullptr, ub);
+      erase_probe(lg, n_items, ei.off, ei.w, lg->items, nullptr, ib);
+      if (E > 0 && (n_users > 0 || n_items > 0)) {
+        k_erase_keys<<<grid_for(E, 256, c->sm_count), 256, 0, s>>>(E, (const unsigned long long *)lg->tkey, ub, ib, lg->tline, drop);
+        c->launches++;
+      }
+    } else {
+      CKR(intern_column(lg, ar, &su, eu, n_users, half));
+      erase_probe(lg, E, lg->tu.off, lg->tu.w, su, lg->tline, drop);
+      erase_probe(lg, E, lg->ti.off, lg->ti.w, si, lg->tline, drop);
+    }
+    erase_probe(lg, R, lg->ri.off, lg->ri.w, si, lg->rline, drop);
+    // property events by their entityId: the retained property lines parsed as every finish parses them
+    Arena par(s);
+    EvLines ev;
+    if (lg->n_prop > 0 && si.n > 0) {
+      CKR(event_pad(c, lg->pb, lg->pb_len));
+      CKR(event_lines(c, par, (const uint64_t *)lg->pb, lg->pb_len, false, 0, &ev));
+      JMember *jm;
+      CKR(par.alloc(&jm, ev.L));
+      k_event_strings<<<grid_for(ev.L, 256, c->sm_count), 256, 0, s>>>(ev.L, nullptr, kEvEntityId, ev.sb, ev.span, lg->pb, jm);
+      c->launches++;
+      DevStrCol ids;
+      long long nb = 0;
+      CKR(json_decode(c, par, ev.L, jm, lg->pb, &ids, &nb));
+      long long *gl;
+      CKR(par.alloc(&gl, ev.L));
+      CK(cudaMemcpyAsync(gl, lg->prop_line.data(), sizeof(long long) * (size_t)ev.L, cudaMemcpyHostToDevice, s));
+      erase_probe(lg, ev.L, ids.off, ids.w, si, gl, drop);
+      CK(cudaStreamSynchronize(s));   // prop_line is read by the copy
+    }
+    // the records of the marked lines: nothing marked leaves the log as it was
+    const long long N = lg->n_rec;
+    unsigned long long *cnt, h_cnt[3] = {0, 0, 0};
+    uint32_t *keep, *pos, *idx, K = 0;
+    CKR(ar.alloc(&cnt, 3));
+    CK(cudaMemsetAsync(cnt, 0, sizeof(h_cnt), s));
+    CKR(ar.alloc(&keep, N + 1));
+    if (N > 0) {
+      k_erase_records<<<grid_for(N, 256, c->sm_count), 256, 0, s>>>(N, lg->rec, drop, keep, cnt);
+      c->launches++;
+    }
+    CKR(select_flagged(c, ar, N, keep, &pos, &idx));
+    CK(cudaMemcpyAsync(h_cnt, cnt, sizeof(h_cnt), cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(&K, pos + N, 4, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    if (h_cnt[0] == 0) return CCO_OK;
+    lg->snap.reset();   // the image is of the log before the erase
+    CKR(ext_keep_records(lg, ar, K, idx));
+    lg->n_erased += (long long)h_cnt[0];
+    lg->n_prop -= (long long)h_cnt[1];
+    lg->n_ignored -= (long long)h_cnt[2];
+    const long long NG = (long long)lg->name_off.size() - 1;
+    CKR(win_compact(lg, drop, lg->tline, lg->train_at, &lg->tu, &lg->ti, lg->history ? &lg->ttime : nullptr, &lg->tline,
+                    lg->intern ? &lg->tkey : nullptr));
+    CKR(win_compact(lg, drop, lg->rline, lg->rank_at, &lg->ri, nullptr, &lg->rtime, &lg->rline));
+    for (long long g = 0; g < NG; ++g) {
+      lg->n_train[g] = lg->train_at[g + 1] - lg->train_at[g];
+      lg->n_rank[g] = lg->rank_at[g + 1] - lg->rank_at[g];
+    }
+    if (lg->intern) CKR(intern_refit(lg));
+    if (h_cnt[1] > 0) {   // the aggregation again, over the property lines left
+      for (void *p : {(void *)lg->p_field, (void *)lg->p_voff, (void *)lg->p_vals, (void *)lg->p_ioff, (void *)lg->p_ibytes}) log_drop(lg, p);
+      lg->p_field = nullptr;
+      lg->p_voff = lg->p_ioff = nullptr;
+      lg->p_vals = lg->p_ibytes = nullptr;
+      lg->p_ibytes_n = lg->n_triples = lg->n_prop_items = lg->n_prop_fields = 0;
+      lg->field_names.clear();
+      if (lg->n_prop > 0) {
+        mail_reset(c);
+        CKR(win_drop_property_lines(lg, par, ev, drop));
+        CKR(event_properties(c, par, lg, ev.L, ev.flag, ev.tm, ev.sb, ev.span, lg->pb, lg->prop_line.data()));
+        CKR(ext_keep_property_lines(lg, par, ev));
+      } else {
+        log_drop(lg, lg->pb);
+        lg->pb = nullptr;
+        lg->pb_len = lg->pb_cap = 0;
+        lg->prop_line = std::vector<long long>();
+      }
+    }
+    if (stats) {
+      stats->n_lines = (int64_t)h_cnt[0];
+      stats->n_training = E - lg->train_at.back();
+      stats->n_ranking = R - lg->rank_at.back();
+      stats->n_property_events = (int64_t)h_cnt[1];
+    }
+    return CCO_OK;
+  }();
+  if (rc == CCO_OK) {
+    CK(cudaStreamSynchronize(s));
+    CK(cudaGetLastError());
+  }
+  release();
+  CK(cudaStreamSynchronize(s));
+  return rc;
+}
+
 // the rankings of cco_format_model_log / cco_rerank_model_log as cco_ranking_t without streams + the log's streams
 static int log_rankings(const cco_event_log *lg, int32_t n_rank, const cco_log_ranking_t *lr, std::vector<cco_ranking_t> *rk, Streams *ls) {
   if (n_rank < 0 || (n_rank > 0 && !lr)) return set_error(CCO_E_INVALID_ARG, "bad rankings");
@@ -5391,6 +5552,37 @@ int cco_event_log_extend(cco_event_log_t *lg, const cco_event_window_t *w) {
       return set_error(CCO_E_INVALID_ARG, "cutoff %lld is before the log's %lld: expired lines are gone", (long long)w->cutoff_ms, lg->cutoff);
   }
   return log_fail(lg, event_log_extend(lg, w));
+}
+
+// the host checks of one id list of cco_event_log_erase
+static int erase_ids_check(const char *what, int64_t n, const int64_t *off, const char *bytes) {
+  if (n < 0) return set_error(CCO_E_INVALID_ARG, "%s: a negative count", what);
+  if (n == 0) return CCO_OK;
+  if (off[0] < 0) return set_error(CCO_E_INVALID_ARG, "%s: offsets[0] = %lld is negative", what, (long long)off[0]);
+  for (int64_t i = 0; i < n; ++i)
+    if (off[i + 1] < off[i]) return set_error(CCO_E_INVALID_ARG, "%s: offsets[%lld] = %lld decreases", what, (long long)i + 1, (long long)off[i + 1]);
+  if (off[n] > off[0] && !bytes) return set_error(CCO_E_INVALID_ARG, "null argument");
+  return CCO_OK;
+}
+
+int cco_event_log_erase(cco_event_log_t *lg, int64_t n_users, const int64_t *user_offsets, const char *user_bytes, int64_t n_items,
+                        const int64_t *item_offsets, const char *item_bytes, cco_event_erase_stats_t *stats) {
+  if (!lg || (n_users > 0 && !user_offsets) || (n_items > 0 && !item_offsets)) return set_error(CCO_E_INVALID_ARG, "null argument");
+  if (stats) *stats = cco_event_erase_stats_t{0, 0, 0, 0};
+  if (!lg->ctx->members.empty()) return set_error(CCO_E_UNSUPPORTED, "an event log is resident on one GPU");
+  CKR(log_state(lg, true));
+  if (!lg->extendable) return set_error(CCO_E_INVALID_ARG, "the log was read without CCO_LOG_EXTENDABLE (cco_event_log_begin_ex)");
+  if (lg->cleaners > 0) return set_error(CCO_E_INVALID_ARG, "a cleaner of the log is open (cco_event_log_clean_free)");
+  CKR(erase_ids_check("users", n_users, user_offsets, user_bytes));
+  CKR(erase_ids_check("items", n_items, item_offsets, item_bytes));
+  return log_fail(lg, event_log_erase(lg, n_users, user_offsets, user_bytes, n_items, item_offsets, item_bytes, stats));
+}
+
+int cco_event_log_erased(const cco_event_log_t *lg, int64_t *n_erased) {
+  if (!lg || !n_erased) return set_error(CCO_E_INVALID_ARG, "null argument");
+  CKR(log_state(lg, true));
+  *n_erased = lg->n_erased;
+  return CCO_OK;
 }
 
 int cco_event_log_intern_stats(const cco_event_log_t *lg, int64_t *n_user_keys, int64_t *n_item_keys) {
@@ -7951,7 +8143,7 @@ static int snap_image(cco_event_log *lg) {
   std::string st;
   const int64_t flags = (lg->history ? CCO_LOG_KEEP_HISTORY : 0) | (lg->extendable ? CCO_LOG_EXTENDABLE : 0) | (lg->intern ? CCO_LOG_INTERN_IDS : 0);
   const int64_t w[kSnapStateWords] = {flags, lg->dedup, lg->cutoff, lg->chunk0, lg->n_lines, lg->n_prop, lg->n_ignored, lg->n_prop_items,
-                                      lg->n_prop_fields, lg->n_expired, lg->n_dup, (int64_t)lg->intern_mask, 0, 0, 0, 0};
+                                      lg->n_prop_fields, lg->n_expired, lg->n_dup, (int64_t)lg->intern_mask, lg->n_erased, 0, 0, 0};
   st.assign((const char *)w, sizeof w);
   host(kSnState, st);
   const long long NG = (long long)lg->name_off.size() - 1;
@@ -8227,7 +8419,8 @@ static int snap_finish(cco_event_log *lg) {
     return set_error(CCO_E_INVALID_ARG, "snapshot section state: unknown flags 0x%llx", (long long)flags);
   bool counters_ok = (st[1] == 0 || st[1] == 1) && st[3] >= 1;
   for (int i = 4; i <= 10; ++i) counters_ok = counters_ok && st[i] >= 0;
-  for (int i = 12; i < kSnapStateWords; ++i) counters_ok = counters_ok && st[i] == 0;
+  counters_ok = counters_ok && st[12] >= 0;
+  for (int i = 13; i < kSnapStateWords; ++i) counters_ok = counters_ok && st[i] == 0;
   if (!counters_ok) return set_error(CCO_E_INVALID_ARG, "snapshot section state: a counter is out of range");
   lg->history = flags & CCO_LOG_KEEP_HISTORY;
   lg->extendable = flags & CCO_LOG_EXTENDABLE;
@@ -8243,6 +8436,7 @@ static int snap_finish(cco_event_log *lg) {
   lg->n_expired = st[9];
   lg->n_dup = st[10];
   lg->intern_mask = (uint64_t)st[11];
+  lg->n_erased = st[12];
   std::vector<std::string> names;
   CKR(snap_unstrings(*sec[kSnNames], &names));
   const long long NG = (long long)names.size();

@@ -42,13 +42,17 @@ __global__ void k_str_check(long long n, const long long *__restrict__ off, int 
     if (off[i + 1] < off[i]) *bad = 1;
 }
 
+// k_str_hash's hash of the id of len bytes at byte a of w, before the mask
+__device__ __forceinline__ uint64_t str_hash_at(const uint64_t *__restrict__ w, long long a, long long len) {
+  uint64_t h = 0x243f6a8885a308d3ULL;
+  for (long long k = 0; k * 8 < len; ++k) h = mix64(h ^ str_mask_tail(str_word(w, a, k), len - k * 8)) + 0x9e3779b97f4a7c15ULL;
+  return mix64(h ^ (uint64_t)len);
+}
 __global__ void k_str_hash(long long n, const long long *__restrict__ off, long long base, const uint64_t *__restrict__ w,
                            uint64_t mask, uint64_t *__restrict__ hash) {
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const long long a = off[i] - base, len = off[i + 1] - off[i];
-    uint64_t h = 0x243f6a8885a308d3ULL;
-    for (long long k = 0; k * 8 < len; ++k) h = mix64(h ^ str_mask_tail(str_word(w, a, k), len - k * 8)) + 0x9e3779b97f4a7c15ULL;
-    hash[i] = mix64(h ^ (uint64_t)len) & mask;
+    hash[i] = str_hash_at(w, a, len) & mask;
   }
 }
 

@@ -337,6 +337,33 @@ def clean_kept(events: Sequence[Event], window: Optional[EventWindow], now_ms: O
     return extend_clean(KeptEvents(), events, window, now_ms)
 
 
+def erased_line(e: Event, users, items) -> bool:
+    """whether EventLog.erase(users, items) takes the line out (cco_event_log_erase): a training event (entityType "user",
+    targetEntityType "item") of one of the users; any line whose targetEntityId is one of the items, whatever its types, as
+    PopModel reads ranking events by id; an item property event ($set / $unset / $delete) of one of the items.  Ids are
+    the decoded strings.  A user's lines without an item target and lines naming an item only as a non-property entityId
+    are never erased: the log holds no id for them."""
+    if e.target_id is not None and e.entity_type == "user" and e.target_type == "item" and e.entity_id in users:
+        return True
+    if e.target_id is not None and e.target_id in items:
+        return True
+    return is_property_event(e) and e.entity_id in items
+
+
+def erase_kept(kept: KeptEvents, users, items) -> tuple[KeptEvents, int]:
+    """the mirror of EventLog.erase: kept without its erased events -> (state, lines erased).  dup_times, n_expired and
+    n_duplicates stay: they count lines read, and the log holds no id for a dropped duplicate.
+
+    The contract: the rule is made of whole removeDuplicates groups (event_identity holds entityId and targetEntityId),
+    so erasing E from clean_kept(X, w) keeps the events clean_events(X - E, w) keeps, X - E being X without E's lines, and
+    an extend after it keeps what clean_events((X - E) + B, w') keeps.  Lines read = retained + expired + duplicates +
+    erased holds across erases and extends."""
+    users, items = set(users), set(items)
+    out = [e for e in kept.events if not erased_line(e, users, items)]
+    return (KeptEvents(out, kept.n_expired, kept.n_duplicates, list(kept.dup_times), kept.cutoff, kept.remove_duplicates),
+            len(kept.events) - len(out))
+
+
 def _fold_line(group: Sequence[Event], lines: Sequence[bytes]) -> bytes:
     """one $set / $unset line for a group of one entity's property lines (no $delete, no target): the fold in (eventTime,
     line) order.  With a $set, aggregate_property_events' state (None at first, so an $unset before the first $set does

@@ -1381,6 +1381,15 @@ class CleanStats:
     n_bytes: int         # bytes written
 
 
+@dataclass
+class EraseStats:
+    """cco_event_erase_stats_t: what one EventLog.erase took out"""
+    n_lines: int             # lines erased
+    n_training: int          # of them training events
+    n_ranking: int           # ranking events (lines with a targetEntityId)
+    n_property_events: int   # item $set / $unset / $delete lines
+
+
 class EventLog:
     """A PredictionIO event export resident on one GPU (cco_event_log_t), from CcoContext.read_events."""
 
@@ -1516,6 +1525,29 @@ class EventLog:
                 except OSError:
                     pass
         return CleanStats(st.n_lines, st.n_written, st.n_expired, st.n_duplicates, st.n_folded, st.n_compressed, st.n_bytes)
+
+    def erase(self, users: Sequence[str] = (), items: Sequence[str] = ()) -> EraseStats:
+        """cco_event_log_erase: the lines of these users and items taken out of the log, without a re-read
+        (events.erased_line says which: a training event of one of the users; any line whose targetEntityId is one of the
+        items; an item's $set / $unset / $delete of one of the items).  Every consumer then gives what a fresh read of the
+        export without those lines gives, and write_clean writes that export.  The log must have been read with
+        extendable=True (then extended or loaded, or not).  Ids are compared decoded and encoded as encode_ids encodes
+        them; ids the log does not hold are fine.  Later extends read new lines of erased ids as any others.  A failed
+        erase fails the log, which must then be freed.  -> EraseStats"""
+        uo, ub = encode_ids(list(users))
+        io, ib = encode_ids(list(items))
+        st = N.EventEraseStatsT()
+        i64 = C.POINTER(C.c_int64)
+        N.check(self._ctx._L.cco_event_log_erase(self._h, len(uo) - 1, uo.ctypes.data_as(i64), ub.ctypes.data, len(io) - 1,
+                                                 io.ctypes.data_as(i64), ib.ctypes.data, C.byref(st)))
+        return EraseStats(st.n_lines, st.n_training, st.n_ranking, st.n_property_events)
+
+    def erased(self) -> int:
+        """cco_event_log_erased: the lines erase has taken out over the log's life (info().n_lines = retained + expired +
+        duplicates + erased)"""
+        n = C.c_int64()
+        N.check(self._ctx._L.cco_event_log_erased(self._h, C.byref(n)))
+        return n.value
 
     def free(self):
         if getattr(self, "_h", None):
